@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """bench.py — the hot-path benchmark (BASELINE.json metric: cross-attn TFLOPS & input-tokens/sec @
-M=65536, N=512, d=1024, H=8, B=8, on 1/2/4/8 B200 with the key axis M sharded across GPUs).
+M=65536, N=512, d=1024, H=8, B=8, on 1/2/4/8 H100 with the key axis M sharded across GPUs).
 
     python bench.py --gpus 1 --steps 20 --warmup 5                    # our arm, one GPU
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 \
@@ -47,7 +47,7 @@ def load_peaks():
             pk = json.load(f)
         return dict(bf16_tflops=float(pk["bf16_tflops"]), hbm_gbs=float(pk["hbm_gbs"]),
                     source="MEASURED_PEAKS.json (measured, burst)")
-    return dict(bf16_tflops=1590.0, hbm_gbs=6650.0, source="B200_PROFILING.md fallback")
+    return dict(bf16_tflops=989.0, hbm_gbs=3350.0, source="H100 SXM data sheet (dense BF16, HBM3; 700 W card)")
 
 
 class ClockSampler:
@@ -329,22 +329,32 @@ def run_ours(args, rank, world, local_rank):
         def core_step():
             return sharded_attention(q_loc, k, v, H, scale, M, m0, merge=args.merge, copy_out=False, group=mgroup)
 
-    def timed(fn, steps, warmup):
+    def timed(fn, steps, warmup, keep=None):
         for _ in range(warmup):
             fn()
         barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(steps):
-            fn()
+            out = fn()
         e1.record()
         barrier()
+        if keep is not None:
+            keep["out"] = out
         return max_over_ranks(e0.elapsed_time(e1)) / steps
 
     # ---- value: device-resident core, exactly K steps -------------------------------------------
     launches0 = _lib.launch_count()
     with ClockSampler(local_rank) as clocks:
-        ms_core = timed(core_step, args.steps, args.warmup)
+        last = {}
+        ms_core = timed(core_step, args.steps, args.warmup, keep=last)
+    if args.dump_outputs and rank == 0:
+        # what the timed path returned in its last step on rank 0 (with several GPUs: rank 0's batch rows), as float32
+        import numpy as np
+
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "attention_out.npy"), last["out"].float().cpu().numpy())
+    last.clear()
     launches_timed = (_lib.launch_count() - launches0) * args.steps // (args.steps + args.warmup)
     clk = clocks.summary()
 
@@ -440,10 +450,10 @@ def run_ours(args, rank, world, local_rank):
                   "flops": mod_flops, "value": mod_tf, "unit": UNIT, "frac_of_tensor_peak": mod_tf / peaks["bf16_tflops"],
                   "library_launches_per_step": l_mod,
                   "min_hbm_bytes": 2.0 * B * M * d + 3 * 2.0 * B * M * d + 8.0 * B * M,   # x read twice (stats + GEMM), K,V written + read
-                  "note": "fused K/V producer: LayerNorm folded into one tcgen05 GEMM; q/o projections on the same kernel"}
+                  "note": "fused K/V producer: LayerNorm folded into one wgmma GEMM; q/o projections on the same kernel"}
         del xq_dev, xkv_dev
 
-    # ---- training: forward (statistics kept) + backward of the attention core on the tcgen05 backward kernels -------
+    # ---- training: forward (statistics kept) + backward of the attention core on the wgmma backward kernels --------
     # (SURVEY.md §8(f)2; reported next to the headline, not part of it).  FLOP counts: forward 4*B*N*M*d, backward
     # 2.5x that (5 tile GEMMs; the two kernels execute 7).
     training = None
@@ -489,7 +499,7 @@ def run_ours(args, rank, world, local_rank):
                 "parallelism": (f"batch x{bg} (independent rows, no collective) * m-shard x{mg}" if world > 1
                                 else "single GPU"),
                 "decomp": args.decomp, "batch_rows_per_gpu": Bl, "keys_per_gpu": Mg,
-                "l2": f"no flush needed: K+V per GPU = {2 * Bl * Mg * d * 2 / 2**20:.0f} MiB > 126 MiB L2",
+                "l2": f"no flush needed: K+V per GPU = {2 * Bl * Mg * d * 2 / 2**20:.0f} MiB > 50 MiB L2",
                 "kernel": args.kernel, "kv_layout": args.kv_layout, "merge": args.merge if mg > 1 else None,
             },
             "e2e": {"value": flops / (ms_e2e * 1e-3) / 1e12, "unit": UNIT, "h2d_bytes_per_step": h2d,
@@ -542,7 +552,10 @@ def main():
     ap.add_argument("--skip-module", action="store_true")
     ap.add_argument("--skip-training", action="store_true", help="skip the backward / dropout leg")
     ap.add_argument("--traffic-bytes", type=float, default=None,
-                    help="dram bytes/launch of the dominant kernel from the committed ncu capture (profiles/)")
+                    help="dram bytes/launch of the dominant kernel, when measured (reported as given)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write the output of the last timed step to DIR/<name>.npy (float32); "
+                         "with several GPUs, rank 0's batch rows")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl == "ours":
         args.warmup = 3
@@ -552,11 +565,6 @@ def main():
     if args.impl == "reference":
         run_reference(args, rank)
     else:
-        if args.traffic_bytes is None:
-            prof = os.path.join(ROOT, "profiles", "traffic_bytes.json")
-            if os.path.exists(prof):
-                with open(prof) as f:
-                    args.traffic_bytes = json.load(f).get("dram_bytes_per_launch")
         run_ours(args, rank, world, local_rank)
 
 

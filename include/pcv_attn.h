@@ -1,5 +1,5 @@
 /*
- * pcv_attn.h — C ABI of libpcv_attn.so: the B200 (sm_100a) latent-attention hot path.
+ * pcv_attn.h — C ABI of libpcv_attn.so: the H100 (sm_90a) latent-attention hot path.
  *
  * This is the drop-in boundary (SURVEY.md §8(b), level 2).  Every entry point takes plain
  * pointers and sizes; no torch types cross it.  The Python host side
@@ -48,12 +48,12 @@ extern "C" {
 /* element type of q/k/v/out */
 enum pcv_dtype { PCV_BF16 = 0, PCV_F16 = 1, PCV_F32 = 2 /* pcv_kv_append only */ };
 
-/* kernel selection; AUTO picks the tcgen05 kernel whenever the shape is supported */
+/* kernel selection; AUTO picks the tensor-core kernel whenever the shape is supported (the names are historical) */
 enum pcv_impl {
-  PCV_IMPL_AUTO = 0,         /* decode kernel for N <= 4 and M >= 1024, tcgen05 kernel when the shape fits, else SIMT */
-  PCV_IMPL_TCGEN05 = 1,      /* tcgen05 single-CTA kernel or error */
+  PCV_IMPL_AUTO = 0,         /* decode kernel for N <= 4 and M >= 1024, single-CTA tensor-core kernel when the shape fits, else SIMT */
+  PCV_IMPL_TCGEN05 = 1,      /* single-CTA tensor-core (sm_90a wgmma) kernel or error */
   PCV_IMPL_SIMT = 2,         /* CUDA-core coverage kernel */
-  PCV_IMPL_TCGEN05_PAIR = 3, /* cta_group::2 CTA-pair kernel (qk and v head dims <= 128; 512 query rows per unit) or error */
+  PCV_IMPL_TCGEN05_PAIR = 3, /* CTA-pair kernel: 2-CTA cluster sharing K/V tiles by multicast (qk and v head dims <= 128; 256 query rows per unit) or error */
   PCV_IMPL_DECODE = 4        /* streaming kernel for N <= 4 query rows against a long cache (HBM-bound) or error */
 };
 
@@ -261,7 +261,7 @@ typedef struct pcv_kvproj_params {
   int64_t rows;
   int32_t C, n_k, n_v;
   int32_t dtype;       /* PCV_BF16 / PCV_F16 */
-  int32_t cta_group;   /* 0 = library default, 1 = one CTA per tile, 2 = CTA pairs (cta_group::2) */
+  int32_t cta_group;   /* 0 = library default (1), 1 = one CTA per tile, 2 = CTA pairs (2-CTA cluster sharing the weight tile) */
   float ln_eps;        /* row_stats == NULL: > 0 = LayerNorm with statistics computed INSIDE the GEMM kernel from the
                           staged input tiles (no separate pass over x), 0 = no LayerNorm.  Ignored when row_stats is given */
 } pcv_kvproj_params;
@@ -347,7 +347,7 @@ typedef struct pcv_device_info {
   int32_t sm_major, sm_minor;
   int32_t num_sms;
   int32_t smem_optin_bytes;
-  int32_t tcgen05_ok;      /* 1 when the tcgen05 kernels can run on this device */
+  int32_t tcgen05_ok;      /* 1 when the tensor-core (sm_90a wgmma) kernels can run on this device */
 } pcv_device_info;
 
 PCV_API int pcv_abi_version(void);

@@ -298,7 +298,7 @@ def profile_end():
 
 
 def debug_read():
-    """The tcgen05 kernel's watchdog record (16 words; word 0 != 0 after a barrier-wait timeout)."""
+    """The tensor-core kernels' watchdog record (16 words; word 0 != 0 after a barrier-wait timeout)."""
     buf = (C.c_uint32 * 16)()
     l = lib()
     l.pcv_debug_read.restype = C.c_int
@@ -307,7 +307,7 @@ def debug_read():
     return list(buf)
 
 
-def debug_plan(B, H, N, M, workers=148, rows_per_unit=256):
+def debug_plan(B, H, N, M, workers=132, rows_per_unit=128):
     """Host-only: the tcgen05 work plan as (counts dict, list of (cta, b, h, q0, ntile, t0, t1, slot))."""
     counts = (C.c_int32 * 4)()
     lib().pcv_debug_plan(B, H, N, M, workers, rows_per_unit, 128, None, 0, counts)  # sizes only

@@ -147,7 +147,7 @@ int pcv_get_device_info(pcv_device_info* info) {
   info->sm_minor = prop.minor;
   info->num_sms = prop.multiProcessorCount;
   info->smem_optin_bytes = (int)prop.sharedMemPerBlockOptin;
-  info->tcgen05_ok = (prop.major == 10) ? 1 : 0;
+  info->tcgen05_ok = (prop.major == 9) ? 1 : 0;
   return PCV_OK;
 }
 

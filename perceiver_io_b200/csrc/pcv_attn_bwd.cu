@@ -1,5 +1,5 @@
-// pcv_attn_bwd.cu — training kernels of the fused attention core on the 5th-generation tensor cores (SURVEY.md
-// §8(f)2): backward (C ABI pcv_attn_bwd) and attention-probability dropout (pcv_attn_fwd_dropout, pcv_attn_dropout_mask).
+// pcv_attn_bwd.cu — training kernels of the fused attention core on the Hopper tensor cores (SURVEY.md §8(f)2):
+// backward (C ABI pcv_attn_bwd) and attention-probability dropout (pcv_attn_fwd_dropout, pcv_attn_dropout_mask).
 //
 // Reference: autograd through perceiver/model/core/modules.py:141-167 (einsum scores, masked_fill_ with the finite
 // fill, softmax, dropout, einsum with V).  With P = softmax(scale * Q K^T + fill), O = P V and the saved row statistics
@@ -11,26 +11,17 @@
 //
 //   bwd_dkdv_kernel  key-tile outer, persistent.  One CTA owns a 128-key tile (K, V resident in shared memory) and walks
 //                    the queries in sub-steps of 64.  Scores are computed TRANSPOSED, S^T = K Q^T and dP^T = V dO^T
-//                    (TMEM lanes = keys), so P^T and dS^T, rounded to bf16/fp16, go back into TMEM and feed
-//                    dV += P^T dO and dK += dS^T Q as the A operand straight from TMEM (B = dO / Q stage read
-//                    MN-major): P and dS never touch shared memory.  Two (S^T, dP^T) sets of 64 columns alternate next
-//                    to the dK / dV accumulators (512 TMEM columns in all); Q / dO arrive through a 5-deep TMA ring.
+//                    (wgmma SS, accumulator rows = keys), so P^T and dS^T, rounded to bf16/fp16, stay in registers and
+//                    feed dV += P^T dO and dK += dS^T Q as the A operand (wgmma RS, B = dO / Q stage read MN-major).
 //   bwd_dq_kernel    query-tile outer.  One CTA owns (b, h, 128 queries) and a range of key tiles (K and V streamed
-//                    through their own TMA rings); S = Q K^T, dP = dO V^T (double buffered), dS -> TMEM,
-//                    dQ += dS K (K tile read MN-major, as V is in the forward).  dQ accumulates in TMEM over the CTA's
-//                    key range and is added into an fp32 buffer with one vector reduction per element per CTA.
-//   fwd_drop_kernel  the dQ kernel's skeleton with O += dropout(P) V instead: the second forward pass of a training
-//                    step with dropout > 0 (normalised probabilities from the saved statistics, no running maximum).
+//                    through a TMA ring); S = Q K^T, dP = dO V^T, dS in registers, dQ += dS K (K tile read MN-major,
+//                    as V is in the forward).  dQ accumulates in registers over the CTA's key range and is added into an
+//                    fp32 buffer once per CTA.  With FWD it is the second forward pass of a training step with dropout:
+//                    O += dropout(P) V from the saved statistics (no running maximum).
 //
-// Recomputing S and dP in both backward kernels costs 7 tile GEMMs per (query tile, key tile) instead of 5; the
-// one-kernel alternative has to reduce a 128 x d fp32 dQ tile into global memory for EVERY (query tile, key tile) pair
-// (8.6 GB of reductions at the north-star shape, ~1.3 cycles per lane each), which is slower than the two extra
-// GEMMs.  All kernels are warp specialised like the forward: warps 0-7 softmax/epilogue (thread = TMEM lane; the two
-// warps of a lane quarter take alternate sub-steps in the dK/dV kernel and split the 128 key columns in the others),
-// warp 8 TMA producer (warp 10: the V ring of the query-outer kernels), warp 9 MMA issuer.  Measurements, versions and
-// the what-if analysis of the dK/dV kernel: profiles/r02_bwd_whatif.md, DESIGN.md §3.9 / §3.10.
+// Warpgroup 0 is the TMA producer (one lane), warpgroups 1 and 2 each own 64 rows of the tile.
 #include "pcv_common.cuh"
-#include "pcv_sm100.cuh"
+#include "pcv_sm90.cuh"
 
 #include <cuda.h>
 #include <cudaTypedefs.h>
@@ -39,25 +30,18 @@
 #include <cmath>
 #include <cstdlib>
 #include <mutex>
+#include <type_traits>
 
 namespace pcv {
 namespace {
 
-using namespace sm100;
+using namespace sm90;
 
-constexpr int kT = 128;                 // tile rows (queries or keys) = TMEM lanes
+constexpr int kT = 128;                 // tile rows (queries or keys)
 constexpr int kBoxBytes = kT * 128;     // one TMA box: 128 rows x 64 16-bit channels, SWIZZLE_128B
 constexpr int kThreads = 384;
-constexpr int kTmaWarp = 8;
-constexpr int kMmaWarp = 9;
+constexpr int kSmemLimit = 227 * 1024;
 constexpr int kStatsBytes = 64 * 12;    // row statistics of one block of 64 queries (see bwd_prep_kernel)
-#ifndef PCV_BWD_POLY_EVERY
-#define PCV_BWD_POLY_EVERY 0
-#endif
-// Experiment (compile time, off): one column pair in kPolyEvery takes its 2^x from a cubic on the FMA/ALU pipes instead
-// of MUFU.  Measured with every 2nd pair: dQ kernel 1.22 -> 1.36 ms, dK/dV kernel +1 % — neither kernel is MUFU bound
-// (XU pipe 21 % busy), the extra issue slots only lengthen the softmax warps' critical path.
-constexpr int kPolyEvery = PCV_BWD_POLY_EVERY;
 constexpr int kBox64 = 64 * 128;        // a 64-row TMA box (the dK/dV kernel stages Q / dO in 64-query pieces)
 
 struct BwdParams {
@@ -122,60 +106,6 @@ __global__ void __launch_bounds__(256) drop_mask_kernel(uint8_t* __restrict__ ke
     const uint32_t q = (uint32_t)(r % N), bh = (uint32_t)(r / N);
     keep[idx] = drop_keep(drop_bits(seed_lo, seed_hi, bh, q, k), q, k, thresh) ? 1 : 0;
   }
-}
-
-__device__ __forceinline__ uint32_t pack2(float lo, float hi, bool bf16) {
-  uint32_t r;
-  if (bf16)
-    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
-  else
-    asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
-  return r;
-}
-
-// 1-D bulk copy global -> shared, completion counted in bytes on an mbarrier (16-byte aligned, size % 16 == 0)
-__device__ __forceinline__ void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(
-                   smem_u32(smem_dst)),
-               "l"(reinterpret_cast<uint64_t>(gsrc)), "r"(bytes), "r"(smem_u32(bar))
-               : "memory");
-}
-
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d)
-               : "memory");
-}
-
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) {
-  uint64_t ra, rb, rd;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(rb) : "f"(b.x), "f"(b.y));
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(rd) : "l"(ra), "l"(rb));
-  float2 d;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(rd));
-  return d;
-}
-
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-
-// 256-bit store (sm_100): `addr` 32-byte aligned
-__device__ __forceinline__ void st_global_v8(void* addr, const uint32_t (&w)[8]) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(addr), "r"(w[0]), "r"(w[1]), "r"(w[2]),
-               "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7])
-               : "memory");
-}
-
-// one arrive per warp on a barrier initialised with count 8 (the eight softmax warps)
-__device__ __forceinline__ void warp_arrive(uint64_t* bar) {
-  __syncwarp();
-  if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -259,1027 +189,354 @@ __global__ void __launch_bounds__(256) bwd_cast_dq_kernel(const float* __restric
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// kernel 1: dK, dV.   A "sub-step" is (key tile, 64 queries): S^T and dP^T are 64 columns each, so two sets fit next to
-// the dK / dV accumulators (2 x 128 + 256 = 512 TMEM columns) and the tensor pipe computes the scores of sub-step u+1
-// while the softmax warps turn those of sub-step u into P^T / dS^T.
+// kernel 1: dK, dV.  CTA = one 128-key tile (K, V resident in shared memory; persistent over tiles), warpgroups 1-2
+// own 64 keys each and walk the queries in sub-steps of 64 (Q / dO pieces through a TMA ring).
 // ---------------------------------------------------------------------------------------------------------------
-template <int DQK, int DV>
+template <int NQB, int NVB>
 struct Cfg1 {
-  static constexpr int kQB = DQK / 64, kVB = DV / 64;
-  static constexpr int kKBytes = kQB * kBoxBytes, kVBytes = kVB * kBoxBytes;
-  static constexpr int kQStage = kQB * kBox64;       // 64 queries of Q
-  static constexpr int kStage = (kQB + kVB) * kBox64;  // ... then the same 64 rows of dO
-  static constexpr int kOffK = 0;
-  static constexpr int kOffV = kKBytes;
-  static constexpr int kOffStage = kKBytes + kVBytes;
-  static constexpr int kAvail = 232448 - 1024 - 512 - kOffStage;
-  static constexpr int kStages = kAvail / kStage > 6 ? 6 : kAvail / kStage;  // 5 at 128/128: the L2 latency of a stage
-  static constexpr int kOffBar = kOffStage + kStages * kStage;               // is ~4 sub-steps of tensor work
-  static constexpr int kNeed = kOffBar + 512 + 1024;
-  static constexpr int kSmem = kNeed > 120 * 1024 ? kNeed : 120 * 1024;  // > half an SM: one CTA (512 TMEM columns) per SM
-  static constexpr uint32_t kColDK = 256, kColDV = 256 + DQK;
-  // set s (0/1): S^T at 128*s, dP^T at 128*s + 64
+  static constexpr int kKVBytes = (NQB + NVB) * kBoxBytes;
+  static constexpr int kStage = (NQB + NVB) * kBox64;
+  static constexpr int kSlots = (kSmemLimit - kKVBytes - 2048) / kStage > 8 ? 8 : (kSmemLimit - kKVBytes - 2048) / kStage;
+  static constexpr int kSmem = kKVBytes + kSlots * kStage + 2048;
 };
 
-struct Bars1 {
-  uint64_t kv_full, kv_empty;
-  uint64_t qdo_full[6], qdo_empty[6];
-  uint64_t s_full[2], dp_full[2], p_ready[2], ds_ready[2];
-  uint64_t acc_full, acc_empty;
-  uint32_t tmem_base;
-};
-
-// One sub-step of one thread: key row (TMEM lane) x all 64 query columns, in two passes of 32.  MASKED: some score of
-// the CTA's tile is filled / out of range (padding keys, causal diagonal, ragged last key tile).
-//   st: the 32 float4 {nlse, nlse, delta, delta} of the sub-step's 64 queries; fp: their 64 fill probabilities.
-// DROP: attention dropout; `dq0` = drop_qword of the sub-step's first query, `dmk` = drop_kside of this thread's key,
-// `ksh` = bit offset of the key's byte within a query's half of the hash (8 * (key & 1)).
-template <bool BF16, bool MASKED, bool DROP>
-__device__ __forceinline__ void dkdv_substep(Bars1& bar, uint32_t set, uint32_t par, uint32_t tS, uint32_t tP,
-                                             const float* st, const float* fp, float scale_log2, bool row_filled,
-                                             bool oob, int nfill, const BwdParams& p, uint32_t dq0, uint32_t dmk,
-                                             uint32_t ksh) {
-  const float4* st4 = reinterpret_cast<const float4*>(st);
-  const float2 sc2 = make_float2(scale_log2, scale_log2);
-  float pf[64];
-  uint32_t keepm[2] = {0u, 0u};  // DROP: bit i of keepm[hh] = column hh*32 + i survives
-  mbar_wait(&bar.s_full[set], par, 21);
-  tc_fence_after_sync();
-#pragma unroll
-  for (int hh = 0; hh < 2; ++hh) {
-    uint32_t s[32];
-    uint32_t pk[16];
-    tmem_ld32(tS + hh * 32, s);
-    float2 nl[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {  // same address for the whole warp; a few KB per (b, h): L1 resident
-      const float4 q = __ldg(st4 + hh * 16 + i);
-      nl[i] = make_float2(q.x, q.y);
-    }
-    tmem_wait_ld();
-#pragma unroll
-    for (int i = 0; i < 32; i += 2) {
-      const float2 x = fma2(make_float2(__uint_as_float(s[i]), __uint_as_float(s[i + 1])), sc2, nl[i >> 1]);
-      float p0, p1;
-      if (kPolyEvery > 0 && ((i >> 1) % kPolyEvery) == kPolyEvery - 1) {  // FMA/ALU pipes instead of the MUFU queue
-        const float2 e = exp2_poly2_fast(x);
-        p0 = e.x;
-        p1 = e.y;
-      } else {
-        p0 = ex2(x.x);
-        p1 = ex2(x.y);
-      }
-      if (MASKED) {
-        if (row_filled || hh * 32 + i < nfill) p0 = __ldg(fp + hh * 32 + i);
-        if (row_filled || hh * 32 + i + 1 < nfill) p1 = __ldg(fp + hh * 32 + i + 1);
-        if (oob) p0 = p1 = 0.f;
-      }
-      pf[hh * 32 + i] = p0;
-      pf[hh * 32 + i + 1] = p1;
-      if (DROP) {  // dV sees the dropped-out, rescaled probabilities; dS below the plain ones
-        const uint32_t bits =
-            drop_finish(drop_qside(p.seed_lo, dq0 + (uint32_t)(hh * 16 + (i >> 1))), dmk);
-        const bool k0 = ((bits >> ksh) & 0xffu) >= p.drop_thresh;
-        const bool k1 = ((bits >> (ksh + 16u)) & 0xffu) >= p.drop_thresh;
-        keepm[hh] |= (k0 ? 1u : 0u) << i;
-        keepm[hh] |= (k1 ? 1u : 0u) << (i + 1);
-        p0 = k0 ? p0 * p.drop_rp : 0.f;
-        p1 = k1 ? p1 * p.drop_rp : 0.f;
-      }
-      pk[i >> 1] = pack2(p0, p1, BF16);
-    }
-    tmem_st16(tS + hh * 32, pk);  // P^T (16-bit) over the first 16 of each 32 S^T columns
-  }
-  tmem_wait_st();
-  tc_fence_before_sync();
-  warp_arrive(&bar.p_ready[set]);
-
-  mbar_wait(&bar.dp_full[set], par, 22);
-  tc_fence_after_sync();
-#pragma unroll
-  for (int hh = 0; hh < 2; ++hh) {
-    uint32_t d[32];
-    uint32_t gk[16];
-    tmem_ld32(tP + hh * 32, d);
-    float2 de[16];
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      const float4 q = __ldg(st4 + hh * 16 + i);
-      de[i] = make_float2(q.z, q.w);
-    }
-    tmem_wait_ld();
-#pragma unroll
-    for (int i = 0; i < 32; i += 2) {
-      float2 dp = make_float2(__uint_as_float(d[i]), __uint_as_float(d[i + 1]));
-      if (DROP) {  // gradient through the dropout: kept elements carry dP / (1 - p), dropped ones nothing
-        dp.x = ((keepm[hh] >> i) & 1u) ? dp.x * p.drop_rp : 0.f;
-        dp.y = ((keepm[hh] >> (i + 1)) & 1u) ? dp.y * p.drop_rp : 0.f;
-      }
-      const float2 t = sub2(dp, de[i >> 1]);
-      float2 g = mul2(make_float2(pf[hh * 32 + i], pf[hh * 32 + i + 1]), t);
-      if (MASKED) {  // a filled score is a constant: no gradient through it
-        if (row_filled || oob || hh * 32 + i < nfill) g.x = 0.f;
-        if (row_filled || oob || hh * 32 + i + 1 < nfill) g.y = 0.f;
-      }
-      gk[i >> 1] = pack2(g.x, g.y, BF16);
-    }
-    tmem_st16(tP + hh * 32, gk);
-  }
-  tmem_wait_st();
-  tc_fence_before_sync();
-  warp_arrive(&bar.ds_ready[set]);
-}
-
-// thread = key row `r` of the tile (TMEM lane).  The two warps of a lane quarter take ALTERNATE sub-steps (warps 0-3 the
-// even ones = TMEM set 0, warps 4-7 the odd ones = set 1), each all 64 query columns: two sub-steps are in flight, so the
-// TMEM round trips and barrier hand-offs of one overlap the arithmetic of the other.
-template <int DQK, int DV, bool BF16>
-__device__ __forceinline__ void softmax_dkdv(const BwdParams& p, Bars1& bar, uint8_t* smem, int warp, int lane) {
-  using C = Cfg1<DQK, DV>;
-  const int quarter = warp & 3, half = warp >> 2;
-  const int r = quarter * 32 + lane;
-  const uint32_t lanef = (uint32_t)(quarter * 32) << 16;
-  const uint32_t tbase = bar.tmem_base + lanef;
-  const int U = 2 * p.nq;
-  uint32_t g = 0, tile_iter = 0;
-  for (int id = blockIdx.x; id < p.total_tiles; id += gridDim.x, ++tile_iter) {
-    const int kt = id % p.nk, bh = id / p.nk;
-    const int h = bh % p.H, b = bh / p.H;
-    const int key = kt * kT + r;
-    const bool oob = key >= p.M;
-    uint4 mw = make_uint4(0u, 0u, 0u, 0u);
-    if (p.pad_bits != nullptr) mw = *reinterpret_cast<const uint4*>(p.pad_bits + (size_t)b * p.pad_wpr + (size_t)kt * 4);
-    const uint32_t myw = quarter == 0 ? mw.x : (quarter == 1 ? mw.y : (quarter == 2 ? mw.z : mw.w));
-    const bool pad = (myw >> lane) & 1u;
-    const bool tile_masked = ((mw.x | mw.y | mw.z | mw.w) != 0u) || (kt * kT + kT > p.M);
-    for (int u = half; u < U; u += 2) {       // U is even and g a multiple of it: set == half
-      const uint32_t gu = g + (uint32_t)u, set = gu & 1u, par = (gu >> 1) & 1u;
-      const int q0 = u * 64;                     // first query column of the sub-step
-      const float* blk = p.stats + ((size_t)bh * U + (size_t)u) * (kStatsBytes / 4);
-      const float* st = blk;                     // {nlse, nlse, delta, delta} of the 32 column pairs
-      const float* fp = blk + 128;               // fill probabilities of the 64 columns
-      const uint32_t tS = tbase + set * 128u, tP = tS + 64u;
-      const bool masked = tile_masked || (p.causal && (kt * kT + kT - 1 > u * 64 + p.cshift));
-      int nfill = 0;  // leading columns (queries) for which this key is causally hidden
-      if (masked && p.causal) nfill = min(max(key - p.cshift - q0, 0), 64);
-      if (p.drop_thresh == 0u) {
-        if (!masked)
-          dkdv_substep<BF16, false, false>(bar, set, par, tS, tP, st, fp, p.scale_log2, false, false, 0, p, 0u, 0u, 0u);
-        else
-          dkdv_substep<BF16, true, false>(bar, set, par, tS, tP, st, fp, p.scale_log2, pad, oob, nfill, p, 0u, 0u, 0u);
-      } else {
-        const uint32_t dq0 = drop_qword((uint32_t)bh, (uint32_t)q0);
-        const uint32_t dmk = drop_kside(p.seed_hi, (uint32_t)key), ksh = ((uint32_t)key & 1u) * 8u;
-        if (!masked)
-          dkdv_substep<BF16, false, true>(bar, set, par, tS, tP, st, fp, p.scale_log2, false, false, 0, p, dq0, dmk, ksh);
-        else
-          dkdv_substep<BF16, true, true>(bar, set, par, tS, tP, st, fp, p.scale_log2, pad, oob, nfill, p, dq0, dmk, ksh);
-      }
-    }
-    g += (uint32_t)U;
-
-    // ---- drain the accumulators of this key tile: half 0 -> dK (scaled), half 1 -> dV ----
-    mbar_wait(&bar.acc_full, tile_iter & 1u, 23);
-    tc_fence_after_sync();
-    {
-      const int cols = half == 0 ? DQK : DV;
-      const int nreal = half == 0 ? p.dqk : p.dv;
-      const float mult = half == 0 ? p.scale : 1.f;
-      const uint32_t tA = bar.tmem_base + lanef + (half == 0 ? C::kColDK : C::kColDV);
-      uint16_t* dst = half == 0
-                          ? reinterpret_cast<uint16_t*>(p.dk) + b * p.dk_sb + (int64_t)key * p.dk_sm + h * p.dk_sh
-                          : reinterpret_cast<uint16_t*>(p.dv_out) + b * p.dv_sb + (int64_t)key * p.dv_sm + h * p.dv_sh;
-      for (int ch = 0; ch < cols / 64; ++ch) {  // 64 accumulator columns per round trip to TMEM
-        uint32_t a[64];
-        tmem_ld32(tA + ch * 64, *reinterpret_cast<uint32_t(*)[32]>(&a[0]));
-        tmem_ld32(tA + ch * 64 + 32, *reinterpret_cast<uint32_t(*)[32]>(&a[32]));
-        tmem_wait_ld();
-        if (!oob) {
-#pragma unroll
-          for (int gq = 0; gq < 4; ++gq) {  // 16 channels = 32 bytes per store
-            const int c = ch * 64 + gq * 16;
-            uint32_t w[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e)
-              w[e] = pack2(__uint_as_float(a[gq * 16 + 2 * e]) * mult, __uint_as_float(a[gq * 16 + 2 * e + 1]) * mult, BF16);
-            if (p.wide_store && c + 16 <= nreal) {
-              st_global_v8(dst + c, w);  // one full 32-byte sector per lane (16-byte stores leave half sectors to L2)
-            } else {
-              if (c < nreal) *reinterpret_cast<uint4*>(dst + c) = make_uint4(w[0], w[1], w[2], w[3]);
-              if (c + 8 < nreal) *reinterpret_cast<uint4*>(dst + c + 8) = make_uint4(w[4], w[5], w[6], w[7]);
-            }
-          }
-        }
-      }
-    }
-    tc_fence_before_sync();
-    warp_arrive(&bar.acc_empty);
-  }
-}
-
-template <int DQK, int DV, bool BF16>
-__global__ void __launch_bounds__(kThreads, 1)
-bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_do,
-                const BwdParams p) {
-  using C = Cfg1<DQK, DV>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  Bars1& bar = *reinterpret_cast<Bars1*>(smem + C::kOffBar);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  if (threadIdx.x == 0) {
-    mbar_init(&bar.kv_full, 1);
-    mbar_init(&bar.kv_empty, 1);
-    for (int i = 0; i < C::kStages; ++i) {
-      mbar_init(&bar.qdo_full[i], 1);
-      mbar_init(&bar.qdo_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&bar.s_full[i], 1);
-      mbar_init(&bar.dp_full[i], 1);
-      mbar_init(&bar.p_ready[i], 4);   // the four warps that own this set
-      mbar_init(&bar.ds_ready[i], 4);
-    }
-    mbar_init(&bar.acc_full, 1);
-    mbar_init(&bar.acc_empty, 8);
-    fence_mbar_init();
-  }
-  if (warp == kMmaWarp) {
-    tmem_alloc(&bar.tmem_base, 512);
-    tmem_relinquish();
-  }
-  if (warp == kTmaWarp && lane == 0) {
-    tma_prefetch_desc(&tmap_q);
-    tma_prefetch_desc(&tmap_k);
-    tma_prefetch_desc(&tmap_v);
-    tma_prefetch_desc(&tmap_do);
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-
-  if (warp < 8) {
-    reg_alloc<208>();
-    softmax_dkdv<DQK, DV, BF16>(p, bar, smem, warp, lane);
-  } else {
-    reg_dealloc<88>();
-  }
-
-  if (warp == kTmaWarp) {
-    // ===== TMA producer: K, V of the key tile once; 64 queries of Q and dO per sub-step through the ring =====
-    const bool leader = elect_one();
-    uint32_t it = 0, tile_iter = 0;
-    for (int id = blockIdx.x; id < p.total_tiles; id += gridDim.x, ++tile_iter) {
-      const int kt = id % p.nk, bh = id / p.nk;
-      const int h = bh % p.H, b = bh / p.H;
-      mbar_wait(&bar.kv_empty, (tile_iter & 1u) ^ 1u, 1);
-      if (leader) {
-        mbar_arrive_expect_tx(&bar.kv_full, (uint32_t)(C::kKBytes + C::kVBytes));
-#pragma unroll
-        for (int bx = 0; bx < C::kQB; ++bx)
-          tma_load_4d(smem + C::kOffK + bx * kBoxBytes, &tmap_k, &bar.kv_full, bx * 64, kt * kT, h, b);
-#pragma unroll
-        for (int bx = 0; bx < C::kVB; ++bx)
-          tma_load_4d(smem + C::kOffV + bx * kBoxBytes, &tmap_v, &bar.kv_full, bx * 64, kt * kT, h, b);
-      }
-      for (int u = 0; u < 2 * p.nq; ++u, ++it) {
-        const uint32_t slot = it % C::kStages;
-        mbar_wait(&bar.qdo_empty[slot], ((it / C::kStages) & 1u) ^ 1u, 2);
-        if (leader) {
-          uint8_t* st = smem + C::kOffStage + slot * C::kStage;
-          mbar_arrive_expect_tx(&bar.qdo_full[slot], (uint32_t)C::kStage);
-#pragma unroll
-          for (int bx = 0; bx < C::kQB; ++bx)
-            tma_load_4d(st + bx * kBox64, &tmap_q, &bar.qdo_full[slot], bx * 64, u * 64, h, p.q_bcast ? 0 : b);
-#pragma unroll
-          for (int bx = 0; bx < C::kVB; ++bx)
-            tma_load_4d(st + C::kQStage + bx * kBox64, &tmap_do, &bar.qdo_full[slot], bx * 64, u * 64, h, b);
-        }
-      }
-    }
-  } else if (warp == kMmaWarp) {
-    // ===== MMA issuer (warp converged, one elected lane issues) =====
-    const bool leader = elect_one();
-    constexpr uint32_t idesc_s = make_idesc(kT, 64, BF16, false);
-    constexpr uint32_t idesc_dv = make_idesc(kT, DV, BF16, true);
-    constexpr uint32_t idesc_dk = make_idesc(kT, DQK, BF16, true);
-    const uint32_t tmem = bar.tmem_base;
-    const uint64_t dK = make_smem_desc(smem_u32(smem + C::kOffK), 16, 1024);
-    const uint64_t dV = make_smem_desc(smem_u32(smem + C::kOffV), 16, 1024);
-    auto stage_q = [&](uint32_t gu) { return smem_u32(smem + C::kOffStage + (gu % C::kStages) * C::kStage); };
-    // sub-step gu: ring slot gu % kStages (64 queries of Q, then of dO), TMEM set gu & 1
-    auto issue_s = [&](uint32_t gu) {  // S^T = K Q^T
-      if (leader) {
-        const uint64_t db = make_smem_desc(stage_q(gu), 16, 1024);
-#pragma unroll
-        for (int kk = 0; kk < DQK / 16; ++kk) {
-          const uint64_t offa = (uint64_t)(((kk >> 2) * kBoxBytes + (kk & 3) * 32) >> 4);
-          const uint64_t offb = (uint64_t)(((kk >> 2) * kBox64 + (kk & 3) * 32) >> 4);
-          mma_ss(tmem + (gu & 1u) * 128u, dK + offa, db + offb, idesc_s, kk > 0 ? 1u : 0u);
-        }
-      }
-    };
-    auto issue_dp = [&](uint32_t gu) {  // dP^T = V dO^T
-      if (leader) {
-        const uint64_t db = make_smem_desc(stage_q(gu) + C::kQStage, 16, 1024);
-#pragma unroll
-        for (int kk = 0; kk < DV / 16; ++kk) {
-          const uint64_t offa = (uint64_t)(((kk >> 2) * kBoxBytes + (kk & 3) * 32) >> 4);
-          const uint64_t offb = (uint64_t)(((kk >> 2) * kBox64 + (kk & 3) * 32) >> 4);
-          mma_ss(tmem + (gu & 1u) * 128u + 64u, dV + offa, db + offb, idesc_s, kk > 0 ? 1u : 0u);
-        }
-      }
-    };
-    auto issue_dv = [&](uint32_t gu, bool acc) {  // dV += P^T(TMEM) dO   (dO read MN-major: 16 queries = 2048 bytes)
-      if (leader) {
-        const uint64_t db = make_smem_desc(stage_q(gu) + C::kQStage, kBox64, 1024);
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk)
-          mma_ts(tmem + C::kColDV, tmem + (gu & 1u) * 128u + (uint32_t)((kk >> 1) * 32 + (kk & 1) * 8),
-                 db + (uint64_t)((kk * 2048) >> 4), idesc_dv, (acc || kk > 0) ? 1u : 0u);
-      }
-    };
-    auto issue_dk = [&](uint32_t gu, bool acc) {  // dK += dS^T(TMEM) Q
-      if (leader) {
-        const uint64_t db = make_smem_desc(stage_q(gu), kBox64, 1024);
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk)
-          mma_ts(tmem + C::kColDK, tmem + (gu & 1u) * 128u + 64u + (uint32_t)((kk >> 1) * 32 + (kk & 1) * 8),
-                 db + (uint64_t)((kk * 2048) >> 4), idesc_dk, (acc || kk > 0) ? 1u : 0u);
-      }
-    };
-    auto commit = [&](uint64_t* bp) {
-      if (leader) tc_commit(bp);
-    };
-
-    const int U = 2 * p.nq;
-    uint32_t g = 0, tile_iter = 0;
-    for (int id = blockIdx.x; id < p.total_tiles; id += gridDim.x, ++tile_iter) {
-      mbar_wait(&bar.kv_full, tile_iter & 1u, 3);
-      // the scores of the first two sub-steps (one per TMEM set); U >= 2
-      for (uint32_t u0 = 0; u0 < 2; ++u0) {
-        const uint32_t gn = g + u0;
-        mbar_wait(&bar.qdo_full[gn % C::kStages], (gn / C::kStages) & 1u, 4);
-        tc_fence_after_sync();
-        issue_s(gn);
-        commit(&bar.s_full[gn & 1u]);
-        issue_dp(gn);
-        commit(&bar.dp_full[gn & 1u]);
-      }
-      if (U == 2) commit(&bar.kv_empty);
-      for (int u = 0; u < U; ++u) {
-        const uint32_t gu = g + (uint32_t)u, set = gu & 1u, par = (gu >> 1) & 1u;
-        const bool more = u + 2 < U;
-        mbar_wait(&bar.p_ready[set], par, 5);
-        if (u == 0) mbar_wait(&bar.acc_empty, (tile_iter & 1u) ^ 1u, 6);
-        tc_fence_after_sync();
-        issue_dv(gu, u > 0);
-        if (more) {
-          // S(u+2) goes into this set's S columns: the softmax warps have read S(u), and dV(u) — the reader of the P
-          // they stored there — is ahead of it in the in-order pipe.  Issuing it here rather than after dK(u) gives
-          // the owners of this set their next scores half a sub-step earlier (measured: -2 %).
-          const uint32_t gn = gu + 2;
-          mbar_wait(&bar.qdo_full[gn % C::kStages], (gn / C::kStages) & 1u, 7);
-          tc_fence_after_sync();
-          issue_s(gn);
-          commit(&bar.s_full[set]);
-        }
-        mbar_wait(&bar.ds_ready[set], par, 8);
-        tc_fence_after_sync();
-        issue_dk(gu, u > 0);
-        commit(&bar.qdo_empty[gu % C::kStages]);
-        if (more) {
-          issue_dp(gu + 2);  // over dS(u), which dK(u) has just been queued to read
-          commit(&bar.dp_full[set]);
-          if (u + 3 == U) commit(&bar.kv_empty);  // K and V are not read again for this key tile
-        }
-      }
-      commit(&bar.acc_full);
-      g += (uint32_t)U;
-    }
-  }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == kMmaWarp) {
-    tc_fence_after_sync();
-    tmem_dealloc(bar.tmem_base, 512);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// kernel 2: dQ.   TMEM: S 0..127, dP double buffered at 128 / 256 (dS overwrites its dP), dQ at 384.
-// ---------------------------------------------------------------------------------------------------------------
-template <int DQK, int DV>
+// kernel 2 (dQ) and 3 (forward with dropout): CTA = (b, h, 128 queries, key range); warpgroups 1-2 own 64 queries each;
+// Q (and dO) stay resident, K / V tiles stream through a TMA ring.
+template <int NQB, int NVB>
 struct Cfg2 {
-  static constexpr int kQB = DQK / 64, kVB = DV / 64;
-  static constexpr int kKBytes = kQB * kBoxBytes, kVBytes = kVB * kBoxBytes;
-  // K_t is read by S(t) and again by dQ(t); V_t only by dP(t): separate rings, so that a V slot is refilled as soon as
-  // dP has consumed it.  The load of a slot is issued when its previous tile retires, i.e. (stages - 1) tiles ahead:
-  // 3 K stages + 2 V stages hide the ~2 us L2 round trip of a tile (2 + 2 measured 3.6k cycles per tile, MMA 1.5k).
-  static constexpr int kKS = 3;
-  static constexpr int kAvail = 232448 - 1024 - 512 - (kKBytes + kVBytes) - kKS * kKBytes;
-  static constexpr int kVS = kAvail / kVBytes >= 3 ? 3 : 2;
-  static constexpr int kOffQ = 0;
-  static constexpr int kOffDO = kKBytes;
-  static constexpr int kOffKRing = kKBytes + kVBytes;
-  static constexpr int kOffVRing = kOffKRing + kKS * kKBytes;
-  static constexpr int kOffBar = kOffVRing + kVS * kVBytes;
-  static constexpr int kNeed = kOffBar + 512 + 1024;
-  static constexpr int kSmem = kNeed > 120 * 1024 ? kNeed : 120 * 1024;
-  static constexpr uint32_t kColS = 0, kColP = 128, kColDQ = 384;
+  static constexpr int kQBytes = (NQB + NVB) * kBoxBytes;
+  static constexpr int kStage = (NQB + NVB) * kBoxBytes;
+  static constexpr int kSlots = (kSmemLimit - kQBytes - 2048) / kStage > 4 ? 4 : (kSmemLimit - kQBytes - 2048) / kStage;
+  static constexpr int kSmem = kQBytes + kSlots * kStage + 2048;
+  static_assert(kSlots >= 2, "shared memory budget");
 };
 
-struct Bars2 {
-  uint64_t q_full;
-  uint64_t k_full[3], k_empty[3], v_full[3], v_empty[3];
-  uint64_t s_full, dp_full[2], s_free, ds_ready;
-  uint64_t dq_full;
-  uint32_t tmem_base;
+struct BwdBarriers {
+  uint64_t full[8], empty[8];
+  uint64_t fix_full, fix_empty;
 };
 
-// one key tile of one thread: query row (TMEM lane) x 64 key columns
-// DROP: `dh1` = this query's half of the dropout hash, `qsh` = 16 * (query & 1), `k0` = first key of the 64 columns
-template <bool BF16, bool MASKED, bool DROP>
-__device__ __forceinline__ void dq_tile(Bars2& bar, uint32_t i_t, uint32_t tS, uint32_t tP, float scale_log2,
-                                        float nlse, float delta, float fillp, uint32_t w0, uint32_t w1, int cmax,
-                                        int oob_from, const BwdParams& p, uint32_t dh1, uint32_t qsh, uint32_t k0) {
-  const float2 sc2 = make_float2(scale_log2, scale_log2), nl2 = make_float2(nlse, nlse), de2 = make_float2(delta, delta);
-  uint32_t s[64];
-  mbar_wait(&bar.s_full, i_t & 1u, 30);
-  tc_fence_after_sync();
-  tmem_ld32(tS, *reinterpret_cast<uint32_t(*)[32]>(&s[0]));
-  tmem_ld32(tS + 32, *reinterpret_cast<uint32_t(*)[32]>(&s[32]));
-  tmem_wait_ld();
-  tc_fence_before_sync();
-  warp_arrive(&bar.s_free);  // S is in registers: the issuer may overwrite it with the next tile's scores
-#pragma unroll
-  for (int i = 0; i < 64; i += 2) {
-    const float2 x = fma2(make_float2(__uint_as_float(s[i]), __uint_as_float(s[i + 1])), sc2, nl2);
-    float p0, p1;
-    if (kPolyEvery > 0 && ((i >> 1) % kPolyEvery) == kPolyEvery - 1) {
-      const float2 e = exp2_poly2_fast(x);
-      p0 = e.x;
-      p1 = e.y;
-    } else {
-      p0 = ex2(x.x);
-      p1 = ex2(x.y);
-    }
-    if (MASKED) {
-      const uint32_t word = i < 32 ? w0 : w1;
-      if (((word >> (i & 31)) & 1u) || i > cmax) p0 = fillp;
-      if (((word >> ((i + 1) & 31)) & 1u) || i + 1 > cmax) p1 = fillp;
-      if (i >= oob_from) p0 = 0.f;
-      if (i + 1 >= oob_from) p1 = 0.f;
-    }
-    s[i] = __float_as_uint(p0);
-    s[i + 1] = __float_as_uint(p1);
-  }
-
-  mbar_wait(&bar.dp_full[i_t & 1u], (i_t >> 1) & 1u, 31);
-  tc_fence_after_sync();
-  {
-    uint32_t d[64];
-    uint32_t gk[32];
-    tmem_ld32(tP, *reinterpret_cast<uint32_t(*)[32]>(&d[0]));
-    tmem_ld32(tP + 32, *reinterpret_cast<uint32_t(*)[32]>(&d[32]));
-    tmem_wait_ld();
-#pragma unroll
-    for (int i = 0; i < 64; i += 2) {
-      float2 dp = make_float2(__uint_as_float(d[i]), __uint_as_float(d[i + 1]));
-      if (DROP) {
-        const uint32_t bits = drop_finish(dh1, drop_kside(p.seed_hi, k0 + (uint32_t)i));
-        dp.x = (((bits >> qsh) & 0xffu) >= p.drop_thresh) ? dp.x * p.drop_rp : 0.f;
-        dp.y = (((bits >> (qsh + 8u)) & 0xffu) >= p.drop_thresh) ? dp.y * p.drop_rp : 0.f;
-      }
-      const float2 t = sub2(dp, de2);
-      float2 g = mul2(make_float2(__uint_as_float(s[i]), __uint_as_float(s[i + 1])), t);
-      if (MASKED) {
-        const uint32_t word = i < 32 ? w0 : w1;
-        if (((word >> (i & 31)) & 1u) || i > cmax || i >= oob_from) g.x = 0.f;
-        if (((word >> ((i + 1) & 31)) & 1u) || i + 1 > cmax || i + 1 >= oob_from) g.y = 0.f;
-      }
-      gk[i >> 1] = pack2(g.x, g.y, BF16);
-    }
-    tmem_st32(tP, gk);  // dS (16-bit) over the first 32 of this warp's 64 dP columns
-    tmem_wait_st();
-  }
-  tc_fence_before_sync();
-  warp_arrive(&bar.ds_ready);
+__device__ __forceinline__ bool filled_key(const BwdParams& p, int b, int j, int n) {
+  if (p.pad_bits != nullptr && ((p.pad_bits[(int64_t)b * p.pad_wpr + (j >> 5)] >> (j & 31)) & 1u)) return true;
+  return p.causal && j > n + p.cshift;
 }
 
-// thread = query row `r` of the tile (TMEM lane); this warp handles key columns [64*half, 64*half + 64)
-template <int DQK, int DV, bool BF16>
-__device__ __forceinline__ void softmax_dq(const BwdParams& p, Bars2& bar, int warp, int lane, int b, int h, int j,
-                                           int t0, int t1) {
-  using C = Cfg2<DQK, DV>;
-  const int quarter = warp & 3, half = warp >> 2;
-  const int r = quarter * 32 + lane;
-  const int nrow = j * kT + r;
-  const uint32_t lanef = (uint32_t)(quarter * 32) << 16;
-  const uint32_t tS = bar.tmem_base + lanef + C::kColS + (uint32_t)(half * 64);
-  const uint32_t tP0 = bar.tmem_base + lanef + C::kColP + (uint32_t)(half * 64);
-  const float* blk = p.stats + (((size_t)b * p.H + h) * (2 * p.nq) + (size_t)(nrow >> 6)) * (kStatsBytes / 4);
-  const float nlse = blk[stat_nlse_idx(r & 63)], delta = blk[stat_delta_idx(r & 63)], fillp = blk[stat_fillp_idx(r & 63)];
-  // dropout: this query's half of the hash and the bit offset of its two bytes within a key pair's hash
-  const uint32_t dh1 = drop_qside(p.seed_lo, drop_qword((uint32_t)(b * p.H + h), (uint32_t)nrow));
-  const uint32_t qsh = ((uint32_t)nrow & 1u) * 16u;
-
-  for (int t = t0; t < t1; ++t) {
-    const uint32_t i_t = (uint32_t)(t - t0);
-    const uint32_t tP = tP0 + (i_t & 1u) * 128u;
-    const int k0 = t * kT + half * 64;  // first key of this thread's 64 columns
-    uint32_t w0 = 0u, w1 = 0u;
-    bool tile_masked = (t * kT + kT > p.M);
-    if (p.pad_bits != nullptr) {
-      const uint4 mw = *reinterpret_cast<const uint4*>(p.pad_bits + (size_t)b * p.pad_wpr + (size_t)t * 4);
-      w0 = half == 0 ? mw.x : mw.z;
-      w1 = half == 0 ? mw.y : mw.w;
-      tile_masked = tile_masked || ((mw.x | mw.y | mw.z | mw.w) != 0u);
-    }
-    const bool masked = tile_masked || (p.causal && (t * kT + kT - 1 > j * kT + p.cshift));
-    const int cmax = p.causal ? (nrow + p.cshift - k0) : 0x7fffffff;  // column i filled iff i > cmax
-    const int oob_from = p.M - k0;                                   // column i beyond the tensor iff i >= oob_from
-    if (p.drop_thresh == 0u) {
-      if (!masked)
-        dq_tile<BF16, false, false>(bar, i_t, tS, tP, p.scale_log2, nlse, delta, fillp, 0u, 0u, 0, 0, p, 0u, 0u, 0u);
-      else
-        dq_tile<BF16, true, false>(bar, i_t, tS, tP, p.scale_log2, nlse, delta, fillp, w0, w1, cmax, oob_from, p, 0u,
-                                   0u, 0u);
-    } else {
-      if (!masked)
-        dq_tile<BF16, false, true>(bar, i_t, tS, tP, p.scale_log2, nlse, delta, fillp, 0u, 0u, 0, 0, p, dh1, qsh,
-                                   (uint32_t)k0);
-      else
-        dq_tile<BF16, true, true>(bar, i_t, tS, tP, p.scale_log2, nlse, delta, fillp, w0, w1, cmax, oob_from, p, dh1,
-                                  qsh, (uint32_t)k0);
-    }
-  }
-
-  // ---- add this CTA's dQ (scaled) into the fp32 buffer ----
-  mbar_wait(&bar.dq_full, 0u, 32);
-  tc_fence_after_sync();
-  {
-    constexpr int kCols = DQK / 2;  // columns per warp half
-    const uint32_t tQ = bar.tmem_base + lanef + C::kColDQ + (uint32_t)(half * kCols);
-    float* dst = p.dq32 + ((size_t)(p.q_bcast ? 0 : b) * p.N + (size_t)nrow) * ((size_t)p.H * p.dqk) + (size_t)h * p.dqk +
-                 (size_t)half * kCols;
-#pragma unroll
-    for (int ch = 0; ch < kCols / 32; ++ch) {
-      uint32_t a[32];
-      tmem_ld32(tQ + ch * 32, a);
-      tmem_wait_ld();
-      if (nrow < p.N) {
-#pragma unroll
-        for (int gq = 0; gq < 8; ++gq) {
-          const int c = half * kCols + ch * 32 + gq * 4;
-          if (c < p.dqk)
-            red_add_v4(dst + ch * 32 + gq * 4, __uint_as_float(a[gq * 4 + 0]) * p.scale,
-                       __uint_as_float(a[gq * 4 + 1]) * p.scale, __uint_as_float(a[gq * 4 + 2]) * p.scale,
-                       __uint_as_float(a[gq * 4 + 3]) * p.scale);
-        }
-      }
-    }
-  }
-}
-
-template <int DQK, int DV, bool BF16>
+template <int NQB, int NVB, bool BF16>
 __global__ void __launch_bounds__(kThreads, 1)
-bwd_dq_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-              const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_do,
-              const BwdParams p) {
-  using C = Cfg2<DQK, DV>;
-  extern __shared__ uint8_t smem_raw[];
+bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq64, const __grid_constant__ CUtensorMap tk,
+                const __grid_constant__ CUtensorMap tv, const __grid_constant__ CUtensorMap tdo64, const BwdParams p) {
+  using C = Cfg1<NQB, NVB>;
+  constexpr int NS = C::kSlots;
+  using T = typename std::conditional<BF16, __nv_bfloat16, __half>::type;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  Bars2& bar = *reinterpret_cast<Bars2*>(smem + C::kOffBar);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  // blockIdx -> (b, h, query tile j, key-tile range); the query tiles of one (b, h) and split are neighbours, so the
-  // CTAs that stream the same K/V range run together and meet in L2
-  const int j = blockIdx.x % p.nq;
-  const int sp = (blockIdx.x / p.nq) % p.splits;
-  const int bh = blockIdx.x / (p.nq * p.splits);
-  const int h = bh % p.H, b = bh / p.H;
-  const int t0 = sp * p.tiles_per_split;
-  const int t1 = min(p.nk, t0 + p.tiles_per_split);
-
+  uint8_t* sK = smem;
+  uint8_t* sV = smem + NQB * kBoxBytes;
+  uint8_t* sRing = smem + C::kKVBytes;
+  BwdBarriers& bar = *reinterpret_cast<BwdBarriers*>(sRing + NS * C::kStage);
+  const int wg = threadIdx.x / 128;
+  const int nq64 = (p.N + 63) / 64;
   if (threadIdx.x == 0) {
-    mbar_init(&bar.q_full, 1);
-    for (int i = 0; i < 3; ++i) {
-      mbar_init(&bar.k_full[i], 1);
-      mbar_init(&bar.k_empty[i], 1);
-      mbar_init(&bar.v_full[i], 1);
-      mbar_init(&bar.v_empty[i], 1);
+    for (int s = 0; s < NS; ++s) {
+      mbar_init(&bar.full[s], 1);
+      mbar_init(&bar.empty[s], 8);
     }
-    mbar_init(&bar.dp_full[0], 1);
-    mbar_init(&bar.dp_full[1], 1);
-    mbar_init(&bar.s_full, 1);
-    mbar_init(&bar.s_free, 8);
-    mbar_init(&bar.ds_ready, 8);
-    mbar_init(&bar.dq_full, 1);
+    mbar_init(&bar.fix_full, 1);
+    mbar_init(&bar.fix_empty, 8);
     fence_mbar_init();
   }
-  if (warp == kMmaWarp) {
-    tmem_alloc(&bar.tmem_base, 512);
-    tmem_relinquish();
-  }
-  if (warp == kTmaWarp && lane == 0) {
-    tma_prefetch_desc(&tmap_q);
-    tma_prefetch_desc(&tmap_k);
-    tma_prefetch_desc(&tmap_v);
-    tma_prefetch_desc(&tmap_do);
-  }
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
 
-  if (warp < 8) {
-    reg_alloc<208>();
-    softmax_dq<DQK, DV, BF16>(p, bar, warp, lane, b, h, j, t0, t1);
-  } else {
-    reg_dealloc<88>();
-  }
-
-  if (warp == kTmaWarp) {
-    const bool leader = elect_one();
-    if (leader) {
-      mbar_arrive_expect_tx(&bar.q_full, (uint32_t)(C::kKBytes + C::kVBytes));
-#pragma unroll
-      for (int bx = 0; bx < C::kQB; ++bx)
-        tma_load_4d(smem + C::kOffQ + bx * kBoxBytes, &tmap_q, &bar.q_full, bx * 64, j * kT, h, p.q_bcast ? 0 : b);
-#pragma unroll
-      for (int bx = 0; bx < C::kVB; ++bx)
-        tma_load_4d(smem + C::kOffDO + bx * kBoxBytes, &tmap_do, &bar.q_full, bx * 64, j * kT, h, b);
-    }
-    for (int t = t0; t < t1; ++t) {  // K ring
-      const uint32_t it = (uint32_t)(t - t0), slot = it % C::kKS;
-      mbar_wait(&bar.k_empty[slot], ((it / C::kKS) & 1u) ^ 1u, 10);
-      if (leader) {
-        uint8_t* st = smem + C::kOffKRing + slot * C::kKBytes;
-        mbar_arrive_expect_tx(&bar.k_full[slot], (uint32_t)C::kKBytes);
-#pragma unroll
-        for (int bx = 0; bx < C::kQB; ++bx)
-          tma_load_4d(st + bx * kBoxBytes, &tmap_k, &bar.k_full[slot], bx * 64, t * kT, h, b);
-      }
-    }
-  } else if (warp == kTmaWarp + 2) {  // V ring: its own warp, so that a full K ring never delays a V load
-    const bool leader = elect_one();
-    for (int t = t0; t < t1; ++t) {
-      const uint32_t it = (uint32_t)(t - t0), slot = it % C::kVS;
-      mbar_wait(&bar.v_empty[slot], ((it / C::kVS) & 1u) ^ 1u, 16);
-      if (leader) {
-        uint8_t* st = smem + C::kOffVRing + slot * C::kVBytes;
-        mbar_arrive_expect_tx(&bar.v_full[slot], (uint32_t)C::kVBytes);
-#pragma unroll
-        for (int bx = 0; bx < C::kVB; ++bx)
-          tma_load_4d(st + bx * kBoxBytes, &tmap_v, &bar.v_full[slot], bx * 64, t * kT, h, b);
-      }
-    }
-  } else if (warp == kMmaWarp) {
-    const bool leader = elect_one();
-    constexpr uint32_t idesc_s = make_idesc(kT, kT, BF16, false);
-    constexpr uint32_t idesc_dq = make_idesc(kT, DQK, BF16, true);
-    const uint32_t tmem = bar.tmem_base;
-    const uint64_t dQ = make_smem_desc(smem_u32(smem + C::kOffQ), 16, 1024);
-    const uint64_t dDO = make_smem_desc(smem_u32(smem + C::kOffDO), 16, 1024);
-    auto kring = [&](uint32_t i) { return smem_u32(smem + C::kOffKRing + (i % C::kKS) * C::kKBytes); };
-    auto vring = [&](uint32_t i) { return smem_u32(smem + C::kOffVRing + (i % C::kVS) * C::kVBytes); };
-    auto issue_s = [&](uint32_t i) {  // S = Q_j K_t^T
-      if (leader) {
-        const uint64_t db = make_smem_desc(kring(i), 16, 1024);
-#pragma unroll
-        for (int kk = 0; kk < DQK / 16; ++kk) {
-          const uint64_t off = (uint64_t)(((kk >> 2) * kBoxBytes + (kk & 3) * 32) >> 4);
-          mma_ss(tmem + C::kColS, dQ + off, db + off, idesc_s, kk > 0 ? 1u : 0u);
+  if (wg == 0) {
+    reg_dealloc<40>();
+    if (threadIdx.x == 0) {
+      uint32_t it = 0, tl = 0;
+      for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++tl) {
+        const int bh = tile / p.nk, kt = tile % p.nk, b = bh / p.H, h = bh % p.H;
+        mbar_wait(&bar.fix_empty, (tl & 1) ^ 1, 21);
+        mbar_arrive_expect_tx(&bar.fix_full, C::kKVBytes);
+        for (int c = 0; c < NQB; ++c) tma_load_4d(sK + c * kBoxBytes, &tk, &bar.fix_full, c * 64, kt * kT, h, b);
+        for (int c = 0; c < NVB; ++c) tma_load_4d(sV + c * kBoxBytes, &tv, &bar.fix_full, c * 64, kt * kT, h, b);
+        for (int qs = 0; qs < nq64; ++qs, ++it) {
+          const uint32_t s = it % NS;
+          mbar_wait(&bar.empty[s], ((it / NS) & 1) ^ 1, 22);
+          mbar_arrive_expect_tx(&bar.full[s], C::kStage);
+          uint8_t* st = sRing + s * C::kStage;
+          for (int c = 0; c < NQB; ++c)
+            tma_load_4d(st + c * kBox64, &tq64, &bar.full[s], c * 64, qs * 64, h, p.q_bcast ? 0 : b);
+          for (int c = 0; c < NVB; ++c)
+            tma_load_4d(st + (NQB + c) * kBox64, &tdo64, &bar.full[s], c * 64, qs * 64, h, b);
         }
       }
-    };
-    auto issue_dp = [&](uint32_t i) {  // dP = dO_j V_t^T into dP buffer i & 1
-      if (leader) {
-        const uint64_t db = make_smem_desc(vring(i), 16, 1024);
-#pragma unroll
-        for (int kk = 0; kk < DV / 16; ++kk) {
-          const uint64_t off = (uint64_t)(((kk >> 2) * kBoxBytes + (kk & 3) * 32) >> 4);
-          mma_ss(tmem + C::kColP + (i & 1u) * 128u, dDO + off, db + off, idesc_s, kk > 0 ? 1u : 0u);
-        }
-      }
-    };
-    auto issue_dq = [&](uint32_t i, bool acc) {  // dQ += dS(TMEM) K_t   (K_t read MN-major)
-      if (leader) {
-        const uint64_t db = make_smem_desc(kring(i), kBoxBytes, 1024);
-#pragma unroll
-        for (int kk = 0; kk < kT / 16; ++kk)
-          mma_ts(tmem + C::kColDQ, tmem + C::kColP + (i & 1u) * 128u + (uint32_t)((kk >> 2) * 64 + (kk & 3) * 8),
-                 db + (uint64_t)((kk * 2048) >> 4), idesc_dq, (acc || kk > 0) ? 1u : 0u);
-      }
-    };
-    auto commit = [&](uint64_t* bp) {
-      if (leader) tc_commit(bp);
-    };
-
-    const int nt = t1 - t0;
-    mbar_wait(&bar.q_full, 0u, 11);
-    mbar_wait(&bar.k_full[0], 0u, 12);
-    tc_fence_after_sync();
-    issue_s(0);
-    commit(&bar.s_full);
-    mbar_wait(&bar.v_full[0], 0u, 17);
-    tc_fence_after_sync();
-    issue_dp(0);
-    commit(&bar.dp_full[0]);
-    commit(&bar.v_empty[0]);
-    for (int i = 0; i < nt; ++i) {
-      const uint32_t ui = (uint32_t)i;
-      if (i + 1 < nt) {
-        const uint32_t un = ui + 1;
-        mbar_wait(&bar.s_free, ui & 1u, 13);  // S_i is in the softmax warps' registers
-        mbar_wait(&bar.k_full[un % C::kKS], (un / C::kKS) & 1u, 14);
-        tc_fence_after_sync();
-        issue_s(un);
-        commit(&bar.s_full);
-        mbar_wait(&bar.v_full[un % C::kVS], (un / C::kVS) & 1u, 18);
-        tc_fence_after_sync();
-        issue_dp(un);  // the other dP buffer: its dS was consumed by dQ(i-1), issued before
-        commit(&bar.dp_full[un & 1u]);
-        commit(&bar.v_empty[un % C::kVS]);
-      }
-      mbar_wait(&bar.ds_ready, ui & 1u, 15);
-      tc_fence_after_sync();
-      issue_dq(ui, i > 0);
-      commit(&bar.k_empty[ui % C::kKS]);
     }
-    commit(&bar.dq_full);
+    return;
   }
 
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == kMmaWarp) {
-    tc_fence_after_sync();
-    tmem_dealloc(bar.tmem_base, 512);
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// kernel 3: forward WITH attention dropout (training).  The fused inference/forward kernel has already produced the row
-// statistics; this pass recomputes S = Q K^T per tile, forms the NORMALISED probabilities 2^(t + nlse) directly (no
-// running maximum: partial sums over key ranges simply add), applies the counter-based dropout mask and accumulates
-// O += dropout(P) V.  Same skeleton as the dQ kernel: query-tile outer, K and V through their own TMA rings, S double
-// buffered in TMEM (P overwrites its S), one fp32 vector reduction per output element per CTA.
-// ---------------------------------------------------------------------------------------------------------------
-template <int DQK, int DV>
-struct Cfg3 {
-  static constexpr int kQB = DQK / 64, kVB = DV / 64;
-  static constexpr int kKBytes = kQB * kBoxBytes, kVBytes = kVB * kBoxBytes;
-  static constexpr int kKS = 3;
-  static constexpr int kAvail = 232448 - 1024 - 512 - kKBytes - kKS * kKBytes;
-  static constexpr int kVS = kAvail / kVBytes >= 3 ? 3 : 2;
-  static constexpr int kOffQ = 0;
-  static constexpr int kOffKRing = kKBytes;
-  static constexpr int kOffVRing = kOffKRing + kKS * kKBytes;
-  static constexpr int kOffBar = kOffVRing + kVS * kVBytes;
-  static constexpr int kNeed = kOffBar + 512 + 1024;
-  static constexpr int kSmem = kNeed > 120 * 1024 ? kNeed : 120 * 1024;
-  static constexpr uint32_t kColO = 256;  // S buffers at 0 and 128
-};
-
-struct Bars3 {
-  uint64_t q_full;
-  uint64_t k_full[3], k_empty[3], v_full[3], v_empty[3];
-  uint64_t s_full[2], p_ready[2];
-  uint64_t o_full;
-  uint32_t tmem_base;
-};
-
-template <bool BF16, bool MASKED>
-__device__ __forceinline__ void fwd_drop_tile(Bars3& bar, uint32_t i_t, uint32_t tS, const BwdParams& p, float nlse,
-                                              float fillp, uint32_t w0, uint32_t w1, int cmax, int oob_from,
-                                              uint32_t dh1, uint32_t qsh, uint32_t k0) {
-  const float2 sc2 = make_float2(p.scale_log2, p.scale_log2), nl2 = make_float2(nlse, nlse);
-  const uint32_t buf = i_t & 1u;
-  uint32_t s[64];
-  uint32_t pk[32];
-  mbar_wait(&bar.s_full[buf], (i_t >> 1) & 1u, 40);
-  tc_fence_after_sync();
-  tmem_ld32(tS, *reinterpret_cast<uint32_t(*)[32]>(&s[0]));
-  tmem_ld32(tS + 32, *reinterpret_cast<uint32_t(*)[32]>(&s[32]));
-  tmem_wait_ld();
+  reg_alloc<232>();
+  const int cw = wg - 1;
+  const int tid = threadIdx.x - 128 * wg;
+  const int warp = tid >> 5, lane = tid & 31;
+  const int kloc = 64 * cw + 16 * warp + (lane >> 2);  // key rows kloc, kloc + 8 of the tile
+  const int cq = 2 * (lane & 3);
+  const uint32_t k_base = smem_u32(sK) + cw * 64 * 128, v_base = smem_u32(sV) + cw * 64 * 128;
+  const uint32_t ring = smem_u32(sRing);
+  uint32_t it = 0, tl = 0;
+  for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++tl) {
+    const int bh = tile / p.nk, kt = tile % p.nk, b = bh / p.H, h = bh % p.H;
+    mbar_wait(&bar.fix_full, tl & 1, 23);
+    float dk[NQB][32], dv[NVB][32];
 #pragma unroll
-  for (int i = 0; i < 64; i += 2) {
-    const float2 x = fma2(make_float2(__uint_as_float(s[i]), __uint_as_float(s[i + 1])), sc2, nl2);
-    float p0 = ex2(x.x), p1 = ex2(x.y);
-    if (MASKED) {
-      const uint32_t word = i < 32 ? w0 : w1;
-      if (((word >> (i & 31)) & 1u) || i > cmax) p0 = fillp;
-      if (((word >> ((i + 1) & 31)) & 1u) || i + 1 > cmax) p1 = fillp;
-      if (i >= oob_from) p0 = 0.f;
-      if (i + 1 >= oob_from) p1 = 0.f;
-    }
-    const uint32_t bits = drop_finish(dh1, drop_kside(p.seed_hi, k0 + (uint32_t)i));
-    p0 = (((bits >> qsh) & 0xffu) >= p.drop_thresh) ? p0 * p.drop_rp : 0.f;
-    p1 = (((bits >> (qsh + 8u)) & 0xffu) >= p.drop_thresh) ? p1 * p.drop_rp : 0.f;
-    pk[i >> 1] = pack2(p0, p1, BF16);
-  }
-  tmem_st32(tS, pk);  // dropout(P) (16-bit) over the first 32 of this warp's 64 S columns
-  tmem_wait_st();
-  tc_fence_before_sync();
-  warp_arrive(&bar.p_ready[buf]);
-}
-
-template <int DQK, int DV, bool BF16>
-__global__ void __launch_bounds__(kThreads, 1)
-fwd_drop_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                const __grid_constant__ CUtensorMap tmap_v, const BwdParams p) {
-  using C = Cfg3<DQK, DV>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  Bars3& bar = *reinterpret_cast<Bars3*>(smem + C::kOffBar);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int j = blockIdx.x % p.nq;
-  const int sp = (blockIdx.x / p.nq) % p.splits;
-  const int bh = blockIdx.x / (p.nq * p.splits);
-  const int h = bh % p.H, b = bh / p.H;
-  const int t0 = sp * p.tiles_per_split;
-  const int t1 = min(p.nk, t0 + p.tiles_per_split);
-
-  if (threadIdx.x == 0) {
-    mbar_init(&bar.q_full, 1);
-    for (int i = 0; i < 3; ++i) {
-      mbar_init(&bar.k_full[i], 1);
-      mbar_init(&bar.k_empty[i], 1);
-      mbar_init(&bar.v_full[i], 1);
-      mbar_init(&bar.v_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&bar.s_full[i], 1);
-      mbar_init(&bar.p_ready[i], 8);
-    }
-    mbar_init(&bar.o_full, 1);
-    fence_mbar_init();
-  }
-  if (warp == kMmaWarp) {
-    tmem_alloc(&bar.tmem_base, 512);
-    tmem_relinquish();
-  }
-  if (warp == kTmaWarp && lane == 0) {
-    tma_prefetch_desc(&tmap_q);
-    tma_prefetch_desc(&tmap_k);
-    tma_prefetch_desc(&tmap_v);
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-
-  if (warp < 8) {
-    reg_alloc<208>();
-    // ===== softmax / dropout: thread = query row, this warp's half of the 128 key columns =====
-    const int quarter = warp & 3, half = warp >> 2;
-    const int r = quarter * 32 + lane;
-    const int nrow = j * kT + r;
-    const uint32_t lanef = (uint32_t)(quarter * 32) << 16;
-    const uint32_t tS0 = bar.tmem_base + lanef + (uint32_t)(half * 64);
-    const float* blk = p.stats + (((size_t)b * p.H + h) * (2 * p.nq) + (size_t)(nrow >> 6)) * (kStatsBytes / 4);
-    const float nlse = blk[stat_nlse_idx(r & 63)], fillp = blk[stat_fillp_idx(r & 63)];
-    const uint32_t dh1 = drop_qside(p.seed_lo, drop_qword((uint32_t)bh, (uint32_t)nrow));
-    const uint32_t qsh = ((uint32_t)nrow & 1u) * 16u;
-    for (int t = t0; t < t1; ++t) {
-      const uint32_t i_t = (uint32_t)(t - t0);
-      const uint32_t tS = tS0 + (i_t & 1u) * 128u;
-      const int k0 = t * kT + half * 64;
-      uint32_t w0 = 0u, w1 = 0u;
-      bool tile_masked = (t * kT + kT > p.M);
-      if (p.pad_bits != nullptr) {
-        const uint4 mw = *reinterpret_cast<const uint4*>(p.pad_bits + (size_t)b * p.pad_wpr + (size_t)t * 4);
-        w0 = half == 0 ? mw.x : mw.z;
-        w1 = half == 0 ? mw.y : mw.w;
-        tile_masked = tile_masked || ((mw.x | mw.y | mw.z | mw.w) != 0u);
-      }
-      const bool masked = tile_masked || (p.causal && (t * kT + kT - 1 > j * kT + p.cshift));
-      const int cmax = p.causal ? (nrow + p.cshift - k0) : 0x7fffffff;
-      const int oob_from = p.M - k0;
-      if (!masked)
-        fwd_drop_tile<BF16, false>(bar, i_t, tS, p, nlse, fillp, 0u, 0u, 0, 0, dh1, qsh, (uint32_t)k0);
-      else
-        fwd_drop_tile<BF16, true>(bar, i_t, tS, p, nlse, fillp, w0, w1, cmax, oob_from, dh1, qsh, (uint32_t)k0);
-    }
-    // ---- add this CTA's part of the output into the fp32 buffer ----
-    mbar_wait(&bar.o_full, 0u, 41);
-    tc_fence_after_sync();
-    {
-      constexpr int kCols = DV / 2;
-      const uint32_t tO = bar.tmem_base + lanef + C::kColO + (uint32_t)(half * kCols);
-      float* dst = p.o32 + ((size_t)b * p.N + (size_t)nrow) * ((size_t)p.H * p.dv) + (size_t)h * p.dv + (size_t)half * kCols;
+    for (int c = 0; c < NQB; ++c)
 #pragma unroll
-      for (int ch = 0; ch < kCols / 32; ++ch) {
-        uint32_t a[32];
-        tmem_ld32(tO + ch * 32, a);
-        tmem_wait_ld();
-        if (nrow < p.N) {
+      for (int i = 0; i < 32; ++i) dk[c][i] = 0.f;
 #pragma unroll
-          for (int gq = 0; gq < 8; ++gq) {
-            const int c = half * kCols + ch * 32 + gq * 4;
-            if (c < p.dv)
-              red_add_v4(dst + ch * 32 + gq * 4, __uint_as_float(a[gq * 4 + 0]), __uint_as_float(a[gq * 4 + 1]),
-                         __uint_as_float(a[gq * 4 + 2]), __uint_as_float(a[gq * 4 + 3]));
+    for (int c = 0; c < NVB; ++c)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) dv[c][i] = 0.f;
+    const int jrow[2] = {kt * kT + kloc, kt * kT + kloc + 8};
+    for (int qs = 0; qs < nq64; ++qs, ++it) {
+      const uint32_t s = it % NS;
+      const uint32_t stq = ring + s * C::kStage, stdo = stq + NQB * kBox64;
+      mbar_wait(&bar.full[s], (it / NS) & 1, 24);
+      float st[32], dpt[32];
+      wgmma_fence();
+#pragma unroll
+      for (int c = 0; c < NQB; ++c)
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk)
+          wgmma_ss<64, BF16>(st, make_desc(k_base + c * kBoxBytes + kk * 32), make_desc(stq + c * kBox64 + kk * 32), (c | kk) != 0);
+#pragma unroll
+      for (int c = 0; c < NVB; ++c)
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk)
+          wgmma_ss<64, BF16>(dpt, make_desc(v_base + c * kBoxBytes + kk * 32), make_desc(stdo + c * kBox64 + kk * 32), (c | kk) != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(st);
+      fence_regs(dpt);
+      const float* blk = p.stats + ((int64_t)bh * (p.Npad / 64) + qs) * (kStatsBytes / 4);
+      uint32_t pa[4][4], da[4][4];
+#pragma unroll
+      for (int g = 0; g < 8; ++g) {
+        float pv[4], dsv[4];
+#pragma unroll
+        for (int e4 = 0; e4 < 4; ++e4) {
+          const int i = e4 >> 1, e = e4 & 1;
+          const int qc = 8 * g + cq + e;
+          const int n = qs * 64 + qc, j = jrow[i];
+          const float nlse = blk[stat_nlse_idx(qc)], delta = blk[stat_delta_idx(qc)], fillp = blk[stat_fillp_idx(qc)];
+          const bool oob = j >= p.M || n >= p.N;
+          const bool filled = !oob && filled_key(p, b, j, n);
+          float P = oob ? 0.f : (filled ? fillp : ex2(fmaf(st[4 * g + e4], p.scale_log2, nlse)));
+          float dP = dpt[4 * g + e4];
+          if (p.drop_thresh) {
+            const bool keep = drop_keep(drop_bits(p.seed_lo, p.seed_hi, (uint32_t)bh, (uint32_t)n, (uint32_t)j), n, j, p.drop_thresh);
+            dP = keep ? dP * p.drop_rp : 0.f;
+            pv[e4] = keep ? P * p.drop_rp : 0.f;
+          } else {
+            pv[e4] = P;
           }
+          dsv[e4] = (oob || filled) ? 0.f : P * (dP - delta);
         }
+        pa[g >> 1][(g & 1) * 2 + 0] = pack2(pv[0], pv[1], BF16);
+        pa[g >> 1][(g & 1) * 2 + 1] = pack2(pv[2], pv[3], BF16);
+        da[g >> 1][(g & 1) * 2 + 0] = pack2(dsv[0], dsv[1], BF16);
+        da[g >> 1][(g & 1) * 2 + 1] = pack2(dsv[2], dsv[3], BF16);
       }
-    }
-  } else {
-    reg_dealloc<88>();
-  }
-
-  if (warp == kTmaWarp) {
-    const bool leader = elect_one();
-    if (leader) {
-      mbar_arrive_expect_tx(&bar.q_full, (uint32_t)C::kKBytes);
+      wgmma_fence();
 #pragma unroll
-      for (int bx = 0; bx < C::kQB; ++bx)
-        tma_load_4d(smem + C::kOffQ + bx * kBoxBytes, &tmap_q, &bar.q_full, bx * 64, j * kT, h, p.q_bcast ? 0 : b);
-    }
-    for (int t = t0; t < t1; ++t) {
-      const uint32_t it = (uint32_t)(t - t0), slot = it % C::kKS;
-      mbar_wait(&bar.k_empty[slot], ((it / C::kKS) & 1u) ^ 1u, 42);
-      if (leader) {
-        uint8_t* st = smem + C::kOffKRing + slot * C::kKBytes;
-        mbar_arrive_expect_tx(&bar.k_full[slot], (uint32_t)C::kKBytes);
+      for (int c = 0; c < NVB; ++c)
 #pragma unroll
-        for (int bx = 0; bx < C::kQB; ++bx)
-          tma_load_4d(st + bx * kBoxBytes, &tmap_k, &bar.k_full[slot], bx * 64, t * kT, h, b);
-      }
-    }
-  } else if (warp == kTmaWarp + 2) {
-    const bool leader = elect_one();
-    for (int t = t0; t < t1; ++t) {
-      const uint32_t it = (uint32_t)(t - t0), slot = it % C::kVS;
-      mbar_wait(&bar.v_empty[slot], ((it / C::kVS) & 1u) ^ 1u, 43);
-      if (leader) {
-        uint8_t* st = smem + C::kOffVRing + slot * C::kVBytes;
-        mbar_arrive_expect_tx(&bar.v_full[slot], (uint32_t)C::kVBytes);
+        for (int kk = 0; kk < 4; ++kk) wgmma_rs<64, BF16>(dv[c], pa[kk], make_desc(stdo + c * kBox64 + kk * 2048));
 #pragma unroll
-        for (int bx = 0; bx < C::kVB; ++bx)
-          tma_load_4d(st + bx * kBoxBytes, &tmap_v, &bar.v_full[slot], bx * 64, t * kT, h, b);
-      }
-    }
-  } else if (warp == kMmaWarp) {
-    const bool leader = elect_one();
-    constexpr uint32_t idesc_s = make_idesc(kT, kT, BF16, false);
-    constexpr uint32_t idesc_pv = make_idesc(kT, DV, BF16, true);
-    const uint32_t tmem = bar.tmem_base;
-    const uint64_t dQ = make_smem_desc(smem_u32(smem + C::kOffQ), 16, 1024);
-    auto issue_s = [&](uint32_t i) {  // S = Q_j K_t^T into S buffer i & 1
-      if (leader) {
-        const uint64_t db = make_smem_desc(smem_u32(smem + C::kOffKRing + (i % C::kKS) * C::kKBytes), 16, 1024);
+      for (int c = 0; c < NQB; ++c)
 #pragma unroll
-        for (int kk = 0; kk < DQK / 16; ++kk) {
-          const uint64_t off = (uint64_t)(((kk >> 2) * kBoxBytes + (kk & 3) * 32) >> 4);
-          mma_ss(tmem + (i & 1u) * 128u, dQ + off, db + off, idesc_s, kk > 0 ? 1u : 0u);
+        for (int kk = 0; kk < 4; ++kk) wgmma_rs<64, BF16>(dk[c], da[kk], make_desc(stq + c * kBox64 + kk * 2048));
+      wgmma_commit();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int c = 0; c < NVB; ++c) fence_regs(dv[c]);
+#pragma unroll
+      for (int c = 0; c < NQB; ++c) fence_regs(dk[c]);
+      warp_arrive(&bar.empty[s]);
+    }
+    warp_arrive(&bar.fix_empty);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int j = jrow[i];
+      if (j >= p.M) continue;
+      T* krow = reinterpret_cast<T*>(p.dk) + (int64_t)b * p.dk_sb + (int64_t)j * p.dk_sm + (int64_t)h * p.dk_sh;
+      T* vrow = reinterpret_cast<T*>(p.dv_out) + (int64_t)b * p.dv_sb + (int64_t)j * p.dv_sm + (int64_t)h * p.dv_sh;
+#pragma unroll
+      for (int c = 0; c < NQB; ++c)
+#pragma unroll
+        for (int g = 0; g < 8; ++g) {
+          const int col = c * 64 + 8 * g + cq;
+          if (col < p.dqk)
+            *reinterpret_cast<uint32_t*>(krow + col) = pack2(dk[c][4 * g + 2 * i] * p.scale, dk[c][4 * g + 2 * i + 1] * p.scale, BF16);
         }
-      }
-    };
-    auto issue_pv = [&](uint32_t i, bool acc) {  // O += dropout(P)(TMEM) V_t   (V_t read MN-major)
-      if (leader) {
-        const uint64_t db = make_smem_desc(smem_u32(smem + C::kOffVRing + (i % C::kVS) * C::kVBytes), kBoxBytes, 1024);
 #pragma unroll
-        for (int kk = 0; kk < kT / 16; ++kk)
-          mma_ts(tmem + C::kColO, tmem + (i & 1u) * 128u + (uint32_t)((kk >> 2) * 64 + (kk & 3) * 8),
-                 db + (uint64_t)((kk * 2048) >> 4), idesc_pv, (acc || kk > 0) ? 1u : 0u);
-      }
-    };
-    auto commit = [&](uint64_t* bp) {
-      if (leader) tc_commit(bp);
-    };
-    const int nt = t1 - t0;
-    mbar_wait(&bar.q_full, 0u, 44);
-    mbar_wait(&bar.k_full[0], 0u, 45);
-    tc_fence_after_sync();
-    issue_s(0);
-    commit(&bar.s_full[0]);
-    commit(&bar.k_empty[0]);
-    for (int i = 0; i < nt; ++i) {
-      const uint32_t ui = (uint32_t)i;
-      if (i + 1 < nt) {
-        const uint32_t un = ui + 1;  // its S buffer held P(i-1), consumed by PV(i-1) which is ahead in the pipe
-        mbar_wait(&bar.k_full[un % C::kKS], (un / C::kKS) & 1u, 46);
-        tc_fence_after_sync();
-        issue_s(un);
-        commit(&bar.s_full[un & 1u]);
-        commit(&bar.k_empty[un % C::kKS]);
-      }
-      mbar_wait(&bar.p_ready[ui & 1u], (ui >> 1) & 1u, 47);
-      mbar_wait(&bar.v_full[ui % C::kVS], (ui / C::kVS) & 1u, 48);
-      tc_fence_after_sync();
-      issue_pv(ui, i > 0);
-      commit(&bar.v_empty[ui % C::kVS]);
+      for (int c = 0; c < NVB; ++c)
+#pragma unroll
+        for (int g = 0; g < 8; ++g) {
+          const int col = c * 64 + 8 * g + cq;
+          if (col < p.dv) *reinterpret_cast<uint32_t*>(vrow + col) = pack2(dv[c][4 * g + 2 * i], dv[c][4 * g + 2 * i + 1], BF16);
+        }
     }
-    commit(&bar.o_full);
   }
+}
 
-  tc_fence_before_sync();
+// FWD = false: dQ += scale * dS K, reduced into p.dq32.   FWD = true: O += dropout(P) V, reduced into p.o32.
+template <int NQB, int NVB, bool BF16, bool FWD>
+__global__ void __launch_bounds__(kThreads, 1)
+bwd_dq_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
+              const __grid_constant__ CUtensorMap tv, const __grid_constant__ CUtensorMap tdo, const BwdParams p) {
+  using C = Cfg2<NQB, NVB>;
+  constexpr int NS = C::kSlots;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sQ = smem;
+  uint8_t* sdO = smem + NQB * kBoxBytes;
+  uint8_t* sRing = smem + C::kQBytes;
+  BwdBarriers& bar = *reinterpret_cast<BwdBarriers*>(sRing + NS * C::kStage);
+  const int wg = threadIdx.x / 128;
+  const int unit = blockIdx.x / p.splits, split = blockIdx.x % p.splits;
+  const int bh = unit / p.nq, qt = unit % p.nq, b = bh / p.H, h = bh % p.H;
+  const int kt0 = split * p.tiles_per_split, kt1 = min(p.nk, kt0 + p.tiles_per_split);
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < NS; ++s) {
+      mbar_init(&bar.full[s], 1);
+      mbar_init(&bar.empty[s], 8);
+    }
+    mbar_init(&bar.fix_full, 1);
+    fence_mbar_init();
+  }
   __syncthreads();
-  if (warp == kMmaWarp) {
-    tc_fence_after_sync();
-    tmem_dealloc(bar.tmem_base, 512);
+
+  if (wg == 0) {
+    reg_dealloc<40>();
+    if (threadIdx.x == 0) {
+      mbar_arrive_expect_tx(&bar.fix_full, (FWD ? NQB : NQB + NVB) * kBoxBytes);
+      for (int c = 0; c < NQB; ++c) tma_load_4d(sQ + c * kBoxBytes, &tq, &bar.fix_full, c * 64, qt * kT, h, p.q_bcast ? 0 : b);
+      if (!FWD)
+        for (int c = 0; c < NVB; ++c) tma_load_4d(sdO + c * kBoxBytes, &tdo, &bar.fix_full, c * 64, qt * kT, h, b);
+      uint32_t it = 0;
+      for (int kt = kt0; kt < kt1; ++kt, ++it) {
+        const uint32_t s = it % NS;
+        mbar_wait(&bar.empty[s], ((it / NS) & 1) ^ 1, 31);
+        mbar_arrive_expect_tx(&bar.full[s], C::kStage);
+        uint8_t* st = sRing + s * C::kStage;
+        for (int c = 0; c < NQB; ++c) tma_load_4d(st + c * kBoxBytes, &tk, &bar.full[s], c * 64, kt * kT, h, b);
+        for (int c = 0; c < NVB; ++c) tma_load_4d(st + (NQB + c) * kBoxBytes, &tv, &bar.full[s], c * 64, kt * kT, h, b);
+      }
+    }
+    return;
+  }
+
+  reg_alloc<232>();
+  const int cw = wg - 1;
+  const int tid = threadIdx.x - 128 * wg;
+  const int warp = tid >> 5, lane = tid & 31;
+  const int qloc = 64 * cw + 16 * warp + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  const uint32_t q_base = smem_u32(sQ) + cw * 64 * 128, do_base = smem_u32(sdO) + cw * 64 * 128;
+  const uint32_t ring = smem_u32(sRing);
+  int nrow[2];
+  float nlse[2], delta[2], fillp[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    nrow[i] = qt * kT + qloc + 8 * i;
+    const float* blk = p.stats + ((int64_t)bh * (p.Npad / 64) + nrow[i] / 64) * (kStatsBytes / 4);
+    const int r = nrow[i] % 64;
+    nlse[i] = blk[stat_nlse_idx(r)];
+    delta[i] = blk[stat_delta_idx(r)];
+    fillp[i] = blk[stat_fillp_idx(r)];
+  }
+  constexpr int NA = FWD ? NVB : NQB;  // accumulator boxes: O (v channels) or dQ (qk channels)
+  float acc[NA][32];
+#pragma unroll
+  for (int c = 0; c < NA; ++c)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
+  mbar_wait(&bar.fix_full, 0, 32);
+  uint32_t it = 0;
+  for (int kt = kt0; kt < kt1; ++kt, ++it) {
+    const uint32_t s = it % NS;
+    const uint32_t stk = ring + s * C::kStage, stv = stk + NQB * kBoxBytes;
+    mbar_wait(&bar.full[s], (it / NS) & 1, 33);
+    float sc[64], dp[FWD ? 1 : 64];
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < NQB; ++c)
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)
+        wgmma_ss<128, BF16>(sc, make_desc(q_base + c * kBoxBytes + kk * 32), make_desc(stk + c * kBoxBytes + kk * 32), (c | kk) != 0);
+    if constexpr (!FWD) {
+#pragma unroll
+      for (int c = 0; c < NVB; ++c)
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk)
+          wgmma_ss<128, BF16>(dp, make_desc(do_base + c * kBoxBytes + kk * 32), make_desc(stv + c * kBoxBytes + kk * 32), (c | kk) != 0);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(sc);
+    if constexpr (!FWD) fence_regs(dp);
+    uint32_t a[8][4];
+#pragma unroll
+    for (int g = 0; g < 16; ++g) {
+      float val[4];
+#pragma unroll
+      for (int e4 = 0; e4 < 4; ++e4) {
+        const int i = e4 >> 1, e = e4 & 1;
+        const int j = kt * kT + 8 * g + cq + e, n = nrow[i];
+        const bool oob = j >= p.M || n >= p.N;
+        const bool filled = !oob && filled_key(p, b, j, n);
+        const float P = oob ? 0.f : (filled ? fillp[i] : ex2(fmaf(sc[4 * g + e4], p.scale_log2, nlse[i])));
+        bool keep = true;
+        if (p.drop_thresh)
+          keep = drop_keep(drop_bits(p.seed_lo, p.seed_hi, (uint32_t)bh, (uint32_t)n, (uint32_t)j), n, j, p.drop_thresh);
+        if constexpr (FWD) {
+          val[e4] = keep ? P * p.drop_rp : 0.f;
+        } else {
+          const float dP = keep ? dp[4 * g + e4] * p.drop_rp : 0.f;
+          val[e4] = (oob || filled) ? 0.f : P * (dP - delta[i]);
+        }
+      }
+      a[g >> 1][(g & 1) * 2 + 0] = pack2(val[0], val[1], BF16);
+      a[g >> 1][(g & 1) * 2 + 1] = pack2(val[2], val[3], BF16);
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < NA; ++c)
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk)
+        wgmma_rs<64, BF16>(acc[c], a[kk], make_desc((FWD ? stv : stk) + c * kBoxBytes + kk * 2048));
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int c = 0; c < NA; ++c) fence_regs(acc[c]);
+    warp_arrive(&bar.empty[s]);
+  }
+  // reduce this CTA's share into the fp32 buffer
+  const int width = FWD ? p.dv : p.dqk;
+  const float mul = FWD ? 1.f : p.scale;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const int n = nrow[i];
+    if (n >= p.N) continue;
+    const int bq = FWD ? b : (p.q_bcast ? 0 : b);
+    float* dst = (FWD ? p.o32 : p.dq32) + (((int64_t)bq * p.N + n) * p.H + h) * width;
+#pragma unroll
+    for (int c = 0; c < NA; ++c)
+#pragma unroll
+      for (int g = 0; g < 8; ++g) {
+        const int col = c * 64 + 8 * g + cq;
+        if (col < width) {
+          atomicAdd(dst + col, acc[c][4 * g + 2 * i] * mul);
+          atomicAdd(dst + col + 1, acc[c][4 * g + 2 * i + 1] * mul);
+        }
+      }
   }
 }
 
@@ -1318,7 +575,7 @@ int bwd_tmap(CUtensorMap* tm, const void* base, int dtype, int channels, int row
 
 inline size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
 
-// watchdog record of THIS translation unit's kernels (mbar_wait in pcv_sm100.cuh): mapped pinned host memory
+// watchdog record of THIS translation unit's kernels (mbar_wait in pcv_sm90.cuh): mapped pinned host memory
 uint32_t* g_bwd_diag_host = nullptr;
 std::mutex g_bwd_diag_mu;
 int g_bwd_diag_dev = -1;
@@ -1332,7 +589,7 @@ int ensure_bwd_diag(int dev) {
   }
   uint32_t* dptr = nullptr;
   PCV_CHECK_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&dptr), g_bwd_diag_host, 0));
-  PCV_CHECK_CUDA(cudaMemcpyToSymbol(sm100::g_wait_diag, &dptr, sizeof(dptr)));
+  PCV_CHECK_CUDA(cudaMemcpyToSymbol(sm90::g_wait_diag, &dptr, sizeof(dptr)));
   g_bwd_diag_dev = dev;
   return PCV_OK;
 }
@@ -1373,10 +630,10 @@ template <int DQK, int DV, bool BF16>
 int launch_bwd_kernels(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const CUtensorMap& tdo,
                        const CUtensorMap& tq64, const CUtensorMap& tdo64, const BwdParams& p, int sms,
                        cudaStream_t stream) {
-  using C1 = Cfg1<DQK, DV>;
-  using C2 = Cfg2<DQK, DV>;
-  auto k1 = bwd_dkdv_kernel<DQK, DV, BF16>;
-  auto k2 = bwd_dq_kernel<DQK, DV, BF16>;
+  using C1 = Cfg1<DQK / 64, DV / 64>;
+  using C2 = Cfg2<DQK / 64, DV / 64>;
+  auto k1 = bwd_dkdv_kernel<DQK / 64, DV / 64, BF16>;
+  auto k2 = bwd_dq_kernel<DQK / 64, DV / 64, BF16, false>;
   // per device and cheap: set on every launch rather than caching per process
   PCV_CHECK_CUDA(cudaFuncSetAttribute(k1, cudaFuncAttributeMaxDynamicSharedMemorySize, C1::kSmem));
   PCV_CHECK_CUDA(cudaFuncSetAttribute(k2, cudaFuncAttributeMaxDynamicSharedMemorySize, C2::kSmem));
@@ -1416,7 +673,7 @@ bool attn_bwd_supported(const pcv_attn_bwd_params& a, const char** why) {
   int dev = 0, major = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return no("no CUDA device");
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-  if (major != 10) return no("needs an sm_100 device");
+  if (major != 9) return no("needs an sm_90 device");
   return true;
 }
 
@@ -1571,11 +828,11 @@ FwdDropLayout fwd_drop_layout(const pcv_attn_params& a) {
 template <int DQK, int DV, bool BF16>
 int launch_fwd_drop_kernel(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const BwdParams& p,
                            cudaStream_t stream) {
-  using C3 = Cfg3<DQK, DV>;
-  auto k3 = fwd_drop_kernel<DQK, DV, BF16>;
+  using C3 = Cfg2<DQK / 64, DV / 64>;
+  auto k3 = bwd_dq_kernel<DQK / 64, DV / 64, BF16, true>;
   PCV_CHECK_CUDA(cudaFuncSetAttribute(k3, cudaFuncAttributeMaxDynamicSharedMemorySize, C3::kSmem));
   const int grid = p.B * p.H * p.nq * p.splits;
-  k3<<<grid, kThreads, C3::kSmem, stream>>>(tq, tk, tv, p);
+  k3<<<grid, kThreads, C3::kSmem, stream>>>(tq, tk, tv, tv, p);  // no dO in the forward pass
   PCV_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PCV_OK;
@@ -1603,7 +860,7 @@ bool attn_fwd_dropout_supported(const pcv_attn_params& a, float dropout_p, const
   int dev = 0, major = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return no("no CUDA device");
   cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
-  if (major != 10) return no("needs an sm_100 device");
+  if (major != 9) return no("needs an sm_90 device");
   return true;
 }
 

@@ -1,4 +1,4 @@
-// pcv_attn_decode.cu — attention for a handful of query rows against a long key/value cache (sm_100a):
+// pcv_attn_decode.cu — attention for a handful of query rows against a long key/value cache (sm_90a):
 // the Perceiver AR decode step (reference modules.py:146-164 with i = 1 query, j = n cached keys; SURVEY.md
 // §8(f)3).  With N <= 4 queries the two contractions are matrix-vector products: every K and V byte is used once,
 // the tensor cores have nothing to amortise (the 128-row tcgen05 tile would waste 127/128 of its MMA rows) and the
@@ -268,7 +268,7 @@ __global__ void __launch_bounds__(kDecThreads) attn_decode_kernel(const DecParam
 }
 
 int choose_split(const pcv_attn_params& a, int* nsplit, int* keys_per_split) {
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int64_t bh = (int64_t)a.B * a.H;

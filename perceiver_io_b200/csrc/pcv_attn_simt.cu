@@ -1,4 +1,4 @@
-// pcv_attn_simt.cu — shape-generic fused attention forward on the CUDA cores (sm_100a).
+// pcv_attn_simt.cu — shape-generic fused attention forward on the CUDA cores (sm_90a).
 //
 // This is the coverage kernel of the library: any head dim (odd ones included), any strides,
 // fp32 math.  It implements exactly the semantics documented in include/pcv_attn.h
@@ -189,7 +189,7 @@ struct SimtPlan {
 SimtPlan make_plan(const pcv_attn_params& p) {
   SimtPlan pl;
   const int64_t ctas = (int64_t)((p.N + kRowsPerCta - 1) / kRowsPerCta) * p.B * p.H;
-  const int64_t want = 148 * 4;  // ~2 waves at 2 CTAs/SM
+  const int64_t want = 132 * 4;  // ~2 waves at 2 CTAs/SM
   int nsplit = (int)((want + ctas - 1) / ctas);
   const int max_split = (p.M + 255) / 256;
   if (nsplit > max_split) nsplit = max_split;

@@ -1,26 +1,23 @@
-// pcv_attn_tc.cu — fused attention forward on the 5th-generation tensor cores (sm_100a only).
+// pcv_attn_tc.cu — fused attention forward on the Hopper tensor cores (sm_90a, warpgroup MMA).
 //
-//   S = Q K^T  (tcgen05.mma, SS: Q and K tiles in SWIZZLE_128B shared memory, S in TMEM)
-//   P = 2^(S*scale*log2e - m)   (softmax warps: one thread per query row, S read with tcgen05.ld,
-//                                 P written back to TMEM as bf16 over the S columns, tcgen05.st)
-//   O += P V   (tcgen05.mma, TS: P from TMEM, V tile MN-major in shared memory, O in TMEM)
+//   S = Q K^T  (wgmma SS: Q and K boxes in SWIZZLE_128B shared memory, S in registers)
+//   P = 2^(S*scale*log2e - m)   (online softmax in registers, rows shared by the four lanes of a quad)
+//   O += P V   (wgmma RS: P re-used in place as the 16-bit A fragment, V box read MN-major, O in registers)
 //
-// CTA = 2 query tiles of 128 rows of one (batch, head) x a contiguous range of 128-key tiles.
-// Warp roles (384 threads, warps 10-11 idle): warps 0-3 softmax of query tile 0, warps 4-7 softmax of query tile 1,
-// warp 8 (one lane) issues every tcgen05.mma, warp 9 (one lane) issues every TMA load.  While the
-// softmax warps of one query tile exponentiate, the tensor core works on the other tile.
-// TMEM (512 columns): S0 [0,128) S1 [128,256) O0 [256,384) O1 [384,512); P_i aliases S_i[0,64).
-//
-// Online softmax with a lazily updated reference maximum: the exponent reference m only moves when the
-// running row maximum exceeds it by more than 8 (log2 units), so O is rescaled in TMEM rarely; the
-// softmax warp that owns the row does that rescale itself (S_i(j) complete implies P_i V_(j-1) complete
-// because tcgen05.mma executes in issue order).
+// CTA = one 128-row query tile of one (batch, head) x a contiguous range of 128-key tiles; 384 threads:
+// warpgroup 0 is the TMA producer (one lane), warpgroups 1 and 2 each own 64 query rows.
+// CTA-pair variant (PAIR, impl = PCV_IMPL_TCGEN05_PAIR): a 2-CTA cluster takes two adjacent query tiles of the same
+// (b, h) and key range; each CTA loads one 64-key half of every K / V box and multicasts it to both, so the pair
+// reads each key tile from L2 once.  A ring slot is refilled only after the consumers of BOTH CTAs released it.  Q stays in shared
+// memory for the segment; K and V arrive as 128-key x 64-channel boxes through one ring of 16 KB slots guarded
+// by full / empty mbarriers, so every head dim (up to 512 for Q/K) uses the same pipeline.  V is processed in
+// passes of at most 128 channels (one launch per pass) to keep the accumulators in registers.
 //
 // Work distribution is a host-built segment table (stream-K over the key axis): segments that cover a
-// whole (b,h,query-block) write the final output; split ones write (numerator, max, denominator) slots that
+// whole (b,h,query tile) write the final output; split ones write (numerator, max, denominator) slots that
 // tc_combine_kernel merges.  Semantics are those of include/pcv_attn.h (finite mask fill, uniform rows).
 #include "pcv_common.cuh"
-#include "pcv_sm100.cuh"
+#include "pcv_sm90.cuh"
 
 #include <cuda.h>
 #include <cudaTypedefs.h>
@@ -37,41 +34,25 @@
 namespace pcv {
 namespace {
 
-using namespace sm100;
+using namespace sm90;
 
-constexpr int kTileM = 128;            // query rows per tile (UMMA M)
-constexpr int kTileN = 128;            // keys per tile (UMMA N of QK^T, K of PV)
+constexpr int kTileM = 128;              // query rows per CTA tile (two warpgroups of 64)
+constexpr int kTileN = 128;              // keys per tile
 constexpr int kBoxBytes = kTileN * 128;  // one TMA box: 128 rows x 64 16-bit channels, SWIZZLE_128B
-constexpr int kRowsPerUnit = 2 * kTileM;
-constexpr int kThreads = 384;  // 12 warps: 8 softmax + MMA + TMA + 2 idle (fills the 3rd warpgroup for setmaxnreg)
-constexpr int kMmaWarp = 8;
-constexpr int kTmaWarp = 9;
-constexpr float kRescaleThreshold = 8.f;  // log2 units
-#ifndef PCV_PAIR_DEFAULT
-#define PCV_PAIR_DEFAULT 0
-#endif
-constexpr bool kPairByDefault = PCV_PAIR_DEFAULT != 0;  // build-time choice after the A/B measurement (DESIGN.md section 5)
-constexpr int kFlagsPerSlot = 16;          // fix-up flags per slot: one per 32-row warp slice of a unit (<= 512 rows)
-// Column pairs (of every 8) of an optimistic tile whose 2^x runs on the FMA / ALU pipes (exp2_poly2_fast: cubic, relative
-// error 1e-4, far below the bf16 rounding of P) instead of the MUFU pipe, which is co-critical with the tensor pipe in
-// this kernel.  Same-box A/B at the north-star shape (DESIGN.md section 5): 0/8 1234, 2/8 1273, 4/8 1225 TFLOP/s.
-#ifndef PCV_POLY_QUARTERS
-#define PCV_POLY_QUARTERS 2
-#endif
-constexpr int kPolyQuarter = PCV_POLY_QUARTERS;
+constexpr int kThreads = 384;            // producer warpgroup + 2 consumer warpgroups
+constexpr int kMaxDvPass = 128;          // V channels per launch (O accumulators stay in registers)
+constexpr int kSmemLimit = 227 * 1024;
 
 struct Segment {
   int b, h;
-  int q0;      // first query row of the block (multiple of 256)
-  int ntile;   // 1 or 2 active query tiles
+  int q0;      // first query row of the tile
+  int ntile;   // 128-row query tiles of the unit that hold rows < N (plan bookkeeping)
   int t0, t1;  // key tiles [t0, t1)
   int slot;    // >= 0: partial slot index; -1: the segment covers every key tile (final)
-  int unit;    // >= 0: index of the split unit (UnitRec) this segment is a part of; -1: whole key range
+  int unit;    // >= 0: index of the split unit (UnitRec) this segment is a part of (host plan checks); -1: whole key range
 };
 
-constexpr int kOwnerMergeMax = 4;  // split units with at most this many parts are merged by their first part (see epilogue_row)
-
-struct UnitRec {  // a (b,h,query-block) whose key range was split over several segments
+struct UnitRec {  // a (b,h,query tile) whose key range was split over several segments
   int b, h, q0;
   int slot_begin, slot_count;
   int pad_[3];
@@ -99,12 +80,7 @@ struct TcParams {
   const Segment* segs;
   const int* cta_seg_begin;
   int B, H, N, M, dv;
-  int dv_off, dv_pass;              // this launch writes output channels [dv_off, dv_off + dv_pass)
-  int nc128;                        // big-head streaming kernel: number of 128-channel chunks of the qk head dim
-  int nc;                           // big-head kernel: number of 64-channel boxes of the qk head dim
-  int v_boxes;                      // big-head kernel: 64-channel boxes of V in this pass
-  int dqk_pad;                      // big-head kernel: qk head dim rounded up to 16 (K-steps of the ragged last box)
-  int dv_cols;                      // big-head kernel: accumulator columns of this pass (v channels rounded up to 16)
+  int dv_off, dv_pass;       // this launch writes output channels [dv_off, dv_off + dv_pass)
   float scale_log2;
   int causal, causal_shift;  // key j (local) masked for query n iff j > n + causal_shift
   const uint32_t* pad_bits;  // (B, pad_wpr) bit set = padding key; nullptr if no mask
@@ -114,662 +90,20 @@ struct TcParams {
   int64_t osb, osn, osh;
   int write_partial;
   float *fin_o, *fin_m, *fin_l;     // caller's partial state (B,H,N,dv),(B,H,N),(B,H,N)
-  float *slot_o, *slot_m, *slot_l;  // workspace slots [slot][256][DV], [slot][256]
-  // in-kernel fix-up of split units (attn_tc_kernel): the segment that starts at key tile 0 is the LAST segment of
-  // its CTA, all other parts of the unit are FIRST segments of theirs (or whole CTAs) — it finishes last, waits for
-  // the per-warp "rows stored" flags of the other parts and folds their slots into its own accumulator rows while
-  // writing the result, so no separate merge kernel (and no extra pass over the state) is needed.
-  const UnitRec* units;
-  unsigned long long* slot_flags;   // [slot][16]: == fixup_tag once warp w of that part has stored its 32 rows
-  unsigned long long fixup_tag;     // unique per launch (workspace memory is not cleared between launches)
-  int rows_per_unit;                // query rows per work unit: 256 (two tiles per CTA) or 128 (wide-dv / big-head)
-  int slot_rows;                    // row stride of the partial slots (>= rows_per_unit)
-  int optimistic;                   // 1: exponentiate against the current reference, verify the range afterwards
-  int mmaopt;                       // attn_tc_kernel issuer: bit 0 = overlapped barrier probes, bit 1 = deferred kv_empty commits
-  unsigned long long* trace;        // debugging aid (PCV_TRACE=1): clock64 stamps of CTA 0, [role][tile][event]
+  float *slot_o, *slot_m, *slot_l;  // workspace slots [slot][slot_rows][DV], [slot][slot_rows]
+  int rows_per_unit;
+  int slot_rows;
   PeerTail tail;
 };
 
-template <int DQK, int DV>
-struct Cfg {
-  static constexpr int kQBoxes = DQK / 64;
-  static constexpr int kVBoxes = DV / 64;
-  static constexpr int kQTileBytes = kQBoxes * kBoxBytes;
-  static constexpr bool kWide = DV > 128;  // one query tile per CTA: the O accumulator takes TMEM columns [256, 256+DV)
-  static constexpr int kQBytes = (kWide ? 1 : 2) * kQTileBytes;
-  static constexpr int kStageBytes = (DQK > DV ? DQK : DV) / 64 * kBoxBytes;
-  static constexpr int kBarrierBytes = 1024;
-  static constexpr int kMaxSmem = 232448 - 1024;  // leave room for the 1024-byte alignment slack
-  static constexpr int kStagesRaw = (kMaxSmem - kQBytes - kBarrierBytes) / kStageBytes;
-  static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
-  static constexpr int kSmemBytes = kQBytes + kStages * kStageBytes + kBarrierBytes + 1024;
-  static_assert(kStages >= 3, "need at least K_j, V_j, K_(j+1) in flight");
-  static_assert(DQK % 64 == 0 && DV % 64 == 0 && DQK <= 128 && DV <= 256, "padded head dims");
-};
-
-constexpr int kTraceTiles = 48, kTraceEvents = 8, kTraceRoles = 3;
-constexpr int kTraceStamps = kTraceRoles * kTraceTiles * kTraceEvents;
-constexpr int kTraceMaxCtas = 1024;  // after the stamps: [cta][8] = globaltimer start, end, SM id, key tiles, clock64 start, end
-// stamp event `ev` of role `role` for key tile `tile` (CTA 0 only, first kTraceTiles tiles, one lane per role)
-#ifdef PCV_ENABLE_TRACE  // developer build only (make TRACE=1): the stamps cost registers in the softmax loop
-#define PCV_TRACE(pp, role, tile, ev, cond)                                                             \
-  do {                                                                                                  \
-    if ((pp).trace != nullptr && blockIdx.x == 0 && (tile) < kTraceTiles && (cond))                       \
-      (pp).trace[((role) * kTraceTiles + (tile)) * kTraceEvents + (ev)] = (unsigned long long)clock64(); \
-  } while (0)
-// whole-CTA record (thread 0): slot 0 = start, 1 = end (ns, globaltimer), 2 = SM id, 3 = key tiles of the CTA,
-// 4 / 5 = clock64 at start / end (cycles / ns = the SM clock the kernel really ran at)
-#define PCV_TRACE_CTA(pp, slot, value)                                                                 \
-  do {                                                                                                 \
-    if ((pp).trace != nullptr && threadIdx.x == 0 && blockIdx.x < kTraceMaxCtas)                        \
-      (pp).trace[kTraceStamps + blockIdx.x * 8 + (slot)] = (unsigned long long)(value);                 \
-  } while (0)
-#else
-#define PCV_TRACE(pp, role, tile, ev, cond) \
-  do {                                      \
-  } while (0)
-#define PCV_TRACE_CTA(pp, slot, value) \
-  do {                                 \
-  } while (0)
-#endif
-
-struct Barriers {
-  uint64_t q_full, q_empty;
-  uint64_t kv_full[8], kv_empty[8];
-  uint64_t s_full[2], p_full[2], o_full[2], o_empty[2];
-  uint32_t tmem_base;
-};
-
-__device__ __forceinline__ uint32_t pack2(float lo, float hi, bool bf16) {
-  uint32_t r;
-  if (bf16)
-    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
-  else
-    asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
-  return r;
-}
-
 // --------------------------------------------------------------------------------------------------
-// softmax + epilogue role: 128 threads, thread = one query row of tile `wg`
-// --------------------------------------------------------------------------------------------------
-struct RowState {
-  float m_ref;  // exponent reference (log2 domain); trails the running row maximum by at most 8
-  float l;      // running denominator relative to m_ref
-};
-
-struct TileCtx;
-__device__ __forceinline__ void arrive_p_full(Barriers& bar, const TileCtx& c);
-
-struct TileCtx {
-  uint32_t p_full_remote;  // 0: arrive on the local p_full[wg]; else shared::cluster address of the pair leader's p_full[wg]
-  uint64_t* pv_bar;      // non-null: barrier (and parity) to wait on before rescaling O — kernels whose S(j) does not imply PV(j-1) done
-  uint32_t pv_parity;
-  uint32_t tS, tO;    // TMEM addresses (lane field included) of this thread's S / O row
-  int wg, row;
-  int j0;             // first key of the tile
-  int cshift;         // key j (local) is causally masked for this row iff j > cshift
-  uint4 mw;           // padding bits of the 128 keys of the tile
-  bool first_tile;    // no accumulator content yet
-  bool trace_on;
-  int tt;
-  float scale_log2;   // p.scale_log2, kept in a register (a constant-bank load right after the S barrier is latency on the chain)
-};
-
-// P of this thread's row is in TMEM (tcgen05.wait::st + fence done by the caller): tell the MMA issuer
-__device__ __forceinline__ void arrive_p_full(Barriers& bar, const TileCtx& c) {
-  // one arrive per warp (every lane has executed tcgen05.wait::st + the tcgen05 fence before the warp sync):
-  // 4 arrivals per tile instead of 128 serialised updates of one shared-memory word
-  __syncwarp();
-  if ((threadIdx.x & 31) == 0) {
-    if (c.p_full_remote == 0)
-      mbar_arrive(&bar.p_full[c.wg]);
-    else
-      mbar_arrive_cluster_relaxed(c.p_full_remote);  // P is in TMEM (tcgen05.wait::st returned): no memory to release
-  }
-}
-
-// Classic tile (max pass first): first tile of a segment, masked tiles, redo after an optimistic miss.  (Making it
-// __noinline__ to relieve register pressure in the tile loop was measured: -12 %, the context then lives on the stack.)
-template <int DV, bool BF16, bool MASKED>
-__device__ __forceinline__ void softmax_tile(const TcParams& p, Barriers& bar, const TileCtx& c, RowState& st) {
-  uint32_t s[4][32];
-  tmem_ld32(c.tS + 0, s[0]);
-  tmem_ld32(c.tS + 32, s[1]);
-  tmem_ld32(c.tS + 64, s[2]);
-  tmem_ld32(c.tS + 96, s[3]);
-  tmem_wait_ld();
-  PCV_TRACE(p, c.wg, c.tt, 1, c.trace_on);
-
-  float m_tile;
-  float mul = p.scale_log2;  // exponent = s * mul - m_ref
-  if (!MASKED) {
-    // 2-input max on purpose: the compiler's fused 3-input FMNMX3 measured ~8 issue cycles per warp
-    // instruction here (4x slower than FMNMX), which made this pass as long as half the exponent phase
-    float mx0 = -INFINITY, mx1 = -INFINITY, mx2 = -INFINITY, mx3 = -INFINITY;
-#pragma unroll
-    for (int i = 0; i < 32; ++i) {
-      mx0 = max2(mx0, __uint_as_float(s[0][i]));
-      mx1 = max2(mx1, __uint_as_float(s[1][i]));
-      mx2 = max2(mx2, __uint_as_float(s[2][i]));
-      mx3 = max2(mx3, __uint_as_float(s[3][i]));
-    }
-    m_tile = fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3)) * p.scale_log2;
-  } else {
-    // rewrite the scores in place in the log2 domain with the reference's finite fill for padding /
-    // causal keys and -inf (weight exactly 0) for keys beyond the end of the tensor
-    const int oob_from = p.M - c.j0;
-    const int cmax = p.causal ? (c.cshift - c.j0) : 0x7fffffff;
-    float mx = -INFINITY;
-#pragma unroll
-    for (int q4 = 0; q4 < 4; ++q4) {
-      const uint32_t word = q4 == 0 ? c.mw.x : (q4 == 1 ? c.mw.y : (q4 == 2 ? c.mw.z : c.mw.w));
-#pragma unroll
-      for (int i = 0; i < 32; ++i) {
-        const int col = q4 * 32 + i;
-        float tv = __uint_as_float(s[q4][i]) * p.scale_log2;
-        if (((word >> i) & 1u) || col > cmax) tv = kMaskedScore;
-        if (col >= oob_from) tv = -INFINITY;
-        mx = fmaxf(mx, tv);
-        s[q4][i] = __float_as_uint(tv);
-      }
-    }
-    m_tile = mx;
-    mul = 1.f;
-  }
-
-  // lazily move the exponent reference; rescale the accumulator row when it moves
-  const float m_new = fmaxf(st.m_ref, m_tile);
-  float alpha = 1.f;
-  bool moved = false;
-  if (m_new - st.m_ref > kRescaleThreshold) {
-    alpha = ex2(st.m_ref - m_new);
-    st.l *= alpha;
-    st.m_ref = m_new;
-    moved = !c.first_tile;
-  }
-  if (__any_sync(0xffffffffu, moved)) {
-    if (c.pv_bar != nullptr) {
-      mbar_wait(c.pv_bar, c.pv_parity, 15);
-      tc_fence_after_sync();
-    }
-#pragma unroll
-    for (int ch = 0; ch < DV / 32; ++ch) {
-      uint32_t o[32];
-      tmem_ld32(c.tO + ch * 32, o);
-      tmem_wait_ld();
-#pragma unroll
-      for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-      tmem_st32(c.tO + ch * 32, o);
-    }
-  }
-
-  PCV_TRACE(p, c.wg, c.tt, 2, c.trace_on);
-  PCV_TRACE(p, c.wg, c.tt, 3, c.trace_on);
-  float2 sum2 = make_float2(0.f, 0.f);
-  const float2 mul2 = make_float2(mul, mul);
-  const float2 negm2 = make_float2(-st.m_ref, -st.m_ref);
-#pragma unroll
-  for (int half = 0; half < 2; ++half) {
-    uint32_t pk[32];
-#pragma unroll
-    for (int qq = 0; qq < 2; ++qq) {
-      const int q4 = half * 2 + qq;
-#pragma unroll
-      for (int i = 0; i < 32; i += 2) {
-        const float2 x = fma2(make_float2(__uint_as_float(s[q4][i]), __uint_as_float(s[q4][i + 1])), mul2, negm2);
-        const float2 e = make_float2(ex2(x.x), ex2(x.y));
-        sum2 = add2(sum2, e);
-        pk[qq * 16 + (i >> 1)] = pack2(e.x, e.y, BF16);
-      }
-    }
-    tmem_st32(c.tS + half * 32, pk);  // P (16-bit) over S columns [0,64)
-  }
-  PCV_TRACE(p, c.wg, c.tt, 4, c.trace_on);
-  st.l += sum2.x + sum2.y;
-  tmem_wait_st();
-  tc_fence_before_sync();
-  arrive_p_full(bar, c);
-  PCV_TRACE(p, c.wg, c.tt, 5, c.trace_on);
-}
-
-// Largest tile sum of exponentials (relative to the current reference) the optimistic path accepts.  Every P
-// entry is <= the tile sum, so the bound keeps P representable (fp16: 2^15 < 65504) and leaves the fp32
-// denominator / accumulator ~2^80 of headroom (bf16 shares fp32's exponent range, so its bound is only about
-// overflow).  The classic path moves the reference whenever the row maximum leads it by more than
-// kRescaleThreshold, i.e. whenever a tile sum could exceed 128 * 2^8 = 2^15, so a redo always makes progress.
-template <bool BF16>
-__device__ __forceinline__ constexpr float optimistic_limit() {
-  return BF16 ? 1.099511627776e12f /* 2^40 */ : 32768.f /* 2^15 */;
-}
-
-// Optimistic tile: exponentiate against the CURRENT reference maximum while the scores stream in from TMEM —
-// no max pass at all (the fused 3-input max the compiler emits for a side-tracked maximum costs more issue
-// time than the packed adds of the row sum).  The row sum doubles as the range check: if any row of the warp
-// exceeds optimistic_limit(), nothing has been stored yet, the warp returns false and the caller redoes the
-// tile on the classic path (max first, reference moves, accumulator rescaled).  After the first tile of a row
-// that is rare.
-template <int DV, bool BF16, int POLY4>
-__device__ __forceinline__ bool softmax_tile_optimistic(const TcParams& p, Barriers& bar, const TileCtx& c,
-                                                        RowState& st) {
-  uint32_t pk_lo[32], pk_hi[32];  // packed P for key columns [0,64) / [64,128)
-  float2 sum2 = make_float2(0.f, 0.f);
-  const float2 mul2 = make_float2(c.scale_log2, c.scale_log2);
-  const float2 negm2 = make_float2(-st.m_ref, -st.m_ref);
-  uint32_t sa[32], sb[32];
-  tmem_ld32(c.tS + 0, sa);
-  tmem_wait_ld();
-  PCV_TRACE(p, c.wg, c.tt, 1, c.trace_on);
-  PCV_TRACE(p, c.wg, c.tt, 3, c.trace_on);
-
-  // chunk q (32 score columns) -> 16 packed words at dst[off..off+16); the next chunk streams from TMEM
-  // into the other buffer meanwhile
-#define PCV_OPT_CHUNK(cur, nxt, q, dst, off)                                                      \
-  do {                                                                                            \
-    if ((q) < 3) tmem_ld32(c.tS + ((q) + 1) * 32, nxt);                                           \
-    _Pragma("unroll") for (int i = 0; i < 32; i += 2) {                                           \
-      const float s0 = __uint_as_float(cur[i]), s1 = __uint_as_float(cur[i + 1]);                \
-      const float2 x = fma2(make_float2(s0, s1), mul2, negm2);                                    \
-      /* POLY4 of every 8 column pairs go through the FMA-pipe exp2 (compile-time pattern) */     \
-      const float2 e = (((i >> 1) & 7) < POLY4) ? exp2_poly2_fast(x) : make_float2(ex2(x.x), ex2(x.y)); \
-      sum2 = add2(sum2, e);                                                                       \
-      dst[(off) + (i >> 1)] = pack2(e.x, e.y, BF16);                                              \
-    }                                                                                             \
-    if ((q) < 3) tmem_wait_ld();                                                                  \
-  } while (0)
-  PCV_OPT_CHUNK(sa, sb, 0, pk_lo, 0);
-  PCV_OPT_CHUNK(sb, sa, 1, pk_lo, 16);
-  PCV_OPT_CHUNK(sa, sb, 2, pk_hi, 0);
-  PCV_OPT_CHUNK(sb, sa, 3, pk_hi, 16);
-#undef PCV_OPT_CHUNK
-  PCV_TRACE(p, c.wg, c.tt, 4, c.trace_on);
-  const float tsum = sum2.x + sum2.y;
-  if (__any_sync(0xffffffffu, !(tsum <= optimistic_limit<BF16>()))) return false;
-  tmem_st32(c.tS + 0, pk_lo);  // P (16-bit) over S columns [0,64); all of S is in registers by now
-  tmem_st32(c.tS + 32, pk_hi);
-  st.l += tsum;
-  tmem_wait_st();
-  tc_fence_before_sync();
-  arrive_p_full(bar, c);
-  PCV_TRACE(p, c.wg, c.tt, 5, c.trace_on);
-  return true;
-}
-
-__device__ __forceinline__ unsigned long long ld_acquire_gpu_u64(const unsigned long long* p) {
-  unsigned long long v;
-  asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void st_release_gpu_u64(unsigned long long* p, unsigned long long v) {
-  asm volatile("st.release.gpu.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-
-// wait (bounded) until another CTA's warp has published its 32 slot rows; call with the whole warp converged
-__device__ __forceinline__ void wait_slot_rows(const TcParams& p, int slot, int warp_in_unit) {
-  const unsigned long long* f = p.slot_flags + (int64_t)slot * kFlagsPerSlot + warp_in_unit;
-  if ((threadIdx.x & 31) == 0) {
-    uint32_t spins = 0;
-    uint64_t t0 = 0;
-    while (ld_acquire_gpu_u64(f) != p.fixup_tag) {
-      if ((++spins & 0xFFu) == 0) {
-        const uint64_t now = globaltimer_ns();
-        if (t0 == 0) {
-          t0 = now;
-        } else if (now - t0 > kWaitTimeoutNs) {
-          uint32_t* d = g_wait_diag;
-          if (d != nullptr && atomicCAS(d, 0u, 1u) == 0u) {
-            d[1] = 40;
-            d[2] = blockIdx.x;
-            d[3] = threadIdx.x;
-            d[4] = (uint32_t)slot;
-            d[5] = spins;
-            __threadfence_system();
-          }
-          __trap();
-        }
-      }
-    }
-  }
-  __syncwarp();
-}
-
-// O row of this thread (TMEM, `DV` accumulator columns starting at tO) -> global memory: the normalised output,
-// the caller's partial state, or a split-M slot.  Channels [0, dv_pass) of the accumulator map to output channels
-// [dv_off, dv_off + dv_pass) (dv_off > 0 only in the second pass of the big-head kernel).  With FIXUP split units are
-// merged inside the kernel: see `owner` below and fixup_merge.
-template <int DV, bool BF16, bool FIXUP>
-__device__ __forceinline__ void epilogue_row(const TcParams& p, const Segment& seg, uint32_t tO, int n,
-                                             int row_in_unit, float l, float m_ref) {
-  const bool valid = n < p.N;
-  // lightly split units (<= kOwnerMergeMax parts): the part that starts at key tile 0 keeps its rows in TMEM and folds the
-  // other parts' slots into them, one thread per row (all 256 rows in flight: best when there are few slots to read);
-  // heavily split units are merged by fixup_merge below, where every part publishes its rows
-  const bool owner = FIXUP && seg.slot >= 0 && seg.t0 == 0 && p.units[seg.unit].slot_count <= kOwnerMergeMax;
-  if (seg.slot >= 0 && !owner) {
-    // one part of a split unit: un-normalised rows into the slot, then (FIXUP) tell the owning part
-    const int64_t r = (int64_t)seg.slot * p.slot_rows + row_in_unit;
-    float* dst = p.slot_o + r * DV;
-    p.slot_m[r] = m_ref;
-    p.slot_l[r] = l;
-#pragma unroll
-    for (int ch = 0; ch < DV / 32; ++ch) {
-      uint32_t o[32];
-      tmem_ld32(tO + ch * 32, o);
-      tmem_wait_ld();
-#pragma unroll
-      for (int c4 = 0; c4 < 8; ++c4)
-        *reinterpret_cast<uint4*>(dst + ch * 32 + c4 * 4) = make_uint4(o[c4 * 4], o[c4 * 4 + 1], o[c4 * 4 + 2], o[c4 * 4 + 3]);
-    }
-    if (FIXUP) {
-      __threadfence();
-      __syncwarp();
-      if ((threadIdx.x & 31) == 0) st_release_gpu_u64(p.slot_flags + (int64_t)seg.slot * kFlagsPerSlot + (row_in_unit >> 5), p.fixup_tag);
-    }
-    return;
-  }
-
-  // this thread writes the row's result: whole key range, or the owning part of a split unit
-  float w_own = 1.f;
-  int s_begin = 0, s_end = 0;
-  if (owner) {
-    const UnitRec u = p.units[seg.unit];
-    s_begin = u.slot_begin;
-    s_end = u.slot_begin + u.slot_count;
-    float m = m_ref;
-    for (int sl = s_begin; sl < s_end; ++sl) {
-      if (sl == seg.slot) continue;
-      wait_slot_rows(p, sl, row_in_unit >> 5);
-      m = fmaxf(m, __ldcg(p.slot_m + (int64_t)sl * p.slot_rows + row_in_unit));
-    }
-    w_own = (m_ref == -INFINITY) ? 0.f : exp2f(m_ref - m);
-    float lt = l * w_own;
-    for (int sl = s_begin; sl < s_end; ++sl) {
-      if (sl == seg.slot) continue;
-      const int64_t r = (int64_t)sl * p.slot_rows + row_in_unit;
-      const float ms = __ldcg(p.slot_m + r);
-      lt = fmaf(__ldcg(p.slot_l + r), (ms == -INFINITY) ? 0.f : exp2f(ms - m), lt);
-    }
-    l = lt;
-    m_ref = m;
-  }
-  const float inv = 1.f / l;
-  const int64_t fr = ((int64_t)seg.b * p.H + seg.h) * p.N + n;
-  char* orow = reinterpret_cast<char*>(p.out) + 2 * ((int64_t)seg.b * p.osb + (int64_t)n * p.osn + (int64_t)seg.h * p.osh);
-  if (p.write_partial && valid) {
-    p.fin_m[fr] = m_ref;
-    p.fin_l[fr] = l;
-  }
-#pragma unroll
-  for (int ch = 0; ch < DV / 32; ++ch) {
-    uint32_t o[32];
-    tmem_ld32(tO + ch * 32, o);
-    tmem_wait_ld();
-    if (owner) {
-#pragma unroll
-      for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * w_own);
-      for (int sl = s_begin; sl < s_end; ++sl) {
-        if (sl == seg.slot) continue;
-        const int64_t r = (int64_t)sl * p.slot_rows + row_in_unit;
-        const float ms = __ldcg(p.slot_m + r);
-        const float w = (ms == -INFINITY) ? 0.f : exp2f(ms - m_ref);
-        const float4* src = reinterpret_cast<const float4*>(p.slot_o + r * DV + ch * 32);
-#pragma unroll
-        for (int c4 = 0; c4 < 8; ++c4) {
-          const float4 x = __ldcg(src + c4);
-          o[c4 * 4 + 0] = __float_as_uint(fmaf(x.x, w, __uint_as_float(o[c4 * 4 + 0])));
-          o[c4 * 4 + 1] = __float_as_uint(fmaf(x.y, w, __uint_as_float(o[c4 * 4 + 1])));
-          o[c4 * 4 + 2] = __float_as_uint(fmaf(x.z, w, __uint_as_float(o[c4 * 4 + 2])));
-          o[c4 * 4 + 3] = __float_as_uint(fmaf(x.w, w, __uint_as_float(o[c4 * 4 + 3])));
-        }
-      }
-    }
-    if (!valid) continue;
-    if (!p.write_partial) {
-#pragma unroll
-      for (int c8 = 0; c8 < 4; ++c8) {
-        const int col = ch * 32 + c8 * 8;
-        if (col < p.dv_pass) {
-          uint4 w;
-          w.x = pack2(__uint_as_float(o[c8 * 8 + 0]) * inv, __uint_as_float(o[c8 * 8 + 1]) * inv, BF16);
-          w.y = pack2(__uint_as_float(o[c8 * 8 + 2]) * inv, __uint_as_float(o[c8 * 8 + 3]) * inv, BF16);
-          w.z = pack2(__uint_as_float(o[c8 * 8 + 4]) * inv, __uint_as_float(o[c8 * 8 + 5]) * inv, BF16);
-          w.w = pack2(__uint_as_float(o[c8 * 8 + 6]) * inv, __uint_as_float(o[c8 * 8 + 7]) * inv, BF16);
-          *reinterpret_cast<uint4*>(orow + 2 * (p.dv_off + col)) = w;
-        }
-      }
-    } else {
-      float* dst = p.fin_o + fr * p.dv + p.dv_off;
-#pragma unroll
-      for (int c4 = 0; c4 < 8; ++c4) {
-        const int col = ch * 32 + c4 * 4;
-        if (col < p.dv_pass)
-          *reinterpret_cast<uint4*>(dst + col) = make_uint4(o[c4 * 4], o[c4 * 4 + 1], o[c4 * 4 + 2], o[c4 * 4 + 3]);
-      }
-    }
-  }
-}
-
-// In-kernel merge of HEAVILY split units (more than kOwnerMergeMax parts), run by the 8 softmax warps AFTER the CTA's last
-// segment.  Every part of such a unit has written its un-normalised rows to its slot (epilogue_row); part i of the S parts merges rows
-// [i*R/S, (i+1)*R/S) of the unit — one warp per row: the lanes wait for the S publishing warps of that row, reduce the
-// row maxima and denominators with shuffles, then stream the S numerator rows (512 coalesced bytes each, all in flight)
-// and write the row's result.  The merge work of a unit is thereby spread over all CTAs that worked on it and runs with
-// coalesced loads: with few, heavily split units (B*H small) the owner-merges-everything scheme serialises
-// S x 133 KB of strided 16-byte reads behind one CTA (B=1 at the north-star shape: 0.219 -> 0.151 ms per launch; the row-serial
-// warps lose to the owner scheme when S is 2-3: B=8 0.864 vs 0.912 ms, hence the split by kOwnerMergeMax).
-// No part ever waits before its own rows are published, and parts are merged only after the CTA's last segment, so the
-// waits cannot form a cycle (all CTAs of the persistent grid are resident).
-//   tile_rows: query rows per tile (128; 256 in the CTA-pair kernel); part_rank / part_ranks: the CTAs of a pair share
-//   their segments and split the rows between them.
-template <int DV, bool BF16>
-__device__ __forceinline__ void fixup_merge(const TcParams& p, int seg_lo, int seg_hi, int warp8, int lane,
-                                            int tile_rows, int part_rank, int part_ranks) {
-  // lane owns columns {lane*4 + 128*v .. +3} (DV >= 128: kV float4 per slot row) or {lane*2, lane*2+1} (DV == 64)
-  constexpr bool kNarrow = DV < 128;
-  constexpr int kV = kNarrow ? 1 : (DV + 127) / 128;
-  for (int sg = seg_lo; sg < seg_hi; ++sg) {
-    const Segment seg = p.segs[sg];
-    if (seg.slot < 0) continue;
-    const UnitRec u = p.units[seg.unit];
-    const int S = u.slot_count, part = seg.slot - u.slot_begin;
-    if (S <= kOwnerMergeMax) continue;  // merged by the owning part in its epilogue
-    const int R = min(seg.ntile * tile_rows, p.N - seg.q0);
-    const int r0 = (int)(((int64_t)R * part) / S), r1 = (int)(((int64_t)R * (part + 1)) / S);
-    for (int r = r0 + warp8 * part_ranks + part_rank; r < r1; r += 8 * part_ranks) {
-      const int rw = r >> 5;
-      // the row of every part is published; row maximum
-      float m = -INFINITY;
-      for (int s0 = 0; s0 < S; s0 += 32) {
-        const int sidx = s0 + lane;
-        float ms = -INFINITY;
-        if (sidx < S) {
-          const unsigned long long* f = p.slot_flags + (int64_t)(u.slot_begin + sidx) * kFlagsPerSlot + rw;
-          uint32_t spins = 0;
-          uint64_t t0 = 0;
-          while (ld_acquire_gpu_u64(f) != p.fixup_tag) {
-            if ((++spins & 0xFFu) == 0) {
-              const uint64_t now = globaltimer_ns();
-              if (t0 == 0) {
-                t0 = now;
-              } else if (now - t0 > kWaitTimeoutNs) {
-                uint32_t* d = g_wait_diag;
-                if (d != nullptr && atomicCAS(d, 0u, 1u) == 0u) {
-                  d[1] = 40;
-                  d[2] = blockIdx.x;
-                  d[3] = threadIdx.x;
-                  d[4] = (uint32_t)(u.slot_begin + sidx);
-                  d[5] = spins;
-                  __threadfence_system();
-                }
-                __trap();
-              }
-            }
-          }
-          ms = __ldcg(p.slot_m + (int64_t)(u.slot_begin + sidx) * p.slot_rows + r);
-        }
-        __syncwarp();
-        m = fmaxf(m, warp_max(ms));
-      }
-      // weights, denominator, numerator
-      float l = 0.f;
-      float4 acc[kV];
-#pragma unroll
-      for (int v = 0; v < kV; ++v) acc[v] = make_float4(0.f, 0.f, 0.f, 0.f);
-      for (int s0 = 0; s0 < S; s0 += 32) {
-        const int sidx = s0 + lane;
-        float w = 0.f, wl = 0.f;
-        if (sidx < S) {
-          const int64_t rr = (int64_t)(u.slot_begin + sidx) * p.slot_rows + r;
-          const float ms = __ldcg(p.slot_m + rr);
-          w = (ms == -INFINITY) ? 0.f : exp2f(ms - m);
-          wl = w * __ldcg(p.slot_l + rr);
-        }
-        l += warp_sum(wl);
-        const int cnt = min(32, S - s0);
-#pragma unroll 4
-        for (int j = 0; j < cnt; ++j) {
-          const float wj = __shfl_sync(0xffffffffu, w, j);
-          const float* src = p.slot_o + ((int64_t)(u.slot_begin + s0 + j) * p.slot_rows + r) * DV;
-          if (kNarrow) {
-            const float2 x = __ldcg(reinterpret_cast<const float2*>(src + lane * 2));
-            acc[0].x = fmaf(x.x, wj, acc[0].x);
-            acc[0].y = fmaf(x.y, wj, acc[0].y);
-          } else {
-#pragma unroll
-            for (int v = 0; v < kV; ++v) {
-              if (v * 128 + lane * 4 >= DV) continue;
-              const float4 x = __ldcg(reinterpret_cast<const float4*>(src + v * 128 + lane * 4));
-              acc[v].x = fmaf(x.x, wj, acc[v].x);
-              acc[v].y = fmaf(x.y, wj, acc[v].y);
-              acc[v].z = fmaf(x.z, wj, acc[v].z);
-              acc[v].w = fmaf(x.w, wj, acc[v].w);
-            }
-          }
-        }
-      }
-      const int n = seg.q0 + r;
-      const int64_t fr = ((int64_t)seg.b * p.H + seg.h) * p.N + n;
-      const float inv = 1.f / l;
-      char* orow = reinterpret_cast<char*>(p.out) +
-                   2 * ((int64_t)seg.b * p.osb + (int64_t)n * p.osn + (int64_t)seg.h * p.osh + p.dv_off);
-      float* frow = p.fin_o + fr * p.dv + p.dv_off;
-#pragma unroll
-      for (int v = 0; v < kV; ++v) {
-        const int col = kNarrow ? lane * 2 : v * 128 + lane * 4;
-        if (col >= p.dv_pass || col >= DV) continue;
-        if (!p.write_partial) {
-          if (kNarrow)
-            *reinterpret_cast<uint32_t*>(orow + 2 * col) = pack2(acc[v].x * inv, acc[v].y * inv, BF16);
-          else
-            *reinterpret_cast<uint2*>(orow + 2 * col) =
-                make_uint2(pack2(acc[v].x * inv, acc[v].y * inv, BF16), pack2(acc[v].z * inv, acc[v].w * inv, BF16));
-        } else {
-          if (kNarrow)
-            *reinterpret_cast<float2*>(frow + col) = make_float2(acc[v].x, acc[v].y);
-          else
-            *reinterpret_cast<float4*>(frow + col) = acc[v];
-        }
-      }
-      if (p.write_partial && lane == 0) {
-        p.fin_m[fr] = m;
-        p.fin_l[fr] = l;
-      }
-    }
-  }
-}
-
-// pair_rank < 0: single-CTA kernel.  Otherwise this CTA is rank `pair_rank` of a cta_group::2 pair: query tile `wg` of
-// the pair spans 256 rows (128 per CTA) and the p_full / o_empty barriers the MMA issuer waits on live in the leader CTA.
-template <int DQK, int DV, bool BF16>
-__device__ __forceinline__ void softmax_role(const TcParams& p, Barriers& bar, int wg, int row, int seg_lo,
-                                             int seg_hi, int pair_rank = -1) {
-  const bool pair = pair_rank >= 0;
-  const int row_in_unit = wg * (pair ? 2 * kTileM : kTileM) + (pair ? pair_rank * kTileM : 0) + row;
-  const uint32_t p_full_remote = (pair && pair_rank != 0) ? mapa_cluster(smem_u32(&bar.p_full[wg]), 0) : 0u;
-  const uint32_t o_empty_remote = (pair && pair_rank != 0) ? mapa_cluster(smem_u32(&bar.o_empty[wg]), 0) : 0u;
-  const uint32_t lane_field = (uint32_t)((row >> 5) * 32) << 16;
-  const uint32_t tS = bar.tmem_base + lane_field + (uint32_t)(wg * 128);
-  const uint32_t tO = bar.tmem_base + lane_field + 256u + (uint32_t)(wg * 128);
-  uint32_t n_s = 0, n_o = 0;
-  // loop-invariant dispatch, decided before the first barrier wait: 0 classic, 1 optimistic
-  const int mode = p.optimistic ? 1 : 0;
-
-  for (int sg = seg_lo; sg < seg_hi; ++sg) {
-    const Segment seg = p.segs[sg];
-    if (wg == 1 && seg.ntile < 2) continue;
-    const int n = seg.q0 + row_in_unit;
-    RowState st;
-    st.m_ref = -INFINITY;
-    st.l = 0.f;
-    TileCtx c;
-    c.tS = tS; c.tO = tO; c.wg = wg; c.row = row;
-    c.p_full_remote = p_full_remote;
-    c.pv_bar = nullptr;
-    c.pv_parity = 0;
-    c.cshift = n + p.causal_shift;
-    c.trace_on = (row == 0 && sg == seg_lo);
-    c.scale_log2 = p.scale_log2;
-
-    for (int t = seg.t0; t < seg.t1; ++t) {
-      c.j0 = t * kTileN;
-      c.tt = t - seg.t0;
-      c.first_tile = (t == seg.t0);
-      c.mw = make_uint4(0, 0, 0, 0);
-      if (p.pad_bits != nullptr)
-        c.mw = *reinterpret_cast<const uint4*>(p.pad_bits + (size_t)seg.b * p.pad_wpr + (size_t)t * 4);
-      // warp-uniform on purpose: the tcgen05.ld/st in the tile body are .sync.aligned and must not sit behind
-      // a lane-divergent branch (the causal test differs between the rows of a warp on diagonal tiles)
-      const bool masked_tile =
-          __any_sync(0xffffffffu, (c.j0 + kTileN > p.M) || ((c.mw.x | c.mw.y | c.mw.z | c.mw.w) != 0u) ||
-                                      (p.causal && (c.j0 + kTileN - 1 > c.cshift)));
-      mbar_wait(&bar.s_full[wg], n_s & 1, 12);
-      ++n_s;
-      tc_fence_after_sync();
-      PCV_TRACE(p, wg, c.tt, 0, c.trace_on);
-      if (masked_tile) {
-        softmax_tile<DV, BF16, true>(p, bar, c, st);
-      } else if (mode != 0 && !c.first_tile) {
-        const bool ok = softmax_tile_optimistic<DV, BF16, kPolyQuarter>(p, bar, c, st);
-        if (!ok) {
-          // the reference must move: nothing was stored, redo on the classic path (max first)
-          softmax_tile<DV, BF16, false>(p, bar, c, st);
-        }
-      } else {
-        softmax_tile<DV, BF16, false>(p, bar, c, st);
-      }
-    }
-    const float l = st.l, m_ref = st.m_ref;
-
-    // ---- epilogue: O row -> global ------------------------------------------------------------------
-    mbar_wait(&bar.o_full[wg], n_o & 1, 13);
-    ++n_o;
-    tc_fence_after_sync();
-    epilogue_row<DV, BF16, true>(p, seg, tO, n, row_in_unit, l, m_ref);
-    tc_fence_before_sync();
-    __syncwarp();
-    if ((threadIdx.x & 31) == 0) {
-      if (o_empty_remote == 0)
-        mbar_arrive(&bar.o_empty[wg]);
-      else
-        mbar_arrive_cluster_relaxed(o_empty_remote);  // the accumulator rows were read with tcgen05.ld + wait::ld
-    }
-  }
-}
-
-// --------------------------------------------------------------------------------------------------
-// fused cross-GPU merge (kernel tail of an M-sharded launch; SURVEY.md §8(e) option 3)
-//
-//   A  grid-wide arrival: every partial-state row of this GPU is written (system-scope fence first; split units
-//      were already folded together by the epilogue fix-up)
-//   2  "ready" flag of this rank is stored (release, system scope) into every peer's flag block
-//   3  wait until every peer's ready flag shows this call's epoch
-//   4  owned rows: pull (m, l, numerator row) of every rank through the NVLink-mapped pointers (relaxed system-scope
-//      loads: the same addresses are re-read every call, they must not be served from a stale L1 line), merge exactly,
-//      push the normalised row into the output buffer of EVERY rank
-//   5  grid-wide arrival, then the "done" flag of this rank goes to every peer; CTA 0 waits for all done flags, so
-//      the kernel only completes when this GPU's output buffer has received every row slice — no host-side barrier
-// Executed by the 8 softmax warps (the control warps hold 88 registers); CTA-level sync is named barrier 2.
-// Every wait is bounded by the watchdog (a dead peer becomes a trap with a diagnosis, not a hung GPU).  Needs all
-// CTAs of the grid co-resident: grid <= #SMs at one CTA per SM, which is how this kernel is always launched.
+// M-sharded merge across GPUs (pcv_attn_fwd_sharded), run in stream order right after the attention kernel of the
+// call: publish "partial state complete" to every rank, wait for all ranks, merge the owned rows of the flattened
+// (b, h, n) space from every rank's state over peer memory and store the normalised rows into EVERY rank's output,
+// then a grid-wide arrival and a second flag exchange so that the call returns when this rank's output is complete.
+// No NCCL and no host barrier on the path.  Flag words per rank: [0, G) partial state of rank i complete, [G, 2G)
+// rank i has pushed all its rows, [18] grid arrival counter, [24, 30) phase clock of CTA 0; all monotonic in the
+// call epoch.  The grid-wide arrival needs every CTA co-resident: the grid is at most one CTA per SM.
 // --------------------------------------------------------------------------------------------------
 constexpr int kTailThreads = 256;
 
@@ -819,16 +153,16 @@ __device__ __forceinline__ void tail_wait_ge(const uint32_t* flag, uint32_t valu
 // all kTailThreads threads of every CTA call this; `counter` is a device-local word, monotonic over calls
 __device__ __forceinline__ void tail_grid_arrive_wait(uint32_t* counter, uint32_t target, uint32_t site) {
   __threadfence_system();  // this thread's partial-state / output stores are visible system-wide before the arrival
-  named_bar_sync(2, kTailThreads);
+  __syncthreads();
   if (threadIdx.x == 0) {
     atomicAdd(counter, 1u);
     tail_wait_ge(counter, target, site);
   }
-  named_bar_sync(2, kTailThreads);
+  __syncthreads();
 }
 
-template <int DV, bool BF16>
-__device__ void peer_tail(const TcParams& p) {
+template <bool BF16>
+__global__ void __launch_bounds__(kTailThreads) peer_tail_kernel(const TcParams p) {
   const PeerTail& t = p.tail;
   const int G = t.num_peers;
   uint32_t* lf = t.flags[t.rank];
@@ -842,15 +176,17 @@ __device__ void peer_tail(const TcParams& p) {
     if (blockIdx.x == 0 && threadIdx.x == 0) lf[24 + (i)] = (uint32_t)(globaltimer_ns() - t_in); \
   } while (0)
 
-  tail_grid_arrive_wait(lf + 16, target, 30);
+  // the attention (and combine) kernels of this call ran before in stream order: the local partial state is complete
   PCV_TAIL_STAMP(0);
-
   PCV_TAIL_STAMP(1);
 
-  // publish: flags[g][rank] = epoch on every rank g (release: ordered after the grid-wide arrival above)
-  if (blockIdx.x == 0 && threadIdx.x < G) st_release_sys_u32(t.flags[threadIdx.x] + t.rank, t.epoch);
+  // publish: flags[g][rank] = epoch on every rank g
+  if (blockIdx.x == 0 && threadIdx.x < G) {
+    __threadfence_system();
+    st_release_sys_u32(t.flags[threadIdx.x] + t.rank, t.epoch);
+  }
   if (threadIdx.x < G) tail_wait_ge(lf + threadIdx.x, t.epoch, 32);
-  named_bar_sync(2, kTailThreads);
+  __syncthreads();
   PCV_TAIL_STAMP(2);
 
   // owned rows: pull, merge, push.  A warp keeps PCV_MAX_PEERS (row, rank) sources in flight at once — with 2 ranks
@@ -919,973 +255,241 @@ __device__ void peer_tail(const TcParams& p) {
       st_release_sys_u32(t.flags[threadIdx.x] + G + t.rank, t.epoch);
       tail_wait_ge(lf + G + threadIdx.x, t.epoch, 34);
     }
-    named_bar_sync(2, kTailThreads);
+    __syncthreads();
   }
   PCV_TAIL_STAMP(5);
 #undef PCV_TAIL_STAMP
 }
 
-// --------------------------------------------------------------------------------------------------
-// the kernel
-// --------------------------------------------------------------------------------------------------
-template <int DQK, int DV, bool BF16>
-__global__ void __launch_bounds__(kThreads, 1)
-attn_tc_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-               const __grid_constant__ CUtensorMap tmap_v, const TcParams p) {
-  using C = Cfg<DQK, DV>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* q_smem = smem;
-  uint8_t* kv_smem = smem + C::kQBytes;
-  Barriers& bar = *reinterpret_cast<Barriers*>(smem + C::kQBytes + C::kStages * C::kStageBytes);
+template <int NQB, int NVB>
+struct FwdCfg {
+  static constexpr int kQBytes = NQB * kBoxBytes;
+  static constexpr int kSlots = (kSmemLimit - kQBytes - 2048) / kBoxBytes > 16 ? 16 : (kSmemLimit - kQBytes - 2048) / kBoxBytes;
+  static constexpr int kSmemBytes = kQBytes + kSlots * kBoxBytes + 2048;  // + barriers + 1024-byte alignment slack
+  static_assert(kSlots >= 2, "shared memory budget");
+};
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int seg_lo = p.cta_seg_begin[blockIdx.x];
-  const int seg_hi = p.cta_seg_begin[blockIdx.x + 1];
-#ifdef PCV_ENABLE_TRACE
-  {
-    unsigned smid;
-    asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
-    int tiles = 0;
-    for (int sg = seg_lo; sg < seg_hi; ++sg) tiles += p.segs[sg].t1 - p.segs[sg].t0;
-    PCV_TRACE_CTA(p, 0, globaltimer_ns());
-    PCV_TRACE_CTA(p, 4, clock64());
-    PCV_TRACE_CTA(p, 2, smid);
-    PCV_TRACE_CTA(p, 3, tiles);
-  }
-#endif
+struct FwdBarriers {
+  uint64_t full[16], empty[16];
+  uint64_t q_full, q_empty;
+};
+
+template <int NQB, int NVB, bool BF16, bool PAIR>
+__global__ void __launch_bounds__(kThreads, 1)
+attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
+                const __grid_constant__ CUtensorMap tv, const TcParams p) {
+  using C = FwdCfg<NQB, NVB>;
+  constexpr int NS = C::kSlots;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sQ = smem;
+  uint8_t* sRing = smem + C::kQBytes;
+  FwdBarriers& bar = *reinterpret_cast<FwdBarriers*>(sRing + NS * kBoxBytes);
+  const int wg = threadIdx.x / 128;
+  const int worker = PAIR ? blockIdx.x / 2 : blockIdx.x;
+  const uint32_t rank = PAIR ? cluster_ctarank() : 0u;
+  const int qoff = 128 * (int)rank;  // this CTA's query tile within the pair's 256-row unit
+  const int seg_lo = p.cta_seg_begin[worker], seg_hi = p.cta_seg_begin[worker + 1];
 
   if (threadIdx.x == 0) {
+    for (int s = 0; s < NS; ++s) {
+      mbar_init(&bar.full[s], 1);
+      mbar_init(&bar.empty[s], PAIR ? 16 : 8);  // one arrive per consumer warp (of both CTAs of a pair)
+    }
     mbar_init(&bar.q_full, 1);
-    mbar_init(&bar.q_empty, 1);
-    for (int i = 0; i < C::kStages; ++i) {
-      mbar_init(&bar.kv_full[i], 1);
-      mbar_init(&bar.kv_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&bar.s_full[i], 1);
-      mbar_init(&bar.p_full[i], 4);   // one arrive per softmax warp
-      mbar_init(&bar.o_full[i], 1);
-      mbar_init(&bar.o_empty[i], 4);
-    }
+    mbar_init(&bar.q_empty, 8);
     fence_mbar_init();
   }
-  if (warp == kMmaWarp) {
-    tmem_alloc(&bar.tmem_base, 512);
-    tmem_relinquish();
-  }
-  if (warp == kTmaWarp && lane == 0) {
-    tma_prefetch_desc(&tmap_q);
-    tma_prefetch_desc(&tmap_k);
-    tma_prefetch_desc(&tmap_v);
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
+  if (PAIR)
+    cluster_sync_all();
+  else
+    __syncthreads();
 
-  if (warp < 8) {
-    reg_alloc<208>();  // 256*208 + 128*88 == 384*168: exactly the registers the CTA was launched with  // softmax warpgroups take the registers the control warpgroup gives up
-    softmax_role<DQK, DV, BF16>(p, bar, warp >> 2, threadIdx.x & 127, seg_lo, seg_hi);
-    fixup_merge<DV, BF16>(p, seg_lo, seg_hi, warp, lane, kTileM, 0, 1);
-    if (p.tail.enabled) peer_tail<DV, BF16>(p);
-  } else {
-    reg_dealloc<88>();
-  }
-  // The two control roles run WARP-CONVERGED (all 32 lanes execute the loops and the barrier waits; one
-  // elected lane issues the TMA / tcgen05 instructions).  Keeping the warp converged lets the compiler hold
-  // addresses, descriptors and counters in uniform registers; a single-lane loop forced an R2UR shuffle in
-  // front of every tcgen05.mma operand and made instruction issue, not the tensor pipe, the bottleneck.
-  if (warp == kTmaWarp) {
-    // ===== TMA producer: Q once per segment, then K_j, V_j through the ring =====
-    const bool leader = elect_one();
-    uint32_t it = 0, n_q = 0;
-    for (int sg = seg_lo; sg < seg_hi; ++sg) {
-      const Segment seg = p.segs[sg];
-      const int bq = p.q_bcast ? 0 : seg.b;
-      mbar_wait(&bar.q_empty, (n_q & 1) ^ 1, 1);
-      ++n_q;
-      if (leader) {
-        mbar_arrive_expect_tx(&bar.q_full, (uint32_t)(seg.ntile * C::kQTileBytes));
-        for (int i = 0; i < seg.ntile; ++i)
-          for (int bx = 0; bx < C::kQBoxes; ++bx)
-            tma_load_4d(q_smem + i * C::kQTileBytes + bx * kBoxBytes, &tmap_q, &bar.q_full, bx * 64,
-                        seg.q0 + i * kTileM, seg.h, bq);
-      }
-      for (int t = seg.t0; t < seg.t1; ++t) {
-        {
-          const uint32_t slot = it % C::kStages, par = (it / C::kStages) & 1;
-          mbar_wait(&bar.kv_empty[slot], par ^ 1, 2);
-          if (leader) {
-            mbar_arrive_expect_tx(&bar.kv_full[slot], (uint32_t)(C::kQBoxes * kBoxBytes));
-#pragma unroll
-            for (int bx = 0; bx < C::kQBoxes; ++bx)
-              tma_load_4d(kv_smem + slot * C::kStageBytes + bx * kBoxBytes, &tmap_k, &bar.kv_full[slot], bx * 64,
-                          t * kTileN, seg.h, seg.b);
-          }
-          ++it;
-        }
-        {
-          const uint32_t slot = it % C::kStages, par = (it / C::kStages) & 1;
-          mbar_wait(&bar.kv_empty[slot], par ^ 1, 3);
-          if (leader) {
-            mbar_arrive_expect_tx(&bar.kv_full[slot], (uint32_t)(C::kVBoxes * kBoxBytes));
-#pragma unroll
-            for (int bx = 0; bx < C::kVBoxes; ++bx)
-              tma_load_4d(kv_smem + slot * C::kStageBytes + bx * kBoxBytes, &tmap_v, &bar.kv_full[slot], bx * 64,
-                          t * kTileN, seg.h, seg.b);
-          }
-          ++it;
-        }
-      }
-    }
-  } else if (warp == kMmaWarp) {
-    // ===== MMA issuer =====
-    const bool leader = elect_one();
-    constexpr uint32_t idesc_qk = make_idesc(kTileM, kTileN, BF16, false);
-    constexpr uint32_t idesc_pv = make_idesc(kTileM, DV, BF16, true);
-    const uint32_t tmem = bar.tmem_base;
-    // descriptors of tile/stage 0; other tiles, stages and K-steps are plain adds on the 16-byte address field
-    const uint64_t dq0 = make_smem_desc(smem_u32(q_smem), 16, 1024);
-    const uint64_t dk0 = make_smem_desc(smem_u32(kv_smem), 16, 1024);
-    const uint64_t dv0 = make_smem_desc(smem_u32(kv_smem), kBoxBytes, 1024);
-    uint32_t it = 0, n_q = 0, n_p0 = 0, n_p1 = 0, n_oe0 = 0, n_oe1 = 0;
-
-    auto issue_qk = [&](int i, uint32_t k_slot) {
-      if (leader) {
-        const uint64_t da = dq0 + (uint64_t)((i * C::kQTileBytes) >> 4);
-        const uint64_t db = dk0 + (uint64_t)((k_slot * C::kStageBytes) >> 4);
-#pragma unroll
-        for (int kk = 0; kk < DQK / 16; ++kk) {
-          const uint64_t off = (uint64_t)(((kk >> 2) * kBoxBytes + (kk & 3) * 32) >> 4);
-          mma_ss(tmem + i * 128, da + off, db + off, idesc_qk, kk > 0 ? 1u : 0u);
-        }
-      }
-    };
-    auto issue_pv = [&](int i, uint32_t v_slot, bool accumulate) {
-      if (leader) {
-        const uint64_t db = dv0 + (uint64_t)((v_slot * C::kStageBytes) >> 4);
-#pragma unroll
-        for (int kk = 0; kk < kTileN / 16; ++kk) {
-          // V tile is MN-major: 16 keys = 16 rows of 128 bytes; 64-channel blocks kBoxBytes apart
-          mma_ts(tmem + 256 + i * 128, tmem + i * 128 + kk * 8, db + (uint64_t)((kk * 2048) >> 4), idesc_pv,
-                 (accumulate || kk > 0) ? 1u : 0u);
-        }
-      }
-    };
-    auto commit = [&](uint64_t* b) {
-      if (leader) tc_commit(b);
-    };
-
-    // Serial-path trimming (p.mmaopt): this one thread is the pacemaker of the CTA — whenever it sits in a barrier
-    // wait or a tcgen05.commit with the MMA queue empty, the tensor pipe idles.  (1) The waits whose barriers are
-    // normally long complete by the time they are reached (V_j, K_(j+1)) are probed together with the P_0 wait, so
-    // their latencies overlap instead of adding up; (2) the kv_empty commits (only the TMA producer waits for them,
-    // several stages ahead) are deferred until the next P_0 V MMAs are queued, when the thread would be blocked on
-    // the full queue anyway.  Deferral needs the 5-stage ring (with 3 stages the producer needs the slot at once).
-    const bool defer = (p.mmaopt & 2) && C::kStages >= 5;
-    int pend0 = -1, pend1 = -1;  // ring slots whose kv_empty commit is still owed
-    auto flush_pending = [&]() {
-      if (pend0 >= 0) commit(&bar.kv_empty[pend0]);
-      if (pend1 >= 0) commit(&bar.kv_empty[pend1]);
-      pend0 = pend1 = -1;
-    };
-    auto release = [&](uint32_t slot) {
-      if (!defer) {
-        commit(&bar.kv_empty[slot]);
-      } else if (pend0 < 0) {
-        pend0 = (int)slot;
-      } else {
-        pend1 = (int)slot;
-      }
-    };
-
-    for (int sg = seg_lo; sg < seg_hi; ++sg) {
-      const Segment seg = p.segs[sg];
-      const bool two = seg.ntile == 2;
-      const int nt = seg.t1 - seg.t0;
-      mbar_wait(&bar.q_full, n_q & 1, 4);
-      ++n_q;
-
-      uint32_t k_slot = it % C::kStages;
-      mbar_wait(&bar.kv_full[k_slot], (it / C::kStages) & 1, 5);
-      ++it;
-      tc_fence_after_sync();
-      issue_qk(0, k_slot);
-      commit(&bar.s_full[0]);
-      if (two) {
-        issue_qk(1, k_slot);
-        commit(&bar.s_full[1]);
-      }
-      commit(&bar.kv_empty[k_slot]);
-
-      for (int j = 0; j < nt; ++j) {
-        const uint32_t v_slot = it % C::kStages, v_par = (it / C::kStages) & 1;
-        ++it;
-        const bool more = (j + 1 < nt);
-        uint32_t k_par = 0;
-        if (more) {
-          k_slot = it % C::kStages;
-          k_par = (it / C::kStages) & 1;
-          ++it;
-        }
-        bool ok_v = false, ok_p = false, ok_k = false;
-        if (p.mmaopt & 1) {  // independent probes: their latencies overlap
-          ok_v = mbar_try_wait(&bar.kv_full[v_slot], v_par);
-          ok_p = mbar_try_wait(&bar.p_full[0], n_p0 & 1);
-          ok_k = more ? mbar_try_wait(&bar.kv_full[k_slot], k_par) : true;
-        }
-        if (!ok_v) mbar_wait(&bar.kv_full[v_slot], v_par, 6);
-        if (j == 0) {
-          mbar_wait(&bar.o_empty[0], (n_oe0 & 1) ^ 1, 7);
-          ++n_oe0;
-        }
-        PCV_TRACE(p, 2, j, 0, leader && sg == seg_lo);
-        if (!ok_p) mbar_wait(&bar.p_full[0], n_p0 & 1, 8);
-        ++n_p0;
-        tc_fence_after_sync();
-        PCV_TRACE(p, 2, j, 1, leader && sg == seg_lo);
-        issue_pv(0, v_slot, j > 0);
-        flush_pending();
-        PCV_TRACE(p, 2, j, 2, leader && sg == seg_lo);
-        if (more) {
-          if (!ok_k) mbar_wait(&bar.kv_full[k_slot], k_par, 9);
-          tc_fence_after_sync();
-          issue_qk(0, k_slot);
-          commit(&bar.s_full[0]);
-        }
-        PCV_TRACE(p, 2, j, 3, leader && sg == seg_lo);
-        if (two) {
-          if (j == 0) {
-            mbar_wait(&bar.o_empty[1], (n_oe1 & 1) ^ 1, 10);
-            ++n_oe1;
-          }
-          mbar_wait(&bar.p_full[1], n_p1 & 1, 11);
-          ++n_p1;
-          tc_fence_after_sync();
-          PCV_TRACE(p, 2, j, 4, leader && sg == seg_lo);
-          issue_pv(1, v_slot, j > 0);
-        }
-        PCV_TRACE(p, 2, j, 6, leader && sg == seg_lo);
-        release(v_slot);
-        if (more) {
-          if (two) {
-            issue_qk(1, k_slot);
-            PCV_TRACE(p, 2, j, 7, leader && sg == seg_lo);
-            commit(&bar.s_full[1]);
-          }
-          release(k_slot);
-        }
-        PCV_TRACE(p, 2, j, 5, leader && sg == seg_lo);
-      }
-      flush_pending();
-      commit(&bar.q_empty);
-      commit(&bar.o_full[0]);
-      if (two) commit(&bar.o_full[1]);
-    }
-  }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  PCV_TRACE_CTA(p, 1, globaltimer_ns());
-  PCV_TRACE_CTA(p, 5, clock64());
-  if (warp == kMmaWarp) {
-    tc_fence_after_sync();
-    tmem_dealloc(bar.tmem_base, 512);
-  }
-}
-
-
-// --------------------------------------------------------------------------------------------------
-// CTA-pair kernel (cta_group::2): one work unit = 512 query rows of one (b, h) on TWO SMs.  Every tcgen05.mma has
-// M = 256 (128 rows from each CTA); each CTA stages its own Q rows, HALF of every K tile (64 keys: N/2 of Q K^T) and
-// HALF of every V tile (64 channels: N/2 of P V), so the SS-mode operand reads of Q K^T drop from 128 to 96 bytes per
-// clock and SM — the shared-memory ceiling the single-CTA kernel's issuing thread blocks on — and the L2 -> SM traffic
-// per SM halves.  Only the leader CTA issues MMAs; tcgen05.commit multicasts to the barriers of both CTAs.
-// Round 1 measured this structure at 0.91 PF (vs 1.25 PF single-CTA) and shelved it; the fused K/V producer's profile
-// (DESIGN.md section 3.4) showed why: every cross-CTA `mbarrier.arrive.release.cluster` compiles to MEMBAR.ALL.GPU +
-// ERRBAR + CGAERRBAR, and the kernel issued one per K/V stage from the peer's producer (ERRBAR waits for the thread's
-// outstanding TMA loads: ring depth 1) and one per tile from EVERY softmax warp, on the critical chain.  Here: the peer
-// producer never arrives (the leader's expect_tx covers both CTAs' bytes), the leader's softmax warps arrive locally,
-// the peer's with `mbarrier.arrive.relaxed.cluster` (P is in TMEM once tcgen05.wait::st returns; nothing to release).
-// --------------------------------------------------------------------------------------------------
-template <int DQK>
-struct PairCfg {
-  static constexpr int DV = 128;
-  static constexpr int kQBoxes = DQK / 64;
-  static constexpr int kQTileBytes = kQBoxes * kBoxBytes;        // 128 rows x DQK
-  static constexpr int kQBytes = 2 * kQTileBytes;
-  static constexpr int kKHalfBytes = kQBoxes * (kBoxBytes / 2);  // 64 keys x DQK: kQBoxes boxes of 64 rows
-  static constexpr int kVHalfBytes = kBoxBytes;                  // 128 keys x 64 channels
-  static constexpr int kStageBytes = kKHalfBytes > kVHalfBytes ? kKHalfBytes : kVHalfBytes;
-  static constexpr int kBarrierBytes = 1024;
-  static constexpr int kMaxSmem = 232448 - 1024;
-  static constexpr int kStagesRaw = (kMaxSmem - kQBytes - kBarrierBytes) / kStageBytes;
-  static constexpr int kStages = kStagesRaw > 8 ? 8 : kStagesRaw;
-  static constexpr int kSmemBytes = kQBytes + kStages * kStageBytes + kBarrierBytes + 1024;
-  static_assert(kStages >= 3, "ring too shallow");
-};
-
-template <int DQK, bool BF16>
-__global__ void __launch_bounds__(kThreads, 1)
-attn_tc_pair_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                    const __grid_constant__ CUtensorMap tmap_v, const TcParams p) {
-  using C = PairCfg<DQK>;
-  constexpr int DV = C::DV;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* q_smem = smem;
-  uint8_t* kv_smem = smem + C::kQBytes;
-  Barriers& bar = *reinterpret_cast<Barriers*>(smem + C::kQBytes + C::kStages * C::kStageBytes);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t rank = cluster_ctarank();  // 0 = leader
-  const int pair_id = blockIdx.x >> 1;
-  const int seg_lo = p.cta_seg_begin[pair_id];
-  const int seg_hi = p.cta_seg_begin[pair_id + 1];
-
-  if (threadIdx.x == 0) {
-    mbar_init(&bar.q_full, 1);    // the leader's arrive.expect_tx announces the bytes of BOTH CTAs; the peer never arrives
-    mbar_init(&bar.q_empty, 1);   // multicast commit
-    for (int i = 0; i < C::kStages; ++i) {
-      mbar_init(&bar.kv_full[i], 1);
-      mbar_init(&bar.kv_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&bar.s_full[i], 1);
-      mbar_init(&bar.p_full[i], 8);   // one arrive per softmax warp, 4 warps x 2 CTAs
-      mbar_init(&bar.o_full[i], 1);
-      mbar_init(&bar.o_empty[i], 8);
-    }
-    fence_mbar_init();
-  }
-  if (warp == kMmaWarp) {
-    tmem_alloc_pair(&bar.tmem_base, 512);
-    tmem_relinquish_pair();
-  }
-  if (warp == kTmaWarp && lane == 0) {
-    tma_prefetch_desc(&tmap_q);
-    tma_prefetch_desc(&tmap_k);
-    tma_prefetch_desc(&tmap_v);
-  }
-  tc_fence_before_sync();
-  cluster_sync_all();  // barriers of both CTAs initialised before any remote arrive / multicast commit
-  tc_fence_after_sync();
-
-  if (warp < 8) {
-    reg_alloc<216>();
-    softmax_role<DQK, DV, BF16>(p, bar, warp >> 2, threadIdx.x & 127, seg_lo, seg_hi, (int)rank);
-    fixup_merge<DV, BF16>(p, seg_lo, seg_hi, warp, lane, 2 * kTileM, (int)rank, 2);
-    if (p.tail.enabled) peer_tail<DV, BF16>(p);
-  } else {
-    reg_dealloc<72>();
-  }
-
-  if (warp == kTmaWarp) {
-    // ===== TMA producer (both CTAs): own Q tiles, own half of every K / V tile; bytes counted on the leader =====
-    const bool leader_lane = elect_one();
-    uint32_t it = 0, n_q = 0;
-    for (int sg = seg_lo; sg < seg_hi; ++sg) {
-      const Segment seg = p.segs[sg];
-      const int bq = p.q_bcast ? 0 : seg.b;
-      mbar_wait(&bar.q_empty, (n_q & 1) ^ 1, 1);
-      ++n_q;
-      if (leader_lane) {
-        if (rank == 0) mbar_arrive_expect_tx(&bar.q_full, (uint32_t)(2 * seg.ntile * C::kQTileBytes));
-        for (int i = 0; i < seg.ntile; ++i)
-          for (int bx = 0; bx < C::kQBoxes; ++bx)
-            tma_load_4d_pair(q_smem + i * C::kQTileBytes + bx * kBoxBytes, &tmap_q, &bar.q_full, bx * 64,
-                             seg.q0 + i * 2 * kTileM + (int)rank * kTileM, seg.h, bq);
-      }
-      for (int t = seg.t0; t < seg.t1; ++t) {
-        {
-          const uint32_t slot = it % C::kStages, par = (it / C::kStages) & 1;
-          mbar_wait(&bar.kv_empty[slot], par ^ 1, 2);
-          if (leader_lane) {
-            if (rank == 0) mbar_arrive_expect_tx(&bar.kv_full[slot], (uint32_t)(2 * C::kKHalfBytes));
-#pragma unroll
-            for (int bx = 0; bx < C::kQBoxes; ++bx)  // K half: 64 keys x 64 channels per box
-              tma_load_4d_pair(kv_smem + slot * C::kStageBytes + bx * (kBoxBytes / 2), &tmap_k, &bar.kv_full[slot],
-                               bx * 64, t * kTileN + (int)rank * 64, seg.h, seg.b);
-          }
-          ++it;
-        }
-        {
-          const uint32_t slot = it % C::kStages, par = (it / C::kStages) & 1;
-          mbar_wait(&bar.kv_empty[slot], par ^ 1, 3);
-          if (leader_lane) {
-            if (rank == 0) mbar_arrive_expect_tx(&bar.kv_full[slot], (uint32_t)(2 * C::kVHalfBytes));
-            // V half: all 128 keys, channels [64*rank, 64*rank + 64)
-            tma_load_4d_pair(kv_smem + slot * C::kStageBytes, &tmap_v, &bar.kv_full[slot], (int)rank * 64, t * kTileN,
-                             seg.h, seg.b);
-          }
-          ++it;
-        }
-      }
-    }
-  } else if (warp == kMmaWarp && rank == 0) {
-    // ===== MMA issuer (leader CTA only) =====
-    const bool leader_lane = elect_one();
-    constexpr uint32_t idesc_qk = make_idesc(2 * kTileM, kTileN, BF16, false);
-    constexpr uint32_t idesc_pv = make_idesc(2 * kTileM, DV, BF16, true);
-    const uint32_t tmem = bar.tmem_base;
-    const uint64_t dq0 = make_smem_desc(smem_u32(q_smem), 16, 1024);
-    const uint64_t dk0 = make_smem_desc(smem_u32(kv_smem), 16, 1024);
-    const uint64_t dv0 = make_smem_desc(smem_u32(kv_smem), kBoxBytes, 1024);
-    uint32_t it = 0, n_q = 0, n_p0 = 0, n_p1 = 0, n_oe0 = 0, n_oe1 = 0;
-
-    auto issue_qk = [&](int i, uint32_t k_slot) {
-      if (leader_lane) {
-        const uint64_t da = dq0 + (uint64_t)((i * C::kQTileBytes) >> 4);
-        const uint64_t db = dk0 + (uint64_t)((k_slot * C::kStageBytes) >> 4);
-#pragma unroll
-        for (int kk = 0; kk < DQK / 16; ++kk) {
-          const uint64_t offa = (uint64_t)(((kk >> 2) * kBoxBytes + (kk & 3) * 32) >> 4);
-          const uint64_t offb = (uint64_t)(((kk >> 2) * (kBoxBytes / 2) + (kk & 3) * 32) >> 4);
-          mma_ss_pair(tmem + i * 128, da + offa, db + offb, idesc_qk, kk > 0 ? 1u : 0u);
-        }
-      }
-    };
-    auto issue_pv = [&](int i, uint32_t v_slot, bool accumulate) {
-      if (leader_lane) {
-        const uint64_t db = dv0 + (uint64_t)((v_slot * C::kStageBytes) >> 4);
-#pragma unroll
-        for (int kk = 0; kk < kTileN / 16; ++kk)
-          mma_ts_pair(tmem + 256 + i * 128, tmem + i * 128 + kk * 8, db + (uint64_t)((kk * 2048) >> 4), idesc_pv,
-                      (accumulate || kk > 0) ? 1u : 0u);
-      }
-    };
-    auto commit = [&](uint64_t* b) {
-      if (leader_lane) tc_commit_pair(b, 3);
-    };
-
-    for (int sg = seg_lo; sg < seg_hi; ++sg) {
-      const Segment seg = p.segs[sg];
-      const bool two = seg.ntile == 2;
-      const int nt = seg.t1 - seg.t0;
-      mbar_wait(&bar.q_full, n_q & 1, 4);
-      ++n_q;
-
-      uint32_t k_slot = it % C::kStages;
-      mbar_wait(&bar.kv_full[k_slot], (it / C::kStages) & 1, 5);
-      ++it;
-      tc_fence_after_sync();
-      issue_qk(0, k_slot);
-      commit(&bar.s_full[0]);
-      if (two) {
-        issue_qk(1, k_slot);
-        commit(&bar.s_full[1]);
-      }
-      commit(&bar.kv_empty[k_slot]);
-
-      for (int j = 0; j < nt; ++j) {
-        const uint32_t v_slot = it % C::kStages;
-        mbar_wait(&bar.kv_full[v_slot], (it / C::kStages) & 1, 6);
-        ++it;
-        if (j == 0) {
-          mbar_wait(&bar.o_empty[0], (n_oe0 & 1) ^ 1, 7);
-          ++n_oe0;
-        }
-        mbar_wait(&bar.p_full[0], n_p0 & 1, 8);
-        ++n_p0;
-        tc_fence_after_sync();
-        issue_pv(0, v_slot, j > 0);
-        const bool more = (j + 1 < nt);
-        if (more) {
-          k_slot = it % C::kStages;
-          mbar_wait(&bar.kv_full[k_slot], (it / C::kStages) & 1, 9);
-          ++it;
-          tc_fence_after_sync();
-          issue_qk(0, k_slot);
-          commit(&bar.s_full[0]);
-        }
-        if (two) {
-          if (j == 0) {
-            mbar_wait(&bar.o_empty[1], (n_oe1 & 1) ^ 1, 10);
-            ++n_oe1;
-          }
-          mbar_wait(&bar.p_full[1], n_p1 & 1, 11);
-          ++n_p1;
-          tc_fence_after_sync();
-          issue_pv(1, v_slot, j > 0);
-        }
-        commit(&bar.kv_empty[v_slot]);
-        if (more) {
-          if (two) {
-            issue_qk(1, k_slot);
-            commit(&bar.s_full[1]);
-          }
-          commit(&bar.kv_empty[k_slot]);
-        }
-      }
-      commit(&bar.q_empty);
-      commit(&bar.o_full[0]);
-      if (two) commit(&bar.o_full[1]);
-    }
-  }
-
-  tc_fence_before_sync();
-  cluster_sync_all();  // neither CTA may exit (or free TMEM) while its pair can still touch its memory / barriers
-  if (warp == kMmaWarp) {
-    tc_fence_after_sync();
-    tmem_dealloc_pair(bar.tmem_base, 512);
-  }
-}
-
-
-// --------------------------------------------------------------------------------------------------
-// Big-head STREAMING kernel (round 1's structure, kept for head dims the resident-Q kernel below handles worse:
-// qk head dim > 384 or v head dim > 384, i.e. the optical-flow decoder's 512 / 512): qk head dims up to 512 and v head
-// dims up to 256 per pass (the optical-flow encoder /
-// decoder geometry, 322 and 512 channels per head).  One query tile (128 rows) per CTA.  Q and K stream through
-// shared memory in 128-channel chunks (Q is re-streamed from L2 for every key tile) and S accumulates over the
-// chunks in TMEM; S is double-buffered (columns [0,128) / [128,256)) so Q K^T of tile j+1 overlaps the softmax
-// of tile j; O occupies columns [256, 256 + 64*v_boxes).  A v head dim above 256 is covered by launching the
-// kernel once per 256-channel slice of V (the scores are recomputed).  256 threads: warps 0-3 softmax (one
-// thread per row), warp 4 MMA issuer, warp 5 TMA producer.
-// --------------------------------------------------------------------------------------------------
-constexpr int kBigStreamThreads = 256;
-constexpr int kBigStreamItems = 3;
-constexpr int kBigStreamItemBytes = 4 * kBoxBytes;  // 64 KB: [Q chunk 32 KB | K chunk 32 KB] or a V tile of <= 256 channels
-constexpr int kBigStreamSmemBytes = kBigStreamItems * kBigStreamItemBytes + 1024 + 1024;
-
-struct BigStreamBarriers {
-  uint64_t item_full[kBigStreamItems], item_empty[kBigStreamItems];
-  uint64_t s_full[2], pv_done, o_full, o_empty;  // s_full per S buffer: a barrier must never run a full phase ahead of its waiter
-  uint32_t tmem_base;
-};
-
-template <bool BF16>
-__global__ void __launch_bounds__(kBigStreamThreads, 1)
-attn_tc_bigstream_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                   const __grid_constant__ CUtensorMap tmap_v, const TcParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  BigStreamBarriers& bb = *reinterpret_cast<BigStreamBarriers*>(smem + kBigStreamItems * kBigStreamItemBytes);
-  // the shared softmax helpers address barriers through the common struct; alias the fields they touch
-  Barriers& bar = *reinterpret_cast<Barriers*>(smem + kBigStreamItems * kBigStreamItemBytes + 512);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int seg_lo = p.cta_seg_begin[blockIdx.x];
-  const int seg_hi = p.cta_seg_begin[blockIdx.x + 1];
-  constexpr int kMma = 4, kTma = 5;
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < kBigStreamItems; ++i) {
-      mbar_init(&bb.item_full[i], 1);
-      mbar_init(&bb.item_empty[i], 1);
-    }
-    mbar_init(&bb.s_full[0], 1);
-    mbar_init(&bb.s_full[1], 1);
-    mbar_init(&bar.p_full[0], 4);  // arrive_p_full() targets bar.p_full[c.wg]; c.wg = S buffer index here
-    mbar_init(&bar.p_full[1], 4);
-    mbar_init(&bb.pv_done, 1);
-    mbar_init(&bb.o_full, 1);
-    mbar_init(&bb.o_empty, 4);
-    fence_mbar_init();
-  }
-  if (warp == kMma) {
-    tmem_alloc(&bb.tmem_base, 512);
-    tmem_relinquish();
-  }
-  if (warp == kTma && lane == 0) {
-    tma_prefetch_desc(&tmap_q);
-    tma_prefetch_desc(&tmap_k);
-    tma_prefetch_desc(&tmap_v);
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem = bb.tmem_base;
-
-  if (warp < 4) {
-    // ===== softmax + epilogue: thread = query row =====
-    const int row = threadIdx.x;
-    const uint32_t lane_field = (uint32_t)((row >> 5) * 32) << 16;
-    const uint32_t tO = tmem + lane_field + 256u;
-    uint32_t n_tile = 0, n_o = 0;  // n_tile: key tiles processed by this CTA so far (all segments)
-    for (int sg = seg_lo; sg < seg_hi; ++sg) {
-      const Segment seg = p.segs[sg];
-      const int n = seg.q0 + row;
-      RowState st;
-      st.m_ref = -INFINITY;
-      st.l = 0.f;
-      TileCtx c;
-      c.tO = tO; c.row = row;
-      c.p_full_remote = 0;
-      c.pv_bar = &bb.pv_done;
-      c.cshift = n + p.causal_shift;
-      c.trace_on = false;
-      c.scale_log2 = p.scale_log2;
-      for (int t = seg.t0; t < seg.t1; ++t) {
-        const int j = t - seg.t0;
-        const uint32_t buf = n_tile & 1;  // S buffer (and its barriers) alternate over ALL tiles of the CTA
-        c.wg = (int)buf;
-        c.tS = tmem + lane_field + buf * 128u;
-        c.j0 = t * kTileN;
-        c.tt = j;
-        c.first_tile = (j == 0);
-        c.pv_parity = (n_tile + 1) & 1;  // phase of the previous tile's PV on pv_done
-        c.mw = make_uint4(0, 0, 0, 0);
-        if (p.pad_bits != nullptr)
-          c.mw = *reinterpret_cast<const uint4*>(p.pad_bits + (size_t)seg.b * p.pad_wpr + (size_t)t * 4);
-        const bool masked_tile =
-            __any_sync(0xffffffffu, (c.j0 + kTileN > p.M) || ((c.mw.x | c.mw.y | c.mw.z | c.mw.w) != 0u) ||
-                                        (p.causal && (c.j0 + kTileN - 1 > c.cshift)));
-        mbar_wait(&bb.s_full[buf], (n_tile >> 1) & 1, 12);
-        tc_fence_after_sync();
-        if (masked_tile) {
-          softmax_tile<256, BF16, true>(p, bar, c, st);
-        } else if (p.optimistic && !c.first_tile) {
-          if (!softmax_tile_optimistic<256, BF16, 0>(p, bar, c, st)) softmax_tile<256, BF16, false>(p, bar, c, st);
-        } else {
-          softmax_tile<256, BF16, false>(p, bar, c, st);
-        }
-        ++n_tile;
-      }
-      mbar_wait(&bb.o_full, n_o & 1, 13);
-      ++n_o;
-      tc_fence_after_sync();
-      epilogue_row<256, BF16, false>(p, seg, tO, n, row, st.l, st.m_ref);
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bb.o_empty);
-    }
-  } else if (warp == kTma) {
-    // ===== TMA producer; item order = consumption order: QK(0), QK(1), V(0), QK(2), V(1), ... =====
-    const bool leader = elect_one();
-    uint32_t it = 0;
-    auto load_qk = [&](const Segment& seg, int t) {
-      const int bq = p.q_bcast ? 0 : seg.b;
-      for (int ch = 0; ch < p.nc128; ++ch) {
-        const uint32_t slot = it % kBigStreamItems, par = (it / kBigStreamItems) & 1;
-        mbar_wait(&bb.item_empty[slot], par ^ 1, 2);
-        if (leader) {
-          uint8_t* base = smem + slot * kBigStreamItemBytes;
-          mbar_arrive_expect_tx(&bb.item_full[slot], (uint32_t)kBigStreamItemBytes);
-          tma_load_4d(base, &tmap_q, &bb.item_full[slot], ch * 128, seg.q0, seg.h, bq);
-          tma_load_4d(base + kBoxBytes, &tmap_q, &bb.item_full[slot], ch * 128 + 64, seg.q0, seg.h, bq);
-          tma_load_4d(base + 2 * kBoxBytes, &tmap_k, &bb.item_full[slot], ch * 128, t * kTileN, seg.h, seg.b);
-          tma_load_4d(base + 3 * kBoxBytes, &tmap_k, &bb.item_full[slot], ch * 128 + 64, t * kTileN, seg.h, seg.b);
-        }
-        ++it;
-      }
-    };
-    auto load_v = [&](const Segment& seg, int t) {
-      const uint32_t slot = it % kBigStreamItems, par = (it / kBigStreamItems) & 1;
-      mbar_wait(&bb.item_empty[slot], par ^ 1, 3);
-      if (leader) {
-        uint8_t* base = smem + slot * kBigStreamItemBytes;
-        mbar_arrive_expect_tx(&bb.item_full[slot], (uint32_t)(p.v_boxes * kBoxBytes));
-        for (int bx = 0; bx < p.v_boxes; ++bx)
-          tma_load_4d(base + bx * kBoxBytes, &tmap_v, &bb.item_full[slot], bx * 64, t * kTileN, seg.h, seg.b);
-      }
-      ++it;
-    };
-    for (int sg = seg_lo; sg < seg_hi; ++sg) {
-      const Segment seg = p.segs[sg];
-      load_qk(seg, seg.t0);
-      for (int t = seg.t0; t < seg.t1; ++t) {
-        if (t + 1 < seg.t1) load_qk(seg, t + 1);
-        load_v(seg, t);
-      }
-    }
-  } else if (warp == kMma) {
-    // ===== MMA issuer =====
-    const bool leader = elect_one();
-    constexpr uint32_t idesc_qk = make_idesc(kTileM, kTileN, BF16, false);
-    const uint32_t idesc_pv = make_idesc(kTileM, 64 * p.v_boxes, BF16, true);
-    const uint64_t d0 = make_smem_desc(smem_u32(smem), 16, 1024);          // K-major operands (Q / K chunks)
-    const uint64_t dv0 = make_smem_desc(smem_u32(smem), kBoxBytes, 1024);  // MN-major V tile
-    uint32_t it = 0, n_qk = 0, n_pvi = 0, n_oe = 0;  // n_qk / n_pvi: tiles whose QK^T / PV have been issued (all segments)
-    auto commit = [&](uint64_t* b) {
-      if (leader) tc_commit(b);
-    };
-    auto issue_qk = [&]() {  // S[n_qk & 1] = Q K^T of the next tile, accumulated over the channel chunks
-      const uint32_t buf = n_qk & 1;
-      for (int ch = 0; ch < p.nc128; ++ch) {
-        const uint32_t slot = it % kBigStreamItems;
-        mbar_wait(&bb.item_full[slot], (it / kBigStreamItems) & 1, 5);
-        ++it;
-        tc_fence_after_sync();
-        if (leader) {
-          const uint64_t da = d0 + (uint64_t)((slot * kBigStreamItemBytes) >> 4);
-          const uint64_t db = da + (uint64_t)((2 * kBoxBytes) >> 4);
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk) {
-            const uint64_t off = (uint64_t)(((kk >> 2) * kBoxBytes + (kk & 3) * 32) >> 4);
-            mma_ss(tmem + buf * 128, da + off, db + off, idesc_qk, (ch > 0 || kk > 0) ? 1u : 0u);
-          }
-        }
-        commit(&bb.item_empty[slot]);
-      }
-      commit(&bb.s_full[buf]);
-      ++n_qk;
-    };
-    for (int sg = seg_lo; sg < seg_hi; ++sg) {
-      const Segment seg = p.segs[sg];
-      const int nt = seg.t1 - seg.t0;
-      issue_qk();
-      for (int j = 0; j < nt; ++j) {
-        if (j + 1 < nt) issue_qk();
-        const uint32_t buf = n_pvi & 1;
-        const uint32_t slot = it % kBigStreamItems;
-        mbar_wait(&bb.item_full[slot], (it / kBigStreamItems) & 1, 6);
-        ++it;
-        if (j == 0) {
-          mbar_wait(&bb.o_empty, (n_oe & 1) ^ 1, 7);
-          ++n_oe;
-        }
-        mbar_wait(&bar.p_full[buf], (n_pvi >> 1) & 1, 8);
-        tc_fence_after_sync();
-        if (leader) {
-          const uint64_t db = dv0 + (uint64_t)((slot * kBigStreamItemBytes) >> 4);
-#pragma unroll
-          for (int kk = 0; kk < kTileN / 16; ++kk)
-            mma_ts(tmem + 256, tmem + buf * 128 + kk * 8, db + (uint64_t)((kk * 2048) >> 4), idesc_pv,
-                   (j > 0 || kk > 0) ? 1u : 0u);
-        }
-        commit(&bb.item_empty[slot]);
-        commit(&bb.pv_done);
-        ++n_pvi;
-      }
-      commit(&bb.o_full);
-    }
-  }
-
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == kMma) {
-    tc_fence_after_sync();
-    tmem_dealloc(bb.tmem_base, 512);
-  }
-}
-
-// --------------------------------------------------------------------------------------------------
-// Big-head kernel: qk head dims up to 512 and up to 384 v channels per pass (the optical-flow encoder / decoder
-// geometry: 322 and 512 channels per head, reference vision/optical_flow/backend.py:22-27,104-109).  One query tile
-// (128 rows) per CTA, 256 threads: warps 0-3 softmax (one thread per row), warp 4 MMA issuer, warp 5 TMA producer.
-//   * Q (128 rows x dqk) is RESIDENT in shared memory for the whole segment: ceil(dqk/64) boxes of 16 KB
-//     (the previous version re-streamed Q from L2 for every key tile).
-//   * K and V stream through ONE ring of 16 KB boxes (128 keys x 64 channels), 14 - #Q boxes slots: per key tile
-//     first the K boxes (K-major B operand of S += Q_box K_box^T, 4 MMAs of K = 16 per box, fewer for the ragged
-//     last box: dqk = 322 costs 21 K-steps, not 24), then the V boxes (MN-major B operand, N = 64 or the ragged
-//     tail, of O[:, box] += P V_box with P read from TMEM).
-//   * TMEM: S in columns [0, 128) (P aliases [0, 64) as in the main kernel), O in [128, 128 + 384): every v channel of
-//     dv <= 384 is produced in ONE pass (the previous version recomputed Q K^T for every 256-channel slice of V).
-//   * S is single-buffered, so per key tile the tensor pipe runs Q K^T, idles while the softmax warps turn S into P
-//     (one query tile per CTA: 1024 MUFU cycles) and runs P V; the in-order pipe makes "S(j) complete" imply
-//     "P V(j-1) complete", which is what the accumulator rescale and the S / P aliasing need.
-// --------------------------------------------------------------------------------------------------
-constexpr int kBigThreads = 256;
-constexpr int kBigSlots = 14;            // 16 KB boxes: Q boxes first, the rest is the K/V ring
-constexpr int kBigDv = 384;              // accumulator columns (one pass)
-constexpr int kBigSmemBytes = kBigSlots * kBoxBytes + 1024 + 1024;
-
-struct BigBarriers {
-  uint64_t box_full[kBigSlots], box_empty[kBigSlots];
-  uint64_t q_full, q_empty, s_full, o_full, o_empty;
-  uint32_t tmem_base;
-};
-
-template <bool BF16>
-__global__ void __launch_bounds__(kBigThreads, 1)
-attn_tc_big_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                   const __grid_constant__ CUtensorMap tmap_v, const TcParams p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  BigBarriers& bb = *reinterpret_cast<BigBarriers*>(smem + kBigSlots * kBoxBytes);
-  // the shared softmax helpers address p_full through the common struct; alias the fields they touch
-  Barriers& bar = *reinterpret_cast<Barriers*>(smem + kBigSlots * kBoxBytes + 512);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int seg_lo = p.cta_seg_begin[blockIdx.x];
-  const int seg_hi = p.cta_seg_begin[blockIdx.x + 1];
-  constexpr int kMma = 4, kTma = 5;
-  const int nqb = p.nc;                   // Q / K boxes (64 channels each)
-  const int nvb = p.v_boxes;              // V boxes of this pass
-  const int ring = kBigSlots - nqb;       // ring slots
-  uint8_t* ring_base = smem + nqb * kBoxBytes;
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < kBigSlots; ++i) {
-      mbar_init(&bb.box_full[i], 1);
-      mbar_init(&bb.box_empty[i], 1);
-    }
-    mbar_init(&bb.q_full, 1);
-    mbar_init(&bb.q_empty, 1);
-    mbar_init(&bb.s_full, 1);
-    mbar_init(&bar.p_full[0], 4);  // arrive_p_full() targets bar.p_full[c.wg], c.wg = 0 here
-    mbar_init(&bb.o_full, 1);
-    mbar_init(&bb.o_empty, 4);
-    fence_mbar_init();
-  }
-  if (warp == kMma) {
-    tmem_alloc(&bb.tmem_base, 512);
-    tmem_relinquish();
-  }
-  if (warp == kTma && lane == 0) {
-    tma_prefetch_desc(&tmap_q);
-    tma_prefetch_desc(&tmap_k);
-    tma_prefetch_desc(&tmap_v);
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem = bb.tmem_base;
-
-  if (warp < 4) {
-    // ===== softmax + epilogue: thread = query row =====
-    const int row = threadIdx.x;
-    const uint32_t lane_field = (uint32_t)((row >> 5) * 32) << 16;
-    const uint32_t tO = tmem + lane_field + 128u;
-    uint32_t n_tile = 0, n_o = 0;  // key tiles / segments processed by this CTA so far
-    for (int sg = seg_lo; sg < seg_hi; ++sg) {
-      const Segment seg = p.segs[sg];
-      const int n = seg.q0 + row;
-      RowState st;
-      st.m_ref = -INFINITY;
-      st.l = 0.f;
-      TileCtx c;
-      c.tS = tmem + lane_field;
-      c.tO = tO;
-      c.row = row;
-      c.wg = 0;
-      c.p_full_remote = 0;
-      c.pv_bar = nullptr;  // S(j) complete implies P V(j-1) complete (single S buffer, in-order tensor pipe)
-      c.pv_parity = 0;
-      c.cshift = n + p.causal_shift;
-      c.trace_on = false;
-      c.scale_log2 = p.scale_log2;
-      for (int t = seg.t0; t < seg.t1; ++t) {
-        c.j0 = t * kTileN;
-        c.tt = t - seg.t0;
-        c.first_tile = (t == seg.t0);
-        c.mw = make_uint4(0, 0, 0, 0);
-        if (p.pad_bits != nullptr)
-          c.mw = *reinterpret_cast<const uint4*>(p.pad_bits + (size_t)seg.b * p.pad_wpr + (size_t)t * 4);
-        const bool masked_tile =
-            __any_sync(0xffffffffu, (c.j0 + kTileN > p.M) || ((c.mw.x | c.mw.y | c.mw.z | c.mw.w) != 0u) ||
-                                        (p.causal && (c.j0 + kTileN - 1 > c.cshift)));
-        mbar_wait(&bb.s_full, n_tile & 1, 12);
-        tc_fence_after_sync();
-        if (masked_tile) {
-          softmax_tile<kBigDv, BF16, true>(p, bar, c, st);
-        } else if (p.optimistic && !c.first_tile) {
-          if (!softmax_tile_optimistic<kBigDv, BF16, 0>(p, bar, c, st)) softmax_tile<kBigDv, BF16, false>(p, bar, c, st);
-        } else {
-          softmax_tile<kBigDv, BF16, false>(p, bar, c, st);
-        }
-        ++n_tile;
-      }
-      mbar_wait(&bb.o_full, n_o & 1, 13);
-      ++n_o;
-      tc_fence_after_sync();
-      epilogue_row<kBigDv, BF16, false>(p, seg, tO, n, row, st.l, st.m_ref);
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bb.o_empty);
-    }
-  } else if (warp == kTma) {
-    // ===== TMA producer: Q boxes once per segment; per key tile the K boxes, then the V boxes, through the ring =====
-    const bool leader = elect_one();
-    uint32_t it = 0, n_q = 0;
-    for (int sg = seg_lo; sg < seg_hi; ++sg) {
-      const Segment seg = p.segs[sg];
-      const int bq = p.q_bcast ? 0 : seg.b;
-      mbar_wait(&bb.q_empty, (n_q & 1) ^ 1, 1);
-      ++n_q;
-      if (leader) {
-        mbar_arrive_expect_tx(&bb.q_full, (uint32_t)(nqb * kBoxBytes));
-        for (int bx = 0; bx < nqb; ++bx)
-          tma_load_4d(smem + bx * kBoxBytes, &tmap_q, &bb.q_full, bx * 64, seg.q0, seg.h, bq);
-      }
-      for (int t = seg.t0; t < seg.t1; ++t) {
-        for (int bx = 0; bx < nqb + nvb; ++bx, ++it) {
-          const uint32_t slot = it % ring, par = (it / ring) & 1;
-          mbar_wait(&bb.box_empty[slot], par ^ 1, 2);
-          if (leader) {
-            mbar_arrive_expect_tx(&bb.box_full[slot], (uint32_t)kBoxBytes);
-            if (bx < nqb)
-              tma_load_4d(ring_base + slot * kBoxBytes, &tmap_k, &bb.box_full[slot], bx * 64, t * kTileN, seg.h, seg.b);
+  if (wg == 0) {
+    reg_dealloc<40>();
+    if (threadIdx.x == 0) {
+      uint32_t it = 0;
+      for (int si = seg_lo; si < seg_hi; ++si) {
+        const Segment sg = p.segs[si];
+        mbar_wait(&bar.q_empty, ((si - seg_lo) & 1) ^ 1, 1);
+        mbar_arrive_expect_tx(&bar.q_full, C::kQBytes);
+        for (int c = 0; c < NQB; ++c)
+          tma_load_4d(sQ + c * kBoxBytes, &tq, &bar.q_full, c * 64, sg.q0 + qoff, sg.h, p.q_bcast ? 0 : sg.b);
+        for (int t = sg.t0; t < sg.t1; ++t) {
+#pragma unroll 1
+          for (int c = 0; c < NQB + NVB; ++c, ++it) {
+            const uint32_t s = it % NS;
+            mbar_wait(&bar.empty[s], ((it / NS) & 1) ^ 1, 2);
+            mbar_arrive_expect_tx(&bar.full[s], kBoxBytes);
+            const CUtensorMap* tm = c < NQB ? &tk : &tv;
+            const int ch = (c < NQB ? c : c - NQB) * 64;
+            if (PAIR)  // 64-key half `rank` of the box, into both CTAs
+              tma_load_4d_mc(sRing + s * kBoxBytes + rank * (kBoxBytes / 2), tm, &bar.full[s], ch,
+                             t * kTileN + 64 * (int)rank, sg.h, sg.b, 0x3);
             else
-              tma_load_4d(ring_base + slot * kBoxBytes, &tmap_v, &bb.box_full[slot], (bx - nqb) * 64, t * kTileN, seg.h,
-                          seg.b);
+              tma_load_4d(sRing + s * kBoxBytes, tm, &bar.full[s], ch, t * kTileN, sg.h, sg.b);
           }
         }
       }
     }
-  } else if (warp == kMma) {
-    // ===== MMA issuer =====
-    const bool leader = elect_one();
-    constexpr uint32_t idesc_qk = make_idesc(kTileM, kTileN, BF16, false);
-    const uint64_t dq0 = make_smem_desc(smem_u32(smem), 16, 1024);               // K-major Q boxes
-    const uint64_t dk0 = make_smem_desc(smem_u32(ring_base), 16, 1024);          // K-major K boxes
-    const uint64_t dv0 = make_smem_desc(smem_u32(ring_base), kBoxBytes, 1024);   // MN-major V boxes
-    uint32_t it = 0, n_q = 0, n_p = 0, n_oe = 0;
-    auto commit = [&](uint64_t* b) {
-      if (leader) tc_commit(b);
-    };
-    for (int sg = seg_lo; sg < seg_hi; ++sg) {
-      const Segment seg = p.segs[sg];
-      const int nt = seg.t1 - seg.t0;
-      mbar_wait(&bb.q_full, n_q & 1, 4);
-      ++n_q;
-      for (int j = 0; j < nt; ++j) {
-        // S = Q K^T over the channel boxes
-        for (int bx = 0; bx < nqb; ++bx, ++it) {
-          const uint32_t slot = it % ring;
-          mbar_wait(&bb.box_full[slot], (it / ring) & 1, 5);
-          tc_fence_after_sync();
-          if (leader) {
-            const int ksteps = min(4, (p.dqk_pad - bx * 64 + 15) / 16);
-            const uint64_t da = dq0 + (uint64_t)((bx * kBoxBytes) >> 4);
-            const uint64_t db = dk0 + (uint64_t)((slot * kBoxBytes) >> 4);
-            for (int kk = 0; kk < ksteps; ++kk)
-              mma_ss(tmem, da + (uint64_t)((kk * 32) >> 4), db + (uint64_t)((kk * 32) >> 4), idesc_qk,
-                     (bx > 0 || kk > 0) ? 1u : 0u);
-          }
-          commit(&bb.box_empty[slot]);
-        }
-        commit(&bb.s_full);
-        if (j == 0) {
-          mbar_wait(&bb.o_empty, (n_oe & 1) ^ 1, 7);
-          ++n_oe;
-        }
-        mbar_wait(&bar.p_full[0], n_p & 1, 8);
-        ++n_p;
-        tc_fence_after_sync();
-        // O[:, box] += P V_box
-        for (int bx = 0; bx < nvb; ++bx, ++it) {
-          const uint32_t slot = it % ring;
-          mbar_wait(&bb.box_full[slot], (it / ring) & 1, 6);
-          tc_fence_after_sync();
-          if (leader) {
-            const int ncols = min(64, p.dv_cols - bx * 64);
-            const uint32_t idesc_pv = make_idesc(kTileM, ncols, BF16, true);
-            const uint64_t db = dv0 + (uint64_t)((slot * kBoxBytes) >> 4);
-#pragma unroll
-            for (int kk = 0; kk < kTileN / 16; ++kk)
-              mma_ts(tmem + 128 + bx * 64, tmem + kk * 8, db + (uint64_t)((kk * 2048) >> 4), idesc_pv,
-                     (j > 0 || kk > 0) ? 1u : 0u);
-          }
-          commit(&bb.box_empty[slot]);
-        }
-      }
-      commit(&bb.q_empty);
-      commit(&bb.o_full);
+    if (PAIR) {
+      __syncwarp();
+      cluster_sync_all();  // the peer may still multicast into / arrive on this CTA's shared memory until here
     }
+    return;
   }
 
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == kMma) {
-    tc_fence_after_sync();
-    tmem_dealloc(bb.tmem_base, 512);
+  reg_alloc<232>();
+  const int cw = wg - 1;                 // consumer warpgroup: query rows [64*cw, 64*cw + 64) of the tile
+  const int tid = threadIdx.x - 128 * wg;
+  const int warp = tid >> 5, lane = tid & 31;
+  const int rloc = 64 * cw + 16 * warp + (lane >> 2);  // rows rloc and rloc + 8
+  const int cq = 2 * (lane & 3);                      // first of the two columns of every 8-column group
+  const uint32_t q_base = smem_u32(sQ) + cw * 64 * 128;
+  const uint32_t ring_base = smem_u32(sRing);
+  uint32_t it = 0;
+
+  for (int si = seg_lo; si < seg_hi; ++si) {
+    const Segment sg = p.segs[si];
+    mbar_wait(&bar.q_full, (si - seg_lo) & 1, 3);
+    float o[NVB][32];
+#pragma unroll
+    for (int v = 0; v < NVB; ++v)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) o[v][i] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+    const int n0 = sg.q0 + qoff + rloc;
+
+    for (int t = sg.t0; t < sg.t1; ++t) {
+      float s[64];
+#pragma unroll
+      for (int c = 0; c < NQB; ++c, ++it) {
+        const uint32_t sl = it % NS;
+        mbar_wait(&bar.full[sl], (it / NS) & 1, 4);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk)
+          wgmma_ss<128, BF16>(s, make_desc(q_base + c * kBoxBytes + kk * 32), make_desc(ring_base + sl * kBoxBytes + kk * 32),
+                              (c | kk) != 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(s);
+        if (PAIR) warp_arrive_pair(&bar.empty[sl]);
+        else warp_arrive(&bar.empty[sl]);
+      }
+      // scores -> log2 domain with the masks; row maxima over the quad
+      const int j0 = t * kTileN;
+      float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+      for (int g = 0; g < 16; ++g) {
+        const int jb = j0 + 8 * g + cq;
+        uint32_t padw = 0;
+        if (p.pad_bits != nullptr) padw = p.pad_bits[(int64_t)sg.b * p.pad_wpr + (jb >> 5)];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int j = jb + (e & 1);
+          const int n = n0 + 8 * (e >> 1);
+          float x = s[4 * g + e] * p.scale_log2;
+          if (j >= p.M) x = -INFINITY;
+          else if (((padw >> (j & 31)) & 1u) || (p.causal && j > n + p.causal_shift)) x = kMaskedScore;
+          s[4 * g + e] = x;
+          mx[e >> 1] = fmaxf(mx[e >> 1], x);
+        }
+      }
+      float mref[2], alpha[2];
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+        const float mn = fmaxf(m_run[r], mx[r]);
+        alpha[r] = (mn == -INFINITY) ? 1.f : ex2(m_run[r] - mn);
+        mref[r] = (mn == -INFINITY) ? 0.f : mn;
+        m_run[r] = mn;
+        l_run[r] *= alpha[r];
+      }
+#pragma unroll
+      for (int v = 0; v < NVB; ++v)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) o[v][i] *= alpha[(i >> 1) & 1];
+      uint32_t pa[8][4];
+#pragma unroll
+      for (int g = 0; g < 16; ++g) {
+        const float e0 = ex2(s[4 * g + 0] - mref[0]), e1 = ex2(s[4 * g + 1] - mref[0]);
+        const float e2 = ex2(s[4 * g + 2] - mref[1]), e3 = ex2(s[4 * g + 3] - mref[1]);
+        l_run[0] += e0 + e1;
+        l_run[1] += e2 + e3;
+        pa[g >> 1][(g & 1) * 2 + 0] = pack2(e0, e1, BF16);
+        pa[g >> 1][(g & 1) * 2 + 1] = pack2(e2, e3, BF16);
+      }
+#pragma unroll
+      for (int v = 0; v < NVB; ++v, ++it) {
+        const uint32_t sl = it % NS;
+        mbar_wait(&bar.full[sl], (it / NS) & 1, 5);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk) wgmma_rs<64, BF16>(o[v], pa[kk], make_desc(ring_base + sl * kBoxBytes + kk * 2048));
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(o[v]);
+        if (PAIR) warp_arrive_pair(&bar.empty[sl]);
+        else warp_arrive(&bar.empty[sl]);
+      }
+    }
+    warp_arrive(&bar.q_empty);  // every wgmma reading Q of this segment has completed
+
+    // epilogue: quad-reduce the denominators, write final rows / caller's partial state / split slots
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
+      l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int rr = qoff + rloc + 8 * r;  // row within the unit (slot row)
+      const int n = sg.q0 + rr;
+      if (n >= p.N) continue;
+      if (sg.slot >= 0) {
+        const int64_t row = (int64_t)sg.slot * p.slot_rows + rr;
+        float* dst = p.slot_o + row * (NVB * 64);
+#pragma unroll
+        for (int v = 0; v < NVB; ++v)
+#pragma unroll
+          for (int g = 0; g < 8; ++g)
+            *reinterpret_cast<float2*>(dst + v * 64 + 8 * g + cq) = make_float2(o[v][4 * g + 2 * r], o[v][4 * g + 2 * r + 1]);
+        if ((lane & 3) == 0) {
+          p.slot_m[row] = m_run[r];
+          p.slot_l[row] = l_run[r];
+        }
+      } else if (p.write_partial) {
+        const int64_t row = ((int64_t)sg.b * p.H + sg.h) * p.N + n;
+        float* dst = p.fin_o + row * p.dv + p.dv_off;
+#pragma unroll
+        for (int v = 0; v < NVB; ++v)
+#pragma unroll
+          for (int g = 0; g < 8; ++g) {
+            const int c = v * 64 + 8 * g + cq;
+            if (c < p.dv_pass) *reinterpret_cast<float2*>(dst + c) = make_float2(o[v][4 * g + 2 * r], o[v][4 * g + 2 * r + 1]);
+          }
+        if ((lane & 3) == 0) {
+          p.fin_m[row] = m_run[r];
+          p.fin_l[row] = l_run[r];
+        }
+      } else {
+        const float inv = 1.f / l_run[r];
+        char* orow = reinterpret_cast<char*>(p.out) +
+                     2 * ((int64_t)sg.b * p.osb + (int64_t)n * p.osn + (int64_t)sg.h * p.osh + p.dv_off);
+#pragma unroll
+        for (int v = 0; v < NVB; ++v)
+#pragma unroll
+          for (int g = 0; g < 8; ++g) {
+            const int c = v * 64 + 8 * g + cq;
+            if (c < p.dv_pass)
+              *reinterpret_cast<uint32_t*>(orow + 2 * c) = pack2(o[v][4 * g + 2 * r] * inv, o[v][4 * g + 2 * r + 1] * inv, BF16);
+          }
+      }
+    }
   }
+  if (PAIR) cluster_sync_all();
 }
 
 // --------------------------------------------------------------------------------------------------
@@ -2047,7 +651,7 @@ void build_plan(Plan& pl, int B, int H, int N, int M, int num_sms, int rows_per_
   pl.num_units = (int)pl.units.size();
 }
 
-// watchdog record shared with the device (see mbar_wait in pcv_sm100.cuh)
+// watchdog record shared with the device (see mbar_wait in pcv_sm90.cuh)
 uint32_t* g_diag_host = nullptr;
 std::map<int, bool> g_diag_set;  // per device
 
@@ -2059,12 +663,11 @@ int ensure_diag(int dev) {
   }
   uint32_t* dptr = nullptr;
   PCV_CHECK_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&dptr), g_diag_host, 0));
-  PCV_CHECK_CUDA(cudaMemcpyToSymbol(sm100::g_wait_diag, &dptr, sizeof(dptr)));
+  PCV_CHECK_CUDA(cudaMemcpyToSymbol(sm90::g_wait_diag, &dptr, sizeof(dptr)));
   g_diag_set[dev] = true;
   return PCV_OK;
 }
 
-unsigned long long* g_trace_dev = nullptr;  // PCV_TRACE=1
 
 std::mutex g_plan_mu;
 std::mutex g_attr_mu;  // guards the per-device cudaFuncSetAttribute flags of every kernel instantiation
@@ -2076,10 +679,10 @@ std::map<PlanKey, std::shared_ptr<Plan>> g_plans;
 uint64_t g_plan_seq = 0;
 constexpr size_t kMaxPlans = 256;
 
+
 struct Mode {
   int rows_per_unit, rows_per_tile, slot_rows;
-  bool big;   // big-head kernels (qk head dim > 128 or v head dim > 256)
-  bool pair;  // cta_group::2 kernel: workers are CTA pairs, 512 query rows per unit
+  bool pair;  // 2-CTA clusters: workers are CTA pairs, 256 query rows per unit
 };
 
 void free_plan_tables(Plan& pl) {
@@ -2187,34 +790,22 @@ int make_tmap(CUtensorMap* tm, const void* base, int dtype, int channels, int ro
 inline int pad64(int d) { return (d + 63) / 64 * 64; }
 
 size_t slots_bytes(const Plan& pl, int DV, int slot_rows) {
-  // [slot][row][DV] numerators, [slot][row] row max, [slot][row] denominators, then [slot][16] 64-bit fix-up flags
-  return sizeof(float) * (size_t)pl.num_slots * slot_rows * (DV + 2) + sizeof(unsigned long long) * (size_t)pl.num_slots * kFlagsPerSlot;
+  // [slot][row][DV] numerators, [slot][row] row max, [slot][row] denominators
+  return sizeof(float) * (size_t)pl.num_slots * slot_rows * (DV + 2);
 }
-
-// The CTA-pair kernel takes a call when it is asked for (impl = PCV_IMPL_TCGEN05_PAIR) or, with impl = AUTO, when the
-// shape is its home ground: v head dim <= 128 and at least two 256-row query tiles per (b, h), i.e. N > 256.
-bool pair_wanted(const pcv_attn_params& a) {
-  if (pad64(a.dv) > 128 || pad64(a.dqk) > 128) return false;
-  int dev = 0, sms = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return false;
-  if (sms < 2 || (sms % 2)) return false;
-  if (a.impl == PCV_IMPL_TCGEN05_PAIR) return true;
-  return kPairByDefault && a.impl == PCV_IMPL_AUTO && a.N > kRowsPerUnit;
-}
-
+// The CTA-pair kernel takes a call only when it is asked for (impl = PCV_IMPL_TCGEN05_PAIR).
 Mode choose_mode(const pcv_attn_params& a) {
-  const int DV = pad64(a.dv);
-  if (pad64(a.dqk) > 128 || DV > 256) return Mode{kTileM, kTileM, kTileM, true, false};
-  if (DV > 128) return Mode{kTileM, kTileM, kRowsPerUnit, false, false};
-  if (pair_wanted(a)) return Mode{4 * kTileM, 2 * kTileM, 4 * kTileM, false, true};
-  return Mode{kRowsPerUnit, kTileM, kRowsPerUnit, false, false};
+  if (a.impl == PCV_IMPL_TCGEN05_PAIR) return Mode{2 * kTileM, kTileM, 2 * kTileM, true};
+  return Mode{kTileM, kTileM, kTileM, false};
 }
 
-template <int DQK, int DV, bool BF16>
-int launch_cfg(const pcv_attn_params& a, const Plan& pl, const CUtensorMap& tq, const CUtensorMap& tk,
-               const CUtensorMap& tv, TcParams& p, cudaStream_t stream) {
-  using C = Cfg<DQK, DV>;
-  auto kern = attn_tc_kernel<DQK, DV, BF16>;
+int dv_pass_width(int dv) { return std::min(kMaxDvPass, pad64(dv)); }
+
+template <int NQB, int NVB, bool BF16, bool PAIR>
+int launch_fwd(const Plan& pl, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const TcParams& p,
+               cudaStream_t stream) {
+  using C = FwdCfg<NQB, NVB>;
+  auto kern = attn_fwd_kernel<NQB, NVB, BF16, PAIR>;
   static bool attr_set[64] = {};  // per instantiation and device
   int dev = 0;
   PCV_CHECK_CUDA(cudaGetDevice(&dev));
@@ -2225,123 +816,78 @@ int launch_cfg(const pcv_attn_params& a, const Plan& pl, const CUtensorMap& tq, 
       if (dev >= 0 && dev < 64) attr_set[dev] = true;
     }
   }
-  if (p.tail.enabled || pl.num_units > 0) {
-    // grid-wide arrivals of the merge tail and the in-kernel fix-up of split units (one part waits for flags written
-    // by other CTAs) both need every CTA of the grid co-resident
-    int sms = 0;
-    PCV_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    PCV_REQUIRE(pl.num_ctas <= sms, PCV_ERR_UNSUPPORTED, "%d CTAs cannot be co-resident on %d SMs", pl.num_ctas, sms);
-  }
   prof_mark_begin(stream);
-  kern<<<pl.num_ctas, kThreads, C::kSmemBytes, stream>>>(tq, tk, tv, p);
-  prof_mark_end(stream);
-  PCV_CHECK_CUDA(cudaGetLastError());
-  count_launch();
-  return PCV_OK;  // split units are merged by the fix-up in the kernel's own epilogue: no second launch
-}
-
-template <int DQK, bool BF16>
-int launch_pair(const pcv_attn_params& a, const Plan& pl, const CUtensorMap& tq, const CUtensorMap& tk,
-                const CUtensorMap& tv, TcParams& p, cudaStream_t stream) {
-  using C = PairCfg<DQK>;
-  auto kern = attn_tc_pair_kernel<DQK, BF16>;
-  static bool attr_set[64] = {};
-  int dev = 0;
-  PCV_CHECK_CUDA(cudaGetDevice(&dev));
-  {
-    std::lock_guard<std::mutex> lk(g_attr_mu);
-    if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-      PCV_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes));
-      if (dev >= 0 && dev < 64) attr_set[dev] = true;
-    }
+  if (PAIR) {
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(2 * pl.num_ctas);  // num_ctas counts CTA pairs in this mode
+    cfg.blockDim = dim3(kThreads);
+    cfg.dynamicSmemBytes = C::kSmemBytes;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = 2;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    PCV_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, tq, tk, tv, p));
+  } else {
+    kern<<<pl.num_ctas, kThreads, C::kSmemBytes, stream>>>(tq, tk, tv, p);
   }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(2 * pl.num_ctas);  // num_ctas counts CTA pairs in this mode
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = C::kSmemBytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  prof_mark_begin(stream);
-  PCV_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, tq, tk, tv, p));
-  prof_mark_end(stream);
-  count_launch();
-  return PCV_OK;  // split units are fixed up inside the kernel
-}
-
-template <bool BF16>
-int launch_bigstream(const Plan& pl, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, TcParams& p,
-                     cudaStream_t stream) {
-  auto kern = attn_tc_bigstream_kernel<BF16>;
-  static bool attr_set[64] = {};
-  int dev = 0;
-  PCV_CHECK_CUDA(cudaGetDevice(&dev));
-  {
-    std::lock_guard<std::mutex> lk(g_attr_mu);
-    if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-      PCV_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kBigStreamSmemBytes));
-      if (dev >= 0 && dev < 64) attr_set[dev] = true;
-    }
-  }
-  prof_mark_begin(stream);
-  kern<<<pl.num_ctas, kBigStreamThreads, kBigStreamSmemBytes, stream>>>(tq, tk, tv, p);
   prof_mark_end(stream);
   PCV_CHECK_CUDA(cudaGetLastError());
   count_launch();
   if (pl.num_units > 0) {
     dim3 grid(pl.num_units, p.slot_rows / 8);
-    tc_combine_kernel<256, BF16><<<grid, 256, 0, stream>>>(pl.d_units, p);
+    if (NVB == 1)
+      tc_combine_kernel<64, BF16><<<grid, 256, 0, stream>>>(pl.d_units, p);
+    else
+      tc_combine_kernel<128, BF16><<<grid, 256, 0, stream>>>(pl.d_units, p);
     PCV_CHECK_CUDA(cudaGetLastError());
     count_launch();
   }
   return PCV_OK;
 }
 
+template <int NQB, bool BF16>
+int launch_nqb(int nvb, bool pair, const Plan& pl, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
+               const TcParams& p, cudaStream_t stream) {
+  if constexpr (NQB <= 2) {
+    if (pair)
+      return nvb == 1 ? launch_fwd<NQB, 1, BF16, true>(pl, tq, tk, tv, p, stream)
+                      : launch_fwd<NQB, 2, BF16, true>(pl, tq, tk, tv, p, stream);
+  }
+  return nvb == 1 ? launch_fwd<NQB, 1, BF16, false>(pl, tq, tk, tv, p, stream)
+                  : launch_fwd<NQB, 2, BF16, false>(pl, tq, tk, tv, p, stream);
+}
+
 template <bool BF16>
-int launch_big(const Plan& pl, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, TcParams& p,
-               cudaStream_t stream) {
-  auto kern = attn_tc_big_kernel<BF16>;
-  static bool attr_set[64] = {};
-  int dev = 0;
-  PCV_CHECK_CUDA(cudaGetDevice(&dev));
-  {
-    std::lock_guard<std::mutex> lk(g_attr_mu);
-    if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-      PCV_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kBigSmemBytes));
-      if (dev >= 0 && dev < 64) attr_set[dev] = true;
-    }
+int launch_dispatch(int nqb, int nvb, bool pair, const Plan& pl, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
+                    const TcParams& p, cudaStream_t stream) {
+  switch (nqb) {
+    case 1: return launch_nqb<1, BF16>(nvb, pair, pl, tq, tk, tv, p, stream);
+    case 2: return launch_nqb<2, BF16>(nvb, pair, pl, tq, tk, tv, p, stream);
+    case 3: return launch_nqb<3, BF16>(nvb, pair, pl, tq, tk, tv, p, stream);
+    case 4: return launch_nqb<4, BF16>(nvb, pair, pl, tq, tk, tv, p, stream);
+    case 5: return launch_nqb<5, BF16>(nvb, pair, pl, tq, tk, tv, p, stream);
+    case 6: return launch_nqb<6, BF16>(nvb, pair, pl, tq, tk, tv, p, stream);
+    case 7: return launch_nqb<7, BF16>(nvb, pair, pl, tq, tk, tv, p, stream);
+    case 8: return launch_nqb<8, BF16>(nvb, pair, pl, tq, tk, tv, p, stream);
   }
-  prof_mark_begin(stream);
-  kern<<<pl.num_ctas, kBigThreads, kBigSmemBytes, stream>>>(tq, tk, tv, p);
-  prof_mark_end(stream);
-  PCV_CHECK_CUDA(cudaGetLastError());
-  count_launch();
-  if (pl.num_units > 0) {
-    dim3 grid(pl.num_units, p.slot_rows / 8);
-    tc_combine_kernel<kBigDv, BF16><<<grid, 256, 0, stream>>>(pl.d_units, p);
-    PCV_CHECK_CUDA(cudaGetLastError());
-    count_launch();
-  }
-  return PCV_OK;
+  set_error("tensor-core attention: qk head dim needs %d 64-channel boxes (at most 8)", nqb);
+  return PCV_ERR_UNSUPPORTED;
 }
 
 }  // namespace
 
 int debug_trace_read(unsigned long long* out, int n) {
-  // n >= 3*48*8: the clock stamps; n >= that + 8*1024: also the per-CTA records
-  const int full = kTraceStamps + 8 * kTraceMaxCtas;
-  if (g_trace_dev == nullptr || n < kTraceStamps) return PCV_ERR_INVALID;
-  const int total = n >= full ? full : kTraceStamps;
-  PCV_CHECK_CUDA(cudaMemcpy(out, g_trace_dev, sizeof(unsigned long long) * total, cudaMemcpyDeviceToHost));
-  return PCV_OK;
+  (void)out;
+  (void)n;
+  set_error("debug_trace_read: the Hopper kernels record no clock trace");
+  return PCV_ERR_UNSUPPORTED;
 }
 
-// Host-only (no CUDA call): the work plan of the tcgen05 kernels for a problem, one record of 8 ints per segment
+// Host-only (no CUDA call): the work plan of the tensor-core kernel for a problem, one record of 8 ints per segment
 // {cta, b, h, q0, ntile, t0, t1, slot}; tests/test_plan_cpu.py checks its invariants on the CPU.
 int debug_plan(int B, int H, int N, int M, int workers, int rows_per_unit, int rows_per_tile, int32_t* segs,
                int max_segs, int32_t* counts) {
@@ -2390,7 +936,7 @@ bool attn_tc_supported(const pcv_attn_params& p, const char** why) {
   int dev = 0, major = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess)
     return fail("no CUDA device");
-  if (major != 10) return fail("device is not sm_100");
+  if (major != 9) return fail("device is not sm_90");
   return true;
 }
 
@@ -2399,7 +945,7 @@ int attn_tc_workspace_bytes(const pcv_attn_params& p, size_t* bytes) {
   const Mode mode = choose_mode(p);
   int rc = get_plan(p.B, p.H, p.N, p.M, mode, &pl);
   if (rc != PCV_OK) return rc;
-  size_t b = slots_bytes(*pl, mode.big ? kBigDv : pad64(p.dv), mode.slot_rows);
+  size_t b = slots_bytes(*pl, dv_pass_width(p.dv), mode.slot_rows);
   b = (b + 255) / 256 * 256;
   if (p.pad_mask != nullptr) b += sizeof(uint32_t) * (size_t)p.B * ((p.M + kTileN - 1) / kTileN * 4);
   *bytes = b;
@@ -2408,11 +954,6 @@ int attn_tc_workspace_bytes(const pcv_attn_params& p, size_t* bytes) {
 
 bool attn_tc_fuse_supported(const pcv_attn_params& a, const char** why) {
   if (!attn_tc_supported(a, why)) return false;
-  const Mode mode = choose_mode(a);
-  if (mode.big) {
-    *why = "the fused merge tail is built into the head-dim <= 128 / v-dim <= 256 kernel only";
-    return false;
-  }
   if (a.dv % 4) {
     *why = "fused merge needs v head dim % 4 == 0";
     return false;
@@ -2421,26 +962,33 @@ bool attn_tc_fuse_supported(const pcv_attn_params& a, const char** why) {
 }
 
 int launch_attn_tc(const pcv_attn_params& a, cudaStream_t stream, const pcv_shard_fuse* fuse) {
+  {
+    const char* why = "";
+    PCV_REQUIRE(attn_tc_supported(a, &why), PCV_ERR_UNSUPPORTED, "tensor-core attention: %s", why);
+  }
   std::shared_ptr<Plan> pl;
-  const int DQK = pad64(a.dqk), DV = pad64(a.dv);
   const Mode mode = choose_mode(a);
-  PCV_REQUIRE(mode.pair || a.impl != PCV_IMPL_TCGEN05_PAIR, PCV_ERR_UNSUPPORTED,
-              "the cta_group::2 kernel needs qk and v head dims <= 128 and an even SM count");
+  if (mode.pair) {
+    int dev = 0, sms = 0;
+    PCV_CHECK_CUDA(cudaGetDevice(&dev));
+    PCV_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    PCV_REQUIRE(pad64(a.dqk) <= 128 && pad64(a.dv) <= 128 && sms >= 2, PCV_ERR_UNSUPPORTED,
+                "the CTA-pair kernel needs qk and v head dims <= 128 and at least two SMs");
+  }
   int rc = get_plan(a.B, a.H, a.N, a.M, mode, &pl);
   if (rc != PCV_OK) return rc;
   size_t need = 0;
-  attn_tc_workspace_bytes(a, &need);
+  rc = attn_tc_workspace_bytes(a, &need);
+  if (rc != PCV_OK) return rc;
   PCV_REQUIRE(need == 0 || (a.workspace != nullptr && a.workspace_bytes >= need), PCV_ERR_WORKSPACE,
-              "tcgen05 attention: workspace of %zu bytes required, %zu given", need, a.workspace_bytes);
+              "tensor-core attention: workspace of %zu bytes required, %zu given", need, a.workspace_bytes);
   PCV_REQUIRE(need == 0 || (reinterpret_cast<uintptr_t>(a.workspace) & 15) == 0, PCV_ERR_WORKSPACE,
-              "tcgen05 attention: workspace must be 16-byte aligned");
+              "tensor-core attention: workspace must be 16-byte aligned");
 
   TcParams p{};
   p.segs = pl->d_segs;
   p.cta_seg_begin = pl->d_cta;
   p.B = a.B; p.H = a.H; p.N = a.N; p.M = a.M; p.dv = a.dv;
-  p.dv_off = 0;
-  p.dv_pass = a.dv;
   p.scale_log2 = a.scale * kLog2e;
   p.causal = a.causal;
   p.causal_shift = (a.m_total - a.N) - a.m_offset;
@@ -2449,19 +997,6 @@ int launch_attn_tc(const pcv_attn_params& a, cudaStream_t stream, const pcv_shar
   p.write_partial = a.write_partial;
   p.rows_per_unit = mode.rows_per_unit;
   p.slot_rows = mode.slot_rows;
-  p.optimistic = 1;
-  p.mmaopt = 3;
-#ifdef PCV_ENABLE_TRACE  // developer build only (make TRACE=1)
-  {
-    static const int trace = [] { const char* e = getenv("PCV_TRACE"); return e ? atoi(e) : 0; }();
-    if (trace) {
-      const size_t bytes = sizeof(unsigned long long) * (kTraceStamps + 8 * kTraceMaxCtas);
-      if (g_trace_dev == nullptr) PCV_CHECK_CUDA(cudaMalloc(&g_trace_dev, bytes));
-      PCV_CHECK_CUDA(cudaMemsetAsync(g_trace_dev, 0, bytes, stream));
-      p.trace = g_trace_dev;
-    }
-  }
-#endif
   p.fin_o = a.part_o; p.fin_m = a.part_m; p.fin_l = a.part_l;
   if (fuse != nullptr) {
     const char* why = "";
@@ -2489,32 +1024,19 @@ int launch_attn_tc(const pcv_attn_params& a, cudaStream_t stream, const pcv_shar
     p.fin_m = const_cast<float*>(t.part_m[fuse->rank]);
     p.fin_l = const_cast<float*>(t.part_l[fuse->rank]);
   }
+  const int slot_dv = dv_pass_width(a.dv);
   char* ws = reinterpret_cast<char*>(a.workspace);
   const size_t nrows = (size_t)pl->num_slots * mode.slot_rows;
-  const int slot_dv = mode.big ? kBigDv : DV;
   p.slot_o = reinterpret_cast<float*>(ws);
   p.slot_m = p.slot_o + nrows * slot_dv;
   p.slot_l = p.slot_m + nrows;
-  p.slot_flags = reinterpret_cast<unsigned long long*>(p.slot_l + nrows);  // 8-byte aligned: nrows is a multiple of 128
-  p.units = pl->d_units;
-  {
-    // unique per launch in this process; the upper bits keep it apart from anything a stale workspace may hold
-    static std::atomic<unsigned long long> launch_seq{0};
-    p.fixup_tag = 0x5043560000000000ull ^ (launch_seq.fetch_add(1, std::memory_order_relaxed) + 1);
-  }
-  if (pl->num_units > 0 && !mode.big) {
-    // The per-launch tag alone is not enough once a launch is REPLAYED from a CUDA graph (the recorded tag repeats and
-    // the flags of the previous replay would satisfy this one): clear the flags in stream order (a memset node under
-    // capture).  num_slots * 128 bytes.
-    PCV_CHECK_CUDA(cudaMemsetAsync(p.slot_flags, 0, sizeof(unsigned long long) * (size_t)pl->num_slots * kFlagsPerSlot, stream));
-  }
   if (a.pad_mask != nullptr) {
     size_t off = (slots_bytes(*pl, slot_dv, mode.slot_rows) + 255) / 256 * 256;
     uint32_t* bits = reinterpret_cast<uint32_t*>(ws + off);
     p.pad_wpr = (a.M + kTileN - 1) / kTileN * 4;
     p.pad_bits = bits;
     const int64_t total = (int64_t)a.B * p.pad_wpr;
-    int blocks = (int)std::min<int64_t>((total + 255) / 256, 148 * 8);
+    int blocks = (int)std::min<int64_t>((total + 255) / 256, 1024);
     pack_pad_kernel<<<blocks, 256, 0, stream>>>(a.pad_mask, a.pad_stride_b, a.B, a.M, p.pad_wpr, bits);
     PCV_CHECK_CUDA(cudaGetLastError());
     count_launch();
@@ -2524,65 +1046,35 @@ int launch_attn_tc(const pcv_attn_params& a, cudaStream_t stream, const pcv_shar
   const int Bq = a.q_stride_b == 0 ? 1 : a.B;
   rc = make_tmap(&tq, a.q, a.dtype, a.dqk, a.N, a.H, Bq, a.q_stride_n, a.q_stride_h, a.q_stride_b);
   if (rc != PCV_OK) return rc;
-  rc = make_tmap(&tk, a.k, a.dtype, a.dqk, a.M, a.H, a.B, a.k_stride_m, a.k_stride_h, a.k_stride_b,
-                 mode.pair ? kTileN / 2 : kTileN);  // the pair kernel loads 64-key halves of every K tile
+  const int kv_box_rows = mode.pair ? kTileN / 2 : kTileN;  // a pair loads 64-key halves of every K / V tile
+  rc = make_tmap(&tk, a.k, a.dtype, a.dqk, a.M, a.H, a.B, a.k_stride_m, a.k_stride_h, a.k_stride_b, kv_box_rows);
   if (rc != PCV_OK) return rc;
-  rc = make_tmap(&tv, a.v, a.dtype, a.dv, a.M, a.H, a.B, a.v_stride_m, a.v_stride_h, a.v_stride_b);
-  if (rc != PCV_OK) return rc;
-
   const bool bf = a.dtype == PCV_BF16;
-  if (mode.big && (a.dqk > kBigDv || a.dv > kBigDv)) {
-    // widest heads (optical-flow decoder 512 / 512): streaming kernel, one launch per 256-channel slice of V
-    p.nc128 = (a.dqk + 127) / 128;
-    for (int off = 0; off < a.dv; off += 256) {
-      p.dv_off = off;
-      p.dv_pass = std::min(256, a.dv - off);
-      p.v_boxes = (p.dv_pass + 63) / 64;
-      const char* vbase = reinterpret_cast<const char*>(a.v) + 2 * (size_t)off;
-      rc = make_tmap(&tv, vbase, a.dtype, p.dv_pass, a.M, a.H, a.B, a.v_stride_m, a.v_stride_h, a.v_stride_b);
-      if (rc != PCV_OK) return rc;
-      rc = bf ? launch_bigstream<true>(*pl, tq, tk, tv, p, stream) : launch_bigstream<false>(*pl, tq, tk, tv, p, stream);
-      if (rc != PCV_OK) return rc;
-    }
-    return PCV_OK;
+  const int nqb = pad64(a.dqk) / 64;
+  // one launch per slice of at most 128 V channels (the scores are recomputed per slice)
+  for (int off = 0; off < a.dv; off += kMaxDvPass) {
+    p.dv_off = off;
+    p.dv_pass = std::min(kMaxDvPass, a.dv - off);
+    const int nvb = (p.dv_pass + 63) / 64;
+    const char* vbase = reinterpret_cast<const char*>(a.v) + 2 * (size_t)off;
+    rc = make_tmap(&tv, vbase, a.dtype, p.dv_pass, a.M, a.H, a.B, a.v_stride_m, a.v_stride_h, a.v_stride_b, kv_box_rows);
+    if (rc != PCV_OK) return rc;
+    rc = bf ? launch_dispatch<true>(nqb, nvb, mode.pair, *pl, tq, tk, tv, p, stream)
+            : launch_dispatch<false>(nqb, nvb, mode.pair, *pl, tq, tk, tv, p, stream);
+    if (rc != PCV_OK) return rc;
   }
-  if (mode.big) {
-    // one launch per 384-channel slice of V (the scores are recomputed per slice; dv <= 384 is a single pass)
-    p.nc = (a.dqk + 63) / 64;
-    p.dqk_pad = (a.dqk + 15) / 16 * 16;
-    for (int off = 0; off < a.dv; off += kBigDv) {
-      p.dv_off = off;
-      p.dv_pass = std::min(kBigDv, a.dv - off);
-      p.v_boxes = (p.dv_pass + 63) / 64;
-      p.dv_cols = (p.dv_pass + 15) / 16 * 16;
-      const char* vbase = reinterpret_cast<const char*>(a.v) + 2 * (size_t)off;
-      rc = make_tmap(&tv, vbase, a.dtype, p.dv_pass, a.M, a.H, a.B, a.v_stride_m, a.v_stride_h, a.v_stride_b);
-      if (rc != PCV_OK) return rc;
-      rc = bf ? launch_big<true>(*pl, tq, tk, tv, p, stream) : launch_big<false>(*pl, tq, tk, tv, p, stream);
-      if (rc != PCV_OK) return rc;
-    }
-    return PCV_OK;
+  if (p.tail.enabled) {
+    int dev = 0, sms = 0;
+    PCV_CHECK_CUDA(cudaGetDevice(&dev));
+    PCV_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    if (bf)
+      peer_tail_kernel<true><<<sms, kTailThreads, 0, stream>>>(p);
+    else
+      peer_tail_kernel<false><<<sms, kTailThreads, 0, stream>>>(p);
+    PCV_CHECK_CUDA(cudaGetLastError());
+    count_launch();
   }
-  if (mode.pair) {
-    if (DQK == 128)
-      return bf ? launch_pair<128, true>(a, *pl, tq, tk, tv, p, stream) : launch_pair<128, false>(a, *pl, tq, tk, tv, p, stream);
-    return bf ? launch_pair<64, true>(a, *pl, tq, tk, tv, p, stream) : launch_pair<64, false>(a, *pl, tq, tk, tv, p, stream);
-  }
-#define PCV_TC_CASE(DQ, DVV)                                                                          \
-  if (DQK == DQ && DV == DVV)                                                                         \
-    return bf ? launch_cfg<DQ, DVV, true>(a, *pl, tq, tk, tv, p, stream)                              \
-              : launch_cfg<DQ, DVV, false>(a, *pl, tq, tk, tv, p, stream);
-  PCV_TC_CASE(128, 128)
-  PCV_TC_CASE(64, 64)
-  PCV_TC_CASE(64, 128)
-  PCV_TC_CASE(128, 64)
-  PCV_TC_CASE(64, 192)
-  PCV_TC_CASE(64, 256)
-  PCV_TC_CASE(128, 192)
-  PCV_TC_CASE(128, 256)
-#undef PCV_TC_CASE
-  set_error("tcgen05 attention: no instantiation for padded head dims (%d, %d)", DQK, DV);
-  return PCV_ERR_UNSUPPORTED;
+  return PCV_OK;
 }
 
 }  // namespace pcv

@@ -1,4 +1,4 @@
-// pcv_aux.cu — the small HBM-bound kernels around the attention core (sm_100a):
+// pcv_aux.cu — the small HBM-bound kernels around the attention core (sm_90a):
 //   combine   : exact merge of partial softmax states (split-M inside a GPU, M-shards across GPUs)
 //   rotary    : RotaryPositionEmbedding.rotate           (reference position.py:30-50)
 //   kv_append : KV-cache concat                          (reference modules.py:117-121)
@@ -343,7 +343,7 @@ int launch_rotary(const pcv_rotary_params& p, cudaStream_t stream) {
   if (p.n == 0) return PCV_OK;
   const int64_t total = (int64_t)p.B * p.n * p.H * ((p.d + 1) / 2);
   int64_t blocks = (total + 255) / 256;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   if (p.dtype == PCV_BF16)
     rotary_kernel<__nv_bfloat16><<<(unsigned)blocks, 256, 0, stream>>>(p);
   else
@@ -383,7 +383,7 @@ int launch_kv_append(const pcv_kv_append_params& p, cudaStream_t stream) {
   }
   if (maxwork == 0) maxwork = 1;
   int64_t blocks = (maxwork + 255) / 256;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > 132 * 8) blocks = 132 * 8;
   dim3 grid((unsigned)blocks, 4, 1);
   kv_append_kernel<<<grid, 256, 0, stream>>>(a);
   PCV_CHECK_CUDA(cudaGetLastError());

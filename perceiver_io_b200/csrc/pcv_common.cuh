@@ -1,4 +1,4 @@
-// pcv_common.cuh — shared host/device helpers for libpcv_attn.so (sm_100a only).
+// pcv_common.cuh — shared host/device helpers for libpcv_attn.so (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>

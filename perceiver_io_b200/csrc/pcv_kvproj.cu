@@ -1,29 +1,24 @@
 // pcv_kvproj.cu — fused K/V producer of the cross-attention module (SURVEY.md §8(f)1): LayerNorm of the
-// (rows, C) input and BOTH projections in one pass over the input, on the 5th-generation tensor cores.
+// (rows, C) input and BOTH projections in one pass over the input, on the Hopper tensor cores (wgmma).
 //
 // Reference (perceiver/model/core/modules.py): kv_norm(x_kv) :226, then k_proj / v_proj :114-115, i.e.
 //     K = LN(x) Wk^T + bk,   V = LN(x) Wv^T + bv,   LN(x) = (x - mu) / sigma * gamma + beta.
 // LayerNorm is folded around the GEMM instead of being materialised:
 //     LN(x) W^T + b = rstd * ( x (gamma.W)^T  -  mu * s )  +  t,      s_n = sum_c gamma_c W_nc,
 //                                                                     t_n = sum_c beta_c  W_nc + b_n
-// so the kernel multiplies the RAW input tile (TMA -> shared memory -> tcgen05.mma, fp32 accumulators in
-// TMEM) with the pre-scaled weights W' = [gamma.Wk ; gamma.Wv] and applies the per-row (mu, rstd) and
-// per-column (s, t) terms in the epilogue, which writes K and V as bf16/fp16 rows with TMA stores.  s is
-// computed from the ROUNDED W' (host side), so the mu*s cancellation is exact with respect to the operands the
-// tensor core actually sees.  Row statistics come from ln_stats_kernel (one HBM pass over x, 8 bytes out per
-// row).  x is read from HBM once by the GEMM (the 8 column tiles of a row block run concurrently and meet in
-// L2), K and V are written once; nothing else touches HBM.
+// so the kernel multiplies the RAW input tile (TMA -> shared memory -> wgmma, fp32 accumulators in registers)
+// with the pre-scaled weights W' = [gamma.Wk ; gamma.Wv] and applies the per-row (mu, rstd) and per-column (s, t)
+// terms in the epilogue.  s is computed from the ROUNDED W' (host side), so the mu*s cancellation is exact with
+// respect to the operands the tensor core actually sees.  Row statistics come from ln_stats_kernel (one HBM pass
+// over x, 8 bytes out per row) or, with FUSE, from the staged input tiles inside the GEMM.
 //
-// Kernel shape (persistent, warp specialised; the canonical sm_100 GEMM):
-//   warp 0   TMA producer   A tile 128 x 64 and B tile (256/CG) x 64 per stage, SWIZZLE_128B, mbarrier ring
-//   warp 1   MMA issuer     one elected lane; tcgen05.mma M = 128*CG, N = 256, K = 16; accumulator double
-//                           buffered in TMEM (2 x 256 columns) so the epilogue of tile i overlaps tile i+1
-//   warps 2-5 epilogue      thread = accumulator row: tcgen05.ld -> fma with (rstd, -rstd*mu) and (s, t) ->
-//                           bf16 -> swizzled staging buffer -> TMA store (64-column boxes)
-// CG = 2 runs the tile on a CTA pair (cta_group::2, 256 x 256 per pair): each CTA stages its 128 rows of A and
-// half of B, which takes the operand reads off the shared-memory ceiling (DESIGN.md §3.4).
+// Kernel shape: CTA = 128 rows x 128 output columns, 384 threads: warpgroup 0 is the TMA producer (one lane;
+// A box 128 x 64 and B box 128 x 64 per stage, SWIZZLE_128B, mbarrier ring), warpgroups 1-2 each own 64 rows.
+// The column tile is the fastest grid index, so the column tiles of a row block run together and meet in L2.
+// CG = 2 (cta_group = 2) runs two adjacent row blocks of the same column tile as a 2-CTA cluster: each CTA loads one
+// 64-row half of every weight box and multicasts it to both, which halves the weight traffic into shared memory.
 #include "pcv_common.cuh"
-#include "pcv_sm100.cuh"
+#include "pcv_sm90.cuh"
 
 #include <cuda.h>
 #include <cudaTypedefs.h>
@@ -35,379 +30,180 @@
 namespace pcv {
 namespace {
 
-using namespace sm100;
+using namespace sm90;
 
-constexpr int kBM = 128;   // accumulator rows per CTA (TMEM lanes)
-constexpr int kBN = 256;   // output columns per tile (UMMA N)
+constexpr int kBM = 128;   // rows per CTA
+constexpr int kBN = 128;   // output columns per CTA
 constexpr int kBK = 64;    // channels per pipeline stage (one 128-byte swizzle atom of 16-bit elements)
-constexpr int kGemmThreads = 192;        // TMA warp, MMA warp, 4 epilogue warps
-constexpr int kGemmThreadsFused = 320;   // + 4 statistics warps (LayerNorm row statistics computed from the staged A tiles)
-constexpr int kEpiWarp0 = 2;
-constexpr int kEpiThreads = 128;
-constexpr int kStatWarp0 = 6;
-constexpr int kStoreBoxCols = 64;
-constexpr int kStoreBoxBytes = kBM * kStoreBoxCols * 2;  // 16 KB
-
-template <int CG>
-struct GemmCfg {
-  static constexpr int kABytes = kBM * kBK * 2;
-  static constexpr int kBRows = kBN / CG;  // rows of W' each CTA stages
-  static constexpr int kBBytes = kBRows * kBK * 2;
-  static constexpr int kStageBytes = kABytes + kBBytes;
-  static constexpr int kStages = CG == 1 ? 4 : 6;
-  static constexpr int kRingBytes = kStages * kStageBytes;
-  static constexpr int kTailBytes = 2048;  // barriers (512 B) + row statistics of the current row block (128 x float2)
-  static constexpr int kSmemBytes = kRingBytes + 2 * kStoreBoxBytes + kTailBytes + 1024 /*alignment slack*/;
-  static_assert(kSmemBytes <= 232448, "shared memory budget");
-};
-
-struct GemmBarriers {
-  uint64_t full[8], empty[8];
-  uint64_t tmem_full[2], tmem_empty[2];
-  uint64_t stats_full, stats_empty;
-  uint64_t landed[8];  // pair mode: "stage s holds valid data" for the statistics warps of BOTH CTAs (see the MMA issuer)
-  uint32_t tmem_base;
-};
+constexpr int kGemmThreads = 384;
+constexpr int kStages = 6;
+constexpr int kBoxBytes = 128 * 128;
+constexpr int kStageBytes = 2 * kBoxBytes;
+constexpr int kSmemBytes = kStages * kStageBytes + 2048 + 1024;  // ring + barriers / row statistics + alignment slack
 
 struct GemmParams {
-  const float2* stats;   // per row (mean, rstd); nullptr = no LayerNorm (plain x W^T + t)
+  const float2* stats;   // per row (mean, rstd); nullptr = no LayerNorm or statistics computed in the kernel
   const float2* col_st;  // per output column (s, t)
+  void* k_out;
+  void* v_out;
+  const void* x;         // raw input (first element of each row: shift of the in-kernel statistics)
+  int64_t x_stride, k_stride, v_stride;
   int64_t rows;
   int n_k, n_total;      // columns [0, n_k) go to K, [n_k, n_total) to V
   int num_kb;            // ceil(C / 64)
-  int tiles_n;           // ceil(n_total / 256)
-  int64_t num_tiles;     // row blocks (of 128*CG rows) x tiles_n
-  int64_t m_blocks;      // row blocks
+  int tiles_n;           // ceil(n_total / 128)
   int C;                 // input channels
   float eps;             // LayerNorm epsilon of the in-kernel statistics
 };
 
-// Tile order.  Separate statistics pass (FUSE = false): column tile fastest over the whole grid, so the 8 column
-// tiles of a row block run concurrently on 8 workers and meet in L2.  In-kernel statistics (FUSE = true): a worker
-// takes whole row blocks and walks their column tiles itself — the statistics are computed once, during the first
-// column tile, from the A tiles that are staged in shared memory anyway, and reused for the other tiles; the worker
-// re-reads its own A tile from L2 (148 x 256 KB live in L2), x still crosses HBM once and NOT a second time for a
-// statistics kernel.
-template <bool FUSE>
-__device__ __forceinline__ bool tile_of(const GemmParams& p, int64_t worker, int64_t workers, int64_t i, int64_t* m_blk,
-                                        int* n_blk) {
-  if (FUSE) {
-    *m_blk = worker + (i / p.tiles_n) * workers;
-    *n_blk = (int)(i % p.tiles_n);
-    return *m_blk < p.m_blocks;
-  }
-  const int64_t t = worker + i * workers;
-  *m_blk = t / p.tiles_n;
-  *n_blk = (int)(t % p.tiles_n);
-  return t < p.num_tiles;
-}
+struct GemmSmem {
+  uint64_t full[kStages], empty[kStages];
+  float2 row_st[kBM];
+};
 
-__device__ __forceinline__ uint32_t pack_pair(float lo, float hi, bool bf16) {
-  uint32_t r;
-  if (bf16)
-    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
-  else
-    asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
-  return r;
-}
-
-template <bool BF16, int CG, bool FUSE>
-__global__ void __launch_bounds__(FUSE ? kGemmThreadsFused : kGemmThreads, 1)
-kvproj_kernel(const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
-              const __grid_constant__ CUtensorMap tmap_k, const __grid_constant__ CUtensorMap tmap_v,
-              const GemmParams p) {
-  using C = GemmCfg<CG>;
-  extern __shared__ uint8_t smem_raw[];
+template <bool BF16, bool FUSE, int CG>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+kvproj_kernel(const __grid_constant__ CUtensorMap tx, const __grid_constant__ CUtensorMap tw, const GemmParams p) {
+  using T = typename std::conditional<BF16, __nv_bfloat16, __half>::type;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* ring = smem;
-  uint8_t* staging = smem + C::kRingBytes;
-  GemmBarriers& bar = *reinterpret_cast<GemmBarriers*>(smem + C::kRingBytes + 2 * kStoreBoxBytes);
-  float2* row_stats = reinterpret_cast<float2*>(smem + C::kRingBytes + 2 * kStoreBoxBytes + 512);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  GemmSmem& sh = *reinterpret_cast<GemmSmem*>(smem + kStages * kStageBytes);
+  const int wg = threadIdx.x / 128;
   const uint32_t rank = CG == 2 ? cluster_ctarank() : 0u;
-  const int64_t workers = gridDim.x / CG;
-  const int64_t worker = blockIdx.x / CG;
+  const int64_t cid = blockIdx.x / CG;
+  const int n_blk = (int)(cid % p.tiles_n);
+  const int64_t m_blk = (cid / p.tiles_n) * CG + rank;
+  const int64_t row0 = m_blk * kBM;
+  const int col0 = n_blk * kBN;
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < C::kStages; ++i) {
-      // ONE arrival: the (leader) producer's arrive.expect_tx, which announces the bytes of BOTH CTAs of a pair.  The
-      // peer never arrives: its loads only complete_tx on the leader's barrier (a transaction count may run negative
-      // until the matching expect_tx lands, and a phase cannot complete before the leader's arrival).  A remote
-      // mbarrier.arrive.release.cluster per stage compiles to MEMBAR + ERRBAR, which made the peer's producer wait for
-      // its own outstanding TMA loads before issuing the next one (measured: 2.6x slower, profiles/r02_kvproj_pair_membar.md).
-      mbar_init(&bar.full[i], 1);
-      // tcgen05.commit (multicast to both CTAs of a pair) + one arrive per statistics warp of this CTA
-      mbar_init(&bar.empty[i], FUSE ? 5 : 1);
-    }
-    mbar_init(&bar.stats_full, 4);
-    mbar_init(&bar.stats_empty, 4);
-    for (int i = 0; i < C::kStages; ++i) mbar_init(&bar.landed[i], 1);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&bar.tmem_full[i], 1);
-      mbar_init(&bar.tmem_empty[i], 4 * CG);  // one arrive per epilogue warp (of both CTAs)
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(&sh.full[s], 1);
+      mbar_init(&sh.empty[s], CG == 2 ? 16 : 8);  // one arrive per consumer warp (of both CTAs of a pair)
     }
     fence_mbar_init();
   }
-  if (warp == 1) {
-    if (CG == 1) {
-      tmem_alloc(&bar.tmem_base, 512);
-      tmem_relinquish();
-    } else {
-      tmem_alloc_pair(&bar.tmem_base, 512);
-      tmem_relinquish_pair();
-    }
-  }
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_x);
-    tma_prefetch_desc(&tmap_w);
-    tma_prefetch_desc(&tmap_k);
-    tma_prefetch_desc(&tmap_v);
-  }
-  tc_fence_before_sync();
-  if (CG == 1)
-    __syncthreads();
-  else
+  if (CG == 2)
     cluster_sync_all();
-  tc_fence_after_sync();
+  else
+    __syncthreads();
 
-  if (warp == 0) {
-    // ===== TMA producer (every CTA: its 128 rows of x, its share of the W' rows) =====
-    const bool leader_lane = elect_one();
-    uint32_t it = 0;
-    int64_t m_blk;
-    int n_blk;
-    for (int64_t ti = 0; tile_of<FUSE>(p, worker, workers, ti, &m_blk, &n_blk); ++ti) {
-      const int row0 = (int)(m_blk * (kBM * CG) + rank * kBM);
-      const int wrow0 = n_blk * kBN + (int)rank * C::kBRows;
-      for (int kb = 0; kb < p.num_kb; ++kb, ++it) {
-        const uint32_t s = it % C::kStages, par = (it / C::kStages) & 1;
-        mbar_wait(&bar.empty[s], par ^ 1, 20);
-        if (leader_lane) {
-          uint8_t* a_dst = ring + s * C::kStageBytes;
-          uint8_t* b_dst = a_dst + C::kABytes;
-          if (CG == 1) {
-            mbar_arrive_expect_tx(&bar.full[s], (uint32_t)C::kStageBytes);
-            tma_load_2d(a_dst, &tmap_x, &bar.full[s], kb * kBK, row0);
-            tma_load_2d(b_dst, &tmap_w, &bar.full[s], kb * kBK, wrow0);
-          } else {
-            if (rank == 0) mbar_arrive_expect_tx(&bar.full[s], (uint32_t)(2 * C::kStageBytes));
-            tma_load_2d_pair(a_dst, &tmap_x, &bar.full[s], kb * kBK, row0);
-            tma_load_2d_pair(b_dst, &tmap_w, &bar.full[s], kb * kBK, wrow0);
-          }
-        }
-      }
-    }
-  } else if (warp == 1 && rank == 0) {
-    // ===== MMA issuer (warp-converged, one elected lane issues; leader CTA only in pair mode) =====
-    const bool leader_lane = elect_one();
-    constexpr uint32_t idesc = make_idesc(kBM * CG, kBN, BF16, false);
-    const uint32_t tmem = bar.tmem_base;
-    const uint64_t da0 = make_smem_desc(smem_u32(ring), 16, 1024);
-    const uint64_t db0 = make_smem_desc(smem_u32(ring + C::kABytes), 16, 1024);
-    uint32_t it = 0, tc = 0;
-    int64_t m_blk;
-    int n_blk;
-    for (int64_t ti = 0; tile_of<FUSE>(p, worker, workers, ti, &m_blk, &n_blk); ++ti, ++tc) {
-      const uint32_t acc = tc & 1;
-      mbar_wait(&bar.tmem_empty[acc], ((tc >> 1) & 1) ^ 1, 21);
-      tc_fence_after_sync();
-      for (int kb = 0; kb < p.num_kb; ++kb, ++it) {
-        const uint32_t s = it % C::kStages, par = (it / C::kStages) & 1;
-        mbar_wait(&bar.full[s], par, 22);
-        tc_fence_after_sync();
-        if (leader_lane) {
-          const uint64_t soff = (uint64_t)((s * C::kStageBytes) >> 4);
-#pragma unroll
-          for (int kk = 0; kk < kBK / 16; ++kk) {
-            const uint64_t off = soff + (uint64_t)((kk * 32) >> 4);
-            if (CG == 1)
-              mma_ss(tmem + acc * kBN, da0 + off, db0 + off, idesc, (kb > 0 || kk > 0) ? 1u : 0u);
-            else
-              mma_ss_pair(tmem + acc * kBN, da0 + off, db0 + off, idesc, (kb > 0 || kk > 0) ? 1u : 0u);
-          }
-          if (CG == 1) {
-            tc_commit(&bar.empty[s]);
-          } else {
-            tc_commit_pair(&bar.empty[s], 3);
-            // TMA bytes of a pair are signalled on the LEADER's full barrier only, so the peer's statistics warps cannot
-            // wait for it; a second multicast commit tells both CTAs "the MMAs of stage s are done" — which implies
-            // that its data had landed — while the stage cannot be recycled before the statistics warps have arrived
-            // on their CTA's empty barrier
-            if (FUSE) tc_commit_pair(&bar.landed[s], 3);
-          }
-        }
-      }
-      if (leader_lane) {
-        if (CG == 1)
-          tc_commit(&bar.tmem_full[acc]);
+  if (wg == 0) {
+    reg_dealloc<40>();
+    if (threadIdx.x == 0) {
+      for (int kb = 0; kb < p.num_kb; ++kb) {
+        const int s = kb % kStages;
+        mbar_wait(&sh.empty[s], ((kb / kStages) & 1) ^ 1, 11);
+        mbar_arrive_expect_tx(&sh.full[s], kStageBytes);
+        tma_load_2d(smem + s * kStageBytes, &tx, &sh.full[s], kb * kBK, (int)row0);
+        if (CG == 2)
+          tma_load_2d_mc(smem + s * kStageBytes + kBoxBytes + rank * (kBoxBytes / 2), &tw, &sh.full[s], kb * kBK,
+                         col0 + 64 * (int)rank, 0x3);
         else
-          tc_commit_pair(&bar.tmem_full[acc], 3);
+          tma_load_2d(smem + s * kStageBytes + kBoxBytes, &tw, &sh.full[s], kb * kBK, col0);
       }
     }
-  } else if (warp >= kEpiWarp0 && warp < kEpiWarp0 + 4) {
-    // ===== epilogue: thread = accumulator row (TMEM lane 32*(warp%4) + lane) =====
-    const int quarter = warp & 3;
-    const int r_in_tile = quarter * 32 + lane;
-    const uint32_t lane_field = (uint32_t)(quarter * 32) << 16;
-    const uint32_t tmem = bar.tmem_base;
-    const bool store_thread = (threadIdx.x == kEpiWarp0 * 32);
-    const uint32_t tmem_empty_addr =
-        CG == 2 ? mapa_cluster(smem_u32(&bar.tmem_empty[0]), 0) : smem_u32(&bar.tmem_empty[0]);
-    uint32_t tc = 0, g = 0, mb = 0;  // tiles / store boxes / row blocks processed by this CTA
-    int64_t m_blk;
-    int n_blk;
-    float a = 1.f, bb = 0.f;
-    for (int64_t ti = 0; tile_of<FUSE>(p, worker, workers, ti, &m_blk, &n_blk); ++ti, ++tc) {
-      const int64_t row0 = m_blk * (kBM * CG) + rank * kBM;
-      const int64_t row = row0 + r_in_tile;
-      if (FUSE) {
-        if (n_blk == 0) {
-          // the statistics warps publish (mean, rstd) of this row block once its first column tile has been staged
-          mbar_wait(&bar.stats_full, mb & 1, 24);
-          ++mb;
-          const float2 ms = row_stats[r_in_tile];
-          a = ms.y;
-          bb = -ms.y * ms.x;
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&bar.stats_empty);
-        }
-      } else if (p.stats != nullptr) {
-        float2 ms = make_float2(0.f, 0.f);
-        if (row < p.rows) ms = __ldg(p.stats + row);
-        a = ms.y;
-        bb = -ms.y * ms.x;
-      }
-      const uint32_t acc = tc & 1;
-      mbar_wait(&bar.tmem_full[acc], (tc >> 1) & 1, 23);
-      tc_fence_after_sync();
-      const int nboxes = min(kBN / kStoreBoxCols, (p.n_total - n_blk * kBN + kStoreBoxCols - 1) / kStoreBoxCols);
-      for (int box = 0; box < nboxes; ++box, ++g) {
-        const int col0 = n_blk * kBN + box * kStoreBoxCols;
-        uint32_t v0[32], v1[32];
-        tmem_ld32(tmem + lane_field + acc * kBN + box * kStoreBoxCols, v0);
-        tmem_ld32(tmem + lane_field + acc * kBN + box * kStoreBoxCols + 32, v1);
-        tmem_wait_ld();
-        if (box == nboxes - 1) {
-          // the accumulator is in registers: hand the TMEM buffer back to the MMA issuer
-          tc_fence_before_sync();
-          __syncwarp();
-          if (lane == 0) {
-            if (CG == 1)
-              mbar_arrive(&bar.tmem_empty[acc]);
-            else
-              mbar_arrive_cluster(tmem_empty_addr + acc * 8);
-          }
-        }
-        uint8_t* buf = staging + (g & 1) * kStoreBoxBytes + r_in_tile * 128;
-        const float2* st = p.col_st + col0;
-#pragma unroll
-        for (int c8 = 0; c8 < 8; ++c8) {
-          uint32_t w[4];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const int i = c8 * 8 + j * 2;  // column within the box
-            const float x0 = __uint_as_float(i < 32 ? v0[i] : v1[i - 32]);
-            const float x1 = __uint_as_float(i < 32 ? v0[i + 1] : v1[i - 31]);
-            const float2 st0 = __ldg(st + i), st1 = __ldg(st + i + 1);
-            const float y0 = fmaf(x0, a, fmaf(st0.x, bb, st0.y));
-            const float y1 = fmaf(x1, a, fmaf(st1.x, bb, st1.y));
-            w[j] = pack_pair(y0, y1, BF16);
-          }
-          // SWIZZLE_128B staging (what the TMA store expects): 16-byte chunk c8 of row r lives at chunk c8 ^ (r & 7)
-          *reinterpret_cast<uint4*>(buf + ((c8 ^ (r_in_tile & 7)) << 4)) = make_uint4(w[0], w[1], w[2], w[3]);
-        }
-        fence_proxy_async_smem();
-        // every earlier store has finished reading its staging buffer before anybody passes the barrier, so the
-        // buffer written for box g+1 (the one store g-1 used) is free
-        if (store_thread) bulk_wait_group_read<0>();
-        named_bar_sync(1, kEpiThreads);
-        if (store_thread) {
-          if (col0 < p.n_k)
-            tma_store_2d(&tmap_k, staging + (g & 1) * kStoreBoxBytes, col0, (int)row0);
-          else
-            tma_store_2d(&tmap_v, staging + (g & 1) * kStoreBoxBytes, col0 - p.n_k, (int)row0);
-          bulk_commit_group();
-        }
-      }
+    if (CG == 2) {
+      __syncwarp();
+      cluster_sync_all();  // the peer may still multicast into / arrive on this CTA's shared memory until here
     }
-    if (store_thread) bulk_wait_group<0>();
-  } else if (FUSE && warp >= kStatWarp0) {
-    // ===== LayerNorm row statistics from the staged A tiles (thread = row of this CTA's 128-row tile) =====
-    // One pass, shifted by the row's first element (pivot): mean = p + S1/C, var = S2/C - (S1/C)^2 with S1 = sum(x-p),
-    // S2 = sum((x-p)^2) — |mean - p| is of the order of sigma, so the subtraction does not cancel however large
-    // |mean| / sigma is.  A row's 128 bytes of a stage are read as 8 x 16 bytes in swizzled order (chunk j of row r
-    // lives at chunk j ^ (r & 7)): conflict-free, and a sum does not care about the order.
-    const int r = (warp - kStatWarp0) * 32 + lane;
-    uint32_t it = 0, mb = 0;
-    int64_t m_blk;
-    int n_blk;
-    for (int64_t ti = 0; tile_of<FUSE>(p, worker, workers, ti, &m_blk, &n_blk); ++ti) {
-      float pivot = 0.f, s1 = 0.f, s2 = 0.f;
-      for (int kb = 0; kb < p.num_kb; ++kb, ++it) {
-        const uint32_t s = it % C::kStages, par = (it / C::kStages) & 1;
-        if (CG == 1)
-          mbar_wait(&bar.full[s], par, 25);
-        else
-          mbar_wait(&bar.landed[s], par, 25);
-        if (n_blk == 0) {
-          const uint8_t* rowp = ring + s * C::kStageBytes + r * 128;
-          const int chunks = min(8, (p.C - kb * kBK) / 8);  // ragged last stage: TMA zero fill is not data
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            if (j < chunks) {
-              const uint4 u = *reinterpret_cast<const uint4*>(rowp + ((j ^ (r & 7)) << 4));
-              const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-              for (int q = 0; q < 4; ++q) {
-                float lo, hi;
-                if (BF16) {
-                  lo = __uint_as_float(w[q] << 16);
-                  hi = __uint_as_float(w[q] & 0xffff0000u);
-                } else {
-                  const __half2 h2 = *reinterpret_cast<const __half2*>(&w[q]);
-                  lo = __low2float(h2);
-                  hi = __high2float(h2);
-                }
-                if (kb == 0 && j == 0 && q == 0) pivot = lo;
-                const float d0 = lo - pivot, d1 = hi - pivot;
-                s1 += d0 + d1;
-                s2 = fmaf(d0, d0, s2);
-                s2 = fmaf(d1, d1, s2);
-              }
-            }
-          }
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bar.empty[s]);  // release: the shared-memory reads above are done
-      }
-      if (n_blk == 0) {
-        mbar_wait(&bar.stats_empty, (mb & 1) ^ 1, 26);  // the epilogue has taken the previous row block's statistics
-        ++mb;
-        const float inv_c = 1.f / (float)p.C;
-        const float d = s1 * inv_c;
-        const float var = fmaxf(fmaf(-d, d, s2 * inv_c), 0.f);
-        row_stats[r] = make_float2(pivot + d, 1.f / sqrtf(var + p.eps));
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bar.stats_full);
-      }
-    }
+    return;
   }
 
-  tc_fence_before_sync();
-  if (CG == 1)
-    __syncthreads();
-  else
-    cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    if (CG == 1)
-      tmem_dealloc(bar.tmem_base, 512);
-    else
-      tmem_dealloc_pair(bar.tmem_base, 512);
+  reg_alloc<232>();
+  const int cw = wg - 1;
+  const int tid = threadIdx.x - 128 * wg;
+  const int warp = tid >> 5, lane = tid & 31;
+  const int rloc = 64 * cw + 16 * warp + (lane >> 2);
+  const int cq = 2 * (lane & 3);
+  const uint32_t base = smem_u32(smem);
+  // in-kernel statistics: two threads per row, each reads half of the row's 128-byte line of every A box;
+  // shifted sums (by the row's first element) keep the one-pass variance free of cancellation
+  const int srow = 64 * cw + (tid >> 1), shalf = tid & 1;
+  float x0 = 0.f, s1 = 0.f, s2 = 0.f;
+  if (FUSE && row0 + srow < p.rows)
+    x0 = Elem<T>::to_f(*(reinterpret_cast<const T*>(p.x) + (row0 + srow) * p.x_stride));
+
+  float acc[64];
+  for (int kb = 0; kb < p.num_kb; ++kb) {
+    const int s = kb % kStages;
+    mbar_wait(&sh.full[s], (kb / kStages) & 1, 12);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)
+      wgmma_ss<128, BF16>(acc, make_desc(base + s * kStageBytes + cw * 64 * 128 + kk * 32),
+                          make_desc(base + s * kStageBytes + kBoxBytes + kk * 32), (kb | kk) != 0);
+    wgmma_commit();
+    if (FUSE) {
+      const uint8_t* line = smem + s * kStageBytes + srow * 128;
+#pragma unroll
+      for (int ch = 0; ch < 4; ++ch) {
+        const int lc = shalf * 4 + ch;  // logical 16-byte chunk of the row
+        const uint4 u = *reinterpret_cast<const uint4*>(line + ((lc ^ (srow & 7)) * 16));
+        const typename Elem<T>::T2* h2 = reinterpret_cast<const typename Elem<T>::T2*>(&u);
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int c = kb * kBK + lc * 8 + 2 * e;
+          const float2 f = Elem<T>::to_f2(h2[e]);
+          if (c < p.C) {
+            const float d = f.x - x0;
+            s1 += d;
+            s2 = fmaf(d, d, s2);
+          }
+          if (c + 1 < p.C) {
+            const float d = f.y - x0;
+            s1 += d;
+            s2 = fmaf(d, d, s2);
+          }
+        }
+      }
+    }
+    wgmma_wait<0>();
+    fence_regs(acc);
+    if (CG == 2) warp_arrive_pair(&sh.empty[s]);
+    else warp_arrive(&sh.empty[s]);
   }
+
+  if (FUSE) {
+    s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
+    s2 += __shfl_xor_sync(0xffffffffu, s2, 1);
+    if (shalf == 0) {
+      const float inv_c = 1.f / (float)p.C;
+      const float dm = s1 * inv_c;
+      const float var = fmaxf(s2 * inv_c - dm * dm, 0.f);
+      sh.row_st[srow] = make_float2(x0 + dm, rsqrtf(var + p.eps));
+    }
+    asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
+  }
+
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int64_t row = row0 + rloc + 8 * r;
+    if (row >= p.rows) continue;
+    float2 st = make_float2(0.f, 1.f);
+    const bool ln = FUSE || p.stats != nullptr;
+    if (FUSE) st = sh.row_st[rloc + 8 * r];
+    else if (p.stats != nullptr) st = p.stats[row];
+#pragma unroll
+    for (int g = 0; g < 16; ++g) {
+      const int n = col0 + 8 * g + cq;
+      if (n >= p.n_total) continue;
+      const float2 c0 = p.col_st[n], c1 = p.col_st[n + 1];
+      float a0 = acc[4 * g + 2 * r], a1 = acc[4 * g + 2 * r + 1];
+      if (ln) {
+        a0 = st.y * (a0 - st.x * c0.x);
+        a1 = st.y * (a1 - st.x * c1.x);
+      }
+      const uint32_t w = pack2(a0 + c0.y, a1 + c1.y, BF16);
+      if (n < p.n_k)
+        *reinterpret_cast<uint32_t*>(reinterpret_cast<T*>(p.k_out) + row * p.k_stride + n) = w;
+      else
+        *reinterpret_cast<uint32_t*>(reinterpret_cast<T*>(p.v_out) + row * p.v_stride + (n - p.n_k)) = w;
+    }
+  }
+  if (CG == 2) cluster_sync_all();
 }
+
 
 // --------------------------------------------------------------------------------------------------
 // LayerNorm row statistics: one warp per row, (mean, 1/sqrt(var + eps)) with the biased variance of
@@ -517,7 +313,7 @@ int launch_ln_stats_t(const pcv_ln_stats_params& p, cudaStream_t stream) {
   const bool reg_ok = (p.C % 256 == 0) && p.C <= 2048 && (p.x_stride_row % 8 == 0) &&
                       ((reinterpret_cast<uintptr_t>(p.x) & 15) == 0);
   if (reg_ok) {
-    const int blocks = (int)std::min<int64_t>((p.rows + 15) / 16, 148 * 8);
+    const int blocks = (int)std::min<int64_t>((p.rows + 15) / 16, 132 * 8);
 #define PCV_LN_CASE(N)                                                                               \
   case N:                                                                                            \
     ln_stats_reg_kernel<T, N><<<blocks, 256, 0, stream>>>(x, p.x_stride_row, p.rows, p.eps, st);     \
@@ -528,7 +324,7 @@ int launch_ln_stats_t(const pcv_ln_stats_params& p, cudaStream_t stream) {
     }
 #undef PCV_LN_CASE
   } else {
-    const int blocks = (int)std::min<int64_t>((p.rows + 7) / 8, 148 * 8);
+    const int blocks = (int)std::min<int64_t>((p.rows + 7) / 8, 132 * 8);
     ln_stats_kernel<T><<<blocks, 256, 0, stream>>>(x, p.x_stride_row, p.rows, p.C, p.eps, st);
   }
   PCV_CHECK_CUDA(cudaGetLastError());
@@ -565,11 +361,9 @@ int make_tmap_2d(CUtensorMap* tm, const void* base, int dtype, int64_t inner, in
   return PCV_OK;
 }
 
-template <bool BF16, int CG, bool FUSE>
-int launch_gemm(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap& tk, const CUtensorMap& tv,
-                const GemmParams& gp, int sms, cudaStream_t stream) {
-  using C = GemmCfg<CG>;
-  auto kern = kvproj_kernel<BF16, CG, FUSE>;
+template <bool BF16, bool FUSE, int CG>
+int launch_gemm(const CUtensorMap& tx, const CUtensorMap& tw, const GemmParams& gp, cudaStream_t stream) {
+  auto kern = kvproj_kernel<BF16, FUSE, CG>;
   static std::mutex mu;
   static bool attr_set[64] = {};
   int dev = 0;
@@ -577,13 +371,17 @@ int launch_gemm(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap&
   {
     std::lock_guard<std::mutex> lk(mu);
     if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-      PCV_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes));
+      PCV_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
       if (dev >= 0 && dev < 64) attr_set[dev] = true;
     }
   }
+  const int64_t m_blocks = (gp.rows + kBM * CG - 1) / (kBM * CG) * CG;  // whole pairs; a pair's spare block is all padding
+  const int64_t tiles = m_blocks * gp.tiles_n;
+  PCV_REQUIRE(tiles <= 0x7fffffff, PCV_ERR_UNSUPPORTED, "kv_project: %lld tiles exceed the grid limit", (long long)tiles);
   cudaLaunchConfig_t cfg{};
-  cfg.blockDim = dim3(FUSE ? kGemmThreadsFused : kGemmThreads);
-  cfg.dynamicSmemBytes = C::kSmemBytes;
+  cfg.gridDim = dim3((unsigned)tiles);
+  cfg.blockDim = dim3(kGemmThreads);
+  cfg.dynamicSmemBytes = kSmemBytes;
   cfg.stream = stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -592,28 +390,10 @@ int launch_gemm(const CUtensorMap& tx, const CUtensorMap& tw, const CUtensorMap&
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  int64_t max_workers = sms;
-  if (CG == 2) {
-    // A persistent kernel must not launch more CTA pairs than can be co-resident (a pair needs both SMs of one TPC
-    // free; the second wave would double the run time): ask the occupancy calculator.
-    static int max_pairs[64] = {};
-    if (dev < 0 || dev >= 64 || max_pairs[dev] == 0) {
-      cfg.gridDim = dim3((unsigned)(sms / 2 * 2));
-      int n = 0;
-      PCV_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&n, kern, &cfg));
-      if (n < 1) n = 1;
-      if (dev >= 0 && dev < 64) max_pairs[dev] = n;
-      max_workers = n;
-    } else {
-      max_workers = max_pairs[dev];
-    }
-    if (getenv("PCV_KVPROJ_VERBOSE")) fprintf(stderr, "[pcv] kvproj: %lld co-resident CTA pairs on %d SMs\n", (long long)max_workers, sms);
-  }
-  const int workers = (int)std::min<int64_t>(max_workers, FUSE ? gp.m_blocks : gp.num_tiles);
-  cfg.gridDim = dim3((unsigned)(workers * CG));
   prof_mark_begin(stream);
-  PCV_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, tx, tw, tk, tv, gp));
+  PCV_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, tx, tw, gp));
   prof_mark_end(stream);
+  PCV_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PCV_OK;
 }
@@ -637,16 +417,17 @@ bool kv_project_supported(const pcv_kvproj_params& p, const char** why) {
   if (p.dtype != PCV_BF16 && p.dtype != PCV_F16) return fail("dtype must be bf16 or fp16");
   if (p.C < 8 || (p.C % 8)) return fail("input channels must be a multiple of 8 (16-byte TMA strides)");
   if (p.n_k < 0 || p.n_v < 0 || p.n_k + p.n_v < 1) return fail("no output columns");
-  if ((p.n_k % 64) != 0) return fail("K width must be a multiple of 64 (a 64-column store box must not straddle K | V)");
+  if ((p.n_k % 64) != 0) return fail("K width must be a multiple of 64");
   if ((p.n_v % 8) != 0) return fail("V width must be a multiple of 8");
   if (!al16(p.x) || !al16(p.w) || (p.n_k && !al16(p.k_out)) || (p.n_v && !al16(p.v_out)))
     return fail("x / w / k_out / v_out must be 16-byte aligned");
   if ((p.x_stride_row % 8) || (p.k_stride_row % 8) || (p.v_stride_row % 8)) return fail("row strides must be multiples of 8 elements");
   if (p.rows < 1 || p.rows > (int64_t)0x7fffff00) return fail("row count out of range");
+  if (p.cta_group < 0 || p.cta_group > 2) return fail("cta_group must be 0, 1 or 2");
   int dev = 0, major = 0;
   if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess)
     return fail("no CUDA device");
-  if (major != 10) return fail("device is not sm_100");
+  if (major != 9) return fail("device is not sm_90");
   return true;
 }
 
@@ -654,59 +435,40 @@ int launch_kv_project(const pcv_kvproj_params& p, cudaStream_t stream) {
   const char* why = "";
   PCV_REQUIRE(p.x && p.w && p.col_st, PCV_ERR_INVALID, "kv_project: NULL pointer");
   PCV_REQUIRE(kv_project_supported(p, &why), PCV_ERR_UNSUPPORTED, "kv_project: %s", why);
-  int dev = 0, sms = 0;
-  PCV_CHECK_CUDA(cudaGetDevice(&dev));
-  PCV_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  // CTA pairs (cta_group::2) by default; PCV_KVPROJ_CG=1 selects the single-CTA variant (A/B measurements)
-  static const int cg_env = [] { const char* e = getenv("PCV_KVPROJ_CG"); return e ? atoi(e) : 0; }();
-  int cg = p.cta_group == 1 || p.cta_group == 2 ? p.cta_group : (cg_env == 1 || cg_env == 2 ? cg_env : 2);
-  if (sms < 2) cg = 1;
-
   const int n_total = p.n_k + p.n_v;
   GemmParams gp{};
   gp.stats = reinterpret_cast<const float2*>(p.row_stats);
   gp.col_st = reinterpret_cast<const float2*>(p.col_st);
+  gp.k_out = p.k_out;
+  gp.v_out = p.v_out;
+  gp.x = p.x;
+  gp.x_stride = p.x_stride_row;
+  gp.k_stride = p.k_stride_row;
+  gp.v_stride = p.v_stride_row;
   gp.rows = p.rows;
   gp.n_k = p.n_k;
   gp.n_total = n_total;
   gp.num_kb = (p.C + kBK - 1) / kBK;
   gp.tiles_n = (n_total + kBN - 1) / kBN;
-  const int64_t rows_per_tile = (int64_t)kBM * cg;
-  gp.m_blocks = (p.rows + rows_per_tile - 1) / rows_per_tile;
-  gp.num_tiles = gp.m_blocks * gp.tiles_n;
   gp.C = p.C;
   gp.eps = p.ln_eps;
   const bool fuse = p.row_stats == nullptr && p.ln_eps > 0.f;
 
-  CUtensorMap tx, tw, tk, tv;
+  CUtensorMap tx, tw;
   int rc = make_tmap_2d(&tx, p.x, p.dtype, p.C, p.rows, p.x_stride_row, kBM);
   if (rc != PCV_OK) return rc;
+  // one CTA per tile by default; cta_group = 2 asks for the 2-CTA clusters (each CTA loads half of the weight box)
+  const int cg = p.cta_group == 2 ? 2 : 1;
   rc = make_tmap_2d(&tw, p.w, p.dtype, p.C, n_total, p.C, kBN / cg);
   if (rc != PCV_OK) return rc;
-  // a width of zero cannot be encoded: point the unused map at the other output (never stored through)
-  const void* kbase = p.n_k ? p.k_out : p.v_out;
-  const void* vbase = p.n_v ? p.v_out : p.k_out;
-  rc = make_tmap_2d(&tk, kbase, p.dtype, p.n_k ? p.n_k : p.n_v, p.rows, p.n_k ? p.k_stride_row : p.v_stride_row, kBM);
-  if (rc != PCV_OK) return rc;
-  rc = make_tmap_2d(&tv, vbase, p.dtype, p.n_v ? p.n_v : p.n_k, p.rows, p.n_v ? p.v_stride_row : p.k_stride_row, kBM);
-  if (rc != PCV_OK) return rc;
-
   const bool bf = p.dtype == PCV_BF16;
-#define PCV_GEMM_CASE(B, G, F) return launch_gemm<B, G, F>(tx, tw, tk, tv, gp, sms, stream)
+#define PCV_GEMM_CASE(G)                                                                                   \
+  if (fuse) return bf ? launch_gemm<true, true, G>(tx, tw, gp, stream) : launch_gemm<false, true, G>(tx, tw, gp, stream); \
+  return bf ? launch_gemm<true, false, G>(tx, tw, gp, stream) : launch_gemm<false, false, G>(tx, tw, gp, stream);
   if (cg == 2) {
-    if (fuse) {
-      if (bf) PCV_GEMM_CASE(true, 2, true);
-      PCV_GEMM_CASE(false, 2, true);
-    }
-    if (bf) PCV_GEMM_CASE(true, 2, false);
-    PCV_GEMM_CASE(false, 2, false);
+    PCV_GEMM_CASE(2)
   }
-  if (fuse) {
-    if (bf) PCV_GEMM_CASE(true, 1, true);
-    PCV_GEMM_CASE(false, 1, true);
-  }
-  if (bf) PCV_GEMM_CASE(true, 1, false);
-  PCV_GEMM_CASE(false, 1, false);
+  PCV_GEMM_CASE(1)
 #undef PCV_GEMM_CASE
 }
 

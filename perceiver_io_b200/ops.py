@@ -35,7 +35,7 @@ def _require_cuda(*tensors: torch.Tensor) -> None:
     for t in tensors:
         if t is not None and not t.is_cuda:
             raise RuntimeError(
-                "perceiver_io_b200 ops run on CUDA (sm_100a) tensors only; got a tensor on "
+                "perceiver_io_b200 ops run on CUDA (sm_90a) tensors only; got a tensor on "
                 f"{t.device}. There is no CPU fallback for the attention path."
             )
 
@@ -284,7 +284,7 @@ def dropout_keep_mask(B: int, H: int, N: int, M: int, dropout_p: float, dropout_
 
 class _FusedAttention(torch.autograd.Function):
     """Forward = the fused CUDA kernel (partial-state mode, so the row max and denominator are kept).
-    Backward = the tcgen05 backward kernels (``attention_backward`` -> pcv_attn_bwd: dK/dV and dQ kernels, SURVEY.md
+    Backward = the tensor-core backward kernels (``attention_backward`` -> pcv_attn_bwd: dK/dV and dQ kernels, SURVEY.md
     §8(f) rank 2) for head dims that are multiples of 8 up to 128.  Other shapes take the labelled SHIM below: the
     flash-attention backward recurrence in plain torch ops, chunked over the key axis from the saved statistics,
     memory bounded by ``backward_config["max_score_bytes"]``; neither path ever holds the (B, H, N, M) score tensor
@@ -883,9 +883,8 @@ def kv_project_supported(x: torch.Tensor, n_k: int, n_v: int) -> bool:
 
 
 #: ``stats``: "separate" = pcv_ln_stats first (two-pass statistics; x is read twice, at the copy bandwidth), "fused" =
-#: statistics computed inside the GEMM kernel from the staged tiles (x crosses HBM once).  Measured equal in time at the
-#: north-star shape (the statistics warps delay the recycling of a ring stage by about what the extra pass costs;
-#: profiles/r02_kvproj_bench.log), so the default is the numerically more conservative two-pass variant.
+#: statistics computed inside the GEMM kernel from the staged tiles (x crosses HBM once).  The default is the numerically
+#: more conservative two-pass variant.
 kv_project_config = {"stats": "separate"}
 
 

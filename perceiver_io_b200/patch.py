@@ -31,7 +31,7 @@ def _is_reference_self_attention(module: nn.Module) -> bool:
 
 
 def patch(model: nn.Module, impl: str = "auto") -> int:
-    """Route every MultiHeadAttention under ``model`` through the sm_100a kernels.
+    """Route every MultiHeadAttention under ``model`` through the sm_90a kernels.
 
     Reference ``CrossAttention`` / ``SelfAttention`` modules (modules.py:173-278) are rebound as well so that their
     LayerNorm -> projection chains run through the LayerNorm-folded tcgen05 GEMM (``modules.project_kv`` /

@@ -1,4 +1,4 @@
-"""-m gpu: the tcgen05 backward kernels (pcv_attn_bwd) against autograd through the reference algorithm.
+"""-m gpu: the tensor-core backward kernels (pcv_attn_bwd) against autograd through the reference algorithm.
 
 Reference gradients come from torch autograd through `gpu_util.torch_core` (the reference's own op sequence,
 modules.py:123-167) in float64 on the SAME rounded operands; the gate is the derived one of the forward tests applied
