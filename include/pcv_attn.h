@@ -400,14 +400,15 @@ PCV_API int pcv_profile_begin(void);
 PCV_API int pcv_profile_end(double* main_kernel_ms_total, int32_t* main_kernel_launches);
 
 /*
- * Watchdog record of the tcgen05 kernel: every in-kernel barrier wait is bounded (4 s); a wait that
- * times out writes {1, site, blockIdx, threadIdx, parity, spins} to a pinned host buffer and traps, so a
- * pipeline bug surfaces as a CUDA error instead of a hung GPU.  Copies up to 16 words; word 0 == 0 means
- * no timeout was recorded.  Readable even after the context died.
+ * Watchdog record of the tensor-core kernels (attention forward and its cross-GPU merge, backward, dropout
+ * forward, K/V projection), one for the whole library: every in-kernel barrier wait is bounded (4 s); the first
+ * wait that times out writes {1, site, blockIdx, threadIdx, parity or expected value, spins or seen value} to a
+ * pinned host buffer and traps, so a pipeline bug surfaces as a CUDA error instead of a hung GPU.  Site numbers
+ * are unique in the library and name the kernel and the wait.  Copies up to 16 words; word 0 == 0 means no timeout
+ * was recorded.  Readable even after the context died.
  */
 PCV_API int pcv_debug_read(uint32_t* out, int32_t n);
-/* Developer aid: with PCV_TRACE=1 in the environment CTA 0 of the tcgen05 kernel stamps clock64() at fixed
- * pipeline points; copies the 3 x 48 x 8 stamps (roles: softmax0, softmax1, mma; tile; event) of the last launch. */
+/* Kept for ABI compatibility: the kernels record no clock trace, so this always returns PCV_ERR_UNSUPPORTED. */
 PCV_API int pcv_debug_trace_read(uint64_t* out, int32_t n);
 
 /*

@@ -115,14 +115,12 @@ int pcv_profile_end(double* main_kernel_ms_total, int32_t* main_kernel_launches)
 
 int pcv_debug_read(uint32_t* out, int32_t n) {
   PCV_REQUIRE(out != nullptr && n >= 0, PCV_ERR_INVALID, "debug_read: bad argument");
-  const int rc = debug_read(out, n);
-  if (rc == PCV_OK && n > 0 && out[0] == 0u) return bwd_debug_read(out, n);  // nothing from the forward kernels
-  return rc;
+  return debug_read(out, n);
 }
 
-int pcv_debug_trace_read(uint64_t* out, int32_t n) {
-  PCV_REQUIRE(out != nullptr, PCV_ERR_INVALID, "trace_read: bad argument");
-  return debug_trace_read(reinterpret_cast<unsigned long long*>(out), n);
+int pcv_debug_trace_read(uint64_t*, int32_t) {
+  set_error("debug_trace_read: the kernels record no clock trace");
+  return PCV_ERR_UNSUPPORTED;
 }
 
 int pcv_debug_plan(int32_t B, int32_t H, int32_t N, int32_t M, int32_t workers, int32_t rows_per_unit,

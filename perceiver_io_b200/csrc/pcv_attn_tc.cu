@@ -19,9 +19,6 @@
 #include "pcv_common.cuh"
 #include "pcv_sm90.cuh"
 
-#include <cuda.h>
-#include <cudaTypedefs.h>
-
 #include <cstdlib>
 #include <algorithm>
 #include <atomic>
@@ -185,7 +182,7 @@ __global__ void __launch_bounds__(kTailThreads) peer_tail_kernel(const TcParams 
     __threadfence_system();
     st_release_sys_u32(t.flags[threadIdx.x] + t.rank, t.epoch);
   }
-  if (threadIdx.x < G) tail_wait_ge(lf + threadIdx.x, t.epoch, 32);
+  if (threadIdx.x < G) tail_wait_ge(lf + threadIdx.x, t.epoch, 41);
   __syncthreads();
   PCV_TAIL_STAMP(2);
 
@@ -248,12 +245,12 @@ __global__ void __launch_bounds__(kTailThreads) peer_tail_kernel(const TcParams 
   }
 
   PCV_TAIL_STAMP(3);
-  tail_grid_arrive_wait(lf + 18, target, 33);
+  tail_grid_arrive_wait(lf + 18, target, 42);
   PCV_TAIL_STAMP(4);
   if (blockIdx.x == 0) {
     if (threadIdx.x < G) {
       st_release_sys_u32(t.flags[threadIdx.x] + G + t.rank, t.epoch);
-      tail_wait_ge(lf + G + threadIdx.x, t.epoch, 34);
+      tail_wait_ge(lf + G + threadIdx.x, t.epoch, 43);
     }
     __syncthreads();
   }
@@ -540,22 +537,6 @@ __global__ void __launch_bounds__(256) tc_combine_kernel(const UnitRec* __restri
   }
 }
 
-// pad_mask bytes (B, M) -> bit words (B, wpr), wpr = 4 * ceil(M/128); bit set = padding key
-__global__ void __launch_bounds__(256) pack_pad_kernel(const uint8_t* __restrict__ pad, int64_t stride_b, int B, int M,
-                                                       int wpr, uint32_t* __restrict__ bits) {
-  const int64_t total = (int64_t)B * wpr;
-  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
-    const int b = (int)(idx / wpr), w = (int)(idx % wpr);
-    uint32_t word = 0;
-    const int j0 = w * 32;
-    for (int i = 0; i < 32; ++i) {
-      const int j = j0 + i;
-      if (j < M && pad[(int64_t)b * stride_b + j] != 0) word |= (1u << i);
-    }
-    bits[idx] = word;
-  }
-}
-
 // --------------------------------------------------------------------------------------------------
 // host: plan (segment table), tensor maps, launch
 // --------------------------------------------------------------------------------------------------
@@ -651,26 +632,7 @@ void build_plan(Plan& pl, int B, int H, int N, int M, int num_sms, int rows_per_
   pl.num_units = (int)pl.units.size();
 }
 
-// watchdog record shared with the device (see mbar_wait in pcv_sm90.cuh)
-uint32_t* g_diag_host = nullptr;
-std::map<int, bool> g_diag_set;  // per device
-
-int ensure_diag(int dev) {
-  if (g_diag_set.count(dev)) return PCV_OK;
-  if (g_diag_host == nullptr) {
-    PCV_CHECK_CUDA(cudaHostAlloc(reinterpret_cast<void**>(&g_diag_host), 64, cudaHostAllocMapped | cudaHostAllocPortable));
-    for (int i = 0; i < 16; ++i) g_diag_host[i] = 0;
-  }
-  uint32_t* dptr = nullptr;
-  PCV_CHECK_CUDA(cudaHostGetDevicePointer(reinterpret_cast<void**>(&dptr), g_diag_host, 0));
-  PCV_CHECK_CUDA(cudaMemcpyToSymbol(sm90::g_wait_diag, &dptr, sizeof(dptr)));
-  g_diag_set[dev] = true;
-  return PCV_OK;
-}
-
-
 std::mutex g_plan_mu;
-std::mutex g_attr_mu;  // guards the per-device cudaFuncSetAttribute flags of every kernel instantiation
 // The plan depends on (N, M) only through the number of query blocks, whether the last block holds one or two
 // query tiles, and the number of 128-key tiles, so the cache is keyed on those: a decode loop whose key count
 // grows by one per step hits the cache for 128 consecutive steps (no cudaMalloc / blocking copy on the step path).
@@ -709,10 +671,6 @@ int get_plan(int B, int H, int N, int M, const Mode& mode, std::shared_ptr<Plan>
   int sms = 0;
   PCV_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   std::lock_guard<std::mutex> lk(g_plan_mu);
-  {
-    int rc = ensure_diag(dev);
-    if (rc != PCV_OK) return rc;
-  }
   if (mode.pair) sms /= 2;  // workers are CTA pairs
   const int QB = (N + mode.rows_per_unit - 1) / mode.rows_per_unit;
   const int T = (M + kTileN - 1) / kTileN;
@@ -757,36 +715,6 @@ int get_plan(int B, int H, int N, int M, const Mode& mode, std::shared_ptr<Plan>
   return PCV_OK;
 }
 
-PFN_cuTensorMapEncodeTiled_v12000 get_encode_fn() {
-  static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
-  static std::once_flag once;
-  std::call_once(once, [] {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(ptr);
-  });
-  return fn;
-}
-
-// (channels, rows, heads, batch) view of a (batch, rows, heads*channels)-style tensor; box = 64 x 128 x 1 x 1
-int make_tmap(CUtensorMap* tm, const void* base, int dtype, int channels, int rows, int heads, int batch,
-              int64_t stride_row, int64_t stride_head, int64_t stride_batch, int box_rows = kTileN) {
-  auto fn = get_encode_fn();
-  PCV_REQUIRE(fn != nullptr, PCV_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
-  cuuint64_t dims[4] = {(cuuint64_t)channels, (cuuint64_t)rows, (cuuint64_t)heads, (cuuint64_t)batch};
-  if (stride_batch == 0) stride_batch = (int64_t)rows * stride_row;  // broadcast batch: dim is 1, stride unused
-  cuuint64_t strides[3] = {(cuuint64_t)stride_row * 2, (cuuint64_t)stride_head * 2, (cuuint64_t)stride_batch * 2};
-  cuuint32_t box[4] = {64, (cuuint32_t)box_rows, 1, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  const CUtensorMapDataType dt = dtype == PCV_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  CUresult r = fn(tm, dt, 4, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  PCV_REQUIRE(r == CUDA_SUCCESS, PCV_ERR_CUDA, "cuTensorMapEncodeTiled failed with CUresult %d", (int)r);
-  return PCV_OK;
-}
-
 inline int pad64(int d) { return (d + 63) / 64 * 64; }
 
 size_t slots_bytes(const Plan& pl, int DV, int slot_rows) {
@@ -804,39 +732,12 @@ int dv_pass_width(int dv) { return std::min(kMaxDvPass, pad64(dv)); }
 template <int NQB, int NVB, bool BF16, bool PAIR>
 int launch_fwd(const Plan& pl, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const TcParams& p,
                cudaStream_t stream) {
-  using C = FwdCfg<NQB, NVB>;
-  auto kern = attn_fwd_kernel<NQB, NVB, BF16, PAIR>;
-  static bool attr_set[64] = {};  // per instantiation and device
-  int dev = 0;
-  PCV_CHECK_CUDA(cudaGetDevice(&dev));
-  {
-    std::lock_guard<std::mutex> lk(g_attr_mu);
-    if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-      PCV_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C::kSmemBytes));
-      if (dev >= 0 && dev < 64) attr_set[dev] = true;
-    }
-  }
   prof_mark_begin(stream);
-  if (PAIR) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(2 * pl.num_ctas);  // num_ctas counts CTA pairs in this mode
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = C::kSmemBytes;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    PCV_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, tq, tk, tv, p));
-  } else {
-    kern<<<pl.num_ctas, kThreads, C::kSmemBytes, stream>>>(tq, tk, tv, p);
-  }
+  // num_ctas counts CTA pairs in the pair mode
+  const int rc = launch_kernel(attn_fwd_kernel<NQB, NVB, BF16, PAIR>, dim3(PAIR ? 2 * pl.num_ctas : pl.num_ctas), kThreads,
+                               FwdCfg<NQB, NVB>::kSmemBytes, PAIR ? 2 : 0, stream, tq, tk, tv, p);
   prof_mark_end(stream);
-  PCV_CHECK_CUDA(cudaGetLastError());
-  count_launch();
+  if (rc != PCV_OK) return rc;
   if (pl.num_units > 0) {
     dim3 grid(pl.num_units, p.slot_rows / 8);
     if (NVB == 1)
@@ -880,13 +781,6 @@ int launch_dispatch(int nqb, int nvb, bool pair, const Plan& pl, const CUtensorM
 
 }  // namespace
 
-int debug_trace_read(unsigned long long* out, int n) {
-  (void)out;
-  (void)n;
-  set_error("debug_trace_read: the Hopper kernels record no clock trace");
-  return PCV_ERR_UNSUPPORTED;
-}
-
 // Host-only (no CUDA call): the work plan of the tensor-core kernel for a problem, one record of 8 ints per segment
 // {cta, b, h, q0, ntile, t0, t1, slot}; tests/test_plan_cpu.py checks its invariants on the CPU.
 int debug_plan(int B, int H, int N, int M, int workers, int rows_per_unit, int rows_per_tile, int32_t* segs,
@@ -907,11 +801,6 @@ int debug_plan(int B, int H, int N, int M, int workers, int rows_per_unit, int r
   return PCV_OK;
 }
 
-int debug_read(uint32_t* out, int n) {
-  for (int i = 0; i < n; ++i) out[i] = (g_diag_host != nullptr && i < 16) ? g_diag_host[i] : 0u;
-  return PCV_OK;
-}
-
 bool attn_tc_supported(const pcv_attn_params& p, const char** why) {
   auto fail = [&](const char* w) {
     *why = w;
@@ -921,7 +810,6 @@ bool attn_tc_supported(const pcv_attn_params& p, const char** why) {
   if (p.dv > 512) return fail("v head dim > 512");
   if ((p.dqk % 8) || (p.dv % 8)) return fail("head dims must be multiples of 8 (16-byte TMA strides)");
   if (!(p.scale > 0.f)) return fail("scale must be positive");
-  auto al16 = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
   if (!al16(p.q) || !al16(p.k) || !al16(p.v)) return fail("q/k/v base pointers must be 16-byte aligned");
   if ((p.q_stride_n % 8) || (p.k_stride_m % 8) || (p.v_stride_m % 8) || (p.q_stride_h % 8) || (p.k_stride_h % 8) ||
       (p.v_stride_h % 8) || (p.q_stride_b % 8) || (p.k_stride_b % 8) || (p.v_stride_b % 8))
@@ -933,10 +821,7 @@ bool attn_tc_supported(const pcv_attn_params& p, const char** why) {
     if (!al16(p.part_o) || (p.dv % 4)) return fail("partial output alignment");
   }
   if ((int64_t)p.N > (1 << 24) || (int64_t)p.M > (1 << 30)) return fail("sequence too long");
-  int dev = 0, major = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess)
-    return fail("no CUDA device");
-  if (major != 9) return fail("device is not sm_90");
+  if (const char* w = device_problem()) return fail(w);
   return true;
 }
 
@@ -947,7 +832,7 @@ int attn_tc_workspace_bytes(const pcv_attn_params& p, size_t* bytes) {
   if (rc != PCV_OK) return rc;
   size_t b = slots_bytes(*pl, dv_pass_width(p.dv), mode.slot_rows);
   b = (b + 255) / 256 * 256;
-  if (p.pad_mask != nullptr) b += sizeof(uint32_t) * (size_t)p.B * ((p.M + kTileN - 1) / kTileN * 4);
+  if (p.pad_mask != nullptr) b += sizeof(uint32_t) * (size_t)p.B * pad_words_per_row(p.M);
   *bytes = b;
   return PCV_OK;
 }
@@ -975,7 +860,9 @@ int launch_attn_tc(const pcv_attn_params& a, cudaStream_t stream, const pcv_shar
     PCV_REQUIRE(pad64(a.dqk) <= 128 && pad64(a.dv) <= 128 && sms >= 2, PCV_ERR_UNSUPPORTED,
                 "the CTA-pair kernel needs qk and v head dims <= 128 and at least two SMs");
   }
-  int rc = get_plan(a.B, a.H, a.N, a.M, mode, &pl);
+  int rc = attach_wait_diag(&g_wait_diag);
+  if (rc != PCV_OK) return rc;
+  rc = get_plan(a.B, a.H, a.N, a.M, mode, &pl);
   if (rc != PCV_OK) return rc;
   size_t need = 0;
   rc = attn_tc_workspace_bytes(a, &need);
@@ -1033,21 +920,18 @@ int launch_attn_tc(const pcv_attn_params& a, cudaStream_t stream, const pcv_shar
   if (a.pad_mask != nullptr) {
     size_t off = (slots_bytes(*pl, slot_dv, mode.slot_rows) + 255) / 256 * 256;
     uint32_t* bits = reinterpret_cast<uint32_t*>(ws + off);
-    p.pad_wpr = (a.M + kTileN - 1) / kTileN * 4;
     p.pad_bits = bits;
-    const int64_t total = (int64_t)a.B * p.pad_wpr;
-    int blocks = (int)std::min<int64_t>((total + 255) / 256, 1024);
-    pack_pad_kernel<<<blocks, 256, 0, stream>>>(a.pad_mask, a.pad_stride_b, a.B, a.M, p.pad_wpr, bits);
-    PCV_CHECK_CUDA(cudaGetLastError());
-    count_launch();
+    p.pad_wpr = pad_words_per_row(a.M);
+    rc = launch_pack_pad(a.pad_mask, a.pad_stride_b, a.B, a.M, bits, stream);
+    if (rc != PCV_OK) return rc;
   }
 
   CUtensorMap tq, tk, tv;
   const int Bq = a.q_stride_b == 0 ? 1 : a.B;
-  rc = make_tmap(&tq, a.q, a.dtype, a.dqk, a.N, a.H, Bq, a.q_stride_n, a.q_stride_h, a.q_stride_b);
+  rc = make_tmap_4d(&tq, a.q, a.dtype, a.dqk, a.N, a.H, Bq, a.q_stride_n, a.q_stride_h, a.q_stride_b, kTileM);
   if (rc != PCV_OK) return rc;
   const int kv_box_rows = mode.pair ? kTileN / 2 : kTileN;  // a pair loads 64-key halves of every K / V tile
-  rc = make_tmap(&tk, a.k, a.dtype, a.dqk, a.M, a.H, a.B, a.k_stride_m, a.k_stride_h, a.k_stride_b, kv_box_rows);
+  rc = make_tmap_4d(&tk, a.k, a.dtype, a.dqk, a.M, a.H, a.B, a.k_stride_m, a.k_stride_h, a.k_stride_b, kv_box_rows);
   if (rc != PCV_OK) return rc;
   const bool bf = a.dtype == PCV_BF16;
   const int nqb = pad64(a.dqk) / 64;
@@ -1057,7 +941,7 @@ int launch_attn_tc(const pcv_attn_params& a, cudaStream_t stream, const pcv_shar
     p.dv_pass = std::min(kMaxDvPass, a.dv - off);
     const int nvb = (p.dv_pass + 63) / 64;
     const char* vbase = reinterpret_cast<const char*>(a.v) + 2 * (size_t)off;
-    rc = make_tmap(&tv, vbase, a.dtype, p.dv_pass, a.M, a.H, a.B, a.v_stride_m, a.v_stride_h, a.v_stride_b, kv_box_rows);
+    rc = make_tmap_4d(&tv, vbase, a.dtype, p.dv_pass, a.M, a.H, a.B, a.v_stride_m, a.v_stride_h, a.v_stride_b, kv_box_rows);
     if (rc != PCV_OK) return rc;
     rc = bf ? launch_dispatch<true>(nqb, nvb, mode.pair, *pl, tq, tk, tv, p, stream)
             : launch_dispatch<false>(nqb, nvb, mode.pair, *pl, tq, tk, tv, p, stream);

@@ -2,9 +2,12 @@
 //   combine   : exact merge of partial softmax states (split-M inside a GPU, M-shards across GPUs)
 //   rotary    : RotaryPositionEmbedding.rotate           (reference position.py:30-50)
 //   kv_append : KV-cache concat                          (reference modules.py:117-121)
-// All three are pure streaming kernels: coalesced 16-byte (or widest legal) accesses, grid sized
+//   pack_pad  : pad-mask bytes -> bit words read by the tensor-core attention kernels
+// All are pure streaming kernels: coalesced 16-byte (or widest legal) accesses, grid sized
 // from the problem, no shared memory.
 #include "pcv_common.cuh"
+
+#include <algorithm>
 
 namespace pcv {
 namespace {
@@ -266,7 +269,33 @@ __global__ void __launch_bounds__(256) kv_append_kernel(const CopyArgs a) {
   }
 }
 
+// pad_mask bytes (B, M) -> bit words (B, wpr), wpr = pad_words_per_row(M); bit set = padding key
+__global__ void __launch_bounds__(256) pack_pad_kernel(const uint8_t* __restrict__ pad, int64_t stride_b, int B, int M,
+                                                       int wpr, uint32_t* __restrict__ bits) {
+  const int64_t total = (int64_t)B * wpr;
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int b = (int)(idx / wpr), w = (int)(idx % wpr);
+    uint32_t word = 0;
+    const int j0 = w * 32;
+    for (int i = 0; i < 32; ++i) {
+      const int j = j0 + i;
+      if (j < M && pad[(int64_t)b * stride_b + j] != 0) word |= (1u << i);
+    }
+    bits[idx] = word;
+  }
+}
+
 }  // namespace
+
+int launch_pack_pad(const uint8_t* pad, int64_t stride_b, int B, int M, uint32_t* bits, cudaStream_t stream) {
+  const int wpr = pad_words_per_row(M);
+  const int64_t total = (int64_t)B * wpr;
+  const int blocks = (int)std::min<int64_t>((total + 255) / 256, 1024);
+  pack_pad_kernel<<<blocks, 256, 0, stream>>>(pad, stride_b, B, M, wpr, bits);
+  PCV_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return PCV_OK;
+}
 
 int launch_combine_ex(const float* po, const float* pm, const float* pl, int nparts, const pcv_attn_params& p,
                       cudaStream_t stream) {

@@ -70,7 +70,13 @@ __device__ __forceinline__ float warp_sum(float v) {
   return v;
 }
 
+inline bool al16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15u) == 0; }
+
 // ---- launchers implemented in the individual .cu files ---------------------------------------
+// pad_mask bytes (B, M) -> bit words (B, pad_words_per_row(M)), bit set = padding key; one row covers whole 128-key tiles
+inline int pad_words_per_row(int M) { return 4 * ((M + 127) / 128); }
+int launch_pack_pad(const uint8_t* pad, int64_t stride_b, int B, int M, uint32_t* bits, cudaStream_t stream);
+
 int launch_attn_simt(const pcv_attn_params& p, cudaStream_t stream);
 int attn_simt_workspace_bytes(const pcv_attn_params& p, size_t* bytes);
 
@@ -78,10 +84,9 @@ bool attn_tc_supported(const pcv_attn_params& p, const char** why);
 int launch_attn_tc(const pcv_attn_params& p, cudaStream_t stream, const pcv_shard_fuse* fuse = nullptr);
 bool attn_tc_fuse_supported(const pcv_attn_params& p, const char** why);
 int attn_tc_workspace_bytes(const pcv_attn_params& p, size_t* bytes);
-int debug_read(uint32_t* out, int n);
+int debug_read(uint32_t* out, int n);  // the watchdog record of the wgmma kernels (16 words)
 int debug_plan(int B, int H, int N, int M, int workers, int rows_per_unit, int rows_per_tile, int32_t* segs,
                int max_segs, int32_t* counts);  // host-only dump of the tcgen05 work plan
-int debug_trace_read(unsigned long long* out, int n);  // PCV_TRACE=1 clock stamps (3 x 48 x 8)  // watchdog record of the tcgen05 kernel (16 words)
 
 bool attn_decode_supported(const pcv_attn_params& p, const char** why);
 int launch_attn_decode(const pcv_attn_params& p, cudaStream_t stream);
@@ -107,7 +112,6 @@ bool attn_fwd_dropout_supported(const pcv_attn_params& p, float dropout_p, const
 int attn_fwd_dropout_workspace_bytes(const pcv_attn_params& p, size_t* bytes);
 int launch_attn_fwd_dropout(const pcv_attn_params& p, const float* stat_m, const float* stat_l, float dropout_p,
                             uint64_t seed, cudaStream_t stream);
-int bwd_debug_read(uint32_t* out, int n);
 int launch_dropout_mask(uint8_t* keep, int B, int H, int N, int M, float dropout_p, uint64_t seed, cudaStream_t stream);
 
 }  // namespace pcv

@@ -20,12 +20,8 @@
 #include "pcv_common.cuh"
 #include "pcv_sm90.cuh"
 
-#include <cuda.h>
-#include <cudaTypedefs.h>
-
 #include <algorithm>
 #include <cstdlib>
-#include <mutex>
 
 namespace pcv {
 namespace {
@@ -332,70 +328,16 @@ int launch_ln_stats_t(const pcv_ln_stats_params& p, cudaStream_t stream) {
   return PCV_OK;
 }
 
-PFN_cuTensorMapEncodeTiled_v12000 encode_fn() {
-  static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
-  static std::once_flag once;
-  std::call_once(once, [] {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-        qres == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(ptr);
-  });
-  return fn;
-}
-
-// (inner, rows) row-major view with a row stride in elements; box = 64 x box_rows, SWIZZLE_128B
-int make_tmap_2d(CUtensorMap* tm, const void* base, int dtype, int64_t inner, int64_t rows, int64_t stride_row,
-                 int box_rows) {
-  auto fn = encode_fn();
-  PCV_REQUIRE(fn != nullptr, PCV_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
-  cuuint64_t dims[2] = {(cuuint64_t)inner, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)stride_row * 2};
-  cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  const CUtensorMapDataType dt = dtype == PCV_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  CUresult r = fn(tm, dt, 2, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  PCV_REQUIRE(r == CUDA_SUCCESS, PCV_ERR_CUDA, "cuTensorMapEncodeTiled (2-D) failed with CUresult %d", (int)r);
-  return PCV_OK;
-}
-
 template <bool BF16, bool FUSE, int CG>
 int launch_gemm(const CUtensorMap& tx, const CUtensorMap& tw, const GemmParams& gp, cudaStream_t stream) {
-  auto kern = kvproj_kernel<BF16, FUSE, CG>;
-  static std::mutex mu;
-  static bool attr_set[64] = {};
-  int dev = 0;
-  PCV_CHECK_CUDA(cudaGetDevice(&dev));
-  {
-    std::lock_guard<std::mutex> lk(mu);
-    if (dev < 0 || dev >= 64 || !attr_set[dev]) {
-      PCV_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes));
-      if (dev >= 0 && dev < 64) attr_set[dev] = true;
-    }
-  }
   const int64_t m_blocks = (gp.rows + kBM * CG - 1) / (kBM * CG) * CG;  // whole pairs; a pair's spare block is all padding
   const int64_t tiles = m_blocks * gp.tiles_n;
   PCV_REQUIRE(tiles <= 0x7fffffff, PCV_ERR_UNSUPPORTED, "kv_project: %lld tiles exceed the grid limit", (long long)tiles);
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)tiles);
-  cfg.blockDim = dim3(kGemmThreads);
-  cfg.dynamicSmemBytes = kSmemBytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CG;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
   prof_mark_begin(stream);
-  PCV_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, tx, tw, gp));
+  const int rc = launch_kernel(kvproj_kernel<BF16, FUSE, CG>, dim3((unsigned)tiles), kGemmThreads, kSmemBytes, CG, stream,
+                               tx, tw, gp);
   prof_mark_end(stream);
-  PCV_CHECK_CUDA(cudaGetLastError());
-  count_launch();
-  return PCV_OK;
+  return rc;
 }
 
 }  // namespace
@@ -413,7 +355,6 @@ bool kv_project_supported(const pcv_kvproj_params& p, const char** why) {
     *why = w;
     return false;
   };
-  auto al16 = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
   if (p.dtype != PCV_BF16 && p.dtype != PCV_F16) return fail("dtype must be bf16 or fp16");
   if (p.C < 8 || (p.C % 8)) return fail("input channels must be a multiple of 8 (16-byte TMA strides)");
   if (p.n_k < 0 || p.n_v < 0 || p.n_k + p.n_v < 1) return fail("no output columns");
@@ -424,10 +365,7 @@ bool kv_project_supported(const pcv_kvproj_params& p, const char** why) {
   if ((p.x_stride_row % 8) || (p.k_stride_row % 8) || (p.v_stride_row % 8)) return fail("row strides must be multiples of 8 elements");
   if (p.rows < 1 || p.rows > (int64_t)0x7fffff00) return fail("row count out of range");
   if (p.cta_group < 0 || p.cta_group > 2) return fail("cta_group must be 0, 1 or 2");
-  int dev = 0, major = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev) != cudaSuccess)
-    return fail("no CUDA device");
-  if (major != 9) return fail("device is not sm_90");
+  if (const char* w = device_problem()) return fail(w);
   return true;
 }
 
@@ -454,8 +392,10 @@ int launch_kv_project(const pcv_kvproj_params& p, cudaStream_t stream) {
   gp.eps = p.ln_eps;
   const bool fuse = p.row_stats == nullptr && p.ln_eps > 0.f;
 
+  int rc = attach_wait_diag(&g_wait_diag);
+  if (rc != PCV_OK) return rc;
   CUtensorMap tx, tw;
-  int rc = make_tmap_2d(&tx, p.x, p.dtype, p.C, p.rows, p.x_stride_row, kBM);
+  rc = make_tmap_2d(&tx, p.x, p.dtype, p.C, p.rows, p.x_stride_row, kBM);
   if (rc != PCV_OK) return rc;
   // one CTA per tile by default; cta_group = 2 asks for the 2-CTA clusters (each CTA loads half of the weight box)
   const int cg = p.cta_group == 2 ? 2 : 1;

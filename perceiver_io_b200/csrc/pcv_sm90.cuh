@@ -1,9 +1,14 @@
 // pcv_sm90.cuh — thin inline-PTX wrappers for the Hopper (sm_90a) features the tensor-core kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), warpgroup MMA (wgmma.mma_async) and its shared-memory descriptors.
+// mbarrier, TMA (cp.async.bulk.tensor), warpgroup MMA (wgmma.mma_async) and its shared-memory descriptors; and the
+// host side of those kernels (tensor maps, watchdog record, launch), implemented in pcv_sm90_host.cu.
 #pragma once
 
 #include <cstdint>
+#include <utility>
+#include <cuda.h>
 #include <cuda_runtime.h>
+
+#include "pcv_common.cuh"
 
 namespace pcv {
 namespace sm90 {
@@ -43,9 +48,10 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Watchdog record (mapped pinned host memory, set by the library at load; may stay null).  A wait that
-// does not complete within kWaitTimeoutNs is a pipeline deadlock: record where, then trap, so that a bug
-// surfaces as a CUDA error with a diagnosis instead of a hung GPU.
+// Watchdog record (the library's one mapped pinned 16-word host record; null until attach_wait_diag ran for this
+// translation unit on the device).  A wait that does not complete within kWaitTimeoutNs is a pipeline deadlock:
+// record where, then trap, so that a bug surfaces as a CUDA error with a diagnosis instead of a hung GPU.
+// Without -rdc every .cu file is its own module with its own copy of this variable.
 __device__ uint32_t* g_wait_diag = nullptr;
 constexpr uint64_t kWaitTimeoutNs = 4000000000ull;
 
@@ -56,6 +62,12 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
 }
 
 // Blocks until the phase with the given parity has completed.  A fresh barrier passes parity 1.
+// Sites (word 1 of the record), unique in the library:
+//    1- 5  attn_fwd_kernel     1 Q slot free, 2 ring slot free, 3 Q loaded, 4 K box loaded, 5 V box loaded
+//   11-12  kvproj_kernel      11 ring slot free, 12 stage loaded
+//   21-24  bwd_dkdv_kernel    21 K/V tile free, 22 Q/dO slot free, 23 K/V tile loaded, 24 Q/dO stage loaded
+//   31-33  bwd_dq_kernel      31 K/V slot free, 32 Q (and dO) loaded, 33 K/V stage loaded
+//   41-43  peer_tail_kernel   41 partial states of all ranks, 42 grid arrival, 43 outputs of all ranks (flag waits)
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, uint32_t site = 0) {
   uint32_t spins = 0;
   uint64_t t0 = 0;
@@ -271,6 +283,50 @@ __device__ __forceinline__ void wgmma_rs<64, false>(float (&d)[32], const uint32
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
+}
+
+// ---- host ------------------------------------------------------------------------------------
+// nullptr when the current device has compute capability 9, else why the wgmma kernels cannot run on it
+const char* device_problem();
+
+// SWIZZLE_128B tensor maps of 16-bit operands with 64-channel boxes (L2_256B promotion, no OOB fill).
+// 4-D (channels, rows, heads, batch) view of a (batch, rows, heads*channels)-style tensor, box 64 x box_rows x 1 x 1;
+// stride_batch == 0 broadcasts one batch row to every b (batch must then be 1).
+int make_tmap_4d(CUtensorMap* tm, const void* base, int dtype, int channels, int rows, int heads, int batch,
+                 int64_t stride_row, int64_t stride_head, int64_t stride_batch, int box_rows);
+// 2-D (inner, rows) row-major view with a row stride in elements, box 64 x box_rows
+int make_tmap_2d(CUtensorMap* tm, const void* base, int dtype, int64_t inner, int64_t rows, int64_t stride_row,
+                 int box_rows);
+
+// Points a translation unit's g_wait_diag (pass &sm90::g_wait_diag) at the library's watchdog record on the current
+// device; cheap after the first call per (symbol, device).
+int attach_wait_diag(const void* symbol);
+
+// Raises the kernel's dynamic shared-memory limit to `smem` once per (kernel, device).
+int set_smem_limit(const void* kernel, int smem);
+
+// Launches a wgmma kernel (cluster > 0: clusters of `cluster` CTAs along x) and counts it.
+template <typename... KArgs, typename... Args>
+int launch_kernel(void (*kernel)(KArgs...), dim3 grid, int threads, int smem, int cluster, cudaStream_t stream,
+                  Args&&... args) {
+  const int rc = set_smem_limit(reinterpret_cast<const void*>(kernel), smem);
+  if (rc != PCV_OK) return rc;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = grid;
+  cfg.blockDim = dim3(threads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = cluster;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = cluster > 0 ? 1 : 0;
+  PCV_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...));
+  PCV_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return PCV_OK;
 }
 
 }  // namespace sm90

@@ -1,13 +1,13 @@
 #!/bin/bash
-# Whole-library SASS evidence (run on the CPU box): per sm_100a kernel the counts of the Blackwell-native mnemonics
-# (UTCHMMA = tcgen05.mma, LDTM/STTM = tcgen05.ld/st, UTMALDG/UTMASTG = TMA load/store, UTCBAR = tcgen05.commit) and of
-# legacy tensor instructions (HMMA), plus the library totals.  usage: tools/sass_summary.sh [lib.so]
+# Whole-library SASS evidence (run on the CPU box): per sm_90a kernel the counts of the Hopper mnemonics
+# (HGMMA = wgmma.mma_async, UTMALDG = TMA load, SYNCS = mbarrier operations), of MUFU (ex2 of the softmax) and of
+# local-memory traffic (LDL/STL: register spills), plus the library totals.  usage: tools/sass_summary.sh [lib.so]
 LIB=${1:-perceiver_io_b200/lib/libpcv_attn.so}
 cuobjdump -sass $LIB > /tmp/sass_all.txt
 python3 - <<'PY'
 import re, collections
 cur=None; per=collections.OrderedDict()
-keys=["UTCHMMA","LDTM","STTM","UTMALDG","UTMASTG","UTCBAR","HMMA","MUFU","SYNCS","LDL","STL"]
+keys=["HGMMA","UTMALDG","SYNCS","MUFU","LDL","STL"]
 for line in open('/tmp/sass_all.txt'):
     m=re.search(r"Function : (\S+)", line)
     if m:
@@ -23,7 +23,7 @@ print("| kernel | " + " | ".join(keys) + " | instructions |"); print("|---|" + "
 import subprocess
 for fn,c in per.items():
     tot.update(c)
-    if c["UTCHMMA"] or c["UTMALDG"] or c["total"]>1500:
+    if c["HGMMA"] or c["UTMALDG"] or c["total"]>1500:
         name=subprocess.run(["c++filt",fn],capture_output=True,text=True).stdout.strip()
         name=re.sub(r"pcv::\(anonymous namespace\)::","",name); name=re.sub(r"\(CUtensorMap_st.*","",name)[:70]
         print(f"| {name} | " + " | ".join(str(c[k]) for k in keys) + f" | {c['total']} |")
