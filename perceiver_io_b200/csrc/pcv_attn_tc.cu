@@ -5,7 +5,9 @@
 //   O += P V   (wgmma RS: P re-used in place as the 16-bit A fragment, V box read MN-major, O in registers)
 //
 // CTA = one 128-row query tile of one (batch, head) x a contiguous range of 128-key tiles; 384 threads:
-// warpgroup 0 is the TMA producer (one lane), warpgroups 1 and 2 each own 64 query rows.
+// warpgroup 0 is the TMA producer (one lane), warpgroups 1 and 2 each own 64 query rows.  For head dims up to 128 a
+// consumer warpgroup overlaps the P V of tile t - 1 with the softmax of tile t, and the two consumer warpgroups take
+// turns at issuing their GEMMs, so the tensor cores work while the softmax runs (see kPipelined in attn_fwd_kernel).
 // CTA-pair variant (PAIR, impl = PCV_IMPL_TCGEN05_PAIR): a 2-CTA cluster takes two adjacent query tiles of the same
 // (b, h) and key range; each CTA loads one 64-key half of every K / V box and multicasts it to both, so the pair
 // reads each key tile from L2 once.  A ring slot is refilled only after the consumers of BOTH CTAs released it.  Q stays in shared
@@ -271,12 +273,96 @@ struct FwdBarriers {
   uint64_t q_full, q_empty;
 };
 
+// Scores of one 128-key tile (this thread's 64 accumulator registers) -> unnormalised probabilities in place: scale to
+// the log2 domain, apply the masks, update the running row maxima and denominators.  alpha is the factor by which the
+// running numerator has to be rescaled before this tile's P V is added.  `interior` (uniform over the warpgroup): no
+// key of the tile is masked for any row of the warpgroup, so the per-element checks and pad-word loads are skipped.
+__device__ __forceinline__ void tile_softmax(float (&s)[64], float (&m_run)[2], float (&l_run)[2], float (&alpha)[2],
+                                             const TcParams& p, int b, int j0, int n0, int cq, bool interior) {
+  float mx[2] = {-INFINITY, -INFINITY};
+  if (interior) {
+#pragma unroll
+    for (int i = 0; i < 64; ++i) {
+      s[i] *= p.scale_log2;
+      mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
+    }
+  } else {
+#pragma unroll
+    for (int g = 0; g < 16; ++g) {
+      const int jb = j0 + 8 * g + cq;
+      uint32_t padw = 0;
+      if (p.pad_bits != nullptr) padw = p.pad_bits[(int64_t)b * p.pad_wpr + (jb >> 5)];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int j = jb + (e & 1);
+        const int n = n0 + 8 * (e >> 1);
+        float x = s[4 * g + e] * p.scale_log2;
+        if (j >= p.M) x = -INFINITY;
+        else if (((padw >> (j & 31)) & 1u) || (p.causal && j > n + p.causal_shift)) x = kMaskedScore;
+        s[4 * g + e] = x;
+        mx[e >> 1] = fmaxf(mx[e >> 1], x);
+      }
+    }
+  }
+  float mref[2];
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+    mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+    const float mn = fmaxf(m_run[r], mx[r]);
+    alpha[r] = (mn == -INFINITY) ? 1.f : ex2(m_run[r] - mn);
+    mref[r] = (mn == -INFINITY) ? 0.f : mn;
+    m_run[r] = mn;
+    l_run[r] *= alpha[r];
+  }
+#pragma unroll
+  for (int g = 0; g < 16; ++g) {
+    const float e0 = ex2(s[4 * g + 0] - mref[0]), e1 = ex2(s[4 * g + 1] - mref[0]);
+    const float e2 = ex2(s[4 * g + 2] - mref[1]), e3 = ex2(s[4 * g + 3] - mref[1]);
+    l_run[0] += e0 + e1;
+    l_run[1] += e2 + e3;
+    s[4 * g + 0] = e0;
+    s[4 * g + 1] = e1;
+    s[4 * g + 2] = e2;
+    s[4 * g + 3] = e3;
+  }
+}
+
+// probabilities -> the 16-bit A fragments of the P V wgmma (k-step kk covers keys [16 kk, 16 kk + 16))
+template <bool BF16>
+__device__ __forceinline__ void pack_p(const float (&s)[64], uint32_t (&pa)[8][4]) {
+#pragma unroll
+  for (int g = 0; g < 16; ++g) {
+    pa[g >> 1][(g & 1) * 2 + 0] = pack2(s[4 * g + 0], s[4 * g + 1], BF16);
+    pa[g >> 1][(g & 1) * 2 + 1] = pack2(s[4 * g + 2], s[4 * g + 3], BF16);
+  }
+}
+
+template <int NVB>
+__device__ __forceinline__ void rescale_o(float (&o)[NVB][32], const float (&alpha)[2]) {
+#pragma unroll
+  for (int v = 0; v < NVB; ++v)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[v][i] *= alpha[(i >> 1) & 1];
+}
+
 template <int NQB, int NVB, bool BF16, bool PAIR>
 __global__ void __launch_bounds__(kThreads, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
                 const __grid_constant__ CUtensorMap tv, const TcParams p) {
   using C = FwdCfg<NQB, NVB>;
   constexpr int NS = C::kSlots;
+  // Head dims up to 128 (NQB <= 2) run the pipelined schedule: per tile one commit group for S = Q K^T and one for
+  // O += P V, the P V of tile t - 1 runs under the softmax of tile t, and the two warpgroups take turns at issuing
+  // their GEMMs (ping-pong), so that one warpgroup's MMAs run while the other computes its softmax.  It holds the K
+  // boxes of tile t and the V boxes of tile t - 1 at once, which larger head dims do not leave ring slots for; they
+  // keep the serial schedule (per box: wait, issue, drain, release).
+  constexpr bool kPipelined = NQB <= 2;
+  static_assert(!kPipelined || NQB + NVB <= NS, "the pipelined schedule holds NQB + NVB ring slots");
+  // registers per thread: producer + 2 x consumer = 504 = the launch bound's 168 x 3; the pipelined consumers keep
+  // S, P and O live at once, the serial schedule's producer (ring index arithmetic by a non-power-of-two) spills at 24
+  constexpr int kProducerRegs = kPipelined ? 24 : 40, kConsumerRegs = kPipelined ? 240 : 232;
+  static_assert(kProducerRegs + 2 * kConsumerRegs == 504, "register split");
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sQ = smem;
@@ -303,7 +389,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
     __syncthreads();
 
   if (wg == 0) {
-    reg_dealloc<40>();
+    reg_dealloc<kProducerRegs>();
     if (threadIdx.x == 0) {
       uint32_t it = 0;
       for (int si = seg_lo; si < seg_hi; ++si) {
@@ -336,7 +422,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
     return;
   }
 
-  reg_alloc<232>();
+  reg_alloc<kConsumerRegs>();
   const int cw = wg - 1;                 // consumer warpgroup: query rows [64*cw, 64*cw + 64) of the tile
   const int tid = threadIdx.x - 128 * wg;
   const int warp = tid >> 5, lane = tid & 31;
@@ -344,8 +430,59 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
   const int cq = 2 * (lane & 3);                      // first of the two columns of every 8-column group
   const uint32_t q_base = smem_u32(sQ) + cw * 64 * 128;
   const uint32_t ring_base = smem_u32(sRing);
-  uint32_t it = 0;
+  uint32_t it = 0;  // ring index of the next box (the producer's order: the NQB K boxes, then the NVB V boxes of a tile)
 
+  auto wait_full = [&](uint32_t i, uint32_t site) { mbar_wait(&bar.full[i % NS], (i / NS) & 1, site); };
+  auto release = [&](uint32_t i) {
+    if (PAIR) warp_arrive_pair(&bar.empty[i % NS]);
+    else warp_arrive(&bar.empty[i % NS]);
+  };
+  // S = Q K^T of the tile whose first K box is ring index i: one commit group
+  auto issue_qk = [&](float (&s)[64], uint32_t i) {
+#pragma unroll
+    for (int c = 0; c < NQB; ++c) wait_full(i + c, 6);
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < NQB; ++c)
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)
+        wgmma_ss<128, BF16>(s, make_desc(q_base + c * kBoxBytes + kk * 32),
+                            make_desc(ring_base + (i + c) % NS * kBoxBytes + kk * 32), (c | kk) != 0);
+    wgmma_commit();
+  };
+  // O += P V of the tile whose first V box is ring index i: one commit group
+  auto issue_pv = [&](float (&o)[NVB][32], const uint32_t (&pa)[8][4], uint32_t i) {
+#pragma unroll
+    for (int v = 0; v < NVB; ++v) wait_full(i + v, 7);
+    wgmma_fence();
+#pragma unroll
+    for (int v = 0; v < NVB; ++v)
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk)
+        wgmma_rs<64, BF16>(o[v], pa[kk], make_desc(ring_base + (i + v) % NS * kBoxBytes + kk * 2048));
+    wgmma_commit();
+  };
+  // Ping-pong turns.  Warpgroup cw waits on its own named barrier (id 1 + cw) before it issues its GEMMs and hands
+  // the turn over by arriving on the other's (id 2 - cw) after it committed them; a phase counts 256 threads (128
+  // syncing + 128 arriving).  Invariant: both warpgroups run the same segments with the same key tiles (the plan is
+  // per CTA, and every segment has at least one tile), so each takes exactly nt + 1 turns per segment of nt tiles.
+  // Warpgroup 1 hands warpgroup 0 the first turn and skips the hand-over after its own last turn, so that both
+  // barriers see as many arrivals as syncs:  id 1: n syncs (wg 0), 1 + (n - 1) arrivals (wg 1);  id 2: n and n.
+  constexpr int kTurnThreads = 256;
+  auto turn_begin = [&] {
+    if (cw == 0) named_bar_sync<1, kTurnThreads>();
+    else named_bar_sync<2, kTurnThreads>();
+  };
+  auto turn_end = [&](bool last) {
+    if (cw == 0) named_bar_arrive<2, kTurnThreads>();
+    else if (!last) named_bar_arrive<1, kTurnThreads>();
+  };
+  if (kPipelined && cw == 1 && seg_lo < seg_hi) named_bar_arrive<1, kTurnThreads>();
+
+  // PAIR: the consumers' closing cluster barrier (the peer may still arrive on this CTA's ring barriers until both
+  // CTAs reach it) is issued inside the segment loop, after the last segment: a barrier after the loop makes ptxas
+  // budget the whole consumer path at the launch bound (168 registers) and serialise the wgmmas.
+  if (PAIR && seg_lo == seg_hi) cluster_sync_all();
   for (int si = seg_lo; si < seg_hi; ++si) {
     const Segment sg = p.segs[si];
     mbar_wait(&bar.q_full, (si - seg_lo) & 1, 3);
@@ -356,80 +493,95 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
       for (int i = 0; i < 32; ++i) o[v][i] = 0.f;
     float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
     const int n0 = sg.q0 + qoff + rloc;
+    const int n_wg = sg.q0 + qoff + 64 * cw;  // first query row of this warpgroup
+    // no key of the tile starting at j0 is masked for any row of this warpgroup
+    auto interior = [&](int j0) {
+      return p.pad_bits == nullptr && j0 + kTileN <= p.M && (!p.causal || j0 + kTileN - 1 <= n_wg + p.causal_shift);
+    };
 
-    for (int t = sg.t0; t < sg.t1; ++t) {
-      float s[64];
-#pragma unroll
-      for (int c = 0; c < NQB; ++c, ++it) {
-        const uint32_t sl = it % NS;
-        mbar_wait(&bar.full[sl], (it / NS) & 1, 4);
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < 4; ++kk)
-          wgmma_ss<128, BF16>(s, make_desc(q_base + c * kBoxBytes + kk * 32), make_desc(ring_base + sl * kBoxBytes + kk * 32),
-                              (c | kk) != 0);
-        wgmma_commit();
+    if constexpr (kPipelined) {
+      float s[64], alpha[2];
+      uint32_t pa[8][4];
+      uint32_t ik = it;  // ring index of the first K box of the current tile
+      if (sg.t1 > sg.t0) {
+        // prologue: S of the first tile, its softmax (O is still zero: nothing to rescale)
+        turn_begin();
+        issue_qk(s, ik);
+        turn_end(false);
         wgmma_wait<0>();
         fence_regs(s);
-        if (PAIR) warp_arrive_pair(&bar.empty[sl]);
-        else warp_arrive(&bar.empty[sl]);
-      }
-      // scores -> log2 domain with the masks; row maxima over the quad
-      const int j0 = t * kTileN;
-      float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-      for (int g = 0; g < 16; ++g) {
-        const int jb = j0 + 8 * g + cq;
-        uint32_t padw = 0;
-        if (p.pad_bits != nullptr) padw = p.pad_bits[(int64_t)sg.b * p.pad_wpr + (jb >> 5)];
+        for (int c = 0; c < NQB; ++c) release(ik + c);
+        tile_softmax(s, m_run, l_run, alpha, p, sg.b, sg.t0 * kTileN, n0, cq, interior(sg.t0 * kTileN));
+        pack_p<BF16>(s, pa);
+        for (int t = sg.t0 + 1; t < sg.t1; ++t) {
+          const uint32_t iv = ik + NQB;  // V boxes of tile t - 1
+          ik += NQB + NVB;
+          turn_begin();
+          issue_qk(s, ik);
+          issue_pv(o, pa, iv);
+          turn_end(false);
+          wgmma_wait<1>();  // S of tile t is ready; P V of tile t - 1 still runs under the softmax below
+          fence_regs(s);
 #pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int j = jb + (e & 1);
-          const int n = n0 + 8 * (e >> 1);
-          float x = s[4 * g + e] * p.scale_log2;
-          if (j >= p.M) x = -INFINITY;
-          else if (((padw >> (j & 31)) & 1u) || (p.causal && j > n + p.causal_shift)) x = kMaskedScore;
-          s[4 * g + e] = x;
-          mx[e >> 1] = fmaxf(mx[e >> 1], x);
+          for (int c = 0; c < NQB; ++c) release(ik + c);
+          tile_softmax(s, m_run, l_run, alpha, p, sg.b, t * kTileN, n0, cq, interior(t * kTileN));
+          wgmma_wait<0>();
+#pragma unroll
+          for (int v = 0; v < NVB; ++v) {
+            fence_regs(o[v]);
+            release(iv + v);
+          }
+          rescale_o(o, alpha);
+          pack_p<BF16>(s, pa);
+        }
+        // epilogue: P V of the last tile
+        turn_begin();
+        issue_pv(o, pa, ik + NQB);
+        turn_end(si + 1 == seg_hi);  // the last turn of this CTA
+        wgmma_wait<0>();
+#pragma unroll
+        for (int v = 0; v < NVB; ++v) {
+          fence_regs(o[v]);
+          release(ik + NQB + v);
         }
       }
-      float mref[2], alpha[2];
+      it += (uint32_t)(sg.t1 - sg.t0) * (NQB + NVB);
+    } else {
+      for (int t = sg.t0; t < sg.t1; ++t) {
+        float s[64];
 #pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-        const float mn = fmaxf(m_run[r], mx[r]);
-        alpha[r] = (mn == -INFINITY) ? 1.f : ex2(m_run[r] - mn);
-        mref[r] = (mn == -INFINITY) ? 0.f : mn;
-        m_run[r] = mn;
-        l_run[r] *= alpha[r];
-      }
+        for (int c = 0; c < NQB; ++c, ++it) {
+          const uint32_t sl = it % NS;
+          mbar_wait(&bar.full[sl], (it / NS) & 1, 4);
+          wgmma_fence();
 #pragma unroll
-      for (int v = 0; v < NVB; ++v)
+          for (int kk = 0; kk < 4; ++kk)
+            wgmma_ss<128, BF16>(s, make_desc(q_base + c * kBoxBytes + kk * 32),
+                                make_desc(ring_base + sl * kBoxBytes + kk * 32), (c | kk) != 0);
+          wgmma_commit();
+          wgmma_wait<0>();
+          fence_regs(s);
+          release(it);
+        }
+        float alpha[2];
+        tile_softmax(s, m_run, l_run, alpha, p, sg.b, t * kTileN, n0, cq, interior(t * kTileN));
+        rescale_o(o, alpha);
+        uint32_t pa[8][4];
+        pack_p<BF16>(s, pa);
 #pragma unroll
-        for (int i = 0; i < 32; ++i) o[v][i] *= alpha[(i >> 1) & 1];
-      uint32_t pa[8][4];
+        for (int v = 0; v < NVB; ++v, ++it) {
+          const uint32_t sl = it % NS;
+          mbar_wait(&bar.full[sl], (it / NS) & 1, 5);
+          wgmma_fence();
 #pragma unroll
-      for (int g = 0; g < 16; ++g) {
-        const float e0 = ex2(s[4 * g + 0] - mref[0]), e1 = ex2(s[4 * g + 1] - mref[0]);
-        const float e2 = ex2(s[4 * g + 2] - mref[1]), e3 = ex2(s[4 * g + 3] - mref[1]);
-        l_run[0] += e0 + e1;
-        l_run[1] += e2 + e3;
-        pa[g >> 1][(g & 1) * 2 + 0] = pack2(e0, e1, BF16);
-        pa[g >> 1][(g & 1) * 2 + 1] = pack2(e2, e3, BF16);
-      }
-#pragma unroll
-      for (int v = 0; v < NVB; ++v, ++it) {
-        const uint32_t sl = it % NS;
-        mbar_wait(&bar.full[sl], (it / NS) & 1, 5);
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) wgmma_rs<64, BF16>(o[v], pa[kk], make_desc(ring_base + sl * kBoxBytes + kk * 2048));
-        wgmma_commit();
-        wgmma_wait<0>();
-        fence_regs(o[v]);
-        if (PAIR) warp_arrive_pair(&bar.empty[sl]);
-        else warp_arrive(&bar.empty[sl]);
+          for (int kk = 0; kk < 8; ++kk)
+            wgmma_rs<64, BF16>(o[v], pa[kk], make_desc(ring_base + sl * kBoxBytes + kk * 2048));
+          wgmma_commit();
+          wgmma_wait<0>();
+          fence_regs(o[v]);
+          release(it);
+        }
       }
     }
     warp_arrive(&bar.q_empty);  // every wgmma reading Q of this segment has completed
@@ -485,8 +637,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
           }
       }
     }
+    if (PAIR && si + 1 == seg_hi) cluster_sync_all();
   }
-  if (PAIR) cluster_sync_all();
 }
 
 // --------------------------------------------------------------------------------------------------

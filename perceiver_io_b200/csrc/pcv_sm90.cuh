@@ -63,7 +63,8 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
 
 // Blocks until the phase with the given parity has completed.  A fresh barrier passes parity 1.
 // Sites (word 1 of the record), unique in the library:
-//    1- 5  attn_fwd_kernel     1 Q slot free, 2 ring slot free, 3 Q loaded, 4 K box loaded, 5 V box loaded
+//    1- 7  attn_fwd_kernel     1 Q slot free, 2 ring slot free, 3 Q loaded, 4 K box loaded, 5 V box loaded (serial
+//                              schedule); 6 K box loaded, 7 V box loaded (pipelined schedule)
 //   11-12  kvproj_kernel      11 ring slot free, 12 stage loaded
 //   21-24  bwd_dkdv_kernel    21 K/V tile free, 22 Q/dO slot free, 23 K/V tile loaded, 24 Q/dO stage loaded
 //   31-33  bwd_dq_kernel      31 K/V slot free, 32 Q (and dO) loaded, 33 K/V stage loaded
@@ -96,6 +97,18 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, uint32
 __device__ __forceinline__ void warp_arrive(uint64_t* bar) {
   __syncwarp();
   if ((threadIdx.x & 31) == 0) mbar_arrive(bar);
+}
+
+// ---- named barriers -----------------------------------------------------------------------------
+// Ids 1-15 (0 is __syncthreads); `threads` counts every thread that syncs or arrives on one phase, a multiple of 32.
+// Not covered by the mbar_wait watchdog: every sync needs its matching arrivals, or the CTA hangs.
+template <int ID, int THREADS>
+__device__ __forceinline__ void named_bar_sync() {
+  asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(THREADS) : "memory");
+}
+template <int ID, int THREADS>
+__device__ __forceinline__ void named_bar_arrive() {
+  asm volatile("bar.arrive %0, %1;" ::"n"(ID), "n"(THREADS) : "memory");
 }
 
 // ---- TMA ------------------------------------------------------------------------------------
