@@ -103,8 +103,8 @@ def masked_scores(q: Tensor, k: Tensor, pad_mask: Optional[Tensor], causal: bool
         s = s.masked_fill(pad_mask[:, None, None, :].bool(), neg)
     if causal:
         mt = m if m_total is None else m_total
-        rows = torch.arange(n)[:, None]
-        cols = torch.arange(m)[None, :] + m_offset
+        rows = torch.arange(n, device=s.device)[:, None]
+        cols = torch.arange(m, device=s.device)[None, :] + m_offset
         s = s.masked_fill(cols > rows + (mt - n), neg)
     return s
 

@@ -69,11 +69,11 @@ def derived_bound(ref64, eager):
     return 2.0 * eager_err + 1e-3 * max(ref_max, 1e-30), eager_err, ref_max
 
 
-def assert_parity(got, q, k, v, H, scale, pad=None, causal=False, what="", eager_dtype=None, floor=0.0):
+def assert_parity(got, q, k, v, H, scale, pad=None, causal=False, what="", eager_dtype=None, floor=0.0, per_row=False):
     """Check `got` against the fp64 reference with the DERIVED gate; returns (err, bound, eager_err).
 
     `floor`: lower limit of the bound for paths that add roundings the eager reference does not have (stated by
-    the caller where used)."""
+    the caller where used).  `per_row`: also apply the gate to every (b, h, n) row on its own (assert_rows)."""
     eager_dtype = q.dtype if eager_dtype is None else eager_dtype
     ref = torch_core(q, k, v, H, scale, pad, causal, torch.float64)
     eager = torch_core(q, k, v, H, scale, pad, causal, eager_dtype)
@@ -85,7 +85,78 @@ def assert_parity(got, q, k, v, H, scale, pad=None, causal=False, what="", eager
     err = (g - ref).abs().max().item()
     print(f"[parity] {what}: err {err:.3e}  bound {bound:.3e} (= 2 x eager {eager_err:.3e} + 1e-3 x max|ref| {ref_max:.3e})")
     assert err <= bound, f"{what}: max err {err:.3e} > derived bound {bound:.3e} (eager bf16 err {eager_err:.3e}, max|ref| {ref_max:.3e})"
+    if per_row:
+        assert_rows(g, ref, eager, H, what, floor)
     return err, bound, eager_err
+
+
+def assert_rows(got, ref, eager, H, what="", floor=0.0):
+    """The derived gate applied to every (b, h, n) output row separately:
+
+        max_c |got - ref|  <=  max(2 * max_c |eager - ref| + 1e-3 * max_c |ref|,  floor * max_c |ref|)
+
+    got / ref / eager are (B, N, H*dv).  One wrong key on one row moves that row by about |v| / (live keys); the
+    whole-tensor gate is set by the largest rows of the case and does not see it.  Prints the worst ratio of error to
+    bound and returns it."""
+    B, N = ref.shape[0], ref.shape[1]
+    r = ref.double().reshape(B, N, H, -1)
+    g = got.double().to(r.device).reshape(B, N, H, -1)
+    e = eager.double().to(r.device).reshape(B, N, H, -1)
+    err = (g - r).abs().amax(-1)
+    rmax = r.abs().amax(-1)
+    bound = torch.maximum(2.0 * (e - r).abs().amax(-1) + 1e-3 * rmax, floor * rmax).clamp_min(1e-30)
+    ratio = err / bound
+    worst = ratio.argmax().item()
+    b, n, h = worst // (N * H), (worst // H) % N, worst % H
+    bad = int((ratio > 1).sum().item())
+    print(f"[parity rows] {what}: worst err/bound {ratio.max().item():.3f} at (b={b}, h={h}, n={n}): "
+          f"err {err[b, n, h].item():.3e} bound {bound[b, n, h].item():.3e} max|ref| {rmax[b, n, h].item():.3e}")
+    assert bad == 0, (f"{what}: {bad} of {ratio.numel()} rows over their derived bound; worst (b={b}, h={h}, n={n}) "
+                      f"err {err[b, n, h].item():.3e} > {bound[b, n, h].item():.3e}")
+    return ratio.max().item()
+
+
+FLT_MAX = torch.finfo(torch.float32).max
+
+
+def assert_partial_state(part, q, k, v, H, scale, pad=None, causal=False, m_total=None, m_offset=0, what=""):
+    """attention_partial's (o, m, l) against oracle.mha_oracle.partial_state, evaluated in fp64 on the device on the
+    same operands (log2 domain: m = row max of the scaled scores, l = sum 2^(t - m), o = sum 2^(t - m) v).
+
+    - m: the kernel keeps the exact running max, so it is the oracle's up to the fp32 score rounding (abs 4e-3);
+    - l: relative 2e-3 (ex2.approx and fp32 sums; a max off by 4e-3 would alone move l by 0.3 %);
+    - o: elementwise within 2^-8 of sum p |v| (+ 1e-6 of it for the fp32 sums): the kernel rounds P to 16 bits before
+      P V, and 2^-8 is the unit roundoff of bf16;
+    - rows without a live key (the shard lies in the row's causal future, or the batch row is fully padded) follow the
+      finite-fill semantics exactly: m = -FLT_MAX (the oracle's -DBL_MAX), l = the shard's key count, and o = the sum
+      of the shard's V rows (fp32 accumulation: 2^-12 of sum |v|).  combine_partials weights such a shard by zero."""
+    po_k, pm_k, pl_k = (t.detach().double() for t in part)
+    dev = po_k.device
+    B, M = k.shape[0], k.shape[1]
+    qh = O.split_heads(q.detach().to(dev, torch.float64).expand(B, -1, -1), H)
+    kh, vh = O.split_heads(k.detach().to(dev, torch.float64), H), O.split_heads(v.detach().to(dev, torch.float64), H)
+    padd = None if pad is None else pad.to(dev)
+    mt = M if m_total is None else m_total
+    po, pm, pl = O.partial_state(qh, kh, vh, scale, padd, causal, mt, m_offset)
+    pa = O.partial_state(qh, kh, vh.abs(), scale, padd, causal, mt, m_offset)[0]
+    dead = pm == -torch.finfo(torch.float64).max
+    live = ~dead
+    assert torch.isfinite(po_k).all() and torch.isfinite(pl_k).all(), f"{what}: non-finite partial state"
+    assert (pm_k[dead] == -FLT_MAX).all(), f"{what}: rows without a live key must have m = -FLT_MAX"
+    l_dead = pl_k[dead]
+    assert (l_dead == pl[dead]).all(), (f"{what}: rows without a live key must have l = {M} (one per masked key); got "
+                                        f"{l_dead.min().item() if l_dead.numel() else None}..{l_dead.max().item() if l_dead.numel() else None}")
+    o_dead_err = ((po_k - po).abs() - 2.0 ** -12 * pa)[dead]
+    assert o_dead_err.numel() == 0 or o_dead_err.max().item() <= 0, f"{what}: o of rows without a live key != sum of V"
+    m_err = (pm_k - pm)[live].abs().max().item() if live.any() else 0.0
+    l_err = ((pl_k - pl).abs() / pl)[live].max().item() if live.any() else 0.0
+    o_ratio = ((po_k - po).abs() / ((2.0 ** -8 + 1e-6) * pa).clamp_min(1e-30))[live].max().item() if live.any() else 0.0
+    print(f"[partial] {what}: {int(dead.sum())} rows without a live key; live rows: |dm| {m_err:.2e}, "
+          f"rel dl {l_err:.2e}, o err / (2^-8 sum p|v|) {o_ratio:.3f}")
+    assert m_err <= 4e-3, f"{what}: row max off by {m_err:.3e} (log2 units)"
+    assert l_err <= 2e-3, f"{what}: denominator off by {l_err:.3e} relative"
+    assert o_ratio <= 1.0, f"{what}: numerator error {o_ratio:.3f} x 2^-8 sum p|v|"
+    return int(dead.sum())
 
 
 def torch_cross_attention(sd, x_q, x_kv, H, pad=None, dtype=torch.float64, device="cuda"):

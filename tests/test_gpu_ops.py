@@ -2,7 +2,7 @@
 import pytest
 import torch
 
-from gpu_util import assert_close, assert_parity, oracle_core, torch_core
+from gpu_util import assert_close, assert_parity, assert_partial_state, oracle_core, torch_core
 from oracle import mha_oracle as O
 
 pytestmark = pytest.mark.gpu
@@ -135,12 +135,11 @@ def test_m_shards_merge_to_the_unsharded_result(impl, causal):
     assert_close(merged, ref, rel, "merged shards")
     single = ops.attention(q, k, v, H, d ** -0.5, pad_mask=padc, causal=causal, impl=impl)
     assert_close(merged, single.double(), 1e-2, "merged vs single pass")
-    # the partial state itself matches the oracle's (log2-domain max, denominator)
-    qh = O.split_heads(q.cpu().double(), H)
-    kh, vh = O.split_heads(k.cpu().double(), H), O.split_heads(v.cpu().double(), H)
-    po, pm, pl = O.partial_state(qh, kh[:, :, :300], vh[:, :, :300], d ** -0.5, pad[:, :300], causal, M, 0)
-    w = torch.exp2(parts[0][1].cpu().double() - pm)     # kernel max may differ from the true max (lazy rescale)
-    assert_close(parts[0][2].cpu().double() * w, pl, 1e-2, "denominator")
+    # every shard's partial state (o, log2-domain row max, denominator) is the oracle's; the kernels keep the exact
+    # running max, and the fully padded shard of batch row 0 has the finite-fill state (m = -FLT_MAX, l = 400)
+    for (a, b), part in zip(zip(cuts[:-1], cuts[1:]), parts):
+        assert_partial_state(part, q, k[:, a:b], v[:, a:b], H, d ** -0.5, pad[:, a:b], causal, M, a,
+                             what=f"{impl} causal={causal} shard [{a}, {b})")
 
 
 def test_rotary_matches_oracle():
@@ -205,8 +204,8 @@ def test_head_major_4d_operands_by_stride():
 @pytest.mark.parametrize("shape", [(1, 256, 3000, 2, 192, 320), (2, 130, 1500, 1, 322, 322), (1, 300, 2000, 1, 512, 512)],
                          ids=lambda s: "x".join(map(str, s)))
 def test_big_head_kernel_multi_tile_with_masks(shape):
-    """qk head dims > 128 / v head dims > 256 (optical-flow geometry): chunked Q K^T, double-buffered S, two V
-    passes; several key tiles per CTA, padding + causal masks, partial-state output."""
+    """qk head dims > 128 / v head dims > 256 (optical-flow geometry): Q K^T over up to eight 64-channel boxes (serial
+    schedule), two V passes; several key tiles per CTA, padding + causal masks, partial-state output."""
     from perceiver_io_b200 import ops
 
     B, N, M, H, dqk, dv = shape
@@ -224,9 +223,9 @@ def test_big_head_kernel_multi_tile_with_masks(shape):
 
 
 def _ramp_qk(B, N, M, H, dqk, step_log2, dtype, seed=5):
-    """Scores that RISE with the key index by `step_log2` (log2 units of the softmax exponent) per 64 keys: the
-    exponent reference has to move again and again (accumulator rescale in TMEM) and, with a small step, the
-    optimistic tiles run far from the reference before their row-sum range check fires."""
+    """Scores that RISE with the key index by `step_log2` (log2 units of the softmax exponent) per 64 keys: the running
+    row max moves at every key tile, so the O accumulators (registers) and the denominator are rescaled again and
+    again by alpha = 2^(m_old - m_new)."""
     g = torch.Generator().manual_seed(seed)
     u = torch.randn(H, dqk, generator=g)
     uq = (u / (u * u).sum(-1, keepdim=True) * dqk ** 0.5).reshape(1, 1, H * dqk)
@@ -239,8 +238,9 @@ def _ramp_qk(B, N, M, H, dqk, step_log2, dtype, seed=5):
 @pytest.mark.parametrize("dtype", [torch.bfloat16, torch.float16], ids=["bf16", "fp16"])
 @pytest.mark.parametrize("step", [12.0, 1.5, -3.0], ids=["steep", "gentle", "falling"])
 def test_moving_reference_rescale_paths(dtype, step):
-    """steep: the reference moves at every half tile; gentle: optimistic tiles drift up to the fp16 (2^15) /
-    bf16 (2^40) row-sum bound before one is redone; falling: the first tile holds the maximum for good."""
+    """steep: the max rises by 24 (log2 units) per key tile, so at every tile alpha = 2^-24 all but clears the old
+    accumulators; gentle: it rises by 3 per tile (alpha = 1/8), so the roundings of many rescales add up; falling: the
+    first tile holds the maximum for good and alpha stays 1."""
     from perceiver_io_b200 import ops
 
     B, N, M, H, d = 2, 300, 2304, 2, 128
@@ -351,8 +351,10 @@ def test_decode_kernel_matches_oracle(shape, dtype):
 @pytest.mark.parametrize("shape", [(2, 300, 700, 2, 128, 128), (1, 512, 2048, 4, 64, 128), (3, 400, 900, 2, 96, 96),
                                    (2, 1024, 4096, 2, 128, 128)], ids=lambda s: "x".join(map(str, s)))
 def test_cta_pair_kernel_matches_oracle(shape):
-    """cta_group::2 kernel (two SMs per 256-row MMA, relaxed cross-CTA hand-offs, in-kernel fix-up of split units),
-    incl. padding + causal masks, ragged N / M, batch-1 queries and the partial-state output."""
+    """CTA-pair kernel (a 2-CTA cluster takes two adjacent 128-row query tiles; each CTA loads one 64-key half of
+    every K / V box and multicasts it to both, and a ring slot is refilled only after both CTAs released it; split
+    units merged by the combine kernel), incl. padding + causal masks, ragged N / M, batch-1 queries and the
+    partial-state output."""
     from perceiver_io_b200 import ops
 
     B, N, M, H, dqk, dv = shape
