@@ -390,6 +390,24 @@ PCV_API int pcv_attn_fwd_dropout(const pcv_attn_params* p, const float* stat_m, 
                                  uint64_t dropout_seed, void* stream);
 PCV_API int pcv_attn_dropout_mask(uint8_t* keep, int32_t B, int32_t H, int32_t N, int32_t M, float dropout_p,
                                   uint64_t dropout_seed, void* stream);
+/*
+ * The keys [key_begin, key_end) of the same keep mask: keep is (B, H, N, key_end - key_begin) bytes, 1 = the element
+ * survives.  pcv_attn_dropout_mask is the range [0, M).  Arguments are checked before any CUDA call.
+ */
+PCV_API int pcv_attn_dropout_mask_range(uint8_t* keep, int32_t B, int32_t H, int32_t N, int32_t key_begin,
+                                        int32_t key_end, float dropout_p, uint64_t dropout_seed, void* stream);
+/*
+ * One-pass training forward WITH attention-probability dropout, for every head dim the tensor-core forward takes (up
+ * to 512).  A write_partial pcv_attn_fwd over all keys (m_total == M, m_offset == 0; impl AUTO or TCGEN05, not the CTA
+ * pair) whose part_o is the numerator with dropout, scaled by 1/(1 - p): every element (b, h, query, key) is dropped
+ * with probability round(256 p)/256 by the same pure function of (dropout_seed, b, h, query, key) that
+ * pcv_attn_dropout_mask exports and pcv_attn_bwd regenerates.  part_m / part_l are the statistics of the dropout-free
+ * softmax, so pcv_attn_combine of the state gives out = dropout(P) V and the backward takes part_m / part_l as its
+ * stat_m / stat_l.  p->workspace must hold pcv_attn_workspace_bytes() of the call with impl = PCV_IMPL_TCGEN05 (with
+ * AUTO and at most 4 query rows it would size the decode kernel's workspace).  Arguments are checked before any CUDA call.
+ */
+PCV_API int pcv_attn_fwd_partial_dropout_supported(const pcv_attn_params* p, float dropout_p);
+PCV_API int pcv_attn_fwd_partial_dropout(const pcv_attn_params* p, float dropout_p, uint64_t dropout_seed, void* stream);
 
 /*
  * Live timing of the dominant kernel (bench.py's roofline leg): between pcv_profile_begin() and

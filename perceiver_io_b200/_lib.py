@@ -45,6 +45,9 @@ EXPORTS = (
     "pcv_attn_fwd_dropout_workspace_bytes",
     "pcv_attn_fwd_dropout",
     "pcv_attn_dropout_mask",
+    "pcv_attn_dropout_mask_range",
+    "pcv_attn_fwd_partial_dropout_supported",
+    "pcv_attn_fwd_partial_dropout",
     "pcv_launch_count",
     "pcv_debug_plan",
     "pcv_profile_begin",
@@ -268,6 +271,13 @@ def lib() -> C.CDLL:
         l.pcv_attn_dropout_mask.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float,
                                             C.c_uint64, C.c_void_p]
         l.pcv_attn_dropout_mask.restype = C.c_int
+        l.pcv_attn_dropout_mask_range.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                                  C.c_float, C.c_uint64, C.c_void_p]
+        l.pcv_attn_dropout_mask_range.restype = C.c_int
+        l.pcv_attn_fwd_partial_dropout_supported.argtypes = [C.POINTER(AttnParams), C.c_float]
+        l.pcv_attn_fwd_partial_dropout_supported.restype = C.c_int
+        l.pcv_attn_fwd_partial_dropout.argtypes = [C.POINTER(AttnParams), C.c_float, C.c_uint64, C.c_void_p]
+        l.pcv_attn_fwd_partial_dropout.restype = C.c_int
         l.pcv_debug_plan.argtypes = [C.c_int32] * 7 + [C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_int32)]
         l.pcv_debug_plan.restype = C.c_int
         for name in ("pcv_get_device_info", "pcv_attn_supported_tcgen05", "pcv_attn_workspace_bytes",

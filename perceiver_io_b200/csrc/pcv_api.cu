@@ -2,6 +2,7 @@
 // Argument validation, kernel-family dispatch and error reporting live here; kernels live in
 // pcv_attn_tc.cu (tcgen05), pcv_attn_simt.cu (CUDA cores) and pcv_aux.cu.
 #include "pcv_common.cuh"
+#include "pcv_dropout.cuh"
 
 #include <atomic>
 #include <cstring>
@@ -67,6 +68,19 @@ static bool use_decode(const pcv_attn_params& p, const char** why) {
     return false;
   }
   return attn_decode_supported(p, why);
+}
+
+// The one-pass dropout forward: the tensor-core kernel's partial state over all keys of an unsharded call.
+static bool partial_dropout_supported(const pcv_attn_params& p, float dropout_p, const char** why) {
+  auto no = [&](const char* w) {
+    *why = w;
+    return false;
+  };
+  if (!(dropout_p > 0.f && dropout_p < 1.f)) return no("dropout_p must be in (0, 1)");
+  if (!p.write_partial) return no("the call must write the partial state (write_partial = 1)");
+  if (p.m_total != p.M || p.m_offset != 0) return no("key sharding takes no dropout");
+  if (p.impl != PCV_IMPL_AUTO && p.impl != PCV_IMPL_TCGEN05) return no("only the single-CTA tensor-core kernel takes dropout");
+  return attn_tc_supported(p, why);
 }
 
 static bool use_tc(const pcv_attn_params& p, const char** why) {
@@ -295,7 +309,30 @@ int pcv_attn_fwd_dropout(const pcv_attn_params* p, const float* stat_m, const fl
 
 int pcv_attn_dropout_mask(uint8_t* keep, int32_t B, int32_t H, int32_t N, int32_t M, float dropout_p,
                           uint64_t dropout_seed, void* stream) {
-  return launch_dropout_mask(keep, B, H, N, M, dropout_p, dropout_seed, reinterpret_cast<cudaStream_t>(stream));
+  return launch_dropout_mask(keep, B, H, N, 0, M, dropout_p, dropout_seed, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pcv_attn_dropout_mask_range(uint8_t* keep, int32_t B, int32_t H, int32_t N, int32_t key_begin, int32_t key_end,
+                                float dropout_p, uint64_t dropout_seed, void* stream) {
+  return launch_dropout_mask(keep, B, H, N, key_begin, key_end, dropout_p, dropout_seed,
+                             reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pcv_attn_fwd_partial_dropout_supported(const pcv_attn_params* p, float dropout_p) {
+  if (validate_attn(p) != PCV_OK) return 0;
+  const char* why = "";
+  const bool ok = partial_dropout_supported(*p, dropout_p, &why);
+  if (!ok) set_error("one-pass dropout forward not applicable: %s", why);
+  return ok ? 1 : 0;
+}
+
+int pcv_attn_fwd_partial_dropout(const pcv_attn_params* p, float dropout_p, uint64_t dropout_seed, void* stream) {
+  int rc = validate_attn(p);
+  if (rc != PCV_OK) return rc;
+  const char* why = "";
+  PCV_REQUIRE(partial_dropout_supported(*p, dropout_p, &why), PCV_ERR_UNSUPPORTED, "attn_fwd_partial_dropout: %s", why);
+  const DropoutRule drop = dropout_rule(dropout_p, dropout_seed);
+  return launch_attn_tc(*p, reinterpret_cast<cudaStream_t>(stream), nullptr, &drop);
 }
 
 }  // extern "C"

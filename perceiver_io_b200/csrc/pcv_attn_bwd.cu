@@ -21,6 +21,7 @@
 //
 // Warpgroup 0 is the TMA producer (one lane), warpgroups 1 and 2 each own 64 rows of the tile.
 #include "pcv_common.cuh"
+#include "pcv_dropout.cuh"
 #include "pcv_sm90.cuh"
 
 #include <algorithm>
@@ -62,43 +63,15 @@ struct BwdParams {
   int splits, tiles_per_split;  // dq kernel
 };
 
-// ---- attention-probability dropout (modules.py:161: nn.Dropout on the softmax output) -----------------------------
-// Counter-based: the keep decision of element (b, h, query q, key k) is a pure function of (seed, b*H+h, q, k), so the
-// forward kernel and both backward kernels regenerate the same mask without storing it.  One 32-bit hash per 2 x 2 block
-// (query pair q>>1, key pair k>>1) yields four random bytes, byte (q&1)*2 + (k&1) belongs to (q, k); an element is
-// dropped iff its byte < drop_thresh, i.e. with probability drop_thresh/256 (the requested p rounded to 1/256; the
-// survivors are scaled by exactly 1/(1 - drop_thresh/256)).  A thread that walks keys (query fixed) or queries (key
-// fixed) needs one hash per two columns either way, and its own side of the input is a per-thread constant.
-// Hash: x = qside ^ kside, then two Philox-style rounds x <- hi(x*C) ^ lo(x*C) ^ K (one IMAD.WIDE + one LOP3 each).
-// Checked on 8M-element masks: keep rate, row / column rates, autocorrelation at lags up to 64 in both directions, across
-// heads and across adjacent seeds all at the sampling-noise floor (one round is NOT enough: seeds correlate at 3 %).
-__device__ __forceinline__ uint32_t drop_qword(uint32_t bh, uint32_t q) { return bh * 0x9E3779B1u + (q >> 1); }
-__device__ __forceinline__ uint32_t drop_qside(uint32_t seed_lo, uint32_t qword) { return qword * 0x9E3779B1u ^ seed_lo; }
-__device__ __forceinline__ uint32_t drop_kside(uint32_t seed_hi, uint32_t k) { return (k >> 1) * 0x85EBCA6Bu ^ seed_hi; }
-__device__ __forceinline__ uint32_t drop_round(uint32_t x, uint32_t c, uint32_t k) {
-  const uint64_t pr = (uint64_t)x * c;
-  return (uint32_t)(pr >> 32) ^ (uint32_t)pr ^ k;
-}
-__device__ __forceinline__ uint32_t drop_finish(uint32_t qside, uint32_t kside) {
-  uint32_t x = qside ^ kside;
-  x = drop_round(x, 0xD2511F53u, 0x9E3779B9u);
-  return drop_round(x, 0xCD9E8D57u, 0xBB67AE85u);
-}
-__device__ __forceinline__ uint32_t drop_bits(uint32_t seed_lo, uint32_t seed_hi, uint32_t bh, uint32_t q, uint32_t k) {
-  return drop_finish(drop_qside(seed_lo, drop_qword(bh, q)), drop_kside(seed_hi, k));
-}
-__device__ __forceinline__ bool drop_keep(uint32_t bits, uint32_t q, uint32_t k, uint32_t thresh) {
-  return ((bits >> (((q & 1u) * 2u + (k & 1u)) * 8u)) & 0xffu) >= thresh;
-}
-
-// keep mask of a whole problem (tests / debugging): keep[b][h][q][k] = 1 if the element survives
-__global__ void __launch_bounds__(256) drop_mask_kernel(uint8_t* __restrict__ keep, int B, int H, int N, int M,
-                                                        uint32_t thresh, uint32_t seed_lo, uint32_t seed_hi) {
-  const int64_t total = (int64_t)B * H * N * M;
+// keep mask of keys [key_begin, key_begin + W) (tests / the backward shim): keep[b][h][q][k - key_begin] = 1 if the
+// element survives
+__global__ void __launch_bounds__(256) drop_mask_kernel(uint8_t* __restrict__ keep, int B, int H, int N, int key_begin,
+                                                        int W, uint32_t thresh, uint32_t seed_lo, uint32_t seed_hi) {
+  const int64_t total = (int64_t)B * H * N * W;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
        idx += (int64_t)gridDim.x * blockDim.x) {
-    const uint32_t k = (uint32_t)(idx % M);
-    const int64_t r = idx / M;
+    const uint32_t k = (uint32_t)(key_begin + idx % W);
+    const int64_t r = idx / W;
     const uint32_t q = (uint32_t)(r % N), bh = (uint32_t)(r / N);
     keep[idx] = drop_keep(drop_bits(seed_lo, seed_hi, bh, q, k), q, k, thresh) ? 1 : 0;
   }
@@ -525,17 +498,12 @@ bwd_dq_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CU
 // ---------------------------------------------------------------------------------------------------------------
 inline size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
 
-// dropout probability -> byte threshold (p rounded to 1/256, at least 1/256 when p > 0) and survivor scale
 void set_dropout(BwdParams& p, float dropout_p, uint64_t seed) {
-  p.drop_thresh = 0;
-  p.drop_rp = 1.f;
-  if (dropout_p > 0.f) {
-    const long t = std::min(255L, std::max(1L, std::lround((double)dropout_p * 256.0)));
-    p.drop_thresh = (uint32_t)t;
-    p.drop_rp = (float)(256.0 / (256.0 - (double)t));
-  }
-  p.seed_lo = (uint32_t)(seed & 0xffffffffu);
-  p.seed_hi = (uint32_t)(seed >> 32);
+  const DropoutRule r = dropout_rule(dropout_p, seed);
+  p.drop_thresh = r.thresh;
+  p.drop_rp = r.scale;
+  p.seed_lo = r.seed_lo;
+  p.seed_hi = r.seed_hi;
 }
 
 // Workspace of the backward and of the dropout forward: the row-statistics blocks, an fp32 accumulator of acc_bytes
@@ -801,14 +769,16 @@ int launch_attn_fwd_dropout(const pcv_attn_params& a, const float* stat_m, const
   return launch_cast(bf16, p.o32, a.out, a.B, a.N, a.H, a.dv, a.o_stride_b, a.o_stride_n, a.o_stride_h, stream);
 }
 
-int launch_dropout_mask(uint8_t* keep, int B, int H, int N, int M, float dropout_p, uint64_t seed, cudaStream_t stream) {
-  PCV_REQUIRE(keep != nullptr && B > 0 && H > 0 && N > 0 && M > 0, PCV_ERR_INVALID, "dropout_mask: bad arguments");
+int launch_dropout_mask(uint8_t* keep, int B, int H, int N, int key_begin, int key_end, float dropout_p, uint64_t seed,
+                        cudaStream_t stream) {
+  PCV_REQUIRE(keep != nullptr && B > 0 && H > 0 && N > 0 && key_begin >= 0 && key_end > key_begin, PCV_ERR_INVALID,
+              "dropout_mask: bad arguments (B=%d H=%d N=%d keys [%d, %d))", B, H, N, key_begin, key_end);
   PCV_REQUIRE(dropout_p >= 0.f && dropout_p < 1.f, PCV_ERR_INVALID, "dropout_mask: dropout_p must be in [0, 1)");
-  BwdParams p{};
-  set_dropout(p, dropout_p, seed);
-  const int64_t total = (int64_t)B * H * N * M;
+  const DropoutRule r = dropout_rule(dropout_p, seed);
+  const int W = key_end - key_begin;
+  const int64_t total = (int64_t)B * H * N * W;
   const int blocks = (int)std::min<int64_t>((total + 255) / 256, 8192);
-  drop_mask_kernel<<<blocks, 256, 0, stream>>>(keep, B, H, N, M, p.drop_thresh, p.seed_lo, p.seed_hi);
+  drop_mask_kernel<<<blocks, 256, 0, stream>>>(keep, B, H, N, key_begin, W, r.thresh, r.seed_lo, r.seed_hi);
   PCV_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PCV_OK;

@@ -19,6 +19,7 @@
 // whole (b,h,query tile) write the final output; split ones write (numerator, max, denominator) slots that
 // tc_combine_kernel merges.  Semantics are those of include/pcv_attn.h (finite mask fill, uniform rows).
 #include "pcv_common.cuh"
+#include "pcv_dropout.cuh"
 #include "pcv_sm90.cuh"
 
 #include <cstdlib>
@@ -93,6 +94,7 @@ struct TcParams {
   int rows_per_unit;
   int slot_rows;
   PeerTail tail;
+  DropoutRule drop;  // attn_fwd_drop_kernel only; last, so that the other kernels' parameter offsets do not move
 };
 
 // --------------------------------------------------------------------------------------------------
@@ -277,8 +279,13 @@ struct FwdBarriers {
 // the log2 domain, apply the masks, update the running row maxima and denominators.  alpha is the factor by which the
 // running numerator has to be rescaled before this tile's P V is added.  `interior` (uniform over the warpgroup): no
 // key of the tile is masked for any row of the warpgroup, so the per-element checks and pad-word loads are skipped.
+// DROP: after the denominators took the tile's probabilities, the dropped elements of the numerator are zeroed (the
+// statistics stay those of the dropout-free softmax; the survivors are scaled once, in the epilogue).  `qside` is the
+// query side of the mask hash of rows n0 and n0 + 8; each thread hashes once per row and key pair (jb, jb + 1).
+template <bool DROP>
 __device__ __forceinline__ void tile_softmax(float (&s)[64], float (&m_run)[2], float (&l_run)[2], float (&alpha)[2],
-                                             const TcParams& p, int b, int j0, int n0, int cq, bool interior) {
+                                             const TcParams& p, int b, int j0, int n0, int cq, bool interior,
+                                             const uint32_t (&qside)[2]) {
   float mx[2] = {-INFINITY, -INFINITY};
   if (interior) {
 #pragma unroll
@@ -317,10 +324,19 @@ __device__ __forceinline__ void tile_softmax(float (&s)[64], float (&m_run)[2], 
   }
 #pragma unroll
   for (int g = 0; g < 16; ++g) {
-    const float e0 = ex2(s[4 * g + 0] - mref[0]), e1 = ex2(s[4 * g + 1] - mref[0]);
-    const float e2 = ex2(s[4 * g + 2] - mref[1]), e3 = ex2(s[4 * g + 3] - mref[1]);
+    float e0 = ex2(s[4 * g + 0] - mref[0]), e1 = ex2(s[4 * g + 1] - mref[0]);
+    float e2 = ex2(s[4 * g + 2] - mref[1]), e3 = ex2(s[4 * g + 3] - mref[1]);
     l_run[0] += e0 + e1;
     l_run[1] += e2 + e3;
+    if constexpr (DROP) {
+      const uint32_t jb = (uint32_t)(j0 + 8 * g + cq), n = (uint32_t)n0;
+      const uint32_t ks = drop_kside(p.drop.seed_hi, jb);
+      const uint32_t x0 = drop_finish(qside[0], ks), x1 = drop_finish(qside[1], ks);
+      if (!drop_keep(x0, n, jb, p.drop.thresh)) e0 = 0.f;
+      if (!drop_keep(x0, n, jb + 1, p.drop.thresh)) e1 = 0.f;
+      if (!drop_keep(x1, n + 8, jb, p.drop.thresh)) e2 = 0.f;
+      if (!drop_keep(x1, n + 8, jb + 1, p.drop.thresh)) e3 = 0.f;
+    }
     s[4 * g + 0] = e0;
     s[4 * g + 1] = e1;
     s[4 * g + 2] = e2;
@@ -346,10 +362,12 @@ __device__ __forceinline__ void rescale_o(float (&o)[NVB][32], const float (&alp
     for (int i = 0; i < 32; ++i) o[v][i] *= alpha[(i >> 1) & 1];
 }
 
-template <int NQB, int NVB, bool BF16, bool PAIR>
-__global__ void __launch_bounds__(kThreads, 1)
-attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
-                const __grid_constant__ CUtensorMap tv, const TcParams p) {
+// The body of attn_fwd_kernel (DROP = false) and of attn_fwd_drop_kernel (DROP = true: attention-probability dropout,
+// see tile_softmax; write_partial = 1 without key sharding, no CTA pair).
+template <int NQB, int NVB, bool BF16, bool PAIR, bool DROP>
+__device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
+                                              const TcParams& p) {
+  static_assert(!(DROP && PAIR), "no dropout in the CTA-pair kernel");
   using C = FwdCfg<NQB, NVB>;
   constexpr int NS = C::kSlots;
   // Head dims up to 128 (NQB <= 2) run the pipelined schedule: per tile one commit group for S = Q K^T and one for
@@ -494,6 +512,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
     float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
     const int n0 = sg.q0 + qoff + rloc;
     const int n_wg = sg.q0 + qoff + 64 * cw;  // first query row of this warpgroup
+    uint32_t qside[2] = {0u, 0u};
+    if constexpr (DROP) {
+      const uint32_t bh = (uint32_t)(sg.b * p.H + sg.h);
+#pragma unroll
+      for (int r = 0; r < 2; ++r) qside[r] = drop_qside(p.drop.seed_lo, drop_qword(bh, (uint32_t)(n0 + 8 * r)));
+    }
     // no key of the tile starting at j0 is masked for any row of this warpgroup
     auto interior = [&](int j0) {
       return p.pad_bits == nullptr && j0 + kTileN <= p.M && (!p.causal || j0 + kTileN - 1 <= n_wg + p.causal_shift);
@@ -512,7 +536,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
         fence_regs(s);
 #pragma unroll
         for (int c = 0; c < NQB; ++c) release(ik + c);
-        tile_softmax(s, m_run, l_run, alpha, p, sg.b, sg.t0 * kTileN, n0, cq, interior(sg.t0 * kTileN));
+        tile_softmax<DROP>(s, m_run, l_run, alpha, p, sg.b, sg.t0 * kTileN, n0, cq, interior(sg.t0 * kTileN), qside);
         pack_p<BF16>(s, pa);
         for (int t = sg.t0 + 1; t < sg.t1; ++t) {
           const uint32_t iv = ik + NQB;  // V boxes of tile t - 1
@@ -525,7 +549,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
           fence_regs(s);
 #pragma unroll
           for (int c = 0; c < NQB; ++c) release(ik + c);
-          tile_softmax(s, m_run, l_run, alpha, p, sg.b, t * kTileN, n0, cq, interior(t * kTileN));
+          tile_softmax<DROP>(s, m_run, l_run, alpha, p, sg.b, t * kTileN, n0, cq, interior(t * kTileN), qside);
           wgmma_wait<0>();
 #pragma unroll
           for (int v = 0; v < NVB; ++v) {
@@ -565,7 +589,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
           release(it);
         }
         float alpha[2];
-        tile_softmax(s, m_run, l_run, alpha, p, sg.b, t * kTileN, n0, cq, interior(t * kTileN));
+        tile_softmax<DROP>(s, m_run, l_run, alpha, p, sg.b, t * kTileN, n0, cq, interior(t * kTileN), qside);
         rescale_o(o, alpha);
         uint32_t pa[8][4];
         pack_p<BF16>(s, pa);
@@ -591,6 +615,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
     for (int r = 0; r < 2; ++r) {
       l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
       l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
+    }
+    if constexpr (DROP) {  // the survivors' scale, once for every store below (tc_combine_kernel is linear in o)
+#pragma unroll
+      for (int v = 0; v < NVB; ++v)
+#pragma unroll
+        for (int i = 0; i < 32; ++i) o[v][i] *= p.drop.scale;
     }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -639,6 +669,22 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
     }
     if (PAIR && si + 1 == seg_hi) cluster_sync_all();
   }
+}
+
+template <int NQB, int NVB, bool BF16, bool PAIR>
+__global__ void __launch_bounds__(kThreads, 1)
+attn_fwd_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
+                const __grid_constant__ CUtensorMap tv, const TcParams p) {
+  attn_fwd_body<NQB, NVB, BF16, PAIR, false>(tq, tk, tv, p);
+}
+
+// One-pass forward with attention-probability dropout (pcv_attn_fwd_partial_dropout): a separate kernel, so that the
+// inference kernel's code is unchanged.
+template <int NQB, int NVB, bool BF16>
+__global__ void __launch_bounds__(kThreads, 1)
+attn_fwd_drop_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
+                     const __grid_constant__ CUtensorMap tv, const TcParams p) {
+  attn_fwd_body<NQB, NVB, BF16, false, true>(tq, tk, tv, p);
 }
 
 // --------------------------------------------------------------------------------------------------
@@ -881,13 +927,18 @@ Mode choose_mode(const pcv_attn_params& a) {
 
 int dv_pass_width(int dv) { return std::min(kMaxDvPass, pad64(dv)); }
 
-template <int NQB, int NVB, bool BF16, bool PAIR>
+template <int NQB, int NVB, bool BF16, bool PAIR, bool DROP>
 int launch_fwd(const Plan& pl, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const TcParams& p,
                cudaStream_t stream) {
   prof_mark_begin(stream);
   // num_ctas counts CTA pairs in the pair mode
-  const int rc = launch_kernel(attn_fwd_kernel<NQB, NVB, BF16, PAIR>, dim3(PAIR ? 2 * pl.num_ctas : pl.num_ctas), kThreads,
-                               FwdCfg<NQB, NVB>::kSmemBytes, PAIR ? 2 : 0, stream, tq, tk, tv, p);
+  int rc;
+  if constexpr (DROP)
+    rc = launch_kernel(attn_fwd_drop_kernel<NQB, NVB, BF16>, dim3(pl.num_ctas), kThreads, FwdCfg<NQB, NVB>::kSmemBytes, 0,
+                       stream, tq, tk, tv, p);
+  else
+    rc = launch_kernel(attn_fwd_kernel<NQB, NVB, BF16, PAIR>, dim3(PAIR ? 2 * pl.num_ctas : pl.num_ctas), kThreads,
+                       FwdCfg<NQB, NVB>::kSmemBytes, PAIR ? 2 : 0, stream, tq, tk, tv, p);
   prof_mark_end(stream);
   if (rc != PCV_OK) return rc;
   if (pl.num_units > 0) {
@@ -902,30 +953,30 @@ int launch_fwd(const Plan& pl, const CUtensorMap& tq, const CUtensorMap& tk, con
   return PCV_OK;
 }
 
-template <int NQB, bool BF16>
+template <int NQB, bool BF16, bool DROP>
 int launch_nqb(int nvb, bool pair, const Plan& pl, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
                const TcParams& p, cudaStream_t stream) {
-  if constexpr (NQB <= 2) {
+  if constexpr (NQB <= 2 && !DROP) {
     if (pair)
-      return nvb == 1 ? launch_fwd<NQB, 1, BF16, true>(pl, tq, tk, tv, p, stream)
-                      : launch_fwd<NQB, 2, BF16, true>(pl, tq, tk, tv, p, stream);
+      return nvb == 1 ? launch_fwd<NQB, 1, BF16, true, false>(pl, tq, tk, tv, p, stream)
+                      : launch_fwd<NQB, 2, BF16, true, false>(pl, tq, tk, tv, p, stream);
   }
-  return nvb == 1 ? launch_fwd<NQB, 1, BF16, false>(pl, tq, tk, tv, p, stream)
-                  : launch_fwd<NQB, 2, BF16, false>(pl, tq, tk, tv, p, stream);
+  return nvb == 1 ? launch_fwd<NQB, 1, BF16, false, DROP>(pl, tq, tk, tv, p, stream)
+                  : launch_fwd<NQB, 2, BF16, false, DROP>(pl, tq, tk, tv, p, stream);
 }
 
-template <bool BF16>
+template <bool BF16, bool DROP>
 int launch_dispatch(int nqb, int nvb, bool pair, const Plan& pl, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
                     const TcParams& p, cudaStream_t stream) {
   switch (nqb) {
-    case 1: return launch_nqb<1, BF16>(nvb, pair, pl, tq, tk, tv, p, stream);
-    case 2: return launch_nqb<2, BF16>(nvb, pair, pl, tq, tk, tv, p, stream);
-    case 3: return launch_nqb<3, BF16>(nvb, pair, pl, tq, tk, tv, p, stream);
-    case 4: return launch_nqb<4, BF16>(nvb, pair, pl, tq, tk, tv, p, stream);
-    case 5: return launch_nqb<5, BF16>(nvb, pair, pl, tq, tk, tv, p, stream);
-    case 6: return launch_nqb<6, BF16>(nvb, pair, pl, tq, tk, tv, p, stream);
-    case 7: return launch_nqb<7, BF16>(nvb, pair, pl, tq, tk, tv, p, stream);
-    case 8: return launch_nqb<8, BF16>(nvb, pair, pl, tq, tk, tv, p, stream);
+    case 1: return launch_nqb<1, BF16, DROP>(nvb, pair, pl, tq, tk, tv, p, stream);
+    case 2: return launch_nqb<2, BF16, DROP>(nvb, pair, pl, tq, tk, tv, p, stream);
+    case 3: return launch_nqb<3, BF16, DROP>(nvb, pair, pl, tq, tk, tv, p, stream);
+    case 4: return launch_nqb<4, BF16, DROP>(nvb, pair, pl, tq, tk, tv, p, stream);
+    case 5: return launch_nqb<5, BF16, DROP>(nvb, pair, pl, tq, tk, tv, p, stream);
+    case 6: return launch_nqb<6, BF16, DROP>(nvb, pair, pl, tq, tk, tv, p, stream);
+    case 7: return launch_nqb<7, BF16, DROP>(nvb, pair, pl, tq, tk, tv, p, stream);
+    case 8: return launch_nqb<8, BF16, DROP>(nvb, pair, pl, tq, tk, tv, p, stream);
   }
   set_error("tensor-core attention: qk head dim needs %d 64-channel boxes (at most 8)", nqb);
   return PCV_ERR_UNSUPPORTED;
@@ -998,11 +1049,14 @@ bool attn_tc_fuse_supported(const pcv_attn_params& a, const char** why) {
   return true;
 }
 
-int launch_attn_tc(const pcv_attn_params& a, cudaStream_t stream, const pcv_shard_fuse* fuse) {
+int launch_attn_tc(const pcv_attn_params& a, cudaStream_t stream, const pcv_shard_fuse* fuse, const DropoutRule* drop) {
   {
     const char* why = "";
     PCV_REQUIRE(attn_tc_supported(a, &why), PCV_ERR_UNSUPPORTED, "tensor-core attention: %s", why);
   }
+  PCV_REQUIRE(drop == nullptr || (fuse == nullptr && a.write_partial && a.impl != PCV_IMPL_TCGEN05_PAIR &&
+                                  a.m_total == a.M && a.m_offset == 0 && drop->thresh > 0),
+              PCV_ERR_UNSUPPORTED, "tensor-core attention: dropout needs a partial-state call over all keys, no CTA pair");
   std::shared_ptr<Plan> pl;
   const Mode mode = choose_mode(a);
   if (mode.pair) {
@@ -1037,6 +1091,7 @@ int launch_attn_tc(const pcv_attn_params& a, cudaStream_t stream, const pcv_shar
   p.rows_per_unit = mode.rows_per_unit;
   p.slot_rows = mode.slot_rows;
   p.fin_o = a.part_o; p.fin_m = a.part_m; p.fin_l = a.part_l;
+  if (drop != nullptr) p.drop = *drop;
   if (fuse != nullptr) {
     const char* why = "";
     PCV_REQUIRE(attn_tc_fuse_supported(a, &why), PCV_ERR_UNSUPPORTED, "fused merge: %s", why);
@@ -1095,8 +1150,12 @@ int launch_attn_tc(const pcv_attn_params& a, cudaStream_t stream, const pcv_shar
     const char* vbase = reinterpret_cast<const char*>(a.v) + 2 * (size_t)off;
     rc = make_tmap_4d(&tv, vbase, a.dtype, p.dv_pass, a.M, a.H, a.B, a.v_stride_m, a.v_stride_h, a.v_stride_b, kv_box_rows);
     if (rc != PCV_OK) return rc;
-    rc = bf ? launch_dispatch<true>(nqb, nvb, mode.pair, *pl, tq, tk, tv, p, stream)
-            : launch_dispatch<false>(nqb, nvb, mode.pair, *pl, tq, tk, tv, p, stream);
+    if (drop != nullptr)
+      rc = bf ? launch_dispatch<true, true>(nqb, nvb, false, *pl, tq, tk, tv, p, stream)
+              : launch_dispatch<false, true>(nqb, nvb, false, *pl, tq, tk, tv, p, stream);
+    else
+      rc = bf ? launch_dispatch<true, false>(nqb, nvb, mode.pair, *pl, tq, tk, tv, p, stream)
+              : launch_dispatch<false, false>(nqb, nvb, mode.pair, *pl, tq, tk, tv, p, stream);
     if (rc != PCV_OK) return rc;
   }
   if (p.tail.enabled) {

@@ -80,8 +80,11 @@ int launch_pack_pad(const uint8_t* pad, int64_t stride_b, int B, int M, uint32_t
 int launch_attn_simt(const pcv_attn_params& p, cudaStream_t stream);
 int attn_simt_workspace_bytes(const pcv_attn_params& p, size_t* bytes);
 
+struct DropoutRule;  // pcv_dropout.cuh
 bool attn_tc_supported(const pcv_attn_params& p, const char** why);
-int launch_attn_tc(const pcv_attn_params& p, cudaStream_t stream, const pcv_shard_fuse* fuse = nullptr);
+// drop != nullptr: the one-pass dropout forward (attn_fwd_drop_kernel; partial state over all keys, no fuse, no pair)
+int launch_attn_tc(const pcv_attn_params& p, cudaStream_t stream, const pcv_shard_fuse* fuse = nullptr,
+                   const DropoutRule* drop = nullptr);
 bool attn_tc_fuse_supported(const pcv_attn_params& p, const char** why);
 int attn_tc_workspace_bytes(const pcv_attn_params& p, size_t* bytes);
 int debug_read(uint32_t* out, int n);  // the watchdog record of the wgmma kernels (16 words)
@@ -112,6 +115,7 @@ bool attn_fwd_dropout_supported(const pcv_attn_params& p, float dropout_p, const
 int attn_fwd_dropout_workspace_bytes(const pcv_attn_params& p, size_t* bytes);
 int launch_attn_fwd_dropout(const pcv_attn_params& p, const float* stat_m, const float* stat_l, float dropout_p,
                             uint64_t seed, cudaStream_t stream);
-int launch_dropout_mask(uint8_t* keep, int B, int H, int N, int M, float dropout_p, uint64_t seed, cudaStream_t stream);
+int launch_dropout_mask(uint8_t* keep, int B, int H, int N, int key_begin, int key_end, float dropout_p, uint64_t seed,
+                        cudaStream_t stream);
 
 }  // namespace pcv

@@ -64,7 +64,8 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
 // Blocks until the phase with the given parity has completed.  A fresh barrier passes parity 1.
 // Sites (word 1 of the record), unique in the library:
 //    1- 7  attn_fwd_kernel     1 Q slot free, 2 ring slot free, 3 Q loaded, 4 K box loaded, 5 V box loaded (serial
-//                              schedule); 6 K box loaded, 7 V box loaded (pipelined schedule)
+//          and                 schedule); 6 K box loaded, 7 V box loaded (pipelined schedule).  The two kernels share
+//          attn_fwd_drop_kernel  one body (attn_fwd_body), so these sites cover both.
 //   11-12  kvproj_kernel      11 ring slot free, 12 stage loaded
 //   21-24  bwd_dkdv_kernel    21 K/V tile free, 22 Q/dO slot free, 23 K/V tile loaded, 24 Q/dO stage loaded
 //   31-33  bwd_dq_kernel      31 K/V slot free, 32 Q (and dO) loaded, 33 K/V stage loaded

@@ -13,6 +13,8 @@ evaluated on the same bf16-rounded operands.
 from __future__ import annotations
 
 import ctypes as C
+import math
+import struct
 from typing import Optional, Tuple
 
 import torch
@@ -273,32 +275,87 @@ def attention_dropout_forward(q, k, v, stat_m, stat_l, num_heads: int, scale: fl
     return out if out.dtype == out_dtype else out.to(out_dtype)
 
 
-def dropout_keep_mask(B: int, H: int, N: int, M: int, dropout_p: float, dropout_seed: int, device="cuda") -> torch.Tensor:
-    """(B, H, N, M) bool keep mask the dropout kernels use for this seed (tests / debugging)."""
-    keep = torch.empty(B, H, N, M, dtype=torch.uint8, device=device)
+def dropout_keep_mask(B: int, H: int, N: int, M: int, dropout_p: float, dropout_seed: int, device="cuda",
+                      key_begin: int = 0, key_end: Optional[int] = None) -> torch.Tensor:
+    """(B, H, N, key_end - key_begin) bool keep mask the dropout kernels use for this seed over the keys
+    [key_begin, key_end) (default: all M keys) — pcv_attn_dropout_mask_range."""
+    key_end = M if key_end is None else int(key_end)
+    keep = torch.empty(B, H, N, max(key_end - key_begin, 0), dtype=torch.uint8, device=device)
     with torch.cuda.device(keep.device):
-        check(_lib.lib().pcv_attn_dropout_mask(keep.data_ptr(), B, H, N, M, float(dropout_p), int(dropout_seed),
-                                               _stream()), "pcv_attn_dropout_mask")
+        check(_lib.lib().pcv_attn_dropout_mask_range(keep.data_ptr(), B, H, N, int(key_begin), key_end, float(dropout_p),
+                                                     int(dropout_seed), _stream()), "pcv_attn_dropout_mask_range")
     return keep.bool()
 
 
+def _dropout_keep(B: int, H: int, N: int, key_begin: int, key_end: int, dropout_p: float, dropout_seed: int,
+                  device) -> torch.Tensor:
+    """The backward shim's view of the dropout mask: keys [key_begin, key_end) as a (B, H, N, key_end - key_begin) bool
+    tensor on `device`.  The one place the shim fetches the mask (a CPU test substitutes the numpy oracle here)."""
+    if torch.device(device).type != "cuda":
+        raise RuntimeError(f"attention dropout: the mask is generated on the GPU, got tensors on {device}")
+    return dropout_keep_mask(B, H, N, key_end, dropout_p, dropout_seed, device=device, key_begin=key_begin,
+                             key_end=key_end)
+
+
+def _dropout_scale(dropout_p: float) -> float:
+    """The survivors' scale 256 / (256 - thresh) of the kernels, thresh = clamp(lround(256 p), 1, 255) of the float32 p."""
+    p32 = struct.unpack("f", struct.pack("f", float(dropout_p)))[0]
+    return 256.0 / (256.0 - min(255, max(1, int(math.floor(p32 * 256.0 + 0.5)))))
+
+
+def _partial_dropout_supported(q, k, v, num_heads: int, pad_mask, causal: bool, dropout_p: float, impl: str) -> bool:
+    """Whether the one-pass dropout forward (attention_partial with dropout_p > 0) takes these operands, head dims
+    padded to multiples of 8 as the forward pads them."""
+    q, k, v, _ = _prep(q, k, v)
+    if _head_dim(q, num_heads) % 8 or _head_dim(v, num_heads) % 8:
+        q, k, v = _pad_heads_to8(q, num_heads), _pad_heads_to8(k, num_heads), _pad_heads_to8(v, num_heads)
+    with torch.cuda.device(k.device):
+        p, keep = _fill_attn_params(q, k, v, num_heads, 1.0, pad_mask, causal, None, 0, impl)
+        dummy = torch.empty(16, device=k.device)
+        p.write_partial = 1
+        p.part_o = p.part_m = p.part_l = dummy.data_ptr()
+        ok = bool(_lib.lib().pcv_attn_fwd_partial_dropout_supported(C.byref(p), float(dropout_p)))
+    del keep
+    return ok
+
+
 class _FusedAttention(torch.autograd.Function):
-    """Forward = the fused CUDA kernel (partial-state mode, so the row max and denominator are kept).
+    """Forward = the fused CUDA kernel (partial-state mode, so the row max and denominator are kept).  With dropout:
+    the partial forward and the second-pass dropout kernel (``attention_dropout_forward``) where that covers the call
+    (head dims that are multiples of 8 up to 128), else the one-pass dropout forward (``attention_partial`` with
+    ``dropout_p``) for every head dim the forward takes.
     Backward = the tensor-core backward kernels (``attention_backward`` -> pcv_attn_bwd: dK/dV and dQ kernels, SURVEY.md
     §8(f) rank 2) for head dims that are multiples of 8 up to 128.  Other shapes take the labelled SHIM below: the
     flash-attention backward recurrence in plain torch ops, chunked over the key axis from the saved statistics,
-    memory bounded by ``backward_config["max_score_bytes"]``; neither path ever holds the (B, H, N, M) score tensor
-    (8.6 GB at the north-star shape).  The inference forward never routes through this class."""
+    memory bounded by ``backward_config["max_score_bytes"]``, with dropout regenerating the mask of each key chunk
+    (``_dropout_keep``); neither path ever holds the (B, H, N, M) score tensor (8.6 GB at the north-star shape).
+    The inference forward never routes through this class."""
 
     @staticmethod
     def forward(ctx, q, k, v, num_heads, scale, pad_mask, causal, impl, dropout_p=0.0, dropout_seed=0):
         dv_true = _head_dim(v, num_heads)
         ctx.dropout = (float(dropout_p), int(dropout_seed))
         if dropout_p > 0.0:
-            # statistics from the fused kernel, then the dropout pass (second kernel) writes the output
-            po, pm, pl = attention_partial(q, k, v, num_heads, scale, pad_mask=pad_mask, causal=causal, impl=impl)
-            del po
-            out = attention_dropout_forward(q, k, v, pm, pl, num_heads, scale, dropout_p, dropout_seed, pad_mask, causal)
+            if attention_dropout_forward(q, k, v, None, None, num_heads, scale, dropout_p, dropout_seed, pad_mask, causal,
+                                         check_only=True):
+                # statistics from the fused kernel, then the dropout pass (second kernel) writes the output
+                po, pm, pl = attention_partial(q, k, v, num_heads, scale, pad_mask=pad_mask, causal=causal, impl=impl)
+                del po
+                out = attention_dropout_forward(q, k, v, pm, pl, num_heads, scale, dropout_p, dropout_seed, pad_mask,
+                                                causal)
+            else:
+                # one pass: the dropped numerator and the dropout-free statistics; zero channels padding the head dims
+                # to multiples of 8 change neither the scores nor the mask
+                qp, kp, vp = q, k, v
+                if _head_dim(q, num_heads) % 8 or dv_true % 8:
+                    qp, kp, vp = (_pad_heads_to8(t, num_heads) for t in (q, k, v))
+                po, pm, pl = attention_partial(qp, kp, vp, num_heads, scale, pad_mask=pad_mask, causal=causal, impl=impl,
+                                               dropout_p=dropout_p, dropout_seed=dropout_seed)
+                out = combine_partials(po[None], pm[None], pl[None], _compute_dtype(q.dtype))
+                B, N, H, dv_pad = po.shape[0], po.shape[2], po.shape[1], po.shape[3]
+                del po
+                if dv_pad != dv_true:
+                    out = out.view(B, N, H, dv_pad)[..., :dv_true].reshape(B, N, H * dv_true)
             out = out if out.dtype == q.dtype else out.to(q.dtype)
             ctx.save_for_backward(q, k, v, pad_mask, out, pm, pl)
             ctx.meta = (num_heads, scale, causal)
@@ -334,9 +391,6 @@ class _FusedAttention(torch.autograd.Function):
             if mode == "kernel":
                 raise RuntimeError("backward_config['impl'] = 'kernel' but pcv_attn_bwd does not cover this call: "
                                    + _lib.lib().pcv_last_error().decode())
-        if drop_p > 0.0:
-            raise RuntimeError("attention dropout needs the backward kernels (pcv_attn_bwd); the torch shim cannot "
-                               "regenerate the mask: " + _lib.lib().pcv_last_error().decode())
         B, M = k.shape[0], k.shape[1]
         N = q.shape[1]
         cdt = _compute_dtype(q.dtype)
@@ -381,8 +435,14 @@ class _FusedAttention(torch.autograd.Function):
             j1 = min(M, j0 + chunk)
             t, filled = scores(j0, j1)
             p = torch.exp2(t - pm[..., None]) * inv_l[..., None]                             # (B,H,N,c) probabilities
-            gv[:, :, j0:j1] = torch.matmul(p.transpose(-1, -2), go)
-            ds = p * (torch.matmul(go, vh[:, :, j0:j1].transpose(-1, -2)) - delta[..., None])
+            dp = torch.matmul(go, vh[:, :, j0:j1].transpose(-1, -2))
+            if drop_p > 0.0:  # O = (P o K r) V:  dV = (P o K r)^T dO,  dP = (dO V^T) o K r
+                kr = _dropout_keep(B, H, N, j0, j1, drop_p, drop_seed, k.device).to(p.dtype) * _dropout_scale(drop_p)
+                gv[:, :, j0:j1] = torch.matmul((p * kr).transpose(-1, -2), go)
+                dp = dp * kr
+            else:
+                gv[:, :, j0:j1] = torch.matmul(p.transpose(-1, -2), go)
+            ds = p * (dp - delta[..., None])
             if filled is not None:
                 ds = ds.masked_fill(filled, 0.0)  # a filled score is a constant (masked_fill_): no gradient through it
             gq += torch.matmul(ds, kh[:, :, j0:j1])
@@ -405,13 +465,15 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, num_heads: int,
     (/root/reference/perceiver/model/core/modules.py): q is scaled by ``scale``, ``pad_mask`` (True =
     padding) and the right-aligned causal mask use the finite fill ``-finfo.max``.  ``dropout_p`` > 0 applies the
     reference's dropout on the attention probabilities (:161) with a counter-based mask derived from
-    ``dropout_seed`` (default: a fresh seed from torch's CPU generator); head dims must be multiples of 8 up to 128.
+    ``dropout_seed`` (default: a fresh seed from torch's CPU generator), for every head dim the forward takes (up to
+    512; above 128 the backward runs on the torch shim).
     """
     if dropout_p > 0.0:
         if not 0.0 < dropout_p < 1.0:
             raise ValueError(f"dropout_p must be in [0, 1), got {dropout_p}")
-        if not attention_dropout_forward(q, k, v, None, None, num_heads, scale, dropout_p, 0, pad_mask, causal,
-                                         check_only=True):
+        if not (attention_dropout_forward(q, k, v, None, None, num_heads, scale, dropout_p, 0, pad_mask, causal,
+                                          check_only=True)
+                or _partial_dropout_supported(q, k, v, num_heads, pad_mask, causal, dropout_p, impl)):
             raise NotImplementedError("attention dropout is not available for this call: "
                                       + _lib.lib().pcv_last_error().decode())
         seed = new_dropout_seed() if dropout_seed is None else int(dropout_seed)
@@ -422,11 +484,14 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, num_heads: int,
 
 
 def attention_partial(q, k, v, num_heads: int, scale: float, pad_mask=None, causal: bool = False,
-                      m_total: Optional[int] = None, m_offset: int = 0, impl: str = "auto", out=None):
+                      m_total: Optional[int] = None, m_offset: int = 0, impl: str = "auto", out=None,
+                      dropout_p: float = 0.0, dropout_seed: int = 0):
     """One M-shard's un-normalised softmax state: (part_o (B,H,N,dv) f32, part_m (B,H,N), part_l (B,H,N)).
 
     ``k``/``v``/``pad_mask`` hold this shard's keys [m_offset, m_offset+M) of ``m_total``.  ``out`` may
-    supply the three (contiguous, float32) destination tensors."""
+    supply the three (contiguous, float32) destination tensors.  ``dropout_p`` > 0 (all keys, no sharding): the
+    one-pass dropout forward (pcv_attn_fwd_partial_dropout) — part_o is the numerator with the mask of
+    ``dropout_keep_mask`` applied and scaled by 1/(1-p), part_m / part_l stay the dropout-free statistics."""
     q, k, v, _ = _prep(q, k, v)
     with torch.cuda.device(k.device):
         p, keep = _fill_attn_params(q, k, v, num_heads, scale, pad_mask, causal, m_total, m_offset, impl)
@@ -444,7 +509,17 @@ def attention_partial(q, k, v, num_heads: int, scale: float, pad_mask=None, caus
             part_l = torch.empty(p.B, p.H, p.N, dtype=torch.float32, device=k.device)
         p.write_partial = 1
         p.part_o, p.part_m, p.part_l = part_o.data_ptr(), part_m.data_ptr(), part_l.data_ptr()
-        _run_attn(p, k.device)
+        if dropout_p > 0.0:
+            if p.impl == _lib.PCV_IMPL_AUTO:  # the dropout forward runs on the tensor-core kernel: size its workspace
+                p.impl = _lib.PCV_IMPL_TCGEN05
+            need = C.c_size_t(0)
+            check(_lib.lib().pcv_attn_workspace_bytes(C.byref(p), C.byref(need)), "pcv_attn_workspace_bytes")
+            ws = torch.empty(max(need.value, 256), dtype=torch.uint8, device=k.device)
+            p.workspace, p.workspace_bytes = ws.data_ptr(), need.value
+            check(_lib.lib().pcv_attn_fwd_partial_dropout(C.byref(p), float(dropout_p), int(dropout_seed), _stream()),
+                  "pcv_attn_fwd_partial_dropout")
+        else:
+            _run_attn(p, k.device)
     del keep
     return part_o, part_m, part_l
 
