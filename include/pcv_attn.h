@@ -307,7 +307,9 @@ typedef struct pcv_shard_fuse {
  * with the masks of the forward (finite fill: a filled score carries no gradient).  Tensors are laid out as in
  * pcv_attn_params ((B, rows, H, d) by strides, in `dtype`); q_stride_b == 0 broadcasts one latent array over the batch and
  * grad_q is then the SUM over the batch, shape (1, N, H*dqk).  Two tcgen05 kernels (dK/dV: key-tile outer; dQ: query-tile
- * outer) — no (B, H, N, M) tensor is ever materialised.  Head dims: multiples of 8, at most 128.
+ * outer) — no (B, H, N, M) tensor is ever materialised.  Head dims: multiples of 8, at most 192.  Above 128 grad_q is
+ * summed from per-(batch contribution, key split) fp32 partials in a fixed order (bitwise reproducible); the workspace
+ * then holds those partials.
  */
 typedef struct pcv_attn_bwd_params {
   const void* q;

@@ -19,6 +19,9 @@
 //                    fp32 buffer once per CTA.  With FWD it is the second forward pass of a training step with dropout:
 //                    O += dropout(P) V from the saved statistics (no running maximum).
 //
+// Head dims above 128 (up to 192: a third 64-channel box) run the dK/dV kernel as a dV pass and a dK pass and the dQ
+// kernel as bwd_dq64_kernel (64-key stages, ordered fp32 partials instead of atomics); see there.
+//
 // Warpgroup 0 is the TMA producer (one lane), warpgroups 1 and 2 each own 64 rows of the tile.
 #include "pcv_common.cuh"
 #include "pcv_dropout.cuh"
@@ -174,12 +177,20 @@ __device__ __forceinline__ bool filled_key(const BwdParams& p, int b, int j, int
   return p.causal && j > n + p.cshift;
 }
 
-template <int NQB, int NVB, bool BF16>
+// Outputs of one bwd_dkdv_kernel launch.  With a head dim above 128 (a third 64-channel box) the dK and dV accumulators
+// do not fit the consumer registers beside S^T, dP^T and the packed operands without spilling (ptxas spills already at
+// (1, 3) and (3, 1)), so the backward runs the kernel twice: a dV pass (K resident, no dP^T GEMM, no dS) and a dK pass
+// (K and V resident).  Each pass computes S^T = K Q^T: one extra GEMM of dqk channels per (key, query) pair.
+enum DkdvOut : int { kOutBoth = 0, kOutDV = 1, kOutDK = 2 };
+
+template <int NQB, int NVB, bool BF16, int OUT = kOutBoth>
 __global__ void __launch_bounds__(kThreads, 1)
 bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq64, const __grid_constant__ CUtensorMap tk,
                 const __grid_constant__ CUtensorMap tv, const __grid_constant__ CUtensorMap tdo64, const BwdParams p) {
   using C = Cfg1<NQB, NVB>;
   constexpr int NS = C::kSlots;
+  constexpr bool kDK = OUT != kOutDV, kDV = OUT != kOutDK;
+  constexpr int kResident = kDK ? C::kKVBytes : NQB * kBoxBytes;  // the dV pass leaves V's boxes empty
   using T = typename std::conditional<BF16, __nv_bfloat16, __half>::type;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -207,9 +218,10 @@ bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq64, const __grid_constant_
       for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++tl) {
         const int bh = tile / p.nk, kt = tile % p.nk, b = bh / p.H, h = bh % p.H;
         mbar_wait(&bar.fix_empty, (tl & 1) ^ 1, 21);
-        mbar_arrive_expect_tx(&bar.fix_full, C::kKVBytes);
+        mbar_arrive_expect_tx(&bar.fix_full, kResident);
         for (int c = 0; c < NQB; ++c) tma_load_4d(sK + c * kBoxBytes, &tk, &bar.fix_full, c * 64, kt * kT, h, b);
-        for (int c = 0; c < NVB; ++c) tma_load_4d(sV + c * kBoxBytes, &tv, &bar.fix_full, c * 64, kt * kT, h, b);
+        if constexpr (kDK)
+          for (int c = 0; c < NVB; ++c) tma_load_4d(sV + c * kBoxBytes, &tv, &bar.fix_full, c * 64, kt * kT, h, b);
         for (int qs = 0; qs < nq64; ++qs, ++it) {
           const uint32_t s = it % NS;
           mbar_wait(&bar.empty[s], ((it / NS) & 1) ^ 1, 22);
@@ -237,13 +249,14 @@ bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq64, const __grid_constant_
   for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++tl) {
     const int bh = tile / p.nk, kt = tile % p.nk, b = bh / p.H, h = bh % p.H;
     mbar_wait(&bar.fix_full, tl & 1, 23);
-    float dk[NQB][32], dv[NVB][32];
+    constexpr int NK = kDK ? NQB : 0, NV = kDV ? NVB : 0;  // accumulator boxes of this launch
+    float dk[kDK ? NQB : 1][32], dv[kDV ? NVB : 1][32];
 #pragma unroll
-    for (int c = 0; c < NQB; ++c)
+    for (int c = 0; c < NK; ++c)
 #pragma unroll
       for (int i = 0; i < 32; ++i) dk[c][i] = 0.f;
 #pragma unroll
-    for (int c = 0; c < NVB; ++c)
+    for (int c = 0; c < NV; ++c)
 #pragma unroll
       for (int i = 0; i < 32; ++i) dv[c][i] = 0.f;
     const int jrow[2] = {kt * kT + kloc, kt * kT + kloc + 8};
@@ -251,24 +264,26 @@ bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq64, const __grid_constant_
       const uint32_t s = it % NS;
       const uint32_t stq = ring + s * C::kStage, stdo = stq + NQB * kBox64;
       mbar_wait(&bar.full[s], (it / NS) & 1, 24);
-      float st[32], dpt[32];
+      float st[32], dpt[kDK ? 32 : 1];
       wgmma_fence();
 #pragma unroll
       for (int c = 0; c < NQB; ++c)
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk)
           wgmma_ss<64, BF16>(st, make_desc(k_base + c * kBoxBytes + kk * 32), make_desc(stq + c * kBox64 + kk * 32), (c | kk) != 0);
+      if constexpr (kDK) {
 #pragma unroll
-      for (int c = 0; c < NVB; ++c)
+        for (int c = 0; c < NVB; ++c)
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk)
-          wgmma_ss<64, BF16>(dpt, make_desc(v_base + c * kBoxBytes + kk * 32), make_desc(stdo + c * kBox64 + kk * 32), (c | kk) != 0);
+          for (int kk = 0; kk < 4; ++kk)
+            wgmma_ss<64, BF16>(dpt, make_desc(v_base + c * kBoxBytes + kk * 32), make_desc(stdo + c * kBox64 + kk * 32), (c | kk) != 0);
+      }
       wgmma_commit();
       wgmma_wait<0>();
       fence_regs(st);
-      fence_regs(dpt);
+      if constexpr (kDK) fence_regs(dpt);
       const float* blk = p.stats + ((int64_t)bh * (p.Npad / 64) + qs) * (kStatsBytes / 4);
-      uint32_t pa[4][4], da[4][4];
+      uint32_t pa[kDV ? 4 : 1][4], da[kDK ? 4 : 1][4];
 #pragma unroll
       for (int g = 0; g < 8; ++g) {
         float pv[4], dsv[4];
@@ -281,36 +296,54 @@ bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq64, const __grid_constant_
           const bool oob = j >= p.M || n >= p.N;
           const bool filled = !oob && filled_key(p, b, j, n);
           float P = oob ? 0.f : (filled ? fillp : ex2(fmaf(st[4 * g + e4], p.scale_log2, nlse)));
-          float dP = dpt[4 * g + e4];
-          if (p.drop_thresh) {
-            const bool keep = drop_keep(drop_bits(p.seed_lo, p.seed_hi, (uint32_t)bh, (uint32_t)n, (uint32_t)j), n, j, p.drop_thresh);
-            dP = keep ? dP * p.drop_rp : 0.f;
-            pv[e4] = keep ? P * p.drop_rp : 0.f;
+          if constexpr (kDK) {
+            float dP = dpt[4 * g + e4];
+            if (p.drop_thresh) {
+              const bool keep = drop_keep(drop_bits(p.seed_lo, p.seed_hi, (uint32_t)bh, (uint32_t)n, (uint32_t)j), n, j, p.drop_thresh);
+              dP = keep ? dP * p.drop_rp : 0.f;
+              pv[e4] = keep ? P * p.drop_rp : 0.f;
+            } else {
+              pv[e4] = P;
+            }
+            dsv[e4] = (oob || filled) ? 0.f : P * (dP - delta);
           } else {
-            pv[e4] = P;
+            (void)delta;  // the dV pass needs no dS
+            if (p.drop_thresh) {
+              const bool keep = drop_keep(drop_bits(p.seed_lo, p.seed_hi, (uint32_t)bh, (uint32_t)n, (uint32_t)j), n, j, p.drop_thresh);
+              pv[e4] = keep ? P * p.drop_rp : 0.f;
+            } else {
+              pv[e4] = P;
+            }
           }
-          dsv[e4] = (oob || filled) ? 0.f : P * (dP - delta);
         }
-        pa[g >> 1][(g & 1) * 2 + 0] = pack2(pv[0], pv[1], BF16);
-        pa[g >> 1][(g & 1) * 2 + 1] = pack2(pv[2], pv[3], BF16);
-        da[g >> 1][(g & 1) * 2 + 0] = pack2(dsv[0], dsv[1], BF16);
-        da[g >> 1][(g & 1) * 2 + 1] = pack2(dsv[2], dsv[3], BF16);
+        if constexpr (kDV) {
+          pa[g >> 1][(g & 1) * 2 + 0] = pack2(pv[0], pv[1], BF16);
+          pa[g >> 1][(g & 1) * 2 + 1] = pack2(pv[2], pv[3], BF16);
+        }
+        if constexpr (kDK) {
+          da[g >> 1][(g & 1) * 2 + 0] = pack2(dsv[0], dsv[1], BF16);
+          da[g >> 1][(g & 1) * 2 + 1] = pack2(dsv[2], dsv[3], BF16);
+        }
       }
       wgmma_fence();
+      if constexpr (kDV) {
 #pragma unroll
-      for (int c = 0; c < NVB; ++c)
+        for (int c = 0; c < NVB; ++c)
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) wgmma_rs<64, BF16>(dv[c], pa[kk], make_desc(stdo + c * kBox64 + kk * 2048));
+          for (int kk = 0; kk < 4; ++kk) wgmma_rs<64, BF16>(dv[c], pa[kk], make_desc(stdo + c * kBox64 + kk * 2048));
+      }
+      if constexpr (kDK) {
 #pragma unroll
-      for (int c = 0; c < NQB; ++c)
+        for (int c = 0; c < NQB; ++c)
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) wgmma_rs<64, BF16>(dk[c], da[kk], make_desc(stq + c * kBox64 + kk * 2048));
+          for (int kk = 0; kk < 4; ++kk) wgmma_rs<64, BF16>(dk[c], da[kk], make_desc(stq + c * kBox64 + kk * 2048));
+      }
       wgmma_commit();
       wgmma_wait<0>();
 #pragma unroll
-      for (int c = 0; c < NVB; ++c) fence_regs(dv[c]);
+      for (int c = 0; c < NV; ++c) fence_regs(dv[c]);
 #pragma unroll
-      for (int c = 0; c < NQB; ++c) fence_regs(dk[c]);
+      for (int c = 0; c < NK; ++c) fence_regs(dk[c]);
       warp_arrive(&bar.empty[s]);
     }
     warp_arrive(&bar.fix_empty);
@@ -321,7 +354,7 @@ bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq64, const __grid_constant_
       T* krow = reinterpret_cast<T*>(p.dk) + (int64_t)b * p.dk_sb + (int64_t)j * p.dk_sm + (int64_t)h * p.dk_sh;
       T* vrow = reinterpret_cast<T*>(p.dv_out) + (int64_t)b * p.dv_sb + (int64_t)j * p.dv_sm + (int64_t)h * p.dv_sh;
 #pragma unroll
-      for (int c = 0; c < NQB; ++c)
+      for (int c = 0; c < NK; ++c)
 #pragma unroll
         for (int g = 0; g < 8; ++g) {
           const int col = c * 64 + 8 * g + cq;
@@ -329,7 +362,7 @@ bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq64, const __grid_constant_
             *reinterpret_cast<uint32_t*>(krow + col) = pack2(dk[c][4 * g + 2 * i] * p.scale, dk[c][4 * g + 2 * i + 1] * p.scale, BF16);
         }
 #pragma unroll
-      for (int c = 0; c < NVB; ++c)
+      for (int c = 0; c < NV; ++c)
 #pragma unroll
         for (int g = 0; g < 8; ++g) {
           const int col = c * 64 + 8 * g + cq;
@@ -494,6 +527,190 @@ bwd_dq_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CU
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// kernel 2 for head dims above 128 (NQB or NVB = 3): dQ with 64-key K / V stages, so S and dP take 32 registers each
+// (a 128-key tile would need 64 + 64 beside the three dQ boxes).  The work items are bwd_dq_kernel's CTAs, (b, h,
+// 128 queries, split of 128-key tiles), walked persistently as the dK/dV kernel walks its key tiles (in the
+// one-item-per-CTA form ptxas spills the dQ accumulators at NQB = 3).  No atomics: every work item stores its dQ share
+// (already scaled) as one fp32 partial (Bq, N, H*dqk) per (batch contribution, split), partial index
+// (q_bcast ? b : 0) * splits + split, and bwd_sum_dq_kernel adds the partials in index order, so dQ is bitwise
+// reproducible.
+// ---------------------------------------------------------------------------------------------------------------
+template <int NQB, int NVB>
+struct Cfg3 {
+  static constexpr int kQBytes = (NQB + NVB) * kBoxBytes;
+  static constexpr int kStage = (NQB + NVB) * kBox64;
+  static constexpr int kSlots = (kSmemLimit - kQBytes - 2048) / kStage > 4 ? 4 : (kSmemLimit - kQBytes - 2048) / kStage;
+  static constexpr int kSmem = kQBytes + kSlots * kStage + 2048;
+  static_assert(kSlots >= 2, "shared memory budget");
+};
+
+template <int NQB, int NVB, bool BF16>
+__global__ void __launch_bounds__(kThreads, 1)
+bwd_dq64_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk64,
+                const __grid_constant__ CUtensorMap tv64, const __grid_constant__ CUtensorMap tdo, const BwdParams p) {
+  using C = Cfg3<NQB, NVB>;
+  constexpr int NS = C::kSlots;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sQ = smem;
+  uint8_t* sdO = smem + NQB * kBoxBytes;
+  uint8_t* sRing = smem + C::kQBytes;
+  BwdBarriers& bar = *reinterpret_cast<BwdBarriers*>(sRing + NS * C::kStage);
+  const int wg = threadIdx.x / 128;
+  const int total = p.B * p.H * p.nq * p.splits;  // work items (b, h, query tile, split)
+  const int nk64 = (p.M + 63) / 64;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < NS; ++s) {
+      mbar_init(&bar.full[s], 1);
+      mbar_init(&bar.empty[s], 8);
+    }
+    mbar_init(&bar.fix_full, 1);
+    mbar_init(&bar.fix_empty, 8);
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    reg_dealloc<40>();
+    if (threadIdx.x == 0) {
+      uint32_t it = 0, wl = 0;
+      for (int w = blockIdx.x; w < total; w += gridDim.x, ++wl) {
+        const int unit = w / p.splits, split = w % p.splits;
+        const int bh = unit / p.nq, qt = unit % p.nq, b = bh / p.H, h = bh % p.H;
+        const int kt0 = 2 * split * p.tiles_per_split, kt1 = min(nk64, kt0 + 2 * p.tiles_per_split);
+        mbar_wait(&bar.fix_empty, (wl & 1) ^ 1, 34);
+        mbar_arrive_expect_tx(&bar.fix_full, C::kQBytes);
+        for (int c = 0; c < NQB; ++c)
+          tma_load_4d(sQ + c * kBoxBytes, &tq, &bar.fix_full, c * 64, qt * kT, h, p.q_bcast ? 0 : b);
+        for (int c = 0; c < NVB; ++c) tma_load_4d(sdO + c * kBoxBytes, &tdo, &bar.fix_full, c * 64, qt * kT, h, b);
+        for (int kt = kt0; kt < kt1; ++kt, ++it) {
+          const uint32_t s = it % NS;
+          mbar_wait(&bar.empty[s], ((it / NS) & 1) ^ 1, 35);
+          mbar_arrive_expect_tx(&bar.full[s], C::kStage);
+          uint8_t* st = sRing + s * C::kStage;
+          for (int c = 0; c < NQB; ++c) tma_load_4d(st + c * kBox64, &tk64, &bar.full[s], c * 64, kt * 64, h, b);
+          for (int c = 0; c < NVB; ++c)
+            tma_load_4d(st + (NQB + c) * kBox64, &tv64, &bar.full[s], c * 64, kt * 64, h, b);
+        }
+      }
+    }
+    return;
+  }
+
+  reg_alloc<232>();
+  const int cw = wg - 1;
+  const int tid = threadIdx.x - 128 * wg;
+  const int warp = tid >> 5, lane = tid & 31;
+  const int qloc = 64 * cw + 16 * warp + (lane >> 2);
+  const int r0 = 16 * warp + (lane >> 2);  // this thread's rows r0, r0 + 8 of its warpgroup's 64-query statistics block
+  const int cq = 2 * (lane & 3);
+  const uint32_t q_base = smem_u32(sQ) + cw * 64 * 128, do_base = smem_u32(sdO) + cw * 64 * 128;
+  const uint32_t ring = smem_u32(sRing);
+  uint32_t it = 0, wl = 0;
+  for (int w = blockIdx.x; w < total; w += gridDim.x, ++wl) {
+    const int unit = w / p.splits, split = w % p.splits;
+    const int bh = unit / p.nq, qt = unit % p.nq, b = bh / p.H, h = bh % p.H;
+    const int kt0 = 2 * split * p.tiles_per_split, kt1 = min(nk64, kt0 + 2 * p.tiles_per_split);
+    const float* blk = p.stats + ((int64_t)bh * (p.Npad / 64) + 2 * qt + cw) * (kStatsBytes / 4);
+    mbar_wait(&bar.fix_full, wl & 1, 36);
+    float acc[NQB][32];
+#pragma unroll
+    for (int c = 0; c < NQB; ++c)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
+    for (int kt = kt0; kt < kt1; ++kt, ++it) {
+      const uint32_t s = it % NS;
+      const uint32_t stk = ring + s * C::kStage, stv = stk + NQB * kBox64;
+      mbar_wait(&bar.full[s], (it / NS) & 1, 37);
+      float sc[32], dp[32];
+      wgmma_fence();
+#pragma unroll
+      for (int c = 0; c < NQB; ++c)
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk)
+          wgmma_ss<64, BF16>(sc, make_desc(q_base + c * kBoxBytes + kk * 32), make_desc(stk + c * kBox64 + kk * 32), (c | kk) != 0);
+#pragma unroll
+      for (int c = 0; c < NVB; ++c)
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk)
+          wgmma_ss<64, BF16>(dp, make_desc(do_base + c * kBoxBytes + kk * 32), make_desc(stv + c * kBox64 + kk * 32), (c | kk) != 0);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(sc);
+      fence_regs(dp);
+      uint32_t a[4][4];
+#pragma unroll
+      for (int g = 0; g < 8; ++g) {
+        float val[4];
+#pragma unroll
+        for (int e4 = 0; e4 < 4; ++e4) {
+          const int i = e4 >> 1, e = e4 & 1;
+          const int j = kt * 64 + 8 * g + cq + e, n = qt * kT + qloc + 8 * i, r = r0 + 8 * i;
+          const float nlse = blk[stat_nlse_idx(r)], delta = blk[stat_delta_idx(r)], fillp = blk[stat_fillp_idx(r)];
+          const bool oob = j >= p.M || n >= p.N;
+          const bool filled = !oob && filled_key(p, b, j, n);
+          const float P = oob ? 0.f : (filled ? fillp : ex2(fmaf(sc[4 * g + e4], p.scale_log2, nlse)));
+          bool keep = true;
+          if (p.drop_thresh)
+            keep = drop_keep(drop_bits(p.seed_lo, p.seed_hi, (uint32_t)bh, (uint32_t)n, (uint32_t)j), n, j, p.drop_thresh);
+          const float dP = keep ? dp[4 * g + e4] * p.drop_rp : 0.f;
+          val[e4] = (oob || filled) ? 0.f : P * (dP - delta);
+        }
+        a[g >> 1][(g & 1) * 2 + 0] = pack2(val[0], val[1], BF16);
+        a[g >> 1][(g & 1) * 2 + 1] = pack2(val[2], val[3], BF16);
+      }
+      wgmma_fence();
+#pragma unroll
+      for (int c = 0; c < NQB; ++c)
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) wgmma_rs<64, BF16>(acc[c], a[kk], make_desc(stk + c * kBox64 + kk * 2048));
+      wgmma_commit();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int c = 0; c < NQB; ++c) fence_regs(acc[c]);
+      warp_arrive(&bar.empty[s]);
+    }
+    warp_arrive(&bar.fix_empty);
+    // this work item's partial: every element of it is written by exactly one work item
+    const int Bq = p.q_bcast ? 1 : p.B, bq = p.q_bcast ? 0 : b;
+    const int64_t part = (int64_t)(p.q_bcast ? b : 0) * p.splits + split;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int n = qt * kT + qloc + 8 * i;
+      if (n >= p.N) continue;
+      float* dst = p.dq32 + (((part * Bq + bq) * p.N + n) * p.H + h) * p.dqk;
+#pragma unroll
+      for (int c = 0; c < NQB; ++c)
+#pragma unroll
+        for (int g = 0; g < 8; ++g) {
+          const int col = c * 64 + 8 * g + cq;
+          if (col < p.dqk)
+            *reinterpret_cast<float2*>(dst + col) = make_float2(acc[c][4 * g + 2 * i] * p.scale, acc[c][4 * g + 2 * i + 1] * p.scale);
+        }
+    }
+  }
+}
+
+// the dQ partials of bwd_dq64_kernel (nparts x (Bq, N, H*dqk) fp32), added in partial order -> dq in the operand dtype
+template <typename T>
+__global__ void __launch_bounds__(256) bwd_sum_dq_kernel(const float* __restrict__ part, int nparts, T* __restrict__ dq,
+                                                         int Bq, int N, int H, int dqk, int64_t sb, int64_t sn, int64_t sh) {
+  const int64_t total = (int64_t)Bq * N * H * dqk;
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+       idx += (int64_t)gridDim.x * blockDim.x) {
+    float s = 0.f;
+    for (int i = 0; i < nparts; ++i) s += part[i * total + idx];
+    const int c = (int)(idx % dqk);
+    int64_t r = idx / dqk;
+    const int h = (int)(r % H);
+    r /= H;
+    const int n = (int)(r % N);
+    const int b = (int)(r / N);
+    dq[b * sb + (int64_t)n * sn + h * sh + c] = Elem<T>::from_f(s);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // host
 // ---------------------------------------------------------------------------------------------------------------
 inline size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
@@ -506,11 +723,30 @@ void set_dropout(BwdParams& p, float dropout_p, uint64_t seed) {
   p.seed_hi = r.seed_hi;
 }
 
+// Split of the dq kernel's key tiles over CTAs: aim at ~64 key tiles per CTA (launch + Q/dO load amortised) but at
+// least ~4 CTAs per SM in total
+void dq_split(int units, int nk, int sms, int& tiles_per_split, int& splits) {
+  int s = std::max(1, (nk + 63) / 64);
+  while (units * s < 4 * sms && s < nk && (nk + s - 1) / s > 4) ++s;
+  tiles_per_split = (nk + s - 1) / s;
+  splits = (nk + tiles_per_split - 1) / tiles_per_split;
+}
+
+// Head dims above 128 take the wide variants: the dK/dV kernel with up to three boxes (in two passes above four boxes
+// in all) and bwd_dq64_kernel with its ordered dQ partials.
+bool wide_bwd(int dqk, int dv) { return dqk > 128 || dv > 128; }
+
+// The wide dQ split is planned for a fixed SM count (the H100 SXM's 132), not the device's: the number of dQ partials,
+// and so the workspace size, follow from the problem alone, and so does the order in which dQ is summed.
+constexpr int kWideSplitSms = 132;
+
 // Workspace of the backward and of the dropout forward: the row-statistics blocks, an fp32 accumulator of acc_bytes
-// (dQ of the backward, O of the dropout forward), then the pad bits.
+// (dQ of the backward, O of the dropout forward; zeroed before the kernels), the pad bits, then part_bytes of dQ
+// partials (the wide backward; written whole by its dQ kernel, so not zeroed).
 struct BwdLayout {
   int Npad, nq, nk;
-  size_t acc_bytes, off_acc, off_pad, total;  // the statistics start at offset 0
+  int dq_splits, dq_tiles_per_split, dq_parts;  // the wide backward's dQ split and partial count (else 0)
+  size_t acc_bytes, off_acc, off_pad, part_bytes, off_part, total;  // the statistics start at offset 0
 };
 
 BwdLayout bwd_layout(int B, int H, int N, int M, bool pad, size_t acc_bytes) {
@@ -518,16 +754,25 @@ BwdLayout bwd_layout(int B, int H, int N, int M, bool pad, size_t acc_bytes) {
   L.nq = (N + kT - 1) / kT;
   L.nk = (M + kT - 1) / kT;
   L.Npad = L.nq * kT;
+  L.dq_splits = L.dq_tiles_per_split = L.dq_parts = 0;
   L.acc_bytes = acc_bytes;
   L.off_acc = align256((size_t)kStatsBytes * B * H * 2 * L.nq);
   L.off_pad = L.off_acc + align256(acc_bytes);
-  L.total = L.off_pad + (pad ? align256(sizeof(uint32_t) * (size_t)B * pad_words_per_row(M)) : 0);
+  L.part_bytes = 0;
+  L.off_part = L.total = L.off_pad + (pad ? align256(sizeof(uint32_t) * (size_t)B * pad_words_per_row(M)) : 0);
   return L;
 }
 
 BwdLayout bwd_layout(const pcv_attn_bwd_params& a) {
   const int Bq = a.q_stride_b == 0 ? 1 : a.B;
-  return bwd_layout(a.B, a.H, a.N, a.M, a.pad_mask != nullptr, sizeof(float) * (size_t)Bq * a.N * a.H * a.dqk);
+  const size_t dq_bytes = sizeof(float) * (size_t)Bq * a.N * a.H * a.dqk;
+  if (!wide_bwd(a.dqk, a.dv)) return bwd_layout(a.B, a.H, a.N, a.M, a.pad_mask != nullptr, dq_bytes);
+  BwdLayout L = bwd_layout(a.B, a.H, a.N, a.M, a.pad_mask != nullptr, 0);
+  dq_split(a.B * a.H * L.nq, L.nk, kWideSplitSms, L.dq_tiles_per_split, L.dq_splits);
+  L.dq_parts = (Bq == 1 ? a.B : 1) * L.dq_splits;  // a batch-1 q receives one contribution per batch row and split
+  L.part_bytes = dq_bytes * L.dq_parts;
+  L.total = L.off_part + align256(L.part_bytes);
+  return L;
 }
 
 BwdLayout fwd_drop_layout(const pcv_attn_params& a) {
@@ -544,6 +789,7 @@ struct DeltaOperands {
 struct BwdMaps {
   CUtensorMap q, k, v;            // 128-row boxes
   CUtensorMap dout, q64, dout64;  // backward only; the dK/dV kernel stages Q and dO in 64-row boxes
+  CUtensorMap k64, v64;           // wide backward only; bwd_dq64_kernel stages K and V in 64-row boxes
 };
 
 // The host steps the backward and the dropout forward share; A is pcv_attn_bwd_params or pcv_attn_params, which name
@@ -568,13 +814,11 @@ int bwd_setup(const A& a, const BwdLayout& L, const float* stat_m, const float* 
   p.cshift = a.M - a.N;
   p.stats = reinterpret_cast<const float*>(ws);
   set_dropout(p, dropout_p, seed);
-  // dq kernel: aim at ~64 key tiles per CTA (launch + Q/dO load amortised) but at least ~4 CTAs per SM in total
-  {
-    const int units = a.B * a.H * L.nq;
-    int splits = std::max(1, (L.nk + 63) / 64);
-    while (units * splits < 4 * sms && splits < L.nk && (L.nk + splits - 1) / splits > 4) ++splits;
-    p.tiles_per_split = (L.nk + splits - 1) / splits;
-    p.splits = (L.nk + p.tiles_per_split - 1) / p.tiles_per_split;
+  if (L.dq_splits > 0) {
+    p.tiles_per_split = L.dq_tiles_per_split;
+    p.splits = L.dq_splits;
+  } else {
+    dq_split(a.B * a.H * L.nq, L.nk, sms, p.tiles_per_split, p.splits);
   }
 
   PCV_CHECK_CUDA(cudaMemsetAsync(ws + L.off_acc, 0, L.acc_bytes, stream));
@@ -630,6 +874,34 @@ int launch_tc(bool fwd, const BwdMaps& m, const BwdParams& p, int sms, cudaStrea
   return p.dv <= 64 ? launch_tc_kernels<2, 1, BF16>(fwd, m, p, sms, stream) : launch_tc_kernels<2, 2, BF16>(fwd, m, p, sms, stream);
 }
 
+// The wide backward (a head dim above 128): the dK/dV kernel as a dV pass and a dK pass, then bwd_dq64_kernel into the
+// dQ partials.
+template <int NQB, int NVB, bool BF16>
+int launch_wide_kernels(const BwdMaps& m, const BwdParams& p, int sms, cudaStream_t stream) {
+  using C1 = Cfg1<NQB, NVB>;
+  const dim3 grid1(std::min(p.total_tiles, sms));
+  int rc = launch_kernel(bwd_dkdv_kernel<NQB, NVB, BF16, kOutDV>, grid1, kThreads, C1::kSmem, 0, stream, m.q64, m.k, m.v,
+                         m.dout64, p);
+  if (rc != PCV_OK) return rc;
+  rc = launch_kernel(bwd_dkdv_kernel<NQB, NVB, BF16, kOutDK>, grid1, kThreads, C1::kSmem, 0, stream, m.q64, m.k, m.v,
+                     m.dout64, p);
+  if (rc != PCV_OK) return rc;
+  return launch_kernel(bwd_dq64_kernel<NQB, NVB, BF16>, dim3(std::min(p.B * p.H * p.nq * p.splits, sms)), kThreads,
+                       Cfg3<NQB, NVB>::kSmem, 0, stream, m.q, m.k64, m.v64, m.dout, p);
+}
+
+// every (NQB, NVB) in {1, 2, 3}^2 with a 3
+template <bool BF16>
+int launch_wide(const BwdMaps& m, const BwdParams& p, int sms, cudaStream_t stream) {
+  const int nqb = (p.dqk + 63) / 64, nvb = (p.dv + 63) / 64;
+  if (nqb == 3) {
+    if (nvb == 1) return launch_wide_kernels<3, 1, BF16>(m, p, sms, stream);
+    if (nvb == 2) return launch_wide_kernels<3, 2, BF16>(m, p, sms, stream);
+    return launch_wide_kernels<3, 3, BF16>(m, p, sms, stream);
+  }
+  return nqb == 1 ? launch_wide_kernels<1, 3, BF16>(m, p, sms, stream) : launch_wide_kernels<2, 3, BF16>(m, p, sms, stream);
+}
+
 // fp32 accumulator (Bq, N, H*width) -> the 16-bit output with its own strides
 int launch_cast(bool bf16, const float* acc, void* dst, int Bq, int N, int H, int width, int64_t sb, int64_t sn,
                 int64_t sh, cudaStream_t stream) {
@@ -645,6 +917,22 @@ int launch_cast(bool bf16, const float* acc, void* dst, int Bq, int N, int H, in
   return PCV_OK;
 }
 
+// the wide backward's dQ partials, summed in order -> dq with its own strides
+int launch_sum_dq(bool bf16, const float* part, int nparts, void* dst, int Bq, int N, int H, int dqk, int64_t sb,
+                  int64_t sn, int64_t sh, cudaStream_t stream) {
+  const int64_t total = (int64_t)Bq * N * H * dqk;
+  const int blocks = (int)std::min<int64_t>((total + 255) / 256, 4096);
+  if (bf16)
+    bwd_sum_dq_kernel<__nv_bfloat16><<<blocks, 256, 0, stream>>>(part, nparts, reinterpret_cast<__nv_bfloat16*>(dst), Bq,
+                                                                 N, H, dqk, sb, sn, sh);
+  else
+    bwd_sum_dq_kernel<__half><<<blocks, 256, 0, stream>>>(part, nparts, reinterpret_cast<__half*>(dst), Bq, N, H, dqk, sb,
+                                                          sn, sh);
+  PCV_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return PCV_OK;
+}
+
 }  // namespace
 
 bool attn_bwd_supported(const pcv_attn_bwd_params& a, const char** why) {
@@ -654,8 +942,9 @@ bool attn_bwd_supported(const pcv_attn_bwd_params& a, const char** why) {
   };
   if (a.dtype != PCV_BF16 && a.dtype != PCV_F16) return no("dtype must be bf16 or fp16");
   if (a.B < 1 || a.H < 1 || a.N < 1 || a.M < 1) return no("empty problem");
-  if (a.dqk < 8 || a.dv < 8 || a.dqk > 128 || a.dv > 128) return no("head dims must be in [8, 128]");
+  if (a.dqk < 8 || a.dv < 8) return no("head dims must be in [8, 192]");
   if (a.dqk % 8 || a.dv % 8) return no("head dims must be multiples of 8");
+  if (a.dqk > 192 || a.dv > 192) return no("head dims must be in [8, 192]");
   if (!(a.dropout_p >= 0.f && a.dropout_p < 1.f)) return no("dropout_p must be in [0, 1)");
   if (!al16(a.q) || !al16(a.k) || !al16(a.v) || !al16(a.out) || !al16(a.grad_out) || !al16(a.grad_q) ||
       !al16(a.grad_k) || !al16(a.grad_v))
@@ -692,7 +981,8 @@ int launch_attn_bwd(const pcv_attn_bwd_params& a, cudaStream_t stream) {
   int sms = 0;
   int rc = bwd_setup(a, L, a.stat_m, a.stat_l, d, a.dropout_p, a.dropout_seed, stream, p, m, sms);
   if (rc != PCV_OK) return rc;
-  p.dq32 = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(a.workspace) + L.off_acc);
+  const bool wide = wide_bwd(a.dqk, a.dv);
+  p.dq32 = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(a.workspace) + (wide ? L.off_part : L.off_acc));
   p.dk = a.grad_k; p.dv_out = a.grad_v;
   p.dk_sb = a.gk_stride_b; p.dk_sm = a.gk_stride_m; p.dk_sh = a.gk_stride_h;
   p.dv_sb = a.gv_stride_b; p.dv_sm = a.gv_stride_m; p.dv_sh = a.gv_stride_h;
@@ -713,6 +1003,16 @@ int launch_attn_bwd(const pcv_attn_bwd_params& a, cudaStream_t stream) {
   if (rc != PCV_OK) return rc;
 
   const bool bf16 = a.dtype == PCV_BF16;
+  if (wide) {
+    rc = make_tmap_4d(&m.k64, a.k, a.dtype, a.dqk, a.M, a.H, a.B, a.k_stride_m, a.k_stride_h, a.k_stride_b, 64);
+    if (rc != PCV_OK) return rc;
+    rc = make_tmap_4d(&m.v64, a.v, a.dtype, a.dv, a.M, a.H, a.B, a.v_stride_m, a.v_stride_h, a.v_stride_b, 64);
+    if (rc != PCV_OK) return rc;
+    rc = bf16 ? launch_wide<true>(m, p, sms, stream) : launch_wide<false>(m, p, sms, stream);
+    if (rc != PCV_OK) return rc;
+    return launch_sum_dq(bf16, p.dq32, L.dq_parts, a.grad_q, Bq, a.N, a.H, a.dqk, a.gq_stride_b, a.gq_stride_n,
+                         a.gq_stride_h, stream);
+  }
   rc = bf16 ? launch_tc<true>(false, m, p, sms, stream) : launch_tc<false>(false, m, p, sms, stream);
   if (rc != PCV_OK) return rc;
   return launch_cast(bf16, p.dq32, a.grad_q, Bq, a.N, a.H, a.dqk, a.gq_stride_b, a.gq_stride_n, a.gq_stride_h, stream);

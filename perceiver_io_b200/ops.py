@@ -216,7 +216,8 @@ def _fill_bwd_params(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, p
 
 def attention_backward(q, k, v, out, grad_out, stat_m, stat_l, num_heads: int, scale: float, pad_mask=None,
                        causal: bool = False, check_only: bool = False, dropout_p: float = 0.0, dropout_seed: int = 0):
-    """Gradients (grad_q, grad_k, grad_v) of ``attention`` on the tcgen05 backward kernels (pcv_attn_bwd).
+    """Gradients (grad_q, grad_k, grad_v) of ``attention`` on the tcgen05 backward kernels (pcv_attn_bwd): head dims
+    that are multiples of 8, up to 192.  Above 128, grad_q is summed in a fixed order (bitwise reproducible).
 
     ``out`` is the forward output, ``stat_m`` / ``stat_l`` the (B, H, N) row statistics of ``attention_partial`` over all
     keys.  grad_q has q's batch size (a batch-1 ``q`` shared by the batch receives the sum).  ``check_only`` launches
@@ -319,13 +320,34 @@ def _partial_dropout_supported(q, k, v, num_heads: int, pad_mask, causal: bool, 
     return ok
 
 
+def _kernel_backward(q, k, v, out, grad_out, stat_m, stat_l, num_heads: int, scale: float, pad_mask, causal: bool,
+                     dropout_p: float, dropout_seed: int):
+    """(grad_q, grad_k, grad_v) of ``_FusedAttention`` on the backward kernels (``attention_backward``), or None where
+    they do not cover the call.  Head dims that are not multiples of 8 are zero-padded per head, as the forward padded
+    them, and the gradients sliced back: zero channels change neither the scores, nor delta = rowsum(dO * O), nor the
+    dropout mask, and the gradients of the padding channels are dropped."""
+    dqk, dv = _head_dim(q, num_heads), _head_dim(v, num_heads)
+    padded = bool(dqk % 8 or dv % 8)
+    if padded:
+        q, k, v, out, grad_out = (_pad_heads_to8(t, num_heads).flatten(2) for t in (q, k, v, out, grad_out))
+    if not attention_backward(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask, causal,
+                              check_only=True, dropout_p=dropout_p, dropout_seed=dropout_seed):
+        return None
+    gq, gk, gv = attention_backward(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask, causal,
+                                    dropout_p=dropout_p, dropout_seed=dropout_seed)
+    if padded:
+        gq, gk, gv = (g.unflatten(2, (num_heads, -1))[..., :d].flatten(2) for g, d in ((gq, dqk), (gk, dqk), (gv, dv)))
+    return gq, gk, gv
+
+
 class _FusedAttention(torch.autograd.Function):
     """Forward = the fused CUDA kernel (partial-state mode, so the row max and denominator are kept).  With dropout:
     the partial forward and the second-pass dropout kernel (``attention_dropout_forward``) where that covers the call
     (head dims that are multiples of 8 up to 128), else the one-pass dropout forward (``attention_partial`` with
     ``dropout_p``) for every head dim the forward takes.
     Backward = the tensor-core backward kernels (``attention_backward`` -> pcv_attn_bwd: dK/dV and dQ kernels, SURVEY.md
-    §8(f) rank 2) for head dims that are multiples of 8 up to 128.  Other shapes take the labelled SHIM below: the
+    §8(f) rank 2) for head dims up to 192; head dims that are not multiples of 8 are zero-padded as in the forward
+    (``_kernel_backward``).  Other shapes (head dims above 192, the decode forward) take the labelled SHIM below: the
     flash-attention backward recurrence in plain torch ops, chunked over the key axis from the saved statistics,
     memory bounded by ``backward_config["max_score_bytes"]``, with dropout regenerating the mask of each key chunk
     (``_dropout_keep``); neither path ever holds the (B, H, N, M) score tensor (8.6 GB at the north-star shape).
@@ -360,13 +382,22 @@ class _FusedAttention(torch.autograd.Function):
             ctx.save_for_backward(q, k, v, pad_mask, out, pm, pl)
             ctx.meta = (num_heads, scale, causal)
             return out
-        if _head_dim(q, num_heads) % 8 or dv_true % 8 or impl == "decode":
-            # head dims the partial-state kernels do not take without padding: plain forward, statistics recomputed
+        if impl == "decode":
+            # the decode kernel keeps no partial state: plain forward, statistics recomputed by the shim
             out = _attention_forward(q, k, v, num_heads, scale, pad_mask, causal, impl)
             ctx.save_for_backward(q, k, v, pad_mask, out, None, None)
         else:
-            po, pm, pl = attention_partial(q, k, v, num_heads, scale, pad_mask=pad_mask, causal=causal, impl=impl)
+            # head dims that are not multiples of 8 are zero-padded (as in the dropout branch), so that the statistics
+            # exist for the backward kernels
+            qp, kp, vp = q, k, v
+            if _head_dim(q, num_heads) % 8 or dv_true % 8:
+                qp, kp, vp = (_pad_heads_to8(t, num_heads) for t in (q, k, v))
+            po, pm, pl = attention_partial(qp, kp, vp, num_heads, scale, pad_mask=pad_mask, causal=causal, impl=impl)
             out = combine_partials(po[None], pm[None], pl[None], _compute_dtype(q.dtype))
+            B, N, H, dv_pad = po.shape[0], po.shape[2], po.shape[1], po.shape[3]
+            del po
+            if dv_pad != dv_true:
+                out = out.view(B, N, H, dv_pad)[..., :dv_true].reshape(B, N, H * dv_true)
             out = out if out.dtype == q.dtype else out.to(q.dtype)
             ctx.save_for_backward(q, k, v, pad_mask, out, pm, pl)
         ctx.meta = (num_heads, scale, causal)
@@ -381,12 +412,11 @@ class _FusedAttention(torch.autograd.Function):
         if mode not in ("auto", "kernel", "shim"):
             raise ValueError(f"backward_config['impl'] = {mode!r}")
         if mode != "shim":
-            ok = (pm is not None and q.is_cuda and q.dim() == 3 and k.dim() == 3 and v.dim() == 3
-                  and attention_backward(q, k, v, out, grad_out, pm, pl, H, scale, pad_mask, causal, check_only=True,
-                                         dropout_p=drop_p, dropout_seed=drop_seed))
-            if ok:
-                gq, gk, gv = attention_backward(q, k, v, out, grad_out, pm, pl, H, scale, pad_mask, causal,
-                                                dropout_p=drop_p, dropout_seed=drop_seed)
+            grads = None
+            if pm is not None and q.is_cuda and q.dim() == 3 and k.dim() == 3 and v.dim() == 3:
+                grads = _kernel_backward(q, k, v, out, grad_out, pm, pl, H, scale, pad_mask, causal, drop_p, drop_seed)
+            if grads is not None:
+                gq, gk, gv = grads
                 return gq.to(q.dtype), gk.to(k.dtype), gv.to(v.dtype), None, None, None, None, None, None, None
             if mode == "kernel":
                 raise RuntimeError("backward_config['impl'] = 'kernel' but pcv_attn_bwd does not cover this call: "
@@ -466,7 +496,8 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, num_heads: int,
     padding) and the right-aligned causal mask use the finite fill ``-finfo.max``.  ``dropout_p`` > 0 applies the
     reference's dropout on the attention probabilities (:161) with a counter-based mask derived from
     ``dropout_seed`` (default: a fresh seed from torch's CPU generator), for every head dim the forward takes (up to
-    512; above 128 the backward runs on the torch shim).
+    512).  Under autograd the backward runs on the tensor-core kernels for head dims up to 192 (odd ones zero-padded
+    to multiples of 8), above that on the torch shim.
     """
     if dropout_p > 0.0:
         if not 0.0 < dropout_p < 1.0:
