@@ -412,6 +412,38 @@ PCV_API int pcv_attn_fwd_partial_dropout_supported(const pcv_attn_params* p, flo
 PCV_API int pcv_attn_fwd_partial_dropout(const pcv_attn_params* p, float dropout_p, uint64_t dropout_seed, void* stream);
 
 /*
+ * Training through a key-sharded attention (each rank holds keys [m_offset, m_offset + M) of m_total).
+ *
+ * pcv_attn_fwd_partial_dropout_shard: pcv_attn_fwd_partial_dropout on the keys [p->m_offset, p->m_offset + p->M) of
+ * p->m_total.  The causal mask and the dropout mask take global key indices: element (b, h, q, m_offset + j) is
+ * dropped exactly as pcv_attn_dropout_mask_range exports it, so the shards of one call drop what the unsharded call
+ * drops.  part_m / part_l are the dropout-free statistics of the local keys.  m_offset must be even (the mask hashes
+ * key pairs).
+ *
+ * pcv_attn_bwd_shard: the backward of one key shard.  stat_m / stat_l are the statistics MERGED over all m_total keys
+ * (the exact merge of every shard's partial state) and out is the merged output.  grad_k / grad_v receive the local
+ * keys' gradients, complete.  grad_q in `p` is ignored (may be NULL): the shard's fp32 contribution to grad_q is
+ * written to s->grad_q32, (B or 1, N, H, dqk) dense (for a batch-1 q already summed over the batch); grad_q is the sum
+ * of the contributions of all shards.  Up to head dim 128 the contribution is accumulated with atomics, above that
+ * summed in a fixed order (bitwise reproducible).  Head dims and alignment as pcv_attn_bwd; s->grad_q32 16-byte
+ * aligned.  The workspace (pcv_attn_bwd_shard_workspace_bytes, computed without a device) holds no dQ accumulator up
+ * to head dim 128.
+ * Every argument is checked before any CUDA call.
+ */
+typedef struct pcv_key_shard {
+  int32_t m_total;   /* keys of the whole problem (all shards)                                   */
+  int32_t m_offset;  /* global index of this call's key 0 (even)                                 */
+  float* grad_q32;   /* (Bq, N, H, dqk) fp32 dense: this shard's contribution to grad_q, WRITTEN  */
+} pcv_key_shard;
+
+PCV_API int pcv_attn_fwd_partial_dropout_shard_supported(const pcv_attn_params* p, float dropout_p);
+PCV_API int pcv_attn_fwd_partial_dropout_shard(const pcv_attn_params* p, float dropout_p, uint64_t dropout_seed,
+                                               void* stream);
+PCV_API int pcv_attn_bwd_shard_supported(const pcv_attn_bwd_params* p, const pcv_key_shard* s);
+PCV_API int pcv_attn_bwd_shard_workspace_bytes(const pcv_attn_bwd_params* p, const pcv_key_shard* s, size_t* bytes);
+PCV_API int pcv_attn_bwd_shard(const pcv_attn_bwd_params* p, const pcv_key_shard* s, void* stream);
+
+/*
  * Live timing of the dominant kernel (bench.py's roofline leg): between pcv_profile_begin() and
  * pcv_profile_end() every attention main-kernel launch is bracketed by CUDA events on its own
  * stream; pcv_profile_end() synchronises those events and returns their summed duration.

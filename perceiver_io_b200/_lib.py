@@ -48,6 +48,11 @@ EXPORTS = (
     "pcv_attn_dropout_mask_range",
     "pcv_attn_fwd_partial_dropout_supported",
     "pcv_attn_fwd_partial_dropout",
+    "pcv_attn_fwd_partial_dropout_shard_supported",
+    "pcv_attn_fwd_partial_dropout_shard",
+    "pcv_attn_bwd_shard_supported",
+    "pcv_attn_bwd_shard_workspace_bytes",
+    "pcv_attn_bwd_shard",
     "pcv_launch_count",
     "pcv_debug_plan",
     "pcv_profile_begin",
@@ -198,6 +203,10 @@ class AttnBwdParams(C.Structure):
     ]
 
 
+class KeyShard(C.Structure):
+    _fields_ = [("m_total", C.c_int32), ("m_offset", C.c_int32), ("grad_q32", C.c_void_p)]
+
+
 class DeviceInfo(C.Structure):
     _fields_ = [
         ("device", C.c_int32), ("sm_major", C.c_int32), ("sm_minor", C.c_int32),
@@ -278,6 +287,17 @@ def lib() -> C.CDLL:
         l.pcv_attn_fwd_partial_dropout_supported.restype = C.c_int
         l.pcv_attn_fwd_partial_dropout.argtypes = [C.POINTER(AttnParams), C.c_float, C.c_uint64, C.c_void_p]
         l.pcv_attn_fwd_partial_dropout.restype = C.c_int
+        l.pcv_attn_fwd_partial_dropout_shard_supported.argtypes = [C.POINTER(AttnParams), C.c_float]
+        l.pcv_attn_fwd_partial_dropout_shard_supported.restype = C.c_int
+        l.pcv_attn_fwd_partial_dropout_shard.argtypes = [C.POINTER(AttnParams), C.c_float, C.c_uint64, C.c_void_p]
+        l.pcv_attn_fwd_partial_dropout_shard.restype = C.c_int
+        l.pcv_attn_bwd_shard_supported.argtypes = [C.POINTER(AttnBwdParams), C.POINTER(KeyShard)]
+        l.pcv_attn_bwd_shard_supported.restype = C.c_int
+        l.pcv_attn_bwd_shard_workspace_bytes.argtypes = [C.POINTER(AttnBwdParams), C.POINTER(KeyShard),
+                                                         C.POINTER(C.c_size_t)]
+        l.pcv_attn_bwd_shard_workspace_bytes.restype = C.c_int
+        l.pcv_attn_bwd_shard.argtypes = [C.POINTER(AttnBwdParams), C.POINTER(KeyShard), C.c_void_p]
+        l.pcv_attn_bwd_shard.restype = C.c_int
         l.pcv_debug_plan.argtypes = [C.c_int32] * 7 + [C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_int32)]
         l.pcv_debug_plan.restype = C.c_int
         for name in ("pcv_get_device_info", "pcv_attn_supported_tcgen05", "pcv_attn_workspace_bytes",

@@ -70,15 +70,18 @@ static bool use_decode(const pcv_attn_params& p, const char** why) {
   return attn_decode_supported(p, why);
 }
 
-// The one-pass dropout forward: the tensor-core kernel's partial state over all keys of an unsharded call.
-static bool partial_dropout_supported(const pcv_attn_params& p, float dropout_p, const char** why) {
+// The one-pass dropout forward: the tensor-core kernel's partial state, over all keys of an unsharded call or (shard)
+// over a key shard starting at an even global key.
+static bool partial_dropout_supported(const pcv_attn_params& p, float dropout_p, bool shard, const char** why) {
   auto no = [&](const char* w) {
     *why = w;
     return false;
   };
   if (!(dropout_p > 0.f && dropout_p < 1.f)) return no("dropout_p must be in (0, 1)");
   if (!p.write_partial) return no("the call must write the partial state (write_partial = 1)");
-  if (p.m_total != p.M || p.m_offset != 0) return no("key sharding takes no dropout");
+  if (!shard && (p.m_total != p.M || p.m_offset != 0))
+    return no("key sharding takes no dropout here (pcv_attn_fwd_partial_dropout_shard)");
+  if (p.m_offset % 2) return no("m_offset must be even (the dropout mask hashes key pairs)");
   if (p.impl != PCV_IMPL_AUTO && p.impl != PCV_IMPL_TCGEN05) return no("only the single-CTA tensor-core kernel takes dropout");
   return attn_tc_supported(p, why);
 }
@@ -270,22 +273,43 @@ int pcv_kv_project(const pcv_kvproj_params* p, void* stream) {
   return launch_kv_project(*p, reinterpret_cast<cudaStream_t>(stream));
 }
 
-int pcv_attn_bwd_supported(const pcv_attn_bwd_params* p) {
+// s == nullptr: the unsharded backward
+static int bwd_check(const pcv_attn_bwd_params* p, const pcv_key_shard* s) {
   if (p == nullptr) return 0;
   const char* why = "";
-  const bool ok = attn_bwd_supported(*p, &why);
+  const bool ok = attn_bwd_supported(*p, s, &why);
   if (!ok) set_error("attn_bwd not applicable: %s", why);
   return ok ? 1 : 0;
 }
 
+int pcv_attn_bwd_supported(const pcv_attn_bwd_params* p) { return bwd_check(p, nullptr); }
+
 int pcv_attn_bwd_workspace_bytes(const pcv_attn_bwd_params* p, size_t* bytes) {
   PCV_REQUIRE(p != nullptr, PCV_ERR_INVALID, "attn_bwd_workspace_bytes: params is NULL");
-  return attn_bwd_workspace_bytes(*p, bytes);
+  return attn_bwd_workspace_bytes(*p, nullptr, bytes);
 }
 
 int pcv_attn_bwd(const pcv_attn_bwd_params* p, void* stream) {
   PCV_REQUIRE(p != nullptr, PCV_ERR_INVALID, "attn_bwd: params is NULL");
-  return launch_attn_bwd(*p, reinterpret_cast<cudaStream_t>(stream));
+  return launch_attn_bwd(*p, nullptr, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pcv_attn_bwd_shard_supported(const pcv_attn_bwd_params* p, const pcv_key_shard* s) {
+  if (s == nullptr) {
+    set_error("attn_bwd_shard: shard is NULL");
+    return 0;
+  }
+  return bwd_check(p, s);
+}
+
+int pcv_attn_bwd_shard_workspace_bytes(const pcv_attn_bwd_params* p, const pcv_key_shard* s, size_t* bytes) {
+  PCV_REQUIRE(p != nullptr && s != nullptr, PCV_ERR_INVALID, "attn_bwd_shard_workspace_bytes: params or shard is NULL");
+  return attn_bwd_workspace_bytes(*p, s, bytes);
+}
+
+int pcv_attn_bwd_shard(const pcv_attn_bwd_params* p, const pcv_key_shard* s, void* stream) {
+  PCV_REQUIRE(p != nullptr && s != nullptr, PCV_ERR_INVALID, "attn_bwd_shard: params or shard is NULL");
+  return launch_attn_bwd(*p, s, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int pcv_attn_fwd_dropout_supported(const pcv_attn_params* p, float dropout_p) {
@@ -318,21 +342,39 @@ int pcv_attn_dropout_mask_range(uint8_t* keep, int32_t B, int32_t H, int32_t N, 
                              reinterpret_cast<cudaStream_t>(stream));
 }
 
-int pcv_attn_fwd_partial_dropout_supported(const pcv_attn_params* p, float dropout_p) {
+static int partial_dropout_check(const pcv_attn_params* p, float dropout_p, bool shard) {
   if (validate_attn(p) != PCV_OK) return 0;
   const char* why = "";
-  const bool ok = partial_dropout_supported(*p, dropout_p, &why);
+  const bool ok = partial_dropout_supported(*p, dropout_p, shard, &why);
   if (!ok) set_error("one-pass dropout forward not applicable: %s", why);
   return ok ? 1 : 0;
 }
 
-int pcv_attn_fwd_partial_dropout(const pcv_attn_params* p, float dropout_p, uint64_t dropout_seed, void* stream) {
+static int partial_dropout_launch(const pcv_attn_params* p, float dropout_p, uint64_t dropout_seed, bool shard,
+                                  void* stream) {
   int rc = validate_attn(p);
   if (rc != PCV_OK) return rc;
   const char* why = "";
-  PCV_REQUIRE(partial_dropout_supported(*p, dropout_p, &why), PCV_ERR_UNSUPPORTED, "attn_fwd_partial_dropout: %s", why);
+  PCV_REQUIRE(partial_dropout_supported(*p, dropout_p, shard, &why), PCV_ERR_UNSUPPORTED,
+              "attn_fwd_partial_dropout: %s", why);
   const DropoutRule drop = dropout_rule(dropout_p, dropout_seed);
   return launch_attn_tc(*p, reinterpret_cast<cudaStream_t>(stream), nullptr, &drop);
+}
+
+int pcv_attn_fwd_partial_dropout_supported(const pcv_attn_params* p, float dropout_p) {
+  return partial_dropout_check(p, dropout_p, false);
+}
+
+int pcv_attn_fwd_partial_dropout(const pcv_attn_params* p, float dropout_p, uint64_t dropout_seed, void* stream) {
+  return partial_dropout_launch(p, dropout_p, dropout_seed, false, stream);
+}
+
+int pcv_attn_fwd_partial_dropout_shard_supported(const pcv_attn_params* p, float dropout_p) {
+  return partial_dropout_check(p, dropout_p, true);
+}
+
+int pcv_attn_fwd_partial_dropout_shard(const pcv_attn_params* p, float dropout_p, uint64_t dropout_seed, void* stream) {
+  return partial_dropout_launch(p, dropout_p, dropout_seed, true, stream);
 }
 
 }  // extern "C"

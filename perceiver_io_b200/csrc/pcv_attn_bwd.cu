@@ -49,7 +49,8 @@ struct BwdParams {
   int Npad, nq, nk;          // query rows padded to tiles, query tiles, key tiles
   int q_bcast;               // q has one batch row shared by all b (latents)
   float scale, scale_log2;
-  int causal, cshift;        // key masked for query n iff key > n + cshift   (cshift = M - N: right aligned)
+  int causal, cshift;        // local key j masked for query n iff j > n + cshift   (right aligned over all keys:
+                             // cshift = (m_total - N) - key_base)
   const uint32_t* pad_bits;  // (B, pad_wpr) bit set = padding key; nullptr if none
   int pad_wpr;
   const float* stats;        // (B, H, 2*nq) blocks of kStatsBytes (layout: see bwd_prep_kernel)
@@ -60,6 +61,7 @@ struct BwdParams {
   int wide_store;            // dk / dv rows are 32-byte aligned: 256-bit stores
   uint32_t drop_thresh;      // attention dropout: element kept iff its random byte >= drop_thresh (0 = no dropout)
   uint32_t seed_lo, seed_hi;
+  int key_base;              // global index of local key 0 (even; 0 unless key-sharded): the mask hashes key_base + j
   float drop_rp;             // 1 / (1 - drop_thresh / 256)
   float* o32;                // forward-with-dropout kernel: (B, N, H*dv) fp32 accumulation buffer
   int total_tiles;           // dkdv kernel: B*H*nk
@@ -296,10 +298,11 @@ bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq64, const __grid_constant_
           const bool oob = j >= p.M || n >= p.N;
           const bool filled = !oob && filled_key(p, b, j, n);
           float P = oob ? 0.f : (filled ? fillp : ex2(fmaf(st[4 * g + e4], p.scale_log2, nlse)));
+          const uint32_t jg = (uint32_t)(p.key_base + j);
           if constexpr (kDK) {
             float dP = dpt[4 * g + e4];
             if (p.drop_thresh) {
-              const bool keep = drop_keep(drop_bits(p.seed_lo, p.seed_hi, (uint32_t)bh, (uint32_t)n, (uint32_t)j), n, j, p.drop_thresh);
+              const bool keep = drop_keep(drop_bits(p.seed_lo, p.seed_hi, (uint32_t)bh, (uint32_t)n, jg), n, jg, p.drop_thresh);
               dP = keep ? dP * p.drop_rp : 0.f;
               pv[e4] = keep ? P * p.drop_rp : 0.f;
             } else {
@@ -309,7 +312,7 @@ bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq64, const __grid_constant_
           } else {
             (void)delta;  // the dV pass needs no dS
             if (p.drop_thresh) {
-              const bool keep = drop_keep(drop_bits(p.seed_lo, p.seed_hi, (uint32_t)bh, (uint32_t)n, (uint32_t)j), n, j, p.drop_thresh);
+              const bool keep = drop_keep(drop_bits(p.seed_lo, p.seed_hi, (uint32_t)bh, (uint32_t)n, jg), n, jg, p.drop_thresh);
               pv[e4] = keep ? P * p.drop_rp : 0.f;
             } else {
               pv[e4] = P;
@@ -480,8 +483,10 @@ bwd_dq_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CU
         const bool filled = !oob && filled_key(p, b, j, n);
         const float P = oob ? 0.f : (filled ? fillp[i] : ex2(fmaf(sc[4 * g + e4], p.scale_log2, nlse[i])));
         bool keep = true;
-        if (p.drop_thresh)
-          keep = drop_keep(drop_bits(p.seed_lo, p.seed_hi, (uint32_t)bh, (uint32_t)n, (uint32_t)j), n, j, p.drop_thresh);
+        if (p.drop_thresh) {
+          const uint32_t jg = (uint32_t)(p.key_base + j);
+          keep = drop_keep(drop_bits(p.seed_lo, p.seed_hi, (uint32_t)bh, (uint32_t)n, jg), n, jg, p.drop_thresh);
+        }
         if constexpr (FWD) {
           val[e4] = keep ? P * p.drop_rp : 0.f;
         } else {
@@ -651,8 +656,10 @@ bwd_dq64_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
           const bool filled = !oob && filled_key(p, b, j, n);
           const float P = oob ? 0.f : (filled ? fillp : ex2(fmaf(sc[4 * g + e4], p.scale_log2, nlse)));
           bool keep = true;
-          if (p.drop_thresh)
-            keep = drop_keep(drop_bits(p.seed_lo, p.seed_hi, (uint32_t)bh, (uint32_t)n, (uint32_t)j), n, j, p.drop_thresh);
+          if (p.drop_thresh) {
+            const uint32_t jg = (uint32_t)(p.key_base + j);
+            keep = drop_keep(drop_bits(p.seed_lo, p.seed_hi, (uint32_t)bh, (uint32_t)n, jg), n, jg, p.drop_thresh);
+          }
           const float dP = keep ? dp[4 * g + e4] * p.drop_rp : 0.f;
           val[e4] = (oob || filled) ? 0.f : P * (dP - delta);
         }
@@ -763,10 +770,13 @@ BwdLayout bwd_layout(int B, int H, int N, int M, bool pad, size_t acc_bytes) {
   return L;
 }
 
-BwdLayout bwd_layout(const pcv_attn_bwd_params& a) {
+// shard != nullptr: a key shard's backward, whose dQ kernel up to head dim 128 accumulates straight into the caller's
+// fp32 grad_q32 (no accumulator in the workspace)
+BwdLayout bwd_layout(const pcv_attn_bwd_params& a, const pcv_key_shard* shard) {
   const int Bq = a.q_stride_b == 0 ? 1 : a.B;
   const size_t dq_bytes = sizeof(float) * (size_t)Bq * a.N * a.H * a.dqk;
-  if (!wide_bwd(a.dqk, a.dv)) return bwd_layout(a.B, a.H, a.N, a.M, a.pad_mask != nullptr, dq_bytes);
+  if (!wide_bwd(a.dqk, a.dv))
+    return bwd_layout(a.B, a.H, a.N, a.M, a.pad_mask != nullptr, shard != nullptr ? 0 : dq_bytes);
   BwdLayout L = bwd_layout(a.B, a.H, a.N, a.M, a.pad_mask != nullptr, 0);
   dq_split(a.B * a.H * L.nq, L.nk, kWideSplitSms, L.dq_tiles_per_split, L.dq_splits);
   L.dq_parts = (Bq == 1 ? a.B : 1) * L.dq_splits;  // a batch-1 q receives one contribution per batch row and split
@@ -794,10 +804,12 @@ struct BwdMaps {
 
 // The host steps the backward and the dropout forward share; A is pcv_attn_bwd_params or pcv_attn_params, which name
 // the q / k / v operands alike.  Fills the BwdParams core and the dq-kernel split, zeroes the fp32 accumulator, writes
-// the row statistics, packs the pad mask and encodes the q / k / v tensor maps.
+// the row statistics, packs the pad mask and encodes the q / k / v tensor maps.  The call's keys are [m_offset,
+// m_offset + M) of m_total (the causal diagonal and the dropout hash use global key indices).
 template <class A>
 int bwd_setup(const A& a, const BwdLayout& L, const float* stat_m, const float* stat_l, const DeltaOperands& d,
-              float dropout_p, uint64_t seed, cudaStream_t stream, BwdParams& p, BwdMaps& m, int& sms) {
+              float dropout_p, uint64_t seed, int m_total, int m_offset, cudaStream_t stream, BwdParams& p, BwdMaps& m,
+              int& sms) {
   int dev = 0;
   PCV_CHECK_CUDA(cudaGetDevice(&dev));
   PCV_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
@@ -811,7 +823,8 @@ int bwd_setup(const A& a, const BwdLayout& L, const float* stat_m, const float* 
   p.scale = a.scale;
   p.scale_log2 = a.scale * kLog2e;
   p.causal = a.causal;
-  p.cshift = a.M - a.N;
+  p.cshift = (m_total - a.N) - m_offset;
+  p.key_base = m_offset;
   p.stats = reinterpret_cast<const float*>(ws);
   set_dropout(p, dropout_p, seed);
   if (L.dq_splits > 0) {
@@ -917,14 +930,17 @@ int launch_cast(bool bf16, const float* acc, void* dst, int Bq, int N, int H, in
   return PCV_OK;
 }
 
-// the wide backward's dQ partials, summed in order -> dq with its own strides
-int launch_sum_dq(bool bf16, const float* part, int nparts, void* dst, int Bq, int N, int H, int dqk, int64_t sb,
+// the wide backward's dQ partials, summed in order -> dq (dtype: bf16, fp16 or fp32) with its own strides
+int launch_sum_dq(int dtype, const float* part, int nparts, void* dst, int Bq, int N, int H, int dqk, int64_t sb,
                   int64_t sn, int64_t sh, cudaStream_t stream) {
   const int64_t total = (int64_t)Bq * N * H * dqk;
   const int blocks = (int)std::min<int64_t>((total + 255) / 256, 4096);
-  if (bf16)
+  if (dtype == PCV_BF16)
     bwd_sum_dq_kernel<__nv_bfloat16><<<blocks, 256, 0, stream>>>(part, nparts, reinterpret_cast<__nv_bfloat16*>(dst), Bq,
                                                                  N, H, dqk, sb, sn, sh);
+  else if (dtype == PCV_F32)
+    bwd_sum_dq_kernel<float><<<blocks, 256, 0, stream>>>(part, nparts, reinterpret_cast<float*>(dst), Bq, N, H, dqk, sb,
+                                                         sn, sh);
   else
     bwd_sum_dq_kernel<__half><<<blocks, 256, 0, stream>>>(part, nparts, reinterpret_cast<__half*>(dst), Bq, N, H, dqk, sb,
                                                           sn, sh);
@@ -935,13 +951,22 @@ int launch_sum_dq(bool bf16, const float* part, int nparts, void* dst, int Bq, i
 
 }  // namespace
 
-bool attn_bwd_supported(const pcv_attn_bwd_params& a, const char** why) {
+bool attn_bwd_supported(const pcv_attn_bwd_params& a, const pcv_key_shard* shard, const char** why) {
   auto no = [&](const char* w) {
     if (why) *why = w;
     return false;
   };
   if (a.dtype != PCV_BF16 && a.dtype != PCV_F16) return no("dtype must be bf16 or fp16");
   if (a.B < 1 || a.H < 1 || a.N < 1 || a.M < 1) return no("empty problem");
+  if (shard != nullptr) {
+    if (shard->grad_q32 == nullptr) return no("key shard: grad_q32 is NULL");
+    if (!al16(shard->grad_q32)) return no("key shard: grad_q32 must be 16-byte aligned");
+    if (shard->m_offset < 0 || (int64_t)shard->m_offset + a.M > shard->m_total)
+      return no("key shard: keys [m_offset, m_offset + M) outside m_total");
+    // the dropout hash covers key pairs (k >> 1): an odd base would pair a shard's keys differently from the mask
+    if (shard->m_offset % 2) return no("key shard: m_offset must be even");
+    if (a.causal && shard->m_total < a.N) return no("key shard: causal attention needs m_total >= N");
+  }
   if (a.dqk < 8 || a.dv < 8) return no("head dims must be in [8, 192]");
   if (a.dqk % 8 || a.dv % 8) return no("head dims must be multiples of 8");
   if (a.dqk > 192 || a.dv > 192) return no("head dims must be in [8, 192]");
@@ -959,17 +984,17 @@ bool attn_bwd_supported(const pcv_attn_bwd_params& a, const char** why) {
   return true;
 }
 
-int attn_bwd_workspace_bytes(const pcv_attn_bwd_params& a, size_t* bytes) {
+int attn_bwd_workspace_bytes(const pcv_attn_bwd_params& a, const pcv_key_shard* shard, size_t* bytes) {
   PCV_REQUIRE(bytes != nullptr, PCV_ERR_INVALID, "attn_bwd_workspace_bytes: bytes is NULL");
-  *bytes = bwd_layout(a).total;
+  *bytes = bwd_layout(a, shard).total;
   return PCV_OK;
 }
 
-int launch_attn_bwd(const pcv_attn_bwd_params& a, cudaStream_t stream) {
+int launch_attn_bwd(const pcv_attn_bwd_params& a, const pcv_key_shard* shard, cudaStream_t stream) {
   const char* why = "";
-  PCV_REQUIRE(attn_bwd_supported(a, &why), PCV_ERR_UNSUPPORTED, "attn_bwd: %s", why);
+  PCV_REQUIRE(attn_bwd_supported(a, shard, &why), PCV_ERR_UNSUPPORTED, "attn_bwd: %s", why);
   PCV_REQUIRE(a.stat_m != nullptr && a.stat_l != nullptr, PCV_ERR_INVALID, "attn_bwd: forward statistics are NULL");
-  const BwdLayout L = bwd_layout(a);
+  const BwdLayout L = bwd_layout(a, shard);
   PCV_REQUIRE(a.workspace != nullptr && a.workspace_bytes >= L.total, PCV_ERR_INVALID,
               "attn_bwd: workspace too small (%zu < %zu)", a.workspace_bytes, L.total);
   PCV_REQUIRE((reinterpret_cast<uintptr_t>(a.workspace) & 255u) == 0, PCV_ERR_INVALID,
@@ -979,10 +1004,16 @@ int launch_attn_bwd(const pcv_attn_bwd_params& a, cudaStream_t stream) {
   BwdParams p{};
   BwdMaps m;
   int sms = 0;
-  int rc = bwd_setup(a, L, a.stat_m, a.stat_l, d, a.dropout_p, a.dropout_seed, stream, p, m, sms);
+  const int m_total = shard != nullptr ? shard->m_total : a.M, m_offset = shard != nullptr ? shard->m_offset : 0;
+  int rc = bwd_setup(a, L, a.stat_m, a.stat_l, d, a.dropout_p, a.dropout_seed, m_total, m_offset, stream, p, m, sms);
   if (rc != PCV_OK) return rc;
   const bool wide = wide_bwd(a.dqk, a.dv);
+  const int Bq = a.q_stride_b == 0 ? 1 : a.B;
   p.dq32 = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(a.workspace) + (wide ? L.off_part : L.off_acc));
+  if (shard != nullptr && !wide) {  // the dQ kernel reduces straight into the caller's fp32 contribution
+    p.dq32 = shard->grad_q32;
+    PCV_CHECK_CUDA(cudaMemsetAsync(p.dq32, 0, sizeof(float) * (size_t)Bq * a.N * a.H * a.dqk, stream));
+  }
   p.dk = a.grad_k; p.dv_out = a.grad_v;
   p.dk_sb = a.gk_stride_b; p.dk_sm = a.gk_stride_m; p.dk_sh = a.gk_stride_h;
   p.dv_sb = a.gv_stride_b; p.dv_sm = a.gv_stride_m; p.dv_sh = a.gv_stride_h;
@@ -994,7 +1025,6 @@ int launch_attn_bwd(const pcv_attn_bwd_params& a, cudaStream_t stream) {
     p.wide_store = wide ? 1 : 0;
   }
 
-  const int Bq = a.q_stride_b == 0 ? 1 : a.B;
   rc = make_tmap_4d(&m.dout, a.grad_out, a.dtype, a.dv, a.N, a.H, a.B, a.go_stride_n, a.go_stride_h, a.go_stride_b, kT);
   if (rc != PCV_OK) return rc;
   rc = make_tmap_4d(&m.q64, a.q, a.dtype, a.dqk, a.N, a.H, Bq, a.q_stride_n, a.q_stride_h, a.q_stride_b, 64);
@@ -1010,11 +1040,14 @@ int launch_attn_bwd(const pcv_attn_bwd_params& a, cudaStream_t stream) {
     if (rc != PCV_OK) return rc;
     rc = bf16 ? launch_wide<true>(m, p, sms, stream) : launch_wide<false>(m, p, sms, stream);
     if (rc != PCV_OK) return rc;
-    return launch_sum_dq(bf16, p.dq32, L.dq_parts, a.grad_q, Bq, a.N, a.H, a.dqk, a.gq_stride_b, a.gq_stride_n,
+    if (shard != nullptr)  // the same fixed-order sum, kept in fp32: (Bq, N, H*dqk) dense
+      return launch_sum_dq(PCV_F32, p.dq32, L.dq_parts, shard->grad_q32, Bq, a.N, a.H, a.dqk,
+                           (int64_t)a.N * a.H * a.dqk, (int64_t)a.H * a.dqk, a.dqk, stream);
+    return launch_sum_dq(a.dtype, p.dq32, L.dq_parts, a.grad_q, Bq, a.N, a.H, a.dqk, a.gq_stride_b, a.gq_stride_n,
                          a.gq_stride_h, stream);
   }
   rc = bf16 ? launch_tc<true>(false, m, p, sms, stream) : launch_tc<false>(false, m, p, sms, stream);
-  if (rc != PCV_OK) return rc;
+  if (rc != PCV_OK || shard != nullptr) return rc;
   return launch_cast(bf16, p.dq32, a.grad_q, Bq, a.N, a.H, a.dqk, a.gq_stride_b, a.gq_stride_n, a.gq_stride_h, stream);
 }
 
@@ -1060,7 +1093,7 @@ int launch_attn_fwd_dropout(const pcv_attn_params& a, const float* stat_m, const
   BwdMaps m;
   int sms = 0;
   // statistics only (no delta): out / grad_out are not read
-  int rc = bwd_setup(a, L, stat_m, stat_l, DeltaOperands{}, dropout_p, seed, stream, p, m, sms);
+  int rc = bwd_setup(a, L, stat_m, stat_l, DeltaOperands{}, dropout_p, seed, a.M, 0, stream, p, m, sms);
   if (rc != PCV_OK) return rc;
   p.o32 = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(a.workspace) + L.off_acc);
   const bool bf16 = a.dtype == PCV_BF16;

@@ -95,6 +95,7 @@ struct TcParams {
   int slot_rows;
   PeerTail tail;
   DropoutRule drop;  // attn_fwd_drop_kernel only; last, so that the other kernels' parameter offsets do not move
+  int drop_key_base; // attn_fwd_drop_kernel: global index of local key 0 (m_offset, even); the mask hashes it + j
 };
 
 // --------------------------------------------------------------------------------------------------
@@ -329,7 +330,7 @@ __device__ __forceinline__ void tile_softmax(float (&s)[64], float (&m_run)[2], 
     l_run[0] += e0 + e1;
     l_run[1] += e2 + e3;
     if constexpr (DROP) {
-      const uint32_t jb = (uint32_t)(j0 + 8 * g + cq), n = (uint32_t)n0;
+      const uint32_t jb = (uint32_t)(p.drop_key_base + j0 + 8 * g + cq), n = (uint32_t)n0;
       const uint32_t ks = drop_kside(p.drop.seed_hi, jb);
       const uint32_t x0 = drop_finish(qside[0], ks), x1 = drop_finish(qside[1], ks);
       if (!drop_keep(x0, n, jb, p.drop.thresh)) e0 = 0.f;
@@ -1055,8 +1056,9 @@ int launch_attn_tc(const pcv_attn_params& a, cudaStream_t stream, const pcv_shar
     PCV_REQUIRE(attn_tc_supported(a, &why), PCV_ERR_UNSUPPORTED, "tensor-core attention: %s", why);
   }
   PCV_REQUIRE(drop == nullptr || (fuse == nullptr && a.write_partial && a.impl != PCV_IMPL_TCGEN05_PAIR &&
-                                  a.m_total == a.M && a.m_offset == 0 && drop->thresh > 0),
-              PCV_ERR_UNSUPPORTED, "tensor-core attention: dropout needs a partial-state call over all keys, no CTA pair");
+                                  a.m_offset % 2 == 0 && drop->thresh > 0),
+              PCV_ERR_UNSUPPORTED,
+              "tensor-core attention: dropout needs a partial-state call starting at an even key, no CTA pair");
   std::shared_ptr<Plan> pl;
   const Mode mode = choose_mode(a);
   if (mode.pair) {
@@ -1091,7 +1093,10 @@ int launch_attn_tc(const pcv_attn_params& a, cudaStream_t stream, const pcv_shar
   p.rows_per_unit = mode.rows_per_unit;
   p.slot_rows = mode.slot_rows;
   p.fin_o = a.part_o; p.fin_m = a.part_m; p.fin_l = a.part_l;
-  if (drop != nullptr) p.drop = *drop;
+  if (drop != nullptr) {
+    p.drop = *drop;
+    p.drop_key_base = a.m_offset;
+  }
   if (fuse != nullptr) {
     const char* why = "";
     PCV_REQUIRE(attn_tc_fuse_supported(a, &why), PCV_ERR_UNSUPPORTED, "fused merge: %s", why);

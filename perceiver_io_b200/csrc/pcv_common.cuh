@@ -58,6 +58,10 @@ template <> struct Elem<__half> {
   static __device__ __forceinline__ __half from_f(float x) { return __float2half_rn(x); }
   static __device__ __forceinline__ float2 to_f2(__half2 x) { return __half22float2(x); }
 };
+template <> struct Elem<float> {  // fp32 outputs (a key shard's grad_q contribution)
+  static __device__ __forceinline__ float to_f(float x) { return x; }
+  static __device__ __forceinline__ float from_f(float x) { return x; }
+};
 
 __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
@@ -82,7 +86,8 @@ int attn_simt_workspace_bytes(const pcv_attn_params& p, size_t* bytes);
 
 struct DropoutRule;  // pcv_dropout.cuh
 bool attn_tc_supported(const pcv_attn_params& p, const char** why);
-// drop != nullptr: the one-pass dropout forward (attn_fwd_drop_kernel; partial state over all keys, no fuse, no pair)
+// drop != nullptr: the one-pass dropout forward (attn_fwd_drop_kernel; partial state, no fuse, no pair; the mask takes
+// global key indices, so a key shard must start at an even m_offset)
 int launch_attn_tc(const pcv_attn_params& p, cudaStream_t stream, const pcv_shard_fuse* fuse = nullptr,
                    const DropoutRule* drop = nullptr);
 bool attn_tc_fuse_supported(const pcv_attn_params& p, const char** why);
@@ -108,9 +113,10 @@ int launch_kv_append(const pcv_kv_append_params& p, cudaStream_t stream);
 int launch_ln_stats(const pcv_ln_stats_params& p, cudaStream_t stream);
 bool kv_project_supported(const pcv_kvproj_params& p, const char** why);
 int launch_kv_project(const pcv_kvproj_params& p, cudaStream_t stream);
-bool attn_bwd_supported(const pcv_attn_bwd_params& p, const char** why);
-int attn_bwd_workspace_bytes(const pcv_attn_bwd_params& p, size_t* bytes);
-int launch_attn_bwd(const pcv_attn_bwd_params& p, cudaStream_t stream);
+// shard == nullptr: the backward over all keys (pcv_attn_bwd); else one key shard's (pcv_attn_bwd_shard)
+bool attn_bwd_supported(const pcv_attn_bwd_params& p, const pcv_key_shard* shard, const char** why);
+int attn_bwd_workspace_bytes(const pcv_attn_bwd_params& p, const pcv_key_shard* shard, size_t* bytes);
+int launch_attn_bwd(const pcv_attn_bwd_params& p, const pcv_key_shard* shard, cudaStream_t stream);
 bool attn_fwd_dropout_supported(const pcv_attn_params& p, float dropout_p, const char** why);
 int attn_fwd_dropout_workspace_bytes(const pcv_attn_params& p, size_t* bytes);
 int launch_attn_fwd_dropout(const pcv_attn_params& p, const float* stat_m, const float* stat_l, float dropout_p,

@@ -108,12 +108,59 @@ def _cuda_finalize(po, pl, out_dtype):
     return ops.combine_partials(po[None], torch.zeros_like(pl)[None], pl[None], out_dtype)
 
 
+def _cuda_partial_dropout(q, k, v, num_heads, scale, pad_mask, causal, m_total, m_offset, out, dropout_p, dropout_seed):
+    """The one-pass dropout forward on the local keys (global key indices in the mask).  Head dims that are not
+    multiples of 8 are zero-padded, which changes neither the scores nor the mask."""
+    from . import ops
+
+    dv = ops._head_dim(v, num_heads)
+    if ops._head_dim(q, num_heads) % 8 == 0 and dv % 8 == 0:
+        ops.attention_partial(q, k, v, num_heads, scale, pad_mask=pad_mask, causal=causal, m_total=m_total,
+                              m_offset=m_offset, out=out, dropout_p=dropout_p, dropout_seed=dropout_seed)
+        return
+    qp, kp, vp = (ops._pad_heads_to8(t, num_heads) for t in (q, k, v))
+    po, pm, pl = ops.attention_partial(qp, kp, vp, num_heads, scale, pad_mask=pad_mask, causal=causal, m_total=m_total,
+                                       m_offset=m_offset, dropout_p=dropout_p, dropout_seed=dropout_seed)
+    out[0].copy_(po[..., :dv])
+    out[1].copy_(pm)
+    out[2].copy_(pl)
+
+
+def _cuda_backward(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask, causal, m_total, m_offset,
+                   dropout_p, dropout_seed):
+    """-> (grad_q32, grad_k, grad_v) of one key shard: the backward kernels (``ops.attention_backward_shard``) where
+    they cover the call, else (head dims above 192, 4-D operands) the torch shim with the key offset.
+    ``ops.backward_config["impl"]`` selects as for the unsharded backward."""
+    from . import _lib, ops
+
+    mode = ops.backward_config["impl"]
+    if mode not in ("auto", "kernel", "shim"):
+        raise ValueError(f"backward_config['impl'] = {mode!r}")
+    if mode != "shim":
+        if q.dim() == 3 and k.dim() == 3 and v.dim() == 3:
+            grads = ops._backward_shard(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, m_total, m_offset,
+                                        pad_mask, causal, dropout_p, dropout_seed, "try")
+            if grads is not None:
+                return grads
+        if mode == "kernel":
+            raise RuntimeError("backward_config['impl'] = 'kernel' but pcv_attn_bwd_shard does not cover this call: "
+                               + _lib.lib().pcv_last_error().decode())
+    return ops._backward_shim(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask, causal, dropout_p,
+                              dropout_seed, m_total, m_offset)
+
+
 @dataclass
 class ShardKernels:
-    """Device math of the sharded path; the defaults are the sm_100a kernels."""
+    """Device math of the sharded path; the defaults are the sm_90a kernels.
+
+    ``partial_dropout`` is ``partial`` with two more arguments (dropout_p, dropout_seed); ``backward`` maps (q, k_shard,
+    v_shard, out, grad_out, m_glob, l_glob, num_heads, scale, pad_mask_shard, causal, m_total, m_offset, dropout_p,
+    dropout_seed) to (grad_q32, grad_k, grad_v), grad_q32 being the shard's fp32 contribution to grad_q."""
     partial: Callable = _cuda_partial
     rescale_: Callable = _cuda_rescale
     finalize: Callable = _cuda_finalize
+    partial_dropout: Callable = _cuda_partial_dropout
+    backward: Callable = _cuda_backward
 
 
 class PeerMerger:
@@ -227,18 +274,118 @@ def _peer_merge_possible(t: torch.Tensor, world: int) -> bool:
     return True
 
 
+def _shared_dropout_seed(group, device) -> int:
+    """A fresh dropout seed drawn on the group's first rank and broadcast (8 bytes), so that every shard drops with
+    the same mask."""
+    from . import ops
+
+    seed = torch.tensor([ops.new_dropout_seed()], dtype=torch.int64, device=device)
+    if dist.is_initialized() and dist.get_world_size(group) > 1:
+        g = group if group is not None else dist.group.WORLD
+        dist.broadcast(seed, src=dist.get_global_rank(g, 0), group=g)
+    return int(seed.item())
+
+
+def _exact_merge(q, k_shard, v_shard, num_heads, scale, m_total, m_offset, pad_mask_shard, causal, group, kernels,
+                 dropout_p, dropout_seed):
+    """The exact merge over torch.distributed collectives: the local partial state, MAX all-reduce of the row maxima,
+    rescale, ONE packed SUM all-reduce of [numerator | denominator].  -> (out, m_glob, l_glob): the normalised output
+    and the row statistics over all m_total keys, on every rank."""
+    B, M_local = k_shard.shape[0], k_shard.shape[1]
+    N = q.shape[1]
+    dv = v_shard.shape[2] // num_heads if v_shard.dim() == 3 else v_shard.shape[3]
+    rows = B * num_heads * N
+    if M_local == 0:
+        raise ValueError("every rank must own at least one key (shard_bounds guarantees it for M >= world*align)")
+    # one allocation so that numerator and denominator ride the same all-reduce
+    flat = torch.empty(rows * dv + rows, dtype=torch.float32, device=k_shard.device)
+    po = flat[: rows * dv].view(B, num_heads, N, dv)
+    pl = flat[rows * dv:].view(B, num_heads, N)
+    pm = torch.empty(B, num_heads, N, dtype=torch.float32, device=k_shard.device)
+    if dropout_p > 0.0:
+        kernels.partial_dropout(q, k_shard, v_shard, num_heads, scale, pad_mask_shard, causal, m_total, m_offset,
+                                (po, pm, pl), dropout_p, dropout_seed)
+    else:
+        kernels.partial(q, k_shard, v_shard, num_heads, scale, pad_mask_shard, causal, m_total, m_offset, (po, pm, pl))
+    world = dist.get_world_size(group) if dist.is_initialized() else 1
+    m_glob = pm
+    if world > 1:
+        m_glob = pm.clone()
+        dist.all_reduce(m_glob, op=dist.ReduceOp.MAX, group=group)
+        kernels.rescale_(po, pm, pl, m_glob)
+        dist.all_reduce(flat, op=dist.ReduceOp.SUM, group=group)
+    return kernels.finalize(po, pl, q.dtype), m_glob, pl
+
+
+class _ShardedAttention(torch.autograd.Function):
+    """Training through the key-sharded attention.  Forward: the exact merge (``_exact_merge``), keeping the merged row
+    statistics.  Backward: the shard backward from those statistics (``ShardKernels.backward``) — dK / dV of the local
+    keys are complete — and ONE all_reduce(SUM) of the fp32 dQ contributions over the group."""
+
+    @staticmethod
+    def forward(ctx, q, k_shard, v_shard, num_heads, scale, m_total, m_offset, pad_mask_shard, causal, group, kernels,
+                dropout_p, dropout_seed):
+        out, m_glob, l_glob = _exact_merge(q, k_shard, v_shard, num_heads, scale, m_total, m_offset, pad_mask_shard,
+                                           causal, group, kernels, dropout_p, dropout_seed)
+        ctx.save_for_backward(q, k_shard, v_shard, pad_mask_shard, out, m_glob, l_glob)
+        ctx.meta = (num_heads, scale, m_total, m_offset, causal, group, kernels, dropout_p, dropout_seed)
+        return out
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        q, k, v, pad, out, m_glob, l_glob = ctx.saved_tensors
+        H, scale, m_total, m_offset, causal, group, kernels, dropout_p, dropout_seed = ctx.meta
+        gq, gk, gv = kernels.backward(q, k, v, out, grad_out, m_glob, l_glob, H, scale, pad, causal, m_total, m_offset,
+                                      dropout_p, dropout_seed)
+        gq = gq.float().contiguous()
+        if dist.is_initialized() and dist.get_world_size(group) > 1:
+            dist.all_reduce(gq, op=dist.ReduceOp.SUM, group=group)
+        return (gq.to(q.dtype), gk.to(k.dtype), gv.to(v.dtype)) + (None,) * 10
+
+
 def sharded_attention(q: torch.Tensor, k_shard: torch.Tensor, v_shard: torch.Tensor, num_heads: int, scale: float,
                       m_total: int, m_offset: int, pad_mask_shard: Optional[torch.Tensor] = None,
                       causal: bool = False, group=None, kernels: Optional[ShardKernels] = None,
-                      merge: str = "auto", copy_out: bool = True) -> torch.Tensor:
+                      merge: str = "auto", copy_out: bool = True, dropout_p: float = 0.0,
+                      dropout_seed: Optional[int] = None) -> torch.Tensor:
     """softmax(QK^T)V with K/V sharded along M over ``group``; every rank returns the full (B,N,H*dv).
 
     ``merge``: "fused" (ONE launch per rank: the merge runs in the attention kernel's tail over NVLink-mapped
     symmetric memory, no host-launched barrier, no NCCL), "peer" (partial-state kernel, signal-pad barrier, separate
     merge kernel, barrier), "nccl" (two all-reduces) or "auto" (fused when the kernel family covers the shapes and all
     shards are equally long, else peer, else nccl).  With the fused / peer merge the result lives in a reused symmetric
-    buffer; ``copy_out=False`` returns that buffer itself (valid until the next call)."""
+    buffer; ``copy_out=False`` returns that buffer itself (valid until the next call).
+
+    Training: under autograd (grad enabled and q, k_shard or v_shard requiring grad) the call is differentiable.  Only
+    the "nccl" merge leaves the merged row statistics on every rank, so "auto" selects it and "fused" / "peer" raise.
+    An inference call made with grad enabled on operands that require grad (e.g. projected by parameters that require
+    grad) is such a training call: run inference under ``torch.no_grad()`` to keep the fused merge.
+    The backward computes dK / dV of the local keys locally and sums the dQ contributions with ONE fp32 all-reduce
+    (B or 1, N, H*dqk floats) over the group — no other communication.  Every rank of the group must pass the SAME
+    ``grad_out``: true when everything downstream is replicated, as after ``cross_attention_sharded``.
+
+    ``dropout_p`` > 0 applies the attention-probability dropout (reference modules.py:161) with the mask of the
+    unsharded call over global key indices (``m_offset`` must be even; ``shard_bounds`` gives 128-aligned offsets).  The
+    seed must be identical on every rank of the group, else the gradients are silently wrong: ``dropout_seed=None``
+    draws one on the group's first rank and broadcasts it (one 8-byte collective and one host read per call); a
+    given seed is used as is."""
     world_now = dist.get_world_size(group) if dist.is_initialized() else 1
+    train = torch.is_grad_enabled() and (q.requires_grad or k_shard.requires_grad or v_shard.requires_grad)
+    if train or dropout_p > 0.0:
+        if dropout_p > 0.0 and not 0.0 < dropout_p < 1.0:
+            raise ValueError(f"dropout_p must be in [0, 1), got {dropout_p}")
+        if merge not in ("auto", "nccl"):
+            raise RuntimeError(f"sharded_attention: merge={merge!r} cannot be used for training or dropout: only the "
+                               "'nccl' merge leaves the merged row statistics (and the dropout forward) on every rank")
+        kernels = kernels or ShardKernels()
+        seed = 0
+        if dropout_p > 0.0:
+            seed = _shared_dropout_seed(group, k_shard.device) if dropout_seed is None else int(dropout_seed)
+        if train:
+            return _ShardedAttention.apply(q, k_shard, v_shard, num_heads, scale, m_total, m_offset, pad_mask_shard,
+                                           causal, group, kernels, float(dropout_p), seed)
+        return _exact_merge(q, k_shard, v_shard, num_heads, scale, m_total, m_offset, pad_mask_shard, causal, group,
+                            kernels, float(dropout_p), seed)[0]
     merge_requested = merge
     if merge == "auto":
         merge = "fused" if (kernels is None and not PeerMerger.disabled and _peer_merge_possible(k_shard, world_now)) else "nccl"
@@ -284,26 +431,8 @@ def sharded_attention(q: torch.Tensor, k_shard: torch.Tensor, v_shard: torch.Ten
         out = pm.merge()
         out = out.clone() if copy_out else out
         return out if out.dtype == q.dtype else out.to(q.dtype)
-    kernels = kernels or ShardKernels()
-    B, M_local = k_shard.shape[0], k_shard.shape[1]
-    N = q.shape[1]
-    dv = v_shard.shape[2] // num_heads
-    rows = B * num_heads * N
-    if M_local == 0:
-        raise ValueError("every rank must own at least one key (shard_bounds guarantees it for M >= world*align)")
-    # one allocation so that numerator and denominator ride the same all-reduce
-    flat = torch.empty(rows * dv + rows, dtype=torch.float32, device=k_shard.device)
-    po = flat[: rows * dv].view(B, num_heads, N, dv)
-    pl = flat[rows * dv:].view(B, num_heads, N)
-    pm = torch.empty(B, num_heads, N, dtype=torch.float32, device=k_shard.device)
-    kernels.partial(q, k_shard, v_shard, num_heads, scale, pad_mask_shard, causal, m_total, m_offset, (po, pm, pl))
-    world = dist.get_world_size(group) if dist.is_initialized() else 1
-    if world > 1:
-        m_glob = pm.clone()
-        dist.all_reduce(m_glob, op=dist.ReduceOp.MAX, group=group)
-        kernels.rescale_(po, pm, pl, m_glob)
-        dist.all_reduce(flat, op=dist.ReduceOp.SUM, group=group)
-    return kernels.finalize(po, pl, q.dtype)
+    return _exact_merge(q, k_shard, v_shard, num_heads, scale, m_total, m_offset, pad_mask_shard, causal, group,
+                        kernels or ShardKernels(), 0.0, 0)[0]
 
 
 def cross_attention_sharded(module, x_q: torch.Tensor, x_kv_shard: torch.Tensor, m_total: int, m_offset: int,
@@ -313,7 +442,13 @@ def cross_attention_sharded(module, x_q: torch.Tensor, x_kv_shard: torch.Tensor,
 
     ``module`` is a CrossAttention (this package's or a patched reference one).  LayerNorm and the K/V
     projections run on the local shard only — they are 2/3 of the module's FLOPs and shard perfectly —
-    then the attention core is merged across ranks and ``o_proj`` is applied replicated."""
+    then the attention core is merged across ranks and ``o_proj`` is applied replicated.
+
+    Training: in training mode the module's attention dropout is applied (one seed per call, broadcast from the group's
+    first rank), and the call is differentiable (``sharded_attention``).  After ``loss.backward()`` the q-side and
+    replicated parameters hold their full gradient on every rank; the parameters that saw only the local shard
+    (kv_norm, k_proj, v_proj and whatever produced ``x_kv_shard``) hold the local share: sum it with
+    ``reduce_shard_grads``."""
     from .utils import ModuleOutput
 
     from .modules import fused_linear, project_kv
@@ -321,6 +456,20 @@ def cross_attention_sharded(module, x_q: torch.Tensor, x_kv_shard: torch.Tensor,
     attn = module.attention
     q = fused_linear(module, "_pcv_q_fold", module.q_norm, attn.q_proj, x_q)
     k, v = project_kv(module, x_kv_shard)  # fused LayerNorm + K/V producer on the local shard
+    drop_p = float(attn.dropout.p) if module.training else 0.0
     o = sharded_attention(q, k, v, attn.num_heads, attn.dp_scale, m_total, m_offset, pad_mask_shard,
-                          attn.causal_attention, group, kernels, merge=merge)
+                          attn.causal_attention, group, kernels, merge=merge, dropout_p=drop_p)
     return ModuleOutput(last_hidden_state=fused_linear(attn, "_pcv_o_fold", None, attn.o_proj, o), kv_cache=None)
+
+
+def reduce_shard_grads(parameters, group=None) -> None:
+    """Sum in place, over ``group``, the ``.grad`` of parameters whose forward saw only the local key shard:
+    kv_norm / k_proj / v_proj of a ``cross_attention_sharded`` module and an input adapter run on the shard.  The
+    q-side and replicated parameters already hold the full gradient on every rank and must NOT be passed.  Every rank
+    must pass the same parameters in the same order (one all-reduce each; parameters without a gradient are skipped on
+    every rank alike).  Wiring into DDP / FSDP (which would average over the batch groups too) is left to the caller."""
+    if not dist.is_initialized() or dist.get_world_size(group) == 1:
+        return
+    for p in parameters:
+        if p.grad is not None:
+            dist.all_reduce(p.grad, op=dist.ReduceOp.SUM, group=group)

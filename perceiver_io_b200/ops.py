@@ -182,7 +182,9 @@ backward_config = {"max_score_bytes": 1 << 30, "impl": "auto"}
 
 
 def _fill_bwd_params(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask, causal, dropout_p=0.0,
-                     dropout_seed=0):
+                     dropout_seed=0, with_grad_q=True):
+    """Backward parameters and the (grad_q, grad_k, grad_v) outputs; ``with_grad_q=False`` (a key shard, which writes an
+    fp32 contribution instead) allocates no grad_q and leaves its pointer NULL."""
     ap, keep = _fill_attn_params(q, k, v, num_heads, scale, pad_mask, causal, None, 0, "auto")
     B, H, N, M, dqk, dv = ap.B, ap.H, ap.N, ap.M, ap.dqk, ap.dv
     for name, t in (("out", out), ("grad_out", grad_out)):
@@ -192,19 +194,20 @@ def _fill_bwd_params(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, p
         if tuple(t.shape) != (B, H, N) or t.dtype != torch.float32 or not t.is_contiguous():
             raise ValueError(f"{name} must be a contiguous float32 (B, H, N) tensor")
     Bq = q.shape[0]
-    gq = torch.empty(Bq, N, H * dqk, dtype=q.dtype, device=q.device)
+    gq = torch.empty(Bq, N, H * dqk, dtype=q.dtype, device=q.device) if with_grad_q else None
     gk = torch.empty(B, M, H * dqk, dtype=q.dtype, device=q.device)
     gv = torch.empty(B, M, H * dv, dtype=q.dtype, device=q.device)
     p = _lib.AttnBwdParams()
     p.q, p.k, p.v, p.out, p.grad_out = ap.q, ap.k, ap.v, out.data_ptr(), grad_out.data_ptr()
     p.stat_m, p.stat_l = stat_m.data_ptr(), stat_l.data_ptr()
-    p.grad_q, p.grad_k, p.grad_v = gq.data_ptr(), gk.data_ptr(), gv.data_ptr()
+    p.grad_q, p.grad_k, p.grad_v = (gq.data_ptr() if with_grad_q else None), gk.data_ptr(), gv.data_ptr()
     for f in ("q_stride_b", "q_stride_n", "q_stride_h", "k_stride_b", "k_stride_m", "k_stride_h",
               "v_stride_b", "v_stride_m", "v_stride_h"):
         setattr(p, f, getattr(ap, f))
     p.o_stride_b, p.o_stride_n, p.o_stride_h = out.stride(0), out.stride(1), dv
     p.go_stride_b, p.go_stride_n, p.go_stride_h = grad_out.stride(0), grad_out.stride(1), dv
-    p.gq_stride_b, p.gq_stride_n, p.gq_stride_h = gq.stride(0), gq.stride(1), dqk
+    if with_grad_q:
+        p.gq_stride_b, p.gq_stride_n, p.gq_stride_h = gq.stride(0), gq.stride(1), dqk
     p.gk_stride_b, p.gk_stride_m, p.gk_stride_h = gk.stride(0), gk.stride(1), dqk
     p.gv_stride_b, p.gv_stride_m, p.gv_stride_h = gv.stride(0), gv.stride(1), dv
     p.B, p.H, p.N, p.M, p.dqk, p.dv = B, H, N, M, dqk, dv
@@ -240,6 +243,57 @@ def attention_backward(q, k, v, out, grad_out, stat_m, stat_l, num_heads: int, s
         check(_lib.lib().pcv_attn_bwd(C.byref(p), _stream()), "pcv_attn_bwd")
     del keep
     return grads
+
+
+def attention_backward_shard(q, k, v, out, grad_out, stat_m, stat_l, num_heads: int, scale: float, m_total: int,
+                             m_offset: int, pad_mask=None, causal: bool = False, dropout_p: float = 0.0,
+                             dropout_seed: int = 0, check_only: bool = False):
+    """Backward of one key shard (pcv_attn_bwd_shard) -> (grad_q32, grad_k, grad_v).
+
+    ``k`` / ``v`` / ``pad_mask`` hold the keys [m_offset, m_offset + M) of ``m_total`` (m_offset even); ``stat_m`` /
+    ``stat_l`` are the row statistics MERGED over all keys and ``out`` the merged output.  grad_k / grad_v are this
+    shard's gradients; grad_q32 is its fp32 contribution to grad_q (q's batch size): the sum over all shards is grad_q.
+    Head dims up to 192; those that are not multiples of 8 are zero-padded as in ``_kernel_backward``.  ``check_only``
+    launches nothing and returns whether the kernels cover these operands."""
+    return _backward_shard(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, m_total, m_offset, pad_mask,
+                           causal, dropout_p, dropout_seed, "check" if check_only else "run")
+
+
+def _backward_shard(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, m_total, m_offset, pad_mask, causal,
+                    dropout_p, dropout_seed, mode):
+    """``attention_backward_shard`` with the operands prepared once.  mode "check": whether the kernels cover the call;
+    "run": the gradients (an uncovered call raises); "try": the gradients, or None where the kernels do not cover the
+    call (the caller then takes the shim)."""
+    dqk, dv = _head_dim(q, num_heads), _head_dim(v, num_heads)
+    padded = bool(dqk % 8 or dv % 8)
+    q, k, v, _ = _prep(q, k, v)
+    cdt = q.dtype
+    out = _rows_contiguous(out if out.dtype == cdt else out.to(cdt))
+    grad_out = _rows_contiguous(grad_out if grad_out.dtype == cdt else grad_out.to(cdt))
+    if padded:
+        q, k, v, out, grad_out = (_pad_heads_to8(t, num_heads).flatten(2) for t in (q, k, v, out, grad_out))
+    _require_cuda(out, grad_out, stat_m, stat_l, pad_mask)
+    with torch.cuda.device(k.device):
+        p, (_, gk, gv), keep = _fill_bwd_params(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask,
+                                                causal, dropout_p, dropout_seed, with_grad_q=False)
+        gq32 = torch.empty(q.shape[0], p.N, p.H * p.dqk, dtype=torch.float32, device=k.device)
+        s = _lib.KeyShard()
+        s.m_total, s.m_offset, s.grad_q32 = int(m_total), int(m_offset), gq32.data_ptr()
+        if mode != "run":
+            ok = bool(_lib.lib().pcv_attn_bwd_shard_supported(C.byref(p), C.byref(s)))
+            if mode == "check" or not ok:
+                return ok if mode == "check" else None
+        need = C.c_size_t(0)
+        check(_lib.lib().pcv_attn_bwd_shard_workspace_bytes(C.byref(p), C.byref(s), C.byref(need)),
+              "pcv_attn_bwd_shard_workspace_bytes")
+        ws = torch.empty(max(need.value, 256), dtype=torch.uint8, device=k.device)
+        p.workspace, p.workspace_bytes = ws.data_ptr(), need.value
+        check(_lib.lib().pcv_attn_bwd_shard(C.byref(p), C.byref(s), _stream()), "pcv_attn_bwd_shard")
+    del keep
+    if padded:
+        gq32, gk, gv = (g.unflatten(2, (num_heads, -1))[..., :d].flatten(2)
+                        for g, d in ((gq32, dqk), (gk, dqk), (gv, dv)))
+    return gq32, gk, gv
 
 
 def new_dropout_seed() -> int:
@@ -421,68 +475,82 @@ class _FusedAttention(torch.autograd.Function):
             if mode == "kernel":
                 raise RuntimeError("backward_config['impl'] = 'kernel' but pcv_attn_bwd does not cover this call: "
                                    + _lib.lib().pcv_last_error().decode())
-        B, M = k.shape[0], k.shape[1]
-        N = q.shape[1]
-        cdt = _compute_dtype(q.dtype)
-        # the kernel saw operands rounded to the compute dtype: differentiate the same function
-        qh = q.to(cdt).float().expand(B, -1, -1).reshape(B, N, H, -1).transpose(1, 2)      # (B,H,N,dqk)
-        kh = k.to(cdt).float().reshape(B, M, H, -1).transpose(1, 2)                         # (B,H,M,dqk)
-        vh = v.to(cdt).float().reshape(B, M, H, -1).transpose(1, 2)                         # (B,H,M,dv)
-        go = grad_out.float().reshape(B, N, H, -1).transpose(1, 2)                          # (B,H,N,dv)
-        oh = out.float().reshape(B, N, H, -1).transpose(1, 2)
-        t_scale = scale * 1.4426950408889634
-        neg = -torch.finfo(torch.float32).max
-        chunk = max(128, int(backward_config["max_score_bytes"] // (4 * B * H * N)) // 128 * 128)
-
-        def scores(j0, j1):  # log2-domain scores with the reference's finite mask fill, and the fill mask
-            t = torch.matmul(qh, kh[:, :, j0:j1].transpose(-1, -2)) * t_scale
-            filled = None
-            if pad_mask is not None:
-                filled = pad_mask[:, j0:j1].bool()[:, None, None, :].expand(B, 1, N, j1 - j0)
-            if causal:
-                rows = torch.arange(N, device=t.device)[:, None] + (M - N)
-                cm = (torch.arange(j0, j1, device=t.device)[None, :] > rows)[None, None]
-                filled = cm if filled is None else (filled | cm)
-            if filled is not None:
-                t = t.masked_fill(filled, neg)
-            return t, filled
-
-        if pm is None:  # statistics were not saved: one chunked pass to rebuild them
-            m_run = torch.full((B, H, N), -float("inf"), device=q.device)
-            l_run = torch.zeros(B, H, N, device=q.device)
-            for j0 in range(0, M, chunk):
-                t, _ = scores(j0, min(M, j0 + chunk))
-                m_new = torch.maximum(m_run, t.amax(-1))
-                l_run = l_run * torch.exp2(m_run - m_new) + torch.exp2(t - m_new[..., None]).sum(-1)
-                m_run = m_new
-            pm, pl = m_run, l_run
-        delta = (go * oh).sum(-1)                                                            # (B,H,N)
-        gq = torch.zeros_like(qh)
-        gk = torch.empty_like(kh)
-        gv = torch.empty_like(vh)
-        inv_l = 1.0 / pl
-        for j0 in range(0, M, chunk):
-            j1 = min(M, j0 + chunk)
-            t, filled = scores(j0, j1)
-            p = torch.exp2(t - pm[..., None]) * inv_l[..., None]                             # (B,H,N,c) probabilities
-            dp = torch.matmul(go, vh[:, :, j0:j1].transpose(-1, -2))
-            if drop_p > 0.0:  # O = (P o K r) V:  dV = (P o K r)^T dO,  dP = (dO V^T) o K r
-                kr = _dropout_keep(B, H, N, j0, j1, drop_p, drop_seed, k.device).to(p.dtype) * _dropout_scale(drop_p)
-                gv[:, :, j0:j1] = torch.matmul((p * kr).transpose(-1, -2), go)
-                dp = dp * kr
-            else:
-                gv[:, :, j0:j1] = torch.matmul(p.transpose(-1, -2), go)
-            ds = p * (dp - delta[..., None])
-            if filled is not None:
-                ds = ds.masked_fill(filled, 0.0)  # a filled score is a constant (masked_fill_): no gradient through it
-            gq += torch.matmul(ds, kh[:, :, j0:j1])
-            gk[:, :, j0:j1] = torch.matmul(ds.transpose(-1, -2), qh)
-        gq = (gq * scale).transpose(1, 2).reshape(B, N, -1)
-        if q.shape[0] == 1 and B > 1:
-            gq = gq.sum(0, keepdim=True)
-        gk = (gk * scale).transpose(1, 2).reshape(B, M, -1)
-        gv = gv.transpose(1, 2).reshape(B, M, -1)
+        gq, gk, gv = _backward_shim(q, k, v, out, grad_out, pm, pl, H, scale, pad_mask, causal, drop_p, drop_seed)
         return gq.to(q.dtype), gk.to(k.dtype), gv.to(v.dtype), None, None, None, None, None, None, None
+
+
+def _backward_shim(q, k, v, out, grad_out, pm, pl, H: int, scale: float, pad_mask, causal: bool, drop_p: float,
+                   drop_seed: int, m_total: Optional[int] = None, m_offset: int = 0):
+    """TRAINING-SUPPORT SHIM: the flash-attention backward recurrence in plain torch ops, chunked over the key axis
+    (see ``_FusedAttention``).  -> fp32 (grad_q, grad_k, grad_v); grad_q has q's batch size (summed for a batch-1 q).
+
+    ``k`` / ``v`` / ``pad_mask`` may be the keys [m_offset, m_offset + M) of ``m_total`` (default: all keys): the causal
+    diagonal and the dropout mask then take global key indices, and ``pm`` / ``pl`` / ``out`` must be the statistics
+    and output merged over all ``m_total`` keys; grad_q is this shard's contribution."""
+    B, M = k.shape[0], k.shape[1]
+    N = q.shape[1]
+    m_total = M if m_total is None else int(m_total)
+    cdt = _compute_dtype(q.dtype)
+    # the kernel saw operands rounded to the compute dtype: differentiate the same function
+    qh = q.to(cdt).float().expand(B, -1, -1).reshape(B, N, H, -1).transpose(1, 2)      # (B,H,N,dqk)
+    kh = k.to(cdt).float().reshape(B, M, H, -1).transpose(1, 2)                         # (B,H,M,dqk)
+    vh = v.to(cdt).float().reshape(B, M, H, -1).transpose(1, 2)                         # (B,H,M,dv)
+    go = grad_out.float().reshape(B, N, H, -1).transpose(1, 2)                          # (B,H,N,dv)
+    oh = out.float().reshape(B, N, H, -1).transpose(1, 2)
+    t_scale = scale * 1.4426950408889634
+    neg = -torch.finfo(torch.float32).max
+    chunk = max(128, int(backward_config["max_score_bytes"] // (4 * B * H * N)) // 128 * 128)
+
+    def scores(j0, j1):  # log2-domain scores with the reference's finite mask fill, and the fill mask
+        t = torch.matmul(qh, kh[:, :, j0:j1].transpose(-1, -2)) * t_scale
+        filled = None
+        if pad_mask is not None:
+            filled = pad_mask[:, j0:j1].bool()[:, None, None, :].expand(B, 1, N, j1 - j0)
+        if causal:
+            rows = torch.arange(N, device=t.device)[:, None] + (m_total - N - m_offset)
+            cm = (torch.arange(j0, j1, device=t.device)[None, :] > rows)[None, None]
+            filled = cm if filled is None else (filled | cm)
+        if filled is not None:
+            t = t.masked_fill(filled, neg)
+        return t, filled
+
+    if pm is None:  # statistics were not saved: one chunked pass to rebuild them
+        m_run = torch.full((B, H, N), -float("inf"), device=q.device)
+        l_run = torch.zeros(B, H, N, device=q.device)
+        for j0 in range(0, M, chunk):
+            t, _ = scores(j0, min(M, j0 + chunk))
+            m_new = torch.maximum(m_run, t.amax(-1))
+            l_run = l_run * torch.exp2(m_run - m_new) + torch.exp2(t - m_new[..., None]).sum(-1)
+            m_run = m_new
+        pm, pl = m_run, l_run
+    delta = (go * oh).sum(-1)                                                            # (B,H,N)
+    gq = torch.zeros_like(qh)
+    gk = torch.empty_like(kh)
+    gv = torch.empty_like(vh)
+    inv_l = 1.0 / pl
+    for j0 in range(0, M, chunk):
+        j1 = min(M, j0 + chunk)
+        t, filled = scores(j0, j1)
+        p = torch.exp2(t - pm[..., None]) * inv_l[..., None]                             # (B,H,N,c) probabilities
+        dp = torch.matmul(go, vh[:, :, j0:j1].transpose(-1, -2))
+        if drop_p > 0.0:  # O = (P o K r) V:  dV = (P o K r)^T dO,  dP = (dO V^T) o K r
+            kr = (_dropout_keep(B, H, N, m_offset + j0, m_offset + j1, drop_p, drop_seed, k.device).to(p.dtype)
+                  * _dropout_scale(drop_p))
+            gv[:, :, j0:j1] = torch.matmul((p * kr).transpose(-1, -2), go)
+            dp = dp * kr
+        else:
+            gv[:, :, j0:j1] = torch.matmul(p.transpose(-1, -2), go)
+        ds = p * (dp - delta[..., None])
+        if filled is not None:
+            ds = ds.masked_fill(filled, 0.0)  # a filled score is a constant (masked_fill_): no gradient through it
+        gq += torch.matmul(ds, kh[:, :, j0:j1])
+        gk[:, :, j0:j1] = torch.matmul(ds.transpose(-1, -2), qh)
+    gq = (gq * scale).transpose(1, 2).reshape(B, N, -1)
+    if q.shape[0] == 1 and B > 1:
+        gq = gq.sum(0, keepdim=True)
+    gk = (gk * scale).transpose(1, 2).reshape(B, M, -1)
+    gv = gv.transpose(1, 2).reshape(B, M, -1)
+    return gq, gk, gv
 
 
 def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, num_heads: int, scale: float,
@@ -520,9 +588,10 @@ def attention_partial(q, k, v, num_heads: int, scale: float, pad_mask=None, caus
     """One M-shard's un-normalised softmax state: (part_o (B,H,N,dv) f32, part_m (B,H,N), part_l (B,H,N)).
 
     ``k``/``v``/``pad_mask`` hold this shard's keys [m_offset, m_offset+M) of ``m_total``.  ``out`` may
-    supply the three (contiguous, float32) destination tensors.  ``dropout_p`` > 0 (all keys, no sharding): the
-    one-pass dropout forward (pcv_attn_fwd_partial_dropout) — part_o is the numerator with the mask of
-    ``dropout_keep_mask`` applied and scaled by 1/(1-p), part_m / part_l stay the dropout-free statistics."""
+    supply the three (contiguous, float32) destination tensors.  ``dropout_p`` > 0: the one-pass dropout forward
+    (pcv_attn_fwd_partial_dropout, or pcv_attn_fwd_partial_dropout_shard on a key shard, m_offset even) — part_o is
+    the numerator with the mask of ``dropout_keep_mask`` over the shard's global key range applied and scaled by
+    1/(1-p), part_m / part_l stay the dropout-free statistics."""
     q, k, v, _ = _prep(q, k, v)
     with torch.cuda.device(k.device):
         p, keep = _fill_attn_params(q, k, v, num_heads, scale, pad_mask, causal, m_total, m_offset, impl)
@@ -547,8 +616,12 @@ def attention_partial(q, k, v, num_heads: int, scale: float, pad_mask=None, caus
             check(_lib.lib().pcv_attn_workspace_bytes(C.byref(p), C.byref(need)), "pcv_attn_workspace_bytes")
             ws = torch.empty(max(need.value, 256), dtype=torch.uint8, device=k.device)
             p.workspace, p.workspace_bytes = ws.data_ptr(), need.value
-            check(_lib.lib().pcv_attn_fwd_partial_dropout(C.byref(p), float(dropout_p), int(dropout_seed), _stream()),
-                  "pcv_attn_fwd_partial_dropout")
+            if p.m_total == p.M and p.m_offset == 0:
+                check(_lib.lib().pcv_attn_fwd_partial_dropout(C.byref(p), float(dropout_p), int(dropout_seed),
+                                                              _stream()), "pcv_attn_fwd_partial_dropout")
+            else:
+                check(_lib.lib().pcv_attn_fwd_partial_dropout_shard(C.byref(p), float(dropout_p), int(dropout_seed),
+                                                                    _stream()), "pcv_attn_fwd_partial_dropout_shard")
         else:
             _run_attn(p, k.device)
     del keep
