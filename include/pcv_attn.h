@@ -46,7 +46,7 @@ extern "C" {
 #endif
 
 /* element type of q/k/v/out */
-enum pcv_dtype { PCV_BF16 = 0, PCV_F16 = 1, PCV_F32 = 2 /* pcv_kv_append only */ };
+enum pcv_dtype { PCV_BF16 = 0, PCV_F16 = 1, PCV_F32 = 2 /* pcv_kv_append only */, PCV_E4M3 = 3 /* pcv_attn_fwd_fp8 only */ };
 
 /* kernel selection; AUTO picks the tensor-core kernel whenever the shape is supported (the names are historical) */
 enum pcv_impl {
@@ -442,6 +442,53 @@ PCV_API int pcv_attn_fwd_partial_dropout_shard(const pcv_attn_params* p, float d
 PCV_API int pcv_attn_bwd_shard_supported(const pcv_attn_bwd_params* p, const pcv_key_shard* s);
 PCV_API int pcv_attn_bwd_shard_workspace_bytes(const pcv_attn_bwd_params* p, const pcv_key_shard* s, size_t* bytes);
 PCV_API int pcv_attn_bwd_shard(const pcv_attn_bwd_params* p, const pcv_key_shard* s, void* stream);
+
+/*
+ * FP8 (e4m3) inference forward on the tensor cores: S = Q K^T and O = P V on the e4m3 wgmma, softmax in fp32.
+ * `p` is a pcv_attn_params with dtype = PCV_E4M3 whose q / k are e4m3 (strides in elements = bytes) and whose v is
+ * V TRANSPOSED, vt (B, H, dv, M_pad) e4m3 with the strides of `f` (keys contiguous, in order; M_pad >= M and a
+ * multiple of 16; keys beyond M are never read).  v_stride_* of `p` are ignored.  With the dequantisation factors
+ *     q = q8 * q_descale[h],   k = k8 * k_descale[h],   v = vt8[b, h, c, :] * v_descale[h, c]
+ * the result is that of pcv_attn_fwd on (q, k, v) except that each probability (relative to the running row maximum
+ * of its 128-key tile) is rounded to e4m3 as e4m3(P * 256) before P V; the denominators are the fp32 sums of the
+ * unrounded probabilities.  Masks, batch-1 q, key sharding (m_total / m_offset) and write_partial behave as in
+ * pcv_attn_fwd; out is written in f->out_dtype (bf16 / fp16), and part_* are the same fp32 state, so pcv_attn_combine
+ * merges it.  Head dims: multiples of 16, dqk <= 256, dv <= 512.  impl must be AUTO or TCGEN05: the CTA pair, the
+ * fused cross-GPU merge, dropout and the decode kernel take no FP8 operands.  The workspace is
+ * pcv_attn_workspace_bytes() of the same params.  Arguments are checked before any CUDA call.
+ */
+typedef struct pcv_fp8_attn {
+  const float* q_descale;  /* (H) f32                                                  */
+  const float* k_descale;  /* (H) f32                                                  */
+  const float* v_descale;  /* (H, dv) f32, dense                                       */
+  int64_t vt_stride_b, vt_stride_h, vt_stride_c;  /* element strides of vt; its key stride is 1 */
+  int32_t out_dtype;       /* PCV_BF16 / PCV_F16: dtype of `out`                      */
+  int32_t reserved;
+} pcv_fp8_attn;
+
+PCV_API int pcv_attn_fwd_fp8_supported(const pcv_attn_params* p, const pcv_fp8_attn* f);
+PCV_API int pcv_attn_fwd_fp8(const pcv_attn_params* p, const pcv_fp8_attn* f, void* stream);
+
+/*
+ * The fused producer (pcv_kv_project) with e4m3 outputs, for pcv_attn_fwd_fp8: the same LayerNorm-folded GEMM with a
+ * bf16 / fp16 mainloop (p->dtype is that of x and w); in the epilogue output column n is multiplied by
+ * inv_scale[n] (1 / its descale) and rounded to e4m3 (nearest even, saturating at +-448).
+ *   K columns [0, n_k)        -> p->k_out, e4m3 rows with the row stride p->k_stride_row (bytes, a multiple of 16)
+ *   V columns [n_k, n_k + n_v) -> vt_out, V transposed: (B, H, v_head_dim, keys) with the strides below, where input
+ *                                row r is key r % keys_per_batch of batch row r / keys_per_batch
+ * p->v_out / p->v_stride_row are unused.  q is produced the same way with n_v = 0.  One CTA per tile (cta_group 0 or
+ * 1).  Arguments are checked before any CUDA call.
+ */
+typedef struct pcv_kvproj_fp8 {
+  const float* inv_scale;  /* (n_k + n_v) f32                                          */
+  void* vt_out;            /* e4m3 V^T; may be NULL when n_v == 0                      */
+  int64_t vt_stride_b, vt_stride_h, vt_stride_c;  /* byte strides of vt_out; keys contiguous */
+  int32_t keys_per_batch;  /* keys per batch row (rows = B * keys_per_batch)           */
+  int32_t v_head_dim;      /* V channels per head (a multiple of 16)                   */
+} pcv_kvproj_fp8;
+
+PCV_API int pcv_kv_project_fp8_supported(const pcv_kvproj_params* p, const pcv_kvproj_fp8* f);
+PCV_API int pcv_kv_project_fp8(const pcv_kvproj_params* p, const pcv_kvproj_fp8* f, void* stream);
 
 /*
  * Live timing of the dominant kernel (bench.py's roofline leg): between pcv_profile_begin() and

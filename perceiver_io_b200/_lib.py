@@ -15,7 +15,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # PCV_LIB_PATH: developer override (A/B-testing two builds of the library on one GPU box)
 LIB_PATH = os.environ.get("PCV_LIB_PATH") or os.path.join(_HERE, "lib", "libpcv_attn.so")
 
-PCV_BF16, PCV_F16, PCV_F32 = 0, 1, 2
+PCV_BF16, PCV_F16, PCV_F32, PCV_E4M3 = 0, 1, 2, 3
 PCV_IMPL_AUTO, PCV_IMPL_TCGEN05, PCV_IMPL_SIMT, PCV_IMPL_TCGEN05_PAIR, PCV_IMPL_DECODE = 0, 1, 2, 3, 4
 IMPL_BY_NAME = {"auto": PCV_IMPL_AUTO, "tcgen05": PCV_IMPL_TCGEN05, "simt": PCV_IMPL_SIMT, "decode": PCV_IMPL_DECODE,
                 "tcgen05_pair": PCV_IMPL_TCGEN05_PAIR}
@@ -53,6 +53,10 @@ EXPORTS = (
     "pcv_attn_bwd_shard_supported",
     "pcv_attn_bwd_shard_workspace_bytes",
     "pcv_attn_bwd_shard",
+    "pcv_attn_fwd_fp8_supported",
+    "pcv_attn_fwd_fp8",
+    "pcv_kv_project_fp8_supported",
+    "pcv_kv_project_fp8",
     "pcv_launch_count",
     "pcv_debug_plan",
     "pcv_profile_begin",
@@ -207,6 +211,22 @@ class KeyShard(C.Structure):
     _fields_ = [("m_total", C.c_int32), ("m_offset", C.c_int32), ("grad_q32", C.c_void_p)]
 
 
+class Fp8Attn(C.Structure):
+    _fields_ = [
+        ("q_descale", C.c_void_p), ("k_descale", C.c_void_p), ("v_descale", C.c_void_p),
+        ("vt_stride_b", C.c_int64), ("vt_stride_h", C.c_int64), ("vt_stride_c", C.c_int64),
+        ("out_dtype", C.c_int32), ("reserved", C.c_int32),
+    ]
+
+
+class KvProjFp8(C.Structure):
+    _fields_ = [
+        ("inv_scale", C.c_void_p), ("vt_out", C.c_void_p),
+        ("vt_stride_b", C.c_int64), ("vt_stride_h", C.c_int64), ("vt_stride_c", C.c_int64),
+        ("keys_per_batch", C.c_int32), ("v_head_dim", C.c_int32),
+    ]
+
+
 class DeviceInfo(C.Structure):
     _fields_ = [
         ("device", C.c_int32), ("sm_major", C.c_int32), ("sm_minor", C.c_int32),
@@ -298,6 +318,14 @@ def lib() -> C.CDLL:
         l.pcv_attn_bwd_shard_workspace_bytes.restype = C.c_int
         l.pcv_attn_bwd_shard.argtypes = [C.POINTER(AttnBwdParams), C.POINTER(KeyShard), C.c_void_p]
         l.pcv_attn_bwd_shard.restype = C.c_int
+        l.pcv_attn_fwd_fp8_supported.argtypes = [C.POINTER(AttnParams), C.POINTER(Fp8Attn)]
+        l.pcv_attn_fwd_fp8_supported.restype = C.c_int
+        l.pcv_attn_fwd_fp8.argtypes = [C.POINTER(AttnParams), C.POINTER(Fp8Attn), C.c_void_p]
+        l.pcv_attn_fwd_fp8.restype = C.c_int
+        l.pcv_kv_project_fp8_supported.argtypes = [C.POINTER(KvProjParams), C.POINTER(KvProjFp8)]
+        l.pcv_kv_project_fp8_supported.restype = C.c_int
+        l.pcv_kv_project_fp8.argtypes = [C.POINTER(KvProjParams), C.POINTER(KvProjFp8), C.c_void_p]
+        l.pcv_kv_project_fp8.restype = C.c_int
         l.pcv_debug_plan.argtypes = [C.c_int32] * 7 + [C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_int32)]
         l.pcv_debug_plan.restype = C.c_int
         for name in ("pcv_get_device_info", "pcv_attn_supported_tcgen05", "pcv_attn_workspace_bytes",

@@ -41,13 +41,17 @@ void prof_mark_end(cudaStream_t stream) {
   cudaEventRecord(g_prof_events.back().second, stream);
 }
 
-static int validate_attn(const pcv_attn_params* p) {
+// fp8: the params of pcv_attn_fwd_fp8 (e4m3 operands) or of the workspace query, which serves both forwards
+static int validate_attn(const pcv_attn_params* p, bool fp8 = false) {
   PCV_REQUIRE(p != nullptr, PCV_ERR_INVALID, "attn: params is NULL");
   PCV_REQUIRE(p->q && p->k && p->v, PCV_ERR_INVALID, "attn: q/k/v pointer is NULL");
   PCV_REQUIRE(p->B >= 1 && p->H >= 1 && p->N >= 1 && p->M >= 1, PCV_ERR_INVALID,
               "attn: B=%d H=%d N=%d M=%d must all be >= 1", p->B, p->H, p->N, p->M);
   PCV_REQUIRE(p->dqk >= 1 && p->dv >= 1, PCV_ERR_INVALID, "attn: dqk=%d dv=%d must be >= 1", p->dqk, p->dv);
-  PCV_REQUIRE(p->dtype == PCV_BF16 || p->dtype == PCV_F16, PCV_ERR_INVALID, "attn: unknown dtype %d", p->dtype);
+  PCV_REQUIRE(fp8 || p->dtype != PCV_E4M3, PCV_ERR_UNSUPPORTED,
+              "attn: e4m3 operands run on pcv_attn_fwd_fp8 only (no CTA pair, fused merge, dropout or decode kernel)");
+  PCV_REQUIRE(p->dtype == PCV_BF16 || p->dtype == PCV_F16 || p->dtype == PCV_E4M3, PCV_ERR_INVALID,
+              "attn: unknown dtype %d", p->dtype);
   PCV_REQUIRE(p->m_total >= p->M && p->m_offset >= 0 && p->m_offset + p->M <= p->m_total, PCV_ERR_INVALID,
               "attn: shard [%d,%d) outside m_total=%d", p->m_offset, p->m_offset + p->M, p->m_total);
   PCV_REQUIRE(!p->causal || p->m_total >= p->N, PCV_ERR_INVALID,
@@ -175,9 +179,10 @@ int pcv_attn_supported_tcgen05(const pcv_attn_params* p) {
 }
 
 int pcv_attn_workspace_bytes(const pcv_attn_params* p, size_t* bytes) {
-  int rc = validate_attn(p);
+  int rc = validate_attn(p, true);
   if (rc != PCV_OK) return rc;
   PCV_REQUIRE(bytes != nullptr, PCV_ERR_INVALID, "attn: bytes is NULL");
+  if (p->dtype == PCV_E4M3) return attn_tc_workspace_bytes(*p, bytes);  // pcv_attn_fwd_fp8: the tensor-core kernel
   const char* why = "";
   if (use_decode(*p, &why)) return attn_decode_workspace_bytes(*p, bytes);
   PCV_REQUIRE(p->impl != PCV_IMPL_DECODE, PCV_ERR_UNSUPPORTED, "attn: decode kernel requested but %s", why);
@@ -375,6 +380,41 @@ int pcv_attn_fwd_partial_dropout_shard_supported(const pcv_attn_params* p, float
 
 int pcv_attn_fwd_partial_dropout_shard(const pcv_attn_params* p, float dropout_p, uint64_t dropout_seed, void* stream) {
   return partial_dropout_launch(p, dropout_p, dropout_seed, true, stream);
+}
+
+int pcv_kv_project_fp8_supported(const pcv_kvproj_params* p, const pcv_kvproj_fp8* f) {
+  if (p == nullptr || f == nullptr) {
+    set_error("kv_project_fp8: params are NULL");
+    return 0;
+  }
+  const char* why = "";
+  const bool ok = kv_project_fp8_supported(*p, *f, &why);
+  if (!ok) set_error("kv_project_fp8 not applicable: %s", why);
+  return ok ? 1 : 0;
+}
+
+int pcv_kv_project_fp8(const pcv_kvproj_params* p, const pcv_kvproj_fp8* f, void* stream) {
+  PCV_REQUIRE(p != nullptr && f != nullptr, PCV_ERR_INVALID, "kv_project_fp8: params are NULL");
+  return launch_kv_project_fp8(*p, *f, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pcv_attn_fwd_fp8_supported(const pcv_attn_params* p, const pcv_fp8_attn* f) {
+  if (f == nullptr) {
+    set_error("attn_fwd_fp8: fp8 params are NULL");
+    return 0;
+  }
+  if (validate_attn(p, true) != PCV_OK) return 0;
+  const char* why = "";
+  const bool ok = attn_tc_fp8_supported(*p, *f, &why);
+  if (!ok) set_error("FP8 attention forward not applicable: %s", why);
+  return ok ? 1 : 0;
+}
+
+int pcv_attn_fwd_fp8(const pcv_attn_params* p, const pcv_fp8_attn* f, void* stream) {
+  PCV_REQUIRE(f != nullptr, PCV_ERR_INVALID, "attn_fwd_fp8: fp8 params are NULL");
+  int rc = validate_attn(p, true);
+  if (rc != PCV_OK) return rc;
+  return launch_attn_tc_fp8(*p, *f, reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -96,6 +96,9 @@ struct TcParams {
   PeerTail tail;
   DropoutRule drop;  // attn_fwd_drop_kernel only; last, so that the other kernels' parameter offsets do not move
   int drop_key_base; // attn_fwd_drop_kernel: global index of local key 0 (m_offset, even); the mask hashes it + j
+  // attn_fwd_fp8_kernel only (appended, as the dropout fields): per-head q / k and per-(head, channel) v descales
+  const float *q_descale, *k_descale, *v_descale;
+  int v_descale_stride;  // floats between heads of v_descale (the full dv)
 };
 
 // --------------------------------------------------------------------------------------------------
@@ -283,15 +286,16 @@ struct FwdBarriers {
 // DROP: after the denominators took the tile's probabilities, the dropped elements of the numerator are zeroed (the
 // statistics stay those of the dropout-free softmax; the survivors are scaled once, in the epilogue).  `qside` is the
 // query side of the mask hash of rows n0 and n0 + 8; each thread hashes once per row and key pair (jb, jb + 1).
-template <bool DROP>
+// FP8: the scores are scaled by `fp8_scale_log2` (p.scale_log2 * q_descale[h] * k_descale[h]) instead of p.scale_log2.
+template <bool DROP, bool FP8 = false>
 __device__ __forceinline__ void tile_softmax(float (&s)[64], float (&m_run)[2], float (&l_run)[2], float (&alpha)[2],
                                              const TcParams& p, int b, int j0, int n0, int cq, bool interior,
-                                             const uint32_t (&qside)[2]) {
+                                             const uint32_t (&qside)[2], float fp8_scale_log2 = 0.f) {
   float mx[2] = {-INFINITY, -INFINITY};
   if (interior) {
 #pragma unroll
     for (int i = 0; i < 64; ++i) {
-      s[i] *= p.scale_log2;
+      s[i] *= (FP8 ? fp8_scale_log2 : p.scale_log2);
       mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
     }
   } else {
@@ -304,7 +308,7 @@ __device__ __forceinline__ void tile_softmax(float (&s)[64], float (&m_run)[2], 
       for (int e = 0; e < 4; ++e) {
         const int j = jb + (e & 1);
         const int n = n0 + 8 * (e >> 1);
-        float x = s[4 * g + e] * p.scale_log2;
+        float x = s[4 * g + e] * (FP8 ? fp8_scale_log2 : p.scale_log2);
         if (j >= p.M) x = -INFINITY;
         else if (((padw >> (j & 31)) & 1u) || (p.causal && j > n + p.causal_shift)) x = kMaskedScore;
         s[4 * g + e] = x;
@@ -355,6 +359,31 @@ __device__ __forceinline__ void pack_p(const float (&s)[64], uint32_t (&pa)[8][4
   }
 }
 
+// probabilities -> the e4m3 A fragments of the FP8 P V wgmma (k-step kk covers keys [32 kk, 32 kk + 32)), each
+// rounded as e4m3(P * 2^8).  This thread's scores hold keys 8j + 2q + {0, 1} of rows r and r + 8 (q = lane % 4), the
+// fragment wants keys 4q .. 4q + 3 and 16 + 4q .. 16 + 4q + 3 of the same rows, so the four lanes of a quad exchange
+// halves: per k-step and row, lane q receives from lanes a = q/2 + 2 (q%2) and a ^ 1 the two-key halves it needs.
+// Sources with odd q send their 8 + 2q / 24 + 2q keys first, even ones their 2q / 16 + 2q keys, so that each of the
+// two shuffles reads one value per source lane.
+__device__ __forceinline__ void pack_p_e4m3(const float (&s)[64], uint32_t (&pa)[4][4], int lane) {
+  const int q = lane & 3;
+  const uint32_t sel_a = (q & 1) ? 0x7632u : 0x5410u, sel_b = (q & 1) ? 0x5410u : 0x7632u;
+  const uint32_t sel_lo = (q & 2) ? 0x1054u : 0x5410u, sel_hi = (q & 2) ? 0x3276u : 0x7632u;
+  const int src_a = (lane & ~3) | (q >> 1) | ((q & 1) << 1), src_b = src_a ^ 1;
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk)
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const float* x = s + 16 * kk + 2 * r;  // groups 4kk .. 4kk + 3 (8 keys each), row half r
+      const uint32_t x0 = cvt_e4m3x2(x[0] * 256.f, x[1] * 256.f) | (cvt_e4m3x2(x[4] * 256.f, x[5] * 256.f) << 16);
+      const uint32_t x1 = cvt_e4m3x2(x[8] * 256.f, x[9] * 256.f) | (cvt_e4m3x2(x[12] * 256.f, x[13] * 256.f) << 16);
+      const uint32_t a = __shfl_sync(0xffffffffu, __byte_perm(x0, x1, sel_a), src_a);
+      const uint32_t b = __shfl_sync(0xffffffffu, __byte_perm(x0, x1, sel_b), src_b);
+      pa[kk][r] = __byte_perm(a, b, sel_lo);
+      pa[kk][2 + r] = __byte_perm(a, b, sel_hi);
+    }
+}
+
 template <int NVB>
 __device__ __forceinline__ void rescale_o(float (&o)[NVB][32], const float (&alpha)[2]) {
 #pragma unroll
@@ -364,20 +393,25 @@ __device__ __forceinline__ void rescale_o(float (&o)[NVB][32], const float (&alp
 }
 
 // The body of attn_fwd_kernel (DROP = false) and of attn_fwd_drop_kernel (DROP = true: attention-probability dropout,
-// see tile_softmax; write_partial = 1 without key sharding, no CTA pair).
-template <int NQB, int NVB, bool BF16, bool PAIR, bool DROP>
+// see tile_softmax; write_partial = 1 without key sharding, no CTA pair), and of attn_fwd_fp8_kernel (FP8 = true:
+// e4m3 q / k and V^T, (B, H, dv, keys).  A Q or K box is 128 rows x 128 e4m3 channels; the V^T box of a tile is 128
+// channels x 128 keys, one ring slot, with the 64-channel halves v at byte offset 8192 v.  BF16 is the output dtype).
+template <int NQB, int NVB, bool BF16, bool PAIR, bool DROP, bool FP8 = false>
 __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv,
                                               const TcParams& p) {
   static_assert(!(DROP && PAIR), "no dropout in the CTA-pair kernel");
+  static_assert(!FP8 || (NQB <= 2 && !PAIR && !DROP), "the FP8 kernel: qk head dims up to 256, no CTA pair, no dropout");
   using C = FwdCfg<NQB, NVB>;
   constexpr int NS = C::kSlots;
+  constexpr int KVB = FP8 ? 1 : NVB;  // ring boxes of V per key tile
+  constexpr int kQkCh = FP8 ? 128 : 64;  // qk channels per box
   // Head dims up to 128 (NQB <= 2) run the pipelined schedule: per tile one commit group for S = Q K^T and one for
   // O += P V, the P V of tile t - 1 runs under the softmax of tile t, and the two warpgroups take turns at issuing
   // their GEMMs (ping-pong), so that one warpgroup's MMAs run while the other computes its softmax.  It holds the K
   // boxes of tile t and the V boxes of tile t - 1 at once, which larger head dims do not leave ring slots for; they
   // keep the serial schedule (per box: wait, issue, drain, release).
   constexpr bool kPipelined = NQB <= 2;
-  static_assert(!kPipelined || NQB + NVB <= NS, "the pipelined schedule holds NQB + NVB ring slots");
+  static_assert(!kPipelined || NQB + KVB <= NS, "the pipelined schedule holds NQB + KVB ring slots");
   // registers per thread: producer + 2 x consumer = 504 = the launch bound's 168 x 3; the pipelined consumers keep
   // S, P and O live at once, the serial schedule's producer (ring index arithmetic by a non-power-of-two) spills at 24
   constexpr int kProducerRegs = kPipelined ? 24 : 40, kConsumerRegs = kPipelined ? 240 : 232;
@@ -416,16 +450,19 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
         mbar_wait(&bar.q_empty, ((si - seg_lo) & 1) ^ 1, 1);
         mbar_arrive_expect_tx(&bar.q_full, C::kQBytes);
         for (int c = 0; c < NQB; ++c)
-          tma_load_4d(sQ + c * kBoxBytes, &tq, &bar.q_full, c * 64, sg.q0 + qoff, sg.h, p.q_bcast ? 0 : sg.b);
+          tma_load_4d(sQ + c * kBoxBytes, &tq, &bar.q_full, c * kQkCh, sg.q0 + qoff, sg.h, p.q_bcast ? 0 : sg.b);
         for (int t = sg.t0; t < sg.t1; ++t) {
 #pragma unroll 1
-          for (int c = 0; c < NQB + NVB; ++c, ++it) {
+          for (int c = 0; c < NQB + KVB; ++c, ++it) {
             const uint32_t s = it % NS;
             mbar_wait(&bar.empty[s], ((it / NS) & 1) ^ 1, 2);
             mbar_arrive_expect_tx(&bar.full[s], kBoxBytes);
             const CUtensorMap* tm = c < NQB ? &tk : &tv;
             const int ch = (c < NQB ? c : c - NQB) * 64;
-            if (PAIR)  // 64-key half `rank` of the box, into both CTAs
+            if constexpr (FP8) {  // K: (channel box c, keys of tile t); V^T: (keys of tile t, channels of the pass)
+              if (c < NQB) tma_load_4d(sRing + s * kBoxBytes, tm, &bar.full[s], c * kQkCh, t * kTileN, sg.h, sg.b);
+              else tma_load_4d(sRing + s * kBoxBytes, tm, &bar.full[s], t * kTileN, 0, sg.h, sg.b);
+            } else if (PAIR)  // 64-key half `rank` of the box, into both CTAs
               tma_load_4d_mc(sRing + s * kBoxBytes + rank * (kBoxBytes / 2), tm, &bar.full[s], ch,
                              t * kTileN + 64 * (int)rank, sg.h, sg.b, 0x3);
             else
@@ -464,22 +501,57 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
 #pragma unroll
     for (int c = 0; c < NQB; ++c)
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk)
-        wgmma_ss<128, BF16>(s, make_desc(q_base + c * kBoxBytes + kk * 32),
-                            make_desc(ring_base + (i + c) % NS * kBoxBytes + kk * 32), (c | kk) != 0);
+      for (int kk = 0; kk < 4; ++kk) {  // k16 steps of 16-bit channels, k32 steps of e4m3 ones: 32 bytes each
+        // FP8 issues all four k32 steps of a box even past dqk (TMA zero fill): a runtime guard around the wgmma makes
+        // ptxas serialise every wgmma of the kernel (C7515)
+        if constexpr (FP8)
+          wgmma_ss_e4m3_n128(s, make_desc(q_base + c * kBoxBytes + kk * 32),
+                             make_desc(ring_base + (i + c) % NS * kBoxBytes + kk * 32), (c | kk) != 0);
+        else
+          wgmma_ss<128, BF16>(s, make_desc(q_base + c * kBoxBytes + kk * 32),
+                              make_desc(ring_base + (i + c) % NS * kBoxBytes + kk * 32), (c | kk) != 0);
+      }
     wgmma_commit();
   };
+  // P as the A operand of P V: 16-bit fragments of 8 k16 steps, or e4m3 fragments of 4 k32 steps
+  using PFrag = uint32_t[FP8 ? 4 : 8][4];
   // O += P V of the tile whose first V box is ring index i: one commit group
-  auto issue_pv = [&](float (&o)[NVB][32], const uint32_t (&pa)[8][4], uint32_t i) {
+  auto issue_pv = [&](float (&o)[NVB][32], const PFrag& pa, uint32_t i) {
 #pragma unroll
-    for (int v = 0; v < NVB; ++v) wait_full(i + v, 7);
+    for (int v = 0; v < KVB; ++v) wait_full(i + v, 7);
     wgmma_fence();
+    if constexpr (FP8) {
 #pragma unroll
-    for (int v = 0; v < NVB; ++v)
+      for (int v = 0; v < NVB; ++v)
 #pragma unroll
-      for (int kk = 0; kk < 8; ++kk)
-        wgmma_rs<64, BF16>(o[v], pa[kk], make_desc(ring_base + (i + v) % NS * kBoxBytes + kk * 2048));
+        for (int kk = 0; kk < 4; ++kk)
+          wgmma_rs_e4m3_n64(o[v], pa[kk], make_desc(ring_base + i % NS * kBoxBytes + v * 8192 + kk * 32));
+    } else {
+#pragma unroll
+      for (int v = 0; v < NVB; ++v)
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk)
+          wgmma_rs<64, BF16>(o[v], pa[kk], make_desc(ring_base + (i + v) % NS * kBoxBytes + kk * 2048));
+    }
     wgmma_commit();
+  };
+  auto pack = [&](const float (&s)[64], PFrag& pa) {
+    if constexpr (FP8) pack_p_e4m3(s, pa, lane);
+    else pack_p<BF16>(s, pa);
+  };
+  // after the P V whose first V box is ring index i completed: O is final in registers, release the V boxes
+  auto pv_done = [&](float (&o)[NVB][32], uint32_t i) {
+    if constexpr (FP8) {
+#pragma unroll
+      for (int v = 0; v < NVB; ++v) fence_regs(o[v]);
+      release(i);
+    } else {
+#pragma unroll
+      for (int v = 0; v < NVB; ++v) {
+        fence_regs(o[v]);
+        release(i + v);
+      }
+    }
   };
   // Ping-pong turns.  Warpgroup cw waits on its own named barrier (id 1 + cw) before it issues its GEMMs and hands
   // the turn over by arriving on the other's (id 2 - cw) after it committed them; a phase counts 256 threads (128
@@ -524,9 +596,12 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
       return p.pad_bits == nullptr && j0 + kTileN <= p.M && (!p.causal || j0 + kTileN - 1 <= n_wg + p.causal_shift);
     };
 
+    // FP8: q_descale * k_descale of the head factors out of every score of the segment
+    float sl2 = 0.f;
+    if constexpr (FP8) sl2 = p.scale_log2 * p.q_descale[sg.h] * p.k_descale[sg.h];
     if constexpr (kPipelined) {
       float s[64], alpha[2];
-      uint32_t pa[8][4];
+      PFrag pa;
       uint32_t ik = it;  // ring index of the first K box of the current tile
       if (sg.t1 > sg.t0) {
         // prologue: S of the first tile, its softmax (O is still zero: nothing to rescale)
@@ -537,11 +612,12 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
         fence_regs(s);
 #pragma unroll
         for (int c = 0; c < NQB; ++c) release(ik + c);
-        tile_softmax<DROP>(s, m_run, l_run, alpha, p, sg.b, sg.t0 * kTileN, n0, cq, interior(sg.t0 * kTileN), qside);
-        pack_p<BF16>(s, pa);
+        tile_softmax<DROP, FP8>(s, m_run, l_run, alpha, p, sg.b, sg.t0 * kTileN, n0, cq, interior(sg.t0 * kTileN), qside,
+                                sl2);
+        pack(s, pa);
         for (int t = sg.t0 + 1; t < sg.t1; ++t) {
           const uint32_t iv = ik + NQB;  // V boxes of tile t - 1
-          ik += NQB + NVB;
+          ik += NQB + KVB;
           turn_begin();
           issue_qk(s, ik);
           issue_pv(o, pa, iv);
@@ -550,28 +626,20 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
           fence_regs(s);
 #pragma unroll
           for (int c = 0; c < NQB; ++c) release(ik + c);
-          tile_softmax<DROP>(s, m_run, l_run, alpha, p, sg.b, t * kTileN, n0, cq, interior(t * kTileN), qside);
+          tile_softmax<DROP, FP8>(s, m_run, l_run, alpha, p, sg.b, t * kTileN, n0, cq, interior(t * kTileN), qside, sl2);
           wgmma_wait<0>();
-#pragma unroll
-          for (int v = 0; v < NVB; ++v) {
-            fence_regs(o[v]);
-            release(iv + v);
-          }
+          pv_done(o, iv);
           rescale_o(o, alpha);
-          pack_p<BF16>(s, pa);
+          pack(s, pa);
         }
         // epilogue: P V of the last tile
         turn_begin();
         issue_pv(o, pa, ik + NQB);
         turn_end(si + 1 == seg_hi);  // the last turn of this CTA
         wgmma_wait<0>();
-#pragma unroll
-        for (int v = 0; v < NVB; ++v) {
-          fence_regs(o[v]);
-          release(ik + NQB + v);
-        }
+        pv_done(o, ik + NQB);
       }
-      it += (uint32_t)(sg.t1 - sg.t0) * (NQB + NVB);
+      it += (uint32_t)(sg.t1 - sg.t0) * (NQB + KVB);
     } else {
       for (int t = sg.t0; t < sg.t1; ++t) {
         float s[64];
@@ -622,6 +690,21 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
       for (int v = 0; v < NVB; ++v)
 #pragma unroll
         for (int i = 0; i < 32; ++i) o[v][i] *= p.drop.scale;
+    }
+    if constexpr (FP8) {  // P was scaled by 2^8 before rounding; v_descale of the channel, once for every store below
+      const float* vd = p.v_descale + (int64_t)sg.h * p.v_descale_stride + p.dv_off;
+#pragma unroll
+      for (int v = 0; v < NVB; ++v)
+#pragma unroll
+        for (int g = 0; g < 8; ++g) {
+          const int c = v * 64 + 8 * g + cq;  // dv_pass is a multiple of 16: c and c + 1 are both in or both out
+          const float d0 = c < p.dv_pass ? vd[c] * (1.f / 256.f) : 0.f;
+          const float d1 = c < p.dv_pass ? vd[c + 1] * (1.f / 256.f) : 0.f;
+          o[v][4 * g + 0] *= d0;
+          o[v][4 * g + 1] *= d1;
+          o[v][4 * g + 2] *= d0;
+          o[v][4 * g + 3] *= d1;
+        }
     }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
@@ -686,6 +769,15 @@ __global__ void __launch_bounds__(kThreads, 1)
 attn_fwd_drop_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
                      const __grid_constant__ CUtensorMap tv, const TcParams p) {
   attn_fwd_body<NQB, NVB, BF16, false, true>(tq, tk, tv, p);
+}
+
+// FP8 inference forward (pcv_attn_fwd_fp8): e4m3 Q / K and V^T, output / partial state as attn_fwd_kernel's; a
+// separate kernel, so that the 16-bit kernels' code is unchanged.
+template <int NQB, int NVB, bool BF16>
+__global__ void __launch_bounds__(kThreads, 1)
+attn_fwd_fp8_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
+                    const __grid_constant__ CUtensorMap tv, const TcParams p) {
+  attn_fwd_body<NQB, NVB, BF16, false, false, true>(tq, tk, tv, p);
 }
 
 // --------------------------------------------------------------------------------------------------
@@ -983,6 +1075,34 @@ int launch_dispatch(int nqb, int nvb, bool pair, const Plan& pl, const CUtensorM
   return PCV_ERR_UNSUPPORTED;
 }
 
+template <int NQB, int NVB, bool BF16>
+int launch_fwd_fp8(const Plan& pl, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const TcParams& p,
+                   cudaStream_t stream) {
+  prof_mark_begin(stream);
+  const int rc = launch_kernel(attn_fwd_fp8_kernel<NQB, NVB, BF16>, dim3(pl.num_ctas), kThreads,
+                               FwdCfg<NQB, NVB>::kSmemBytes, 0, stream, tq, tk, tv, p);
+  prof_mark_end(stream);
+  if (rc != PCV_OK) return rc;
+  if (pl.num_units > 0) {
+    dim3 grid(pl.num_units, p.slot_rows / 8);
+    if (NVB == 1)
+      tc_combine_kernel<64, BF16><<<grid, 256, 0, stream>>>(pl.d_units, p);
+    else
+      tc_combine_kernel<128, BF16><<<grid, 256, 0, stream>>>(pl.d_units, p);
+    PCV_CHECK_CUDA(cudaGetLastError());
+    count_launch();
+  }
+  return PCV_OK;
+}
+
+template <bool BF16>
+int launch_dispatch_fp8(int nqb, int nvb, const Plan& pl, const CUtensorMap& tq, const CUtensorMap& tk,
+                        const CUtensorMap& tv, const TcParams& p, cudaStream_t stream) {
+  if (nqb == 1)
+    return nvb == 1 ? launch_fwd_fp8<1, 1, BF16>(pl, tq, tk, tv, p, stream) : launch_fwd_fp8<1, 2, BF16>(pl, tq, tk, tv, p, stream);
+  return nvb == 1 ? launch_fwd_fp8<2, 1, BF16>(pl, tq, tk, tv, p, stream) : launch_fwd_fp8<2, 2, BF16>(pl, tq, tk, tv, p, stream);
+}
+
 }  // namespace
 
 // Host-only (no CUDA call): the work plan of the tensor-core kernel for a problem, one record of 8 ints per segment
@@ -1173,6 +1293,112 @@ int launch_attn_tc(const pcv_attn_params& a, cudaStream_t stream, const pcv_shar
       peer_tail_kernel<false><<<sms, kTailThreads, 0, stream>>>(p);
     PCV_CHECK_CUDA(cudaGetLastError());
     count_launch();
+  }
+  return PCV_OK;
+}
+
+// Host-only (no CUDA call except the device check at the end).
+bool attn_tc_fp8_supported(const pcv_attn_params& p, const pcv_fp8_attn& f, const char** why) {
+  auto fail = [&](const char* w) {
+    *why = w;
+    return false;
+  };
+  if (p.dtype != PCV_E4M3) return fail("q / k / v^T must be e4m3 (dtype PCV_E4M3)");
+  if (f.out_dtype != PCV_BF16 && f.out_dtype != PCV_F16) return fail("out_dtype must be bf16 or fp16");
+  if (p.impl != PCV_IMPL_AUTO && p.impl != PCV_IMPL_TCGEN05)
+    return fail("FP8 runs on the single-CTA tensor-core kernel only (no CTA pair, SIMT or decode kernel)");
+  if (p.dqk > 256) return fail("qk head dim > 256");
+  if (p.dv > 512) return fail("v head dim > 512");
+  if ((p.dqk % 16) || (p.dv % 16)) return fail("head dims must be multiples of 16");
+  if (!(p.scale > 0.f)) return fail("scale must be positive");
+  if (f.q_descale == nullptr || f.k_descale == nullptr || f.v_descale == nullptr) return fail("a descale pointer is NULL");
+  if (!al16(p.q) || !al16(p.k) || !al16(p.v)) return fail("q / k / v^T base pointers must be 16-byte aligned");
+  if ((p.q_stride_n % 16) || (p.k_stride_m % 16) || (p.q_stride_h % 16) || (p.k_stride_h % 16) || (p.q_stride_b % 16) ||
+      (p.k_stride_b % 16) || (f.vt_stride_b % 16) || (f.vt_stride_h % 16) || (f.vt_stride_c % 16))
+    return fail("q / k / v^T strides must be multiples of 16 elements");
+  if (f.vt_stride_c < p.M) return fail("v^T channel stride must cover the M keys");
+  if (p.B > 1 && (p.k_stride_b == 0 || f.vt_stride_b == 0))
+    return fail("k and v^T need a non-zero batch stride when B > 1 (only q broadcasts over the batch)");
+  if (!p.write_partial) {
+    if (!al16(p.out) || (p.o_stride_n % 8) || (p.o_stride_h % 8) || (p.o_stride_b % 8))
+      return fail("output must be 16-byte aligned with strides in multiples of 8 elements");
+  } else {
+    if (!al16(p.part_o)) return fail("partial output alignment");
+  }
+  if ((int64_t)p.N > (1 << 24) || (int64_t)p.M > (1 << 30)) return fail("sequence too long");
+  if (const char* w = device_problem()) return fail(w);
+  return true;
+}
+
+int launch_attn_tc_fp8(const pcv_attn_params& a, const pcv_fp8_attn& f, cudaStream_t stream) {
+  {
+    const char* why = "";
+    PCV_REQUIRE(attn_tc_fp8_supported(a, f, &why), PCV_ERR_UNSUPPORTED, "FP8 tensor-core attention: %s", why);
+  }
+  std::shared_ptr<Plan> pl;
+  const Mode mode = choose_mode(a);
+  int rc = attach_wait_diag(&g_wait_diag);
+  if (rc != PCV_OK) return rc;
+  rc = get_plan(a.B, a.H, a.N, a.M, mode, &pl);
+  if (rc != PCV_OK) return rc;
+  size_t need = 0;
+  rc = attn_tc_workspace_bytes(a, &need);
+  if (rc != PCV_OK) return rc;
+  PCV_REQUIRE(need == 0 || (a.workspace != nullptr && a.workspace_bytes >= need), PCV_ERR_WORKSPACE,
+              "FP8 tensor-core attention: workspace of %zu bytes required, %zu given", need, a.workspace_bytes);
+  PCV_REQUIRE(need == 0 || (reinterpret_cast<uintptr_t>(a.workspace) & 15) == 0, PCV_ERR_WORKSPACE,
+              "FP8 tensor-core attention: workspace must be 16-byte aligned");
+
+  TcParams p{};
+  p.segs = pl->d_segs;
+  p.cta_seg_begin = pl->d_cta;
+  p.B = a.B; p.H = a.H; p.N = a.N; p.M = a.M; p.dv = a.dv;
+  p.scale_log2 = a.scale * kLog2e;
+  p.causal = a.causal;
+  p.causal_shift = (a.m_total - a.N) - a.m_offset;
+  p.q_bcast = (a.q_stride_b == 0) ? 1 : 0;
+  p.out = a.out; p.osb = a.o_stride_b; p.osn = a.o_stride_n; p.osh = a.o_stride_h;
+  p.write_partial = a.write_partial;
+  p.rows_per_unit = mode.rows_per_unit;
+  p.slot_rows = mode.slot_rows;
+  p.fin_o = a.part_o; p.fin_m = a.part_m; p.fin_l = a.part_l;
+  p.q_descale = f.q_descale; p.k_descale = f.k_descale; p.v_descale = f.v_descale;
+  p.v_descale_stride = a.dv;
+  const int slot_dv = dv_pass_width(a.dv);
+  char* ws = reinterpret_cast<char*>(a.workspace);
+  const size_t nrows = (size_t)pl->num_slots * mode.slot_rows;
+  p.slot_o = reinterpret_cast<float*>(ws);
+  p.slot_m = p.slot_o + nrows * slot_dv;
+  p.slot_l = p.slot_m + nrows;
+  if (a.pad_mask != nullptr) {
+    size_t off = (slots_bytes(*pl, slot_dv, mode.slot_rows) + 255) / 256 * 256;
+    uint32_t* bits = reinterpret_cast<uint32_t*>(ws + off);
+    p.pad_bits = bits;
+    p.pad_wpr = pad_words_per_row(a.M);
+    rc = launch_pack_pad(a.pad_mask, a.pad_stride_b, a.B, a.M, bits, stream);
+    if (rc != PCV_OK) return rc;
+  }
+
+  CUtensorMap tq, tk, tv;
+  const int Bq = a.q_stride_b == 0 ? 1 : a.B;
+  rc = make_tmap_4d(&tq, a.q, PCV_E4M3, a.dqk, a.N, a.H, Bq, a.q_stride_n, a.q_stride_h, a.q_stride_b, kTileM);
+  if (rc != PCV_OK) return rc;
+  rc = make_tmap_4d(&tk, a.k, PCV_E4M3, a.dqk, a.M, a.H, a.B, a.k_stride_m, a.k_stride_h, a.k_stride_b, kTileN);
+  if (rc != PCV_OK) return rc;
+  const bool bf = f.out_dtype == PCV_BF16;
+  const int nqb = (a.dqk + 127) / 128;
+  // one launch per slice of at most 128 V channels; V^T is viewed as (keys M, channels of the slice, H, B), so keys
+  // past M and channels past the slice read as zero
+  for (int off = 0; off < a.dv; off += kMaxDvPass) {
+    p.dv_off = off;
+    p.dv_pass = std::min(kMaxDvPass, a.dv - off);
+    const int nvb = (p.dv_pass + 63) / 64;
+    const char* vbase = reinterpret_cast<const char*>(a.v) + (size_t)off * f.vt_stride_c;
+    rc = make_tmap_4d(&tv, vbase, PCV_E4M3, a.M, p.dv_pass, a.H, a.B, f.vt_stride_c, f.vt_stride_h, f.vt_stride_b, kMaxDvPass);
+    if (rc != PCV_OK) return rc;
+    rc = bf ? launch_dispatch_fp8<true>(nqb, nvb, *pl, tq, tk, tv, p, stream)
+            : launch_dispatch_fp8<false>(nqb, nvb, *pl, tq, tk, tv, p, stream);
+    if (rc != PCV_OK) return rc;
   }
   return PCV_OK;
 }

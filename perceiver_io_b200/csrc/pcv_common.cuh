@@ -92,6 +92,9 @@ int launch_attn_tc(const pcv_attn_params& p, cudaStream_t stream, const pcv_shar
                    const DropoutRule* drop = nullptr);
 bool attn_tc_fuse_supported(const pcv_attn_params& p, const char** why);
 int attn_tc_workspace_bytes(const pcv_attn_params& p, size_t* bytes);
+// the FP8 forward (attn_fwd_fp8_kernel): e4m3 q / k / V^T; workspace as attn_tc_workspace_bytes
+bool attn_tc_fp8_supported(const pcv_attn_params& p, const pcv_fp8_attn& f, const char** why);
+int launch_attn_tc_fp8(const pcv_attn_params& p, const pcv_fp8_attn& f, cudaStream_t stream);
 int debug_read(uint32_t* out, int n);  // the watchdog record of the wgmma kernels (16 words)
 int debug_plan(int B, int H, int N, int M, int workers, int rows_per_unit, int rows_per_tile, int32_t* segs,
                int max_segs, int32_t* counts);  // host-only dump of the tcgen05 work plan
@@ -113,6 +116,8 @@ int launch_kv_append(const pcv_kv_append_params& p, cudaStream_t stream);
 int launch_ln_stats(const pcv_ln_stats_params& p, cudaStream_t stream);
 bool kv_project_supported(const pcv_kvproj_params& p, const char** why);
 int launch_kv_project(const pcv_kvproj_params& p, cudaStream_t stream);
+bool kv_project_fp8_supported(const pcv_kvproj_params& p, const pcv_kvproj_fp8& f, const char** why);
+int launch_kv_project_fp8(const pcv_kvproj_params& p, const pcv_kvproj_fp8& f, cudaStream_t stream);
 // shard == nullptr: the backward over all keys (pcv_attn_bwd); else one key shard's (pcv_attn_bwd_shard)
 bool attn_bwd_supported(const pcv_attn_bwd_params& p, const pcv_key_shard* shard, const char** why);
 int attn_bwd_workspace_bytes(const pcv_attn_bwd_params& p, const pcv_key_shard* shard, size_t* bytes);

@@ -52,14 +52,28 @@ struct GemmParams {
   float eps;             // LayerNorm epsilon of the in-kernel statistics
 };
 
+// e4m3 outputs of kvproj_fp8_kernel (its own argument, so that kvproj_kernel's parameters are unchanged): column n is
+// multiplied by inv_scale[n] and rounded to e4m3 (satfinite); K columns go to k_out as e4m3 rows, V columns to vt_out
+// transposed, (B, H, dv, keys), row r being key r % keys_per_batch of batch row r / keys_per_batch (a 128-row tile
+// may cross a batch boundary)
+struct Fp8Out {
+  const float* inv_scale;
+  void* vt_out;
+  int64_t vt_sb, vt_sh, vt_sc;
+  int64_t keys_per_batch;
+  int v_dv;              // channels per V head
+};
+
 struct GemmSmem {
   uint64_t full[kStages], empty[kStages];
   float2 row_st[kBM];
 };
 
-template <bool BF16, bool FUSE, int CG>
-__global__ void __launch_bounds__(kGemmThreads, 1)
-kvproj_kernel(const __grid_constant__ CUtensorMap tx, const __grid_constant__ CUtensorMap tw, const GemmParams p) {
+// The body of kvproj_kernel (F8 = false: 16-bit outputs) and kvproj_fp8_kernel (F8 = true: e4m3 outputs, see Fp8Out)
+template <bool BF16, bool FUSE, int CG, bool F8>
+__device__ __forceinline__ void kvproj_body(const CUtensorMap& tx, const CUtensorMap& tw, const GemmParams& p,
+                                            const Fp8Out& f8) {
+  static_assert(!F8 || CG == 1, "the e4m3 producer runs one CTA per tile");
   using T = typename std::conditional<BF16, __nv_bfloat16, __half>::type;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -190,14 +204,42 @@ kvproj_kernel(const __grid_constant__ CUtensorMap tx, const __grid_constant__ CU
         a0 = st.y * (a0 - st.x * c0.x);
         a1 = st.y * (a1 - st.x * c1.x);
       }
-      const uint32_t w = pack2(a0 + c0.y, a1 + c1.y, BF16);
-      if (n < p.n_k)
-        *reinterpret_cast<uint32_t*>(reinterpret_cast<T*>(p.k_out) + row * p.k_stride + n) = w;
-      else
-        *reinterpret_cast<uint32_t*>(reinterpret_cast<T*>(p.v_out) + row * p.v_stride + (n - p.n_k)) = w;
+      if constexpr (F8) {
+        const uint32_t w8 = cvt_e4m3x2((a0 + c0.y) * f8.inv_scale[n], (a1 + c1.y) * f8.inv_scale[n + 1]);
+        if (n < p.n_k) {
+          *reinterpret_cast<uint16_t*>(reinterpret_cast<uint8_t*>(p.k_out) + row * p.k_stride + n) = (uint16_t)w8;
+        } else {  // channels c and c + 1 of one head (dv is even): two rows of V^T, key m
+          const int c = n - p.n_k, h = c / f8.v_dv;
+          const int64_t b = row / f8.keys_per_batch, m = row - b * f8.keys_per_batch;
+          uint8_t* dst = reinterpret_cast<uint8_t*>(f8.vt_out) + b * f8.vt_sb + h * f8.vt_sh +
+                         (int64_t)(c - h * f8.v_dv) * f8.vt_sc + m;
+          dst[0] = (uint8_t)(w8 & 0xffu);
+          dst[f8.vt_sc] = (uint8_t)(w8 >> 8);
+        }
+      } else {
+        const uint32_t w = pack2(a0 + c0.y, a1 + c1.y, BF16);
+        if (n < p.n_k)
+          *reinterpret_cast<uint32_t*>(reinterpret_cast<T*>(p.k_out) + row * p.k_stride + n) = w;
+        else
+          *reinterpret_cast<uint32_t*>(reinterpret_cast<T*>(p.v_out) + row * p.v_stride + (n - p.n_k)) = w;
+      }
     }
   }
   if (CG == 2) cluster_sync_all();
+}
+
+template <bool BF16, bool FUSE, int CG>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+kvproj_kernel(const __grid_constant__ CUtensorMap tx, const __grid_constant__ CUtensorMap tw, const GemmParams p) {
+  kvproj_body<BF16, FUSE, CG, false>(tx, tw, p, Fp8Out{});
+}
+
+// LayerNorm-folded projection with e4m3 outputs (pcv_kv_project_fp8): a separate kernel, one CTA per tile
+template <bool BF16, bool FUSE>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+kvproj_fp8_kernel(const __grid_constant__ CUtensorMap tx, const __grid_constant__ CUtensorMap tw, const GemmParams p,
+                  const Fp8Out f8) {
+  kvproj_body<BF16, FUSE, 1, true>(tx, tw, p, f8);
 }
 
 
@@ -328,14 +370,20 @@ int launch_ln_stats_t(const pcv_ln_stats_params& p, cudaStream_t stream) {
   return PCV_OK;
 }
 
-template <bool BF16, bool FUSE, int CG>
-int launch_gemm(const CUtensorMap& tx, const CUtensorMap& tw, const GemmParams& gp, cudaStream_t stream) {
+template <bool BF16, bool FUSE, int CG, bool F8 = false>
+int launch_gemm(const CUtensorMap& tx, const CUtensorMap& tw, const GemmParams& gp, cudaStream_t stream,
+                const Fp8Out& f8 = Fp8Out{}) {
   const int64_t m_blocks = (gp.rows + kBM * CG - 1) / (kBM * CG) * CG;  // whole pairs; a pair's spare block is all padding
   const int64_t tiles = m_blocks * gp.tiles_n;
   PCV_REQUIRE(tiles <= 0x7fffffff, PCV_ERR_UNSUPPORTED, "kv_project: %lld tiles exceed the grid limit", (long long)tiles);
   prof_mark_begin(stream);
-  const int rc = launch_kernel(kvproj_kernel<BF16, FUSE, CG>, dim3((unsigned)tiles), kGemmThreads, kSmemBytes, CG, stream,
-                               tx, tw, gp);
+  int rc;
+  if constexpr (F8)
+    rc = launch_kernel(kvproj_fp8_kernel<BF16, FUSE>, dim3((unsigned)tiles), kGemmThreads, kSmemBytes, 0, stream, tx, tw,
+                       gp, f8);
+  else
+    rc = launch_kernel(kvproj_kernel<BF16, FUSE, CG>, dim3((unsigned)tiles), kGemmThreads, kSmemBytes, CG, stream,
+                       tx, tw, gp);
   prof_mark_end(stream);
   return rc;
 }
@@ -367,6 +415,69 @@ bool kv_project_supported(const pcv_kvproj_params& p, const char** why) {
   if (p.cta_group < 0 || p.cta_group > 2) return fail("cta_group must be 0, 1 or 2");
   if (const char* w = device_problem()) return fail(w);
   return true;
+}
+
+bool kv_project_fp8_supported(const pcv_kvproj_params& p, const pcv_kvproj_fp8& f, const char** why) {
+  auto fail = [&](const char* w) {
+    *why = w;
+    return false;
+  };
+  if (f.inv_scale == nullptr) return fail("inv_scale is NULL");
+  if (p.cta_group == 2) return fail("the e4m3 producer runs one CTA per tile (cta_group 0 or 1)");
+  if (p.n_k % 16) return fail("K width must be a multiple of 16");
+  if (p.n_v > 0) {
+    if (f.vt_out == nullptr) return fail("vt_out is NULL");
+    if (f.v_head_dim < 16 || (f.v_head_dim % 16) || (p.n_v % f.v_head_dim)) return fail("v_head_dim must be a multiple of 16 dividing n_v");
+    if (f.keys_per_batch < 1 || (p.rows % f.keys_per_batch)) return fail("keys_per_batch must divide the row count");
+    if (f.vt_stride_c < f.keys_per_batch || (f.vt_stride_c % 16) || (f.vt_stride_h % 16) || (f.vt_stride_b % 16))
+      return fail("v^T strides must be multiples of 16 bytes and cover keys_per_batch keys");
+  }
+  if (p.n_k > 0 && (p.k_stride_row % 16)) return fail("the e4m3 K row stride must be a multiple of 16 bytes");
+  // the 16-bit conditions of pcv_kv_project (v_out / v_stride_row are unused here)
+  pcv_kvproj_params q = p;
+  q.v_out = q.k_out != nullptr ? q.k_out : const_cast<void*>(q.x);
+  q.v_stride_row = 0;
+  q.k_stride_row = 0;
+  return kv_project_supported(q, why);
+}
+
+int launch_kv_project_fp8(const pcv_kvproj_params& p, const pcv_kvproj_fp8& f, cudaStream_t stream) {
+  const char* why = "";
+  PCV_REQUIRE(p.x && p.w && p.col_st, PCV_ERR_INVALID, "kv_project_fp8: NULL pointer");
+  PCV_REQUIRE(kv_project_fp8_supported(p, f, &why), PCV_ERR_UNSUPPORTED, "kv_project_fp8: %s", why);
+  const int n_total = p.n_k + p.n_v;
+  GemmParams gp{};
+  gp.stats = reinterpret_cast<const float2*>(p.row_stats);
+  gp.col_st = reinterpret_cast<const float2*>(p.col_st);
+  gp.k_out = p.k_out;
+  gp.x = p.x;
+  gp.x_stride = p.x_stride_row;
+  gp.k_stride = p.k_stride_row;
+  gp.rows = p.rows;
+  gp.n_k = p.n_k;
+  gp.n_total = n_total;
+  gp.num_kb = (p.C + kBK - 1) / kBK;
+  gp.tiles_n = (n_total + kBN - 1) / kBN;
+  gp.C = p.C;
+  gp.eps = p.ln_eps;
+  Fp8Out f8{};
+  f8.inv_scale = f.inv_scale;
+  f8.vt_out = f.vt_out;
+  f8.vt_sb = f.vt_stride_b; f8.vt_sh = f.vt_stride_h; f8.vt_sc = f.vt_stride_c;
+  f8.keys_per_batch = f.keys_per_batch > 0 ? f.keys_per_batch : p.rows;
+  f8.v_dv = f.v_head_dim > 0 ? f.v_head_dim : 16;
+  const bool fuse = p.row_stats == nullptr && p.ln_eps > 0.f;
+  int rc = attach_wait_diag(&g_wait_diag);
+  if (rc != PCV_OK) return rc;
+  CUtensorMap tx, tw;
+  rc = make_tmap_2d(&tx, p.x, p.dtype, p.C, p.rows, p.x_stride_row, kBM);
+  if (rc != PCV_OK) return rc;
+  rc = make_tmap_2d(&tw, p.w, p.dtype, p.C, n_total, p.C, kBN);
+  if (rc != PCV_OK) return rc;
+  const bool bf = p.dtype == PCV_BF16;
+  if (fuse)
+    return bf ? launch_gemm<true, true, 1, true>(tx, tw, gp, stream, f8) : launch_gemm<false, true, 1, true>(tx, tw, gp, stream, f8);
+  return bf ? launch_gemm<true, false, 1, true>(tx, tw, gp, stream, f8) : launch_gemm<false, false, 1, true>(tx, tw, gp, stream, f8);
 }
 
 int launch_kv_project(const pcv_kvproj_params& p, cudaStream_t stream) {

@@ -301,12 +301,43 @@ __device__ __forceinline__ void wgmma_rs<64, false>(float (&d)[32], const uint32
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
 }
 
+// ---- e4m3 (FP8) wgmma ---------------------------------------------------------------------------
+// 8-bit operands have no transpose: A and B are both K-major.  A k32 step covers 32 bytes of a 128-byte SWIZZLE_128B
+// row, so the descriptors step exactly as the 16-bit k16 ones do.
+// D(64 x 128, f32) (+)= A(64 x 32 e4m3, K-major smem) * B(32 x 128 e4m3, K-major smem); scale_d = 0 overwrites D.
+__device__ __forceinline__ void wgmma_ss_e4m3_n128(float (&d)[64], uint64_t a, uint64_t b, int scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a), "l"(b), "r"(scale_d));
+}
+// D(64 x 64, f32) += A(64 x 32 e4m3, registers) * B(32 x 64 e4m3, K-major smem).  A fragment (thread t of the
+// warpgroup, l = t % 32, q = l % 4): register 0 holds row 16*w + l/4, columns 4q .. 4q+3 (lowest byte first);
+// register 1 the same columns of row + 8; registers 2 and 3 columns 16 + 4q .. 16 + 4q + 3 of those two rows.
+__device__ __forceinline__ void wgmma_rs_e4m3_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t b) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k32.f32.e4m3.e4m3 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b));
+}
+// two floats -> two e4m3 bytes (round to nearest even, saturating at +-448), `lo` in the low byte
+__device__ __forceinline__ uint32_t cvt_e4m3x2(float lo, float hi) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+
 // ---- host ------------------------------------------------------------------------------------
 // nullptr when the current device has compute capability 9, else why the wgmma kernels cannot run on it
 const char* device_problem();
 
-// SWIZZLE_128B tensor maps of 16-bit operands with 64-channel boxes (L2_256B promotion, no OOB fill).
-// 4-D (channels, rows, heads, batch) view of a (batch, rows, heads*channels)-style tensor, box 64 x box_rows x 1 x 1;
+// SWIZZLE_128B tensor maps with 128-byte box rows: 64 channels of a 16-bit dtype, 128 of PCV_E4M3 (L2_256B
+// promotion; out-of-bounds elements read as zero).  Strides are in elements of `dtype`.
+// 4-D (channels, rows, heads, batch) view of a (batch, rows, heads*channels)-style tensor, box 128 bytes x box_rows x 1 x 1;
 // stride_batch == 0 broadcasts one batch row to every b (batch must then be 1).
 int make_tmap_4d(CUtensorMap* tm, const void* base, int dtype, int channels, int rows, int heads, int batch,
                  int64_t stride_row, int64_t stride_head, int64_t stride_batch, int box_rows);

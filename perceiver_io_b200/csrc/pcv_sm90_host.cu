@@ -29,7 +29,9 @@ int encode(CUtensorMap* tm, int dtype, int rank, const void* base, const cuuint6
   auto fn = encode_fn();
   PCV_REQUIRE(fn != nullptr, PCV_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
   const cuuint32_t estr[4] = {1, 1, 1, 1};
-  const CUtensorMapDataType dt = dtype == PCV_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const CUtensorMapDataType dt = dtype == PCV_BF16   ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16
+                                 : dtype == PCV_E4M3 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                                                     : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   CUresult r = fn(tm, dt, rank, const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   PCV_REQUIRE(r == CUDA_SUCCESS, PCV_ERR_CUDA, "cuTensorMapEncodeTiled (%d-D) failed with CUresult %d", rank, (int)r);
@@ -56,8 +58,9 @@ int make_tmap_4d(CUtensorMap* tm, const void* base, int dtype, int channels, int
                  int64_t stride_row, int64_t stride_head, int64_t stride_batch, int box_rows) {
   const cuuint64_t dims[4] = {(cuuint64_t)channels, (cuuint64_t)rows, (cuuint64_t)heads, (cuuint64_t)batch};
   if (stride_batch == 0) stride_batch = (int64_t)rows * stride_row;  // broadcast batch: dim is 1, stride unused
-  const cuuint64_t strides[3] = {(cuuint64_t)stride_row * 2, (cuuint64_t)stride_head * 2, (cuuint64_t)stride_batch * 2};
-  const cuuint32_t box[4] = {64, (cuuint32_t)box_rows, 1, 1};
+  const int es = dtype == PCV_E4M3 ? 1 : 2;  // bytes per element
+  const cuuint64_t strides[3] = {(cuuint64_t)stride_row * es, (cuuint64_t)stride_head * es, (cuuint64_t)stride_batch * es};
+  const cuuint32_t box[4] = {(cuuint32_t)(128 / es), (cuuint32_t)box_rows, 1, 1};
   return encode(tm, dtype, 4, base, dims, strides, box);
 }
 

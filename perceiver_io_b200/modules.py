@@ -229,6 +229,76 @@ def project_qkv(self_attn, x: torch.Tensor):
     return q, kv[..., :n_k], kv[..., n_k:]
 
 
+#: FP8 (e4m3) inference route of ``CrossAttention.forward`` with ``x_kv`` (this package's class and reference modules
+#: rebound by ``patch()``): q, K and V^T come out of the LayerNorm-folded producer as e4m3 (``ops.kv_project_fp8``,
+#: scales derived once per weight set by ``ops.fp8_descales``) and the attention runs on the e4m3 tensor cores
+#: (``ops.attention_fp8``).  Off by default because it changes the numbers; calls it does not cover (training mode,
+#: autograd, fp32, rotary, a KV cache, head dims that are not multiples of 16 or dqk > 256) take the bf16 path.
+fp8_config = {"enabled": False}
+
+
+def _fp8_scales(cross_attn, dtype: torch.dtype):
+    """(q_descale (H,), k_descale (H,), v_descale (H, dv), inv_q (n_q,), inv_kv (n_k + n_v,)) of a CrossAttention,
+    cached on it next to the folded weights and rebuilt when a parameter changes (as ``_fold_cache``)."""
+    attn, H = cross_attn.attention, cross_attn.attention.num_heads
+    qn, kvn = cross_attn.q_norm, cross_attn.kv_norm
+    tensors = [qn.weight, qn.bias, kvn.weight, kvn.bias] + [t for lin in (attn.q_proj, attn.k_proj, attn.v_proj)
+                                                             for t in (lin.weight, lin.bias)]
+    key = (dtype,) + tuple((None if t is None else (t.data_ptr(), t._version)) for t in tensors)
+    hit = cross_attn.__dict__.get("_pcv_fp8_scales")
+    if hit is not None and hit[0] == key:
+        return hit[1]
+    qd = ops.fp8_descales(qn.weight, qn.bias, attn.q_proj.weight, attn.q_proj.bias, H)
+    kd = ops.fp8_descales(kvn.weight, kvn.bias, attn.k_proj.weight, attn.k_proj.bias, H)
+    vd = ops.fp8_descales(kvn.weight, kvn.bias, attn.v_proj.weight, attn.v_proj.bias, H, per_channel=True)
+    dqk = attn.q_proj.out_features // H
+    inv_q = (1.0 / qd).repeat_interleave(dqk).contiguous()
+    inv_kv = torch.cat([(1.0 / kd).repeat_interleave(attn.k_proj.out_features // H), (1.0 / vd).reshape(-1)]).contiguous()
+    val = (qd, kd, vd, inv_q, inv_kv)
+    cross_attn.__dict__["_pcv_fp8_scales"] = (key, val)
+    return val
+
+
+def _fp8_cross_attention(cross_attn, x_q, x_kv, pad_mask, rot_pos_emb_q, rot_pos_emb_k, kv_cache):
+    """The FP8 route of CrossAttention.forward, or None when it does not cover the call."""
+    if not fp8_config["enabled"] or rot_pos_emb_q is not None or rot_pos_emb_k is not None or kv_cache is not None:
+        return None
+    attn = cross_attn.attention
+    if cross_attn.training or attn.training or x_q.dim() != 3 or x_kv.dim() != 3 or x_q.dtype != x_kv.dtype:
+        return None
+    H = attn.num_heads
+    n_q, n_k, n_v = attn.q_proj.out_features, attn.k_proj.out_features, attn.v_proj.out_features
+    if n_q != n_k or n_q % H or n_v % H:
+        return None
+    dqk, dv = n_q // H, n_v // H
+    if dqk % 16 or dv % 16 or dqk > 256 or dv > 512:
+        return None
+    for norm, x, lins in ((cross_attn.q_norm, x_q, [attn.q_proj]), (cross_attn.kv_norm, x_kv, [attn.k_proj, attn.v_proj])):
+        if not isinstance(norm, nn.LayerNorm) or norm.weight is None:
+            return None
+        if not x.is_cuda or x.dtype not in (torch.bfloat16, torch.float16) or len(norm.normalized_shape) != 1:
+            return None
+        if norm.normalized_shape[0] != x.shape[-1] or any(l.weight.dtype != x.dtype or l.in_features != x.shape[-1]
+                                                          for l in lins):
+            return None
+        if torch.is_autocast_enabled():
+            return None
+        if torch.is_grad_enabled() and (x.requires_grad or norm.weight.requires_grad
+                                        or any(l.weight.requires_grad for l in lins)):
+            return None
+    if not (ops.kv_project_fp8_supported(x_q, n_q, 0, H) and ops.kv_project_fp8_supported(x_kv, n_k, n_v, H)):
+        return None
+    qd, kd, vd, inv_q, inv_kv = _fp8_scales(cross_attn, x_kv.dtype)
+    wq, stq = _fold_cache(cross_attn, "_pcv_q_fold", cross_attn.q_norm, [attn.q_proj], x_q.dtype)
+    wkv, stkv = _fold_cache(cross_attn, "_pcv_kv_fold", cross_attn.kv_norm, [attn.k_proj, attn.v_proj], x_kv.dtype)
+    q8, _ = ops.kv_project_fp8(x_q, wq, stq, inv_q, n_q, 0, H, eps=cross_attn.q_norm.eps)
+    k8, vt8 = ops.kv_project_fp8(x_kv, wkv, stkv, inv_kv, n_k, n_v, H, eps=cross_attn.kv_norm.eps)
+    o = ops.attention_fp8(q8, k8, vt8, qd, kd, vd, H, attn.dp_scale, pad_mask=pad_mask, causal=attn.causal_attention,
+                          out_dtype=x_kv.dtype)
+    o = fused_linear(attn, "_pcv_o_fold", None, attn.o_proj, o)
+    return ModuleOutput(last_hidden_state=o, kv_cache=None)
+
+
 class CrossAttention(nn.Module):
     """Pre-LayerNorm cross-attention (reference modules.py:173-230)."""
 
@@ -278,6 +348,9 @@ class CrossAttention(nn.Module):
             x_kv = torch.cat([self.kv_norm(x_kv_prefix), x_q], dim=1)
             return self.attention(x_q, x_kv, pad_mask=pad_mask, rot_pos_emb_q=rot_pos_emb_q,
                                   rot_pos_emb_k=rot_pos_emb_k, kv_cache=kv_cache)
+        out = _fp8_cross_attention(self, x_q, x_kv, pad_mask, rot_pos_emb_q, rot_pos_emb_k, kv_cache)
+        if out is not None:
+            return out
         q = fused_linear(self, "_pcv_q_fold", self.q_norm, self.attention.q_proj, x_q)
         k, v = project_kv(self, x_kv)
         return attend(self.attention, q, k, v, pad_mask, rot_pos_emb_q, rot_pos_emb_k, kv_cache)

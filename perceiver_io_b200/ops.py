@@ -26,6 +26,8 @@ from ._lib import (AttnParams, CombineParams, KvAppendParams, KvProjParams, LnSt
 __all__ = [
     "attention", "attention_partial", "attention_sharded_fused", "combine_partials", "merge_partials", "rescale_partial_", "rotary", "kv_append",
     "device_info", "tcgen05_supported", "rotated_cache_keys", "ln_stats", "fold_ln_linear", "kv_project", "kv_project_supported",
+    "attention_fp8", "attention_fp8_supported", "fp8_descales", "fp8_quantize", "fp8_transpose_v", "kv_project_fp8",
+    "kv_project_fp8_supported",
 ]
 
 
@@ -65,7 +67,9 @@ def device_info() -> dict:
     return {f[0]: getattr(info, f[0]) for f in info._fields_}
 
 
-def _fill_attn_params(q, k, v, num_heads, scale, pad_mask, causal, m_total, m_offset, impl) -> Tuple[AttnParams, tuple]:
+def _fill_attn_params(q, k, v, num_heads, scale, pad_mask, causal, m_total, m_offset, impl,
+                      dtype: Optional[int] = None) -> Tuple[AttnParams, tuple]:
+    # ``dtype``: the pcv_dtype of the operands when it is not that of q's torch dtype (PCV_E4M3).
     # Each operand is either (B, L, H*d) — heads split by stride arithmetic — or an explicit 4-D
     # (B, L, H, d) view with arbitrary batch/row/head strides (e.g. a head-major (B,H,L,d) buffer permuted).
     def geom(t, name):
@@ -100,7 +104,7 @@ def _fill_attn_params(q, k, v, num_heads, scale, pad_mask, causal, m_total, m_of
     p.v_stride_b, p.v_stride_m, p.v_stride_h = v_sb, v_sm, v_sh
     p.B, p.H, p.N, p.M, p.dqk, p.dv = B, H, N, M, dqk, dv
     p.scale = float(scale)
-    p.dtype = _pcv_dtype(q.dtype)
+    p.dtype = _pcv_dtype(q.dtype) if dtype is None else dtype
     p.causal = 1 if causal else 0
     p.m_total = M if m_total is None else int(m_total)
     p.m_offset = int(m_offset)
@@ -628,6 +632,95 @@ def attention_partial(q, k, v, num_heads: int, scale: float, pad_mask=None, caus
     return part_o, part_m, part_l
 
 
+def _fill_fp8_params(q8, k8, vt8, q_descale, k_descale, v_descale, num_heads, scale, pad_mask, causal, m_total,
+                     m_offset, out_dtype):
+    """(AttnParams, Fp8Attn, tensors to keep alive) of an FP8 forward; shapes as in :func:`attention_fp8`."""
+    _require_cuda(q8, k8, vt8, q_descale, k_descale, v_descale, pad_mask)
+    f8 = torch.float8_e4m3fn
+    for name, t in (("q8", q8), ("k8", k8), ("vt8", vt8)):
+        if t.dtype != f8:
+            raise ValueError(f"attention_fp8: {name} must be torch.float8_e4m3fn, got {t.dtype}")
+    if vt8.dim() != 4 or vt8.stride(3) != 1:
+        raise ValueError("attention_fp8: vt8 must be (B, H, dv, M_pad) with contiguous keys")
+    B, H, dv, m_pad = vt8.shape
+    if H != num_heads:
+        raise ValueError(f"attention_fp8: vt8 has {H} heads, expected {num_heads}")
+    q8, k8 = _rows_contiguous(q8), _rows_contiguous(k8)
+    # the (B, M, H, d) geometry of q / k; v is described by the Fp8Attn strides (its AttnParams strides are unused)
+    v_geom = vt8.as_strided((B, k8.shape[1], H, dv), (0, 0, 0, 1))
+    p, keep = _fill_attn_params(q8, k8, v_geom, num_heads, scale, pad_mask, causal, m_total, m_offset, "tcgen05",
+                                dtype=_lib.PCV_E4M3)
+    if m_pad < p.M:
+        raise ValueError(f"attention_fp8: vt8 holds {m_pad} keys, fewer than the {p.M} of k8")
+    p.v = vt8.data_ptr()
+    p.v_stride_b = p.v_stride_m = p.v_stride_h = 0
+    qd, kd = q_descale.float().contiguous(), k_descale.float().contiguous()
+    vd = v_descale.float().contiguous()
+    if qd.shape != (H,) or kd.shape != (H,) or vd.shape != (H, dv):
+        raise ValueError(f"attention_fp8: descales must be (H,), (H,) and (H, dv) = ({H},), ({H},), ({H}, {dv})")
+    f = _lib.Fp8Attn()
+    f.q_descale, f.k_descale, f.v_descale = qd.data_ptr(), kd.data_ptr(), vd.data_ptr()
+    f.vt_stride_b, f.vt_stride_h, f.vt_stride_c = vt8.stride(0), vt8.stride(1), vt8.stride(2)
+    f.out_dtype = _pcv_dtype(out_dtype)
+    return p, f, keep + (q8, k8, vt8, qd, kd, vd)
+
+
+def attention_fp8_supported(q8, k8, vt8, q_descale, k_descale, v_descale, num_heads: int, scale: float = 1.0,
+                            pad_mask=None, causal: bool = False, m_total: Optional[int] = None, m_offset: int = 0,
+                            out_dtype: torch.dtype = torch.bfloat16, partial: bool = False) -> bool:
+    """Whether :func:`attention_fp8` covers these operands (no launch; the reason is in ``_lib.lib().pcv_last_error()``)."""
+    with torch.cuda.device(k8.device):
+        p, f, keep = _fill_fp8_params(q8, k8, vt8, q_descale, k_descale, v_descale, num_heads, scale, pad_mask, causal,
+                                      m_total, m_offset, out_dtype)
+        dummy = torch.empty(64, device=k8.device)
+        if partial:
+            p.write_partial = 1
+            p.part_o = p.part_m = p.part_l = dummy.data_ptr()
+        else:
+            p.out = dummy.data_ptr()
+            p.o_stride_b, p.o_stride_n, p.o_stride_h = p.N * p.H * p.dv, p.H * p.dv, p.dv
+        return bool(_lib.lib().pcv_attn_fwd_fp8_supported(C.byref(p), C.byref(f)))
+
+
+def attention_fp8(q8, k8, vt8, q_descale, k_descale, v_descale, num_heads: int, scale: float, pad_mask=None,
+                  causal: bool = False, m_total: Optional[int] = None, m_offset: int = 0,
+                  out_dtype: torch.dtype = torch.bfloat16, partial: bool = False):
+    """FP8 (e4m3) inference attention on already quantised operands (pcv_attn_fwd_fp8).
+
+    q8: (B or 1, N, H*dqk), k8: (B, M, H*dqk) (or 4-D (B, L, H, d) views), vt8: V transposed, (B, H, dv, M_pad) with
+    contiguous keys in order and M_pad >= M (a multiple of 16 keeps the strides TMA-aligned), all
+    ``torch.float8_e4m3fn``.  The operands stand for ``q8 * q_descale[h]``, ``k8 * k_descale[h]`` and
+    ``vt8[:, h, c] * v_descale[h, c]`` (float32 descales of shapes (H,), (H,), (H, dv)).  Masks and key sharding
+    (``m_total`` / ``m_offset``) as in :func:`attention_partial`.  Each probability is rounded to e4m3 as
+    ``e4m3(P * 2^8)`` relative to the running row maximum of its 128-key tile; the denominators are fp32 sums of the
+    unrounded probabilities.  Returns (B, N, H*dv) in ``out_dtype`` (bf16 / fp16), or with ``partial`` the fp32 state
+    ``(part_o, part_m, part_l)`` that :func:`combine_partials` merges.  Head dims: multiples of 16, dqk <= 256, dv <= 512.
+    No autograd: this is an inference path."""
+    with torch.cuda.device(k8.device):
+        p, f, keep = _fill_fp8_params(q8, k8, vt8, q_descale, k_descale, v_descale, num_heads, scale, pad_mask, causal,
+                                      m_total, m_offset, out_dtype)
+        dev = k8.device
+        if partial:
+            part_o = torch.empty(p.B, p.H, p.N, p.dv, dtype=torch.float32, device=dev)
+            part_m = torch.empty(p.B, p.H, p.N, dtype=torch.float32, device=dev)
+            part_l = torch.empty(p.B, p.H, p.N, dtype=torch.float32, device=dev)
+            p.write_partial = 1
+            p.part_o, p.part_m, p.part_l = part_o.data_ptr(), part_m.data_ptr(), part_l.data_ptr()
+        else:
+            out = torch.empty(p.B, p.N, p.H * p.dv, dtype=out_dtype, device=dev)
+            p.out = out.data_ptr()
+            p.o_stride_b, p.o_stride_n, p.o_stride_h = out.stride(0), out.stride(1), p.dv
+        need = C.c_size_t(0)
+        check(_lib.lib().pcv_attn_workspace_bytes(C.byref(p), C.byref(need)), "pcv_attn_workspace_bytes")
+        ws = None
+        if need.value:
+            ws = torch.empty(need.value, dtype=torch.uint8, device=dev)
+            p.workspace, p.workspace_bytes = ws.data_ptr(), need.value
+        check(_lib.lib().pcv_attn_fwd_fp8(C.byref(p), C.byref(f), _stream()), "pcv_attn_fwd_fp8")
+    del keep, ws
+    return (part_o, part_m, part_l) if partial else out
+
+
 def attention_sharded_fused(q, k, v, num_heads: int, scale: float, fuse, pad_mask=None, causal: bool = False,
                             m_total: Optional[int] = None, m_offset: int = 0, check_only: bool = False):
     """One launch: partial state of this rank's key shard + cross-GPU merge in the kernel tail (pcv_attn_fwd_sharded).
@@ -1037,6 +1130,31 @@ def fold_ln_linear(norm_weight, norm_bias, weights, biases, dtype: torch.dtype):
     return w_cat, col_st
 
 
+E4M3_MAX = 448.0  # largest finite float8_e4m3fn
+
+
+def fp8_descales(norm_weight, norm_bias, weight, bias, num_heads: int, per_channel: bool = False) -> torch.Tensor:
+    """FP8 dequantisation factors of ``y = LN(x) W^T + b`` derived from the weights alone (once per set of weights).
+
+    For a LayerNorm'd row ``||x_hat||_2 <= sqrt(C)``, so output column n obeys
+    ``|y_n| <= sqrt(C) * ||gamma * W_n||_2 + |t_n|`` with ``t`` the folded bias of :func:`fold_ln_linear`.  Returns that
+    bound / 448 per head (``(H,)``: the max over the head's channels, for q and k) or per channel (``(H, d)``, for v),
+    float32.  Quantising ``y / descale`` to e4m3 then never saturates.  ``norm_weight`` None = no LayerNorm: the bound
+    is not valid then, so it is refused."""
+    if norm_weight is None:
+        raise ValueError("fp8_descales: the bound needs the LayerNorm in front of the projection")
+    w, col_st = fold_ln_linear(norm_weight, norm_bias, [weight], [bias], torch.float32)
+    n, cin = w.shape
+    if n % num_heads:
+        raise ValueError(f"fp8_descales: {n} output channels are not divisible by {num_heads} heads")
+    bound = math.sqrt(cin) * w.double().norm(dim=1) + col_st[:, 1].double().abs()
+    bound = bound.view(num_heads, n // num_heads)
+    if not per_channel:
+        bound = bound.amax(dim=1)
+    # a channel with an all-zero weight row and bias is exactly zero: any positive descale quantises it exactly
+    return (bound / E4M3_MAX).clamp_min(torch.finfo(torch.float32).tiny).float().contiguous()
+
+
 def _fill_kvproj(x2, w_cat, col_st, n_k, n_v, stats, k_out, v_out, cta_group=0, ln_eps=0.0) -> KvProjParams:
     p = KvProjParams()
     p.x, p.w, p.col_st = x2.data_ptr(), w_cat.data_ptr(), col_st.data_ptr()
@@ -1092,3 +1210,97 @@ def kv_project(x: torch.Tensor, w_cat: torch.Tensor, col_st: torch.Tensor, n_k: 
     k = None if k_out is None else k_out.view(*lead, n_k)
     v = None if v_out is None else v_out.view(*lead, n_v)
     return k, v
+
+
+def fp8_quantize(x: torch.Tensor, descale: torch.Tensor, num_heads: int) -> torch.Tensor:
+    """(..., H*d) values -> e4m3 codes of ``x / descale`` (descale (H,) per head or (H, d) per channel), rounded to
+    nearest even and saturated at +-448.  A torch reference of the producer's e4m3 epilogue for tests and tools; the
+    module's FP8 route quantises inside :func:`kv_project_fp8` instead."""
+    H = num_heads
+    xs = x.float().reshape(*x.shape[:-1], H, x.shape[-1] // H)
+    d = descale.float().to(x.device)
+    d = d[:, None] if d.dim() == 1 else d
+    return (xs / d).clamp(-E4M3_MAX, E4M3_MAX).to(torch.float8_e4m3fn).reshape(x.shape)
+
+
+def fp8_transpose_v(v8: torch.Tensor, num_heads: int, m_pad: Optional[int] = None) -> torch.Tensor:
+    """(B, M, H*dv) e4m3 -> V^T (B, H, dv, M_pad) e4m3, keys contiguous and in order (M_pad: M rounded up to 16; the
+    pad keys are zero and never read).  The layout :func:`attention_fp8` takes and :func:`kv_project_fp8` writes."""
+    B, M, Cv = v8.shape
+    dv = Cv // num_heads
+    m_pad = (M + 15) // 16 * 16 if m_pad is None else m_pad
+    vt = torch.zeros(B, num_heads, dv, m_pad, dtype=torch.uint8, device=v8.device)
+    vt[..., :M] = v8.view(torch.uint8).reshape(B, M, num_heads, dv).permute(0, 2, 3, 1)
+    return vt.view(torch.float8_e4m3fn)
+
+
+def _fill_kvproj_fp8(x2, w_cat, col_st, inv_scale, n_k, n_v, stats, k8, vt8, keys_per_batch, v_head_dim, ln_eps):
+    p = _fill_kvproj(x2, w_cat, col_st, n_k, n_v, stats, k8, None, 0, ln_eps)
+    p.k_stride_row = n_k
+    p.v_stride_row = 0
+    f = _lib.KvProjFp8()
+    f.inv_scale = inv_scale.data_ptr()
+    if vt8 is not None:
+        f.vt_out = vt8.data_ptr()
+        f.vt_stride_b, f.vt_stride_h, f.vt_stride_c = vt8.stride(0), vt8.stride(1), vt8.stride(2)
+    f.keys_per_batch = int(keys_per_batch)
+    f.v_head_dim = int(v_head_dim)
+    return p, f
+
+
+def kv_project_fp8_supported(x: torch.Tensor, n_k: int, n_v: int, num_heads: int) -> bool:
+    """Whether :func:`kv_project_fp8` covers x (..., C) with these widths (no launch)."""
+    if not x.is_cuda or x.dtype not in (torch.bfloat16, torch.float16) or x.dim() < 2:
+        return False
+    x2 = _rows2d(x)
+    rows = x2.shape[0]
+    p = KvProjParams()
+    p.x = p.w = p.col_st = x2.data_ptr()
+    p.k_out = x2.data_ptr() if n_k else None
+    p.x_stride_row, p.k_stride_row, p.rows = x2.stride(0), n_k, rows
+    p.C, p.n_k, p.n_v, p.dtype = x2.shape[1], n_k, n_v, _pcv_dtype(x.dtype)
+    f = _lib.KvProjFp8()
+    f.inv_scale = x2.data_ptr()
+    dv = n_v // num_heads if n_v else 16
+    m = x.shape[-2] if x.dim() >= 3 else rows
+    f.vt_out = x2.data_ptr() if n_v else None
+    mp = (m + 15) // 16 * 16
+    f.vt_stride_c, f.vt_stride_h, f.vt_stride_b = mp, mp * dv, mp * dv * num_heads
+    f.keys_per_batch, f.v_head_dim = m, dv
+    with torch.cuda.device(x.device):
+        return bool(_lib.lib().pcv_kv_project_fp8_supported(C.byref(p), C.byref(f)))
+
+
+def kv_project_fp8(x: torch.Tensor, w_cat: torch.Tensor, col_st: torch.Tensor, inv_scale: torch.Tensor, n_k: int,
+                   n_v: int, num_heads: int, eps: Optional[float] = 1e-5):
+    """The fused producer with e4m3 outputs (pcv_kv_project_fp8): ``LN(x) W^T + b`` of x (B, M, C), column n
+    multiplied by ``inv_scale[n]`` (float32, n_k + n_v; 1 / the descales of :func:`fp8_descales`) and rounded to e4m3.
+
+    Returns ``(k8, vt8)``: k8 (B, M, n_k) e4m3 rows (or None), vt8 the V columns transposed, (B, H, n_v / H, M_pad)
+    e4m3 as :func:`attention_fp8` takes them (or None).  With n_v = 0 this produces q.  No extra pass over the data:
+    the LayerNorm statistics come from the GEMM kernel (or pcv_ln_stats) as in :func:`kv_project`."""
+    _require_cuda(x, w_cat, col_st, inv_scale)
+    if x.dim() != 3:
+        raise ValueError("kv_project_fp8: x must be (B, M, C)")
+    if w_cat.dtype != x.dtype or w_cat.shape != (n_k + n_v, x.shape[-1]) or not w_cat.is_contiguous():
+        raise ValueError("kv_project_fp8: w_cat must be a contiguous (n_k + n_v, C) tensor in x's dtype")
+    if col_st.dtype != torch.float32 or col_st.shape != (n_k + n_v, 2) or not col_st.is_contiguous():
+        raise ValueError("kv_project_fp8: col_st must be a contiguous (n_k + n_v, 2) float32 tensor")
+    inv = inv_scale.float().contiguous()
+    if inv.shape != (n_k + n_v,):
+        raise ValueError("kv_project_fp8: inv_scale must be (n_k + n_v,)")
+    B, M, _ = x.shape
+    x2 = _rows2d(x)
+    mode = kv_project_config["stats"]
+    dv = n_v // num_heads if n_v else 16
+    with torch.cuda.device(x.device):
+        st = ln_stats(x2, eps) if (eps is not None and mode != "fused") else None
+        k8 = torch.empty(B * M, n_k, dtype=torch.float8_e4m3fn, device=x.device) if n_k else None
+        vt8 = None
+        if n_v:
+            m_pad = (M + 15) // 16 * 16
+            vt8 = torch.empty(B, num_heads, dv, m_pad, dtype=torch.float8_e4m3fn, device=x.device)  # pad keys: never read
+        p, f = _fill_kvproj_fp8(x2, w_cat, col_st, inv, n_k, n_v, st, k8, vt8, M, dv,
+                                eps if (eps is not None and mode == "fused") else 0.0)
+        check(_lib.lib().pcv_kv_project_fp8(C.byref(p), C.byref(f), _stream()), "pcv_kv_project_fp8")
+    return (None if k8 is None else k8.view(B, M, n_k)), vt8
