@@ -1020,13 +1020,16 @@ Mode choose_mode(const pcv_attn_params& a) {
 
 int dv_pass_width(int dv) { return std::min(kMaxDvPass, pad64(dv)); }
 
-template <int NQB, int NVB, bool BF16, bool PAIR, bool DROP>
+template <int NQB, int NVB, bool BF16, bool PAIR, bool DROP, bool FP8 = false>
 int launch_fwd(const Plan& pl, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const TcParams& p,
                cudaStream_t stream) {
   prof_mark_begin(stream);
   // num_ctas counts CTA pairs in the pair mode
   int rc;
-  if constexpr (DROP)
+  if constexpr (FP8)
+    rc = launch_kernel(attn_fwd_fp8_kernel<NQB, NVB, BF16>, dim3(pl.num_ctas), kThreads, FwdCfg<NQB, NVB>::kSmemBytes, 0,
+                       stream, tq, tk, tv, p);
+  else if constexpr (DROP)
     rc = launch_kernel(attn_fwd_drop_kernel<NQB, NVB, BF16>, dim3(pl.num_ctas), kThreads, FwdCfg<NQB, NVB>::kSmemBytes, 0,
                        stream, tq, tk, tv, p);
   else
@@ -1075,32 +1078,85 @@ int launch_dispatch(int nqb, int nvb, bool pair, const Plan& pl, const CUtensorM
   return PCV_ERR_UNSUPPORTED;
 }
 
-template <int NQB, int NVB, bool BF16>
-int launch_fwd_fp8(const Plan& pl, const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const TcParams& p,
-                   cudaStream_t stream) {
-  prof_mark_begin(stream);
-  const int rc = launch_kernel(attn_fwd_fp8_kernel<NQB, NVB, BF16>, dim3(pl.num_ctas), kThreads,
-                               FwdCfg<NQB, NVB>::kSmemBytes, 0, stream, tq, tk, tv, p);
-  prof_mark_end(stream);
-  if (rc != PCV_OK) return rc;
-  if (pl.num_units > 0) {
-    dim3 grid(pl.num_units, p.slot_rows / 8);
-    if (NVB == 1)
-      tc_combine_kernel<64, BF16><<<grid, 256, 0, stream>>>(pl.d_units, p);
-    else
-      tc_combine_kernel<128, BF16><<<grid, 256, 0, stream>>>(pl.d_units, p);
-    PCV_CHECK_CUDA(cudaGetLastError());
-    count_launch();
-  }
-  return PCV_OK;
-}
-
 template <bool BF16>
 int launch_dispatch_fp8(int nqb, int nvb, const Plan& pl, const CUtensorMap& tq, const CUtensorMap& tk,
                         const CUtensorMap& tv, const TcParams& p, cudaStream_t stream) {
   if (nqb == 1)
-    return nvb == 1 ? launch_fwd_fp8<1, 1, BF16>(pl, tq, tk, tv, p, stream) : launch_fwd_fp8<1, 2, BF16>(pl, tq, tk, tv, p, stream);
-  return nvb == 1 ? launch_fwd_fp8<2, 1, BF16>(pl, tq, tk, tv, p, stream) : launch_fwd_fp8<2, 2, BF16>(pl, tq, tk, tv, p, stream);
+    return nvb == 1 ? launch_fwd<1, 1, BF16, false, false, true>(pl, tq, tk, tv, p, stream)
+                    : launch_fwd<1, 2, BF16, false, false, true>(pl, tq, tk, tv, p, stream);
+  return nvb == 1 ? launch_fwd<2, 1, BF16, false, false, true>(pl, tq, tk, tv, p, stream)
+                  : launch_fwd<2, 2, BF16, false, false, true>(pl, tq, tk, tv, p, stream);
+}
+
+// The checks attn_tc_supported and attn_tc_fp8_supported end with: the output, the sequence lengths and the device
+// (an FP8 call has passed dv % 16 == 0 before, so the dv % 4 of the partial state never refuses it).
+bool tc_output_supported(const pcv_attn_params& p, const char** why) {
+  auto fail = [&](const char* w) {
+    *why = w;
+    return false;
+  };
+  if (!p.write_partial) {
+    if (!al16(p.out) || (p.o_stride_n % 8) || (p.o_stride_h % 8) || (p.o_stride_b % 8))
+      return fail("output must be 16-byte aligned with strides in multiples of 8 elements");
+  } else {
+    if (!al16(p.part_o) || (p.dv % 4)) return fail("partial output alignment");
+  }
+  if ((int64_t)p.N > (1 << 24) || (int64_t)p.M > (1 << 30)) return fail("sequence too long");
+  if (const char* w = device_problem()) return fail(w);
+  return true;
+}
+
+// What the 16-bit and the FP8 launches share, after their own checks: the plan and the workspace checks (error
+// messages prefixed with `what`), the TcParams core, the workspace slots, the packed pad mask and the Q / K tensor maps
+// (K boxes of `k_box_rows` keys).  The caller adds its own fields to `p` and launches one pass per V slice.
+int tc_setup(const pcv_attn_params& a, const Mode& mode, const char* what, int k_box_rows, cudaStream_t stream,
+             std::shared_ptr<Plan>* plan, TcParams* tp, CUtensorMap* tq, CUtensorMap* tk) {
+  int rc = attach_wait_diag(&g_wait_diag);
+  if (rc != PCV_OK) return rc;
+  rc = get_plan(a.B, a.H, a.N, a.M, mode, plan);
+  if (rc != PCV_OK) return rc;
+  const Plan& pl = **plan;
+  size_t need = 0;
+  rc = attn_tc_workspace_bytes(a, &need);
+  if (rc != PCV_OK) return rc;
+  PCV_REQUIRE(need == 0 || (a.workspace != nullptr && a.workspace_bytes >= need), PCV_ERR_WORKSPACE,
+              "%s: workspace of %zu bytes required, %zu given", what, need, a.workspace_bytes);
+  PCV_REQUIRE(need == 0 || (reinterpret_cast<uintptr_t>(a.workspace) & 15) == 0, PCV_ERR_WORKSPACE,
+              "%s: workspace must be 16-byte aligned", what);
+
+  TcParams& p = *tp;
+  p = TcParams{};
+  p.segs = pl.d_segs;
+  p.cta_seg_begin = pl.d_cta;
+  p.B = a.B; p.H = a.H; p.N = a.N; p.M = a.M; p.dv = a.dv;
+  p.scale_log2 = a.scale * kLog2e;
+  p.causal = a.causal;
+  p.causal_shift = (a.m_total - a.N) - a.m_offset;
+  p.q_bcast = (a.q_stride_b == 0) ? 1 : 0;
+  p.out = a.out; p.osb = a.o_stride_b; p.osn = a.o_stride_n; p.osh = a.o_stride_h;
+  p.write_partial = a.write_partial;
+  p.rows_per_unit = mode.rows_per_unit;
+  p.slot_rows = mode.slot_rows;
+  p.fin_o = a.part_o; p.fin_m = a.part_m; p.fin_l = a.part_l;
+  const int slot_dv = dv_pass_width(a.dv);
+  char* ws = reinterpret_cast<char*>(a.workspace);
+  const size_t nrows = (size_t)pl.num_slots * mode.slot_rows;
+  p.slot_o = reinterpret_cast<float*>(ws);
+  p.slot_m = p.slot_o + nrows * slot_dv;
+  p.slot_l = p.slot_m + nrows;
+  if (a.pad_mask != nullptr) {
+    size_t off = (slots_bytes(pl, slot_dv, mode.slot_rows) + 255) / 256 * 256;
+    uint32_t* bits = reinterpret_cast<uint32_t*>(ws + off);
+    p.pad_bits = bits;
+    p.pad_wpr = pad_words_per_row(a.M);
+    rc = launch_pack_pad(a.pad_mask, a.pad_stride_b, a.B, a.M, bits, stream);
+    if (rc != PCV_OK) return rc;
+  }
+
+  const int Bq = a.q_stride_b == 0 ? 1 : a.B;
+  rc = make_tmap_4d(tq, a.q, a.dtype, a.dqk, a.N, a.H, Bq, a.q_stride_n, a.q_stride_h, a.q_stride_b, kTileM);
+  if (rc != PCV_OK) return rc;
+  return make_tmap_4d(tk, a.k, a.dtype, a.dqk, a.M, a.H, a.B, a.k_stride_m, a.k_stride_h, a.k_stride_b, k_box_rows);
 }
 
 }  // namespace
@@ -1138,15 +1194,7 @@ bool attn_tc_supported(const pcv_attn_params& p, const char** why) {
   if ((p.q_stride_n % 8) || (p.k_stride_m % 8) || (p.v_stride_m % 8) || (p.q_stride_h % 8) || (p.k_stride_h % 8) ||
       (p.v_stride_h % 8) || (p.q_stride_b % 8) || (p.k_stride_b % 8) || (p.v_stride_b % 8))
     return fail("q/k/v strides must be multiples of 8 elements");
-  if (!p.write_partial) {
-    if (!al16(p.out) || (p.o_stride_n % 8) || (p.o_stride_h % 8) || (p.o_stride_b % 8))
-      return fail("output must be 16-byte aligned with strides in multiples of 8 elements");
-  } else {
-    if (!al16(p.part_o) || (p.dv % 4)) return fail("partial output alignment");
-  }
-  if ((int64_t)p.N > (1 << 24) || (int64_t)p.M > (1 << 30)) return fail("sequence too long");
-  if (const char* w = device_problem()) return fail(w);
-  return true;
+  return tc_output_supported(p, why);
 }
 
 int attn_tc_workspace_bytes(const pcv_attn_params& p, size_t* bytes) {
@@ -1179,7 +1227,11 @@ int launch_attn_tc(const pcv_attn_params& a, cudaStream_t stream, const pcv_shar
                                   a.m_offset % 2 == 0 && drop->thresh > 0),
               PCV_ERR_UNSUPPORTED,
               "tensor-core attention: dropout needs a partial-state call starting at an even key, no CTA pair");
-  std::shared_ptr<Plan> pl;
+  if (fuse != nullptr) {
+    const char* why = "";
+    PCV_REQUIRE(attn_tc_fuse_supported(a, &why), PCV_ERR_UNSUPPORTED, "fused merge: %s", why);
+    PCV_REQUIRE(a.write_partial, PCV_ERR_INVALID, "fused merge: the launch must write the partial state (write_partial = 1)");
+  }
   const Mode mode = choose_mode(a);
   if (mode.pair) {
     int dev = 0, sms = 0;
@@ -1188,39 +1240,17 @@ int launch_attn_tc(const pcv_attn_params& a, cudaStream_t stream, const pcv_shar
     PCV_REQUIRE(pad64(a.dqk) <= 128 && pad64(a.dv) <= 128 && sms >= 2, PCV_ERR_UNSUPPORTED,
                 "the CTA-pair kernel needs qk and v head dims <= 128 and at least two SMs");
   }
-  int rc = attach_wait_diag(&g_wait_diag);
+  std::shared_ptr<Plan> pl;
+  TcParams p;
+  CUtensorMap tq, tk, tv;
+  const int kv_box_rows = mode.pair ? kTileN / 2 : kTileN;  // a pair loads 64-key halves of every K / V tile
+  int rc = tc_setup(a, mode, "tensor-core attention", kv_box_rows, stream, &pl, &p, &tq, &tk);
   if (rc != PCV_OK) return rc;
-  rc = get_plan(a.B, a.H, a.N, a.M, mode, &pl);
-  if (rc != PCV_OK) return rc;
-  size_t need = 0;
-  rc = attn_tc_workspace_bytes(a, &need);
-  if (rc != PCV_OK) return rc;
-  PCV_REQUIRE(need == 0 || (a.workspace != nullptr && a.workspace_bytes >= need), PCV_ERR_WORKSPACE,
-              "tensor-core attention: workspace of %zu bytes required, %zu given", need, a.workspace_bytes);
-  PCV_REQUIRE(need == 0 || (reinterpret_cast<uintptr_t>(a.workspace) & 15) == 0, PCV_ERR_WORKSPACE,
-              "tensor-core attention: workspace must be 16-byte aligned");
-
-  TcParams p{};
-  p.segs = pl->d_segs;
-  p.cta_seg_begin = pl->d_cta;
-  p.B = a.B; p.H = a.H; p.N = a.N; p.M = a.M; p.dv = a.dv;
-  p.scale_log2 = a.scale * kLog2e;
-  p.causal = a.causal;
-  p.causal_shift = (a.m_total - a.N) - a.m_offset;
-  p.q_bcast = (a.q_stride_b == 0) ? 1 : 0;
-  p.out = a.out; p.osb = a.o_stride_b; p.osn = a.o_stride_n; p.osh = a.o_stride_h;
-  p.write_partial = a.write_partial;
-  p.rows_per_unit = mode.rows_per_unit;
-  p.slot_rows = mode.slot_rows;
-  p.fin_o = a.part_o; p.fin_m = a.part_m; p.fin_l = a.part_l;
   if (drop != nullptr) {
     p.drop = *drop;
     p.drop_key_base = a.m_offset;
   }
   if (fuse != nullptr) {
-    const char* why = "";
-    PCV_REQUIRE(attn_tc_fuse_supported(a, &why), PCV_ERR_UNSUPPORTED, "fused merge: %s", why);
-    PCV_REQUIRE(a.write_partial, PCV_ERR_INVALID, "fused merge: the launch must write the partial state (write_partial = 1)");
     PeerTail& t = p.tail;
     t.enabled = 1;
     t.num_peers = fuse->num_peers;
@@ -1243,28 +1273,6 @@ int launch_attn_tc(const pcv_attn_params& a, cudaStream_t stream, const pcv_shar
     p.fin_m = const_cast<float*>(t.part_m[fuse->rank]);
     p.fin_l = const_cast<float*>(t.part_l[fuse->rank]);
   }
-  const int slot_dv = dv_pass_width(a.dv);
-  char* ws = reinterpret_cast<char*>(a.workspace);
-  const size_t nrows = (size_t)pl->num_slots * mode.slot_rows;
-  p.slot_o = reinterpret_cast<float*>(ws);
-  p.slot_m = p.slot_o + nrows * slot_dv;
-  p.slot_l = p.slot_m + nrows;
-  if (a.pad_mask != nullptr) {
-    size_t off = (slots_bytes(*pl, slot_dv, mode.slot_rows) + 255) / 256 * 256;
-    uint32_t* bits = reinterpret_cast<uint32_t*>(ws + off);
-    p.pad_bits = bits;
-    p.pad_wpr = pad_words_per_row(a.M);
-    rc = launch_pack_pad(a.pad_mask, a.pad_stride_b, a.B, a.M, bits, stream);
-    if (rc != PCV_OK) return rc;
-  }
-
-  CUtensorMap tq, tk, tv;
-  const int Bq = a.q_stride_b == 0 ? 1 : a.B;
-  rc = make_tmap_4d(&tq, a.q, a.dtype, a.dqk, a.N, a.H, Bq, a.q_stride_n, a.q_stride_h, a.q_stride_b, kTileM);
-  if (rc != PCV_OK) return rc;
-  const int kv_box_rows = mode.pair ? kTileN / 2 : kTileN;  // a pair loads 64-key halves of every K / V tile
-  rc = make_tmap_4d(&tk, a.k, a.dtype, a.dqk, a.M, a.H, a.B, a.k_stride_m, a.k_stride_h, a.k_stride_b, kv_box_rows);
-  if (rc != PCV_OK) return rc;
   const bool bf = a.dtype == PCV_BF16;
   const int nqb = pad64(a.dqk) / 64;
   // one launch per slice of at most 128 V channels (the scores are recomputed per slice)
@@ -1319,15 +1327,7 @@ bool attn_tc_fp8_supported(const pcv_attn_params& p, const pcv_fp8_attn& f, cons
   if (f.vt_stride_c < p.M) return fail("v^T channel stride must cover the M keys");
   if (p.B > 1 && (p.k_stride_b == 0 || f.vt_stride_b == 0))
     return fail("k and v^T need a non-zero batch stride when B > 1 (only q broadcasts over the batch)");
-  if (!p.write_partial) {
-    if (!al16(p.out) || (p.o_stride_n % 8) || (p.o_stride_h % 8) || (p.o_stride_b % 8))
-      return fail("output must be 16-byte aligned with strides in multiples of 8 elements");
-  } else {
-    if (!al16(p.part_o)) return fail("partial output alignment");
-  }
-  if ((int64_t)p.N > (1 << 24) || (int64_t)p.M > (1 << 30)) return fail("sequence too long");
-  if (const char* w = device_problem()) return fail(w);
-  return true;
+  return tc_output_supported(p, why);
 }
 
 int launch_attn_tc_fp8(const pcv_attn_params& a, const pcv_fp8_attn& f, cudaStream_t stream) {
@@ -1335,56 +1335,14 @@ int launch_attn_tc_fp8(const pcv_attn_params& a, const pcv_fp8_attn& f, cudaStre
     const char* why = "";
     PCV_REQUIRE(attn_tc_fp8_supported(a, f, &why), PCV_ERR_UNSUPPORTED, "FP8 tensor-core attention: %s", why);
   }
+  // a.dtype is PCV_E4M3 (checked above): the Q / K boxes hold 128 e4m3 channels
   std::shared_ptr<Plan> pl;
-  const Mode mode = choose_mode(a);
-  int rc = attach_wait_diag(&g_wait_diag);
+  TcParams p;
+  CUtensorMap tq, tk, tv;
+  int rc = tc_setup(a, choose_mode(a), "FP8 tensor-core attention", kTileN, stream, &pl, &p, &tq, &tk);
   if (rc != PCV_OK) return rc;
-  rc = get_plan(a.B, a.H, a.N, a.M, mode, &pl);
-  if (rc != PCV_OK) return rc;
-  size_t need = 0;
-  rc = attn_tc_workspace_bytes(a, &need);
-  if (rc != PCV_OK) return rc;
-  PCV_REQUIRE(need == 0 || (a.workspace != nullptr && a.workspace_bytes >= need), PCV_ERR_WORKSPACE,
-              "FP8 tensor-core attention: workspace of %zu bytes required, %zu given", need, a.workspace_bytes);
-  PCV_REQUIRE(need == 0 || (reinterpret_cast<uintptr_t>(a.workspace) & 15) == 0, PCV_ERR_WORKSPACE,
-              "FP8 tensor-core attention: workspace must be 16-byte aligned");
-
-  TcParams p{};
-  p.segs = pl->d_segs;
-  p.cta_seg_begin = pl->d_cta;
-  p.B = a.B; p.H = a.H; p.N = a.N; p.M = a.M; p.dv = a.dv;
-  p.scale_log2 = a.scale * kLog2e;
-  p.causal = a.causal;
-  p.causal_shift = (a.m_total - a.N) - a.m_offset;
-  p.q_bcast = (a.q_stride_b == 0) ? 1 : 0;
-  p.out = a.out; p.osb = a.o_stride_b; p.osn = a.o_stride_n; p.osh = a.o_stride_h;
-  p.write_partial = a.write_partial;
-  p.rows_per_unit = mode.rows_per_unit;
-  p.slot_rows = mode.slot_rows;
-  p.fin_o = a.part_o; p.fin_m = a.part_m; p.fin_l = a.part_l;
   p.q_descale = f.q_descale; p.k_descale = f.k_descale; p.v_descale = f.v_descale;
   p.v_descale_stride = a.dv;
-  const int slot_dv = dv_pass_width(a.dv);
-  char* ws = reinterpret_cast<char*>(a.workspace);
-  const size_t nrows = (size_t)pl->num_slots * mode.slot_rows;
-  p.slot_o = reinterpret_cast<float*>(ws);
-  p.slot_m = p.slot_o + nrows * slot_dv;
-  p.slot_l = p.slot_m + nrows;
-  if (a.pad_mask != nullptr) {
-    size_t off = (slots_bytes(*pl, slot_dv, mode.slot_rows) + 255) / 256 * 256;
-    uint32_t* bits = reinterpret_cast<uint32_t*>(ws + off);
-    p.pad_bits = bits;
-    p.pad_wpr = pad_words_per_row(a.M);
-    rc = launch_pack_pad(a.pad_mask, a.pad_stride_b, a.B, a.M, bits, stream);
-    if (rc != PCV_OK) return rc;
-  }
-
-  CUtensorMap tq, tk, tv;
-  const int Bq = a.q_stride_b == 0 ? 1 : a.B;
-  rc = make_tmap_4d(&tq, a.q, PCV_E4M3, a.dqk, a.N, a.H, Bq, a.q_stride_n, a.q_stride_h, a.q_stride_b, kTileM);
-  if (rc != PCV_OK) return rc;
-  rc = make_tmap_4d(&tk, a.k, PCV_E4M3, a.dqk, a.M, a.H, a.B, a.k_stride_m, a.k_stride_h, a.k_stride_b, kTileN);
-  if (rc != PCV_OK) return rc;
   const bool bf = f.out_dtype == PCV_BF16;
   const int nqb = (a.dqk + 127) / 128;
   // one launch per slice of at most 128 V channels; V^T is viewed as (keys M, channels of the slice, H, B), so keys

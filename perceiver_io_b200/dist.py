@@ -110,43 +110,27 @@ def _cuda_finalize(po, pl, out_dtype):
 
 def _cuda_partial_dropout(q, k, v, num_heads, scale, pad_mask, causal, m_total, m_offset, out, dropout_p, dropout_seed):
     """The one-pass dropout forward on the local keys (global key indices in the mask).  Head dims that are not
-    multiples of 8 are zero-padded, which changes neither the scores nor the mask."""
+    multiples of 8 are zero-padded as in ``ops._prep``, and the caller's buffers get the true head dim back."""
     from . import ops
 
-    dv = ops._head_dim(v, num_heads)
-    if ops._head_dim(q, num_heads) % 8 == 0 and dv % 8 == 0:
-        ops.attention_partial(q, k, v, num_heads, scale, pad_mask=pad_mask, causal=causal, m_total=m_total,
-                              m_offset=m_offset, out=out, dropout_p=dropout_p, dropout_seed=dropout_seed)
-        return
-    qp, kp, vp = (ops._pad_heads_to8(t, num_heads) for t in (q, k, v))
-    po, pm, pl = ops.attention_partial(qp, kp, vp, num_heads, scale, pad_mask=pad_mask, causal=causal, m_total=m_total,
-                                       m_offset=m_offset, dropout_p=dropout_p, dropout_seed=dropout_seed)
-    out[0].copy_(po[..., :dv])
-    out[1].copy_(pm)
-    out[2].copy_(pl)
+    q, k, v, dims = ops._prep(q, k, v, num_heads=num_heads, pad=True)
+    state = ops.attention_partial(q, k, v, num_heads, scale, pad_mask=pad_mask, causal=causal, m_total=m_total,
+                                  m_offset=m_offset, out=None if dims else out, dropout_p=dropout_p,
+                                  dropout_seed=dropout_seed)
+    if dims is not None:
+        po, pm, pl = state
+        for dst, src in zip(out, (ops._unpad_heads(po, num_heads, dims[1]), pm, pl)):
+            dst.copy_(src)
 
 
 def _cuda_backward(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask, causal, m_total, m_offset,
                    dropout_p, dropout_seed):
-    """-> (grad_q32, grad_k, grad_v) of one key shard: the backward kernels (``ops.attention_backward_shard``) where
-    they cover the call, else (head dims above 192, 4-D operands) the torch shim with the key offset.
-    ``ops.backward_config["impl"]`` selects as for the unsharded backward."""
-    from . import _lib, ops
+    """-> (grad_q32, grad_k, grad_v) of one key shard: the backward kernels where they cover the call, else (head dims
+    above 192, 4-D operands) the torch shim with the key offset, as ``ops.backward_config["impl"]`` selects."""
+    from . import ops
 
-    mode = ops.backward_config["impl"]
-    if mode not in ("auto", "kernel", "shim"):
-        raise ValueError(f"backward_config['impl'] = {mode!r}")
-    if mode != "shim":
-        if q.dim() == 3 and k.dim() == 3 and v.dim() == 3:
-            grads = ops._backward_shard(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, m_total, m_offset,
-                                        pad_mask, causal, dropout_p, dropout_seed, "try")
-            if grads is not None:
-                return grads
-        if mode == "kernel":
-            raise RuntimeError("backward_config['impl'] = 'kernel' but pcv_attn_bwd_shard does not cover this call: "
-                               + _lib.lib().pcv_last_error().decode())
-    return ops._backward_shim(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask, causal, dropout_p,
-                              dropout_seed, m_total, m_offset)
+    return ops._attention_grads(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask, causal, dropout_p,
+                                dropout_seed, shard=(m_total, m_offset))
 
 
 @dataclass

@@ -126,22 +126,89 @@ def _fill_attn_params(q, k, v, num_heads, scale, pad_mask, causal, m_total, m_of
     return p, tuple(keep)
 
 
-def _run_attn(p: AttnParams, device) -> None:
+def _workspace(p, device, entry: str, *args) -> Optional[torch.Tensor]:
+    """Size (by ``<entry>_workspace_bytes(*args)``), allocate and attach the workspace of the launch ``p`` describes.
+    Returns the tensor, to be kept until the launch is enqueued, or None when the launch needs no bytes.  torch aligns
+    every block to 512 bytes, beyond the 256 the backward and dropout forward entry points require."""
+    query = entry + "_workspace_bytes"
     need = C.c_size_t(0)
-    check(_lib.lib().pcv_attn_workspace_bytes(C.byref(p), C.byref(need)), "pcv_attn_workspace_bytes")
-    ws = None
-    if need.value:
-        ws = torch.empty(need.value, dtype=torch.uint8, device=device)
-        p.workspace, p.workspace_bytes = ws.data_ptr(), need.value
+    check(getattr(_lib.lib(), query)(*args, C.byref(need)), query)
+    if not need.value:
+        return None
+    ws = torch.empty(need.value, dtype=torch.uint8, device=device)
+    p.workspace, p.workspace_bytes = ws.data_ptr(), need.value
+    return ws
+
+
+def _run_attn(p: AttnParams, device) -> None:
+    ws = _workspace(p, device, "pcv_attn", C.byref(p))
     check(_lib.lib().pcv_attn_fwd(C.byref(p), _stream()), "pcv_attn_fwd")
+    del ws
 
 
-def _prep(q, k, v):
-    _require_cuda(q, k, v)
-    out_dtype = q.dtype
+def _new_output(p, dtype: torch.dtype, device) -> torch.Tensor:
+    """A new (B, N, H*dv) output for the launch ``p`` describes, attached to it."""
+    out = torch.empty(p.B, p.N, p.H * p.dv, dtype=dtype, device=device)
+    p.out = out.data_ptr()
+    p.o_stride_b, p.o_stride_n, p.o_stride_h = out.stride(0), out.stride(1), p.dv
+    return out
+
+
+def _partial_state(p, device, out=None):
+    """The float32 partial state (part_o (B,H,N,dv), part_m (B,H,N), part_l (B,H,N)) the launch ``p`` describes writes,
+    attached to it: the caller's ``out`` tensors, checked, or new ones."""
+    if out is not None:
+        part_o, part_m, part_l = out
+        if (tuple(part_o.shape) != (p.B, p.H, p.N, p.dv) or tuple(part_m.shape) != (p.B, p.H, p.N)
+                or tuple(part_l.shape) != (p.B, p.H, p.N)):
+            raise ValueError("attention_partial: `out` tensors have the wrong shape")
+        for t in out:
+            if t.dtype != torch.float32 or not t.is_contiguous() or not t.is_cuda:
+                raise ValueError("attention_partial: `out` tensors must be contiguous float32 CUDA tensors")
+    else:
+        part_o = torch.empty(p.B, p.H, p.N, p.dv, dtype=torch.float32, device=device)
+        part_m = torch.empty(p.B, p.H, p.N, dtype=torch.float32, device=device)
+        part_l = torch.empty(p.B, p.H, p.N, dtype=torch.float32, device=device)
+    p.write_partial = 1
+    p.part_o, p.part_m, p.part_l = part_o.data_ptr(), part_m.data_ptr(), part_l.data_ptr()
+    return part_o, part_m, part_l
+
+
+def _check_stats(p, stat_m, stat_l) -> None:
+    """The forward's row statistics, as the launch ``p`` describes them: contiguous float32 (B, H, N)."""
+    for name, t in (("stat_m", stat_m), ("stat_l", stat_l)):
+        if tuple(t.shape) != (p.B, p.H, p.N) or t.dtype != torch.float32 or not t.is_contiguous():
+            raise ValueError(f"{name} must be a contiguous float32 (B, H, N) tensor")
+
+
+def _prep(q, k, v, *more, num_heads: Optional[int] = None, pad: bool = False):
+    """Attention operands on the kernels' terms -> ``(q, k, v, *more, dims)``.
+
+    Every operand must be on CUDA; it is cast to the compute dtype of q (fp32 -> bf16) and given unit channel stride.
+    ``more`` are (B, N, H*dv) tensors that go with v (the backward's out and grad_out).  With ``pad``, head dims that are
+    not multiples of 8 are zero-padded per head (``_pad_heads_to8``) and every operand is returned as (B, L, H*d8), so
+    that the tensor-core kernels (TMA) can take them: zero channels change neither the scores, nor the first dv channels
+    of P V, nor delta = rowsum(dO * O), nor the dropout mask.  ``dims`` is then the true (dqk, dv), to slice results back
+    with ``_unpad_heads``; it is None when nothing was padded."""
+    ts = (q, k, v) + more
+    _require_cuda(*ts)
     cdt = _compute_dtype(q.dtype)
-    q, k, v = (_rows_contiguous(t if t.dtype == cdt else t.to(cdt)) for t in (q, k, v))
-    return q, k, v, out_dtype
+    ts = tuple(_rows_contiguous(t if t.dtype == cdt else t.to(cdt)) for t in ts)
+    dims = None
+    if pad:
+        dqk, dv = _head_dim(q, num_heads), _head_dim(v, num_heads)
+        if dqk % 8 or dv % 8:
+            dims = (dqk, dv)
+            ts = tuple(_pad_heads_to8(t, num_heads).flatten(2) for t in ts)
+    return ts + (dims,)
+
+
+def _unpad_heads(t: torch.Tensor, num_heads: int, d: int) -> torch.Tensor:
+    """The first ``d`` channels of every head of a result computed from ``_prep(pad=True)`` operands: a (B, L, H*d8)
+    output or gradient, or a (B, H, N, d8) partial numerator."""
+    if t.dim() == 4:
+        return t[..., :d]
+    return t.unflatten(2, (num_heads, -1))[..., :d].flatten(2)
 
 
 def _pad_heads_to8(t: torch.Tensor, num_heads: int) -> torch.Tensor:
@@ -160,22 +227,16 @@ def _head_dim(t: torch.Tensor, num_heads: int) -> int:
 
 
 def _attention_forward(q, k, v, num_heads, scale, pad_mask, causal, impl):
-    q, k, v, out_dtype = _prep(q, k, v)
-    if pad_mask is not None:
-        _require_cuda(pad_mask)
-    dv_true = _head_dim(v, num_heads)
-    if impl != "simt" and (_head_dim(q, num_heads) % 8 or dv_true % 8):
-        # odd head dims: pad to a multiple of 8 so that the tensor-core kernels (TMA) can take them
-        q, k, v = _pad_heads_to8(q, num_heads), _pad_heads_to8(k, num_heads), _pad_heads_to8(v, num_heads)
+    out_dtype = q.dtype
+    q, k, v, dims = _prep(q, k, v, num_heads=num_heads, pad=impl != "simt")
+    _require_cuda(pad_mask)
     with torch.cuda.device(k.device):
         p, keep = _fill_attn_params(q, k, v, num_heads, scale, pad_mask, causal, None, 0, impl)
-        out = torch.empty(p.B, p.N, p.H * p.dv, dtype=q.dtype, device=k.device)
-        p.out = out.data_ptr()
-        p.o_stride_b, p.o_stride_n, p.o_stride_h = out.stride(0), out.stride(1), p.dv
+        out = _new_output(p, q.dtype, k.device)
         _run_attn(p, k.device)
     del keep
-    if p.dv != dv_true:
-        out = out.view(p.B, p.N, p.H, p.dv)[..., :dv_true].reshape(p.B, p.N, p.H * dv_true)
+    if dims is not None:
+        out = _unpad_heads(out, num_heads, dims[1])
     return out if out.dtype == out_dtype else out.to(out_dtype)
 
 
@@ -185,40 +246,84 @@ def _attention_forward(q, k, v, num_heads, scale, pad_mask, causal, impl):
 backward_config = {"max_score_bytes": 1 << 30, "impl": "auto"}
 
 
-def _fill_bwd_params(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask, causal, dropout_p=0.0,
-                     dropout_seed=0, with_grad_q=True):
-    """Backward parameters and the (grad_q, grad_k, grad_v) outputs; ``with_grad_q=False`` (a key shard, which writes an
-    fp32 contribution instead) allocates no grad_q and leaves its pointer NULL."""
+def _fill_bwd_params(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask, causal, dropout_p,
+                     dropout_seed):
+    """Backward parameters of prepared operands, with the strides of dense (B, L, H*d) gradients but no gradient
+    pointers yet."""
     ap, keep = _fill_attn_params(q, k, v, num_heads, scale, pad_mask, causal, None, 0, "auto")
     B, H, N, M, dqk, dv = ap.B, ap.H, ap.N, ap.M, ap.dqk, ap.dv
     for name, t in (("out", out), ("grad_out", grad_out)):
         if tuple(t.shape) != (B, N, H * dv) or t.stride(2) != 1:
             raise ValueError(f"{name} must be a (B, N, H*dv) tensor with unit channel stride, got {tuple(t.shape)}")
-    for name, t in (("stat_m", stat_m), ("stat_l", stat_l)):
-        if tuple(t.shape) != (B, H, N) or t.dtype != torch.float32 or not t.is_contiguous():
-            raise ValueError(f"{name} must be a contiguous float32 (B, H, N) tensor")
-    Bq = q.shape[0]
-    gq = torch.empty(Bq, N, H * dqk, dtype=q.dtype, device=q.device) if with_grad_q else None
-    gk = torch.empty(B, M, H * dqk, dtype=q.dtype, device=q.device)
-    gv = torch.empty(B, M, H * dv, dtype=q.dtype, device=q.device)
+    _check_stats(ap, stat_m, stat_l)
     p = _lib.AttnBwdParams()
     p.q, p.k, p.v, p.out, p.grad_out = ap.q, ap.k, ap.v, out.data_ptr(), grad_out.data_ptr()
     p.stat_m, p.stat_l = stat_m.data_ptr(), stat_l.data_ptr()
-    p.grad_q, p.grad_k, p.grad_v = (gq.data_ptr() if with_grad_q else None), gk.data_ptr(), gv.data_ptr()
     for f in ("q_stride_b", "q_stride_n", "q_stride_h", "k_stride_b", "k_stride_m", "k_stride_h",
               "v_stride_b", "v_stride_m", "v_stride_h"):
         setattr(p, f, getattr(ap, f))
     p.o_stride_b, p.o_stride_n, p.o_stride_h = out.stride(0), out.stride(1), dv
     p.go_stride_b, p.go_stride_n, p.go_stride_h = grad_out.stride(0), grad_out.stride(1), dv
-    if with_grad_q:
-        p.gq_stride_b, p.gq_stride_n, p.gq_stride_h = gq.stride(0), gq.stride(1), dqk
-    p.gk_stride_b, p.gk_stride_m, p.gk_stride_h = gk.stride(0), gk.stride(1), dqk
-    p.gv_stride_b, p.gv_stride_m, p.gv_stride_h = gv.stride(0), gv.stride(1), dv
+    p.gq_stride_b, p.gq_stride_n, p.gq_stride_h = N * H * dqk, H * dqk, dqk
+    p.gk_stride_b, p.gk_stride_m, p.gk_stride_h = M * H * dqk, H * dqk, dqk
+    p.gv_stride_b, p.gv_stride_m, p.gv_stride_h = M * H * dv, H * dv, dv
     p.B, p.H, p.N, p.M, p.dqk, p.dv = B, H, N, M, dqk, dv
     p.scale, p.dtype, p.causal = float(scale), ap.dtype, ap.causal
     p.pad_mask, p.pad_stride_b = ap.pad_mask, ap.pad_stride_b
     p.dropout_p, p.dropout_seed = float(dropout_p), int(dropout_seed)
-    return p, (gq, gk, gv), keep + (out, grad_out, stat_m, stat_l)
+    return p, keep + (out, grad_out, stat_m, stat_l)
+
+
+def _backward_kernels(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask, causal, dropout_p,
+                      dropout_seed, shard, mode):
+    """pcv_attn_bwd, or pcv_attn_bwd_shard for a key shard ``shard = (m_total, m_offset)``, on operands ``_prep``
+    prepared -> (grad_q, grad_k, grad_v); a shard's grad_q is its fp32 contribution grad_q32.  ``mode`` as in
+    ``_backward``.  The support check and the launch read the same params; the check allocates no gradient."""
+    lib = _lib.lib()
+    with torch.cuda.device(k.device):
+        p, keep = _fill_bwd_params(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask, causal,
+                                   dropout_p, dropout_seed)
+        entry, args = "pcv_attn_bwd", (C.byref(p),)
+        if shard is not None:
+            s = _lib.KeyShard()
+            s.m_total, s.m_offset = int(shard[0]), int(shard[1])
+            entry, args = "pcv_attn_bwd_shard", (C.byref(p), C.byref(s))
+        if mode != "run":
+            if shard is not None:  # the check reads only the alignment of grad_q32
+                placeholder = torch.empty(16, device=k.device)
+                s.grad_q32 = placeholder.data_ptr()
+            ok = bool(getattr(lib, entry + "_supported")(*args))
+            if mode == "check" or not ok:
+                return ok if mode == "check" else None
+        gq = torch.empty(q.shape[0], p.N, p.H * p.dqk, dtype=q.dtype if shard is None else torch.float32,
+                         device=k.device)
+        gk = torch.empty(p.B, p.M, p.H * p.dqk, dtype=q.dtype, device=k.device)
+        gv = torch.empty(p.B, p.M, p.H * p.dv, dtype=q.dtype, device=k.device)
+        p.grad_k, p.grad_v = gk.data_ptr(), gv.data_ptr()
+        if shard is None:
+            p.grad_q = gq.data_ptr()
+        else:
+            s.grad_q32 = gq.data_ptr()
+        ws = _workspace(p, k.device, entry, *args)
+        check(getattr(lib, entry)(*args, _stream()), entry)
+    del keep, ws
+    return gq, gk, gv
+
+
+def _backward(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask, causal, dropout_p, dropout_seed,
+              shard=None, mode="try", pad=True):
+    """The backward kernels (of the key shard ``shard = (m_total, m_offset)``) with the operands prepared once.  With
+    ``pad``, head dims that are not multiples of 8 are zero-padded per head, as the forward padded them, and the
+    gradients of the padding channels dropped.  mode "check": whether the kernels cover the call; "run": the gradients
+    (an uncovered call raises); "try": the gradients, or None where the kernels do not cover the call."""
+    q, k, v, out, grad_out, dims = _prep(q, k, v, out, grad_out, num_heads=num_heads, pad=pad)
+    _require_cuda(stat_m, stat_l, pad_mask)
+    grads = _backward_kernels(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask, causal, dropout_p,
+                              dropout_seed, shard, mode)
+    if mode == "check" or grads is None or dims is None:
+        return grads
+    dqk, dv = dims
+    return tuple(_unpad_heads(g, num_heads, d) for g, d in zip(grads, (dqk, dqk, dv)))
 
 
 def attention_backward(q, k, v, out, grad_out, stat_m, stat_l, num_heads: int, scale: float, pad_mask=None,
@@ -230,23 +335,8 @@ def attention_backward(q, k, v, out, grad_out, stat_m, stat_l, num_heads: int, s
     keys.  grad_q has q's batch size (a batch-1 ``q`` shared by the batch receives the sum).  ``check_only`` launches
     nothing and returns whether the kernels cover these operands.  ``dropout_p`` / ``dropout_seed``: the values the
     forward (``attention_dropout_forward``) ran with — the kernels regenerate its mask."""
-    q, k, v, _ = _prep(q, k, v)
-    cdt = q.dtype
-    out = _rows_contiguous(out if out.dtype == cdt else out.to(cdt))
-    grad_out = _rows_contiguous(grad_out if grad_out.dtype == cdt else grad_out.to(cdt))
-    _require_cuda(out, grad_out, stat_m, stat_l, pad_mask)
-    with torch.cuda.device(k.device):
-        p, grads, keep = _fill_bwd_params(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask, causal,
-                                          dropout_p, dropout_seed)
-        if check_only:
-            return bool(_lib.lib().pcv_attn_bwd_supported(C.byref(p)))
-        need = C.c_size_t(0)
-        check(_lib.lib().pcv_attn_bwd_workspace_bytes(C.byref(p), C.byref(need)), "pcv_attn_bwd_workspace_bytes")
-        ws = torch.empty(max(need.value, 256), dtype=torch.uint8, device=k.device)
-        p.workspace, p.workspace_bytes = ws.data_ptr(), need.value
-        check(_lib.lib().pcv_attn_bwd(C.byref(p), _stream()), "pcv_attn_bwd")
-    del keep
-    return grads
+    return _backward(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask, causal, dropout_p, dropout_seed,
+                     mode="check" if check_only else "run", pad=False)
 
 
 def attention_backward_shard(q, k, v, out, grad_out, stat_m, stat_l, num_heads: int, scale: float, m_total: int,
@@ -257,47 +347,33 @@ def attention_backward_shard(q, k, v, out, grad_out, stat_m, stat_l, num_heads: 
     ``k`` / ``v`` / ``pad_mask`` hold the keys [m_offset, m_offset + M) of ``m_total`` (m_offset even); ``stat_m`` /
     ``stat_l`` are the row statistics MERGED over all keys and ``out`` the merged output.  grad_k / grad_v are this
     shard's gradients; grad_q32 is its fp32 contribution to grad_q (q's batch size): the sum over all shards is grad_q.
-    Head dims up to 192; those that are not multiples of 8 are zero-padded as in ``_kernel_backward``.  ``check_only``
+    Head dims up to 192; those that are not multiples of 8 are zero-padded as in the autograd backward.  ``check_only``
     launches nothing and returns whether the kernels cover these operands."""
-    return _backward_shard(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, m_total, m_offset, pad_mask,
-                           causal, dropout_p, dropout_seed, "check" if check_only else "run")
+    return _backward(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask, causal, dropout_p, dropout_seed,
+                     shard=(m_total, m_offset), mode="check" if check_only else "run")
 
 
-def _backward_shard(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, m_total, m_offset, pad_mask, causal,
-                    dropout_p, dropout_seed, mode):
-    """``attention_backward_shard`` with the operands prepared once.  mode "check": whether the kernels cover the call;
-    "run": the gradients (an uncovered call raises); "try": the gradients, or None where the kernels do not cover the
-    call (the caller then takes the shim)."""
-    dqk, dv = _head_dim(q, num_heads), _head_dim(v, num_heads)
-    padded = bool(dqk % 8 or dv % 8)
-    q, k, v, _ = _prep(q, k, v)
-    cdt = q.dtype
-    out = _rows_contiguous(out if out.dtype == cdt else out.to(cdt))
-    grad_out = _rows_contiguous(grad_out if grad_out.dtype == cdt else grad_out.to(cdt))
-    if padded:
-        q, k, v, out, grad_out = (_pad_heads_to8(t, num_heads).flatten(2) for t in (q, k, v, out, grad_out))
-    _require_cuda(out, grad_out, stat_m, stat_l, pad_mask)
-    with torch.cuda.device(k.device):
-        p, (_, gk, gv), keep = _fill_bwd_params(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask,
-                                                causal, dropout_p, dropout_seed, with_grad_q=False)
-        gq32 = torch.empty(q.shape[0], p.N, p.H * p.dqk, dtype=torch.float32, device=k.device)
-        s = _lib.KeyShard()
-        s.m_total, s.m_offset, s.grad_q32 = int(m_total), int(m_offset), gq32.data_ptr()
-        if mode != "run":
-            ok = bool(_lib.lib().pcv_attn_bwd_shard_supported(C.byref(p), C.byref(s)))
-            if mode == "check" or not ok:
-                return ok if mode == "check" else None
-        need = C.c_size_t(0)
-        check(_lib.lib().pcv_attn_bwd_shard_workspace_bytes(C.byref(p), C.byref(s), C.byref(need)),
-              "pcv_attn_bwd_shard_workspace_bytes")
-        ws = torch.empty(max(need.value, 256), dtype=torch.uint8, device=k.device)
-        p.workspace, p.workspace_bytes = ws.data_ptr(), need.value
-        check(_lib.lib().pcv_attn_bwd_shard(C.byref(p), C.byref(s), _stream()), "pcv_attn_bwd_shard")
-    del keep
-    if padded:
-        gq32, gk, gv = (g.unflatten(2, (num_heads, -1))[..., :d].flatten(2)
-                        for g, d in ((gq32, dqk), (gk, dqk), (gv, dv)))
-    return gq32, gk, gv
+def _attention_grads(q, k, v, out, grad_out, pm, pl, num_heads: int, scale: float, pad_mask, causal: bool,
+                     dropout_p: float, dropout_seed: int, shard=None):
+    """The gradients of attention, or of the key shard ``shard = (m_total, m_offset)`` (grad_q then being its
+    contribution), as ``backward_config["impl"]`` selects: the backward kernels, or the torch shim."""
+    mode = backward_config["impl"]
+    if mode not in ("auto", "kernel", "shim"):
+        raise ValueError(f"backward_config['impl'] = {mode!r}")
+    if mode != "shim":
+        grads = None
+        if pm is not None and q.is_cuda and q.dim() == 3 and k.dim() == 3 and v.dim() == 3:
+            grads = _backward(q, k, v, out, grad_out, pm, pl, num_heads, scale, pad_mask, causal, dropout_p,
+                              dropout_seed, shard)
+        if grads is not None:
+            return grads
+        if mode == "kernel":
+            entry = "pcv_attn_bwd" if shard is None else "pcv_attn_bwd_shard"
+            raise RuntimeError(f"backward_config['impl'] = 'kernel' but {entry} does not cover this call: "
+                               + _lib.lib().pcv_last_error().decode())
+    m_total, m_offset = (None, 0) if shard is None else shard
+    return _backward_shim(q, k, v, out, grad_out, pm, pl, num_heads, scale, pad_mask, causal, dropout_p, dropout_seed,
+                          m_total, m_offset)
 
 
 def new_dropout_seed() -> int:
@@ -311,26 +387,19 @@ def attention_dropout_forward(q, k, v, stat_m, stat_l, num_heads: int, scale: fl
     over all keys (``stat_m`` / ``stat_l`` = its part_m / part_l): pcv_attn_fwd_dropout.  The keep decision of every
     (b, h, query, key) is a pure function of ``dropout_seed`` (``dropout_keep_mask`` exports it); the drop probability is
     ``dropout_p`` rounded to 1/256.  ``check_only``: launch nothing, return whether the kernel covers the operands."""
-    q, k, v, out_dtype = _prep(q, k, v)
+    out_dtype = q.dtype
+    q, k, v, _ = _prep(q, k, v)
     _require_cuda(stat_m, stat_l, pad_mask)
     with torch.cuda.device(k.device):
         p, keep = _fill_attn_params(q, k, v, num_heads, scale, pad_mask, causal, None, 0, "auto")
         if check_only:
             return bool(_lib.lib().pcv_attn_fwd_dropout_supported(C.byref(p), float(dropout_p)))
-        for name, t in (("stat_m", stat_m), ("stat_l", stat_l)):
-            if tuple(t.shape) != (p.B, p.H, p.N) or t.dtype != torch.float32 or not t.is_contiguous():
-                raise ValueError(f"{name} must be a contiguous float32 (B, H, N) tensor")
-        out = torch.empty(p.B, p.N, p.H * p.dv, dtype=q.dtype, device=k.device)
-        p.out = out.data_ptr()
-        p.o_stride_b, p.o_stride_n, p.o_stride_h = out.stride(0), out.stride(1), p.dv
-        need = C.c_size_t(0)
-        check(_lib.lib().pcv_attn_fwd_dropout_workspace_bytes(C.byref(p), C.byref(need)),
-              "pcv_attn_fwd_dropout_workspace_bytes")
-        ws = torch.empty(max(need.value, 256), dtype=torch.uint8, device=k.device)
-        p.workspace, p.workspace_bytes = ws.data_ptr(), need.value
+        _check_stats(p, stat_m, stat_l)
+        out = _new_output(p, q.dtype, k.device)
+        ws = _workspace(p, k.device, "pcv_attn_fwd_dropout", C.byref(p))
         check(_lib.lib().pcv_attn_fwd_dropout(C.byref(p), stat_m.data_ptr(), stat_l.data_ptr(), float(dropout_p),
                                               int(dropout_seed), _stream()), "pcv_attn_fwd_dropout")
-    del keep
+    del keep, ws
     return out if out.dtype == out_dtype else out.to(out_dtype)
 
 
@@ -363,39 +432,13 @@ def _dropout_scale(dropout_p: float) -> float:
 
 
 def _partial_dropout_supported(q, k, v, num_heads: int, pad_mask, causal: bool, dropout_p: float, impl: str) -> bool:
-    """Whether the one-pass dropout forward (attention_partial with dropout_p > 0) takes these operands, head dims
-    padded to multiples of 8 as the forward pads them."""
-    q, k, v, _ = _prep(q, k, v)
-    if _head_dim(q, num_heads) % 8 or _head_dim(v, num_heads) % 8:
-        q, k, v = _pad_heads_to8(q, num_heads), _pad_heads_to8(k, num_heads), _pad_heads_to8(v, num_heads)
+    """Whether the one-pass dropout forward (attention_partial with dropout_p > 0) takes these prepared operands."""
     with torch.cuda.device(k.device):
         p, keep = _fill_attn_params(q, k, v, num_heads, 1.0, pad_mask, causal, None, 0, impl)
         dummy = torch.empty(16, device=k.device)
         p.write_partial = 1
         p.part_o = p.part_m = p.part_l = dummy.data_ptr()
-        ok = bool(_lib.lib().pcv_attn_fwd_partial_dropout_supported(C.byref(p), float(dropout_p)))
-    del keep
-    return ok
-
-
-def _kernel_backward(q, k, v, out, grad_out, stat_m, stat_l, num_heads: int, scale: float, pad_mask, causal: bool,
-                     dropout_p: float, dropout_seed: int):
-    """(grad_q, grad_k, grad_v) of ``_FusedAttention`` on the backward kernels (``attention_backward``), or None where
-    they do not cover the call.  Head dims that are not multiples of 8 are zero-padded per head, as the forward padded
-    them, and the gradients sliced back: zero channels change neither the scores, nor delta = rowsum(dO * O), nor the
-    dropout mask, and the gradients of the padding channels are dropped."""
-    dqk, dv = _head_dim(q, num_heads), _head_dim(v, num_heads)
-    padded = bool(dqk % 8 or dv % 8)
-    if padded:
-        q, k, v, out, grad_out = (_pad_heads_to8(t, num_heads).flatten(2) for t in (q, k, v, out, grad_out))
-    if not attention_backward(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask, causal,
-                              check_only=True, dropout_p=dropout_p, dropout_seed=dropout_seed):
-        return None
-    gq, gk, gv = attention_backward(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask, causal,
-                                    dropout_p=dropout_p, dropout_seed=dropout_seed)
-    if padded:
-        gq, gk, gv = (g.unflatten(2, (num_heads, -1))[..., :d].flatten(2) for g, d in ((gq, dqk), (gk, dqk), (gv, dv)))
-    return gq, gk, gv
+        return bool(_lib.lib().pcv_attn_fwd_partial_dropout_supported(C.byref(p), float(dropout_p)))
 
 
 class _FusedAttention(torch.autograd.Function):
@@ -403,9 +446,9 @@ class _FusedAttention(torch.autograd.Function):
     the partial forward and the second-pass dropout kernel (``attention_dropout_forward``) where that covers the call
     (head dims that are multiples of 8 up to 128), else the one-pass dropout forward (``attention_partial`` with
     ``dropout_p``) for every head dim the forward takes.
-    Backward = the tensor-core backward kernels (``attention_backward`` -> pcv_attn_bwd: dK/dV and dQ kernels, SURVEY.md
-    §8(f) rank 2) for head dims up to 192; head dims that are not multiples of 8 are zero-padded as in the forward
-    (``_kernel_backward``).  Other shapes (head dims above 192, the decode forward) take the labelled SHIM below: the
+    Backward = the tensor-core backward kernels (pcv_attn_bwd: dK/dV and dQ kernels, SURVEY.md §8(f) rank 2) for head
+    dims up to 192; head dims that are not multiples of 8 are zero-padded as in the forward (``_backward``).  Other
+    shapes (head dims above 192, the decode forward) take the labelled SHIM below: the
     flash-attention backward recurrence in plain torch ops, chunked over the key axis from the saved statistics,
     memory bounded by ``backward_config["max_score_bytes"]``, with dropout regenerating the mask of each key chunk
     (``_dropout_keep``); neither path ever holds the (B, H, N, M) score tensor (8.6 GB at the north-star shape).
@@ -413,52 +456,35 @@ class _FusedAttention(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, q, k, v, num_heads, scale, pad_mask, causal, impl, dropout_p=0.0, dropout_seed=0):
-        dv_true = _head_dim(v, num_heads)
         ctx.dropout = (float(dropout_p), int(dropout_seed))
-        if dropout_p > 0.0:
-            if attention_dropout_forward(q, k, v, None, None, num_heads, scale, dropout_p, dropout_seed, pad_mask, causal,
-                                         check_only=True):
-                # statistics from the fused kernel, then the dropout pass (second kernel) writes the output
-                po, pm, pl = attention_partial(q, k, v, num_heads, scale, pad_mask=pad_mask, causal=causal, impl=impl)
-                del po
-                out = attention_dropout_forward(q, k, v, pm, pl, num_heads, scale, dropout_p, dropout_seed, pad_mask,
-                                                causal)
-            else:
-                # one pass: the dropped numerator and the dropout-free statistics; zero channels padding the head dims
-                # to multiples of 8 change neither the scores nor the mask
-                qp, kp, vp = q, k, v
-                if _head_dim(q, num_heads) % 8 or dv_true % 8:
-                    qp, kp, vp = (_pad_heads_to8(t, num_heads) for t in (q, k, v))
-                po, pm, pl = attention_partial(qp, kp, vp, num_heads, scale, pad_mask=pad_mask, causal=causal, impl=impl,
-                                               dropout_p=dropout_p, dropout_seed=dropout_seed)
-                out = combine_partials(po[None], pm[None], pl[None], _compute_dtype(q.dtype))
-                B, N, H, dv_pad = po.shape[0], po.shape[2], po.shape[1], po.shape[3]
-                del po
-                if dv_pad != dv_true:
-                    out = out.view(B, N, H, dv_pad)[..., :dv_true].reshape(B, N, H * dv_true)
-            out = out if out.dtype == q.dtype else out.to(q.dtype)
-            ctx.save_for_backward(q, k, v, pad_mask, out, pm, pl)
-            ctx.meta = (num_heads, scale, causal)
-            return out
-        if impl == "decode":
+        ctx.meta = (num_heads, scale, causal)
+        if impl == "decode" and not dropout_p > 0.0:
             # the decode kernel keeps no partial state: plain forward, statistics recomputed by the shim
             out = _attention_forward(q, k, v, num_heads, scale, pad_mask, causal, impl)
             ctx.save_for_backward(q, k, v, pad_mask, out, None, None)
+            return out
+        # head dims that are not multiples of 8 are zero-padded, so that the statistics exist for the backward kernels
+        qc, kc, vc, dims = _prep(q, k, v, num_heads=num_heads, pad=True)
+        if dropout_p > 0.0 and dims is None and attention_dropout_forward(
+                qc, kc, vc, None, None, num_heads, scale, dropout_p, dropout_seed, pad_mask, causal, check_only=True):
+            # statistics from the fused kernel, then the dropout pass (second kernel) writes the output
+            pm, pl = attention_partial(qc, kc, vc, num_heads, scale, pad_mask=pad_mask, causal=causal, impl=impl)[1:]
+            out = attention_dropout_forward(qc, kc, vc, pm, pl, num_heads, scale, dropout_p, dropout_seed, pad_mask,
+                                            causal)
         else:
-            # head dims that are not multiples of 8 are zero-padded (as in the dropout branch), so that the statistics
-            # exist for the backward kernels
-            qp, kp, vp = q, k, v
-            if _head_dim(q, num_heads) % 8 or dv_true % 8:
-                qp, kp, vp = (_pad_heads_to8(t, num_heads) for t in (q, k, v))
-            po, pm, pl = attention_partial(qp, kp, vp, num_heads, scale, pad_mask=pad_mask, causal=causal, impl=impl)
-            out = combine_partials(po[None], pm[None], pl[None], _compute_dtype(q.dtype))
-            B, N, H, dv_pad = po.shape[0], po.shape[2], po.shape[1], po.shape[3]
+            # one pass: the (dropped) numerator and the dropout-free statistics, merged by the combine kernel
+            if dropout_p > 0.0 and not _partial_dropout_supported(qc, kc, vc, num_heads, pad_mask, causal, dropout_p,
+                                                                  impl):
+                raise NotImplementedError("attention dropout is not available for this call: "
+                                          + _lib.lib().pcv_last_error().decode())
+            po, pm, pl = attention_partial(qc, kc, vc, num_heads, scale, pad_mask=pad_mask, causal=causal, impl=impl,
+                                           dropout_p=dropout_p, dropout_seed=dropout_seed)
+            out = combine_partials(po[None], pm[None], pl[None], qc.dtype)
             del po
-            if dv_pad != dv_true:
-                out = out.view(B, N, H, dv_pad)[..., :dv_true].reshape(B, N, H * dv_true)
-            out = out if out.dtype == q.dtype else out.to(q.dtype)
-            ctx.save_for_backward(q, k, v, pad_mask, out, pm, pl)
-        ctx.meta = (num_heads, scale, causal)
+            if dims is not None:
+                out = _unpad_heads(out, num_heads, dims[1])
+        out = out if out.dtype == q.dtype else out.to(q.dtype)
+        ctx.save_for_backward(q, k, v, pad_mask, out, pm, pl)
         return out
 
     @staticmethod
@@ -466,20 +492,7 @@ class _FusedAttention(torch.autograd.Function):
         q, k, v, pad_mask, out, pm, pl = ctx.saved_tensors
         H, scale, causal = ctx.meta
         drop_p, drop_seed = getattr(ctx, "dropout", (0.0, 0))
-        mode = backward_config["impl"]
-        if mode not in ("auto", "kernel", "shim"):
-            raise ValueError(f"backward_config['impl'] = {mode!r}")
-        if mode != "shim":
-            grads = None
-            if pm is not None and q.is_cuda and q.dim() == 3 and k.dim() == 3 and v.dim() == 3:
-                grads = _kernel_backward(q, k, v, out, grad_out, pm, pl, H, scale, pad_mask, causal, drop_p, drop_seed)
-            if grads is not None:
-                gq, gk, gv = grads
-                return gq.to(q.dtype), gk.to(k.dtype), gv.to(v.dtype), None, None, None, None, None, None, None
-            if mode == "kernel":
-                raise RuntimeError("backward_config['impl'] = 'kernel' but pcv_attn_bwd does not cover this call: "
-                                   + _lib.lib().pcv_last_error().decode())
-        gq, gk, gv = _backward_shim(q, k, v, out, grad_out, pm, pl, H, scale, pad_mask, causal, drop_p, drop_seed)
+        gq, gk, gv = _attention_grads(q, k, v, out, grad_out, pm, pl, H, scale, pad_mask, causal, drop_p, drop_seed)
         return gq.to(q.dtype), gk.to(k.dtype), gv.to(v.dtype), None, None, None, None, None, None, None
 
 
@@ -574,12 +587,7 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, num_heads: int,
     if dropout_p > 0.0:
         if not 0.0 < dropout_p < 1.0:
             raise ValueError(f"dropout_p must be in [0, 1), got {dropout_p}")
-        if not (attention_dropout_forward(q, k, v, None, None, num_heads, scale, dropout_p, 0, pad_mask, causal,
-                                          check_only=True)
-                or _partial_dropout_supported(q, k, v, num_heads, pad_mask, causal, dropout_p, impl)):
-            raise NotImplementedError("attention dropout is not available for this call: "
-                                      + _lib.lib().pcv_last_error().decode())
-        seed = new_dropout_seed() if dropout_seed is None else int(dropout_seed)
+        seed =new_dropout_seed() if dropout_seed is None else int(dropout_seed)
         return _FusedAttention.apply(q, k, v, num_heads, scale, pad_mask, causal, impl, float(dropout_p), seed)
     if torch.is_grad_enabled() and (q.requires_grad or k.requires_grad or v.requires_grad):
         return _FusedAttention.apply(q, k, v, num_heads, scale, pad_mask, causal, impl)
@@ -599,37 +607,20 @@ def attention_partial(q, k, v, num_heads: int, scale: float, pad_mask=None, caus
     q, k, v, _ = _prep(q, k, v)
     with torch.cuda.device(k.device):
         p, keep = _fill_attn_params(q, k, v, num_heads, scale, pad_mask, causal, m_total, m_offset, impl)
-        if out is not None:
-            part_o, part_m, part_l = out
-            if (tuple(part_o.shape) != (p.B, p.H, p.N, p.dv) or tuple(part_m.shape) != (p.B, p.H, p.N)
-                    or tuple(part_l.shape) != (p.B, p.H, p.N)):
-                raise ValueError("attention_partial: `out` tensors have the wrong shape")
-            for t in out:
-                if t.dtype != torch.float32 or not t.is_contiguous() or not t.is_cuda:
-                    raise ValueError("attention_partial: `out` tensors must be contiguous float32 CUDA tensors")
-        else:
-            part_o = torch.empty(p.B, p.H, p.N, p.dv, dtype=torch.float32, device=k.device)
-            part_m = torch.empty(p.B, p.H, p.N, dtype=torch.float32, device=k.device)
-            part_l = torch.empty(p.B, p.H, p.N, dtype=torch.float32, device=k.device)
-        p.write_partial = 1
-        p.part_o, p.part_m, p.part_l = part_o.data_ptr(), part_m.data_ptr(), part_l.data_ptr()
+        state = _partial_state(p, k.device, out)
         if dropout_p > 0.0:
             if p.impl == _lib.PCV_IMPL_AUTO:  # the dropout forward runs on the tensor-core kernel: size its workspace
                 p.impl = _lib.PCV_IMPL_TCGEN05
-            need = C.c_size_t(0)
-            check(_lib.lib().pcv_attn_workspace_bytes(C.byref(p), C.byref(need)), "pcv_attn_workspace_bytes")
-            ws = torch.empty(max(need.value, 256), dtype=torch.uint8, device=k.device)
-            p.workspace, p.workspace_bytes = ws.data_ptr(), need.value
-            if p.m_total == p.M and p.m_offset == 0:
-                check(_lib.lib().pcv_attn_fwd_partial_dropout(C.byref(p), float(dropout_p), int(dropout_seed),
-                                                              _stream()), "pcv_attn_fwd_partial_dropout")
-            else:
-                check(_lib.lib().pcv_attn_fwd_partial_dropout_shard(C.byref(p), float(dropout_p), int(dropout_seed),
-                                                                    _stream()), "pcv_attn_fwd_partial_dropout_shard")
+            ws = _workspace(p, k.device, "pcv_attn", C.byref(p))
+            entry = "pcv_attn_fwd_partial_dropout"
+            if p.m_total != p.M or p.m_offset != 0:
+                entry += "_shard"
+            check(getattr(_lib.lib(), entry)(C.byref(p), float(dropout_p), int(dropout_seed), _stream()), entry)
+            del ws
         else:
             _run_attn(p, k.device)
     del keep
-    return part_o, part_m, part_l
+    return state
 
 
 def _fill_fp8_params(q8, k8, vt8, q_descale, k_descale, v_descale, num_heads, scale, pad_mask, causal, m_total,
@@ -699,26 +690,11 @@ def attention_fp8(q8, k8, vt8, q_descale, k_descale, v_descale, num_heads: int, 
     with torch.cuda.device(k8.device):
         p, f, keep = _fill_fp8_params(q8, k8, vt8, q_descale, k_descale, v_descale, num_heads, scale, pad_mask, causal,
                                       m_total, m_offset, out_dtype)
-        dev = k8.device
-        if partial:
-            part_o = torch.empty(p.B, p.H, p.N, p.dv, dtype=torch.float32, device=dev)
-            part_m = torch.empty(p.B, p.H, p.N, dtype=torch.float32, device=dev)
-            part_l = torch.empty(p.B, p.H, p.N, dtype=torch.float32, device=dev)
-            p.write_partial = 1
-            p.part_o, p.part_m, p.part_l = part_o.data_ptr(), part_m.data_ptr(), part_l.data_ptr()
-        else:
-            out = torch.empty(p.B, p.N, p.H * p.dv, dtype=out_dtype, device=dev)
-            p.out = out.data_ptr()
-            p.o_stride_b, p.o_stride_n, p.o_stride_h = out.stride(0), out.stride(1), p.dv
-        need = C.c_size_t(0)
-        check(_lib.lib().pcv_attn_workspace_bytes(C.byref(p), C.byref(need)), "pcv_attn_workspace_bytes")
-        ws = None
-        if need.value:
-            ws = torch.empty(need.value, dtype=torch.uint8, device=dev)
-            p.workspace, p.workspace_bytes = ws.data_ptr(), need.value
+        result = _partial_state(p, k8.device) if partial else _new_output(p, out_dtype, k8.device)
+        ws = _workspace(p, k8.device, "pcv_attn", C.byref(p))
         check(_lib.lib().pcv_attn_fwd_fp8(C.byref(p), C.byref(f), _stream()), "pcv_attn_fwd_fp8")
     del keep, ws
-    return (part_o, part_m, part_l) if partial else out
+    return result
 
 
 def attention_sharded_fused(q, k, v, num_heads: int, scale: float, fuse, pad_mask=None, causal: bool = False,
@@ -737,14 +713,9 @@ def attention_sharded_fused(q, k, v, num_heads: int, scale: float, fuse, pad_mas
             return bool(_lib.lib().pcv_attn_fwd_sharded_supported(C.byref(p)))
         dummy_ptr = fuse.part[fuse.rank]
         p.part_o = p.part_m = p.part_l = dummy_ptr
-        need = C.c_size_t(0)
-        check(_lib.lib().pcv_attn_workspace_bytes(C.byref(p), C.byref(need)), "pcv_attn_workspace_bytes")
-        ws = None
-        if need.value:
-            ws = torch.empty(need.value, dtype=torch.uint8, device=k.device)
-            p.workspace, p.workspace_bytes = ws.data_ptr(), need.value
+        ws = _workspace(p, k.device, "pcv_attn", C.byref(p))
         check(_lib.lib().pcv_attn_fwd_sharded(C.byref(p), C.byref(fuse), _stream()), "pcv_attn_fwd_sharded")
-    del keep
+    del keep, ws
 
 
 def combine_partials(part_o: torch.Tensor, part_m: torch.Tensor, part_l: torch.Tensor,
@@ -1068,15 +1039,12 @@ def rotated_cache_keys(k: torch.Tensor, q: torch.Tensor, num_heads: int, inv_fre
 
 def tcgen05_supported(q, k, v, num_heads: int, pad_mask=None, causal: bool = False) -> bool:
     """True when pcv_attn_fwd would pick the tcgen05 kernel for these operands."""
-    q, k, v, _ = _prep(q, k, v)
-    if _head_dim(q, num_heads) % 8 or _head_dim(v, num_heads) % 8:  # same padding rule as the forward
-        q, k, v = _pad_heads_to8(q, num_heads), _pad_heads_to8(k, num_heads), _pad_heads_to8(v, num_heads)
-    p, keep = _fill_attn_params(q, k, v, num_heads, 1.0, pad_mask, causal, None, 0, "auto")
-    dummy = torch.empty(16, device=k.device)
-    p.out = dummy.data_ptr()
-    ok = bool(_lib.lib().pcv_attn_supported_tcgen05(C.byref(p)))
-    del keep
-    return ok
+    q, k, v, _ = _prep(q, k, v, num_heads=num_heads, pad=True)  # the forward's padding rule
+    with torch.cuda.device(k.device):
+        p, keep = _fill_attn_params(q, k, v, num_heads, 1.0, pad_mask, causal, None, 0, "auto")
+        dummy = torch.empty(16, device=k.device)
+        p.out = dummy.data_ptr()
+        return bool(_lib.lib().pcv_attn_supported_tcgen05(C.byref(p)))
 
 
 # --------------------------------------------------------------------------------------------------

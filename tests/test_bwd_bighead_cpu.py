@@ -130,7 +130,7 @@ def _stats(q, k, H, scale, pad, causal):
 
 @pytest.mark.parametrize("with_pad", [False, True])
 @pytest.mark.parametrize("causal", [False, True])
-def test_odd_head_dims_are_padded_for_the_kernels_and_sliced_back(with_pad, causal, monkeypatch):
+def test_odd_head_dims_are_padded_around_the_backward_kernels(with_pad, causal, monkeypatch):
     """131 / 131 (the image classifier's encoder cross-attention), batch-1 q: the operands reach the kernels padded to
     136 per head with zeros, and the gradients that come back equal fp64 autograd of the unpadded eager formula."""
     B, N, M, H, d = 2, 5, 40, 2, 131
@@ -148,35 +148,32 @@ def test_odd_head_dims_are_padded_for_the_kernels_and_sliced_back(with_pad, caus
     go = torch.randn(o.shape, generator=g, dtype=torch.float64)
     ref = torch.autograd.grad(o, (q, k, v), go)
     pm, pl = _stats(q.detach(), k.detach(), H, scale, pad, causal)
-    calls = []
 
-    def fp64_kernels(q_, k_, v_, out_, go_, pm_, pl_, H_, scale_, pad_, causal_, check_only=False, dropout_p=0.0,
-                     dropout_seed=0):
+    def fp64_kernels(q_, k_, v_, out_, go_, pm_, pl_, H_, scale_, pad_, causal_, dropout_p, dropout_seed, shard, mode):
         for t in (q_, k_, v_, out_, go_):
             assert t.dim() == 3 and t.shape[2] == H * 136
             assert (t.unflatten(2, (H, 136))[..., d:] == 0).all()
         assert pm_ is pm and pl_ is pl and pad_ is pad and causal_ == causal and scale_ == scale
-        calls.append(check_only)
-        if check_only:
-            return True
+        assert shard is None and mode == "try"
         qq, kk, vv = (t.detach().clone().requires_grad_() for t in (q_, k_, v_))
         oo = _eager(qq, kk, vv, H, scale_, pad_, causal_)
         # the kernels take out and delta = rowsum(dO * O) from their operands: the padded out must be the forward's
         assert torch.allclose(oo.detach(), out_, rtol=0, atol=1e-12)
         return torch.autograd.grad(oo, (qq, kk, vv), go_)
 
-    monkeypatch.setattr(ops, "attention_backward", fp64_kernels)
-    got = ops._kernel_backward(q.detach(), k.detach(), v.detach(), o.detach(), go, pm, pl, H, scale, pad, causal,
-                               0.0, 0)
-    assert calls == [True, False]
+    monkeypatch.setattr(ops, "_backward_kernels", fp64_kernels)
+    monkeypatch.setattr(ops, "_require_cuda", lambda *a: None)
+    monkeypatch.setattr(ops, "_compute_dtype", lambda dt: dt)  # the fp64 stand-in takes the fp64 operands
+    got = ops._backward(q.detach(), k.detach(), v.detach(), o.detach(), go, pm, pl, H, scale, pad, causal, 0.0, 0)
     for gr, r, name in zip(got, ref, "qkv"):
         assert gr.shape == r.shape, name
         err = (gr - r).abs().max().item()
         assert err <= 1e-12 * max(1.0, r.abs().max().item()), (name, err)
 
 
-def test_kernel_backward_declines_what_the_kernels_do_not_cover(monkeypatch):
-    monkeypatch.setattr(ops, "attention_backward", lambda *a, **kw: False)
+def test_backward_route_declines_what_the_kernels_do_not_cover(monkeypatch):
+    monkeypatch.setattr(ops, "_backward_kernels", lambda *a: None)
+    monkeypatch.setattr(ops, "_require_cuda", lambda *a: None)
     q = torch.zeros(1, 3, 8 * 2)
     k = v = torch.zeros(1, 4, 8 * 2)
-    assert ops._kernel_backward(q, k, v, q, q, None, None, 2, 1.0, None, False, 0.0, 0) is None
+    assert ops._backward(q, k, v, q, q, None, None, 2, 1.0, None, False, 0.0, 0) is None
