@@ -491,6 +491,53 @@ PCV_API int pcv_kv_project_fp8_supported(const pcv_kvproj_params* p, const pcv_k
 PCV_API int pcv_kv_project_fp8(const pcv_kvproj_params* p, const pcv_kvproj_fp8* f, void* stream);
 
 /*
+ * Backward of the LayerNorm -> Linear chain pcv_kv_project computes (training through kv_norm -> k_proj / v_proj,
+ * q_norm -> q_proj, norm -> q/k/v_proj).  With x_hat = (x - mean) * rstd (row_stats of pcv_ln_stats),
+ * y = x_hat * gamma + beta, out = y W^T + b, W = [W_k ; W_v] (n_k + n_v, C) and G = [grad_k | grad_v] (rows, n):
+ *   grad_b = G^T 1,  grad_w = (G^T x_hat) diag(gamma) + grad_b beta^T,
+ *   dy = G W,  grad_gamma = sum_rows dy * x_hat,  grad_beta = sum_rows dy,
+ *   grad_x = rstd * (dx_hat - (a + x_hat * b) / C),  dx_hat = gamma * dy,  a = sum_c dx_hat,  b = sum_c dx_hat * x_hat.
+ * Two wgmma GEMMs (dy = G W with dx_hat written to grad_x and per-tile fp32 row / column partials; G^T x_hat with x_hat
+ * formed in registers from x and the statistics and rounded to 16 bits) and three small kernels that sum the partials
+ * in a fixed order: no atomics, every gradient is bitwise reproducible.
+ *   x          : (rows, C) with a row stride; w: (n_k + n_v, C) contiguous, the UNFOLDED weights
+ *   gamma/beta : (C) or NULL (gamma NULL = 1, beta NULL = 0)
+ *   grad_k/v   : (rows, n_k) / (rows, n_v), each with its own row stride (as k_out / v_out of pcv_kv_project)
+ *   grad_x     : (rows, C) contiguous; grad_w (n_k + n_v, C) contiguous; grad_b (n_k + n_v); grad_gamma / grad_beta
+ *                (C).  Each may be NULL when it is not needed.
+ * All tensors are in `dtype`.  Widths and alignment as pcv_kv_project (C and n_v multiples of 8, n_k a multiple of 64,
+ * strides multiples of 8 elements, 16-byte aligned x / w / grad_k / grad_v / grad_x).  The workspace
+ * (pcv_ln_linear_bwd_workspace_bytes, a function of rows, C, n_k and n_v alone) is 256-byte aligned.  Arguments are
+ * checked before any CUDA call.
+ */
+typedef struct pcv_ln_linear_bwd_params {
+  const void* x;
+  int64_t x_stride_row;
+  const float* row_stats;  /* (rows, 2) f32 (mean, rstd) */
+  const void* w;
+  const void* gamma;
+  const void* beta;
+  const void* grad_k;
+  const void* grad_v;
+  int64_t gk_stride_row, gv_stride_row;
+  void* grad_x;
+  void* grad_w;
+  void* grad_b;
+  void* grad_gamma;
+  void* grad_beta;
+  int64_t rows;
+  int32_t C, n_k, n_v;
+  int32_t dtype;           /* PCV_BF16 / PCV_F16 */
+  void* workspace;
+  size_t workspace_bytes;
+} pcv_ln_linear_bwd_params;
+
+/* 1 if pcv_ln_linear_bwd covers this problem, else 0 (reason via pcv_last_error) */
+PCV_API int pcv_ln_linear_bwd_supported(const pcv_ln_linear_bwd_params* p);
+PCV_API int pcv_ln_linear_bwd_workspace_bytes(const pcv_ln_linear_bwd_params* p, size_t* bytes);
+PCV_API int pcv_ln_linear_bwd(const pcv_ln_linear_bwd_params* p, void* stream);
+
+/*
  * Live timing of the dominant kernel (bench.py's roofline leg): between pcv_profile_begin() and
  * pcv_profile_end() every attention main-kernel launch is bracketed by CUDA events on its own
  * stream; pcv_profile_end() synchronises those events and returns their summed duration.

@@ -57,6 +57,9 @@ EXPORTS = (
     "pcv_attn_fwd_fp8",
     "pcv_kv_project_fp8_supported",
     "pcv_kv_project_fp8",
+    "pcv_ln_linear_bwd_supported",
+    "pcv_ln_linear_bwd_workspace_bytes",
+    "pcv_ln_linear_bwd",
     "pcv_launch_count",
     "pcv_debug_plan",
     "pcv_profile_begin",
@@ -227,6 +230,20 @@ class KvProjFp8(C.Structure):
     ]
 
 
+class LnLinearBwdParams(C.Structure):
+    _fields_ = [
+        ("x", C.c_void_p), ("x_stride_row", C.c_int64), ("row_stats", C.c_void_p),
+        ("w", C.c_void_p), ("gamma", C.c_void_p), ("beta", C.c_void_p),
+        ("grad_k", C.c_void_p), ("grad_v", C.c_void_p),
+        ("gk_stride_row", C.c_int64), ("gv_stride_row", C.c_int64),
+        ("grad_x", C.c_void_p), ("grad_w", C.c_void_p), ("grad_b", C.c_void_p),
+        ("grad_gamma", C.c_void_p), ("grad_beta", C.c_void_p),
+        ("rows", C.c_int64),
+        ("C", C.c_int32), ("n_k", C.c_int32), ("n_v", C.c_int32), ("dtype", C.c_int32),
+        ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t),
+    ]
+
+
 class DeviceInfo(C.Structure):
     _fields_ = [
         ("device", C.c_int32), ("sm_major", C.c_int32), ("sm_minor", C.c_int32),
@@ -326,6 +343,12 @@ def lib() -> C.CDLL:
         l.pcv_kv_project_fp8_supported.restype = C.c_int
         l.pcv_kv_project_fp8.argtypes = [C.POINTER(KvProjParams), C.POINTER(KvProjFp8), C.c_void_p]
         l.pcv_kv_project_fp8.restype = C.c_int
+        l.pcv_ln_linear_bwd_supported.argtypes = [C.POINTER(LnLinearBwdParams)]
+        l.pcv_ln_linear_bwd_supported.restype = C.c_int
+        l.pcv_ln_linear_bwd_workspace_bytes.argtypes = [C.POINTER(LnLinearBwdParams), C.POINTER(C.c_size_t)]
+        l.pcv_ln_linear_bwd_workspace_bytes.restype = C.c_int
+        l.pcv_ln_linear_bwd.argtypes = [C.POINTER(LnLinearBwdParams), C.c_void_p]
+        l.pcv_ln_linear_bwd.restype = C.c_int
         l.pcv_debug_plan.argtypes = [C.c_int32] * 7 + [C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_int32)]
         l.pcv_debug_plan.restype = C.c_int
         for name in ("pcv_get_device_info", "pcv_attn_supported_tcgen05", "pcv_attn_workspace_bytes",

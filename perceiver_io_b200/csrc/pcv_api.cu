@@ -278,6 +278,27 @@ int pcv_kv_project(const pcv_kvproj_params* p, void* stream) {
   return launch_kv_project(*p, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int pcv_ln_linear_bwd_supported(const pcv_ln_linear_bwd_params* p) {
+  if (p == nullptr) {
+    set_error("ln_linear_bwd: params is NULL");
+    return 0;
+  }
+  const char* why = "";
+  const bool ok = ln_linear_bwd_supported(*p, &why);
+  if (!ok) set_error("ln_linear_bwd not applicable: %s", why);
+  return ok ? 1 : 0;
+}
+
+int pcv_ln_linear_bwd_workspace_bytes(const pcv_ln_linear_bwd_params* p, size_t* bytes) {
+  PCV_REQUIRE(p != nullptr, PCV_ERR_INVALID, "ln_linear_bwd_workspace_bytes: params is NULL");
+  return ln_linear_bwd_workspace_bytes(*p, bytes);
+}
+
+int pcv_ln_linear_bwd(const pcv_ln_linear_bwd_params* p, void* stream) {
+  PCV_REQUIRE(p != nullptr, PCV_ERR_INVALID, "ln_linear_bwd: params is NULL");
+  return launch_ln_linear_bwd(*p, reinterpret_cast<cudaStream_t>(stream));
+}
+
 // s == nullptr: the unsharded backward
 static int bwd_check(const pcv_attn_bwd_params* p, const pcv_key_shard* s) {
   if (p == nullptr) return 0;

@@ -118,6 +118,9 @@ bool kv_project_supported(const pcv_kvproj_params& p, const char** why);
 int launch_kv_project(const pcv_kvproj_params& p, cudaStream_t stream);
 bool kv_project_fp8_supported(const pcv_kvproj_params& p, const pcv_kvproj_fp8& f, const char** why);
 int launch_kv_project_fp8(const pcv_kvproj_params& p, const pcv_kvproj_fp8& f, cudaStream_t stream);
+bool ln_linear_bwd_supported(const pcv_ln_linear_bwd_params& p, const char** why);
+int ln_linear_bwd_workspace_bytes(const pcv_ln_linear_bwd_params& p, size_t* bytes);
+int launch_ln_linear_bwd(const pcv_ln_linear_bwd_params& p, cudaStream_t stream);
 // shard == nullptr: the backward over all keys (pcv_attn_bwd); else one key shard's (pcv_attn_bwd_shard)
 bool attn_bwd_supported(const pcv_attn_bwd_params& p, const pcv_key_shard* shard, const char** why);
 int attn_bwd_workspace_bytes(const pcv_attn_bwd_params& p, const pcv_key_shard* shard, size_t* bytes);

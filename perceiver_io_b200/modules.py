@@ -144,7 +144,11 @@ def attend(mha, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, pad_mask=None
 #: (B*N of a few thousand rows) is bound by host-side dispatch, where ATen's nn.Linear path is leaner than three ctypes
 #: calls; under a CUDA graph (``graphs.graph_latent_block`` lowers the threshold while recording) the fused path wins
 #: because it launches 4 kernels per layer instead of 7 (tools/latent_stack_bench.py).
-kv_producer_config = {"enabled": True, "min_rows": 512, "min_rows_latent": 4096}
+#: ``training``: under autograd, route the LayerNorm -> projection chains (``project_kv``, ``fused_linear`` with a norm,
+#: ``project_qkv``) through ``ops.ln_linear`` (the fused producer forward, which saves x and the row statistics instead
+#: of the LayerNorm output, and the ``pcv_ln_linear_bwd`` backward).  Off by default: training then runs LayerNorm + the
+#: library GEMMs as before.
+kv_producer_config = {"enabled": True, "min_rows": 512, "min_rows_latent": 4096, "training": False}
 
 
 def _fold_cache(owner: nn.Module, slot: str, norm: Optional[nn.Module], linears, dtype: torch.dtype):
@@ -165,9 +169,10 @@ def _fold_cache(owner: nn.Module, slot: str, norm: Optional[nn.Module], linears,
     return w_cat, col_st
 
 
-def _fusable(x: torch.Tensor, linears, norm, min_rows_key: str = "min_rows") -> bool:
+def _fusable(x: torch.Tensor, linears, norm, min_rows_key: str = "min_rows", allow_grad: bool = False) -> bool:
     """Inference on bf16/fp16 CUDA rows with parameters in the same dtype: the case the tcgen05 projection kernel
-    (ops.kv_project) covers; autograd, autocast, fp32 and tiny inputs stay on LayerNorm + nn.Linear (library GEMMs)."""
+    (ops.kv_project) covers; autograd, autocast, fp32 and tiny inputs stay on LayerNorm + nn.Linear (library GEMMs).
+    ``allow_grad``: the same conditions without the one on autograd (the training route, ``_trains_fused``)."""
     if not kv_producer_config["enabled"] or not x.is_cuda or x.dtype not in (torch.bfloat16, torch.float16):
         return False
     if x.numel() // max(x.shape[-1], 1) < kv_producer_config[min_rows_key] or torch.is_autocast_enabled():
@@ -177,10 +182,23 @@ def _fusable(x: torch.Tensor, linears, norm, min_rows_key: str = "min_rows") -> 
         return False
     if any(lin.weight.dtype != x.dtype or lin.in_features != x.shape[-1] for lin in linears):
         return False
-    if torch.is_grad_enabled() and (x.requires_grad or any(lin.weight.requires_grad for lin in linears)
+    if not allow_grad and torch.is_grad_enabled() and (x.requires_grad or any(lin.weight.requires_grad for lin in linears)
                                     or (norm is not None and norm.weight is not None and norm.weight.requires_grad)):
         return False
     return True
+
+
+def _trains_fused(x: torch.Tensor, linears, norm, min_rows_key: str = "min_rows") -> bool:
+    """A LayerNorm -> projection chain under autograd that ``kv_producer_config["training"]`` sends to ops.ln_linear."""
+    return (kv_producer_config["training"] and norm is not None and torch.is_grad_enabled()
+            and _fusable(x, linears, norm, min_rows_key, allow_grad=True))
+
+
+def _ln_linear(owner: nn.Module, slot: str, norm: nn.LayerNorm, linears, x: torch.Tensor, n_k: int, n_v: int):
+    """ops.ln_linear of ``linears(norm(x))`` with the folded weights cached on ``owner`` (rebuilt per weight version)."""
+    w_cat, col_st = _fold_cache(owner, slot, norm if norm.weight is not None else None, linears, x.dtype)
+    return ops.ln_linear(x, norm.weight, norm.bias, [lin.weight for lin in linears], [lin.bias for lin in linears],
+                         n_k, n_v, norm.eps, w_cat, col_st)
 
 
 def fused_linear(owner: nn.Module, slot: str, norm: Optional[nn.Module], linear: nn.Linear, x: torch.Tensor,
@@ -189,6 +207,8 @@ def fused_linear(owner: nn.Module, slot: str, norm: Optional[nn.Module], linear:
     q_proj chain of CrossAttention (reference modules.py:220, :113) and o_proj (:168) — else the library path."""
     n_out = linear.out_features
     if not (_fusable(x, [linear], norm, min_rows_key) and ops.kv_project_supported(x, n_out, 0)):
+        if _trains_fused(x, [linear], norm, min_rows_key) and ops.kv_project_supported(x, n_out, 0):
+            return _ln_linear(owner, slot, norm, [linear], x, n_out, 0)[0]
         return linear(x if norm is None else norm(x))
     affine = norm if (norm is not None and norm.weight is not None) else None
     w_cat, col_st = _fold_cache(owner, slot, affine, [linear], x.dtype)
@@ -206,6 +226,8 @@ def project_kv(cross_attn, x_kv: torch.Tensor):
     norm = cross_attn.kv_norm
     n_k, n_v = attn.k_proj.out_features, attn.v_proj.out_features
     if not (_fusable(x_kv, [attn.k_proj, attn.v_proj], norm) and ops.kv_project_supported(x_kv, n_k, n_v)):
+        if _trains_fused(x_kv, [attn.k_proj, attn.v_proj], norm) and ops.kv_project_supported(x_kv, n_k, n_v):
+            return _ln_linear(cross_attn, "_pcv_kv_fold", norm, [attn.k_proj, attn.v_proj], x_kv, n_k, n_v)
         x = norm(x_kv)
         return attn.k_proj(x), attn.v_proj(x)
     w_cat, col_st = _fold_cache(cross_attn, "_pcv_kv_fold", norm if norm.weight is not None else None,
@@ -220,8 +242,11 @@ def project_qkv(self_attn, x: torch.Tensor):
     the fused path does not apply (autograd, fp32, autocast, tiny inputs): the caller then runs the library path."""
     attn, norm = self_attn.attention, self_attn.norm
     n_q, n_k, n_v = attn.q_proj.out_features, attn.k_proj.out_features, attn.v_proj.out_features
-    if not (_fusable(x, [attn.q_proj, attn.k_proj, attn.v_proj], norm, "min_rows_latent")
-            and ops.kv_project_supported(x, n_q, n_k + n_v)):
+    linears = [attn.q_proj, attn.k_proj, attn.v_proj]
+    if not (_fusable(x, linears, norm, "min_rows_latent") and ops.kv_project_supported(x, n_q, n_k + n_v)):
+        if _trains_fused(x, linears, norm, "min_rows_latent") and ops.kv_project_supported(x, n_q, n_k + n_v):
+            q, kv = _ln_linear(self_attn, "_pcv_qkv_fold", norm, linears, x, n_q, n_k + n_v)
+            return q, kv[..., :n_k], kv[..., n_k:]
         return None
     w_cat, col_st = _fold_cache(self_attn, "_pcv_qkv_fold", norm if norm.weight is not None else None,
                                 [attn.q_proj, attn.k_proj, attn.v_proj], x.dtype)

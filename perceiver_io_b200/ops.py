@@ -27,7 +27,7 @@ __all__ = [
     "attention", "attention_partial", "attention_sharded_fused", "combine_partials", "merge_partials", "rescale_partial_", "rotary", "kv_append",
     "device_info", "tcgen05_supported", "rotated_cache_keys", "ln_stats", "fold_ln_linear", "kv_project", "kv_project_supported",
     "attention_fp8", "attention_fp8_supported", "fp8_descales", "fp8_quantize", "fp8_transpose_v", "kv_project_fp8",
-    "kv_project_fp8_supported",
+    "kv_project_fp8_supported", "ln_linear", "ln_linear_backward",
 ]
 
 
@@ -1272,3 +1272,116 @@ def kv_project_fp8(x: torch.Tensor, w_cat: torch.Tensor, col_st: torch.Tensor, i
                                 eps if (eps is not None and mode == "fused") else 0.0)
         check(_lib.lib().pcv_kv_project_fp8(C.byref(p), C.byref(f), _stream()), "pcv_kv_project_fp8")
     return (None if k8 is None else k8.view(B, M, n_k)), vt8
+
+
+# --------------------------------------------------------------------------------------------------
+# training through the LayerNorm -> Linear chain: the fused producer forward + pcv_ln_linear_bwd
+# --------------------------------------------------------------------------------------------------
+def _gemm_rows(t: torch.Tensor, n: int) -> torch.Tensor:
+    """(..., n) -> (rows, n) with unit column stride, a row stride that is a multiple of 8 elements and covers the row,
+    and 16-byte alignment (copied if not: a gradient broadcast along the rows has row stride 0)."""
+    t2 = t.reshape(-1, n)
+    if t2.stride(1) != 1 or t2.stride(0) < n or t2.stride(0) % 8 or t2.data_ptr() % 16:
+        t2 = t2.contiguous() if not t2.is_contiguous() else t2.clone()
+    return t2
+
+
+def ln_linear_backward(x: torch.Tensor, stats: torch.Tensor, w: torch.Tensor, gamma: Optional[torch.Tensor],
+                       beta: Optional[torch.Tensor], grad_k: Optional[torch.Tensor], grad_v: Optional[torch.Tensor],
+                       n_k: int, n_v: int, needs=(True, True, True, True, True)):
+    """Gradients of ``[k | v] = LN(x) W^T + b`` (LN(x) = (x - mean) * rstd * gamma + beta) through pcv_ln_linear_bwd.
+
+    x (rows, C) 16-bit with ``stats`` (rows, 2) f32 from :func:`ln_stats`; w the UNFOLDED (n_k + n_v, C) weights; gamma /
+    beta (C) or None; grad_k (rows, n_k), grad_v (rows, n_v) (None for a width of 0).  ``needs`` selects
+    (grad_x, grad_w, grad_b, grad_gamma, grad_beta); unneeded ones come back as None.  Bitwise reproducible."""
+    _require_cuda(x, stats, w, gamma, beta, grad_k, grad_v)
+    dt = x.dtype
+    rows, Cin = x.shape
+    if w.dtype != dt or w.shape != (n_k + n_v, Cin) or not w.is_contiguous():
+        raise ValueError("ln_linear_backward: w must be a contiguous (n_k + n_v, C) tensor in x's dtype")
+    for name, t in (("gamma", gamma), ("beta", beta)):
+        if t is not None and (t.dtype != dt or t.shape != (Cin,) or not t.is_contiguous()):
+            raise ValueError(f"ln_linear_backward: {name} must be a contiguous (C,) tensor in x's dtype")
+    gk = _gemm_rows(grad_k.to(dt), n_k) if n_k else None
+    gv = _gemm_rows(grad_v.to(dt), n_v) if n_v else None
+    dev = x.device
+    out = [torch.empty(rows, Cin, dtype=dt, device=dev) if needs[0] else None,
+           torch.empty(n_k + n_v, Cin, dtype=dt, device=dev) if needs[1] else None,
+           torch.empty(n_k + n_v, dtype=dt, device=dev) if needs[2] else None,
+           torch.empty(Cin, dtype=dt, device=dev) if needs[3] else None,
+           torch.empty(Cin, dtype=dt, device=dev) if needs[4] else None]
+    if all(o is None for o in out):
+        return tuple(out)
+    ptr = lambda t: None if t is None else t.data_ptr()
+    p = _lib.LnLinearBwdParams()
+    p.x, p.x_stride_row, p.row_stats = x.data_ptr(), x.stride(0), stats.data_ptr()
+    p.w, p.gamma, p.beta = w.data_ptr(), ptr(gamma), ptr(beta)
+    p.grad_k, p.grad_v = ptr(gk), ptr(gv)
+    p.gk_stride_row = gk.stride(0) if gk is not None else 0
+    p.gv_stride_row = gv.stride(0) if gv is not None else 0
+    p.grad_x, p.grad_w, p.grad_b, p.grad_gamma, p.grad_beta = (ptr(o) for o in out)
+    p.rows, p.C, p.n_k, p.n_v, p.dtype = rows, Cin, n_k, n_v, _pcv_dtype(dt)
+    with torch.cuda.device(dev):
+        ws = _workspace(p, dev, "pcv_ln_linear_bwd", C.byref(p))  # noqa: F841 (kept until the launch is enqueued)
+        check(_lib.lib().pcv_ln_linear_bwd(C.byref(p), _stream()), "pcv_ln_linear_bwd")
+    return tuple(out)
+
+
+class _LnLinear(torch.autograd.Function):
+    """[k | v] = LN(x) W^T + b: forward by pcv_ln_stats + the fused producer (y is never materialised), backward by
+    pcv_ln_linear_bwd.  Saves x, the row statistics and the parameters."""
+
+    @staticmethod
+    def forward(ctx, x, gamma, beta, w, b, w_cat, col_st, n_k: int, n_v: int, eps: float):
+        lead = x.shape[:-1]
+        x2 = _rows2d(x)
+        with torch.cuda.device(x.device):
+            st = ln_stats(x2, eps)
+            k_out = torch.empty(x2.shape[0], n_k, dtype=x.dtype, device=x.device) if n_k else None
+            v_out = torch.empty(x2.shape[0], n_v, dtype=x.dtype, device=x.device) if n_v else None
+            p = _fill_kvproj(x2, w_cat, col_st, n_k, n_v, st, k_out, v_out)
+            check(_lib.lib().pcv_kv_project(C.byref(p), _stream()), "pcv_kv_project")
+        ctx.save_for_backward(x2, st, w, gamma, beta)
+        ctx.dims = (x.shape, n_k, n_v, b is not None)
+        outs = [o.view(*lead, o.shape[1]) for o in (k_out, v_out) if o is not None]
+        return tuple(outs)
+
+    @staticmethod
+    def backward(ctx, *grads):
+        x2, st, w, gamma, beta = ctx.saved_tensors
+        shape, n_k, n_v, has_b = ctx.dims
+        ni = ctx.needs_input_grad
+        rows = x2.shape[0]
+        g = list(grads)
+        for i, n in enumerate(d for d in (n_k, n_v) if d):
+            if g[i] is None:
+                g[i] = torch.zeros(rows, n, dtype=x2.dtype, device=x2.device)
+        gk = g[0] if n_k else None
+        gv = (g[1] if n_k else g[0]) if n_v else None
+        needs = (ni[0], ni[3], ni[4] and has_b, ni[1] and gamma is not None, ni[2] and beta is not None)
+        dx, dw, db, dgamma, dbeta = ln_linear_backward(x2, st, w, gamma, beta, gk, gv, n_k, n_v, needs)
+        return (None if dx is None else dx.view(shape)), dgamma, dbeta, dw, db, None, None, None, None, None
+
+
+def ln_linear(x: torch.Tensor, norm_weight: Optional[torch.Tensor], norm_bias: Optional[torch.Tensor], weights, biases,
+              n_k: int, n_v: int, eps: float = 1e-5, w_cat: Optional[torch.Tensor] = None,
+              col_st: Optional[torch.Tensor] = None):
+    """Differentiable ``LN(x) [W_k; W_v]^T + [b_k; b_v]`` of x (..., C) on this package's kernels: the forward is
+    :func:`kv_project` with separate statistics, the backward :func:`ln_linear_backward`.  ``weights`` / ``biases``
+    are the Linear layers' tensors (biases may be None) whose concatenation has n_k + n_v rows; ``norm_weight`` /
+    ``norm_bias`` the LayerNorm's (None = no affine part).  ``w_cat`` / ``col_st``: the folded weights of
+    :func:`fold_ln_linear` when the caller caches them.  Returns (k, v), v None when n_v == 0."""
+    _require_cuda(x)
+    dt = x.dtype
+    if w_cat is None or col_st is None:
+        w_cat, col_st = fold_ln_linear(norm_weight, norm_bias, list(weights), list(biases), dt)
+    w = torch.cat([wi.to(dt) for wi in weights], dim=0) if len(weights) > 1 else weights[0].to(dt)
+    if all(bi is None for bi in biases):
+        b = None
+    else:
+        b = torch.cat([(torch.zeros(wi.shape[0], dtype=dt, device=x.device) if bi is None else bi.to(dt))
+                       for wi, bi in zip(weights, biases)])
+    gamma = None if norm_weight is None else norm_weight.to(dt)
+    beta = None if norm_bias is None else norm_bias.to(dt)
+    outs = _LnLinear.apply(x, gamma, beta, w.contiguous(), b, w_cat, col_st, n_k, n_v, float(eps))
+    return (outs[0], outs[1]) if (n_k and n_v) else ((outs[0], None) if n_k else (None, outs[0]))
