@@ -46,7 +46,7 @@ extern "C" {
 #endif
 
 /* element type of q/k/v/out */
-enum pcv_dtype { PCV_BF16 = 0, PCV_F16 = 1, PCV_F32 = 2 /* pcv_kv_append only */, PCV_E4M3 = 3 /* pcv_attn_fwd_fp8 only */ };
+enum pcv_dtype { PCV_BF16 = 0, PCV_F16 = 1, PCV_F32 = 2 /* pcv_kv_append only */, PCV_E4M3 = 3 /* the *_fp8 entry points only */ };
 
 /* kernel selection; AUTO picks the tensor-core kernel whenever the shape is supported (the names are historical) */
 enum pcv_impl {
@@ -489,6 +489,57 @@ typedef struct pcv_kvproj_fp8 {
 
 PCV_API int pcv_kv_project_fp8_supported(const pcv_kvproj_params* p, const pcv_kvproj_fp8* f);
 PCV_API int pcv_kv_project_fp8(const pcv_kvproj_params* p, const pcv_kvproj_fp8* f, void* stream);
+
+/*
+ * FP8 (e4m3) KV cache of cached generation: the three kernels below keep a cache's K and V rows as e4m3 codes
+ * (strides in elements = bytes) with scales that are not stored in the cache (the caller derives them from the
+ * weights).  k / v hold the codes of k_true[h, c] / k_descale[h] and v_true[h, c] / v_descale[h, c].
+ *
+ * pcv_attn_decode_fp8: the streaming decode kernel (PCV_IMPL_DECODE's) on an e4m3 cache.  `p` is a pcv_attn_params in
+ * which dtype (PCV_BF16 / PCV_F16) is that of q and out, and k / v are e4m3 rows whose strides are multiples of 16
+ * (16 channels per 16-byte load).  The result is pcv_attn_fwd's on (q, k8 * k_descale[h], v8 * v_descale[h, c]) with
+ * fp32 probabilities: k_descale is folded into the scaled q, v_descale multiplies the accumulator once.  Masks and
+ * batch-1 q as in pcv_attn_fwd.  N <= 4 query rows, any M >= 1, head dims multiples of 16 and at most 256; impl AUTO or
+ * DECODE.  It writes `out` only: write_partial and key shards (m_total != M or m_offset != 0) are refused.  The
+ * workspace is pcv_attn_decode_fp8_workspace_bytes() of the same params.  Arguments are checked before any CUDA call.
+ */
+typedef struct pcv_decode_fp8 {
+  const float* k_descale;  /* (H) f32                                                  */
+  const float* v_descale;  /* (H, dv) f32, dense                                       */
+} pcv_decode_fp8;
+
+PCV_API int pcv_attn_decode_fp8_supported(const pcv_attn_params* p, const pcv_decode_fp8* f);
+PCV_API int pcv_attn_decode_fp8_workspace_bytes(const pcv_attn_params* p, size_t* bytes);
+PCV_API int pcv_attn_decode_fp8(const pcv_attn_params* p, const pcv_decode_fp8* f, void* stream);
+
+/*
+ * pcv_kv_append_fp8: pcv_kv_append onto e4m3 caches.  p->dtype (PCV_BF16 / PCV_F16) is that of k_new / v_new; k_cache,
+ * v_cache, k_dst and v_dst are e4m3 (strides in bytes).  The old rows are copied byte for byte (skipped for a half
+ * whose cache pointer equals its dst pointer, as in pcv_kv_append); new row channel c becomes
+ * e4m3(x[c] * inv_scale[c]) (fp32 product, round to nearest even, saturating at +-448).  Ck and Cv multiples of 16,
+ * every pointer (the scales included) 16-byte aligned, e4m3 strides multiples of 16, new-row strides multiples of 8
+ * elements.  pcv_kv_append refuses e4m3.  Arguments are checked before any CUDA call.
+ */
+typedef struct pcv_kv_fp8_scales {
+  const float* k_inv_scale;  /* (Ck) f32: 1 / descale of every K channel               */
+  const float* v_inv_scale;  /* (Cv) f32                                               */
+} pcv_kv_fp8_scales;
+
+PCV_API int pcv_kv_append_fp8_supported(const pcv_kv_append_params* p, const pcv_kv_fp8_scales* f);
+PCV_API int pcv_kv_append_fp8(const pcv_kv_append_params* p, const pcv_kv_fp8_scales* f, void* stream);
+
+/*
+ * pcv_rotary_apply_fp8: pcv_rotary_apply with e4m3 output: y = e4m3(rotate(x)[h, c] * y_inv_scale[h]).  p->dtype is that
+ * of x: PCV_BF16 / PCV_F16, or PCV_E4M3 with x = codes * x_descale[h].  The rotation is computed in fp32 and rounded once.
+ * d and every stride even (a channel pair is one 16-bit store).  Arguments are checked before any CUDA call.
+ */
+typedef struct pcv_rotary_fp8 {
+  const float* x_descale;    /* (H) f32, read when p->dtype == PCV_E4M3, else may be NULL */
+  const float* y_inv_scale;  /* (H) f32                                                  */
+} pcv_rotary_fp8;
+
+PCV_API int pcv_rotary_fp8_supported(const pcv_rotary_params* p, const pcv_rotary_fp8* f);
+PCV_API int pcv_rotary_apply_fp8(const pcv_rotary_params* p, const pcv_rotary_fp8* f, void* stream);
 
 /*
  * Backward of the LayerNorm -> Linear chain pcv_kv_project computes (training through kv_norm -> k_proj / v_proj,

@@ -57,6 +57,13 @@ EXPORTS = (
     "pcv_attn_fwd_fp8",
     "pcv_kv_project_fp8_supported",
     "pcv_kv_project_fp8",
+    "pcv_attn_decode_fp8_supported",
+    "pcv_attn_decode_fp8_workspace_bytes",
+    "pcv_attn_decode_fp8",
+    "pcv_kv_append_fp8_supported",
+    "pcv_kv_append_fp8",
+    "pcv_rotary_fp8_supported",
+    "pcv_rotary_apply_fp8",
     "pcv_ln_linear_bwd_supported",
     "pcv_ln_linear_bwd_workspace_bytes",
     "pcv_ln_linear_bwd",
@@ -230,6 +237,18 @@ class KvProjFp8(C.Structure):
     ]
 
 
+class DecodeFp8(C.Structure):
+    _fields_ = [("k_descale", C.c_void_p), ("v_descale", C.c_void_p)]
+
+
+class KvFp8Scales(C.Structure):
+    _fields_ = [("k_inv_scale", C.c_void_p), ("v_inv_scale", C.c_void_p)]
+
+
+class RotaryFp8(C.Structure):
+    _fields_ = [("x_descale", C.c_void_p), ("y_inv_scale", C.c_void_p)]
+
+
 class LnLinearBwdParams(C.Structure):
     _fields_ = [
         ("x", C.c_void_p), ("x_stride_row", C.c_int64), ("row_stats", C.c_void_p),
@@ -343,6 +362,20 @@ def lib() -> C.CDLL:
         l.pcv_kv_project_fp8_supported.restype = C.c_int
         l.pcv_kv_project_fp8.argtypes = [C.POINTER(KvProjParams), C.POINTER(KvProjFp8), C.c_void_p]
         l.pcv_kv_project_fp8.restype = C.c_int
+        l.pcv_attn_decode_fp8_supported.argtypes = [C.POINTER(AttnParams), C.POINTER(DecodeFp8)]
+        l.pcv_attn_decode_fp8_supported.restype = C.c_int
+        l.pcv_attn_decode_fp8_workspace_bytes.argtypes = [C.POINTER(AttnParams), C.POINTER(C.c_size_t)]
+        l.pcv_attn_decode_fp8_workspace_bytes.restype = C.c_int
+        l.pcv_attn_decode_fp8.argtypes = [C.POINTER(AttnParams), C.POINTER(DecodeFp8), C.c_void_p]
+        l.pcv_attn_decode_fp8.restype = C.c_int
+        l.pcv_kv_append_fp8_supported.argtypes = [C.POINTER(KvAppendParams), C.POINTER(KvFp8Scales)]
+        l.pcv_kv_append_fp8_supported.restype = C.c_int
+        l.pcv_kv_append_fp8.argtypes = [C.POINTER(KvAppendParams), C.POINTER(KvFp8Scales), C.c_void_p]
+        l.pcv_kv_append_fp8.restype = C.c_int
+        l.pcv_rotary_fp8_supported.argtypes = [C.POINTER(RotaryParams), C.POINTER(RotaryFp8)]
+        l.pcv_rotary_fp8_supported.restype = C.c_int
+        l.pcv_rotary_apply_fp8.argtypes = [C.POINTER(RotaryParams), C.POINTER(RotaryFp8), C.c_void_p]
+        l.pcv_rotary_apply_fp8.restype = C.c_int
         l.pcv_ln_linear_bwd_supported.argtypes = [C.POINTER(LnLinearBwdParams)]
         l.pcv_ln_linear_bwd_supported.restype = C.c_int
         l.pcv_ln_linear_bwd_workspace_bytes.argtypes = [C.POINTER(LnLinearBwdParams), C.POINTER(C.c_size_t)]

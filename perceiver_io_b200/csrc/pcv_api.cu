@@ -438,4 +438,62 @@ int pcv_attn_fwd_fp8(const pcv_attn_params* p, const pcv_fp8_attn* f, void* stre
   return launch_attn_tc_fp8(*p, *f, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int pcv_attn_decode_fp8_supported(const pcv_attn_params* p, const pcv_decode_fp8* f) {
+  if (f == nullptr) {
+    set_error("attn_decode_fp8: fp8 params are NULL");
+    return 0;
+  }
+  if (validate_attn(p) != PCV_OK) return 0;
+  const char* why = "";
+  const bool ok = attn_decode_fp8_supported(*p, *f, &why);
+  if (!ok) set_error("e4m3 decode attention not applicable: %s", why);
+  return ok ? 1 : 0;
+}
+
+int pcv_attn_decode_fp8_workspace_bytes(const pcv_attn_params* p, size_t* bytes) {
+  int rc = validate_attn(p);
+  if (rc != PCV_OK) return rc;
+  PCV_REQUIRE(bytes != nullptr, PCV_ERR_INVALID, "attn_decode_fp8: bytes is NULL");
+  return attn_decode_workspace_bytes(*p, bytes);
+}
+
+int pcv_attn_decode_fp8(const pcv_attn_params* p, const pcv_decode_fp8* f, void* stream) {
+  PCV_REQUIRE(f != nullptr, PCV_ERR_INVALID, "attn_decode_fp8: fp8 params are NULL");
+  int rc = validate_attn(p);
+  if (rc != PCV_OK) return rc;
+  return launch_attn_decode_fp8(*p, *f, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pcv_kv_append_fp8_supported(const pcv_kv_append_params* p, const pcv_kv_fp8_scales* f) {
+  if (p == nullptr || f == nullptr) {
+    set_error("kv_append_fp8: params are NULL");
+    return 0;
+  }
+  const char* why = "";
+  const bool ok = kv_append_fp8_supported(*p, *f, &why);
+  if (!ok) set_error("kv_append_fp8 not applicable: %s", why);
+  return ok ? 1 : 0;
+}
+
+int pcv_kv_append_fp8(const pcv_kv_append_params* p, const pcv_kv_fp8_scales* f, void* stream) {
+  PCV_REQUIRE(p != nullptr && f != nullptr, PCV_ERR_INVALID, "kv_append_fp8: params are NULL");
+  return launch_kv_append_fp8(*p, *f, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pcv_rotary_fp8_supported(const pcv_rotary_params* p, const pcv_rotary_fp8* f) {
+  if (p == nullptr || f == nullptr) {
+    set_error("rotary_fp8: params are NULL");
+    return 0;
+  }
+  const char* why = "";
+  const bool ok = rotary_fp8_supported(*p, *f, &why);
+  if (!ok) set_error("rotary_fp8 not applicable: %s", why);
+  return ok ? 1 : 0;
+}
+
+int pcv_rotary_apply_fp8(const pcv_rotary_params* p, const pcv_rotary_fp8* f, void* stream) {
+  PCV_REQUIRE(p != nullptr && f != nullptr, PCV_ERR_INVALID, "rotary_fp8: params are NULL");
+  return launch_rotary_fp8(*p, *f, reinterpret_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"

@@ -16,9 +16,12 @@
 //   CTA of every (b, h) (atomic ticket) merges them and writes the normalised output or the partial state: one
 //   launch, no follow-up merge kernel (CUDA-graph friendly).
 // Masks follow include/pcv_attn.h: finite fill for padding / causal keys (a fully masked row is the uniform average).
+// The e4m3 variant (attn_decode_fp8_kernel, pcv_attn_decode_fp8) reads an FP8 KV cache through the same body: a 16-byte
+// load carries 16 channels, so it moves half the bytes per key.
 #include "pcv_common.cuh"
 
 #include <algorithm>
+#include <type_traits>
 
 namespace pcv {
 namespace {
@@ -52,10 +55,24 @@ __device__ __forceinline__ void unpack8(const uint4& u, float (&f)[8]) {
   }
 }
 
+// One 16-byte chunk of a K / V row -> floats: 8 bf16 / fp16 channels, or 16 e4m3 channels (FP8)
+template <typename T, bool FP8>
+__device__ __forceinline__ void unpack_chunk(const uint4& u, float (&f)[FP8 ? 16 : 8]) {
+  if constexpr (FP8)
+    unpack16_e4m3(u, f);
+  else
+    unpack8<T>(u, f);
+}
+
+// The kernel body.  FP8: K / V are e4m3 rows (a 16-byte chunk carries 16 channels), k_descale[h] is folded into the
+// scaled q and v_descale[h, c] multiplies the accumulator once, before the merge; everything else is shared.
 // LPK lanes share one key; NQ query rows
-template <typename T, int LPK, int NQ>
-__global__ void __launch_bounds__(kDecThreads) attn_decode_kernel(const DecParams p) {
-  constexpr int kUnroll = Unroll<NQ>::value;
+template <typename T, int LPK, int NQ, bool FP8>
+__device__ __forceinline__ void attn_decode_body(const DecParams& p, const pcv_decode_fp8& f8) {
+  constexpr int CH = FP8 ? 16 : 8;        // channels per 16-byte chunk of a K / V row
+  using KV = typename std::conditional<FP8, uint8_t, T>::type;
+  // e4m3 rows hold twice the channels per register: four query rows take half the unroll to stay out of local memory
+  constexpr int kUnroll = (FP8 && NQ > 1) ? 2 : Unroll<NQ>::value;
   constexpr int KPW = 32 / LPK;           // keys per warp step
   constexpr int KPB = KPW * kUnroll;      // keys per warp block
   const pcv_attn_params& a = p.a;
@@ -69,33 +86,46 @@ __global__ void __launch_bounds__(kDecThreads) attn_decode_kernel(const DecParam
   const int bh = b * a.H + h;
   const int kb = split * p.keys_per_split;
   const int ke = min(a.M, kb + p.keys_per_split);
-  const int c0 = sub * 8;
+  const int c0 = sub * CH;
   const bool kq_live = c0 < a.dqk, v_live = c0 < a.dv;
 
   const T* qp = reinterpret_cast<const T*>(a.q) + (a.q_stride_b ? (int64_t)b * a.q_stride_b : 0) + (int64_t)h * a.q_stride_h + c0;
-  const T* kp = reinterpret_cast<const T*>(a.k) + (int64_t)b * a.k_stride_b + (int64_t)h * a.k_stride_h + c0;
-  const T* vp = reinterpret_cast<const T*>(a.v) + (int64_t)b * a.v_stride_b + (int64_t)h * a.v_stride_h + c0;
+  const KV* kp = reinterpret_cast<const KV*>(a.k) + (int64_t)b * a.k_stride_b + (int64_t)h * a.k_stride_h + c0;
+  const KV* vp = reinterpret_cast<const KV*>(a.v) + (int64_t)b * a.v_stride_b + (int64_t)h * a.v_stride_h + c0;
   const uint8_t* pad = a.pad_mask ? a.pad_mask + (int64_t)b * a.pad_stride_b : nullptr;
 
   const float scale_log2 = a.scale * kLog2e;
-  float q[NQ][8];
+  float q[NQ][CH];
 #pragma unroll
   for (int i = 0; i < NQ; ++i) {
-    uint4 u = make_uint4(0, 0, 0, 0);
-    if (kq_live && i < a.N) u = *reinterpret_cast<const uint4*>(qp + (int64_t)i * a.q_stride_n);
-    unpack8<T>(u, q[i]);
+    if constexpr (FP8) {
+      const float qs = scale_log2 * f8.k_descale[h];  // scores of the dequantised keys, in the log2 domain
 #pragma unroll
-    for (int c = 0; c < 8; ++c) q[i][c] *= scale_log2;   // scores come out in the log2 domain
+      for (int half = 0; half < 2; ++half) {
+        uint4 u = make_uint4(0, 0, 0, 0);
+        if (kq_live && i < a.N) u = *reinterpret_cast<const uint4*>(qp + (int64_t)i * a.q_stride_n + 8 * half);
+        float x[8];
+        unpack8<T>(u, x);
+#pragma unroll
+        for (int c = 0; c < 8; ++c) q[i][8 * half + c] = x[c] * qs;
+      }
+    } else {
+      uint4 u = make_uint4(0, 0, 0, 0);
+      if (kq_live && i < a.N) u = *reinterpret_cast<const uint4*>(qp + (int64_t)i * a.q_stride_n);
+      unpack8<T>(u, q[i]);
+#pragma unroll
+      for (int c = 0; c < 8; ++c) q[i][c] *= scale_log2;   // scores come out in the log2 domain
+    }
   }
   const int causal_shift = a.m_total - a.N;  // key jg masked for query n iff jg > n + causal_shift
 
-  float m[NQ], l[NQ], acc[NQ][8];
+  float m[NQ], l[NQ], acc[NQ][CH];
 #pragma unroll
   for (int i = 0; i < NQ; ++i) {
     m[i] = -INFINITY;
     l[i] = 0.f;
 #pragma unroll
-    for (int c = 0; c < 8; ++c) acc[i][c] = 0.f;
+    for (int c = 0; c < CH; ++c) acc[i][c] = 0.f;
   }
 
   // keys of this CTA are dealt to the warps in blocks of KPB keys: warp w takes blocks w, w + kDecWarps, ...
@@ -121,14 +151,14 @@ __global__ void __launch_bounds__(kDecThreads) attn_decode_kernel(const DecParam
     float s[NQ][kUnroll];
 #pragma unroll
     for (int u = 0; u < kUnroll; ++u) {
-      float kf[8];
-      unpack8<T>(ku[buf][u], kf);
+      float kf[CH];
+      unpack_chunk<T, FP8>(ku[buf][u], kf);
       const int j = j0 + u * KPW + grp;
 #pragma unroll
       for (int i = 0; i < NQ; ++i) {
         float d = 0.f;
 #pragma unroll
-        for (int c = 0; c < 8; ++c) d = fmaf(q[i][c], kf[c], d);
+        for (int c = 0; c < CH; ++c) d = fmaf(q[i][c], kf[c], d);
 #pragma unroll
         for (int o = LPK / 2; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
         if (masked[buf][u] || (a.causal && a.m_offset + j > i + causal_shift)) d = kMaskedScore;
@@ -147,15 +177,15 @@ __global__ void __launch_bounds__(kDecThreads) attn_decode_kernel(const DecParam
       m[i] = m_new;
       l[i] *= alpha;
 #pragma unroll
-      for (int c = 0; c < 8; ++c) acc[i][c] *= alpha;
+      for (int c = 0; c < CH; ++c) acc[i][c] *= alpha;
 #pragma unroll
       for (int u = 0; u < kUnroll; ++u) {
         const float pe = exp2f(s[i][u] - m_new);
         l[i] += pe;
-        float vf[8];
-        unpack8<T>(vu[buf][u], vf);
+        float vf[CH];
+        unpack_chunk<T, FP8>(vu[buf][u], vf);
 #pragma unroll
-        for (int c = 0; c < 8; ++c) acc[i][c] = fmaf(pe, vf[c], acc[i][c]);
+        for (int c = 0; c < CH; ++c) acc[i][c] = fmaf(pe, vf[c], acc[i][c]);
       }
     }
   };
@@ -173,10 +203,20 @@ __global__ void __launch_bounds__(kDecThreads) attn_decode_kernel(const DecParam
       j0 += kStride;
     }
   }
+  if constexpr (FP8) {  // the V dequantisation factors of this lane's channels
+    if (v_live) {
+#pragma unroll
+      for (int c = 0; c < CH; ++c) {
+        const float vd = f8.v_descale[(int64_t)h * a.dv + c0 + c];
+#pragma unroll
+        for (int i = 0; i < NQ; ++i) acc[i][c] *= vd;
+      }
+    }
+  }
 
   // ---- merge: lane groups of a warp -> warps of the CTA (shared memory) -----------------------------------
   __shared__ float sm_m[kDecWarps][NQ], sm_l[kDecWarps][NQ];
-  __shared__ float sm_o[kDecWarps][NQ][LPK * 8];
+  __shared__ float sm_o[kDecWarps][NQ][LPK * CH];
 #pragma unroll
   for (int i = 0; i < NQ; ++i) {
     // groups: lanes with equal `sub` hold the same channels for different keys
@@ -189,7 +229,7 @@ __global__ void __launch_bounds__(kDecThreads) attn_decode_kernel(const DecParam
       const float wb = (m_o == -INFINITY) ? 0.f : exp2f(m_o - m_new);
       l[i] = l[i] * wa + l_o * wb;
 #pragma unroll
-      for (int c = 0; c < 8; ++c) {
+      for (int c = 0; c < CH; ++c) {
         const float a_o = __shfl_xor_sync(0xffffffffu, acc[i][c], o);
         acc[i][c] = acc[i][c] * wa + a_o * wb;
       }
@@ -201,12 +241,12 @@ __global__ void __launch_bounds__(kDecThreads) attn_decode_kernel(const DecParam
         sm_l[warp][i] = l[i];
       }
 #pragma unroll
-      for (int c = 0; c < 8; ++c) sm_o[warp][i][c0 + c] = acc[i][c];
+      for (int c = 0; c < CH; ++c) sm_o[warp][i][c0 + c] = acc[i][c];
     }
   }
   __syncthreads();
 
-  const int dvp = LPK * 8;
+  const int dvp = LPK * CH;
   // CTA state -> workspace: thread t handles (query i, channel c)
   const int64_t wbase = ((int64_t)bh * p.nsplit + split) * NQ;
   for (int idx = threadIdx.x; idx < NQ * dvp; idx += kDecThreads) {
@@ -267,6 +307,17 @@ __global__ void __launch_bounds__(kDecThreads) attn_decode_kernel(const DecParam
   }
 }
 
+template <typename T, int LPK, int NQ>
+__global__ void __launch_bounds__(kDecThreads) attn_decode_kernel(const DecParams p) {
+  attn_decode_body<T, LPK, NQ, false>(p, pcv_decode_fp8{});
+}
+
+// e4m3 K / V rows (pcv_attn_decode_fp8)
+template <typename T, int LPK, int NQ>
+__global__ void __launch_bounds__(kDecThreads) attn_decode_fp8_kernel(const DecParams p, const pcv_decode_fp8 f8) {
+  attn_decode_body<T, LPK, NQ, true>(p, f8);
+}
+
 int choose_split(const pcv_attn_params& a, int* nsplit, int* keys_per_split) {
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
@@ -317,6 +368,29 @@ int lanes_per_key(const pcv_attn_params& a) {
   return lpk;
 }
 
+template <typename T, int LPK>
+int launch_nq_fp8(const DecParams& p, const pcv_decode_fp8& f, cudaStream_t stream) {
+  dim3 grid((unsigned)((int64_t)p.nsplit * p.a.B * p.a.H));
+  if (p.a.N == 1)
+    attn_decode_fp8_kernel<T, LPK, 1><<<grid, kDecThreads, 0, stream>>>(p, f);
+  else
+    attn_decode_fp8_kernel<T, LPK, 4><<<grid, kDecThreads, 0, stream>>>(p, f);
+  PCV_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return PCV_OK;
+}
+
+template <typename T>
+int launch_lpk_fp8(const DecParams& p, const pcv_decode_fp8& f, int lpk, cudaStream_t stream) {
+  switch (lpk) {  // rows of up to 64 channels use the 4-lane instantiation with idle lanes
+    case 1:
+    case 2:
+    case 4: return launch_nq_fp8<T, 4>(p, f, stream);
+    case 8: return launch_nq_fp8<T, 8>(p, f, stream);
+    default: return launch_nq_fp8<T, 16>(p, f, stream);
+  }
+}
+
 }  // namespace
 
 bool attn_decode_supported(const pcv_attn_params& a, const char** why) {
@@ -345,29 +419,75 @@ int attn_decode_workspace_bytes(const pcv_attn_params& a, size_t* bytes) {
   return PCV_OK;
 }
 
-int launch_attn_decode(const pcv_attn_params& a, cudaStream_t stream) {
+// Checks the workspace, fills the kernel params and zeroes the tickets.
+static int decode_setup(const pcv_attn_params& a, DecParams* p, cudaStream_t stream) {
   size_t need = 0;
   attn_decode_workspace_bytes(a, &need);
   PCV_REQUIRE(a.workspace != nullptr && a.workspace_bytes >= need, PCV_ERR_WORKSPACE,
               "decode attention: workspace of %zu bytes required, %zu given", need, a.workspace_bytes);
-  DecParams p{};
-  p.a = a;
-  choose_split(a, &p.nsplit, &p.keys_per_split);
+  *p = DecParams{};
+  p->a = a;
+  choose_split(a, &p->nsplit, &p->keys_per_split);
   const int nq = a.N <= 1 ? 1 : 4;
-  const size_t rows = (size_t)a.B * a.H * p.nsplit * nq;
+  const size_t rows = (size_t)a.B * a.H * p->nsplit * nq;
   char* ws = reinterpret_cast<char*>(a.workspace);
-  p.ws_o = reinterpret_cast<float*>(ws);
+  p->ws_o = reinterpret_cast<float*>(ws);
   ws += align256(rows * a.dv * 4);
-  p.ws_m = reinterpret_cast<float*>(ws);
+  p->ws_m = reinterpret_cast<float*>(ws);
   ws += align256(rows * 4);
-  p.ws_l = reinterpret_cast<float*>(ws);
+  p->ws_l = reinterpret_cast<float*>(ws);
   ws += align256(rows * 4);
-  p.tickets = reinterpret_cast<unsigned int*>(ws);
+  p->tickets = reinterpret_cast<unsigned int*>(ws);
   // the workspace is caller memory with arbitrary contents: the tickets must start at zero
-  PCV_CHECK_CUDA(cudaMemsetAsync(p.tickets, 0, (size_t)a.B * a.H * 4, stream));
+  PCV_CHECK_CUDA(cudaMemsetAsync(p->tickets, 0, (size_t)a.B * a.H * 4, stream));
+  return PCV_OK;
+}
+
+int launch_attn_decode(const pcv_attn_params& a, cudaStream_t stream) {
+  DecParams p;
+  const int rc0 = decode_setup(a, &p, stream);
+  if (rc0 != PCV_OK) return rc0;
   const int lpk = lanes_per_key(a);
   prof_mark_begin(stream);
   const int rc = a.dtype == PCV_BF16 ? launch_lpk<__nv_bfloat16>(p, lpk, stream) : launch_lpk<__half>(p, lpk, stream);
+  prof_mark_end(stream);
+  return rc;
+}
+
+bool attn_decode_fp8_supported(const pcv_attn_params& a, const pcv_decode_fp8& f, const char** why) {
+  auto fail = [&](const char* w) {
+    *why = w;
+    return false;
+  };
+  if (a.dtype != PCV_BF16 && a.dtype != PCV_F16) return fail("dtype (of q and out) must be bf16 or fp16");
+  if (a.impl != PCV_IMPL_AUTO && a.impl != PCV_IMPL_DECODE) return fail("impl must be AUTO or DECODE");
+  if (a.N > kMaxQ) return fail("more than 4 query rows");
+  if (a.dqk > 256 || a.dv > 256) return fail("head dim > 256");
+  if ((a.dqk % 16) || (a.dv % 16)) return fail("head dims must be multiples of 16");
+  if (a.write_partial) return fail("the e4m3 decode writes the normalised output only (no write_partial)");
+  if (a.m_total != a.M || a.m_offset != 0) return fail("the e4m3 decode takes no key shard (m_total != M or m_offset != 0)");
+  if (f.k_descale == nullptr || f.v_descale == nullptr) return fail("k_descale / v_descale are NULL");
+  auto al16 = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
+  if (!al16(a.q) || !al16(a.k) || !al16(a.v)) return fail("q/k/v must be 16-byte aligned");
+  if ((a.q_stride_n % 8) || (a.q_stride_h % 8) || (a.q_stride_b % 8))
+    return fail("q strides must be multiples of 8 elements");
+  if ((a.k_stride_m % 16) || (a.v_stride_m % 16) || (a.k_stride_h % 16) || (a.v_stride_h % 16) || (a.k_stride_b % 16) ||
+      (a.v_stride_b % 16))
+    return fail("e4m3 k/v strides must be multiples of 16 elements");
+  return true;
+}
+
+int launch_attn_decode_fp8(const pcv_attn_params& a, const pcv_decode_fp8& f, cudaStream_t stream) {
+  const char* why = "";
+  PCV_REQUIRE(attn_decode_fp8_supported(a, f, &why), PCV_ERR_UNSUPPORTED, "e4m3 decode attention: %s", why);
+  DecParams p;
+  const int rc0 = decode_setup(a, &p, stream);
+  if (rc0 != PCV_OK) return rc0;
+  int lpk = 1;  // 16 channels per 16-byte chunk
+  while (lpk * 16 < std::max(a.dqk, a.dv)) lpk <<= 1;
+  prof_mark_begin(stream);
+  const int rc = a.dtype == PCV_BF16 ? launch_lpk_fp8<__nv_bfloat16>(p, f, lpk, stream)
+                                     : launch_lpk_fp8<__half>(p, f, lpk, stream);
   prof_mark_end(stream);
   return rc;
 }

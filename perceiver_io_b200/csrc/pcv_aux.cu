@@ -8,6 +8,7 @@
 #include "pcv_common.cuh"
 
 #include <algorithm>
+#include <type_traits>
 
 namespace pcv {
 namespace {
@@ -269,6 +270,97 @@ __global__ void __launch_bounds__(256) kv_append_kernel(const CopyArgs a) {
   }
 }
 
+// ---------------------------------------------------------------------------------------------
+// kv_append_fp8: kv_append onto e4m3 caches.  blockIdx.y as in kv_append; every thread moves 16 channels: segments 0 / 2
+// copy 16 bytes of old e4m3 rows, segments 1 / 3 read 16 bf16 / fp16 channels of a new row, multiply them by the
+// channels' inverse scales and round them to e4m3 (row_bytes = channels = e4m3 bytes of a row in every segment).
+// ---------------------------------------------------------------------------------------------
+struct QuantArgs {
+  CopySeg seg[4];        // byte strides; the new rows' source strides are those of their 16-bit elements
+  const float* inv[4];   // [1] / [3]: per-channel inverse scales of the new K / V rows
+  int B;
+};
+
+template <typename T>
+__global__ void __launch_bounds__(256) kv_append_fp8_kernel(const QuantArgs a) {
+  const CopySeg s = a.seg[blockIdx.y];
+  if (s.rows == 0 || s.src == nullptr) return;
+  const bool quant = blockIdx.y & 1;
+  const float* inv = a.inv[blockIdx.y];
+  const int vpr = s.row_bytes >> 4;
+  const int64_t total = (int64_t)a.B * s.rows * vpr;
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int w = (int)(idx % vpr);
+    const int64_t rr = idx / vpr;
+    const int row = (int)(rr % s.rows);
+    const int b = (int)(rr / s.rows);
+    const char* src = s.src + b * s.s_sb + row * s.s_sl;
+    int4* dst = reinterpret_cast<int4*>(s.dst + b * s.d_sb + (int64_t)(s.dst_row0 + row) * s.d_sl + ((int64_t)w << 4));
+    if (!quant) {
+      *dst = *reinterpret_cast<const int4*>(src + ((int64_t)w << 4));
+      continue;
+    }
+    const uint4* x = reinterpret_cast<const uint4*>(src + ((int64_t)w << 5));
+    const uint4 u[2] = {x[0], x[1]};
+    const float4* iv = reinterpret_cast<const float4*>(inv + 16 * w);
+    uint32_t packed[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {  // channels 4k .. 4k + 3
+      const typename Elem<T>::T2* h = reinterpret_cast<const typename Elem<T>::T2*>(&u[k >> 1]) + 2 * (k & 1);
+      const float2 lo = Elem<T>::to_f2(h[0]), hi = Elem<T>::to_f2(h[1]);
+      const float4 sc = iv[k];
+      packed[k] = cvt_e4m3x2(lo.x * sc.x, lo.y * sc.y) | (cvt_e4m3x2(hi.x * sc.z, hi.y * sc.w) << 16);
+    }
+    *dst = make_int4((int)packed[0], (int)packed[1], (int)packed[2], (int)packed[3]);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
+// rotary_fp8: rotary with e4m3 output, one thread per channel pair (one 16-bit store).  T is the input: bf16 / fp16,
+// or uint8_t for e4m3 codes dequantised with x_descale[h].  The pair is rotated in fp32 and rounded once.
+// ---------------------------------------------------------------------------------------------
+template <typename T>
+__global__ void __launch_bounds__(256) rotary_fp8_kernel(const pcv_rotary_params p, const pcv_rotary_fp8 f) {
+  const int d2 = p.d >> 1;
+  const int64_t total = (int64_t)p.B * p.n * p.H * d2;
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
+       idx += (int64_t)gridDim.x * blockDim.x) {
+    const int pr = (int)(idx % d2);
+    int64_t rest = idx / d2;
+    const int h = (int)(rest % p.H);
+    rest /= p.H;
+    const int i = (int)(rest % p.n);
+    const int b = (int)(rest / p.n);
+    const int c = 2 * pr;
+    const T* x = reinterpret_cast<const T*>(p.x) + (int64_t)b * p.x_stride_b + (int64_t)i * p.x_stride_n +
+                 (int64_t)h * p.x_stride_h;
+    uint8_t* y = reinterpret_cast<uint8_t*>(p.y) + (int64_t)b * p.y_stride_b + (int64_t)i * p.y_stride_n +
+                 (int64_t)h * p.y_stride_h;
+    float x0, x1;
+    if constexpr (std::is_same<T, uint8_t>::value) {
+      const float2 v = e4m3x2_to_f2(*reinterpret_cast<const uint16_t*>(x + c));
+      const float ds = f.x_descale[h];
+      x0 = v.x * ds;
+      x1 = v.y * ds;
+    } else {
+      x0 = Elem<T>::to_f(x[c]);
+      x1 = Elem<T>::to_f(x[c + 1]);
+    }
+    float y0 = x0, y1 = x1;
+    if (c + 1 < p.rotate_dim) {
+      const float* a = p.angles + (p.a_stride_b ? (int64_t)b * p.a_stride_b : 0) +
+                       (int64_t)(p.angle_row0 + i) * p.a_stride_n;
+      float s0, c0, s1, c1;
+      sincosf(a[c], &s0, &c0);
+      sincosf(a[c + 1], &s1, &c1);
+      y0 = x0 * c0 - x1 * s0;
+      y1 = x1 * c1 + x0 * s1;
+    }
+    const float inv = f.y_inv_scale[h];
+    *reinterpret_cast<uint16_t*>(y + c) = (uint16_t)cvt_e4m3x2(y0 * inv, y1 * inv);
+  }
+}
+
 // pad_mask bytes (B, M) -> bit words (B, wpr), wpr = pad_words_per_row(M); bit set = padding key
 __global__ void __launch_bounds__(256) pack_pad_kernel(const uint8_t* __restrict__ pad, int64_t stride_b, int B, int M,
                                                        int wpr, uint32_t* __restrict__ bits) {
@@ -415,6 +507,100 @@ int launch_kv_append(const pcv_kv_append_params& p, cudaStream_t stream) {
   if (blocks > 132 * 8) blocks = 132 * 8;
   dim3 grid((unsigned)blocks, 4, 1);
   kv_append_kernel<<<grid, 256, 0, stream>>>(a);
+  PCV_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return PCV_OK;
+}
+
+bool kv_append_fp8_supported(const pcv_kv_append_params& p, const pcv_kv_fp8_scales& f, const char** why) {
+  auto fail = [&](const char* w) {
+    *why = w;
+    return false;
+  };
+  if (!p.k_dst || !p.v_dst || (p.n > 0 && (!p.k_new || !p.v_new))) return fail("null pointer argument");
+  if (f.k_inv_scale == nullptr || f.v_inv_scale == nullptr) return fail("k_inv_scale / v_inv_scale are NULL");
+  if (p.B < 1 || p.L_old < 0 || p.n < 0 || p.Ck < 1 || p.Cv < 1) return fail("bad dimension");
+  if (p.L_old > 0 && (!p.k_cache || !p.v_cache)) return fail("cache pointers required");
+  if (p.dtype != PCV_BF16 && p.dtype != PCV_F16) return fail("the new rows must be bf16 or fp16");
+  if ((p.Ck % 16) || (p.Cv % 16)) return fail("Ck and Cv must be multiples of 16");
+  const void* ptrs[] = {p.k_cache, p.v_cache, p.k_new, p.v_new, p.k_dst, p.v_dst, f.k_inv_scale, f.v_inv_scale};
+  for (const void* ptr : ptrs)
+    if (!al16(ptr)) return fail("pointers must be 16-byte aligned");
+  if ((p.kc_stride_b | p.kc_stride_l | p.vc_stride_b | p.vc_stride_l | p.kd_stride_b | p.kd_stride_l | p.vd_stride_b |
+       p.vd_stride_l) & 15)
+    return fail("e4m3 strides must be multiples of 16 bytes");
+  if ((p.kn_stride_b | p.kn_stride_l | p.vn_stride_b | p.vn_stride_l) & 7)
+    return fail("new-row strides must be multiples of 8 elements");
+  return true;
+}
+
+int launch_kv_append_fp8(const pcv_kv_append_params& p, const pcv_kv_fp8_scales& f, cudaStream_t stream) {
+  const char* why = "";
+  PCV_REQUIRE(kv_append_fp8_supported(p, f, &why), PCV_ERR_INVALID, "kv_append_fp8: %s", why);
+  QuantArgs a;
+  a.B = p.B;
+  auto seg = [&](const void* src, void* dst, int64_t ssb, int64_t ssl, int64_t dsb, int64_t dsl, int rows, int C,
+                 int row0, int src_es) {
+    CopySeg s;
+    s.src = reinterpret_cast<const char*>(src);
+    s.dst = reinterpret_cast<char*>(dst);
+    s.s_sb = ssb * src_es; s.s_sl = ssl * src_es; s.d_sb = dsb; s.d_sl = dsl;
+    s.rows = rows; s.row_bytes = C; s.dst_row0 = row0;
+    if (src == dst && row0 == 0) s.rows = 0;  // in-place arena: the old rows are already there
+    return s;
+  };
+  a.seg[0] = seg(p.k_cache, p.k_dst, p.kc_stride_b, p.kc_stride_l, p.kd_stride_b, p.kd_stride_l, p.L_old, p.Ck, 0, 1);
+  a.seg[1] = seg(p.k_new, p.k_dst, p.kn_stride_b, p.kn_stride_l, p.kd_stride_b, p.kd_stride_l, p.n, p.Ck, p.L_old, 2);
+  a.seg[2] = seg(p.v_cache, p.v_dst, p.vc_stride_b, p.vc_stride_l, p.vd_stride_b, p.vd_stride_l, p.L_old, p.Cv, 0, 1);
+  a.seg[3] = seg(p.v_new, p.v_dst, p.vn_stride_b, p.vn_stride_l, p.vd_stride_b, p.vd_stride_l, p.n, p.Cv, p.L_old, 2);
+  a.inv[0] = a.inv[2] = nullptr;
+  a.inv[1] = f.k_inv_scale;
+  a.inv[3] = f.v_inv_scale;
+  int64_t maxwork = 1;
+  for (int i = 0; i < 4; ++i) maxwork = std::max<int64_t>(maxwork, (int64_t)p.B * a.seg[i].rows * (a.seg[i].row_bytes >> 4));
+  const int64_t blocks = std::min<int64_t>((maxwork + 255) / 256, 132 * 8);
+  dim3 grid((unsigned)blocks, 4, 1);
+  if (p.dtype == PCV_BF16)
+    kv_append_fp8_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(a);
+  else
+    kv_append_fp8_kernel<__half><<<grid, 256, 0, stream>>>(a);
+  PCV_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return PCV_OK;
+}
+
+bool rotary_fp8_supported(const pcv_rotary_params& p, const pcv_rotary_fp8& f, const char** why) {
+  auto fail = [&](const char* w) {
+    *why = w;
+    return false;
+  };
+  if (!p.x || !p.y || !p.angles) return fail("null pointer argument");
+  if (f.y_inv_scale == nullptr) return fail("y_inv_scale is NULL");
+  if (p.dtype != PCV_BF16 && p.dtype != PCV_F16 && p.dtype != PCV_E4M3) return fail("x must be bf16, fp16 or e4m3");
+  if (p.dtype == PCV_E4M3 && f.x_descale == nullptr) return fail("e4m3 input needs x_descale");
+  if (p.B < 1 || p.n < 0 || p.H < 1 || p.d < 2) return fail("bad dimension");
+  if (p.d % 2) return fail("d must be even");
+  if (p.rotate_dim < 0 || p.rotate_dim > p.d || (p.rotate_dim % 2)) return fail("rotate_dim must be even and <= d");
+  if (p.angle_row0 < 0) return fail("negative angle_row0");
+  if ((p.x_stride_b | p.x_stride_n | p.x_stride_h | p.y_stride_b | p.y_stride_n | p.y_stride_h) & 1)
+    return fail("strides must be even");
+  if ((reinterpret_cast<uintptr_t>(p.y) & 1) || (p.dtype == PCV_E4M3 && (reinterpret_cast<uintptr_t>(p.x) & 1)))
+    return fail("e4m3 pointers must be 2-byte aligned");
+  return true;
+}
+
+int launch_rotary_fp8(const pcv_rotary_params& p, const pcv_rotary_fp8& f, cudaStream_t stream) {
+  const char* why = "";
+  PCV_REQUIRE(rotary_fp8_supported(p, f, &why), PCV_ERR_INVALID, "rotary_fp8: %s", why);
+  if (p.n == 0) return PCV_OK;
+  const int64_t total = (int64_t)p.B * p.n * p.H * (p.d / 2);
+  const int64_t blocks = std::min<int64_t>((total + 255) / 256, 132 * 16);
+  if (p.dtype == PCV_BF16)
+    rotary_fp8_kernel<__nv_bfloat16><<<(unsigned)blocks, 256, 0, stream>>>(p, f);
+  else if (p.dtype == PCV_F16)
+    rotary_fp8_kernel<__half><<<(unsigned)blocks, 256, 0, stream>>>(p, f);
+  else
+    rotary_fp8_kernel<uint8_t><<<(unsigned)blocks, 256, 0, stream>>>(p, f);
   PCV_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PCV_OK;

@@ -63,6 +63,30 @@ template <> struct Elem<float> {  // fp32 outputs (a key shard's grad_q contribu
   static __device__ __forceinline__ float from_f(float x) { return x; }
 };
 
+// ---- e4m3 ------------------------------------------------------------------------------------
+// two floats -> two e4m3 bytes (round to nearest even, saturating at +-448), `lo` in the low byte
+__device__ __forceinline__ uint32_t cvt_e4m3x2(float lo, float hi) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+// two e4m3 bytes (low byte first) -> two floats; exact (every e4m3 value is an f16 value)
+__device__ __forceinline__ float2 e4m3x2_to_f2(uint16_t x) {
+  uint32_t h;
+  asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h) : "h"(x));
+  return __half22float2(*reinterpret_cast<const __half2*>(&h));
+}
+// 16 e4m3 bytes -> 16 floats
+__device__ __forceinline__ void unpack16_e4m3(const uint4& u, float (&f)[16]) {
+  const uint16_t* b = reinterpret_cast<const uint16_t*>(&u);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const float2 x = e4m3x2_to_f2(b[i]);
+    f[2 * i] = x.x;
+    f[2 * i + 1] = x.y;
+  }
+}
+
 __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
@@ -102,6 +126,9 @@ int debug_plan(int B, int H, int N, int M, int workers, int rows_per_unit, int r
 bool attn_decode_supported(const pcv_attn_params& p, const char** why);
 int launch_attn_decode(const pcv_attn_params& p, cudaStream_t stream);
 int attn_decode_workspace_bytes(const pcv_attn_params& p, size_t* bytes);
+// the e4m3-cache decode (attn_decode_kernel with e4m3 K / V rows); workspace as attn_decode_workspace_bytes
+bool attn_decode_fp8_supported(const pcv_attn_params& p, const pcv_decode_fp8& f, const char** why);
+int launch_attn_decode_fp8(const pcv_attn_params& p, const pcv_decode_fp8& f, cudaStream_t stream);
 
 int launch_combine(const pcv_combine_params& p, cudaStream_t stream);
 // Merge `nparts` partial states laid out [part][B][H][N]([dv]) either into p.out (normalised) or,
@@ -113,6 +140,10 @@ int launch_merge_partials(const pcv_merge_params& p, cudaStream_t stream);
 int launch_rescale(const pcv_rescale_params& p, cudaStream_t stream);
 int launch_rotary(const pcv_rotary_params& p, cudaStream_t stream);
 int launch_kv_append(const pcv_kv_append_params& p, cudaStream_t stream);
+bool kv_append_fp8_supported(const pcv_kv_append_params& p, const pcv_kv_fp8_scales& f, const char** why);
+int launch_kv_append_fp8(const pcv_kv_append_params& p, const pcv_kv_fp8_scales& f, cudaStream_t stream);
+bool rotary_fp8_supported(const pcv_rotary_params& p, const pcv_rotary_fp8& f, const char** why);
+int launch_rotary_fp8(const pcv_rotary_params& p, const pcv_rotary_fp8& f, cudaStream_t stream);
 int launch_ln_stats(const pcv_ln_stats_params& p, cudaStream_t stream);
 bool kv_project_supported(const pcv_kvproj_params& p, const char** why);
 int launch_kv_project(const pcv_kvproj_params& p, cudaStream_t stream);

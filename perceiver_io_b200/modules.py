@@ -23,7 +23,7 @@ Inputs must be CUDA tensors; there is no CPU implementation in this package.
 """
 from __future__ import annotations
 
-from typing import List, Optional, Tuple
+from typing import List, NamedTuple, Optional, Tuple
 
 import torch
 from torch import nn
@@ -109,10 +109,12 @@ class MultiHeadAttention(nn.Module):
 
 
 def attend(mha, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, pad_mask=None, rot_pos_emb_q=None,
-           rot_pos_emb_k=None, kv_cache: Optional[KVCache] = None, min_rows_key: str = "min_rows"):
+           rot_pos_emb_k=None, kv_cache: Optional[KVCache] = None, min_rows_key: str = "min_rows", kv8=None):
     """Everything of ``MultiHeadAttention.forward`` after the q/k/v projections (reference modules.py:117-170):
     cache append, rotary, fused attention, ``o_proj``.  ``mha`` is this package's module or a patched reference
-    one (only its attributes are used)."""
+    one (only its attributes are used).  ``kv8``: the scales of an FP8 KV cache (``_kv8_route``)."""
+    if kv8 is not None:
+        return _attend_kv8(mha, q, k, v, pad_mask, rot_pos_emb_q, rot_pos_emb_k, kv_cache, min_rows_key, kv8)
     # attention-probability dropout (reference :161): fused into the training kernels (ops.attention dropout_p)
     drop_p = float(mha.dropout.p) if mha.training else 0.0
     if kv_cache is not None:
@@ -136,6 +138,47 @@ def attend(mha, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, pad_mask=None
                       causal=mha.causal_attention, impl=getattr(mha, "kernel_impl", "auto"), dropout_p=drop_p)
     o = fused_linear(mha, "_pcv_o_fold", None, mha.o_proj, o, min_rows_key)
     return ModuleOutput(last_hidden_state=o, kv_cache=kv_cache)
+
+
+def _attend_kv8(mha, q, k, v, pad_mask, rot_pos_emb_q, rot_pos_emb_k, kv_cache, min_rows_key, kv8):
+    """``attend`` with an FP8 (e4m3) KV cache: the new rows are quantised into the cache (ops.kv_append_fp8).  An empty
+    incoming cache (the prompt) attends over this call's own bf16 / fp16 rows.  A cached step takes its rotated keys
+    from the e4m3 shadow (ops.rotated_cache_keys) when the rotary object carries the frequency table (``inv_freq``, as
+    this package's models pass it); without one (the reference's RotaryPositionEmbedding) the whole cache is rotated at
+    the window-relative angles, e4m3 to e4m3 (ops.rotary_fp8), as the reference rotates it every step.  With at most 4
+    query rows the e4m3 decode kernel runs; more query rows dequantise the cache and take the bf16 path (correct, slow)."""
+    H = mha.num_heads
+    L_old = kv_cache[0].shape[1]
+    k8, v8 = ops.kv_append_fp8(kv_cache[0], kv_cache[1], k, v, kv8.k_inv, kv8.v_inv)
+    inv_freq = None if rot_pos_emb_k is None else getattr(rot_pos_emb_k, "inv_freq", None)
+    shadow = None
+    if (rot_pos_emb_q is not None and rot_pos_emb_k is not None and inv_freq is not None
+            and bool(rot_pos_emb_k.right_align) and bool(rot_pos_emb_q.right_align)):
+        shadow = ops.rotated_cache_keys(k8, q, H, inv_freq, k_new=k, k_descale=kv8.k_descale)
+    impl = getattr(mha, "kernel_impl", "auto")
+    if L_old == 0:
+        if shadow is not None:   # the prompt's own rows, rotated like q at the shadow's absolute positions
+            q_att, k_att = shadow[0], ops.rotary_at(k, H, inv_freq, ops.rotated_cache_shadow(k8)[1])
+        else:                    # the prompt's own rows, exactly as without a cache
+            q_att = q if rot_pos_emb_q is None else _rotate_rows(rot_pos_emb_q, q, H)
+            k_att = k if rot_pos_emb_k is None else _rotate_rows(rot_pos_emb_k, k, H)
+        o = ops.attention(q_att, k_att, v, H, mha.dp_scale, pad_mask=pad_mask, causal=mha.causal_attention, impl=impl)
+    else:
+        if shadow is not None:
+            q_att, k8_att = shadow
+        else:
+            q_att = q if rot_pos_emb_q is None else _rotate_rows(rot_pos_emb_q, q, H)
+            k8_att = k8 if rot_pos_emb_k is None else ops.rotary_fp8(k8, H, rot_pos_emb_k.frq_pos_enc,
+                                                                     bool(rot_pos_emb_k.right_align), kv8.k_descale)
+        if q.shape[1] <= 4:
+            o = ops.attention_decode_fp8(q_att, k8_att, v8, kv8.k_descale, kv8.v_descale, H, mha.dp_scale,
+                                         pad_mask=pad_mask, causal=mha.causal_attention)
+        else:
+            o = ops.attention(q_att, ops.fp8_dequantize(k8_att, kv8.k_descale, H, q.dtype),
+                              ops.fp8_dequantize(v8, kv8.v_descale, H, q.dtype), H, mha.dp_scale, pad_mask=pad_mask,
+                              causal=mha.causal_attention, impl=impl)
+    o = fused_linear(mha, "_pcv_o_fold", None, mha.o_proj, o, min_rows_key)
+    return ModuleOutput(last_hidden_state=o, kv_cache=(k8, v8))
 
 
 #: Policy of the fused K/V producer (LayerNorm + k_proj + v_proj as one tcgen05 GEMM, ``ops.kv_project``).
@@ -259,7 +302,72 @@ def project_qkv(self_attn, x: torch.Tensor):
 #: scales derived once per weight set by ``ops.fp8_descales``) and the attention runs on the e4m3 tensor cores
 #: (``ops.attention_fp8``).  Off by default because it changes the numbers; calls it does not cover (training mode,
 #: autograd, fp32, rotary, a KV cache, head dims that are not multiples of 16 or dqk > 256) take the bf16 path.
-fp8_config = {"enabled": False}
+#: ``kv_cache``: FP8 (e4m3) KV caches for cached generation, independent of ``enabled``: an empty incoming cache of a
+#: covered CrossAttention / SelfAttention call becomes an e4m3 cache (``_kv8_route``), whose cached steps run the e4m3
+#: decode kernel (``_attend_kv8``).  Off by default because it changes the numbers.
+fp8_config = {"enabled": False, "kv_cache": False}
+
+
+class _Kv8Scales(NamedTuple):
+    k_descale: torch.Tensor  # (H,) per-head K descale (pair-norm bound under rotary)
+    v_descale: torch.Tensor  # (H, dv) per-channel V descale
+    k_inv: torch.Tensor      # (H*dqk,) 1 / k_descale of every K channel
+    v_inv: torch.Tensor      # (H*dv,)
+
+
+def _kv8_scales(owner: nn.Module, norms, rotate_dim: int) -> _Kv8Scales:
+    """Scales of the e4m3 KV cache of ``owner.attention``, whose k / v projections read rows normalised by ``norms``
+    (one LayerNorm, or Perceiver AR's kv_norm and q_norm: its keys come from both, reference modules.py:222-224, so each
+    bound is the elementwise max of the two).  Cached on ``owner`` next to the folded weights and rebuilt when a
+    parameter changes (as ``_fold_cache``)."""
+    attn = owner.attention
+    H = attn.num_heads
+    tensors = [t for n in norms for t in (n.weight, n.bias)] + [t for lin in (attn.k_proj, attn.v_proj)
+                                                                for t in (lin.weight, lin.bias)]
+    key = (rotate_dim,) + tuple((None if t is None else (t.data_ptr(), t._version)) for t in tensors)
+    hit = owner.__dict__.get("_pcv_kv8_scales")
+    if hit is not None and hit[0] == key:
+        return hit[1]
+    kc = torch.stack([ops.fp8_descales(n.weight, n.bias, attn.k_proj.weight, attn.k_proj.bias, H, per_channel=True)
+                      for n in norms]).amax(dim=0)
+    vd = torch.stack([ops.fp8_descales(n.weight, n.bias, attn.v_proj.weight, attn.v_proj.bias, H, per_channel=True)
+                      for n in norms]).amax(dim=0).contiguous()
+    kd = ops.fp8_pair_descale(kc, rotate_dim)
+    val = _Kv8Scales(kd, vd, (1.0 / kd).repeat_interleave(kc.shape[1]).contiguous(), (1.0 / vd).reshape(-1).contiguous())
+    owner.__dict__["_pcv_kv8_scales"] = (key, val)
+    return val
+
+
+def _kv8_route(owner: nn.Module, norms, x: torch.Tensor, rot_pos_emb_k, kv_cache) -> Optional[_Kv8Scales]:
+    """The scales of the FP8 KV cache of this call of ``owner`` (a CrossAttention / SelfAttention, or a reference module
+    rebound by ``patch()``), or None for the bf16 cache.  An e4m3 incoming cache always stays e4m3; an empty one becomes
+    e4m3 when ``fp8_config["kv_cache"]`` is on and the call is covered: inference (no autograd, no autocast, no
+    attention dropout of a module in training mode) on bf16 / fp16 CUDA rows, head dims multiples of 16 and at most 256,
+    LayerNorms with an affine weight in front of k / v."""
+    if kv_cache is None:
+        return None
+    sticky = kv_cache[0].dtype == ops.F8
+    if not sticky and not (fp8_config["kv_cache"] and kv_cache[0].shape[1] == 0):
+        return None
+    attn = owner.attention
+    H = attn.num_heads
+    lins = (attn.k_proj, attn.v_proj)
+    dqk, dv = attn.k_proj.out_features // H, attn.v_proj.out_features // H
+    covered = (x.is_cuda and x.dtype in (torch.bfloat16, torch.float16) and not torch.is_autocast_enabled()
+               and dqk % 16 == 0 and dv % 16 == 0 and dqk <= 256 and dv <= 256
+               and all(isinstance(n, nn.LayerNorm) and n.weight is not None for n in norms)
+               and all(l.weight.dtype == x.dtype for l in lins))
+    grad = torch.is_grad_enabled() and (x.requires_grad or any(l.weight.requires_grad for l in lins))
+    # attention dropout of a module left in training mode runs on the bf16 path only
+    dropout = attn.training and float(attn.dropout.p) > 0.0
+    if sticky and (grad or dropout or not covered):
+        raise RuntimeError("an FP8 (e4m3) KV cache is inference-only: it needs bf16 / fp16 CUDA rows without autograd, "
+                           "autocast or attention dropout, and a LayerNorm with an affine weight in front of k_proj / "
+                           "v_proj")
+    if grad or dropout or not covered:
+        return None
+    rotate_dim = 0 if rot_pos_emb_k is None else int(rot_pos_emb_k.frq_pos_enc.shape[-1])
+    return _kv8_scales(owner, norms, rotate_dim)
 
 
 def _fp8_scales(cross_attn, dtype: torch.dtype):
@@ -371,6 +479,11 @@ class CrossAttention(nn.Module):
         if x_kv is None:
             x_q = self.q_norm(x_q)
             x_kv = torch.cat([self.kv_norm(x_kv_prefix), x_q], dim=1)
+            kv8 = _kv8_route(self, (self.kv_norm, self.q_norm), x_kv, rot_pos_emb_k, kv_cache)
+            if kv8 is not None:
+                a = self.attention
+                return attend(a, a.q_proj(x_q), a.k_proj(x_kv), a.v_proj(x_kv), pad_mask, rot_pos_emb_q, rot_pos_emb_k,
+                              kv_cache, kv8=kv8)
             return self.attention(x_q, x_kv, pad_mask=pad_mask, rot_pos_emb_q=rot_pos_emb_q,
                                   rot_pos_emb_k=rot_pos_emb_k, kv_cache=kv_cache)
         out = _fp8_cross_attention(self, x_q, x_kv, pad_mask, rot_pos_emb_q, rot_pos_emb_k, kv_cache)
@@ -378,7 +491,8 @@ class CrossAttention(nn.Module):
             return out
         q = fused_linear(self, "_pcv_q_fold", self.q_norm, self.attention.q_proj, x_q)
         k, v = project_kv(self, x_kv)
-        return attend(self.attention, q, k, v, pad_mask, rot_pos_emb_q, rot_pos_emb_k, kv_cache)
+        return attend(self.attention, q, k, v, pad_mask, rot_pos_emb_q, rot_pos_emb_k, kv_cache,
+                      kv8=_kv8_route(self, (self.kv_norm,), x_kv, rot_pos_emb_k, kv_cache))
 
 
 class SelfAttention(nn.Module):
@@ -418,10 +532,14 @@ class SelfAttention(nn.Module):
         rot_pos_emb: Optional[RotaryPositionEmbedding] = None,
         kv_cache: Optional[KVCache] = None,
     ):
+        kv8 = _kv8_route(self, (self.norm,), x, rot_pos_emb, kv_cache)
         qkv = project_qkv(self, x)
+        if qkv is None and kv8 is not None:
+            a, xn = self.attention, self.norm(x)
+            qkv = a.q_proj(xn), a.k_proj(xn), a.v_proj(xn)
         if qkv is not None:
             return attend(self.attention, qkv[0], qkv[1], qkv[2], pad_mask, rot_pos_emb, rot_pos_emb, kv_cache,
-                          min_rows_key="min_rows_latent")
+                          min_rows_key="min_rows_latent", kv8=kv8)
         x = self.norm(x)
         return self.attention(x, x, pad_mask=pad_mask, rot_pos_emb_q=rot_pos_emb, rot_pos_emb_k=rot_pos_emb,
                               kv_cache=kv_cache)

@@ -27,7 +27,8 @@ __all__ = [
     "attention", "attention_partial", "attention_sharded_fused", "combine_partials", "merge_partials", "rescale_partial_", "rotary", "kv_append",
     "device_info", "tcgen05_supported", "rotated_cache_keys", "ln_stats", "fold_ln_linear", "kv_project", "kv_project_supported",
     "attention_fp8", "attention_fp8_supported", "fp8_descales", "fp8_quantize", "fp8_transpose_v", "kv_project_fp8",
-    "kv_project_fp8_supported", "ln_linear", "ln_linear_backward",
+    "kv_project_fp8_supported", "ln_linear", "ln_linear_backward", "kv_append_fp8", "attention_decode_fp8",
+    "attention_decode_fp8_supported", "fp8_pair_descale", "fp8_dequantize", "rotated_cache_shadow", "rotary_at", "rotary_fp8",
 ]
 
 
@@ -926,8 +927,9 @@ def _arena_target(cache: torch.Tensor, n: int):
     return buf[:, :L + n], False
 
 
-def _launch_kv_append(k_cache, v_cache, k_new, v_new, k_dst, v_dst, k_in_place, v_in_place) -> None:
-    """One launch: dst[:, :L] = cache (skipped for a half appended in place), dst[:, L:] = new rows."""
+def _launch_kv_append(k_cache, v_cache, k_new, v_new, k_dst, v_dst, k_in_place, v_in_place, scales=None) -> None:
+    """One launch: dst[:, :L] = cache (skipped for a half appended in place), dst[:, L:] = new rows.  ``scales``: the
+    (k_inv_scale, v_inv_scale) of e4m3 caches (pcv_kv_append_fp8: the new rows are quantised on the way in)."""
     dt = k_new.dtype
     codes = {torch.bfloat16: _lib.PCV_BF16, torch.float16: _lib.PCV_F16, torch.float32: _lib.PCV_F32}
     B, L_old, Ck = k_cache.shape
@@ -946,7 +948,12 @@ def _launch_kv_append(k_cache, v_cache, k_new, v_new, k_dst, v_dst, k_in_place, 
     p.B, p.L_old, p.n, p.Ck, p.Cv = B, L_old, k_new.shape[1], Ck, v_new.shape[2]
     p.dtype = codes[dt]
     with torch.cuda.device(k_new.device):
-        check(_lib.lib().pcv_kv_append(C.byref(p), _stream()), "pcv_kv_append")
+        if scales is None:
+            check(_lib.lib().pcv_kv_append(C.byref(p), _stream()), "pcv_kv_append")
+        else:
+            f = _lib.KvFp8Scales()
+            f.k_inv_scale, f.v_inv_scale = scales[0].data_ptr(), scales[1].data_ptr()
+            check(_lib.lib().pcv_kv_append_fp8(C.byref(p), C.byref(f), _stream()), "pcv_kv_append_fp8")
 
 
 def kv_append(k_cache: torch.Tensor, v_cache: torch.Tensor, k_new: torch.Tensor, v_new: torch.Tensor):
@@ -976,14 +983,46 @@ def kv_append(k_cache: torch.Tensor, v_cache: torch.Tensor, k_new: torch.Tensor,
     dt = k_new.dtype
     if dt not in (torch.bfloat16, torch.float16, torch.float32):
         raise RuntimeError(f"kv_append supports bf16/fp16/fp32 caches, got {dt}")
+    return _append(k_cache, v_cache, k_new, v_new)
+
+
+def _append(k_cache, v_cache, k_new, v_new, scales=None):
+    """The arena step of :func:`kv_append` / :func:`kv_append_fp8`: destinations by :func:`_arena_target`, one launch."""
     k_cache, v_cache, k_new, v_new = (_rows_contiguous(t) for t in (k_cache, v_cache, k_new, v_new))
     L_old, n = k_cache.shape[1], k_new.shape[1]
     k_dst, k_in_place = _arena_target(k_cache, n)
     v_dst, v_in_place = _arena_target(v_cache, n)
     if L_old + n == 0:
         return k_dst, v_dst
-    _launch_kv_append(k_cache, v_cache, k_new, v_new, k_dst, v_dst, k_in_place, v_in_place)
+    args = (k_cache, v_cache, k_new, v_new, k_dst, v_dst, k_in_place, v_in_place)
+    if scales is None:
+        _launch_kv_append(*args)
+    else:
+        _launch_kv_append(*args, scales=scales)
     return k_dst, v_dst
+
+
+F8 = torch.float8_e4m3fn
+
+
+def kv_append_fp8(k_cache: torch.Tensor, v_cache: torch.Tensor, k_new: torch.Tensor, v_new: torch.Tensor,
+                  k_inv_scale: torch.Tensor, v_inv_scale: torch.Tensor):
+    """:func:`kv_append` onto an FP8 (e4m3) KV cache, in one launch (pcv_kv_append_fp8).
+
+    ``k_cache`` / ``v_cache`` are ``torch.float8_e4m3fn`` (B, L, C) caches, or empty caches of any dtype (the first
+    append decides the cache dtype); ``k_new`` / ``v_new`` are bf16 / fp16 rows, stored as the codes of
+    ``clamp(x.float() * inv_scale, +-448)`` (per-channel ``inv_scale`` (C,) float32, round to nearest even).  The result
+    is a row range of an e4m3 arena with the functional semantics of :func:`kv_append`."""
+    _require_cuda(k_cache, v_cache, k_new, v_new, k_inv_scale, v_inv_scale)
+    k_cache, v_cache = (c.to(F8) if c.shape[1] == 0 else c for c in (k_cache, v_cache))
+    if k_cache.dtype != F8 or v_cache.dtype != F8:
+        raise ValueError(f"kv_append_fp8: the caches must be float8_e4m3fn or empty, got {k_cache.dtype} / {v_cache.dtype}")
+    if k_new.dtype not in (torch.bfloat16, torch.float16) or v_new.dtype != k_new.dtype:
+        raise ValueError(f"kv_append_fp8: new rows must be bf16 / fp16 of one dtype, got {k_new.dtype} / {v_new.dtype}")
+    scales = tuple(t.float().contiguous() for t in (k_inv_scale, v_inv_scale))
+    if scales[0].shape != (k_new.shape[-1],) or scales[1].shape != (v_new.shape[-1],):
+        raise ValueError("kv_append_fp8: inverse scales must be (Ck,) and (Cv,)")
+    return _append(k_cache, v_cache, k_new, v_new, scales)
 
 
 #: Rotated-key cache of the decode path (``enabled=False``: re-rotate the whole cache every step like the reference).
@@ -997,7 +1036,56 @@ def _abs_angles(inv_freq: torch.Tensor, row0: int, n: int) -> torch.Tensor:
     return (pos[None, :, None] * inv_freq[None, None, :]).repeat_interleave(2, dim=-1).float()
 
 
-def rotated_cache_keys(k: torch.Tensor, q: torch.Tensor, num_heads: int, inv_freq: torch.Tensor):
+def _rotary_fp8(x: torch.Tensor, num_heads: int, angles: torch.Tensor, y: torch.Tensor, y_inv_scale: torch.Tensor,
+                x_descale: Optional[torch.Tensor] = None, right_align: bool = False) -> None:
+    """y (B, n, H*d) e4m3 <- e4m3(rotate(x) * y_inv_scale[h]) (pcv_rotary_apply_fp8).  x is bf16 / fp16, or e4m3 codes
+    standing for ``x * x_descale[h]``; ``angles`` (B or 1, n_angles, f) float32, rows as in :func:`rotary`."""
+    B, n, Cx = x.shape
+    d = Cx // num_heads
+    p = RotaryParams()
+    p.x, p.y, p.angles = x.data_ptr(), y.data_ptr(), angles.data_ptr()
+    p.x_stride_b, p.x_stride_n, p.x_stride_h = x.stride(0), x.stride(1), d
+    p.y_stride_b, p.y_stride_n, p.y_stride_h = y.stride(0), y.stride(1), d
+    p.a_stride_b = 0 if (angles.shape[0] == 1 and B > 1) else angles.stride(0)
+    p.a_stride_n = angles.stride(1)
+    p.B, p.n, p.H, p.d = B, n, num_heads, d
+    p.rotate_dim = angles.shape[-1]
+    p.angle_row0 = (angles.shape[1] - n) if right_align else 0
+    p.dtype = _lib.PCV_E4M3 if x.dtype == F8 else _pcv_dtype(x.dtype)
+    f = _lib.RotaryFp8()
+    f.x_descale = None if x_descale is None else x_descale.data_ptr()
+    f.y_inv_scale = y_inv_scale.data_ptr()
+    with torch.cuda.device(x.device):
+        check(_lib.lib().pcv_rotary_apply_fp8(C.byref(p), C.byref(f), _stream()), "pcv_rotary_apply_fp8")
+
+
+def rotary_fp8(x8: torch.Tensor, num_heads: int, angles: torch.Tensor, right_align: bool,
+               descale: torch.Tensor) -> torch.Tensor:
+    """e4m3 codes x8 (B, n, H*d) standing for ``x8 * descale[h]`` (descale (H,)), rotated like :func:`rotary` (the
+    reference's ``frq_pos_enc`` angles, (B or 1, [1,] n_angles, rotate_dim)) and requantised with the same descale, in
+    one pass (pcv_rotary_apply_fp8): a new (B, n, H*d) e4m3 tensor.  The descale must bound the rotated rows too
+    (:func:`fp8_pair_descale`).  Each code is rounded a second time."""
+    _require_cuda(x8, angles, descale)
+    if x8.dtype != F8:
+        raise ValueError(f"rotary_fp8: x8 must be torch.float8_e4m3fn, got {x8.dtype}")
+    if angles.dim() == 4:  # (B, 1, n, f) as stored by RotaryPositionEmbedding
+        angles = angles[:, 0]
+    angles = angles.float()
+    if angles.stride(-1) != 1:
+        angles = angles.contiguous()
+    B, n, _ = x8.shape
+    if angles.shape[0] not in (1, B) or angles.shape[1] < n:
+        raise ValueError(f"rotary_fp8: angles {tuple(angles.shape)} do not cover x8 {tuple(x8.shape)}")
+    x8 = _rows_contiguous(x8)
+    kd = descale.float().contiguous()
+    y = torch.empty(x8.shape, dtype=F8, device=x8.device)
+    if n:
+        _rotary_fp8(x8, num_heads, angles, y, 1.0 / kd, kd, bool(right_align))
+    return y
+
+
+def rotated_cache_keys(k: torch.Tensor, q: torch.Tensor, num_heads: int, inv_freq: torch.Tensor,
+                       k_new: Optional[torch.Tensor] = None, k_descale: Optional[torch.Tensor] = None):
     """Rotary embedding of a cached decode step WITHOUT re-rotating the cache: returns ``(q_rot, k_rot)`` or None.
 
     ``k`` (B, L, C) must be a row range of a KV arena (what :func:`kv_append` returns) and the rows of ``q`` (B, N, C)
@@ -1008,12 +1096,20 @@ def rotated_cache_keys(k: torch.Tensor, q: torch.Tensor, num_heads: int, inv_fre
     the arena", into a shadow buffer kept beside the arena; q is rotated at the row index of its own token.  For every
     non-masked (query, key) pair the angle difference equals the reference's (pos_q - pos_k = row_q - row_k; padded
     rows are masked out), so the scores agree up to rounding, and a decode step rotates N new rows instead of L.
-    Arena rows are write-once (an append that is not at the frontier gets a fresh arena), so shadow rows never go stale."""
+    Arena rows are write-once (an append that is not at the frontier gets a fresh arena), so shadow rows never go stale.
+
+    An e4m3 arena (:func:`kv_append_fp8`) gets an e4m3 shadow with the per-head ``k_descale`` (H,) of its codes, which
+    must bound the rotated rows too (:func:`fp8_pair_descale`).  ``k_new`` are the bf16 / fp16 rows this call appended
+    (the last ``k_new.shape[1]`` rows of ``k``): their shadow rows are rotated from those values and rounded once.  Older
+    rows the shadow lacks (a fresh or re-ordered arena) are rebuilt from the codes: dequantised, rotated, requantised."""
     if not rotated_cache_config["enabled"]:
         return None
     hit = _arena_of(k)
-    if hit is None or inv_freq is None or q.shape[1] > k.shape[1] or k.dtype not in (torch.bfloat16, torch.float16):
+    fp8 = k.dtype == F8
+    if hit is None or inv_freq is None or q.shape[1] > k.shape[1] or k.dtype not in (torch.bfloat16, torch.float16, F8):
         return None
+    if fp8 and k_descale is None:
+        raise ValueError("rotated_cache_keys: an e4m3 cache needs k_descale")
     arena, start = hit
     root = k._base if k._base is not None else k
     L, N = k.shape[1], q.shape[1]
@@ -1029,12 +1125,43 @@ def rotated_cache_keys(k: torch.Tensor, q: torch.Tensor, num_heads: int, inv_fre
     end = start + L
     if not (rot["lo"] <= start <= rot["hi"]):   # nothing reusable: rotate the whole range once
         rot["lo"], rot["hi"] = start, start
-    if rot["hi"] < end:
+    if rot["hi"] < end and fp8:
+        kd = k_descale.float().contiguous()
+        inv = 1.0 / kd
+        a, b = rot["hi"], end
+        fresh = end - (0 if k_new is None else k_new.shape[1])   # first row this call appended
+        if a < fresh:   # rebuilt from the codes: rounded twice
+            _rotary_fp8(root[:, a:fresh], num_heads, _abs_angles(inv_freq, a, fresh - a), rot["buf"][:, a:fresh], inv, kd)
+        a = max(a, fresh)
+        if a < b:       # rotated from this call's bf16 / fp16 rows: rounded once
+            _rotary_fp8(_rows_contiguous(k_new[:, a - fresh:]), num_heads, _abs_angles(inv_freq, a, b - a),
+                        rot["buf"][:, a:b], inv)
+        rot["hi"] = end
+    elif rot["hi"] < end:
         a, b = rot["hi"], end
         _rotary_forward(root[:, a:b], num_heads, _abs_angles(inv_freq, a, b - a), False, out=rot["buf"][:, a:b])
         rot["hi"] = end
     q_rot = _rotary_forward(q, num_heads, _abs_angles(inv_freq, end - N, N), False)
     return q_rot, rot["buf"][:, start:end]
+
+
+def rotary_at(x: torch.Tensor, num_heads: int, inv_freq: torch.Tensor, row0: int) -> torch.Tensor:
+    """x (B, n, H*d) rotated at the absolute positions row0 .. row0 + n - 1 (fp32 angles from ``inv_freq``), as
+    :func:`rotated_cache_keys` rotates q and the shadow rows."""
+    return _rotary_forward(x, num_heads, _abs_angles(inv_freq.detach().float(), row0, x.shape[1]), False)
+
+
+def rotated_cache_shadow(k: torch.Tensor):
+    """``(rows, first_position)`` of the rotated-key shadow that :func:`rotated_cache_keys` keeps for the cache ``k``:
+    ``rows`` (B, L, C) are k's rows rotated at the absolute positions ``first_position`` .. ``first_position + L - 1``
+    (bf16 / fp16, or the e4m3 codes of an FP8 cache).  None when k has no complete shadow (yet)."""
+    hit = _arena_of(k)
+    if hit is None or hit[0].rot is None:
+        return None
+    rot, start = hit[0].rot, hit[1]
+    if not (rot["lo"] <= start and start + k.shape[1] <= rot["hi"]):
+        return None
+    return rot["buf"][:, start:start + k.shape[1]], start
 
 
 def tcgen05_supported(q, k, v, num_heads: int, pad_mask=None, causal: bool = False) -> bool:
@@ -1121,6 +1248,74 @@ def fp8_descales(norm_weight, norm_bias, weight, bias, num_heads: int, per_chann
         bound = bound.amax(dim=1)
     # a channel with an all-zero weight row and bias is exactly zero: any positive descale quantises it exactly
     return (bound / E4M3_MAX).clamp_min(torch.finfo(torch.float32).tiny).float().contiguous()
+
+
+def fp8_pair_descale(channel_descale: torch.Tensor, rotate_dim: int = 0) -> torch.Tensor:
+    """Per-head K descale (H,) of an FP8 KV cache from the per-channel descales (H, d) of :func:`fp8_descales`.
+
+    A rotary channel mixes its pair, ``a cos - b sin``, so under rotation channels 2p and 2p+1 of the first
+    ``rotate_dim`` channels are bounded by the pair norm ``sqrt(b_2p^2 + b_2p+1^2)`` of their single-channel bounds, not
+    by either alone; the other channels by their own bound.  The per-head maximum of these bounds holds for the rows
+    before and after rotation, so one descale serves a cache and its rotated shadow."""
+    b = channel_descale.double()
+    if rotate_dim:
+        if rotate_dim % 2 or rotate_dim > b.shape[1]:
+            raise ValueError(f"fp8_pair_descale: rotate_dim {rotate_dim} must be even and <= {b.shape[1]}")
+        pair = b[:, :rotate_dim].reshape(b.shape[0], -1, 2).norm(dim=-1)
+        b = torch.cat([pair.repeat_interleave(2, dim=1), b[:, rotate_dim:]], dim=1)
+    return b.amax(dim=1).float().contiguous()
+
+
+def fp8_dequantize(x8: torch.Tensor, descale: torch.Tensor, num_heads: int, dtype: torch.dtype) -> torch.Tensor:
+    """(..., H*d) e4m3 codes -> ``codes * descale`` in ``dtype`` (descale (H,) per head or (H, d) per channel)."""
+    xs = x8.float().reshape(*x8.shape[:-1], num_heads, x8.shape[-1] // num_heads)
+    d = descale.float().to(x8.device)
+    d = d[:, None] if d.dim() == 1 else d
+    return (xs * d).reshape(x8.shape).to(dtype)
+
+
+def _fill_decode_fp8(q, k8, v8, k_descale, v_descale, num_heads, scale, pad_mask, causal):
+    """(AttnParams, DecodeFp8, tensors to keep alive) of an e4m3-cache decode; shapes as in :func:`attention_decode_fp8`."""
+    _require_cuda(q, k8, v8, k_descale, v_descale, pad_mask)
+    if k8.dtype != F8 or v8.dtype != F8:
+        raise ValueError(f"attention_decode_fp8: k8 / v8 must be torch.float8_e4m3fn, got {k8.dtype} / {v8.dtype}")
+    q = _rows_contiguous(q if q.dtype in (torch.bfloat16, torch.float16) else q.to(torch.bfloat16))
+    k8, v8 = _rows_contiguous(k8), _rows_contiguous(v8)
+    p, keep = _fill_attn_params(q, k8, v8, num_heads, scale, pad_mask, causal, None, 0, "decode")
+    kd, vd = k_descale.float().contiguous(), v_descale.float().contiguous()
+    if kd.shape != (p.H,) or vd.shape != (p.H, p.dv):
+        raise ValueError(f"attention_decode_fp8: descales must be (H,) and (H, dv) = ({p.H},), ({p.H}, {p.dv})")
+    f = _lib.DecodeFp8()
+    f.k_descale, f.v_descale = kd.data_ptr(), vd.data_ptr()
+    return p, f, keep + (q, kd, vd)
+
+
+def attention_decode_fp8_supported(q, k8, v8, k_descale, v_descale, num_heads: int, scale: float = 1.0,
+                                   pad_mask=None, causal: bool = False) -> bool:
+    """Whether :func:`attention_decode_fp8` covers these operands (no launch; reason in ``_lib.lib().pcv_last_error()``)."""
+    with torch.cuda.device(k8.device):
+        p, f, keep = _fill_decode_fp8(q, k8, v8, k_descale, v_descale, num_heads, scale, pad_mask, causal)
+        dummy = torch.empty(64, device=k8.device)
+        p.out = dummy.data_ptr()
+        p.o_stride_b, p.o_stride_n, p.o_stride_h = p.N * p.H * p.dv, p.H * p.dv, p.dv
+        return bool(_lib.lib().pcv_attn_decode_fp8_supported(C.byref(p), C.byref(f)))
+
+
+def attention_decode_fp8(q, k8, v8, k_descale, v_descale, num_heads: int, scale: float, pad_mask=None,
+                         causal: bool = False) -> torch.Tensor:
+    """Attention of at most 4 query rows on an FP8 (e4m3) KV cache (pcv_attn_decode_fp8, the streaming decode kernel).
+
+    q: (B or 1, N <= 4, H*dqk) bf16 / fp16; k8: (B, M, H*dqk), v8: (B, M, H*dv) ``torch.float8_e4m3fn`` rows standing for
+    ``k8 * k_descale[h]`` and ``v8[..., h, c] * v_descale[h, c]`` (float32 (H,) and (H, dv)).  Masks as in
+    :func:`attention`.  Returns (B, N, H*dv) in q's dtype; probabilities stay fp32.  Head dims: multiples of 16, at most
+    256.  No autograd: this is an inference path."""
+    with torch.cuda.device(k8.device):
+        p, f, keep = _fill_decode_fp8(q, k8, v8, k_descale, v_descale, num_heads, scale, pad_mask, causal)
+        out = _new_output(p, _compute_dtype(q.dtype), k8.device)
+        ws = _workspace(p, k8.device, "pcv_attn_decode_fp8", C.byref(p))
+        check(_lib.lib().pcv_attn_decode_fp8(C.byref(p), C.byref(f), _stream()), "pcv_attn_decode_fp8")
+    del keep, ws
+    return out
 
 
 def _fill_kvproj(x2, w_cat, col_st, n_k, n_v, stats, k_out, v_out, cta_group=0, ln_eps=0.0) -> KvProjParams:
