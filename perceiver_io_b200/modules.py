@@ -38,12 +38,27 @@ from .utils import ModuleOutput, Residual, init_parameters
 KVCache = Tuple[torch.Tensor, torch.Tensor]
 
 
-def _rotate_rows(rot, x: torch.Tensor, num_heads: int) -> torch.Tensor:
-    """Apply a rotary embedding object to pre-head-split rows (B, n, H*d).
+def _rotate_qk(num_heads: int, q: torch.Tensor, k: torch.Tensor, rot_q, rot_k, cache_k=None, k_descale=None, **shadow):
+    """``(q, k, from_shadow)``: q and k (B, n, H*d) as the attention takes them after the rotary embedding.
 
-    Accepts this package's ``RotaryPositionEmbedding`` or any object with the reference's attributes
-    (``frq_pos_enc`` (B,1,n,f), ``right_align``) — e.g. one built by reference code."""
-    return ops.rotary(x, num_heads, rot.frq_pos_enc, bool(rot.right_align))
+    With ``cache_k`` (the cache's keys after this call's append) both come from the rotated-key shadow
+    (``ops.rotated_cache_keys``: keys are rotated once, when they enter the cache) when it can serve: both rotary objects
+    right-aligned and the key one carrying its frequency table ``inv_freq``, as this package's models pass it.
+    Otherwise each is rotated by its own rotary object, this package's ``RotaryPositionEmbedding`` or any object with the
+    reference's attributes (``frq_pos_enc`` (B,1,n,f), ``right_align``); e4m3 keys with their per-head ``k_descale``,
+    e4m3 to e4m3 (``ops.rotary_fp8``)."""
+    if (cache_k is not None and rot_q is not None and getattr(rot_k, "inv_freq", None) is not None
+            and bool(rot_q.right_align) and bool(rot_k.right_align)):
+        hit = ops.rotated_cache_keys(cache_k, q, num_heads, rot_k.inv_freq, k_descale=k_descale, **shadow)
+        if hit is not None:
+            return hit[0], hit[1], True
+    if rot_q is not None:
+        q = ops.rotary(q, num_heads, rot_q.frq_pos_enc, bool(rot_q.right_align))
+    if rot_k is not None and k.dtype == ops.F8:
+        k = ops.rotary_fp8(k, num_heads, rot_k.frq_pos_enc, bool(rot_k.right_align), k_descale)
+    elif rot_k is not None:
+        k = ops.rotary(k, num_heads, rot_k.frq_pos_enc, bool(rot_k.right_align))
+    return q, k, False
 
 
 class MultiHeadAttention(nn.Module):
@@ -121,19 +136,9 @@ def attend(mha, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, pad_mask=None
         k, v = ops.kv_append(kv_cache[0], kv_cache[1], k, v)
         kv_cache = (k, v)
 
-    k_att = None
-    if (kv_cache is not None and rot_pos_emb_q is not None and rot_pos_emb_k is not None
-            and getattr(rot_pos_emb_k, "inv_freq", None) is not None and bool(rot_pos_emb_k.right_align)
-            and bool(rot_pos_emb_q.right_align) and not (torch.is_grad_enabled() and (q.requires_grad or k.requires_grad))):
-        # decode path: keys are rotated once, when they enter the cache (ops.rotated_cache_keys)
-        hit = ops.rotated_cache_keys(k, q, mha.num_heads, rot_pos_emb_k.inv_freq)
-        if hit is not None:
-            q, k_att = hit
-    if k_att is None:
-        if rot_pos_emb_q is not None:
-            q = _rotate_rows(rot_pos_emb_q, q, mha.num_heads)
-        k_att = k if rot_pos_emb_k is None else _rotate_rows(rot_pos_emb_k, k, mha.num_heads)
-
+    # the shadow has no autograd: rows that need a gradient are rotated by the rotary objects
+    shadow = kv_cache is not None and not (torch.is_grad_enabled() and (q.requires_grad or k.requires_grad))
+    q, k_att, _ = _rotate_qk(mha.num_heads, q, k, rot_pos_emb_q, rot_pos_emb_k, k if shadow else None)
     o = ops.attention(q, k_att, v, mha.num_heads, mha.dp_scale, pad_mask=pad_mask,
                       causal=mha.causal_attention, impl=getattr(mha, "kernel_impl", "auto"), dropout_p=drop_p)
     o = fused_linear(mha, "_pcv_o_fold", None, mha.o_proj, o, min_rows_key)
@@ -150,33 +155,21 @@ def _attend_kv8(mha, q, k, v, pad_mask, rot_pos_emb_q, rot_pos_emb_k, kv_cache, 
     H = mha.num_heads
     L_old = kv_cache[0].shape[1]
     k8, v8 = ops.kv_append_fp8(kv_cache[0], kv_cache[1], k, v, kv8.k_inv, kv8.v_inv)
-    inv_freq = None if rot_pos_emb_k is None else getattr(rot_pos_emb_k, "inv_freq", None)
-    shadow = None
-    if (rot_pos_emb_q is not None and rot_pos_emb_k is not None and inv_freq is not None
-            and bool(rot_pos_emb_k.right_align) and bool(rot_pos_emb_q.right_align)):
-        shadow = ops.rotated_cache_keys(k8, q, H, inv_freq, k_new=k, k_descale=kv8.k_descale)
+    # the prompt attends over its own bf16 / fp16 rows, a cached step over the e4m3 rows
+    q_att, k_att, shadowed = _rotate_qk(H, q, k if L_old == 0 else k8, rot_pos_emb_q, rot_pos_emb_k, k8, kv8.k_descale,
+                                        k_new=k)
     impl = getattr(mha, "kernel_impl", "auto")
     if L_old == 0:
-        if shadow is not None:   # the prompt's own rows, rotated like q at the shadow's absolute positions
-            q_att, k_att = shadow[0], ops.rotary_at(k, H, inv_freq, ops.rotated_cache_shadow(k8)[1])
-        else:                    # the prompt's own rows, exactly as without a cache
-            q_att = q if rot_pos_emb_q is None else _rotate_rows(rot_pos_emb_q, q, H)
-            k_att = k if rot_pos_emb_k is None else _rotate_rows(rot_pos_emb_k, k, H)
+        if shadowed:   # the prompt's own rows, rotated like q at the shadow's absolute positions
+            k_att = ops.rotary_at(k, H, rot_pos_emb_k.inv_freq, ops.rotated_cache_shadow(k8)[1])
         o = ops.attention(q_att, k_att, v, H, mha.dp_scale, pad_mask=pad_mask, causal=mha.causal_attention, impl=impl)
+    elif q.shape[1] <= 4:
+        o = ops.attention_decode_fp8(q_att, k_att, v8, kv8.k_descale, kv8.v_descale, H, mha.dp_scale,
+                                     pad_mask=pad_mask, causal=mha.causal_attention)
     else:
-        if shadow is not None:
-            q_att, k8_att = shadow
-        else:
-            q_att = q if rot_pos_emb_q is None else _rotate_rows(rot_pos_emb_q, q, H)
-            k8_att = k8 if rot_pos_emb_k is None else ops.rotary_fp8(k8, H, rot_pos_emb_k.frq_pos_enc,
-                                                                     bool(rot_pos_emb_k.right_align), kv8.k_descale)
-        if q.shape[1] <= 4:
-            o = ops.attention_decode_fp8(q_att, k8_att, v8, kv8.k_descale, kv8.v_descale, H, mha.dp_scale,
-                                         pad_mask=pad_mask, causal=mha.causal_attention)
-        else:
-            o = ops.attention(q_att, ops.fp8_dequantize(k8_att, kv8.k_descale, H, q.dtype),
-                              ops.fp8_dequantize(v8, kv8.v_descale, H, q.dtype), H, mha.dp_scale, pad_mask=pad_mask,
-                              causal=mha.causal_attention, impl=impl)
+        o = ops.attention(q_att, ops.fp8_dequantize(k_att, kv8.k_descale, H, q.dtype),
+                          ops.fp8_dequantize(v8, kv8.v_descale, H, q.dtype), H, mha.dp_scale, pad_mask=pad_mask,
+                          causal=mha.causal_attention, impl=impl)
     o = fused_linear(mha, "_pcv_o_fold", None, mha.o_proj, o, min_rows_key)
     return ModuleOutput(last_hidden_state=o, kv_cache=(k8, v8))
 
@@ -187,54 +180,58 @@ def _attend_kv8(mha, q, k, v, pad_mask, rot_pos_emb_q, rot_pos_emb_k, kv_cache, 
 #: (B*N of a few thousand rows) is bound by host-side dispatch, where ATen's nn.Linear path is leaner than three ctypes
 #: calls; under a CUDA graph (``graphs.graph_latent_block`` lowers the threshold while recording) the fused path wins
 #: because it launches 4 kernels per layer instead of 7 (tools/latent_stack_bench.py).
-#: ``training``: under autograd, route the LayerNorm -> projection chains (``project_kv``, ``fused_linear`` with a norm,
-#: ``project_qkv``) through ``ops.ln_linear`` (the fused producer forward, which saves x and the row statistics instead
-#: of the LayerNorm output, and the ``pcv_ln_linear_bwd`` backward).  Off by default: training then runs LayerNorm + the
-#: library GEMMs as before.
+#: ``training``: the route of a LayerNorm -> projection chain that autograd needs (``_needs_grad``: grad mode on and x or
+#: any weight or bias of the LayerNorm or the Linear layers requires grad).  On: ``ops.ln_linear`` (the fused producer
+#: forward, which saves x and the row statistics instead of the LayerNorm output, and the ``pcv_ln_linear_bwd``
+#: backward) for ``project_kv``, ``fused_linear`` with a norm and ``project_qkv``.  Off by default: such chains then run
+#: LayerNorm + the library GEMMs.  A chain autograd does not need takes the inference kernel either way.
 kv_producer_config = {"enabled": True, "min_rows": 512, "min_rows_latent": 4096, "training": False}
 
 
-def _fold_cache(owner: nn.Module, slot: str, norm: Optional[nn.Module], linears, dtype: torch.dtype):
-    """Folded weights of ``norm`` followed by ``linears`` (ops.fold_ln_linear), cached on ``owner`` and rebuilt
-    whenever a parameter was modified in place, replaced or moved (data_ptr / ``_version`` of every tensor)."""
-    tensors = []
-    if norm is not None:
-        tensors += [norm.weight, norm.bias]
-    for lin in linears:
-        tensors += [lin.weight, lin.bias]
-    key = (dtype,) + tuple((None if t is None else (t.data_ptr(), t._version)) for t in tensors)
+def _weight_cache(owner: nn.Module, slot: str, tensors, extra_key, build):
+    """``build()`` cached on ``owner`` as ``owner.__dict__[slot] = (key, value)`` and rebuilt whenever ``extra_key``
+    changes or one of ``tensors`` (entries may be None) was modified in place, replaced or moved (data_ptr /
+    ``_version``)."""
+    key = (extra_key,) + tuple((None if t is None else (t.data_ptr(), t._version)) for t in tensors)
     hit = owner.__dict__.get(slot)
     if hit is not None and hit[0] == key:
-        return hit[1], hit[2]
-    w_cat, col_st = ops.fold_ln_linear(None if norm is None else norm.weight, None if norm is None else norm.bias,
-                                       [lin.weight for lin in linears], [lin.bias for lin in linears], dtype)
-    owner.__dict__[slot] = (key, w_cat, col_st)
-    return w_cat, col_st
+        return hit[1]
+    value = build()
+    owner.__dict__[slot] = (key, value)
+    return value
 
 
-def _fusable(x: torch.Tensor, linears, norm, min_rows_key: str = "min_rows", allow_grad: bool = False) -> bool:
-    """Inference on bf16/fp16 CUDA rows with parameters in the same dtype: the case the tcgen05 projection kernel
-    (ops.kv_project) covers; autograd, autocast, fp32 and tiny inputs stay on LayerNorm + nn.Linear (library GEMMs).
-    ``allow_grad``: the same conditions without the one on autograd (the training route, ``_trains_fused``)."""
-    if not kv_producer_config["enabled"] or not x.is_cuda or x.dtype not in (torch.bfloat16, torch.float16):
-        return False
-    if x.numel() // max(x.shape[-1], 1) < kv_producer_config[min_rows_key] or torch.is_autocast_enabled():
-        return False
-    if norm is not None and not (isinstance(norm, nn.LayerNorm) and len(norm.normalized_shape) == 1
-                                 and norm.normalized_shape[0] == x.shape[-1]):
-        return False
-    if any(lin.weight.dtype != x.dtype or lin.in_features != x.shape[-1] for lin in linears):
-        return False
-    if not allow_grad and torch.is_grad_enabled() and (x.requires_grad or any(lin.weight.requires_grad for lin in linears)
-                                    or (norm is not None and norm.weight is not None and norm.weight.requires_grad)):
-        return False
-    return True
+def _params(norm: Optional[nn.Module], linears):
+    """The weights and biases of ``norm`` (may be None) and ``linears``, in that order (entries may be None)."""
+    return ([] if norm is None else [norm.weight, norm.bias]) + [t for lin in linears for t in (lin.weight, lin.bias)]
 
 
-def _trains_fused(x: torch.Tensor, linears, norm, min_rows_key: str = "min_rows") -> bool:
-    """A LayerNorm -> projection chain under autograd that ``kv_producer_config["training"]`` sends to ops.ln_linear."""
-    return (kv_producer_config["training"] and norm is not None and torch.is_grad_enabled()
-            and _fusable(x, linears, norm, min_rows_key, allow_grad=True))
+def _fold_cache(owner: nn.Module, slot: str, norm: Optional[nn.Module], linears, dtype: torch.dtype):
+    """Folded weights ``(w_cat, col_st)`` of ``norm`` followed by ``linears`` (ops.fold_ln_linear), cached on ``owner``
+    per weight version (``_weight_cache``)."""
+    return _weight_cache(owner, slot, _params(norm, linears), dtype, lambda: ops.fold_ln_linear(
+        None if norm is None else norm.weight, None if norm is None else norm.bias,
+        [lin.weight for lin in linears], [lin.bias for lin in linears], dtype))
+
+
+def _needs_grad(x: torch.Tensor, norm: Optional[nn.Module], linears) -> bool:
+    """Whether autograd needs ``linears(norm(x))``: grad mode on and x, or any weight or bias of ``norm`` and
+    ``linears``, requires grad.  Every kernel route that is not differentiable declines such a call."""
+    return torch.is_grad_enabled() and (x.requires_grad or any(t is not None and t.requires_grad
+                                                               for t in _params(norm, linears)))
+
+
+def _covered(x: torch.Tensor, norm: Optional[nn.Module], linears) -> bool:
+    """The conditions every LayerNorm-folded producer route shares: bf16 / fp16 CUDA rows outside autocast, a 1-D
+    ``nn.LayerNorm`` over the channels of x (or no norm) and Linear weights in x's dtype reading those channels."""
+    C = x.shape[-1]
+    return (x.is_cuda and x.dtype in (torch.bfloat16, torch.float16) and not torch.is_autocast_enabled()
+            and (norm is None or (isinstance(norm, nn.LayerNorm) and tuple(norm.normalized_shape) == (C,)))
+            and all(lin.weight.dtype == x.dtype and lin.in_features == C for lin in linears))
+
+
+def _has_affine(norm) -> bool:
+    return isinstance(norm, nn.LayerNorm) and norm.weight is not None
 
 
 def _ln_linear(owner: nn.Module, slot: str, norm: nn.LayerNorm, linears, x: torch.Tensor, n_k: int, n_v: int):
@@ -244,64 +241,71 @@ def _ln_linear(owner: nn.Module, slot: str, norm: nn.LayerNorm, linears, x: torc
                          n_k, n_v, norm.eps, w_cat, col_st)
 
 
+def _ln_project(owner: nn.Module, slot: str, norm: Optional[nn.Module], linears, x: torch.Tensor,
+                min_rows_key: str = "min_rows"):
+    """``linears(norm(x))`` (``norm`` may be None), one output per Linear, from ONE LayerNorm-folded tcgen05 GEMM over
+    the concatenated weights (the first Linear as the producer's first output, the others as column ranges of its
+    second), folded weights cached on ``owner.__dict__[slot]``.  A chain autograd does not need (``_needs_grad``) runs
+    the inference kernel (``ops.kv_project``); one it needs runs the training route (``_ln_linear``) when
+    ``kv_producer_config["training"]`` is on and there is a norm.  None when neither covers the call: the caller then
+    runs the library path."""
+    n_k, n_v = linears[0].out_features, sum(lin.out_features for lin in linears[1:])
+    if not (kv_producer_config["enabled"] and x.numel() // max(x.shape[-1], 1) >= kv_producer_config[min_rows_key]
+            and _covered(x, norm, linears) and ops.kv_project_supported(x, n_k, n_v)):
+        return None
+    if not _needs_grad(x, norm, linears):
+        w_cat, col_st = _fold_cache(owner, slot, norm if _has_affine(norm) else None, linears, x.dtype)
+        first, rest = ops.kv_project(x, w_cat, col_st, n_k, n_v, eps=None if norm is None else norm.eps)
+    elif kv_producer_config["training"] and norm is not None:
+        first, rest = _ln_linear(owner, slot, norm, linears, x, n_k, n_v)
+    else:
+        return None
+    if len(linears) == 1:
+        return (first,)
+    if len(linears) == 2:
+        return first, rest
+    n = linears[1].out_features
+    return first, rest[..., :n], rest[..., n:]
+
+
 def fused_linear(owner: nn.Module, slot: str, norm: Optional[nn.Module], linear: nn.Linear, x: torch.Tensor,
                  min_rows_key: str = "min_rows"):
     """``linear(norm(x))`` (``norm`` may be None) through the tcgen05 projection kernel when it applies — the q_norm ->
     q_proj chain of CrossAttention (reference modules.py:220, :113) and o_proj (:168) — else the library path."""
-    n_out = linear.out_features
-    if not (_fusable(x, [linear], norm, min_rows_key) and ops.kv_project_supported(x, n_out, 0)):
-        if _trains_fused(x, [linear], norm, min_rows_key) and ops.kv_project_supported(x, n_out, 0):
-            return _ln_linear(owner, slot, norm, [linear], x, n_out, 0)[0]
-        return linear(x if norm is None else norm(x))
-    affine = norm if (norm is not None and norm.weight is not None) else None
-    w_cat, col_st = _fold_cache(owner, slot, affine, [linear], x.dtype)
-    y, _ = ops.kv_project(x, w_cat, col_st, n_out, 0, eps=None if norm is None else norm.eps)
-    return y
+    y = _ln_project(owner, slot, norm, [linear], x, min_rows_key)
+    return linear(x if norm is None else norm(x)) if y is None else y[0]
 
 
 def project_kv(cross_attn, x_kv: torch.Tensor):
     """``k_proj(kv_norm(x_kv)), v_proj(kv_norm(x_kv))`` of a CrossAttention (reference modules.py:226, :114-115).
 
-    Inference on bf16/fp16 CUDA rows goes through the fused producer (one pass over x_kv on the tensor cores,
-    LayerNorm folded into the GEMM epilogue, ``pcv_ln_stats`` + ``pcv_kv_project``); everything else — autograd,
-    fp32, widths TMA cannot address, tiny inputs — uses LayerNorm + the two ``nn.Linear`` (library GEMMs)."""
-    attn = cross_attn.attention
-    norm = cross_attn.kv_norm
-    n_k, n_v = attn.k_proj.out_features, attn.v_proj.out_features
-    if not (_fusable(x_kv, [attn.k_proj, attn.v_proj], norm) and ops.kv_project_supported(x_kv, n_k, n_v)):
-        if _trains_fused(x_kv, [attn.k_proj, attn.v_proj], norm) and ops.kv_project_supported(x_kv, n_k, n_v):
-            return _ln_linear(cross_attn, "_pcv_kv_fold", norm, [attn.k_proj, attn.v_proj], x_kv, n_k, n_v)
+    bf16/fp16 CUDA rows go through the fused producer (one pass over x_kv on the tensor cores, LayerNorm folded into
+    the GEMM epilogue, ``pcv_ln_stats`` + ``pcv_kv_project``; under autograd only on the training route); everything
+    else — fp32, autocast, widths TMA cannot address, tiny inputs — uses LayerNorm + the two ``nn.Linear``."""
+    attn, norm = cross_attn.attention, cross_attn.kv_norm
+    kv = _ln_project(cross_attn, "_pcv_kv_fold", norm, [attn.k_proj, attn.v_proj], x_kv)
+    if kv is None:
         x = norm(x_kv)
-        return attn.k_proj(x), attn.v_proj(x)
-    w_cat, col_st = _fold_cache(cross_attn, "_pcv_kv_fold", norm if norm.weight is not None else None,
-                                [attn.k_proj, attn.v_proj], x_kv.dtype)
-    return ops.kv_project(x_kv, w_cat, col_st, n_k, n_v, eps=norm.eps)
+        kv = attn.k_proj(x), attn.v_proj(x)
+    return kv
 
 
 def project_qkv(self_attn, x: torch.Tensor):
     """``q_proj(norm(x)), k_proj(norm(x)), v_proj(norm(x))`` of a SelfAttention (reference modules.py:276, :113-115) as
     ONE LayerNorm-folded tcgen05 GEMM over [Wq; Wk; Wv] (``ops.kv_project`` with q as its first output and [k | v] as
     the second: k and v are column ranges of one buffer, the attention kernel takes them by stride).  Returns None when
-    the fused path does not apply (autograd, fp32, autocast, tiny inputs): the caller then runs the library path."""
-    attn, norm = self_attn.attention, self_attn.norm
-    n_q, n_k, n_v = attn.q_proj.out_features, attn.k_proj.out_features, attn.v_proj.out_features
-    linears = [attn.q_proj, attn.k_proj, attn.v_proj]
-    if not (_fusable(x, linears, norm, "min_rows_latent") and ops.kv_project_supported(x, n_q, n_k + n_v)):
-        if _trains_fused(x, linears, norm, "min_rows_latent") and ops.kv_project_supported(x, n_q, n_k + n_v):
-            q, kv = _ln_linear(self_attn, "_pcv_qkv_fold", norm, linears, x, n_q, n_k + n_v)
-            return q, kv[..., :n_k], kv[..., n_k:]
-        return None
-    w_cat, col_st = _fold_cache(self_attn, "_pcv_qkv_fold", norm if norm.weight is not None else None,
-                                [attn.q_proj, attn.k_proj, attn.v_proj], x.dtype)
-    q, kv = ops.kv_project(x, w_cat, col_st, n_q, n_k + n_v, eps=norm.eps)
-    return q, kv[..., :n_k], kv[..., n_k:]
+    the fused path does not apply (``_ln_project``): the caller then runs the library path."""
+    attn = self_attn.attention
+    return _ln_project(self_attn, "_pcv_qkv_fold", self_attn.norm, [attn.q_proj, attn.k_proj, attn.v_proj], x,
+                       "min_rows_latent")
 
 
 #: FP8 (e4m3) inference route of ``CrossAttention.forward`` with ``x_kv`` (this package's class and reference modules
 #: rebound by ``patch()``): q, K and V^T come out of the LayerNorm-folded producer as e4m3 (``ops.kv_project_fp8``,
 #: scales derived once per weight set by ``ops.fp8_descales``) and the attention runs on the e4m3 tensor cores
 #: (``ops.attention_fp8``).  Off by default because it changes the numbers; calls it does not cover (training mode,
-#: autograd, fp32, rotary, a KV cache, head dims that are not multiples of 16 or dqk > 256) take the bf16 path.
+#: a q / K / V chain autograd needs (``_needs_grad``), fp32, rotary, a KV cache, head dims that are not multiples of 16,
+#: dqk > 256 or dv > 512) take the bf16 path.
 #: ``kv_cache``: FP8 (e4m3) KV caches for cached generation, independent of ``enabled``: an empty incoming cache of a
 #: covered CrossAttention / SelfAttention call becomes an e4m3 cache (``_kv8_route``), whose cached steps run the e4m3
 #: decode kernel (``_attend_kv8``).  Off by default because it changes the numbers.
@@ -318,31 +322,28 @@ class _Kv8Scales(NamedTuple):
 def _kv8_scales(owner: nn.Module, norms, rotate_dim: int) -> _Kv8Scales:
     """Scales of the e4m3 KV cache of ``owner.attention``, whose k / v projections read rows normalised by ``norms``
     (one LayerNorm, or Perceiver AR's kv_norm and q_norm: its keys come from both, reference modules.py:222-224, so each
-    bound is the elementwise max of the two).  Cached on ``owner`` next to the folded weights and rebuilt when a
-    parameter changes (as ``_fold_cache``)."""
+    bound is the elementwise max of the two).  Cached on ``owner`` per weight version (``_weight_cache``)."""
     attn = owner.attention
     H = attn.num_heads
-    tensors = [t for n in norms for t in (n.weight, n.bias)] + [t for lin in (attn.k_proj, attn.v_proj)
-                                                                for t in (lin.weight, lin.bias)]
-    key = (rotate_dim,) + tuple((None if t is None else (t.data_ptr(), t._version)) for t in tensors)
-    hit = owner.__dict__.get("_pcv_kv8_scales")
-    if hit is not None and hit[0] == key:
-        return hit[1]
-    kc = torch.stack([ops.fp8_descales(n.weight, n.bias, attn.k_proj.weight, attn.k_proj.bias, H, per_channel=True)
-                      for n in norms]).amax(dim=0)
-    vd = torch.stack([ops.fp8_descales(n.weight, n.bias, attn.v_proj.weight, attn.v_proj.bias, H, per_channel=True)
-                      for n in norms]).amax(dim=0).contiguous()
-    kd = ops.fp8_pair_descale(kc, rotate_dim)
-    val = _Kv8Scales(kd, vd, (1.0 / kd).repeat_interleave(kc.shape[1]).contiguous(), (1.0 / vd).reshape(-1).contiguous())
-    owner.__dict__["_pcv_kv8_scales"] = (key, val)
-    return val
+    tensors = [t for n in norms for t in (n.weight, n.bias)] + _params(None, (attn.k_proj, attn.v_proj))
+
+    def build():
+        kc = torch.stack([ops.fp8_descales(n.weight, n.bias, attn.k_proj.weight, attn.k_proj.bias, H, per_channel=True)
+                          for n in norms]).amax(dim=0)
+        vd = torch.stack([ops.fp8_descales(n.weight, n.bias, attn.v_proj.weight, attn.v_proj.bias, H, per_channel=True)
+                          for n in norms]).amax(dim=0).contiguous()
+        kd = ops.fp8_pair_descale(kc, rotate_dim)
+        return _Kv8Scales(kd, vd, (1.0 / kd).repeat_interleave(kc.shape[1]).contiguous(),
+                          (1.0 / vd).reshape(-1).contiguous())
+
+    return _weight_cache(owner, "_pcv_kv8_scales", tensors, rotate_dim, build)
 
 
 def _kv8_route(owner: nn.Module, norms, x: torch.Tensor, rot_pos_emb_k, kv_cache) -> Optional[_Kv8Scales]:
     """The scales of the FP8 KV cache of this call of ``owner`` (a CrossAttention / SelfAttention, or a reference module
     rebound by ``patch()``), or None for the bf16 cache.  An e4m3 incoming cache always stays e4m3; an empty one becomes
-    e4m3 when ``fp8_config["kv_cache"]`` is on and the call is covered: inference (no autograd, no autocast, no
-    attention dropout of a module in training mode) on bf16 / fp16 CUDA rows, head dims multiples of 16 and at most 256,
+    e4m3 when ``fp8_config["kv_cache"]`` is on and the call is covered: inference (no chain autograd needs, no attention
+    dropout of a module in training mode) on the rows ``_covered`` takes, head dims multiples of 16 and at most 256,
     LayerNorms with an affine weight in front of k / v."""
     if kv_cache is None:
         return None
@@ -353,18 +354,15 @@ def _kv8_route(owner: nn.Module, norms, x: torch.Tensor, rot_pos_emb_k, kv_cache
     H = attn.num_heads
     lins = (attn.k_proj, attn.v_proj)
     dqk, dv = attn.k_proj.out_features // H, attn.v_proj.out_features // H
-    covered = (x.is_cuda and x.dtype in (torch.bfloat16, torch.float16) and not torch.is_autocast_enabled()
-               and dqk % 16 == 0 and dv % 16 == 0 and dqk <= 256 and dv <= 256
-               and all(isinstance(n, nn.LayerNorm) and n.weight is not None for n in norms)
-               and all(l.weight.dtype == x.dtype for l in lins))
-    grad = torch.is_grad_enabled() and (x.requires_grad or any(l.weight.requires_grad for l in lins))
     # attention dropout of a module left in training mode runs on the bf16 path only
-    dropout = attn.training and float(attn.dropout.p) > 0.0
-    if sticky and (grad or dropout or not covered):
-        raise RuntimeError("an FP8 (e4m3) KV cache is inference-only: it needs bf16 / fp16 CUDA rows without autograd, "
-                           "autocast or attention dropout, and a LayerNorm with an affine weight in front of k_proj / "
-                           "v_proj")
-    if grad or dropout or not covered:
+    covered = (dqk % 16 == 0 and dv % 16 == 0 and dqk <= 256 and dv <= 256
+               and not (attn.training and float(attn.dropout.p) > 0.0)
+               and all(_covered(x, n, lins) and _has_affine(n) and not _needs_grad(x, n, lins) for n in norms))
+    if not covered:
+        if sticky:
+            raise RuntimeError("an FP8 (e4m3) KV cache is inference-only: it needs bf16 / fp16 CUDA rows without "
+                               "autograd, autocast or attention dropout, and a LayerNorm with an affine weight in front "
+                               "of k_proj / v_proj")
         return None
     rotate_dim = 0 if rot_pos_emb_k is None else int(rot_pos_emb_k.frq_pos_enc.shape[-1])
     return _kv8_scales(owner, norms, rotate_dim)
@@ -372,24 +370,21 @@ def _kv8_route(owner: nn.Module, norms, x: torch.Tensor, rot_pos_emb_k, kv_cache
 
 def _fp8_scales(cross_attn, dtype: torch.dtype):
     """(q_descale (H,), k_descale (H,), v_descale (H, dv), inv_q (n_q,), inv_kv (n_k + n_v,)) of a CrossAttention,
-    cached on it next to the folded weights and rebuilt when a parameter changes (as ``_fold_cache``)."""
+    cached on it per weight version (``_weight_cache``)."""
     attn, H = cross_attn.attention, cross_attn.attention.num_heads
     qn, kvn = cross_attn.q_norm, cross_attn.kv_norm
-    tensors = [qn.weight, qn.bias, kvn.weight, kvn.bias] + [t for lin in (attn.q_proj, attn.k_proj, attn.v_proj)
-                                                             for t in (lin.weight, lin.bias)]
-    key = (dtype,) + tuple((None if t is None else (t.data_ptr(), t._version)) for t in tensors)
-    hit = cross_attn.__dict__.get("_pcv_fp8_scales")
-    if hit is not None and hit[0] == key:
-        return hit[1]
-    qd = ops.fp8_descales(qn.weight, qn.bias, attn.q_proj.weight, attn.q_proj.bias, H)
-    kd = ops.fp8_descales(kvn.weight, kvn.bias, attn.k_proj.weight, attn.k_proj.bias, H)
-    vd = ops.fp8_descales(kvn.weight, kvn.bias, attn.v_proj.weight, attn.v_proj.bias, H, per_channel=True)
-    dqk = attn.q_proj.out_features // H
-    inv_q = (1.0 / qd).repeat_interleave(dqk).contiguous()
-    inv_kv = torch.cat([(1.0 / kd).repeat_interleave(attn.k_proj.out_features // H), (1.0 / vd).reshape(-1)]).contiguous()
-    val = (qd, kd, vd, inv_q, inv_kv)
-    cross_attn.__dict__["_pcv_fp8_scales"] = (key, val)
-    return val
+    tensors = [qn.weight, qn.bias] + _params(kvn, (attn.q_proj, attn.k_proj, attn.v_proj))
+
+    def build():
+        qd = ops.fp8_descales(qn.weight, qn.bias, attn.q_proj.weight, attn.q_proj.bias, H)
+        kd = ops.fp8_descales(kvn.weight, kvn.bias, attn.k_proj.weight, attn.k_proj.bias, H)
+        vd = ops.fp8_descales(kvn.weight, kvn.bias, attn.v_proj.weight, attn.v_proj.bias, H, per_channel=True)
+        inv_q = (1.0 / qd).repeat_interleave(attn.q_proj.out_features // H).contiguous()
+        inv_kv = torch.cat([(1.0 / kd).repeat_interleave(attn.k_proj.out_features // H),
+                            (1.0 / vd).reshape(-1)]).contiguous()
+        return qd, kd, vd, inv_q, inv_kv
+
+    return _weight_cache(cross_attn, "_pcv_fp8_scales", tensors, dtype, build)
 
 
 def _fp8_cross_attention(cross_attn, x_q, x_kv, pad_mask, rot_pos_emb_q, rot_pos_emb_k, kv_cache):
@@ -406,19 +401,9 @@ def _fp8_cross_attention(cross_attn, x_q, x_kv, pad_mask, rot_pos_emb_q, rot_pos
     dqk, dv = n_q // H, n_v // H
     if dqk % 16 or dv % 16 or dqk > 256 or dv > 512:
         return None
-    for norm, x, lins in ((cross_attn.q_norm, x_q, [attn.q_proj]), (cross_attn.kv_norm, x_kv, [attn.k_proj, attn.v_proj])):
-        if not isinstance(norm, nn.LayerNorm) or norm.weight is None:
-            return None
-        if not x.is_cuda or x.dtype not in (torch.bfloat16, torch.float16) or len(norm.normalized_shape) != 1:
-            return None
-        if norm.normalized_shape[0] != x.shape[-1] or any(l.weight.dtype != x.dtype or l.in_features != x.shape[-1]
-                                                          for l in lins):
-            return None
-        if torch.is_autocast_enabled():
-            return None
-        if torch.is_grad_enabled() and (x.requires_grad or norm.weight.requires_grad
-                                        or any(l.weight.requires_grad for l in lins)):
-            return None
+    chains = ((cross_attn.q_norm, x_q, [attn.q_proj]), (cross_attn.kv_norm, x_kv, [attn.k_proj, attn.v_proj]))
+    if not all(_covered(x, n, lins) and _has_affine(n) and not _needs_grad(x, n, lins) for n, x, lins in chains):
+        return None
     if not (ops.kv_project_fp8_supported(x_q, n_q, 0, H) and ops.kv_project_fp8_supported(x_kv, n_k, n_v, H)):
         return None
     qd, kd, vd, inv_q, inv_kv = _fp8_scales(cross_attn, x_kv.dtype)
@@ -541,6 +526,8 @@ class SelfAttention(nn.Module):
             return attend(self.attention, qkv[0], qkv[1], qkv[2], pad_mask, rot_pos_emb, rot_pos_emb, kv_cache,
                           min_rows_key="min_rows_latent", kv8=kv8)
         x = self.norm(x)
+        # a module call, so that hooks and wrappers (FSDP) see it
+        # its o_proj gates on min_rows, not min_rows_latent: moving that would change the launch counts of eager latents
         return self.attention(x, x, pad_mask=pad_mask, rot_pos_emb_q=rot_pos_emb, rot_pos_emb_k=rot_pos_emb,
                               kv_cache=kv_cache)
 

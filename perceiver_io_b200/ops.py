@@ -773,6 +773,32 @@ def rescale_partial_(part_o: torch.Tensor, part_m: torch.Tensor, part_l: torch.T
         check(_lib.lib().pcv_partial_rescale(C.byref(p), _stream()), "pcv_partial_rescale")
 
 
+def _rotary_params(x: torch.Tensor, y: torch.Tensor, num_heads: int, angles: torch.Tensor, right_align: bool,
+                   dtype: int) -> RotaryParams:
+    """RotaryParams of y <- rotate(x), x and y (B, n, H*d), angles as :func:`_rotary_angles` leaves them."""
+    B, n, Cx = x.shape
+    d = Cx // num_heads
+    p = RotaryParams()
+    p.x, p.y, p.angles = x.data_ptr(), y.data_ptr(), angles.data_ptr()
+    p.x_stride_b, p.x_stride_n, p.x_stride_h = x.stride(0), x.stride(1), d
+    p.y_stride_b, p.y_stride_n, p.y_stride_h = y.stride(0), y.stride(1), d
+    p.a_stride_b = 0 if (angles.shape[0] == 1 and B > 1) else angles.stride(0)
+    p.a_stride_n = angles.stride(1)
+    p.B, p.n, p.H, p.d = B, n, num_heads, d
+    p.rotate_dim = angles.shape[-1]
+    p.angle_row0 = (angles.shape[1] - n) if right_align else 0
+    p.dtype = dtype
+    return p
+
+
+def _rotary_angles(angles: torch.Tensor) -> torch.Tensor:
+    """``frq_pos_enc`` (B or 1, [1,] n_angles, f) as the rotary kernels take it: 3-D float32, unit stride."""
+    if angles.dim() == 4:  # (B, 1, n, f) as stored by RotaryPositionEmbedding
+        angles = angles[:, 0]
+    angles = angles.float()
+    return angles if angles.stride(-1) == 1 else angles.contiguous()
+
+
 def _rotary_forward(x: torch.Tensor, num_heads: int, angles: torch.Tensor, right_align: bool,
                     out: Optional[torch.Tensor] = None) -> torch.Tensor:
     _require_cuda(x, angles)
@@ -780,8 +806,6 @@ def _rotary_forward(x: torch.Tensor, num_heads: int, angles: torch.Tensor, right
     cdt = _compute_dtype(x.dtype)
     x = _rows_contiguous(x if x.dtype == cdt else x.to(cdt))
     B, n, Cx = x.shape
-    d = Cx // num_heads
-    Ba, n_angles, f = angles.shape
     if out is not None:
         if out.shape != x.shape or out.dtype != cdt or out.stride(2) != 1:
             raise ValueError("rotary: `out` must match x in shape and compute dtype with unit channel stride")
@@ -790,16 +814,7 @@ def _rotary_forward(x: torch.Tensor, num_heads: int, angles: torch.Tensor, right
         y = torch.empty(B, n, Cx, dtype=cdt, device=x.device)
     if n == 0:
         return y if out is not None else y.to(out_dtype)
-    p = RotaryParams()
-    p.x, p.y, p.angles = x.data_ptr(), y.data_ptr(), angles.data_ptr()
-    p.x_stride_b, p.x_stride_n, p.x_stride_h = x.stride(0), x.stride(1), d
-    p.y_stride_b, p.y_stride_n, p.y_stride_h = y.stride(0), y.stride(1), d
-    p.a_stride_b = 0 if (Ba == 1 and B > 1) else angles.stride(0)
-    p.a_stride_n = angles.stride(1)
-    p.B, p.n, p.H, p.d = B, n, num_heads, d
-    p.rotate_dim = f
-    p.angle_row0 = (n_angles - n) if right_align else 0
-    p.dtype = _pcv_dtype(cdt)
+    p = _rotary_params(x, y, num_heads, angles, right_align, _pcv_dtype(cdt))
     with torch.cuda.device(x.device):
         check(_lib.lib().pcv_rotary_apply(C.byref(p), _stream()), "pcv_rotary_apply")
     if out is not None:
@@ -843,11 +858,7 @@ def rotary(x: torch.Tensor, num_heads: int, angles: torch.Tensor, right_align: b
     ``angles`` is the reference's ``frq_pos_enc`` (B or 1, n_angles, rotate_dim); row selection follows
     /root/reference/perceiver/model/core/position.py:32-37 (last n rows if right_align else first n)."""
     _require_cuda(x, angles)
-    if angles.dim() == 4:  # (B, 1, n, f) as stored by RotaryPositionEmbedding
-        angles = angles[:, 0]
-    angles = angles.float()
-    if angles.stride(-1) != 1:
-        angles = angles.contiguous()
+    angles = _rotary_angles(angles)
     B, n, _ = x.shape
     Ba, n_angles, _ = angles.shape
     if Ba not in (1, B):
@@ -1040,18 +1051,7 @@ def _rotary_fp8(x: torch.Tensor, num_heads: int, angles: torch.Tensor, y: torch.
                 x_descale: Optional[torch.Tensor] = None, right_align: bool = False) -> None:
     """y (B, n, H*d) e4m3 <- e4m3(rotate(x) * y_inv_scale[h]) (pcv_rotary_apply_fp8).  x is bf16 / fp16, or e4m3 codes
     standing for ``x * x_descale[h]``; ``angles`` (B or 1, n_angles, f) float32, rows as in :func:`rotary`."""
-    B, n, Cx = x.shape
-    d = Cx // num_heads
-    p = RotaryParams()
-    p.x, p.y, p.angles = x.data_ptr(), y.data_ptr(), angles.data_ptr()
-    p.x_stride_b, p.x_stride_n, p.x_stride_h = x.stride(0), x.stride(1), d
-    p.y_stride_b, p.y_stride_n, p.y_stride_h = y.stride(0), y.stride(1), d
-    p.a_stride_b = 0 if (angles.shape[0] == 1 and B > 1) else angles.stride(0)
-    p.a_stride_n = angles.stride(1)
-    p.B, p.n, p.H, p.d = B, n, num_heads, d
-    p.rotate_dim = angles.shape[-1]
-    p.angle_row0 = (angles.shape[1] - n) if right_align else 0
-    p.dtype = _lib.PCV_E4M3 if x.dtype == F8 else _pcv_dtype(x.dtype)
+    p = _rotary_params(x, y, num_heads, angles, right_align, _lib.PCV_E4M3 if x.dtype == F8 else _pcv_dtype(x.dtype))
     f = _lib.RotaryFp8()
     f.x_descale = None if x_descale is None else x_descale.data_ptr()
     f.y_inv_scale = y_inv_scale.data_ptr()
@@ -1068,11 +1068,7 @@ def rotary_fp8(x8: torch.Tensor, num_heads: int, angles: torch.Tensor, right_ali
     _require_cuda(x8, angles, descale)
     if x8.dtype != F8:
         raise ValueError(f"rotary_fp8: x8 must be torch.float8_e4m3fn, got {x8.dtype}")
-    if angles.dim() == 4:  # (B, 1, n, f) as stored by RotaryPositionEmbedding
-        angles = angles[:, 0]
-    angles = angles.float()
-    if angles.stride(-1) != 1:
-        angles = angles.contiguous()
+    angles = _rotary_angles(angles)
     B, n, _ = x8.shape
     if angles.shape[0] not in (1, B) or angles.shape[1] < n:
         raise ValueError(f"rotary_fp8: angles {tuple(angles.shape)} do not cover x8 {tuple(x8.shape)}")
@@ -1334,6 +1330,28 @@ def _fill_kvproj(x2, w_cat, col_st, n_k, n_v, stats, k_out, v_out, cta_group=0, 
     return p
 
 
+def _check_folded(fn: str, x: torch.Tensor, w_cat: torch.Tensor, col_st: torch.Tensor, n: int) -> None:
+    if w_cat.dtype != x.dtype or w_cat.shape != (n, x.shape[-1]) or not w_cat.is_contiguous():
+        raise ValueError(f"{fn}: w_cat must be a contiguous (n_k + n_v, C) tensor in x's dtype")
+    if col_st.dtype != torch.float32 or col_st.shape != (n, 2) or not col_st.is_contiguous():
+        raise ValueError(f"{fn}: col_st must be a contiguous (n_k + n_v, 2) float32 tensor")
+
+
+def _producer_stats(x2: torch.Tensor, eps: Optional[float], mode: str):
+    """``(row statistics, ln_eps)`` of the producer's LayerNorm (``eps`` None: none): pcv_ln_stats, or in-kernel."""
+    fused = eps is not None and mode == "fused"
+    return (None if eps is None or fused else ln_stats(x2, eps)), (eps if fused else 0.0)
+
+
+def _project_rows(x2: torch.Tensor, w_cat, col_st, n_k: int, n_v: int, stats, ln_eps=0.0, cta_group: int = 0):
+    """pcv_kv_project of x2 (rows, C): new (rows, n_k) and (rows, n_v) tensors in x2's dtype (None for a width of 0)."""
+    k_out = torch.empty(x2.shape[0], n_k, dtype=x2.dtype, device=x2.device) if n_k else None
+    v_out = torch.empty(x2.shape[0], n_v, dtype=x2.dtype, device=x2.device) if n_v else None
+    p = _fill_kvproj(x2, w_cat, col_st, n_k, n_v, stats, k_out, v_out, cta_group, ln_eps)
+    check(_lib.lib().pcv_kv_project(C.byref(p), _stream()), "pcv_kv_project")
+    return k_out, v_out
+
+
 def kv_project_supported(x: torch.Tensor, n_k: int, n_v: int) -> bool:
     """True when ``kv_project`` covers (x, n_k, n_v): CUDA bf16/fp16 rows, widths/strides TMA can address."""
     if not x.is_cuda or x.dtype not in (torch.bfloat16, torch.float16) or x.numel() == 0:
@@ -1356,23 +1374,13 @@ def kv_project(x: torch.Tensor, w_cat: torch.Tensor, col_st: torch.Tensor, n_k: 
     ``w_cat`` / ``col_st`` come from :func:`fold_ln_linear`; ``eps=None`` skips the LayerNorm (plain projection).
     Returns contiguous (..., n_k) and (..., n_v) tensors in x's dtype (``None`` for a width of 0)."""
     _require_cuda(x, w_cat, col_st)
-    if w_cat.dtype != x.dtype or w_cat.shape != (n_k + n_v, x.shape[-1]) or not w_cat.is_contiguous():
-        raise ValueError("kv_project: w_cat must be a contiguous (n_k + n_v, C) tensor in x's dtype")
-    if col_st.dtype != torch.float32 or col_st.shape != (n_k + n_v, 2) or not col_st.is_contiguous():
-        raise ValueError("kv_project: col_st must be a contiguous (n_k + n_v, 2) float32 tensor")
+    _check_folded("kv_project", x, w_cat, col_st, n_k + n_v)
     lead = x.shape[:-1]
     x2 = _rows2d(x)
-    mode = kv_project_config["stats"] if stats is None else stats
     with torch.cuda.device(x.device):
-        st = ln_stats(x2, eps) if (eps is not None and mode != "fused") else None
-        k_out = torch.empty(x2.shape[0], n_k, dtype=x.dtype, device=x.device) if n_k else None
-        v_out = torch.empty(x2.shape[0], n_v, dtype=x.dtype, device=x.device) if n_v else None
-        p = _fill_kvproj(x2, w_cat, col_st, n_k, n_v, st, k_out, v_out, cta_group,
-                         ln_eps=(eps if (eps is not None and mode == "fused") else 0.0))
-        check(_lib.lib().pcv_kv_project(C.byref(p), _stream()), "pcv_kv_project")
-    k = None if k_out is None else k_out.view(*lead, n_k)
-    v = None if v_out is None else v_out.view(*lead, n_v)
-    return k, v
+        st, ln_eps = _producer_stats(x2, eps, kv_project_config["stats"] if stats is None else stats)
+        k_out, v_out = _project_rows(x2, w_cat, col_st, n_k, n_v, st, ln_eps, cta_group)
+    return tuple(None if o is None else o.view(*lead, o.shape[1]) for o in (k_out, v_out))
 
 
 def fp8_quantize(x: torch.Tensor, descale: torch.Tensor, num_heads: int) -> torch.Tensor:
@@ -1399,8 +1407,6 @@ def fp8_transpose_v(v8: torch.Tensor, num_heads: int, m_pad: Optional[int] = Non
 
 def _fill_kvproj_fp8(x2, w_cat, col_st, inv_scale, n_k, n_v, stats, k8, vt8, keys_per_batch, v_head_dim, ln_eps):
     p = _fill_kvproj(x2, w_cat, col_st, n_k, n_v, stats, k8, None, 0, ln_eps)
-    p.k_stride_row = n_k
-    p.v_stride_row = 0
     f = _lib.KvProjFp8()
     f.inv_scale = inv_scale.data_ptr()
     if vt8 is not None:
@@ -1445,26 +1451,21 @@ def kv_project_fp8(x: torch.Tensor, w_cat: torch.Tensor, col_st: torch.Tensor, i
     _require_cuda(x, w_cat, col_st, inv_scale)
     if x.dim() != 3:
         raise ValueError("kv_project_fp8: x must be (B, M, C)")
-    if w_cat.dtype != x.dtype or w_cat.shape != (n_k + n_v, x.shape[-1]) or not w_cat.is_contiguous():
-        raise ValueError("kv_project_fp8: w_cat must be a contiguous (n_k + n_v, C) tensor in x's dtype")
-    if col_st.dtype != torch.float32 or col_st.shape != (n_k + n_v, 2) or not col_st.is_contiguous():
-        raise ValueError("kv_project_fp8: col_st must be a contiguous (n_k + n_v, 2) float32 tensor")
+    _check_folded("kv_project_fp8", x, w_cat, col_st, n_k + n_v)
     inv = inv_scale.float().contiguous()
     if inv.shape != (n_k + n_v,):
         raise ValueError("kv_project_fp8: inv_scale must be (n_k + n_v,)")
     B, M, _ = x.shape
     x2 = _rows2d(x)
-    mode = kv_project_config["stats"]
     dv = n_v // num_heads if n_v else 16
     with torch.cuda.device(x.device):
-        st = ln_stats(x2, eps) if (eps is not None and mode != "fused") else None
+        st, ln_eps = _producer_stats(x2, eps, kv_project_config["stats"])
         k8 = torch.empty(B * M, n_k, dtype=torch.float8_e4m3fn, device=x.device) if n_k else None
         vt8 = None
         if n_v:
             m_pad = (M + 15) // 16 * 16
             vt8 = torch.empty(B, num_heads, dv, m_pad, dtype=torch.float8_e4m3fn, device=x.device)  # pad keys: never read
-        p, f = _fill_kvproj_fp8(x2, w_cat, col_st, inv, n_k, n_v, st, k8, vt8, M, dv,
-                                eps if (eps is not None and mode == "fused") else 0.0)
+        p, f = _fill_kvproj_fp8(x2, w_cat, col_st, inv, n_k, n_v, st, k8, vt8, M, dv, ln_eps)
         check(_lib.lib().pcv_kv_project_fp8(C.byref(p), C.byref(f), _stream()), "pcv_kv_project_fp8")
     return (None if k8 is None else k8.view(B, M, n_k)), vt8
 
@@ -1532,10 +1533,7 @@ class _LnLinear(torch.autograd.Function):
         x2 = _rows2d(x)
         with torch.cuda.device(x.device):
             st = ln_stats(x2, eps)
-            k_out = torch.empty(x2.shape[0], n_k, dtype=x.dtype, device=x.device) if n_k else None
-            v_out = torch.empty(x2.shape[0], n_v, dtype=x.dtype, device=x.device) if n_v else None
-            p = _fill_kvproj(x2, w_cat, col_st, n_k, n_v, st, k_out, v_out)
-            check(_lib.lib().pcv_kv_project(C.byref(p), _stream()), "pcv_kv_project")
+            k_out, v_out = _project_rows(x2, w_cat, col_st, n_k, n_v, st)
         ctx.save_for_backward(x2, st, w, gamma, beta)
         ctx.dims = (x.shape, n_k, n_v, b is not None)
         outs = [o.view(*lead, o.shape[1]) for o in (k_out, v_out) if o is not None]

@@ -110,8 +110,110 @@ def run(root: str, out_path: str) -> None:
                     record(f"{tag} attention_fp8 partial={partial}",
                            lambda partial=partial: ops.attention_fp8(q8, k8, vt8, qd, kd, vd, H, scale, partial=partial,
                                                                      **kw))
+    _modules(record)
     torch.save(results, out_path)
     print(f"{len(results)} calls -> {out_path}")
+
+
+def _modules(record):
+    """The modules' routing (modules.py): seeded module calls recording the output, the parameter and input gradients
+    of autograd calls (held as fp32-atomics results: they sit downstream of grad_q), the returned caches and their
+    dtypes, and, as the fingerprint of the routes taken, the ``_pcv_*`` slots each module holds afterwards."""
+    import perceiver_io_b200 as P
+    from perceiver_io_b200 import modules
+
+    dev = "cuda"
+
+    def fresh(model):
+        for m in model.modules():
+            for k in [k for k in m.__dict__ if k.startswith("_pcv_")]:
+                del m.__dict__[k]
+        return model
+
+    def slots(model):
+        return sorted(f"{n}.{k}" for n, m in model.named_modules() for k in m.__dict__ if k.startswith("_pcv_"))
+
+    def call(name, model, inputs, grad=False, seed=0, autocast=False):
+        def fn():
+            fresh(model).zero_grad(set_to_none=True)
+            ins = [t.detach().clone().requires_grad_(grad) for t in inputs]
+            torch.manual_seed(seed)
+            with torch.set_grad_enabled(grad), torch.autocast("cuda", dtype=torch.bfloat16, enabled=autocast):
+                out = model(*ins).last_hidden_state
+            if not grad:
+                return [out, slots(model)]
+            out.float().square().sum().backward()
+            grads = [p.grad for _, p in sorted(model.named_parameters())] + [t.grad for t in ins]
+            return [out, slots(model)] + grads
+        n_grads = len(list(model.parameters())) + len(inputs) if grad else 0
+        record(f"modules {name}", fn, atomic=tuple(range(2, 2 + n_grads)))
+
+    def cross(dtype, dropout=0.0):
+        torch.manual_seed(1)
+        return P.CrossAttention(num_heads=4, num_q_input_channels=256, num_kv_input_channels=512,
+                                dropout=dropout).to(dev, dtype)
+
+    g = torch.Generator().manual_seed(SEED + 1)
+    x_q = torch.randn(1, 256, 256, generator=g).to(dev)
+    for M in (256, 1024):
+        x_kv = torch.randn(2, M, 512, generator=g).to(dev)
+        for dtype in (torch.bfloat16, torch.float32):
+            call(f"CrossAttention eval M={M} {str(dtype)[6:]}", cross(dtype).eval(), [x_q.to(dtype), x_kv.to(dtype)])
+        call(f"CrossAttention eval M={M} autocast", cross(torch.float32).eval(), [x_q, x_kv], autocast=True)
+        modules.fp8_config["enabled"] = True
+        try:
+            call(f"CrossAttention eval M={M} fp8", cross(torch.bfloat16).eval(), [x_q.bfloat16(), x_kv.bfloat16()])
+        finally:
+            modules.fp8_config["enabled"] = False
+    x_kv = x_kv.bfloat16()
+    for training in (False, True):
+        for p in (0.0, 0.1):
+            modules.kv_producer_config["training"] = training
+            try:
+                call(f"CrossAttention train route={training} p={p}", cross(torch.bfloat16, p).train(),
+                     [x_q.bfloat16(), x_kv], grad=True, seed=3)
+            finally:
+                modules.kv_producer_config["training"] = False
+
+    for n in (128, 512, 2048):  # 256, 1024 and 4096 latent rows: below min_rows, the eager band, min_rows_latent
+        torch.manual_seed(2)
+        sa = P.SelfAttention(num_heads=4, num_channels=256).to(dev, torch.bfloat16)
+        x = torch.randn(2, n, 256, generator=g).to(dev, torch.bfloat16)
+        call(f"SelfAttention eval rows={2 * n}", sa.eval(), [x])
+        for training in (False, True):
+            modules.kv_producer_config["training"] = training
+            try:
+                call(f"SelfAttention train rows={2 * n} route={training}", sa.train(), [x], grad=True)
+            finally:
+                modules.kv_producer_config["training"] = False
+
+    torch.manual_seed(4)
+    cfg = P.CausalSequenceModelConfig(vocab_size=64, max_seq_len=96, max_latents=32, num_channels=128, num_heads=4,
+                                      num_self_attention_layers=2, cross_attention_dropout=0.0)
+    model = P.CausalSequenceModel(cfg).to(dev, torch.bfloat16).eval()
+    tokens = torch.randint(0, 64, (2, 64 + 16), generator=g).to(dev)
+
+    def generate():
+        fresh(model)
+        with torch.no_grad():
+            out = model(tokens[:, :64], prefix_len=32, kv_cache=[])
+            logits, cache, pos = [out.logits], out.kv_cache, 64
+            for step in range(8):
+                m = 5 if step == 3 else 1
+                if step == 5:  # beam reordering
+                    cache = [(k.index_select(0, torch.tensor([1, 0], device=dev)),
+                              v.index_select(0, torch.tensor([1, 0], device=dev))) for k, v in cache]
+                out = model(tokens[:, pos:pos + m], prefix_len=32, kv_cache=cache)
+                logits.append(out.logits)
+                cache, pos = out.kv_cache, pos + m
+        return logits + [t for kv in cache for t in kv] + [[str(k.dtype) for k, _ in cache], slots(model)]
+
+    for kv8 in (False, True):
+        modules.fp8_config["kv_cache"] = kv8
+        try:
+            record(f"modules CausalSequenceModel decode kv8={kv8}", generate)
+        finally:
+            modules.fp8_config["kv_cache"] = False
 
 
 def _same(a, b):
