@@ -266,10 +266,14 @@ __global__ void __launch_bounds__(kTailThreads) peer_tail_kernel(const TcParams 
 #undef PCV_TAIL_STAMP
 }
 
+// The pipelined schedule (NQB <= 2) uses a multiple of NQB + NVB ring slots: every key tile then starts at a ring
+// index that is a multiple of NQB + NVB, so the V boxes of a tile are adjacent slots that never wrap and one
+// m64n128 wgmma reads both (issue_pv).
 template <int NQB, int NVB>
 struct FwdCfg {
   static constexpr int kQBytes = NQB * kBoxBytes;
-  static constexpr int kSlots = (kSmemLimit - kQBytes - 2048) / kBoxBytes > 16 ? 16 : (kSmemLimit - kQBytes - 2048) / kBoxBytes;
+  static constexpr int kFit = (kSmemLimit - kQBytes - 2048) / kBoxBytes > 16 ? 16 : (kSmemLimit - kQBytes - 2048) / kBoxBytes;
+  static constexpr int kSlots = NQB <= 2 ? kFit / (NQB + NVB) * (NQB + NVB) : kFit;
   static constexpr int kSmemBytes = kQBytes + kSlots * kBoxBytes + 2048;  // + barriers + 1024-byte alignment slack
   static_assert(kSlots >= 2, "shared memory budget");
 };
@@ -287,38 +291,64 @@ struct FwdBarriers {
 // statistics stay those of the dropout-free softmax; the survivors are scaled once, in the epilogue).  `qside` is the
 // query side of the mask hash of rows n0 and n0 + 8; each thread hashes once per row and key pair (jb, jb + 1).
 // FP8: the scores are scaled by `fp8_scale_log2` (p.scale_log2 * q_descale[h] * k_descale[h]) instead of p.scale_log2.
+// The scale c is folded into the exponent, 2^(s c - m) with the raw score s, and the row maximum is taken on the raw
+// scores: c > 0 (attn_tc_supported) and rounding is monotonic, so the raw maximum times c is exactly the maximum of the
+// scaled scores.  Where a thread holds a padded or causally masked score of a row in the tile, it writes that row's
+// scores scaled and masked (the finite fill kMaskedScore) and takes 2^(x - m) instead.  Which formula a score gets
+// depends on the masked set alone, so an all-false pad mask gives the unmasked result bit for bit.
 template <bool DROP, bool FP8 = false>
 __device__ __forceinline__ void tile_softmax(float (&s)[64], float (&m_run)[2], float (&l_run)[2], float (&alpha)[2],
                                              const TcParams& p, int b, int j0, int n0, int cq, bool interior,
                                              const uint32_t (&qside)[2], float fp8_scale_log2 = 0.f) {
+  const float c = FP8 ? fp8_scale_log2 : p.scale_log2;
   float mx[2] = {-INFINITY, -INFINITY};
+  bool filled[2] = {false, false};  // this thread holds a padded or causally masked score of row r
   if (interior) {
+    // four independent chains per row: one chain of 32 dependent FMNMX would put its latency on the critical path
+    float m4[2][4] = {{-INFINITY, -INFINITY, -INFINITY, -INFINITY}, {-INFINITY, -INFINITY, -INFINITY, -INFINITY}};
 #pragma unroll
-    for (int i = 0; i < 64; ++i) {
-      s[i] *= (FP8 ? fp8_scale_log2 : p.scale_log2);
-      mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], s[i]);
-    }
+    for (int i = 0; i < 64; ++i) m4[(i >> 1) & 1][((i >> 2) & 1) * 2 + (i & 1)] = fmaxf(m4[(i >> 1) & 1][((i >> 2) & 1) * 2 + (i & 1)], s[i]);
+#pragma unroll
+    for (int r = 0; r < 2; ++r) mx[r] = fmaxf(fmaxf(m4[r][0], m4[r][1]), fmaxf(m4[r][2], m4[r][3]));
   } else {
+    // element e of the 8-key group g: 0 live, 1 padded or causally masked, 2 past M
+    auto pad_word = [&](int g) { return p.pad_bits != nullptr ? p.pad_bits[(int64_t)b * p.pad_wpr + ((j0 + 8 * g + cq) >> 5)] : 0u; };
+    auto kind = [&](int g, int e, uint32_t padw) {
+      const int j = j0 + 8 * g + cq + (e & 1);
+      if (j >= p.M) return 2;
+      return (((padw >> (j & 31)) & 1u) || (p.causal && j > n0 + 8 * (e >> 1) + p.causal_shift)) ? 1 : 0;
+    };
 #pragma unroll
     for (int g = 0; g < 16; ++g) {
-      const int jb = j0 + 8 * g + cq;
-      uint32_t padw = 0;
-      if (p.pad_bits != nullptr) padw = p.pad_bits[(int64_t)b * p.pad_wpr + (jb >> 5)];
+      const uint32_t padw = pad_word(g);
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
-        const int j = jb + (e & 1);
-        const int n = n0 + 8 * (e >> 1);
-        float x = s[4 * g + e] * (FP8 ? fp8_scale_log2 : p.scale_log2);
-        if (j >= p.M) x = -INFINITY;
-        else if (((padw >> (j & 31)) & 1u) || (p.causal && j > n + p.causal_shift)) x = kMaskedScore;
-        s[4 * g + e] = x;
-        mx[e >> 1] = fmaxf(mx[e >> 1], x);
+        const int kd = kind(g, e, padw);
+        if (kd == 0) mx[e >> 1] = fmaxf(mx[e >> 1], s[4 * g + e]);
+        else if (kd == 2) s[4 * g + e] = -INFINITY;
+        else filled[e >> 1] = true;
+      }
+    }
+    if (filled[0] || filled[1]) {
+#pragma unroll
+      for (int g = 0; g < 16; ++g) {
+        const uint32_t padw = pad_word(g);
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+          if (filled[e >> 1]) {
+            const int kd = kind(g, e, padw);
+            if (kd == 0) s[4 * g + e] *= c;
+            else if (kd == 1) s[4 * g + e] = kMaskedScore;
+          }
       }
     }
   }
-  float mref[2];
+  float mref[2], cr[2];  // the exponent of score s of row r is s * cr[r] - mref[r]
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
+    mx[r] *= c;
+    if (filled[r]) mx[r] = fmaxf(mx[r], kMaskedScore);
+    cr[r] = filled[r] ? 1.f : c;
     mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
     mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
     const float mn = fmaxf(m_run[r], mx[r]);
@@ -327,12 +357,13 @@ __device__ __forceinline__ void tile_softmax(float (&s)[64], float (&m_run)[2], 
     m_run[r] = mn;
     l_run[r] *= alpha[r];
   }
+  float lsum[2][2] = {{0.f, 0.f}, {0.f, 0.f}};  // two partial row sums: half the dependent FADD chain
 #pragma unroll
   for (int g = 0; g < 16; ++g) {
-    float e0 = ex2(s[4 * g + 0] - mref[0]), e1 = ex2(s[4 * g + 1] - mref[0]);
-    float e2 = ex2(s[4 * g + 2] - mref[1]), e3 = ex2(s[4 * g + 3] - mref[1]);
-    l_run[0] += e0 + e1;
-    l_run[1] += e2 + e3;
+    float e0 = ex2(fmaf(s[4 * g + 0], cr[0], -mref[0])), e1 = ex2(fmaf(s[4 * g + 1], cr[0], -mref[0]));
+    float e2 = ex2(fmaf(s[4 * g + 2], cr[1], -mref[1])), e3 = ex2(fmaf(s[4 * g + 3], cr[1], -mref[1]));
+    lsum[0][g & 1] += e0 + e1;
+    lsum[1][g & 1] += e2 + e3;
     if constexpr (DROP) {
       const uint32_t jb = (uint32_t)(p.drop_key_base + j0 + 8 * g + cq), n = (uint32_t)n0;
       const uint32_t ks = drop_kside(p.drop.seed_hi, jb);
@@ -347,6 +378,8 @@ __device__ __forceinline__ void tile_softmax(float (&s)[64], float (&m_run)[2], 
     s[4 * g + 2] = e2;
     s[4 * g + 3] = e3;
   }
+  l_run[0] += lsum[0][0] + lsum[0][1];
+  l_run[1] += lsum[1][0] + lsum[1][1];
 }
 
 // probabilities -> the 16-bit A fragments of the P V wgmma (k-step kk covers keys [16 kk, 16 kk + 16))
@@ -384,8 +417,11 @@ __device__ __forceinline__ void pack_p_e4m3(const float (&s)[64], uint32_t (&pa)
     }
 }
 
+// Skipped when no row of the warp moved its maximum (alpha is exactly 1, and o * 1 is o): after the first few key tiles
+// that is the common case.
 template <int NVB>
 __device__ __forceinline__ void rescale_o(float (&o)[NVB][32], const float (&alpha)[2]) {
+  if (__all_sync(0xffffffffu, alpha[0] == 1.f && alpha[1] == 1.f)) return;
 #pragma unroll
   for (int v = 0; v < NVB; ++v)
 #pragma unroll
@@ -412,6 +448,7 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
   // keep the serial schedule (per box: wait, issue, drain, release).
   constexpr bool kPipelined = NQB <= 2;
   static_assert(!kPipelined || NQB + KVB <= NS, "the pipelined schedule holds NQB + KVB ring slots");
+  static_assert(!kPipelined || NS % (NQB + KVB) == 0, "a key tile's V boxes must not wrap around the ring");
   // registers per thread: producer + 2 x consumer = 504 = the launch bound's 168 x 3; the pipelined consumers keep
   // S, P and O live at once, the serial schedule's producer (ring index arithmetic by a non-power-of-two) spills at 24
   constexpr int kProducerRegs = kPipelined ? 24 : 40, kConsumerRegs = kPipelined ? 240 : 232;
@@ -526,12 +563,14 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk)
           wgmma_rs_e4m3_n64(o[v], pa[kk], make_desc(ring_base + i % NS * kBoxBytes + v * 8192 + kk * 32));
+    } else if constexpr (NVB == 2) {  // both V boxes in one m64n128 per k16 step (adjacent slots, see FwdCfg)
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk)
+        wgmma_rs<128, BF16>(reinterpret_cast<float(&)[64]>(o), pa[kk],
+                            make_desc(ring_base + i % NS * kBoxBytes + kk * 2048, kBoxBytes));
     } else {
 #pragma unroll
-      for (int v = 0; v < NVB; ++v)
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk)
-          wgmma_rs<64, BF16>(o[v], pa[kk], make_desc(ring_base + (i + v) % NS * kBoxBytes + kk * 2048));
+      for (int kk = 0; kk < 8; ++kk) wgmma_rs<64, BF16>(o[0], pa[kk], make_desc(ring_base + i % NS * kBoxBytes + kk * 2048));
     }
     wgmma_commit();
   };
