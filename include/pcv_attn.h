@@ -542,6 +542,50 @@ PCV_API int pcv_rotary_fp8_supported(const pcv_rotary_params* p, const pcv_rotar
 PCV_API int pcv_rotary_apply_fp8(const pcv_rotary_params* p, const pcv_rotary_fp8* f, void* stream);
 
 /*
+ * Device-resident rows: the entry points below read the rows they work on from device memory when the kernel runs, so
+ * one recorded CUDA graph serves every step of a decode loop whose lengths change each token.  Every pointer and size
+ * in their params is fixed for the life of a graph; only the int32s behind `bounds` change (in-graph tensor ops write
+ * them).  None of these entry points synchronises or reads device memory on the host.
+ *
+ * pcv_attn_decode_window (_fp8): the streaming decode kernel on the key window [bounds[0], bounds[1]) of an arena.
+ * k, v and pad_mask point at arena row 0 and M == capacity (the arena's rows); pad bytes are indexed by the absolute
+ * arena row.  The split count is planned on the host from `capacity`, so the grid and the workspace
+ * (pcv_attn_decode_window_workspace_bytes) do not depend on the window; each split takes an equal share of the window's
+ * keys when the kernel runs.  The causal mask is right-aligned to the window's end: query i sits at row end - N + i.
+ * Any window length >= 1 is valid (the pcv_attn_fwd decode kernel's 1024-key floor does not apply); a window of length
+ * <= 0 writes zeros.  The window is clamped to [0, capacity).  N <= 4, head dims multiples of 8 (bf16 / fp16 rows) or
+ * 16 (e4m3 rows, with pcv_decode_fp8 as in pcv_attn_decode_fp8) and at most 256; no write_partial, no key shard.
+ *
+ * pcv_kv_append_at (_fp8): pcv_kv_append (_fp8) of the n new rows to arena rows bounds[0] .. bounds[0] + n - 1, with
+ * k_cache = v_cache = NULL and L_old = 0; k_dst / v_dst point at arena row 0.  Rows that would land at or past
+ * `capacity` are skipped.
+ *
+ * pcv_rotary_apply_at (_fp8): pcv_rotary_apply (_fp8) with the angle rows of a precomputed (capacity, rotate_dim) fp32
+ * table (`angles`, a_stride_b = 0): input row i uses table row bounds[0] + i and is written to output row bounds[0] + i
+ * when bounds[1] != 0 (a new key rotated straight into a rotated-key arena), else to row i (q into a fixed buffer).
+ * angle_row0 is ignored; rows whose table row is at or past `capacity` are skipped.
+ */
+typedef struct pcv_dev_rows {
+  const int32_t* bounds;   /* device int32s; meaning per entry point above                  */
+  int32_t capacity;        /* rows of the arena (host-known, fixed for the life of a graph) */
+  int32_t reserved;
+} pcv_dev_rows;
+
+PCV_API int pcv_attn_decode_window_supported(const pcv_attn_params* p, const pcv_dev_rows* rows);
+PCV_API int pcv_attn_decode_window_workspace_bytes(const pcv_attn_params* p, size_t* bytes);
+PCV_API int pcv_attn_decode_window(const pcv_attn_params* p, const pcv_dev_rows* rows, void* stream);
+PCV_API int pcv_attn_decode_window_fp8_supported(const pcv_attn_params* p, const pcv_decode_fp8* f,
+                                                 const pcv_dev_rows* rows);
+PCV_API int pcv_attn_decode_window_fp8(const pcv_attn_params* p, const pcv_decode_fp8* f, const pcv_dev_rows* rows,
+                                       void* stream);
+PCV_API int pcv_kv_append_at(const pcv_kv_append_params* p, const pcv_dev_rows* rows, void* stream);
+PCV_API int pcv_kv_append_at_fp8(const pcv_kv_append_params* p, const pcv_kv_fp8_scales* f, const pcv_dev_rows* rows,
+                                 void* stream);
+PCV_API int pcv_rotary_apply_at(const pcv_rotary_params* p, const pcv_dev_rows* rows, void* stream);
+PCV_API int pcv_rotary_apply_at_fp8(const pcv_rotary_params* p, const pcv_rotary_fp8* f, const pcv_dev_rows* rows,
+                                    void* stream);
+
+/*
  * Backward of the LayerNorm -> Linear chain pcv_kv_project computes (training through kv_norm -> k_proj / v_proj,
  * q_norm -> q_proj, norm -> q/k/v_proj).  With x_hat = (x - mean) * rstd (row_stats of pcv_ln_stats),
  * y = x_hat * gamma + beta, out = y W^T + b, W = [W_k ; W_v] (n_k + n_v, C) and G = [grad_k | grad_v] (rows, n):

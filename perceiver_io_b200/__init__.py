@@ -10,6 +10,7 @@ Layout (tier scope: SURVEY.md §8 only):
   dist.py      M-sharded cross-attention across the GPUs of one box
   patch.py     swap the attention arithmetic inside an already-built reference model
   streaming.py host-resident K/V input pipelined against PCIe;  graphs.py  CUDA-graph capture of static-shape forwards
+  generation.py  graph-replayed Perceiver AR decoding (GraphedDecoder: one generated token = one graph replay)
 """
 from .utils import ModuleOutput, Residual, init_parameters, freeze  # noqa: F401
 from .position import positions, RotaryPositionEmbedding, FrequencyPositionEncoding  # noqa: F401
@@ -31,5 +32,6 @@ from .modules import (  # noqa: F401
 )
 from .config import PerceiverARConfig, CausalSequenceModelConfig  # noqa: F401
 from .patch import patch  # noqa: F401
+from .generation import GraphedDecoder, decode_windows  # noqa: F401
 
 __version__ = "0.1.0"

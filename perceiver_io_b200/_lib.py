@@ -64,6 +64,15 @@ EXPORTS = (
     "pcv_kv_append_fp8",
     "pcv_rotary_fp8_supported",
     "pcv_rotary_apply_fp8",
+    "pcv_attn_decode_window_supported",
+    "pcv_attn_decode_window_workspace_bytes",
+    "pcv_attn_decode_window",
+    "pcv_attn_decode_window_fp8_supported",
+    "pcv_attn_decode_window_fp8",
+    "pcv_kv_append_at",
+    "pcv_kv_append_at_fp8",
+    "pcv_rotary_apply_at",
+    "pcv_rotary_apply_at_fp8",
     "pcv_ln_linear_bwd_supported",
     "pcv_ln_linear_bwd_workspace_bytes",
     "pcv_ln_linear_bwd",
@@ -249,6 +258,10 @@ class RotaryFp8(C.Structure):
     _fields_ = [("x_descale", C.c_void_p), ("y_inv_scale", C.c_void_p)]
 
 
+class DevRows(C.Structure):
+    _fields_ = [("bounds", C.c_void_p), ("capacity", C.c_int32), ("reserved", C.c_int32)]
+
+
 class LnLinearBwdParams(C.Structure):
     _fields_ = [
         ("x", C.c_void_p), ("x_stride_row", C.c_int64), ("row_stats", C.c_void_p),
@@ -376,6 +389,20 @@ def lib() -> C.CDLL:
         l.pcv_rotary_fp8_supported.restype = C.c_int
         l.pcv_rotary_apply_fp8.argtypes = [C.POINTER(RotaryParams), C.POINTER(RotaryFp8), C.c_void_p]
         l.pcv_rotary_apply_fp8.restype = C.c_int
+        rows = C.POINTER(DevRows)
+        l.pcv_attn_decode_window_supported.argtypes = [C.POINTER(AttnParams), rows]
+        l.pcv_attn_decode_window_workspace_bytes.argtypes = [C.POINTER(AttnParams), C.POINTER(C.c_size_t)]
+        l.pcv_attn_decode_window.argtypes = [C.POINTER(AttnParams), rows, C.c_void_p]
+        l.pcv_attn_decode_window_fp8_supported.argtypes = [C.POINTER(AttnParams), C.POINTER(DecodeFp8), rows]
+        l.pcv_attn_decode_window_fp8.argtypes = [C.POINTER(AttnParams), C.POINTER(DecodeFp8), rows, C.c_void_p]
+        l.pcv_kv_append_at.argtypes = [C.POINTER(KvAppendParams), rows, C.c_void_p]
+        l.pcv_kv_append_at_fp8.argtypes = [C.POINTER(KvAppendParams), C.POINTER(KvFp8Scales), rows, C.c_void_p]
+        l.pcv_rotary_apply_at.argtypes = [C.POINTER(RotaryParams), rows, C.c_void_p]
+        l.pcv_rotary_apply_at_fp8.argtypes = [C.POINTER(RotaryParams), C.POINTER(RotaryFp8), rows, C.c_void_p]
+        for name in ("pcv_attn_decode_window_supported", "pcv_attn_decode_window_workspace_bytes",
+                     "pcv_attn_decode_window", "pcv_attn_decode_window_fp8_supported", "pcv_attn_decode_window_fp8",
+                     "pcv_kv_append_at", "pcv_kv_append_at_fp8", "pcv_rotary_apply_at", "pcv_rotary_apply_at_fp8"):
+            getattr(l, name).restype = C.c_int
         l.pcv_ln_linear_bwd_supported.argtypes = [C.POINTER(LnLinearBwdParams)]
         l.pcv_ln_linear_bwd_supported.restype = C.c_int
         l.pcv_ln_linear_bwd_workspace_bytes.argtypes = [C.POINTER(LnLinearBwdParams), C.POINTER(C.c_size_t)]

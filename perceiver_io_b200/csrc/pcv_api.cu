@@ -496,4 +496,72 @@ int pcv_rotary_apply_fp8(const pcv_rotary_params* p, const pcv_rotary_fp8* f, vo
   return launch_rotary_fp8(*p, *f, reinterpret_cast<cudaStream_t>(stream));
 }
 
+static int decode_window_supported(const pcv_attn_params* p, const pcv_decode_fp8* f, const pcv_dev_rows* rows) {
+  if (rows == nullptr) {
+    set_error("attn_decode_window: rows is NULL");
+    return 0;
+  }
+  if (validate_attn(p) != PCV_OK) return 0;
+  const char* why = "";
+  const bool ok = attn_decode_window_supported(*p, f, *rows, &why);
+  if (!ok) set_error("window decode attention not applicable: %s", why);
+  return ok ? 1 : 0;
+}
+
+int pcv_attn_decode_window_supported(const pcv_attn_params* p, const pcv_dev_rows* rows) {
+  return decode_window_supported(p, nullptr, rows);
+}
+
+int pcv_attn_decode_window_fp8_supported(const pcv_attn_params* p, const pcv_decode_fp8* f, const pcv_dev_rows* rows) {
+  if (f == nullptr) {
+    set_error("attn_decode_window_fp8: fp8 params are NULL");
+    return 0;
+  }
+  return decode_window_supported(p, f, rows);
+}
+
+int pcv_attn_decode_window_workspace_bytes(const pcv_attn_params* p, size_t* bytes) {
+  int rc = validate_attn(p);
+  if (rc != PCV_OK) return rc;
+  PCV_REQUIRE(bytes != nullptr, PCV_ERR_INVALID, "attn_decode_window: bytes is NULL");
+  return attn_decode_workspace_bytes(*p, bytes);
+}
+
+int pcv_attn_decode_window(const pcv_attn_params* p, const pcv_dev_rows* rows, void* stream) {
+  PCV_REQUIRE(rows != nullptr, PCV_ERR_INVALID, "attn_decode_window: rows is NULL");
+  int rc = validate_attn(p);
+  if (rc != PCV_OK) return rc;
+  return launch_attn_decode_window(*p, nullptr, *rows, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pcv_attn_decode_window_fp8(const pcv_attn_params* p, const pcv_decode_fp8* f, const pcv_dev_rows* rows,
+                               void* stream) {
+  PCV_REQUIRE(f != nullptr && rows != nullptr, PCV_ERR_INVALID, "attn_decode_window_fp8: fp8 params or rows are NULL");
+  int rc = validate_attn(p);
+  if (rc != PCV_OK) return rc;
+  return launch_attn_decode_window(*p, f, *rows, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pcv_kv_append_at(const pcv_kv_append_params* p, const pcv_dev_rows* rows, void* stream) {
+  PCV_REQUIRE(p != nullptr && rows != nullptr, PCV_ERR_INVALID, "kv_append_at: params or rows are NULL");
+  return launch_kv_append(*p, reinterpret_cast<cudaStream_t>(stream), rows);
+}
+
+int pcv_kv_append_at_fp8(const pcv_kv_append_params* p, const pcv_kv_fp8_scales* f, const pcv_dev_rows* rows,
+                         void* stream) {
+  PCV_REQUIRE(p != nullptr && f != nullptr && rows != nullptr, PCV_ERR_INVALID, "kv_append_at_fp8: params are NULL");
+  return launch_kv_append_fp8(*p, *f, reinterpret_cast<cudaStream_t>(stream), rows);
+}
+
+int pcv_rotary_apply_at(const pcv_rotary_params* p, const pcv_dev_rows* rows, void* stream) {
+  PCV_REQUIRE(p != nullptr && rows != nullptr, PCV_ERR_INVALID, "rotary_at: params or rows are NULL");
+  return launch_rotary(*p, reinterpret_cast<cudaStream_t>(stream), rows);
+}
+
+int pcv_rotary_apply_at_fp8(const pcv_rotary_params* p, const pcv_rotary_fp8* f, const pcv_dev_rows* rows,
+                            void* stream) {
+  PCV_REQUIRE(p != nullptr && f != nullptr && rows != nullptr, PCV_ERR_INVALID, "rotary_at_fp8: params are NULL");
+  return launch_rotary_fp8(*p, *f, reinterpret_cast<cudaStream_t>(stream), rows);
+}
+
 }  // extern "C"

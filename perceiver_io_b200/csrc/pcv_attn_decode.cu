@@ -66,9 +66,12 @@ __device__ __forceinline__ void unpack_chunk(const uint4& u, float (&f)[FP8 ? 16
 
 // The kernel body.  FP8: K / V are e4m3 rows (a 16-byte chunk carries 16 channels), k_descale[h] is folded into the
 // scaled q and v_descale[h, c] multiplies the accumulator once, before the merge; everything else is shared.
-// LPK lanes share one key; NQ query rows
-template <typename T, int LPK, int NQ, bool FP8>
-__device__ __forceinline__ void attn_decode_body(const DecParams& p, const pcv_decode_fp8& f8) {
+// LPK lanes share one key; NQ query rows.  WIN: the keys are the window [win[0], win[1]) of an arena of a.M rows, read
+// from device memory (pcv_attn_decode_window): every split takes an equal share of the window, the causal mask is
+// right-aligned to its end, and an empty window writes zeros.
+template <typename T, int LPK, int NQ, bool FP8, bool WIN = false>
+__device__ __forceinline__ void attn_decode_body(const DecParams& p, const pcv_decode_fp8& f8,
+                                                 const int32_t* win = nullptr) {
   constexpr int CH = FP8 ? 16 : 8;        // channels per 16-byte chunk of a K / V row
   using KV = typename std::conditional<FP8, uint8_t, T>::type;
   // e4m3 rows hold twice the channels per register: four query rows take half the unroll to stay out of local memory
@@ -84,8 +87,17 @@ __device__ __forceinline__ void attn_decode_body(const DecParams& p, const pcv_d
   const int split = (blockIdx.x / a.H) % p.nsplit;
   const int b = blockIdx.x / (a.H * p.nsplit);
   const int bh = b * a.H + h;
-  const int kb = split * p.keys_per_split;
-  const int ke = min(a.M, kb + p.keys_per_split);
+  int kb, ke, wend = 0;
+  if constexpr (WIN) {
+    const int w0 = max(win[0], 0);
+    wend = min(win[1], a.M);
+    const int kps = (max(wend - w0, 0) + p.nsplit - 1) / p.nsplit;
+    kb = w0 + split * kps;
+    ke = min(wend, kb + kps);
+  } else {
+    kb = split * p.keys_per_split;
+    ke = min(a.M, kb + p.keys_per_split);
+  }
   const int c0 = sub * CH;
   const bool kq_live = c0 < a.dqk, v_live = c0 < a.dv;
 
@@ -117,7 +129,8 @@ __device__ __forceinline__ void attn_decode_body(const DecParams& p, const pcv_d
       for (int c = 0; c < 8; ++c) q[i][c] *= scale_log2;   // scores come out in the log2 domain
     }
   }
-  const int causal_shift = a.m_total - a.N;  // key jg masked for query n iff jg > n + causal_shift
+  // key jg masked for query n iff jg > n + causal_shift (a window: right-aligned to its end)
+  const int causal_shift = (WIN ? wend : a.m_total) - a.N;
 
   float m[NQ], l[NQ], acc[NQ][CH];
 #pragma unroll
@@ -293,7 +306,10 @@ __device__ __forceinline__ void attn_decode_body(const DecParams& p, const pcv_d
       o = fmaf(__ldcg(p.ws_o + (sb + (int64_t)sp * NQ) * a.dv + c), wt, o);
       ll = fmaf(__ldcg(p.ws_l + sb + (int64_t)sp * NQ), wt, ll);
     }
-    if (!a.write_partial) {
+    if constexpr (WIN) {  // an empty window (ll == 0) writes zeros
+      T* out = reinterpret_cast<T*>(a.out) + (int64_t)b * a.o_stride_b + (int64_t)i * a.o_stride_n + (int64_t)h * a.o_stride_h;
+      out[c] = Elem<T>::from_f(ll > 0.f ? o / ll : 0.f);
+    } else if (!a.write_partial) {
       T* out = reinterpret_cast<T*>(a.out) + (int64_t)b * a.o_stride_b + (int64_t)i * a.o_stride_n + (int64_t)h * a.o_stride_h;
       out[c] = Elem<T>::from_f(o / ll);
     } else {
@@ -316,6 +332,13 @@ __global__ void __launch_bounds__(kDecThreads) attn_decode_kernel(const DecParam
 template <typename T, int LPK, int NQ>
 __global__ void __launch_bounds__(kDecThreads) attn_decode_fp8_kernel(const DecParams p, const pcv_decode_fp8 f8) {
   attn_decode_body<T, LPK, NQ, true>(p, f8);
+}
+
+// pcv_attn_decode_window (_fp8): bf16 / fp16 or e4m3 K / V rows, the key window read from device memory
+template <typename T, int LPK, int NQ, bool FP8>
+__global__ void __launch_bounds__(kDecThreads)
+    attn_decode_window_kernel(const DecParams p, const pcv_decode_fp8 f8, const int32_t* win) {
+  attn_decode_body<T, LPK, NQ, FP8, true>(p, f8, win);
 }
 
 int choose_split(const pcv_attn_params& a, int* nsplit, int* keys_per_split) {
@@ -391,9 +414,29 @@ int launch_lpk_fp8(const DecParams& p, const pcv_decode_fp8& f, int lpk, cudaStr
   }
 }
 
-}  // namespace
+template <typename T, int LPK, bool FP8>
+int launch_window_nq(const DecParams& p, const pcv_decode_fp8& f, const int32_t* win, cudaStream_t stream) {
+  dim3 grid((unsigned)((int64_t)p.nsplit * p.a.B * p.a.H));
+  if (p.a.N == 1)
+    attn_decode_window_kernel<T, LPK, 1, FP8><<<grid, kDecThreads, 0, stream>>>(p, f, win);
+  else
+    attn_decode_window_kernel<T, LPK, 4, FP8><<<grid, kDecThreads, 0, stream>>>(p, f, win);
+  PCV_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return PCV_OK;
+}
 
-bool attn_decode_supported(const pcv_attn_params& a, const char** why) {
+// the lane counts of launch_lpk (bf16 / fp16 rows) and launch_lpk_fp8 (e4m3 rows)
+template <typename T, bool FP8>
+int launch_window_lpk(const DecParams& p, const pcv_decode_fp8& f, const int32_t* win, int lpk, cudaStream_t stream) {
+  if (lpk <= 4) return launch_window_nq<T, 4, FP8>(p, f, win, stream);
+  if (lpk == 8) return launch_window_nq<T, 8, FP8>(p, f, win, stream);
+  if (FP8 || lpk == 16) return launch_window_nq<T, 16, FP8>(p, f, win, stream);
+  return launch_window_nq<T, 32, FP8>(p, f, win, stream);
+}
+
+// N, head dims, alignment and strides of the bf16 / fp16 decode kernel (any key count)
+bool decode_rows_supported(const pcv_attn_params& a, const char** why) {
   auto fail = [&](const char* w) {
     *why = w;
     return false;
@@ -406,7 +449,17 @@ bool attn_decode_supported(const pcv_attn_params& a, const char** why) {
   if ((a.q_stride_n % 8) || (a.k_stride_m % 8) || (a.v_stride_m % 8) || (a.q_stride_h % 8) || (a.k_stride_h % 8) ||
       (a.v_stride_h % 8) || (a.q_stride_b % 8) || (a.k_stride_b % 8) || (a.v_stride_b % 8))
     return fail("strides must be multiples of 8 elements");
-  if (a.M < 1024) return fail("short key axis (the general kernels are as fast)");
+  return true;
+}
+
+}  // namespace
+
+bool attn_decode_supported(const pcv_attn_params& a, const char** why) {
+  if (!decode_rows_supported(a, why)) return false;
+  if (a.M < 1024) {
+    *why = "short key axis (the general kernels are as fast)";
+    return false;
+  }
   return true;
 }
 
@@ -488,6 +541,46 @@ int launch_attn_decode_fp8(const pcv_attn_params& a, const pcv_decode_fp8& f, cu
   prof_mark_begin(stream);
   const int rc = a.dtype == PCV_BF16 ? launch_lpk_fp8<__nv_bfloat16>(p, f, lpk, stream)
                                      : launch_lpk_fp8<__half>(p, f, lpk, stream);
+  prof_mark_end(stream);
+  return rc;
+}
+
+bool attn_decode_window_supported(const pcv_attn_params& a, const pcv_decode_fp8* f, const pcv_dev_rows& r,
+                                  const char** why) {
+  auto fail = [&](const char* w) {
+    *why = w;
+    return false;
+  };
+  if (r.bounds == nullptr) return fail("rows->bounds is NULL");
+  if (r.capacity != a.M) return fail("M must equal rows->capacity (k / v / pad_mask point at arena row 0)");
+  if (a.dtype != PCV_BF16 && a.dtype != PCV_F16) return fail("dtype (of q and out) must be bf16 or fp16");
+  if (a.impl != PCV_IMPL_AUTO && a.impl != PCV_IMPL_DECODE) return fail("impl must be AUTO or DECODE");
+  if (a.write_partial) return fail("the window decode writes the normalised output only (no write_partial)");
+  if (a.m_total != a.M || a.m_offset != 0) return fail("the window decode takes no key shard (m_total != M or m_offset != 0)");
+  return f != nullptr ? attn_decode_fp8_supported(a, *f, why) : decode_rows_supported(a, why);
+}
+
+int launch_attn_decode_window(const pcv_attn_params& a, const pcv_decode_fp8* f, const pcv_dev_rows& r,
+                              cudaStream_t stream) {
+  const char* why = "";
+  PCV_REQUIRE(attn_decode_window_supported(a, f, r, &why), PCV_ERR_UNSUPPORTED, "window decode attention: %s", why);
+  DecParams p;
+  const int rc0 = decode_setup(a, &p, stream);  // split plan and workspace of the full arena: fixed for a graph
+  if (rc0 != PCV_OK) return rc0;
+  int lpk = lanes_per_key(a);
+  if (f != nullptr) {  // 16 channels per 16-byte chunk
+    lpk = 1;
+    while (lpk * 16 < std::max(a.dqk, a.dv)) lpk <<= 1;
+  }
+  const pcv_decode_fp8 f8 = f != nullptr ? *f : pcv_decode_fp8{};
+  prof_mark_begin(stream);
+  int rc;
+  if (f != nullptr)
+    rc = a.dtype == PCV_BF16 ? launch_window_lpk<__nv_bfloat16, true>(p, f8, r.bounds, lpk, stream)
+                             : launch_window_lpk<__half, true>(p, f8, r.bounds, lpk, stream);
+  else
+    rc = a.dtype == PCV_BF16 ? launch_window_lpk<__nv_bfloat16, false>(p, f8, r.bounds, lpk, stream)
+                             : launch_window_lpk<__half, false>(p, f8, r.bounds, lpk, stream);
   prof_mark_end(stream);
   return rc;
 }

@@ -184,9 +184,24 @@ __global__ void __launch_bounds__(256) rescale_kernel(const pcv_rescale_params p
 
 // ---------------------------------------------------------------------------------------------
 // rotary: one thread per channel pair.
+// AT (pcv_rotary_apply_at): the angle row of input row i is at.bounds[0] + i, and so is its output row when
+// at.bounds[1] != 0; rows whose angle row lies outside [0, at.capacity) are skipped.
 // ---------------------------------------------------------------------------------------------
-template <typename T>
-__global__ void __launch_bounds__(256) rotary_kernel(const pcv_rotary_params p) {
+template <bool AT>
+__device__ __forceinline__ bool at_rows(const pcv_rotary_params& p, const pcv_dev_rows& at, int i, int* arow, int* yrow) {
+  if constexpr (AT) {
+    *arow = at.bounds[0] + i;
+    *yrow = at.bounds[1] ? *arow : i;
+    return *arow >= 0 && *arow < at.capacity;
+  } else {
+    *arow = p.angle_row0 + i;
+    *yrow = i;
+    return true;
+  }
+}
+
+template <typename T, bool AT>
+__device__ __forceinline__ void rotary_body(const pcv_rotary_params& p, const pcv_dev_rows& at) {
   const int d2 = (p.d + 1) >> 1;
   const int64_t total = (int64_t)p.B * p.n * p.H * d2;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
@@ -198,15 +213,16 @@ __global__ void __launch_bounds__(256) rotary_kernel(const pcv_rotary_params p) 
     const int i = (int)(rest % p.n);
     const int b = (int)(rest / p.n);
     const int c = 2 * pr;
+    int arow, yrow;
+    if (!at_rows<AT>(p, at, i, &arow, &yrow)) continue;
     const T* x = reinterpret_cast<const T*>(p.x) + (int64_t)b * p.x_stride_b + (int64_t)i * p.x_stride_n +
                  (int64_t)h * p.x_stride_h;
-    T* y = reinterpret_cast<T*>(p.y) + (int64_t)b * p.y_stride_b + (int64_t)i * p.y_stride_n +
+    T* y = reinterpret_cast<T*>(p.y) + (int64_t)b * p.y_stride_b + (int64_t)yrow * p.y_stride_n +
            (int64_t)h * p.y_stride_h;
     const float x0 = Elem<T>::to_f(x[c]);
     const float x1 = (c + 1 < p.d) ? Elem<T>::to_f(x[c + 1]) : 0.f;
     if (c + 1 < p.rotate_dim) {
-      const float* a = p.angles + (p.a_stride_b ? (int64_t)b * p.a_stride_b : 0) +
-                       (int64_t)(p.angle_row0 + i) * p.a_stride_n;
+      const float* a = p.angles + (p.a_stride_b ? (int64_t)b * p.a_stride_b : 0) + (int64_t)arow * p.a_stride_n;
       float s0, c0, s1, c1;
       sincosf(a[c], &s0, &c0);
       sincosf(a[c + 1], &s1, &c1);
@@ -217,6 +233,16 @@ __global__ void __launch_bounds__(256) rotary_kernel(const pcv_rotary_params p) 
       if (c + 1 < p.d) y[c + 1] = Elem<T>::from_f(x1);
     }
   }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) rotary_kernel(const pcv_rotary_params p) {
+  rotary_body<T, false>(p, pcv_dev_rows{});
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) rotary_at_kernel(const pcv_rotary_params p, const pcv_dev_rows at) {
+  rotary_body<T, true>(p, at);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -236,7 +262,20 @@ struct CopyArgs {
   int B;
 };
 
-__global__ void __launch_bounds__(256) kv_append_kernel(const CopyArgs a) {
+// AT (pcv_kv_append_at): the first destination row is at.bounds[0]; rows outside [0, at.capacity) are skipped
+template <bool AT>
+__device__ __forceinline__ bool dst_row(const CopySeg& s, const pcv_dev_rows& at, int row, int* r) {
+  if constexpr (AT) {
+    *r = at.bounds[0] + row;
+    return *r >= 0 && *r < at.capacity;
+  } else {
+    *r = s.dst_row0 + row;
+    return true;
+  }
+}
+
+template <bool AT>
+__device__ __forceinline__ void kv_append_body(const CopyArgs& a, const pcv_dev_rows& at) {
   const CopySeg s = a.seg[blockIdx.y];
   if (s.rows == 0 || s.src == nullptr) return;
   const bool vec = ((reinterpret_cast<uintptr_t>(s.src) | reinterpret_cast<uintptr_t>(s.dst) | (uintptr_t)s.s_sb |
@@ -250,8 +289,10 @@ __global__ void __launch_bounds__(256) kv_append_kernel(const CopyArgs a) {
       const int64_t rr = idx / vpr;
       const int row = (int)(rr % s.rows);
       const int b = (int)(rr / s.rows);
+      int drow;
+      if (!dst_row<AT>(s, at, row, &drow)) continue;
       const int4 val = *reinterpret_cast<const int4*>(s.src + b * s.s_sb + row * s.s_sl + ((int64_t)w << 4));
-      *reinterpret_cast<int4*>(s.dst + b * s.d_sb + (int64_t)(s.dst_row0 + row) * s.d_sl + ((int64_t)w << 4)) = val;
+      *reinterpret_cast<int4*>(s.dst + b * s.d_sb + (int64_t)drow * s.d_sl + ((int64_t)w << 4)) = val;
     }
   } else {
     const int epr = s.row_bytes >> 1;
@@ -262,12 +303,19 @@ __global__ void __launch_bounds__(256) kv_append_kernel(const CopyArgs a) {
       const int64_t rr = idx / epr;
       const int row = (int)(rr % s.rows);
       const int b = (int)(rr / s.rows);
+      int drow;
+      if (!dst_row<AT>(s, at, row, &drow)) continue;
       const unsigned short val =
           *reinterpret_cast<const unsigned short*>(s.src + b * s.s_sb + row * s.s_sl + ((int64_t)w << 1));
-      *reinterpret_cast<unsigned short*>(s.dst + b * s.d_sb + (int64_t)(s.dst_row0 + row) * s.d_sl +
-                                         ((int64_t)w << 1)) = val;
+      *reinterpret_cast<unsigned short*>(s.dst + b * s.d_sb + (int64_t)drow * s.d_sl + ((int64_t)w << 1)) = val;
     }
   }
+}
+
+__global__ void __launch_bounds__(256) kv_append_kernel(const CopyArgs a) { kv_append_body<false>(a, pcv_dev_rows{}); }
+
+__global__ void __launch_bounds__(256) kv_append_at_kernel(const CopyArgs a, const pcv_dev_rows at) {
+  kv_append_body<true>(a, at);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -281,8 +329,8 @@ struct QuantArgs {
   int B;
 };
 
-template <typename T>
-__global__ void __launch_bounds__(256) kv_append_fp8_kernel(const QuantArgs a) {
+template <typename T, bool AT>
+__device__ __forceinline__ void kv_append_fp8_body(const QuantArgs& a, const pcv_dev_rows& at) {
   const CopySeg s = a.seg[blockIdx.y];
   if (s.rows == 0 || s.src == nullptr) return;
   const bool quant = blockIdx.y & 1;
@@ -294,8 +342,10 @@ __global__ void __launch_bounds__(256) kv_append_fp8_kernel(const QuantArgs a) {
     const int64_t rr = idx / vpr;
     const int row = (int)(rr % s.rows);
     const int b = (int)(rr / s.rows);
+    int drow;
+    if (!dst_row<AT>(s, at, row, &drow)) continue;
     const char* src = s.src + b * s.s_sb + row * s.s_sl;
-    int4* dst = reinterpret_cast<int4*>(s.dst + b * s.d_sb + (int64_t)(s.dst_row0 + row) * s.d_sl + ((int64_t)w << 4));
+    int4* dst = reinterpret_cast<int4*>(s.dst + b * s.d_sb + (int64_t)drow * s.d_sl + ((int64_t)w << 4));
     if (!quant) {
       *dst = *reinterpret_cast<const int4*>(src + ((int64_t)w << 4));
       continue;
@@ -315,12 +365,23 @@ __global__ void __launch_bounds__(256) kv_append_fp8_kernel(const QuantArgs a) {
   }
 }
 
+template <typename T>
+__global__ void __launch_bounds__(256) kv_append_fp8_kernel(const QuantArgs a) {
+  kv_append_fp8_body<T, false>(a, pcv_dev_rows{});
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) kv_append_at_fp8_kernel(const QuantArgs a, const pcv_dev_rows at) {
+  kv_append_fp8_body<T, true>(a, at);
+}
+
 // ---------------------------------------------------------------------------------------------
 // rotary_fp8: rotary with e4m3 output, one thread per channel pair (one 16-bit store).  T is the input: bf16 / fp16,
 // or uint8_t for e4m3 codes dequantised with x_descale[h].  The pair is rotated in fp32 and rounded once.
 // ---------------------------------------------------------------------------------------------
-template <typename T>
-__global__ void __launch_bounds__(256) rotary_fp8_kernel(const pcv_rotary_params p, const pcv_rotary_fp8 f) {
+template <typename T, bool AT>
+__device__ __forceinline__ void rotary_fp8_body(const pcv_rotary_params& p, const pcv_rotary_fp8& f,
+                                                const pcv_dev_rows& at) {
   const int d2 = p.d >> 1;
   const int64_t total = (int64_t)p.B * p.n * p.H * d2;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
@@ -332,9 +393,11 @@ __global__ void __launch_bounds__(256) rotary_fp8_kernel(const pcv_rotary_params
     const int i = (int)(rest % p.n);
     const int b = (int)(rest / p.n);
     const int c = 2 * pr;
+    int arow, yrow;
+    if (!at_rows<AT>(p, at, i, &arow, &yrow)) continue;
     const T* x = reinterpret_cast<const T*>(p.x) + (int64_t)b * p.x_stride_b + (int64_t)i * p.x_stride_n +
                  (int64_t)h * p.x_stride_h;
-    uint8_t* y = reinterpret_cast<uint8_t*>(p.y) + (int64_t)b * p.y_stride_b + (int64_t)i * p.y_stride_n +
+    uint8_t* y = reinterpret_cast<uint8_t*>(p.y) + (int64_t)b * p.y_stride_b + (int64_t)yrow * p.y_stride_n +
                  (int64_t)h * p.y_stride_h;
     float x0, x1;
     if constexpr (std::is_same<T, uint8_t>::value) {
@@ -348,8 +411,7 @@ __global__ void __launch_bounds__(256) rotary_fp8_kernel(const pcv_rotary_params
     }
     float y0 = x0, y1 = x1;
     if (c + 1 < p.rotate_dim) {
-      const float* a = p.angles + (p.a_stride_b ? (int64_t)b * p.a_stride_b : 0) +
-                       (int64_t)(p.angle_row0 + i) * p.a_stride_n;
+      const float* a = p.angles + (p.a_stride_b ? (int64_t)b * p.a_stride_b : 0) + (int64_t)arow * p.a_stride_n;
       float s0, c0, s1, c1;
       sincosf(a[c], &s0, &c0);
       sincosf(a[c + 1], &s1, &c1);
@@ -359,6 +421,17 @@ __global__ void __launch_bounds__(256) rotary_fp8_kernel(const pcv_rotary_params
     const float inv = f.y_inv_scale[h];
     *reinterpret_cast<uint16_t*>(y + c) = (uint16_t)cvt_e4m3x2(y0 * inv, y1 * inv);
   }
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) rotary_fp8_kernel(const pcv_rotary_params p, const pcv_rotary_fp8 f) {
+  rotary_fp8_body<T, false>(p, f, pcv_dev_rows{});
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) rotary_at_fp8_kernel(const pcv_rotary_params p, const pcv_rotary_fp8 f,
+                                                            const pcv_dev_rows at) {
+  rotary_fp8_body<T, true>(p, f, at);
 }
 
 // pad_mask bytes (B, M) -> bit words (B, wpr), wpr = pad_words_per_row(M); bit set = padding key
@@ -454,8 +527,10 @@ int launch_rescale(const pcv_rescale_params& p, cudaStream_t stream) {
   return PCV_OK;
 }
 
-int launch_rotary(const pcv_rotary_params& p, cudaStream_t stream) {
+int launch_rotary(const pcv_rotary_params& p, cudaStream_t stream, const pcv_dev_rows* at) {
   PCV_REQUIRE(p.x && p.y && p.angles, PCV_ERR_INVALID, "rotary: null pointer argument");
+  PCV_REQUIRE(at == nullptr || (at->bounds != nullptr && at->capacity >= 1), PCV_ERR_INVALID,
+              "rotary_at: rows->bounds NULL or capacity < 1");
   PCV_REQUIRE(p.B >= 1 && p.n >= 0 && p.H >= 1 && p.d >= 1, PCV_ERR_INVALID, "rotary: bad dimension");
   PCV_REQUIRE(p.rotate_dim >= 0 && p.rotate_dim <= p.d && (p.rotate_dim % 2) == 0, PCV_ERR_INVALID,
               "rotary: rotate_dim=%d must be even and <= d=%d", p.rotate_dim, p.d);
@@ -465,7 +540,11 @@ int launch_rotary(const pcv_rotary_params& p, cudaStream_t stream) {
   const int64_t total = (int64_t)p.B * p.n * p.H * ((p.d + 1) / 2);
   int64_t blocks = (total + 255) / 256;
   if (blocks > 132 * 16) blocks = 132 * 16;
-  if (p.dtype == PCV_BF16)
+  if (at != nullptr && p.dtype == PCV_BF16)
+    rotary_at_kernel<__nv_bfloat16><<<(unsigned)blocks, 256, 0, stream>>>(p, *at);
+  else if (at != nullptr)
+    rotary_at_kernel<__half><<<(unsigned)blocks, 256, 0, stream>>>(p, *at);
+  else if (p.dtype == PCV_BF16)
     rotary_kernel<__nv_bfloat16><<<(unsigned)blocks, 256, 0, stream>>>(p);
   else
     rotary_kernel<__half><<<(unsigned)blocks, 256, 0, stream>>>(p);
@@ -474,8 +553,19 @@ int launch_rotary(const pcv_rotary_params& p, cudaStream_t stream) {
   return PCV_OK;
 }
 
-int launch_kv_append(const pcv_kv_append_params& p, cudaStream_t stream) {
+// the arguments of an append at device rows (pcv_kv_append_at / _fp8)
+static int check_at(const pcv_kv_append_params& p, const pcv_dev_rows* at, const char* what) {
+  if (at == nullptr) return PCV_OK;
+  PCV_REQUIRE(at->bounds != nullptr && at->capacity >= 1, PCV_ERR_INVALID, "%s: rows->bounds NULL or capacity < 1", what);
+  PCV_REQUIRE(p.L_old == 0 && p.k_cache == nullptr && p.v_cache == nullptr, PCV_ERR_INVALID,
+              "%s: an append at device rows takes no cache (k_cache = v_cache = NULL, L_old = 0)", what);
+  return PCV_OK;
+}
+
+int launch_kv_append(const pcv_kv_append_params& p, cudaStream_t stream, const pcv_dev_rows* at) {
   PCV_REQUIRE(p.k_new && p.v_new && p.k_dst && p.v_dst, PCV_ERR_INVALID, "kv_append: null pointer argument");
+  const int rc_at = check_at(p, at, "kv_append_at");
+  if (rc_at != PCV_OK) return rc_at;
   PCV_REQUIRE(p.B >= 1 && p.L_old >= 0 && p.n >= 0 && p.Ck >= 1 && p.Cv >= 1, PCV_ERR_INVALID,
               "kv_append: bad dimension");
   PCV_REQUIRE(p.L_old == 0 || (p.k_cache && p.v_cache), PCV_ERR_INVALID, "kv_append: cache pointers required");
@@ -506,7 +596,10 @@ int launch_kv_append(const pcv_kv_append_params& p, cudaStream_t stream) {
   int64_t blocks = (maxwork + 255) / 256;
   if (blocks > 132 * 8) blocks = 132 * 8;
   dim3 grid((unsigned)blocks, 4, 1);
-  kv_append_kernel<<<grid, 256, 0, stream>>>(a);
+  if (at != nullptr)
+    kv_append_at_kernel<<<grid, 256, 0, stream>>>(a, *at);
+  else
+    kv_append_kernel<<<grid, 256, 0, stream>>>(a);
   PCV_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PCV_OK;
@@ -534,9 +627,12 @@ bool kv_append_fp8_supported(const pcv_kv_append_params& p, const pcv_kv_fp8_sca
   return true;
 }
 
-int launch_kv_append_fp8(const pcv_kv_append_params& p, const pcv_kv_fp8_scales& f, cudaStream_t stream) {
+int launch_kv_append_fp8(const pcv_kv_append_params& p, const pcv_kv_fp8_scales& f, cudaStream_t stream,
+                         const pcv_dev_rows* at) {
   const char* why = "";
   PCV_REQUIRE(kv_append_fp8_supported(p, f, &why), PCV_ERR_INVALID, "kv_append_fp8: %s", why);
+  const int rc_at = check_at(p, at, "kv_append_at_fp8");
+  if (rc_at != PCV_OK) return rc_at;
   QuantArgs a;
   a.B = p.B;
   auto seg = [&](const void* src, void* dst, int64_t ssb, int64_t ssl, int64_t dsb, int64_t dsl, int rows, int C,
@@ -560,7 +656,11 @@ int launch_kv_append_fp8(const pcv_kv_append_params& p, const pcv_kv_fp8_scales&
   for (int i = 0; i < 4; ++i) maxwork = std::max<int64_t>(maxwork, (int64_t)p.B * a.seg[i].rows * (a.seg[i].row_bytes >> 4));
   const int64_t blocks = std::min<int64_t>((maxwork + 255) / 256, 132 * 8);
   dim3 grid((unsigned)blocks, 4, 1);
-  if (p.dtype == PCV_BF16)
+  if (at != nullptr && p.dtype == PCV_BF16)
+    kv_append_at_fp8_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(a, *at);
+  else if (at != nullptr)
+    kv_append_at_fp8_kernel<__half><<<grid, 256, 0, stream>>>(a, *at);
+  else if (p.dtype == PCV_BF16)
     kv_append_fp8_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(a);
   else
     kv_append_fp8_kernel<__half><<<grid, 256, 0, stream>>>(a);
@@ -589,13 +689,22 @@ bool rotary_fp8_supported(const pcv_rotary_params& p, const pcv_rotary_fp8& f, c
   return true;
 }
 
-int launch_rotary_fp8(const pcv_rotary_params& p, const pcv_rotary_fp8& f, cudaStream_t stream) {
+int launch_rotary_fp8(const pcv_rotary_params& p, const pcv_rotary_fp8& f, cudaStream_t stream, const pcv_dev_rows* at) {
   const char* why = "";
   PCV_REQUIRE(rotary_fp8_supported(p, f, &why), PCV_ERR_INVALID, "rotary_fp8: %s", why);
+  PCV_REQUIRE(at == nullptr || (at->bounds != nullptr && at->capacity >= 1), PCV_ERR_INVALID,
+              "rotary_at_fp8: rows->bounds NULL or capacity < 1");
   if (p.n == 0) return PCV_OK;
   const int64_t total = (int64_t)p.B * p.n * p.H * (p.d / 2);
   const int64_t blocks = std::min<int64_t>((total + 255) / 256, 132 * 16);
-  if (p.dtype == PCV_BF16)
+  if (at != nullptr) {
+    if (p.dtype == PCV_BF16)
+      rotary_at_fp8_kernel<__nv_bfloat16><<<(unsigned)blocks, 256, 0, stream>>>(p, f, *at);
+    else if (p.dtype == PCV_F16)
+      rotary_at_fp8_kernel<__half><<<(unsigned)blocks, 256, 0, stream>>>(p, f, *at);
+    else
+      rotary_at_fp8_kernel<uint8_t><<<(unsigned)blocks, 256, 0, stream>>>(p, f, *at);
+  } else if (p.dtype == PCV_BF16)
     rotary_fp8_kernel<__nv_bfloat16><<<(unsigned)blocks, 256, 0, stream>>>(p, f);
   else if (p.dtype == PCV_F16)
     rotary_fp8_kernel<__half><<<(unsigned)blocks, 256, 0, stream>>>(p, f);

@@ -1,0 +1,265 @@
+"""Graph-replayed cached generation of a Perceiver AR ``CausalSequenceModel``: one generated token is one CUDA-graph
+replay.
+
+An eager cached step spends most of its time on the host (module code, arena and rotated-shadow bookkeeping, a few
+hundred ctypes / ATen launches).  Every length in it changes each token, so it cannot be recorded as it is.
+``GraphedDecoder`` keeps the caches in static arenas and the lengths in a few device int32s: per layer group the key
+window ``[begin, end)`` and the new token's row.  The append (``ops.kv_append_at``), the rotary embedding
+(``ops.rotary_apply_at``) and the decode attention (``ops.attention_decode_window``) read their rows from there when they
+run, and in-graph int32 ops advance them at the end of each step.
+
+    dec = GraphedDecoder(model, batch=B, max_new_tokens=T, kv_cache="bf16")   # or "fp8": e4m3 arenas
+    logits = dec.prefill(input_ids, prefix_len, pad_mask=None)                # (B, vocab): eager prompt pass
+    logits = dec.step(token_ids)                                              # (B, 1) int64 -> (B, vocab), one replay
+    dec.reorder(beam_idx)                                                     # beam search (eager)
+
+Rows: cross-attention arena row r holds token r of the sequence (prompt and generated tokens); self-attention arena
+row r holds token ``prefix_len + r`` (prefix_len of the prompt).  The windows follow the 🤗 wrapper's truncation, as
+:func:`decode_windows` states it.  ``step`` returns a view of the graph's static logits, valid until the next step.
+
+Not covered: steps of more than one token, contrastive search, a ring buffer bounded at ``max_seq_len`` (the arenas
+grow by ``max_new_tokens`` rows) and wiring into 🤗 ``generate()``.
+"""
+from __future__ import annotations
+
+from typing import List, NamedTuple
+
+import torch
+
+from . import modules, ops
+from .graphs import GraphedForward
+from .utils import Residual
+
+# bounds columns of one layer group: [window begin, window end, new row, 1, new row, 0]
+#   [0:2] the decode window, [2:3] the append row, [2:4] rotary into the rotated-key arena, [4:6] rotary of q
+_NCOL = 6
+
+
+class Window(NamedTuple):
+    ca_begin: int    # cross-attention key window [ca_begin, ca_end) in cross-attention arena rows (= token index)
+    ca_end: int
+    sa_begin: int    # self-attention key window in self-attention arena rows (token index - prompt prefix_len)
+    sa_end: int
+    prefix_len: int  # the prefix_len an eager cached call of this step passes
+
+
+def decode_windows(prompt_len: int, prefix_len: int, steps: int, max_seq_len: int, max_latents: int) -> List[Window]:
+    """The key windows of ``steps`` one-token cached steps after a prompt of ``prompt_len`` tokens whose first
+    ``prefix_len`` are prefix — the truncation of the 🤗 wrapper (``prepare_inputs_for_generation`` and the
+    ``_truncate_*_past_key_values`` helpers): before each step the cross-attention cache keeps at most
+    ``max_seq_len - 1`` old rows and the self-attention caches at most ``max_latents - 1``, so the prefix grows by one
+    token per step once the latents are full.  Each window includes the step's new token (its last row)."""
+    out = []
+    for s in range(steps):
+        ca_end = prompt_len + s + 1
+        sa_end = prompt_len - prefix_len + s + 1
+        ca_begin, sa_begin = max(0, ca_end - max_seq_len), max(0, sa_end - max_latents)
+        out.append(Window(ca_begin, ca_end, sa_begin, sa_end, (ca_end - ca_begin) - (sa_end - sa_begin)))
+    return out
+
+
+def window_positions(pad: torch.Tensor, window: torch.Tensor, cols: torch.Tensor) -> torch.Tensor:
+    """(B, 1) int64 absolute position of the last token of the window ``[window[0], window[1])`` of left-padded rows:
+    ``positions(b, n, shift)[:, -1:]`` of the eager call, with ``n`` the window length and ``shift`` its padding count,
+    computed from tensors alone (no host read).  ``pad`` (B, rows) bytes, non-zero = padding; ``cols`` = arange(rows)."""
+    inside = (cols >= window[0]) & (cols < window[1])
+    shift = ((pad != 0) & inside).sum(dim=1, keepdim=True)
+    return (window[1] - window[0] - 1 - shift).clamp_min(0).long()
+
+
+class _Attn:
+    """Static state of one attention layer: arenas, rotated-key arena, scales."""
+
+    def __init__(self, owner, group: int, rotary: bool, norms, key: str):
+        self.owner, self.mha, self.group, self.rotary, self.norms, self.key = owner, owner.attention, group, rotary, norms, key
+        self.K = self.V = self.S = None
+        self.kv8 = self.k_inv_h = None
+
+
+class GraphedDecoder:
+    def __init__(self, model, batch: int, max_new_tokens: int, kv_cache: str = "bf16"):
+        if max_new_tokens < 1:
+            raise ValueError(f"GraphedDecoder: max_new_tokens must be >= 1, got {max_new_tokens}")
+        if batch < 1:
+            raise ValueError(f"GraphedDecoder: batch must be >= 1, got {batch}")
+        if kv_cache not in ("bf16", "fp8"):
+            raise ValueError(f"GraphedDecoder: kv_cache must be 'bf16' or 'fp8', got {kv_cache!r}")
+        if not isinstance(model, modules.CausalSequenceModel):
+            raise TypeError("GraphedDecoder covers this package's CausalSequenceModel")
+        if model.training:
+            raise RuntimeError("GraphedDecoder is inference-only: put the model in eval mode")
+        w = model.input_adapter.txt_embedding.weight
+        if not w.is_cuda:
+            raise RuntimeError(f"GraphedDecoder runs on CUDA (sm_90a); the model is on {w.device}")
+        if w.dtype not in (torch.bfloat16, torch.float16):
+            raise RuntimeError(f"GraphedDecoder needs a bf16 / fp16 model, got {w.dtype}")
+        inv_freq = getattr(getattr(model.input_adapter, "frq_pos_encoding", None), "inv_freq", None)
+        if inv_freq is None:
+            raise RuntimeError("GraphedDecoder needs the rotary frequency table (inv_freq) of this package's adapter")
+        H = model.cross_attention[0].module.attention.num_heads
+        mult = 16 if kv_cache == "fp8" else 8
+        for m in model.modules():
+            if isinstance(m, modules.MultiHeadAttention):
+                dqk, dv = m.num_qk_channels // m.num_heads, m.num_v_channels // m.num_heads
+                if dqk % mult or dv % mult or dqk > 256 or dv > 256:
+                    raise RuntimeError(f"GraphedDecoder: head dims ({dqk}, {dv}) must be multiples of {mult} and <= 256 "
+                                       f"for the {kv_cache} cache")
+        self.model, self.batch, self.max_new_tokens, self.kv_cache = model, batch, max_new_tokens, kv_cache
+        self.fp8 = kv_cache == "fp8"
+        self.num_heads = H
+        self.inv_freq = inv_freq
+        self.device = w.device
+        self.dtype = w.dtype
+        self.captures = 0
+        self._graph = None
+        self._bounds = None
+        self._remaining = 0
+        sa = model.self_attention
+        nrot = sa.num_rotary_layers
+        ca = model.cross_attention[0].module
+        self._layers = [_Attn(ca, 0, True, (ca.kv_norm, ca.q_norm), "min_rows")]
+        for idx, layer in enumerate(sa):
+            self._layers.append(_Attn(layer[0].module, 1, nrot == -1 or idx < nrot, (layer[0].module.norm,),
+                                      "min_rows_latent"))
+
+    # ---- prompt ------------------------------------------------------------------------------------------------------
+    def prefill(self, input_ids: torch.Tensor, prefix_len: int, pad_mask=None) -> torch.Tensor:
+        """Run the prompt through the eager model (``kv_cache=[]``), load its caches and rotated keys into the arenas
+        and return the last position's logits (B, vocab).  Resets the step budget to ``max_new_tokens``."""
+        m, T = self.model, self.max_new_tokens
+        B, n0 = input_ids.shape
+        if B != self.batch:
+            raise ValueError(f"GraphedDecoder: batch {B} != {self.batch}")
+        old = modules.fp8_config["kv_cache"]
+        modules.fp8_config["kv_cache"] = self.fp8
+        try:
+            with torch.no_grad():
+                out = m(input_ids, prefix_len=prefix_len, pad_mask=pad_mask, kv_cache=[])
+        finally:
+            modules.fp8_config["kv_cache"] = old
+        caches = out.kv_cache
+        caps = (n0 + T, n0 - prefix_len + T)
+        dev = self.device
+        self._table = ops.rotary_angle_table(self.inv_freq, caps[0])
+        rotate_dim = self._table.shape[1]
+        for a, (k, v) in zip(self._layers, caches):
+            if self.fp8 and (k.dtype != ops.F8 or v.dtype != ops.F8):
+                raise RuntimeError("GraphedDecoder: the prompt pass did not produce an e4m3 cache (call not covered)")
+            cap, L = caps[a.group], k.shape[1]
+            a.K = torch.zeros(B, cap, k.shape[2], dtype=k.dtype, device=dev)
+            a.V = torch.zeros(B, cap, v.shape[2], dtype=v.dtype, device=dev)
+            a.K[:, :L].copy_(k)
+            a.V[:, :L].copy_(v)
+            a.table = self._table[:cap]
+            if a.rotary:
+                hit = ops.rotated_cache_shadow(k)
+                if hit is None or hit[1] != 0:
+                    raise RuntimeError("GraphedDecoder: the prompt pass left no rotated-key shadow at position 0")
+                a.S = torch.zeros_like(a.K)
+                a.S[:, :L].copy_(hit[0])
+            if self.fp8:
+                a.kv8 = modules._kv8_scales(a.owner, a.norms, rotate_dim if a.rotary else 0)
+                a.k_inv_h = 1.0 / a.kv8.k_descale.float().contiguous()
+        self._pad = torch.zeros(B, caps[0], dtype=torch.uint8, device=dev)
+        if pad_mask is not None:
+            self._pad[:, :n0].copy_(pad_mask != 0)
+        self._cols = torch.arange(caps[0], device=dev, dtype=torch.int32)
+        w = decode_windows(n0, prefix_len, 1, m.max_seq_len, m.max_latents)[0]
+        rows = (n0, n0 - prefix_len)
+        self._bounds = torch.tensor([[w.ca_begin, w.ca_end, rows[0], 1, rows[0], 0],
+                                     [w.sa_begin, w.sa_end, rows[1], 1, rows[1], 0]], dtype=torch.int32, device=dev)
+        self._inc = torch.tensor([0, 1, 1, 0, 1, 0], dtype=torch.int32, device=dev)
+        self._wmax = torch.tensor([m.max_seq_len, m.max_latents], dtype=torch.int32, device=dev)
+        self._token = torch.zeros(B, 1, dtype=torch.long, device=dev)
+        self._graph = None
+        self._remaining = T
+        return out.logits[:, -1]
+
+    # ---- one token ---------------------------------------------------------------------------------------------------
+    def _attend(self, a: _Attn, q, k, v):
+        H, g = a.mha.num_heads, self._bounds[a.group]
+        fp8 = self.fp8
+        ops.kv_append_at(a.K, a.V, k, v, g[2:3], *((a.kv8.k_inv, a.kv8.v_inv) if fp8 else ()))
+        keys = a.K
+        if a.rotary:   # the new key into the rotated-key arena, q at the new token's row
+            ops.rotary_apply_at(k, H, a.table, g[2:4], a.S, a.k_inv_h)
+            q = ops.rotary_apply_at(q, H, a.table, g[4:6], torch.empty(q.shape, dtype=q.dtype, device=q.device))
+            keys = a.S
+        o = ops.attention_decode_window(q, keys, a.V, g[0:2], H, a.mha.dp_scale,
+                                        pad_mask=self._pad if a.group == 0 else None, causal=a.mha.causal_attention,
+                                        k_descale=a.kv8.k_descale if fp8 else None,
+                                        v_descale=a.kv8.v_descale if fp8 else None)
+        return modules.fused_linear(a.mha, "_pcv_o_fold", None, a.mha.o_proj, o, a.key)
+
+    @staticmethod
+    def _residual(block, y, x):
+        return block.dropout(y) + x if isinstance(block, Residual) else y
+
+    def _step_fn(self, token: torch.Tensor) -> torch.Tensor:
+        m = self.model
+        adapter = m.input_adapter
+        x = adapter.txt_embedding(token)
+        if getattr(adapter, "_abs_pos_emb", False):
+            x = x + adapter.pos_embedding(window_positions(self._pad, self._bounds[0, 0:2], self._cols))
+        # cross-attention (cached: the keys of this token are its own q_norm'd row, reference modules.py:222-224)
+        ca_layer, ca = m.cross_attention, self._layers[0].owner
+        xq = ca.q_norm(x)
+        a = ca.attention
+        h = self._residual(ca_layer[0], self._attend(self._layers[0], a.q_proj(xq), a.k_proj(xq), a.v_proj(xq)), x)
+        h = ca_layer[1](h).last_hidden_state
+        for layer, st in zip(m.self_attention, self._layers[1:]):
+            sa = st.owner
+            qkv = modules.project_qkv(sa, h)
+            if qkv is None:
+                xn = sa.norm(h)
+                qkv = sa.attention.q_proj(xn), sa.attention.k_proj(xn), sa.attention.v_proj(xn)
+            h = self._residual(layer[0], self._attend(st, *qkv), h)
+            h = layer[1](h).last_hidden_state
+        if m.config.output_norm:
+            h = m.out_norm(h)
+        logits = m.output_adapter(h, txt_embedding=adapter.txt_embedding)[:, -1]
+        # the next step's rows and windows: row += 1, end += 1, begin = max(0, end - window limit)
+        b = self._bounds
+        b.add_(self._inc)
+        b[:, 0].copy_((b[:, 1] - self._wmax).clamp_min_(0))
+        return logits
+
+    def _capture(self) -> None:
+        snapshot = self._bounds.clone()   # the warm-up calls advance the rows; their arena writes are rewritten later
+        old = torch.cuda.get_sync_debug_mode()
+        torch.cuda.set_sync_debug_mode(0)  # recording a graph synchronises the device once
+        try:
+            self._graph = GraphedForward(self._step_fn, self._token)
+        finally:
+            torch.cuda.set_sync_debug_mode(old)
+        self._bounds.copy_(snapshot)
+        self.captures += 1
+
+    def step(self, token_ids: torch.Tensor) -> torch.Tensor:
+        """Append the tokens ``token_ids`` (B, 1) int64 and return the next logits (B, vocab) — one graph replay (the
+        first call records the graph).  A view of the graph's static output, valid until the next step."""
+        if self._bounds is None:
+            raise RuntimeError("GraphedDecoder: call prefill() first")
+        if self._remaining < 1:
+            raise RuntimeError(f"GraphedDecoder: {self._remaining} of max_new_tokens={self.max_new_tokens} steps remain "
+                               "(the arenas are full); call prefill() again")
+        if tuple(token_ids.shape) != (self.batch, 1) or token_ids.dtype != torch.long:
+            raise ValueError(f"GraphedDecoder.step takes ({self.batch}, 1) int64 tokens, got {tuple(token_ids.shape)} "
+                             f"{token_ids.dtype}")
+        if torch.is_autocast_enabled():
+            raise RuntimeError("GraphedDecoder does not run under autocast")
+        if self._graph is None:
+            self._token.copy_(token_ids)
+            self._capture()
+        out = self._graph(token_ids)
+        self._remaining -= 1
+        return out
+
+    def reorder(self, beam_idx: torch.Tensor) -> None:
+        """Permute the batch rows of every arena, rotated-key arena and the pad rows (beam search), eagerly."""
+        idx = beam_idx.to(device=self.device, dtype=torch.long)
+        for a in self._layers:
+            for t in (a.K, a.V, a.S):
+                if t is not None:
+                    t.copy_(t.index_select(0, idx))
+        self._pad.copy_(self._pad.index_select(0, idx))

@@ -29,6 +29,7 @@ __all__ = [
     "attention_fp8", "attention_fp8_supported", "fp8_descales", "fp8_quantize", "fp8_transpose_v", "kv_project_fp8",
     "kv_project_fp8_supported", "ln_linear", "ln_linear_backward", "kv_append_fp8", "attention_decode_fp8",
     "attention_decode_fp8_supported", "fp8_pair_descale", "fp8_dequantize", "rotated_cache_shadow", "rotary_at", "rotary_fp8",
+    "attention_decode_window", "kv_append_at", "rotary_apply_at", "rotary_angle_table",
 ]
 
 
@@ -1158,6 +1159,119 @@ def rotated_cache_shadow(k: torch.Tensor):
     if not (rot["lo"] <= start and start + k.shape[1] <= rot["hi"]):
         return None
     return rot["buf"][:, start:start + k.shape[1]], start
+
+
+# --------------------------------------------------------------------------------------------------
+# device-resident rows: decode, append and rotary whose rows are read from device int32s when the kernel runs, so a
+# recorded CUDA graph replays every step of a decode loop (generation.GraphedDecoder).  They do no arena bookkeeping.
+# --------------------------------------------------------------------------------------------------
+def _dev_rows(bounds: torch.Tensor, capacity: int):
+    if bounds.dtype != torch.int32 or not bounds.is_cuda or bounds.numel() < 1 or bounds.stride(-1) != 1:
+        raise ValueError("bounds must be a CUDA int32 tensor with unit stride")
+    r = _lib.DevRows()
+    r.bounds, r.capacity = bounds.data_ptr(), int(capacity)
+    return r
+
+
+def rotary_angle_table(inv_freq: torch.Tensor, capacity: int) -> torch.Tensor:
+    """(capacity, 2*len(inv_freq)) float32 angles of the absolute positions 0 .. capacity - 1, with exactly the arithmetic
+    of the angles :func:`rotated_cache_keys` and :func:`rotary_at` build, so rotations from it are bit-equal to theirs."""
+    return _abs_angles(inv_freq.detach().float(), 0, capacity)[0].contiguous()
+
+
+def attention_decode_window(q, k, v, bounds: torch.Tensor, num_heads: int, scale: float, pad_mask=None,
+                            causal: bool = False, k_descale=None, v_descale=None) -> torch.Tensor:
+    """Attention of at most 4 query rows on the key window ``[bounds[0], bounds[1])`` of KV arenas, the window read from
+    device memory when the kernel runs (pcv_attn_decode_window / _fp8): nothing is read back to the host, so the call
+    can be recorded in a CUDA graph and replayed for every window.
+
+    q: (B or 1, N <= 4, H*dqk) bf16 / fp16; k, v: (B, capacity, H*d) arenas, bf16 / fp16 like q or ``float8_e4m3fn``
+    codes (then ``k_descale`` (H,) and ``v_descale`` (H, dv) as in :func:`attention_decode_fp8`); ``pad_mask`` (B,
+    capacity), indexed by the absolute arena row; ``bounds`` a CUDA int32 tensor whose first two entries are the window.
+    The causal mask is right-aligned to the window's end; a window of length <= 0 gives zeros.  Returns (B, N, H*dv)."""
+    _require_cuda(q, k, v, bounds, pad_mask)
+    fp8 = k.dtype == F8
+    with torch.cuda.device(k.device):
+        if fp8:
+            p, f, keep = _fill_decode_fp8(q, k, v, k_descale, v_descale, num_heads, scale, pad_mask, causal)
+        else:
+            q, k, v, _ = _prep(q, k, v)
+            p, keep = _fill_attn_params(q, k, v, num_heads, scale, pad_mask, causal, None, 0, "decode")
+        rows = _dev_rows(bounds, p.M)
+        out = _new_output(p, _compute_dtype(q.dtype), k.device)
+        ws = _workspace(p, k.device, "pcv_attn_decode_window", C.byref(p))
+        if fp8:
+            check(_lib.lib().pcv_attn_decode_window_fp8(C.byref(p), C.byref(f), C.byref(rows), _stream()),
+                  "pcv_attn_decode_window_fp8")
+        else:
+            check(_lib.lib().pcv_attn_decode_window(C.byref(p), C.byref(rows), _stream()), "pcv_attn_decode_window")
+    del keep, ws
+    return out
+
+
+def kv_append_at(k_arena: torch.Tensor, v_arena: torch.Tensor, k_new: torch.Tensor, v_new: torch.Tensor,
+                 row: torch.Tensor, k_inv_scale=None, v_inv_scale=None) -> None:
+    """Write the new rows k_new / v_new (B, n, C) to rows ``row[0] .. row[0] + n - 1`` of the arenas (B, capacity, C), the
+    row read from device memory when the kernel runs (pcv_kv_append_at); rows at or past capacity are skipped.
+    ``float8_e4m3fn`` arenas store ``clamp(x * inv_scale, +-448)`` rounded to e4m3 (pcv_kv_append_at_fp8, per-channel
+    ``k_inv_scale`` / ``v_inv_scale`` as in :func:`kv_append_fp8`)."""
+    _require_cuda(k_arena, v_arena, k_new, v_new, row)
+    fp8 = k_arena.dtype == F8
+    if v_arena.dtype != k_arena.dtype or k_arena.shape[:2] != v_arena.shape[:2]:
+        raise ValueError("kv_append_at: the K and V arenas must agree in dtype, batch and capacity")
+    if not fp8 and (k_new.dtype != k_arena.dtype or v_new.dtype != k_arena.dtype):
+        raise ValueError(f"kv_append_at: new rows {k_new.dtype} / {v_new.dtype} into a {k_arena.dtype} arena")
+    if k_arena.stride(-1) != 1 or v_arena.stride(-1) != 1:
+        raise ValueError("kv_append_at: arenas need unit channel stride")
+    k_new, v_new = _rows_contiguous(k_new), _rows_contiguous(v_new)
+    codes = {torch.bfloat16: _lib.PCV_BF16, torch.float16: _lib.PCV_F16, torch.float32: _lib.PCV_F32}
+    p = KvAppendParams()
+    p.k_cache = p.v_cache = None
+    p.k_new, p.v_new, p.k_dst, p.v_dst = k_new.data_ptr(), v_new.data_ptr(), k_arena.data_ptr(), v_arena.data_ptr()
+    p.kn_stride_b, p.kn_stride_l = k_new.stride(0), k_new.stride(1)
+    p.vn_stride_b, p.vn_stride_l = v_new.stride(0), v_new.stride(1)
+    p.kd_stride_b, p.kd_stride_l = k_arena.stride(0), k_arena.stride(1)
+    p.vd_stride_b, p.vd_stride_l = v_arena.stride(0), v_arena.stride(1)
+    p.B, p.L_old, p.n, p.Ck, p.Cv = k_new.shape[0], 0, k_new.shape[1], k_new.shape[2], v_new.shape[2]
+    p.dtype = codes[k_new.dtype]
+    rows = _dev_rows(row, k_arena.shape[1])
+    with torch.cuda.device(k_new.device):
+        if fp8:
+            f = _lib.KvFp8Scales()
+            f.k_inv_scale, f.v_inv_scale = k_inv_scale.data_ptr(), v_inv_scale.data_ptr()
+            check(_lib.lib().pcv_kv_append_at_fp8(C.byref(p), C.byref(f), C.byref(rows), _stream()),
+                  "pcv_kv_append_at_fp8")
+        else:
+            check(_lib.lib().pcv_kv_append_at(C.byref(p), C.byref(rows), _stream()), "pcv_kv_append_at")
+
+
+def rotary_apply_at(x: torch.Tensor, num_heads: int, table: torch.Tensor, rows: torch.Tensor, out: torch.Tensor,
+                    y_inv_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """``out`` <- x (B, n, H*d) bf16 / fp16 rotated at the angle rows ``rows[0] + i`` of ``table`` (capacity, rotate_dim)
+    (:func:`rotary_angle_table`), the rows read from device memory when the kernel runs (pcv_rotary_apply_at / _fp8).
+    Row i goes to ``out[:, rows[0] + i]`` when ``rows[1] != 0`` (a key into a rotated-key arena of at least capacity
+    rows), else to ``out[:, i]``.  An e4m3 ``out`` stores the codes of the rotated rows times ``y_inv_scale[h]`` (H,).
+    Bit-equal to :func:`rotary_at` / the rotated-key shadow of :func:`rotated_cache_keys` at the same positions."""
+    _require_cuda(x, table, rows, out)
+    x = _rows_contiguous(x)
+    if out.stride(-1) != 1 or out.shape[0] != x.shape[0] or out.shape[2] != x.shape[2]:
+        raise ValueError("rotary_apply_at: `out` must be (B, rows, H*d) like x with unit channel stride")
+    if table.dim() != 2 or table.dtype != torch.float32 or table.stride(-1) != 1:
+        raise ValueError("rotary_apply_at: the angle table must be a (capacity, rotate_dim) float32 tensor")
+    fp8 = out.dtype == F8
+    if not fp8 and out.dtype != x.dtype:
+        raise ValueError(f"rotary_apply_at: `out` {out.dtype} must be x's dtype {x.dtype} or float8_e4m3fn")
+    p = _rotary_params(x, out, num_heads, table[None], False, _pcv_dtype(x.dtype))
+    r = _dev_rows(rows, table.shape[0])
+    with torch.cuda.device(x.device):
+        if fp8:
+            f = _lib.RotaryFp8()
+            f.x_descale, f.y_inv_scale = None, y_inv_scale.data_ptr()
+            check(_lib.lib().pcv_rotary_apply_at_fp8(C.byref(p), C.byref(f), C.byref(r), _stream()),
+                  "pcv_rotary_apply_at_fp8")
+        else:
+            check(_lib.lib().pcv_rotary_apply_at(C.byref(p), C.byref(r), _stream()), "pcv_rotary_apply_at")
+    return out
 
 
 def tcgen05_supported(q, k, v, num_heads: int, pad_mask=None, causal: bool = False) -> bool:
