@@ -1,5 +1,9 @@
 """Helpers shared by the -m gpu parity tests: the oracle is evaluated in fp64 on the SAME bf16-rounded
 operands the kernel sees; tolerance is stated relative to the largest reference magnitude."""
+import math
+from typing import NamedTuple
+
+import numpy as np
 import torch
 
 from oracle import mha_oracle as O
@@ -114,6 +118,132 @@ def assert_rows(got, ref, eager, H, what="", floor=0.0):
     assert bad == 0, (f"{what}: {bad} of {ratio.numel()} rows over their derived bound; worst (b={b}, h={h}, n={n}) "
                       f"err {err[b, n, h].item():.3e} > {bound[b, n, h].item():.3e}")
     return ratio.max().item()
+
+
+# --------------------------------------------------------------------------------------------------
+# The gradient gate of the attention backward tests.  Gradient rows differ in size by orders of magnitude (a padded
+# key's dK row is 0, a key only late queries see has a small dK, a peaked row a small dQ), so a gate set by max|ref|
+# does not see a wrong row of a small gradient.  assert_grads adds an element-wise gate scaled by the fp64 reference of
+# the same gradient on magnitudes (grad_magnitudes).
+#
+# KAPPA, from the rounding points of the backward kernels (csrc/pcv_attn_bwd.cu), u = the 16-bit unit roundoff:
+#   - P (times keep / (1 - p) under dropout) is rounded to 16 bits before P^T dO:         dV error  u * dV_abs;
+#   - dS is rounded to 16 bits before dS^T Q and dS K:                                    dK, dQ    u * dK_abs, u * dQ_abs;
+#   - delta = rowsum(dO * O) reads the 16-bit forward output, which carries the forward's own P rounding and its output
+#     rounding, |O - O*| <= 2u sum_j p|v|; so |delta - delta*| <= 2u rowsum(P A) and dS moves by 2u P rowsum(P A),
+#     which dS_abs holds:                                                                 dK, dQ    2u * abs;
+#   - the gradient is rounded to 16 bits on output:                                       all       u * abs.
+# That is 2u for dV and 4u for dK / dQ.  The rest is fp32 (the scores, ex2 of the fp32 statistics, the accumulations)
+# and far below u.  KAPPA = 8 is twice the largest sum; the CPU emulation of this arithmetic (test_bwd_variants_cpu.py)
+# stays at or below half of the bound it sets.  The backward shim (head dims above 192) keeps P and dS in fp32 and
+# has only the delta and output terms.
+#
+# fp16 has subnormals below 2^-14 with spacing 2^-24: a rounded P or dS element there is off by up to 2^-24 whatever
+# its size, so the gate adds 2^-24 times the sum of the magnitudes each such element multiplies (GradMagnitude.sub),
+# plus one spacing for the output.  bf16 has the exponent range of fp32: its only absolute error is ex2's flush below
+# 2^-126, which the same term with 2^-126 covers.
+# --------------------------------------------------------------------------------------------------
+KAPPA = 8.0
+UNIT_ROUNDOFF = {torch.bfloat16: 2.0 ** -8, torch.float16: 2.0 ** -11}
+ABS_SPACING = {torch.bfloat16: 2.0 ** -126, torch.float16: 2.0 ** -24}
+GRAD_FLOOR = 6e-3  # of max|ref|, the whole-tensor gate's floor: two 2^-9 roundings (P / dS, then the gradient)
+
+
+class GradMagnitude(NamedTuple):
+    """The element-wise scale of one gradient: `abs`, the fp64 gradient evaluated on magnitudes, and `sub`, the sum of
+    magnitudes that multiplies one absolute spacing per rounded P / dS element (plus 1 for the output)."""
+    abs: torch.Tensor
+    sub: torch.Tensor
+
+
+def grad_magnitudes(q, k, v, go, H, scale, pad=None, causal=False, keep=None, rp=1.0):
+    """(dq, dk, dv) GradMagnitude of the attention backward, fp64 on q's device; shapes those of the gradients.
+
+    With A = |dO| |V|^T and P the fp64 probabilities (P_d = P * keep * rp under dropout):
+        dS_abs = P * (A_d + rowsum(P_d * A))   (0 where the score is filled; the second term bounds delta)
+        dV_abs = P_d^T |dO|      dK_abs = scale * dS_abs^T |Q|      dQ_abs = scale * dS_abs |K| (summed over the batch
+    for a batch-1 q).  `sub` takes 1 for each P / dS element and P * rowsum(A) for the forward's P inside delta."""
+    f64 = torch.float64
+    dev = q.device
+    B, M, N = k.shape[0], k.shape[1], q.shape[1]
+    qh = q.detach().to(f64).expand(B, -1, -1).reshape(B, N, H, -1).transpose(1, 2).abs()
+    kh = k.detach().to(f64).reshape(B, M, H, -1).transpose(1, 2)
+    vh = v.detach().to(f64).reshape(B, M, H, -1).transpose(1, 2).abs()
+    gh = go.detach().to(dev, f64).reshape(B, N, H, -1).transpose(1, 2).abs()
+    s = (q.detach().to(f64).expand(B, -1, -1).reshape(B, N, H, -1).transpose(1, 2) * scale) @ kh.transpose(-1, -2)
+    filled = torch.zeros(B, 1, N, M, dtype=torch.bool, device=dev)
+    if pad is not None:
+        filled = filled | pad.to(dev).bool()[:, None, None, :]
+    if causal:
+        filled = filled | torch.ones(N, M, dtype=torch.bool, device=dev).triu(M - N + 1)
+    P = s.masked_fill(filled, -torch.finfo(f64).max).softmax(-1)
+    del s
+    kr = None if keep is None else keep.to(dev, f64) * rp
+    Pd = P if kr is None else P * kr
+    A = gh @ vh.transpose(-1, -2)
+    ds = P * ((A if kr is None else A * kr) + (Pd * A).sum(-1, keepdim=True))
+    ds = ds.masked_fill(filled, 0.0)
+    ds_sub = P * A.sum(-1, keepdim=True) + 1.0
+    del A
+    kh = kh.abs()
+    dq = (scale * ds @ kh, scale * ds_sub @ kh + 1.0)
+    dk = (scale * ds.transpose(-1, -2) @ qh, scale * ds_sub.transpose(-1, -2) @ qh + 1.0)
+    dv = (Pd.transpose(-1, -2) @ gh, (gh.sum(-2, keepdim=True) + 1.0).expand(B, H, M, gh.shape[-1]))
+
+    def merge(t, L):
+        return t.transpose(1, 2).reshape(B, L, -1)
+
+    dq = [merge(t, N) for t in dq]
+    if q.shape[0] == 1 and B > 1:
+        dq = [t.sum(0, keepdim=True) for t in dq]
+    return (GradMagnitude(*dq), GradMagnitude(*(merge(t, M) for t in dk)), GradMagnitude(*(merge(t, M) for t in dv)))
+
+
+def element_bound(absref, dtype):
+    """The element-wise bound of assert_grads: KAPPA * u * absref.abs + spacing * absref.sub."""
+    return KAPPA * UNIT_ROUNDOFF[dtype] * absref.abs + ABS_SPACING[dtype] * absref.sub
+
+
+def assert_grads(got, ref64, eager, absref, dtype, what="", whole=True):
+    """One gradient of the attention backward against its fp64 reference, with two gates:
+
+      - the whole-tensor derived gate: max|got - ref| <= max(2 max|eager - ref| + 1e-3 max|ref|, GRAD_FLOOR max|ref|),
+        eager being 16-bit autograd of the reference algorithm (its bound is the floor alone if eager overflowed).
+        `whole=False` leaves it out: with at most two keys per row the gradients are small by cancellation (the dS of
+        a row sum to 0), and the CPU emulation of the kernels' arithmetic already exceeds this gate there
+        (test_bwd_variants_cpu.py), so eager's error is no yardstick;
+      - the element-wise gate: |got - ref| <= KAPPA * u * absref.abs + spacing * absref.sub (see KAPPA).
+
+    Prints the whole-tensor error and the worst element's err / bound; returns that worst ratio."""
+    r = ref64.detach().double()
+    g = got.detach().double().to(r.device)
+    assert g.shape == r.shape, (what, g.shape, r.shape)
+    assert torch.isfinite(g).all(), f"{what}: non-finite values in the gradient"
+    bound, eager_err, ref_max = derived_bound(r, eager)
+    if not math.isfinite(bound):
+        bound = 0.0
+    bound = max(bound, GRAD_FLOOR * ref_max)
+    diff = (g - r).abs()
+    err = diff.max().item()
+    assert not whole or err <= bound, (f"{what}: max err {err:.3e} > whole-tensor bound {bound:.3e} (eager {eager_err:.3e}, "
+                          f"max|ref| {ref_max:.3e})")
+    eb = element_bound(absref, dtype).to(r.device)
+    ratio = diff / eb
+    flat = int(ratio.argmax().item())
+    idx = tuple(int(i) for i in np.unravel_index(flat, tuple(ratio.shape)))
+    worst = ratio[idx].item()
+    bad = int((ratio > 1).sum().item())
+    print(f"[grad elems] {what}: err {err:.3e} {'<=' if whole else 'whole-tensor gate off,'} {bound:.3e}; worst err/bound {worst:.3f} at {idx}: err "
+          f"{diff[idx].item():.3e} bound {eb[idx].item():.3e} ref {r[idx].item():.3e} abs {absref.abs[idx].item():.3e}")
+    assert bad == 0, (f"{what}: {bad} of {ratio.numel()} elements over their bound; worst at {idx} (b, row, channel): "
+                      f"got {g[idx].item():.6e} ref {r[idx].item():.6e} bound {eb[idx].item():.3e}")
+    return worst
+
+
+def assert_grad_set(got, ref64, eager, mags, dtype, what="", whole=True):
+    """assert_grads on (dq, dk, dv); returns {name: worst err / bound}."""
+    return {name: assert_grads(g_, r_, e_, m_, dtype, f"{what} {name}", whole)
+            for name, g_, r_, e_, m_ in zip(("dq", "dk", "dv"), got, ref64, eager, mags)}
 
 
 FLT_MAX = torch.finfo(torch.float32).max

@@ -1,13 +1,13 @@
 """-m gpu: the attention backward for head dims above 128 (up to 192): the dK/dV kernel's dV and dK passes and
 bwd_dq64_kernel (64-key stages, ordered dQ partials), against float64 autograd of the reference algorithm with the
-derived gate of test_gpu_bwd.py (2 x eager error + 1e-3 max|ref|, floor 6e-3 of max|ref|)."""
+gates of test_gpu_bwd.py (gpu_util.assert_grads)."""
 import pytest
 import torch
 
-from gpu_util import derived_bound
+from gpu_util import assert_grad_set, grad_magnitudes
 from perceiver_io_b200 import _lib, ops
 from test_gpu_bwd import _case, _check
-from test_gpu_dropout import FLOOR, _core_drop, _rp
+from test_gpu_dropout import _drop_ref, _rp
 from test_gpu_dropout_bighead import _mlm_encoder, _mnist_encoder
 
 pytestmark = pytest.mark.gpu
@@ -78,19 +78,9 @@ def test_wide_dropout_gradients_match_the_reference_on_the_exported_mask(case):
     got = ops.attention_backward(q, k, v, out, go, pm, pl, H, scale, pad_mask=pad, causal=causal, dropout_p=p,
                                  dropout_seed=SEED)
 
-    def ref(dt):
-        a, b_, c = (t.detach().to(dt).requires_grad_() for t in (q, k, v))
-        _core_drop(a, b_, c, H, scale, pad, causal, dt, keep, rp).backward(go.to(dt))
-        return a.grad, b_.grad, c.grad
-
-    r64, eager = ref(torch.float64), ref(dtype)
-    for name, g_, r_, e_ in zip(("dq", "dk", "dv"), got, r64, eager):
-        assert torch.isfinite(g_).all(), name
-        bound, eager_err, ref_max = derived_bound(r_, e_)
-        bound = max(bound, FLOOR * ref_max)
-        err = (g_.double() - r_).abs().max().item()
-        print(f"[wide bwd dropout] {case[4]}x{case[5]} {name}: err {err:.3e} bound {bound:.3e} (eager {eager_err:.3e})")
-        assert err <= bound, f"{name}: err {err:.3e} > bound {bound:.3e}"
+    r64, eager = (_drop_ref(q, k, v, go, H, scale, pad, causal, dt, keep, rp)[1:] for dt in (torch.float64, dtype))
+    mags = grad_magnitudes(q, k, v, go, H, scale, pad, causal, keep, rp)
+    assert_grad_set(got, r64, eager, mags, dtype, f"wide bwd dropout {case[4]}x{case[5]}")
 
 
 def test_wide_dq_is_bitwise_reproducible():

@@ -2,16 +2,17 @@
 
 The mask is counter-based (a pure function of seed, b, h, query, key), so the tests export it with
 `ops.dropout_keep_mask` and evaluate the reference algorithm — softmax, mask * 1/(1-p), P V — with exactly that mask in
-float64; forward and backward are then held to the derived gate of the other parity tests."""
+float64; the forward is then held to the derived gate of the other parity tests, the gradients to gpu_util.assert_grads
+(the derived gate and the element-wise one)."""
 import pytest
 import torch
 
-from gpu_util import derived_bound
+from gpu_util import GRAD_FLOOR, assert_grad_set, derived_bound, grad_magnitudes
 from perceiver_io_b200 import modules, ops
 
 pytestmark = pytest.mark.gpu
 
-FLOOR = 6e-3
+FLOOR = GRAD_FLOOR
 
 
 def _rp(p):
@@ -36,6 +37,14 @@ def _core_drop(q, k, v, H, scale, pad, causal, dtype, keep, rp):
     attn = attn * keep.to(dtype) * rp                                   # nn.Dropout in training mode
     o = torch.einsum("bhij,bhjc->bhic", attn, vh)
     return o.transpose(1, 2).reshape(B, N, -1)
+
+
+def _drop_ref(q, k, v, go, H, scale, pad, causal, dtype, keep, rp):
+    """Autograd of _core_drop in `dtype` on the given keep mask -> (out, grad_q, grad_k, grad_v)."""
+    a, b_, c = (t.detach().to(dtype).requires_grad_() for t in (q, k, v))
+    o = _core_drop(a, b_, c, H, scale, pad, causal, dtype, keep, rp)
+    o.backward(go.to(dtype))
+    return o.detach(), a.grad, b_.grad, c.grad
 
 
 def _inputs(B, N, M, H, dqk, dv, pad_kind, bcast, seed, dtype=torch.bfloat16):
@@ -103,21 +112,15 @@ def test_dropout_forward_and_backward_match_reference_on_the_exported_mask(case)
     finally:
         ops.backward_config["impl"] = "auto"
 
-    def ref(dtype):
-        a, b_, c = (t.detach().to(dtype).requires_grad_() for t in (q, k, v))
-        o = _core_drop(a, b_, c, H, scale, pad, causal, dtype, keep, rp)
-        o.backward(go.to(dtype))
-        return o.detach(), a.grad, b_.grad, c.grad
-
-    r64, e16 = ref(torch.float64), ref(torch.bfloat16)
-    for name, got, r_, e_ in zip(("out", "dq", "dk", "dv"), (out, qq.grad, kk.grad, vv.grad), r64, e16):
-        assert got.shape == r_.shape, (name, got.shape, r_.shape)
-        assert torch.isfinite(got).all(), name
-        bound, eager_err, ref_max = derived_bound(r_, e_)
-        bound = max(bound, FLOOR * ref_max)
-        err = (got.double() - r_).abs().max().item()
-        print(f"[dropout parity] {case} {name}: err {err:.3e} bound {bound:.3e} (eager {eager_err:.3e}, max|ref| {ref_max:.3e})")
-        assert err <= bound, f"{name}: err {err:.3e} > bound {bound:.3e}"
+    r64, e16 = (_drop_ref(q, k, v, go, H, scale, pad, causal, dt, keep, rp) for dt in (torch.float64, torch.bfloat16))
+    assert out.shape == r64[0].shape and torch.isfinite(out).all()
+    bound, eager_err, ref_max = derived_bound(r64[0], e16[0])
+    bound = max(bound, FLOOR * ref_max)
+    err = (out.double() - r64[0]).abs().max().item()
+    print(f"[dropout parity] {case} out: err {err:.3e} bound {bound:.3e} (eager {eager_err:.3e}, max|ref| {ref_max:.3e})")
+    assert err <= bound, f"out: err {err:.3e} > bound {bound:.3e}"
+    mags = grad_magnitudes(q, k, v, go, H, scale, pad, causal, keep, rp)
+    assert_grad_set((qq.grad, kk.grad, vv.grad), r64[1:], e16[1:], mags, q.dtype, f"dropout {case}")
 
 
 def test_module_dropout_train_and_eval():

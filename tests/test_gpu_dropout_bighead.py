@@ -4,14 +4,14 @@ shim with dropout, for the head dims the second-pass dropout kernel does not tak
 - The kernel leaves the softmax statistics alone: part_m / part_l equal the dropout-free kernel's bit for bit.
 - The mask it applies is the exported one: with q = 0 every score is 0, so with v = e_(j mod dv) part_o counts the kept
   keys per channel.
-- Forward and gradients through ops.attention meet the derived gate of test_gpu_dropout.py on the exported mask."""
+- Forward and gradients through ops.attention meet the gates of test_gpu_dropout.py on the exported mask."""
 import pytest
 import torch
 
 from fwd_variants import BF16, SCHEDULE_SHAPES, VARIANT_CASES, case_id, check_schedule, workers_for
-from gpu_util import derived_bound
+from gpu_util import assert_grad_set, derived_bound, grad_magnitudes
 from perceiver_io_b200 import adapter, modules, ops
-from test_gpu_dropout import FLOOR, _core_drop, _inputs, _rp
+from test_gpu_dropout import FLOOR, _drop_ref, _inputs, _rp
 
 pytestmark = pytest.mark.gpu
 
@@ -123,22 +123,16 @@ def test_forward_and_gradients_match_the_reference_on_the_exported_mask(case):
     out = ops.attention(qq, kk, vv, H, scale, pad_mask=pad, causal=causal, dropout_p=p, dropout_seed=SEED)
     out.backward(go)
 
-    def ref(dt):
-        a, b_, c = (t.detach().to(dt).requires_grad_() for t in (q, k, v))
-        o = _core_drop(a, b_, c, H, scale, pad, causal, dt, keep, rp)
-        o.backward(go.to(dt))
-        return o.detach(), a.grad, b_.grad, c.grad
-
-    r64, eager = ref(torch.float64), ref(dtype)
-    for name, got, r_, e_ in zip(("out", "dq", "dk", "dv"), (out, qq.grad, kk.grad, vv.grad), r64, eager):
-        assert got.shape == r_.shape, (name, got.shape, r_.shape)
-        assert torch.isfinite(got).all(), name
-        bound, eager_err, ref_max = derived_bound(r_, e_)
-        bound = max(bound, FLOOR * ref_max)
-        err = (got.double() - r_).abs().max().item()
-        print(f"[bighead dropout parity] {_pid(case)} {name}: err {err:.3e} bound {bound:.3e} "
-              f"(eager {eager_err:.3e}, max|ref| {ref_max:.3e})")
-        assert err <= bound, f"{name}: err {err:.3e} > bound {bound:.3e}"
+    r64, eager = (_drop_ref(q, k, v, go, H, scale, pad, causal, dt, keep, rp) for dt in (torch.float64, dtype))
+    assert out.shape == r64[0].shape and torch.isfinite(out).all()
+    bound, eager_err, ref_max = derived_bound(r64[0], eager[0])
+    bound = max(bound, FLOOR * ref_max)
+    err = (out.double() - r64[0]).abs().max().item()
+    print(f"[bighead dropout parity] {_pid(case)} out: err {err:.3e} bound {bound:.3e} "
+          f"(eager {eager_err:.3e}, max|ref| {ref_max:.3e})")
+    assert err <= bound, f"out: err {err:.3e} > bound {bound:.3e}"
+    mags = grad_magnitudes(q, k, v, go, H, scale, pad, causal, keep, rp)
+    assert_grad_set((qq.grad, kk.grad, vv.grad), r64[1:], eager[1:], mags, dtype, f"bighead dropout {_pid(case)}")
 
 
 def test_head_dims_beyond_the_forward_kernel_stay_unsupported():

@@ -3,7 +3,7 @@
 - Sequential shards: the shard partial states (with dropout: pcv_attn_fwd_partial_dropout_shard) merged on the device,
   each shard's backward (pcv_attn_bwd_shard, or the shim with a key offset above head dim 192) from the merged
   statistics, grad_q32 summed and grad_k / grad_v concatenated, against fp64 autograd on the globally exported mask
-  with the derived gate of test_gpu_bwd.py.
+  with the gates of test_gpu_bwd.py (gpu_util.assert_grads).
 - dK / dV of 128-aligned shards equal the unsharded backward's rows bit for bit (same key tiles, same arithmetic).
 - The sharded dropout forward applies dropout_keep_mask over the global key range and leaves part_m / part_l alone.
 - Two processes on cuda:0 with a gloo group: a cross_attention_sharded training step plus reduce_shard_grads gives every
@@ -15,10 +15,10 @@ import pytest
 import torch
 import torch.multiprocessing as mp
 
-from gpu_util import derived_bound
+from gpu_util import GRAD_FLOOR, assert_grad_set, derived_bound, grad_magnitudes
 from perceiver_io_b200 import _lib, dist as pdist, ops
-from test_gpu_bwd import FLOOR, _case
-from test_gpu_dropout import _core_drop, _rp
+from test_gpu_bwd import _case
+from test_gpu_dropout import _drop_ref, _rp
 
 pytestmark = pytest.mark.gpu
 
@@ -95,20 +95,15 @@ def test_sequential_shards_match_autograd(case):
                                                                                 device="cuda")
     rp = _rp(p)[1] if p > 0 else 1.0
 
-    def ref(dt_):
-        a, b_, c = (t.detach().to(dt_).requires_grad_() for t in (q, k, v))
-        o = _core_drop(a, b_, c, H, scale, pad, causal, dt_, keep, rp)
-        o.backward(go.to(dt_))
-        return o.detach(), a.grad, b_.grad, c.grad
-
-    r64, eager = ref(torch.float64), ref(dtype)
-    for name, g_, r_, e_ in zip(("out", "dq", "dk", "dv"), [out] + got, r64, eager):
-        assert g_.shape == r_.shape and torch.isfinite(g_).all(), name
-        bound, eager_err, ref_max = derived_bound(r_, e_)
-        bound = max(bound, FLOOR * ref_max)
-        err = (g_.double() - r_).abs().max().item()
-        print(f"[shard train] {case} {name}: err {err:.3e} bound {bound:.3e} (eager {eager_err:.3e})")
-        assert err <= bound, f"{name}: err {err:.3e} > bound {bound:.3e}"
+    r64, eager = (_drop_ref(q, k, v, go, H, scale, pad, causal, dt_, keep, rp) for dt_ in (torch.float64, dtype))
+    assert out.shape == r64[0].shape and torch.isfinite(out).all()
+    bound, eager_err, ref_max = derived_bound(r64[0], eager[0])
+    bound = max(bound, GRAD_FLOOR * ref_max)
+    err = (out.double() - r64[0]).abs().max().item()
+    print(f"[shard train] {case} out: err {err:.3e} bound {bound:.3e} (eager {eager_err:.3e})")
+    assert err <= bound, f"out: err {err:.3e} > bound {bound:.3e}"
+    mags = grad_magnitudes(q, k, v, go, H, scale, pad, causal, keep if p > 0 else None, rp)
+    assert_grad_set(got, r64[1:], eager[1:], mags, dtype, f"shard train {case}")
 
 
 @pytest.mark.parametrize("dims, p, causal, pad_kind", [
