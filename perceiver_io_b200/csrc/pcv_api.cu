@@ -71,7 +71,9 @@ static bool use_decode(const pcv_attn_params& p, const char** why) {
     *why = "another kernel was requested";
     return false;
   }
-  return attn_decode_supported(p, why);
+  if (!attn_decode_supported(p, nullptr, nullptr, why)) return false;
+  if (p.M < 1024) *why = "short key axis (the general kernels are as fast)";
+  return p.M >= 1024;
 }
 
 // The one-pass dropout forward: the tensor-core kernel's partial state, over all keys of an unsharded call or (shard)
@@ -196,7 +198,7 @@ int pcv_attn_fwd(const pcv_attn_params* p, void* stream) {
   int rc = validate_attn(p);
   if (rc != PCV_OK) return rc;
   const char* why = "";
-  if (use_decode(*p, &why)) return launch_attn_decode(*p, reinterpret_cast<cudaStream_t>(stream));
+  if (use_decode(*p, &why)) return launch_attn_decode(*p, nullptr, nullptr, reinterpret_cast<cudaStream_t>(stream));
   PCV_REQUIRE(p->impl != PCV_IMPL_DECODE, PCV_ERR_UNSUPPORTED, "attn: decode kernel requested but %s", why);
   if (use_tc(*p, &why)) return launch_attn_tc(*p, reinterpret_cast<cudaStream_t>(stream));
   PCV_REQUIRE(p->impl != PCV_IMPL_TCGEN05 && p->impl != PCV_IMPL_TCGEN05_PAIR, PCV_ERR_UNSUPPORTED,
@@ -252,12 +254,12 @@ int pcv_partial_rescale(const pcv_rescale_params* p, void* stream) {
 
 int pcv_rotary_apply(const pcv_rotary_params* p, void* stream) {
   PCV_REQUIRE(p != nullptr, PCV_ERR_INVALID, "rotary: params is NULL");
-  return launch_rotary(*p, reinterpret_cast<cudaStream_t>(stream));
+  return launch_rotary(*p, nullptr, nullptr, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int pcv_kv_append(const pcv_kv_append_params* p, void* stream) {
   PCV_REQUIRE(p != nullptr, PCV_ERR_INVALID, "kv_append: params is NULL");
-  return launch_kv_append(*p, reinterpret_cast<cudaStream_t>(stream));
+  return launch_kv_append(*p, nullptr, nullptr, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int pcv_kv_project_supported(const pcv_kvproj_params* p) {
@@ -438,16 +440,36 @@ int pcv_attn_fwd_fp8(const pcv_attn_params* p, const pcv_fp8_attn* f, void* stre
   return launch_attn_tc_fp8(*p, *f, reinterpret_cast<cudaStream_t>(stream));
 }
 
-int pcv_attn_decode_fp8_supported(const pcv_attn_params* p, const pcv_decode_fp8* f) {
-  if (f == nullptr) {
-    set_error("attn_decode_fp8: fp8 params are NULL");
+// The e4m3-row (fp8: f) and device-row (window: rows) decode entry points; each refuses a NULL f / rows it takes.
+static int decode_check(const pcv_attn_params* p, const pcv_decode_fp8* f, const pcv_dev_rows* rows, bool fp8,
+                        bool window) {
+  if ((fp8 && f == nullptr) || (window && rows == nullptr)) {
+    if (fp8 && f == nullptr) set_error("%s: fp8 params are NULL", window ? "attn_decode_window_fp8" : "attn_decode_fp8");
+    else set_error("attn_decode_window: rows is NULL");
     return 0;
   }
   if (validate_attn(p) != PCV_OK) return 0;
   const char* why = "";
-  const bool ok = attn_decode_fp8_supported(*p, *f, &why);
-  if (!ok) set_error("e4m3 decode attention not applicable: %s", why);
+  const bool ok = attn_decode_supported(*p, f, rows, &why);
+  if (!ok) set_error("%s decode attention not applicable: %s", window ? "window" : "e4m3", why);
   return ok ? 1 : 0;
+}
+
+static int decode_launch(const pcv_attn_params* p, const pcv_decode_fp8* f, const pcv_dev_rows* rows, bool fp8,
+                         bool window, void* stream) {
+  PCV_REQUIRE((f != nullptr || !fp8) && (rows != nullptr || !window), PCV_ERR_INVALID, "%s",
+              !window ? "attn_decode_fp8: fp8 params are NULL"
+                      : (fp8 ? "attn_decode_window_fp8: fp8 params or rows are NULL" : "attn_decode_window: rows is NULL"));
+  int rc = validate_attn(p);
+  if (rc != PCV_OK) return rc;
+  const char* why = "";
+  PCV_REQUIRE(attn_decode_supported(*p, f, rows, &why), PCV_ERR_UNSUPPORTED, "%s decode attention: %s",
+              window ? "window" : "e4m3", why);
+  return launch_attn_decode(*p, f, rows, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pcv_attn_decode_fp8_supported(const pcv_attn_params* p, const pcv_decode_fp8* f) {
+  return decode_check(p, f, nullptr, true, false);
 }
 
 int pcv_attn_decode_fp8_workspace_bytes(const pcv_attn_params* p, size_t* bytes) {
@@ -458,10 +480,7 @@ int pcv_attn_decode_fp8_workspace_bytes(const pcv_attn_params* p, size_t* bytes)
 }
 
 int pcv_attn_decode_fp8(const pcv_attn_params* p, const pcv_decode_fp8* f, void* stream) {
-  PCV_REQUIRE(f != nullptr, PCV_ERR_INVALID, "attn_decode_fp8: fp8 params are NULL");
-  int rc = validate_attn(p);
-  if (rc != PCV_OK) return rc;
-  return launch_attn_decode_fp8(*p, *f, reinterpret_cast<cudaStream_t>(stream));
+  return decode_launch(p, f, nullptr, true, false, stream);
 }
 
 int pcv_kv_append_fp8_supported(const pcv_kv_append_params* p, const pcv_kv_fp8_scales* f) {
@@ -477,7 +496,7 @@ int pcv_kv_append_fp8_supported(const pcv_kv_append_params* p, const pcv_kv_fp8_
 
 int pcv_kv_append_fp8(const pcv_kv_append_params* p, const pcv_kv_fp8_scales* f, void* stream) {
   PCV_REQUIRE(p != nullptr && f != nullptr, PCV_ERR_INVALID, "kv_append_fp8: params are NULL");
-  return launch_kv_append_fp8(*p, *f, reinterpret_cast<cudaStream_t>(stream));
+  return launch_kv_append(*p, f, nullptr, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int pcv_rotary_fp8_supported(const pcv_rotary_params* p, const pcv_rotary_fp8* f) {
@@ -493,31 +512,15 @@ int pcv_rotary_fp8_supported(const pcv_rotary_params* p, const pcv_rotary_fp8* f
 
 int pcv_rotary_apply_fp8(const pcv_rotary_params* p, const pcv_rotary_fp8* f, void* stream) {
   PCV_REQUIRE(p != nullptr && f != nullptr, PCV_ERR_INVALID, "rotary_fp8: params are NULL");
-  return launch_rotary_fp8(*p, *f, reinterpret_cast<cudaStream_t>(stream));
-}
-
-static int decode_window_supported(const pcv_attn_params* p, const pcv_decode_fp8* f, const pcv_dev_rows* rows) {
-  if (rows == nullptr) {
-    set_error("attn_decode_window: rows is NULL");
-    return 0;
-  }
-  if (validate_attn(p) != PCV_OK) return 0;
-  const char* why = "";
-  const bool ok = attn_decode_window_supported(*p, f, *rows, &why);
-  if (!ok) set_error("window decode attention not applicable: %s", why);
-  return ok ? 1 : 0;
+  return launch_rotary(*p, f, nullptr, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int pcv_attn_decode_window_supported(const pcv_attn_params* p, const pcv_dev_rows* rows) {
-  return decode_window_supported(p, nullptr, rows);
+  return decode_check(p, nullptr, rows, false, true);
 }
 
 int pcv_attn_decode_window_fp8_supported(const pcv_attn_params* p, const pcv_decode_fp8* f, const pcv_dev_rows* rows) {
-  if (f == nullptr) {
-    set_error("attn_decode_window_fp8: fp8 params are NULL");
-    return 0;
-  }
-  return decode_window_supported(p, f, rows);
+  return decode_check(p, f, rows, true, true);
 }
 
 int pcv_attn_decode_window_workspace_bytes(const pcv_attn_params* p, size_t* bytes) {
@@ -528,40 +531,34 @@ int pcv_attn_decode_window_workspace_bytes(const pcv_attn_params* p, size_t* byt
 }
 
 int pcv_attn_decode_window(const pcv_attn_params* p, const pcv_dev_rows* rows, void* stream) {
-  PCV_REQUIRE(rows != nullptr, PCV_ERR_INVALID, "attn_decode_window: rows is NULL");
-  int rc = validate_attn(p);
-  if (rc != PCV_OK) return rc;
-  return launch_attn_decode_window(*p, nullptr, *rows, reinterpret_cast<cudaStream_t>(stream));
+  return decode_launch(p, nullptr, rows, false, true, stream);
 }
 
 int pcv_attn_decode_window_fp8(const pcv_attn_params* p, const pcv_decode_fp8* f, const pcv_dev_rows* rows,
                                void* stream) {
-  PCV_REQUIRE(f != nullptr && rows != nullptr, PCV_ERR_INVALID, "attn_decode_window_fp8: fp8 params or rows are NULL");
-  int rc = validate_attn(p);
-  if (rc != PCV_OK) return rc;
-  return launch_attn_decode_window(*p, f, *rows, reinterpret_cast<cudaStream_t>(stream));
+  return decode_launch(p, f, rows, true, true, stream);
 }
 
 int pcv_kv_append_at(const pcv_kv_append_params* p, const pcv_dev_rows* rows, void* stream) {
   PCV_REQUIRE(p != nullptr && rows != nullptr, PCV_ERR_INVALID, "kv_append_at: params or rows are NULL");
-  return launch_kv_append(*p, reinterpret_cast<cudaStream_t>(stream), rows);
+  return launch_kv_append(*p, nullptr, rows, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int pcv_kv_append_at_fp8(const pcv_kv_append_params* p, const pcv_kv_fp8_scales* f, const pcv_dev_rows* rows,
                          void* stream) {
   PCV_REQUIRE(p != nullptr && f != nullptr && rows != nullptr, PCV_ERR_INVALID, "kv_append_at_fp8: params are NULL");
-  return launch_kv_append_fp8(*p, *f, reinterpret_cast<cudaStream_t>(stream), rows);
+  return launch_kv_append(*p, f, rows, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int pcv_rotary_apply_at(const pcv_rotary_params* p, const pcv_dev_rows* rows, void* stream) {
   PCV_REQUIRE(p != nullptr && rows != nullptr, PCV_ERR_INVALID, "rotary_at: params or rows are NULL");
-  return launch_rotary(*p, reinterpret_cast<cudaStream_t>(stream), rows);
+  return launch_rotary(*p, nullptr, rows, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int pcv_rotary_apply_at_fp8(const pcv_rotary_params* p, const pcv_rotary_fp8* f, const pcv_dev_rows* rows,
                             void* stream) {
   PCV_REQUIRE(p != nullptr && f != nullptr && rows != nullptr, PCV_ERR_INVALID, "rotary_at_fp8: params are NULL");
-  return launch_rotary_fp8(*p, *f, reinterpret_cast<cudaStream_t>(stream), rows);
+  return launch_rotary(*p, f, rows, reinterpret_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

@@ -16,7 +16,7 @@
 //   CTA of every (b, h) (atomic ticket) merges them and writes the normalised output or the partial state: one
 //   launch, no follow-up merge kernel (CUDA-graph friendly).
 // Masks follow include/pcv_attn.h: finite fill for padding / causal keys (a fully masked row is the uniform average).
-// The e4m3 variant (attn_decode_fp8_kernel, pcv_attn_decode_fp8) reads an FP8 KV cache through the same body: a 16-byte
+// The e4m3 variant (FP8, pcv_attn_decode_fp8) reads an FP8 KV cache through the same body: a 16-byte
 // load carries 16 channels, so it moves half the bytes per key.
 #include "pcv_common.cuh"
 
@@ -64,14 +64,14 @@ __device__ __forceinline__ void unpack_chunk(const uint4& u, float (&f)[FP8 ? 16
     unpack8<T>(u, f);
 }
 
-// The kernel body.  FP8: K / V are e4m3 rows (a 16-byte chunk carries 16 channels), k_descale[h] is folded into the
-// scaled q and v_descale[h, c] multiplies the accumulator once, before the merge; everything else is shared.
-// LPK lanes share one key; NQ query rows.  WIN: the keys are the window [win[0], win[1]) of an arena of a.M rows, read
-// from device memory (pcv_attn_decode_window): every split takes an equal share of the window, the causal mask is
-// right-aligned to its end, and an empty window writes zeros.
-template <typename T, int LPK, int NQ, bool FP8, bool WIN = false>
-__device__ __forceinline__ void attn_decode_body(const DecParams& p, const pcv_decode_fp8& f8,
-                                                 const int32_t* win = nullptr) {
+// LPK lanes share one key; NQ query rows.  FP8 (pcv_attn_decode_fp8): K / V are e4m3 rows (a 16-byte chunk carries 16
+// channels), k_descale[h] is folded into the scaled q and v_descale[h, c] multiplies the accumulator once, before the
+// merge; everything else is shared.  WIN (pcv_attn_decode_window): the keys are the window [win[0], win[1]) of an arena
+// of a.M rows, read from device memory: every split takes an equal share of the window, the causal mask is
+// right-aligned to its end, and an empty window writes zeros.  f8 and win are unused without FP8 / WIN.
+template <typename T, int LPK, int NQ, bool FP8, bool WIN>
+__global__ void __launch_bounds__(kDecThreads)
+    attn_decode_kernel(const DecParams p, const pcv_decode_fp8 f8, const int32_t* win) {
   constexpr int CH = FP8 ? 16 : 8;        // channels per 16-byte chunk of a K / V row
   using KV = typename std::conditional<FP8, uint8_t, T>::type;
   // e4m3 rows hold twice the channels per register: four query rows take half the unroll to stay out of local memory
@@ -323,24 +323,6 @@ __device__ __forceinline__ void attn_decode_body(const DecParams& p, const pcv_d
   }
 }
 
-template <typename T, int LPK, int NQ>
-__global__ void __launch_bounds__(kDecThreads) attn_decode_kernel(const DecParams p) {
-  attn_decode_body<T, LPK, NQ, false>(p, pcv_decode_fp8{});
-}
-
-// e4m3 K / V rows (pcv_attn_decode_fp8)
-template <typename T, int LPK, int NQ>
-__global__ void __launch_bounds__(kDecThreads) attn_decode_fp8_kernel(const DecParams p, const pcv_decode_fp8 f8) {
-  attn_decode_body<T, LPK, NQ, true>(p, f8);
-}
-
-// pcv_attn_decode_window (_fp8): bf16 / fp16 or e4m3 K / V rows, the key window read from device memory
-template <typename T, int LPK, int NQ, bool FP8>
-__global__ void __launch_bounds__(kDecThreads)
-    attn_decode_window_kernel(const DecParams p, const pcv_decode_fp8 f8, const int32_t* win) {
-  attn_decode_body<T, LPK, NQ, FP8, true>(p, f8, win);
-}
-
 int choose_split(const pcv_attn_params& a, int* nsplit, int* keys_per_split) {
   int dev = 0, sms = 132;
   cudaGetDevice(&dev);
@@ -360,106 +342,74 @@ int choose_split(const pcv_attn_params& a, int* nsplit, int* keys_per_split) {
 
 size_t align256(size_t x) { return (x + 255) / 256 * 256; }
 
-template <typename T, int LPK>
-int launch_nq(const DecParams& p, cudaStream_t stream) {
-  dim3 grid((unsigned)((int64_t)p.nsplit * p.a.B * p.a.H));
-  if (p.a.N == 1)
-    attn_decode_kernel<T, LPK, 1><<<grid, kDecThreads, 0, stream>>>(p);
-  else  // 2-4 query rows share the four-row instantiation (rows beyond N are zero queries whose results are dropped)
-    attn_decode_kernel<T, LPK, 4><<<grid, kDecThreads, 0, stream>>>(p);
+// rows of up to 4 chunks use the 4-lane instantiation with idle lanes; e4m3 rows of up to 256 channels take 16 chunks
+template <typename T, bool FP8, bool WIN>
+int launch_decode(const DecParams& p, const pcv_decode_fp8& f, const int32_t* win, int lpk, cudaStream_t stream) {
+  const dim3 grid((unsigned)((int64_t)p.nsplit * p.a.B * p.a.H));
+  auto run = [&](auto lanes) {
+    constexpr int LPK = decltype(lanes)::value;
+    if (p.a.N == 1)
+      attn_decode_kernel<T, LPK, 1, FP8, WIN><<<grid, kDecThreads, 0, stream>>>(p, f, win);
+    else  // 2-4 query rows share the four-row instantiation (rows beyond N are zero queries whose results are dropped)
+      attn_decode_kernel<T, LPK, 4, FP8, WIN><<<grid, kDecThreads, 0, stream>>>(p, f, win);
+  };
+  if (lpk <= 4)
+    run(std::integral_constant<int, 4>{});
+  else if (lpk == 8)
+    run(std::integral_constant<int, 8>{});
+  else if (FP8 || lpk == 16)
+    run(std::integral_constant<int, 16>{});
+  else if constexpr (!FP8)
+    run(std::integral_constant<int, 32>{});
   PCV_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PCV_OK;
 }
 
-template <typename T>
-int launch_lpk(const DecParams& p, int lpk, cudaStream_t stream) {
-  switch (lpk) {  // rows of up to 32 channels use the 4-lane instantiation with idle lanes
-    case 1:
-    case 2:
-    case 4: return launch_nq<T, 4>(p, stream);
-    case 8: return launch_nq<T, 8>(p, stream);
-    case 16: return launch_nq<T, 16>(p, stream);
-    default: return launch_nq<T, 32>(p, stream);
-  }
-}
-
-int lanes_per_key(const pcv_attn_params& a) {
-  const int chunks = (std::max(a.dqk, a.dv) + 7) / 8;
+// lanes per key: 16-byte chunks of the longer head row (8 bf16 / fp16 or 16 e4m3 channels each), a power of two
+int lanes_per_key(const pcv_attn_params& a, bool fp8) {
+  const int ch = fp8 ? 16 : 8;
+  const int chunks = (std::max(a.dqk, a.dv) + ch - 1) / ch;
   int lpk = 1;
   while (lpk < chunks) lpk <<= 1;
   return lpk;
 }
 
-template <typename T, int LPK>
-int launch_nq_fp8(const DecParams& p, const pcv_decode_fp8& f, cudaStream_t stream) {
-  dim3 grid((unsigned)((int64_t)p.nsplit * p.a.B * p.a.H));
-  if (p.a.N == 1)
-    attn_decode_fp8_kernel<T, LPK, 1><<<grid, kDecThreads, 0, stream>>>(p, f);
-  else
-    attn_decode_fp8_kernel<T, LPK, 4><<<grid, kDecThreads, 0, stream>>>(p, f);
-  PCV_CHECK_CUDA(cudaGetLastError());
-  count_launch();
-  return PCV_OK;
-}
+}  // namespace
 
-template <typename T>
-int launch_lpk_fp8(const DecParams& p, const pcv_decode_fp8& f, int lpk, cudaStream_t stream) {
-  switch (lpk) {  // rows of up to 64 channels use the 4-lane instantiation with idle lanes
-    case 1:
-    case 2:
-    case 4: return launch_nq_fp8<T, 4>(p, f, stream);
-    case 8: return launch_nq_fp8<T, 8>(p, f, stream);
-    default: return launch_nq_fp8<T, 16>(p, f, stream);
-  }
-}
-
-template <typename T, int LPK, bool FP8>
-int launch_window_nq(const DecParams& p, const pcv_decode_fp8& f, const int32_t* win, cudaStream_t stream) {
-  dim3 grid((unsigned)((int64_t)p.nsplit * p.a.B * p.a.H));
-  if (p.a.N == 1)
-    attn_decode_window_kernel<T, LPK, 1, FP8><<<grid, kDecThreads, 0, stream>>>(p, f, win);
-  else
-    attn_decode_window_kernel<T, LPK, 4, FP8><<<grid, kDecThreads, 0, stream>>>(p, f, win);
-  PCV_CHECK_CUDA(cudaGetLastError());
-  count_launch();
-  return PCV_OK;
-}
-
-// the lane counts of launch_lpk (bf16 / fp16 rows) and launch_lpk_fp8 (e4m3 rows)
-template <typename T, bool FP8>
-int launch_window_lpk(const DecParams& p, const pcv_decode_fp8& f, const int32_t* win, int lpk, cudaStream_t stream) {
-  if (lpk <= 4) return launch_window_nq<T, 4, FP8>(p, f, win, stream);
-  if (lpk == 8) return launch_window_nq<T, 8, FP8>(p, f, win, stream);
-  if (FP8 || lpk == 16) return launch_window_nq<T, 16, FP8>(p, f, win, stream);
-  return launch_window_nq<T, 32, FP8>(p, f, win, stream);
-}
-
-// N, head dims, alignment and strides of the bf16 / fp16 decode kernel (any key count)
-bool decode_rows_supported(const pcv_attn_params& a, const char** why) {
+bool attn_decode_supported(const pcv_attn_params& a, const pcv_decode_fp8* f, const pcv_dev_rows* rows,
+                           const char** why) {
   auto fail = [&](const char* w) {
     *why = w;
     return false;
   };
+  if (rows != nullptr) {
+    if (rows->bounds == nullptr) return fail("rows->bounds is NULL");
+    if (rows->capacity != a.M) return fail("M must equal rows->capacity (k / v / pad_mask point at arena row 0)");
+  }
+  if (a.dtype != PCV_BF16 && a.dtype != PCV_F16) return fail("dtype (of q and out) must be bf16 or fp16");
+  if (a.impl != PCV_IMPL_AUTO && a.impl != PCV_IMPL_DECODE) return fail("impl must be AUTO or DECODE");
+  if (rows != nullptr) {
+    if (a.write_partial) return fail("the window decode writes the normalised output only (no write_partial)");
+    if (a.m_total != a.M || a.m_offset != 0) return fail("the window decode takes no key shard (m_total != M or m_offset != 0)");
+  }
   if (a.N > kMaxQ) return fail("more than 4 query rows");
   if (a.dqk > 256 || a.dv > 256) return fail("head dim > 256");
-  if ((a.dqk % 8) || (a.dv % 8)) return fail("head dims must be multiples of 8");
-  auto al16 = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
-  if (!al16(a.q) || !al16(a.k) || !al16(a.v)) return fail("q/k/v must be 16-byte aligned");
-  if ((a.q_stride_n % 8) || (a.k_stride_m % 8) || (a.v_stride_m % 8) || (a.q_stride_h % 8) || (a.k_stride_h % 8) ||
-      (a.v_stride_h % 8) || (a.q_stride_b % 8) || (a.k_stride_b % 8) || (a.v_stride_b % 8))
-    return fail("strides must be multiples of 8 elements");
-  return true;
-}
-
-}  // namespace
-
-bool attn_decode_supported(const pcv_attn_params& a, const char** why) {
-  if (!decode_rows_supported(a, why)) return false;
-  if (a.M < 1024) {
-    *why = "short key axis (the general kernels are as fast)";
-    return false;
+  const int64_t kv = f != nullptr ? 16 : 8;  // K / V elements per 16-byte chunk
+  if ((a.dqk % kv) || (a.dv % kv))
+    return fail(f != nullptr ? "head dims must be multiples of 16" : "head dims must be multiples of 8");
+  if (f != nullptr) {
+    if (a.write_partial) return fail("the e4m3 decode writes the normalised output only (no write_partial)");
+    if (a.m_total != a.M || a.m_offset != 0) return fail("the e4m3 decode takes no key shard (m_total != M or m_offset != 0)");
+    if (f->k_descale == nullptr || f->v_descale == nullptr) return fail("k_descale / v_descale are NULL");
   }
+  if (!al16(a.q) || !al16(a.k) || !al16(a.v)) return fail("q/k/v must be 16-byte aligned");
+  if ((a.q_stride_n % 8) || (a.q_stride_h % 8) || (a.q_stride_b % 8))
+    return fail("q strides must be multiples of 8 elements");
+  if ((a.k_stride_m % kv) || (a.v_stride_m % kv) || (a.k_stride_h % kv) || (a.v_stride_h % kv) || (a.k_stride_b % kv) ||
+      (a.v_stride_b % kv))
+    return fail(f != nullptr ? "e4m3 k/v strides must be multiples of 16 elements"
+                             : "k/v strides must be multiples of 8 elements");
   return true;
 }
 
@@ -496,91 +446,24 @@ static int decode_setup(const pcv_attn_params& a, DecParams* p, cudaStream_t str
   return PCV_OK;
 }
 
-int launch_attn_decode(const pcv_attn_params& a, cudaStream_t stream) {
+int launch_attn_decode(const pcv_attn_params& a, const pcv_decode_fp8* f, const pcv_dev_rows* rows,
+                       cudaStream_t stream) {
   DecParams p;
-  const int rc0 = decode_setup(a, &p, stream);
+  const int rc0 = decode_setup(a, &p, stream);  // with rows: planned on the whole arena, fixed for a graph
   if (rc0 != PCV_OK) return rc0;
-  const int lpk = lanes_per_key(a);
-  prof_mark_begin(stream);
-  const int rc = a.dtype == PCV_BF16 ? launch_lpk<__nv_bfloat16>(p, lpk, stream) : launch_lpk<__half>(p, lpk, stream);
-  prof_mark_end(stream);
-  return rc;
-}
-
-bool attn_decode_fp8_supported(const pcv_attn_params& a, const pcv_decode_fp8& f, const char** why) {
-  auto fail = [&](const char* w) {
-    *why = w;
-    return false;
-  };
-  if (a.dtype != PCV_BF16 && a.dtype != PCV_F16) return fail("dtype (of q and out) must be bf16 or fp16");
-  if (a.impl != PCV_IMPL_AUTO && a.impl != PCV_IMPL_DECODE) return fail("impl must be AUTO or DECODE");
-  if (a.N > kMaxQ) return fail("more than 4 query rows");
-  if (a.dqk > 256 || a.dv > 256) return fail("head dim > 256");
-  if ((a.dqk % 16) || (a.dv % 16)) return fail("head dims must be multiples of 16");
-  if (a.write_partial) return fail("the e4m3 decode writes the normalised output only (no write_partial)");
-  if (a.m_total != a.M || a.m_offset != 0) return fail("the e4m3 decode takes no key shard (m_total != M or m_offset != 0)");
-  if (f.k_descale == nullptr || f.v_descale == nullptr) return fail("k_descale / v_descale are NULL");
-  auto al16 = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
-  if (!al16(a.q) || !al16(a.k) || !al16(a.v)) return fail("q/k/v must be 16-byte aligned");
-  if ((a.q_stride_n % 8) || (a.q_stride_h % 8) || (a.q_stride_b % 8))
-    return fail("q strides must be multiples of 8 elements");
-  if ((a.k_stride_m % 16) || (a.v_stride_m % 16) || (a.k_stride_h % 16) || (a.v_stride_h % 16) || (a.k_stride_b % 16) ||
-      (a.v_stride_b % 16))
-    return fail("e4m3 k/v strides must be multiples of 16 elements");
-  return true;
-}
-
-int launch_attn_decode_fp8(const pcv_attn_params& a, const pcv_decode_fp8& f, cudaStream_t stream) {
-  const char* why = "";
-  PCV_REQUIRE(attn_decode_fp8_supported(a, f, &why), PCV_ERR_UNSUPPORTED, "e4m3 decode attention: %s", why);
-  DecParams p;
-  const int rc0 = decode_setup(a, &p, stream);
-  if (rc0 != PCV_OK) return rc0;
-  int lpk = 1;  // 16 channels per 16-byte chunk
-  while (lpk * 16 < std::max(a.dqk, a.dv)) lpk <<= 1;
-  prof_mark_begin(stream);
-  const int rc = a.dtype == PCV_BF16 ? launch_lpk_fp8<__nv_bfloat16>(p, f, lpk, stream)
-                                     : launch_lpk_fp8<__half>(p, f, lpk, stream);
-  prof_mark_end(stream);
-  return rc;
-}
-
-bool attn_decode_window_supported(const pcv_attn_params& a, const pcv_decode_fp8* f, const pcv_dev_rows& r,
-                                  const char** why) {
-  auto fail = [&](const char* w) {
-    *why = w;
-    return false;
-  };
-  if (r.bounds == nullptr) return fail("rows->bounds is NULL");
-  if (r.capacity != a.M) return fail("M must equal rows->capacity (k / v / pad_mask point at arena row 0)");
-  if (a.dtype != PCV_BF16 && a.dtype != PCV_F16) return fail("dtype (of q and out) must be bf16 or fp16");
-  if (a.impl != PCV_IMPL_AUTO && a.impl != PCV_IMPL_DECODE) return fail("impl must be AUTO or DECODE");
-  if (a.write_partial) return fail("the window decode writes the normalised output only (no write_partial)");
-  if (a.m_total != a.M || a.m_offset != 0) return fail("the window decode takes no key shard (m_total != M or m_offset != 0)");
-  return f != nullptr ? attn_decode_fp8_supported(a, *f, why) : decode_rows_supported(a, why);
-}
-
-int launch_attn_decode_window(const pcv_attn_params& a, const pcv_decode_fp8* f, const pcv_dev_rows& r,
-                              cudaStream_t stream) {
-  const char* why = "";
-  PCV_REQUIRE(attn_decode_window_supported(a, f, r, &why), PCV_ERR_UNSUPPORTED, "window decode attention: %s", why);
-  DecParams p;
-  const int rc0 = decode_setup(a, &p, stream);  // split plan and workspace of the full arena: fixed for a graph
-  if (rc0 != PCV_OK) return rc0;
-  int lpk = lanes_per_key(a);
-  if (f != nullptr) {  // 16 channels per 16-byte chunk
-    lpk = 1;
-    while (lpk * 16 < std::max(a.dqk, a.dv)) lpk <<= 1;
-  }
+  const int lpk = lanes_per_key(a, f != nullptr);
   const pcv_decode_fp8 f8 = f != nullptr ? *f : pcv_decode_fp8{};
+  const int32_t* win = rows != nullptr ? rows->bounds : nullptr;
+  auto launch = [&](auto t) {
+    using T = decltype(t);
+    if (f != nullptr)
+      return win != nullptr ? launch_decode<T, true, true>(p, f8, win, lpk, stream)
+                            : launch_decode<T, true, false>(p, f8, win, lpk, stream);
+    return win != nullptr ? launch_decode<T, false, true>(p, f8, win, lpk, stream)
+                          : launch_decode<T, false, false>(p, f8, win, lpk, stream);
+  };
   prof_mark_begin(stream);
-  int rc;
-  if (f != nullptr)
-    rc = a.dtype == PCV_BF16 ? launch_window_lpk<__nv_bfloat16, true>(p, f8, r.bounds, lpk, stream)
-                             : launch_window_lpk<__half, true>(p, f8, r.bounds, lpk, stream);
-  else
-    rc = a.dtype == PCV_BF16 ? launch_window_lpk<__nv_bfloat16, false>(p, f8, r.bounds, lpk, stream)
-                             : launch_window_lpk<__half, false>(p, f8, r.bounds, lpk, stream);
+  const int rc = a.dtype == PCV_BF16 ? launch(__nv_bfloat16{}) : launch(__half{});
   prof_mark_end(stream);
   return rc;
 }

@@ -201,7 +201,7 @@ __device__ __forceinline__ bool at_rows(const pcv_rotary_params& p, const pcv_de
 }
 
 template <typename T, bool AT>
-__device__ __forceinline__ void rotary_body(const pcv_rotary_params& p, const pcv_dev_rows& at) {
+__global__ void __launch_bounds__(256) rotary_kernel(const pcv_rotary_params p, const pcv_dev_rows at) {
   const int d2 = (p.d + 1) >> 1;
   const int64_t total = (int64_t)p.B * p.n * p.H * d2;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
@@ -235,16 +235,6 @@ __device__ __forceinline__ void rotary_body(const pcv_rotary_params& p, const pc
   }
 }
 
-template <typename T>
-__global__ void __launch_bounds__(256) rotary_kernel(const pcv_rotary_params p) {
-  rotary_body<T, false>(p, pcv_dev_rows{});
-}
-
-template <typename T>
-__global__ void __launch_bounds__(256) rotary_at_kernel(const pcv_rotary_params p, const pcv_dev_rows at) {
-  rotary_body<T, true>(p, at);
-}
-
 // ---------------------------------------------------------------------------------------------
 // kv_append: rows of C elements copied with 16-byte vectors when alignment allows.
 // blockIdx.y selects the segment: 0 = K cache, 1 = K fresh, 2 = V cache, 3 = V fresh.
@@ -275,7 +265,7 @@ __device__ __forceinline__ bool dst_row(const CopySeg& s, const pcv_dev_rows& at
 }
 
 template <bool AT>
-__device__ __forceinline__ void kv_append_body(const CopyArgs& a, const pcv_dev_rows& at) {
+__global__ void __launch_bounds__(256) kv_append_kernel(const CopyArgs a, const pcv_dev_rows at) {
   const CopySeg s = a.seg[blockIdx.y];
   if (s.rows == 0 || s.src == nullptr) return;
   const bool vec = ((reinterpret_cast<uintptr_t>(s.src) | reinterpret_cast<uintptr_t>(s.dst) | (uintptr_t)s.s_sb |
@@ -312,12 +302,6 @@ __device__ __forceinline__ void kv_append_body(const CopyArgs& a, const pcv_dev_
   }
 }
 
-__global__ void __launch_bounds__(256) kv_append_kernel(const CopyArgs a) { kv_append_body<false>(a, pcv_dev_rows{}); }
-
-__global__ void __launch_bounds__(256) kv_append_at_kernel(const CopyArgs a, const pcv_dev_rows at) {
-  kv_append_body<true>(a, at);
-}
-
 // ---------------------------------------------------------------------------------------------
 // kv_append_fp8: kv_append onto e4m3 caches.  blockIdx.y as in kv_append; every thread moves 16 channels: segments 0 / 2
 // copy 16 bytes of old e4m3 rows, segments 1 / 3 read 16 bf16 / fp16 channels of a new row, multiply them by the
@@ -330,7 +314,7 @@ struct QuantArgs {
 };
 
 template <typename T, bool AT>
-__device__ __forceinline__ void kv_append_fp8_body(const QuantArgs& a, const pcv_dev_rows& at) {
+__global__ void __launch_bounds__(256) kv_append_fp8_kernel(const QuantArgs a, const pcv_dev_rows at) {
   const CopySeg s = a.seg[blockIdx.y];
   if (s.rows == 0 || s.src == nullptr) return;
   const bool quant = blockIdx.y & 1;
@@ -365,23 +349,13 @@ __device__ __forceinline__ void kv_append_fp8_body(const QuantArgs& a, const pcv
   }
 }
 
-template <typename T>
-__global__ void __launch_bounds__(256) kv_append_fp8_kernel(const QuantArgs a) {
-  kv_append_fp8_body<T, false>(a, pcv_dev_rows{});
-}
-
-template <typename T>
-__global__ void __launch_bounds__(256) kv_append_at_fp8_kernel(const QuantArgs a, const pcv_dev_rows at) {
-  kv_append_fp8_body<T, true>(a, at);
-}
-
 // ---------------------------------------------------------------------------------------------
 // rotary_fp8: rotary with e4m3 output, one thread per channel pair (one 16-bit store).  T is the input: bf16 / fp16,
 // or uint8_t for e4m3 codes dequantised with x_descale[h].  The pair is rotated in fp32 and rounded once.
 // ---------------------------------------------------------------------------------------------
 template <typename T, bool AT>
-__device__ __forceinline__ void rotary_fp8_body(const pcv_rotary_params& p, const pcv_rotary_fp8& f,
-                                                const pcv_dev_rows& at) {
+__global__ void __launch_bounds__(256)
+    rotary_fp8_kernel(const pcv_rotary_params p, const pcv_rotary_fp8 f, const pcv_dev_rows at) {
   const int d2 = p.d >> 1;
   const int64_t total = (int64_t)p.B * p.n * p.H * d2;
   for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
@@ -421,17 +395,6 @@ __device__ __forceinline__ void rotary_fp8_body(const pcv_rotary_params& p, cons
     const float inv = f.y_inv_scale[h];
     *reinterpret_cast<uint16_t*>(y + c) = (uint16_t)cvt_e4m3x2(y0 * inv, y1 * inv);
   }
-}
-
-template <typename T>
-__global__ void __launch_bounds__(256) rotary_fp8_kernel(const pcv_rotary_params p, const pcv_rotary_fp8 f) {
-  rotary_fp8_body<T, false>(p, f, pcv_dev_rows{});
-}
-
-template <typename T>
-__global__ void __launch_bounds__(256) rotary_at_fp8_kernel(const pcv_rotary_params p, const pcv_rotary_fp8 f,
-                                                            const pcv_dev_rows at) {
-  rotary_fp8_body<T, true>(p, f, at);
 }
 
 // pad_mask bytes (B, M) -> bit words (B, wpr), wpr = pad_words_per_row(M); bit set = padding key
@@ -527,79 +490,65 @@ int launch_rescale(const pcv_rescale_params& p, cudaStream_t stream) {
   return PCV_OK;
 }
 
-int launch_rotary(const pcv_rotary_params& p, cudaStream_t stream, const pcv_dev_rows* at) {
-  PCV_REQUIRE(p.x && p.y && p.angles, PCV_ERR_INVALID, "rotary: null pointer argument");
-  PCV_REQUIRE(at == nullptr || (at->bounds != nullptr && at->capacity >= 1), PCV_ERR_INVALID,
-              "rotary_at: rows->bounds NULL or capacity < 1");
-  PCV_REQUIRE(p.B >= 1 && p.n >= 0 && p.H >= 1 && p.d >= 1, PCV_ERR_INVALID, "rotary: bad dimension");
-  PCV_REQUIRE(p.rotate_dim >= 0 && p.rotate_dim <= p.d && (p.rotate_dim % 2) == 0, PCV_ERR_INVALID,
-              "rotary: rotate_dim=%d must be even and <= d=%d", p.rotate_dim, p.d);
-  PCV_REQUIRE(p.angle_row0 >= 0, PCV_ERR_INVALID, "rotary: negative angle_row0");
-  PCV_REQUIRE(p.dtype == PCV_BF16 || p.dtype == PCV_F16, PCV_ERR_INVALID, "rotary: unknown dtype %d", p.dtype);
-  if (p.n == 0) return PCV_OK;
-  const int64_t total = (int64_t)p.B * p.n * p.H * ((p.d + 1) / 2);
-  int64_t blocks = (total + 255) / 256;
-  if (blocks > 132 * 16) blocks = 132 * 16;
-  if (at != nullptr && p.dtype == PCV_BF16)
-    rotary_at_kernel<__nv_bfloat16><<<(unsigned)blocks, 256, 0, stream>>>(p, *at);
-  else if (at != nullptr)
-    rotary_at_kernel<__half><<<(unsigned)blocks, 256, 0, stream>>>(p, *at);
-  else if (p.dtype == PCV_BF16)
-    rotary_kernel<__nv_bfloat16><<<(unsigned)blocks, 256, 0, stream>>>(p);
-  else
-    rotary_kernel<__half><<<(unsigned)blocks, 256, 0, stream>>>(p);
-  PCV_CHECK_CUDA(cudaGetLastError());
-  count_launch();
-  return PCV_OK;
-}
+// the device rows of the *_at entry points
+static bool dev_rows_ok(const pcv_dev_rows* at) { return at == nullptr || (at->bounds != nullptr && at->capacity >= 1); }
 
-// the arguments of an append at device rows (pcv_kv_append_at / _fp8)
-static int check_at(const pcv_kv_append_params& p, const pcv_dev_rows* at, const char* what) {
-  if (at == nullptr) return PCV_OK;
-  PCV_REQUIRE(at->bounds != nullptr && at->capacity >= 1, PCV_ERR_INVALID, "%s: rows->bounds NULL or capacity < 1", what);
-  PCV_REQUIRE(p.L_old == 0 && p.k_cache == nullptr && p.v_cache == nullptr, PCV_ERR_INVALID,
-              "%s: an append at device rows takes no cache (k_cache = v_cache = NULL, L_old = 0)", what);
-  return PCV_OK;
-}
-
-int launch_kv_append(const pcv_kv_append_params& p, cudaStream_t stream, const pcv_dev_rows* at) {
-  PCV_REQUIRE(p.k_new && p.v_new && p.k_dst && p.v_dst, PCV_ERR_INVALID, "kv_append: null pointer argument");
-  const int rc_at = check_at(p, at, "kv_append_at");
-  if (rc_at != PCV_OK) return rc_at;
-  PCV_REQUIRE(p.B >= 1 && p.L_old >= 0 && p.n >= 0 && p.Ck >= 1 && p.Cv >= 1, PCV_ERR_INVALID,
-              "kv_append: bad dimension");
-  PCV_REQUIRE(p.L_old == 0 || (p.k_cache && p.v_cache), PCV_ERR_INVALID, "kv_append: cache pointers required");
-  CopyArgs a;
-  a.B = p.B;
-  PCV_REQUIRE(p.dtype >= PCV_BF16 && p.dtype <= PCV_F32, PCV_ERR_INVALID, "kv_append: unknown dtype %d", p.dtype);
-  const int es = (p.dtype == PCV_F32) ? 4 : 2;
-  auto seg = [&](const void* src, void* dst, int64_t ssb, int64_t ssl, int64_t dsb, int64_t dsl, int rows, int C,
-                 int row0) {
-    CopySeg s;
-    s.src = reinterpret_cast<const char*>(src);
-    s.dst = reinterpret_cast<char*>(dst);
-    s.s_sb = ssb * es; s.s_sl = ssl * es; s.d_sb = dsb * es; s.d_sl = dsl * es;
-    s.rows = rows; s.row_bytes = C * es; s.dst_row0 = row0;
-    if (src == dst && row0 == 0) s.rows = 0;  // in-place arena: the old rows are already there
-    return s;
+bool rotary_fp8_supported(const pcv_rotary_params& p, const pcv_rotary_fp8& f, const char** why) {
+  auto fail = [&](const char* w) {
+    *why = w;
+    return false;
   };
-  a.seg[0] = seg(p.k_cache, p.k_dst, p.kc_stride_b, p.kc_stride_l, p.kd_stride_b, p.kd_stride_l, p.L_old, p.Ck, 0);
-  a.seg[1] = seg(p.k_new, p.k_dst, p.kn_stride_b, p.kn_stride_l, p.kd_stride_b, p.kd_stride_l, p.n, p.Ck, p.L_old);
-  a.seg[2] = seg(p.v_cache, p.v_dst, p.vc_stride_b, p.vc_stride_l, p.vd_stride_b, p.vd_stride_l, p.L_old, p.Cv, 0);
-  a.seg[3] = seg(p.v_new, p.v_dst, p.vn_stride_b, p.vn_stride_l, p.vd_stride_b, p.vd_stride_l, p.n, p.Cv, p.L_old);
-  int64_t maxwork = 0;
-  for (int i = 0; i < 4; ++i) {
-    const int64_t w = (int64_t)p.B * a.seg[i].rows * (a.seg[i].row_bytes >> 4);
-    if (w > maxwork) maxwork = w;
+  if (!p.x || !p.y || !p.angles) return fail("null pointer argument");
+  if (f.y_inv_scale == nullptr) return fail("y_inv_scale is NULL");
+  if (p.dtype != PCV_BF16 && p.dtype != PCV_F16 && p.dtype != PCV_E4M3) return fail("x must be bf16, fp16 or e4m3");
+  if (p.dtype == PCV_E4M3 && f.x_descale == nullptr) return fail("e4m3 input needs x_descale");
+  if (p.B < 1 || p.n < 0 || p.H < 1 || p.d < 2) return fail("bad dimension");
+  if (p.d % 2) return fail("d must be even");
+  if (p.rotate_dim < 0 || p.rotate_dim > p.d || (p.rotate_dim % 2)) return fail("rotate_dim must be even and <= d");
+  if (p.angle_row0 < 0) return fail("negative angle_row0");
+  if ((p.x_stride_b | p.x_stride_n | p.x_stride_h | p.y_stride_b | p.y_stride_n | p.y_stride_h) & 1)
+    return fail("strides must be even");
+  if ((reinterpret_cast<uintptr_t>(p.y) & 1) || (p.dtype == PCV_E4M3 && (reinterpret_cast<uintptr_t>(p.x) & 1)))
+    return fail("e4m3 pointers must be 2-byte aligned");
+  return true;
+}
+
+template <typename T>
+static void rotary_t(const pcv_rotary_params& p, const pcv_rotary_fp8* f, const pcv_dev_rows* at, unsigned blocks,
+                     cudaStream_t stream) {
+  const pcv_dev_rows r = at != nullptr ? *at : pcv_dev_rows{};
+  if (f != nullptr) {
+    auto* kernel = at != nullptr ? rotary_fp8_kernel<T, true> : rotary_fp8_kernel<T, false>;
+    kernel<<<blocks, 256, 0, stream>>>(p, *f, r);
+  } else if constexpr (!std::is_same<T, uint8_t>::value) {  // e4m3 input: e4m3 output only (rotary_fp8_supported)
+    auto* kernel = at != nullptr ? rotary_kernel<T, true> : rotary_kernel<T, false>;
+    kernel<<<blocks, 256, 0, stream>>>(p, r);
   }
-  if (maxwork == 0) maxwork = 1;
-  int64_t blocks = (maxwork + 255) / 256;
-  if (blocks > 132 * 8) blocks = 132 * 8;
-  dim3 grid((unsigned)blocks, 4, 1);
-  if (at != nullptr)
-    kv_append_at_kernel<<<grid, 256, 0, stream>>>(a, *at);
+}
+
+int launch_rotary(const pcv_rotary_params& p, const pcv_rotary_fp8* f, const pcv_dev_rows* at, cudaStream_t stream) {
+  if (f != nullptr) {
+    const char* why = "";
+    PCV_REQUIRE(rotary_fp8_supported(p, *f, &why), PCV_ERR_INVALID, "rotary_fp8: %s", why);
+  } else {
+    PCV_REQUIRE(p.x && p.y && p.angles, PCV_ERR_INVALID, "rotary: null pointer argument");
+    PCV_REQUIRE(p.B >= 1 && p.n >= 0 && p.H >= 1 && p.d >= 1, PCV_ERR_INVALID, "rotary: bad dimension");
+    PCV_REQUIRE(p.rotate_dim >= 0 && p.rotate_dim <= p.d && (p.rotate_dim % 2) == 0, PCV_ERR_INVALID,
+                "rotary: rotate_dim=%d must be even and <= d=%d", p.rotate_dim, p.d);
+    PCV_REQUIRE(p.angle_row0 >= 0, PCV_ERR_INVALID, "rotary: negative angle_row0");
+    PCV_REQUIRE(p.dtype == PCV_BF16 || p.dtype == PCV_F16, PCV_ERR_INVALID, "rotary: unknown dtype %d", p.dtype);
+  }
+  PCV_REQUIRE(dev_rows_ok(at), PCV_ERR_INVALID, "%s: rows->bounds NULL or capacity < 1",
+              f != nullptr ? "rotary_at_fp8" : "rotary_at");
+  if (p.n == 0) return PCV_OK;
+  const int64_t total = (int64_t)p.B * p.n * p.H * ((p.d + 1) / 2);  // one thread per channel pair
+  const unsigned blocks = (unsigned)std::min<int64_t>((total + 255) / 256, 132 * 16);
+  if (p.dtype == PCV_BF16)
+    rotary_t<__nv_bfloat16>(p, f, at, blocks, stream);
+  else if (p.dtype == PCV_F16)
+    rotary_t<__half>(p, f, at, blocks, stream);
   else
-    kv_append_kernel<<<grid, 256, 0, stream>>>(a);
+    rotary_t<uint8_t>(p, f, at, blocks, stream);
   PCV_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PCV_OK;
@@ -627,89 +576,64 @@ bool kv_append_fp8_supported(const pcv_kv_append_params& p, const pcv_kv_fp8_sca
   return true;
 }
 
-int launch_kv_append_fp8(const pcv_kv_append_params& p, const pcv_kv_fp8_scales& f, cudaStream_t stream,
-                         const pcv_dev_rows* at) {
-  const char* why = "";
-  PCV_REQUIRE(kv_append_fp8_supported(p, f, &why), PCV_ERR_INVALID, "kv_append_fp8: %s", why);
-  const int rc_at = check_at(p, at, "kv_append_at_fp8");
-  if (rc_at != PCV_OK) return rc_at;
-  QuantArgs a;
-  a.B = p.B;
+int launch_kv_append(const pcv_kv_append_params& p, const pcv_kv_fp8_scales* f, const pcv_dev_rows* at,
+                     cudaStream_t stream) {
+  if (f != nullptr) {
+    const char* why = "";
+    PCV_REQUIRE(kv_append_fp8_supported(p, *f, &why), PCV_ERR_INVALID, "kv_append_fp8: %s", why);
+  } else {
+    PCV_REQUIRE(p.k_new && p.v_new && p.k_dst && p.v_dst, PCV_ERR_INVALID, "kv_append: null pointer argument");
+    PCV_REQUIRE(p.B >= 1 && p.L_old >= 0 && p.n >= 0 && p.Ck >= 1 && p.Cv >= 1, PCV_ERR_INVALID,
+                "kv_append: bad dimension");
+    PCV_REQUIRE(p.L_old == 0 || (p.k_cache && p.v_cache), PCV_ERR_INVALID, "kv_append: cache pointers required");
+    PCV_REQUIRE(p.dtype >= PCV_BF16 && p.dtype <= PCV_F32, PCV_ERR_INVALID, "kv_append: unknown dtype %d", p.dtype);
+  }
+  if (at != nullptr) {
+    const char* what = f != nullptr ? "kv_append_at_fp8" : "kv_append_at";
+    PCV_REQUIRE(dev_rows_ok(at), PCV_ERR_INVALID, "%s: rows->bounds NULL or capacity < 1", what);
+    PCV_REQUIRE(p.L_old == 0 && p.k_cache == nullptr && p.v_cache == nullptr, PCV_ERR_INVALID,
+                "%s: an append at device rows takes no cache (k_cache = v_cache = NULL, L_old = 0)", what);
+  }
+  // element sizes: es of the new rows; ds of the cache and destination rows (1 for e4m3 caches, else es)
+  const int es = p.dtype == PCV_F32 ? 4 : 2, ds = f != nullptr ? 1 : es;
   auto seg = [&](const void* src, void* dst, int64_t ssb, int64_t ssl, int64_t dsb, int64_t dsl, int rows, int C,
                  int row0, int src_es) {
     CopySeg s;
     s.src = reinterpret_cast<const char*>(src);
     s.dst = reinterpret_cast<char*>(dst);
-    s.s_sb = ssb * src_es; s.s_sl = ssl * src_es; s.d_sb = dsb; s.d_sl = dsl;
-    s.rows = rows; s.row_bytes = C; s.dst_row0 = row0;
+    s.s_sb = ssb * src_es; s.s_sl = ssl * src_es; s.d_sb = dsb * ds; s.d_sl = dsl * ds;
+    s.rows = rows; s.row_bytes = C * ds; s.dst_row0 = row0;
     if (src == dst && row0 == 0) s.rows = 0;  // in-place arena: the old rows are already there
     return s;
   };
-  a.seg[0] = seg(p.k_cache, p.k_dst, p.kc_stride_b, p.kc_stride_l, p.kd_stride_b, p.kd_stride_l, p.L_old, p.Ck, 0, 1);
-  a.seg[1] = seg(p.k_new, p.k_dst, p.kn_stride_b, p.kn_stride_l, p.kd_stride_b, p.kd_stride_l, p.n, p.Ck, p.L_old, 2);
-  a.seg[2] = seg(p.v_cache, p.v_dst, p.vc_stride_b, p.vc_stride_l, p.vd_stride_b, p.vd_stride_l, p.L_old, p.Cv, 0, 1);
-  a.seg[3] = seg(p.v_new, p.v_dst, p.vn_stride_b, p.vn_stride_l, p.vd_stride_b, p.vd_stride_l, p.n, p.Cv, p.L_old, 2);
-  a.inv[0] = a.inv[2] = nullptr;
-  a.inv[1] = f.k_inv_scale;
-  a.inv[3] = f.v_inv_scale;
+  const CopySeg segs[4] = {
+      seg(p.k_cache, p.k_dst, p.kc_stride_b, p.kc_stride_l, p.kd_stride_b, p.kd_stride_l, p.L_old, p.Ck, 0, ds),
+      seg(p.k_new, p.k_dst, p.kn_stride_b, p.kn_stride_l, p.kd_stride_b, p.kd_stride_l, p.n, p.Ck, p.L_old, es),
+      seg(p.v_cache, p.v_dst, p.vc_stride_b, p.vc_stride_l, p.vd_stride_b, p.vd_stride_l, p.L_old, p.Cv, 0, ds),
+      seg(p.v_new, p.v_dst, p.vn_stride_b, p.vn_stride_l, p.vd_stride_b, p.vd_stride_l, p.n, p.Cv, p.L_old, es)};
   int64_t maxwork = 1;
-  for (int i = 0; i < 4; ++i) maxwork = std::max<int64_t>(maxwork, (int64_t)p.B * a.seg[i].rows * (a.seg[i].row_bytes >> 4));
-  const int64_t blocks = std::min<int64_t>((maxwork + 255) / 256, 132 * 8);
-  dim3 grid((unsigned)blocks, 4, 1);
-  if (at != nullptr && p.dtype == PCV_BF16)
-    kv_append_at_fp8_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(a, *at);
-  else if (at != nullptr)
-    kv_append_at_fp8_kernel<__half><<<grid, 256, 0, stream>>>(a, *at);
-  else if (p.dtype == PCV_BF16)
-    kv_append_fp8_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(a);
-  else
-    kv_append_fp8_kernel<__half><<<grid, 256, 0, stream>>>(a);
-  PCV_CHECK_CUDA(cudaGetLastError());
-  count_launch();
-  return PCV_OK;
-}
-
-bool rotary_fp8_supported(const pcv_rotary_params& p, const pcv_rotary_fp8& f, const char** why) {
-  auto fail = [&](const char* w) {
-    *why = w;
-    return false;
-  };
-  if (!p.x || !p.y || !p.angles) return fail("null pointer argument");
-  if (f.y_inv_scale == nullptr) return fail("y_inv_scale is NULL");
-  if (p.dtype != PCV_BF16 && p.dtype != PCV_F16 && p.dtype != PCV_E4M3) return fail("x must be bf16, fp16 or e4m3");
-  if (p.dtype == PCV_E4M3 && f.x_descale == nullptr) return fail("e4m3 input needs x_descale");
-  if (p.B < 1 || p.n < 0 || p.H < 1 || p.d < 2) return fail("bad dimension");
-  if (p.d % 2) return fail("d must be even");
-  if (p.rotate_dim < 0 || p.rotate_dim > p.d || (p.rotate_dim % 2)) return fail("rotate_dim must be even and <= d");
-  if (p.angle_row0 < 0) return fail("negative angle_row0");
-  if ((p.x_stride_b | p.x_stride_n | p.x_stride_h | p.y_stride_b | p.y_stride_n | p.y_stride_h) & 1)
-    return fail("strides must be even");
-  if ((reinterpret_cast<uintptr_t>(p.y) & 1) || (p.dtype == PCV_E4M3 && (reinterpret_cast<uintptr_t>(p.x) & 1)))
-    return fail("e4m3 pointers must be 2-byte aligned");
-  return true;
-}
-
-int launch_rotary_fp8(const pcv_rotary_params& p, const pcv_rotary_fp8& f, cudaStream_t stream, const pcv_dev_rows* at) {
-  const char* why = "";
-  PCV_REQUIRE(rotary_fp8_supported(p, f, &why), PCV_ERR_INVALID, "rotary_fp8: %s", why);
-  PCV_REQUIRE(at == nullptr || (at->bounds != nullptr && at->capacity >= 1), PCV_ERR_INVALID,
-              "rotary_at_fp8: rows->bounds NULL or capacity < 1");
-  if (p.n == 0) return PCV_OK;
-  const int64_t total = (int64_t)p.B * p.n * p.H * (p.d / 2);
-  const int64_t blocks = std::min<int64_t>((total + 255) / 256, 132 * 16);
-  if (at != nullptr) {
-    if (p.dtype == PCV_BF16)
-      rotary_at_fp8_kernel<__nv_bfloat16><<<(unsigned)blocks, 256, 0, stream>>>(p, f, *at);
-    else if (p.dtype == PCV_F16)
-      rotary_at_fp8_kernel<__half><<<(unsigned)blocks, 256, 0, stream>>>(p, f, *at);
-    else
-      rotary_at_fp8_kernel<uint8_t><<<(unsigned)blocks, 256, 0, stream>>>(p, f, *at);
-  } else if (p.dtype == PCV_BF16)
-    rotary_fp8_kernel<__nv_bfloat16><<<(unsigned)blocks, 256, 0, stream>>>(p, f);
-  else if (p.dtype == PCV_F16)
-    rotary_fp8_kernel<__half><<<(unsigned)blocks, 256, 0, stream>>>(p, f);
-  else
-    rotary_fp8_kernel<uint8_t><<<(unsigned)blocks, 256, 0, stream>>>(p, f);
+  for (const CopySeg& s : segs) maxwork = std::max<int64_t>(maxwork, (int64_t)p.B * s.rows * (s.row_bytes >> 4));
+  const dim3 grid((unsigned)std::min<int64_t>((maxwork + 255) / 256, 132 * 8), 4, 1);
+  const pcv_dev_rows r = at != nullptr ? *at : pcv_dev_rows{};
+  if (f == nullptr) {
+    CopyArgs a;
+    std::copy(segs, segs + 4, a.seg);
+    a.B = p.B;
+    auto* kernel = at != nullptr ? kv_append_kernel<true> : kv_append_kernel<false>;
+    kernel<<<grid, 256, 0, stream>>>(a, r);
+  } else {
+    QuantArgs a;
+    std::copy(segs, segs + 4, a.seg);
+    a.inv[0] = a.inv[2] = nullptr;
+    a.inv[1] = f->k_inv_scale;
+    a.inv[3] = f->v_inv_scale;
+    a.B = p.B;
+    auto* kernel = p.dtype == PCV_BF16 ? (at != nullptr ? kv_append_fp8_kernel<__nv_bfloat16, true>
+                                                        : kv_append_fp8_kernel<__nv_bfloat16, false>)
+                                       : (at != nullptr ? kv_append_fp8_kernel<__half, true>
+                                                        : kv_append_fp8_kernel<__half, false>);
+    kernel<<<grid, 256, 0, stream>>>(a, r);
+  }
   PCV_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PCV_OK;

@@ -123,18 +123,11 @@ int debug_read(uint32_t* out, int n);  // the watchdog record of the wgmma kerne
 int debug_plan(int B, int H, int N, int M, int workers, int rows_per_unit, int rows_per_tile, int32_t* segs,
                int max_segs, int32_t* counts);  // host-only dump of the tcgen05 work plan
 
-bool attn_decode_supported(const pcv_attn_params& p, const char** why);
-int launch_attn_decode(const pcv_attn_params& p, cudaStream_t stream);
+// the streaming decode kernel: f != nullptr for e4m3 K / V rows (pcv_attn_decode_fp8), rows != nullptr for the key
+// window read from device memory (pcv_attn_decode_window (_fp8), M = the arena's capacity)
+bool attn_decode_supported(const pcv_attn_params& p, const pcv_decode_fp8* f, const pcv_dev_rows* rows, const char** why);
+int launch_attn_decode(const pcv_attn_params& p, const pcv_decode_fp8* f, const pcv_dev_rows* rows, cudaStream_t stream);
 int attn_decode_workspace_bytes(const pcv_attn_params& p, size_t* bytes);
-// the e4m3-cache decode (attn_decode_kernel with e4m3 K / V rows); workspace as attn_decode_workspace_bytes
-bool attn_decode_fp8_supported(const pcv_attn_params& p, const pcv_decode_fp8& f, const char** why);
-int launch_attn_decode_fp8(const pcv_attn_params& p, const pcv_decode_fp8& f, cudaStream_t stream);
-// the window decode (attn_decode_window_kernel): f == nullptr for bf16 / fp16 K / V rows, else e4m3 rows; workspace as
-// attn_decode_workspace_bytes with M = capacity
-bool attn_decode_window_supported(const pcv_attn_params& p, const pcv_decode_fp8* f, const pcv_dev_rows& r,
-                                  const char** why);
-int launch_attn_decode_window(const pcv_attn_params& p, const pcv_decode_fp8* f, const pcv_dev_rows& r,
-                              cudaStream_t stream);
 
 int launch_combine(const pcv_combine_params& p, cudaStream_t stream);
 // Merge `nparts` partial states laid out [part][B][H][N]([dv]) either into p.out (normalised) or,
@@ -144,15 +137,13 @@ int launch_combine_ex(const float* po, const float* pm, const float* pl, int npa
 int launch_combine_peers(const pcv_peer_combine_params& p, cudaStream_t stream);
 int launch_merge_partials(const pcv_merge_params& p, cudaStream_t stream);
 int launch_rescale(const pcv_rescale_params& p, cudaStream_t stream);
-// at != nullptr: the *_at entry points (rows read from device memory, pcv_dev_rows)
-int launch_rotary(const pcv_rotary_params& p, cudaStream_t stream, const pcv_dev_rows* at = nullptr);
-int launch_kv_append(const pcv_kv_append_params& p, cudaStream_t stream, const pcv_dev_rows* at = nullptr);
+// f != nullptr: the *_fp8 entry points (e4m3 caches / output); at != nullptr: the *_at entry points (rows read from
+// device memory, pcv_dev_rows)
+int launch_rotary(const pcv_rotary_params& p, const pcv_rotary_fp8* f, const pcv_dev_rows* at, cudaStream_t stream);
+int launch_kv_append(const pcv_kv_append_params& p, const pcv_kv_fp8_scales* f, const pcv_dev_rows* at,
+                     cudaStream_t stream);
 bool kv_append_fp8_supported(const pcv_kv_append_params& p, const pcv_kv_fp8_scales& f, const char** why);
-int launch_kv_append_fp8(const pcv_kv_append_params& p, const pcv_kv_fp8_scales& f, cudaStream_t stream,
-                         const pcv_dev_rows* at = nullptr);
 bool rotary_fp8_supported(const pcv_rotary_params& p, const pcv_rotary_fp8& f, const char** why);
-int launch_rotary_fp8(const pcv_rotary_params& p, const pcv_rotary_fp8& f, cudaStream_t stream,
-                      const pcv_dev_rows* at = nullptr);
 int launch_ln_stats(const pcv_ln_stats_params& p, cudaStream_t stream);
 bool kv_project_supported(const pcv_kvproj_params& p, const char** why);
 int launch_kv_project(const pcv_kvproj_params& p, cudaStream_t stream);

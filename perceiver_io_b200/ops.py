@@ -792,6 +792,13 @@ def _rotary_params(x: torch.Tensor, y: torch.Tensor, num_heads: int, angles: tor
     return p
 
 
+def _launch_rotary(p: RotaryParams, f=None, rows=None) -> None:
+    """Enqueue the rotary launch ``p``: e4m3 output when ``f`` (RotaryFp8) is given, angle and output rows read from
+    device memory when ``rows`` (DevRows) is (pcv_rotary_apply, _fp8, _at, _at_fp8)."""
+    entry = "pcv_rotary_apply" + ("_at" if rows is not None else "") + ("_fp8" if f is not None else "")
+    check(getattr(_lib.lib(), entry)(*(C.byref(s) for s in (p, f, rows) if s is not None), _stream()), entry)
+
+
 def _rotary_angles(angles: torch.Tensor) -> torch.Tensor:
     """``frq_pos_enc`` (B or 1, [1,] n_angles, f) as the rotary kernels take it: 3-D float32, unit stride."""
     if angles.dim() == 4:  # (B, 1, n, f) as stored by RotaryPositionEmbedding
@@ -817,7 +824,7 @@ def _rotary_forward(x: torch.Tensor, num_heads: int, angles: torch.Tensor, right
         return y if out is not None else y.to(out_dtype)
     p = _rotary_params(x, y, num_heads, angles, right_align, _pcv_dtype(cdt))
     with torch.cuda.device(x.device):
-        check(_lib.lib().pcv_rotary_apply(C.byref(p), _stream()), "pcv_rotary_apply")
+        _launch_rotary(p)
     if out is not None:
         return y
     return y if cdt == out_dtype else y.to(out_dtype)
@@ -939,33 +946,32 @@ def _arena_target(cache: torch.Tensor, n: int):
     return buf[:, :L + n], False
 
 
-def _launch_kv_append(k_cache, v_cache, k_new, v_new, k_dst, v_dst, k_in_place, v_in_place, scales=None) -> None:
+def _launch_kv_append(k_cache, v_cache, k_new, v_new, k_dst, v_dst, k_in_place, v_in_place, scales=None,
+                      rows=None) -> None:
     """One launch: dst[:, :L] = cache (skipped for a half appended in place), dst[:, L:] = new rows.  ``scales``: the
-    (k_inv_scale, v_inv_scale) of e4m3 caches (pcv_kv_append_fp8: the new rows are quantised on the way in)."""
-    dt = k_new.dtype
+    (k_inv_scale, v_inv_scale) of e4m3 caches (the new rows are quantised on the way in).  ``rows`` (DevRows, no cache):
+    the new rows go to dst rows ``rows.bounds[0]`` on, read from device memory (pcv_kv_append, _fp8, _at, _at_fp8)."""
     codes = {torch.bfloat16: _lib.PCV_BF16, torch.float16: _lib.PCV_F16, torch.float32: _lib.PCV_F32}
-    B, L_old, Ck = k_cache.shape
     p = KvAppendParams()
-    # an in-place half passes its own destination as the cache pointer: the library skips that copy
-    kc = k_dst if k_in_place else k_cache
-    vc = v_dst if v_in_place else v_cache
-    p.k_cache, p.v_cache = (kc.data_ptr(), vc.data_ptr()) if L_old else (None, None)
+    if k_cache is not None:
+        # an in-place half passes its own destination as the cache pointer: the library skips that copy
+        kc = k_dst if k_in_place else k_cache
+        vc = v_dst if v_in_place else v_cache
+        p.L_old = k_cache.shape[1]
+        p.k_cache, p.v_cache = (kc.data_ptr(), vc.data_ptr()) if p.L_old else (None, None)
+        p.kc_stride_b, p.kc_stride_l = kc.stride(0), kc.stride(1)
+        p.vc_stride_b, p.vc_stride_l = vc.stride(0), vc.stride(1)
     p.k_new, p.v_new, p.k_dst, p.v_dst = k_new.data_ptr(), v_new.data_ptr(), k_dst.data_ptr(), v_dst.data_ptr()
-    p.kc_stride_b, p.kc_stride_l = kc.stride(0), kc.stride(1)
-    p.vc_stride_b, p.vc_stride_l = vc.stride(0), vc.stride(1)
     p.kn_stride_b, p.kn_stride_l = k_new.stride(0), k_new.stride(1)
     p.vn_stride_b, p.vn_stride_l = v_new.stride(0), v_new.stride(1)
     p.kd_stride_b, p.kd_stride_l = k_dst.stride(0), k_dst.stride(1)
     p.vd_stride_b, p.vd_stride_l = v_dst.stride(0), v_dst.stride(1)
-    p.B, p.L_old, p.n, p.Ck, p.Cv = B, L_old, k_new.shape[1], Ck, v_new.shape[2]
-    p.dtype = codes[dt]
+    p.B, p.n, p.Ck, p.Cv = k_new.shape[0], k_new.shape[1], k_new.shape[2], v_new.shape[2]
+    p.dtype = codes[k_new.dtype]
+    f = None if scales is None else _lib.KvFp8Scales(k_inv_scale=scales[0].data_ptr(), v_inv_scale=scales[1].data_ptr())
+    entry = "pcv_kv_append" + ("_at" if rows is not None else "") + ("_fp8" if f is not None else "")
     with torch.cuda.device(k_new.device):
-        if scales is None:
-            check(_lib.lib().pcv_kv_append(C.byref(p), _stream()), "pcv_kv_append")
-        else:
-            f = _lib.KvFp8Scales()
-            f.k_inv_scale, f.v_inv_scale = scales[0].data_ptr(), scales[1].data_ptr()
-            check(_lib.lib().pcv_kv_append_fp8(C.byref(p), C.byref(f), _stream()), "pcv_kv_append_fp8")
+        check(getattr(_lib.lib(), entry)(*(C.byref(s) for s in (p, f, rows) if s is not None), _stream()), entry)
 
 
 def kv_append(k_cache: torch.Tensor, v_cache: torch.Tensor, k_new: torch.Tensor, v_new: torch.Tensor):
@@ -1057,7 +1063,7 @@ def _rotary_fp8(x: torch.Tensor, num_heads: int, angles: torch.Tensor, y: torch.
     f.x_descale = None if x_descale is None else x_descale.data_ptr()
     f.y_inv_scale = y_inv_scale.data_ptr()
     with torch.cuda.device(x.device):
-        check(_lib.lib().pcv_rotary_apply_fp8(C.byref(p), C.byref(f), _stream()), "pcv_rotary_apply_fp8")
+        _launch_rotary(p, f)
 
 
 def rotary_fp8(x8: torch.Tensor, num_heads: int, angles: torch.Tensor, right_align: bool,
@@ -1190,22 +1196,11 @@ def attention_decode_window(q, k, v, bounds: torch.Tensor, num_heads: int, scale
     capacity), indexed by the absolute arena row; ``bounds`` a CUDA int32 tensor whose first two entries are the window.
     The causal mask is right-aligned to the window's end; a window of length <= 0 gives zeros.  Returns (B, N, H*dv)."""
     _require_cuda(q, k, v, bounds, pad_mask)
-    fp8 = k.dtype == F8
     with torch.cuda.device(k.device):
-        if fp8:
-            p, f, keep = _fill_decode_fp8(q, k, v, k_descale, v_descale, num_heads, scale, pad_mask, causal)
-        else:
-            q, k, v, _ = _prep(q, k, v)
-            p, keep = _fill_attn_params(q, k, v, num_heads, scale, pad_mask, causal, None, 0, "decode")
-        rows = _dev_rows(bounds, p.M)
+        p, f, keep = _fill_decode(q, k, v, num_heads, scale, pad_mask, causal, k_descale, v_descale)
         out = _new_output(p, _compute_dtype(q.dtype), k.device)
-        ws = _workspace(p, k.device, "pcv_attn_decode_window", C.byref(p))
-        if fp8:
-            check(_lib.lib().pcv_attn_decode_window_fp8(C.byref(p), C.byref(f), C.byref(rows), _stream()),
-                  "pcv_attn_decode_window_fp8")
-        else:
-            check(_lib.lib().pcv_attn_decode_window(C.byref(p), C.byref(rows), _stream()), "pcv_attn_decode_window")
-    del keep, ws
+        _run_decode(p, f, _dev_rows(bounds, p.M), k.device)
+    del keep
     return out
 
 
@@ -1223,26 +1218,8 @@ def kv_append_at(k_arena: torch.Tensor, v_arena: torch.Tensor, k_new: torch.Tens
         raise ValueError(f"kv_append_at: new rows {k_new.dtype} / {v_new.dtype} into a {k_arena.dtype} arena")
     if k_arena.stride(-1) != 1 or v_arena.stride(-1) != 1:
         raise ValueError("kv_append_at: arenas need unit channel stride")
-    k_new, v_new = _rows_contiguous(k_new), _rows_contiguous(v_new)
-    codes = {torch.bfloat16: _lib.PCV_BF16, torch.float16: _lib.PCV_F16, torch.float32: _lib.PCV_F32}
-    p = KvAppendParams()
-    p.k_cache = p.v_cache = None
-    p.k_new, p.v_new, p.k_dst, p.v_dst = k_new.data_ptr(), v_new.data_ptr(), k_arena.data_ptr(), v_arena.data_ptr()
-    p.kn_stride_b, p.kn_stride_l = k_new.stride(0), k_new.stride(1)
-    p.vn_stride_b, p.vn_stride_l = v_new.stride(0), v_new.stride(1)
-    p.kd_stride_b, p.kd_stride_l = k_arena.stride(0), k_arena.stride(1)
-    p.vd_stride_b, p.vd_stride_l = v_arena.stride(0), v_arena.stride(1)
-    p.B, p.L_old, p.n, p.Ck, p.Cv = k_new.shape[0], 0, k_new.shape[1], k_new.shape[2], v_new.shape[2]
-    p.dtype = codes[k_new.dtype]
-    rows = _dev_rows(row, k_arena.shape[1])
-    with torch.cuda.device(k_new.device):
-        if fp8:
-            f = _lib.KvFp8Scales()
-            f.k_inv_scale, f.v_inv_scale = k_inv_scale.data_ptr(), v_inv_scale.data_ptr()
-            check(_lib.lib().pcv_kv_append_at_fp8(C.byref(p), C.byref(f), C.byref(rows), _stream()),
-                  "pcv_kv_append_at_fp8")
-        else:
-            check(_lib.lib().pcv_kv_append_at(C.byref(p), C.byref(rows), _stream()), "pcv_kv_append_at")
+    _launch_kv_append(None, None, _rows_contiguous(k_new), _rows_contiguous(v_new), k_arena, v_arena, False, False,
+                      (k_inv_scale, v_inv_scale) if fp8 else None, _dev_rows(row, k_arena.shape[1]))
 
 
 def rotary_apply_at(x: torch.Tensor, num_heads: int, table: torch.Tensor, rows: torch.Tensor, out: torch.Tensor,
@@ -1262,15 +1239,9 @@ def rotary_apply_at(x: torch.Tensor, num_heads: int, table: torch.Tensor, rows: 
     if not fp8 and out.dtype != x.dtype:
         raise ValueError(f"rotary_apply_at: `out` {out.dtype} must be x's dtype {x.dtype} or float8_e4m3fn")
     p = _rotary_params(x, out, num_heads, table[None], False, _pcv_dtype(x.dtype))
-    r = _dev_rows(rows, table.shape[0])
+    f = _lib.RotaryFp8(x_descale=None, y_inv_scale=y_inv_scale.data_ptr()) if fp8 else None
     with torch.cuda.device(x.device):
-        if fp8:
-            f = _lib.RotaryFp8()
-            f.x_descale, f.y_inv_scale = None, y_inv_scale.data_ptr()
-            check(_lib.lib().pcv_rotary_apply_at_fp8(C.byref(p), C.byref(f), C.byref(r), _stream()),
-                  "pcv_rotary_apply_at_fp8")
-        else:
-            check(_lib.lib().pcv_rotary_apply_at(C.byref(p), C.byref(r), _stream()), "pcv_rotary_apply_at")
+        _launch_rotary(p, f, _dev_rows(rows, table.shape[0]))
     return out
 
 
@@ -1384,14 +1355,19 @@ def fp8_dequantize(x8: torch.Tensor, descale: torch.Tensor, num_heads: int, dtyp
     return (xs * d).reshape(x8.shape).to(dtype)
 
 
-def _fill_decode_fp8(q, k8, v8, k_descale, v_descale, num_heads, scale, pad_mask, causal):
-    """(AttnParams, DecodeFp8, tensors to keep alive) of an e4m3-cache decode; shapes as in :func:`attention_decode_fp8`."""
-    _require_cuda(q, k8, v8, k_descale, v_descale, pad_mask)
-    if k8.dtype != F8 or v8.dtype != F8:
-        raise ValueError(f"attention_decode_fp8: k8 / v8 must be torch.float8_e4m3fn, got {k8.dtype} / {v8.dtype}")
+def _fill_decode(q, k, v, num_heads, scale, pad_mask, causal, k_descale=None, v_descale=None):
+    """(AttnParams, DecodeFp8 or None, tensors to keep alive) of a decode launch.  bf16 / fp16 K / V rows are taken like
+    :func:`attention` takes them (f None); e4m3 rows, or given descales, are those of :func:`attention_decode_fp8`."""
+    if k.dtype != F8 and v.dtype != F8 and k_descale is None and v_descale is None:
+        q, k, v, _ = _prep(q, k, v)
+        p, keep = _fill_attn_params(q, k, v, num_heads, scale, pad_mask, causal, None, 0, "decode")
+        return p, None, keep
+    _require_cuda(q, k, v, k_descale, v_descale, pad_mask)
+    if k.dtype != F8 or v.dtype != F8:
+        raise ValueError(f"attention_decode_fp8: k8 / v8 must be torch.float8_e4m3fn, got {k.dtype} / {v.dtype}")
     q = _rows_contiguous(q if q.dtype in (torch.bfloat16, torch.float16) else q.to(torch.bfloat16))
-    k8, v8 = _rows_contiguous(k8), _rows_contiguous(v8)
-    p, keep = _fill_attn_params(q, k8, v8, num_heads, scale, pad_mask, causal, None, 0, "decode")
+    k, v = _rows_contiguous(k), _rows_contiguous(v)
+    p, keep = _fill_attn_params(q, k, v, num_heads, scale, pad_mask, causal, None, 0, "decode")
     kd, vd = k_descale.float().contiguous(), v_descale.float().contiguous()
     if kd.shape != (p.H,) or vd.shape != (p.H, p.dv):
         raise ValueError(f"attention_decode_fp8: descales must be (H,) and (H, dv) = ({p.H},), ({p.H}, {p.dv})")
@@ -1400,11 +1376,21 @@ def _fill_decode_fp8(q, k8, v8, k_descale, v_descale, num_heads, scale, pad_mask
     return p, f, keep + (q, kd, vd)
 
 
+def _run_decode(p, f, rows, device) -> None:
+    """Size and attach the workspace of the decode launch ``p`` and enqueue it: e4m3 K / V rows when ``f`` (DecodeFp8)
+    is given, the key window read from device memory when ``rows`` (DevRows) is (pcv_attn_decode_fp8, _window,
+    _window_fp8)."""
+    ws = _workspace(p, device, "pcv_attn_decode_window" if rows is not None else "pcv_attn_decode_fp8", C.byref(p))
+    entry = "pcv_attn_decode" + ("_window" if rows is not None else "") + ("_fp8" if f is not None else "")
+    check(getattr(_lib.lib(), entry)(*(C.byref(s) for s in (p, f, rows) if s is not None), _stream()), entry)
+    del ws
+
+
 def attention_decode_fp8_supported(q, k8, v8, k_descale, v_descale, num_heads: int, scale: float = 1.0,
                                    pad_mask=None, causal: bool = False) -> bool:
     """Whether :func:`attention_decode_fp8` covers these operands (no launch; reason in ``_lib.lib().pcv_last_error()``)."""
     with torch.cuda.device(k8.device):
-        p, f, keep = _fill_decode_fp8(q, k8, v8, k_descale, v_descale, num_heads, scale, pad_mask, causal)
+        p, f, keep = _fill_decode(q, k8, v8, num_heads, scale, pad_mask, causal, k_descale, v_descale)
         dummy = torch.empty(64, device=k8.device)
         p.out = dummy.data_ptr()
         p.o_stride_b, p.o_stride_n, p.o_stride_h = p.N * p.H * p.dv, p.H * p.dv, p.dv
@@ -1420,11 +1406,10 @@ def attention_decode_fp8(q, k8, v8, k_descale, v_descale, num_heads: int, scale:
     :func:`attention`.  Returns (B, N, H*dv) in q's dtype; probabilities stay fp32.  Head dims: multiples of 16, at most
     256.  No autograd: this is an inference path."""
     with torch.cuda.device(k8.device):
-        p, f, keep = _fill_decode_fp8(q, k8, v8, k_descale, v_descale, num_heads, scale, pad_mask, causal)
+        p, f, keep = _fill_decode(q, k8, v8, num_heads, scale, pad_mask, causal, k_descale, v_descale)
         out = _new_output(p, _compute_dtype(q.dtype), k8.device)
-        ws = _workspace(p, k8.device, "pcv_attn_decode_fp8", C.byref(p))
-        check(_lib.lib().pcv_attn_decode_fp8(C.byref(p), C.byref(f), _stream()), "pcv_attn_decode_fp8")
-    del keep, ws
+        _run_decode(p, f, None, k8.device)
+    del keep
     return out
 
 
