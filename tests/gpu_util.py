@@ -249,6 +249,79 @@ def assert_grad_set(got, ref64, eager, mags, dtype, what="", whole=True):
 FLT_MAX = torch.finfo(torch.float32).max
 
 
+# --------------------------------------------------------------------------------------------------
+# The element-wise gate of the streaming decode kernel (csrc/pcv_attn_decode.cu).  The kernel keeps P in fp32: its one
+# 16-bit rounding is the output, so the derived gate (twice eager's error, which rounds P to 16 bits) is far wider than
+# the kernel's own error, and a missing or leaked key in a long row fits inside it.  decode_element_bound follows the
+# kernel's rounding points instead, u = the 16-bit unit roundoff, u32 = 2^-24:
+#   - the output is rounded to 16 bits once:                                              u |o|
+#   - the scores: q is scaled by scale * log2e (and k_descale for e4m3 rows), then dqk products are summed in fp32
+#     (fma chains of 8 / 16 channels and a shuffle tree over the lanes): |dt_j| <= (dqk + 8) u32 A_j with
+#     A_j = scale * log2e * sum_c |q_c k_c|.  A score error moves p_j by ln2 (dt_j - sum_k p_k dt_k) relative, so o moves by
+#     at most ln2 (dqk + 8) u32 (sum_j p_j A_j |v_j| + (sum_j p_j A_j) (sum_j p_j |v_j|));
+#   - ex2 (2 ulp = 2^-22 relative) and the fp32 accumulation of p and p v: each term passes through at most `depth`
+#     roundings and ex2 factors (the keys and block rescales of one lane group, the lane-group shuffle tree, the warps
+#     and the splits; decode_variants.serial_depth), on the numerator and the denominator alike:
+#     2 depth (u32 + 2^-22) sum_j p_j |v_j|;
+#   - fp16 outputs below 2^-14 are subnormal: one absolute spacing 2^-24.
+# The bound is twice the sum of the relative terms plus the spacing.  The factor 2 is what lets the kernel's fp32 error
+# use the space the output rounding leaves: |RN(x) - ref| <= u |ref| + (1 + u) |x - ref|.  The CPU emulation of the
+# kernel's arithmetic in its split and lane-group order (test_decode_variants_cpu.py) stays at or below half of it.
+# --------------------------------------------------------------------------------------------------
+EX2_ULP = 2.0 ** -22
+
+
+def decode_element_bound(q, k, v, H, scale, pad, causal, dtype, depth, ref=None):
+    """(bound, ref) of the decode kernel's element-wise gate (see above), fp64 on k's device, (B, N, H*dv).  q (Bq, N,
+    H*dqk), k (B, M, H*dqk), v (B, M, H*dv) are the operands the kernel computes on (e4m3 rows dequantised); `depth` the
+    longest chain of fp32 roundings a probability passes through."""
+    f64, dev = torch.float64, k.device
+    B, M, N = k.shape[0], k.shape[1], q.shape[1]
+    qh = q.detach().to(dev, f64).expand(B, -1, -1).reshape(B, N, H, -1).transpose(1, 2)
+    kh = k.detach().to(f64).reshape(B, M, H, -1).transpose(1, 2)
+    vh = v.detach().to(dev, f64).reshape(B, M, H, -1).transpose(1, 2)
+    dqk = qh.shape[-1]
+    if ref is None:
+        ref = torch_core(q.to(dev), k, v.to(dev), H, scale, pad, causal, f64)
+    s = (qh * scale) @ kh.transpose(-1, -2)
+    filled = torch.zeros(B, 1, N, M, dtype=torch.bool, device=dev)
+    if pad is not None:
+        filled = filled | pad.to(dev).bool()[:, None, None, :]
+    if causal:
+        filled = filled | torch.ones(N, M, dtype=torch.bool, device=dev).triu(M - N + 1)
+    P = s.masked_fill(filled, -torch.finfo(f64).max).softmax(-1)
+    A = (qh.abs() * (scale * 1.4426950408889634)) @ kh.abs().transpose(-1, -2)
+    va = vh.abs()
+    pv = P @ va
+    pa = P * A
+    score = math.log(2.0) * (dqk + 8) * 2.0 ** -24 * (pa @ va + pa.sum(-1, keepdim=True) * pv)
+    accum = 2.0 * depth * (2.0 ** -24 + EX2_ULP) * pv
+    e32 = (score + accum).transpose(1, 2).reshape(B, N, -1)
+    u = UNIT_ROUNDOFF[dtype]
+    sp = 2.0 ** -24 if dtype == torch.float16 else 0.0
+    return 2.0 * (u * ref.abs() + e32) + sp, ref
+
+
+def assert_decode_elements(got, q, k, v, H, scale, pad, causal, dtype, depth, what=""):
+    """The decode kernel's output against fp64 attention on the same operands: the derived gate row by row
+    (assert_parity(per_row=True)) and the element-wise gate of decode_element_bound.  Returns the worst element's
+    err / bound."""
+    # the row gate's floor is the one output rounding: on a row of few keys eager's error can be smaller by chance
+    assert_parity(got, q, k, v, H, scale, pad, causal, what=what, eager_dtype=dtype, per_row=True,
+                  floor=UNIT_ROUNDOFF[dtype])
+    bound, ref = decode_element_bound(q, k, v, H, scale, pad, causal, dtype, depth)
+    g = got.detach().double().to(ref.device)
+    ratio = (g - ref).abs() / bound
+    flat = int(ratio.argmax().item())
+    idx = tuple(int(i) for i in np.unravel_index(flat, tuple(ratio.shape)))
+    worst = ratio[idx].item()
+    bad = int((ratio > 1).sum().item())
+    print(f"[decode elems] {what}: worst err/bound {worst:.3f} at {idx}: got {g[idx].item():.6e} ref {ref[idx].item():.6e} "
+          f"bound {bound[idx].item():.3e}")
+    assert bad == 0, f"{what}: {bad} of {ratio.numel()} elements over their bound; worst at {idx}"
+    return worst
+
+
 def assert_partial_state(part, q, k, v, H, scale, pad=None, causal=False, m_total=None, m_offset=0, what=""):
     """attention_partial's (o, m, l) against oracle.mha_oracle.partial_state, evaluated in fp64 on the device on the
     same operands (log2 domain: m = row max of the scaled scores, l = sum 2^(t - m), o = sum 2^(t - m) v).
