@@ -244,6 +244,10 @@ typedef struct pcv_peer_combine_params {
  * extra read of x) or — row_stats == NULL and ln_eps > 0 — from the GEMM kernel itself, which computes them in one
  * pass (shifted by the row's first element) from the input tiles it stages anyway.
  * row_stats == NULL and ln_eps == 0 means "no LayerNorm": out = x w^T + t (a plain projection with bias).
+ * A zero-variance row has x_hat == 0, so its output is t exactly (the fold would otherwise scale the fp32 residue of
+ * x.w - mean * s by eps^-1/2).  The in-kernel statistics detect such rows exactly.  With row_stats, pass their eps as
+ * ln_eps: a row whose rstd equals 1 / sqrtf(ln_eps), the value pcv_ln_stats writes when var + eps rounds to eps in
+ * fp32 (var < ~2^-24 eps, |x_hat| < 2^-12 in RMS), is written as t.
  *   x      : (rows, C) with an element row stride (rows = B*M flattened)
  *   k_out  : (rows, n_k), v_out : (rows, n_v), each with its own row stride — the un-rotated, pre-head-split
  *            K / V rows the reference would have produced (and caches, modules.py:117-121)
@@ -263,7 +267,8 @@ typedef struct pcv_kvproj_params {
   int32_t dtype;       /* PCV_BF16 / PCV_F16 */
   int32_t cta_group;   /* 0 = library default (1), 1 = one CTA per tile, 2 = CTA pairs (2-CTA cluster sharing the weight tile) */
   float ln_eps;        /* row_stats == NULL: > 0 = LayerNorm with statistics computed INSIDE the GEMM kernel from the
-                          staged input tiles (no separate pass over x), 0 = no LayerNorm.  Ignored when row_stats is given */
+                          staged input tiles (no separate pass over x), 0 = no LayerNorm.  With row_stats: the eps
+                          they were computed with (0 = unknown: zero-variance rows are not detected) */
 } pcv_kvproj_params;
 
 /* LayerNorm row statistics (nn.LayerNorm semantics: biased variance): stats[r] = (mean, 1/sqrt(var + eps)) */

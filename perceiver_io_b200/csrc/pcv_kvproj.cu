@@ -181,19 +181,28 @@ __device__ __forceinline__ void kvproj_body(const CUtensorMap& tx, const CUtenso
       const float inv_c = 1.f / (float)p.C;
       const float dm = s1 * inv_c;
       const float var = fmaxf(s2 * inv_c - dm * dm, 0.f);
-      sh.row_st[srow] = make_float2(x0 + dm, rsqrtf(var + p.eps));
+      // a constant row (every shifted element is 0) has x_hat == 0: rstd = 0 makes the epilogue write t exactly
+      // instead of amplifying the fp32 residue of x.w' - mean * s by eps^-1/2
+      sh.row_st[srow] = make_float2(x0 + dm, var > 0.f ? rsqrtf(var + p.eps) : 0.f);
     }
     asm volatile("bar.sync %0, 128;" ::"r"(1 + cw) : "memory");
   }
 
+  // given statistics of eps = p.eps > 0: rstd == 1 / sqrtf(0 + eps), the value pcv_ln_stats writes for a zero-variance
+  // row, marks x_hat == 0 (the statistics themselves stay as pcv_ln_linear_bwd reads them)
+  const float rstd_flat = p.eps > 0.f ? 1.f / sqrtf(p.eps) : -1.f;
 #pragma unroll
   for (int r = 0; r < 2; ++r) {
     const int64_t row = row0 + rloc + 8 * r;
     if (row >= p.rows) continue;
     float2 st = make_float2(0.f, 1.f);
     const bool ln = FUSE || p.stats != nullptr;
-    if (FUSE) st = sh.row_st[rloc + 8 * r];
-    else if (p.stats != nullptr) st = p.stats[row];
+    if (FUSE) {
+      st = sh.row_st[rloc + 8 * r];
+    } else if (p.stats != nullptr) {
+      st = p.stats[row];
+      if (st.y == rstd_flat) st.y = 0.f;
+    }
 #pragma unroll
     for (int g = 0; g < 16; ++g) {
       const int n = col0 + 8 * g + cq;
@@ -278,7 +287,9 @@ __global__ void __launch_bounds__(256) ln_stats_reg_kernel(const T* __restrict__
           sum += f.x + f.y;
         }
       }
-      const float mean = warp_sum(sum) * (1.f / (float)C);
+      // divided, not multiplied by RN(1 / C): for C = 1792 that reciprocal is off by more than 2^-25, so a constant
+      // row's mean would land one ulp off its value, give var > 0 and escape the producer's zero-variance rule
+      const float mean = warp_sum(sum) / (float)C;
       float sq = 0.f;
 #pragma unroll
       for (int i = 0; i < NCH; ++i) {

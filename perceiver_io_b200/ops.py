@@ -1437,9 +1437,15 @@ def _check_folded(fn: str, x: torch.Tensor, w_cat: torch.Tensor, col_st: torch.T
 
 
 def _producer_stats(x2: torch.Tensor, eps: Optional[float], mode: str):
-    """``(row statistics, ln_eps)`` of the producer's LayerNorm (``eps`` None: none): pcv_ln_stats, or in-kernel."""
-    fused = eps is not None and mode == "fused"
-    return (None if eps is None or fused else ln_stats(x2, eps)), (eps if fused else 0.0)
+    """``(row statistics, ln_eps)`` of the producer's LayerNorm (``eps`` None: none): pcv_ln_stats, or in-kernel.
+    The kernel computes statistics in-kernel only for ``ln_eps > 0`` (without statistics it reads ``ln_eps = 0`` as "no
+    LayerNorm"), so a LayerNorm with ``eps = 0`` takes pcv_ln_stats whatever the mode.  With statistics, ``ln_eps`` is
+    the eps they were computed with: the kernel writes the folded bias for their zero-variance rows."""
+    if eps is None:
+        return None, 0.0
+    if eps > 0.0 and mode == "fused":
+        return None, eps
+    return ln_stats(x2, eps), eps
 
 
 def _project_rows(x2: torch.Tensor, w_cat, col_st, n_k: int, n_v: int, stats, ln_eps=0.0, cta_group: int = 0):
@@ -1632,7 +1638,7 @@ class _LnLinear(torch.autograd.Function):
         x2 = _rows2d(x)
         with torch.cuda.device(x.device):
             st = ln_stats(x2, eps)
-            k_out, v_out = _project_rows(x2, w_cat, col_st, n_k, n_v, st)
+            k_out, v_out = _project_rows(x2, w_cat, col_st, n_k, n_v, st, eps)
         ctx.save_for_backward(x2, st, w, gamma, beta)
         ctx.dims = (x.shape, n_k, n_v, b is not None)
         outs = [o.view(*lead, o.shape[1]) for o in (k_out, v_out) if o is not None]

@@ -379,3 +379,158 @@ def torch_cross_attention(sd, x_q, x_kv, H, pad=None, dtype=torch.float64, devic
     scale = (q.shape[-1] // H) ** -0.5                                                          # :73
     o = torch_core(q, k, v, H, scale, None if pad is None else pad.to(device), False, dtype)
     return F.linear(o, w[a + "o_proj.weight"], w.get(a + "o_proj.bias"))                        # :168
+
+
+# --------------------------------------------------------------------------------------------------
+# The element-wise gates of the LayerNorm-folded projection (csrc/pcv_kvproj.cu) and its backward (csrc/pcv_lnlin_bwd.cu).
+# u = the output's unit roundoff (2^-8 bf16, 2^-11 fp16, 2^-4 e4m3), u32 = 2^-24.
+#
+# Producer, against the operand-exact reference rstd (x.w'^T - mean s) + t on the kernel's own w' (w_cat) and (s, t)
+# (col_st), mean / rstd in fp64:
+#   - the output is rounded once:                                                         u |ref|
+#   - x.w' is C / 16 fp32 additions of exact k16 partial sums on the tensor core, and the epilogue adds four roundings
+#     (mean s, the difference, rstd, + t):              (C / 16 + 16) u32 (rstd sum_c |x_c w'_c| + rstd mu_abs |s| + |t|)
+#     mu_abs = mean |x| + |x_0| bounds the error of the mean, which sums |x| (two-pass) or |x - x_0| (in-kernel) in fp32;
+#   - rstd's relative error scales rstd (x.w' - mean s) <= rstd (sum |x w'| + |mean| |s|): (C / 32 + 16) u32 for
+#     pcv_ln_stats (a lane's serial sum, the shuffle tree, sqrt, divide); for the in-kernel one-pass statistics the C / 2
+#     serial additions of each half row enter var + (mean - x_0)^2 and leave var, so their term is multiplied by
+#     1 + ((mean - x_0) rstd)^2.
+# The bound is 2 (u |ref| + E32) + one absolute spacing: |RN(y) - ref| <= u |ref| + (1 + u) |y - ref|.  The term
+# rstd mu_abs |s| is the fold's cancellation: a row with |mean| >> std leaves x.w' - mean s to fp32 and multiplies what
+# remains by rstd.  A zero-variance row is written as t exactly (pcv_kvproj.cu); a near-constant row keeps this term.
+# Against module semantics (fp64 LayerNorm -> Linear on the 16-bit parameters) the fold's one rounding of gamma W adds
+# u sum_c |x_hat_c| |gamma_c W_nc|: kernel error on one side, design error on the other.
+# --------------------------------------------------------------------------------------------------
+U32 = 2.0 ** -24
+E4M3_U = 2.0 ** -4
+
+
+def proj_reference(x, w_cat, col_st, eps, fuse=False):
+    """(ref, E32) of the producer: the operand-exact fp64 reference and the fp32 error term above (fp64, (rows, n)).
+    eps None: no LayerNorm (out = x w^T + t)."""
+    xd, wd = x.double(), w_cat.double().to(x.device)
+    cs = col_st.double().to(x.device)
+    s, t = cs[:, 0], cs[:, 1]
+    C = xd.shape[1]
+    xw = xd @ wd.T
+    xwa = xd.abs() @ wd.abs().T
+    if eps is None:
+        return xw + t, (C / 16 + 16) * U32 * (xwa + t.abs())
+    mean = xd.mean(1, keepdim=True)
+    rstd = 1.0 / (xd.var(1, unbiased=False, keepdim=True) + eps).sqrt()
+    ref = rstd * (xw - mean * s) + t
+    mu_abs = xd.abs().mean(1, keepdim=True) + xd[:, :1].abs()
+    e_gemm = (C / 16 + 16) * U32 * (rstd * xwa + rstd * mu_abs * s.abs() + t.abs())
+    if fuse:
+        rel = ((C / 2 + 8) / 2 * (1 + ((mean - xd[:, :1]) * rstd) ** 2) + 8) * U32
+    else:
+        rel = (C / 32 + 16) * U32
+    return ref, e_gemm + rel * rstd * (xwa + mean.abs() * s.abs())
+
+
+def _report(ratio, what, got, ref, bound, tag):
+    flat = int(ratio.argmax().item())
+    idx = tuple(int(i) for i in np.unravel_index(flat, tuple(ratio.shape)))
+    worst = ratio[idx].item()
+    bad = int((ratio > 1).sum().item())
+    print(f"[{tag}] {what}: worst err/bound {worst:.3f} at {idx}: got {got[idx].item():.6e} ref {ref[idx].item():.6e} "
+          f"bound {bound[idx].item():.3e}")
+    assert bad == 0, (f"{what}: {bad} of {ratio.numel()} elements over their bound; worst at {idx}: got "
+                      f"{got[idx].item():.6e} ref {ref[idx].item():.6e} bound {bound[idx].item():.3e}")
+    return worst
+
+
+def assert_proj_elements(got, ref, e32, dtype, what=""):
+    """A 16-bit producer output against the operand-exact reference: |got - ref| <= 2 (u |ref| + E32) + spacing."""
+    g = got.detach().double().to(ref.device)
+    assert g.shape == ref.shape, (what, g.shape, ref.shape)
+    assert torch.isfinite(g).all(), f"{what}: non-finite output"
+    sp = 2.0 ** -24 if dtype == torch.float16 else 0.0
+    bound = 2.0 * (UNIT_ROUNDOFF[dtype] * ref.abs() + e32) + sp
+    return _report((g - ref).abs() / bound, what, g, ref, bound, "proj elems")
+
+
+def assert_e4m3_codes(codes, ref, e32, inv_scale, what=""):
+    """e4m3 producer codes against RN(ref * inv_scale): a code may differ from it only where a rounding midpoint lies
+    within 2 E32 of ref, i.e. its value must lie between RN((ref - 2 E32) inv) and RN((ref + 2 E32) inv)."""
+    f8 = torch.float8_e4m3fn
+    inv = inv_scale.double().to(ref.device)
+    q = lambda v: (v * inv).clamp(-448.0, 448.0).float().to(f8).view(torch.uint8)
+    lo, hi, mid = q(ref - 2.0 * e32), q(ref + 2.0 * e32), q(ref)
+    c = codes.detach().to(ref.device).view(torch.uint8)
+    val = lambda u8: u8.view(f8).double()
+    ok = (val(c) >= val(lo)) & (val(c) <= val(hi))
+    exact = int((c == mid).sum().item())
+    print(f"[e4m3 codes] {what}: {exact} of {c.numel()} codes equal RN(ref * inv); "
+          f"{int((~ok).sum().item())} outside the midpoint band")
+    if not bool(ok.all()):
+        bad = (~ok).nonzero()[0].tolist()
+        raise AssertionError(f"{what}: code {int(c[tuple(bad)])} at {bad} is neither RN of ref +- 2 E32 "
+                             f"({int(lo[tuple(bad)])}, {int(hi[tuple(bad)])}); ref {ref[tuple(bad)].item():.6e}")
+    return exact
+
+
+def fold_term(x, gamma, w, eps, dtype):
+    """u sum_c |x_hat_c| |gamma_c W_nc|: the one rounding of the folded weights gamma W (fp64, (rows, n))."""
+    xd = x.double()
+    xh = (xd - xd.mean(1, keepdim=True)) / (xd.var(1, unbiased=False, keepdim=True) + eps).sqrt()
+    gw = (w.double() * gamma.double().to(w.device)[None, :]).abs()
+    return UNIT_ROUNDOFF[dtype] * xh.abs() @ gw.to(xd.device).T
+
+
+# --------------------------------------------------------------------------------------------------
+# The backward's element-wise gate.  With x_hat rebuilt in fp32 from x and the statistics, its 16-bit rounding points
+# (pcv_lnlin_bwd.cu) are: dx_hat = gamma dy is written to grad_x in 16 bits before the fixup reads it back; x_hat is
+# rounded to 16 bits before the dW GEMM; every output is rounded once.  So dx and dW carry 2u of their magnitude
+# gradient, db / dgamma / dbeta 1u.  The fp32 sums add `depth` u32 each: dx (n / 16 tensor-core adds, the column-tile
+# partials, the fixup), dW (the rows of a split on the tensor core, the splits, the rank-1 term), db (a thread's serial
+# sum over the rows of a split, the splits), dgamma / dbeta (two rows per thread, the shuffle tree, 8 warps, the row
+# blocks of a range, the ranges).  The magnitudes are the closed-form gradient on |G|, |W|, |x_hat|, |gamma|, |beta|:
+#   dy_a = |G| |W|, dxh_a = |gamma| dy_a, dx_a = rstd (dxh_a + (sum dxh_a + |x_hat| sum dxh_a |x_hat|) / C),
+#   dW_a = (|x_hat|^T |G|) |gamma| + db_a |beta|, db_a = sum |G|, dgamma_a = sum dy_a |x_hat|, dbeta_a = sum dy_a.
+# The bound is 2 (rounds u + depth u32) abs + spacing (fp16: 2^-24 times (1 + 2 rstd) for dx, whose dx_hat may be
+# subnormal).
+# --------------------------------------------------------------------------------------------------
+def lnlin_magnitudes(x, stats, w, gamma, beta, G):
+    """(dx, dW, db, dgamma, dbeta) magnitudes and (rstd) of the backward, fp64 on x's device."""
+    xd = x.double()
+    st = stats.double()
+    rstd = st[:, 1:2]
+    xh = ((xd - st[:, :1]) * rstd).abs()
+    C = xd.shape[1]
+    g = torch.ones(C, dtype=torch.float64, device=xd.device) if gamma is None else gamma.double().abs()
+    b = torch.zeros(C, dtype=torch.float64, device=xd.device) if beta is None else beta.double().abs()
+    Ga, Wa = G.double().abs(), w.double().abs()
+    dy = Ga @ Wa
+    dxh = dy * g
+    dx = rstd * (dxh + (dxh.sum(1, keepdim=True) + xh * (dxh * xh).sum(1, keepdim=True)) / C)
+    db = Ga.sum(0)
+    dW = (xh.T @ Ga).T * g[None, :] + db[:, None] * b[None, :]
+    return (dx, dW, db, (dy * xh).sum(0), dy.sum(0)), rstd
+
+
+def lnlin_element_bounds(mags, rstd, dtype, rows, C, n, splits, m_blocks):
+    u = UNIT_ROUNDOFF[dtype]
+    rps = -(-rows // splits)
+    depth = (n / 16 + C / 128 + 8, rps / 16 + splits + 8, rps / 2 + splits + 4, 16 + m_blocks / 8 + 8,
+             16 + m_blocks / 8 + 8)
+    rounds = (2, 2, 1, 1, 1)
+    sp = 2.0 ** -24 if dtype == torch.float16 else 0.0
+    out = []
+    for i, (m, d, r) in enumerate(zip(mags, depth, rounds)):
+        extra = sp * (1 + 2 * rstd) if i == 0 else sp
+        out.append(2.0 * (r * u + d * U32) * m + extra)
+    return out
+
+
+def assert_lnlin_elements(got, ref, bounds, names, what=""):
+    """Each requested backward output against fp64 autograd under its element bound; returns {name: worst}."""
+    out = {}
+    for name, g_, r_, b_ in zip(names, got, ref, bounds):
+        if g_ is None:
+            continue
+        g = g_.detach().double().to(r_.device)
+        assert g.shape == r_.shape, (what, name, g.shape, r_.shape)
+        assert torch.isfinite(g).all(), f"{what} {name}: non-finite"
+        out[name] = _report((g - r_.double()).abs() / b_, f"{what} {name}", g, r_.double(), b_, "lnlin elems")
+    return out
