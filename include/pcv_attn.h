@@ -518,6 +518,22 @@ PCV_API int pcv_attn_decode_fp8_workspace_bytes(const pcv_attn_params* p, size_t
 PCV_API int pcv_attn_decode_fp8(const pcv_attn_params* p, const pcv_decode_fp8* f, void* stream);
 
 /*
+ * pcv_attn_cached_fp8: attention of 1 to 64 query rows on an e4m3 cache on the tensor cores: a cached step that
+ * appends several tokens at once.  Operands, descales and result as in pcv_attn_decode_fp8: attention on (q,
+ * k8 * k_descale[h], v8 * v_descale[h, c]), with q and out bf16 / fp16 (dtype) and k / v e4m3 rows whose strides are
+ * multiples of 16.  The e4m3 tiles are converted to q's 16-bit type in shared memory (exact); q enters unrounded;
+ * scale * k_descale[h] multiplies the fp32 scores once, in the exponent; P is rounded to q's 16-bit type before P V
+ * (as in pcv_attn_fwd's tensor-core kernel) and v_descale multiplies the fp32 accumulator once.  Masks and batch-1 q
+ * as in pcv_attn_fwd.  N <= 64 query rows, any M >= 1, head dims multiples of 16 and at most 256 (independently);
+ * impl AUTO.  It writes `out` only: write_partial and key shards are refused, as are an e4m3 q and NULL descales.
+ * The workspace is pcv_attn_cached_fp8_workspace_bytes() of the same params; one launch, bitwise reproducible.
+ * Arguments are checked before any CUDA call.
+ */
+PCV_API int pcv_attn_cached_fp8_supported(const pcv_attn_params* p, const pcv_decode_fp8* f);
+PCV_API int pcv_attn_cached_fp8_workspace_bytes(const pcv_attn_params* p, size_t* bytes);
+PCV_API int pcv_attn_cached_fp8(const pcv_attn_params* p, const pcv_decode_fp8* f, void* stream);
+
+/*
  * pcv_kv_append_fp8: pcv_kv_append onto e4m3 caches.  p->dtype (PCV_BF16 / PCV_F16) is that of k_new / v_new; k_cache,
  * v_cache, k_dst and v_dst are e4m3 (strides in bytes).  The old rows are copied byte for byte (skipped for a half
  * whose cache pointer equals its dst pointer, as in pcv_kv_append); new row channel c becomes

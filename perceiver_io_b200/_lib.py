@@ -60,6 +60,9 @@ EXPORTS = (
     "pcv_attn_decode_fp8_supported",
     "pcv_attn_decode_fp8_workspace_bytes",
     "pcv_attn_decode_fp8",
+    "pcv_attn_cached_fp8_supported",
+    "pcv_attn_cached_fp8_workspace_bytes",
+    "pcv_attn_cached_fp8",
     "pcv_kv_append_fp8_supported",
     "pcv_kv_append_fp8",
     "pcv_rotary_fp8_supported",
@@ -381,6 +384,12 @@ def lib() -> C.CDLL:
         l.pcv_attn_decode_fp8_workspace_bytes.restype = C.c_int
         l.pcv_attn_decode_fp8.argtypes = [C.POINTER(AttnParams), C.POINTER(DecodeFp8), C.c_void_p]
         l.pcv_attn_decode_fp8.restype = C.c_int
+        l.pcv_attn_cached_fp8_supported.argtypes = [C.POINTER(AttnParams), C.POINTER(DecodeFp8)]
+        l.pcv_attn_cached_fp8_supported.restype = C.c_int
+        l.pcv_attn_cached_fp8_workspace_bytes.argtypes = [C.POINTER(AttnParams), C.POINTER(C.c_size_t)]
+        l.pcv_attn_cached_fp8_workspace_bytes.restype = C.c_int
+        l.pcv_attn_cached_fp8.argtypes = [C.POINTER(AttnParams), C.POINTER(DecodeFp8), C.c_void_p]
+        l.pcv_attn_cached_fp8.restype = C.c_int
         l.pcv_kv_append_fp8_supported.argtypes = [C.POINTER(KvAppendParams), C.POINTER(KvFp8Scales)]
         l.pcv_kv_append_fp8_supported.restype = C.c_int
         l.pcv_kv_append_fp8.argtypes = [C.POINTER(KvAppendParams), C.POINTER(KvFp8Scales), C.c_void_p]

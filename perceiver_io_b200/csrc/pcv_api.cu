@@ -483,6 +483,34 @@ int pcv_attn_decode_fp8(const pcv_attn_params* p, const pcv_decode_fp8* f, void*
   return decode_launch(p, f, nullptr, true, false, stream);
 }
 
+// The tensor-core attention of 1 to 64 query rows on an e4m3 cache (pcv_attn_cached.cu).
+static int cached_check(const pcv_attn_params* p, const pcv_decode_fp8* f) {
+  PCV_REQUIRE(f != nullptr, PCV_ERR_INVALID, "attn_cached_fp8: fp8 params are NULL");
+  int rc = validate_attn(p);
+  if (rc != PCV_OK) return rc;
+  const char* why = "";
+  PCV_REQUIRE(attn_cached_fp8_supported(*p, *f, &why), PCV_ERR_UNSUPPORTED,
+              "cached e4m3 attention not applicable: %s", why);
+  return PCV_OK;
+}
+
+int pcv_attn_cached_fp8_supported(const pcv_attn_params* p, const pcv_decode_fp8* f) {
+  return cached_check(p, f) == PCV_OK ? 1 : 0;
+}
+
+int pcv_attn_cached_fp8_workspace_bytes(const pcv_attn_params* p, size_t* bytes) {
+  int rc = validate_attn(p);
+  if (rc != PCV_OK) return rc;
+  PCV_REQUIRE(bytes != nullptr, PCV_ERR_INVALID, "attn_cached_fp8: bytes is NULL");
+  return attn_cached_fp8_workspace_bytes(*p, bytes);
+}
+
+int pcv_attn_cached_fp8(const pcv_attn_params* p, const pcv_decode_fp8* f, void* stream) {
+  const int rc = cached_check(p, f);
+  if (rc != PCV_OK) return rc;
+  return launch_attn_cached_fp8(*p, *f, reinterpret_cast<cudaStream_t>(stream));
+}
+
 int pcv_kv_append_fp8_supported(const pcv_kv_append_params* p, const pcv_kv_fp8_scales* f) {
   if (p == nullptr || f == nullptr) {
     set_error("kv_append_fp8: params are NULL");

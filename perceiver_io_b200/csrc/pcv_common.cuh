@@ -128,6 +128,10 @@ int debug_plan(int B, int H, int N, int M, int workers, int rows_per_unit, int r
 bool attn_decode_supported(const pcv_attn_params& p, const pcv_decode_fp8* f, const pcv_dev_rows* rows, const char** why);
 int launch_attn_decode(const pcv_attn_params& p, const pcv_decode_fp8* f, const pcv_dev_rows* rows, cudaStream_t stream);
 int attn_decode_workspace_bytes(const pcv_attn_params& p, size_t* bytes);
+// the tensor-core attention of 1 to 64 query rows over e4m3 K / V rows (pcv_attn_cached_fp8, pcv_attn_cached.cu)
+bool attn_cached_fp8_supported(const pcv_attn_params& p, const pcv_decode_fp8& f, const char** why);
+int attn_cached_fp8_workspace_bytes(const pcv_attn_params& p, size_t* bytes);
+int launch_attn_cached_fp8(const pcv_attn_params& p, const pcv_decode_fp8& f, cudaStream_t stream);
 
 int launch_combine(const pcv_combine_params& p, cudaStream_t stream);
 // Merge `nparts` partial states laid out [part][B][H][N]([dv]) either into p.out (normalised) or,

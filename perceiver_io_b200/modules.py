@@ -145,13 +145,20 @@ def attend(mha, q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, pad_mask=None
     return ModuleOutput(last_hidden_state=o, kv_cache=kv_cache)
 
 
+#: Query rows up to which a cached step on an FP8 KV cache reads the e4m3 rows directly (ops.attention_decode_fp8).
+KV8_MAX_ROWS = 64
+
+
 def _attend_kv8(mha, q, k, v, pad_mask, rot_pos_emb_q, rot_pos_emb_k, kv_cache, min_rows_key, kv8):
     """``attend`` with an FP8 (e4m3) KV cache: the new rows are quantised into the cache (ops.kv_append_fp8).  An empty
     incoming cache (the prompt) attends over this call's own bf16 / fp16 rows.  A cached step takes its rotated keys
     from the e4m3 shadow (ops.rotated_cache_keys) when the rotary object carries the frequency table (``inv_freq``, as
     this package's models pass it); without one (the reference's RotaryPositionEmbedding) the whole cache is rotated at
-    the window-relative angles, e4m3 to e4m3 (ops.rotary_fp8), as the reference rotates it every step.  With at most 4
-    query rows the e4m3 decode kernel runs; more query rows dequantise the cache and take the bf16 path (correct, slow)."""
+    the window-relative angles, e4m3 to e4m3 (ops.rotary_fp8), as the reference rotates it every step.  Up to
+    ``KV8_MAX_ROWS`` (64) query rows read the e4m3 rows directly (ops.attention_decode_fp8: the streaming decode kernel
+    up to 4 rows, the tensor-core kernel that converts e4m3 tiles in shared memory from 5 to 64).  More query rows
+    dequantise the cache and take the bf16 path: there the O(N M) attention amortises the O(M) conversion, and the
+    tuned forward kernel is the better one."""
     H = mha.num_heads
     L_old = kv_cache[0].shape[1]
     k8, v8 = ops.kv_append_fp8(kv_cache[0], kv_cache[1], k, v, kv8.k_inv, kv8.v_inv)
@@ -163,7 +170,7 @@ def _attend_kv8(mha, q, k, v, pad_mask, rot_pos_emb_q, rot_pos_emb_k, kv_cache, 
         if shadowed:   # the prompt's own rows, rotated like q at the shadow's absolute positions
             k_att = ops.rotary_at(k, H, rot_pos_emb_k.inv_freq, ops.rotated_cache_shadow(k8)[1])
         o = ops.attention(q_att, k_att, v, H, mha.dp_scale, pad_mask=pad_mask, causal=mha.causal_attention, impl=impl)
-    elif q.shape[1] <= 4:
+    elif q.shape[1] <= KV8_MAX_ROWS:
         o = ops.attention_decode_fp8(q_att, k_att, v8, kv8.k_descale, kv8.v_descale, H, mha.dp_scale,
                                      pad_mask=pad_mask, causal=mha.causal_attention)
     else:
@@ -307,8 +314,10 @@ def project_qkv(self_attn, x: torch.Tensor):
 #: a q / K / V chain autograd needs (``_needs_grad``), fp32, rotary, a KV cache, head dims that are not multiples of 16,
 #: dqk > 256 or dv > 512) take the bf16 path.
 #: ``kv_cache``: FP8 (e4m3) KV caches for cached generation, independent of ``enabled``: an empty incoming cache of a
-#: covered CrossAttention / SelfAttention call becomes an e4m3 cache (``_kv8_route``), whose cached steps run the e4m3
-#: decode kernel (``_attend_kv8``).  Off by default because it changes the numbers.
+#: covered CrossAttention / SelfAttention call becomes an e4m3 cache (``_kv8_route``), whose cached steps of up to 64
+#: new tokens read the e4m3 rows directly (the e4m3 decode kernel up to 4, the tensor-core kernel of
+#: ``pcv_attn_cached_fp8`` from 5 to 64; ``_attend_kv8``); longer steps dequantise the cache.  Off by default because
+#: it changes the numbers.
 fp8_config = {"enabled": False, "kv_cache": False}
 
 

@@ -1376,12 +1376,27 @@ def _fill_decode(q, k, v, num_heads, scale, pad_mask, causal, k_descale=None, v_
     return p, f, keep + (q, kd, vd)
 
 
+#: Query rows up to which an e4m3-cache call runs the streaming decode kernel; more rows (up to 64) take the
+#: tensor-core kernel of pcv_attn_cached_fp8.
+DECODE_MAX_ROWS = 4
+
+
+def _fp8_entry(p, f, rows) -> str:
+    """The entry point of a decode launch: pcv_attn_cached_fp8 for e4m3 rows of more than DECODE_MAX_ROWS query rows
+    without a window (its impl is AUTO), else pcv_attn_decode(_window)(_fp8)."""
+    if f is not None and rows is None and p.N > DECODE_MAX_ROWS:
+        p.impl = _lib.PCV_IMPL_AUTO
+        return "pcv_attn_cached_fp8"
+    return "pcv_attn_decode" + ("_window" if rows is not None else "") + ("_fp8" if f is not None else "")
+
+
 def _run_decode(p, f, rows, device) -> None:
     """Size and attach the workspace of the decode launch ``p`` and enqueue it: e4m3 K / V rows when ``f`` (DecodeFp8)
     is given, the key window read from device memory when ``rows`` (DevRows) is (pcv_attn_decode_fp8, _window,
-    _window_fp8)."""
-    ws = _workspace(p, device, "pcv_attn_decode_window" if rows is not None else "pcv_attn_decode_fp8", C.byref(p))
-    entry = "pcv_attn_decode" + ("_window" if rows is not None else "") + ("_fp8" if f is not None else "")
+    _window_fp8, or pcv_attn_cached_fp8 for 5 to 64 query rows on e4m3 rows)."""
+    entry = _fp8_entry(p, f, rows)
+    sizer = "pcv_attn_decode_window" if rows is not None else "pcv_attn_decode_fp8"  # the four decode entries' workspace
+    ws = _workspace(p, device, entry if entry == "pcv_attn_cached_fp8" else sizer, C.byref(p))
     check(getattr(_lib.lib(), entry)(*(C.byref(s) for s in (p, f, rows) if s is not None), _stream()), entry)
     del ws
 
@@ -1394,17 +1409,20 @@ def attention_decode_fp8_supported(q, k8, v8, k_descale, v_descale, num_heads: i
         dummy = torch.empty(64, device=k8.device)
         p.out = dummy.data_ptr()
         p.o_stride_b, p.o_stride_n, p.o_stride_h = p.N * p.H * p.dv, p.H * p.dv, p.dv
-        return bool(_lib.lib().pcv_attn_decode_fp8_supported(C.byref(p), C.byref(f)))
+        entry = _fp8_entry(p, f, None)
+        return bool(getattr(_lib.lib(), entry + "_supported")(C.byref(p), C.byref(f)))
 
 
 def attention_decode_fp8(q, k8, v8, k_descale, v_descale, num_heads: int, scale: float, pad_mask=None,
                          causal: bool = False) -> torch.Tensor:
-    """Attention of at most 4 query rows on an FP8 (e4m3) KV cache (pcv_attn_decode_fp8, the streaming decode kernel).
+    """Attention of 1 to 64 query rows on an FP8 (e4m3) KV cache.
 
-    q: (B or 1, N <= 4, H*dqk) bf16 / fp16; k8: (B, M, H*dqk), v8: (B, M, H*dv) ``torch.float8_e4m3fn`` rows standing for
+    q: (B or 1, N <= 64, H*dqk) bf16 / fp16; k8: (B, M, H*dqk), v8: (B, M, H*dv) ``torch.float8_e4m3fn`` rows standing for
     ``k8 * k_descale[h]`` and ``v8[..., h, c] * v_descale[h, c]`` (float32 (H,) and (H, dv)).  Masks as in
-    :func:`attention`.  Returns (B, N, H*dv) in q's dtype; probabilities stay fp32.  Head dims: multiples of 16, at most
-    256.  No autograd: this is an inference path."""
+    :func:`attention`.  Returns (B, N, H*dv) in q's dtype.  Up to DECODE_MAX_ROWS (4) query rows run the streaming
+    decode kernel (pcv_attn_decode_fp8), whose probabilities stay fp32; 5 to 64 rows the tensor-core kernel
+    (pcv_attn_cached_fp8), which converts the e4m3 tiles to q's dtype in shared memory and rounds P to q's dtype before
+    P V, as :func:`attention` does.  Head dims: multiples of 16, at most 256.  No autograd: this is an inference path."""
     with torch.cuda.device(k8.device):
         p, f, keep = _fill_decode(q, k8, v8, num_heads, scale, pad_mask, causal, k_descale, v_descale)
         out = _new_output(p, _compute_dtype(q.dtype), k8.device)
