@@ -684,6 +684,12 @@ PCV_API int pcv_debug_trace_read(uint64_t* out, int32_t n);
 PCV_API int pcv_debug_plan(int32_t B, int32_t H, int32_t N, int32_t M, int32_t workers, int32_t rows_per_unit,
                            int32_t rows_per_tile, int32_t* segs, int32_t max_segs, int32_t* counts);
 
+/*
+ * The current device's CTA-pair plan: *workers CTA pairs, of the *clusters_fit 2-CTA clusters of the pair kernel that
+ * can be resident at once (cudaOccupancyMaxActiveClusters).
+ */
+PCV_API int pcv_debug_pair_workers(int32_t* workers, int32_t* clusters_fit);
+
 /* number of kernel launches issued by this library in the calling process (for bench.py's
  * gpu_launches claim) */
 PCV_API uint64_t pcv_launch_count(void);

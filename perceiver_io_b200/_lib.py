@@ -81,6 +81,7 @@ EXPORTS = (
     "pcv_ln_linear_bwd",
     "pcv_launch_count",
     "pcv_debug_plan",
+    "pcv_debug_pair_workers",
     "pcv_profile_begin",
     "pcv_profile_end",
     "pcv_debug_read",
@@ -420,6 +421,8 @@ def lib() -> C.CDLL:
         l.pcv_ln_linear_bwd.restype = C.c_int
         l.pcv_debug_plan.argtypes = [C.c_int32] * 7 + [C.POINTER(C.c_int32), C.c_int32, C.POINTER(C.c_int32)]
         l.pcv_debug_plan.restype = C.c_int
+        l.pcv_debug_pair_workers.argtypes = [C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
+        l.pcv_debug_pair_workers.restype = C.c_int
         for name in ("pcv_get_device_info", "pcv_attn_supported_tcgen05", "pcv_attn_workspace_bytes",
                      "pcv_attn_fwd", "pcv_attn_combine", "pcv_rotary_apply", "pcv_kv_append",
                      "pcv_partial_rescale"):
@@ -466,6 +469,13 @@ def debug_plan(B, H, N, M, workers=132, rows_per_unit=128):
     check(lib().pcv_debug_plan(B, H, N, M, workers, rows_per_unit, 128, segs, n, counts), "pcv_debug_plan")
     recs = [tuple(segs[8 * i + j] for j in range(8)) for i in range(n)]
     return {"segments": counts[0], "ctas": counts[1], "slots": counts[2], "units": counts[3]}, recs
+
+
+def debug_pair_workers():
+    """-> (CTA pairs of the current device's pair plan, 2-CTA clusters of the pair kernel that can be resident)."""
+    w, fit = C.c_int32(0), C.c_int32(0)
+    check(lib().pcv_debug_pair_workers(C.byref(w), C.byref(fit)), "pcv_debug_pair_workers")
+    return w.value, fit.value
 
 
 def launch_count() -> int:

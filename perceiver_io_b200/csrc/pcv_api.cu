@@ -155,6 +155,11 @@ int pcv_debug_plan(int32_t B, int32_t H, int32_t N, int32_t M, int32_t workers, 
   return debug_plan(B, H, N, M, workers, rows_per_unit, rows_per_tile, segs, max_segs, counts);
 }
 
+int pcv_debug_pair_workers(int32_t* workers, int32_t* clusters_fit) {
+  PCV_REQUIRE(workers != nullptr && clusters_fit != nullptr, PCV_ERR_INVALID, "debug_pair_workers: NULL argument");
+  return debug_pair_workers(workers, clusters_fit);
+}
+
 uint64_t pcv_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }
 
 int pcv_get_device_info(pcv_device_info* info) {

@@ -12,7 +12,9 @@
 // (b, h) and key range; each CTA loads one 64-key half of every K / V box and multicasts it to both, so the pair
 // reads each key tile from L2 once.  A ring slot is refilled only after the consumers of BOTH CTAs released it.  Q stays in shared
 // memory for the segment; K and V arrive as 128-key x 64-channel boxes through one ring of 16 KB slots guarded
-// by full / empty mbarriers, so every head dim (up to 512 for Q/K) uses the same pipeline.  V is processed in
+// by full / empty mbarriers, so every head dim (up to 512 for Q/K) uses the same pipeline: at head dims up to 128 one
+// pair per tile's K boxes and one per its V boxes, each released by one arrive per consumer warpgroup (and CTA of
+// a pair), so a tile costs two waits and two releases.  V is processed in
 // passes of at most 128 channels (one launch per pass) to keep the accumulators in registers.
 //
 // Work distribution is a host-built segment table (stream-K over the key axis): segments that cover a
@@ -467,7 +469,7 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
   if (threadIdx.x == 0) {
     for (int s = 0; s < NS; ++s) {
       mbar_init(&bar.full[s], 1);
-      mbar_init(&bar.empty[s], PAIR ? 16 : 8);  // one arrive per consumer warp (of both CTAs of a pair)
+      mbar_init(&bar.empty[s], PAIR ? 4 : 2);  // one arrive per consumer warpgroup (of both CTAs of a pair)
     }
     mbar_init(&bar.q_full, 1);
     mbar_init(&bar.q_empty, 8);
@@ -489,21 +491,43 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
         for (int c = 0; c < NQB; ++c)
           tma_load_4d(sQ + c * kBoxBytes, &tq, &bar.q_full, c * kQkCh, sg.q0 + qoff, sg.h, p.q_bcast ? 0 : sg.b);
         for (int t = sg.t0; t < sg.t1; ++t) {
-#pragma unroll 1
-          for (int c = 0; c < NQB + KVB; ++c, ++it) {
-            const uint32_t s = it % NS;
-            mbar_wait(&bar.empty[s], ((it / NS) & 1) ^ 1, 2);
-            mbar_arrive_expect_tx(&bar.full[s], kBoxBytes);
+          // box c of the tile into ring slot s, its bytes counted on full barrier fb
+          auto load_box = [&](int c, uint32_t s, uint64_t* fb) {
+            uint8_t* dst = sRing + s * kBoxBytes;
             const CUtensorMap* tm = c < NQB ? &tk : &tv;
             const int ch = (c < NQB ? c : c - NQB) * 64;
             if constexpr (FP8) {  // K: (channel box c, keys of tile t); V^T: (keys of tile t, channels of the pass)
-              if (c < NQB) tma_load_4d(sRing + s * kBoxBytes, tm, &bar.full[s], c * kQkCh, t * kTileN, sg.h, sg.b);
-              else tma_load_4d(sRing + s * kBoxBytes, tm, &bar.full[s], t * kTileN, 0, sg.h, sg.b);
+              if (c < NQB) tma_load_4d(dst, tm, fb, c * kQkCh, t * kTileN, sg.h, sg.b);
+              else tma_load_4d(dst, tm, fb, t * kTileN, 0, sg.h, sg.b);
             } else if (PAIR)  // 64-key half `rank` of the box, into both CTAs
-              tma_load_4d_mc(sRing + s * kBoxBytes + rank * (kBoxBytes / 2), tm, &bar.full[s], ch,
-                             t * kTileN + 64 * (int)rank, sg.h, sg.b, 0x3);
+              tma_load_4d_mc(dst + rank * (kBoxBytes / 2), tm, fb, ch, t * kTileN + 64 * (int)rank, sg.h, sg.b, 0x3);
             else
-              tma_load_4d(sRing + s * kBoxBytes, tm, &bar.full[s], ch, t * kTileN, sg.h, sg.b);
+              tma_load_4d(dst, tm, fb, ch, t * kTileN, sg.h, sg.b);
+          };
+          // the next nb boxes, from ring index it on: wait until their slots are free, expect their bytes
+          auto begin_group = [&](int nb) {
+            const uint32_t g = it % NS;
+            mbar_wait(&bar.empty[g], ((it / NS) & 1) ^ 1, 2);
+            mbar_arrive_expect_tx(&bar.full[g], nb * kBoxBytes);
+            it += nb;
+            return g;
+          };
+          // The pipelined schedule guards the K boxes of a tile with one full / empty pair and its V boxes with
+          // another, those of the group's first slot (a tile's boxes never wrap around the ring); the serial schedule
+          // every box with its own.
+          if constexpr (kPipelined) {
+            const uint32_t gk = begin_group(NQB);
+#pragma unroll
+            for (int c = 0; c < NQB; ++c) load_box(c, gk + c, &bar.full[gk]);
+            const uint32_t gv = begin_group(KVB);
+#pragma unroll
+            for (int c = 0; c < KVB; ++c) load_box(NQB + c, gv + c, &bar.full[gv]);
+          } else {
+#pragma unroll 1
+            for (int c = 0; c < NQB + KVB; ++c) {
+              const uint32_t s = begin_group(1);
+              load_box(c, s, &bar.full[s]);
+            }
           }
         }
       }
@@ -526,14 +550,14 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
   uint32_t it = 0;  // ring index of the next box (the producer's order: the NQB K boxes, then the NVB V boxes of a tile)
 
   auto wait_full = [&](uint32_t i, uint32_t site) { mbar_wait(&bar.full[i % NS], (i / NS) & 1, site); };
+  // releases the box group (see the producer) whose first box is ring index i
   auto release = [&](uint32_t i) {
-    if (PAIR) warp_arrive_pair(&bar.empty[i % NS]);
-    else warp_arrive(&bar.empty[i % NS]);
+    if (PAIR) wg_arrive_pair(&bar.empty[i % NS]);
+    else wg_arrive(&bar.empty[i % NS]);
   };
   // S = Q K^T of the tile whose first K box is ring index i: one commit group
   auto issue_qk = [&](float (&s)[64], uint32_t i) {
-#pragma unroll
-    for (int c = 0; c < NQB; ++c) wait_full(i + c, 6);
+    wait_full(i, 6);
     wgmma_fence();
 #pragma unroll
     for (int c = 0; c < NQB; ++c)
@@ -554,8 +578,7 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
   using PFrag = uint32_t[FP8 ? 4 : 8][4];
   // O += P V of the tile whose first V box is ring index i: one commit group
   auto issue_pv = [&](float (&o)[NVB][32], const PFrag& pa, uint32_t i) {
-#pragma unroll
-    for (int v = 0; v < KVB; ++v) wait_full(i + v, 7);
+    wait_full(i, 7);
     wgmma_fence();
     if constexpr (FP8) {
 #pragma unroll
@@ -580,17 +603,9 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
   };
   // after the P V whose first V box is ring index i completed: O is final in registers, release the V boxes
   auto pv_done = [&](float (&o)[NVB][32], uint32_t i) {
-    if constexpr (FP8) {
 #pragma unroll
-      for (int v = 0; v < NVB; ++v) fence_regs(o[v]);
-      release(i);
-    } else {
-#pragma unroll
-      for (int v = 0; v < NVB; ++v) {
-        fence_regs(o[v]);
-        release(i + v);
-      }
-    }
+    for (int v = 0; v < NVB; ++v) fence_regs(o[v]);
+    release(i);
   };
   // Ping-pong turns.  Warpgroup cw waits on its own named barrier (id 1 + cw) before it issues its GEMMs and hands
   // the turn over by arriving on the other's (id 2 - cw) after it committed them; a phase counts 256 threads (128
@@ -649,8 +664,7 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
         turn_end(false);
         wgmma_wait<0>();
         fence_regs(s);
-#pragma unroll
-        for (int c = 0; c < NQB; ++c) release(ik + c);
+        release(ik);
         tile_softmax<DROP, FP8>(s, m_run, l_run, alpha, p, sg.b, sg.t0 * kTileN, n0, cq, interior(sg.t0 * kTileN), qside,
                                 sl2);
         pack(s, pa);
@@ -663,8 +677,7 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
           turn_end(false);
           wgmma_wait<1>();  // S of tile t is ready; P V of tile t - 1 still runs under the softmax below
           fence_regs(s);
-#pragma unroll
-          for (int c = 0; c < NQB; ++c) release(ik + c);
+          release(ik);
           tile_softmax<DROP, FP8>(s, m_run, l_run, alpha, p, sg.b, t * kTileN, n0, cq, interior(t * kTileN), qside, sl2);
           wgmma_wait<0>();
           pv_done(o, iv);
@@ -992,6 +1005,46 @@ void free_plan_tables(Plan& pl) {
   if (cur != pl.dev) cudaSetDevice(cur);
 }
 
+// Workers of the CTA-pair plan: SMs / 2, capped at the 2-CTA clusters of the pair kernel that can be resident at
+// once.  Both CTAs of a cluster must sit in one GPC, so a GPC with an odd number of SMs leaves one of them idle; a pair
+// past that cap would start only when another has finished all its work, doubling the kernel time.  Every pair
+// instantiation takes one CTA per SM (more than half the shared memory), so one of them stands for all.
+int pair_workers(int dev, int* workers, int* fit_out = nullptr) {
+  static std::mutex mu;
+  static std::map<int, std::pair<int, int>> cache;  // device -> (workers, clusters that fit)
+  std::lock_guard<std::mutex> lk(mu);
+  auto it = cache.find(dev);
+  if (it != cache.end()) {
+    *workers = it->second.first;
+    if (fit_out != nullptr) *fit_out = it->second.second;
+    return PCV_OK;
+  }
+  int sms = 0;
+  PCV_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  auto kernel = attn_fwd_kernel<2, 2, true, true>;
+  constexpr int smem = FwdCfg<2, 2>::kSmemBytes;
+  const int rc = set_smem_limit(reinterpret_cast<const void*>(kernel), smem);
+  if (rc != PCV_OK) return rc;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(sms / 2 * 2);
+  cfg.blockDim = dim3(kThreads);
+  cfg.dynamicSmemBytes = smem;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 2;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  int fit = 0;
+  PCV_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&fit, kernel, &cfg));
+  PCV_REQUIRE(fit >= 1, PCV_ERR_UNSUPPORTED, "the CTA-pair kernel: no 2-CTA cluster fits on device %d", dev);
+  *workers = std::min(sms / 2, fit);
+  if (fit_out != nullptr) *fit_out = fit;
+  cache[dev] = {*workers, fit};
+  return PCV_OK;
+}
+
 // The returned shared_ptr keeps the host-side plan alive for the caller even if another thread evicts it; the
 // device tables of an evicted plan are released only after a synchronize of their device, and eviction removes
 // the least recently used half (never the entry being returned).
@@ -999,9 +1052,13 @@ int get_plan(int B, int H, int N, int M, const Mode& mode, std::shared_ptr<Plan>
   int dev = 0;
   PCV_CHECK_CUDA(cudaGetDevice(&dev));
   int sms = 0;
-  PCV_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  if (mode.pair) {
+    const int rc = pair_workers(dev, &sms);  // workers are CTA pairs
+    if (rc != PCV_OK) return rc;
+  } else {
+    PCV_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  }
   std::lock_guard<std::mutex> lk(g_plan_mu);
-  if (mode.pair) sms /= 2;  // workers are CTA pairs
   const int QB = (N + mode.rows_per_unit - 1) / mode.rows_per_unit;
   const int T = (M + kTileN - 1) / kTileN;
   const int last_ntile =
@@ -1051,7 +1108,8 @@ size_t slots_bytes(const Plan& pl, int DV, int slot_rows) {
   // [slot][row][DV] numerators, [slot][row] row max, [slot][row] denominators
   return sizeof(float) * (size_t)pl.num_slots * slot_rows * (DV + 2);
 }
-// The CTA-pair kernel takes a call only when it is asked for (impl = PCV_IMPL_TCGEN05_PAIR).
+// The CTA-pair kernel takes a call only when it is asked for (impl = PCV_IMPL_TCGEN05_PAIR): at head dim 128 it is
+// slower than the single-CTA kernel at every N measured (README).
 Mode choose_mode(const pcv_attn_params& a) {
   if (a.impl == PCV_IMPL_TCGEN05_PAIR) return Mode{2 * kTileM, kTileM, 2 * kTileM, true};
   return Mode{kTileM, kTileM, kTileM, false};
@@ -1217,6 +1275,16 @@ int debug_plan(int B, int H, int N, int M, int workers, int rows_per_unit, int r
       int32_t* r = segs + 8 * s;
       r[0] = c; r[1] = g.b; r[2] = g.h; r[3] = g.q0; r[4] = g.ntile; r[5] = g.t0; r[6] = g.t1; r[7] = g.slot;
     }
+  return PCV_OK;
+}
+
+int debug_pair_workers(int32_t* workers, int32_t* clusters_fit) {
+  int dev = 0, w = 0, fit = 0;
+  PCV_CHECK_CUDA(cudaGetDevice(&dev));
+  const int rc = pair_workers(dev, &w, &fit);
+  if (rc != PCV_OK) return rc;
+  *workers = w;
+  *clusters_fit = fit;
   return PCV_OK;
 }
 

@@ -122,6 +122,7 @@ int launch_attn_tc_fp8(const pcv_attn_params& p, const pcv_fp8_attn& f, cudaStre
 int debug_read(uint32_t* out, int n);  // the watchdog record of the wgmma kernels (16 words)
 int debug_plan(int B, int H, int N, int M, int workers, int rows_per_unit, int rows_per_tile, int32_t* segs,
                int max_segs, int32_t* counts);  // host-only dump of the tcgen05 work plan
+int debug_pair_workers(int32_t* workers, int32_t* clusters_fit);  // the current device's CTA-pair plan width
 
 // the streaming decode kernel: f != nullptr for e4m3 K / V rows (pcv_attn_decode_fp8), rows != nullptr for the key
 // window read from device memory (pcv_attn_decode_window (_fp8), M = the arena's capacity)

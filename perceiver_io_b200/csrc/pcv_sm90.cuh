@@ -160,6 +160,18 @@ __device__ __forceinline__ void warp_arrive_pair(uint64_t* bar) {
     mbar_arrive_cta(bar, 1);
   }
 }
+// One arrive per warpgroup, by its first thread; every thread of the warpgroup calls it after the wgmma.wait_group
+// that completed the warpgroup's reads of the released slot (one wgmma runs for all four warps of the warpgroup).
+__device__ __forceinline__ void wg_arrive(uint64_t* bar) {
+  if ((threadIdx.x & 127) == 0) mbar_arrive(bar);
+}
+// The same for a slot that both CTAs of a pair read: one arrive on this CTA's barrier and one on the barrier at the
+// same offset in the other CTA of the pair, from two different warps so that neither waits for the other.
+__device__ __forceinline__ void wg_arrive_pair(uint64_t* bar) {
+  const uint32_t t = threadIdx.x & 127;
+  if (t == 0) mbar_arrive(bar);
+  else if (t == 32) mbar_arrive_cta(bar, cluster_ctarank() ^ 1u);
+}
 // multicast loads: the box lands at the same offset in every CTA of `mask`, and the transaction bytes are signalled on
 // the barrier at the same offset in each of them
 __device__ __forceinline__ void tma_load_4d_mc(void* smem_dst, const void* tmap, uint64_t* bar, int c0, int c1, int c2,
