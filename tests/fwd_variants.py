@@ -100,9 +100,10 @@ def plan_segments(B, H, N, M, workers, pair):
     return counts, per_cta
 
 
-def check_schedule(shape_name, case, workers):
+def check_schedule(shape_name, case, workers, boxes_per_tile=None, slots=None):
     """Assert that the plan of SCHEDULE_SHAPES[shape_name] has the structure the shape is meant to exercise for the
-    variant `case`, with `workers` CTAs (CTA pairs for the pair kernel).  Returns a one-line description."""
+    variant `case`, with `workers` CTAs (CTA pairs for the pair kernel).  `boxes_per_tile` / `slots` override the
+    16-bit kernel's ring boxes per key tile and ring slots (the FP8 kernel's differ).  Returns a one-line description."""
     B, H, N, M = SCHEDULE_SHAPES[shape_name]
     dqk, dv, _dt, pair = case
     counts, per_cta = plan_segments(B, H, N, M, workers, pair)
@@ -116,8 +117,10 @@ def check_schedule(shape_name, case, workers):
     elif shape_name == "ring":
         assert counts["slots"] > 0 and counts["units"] > 0, "expected the split plan"
         nq = nqb_of(dqk)
-        boxes = max(lengths) * (nq + min(nvb_passes(dv)))
-        assert boxes >= 2 * ring_slots(nq), f"longest segment streams {boxes} boxes through {ring_slots(nq)} slots"
+        per_tile = nq + min(nvb_passes(dv)) if boxes_per_tile is None else boxes_per_tile
+        ns = ring_slots(nq) if slots is None else slots
+        boxes = max(lengths) * per_tile
+        assert boxes >= 2 * ns, f"longest segment streams {boxes} boxes through {ns} slots"
         mixed = [v for v in per_cta.values() if len({(b, h) for b, h, *_ in v}) > 1]
         assert mixed, "no CTA runs segments of two (b, h)"
         assert any(t0 > 0 and slot >= 0 for v in mixed for _b, _h, _q0, t0, _t1, slot in v), "no split segment with t0 > 0"
