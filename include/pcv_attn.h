@@ -599,6 +599,34 @@ PCV_API int pcv_attn_decode_window_fp8_supported(const pcv_attn_params* p, const
                                                  const pcv_dev_rows* rows);
 PCV_API int pcv_attn_decode_window_fp8(const pcv_attn_params* p, const pcv_decode_fp8* f, const pcv_dev_rows* rows,
                                        void* stream);
+
+/*
+ * pcv_attn_cached_window (_fp8): attention of 1 to 64 query rows on the key window [bounds[0], bounds[1]) of an arena on
+ * the tensor cores, with an optional causal band: a k-token step of a decode loop in which every token sees exactly the
+ * keys a one-token step gives it.  k, v and pad_mask point at arena row 0 and M == rows->capacity (>= 1); pad bytes
+ * are indexed by the absolute arena row.  The window is clamped to [0, capacity); a window of length <= 0 writes zeros.
+ * The split count is planned on the host from capacity, so the grid and the workspace
+ * (pcv_attn_cached_window (_fp8)_workspace_bytes) do not depend on the window; each split takes an equal share of the
+ * window's 64-key tiles when the kernel runs.  Query i sits at row r_i = end - N + i.
+ *   band == 0: the causal mask (if set) is right-aligned to the window's end; padded and causally masked keys take the
+ *              finite fill, as in pcv_attn_cached_fp8 (a fully masked row is the uniform average of the window);
+ *   band  > 0: causal only; query i sees the keys [r_i + 1 - band, r_i] of the window and nothing else: a key outside
+ *              that band contributes nothing (no fill), padded keys inside it take the fill.
+ * pcv_attn_cached_window: k / v are rows of q's type (dtype PCV_BF16 / PCV_F16), head dims multiples of 8.
+ * pcv_attn_cached_window_fp8: k / v are e4m3 rows with pcv_decode_fp8 descales as in pcv_attn_cached_fp8, head dims
+ * multiples of 16.  Arithmetic as pcv_attn_cached_fp8: q unrounded, P rounded to q's type before P V, fp32
+ * denominators, v_descale applied to the accumulator once; with the window [0, capacity) and no band the e4m3 entry
+ * computes pcv_attn_cached_fp8's result bit for bit.  Head dims at most 256; impl AUTO; no write_partial, no key shard.
+ * One launch, bitwise reproducible.  Arguments are checked before any CUDA call.
+ */
+PCV_API int pcv_attn_cached_window_supported(const pcv_attn_params* p, const pcv_dev_rows* rows, int32_t band);
+PCV_API int pcv_attn_cached_window_workspace_bytes(const pcv_attn_params* p, size_t* bytes);
+PCV_API int pcv_attn_cached_window(const pcv_attn_params* p, const pcv_dev_rows* rows, int32_t band, void* stream);
+PCV_API int pcv_attn_cached_window_fp8_supported(const pcv_attn_params* p, const pcv_decode_fp8* f,
+                                                 const pcv_dev_rows* rows, int32_t band);
+PCV_API int pcv_attn_cached_window_fp8_workspace_bytes(const pcv_attn_params* p, size_t* bytes);
+PCV_API int pcv_attn_cached_window_fp8(const pcv_attn_params* p, const pcv_decode_fp8* f, const pcv_dev_rows* rows,
+                                       int32_t band, void* stream);
 PCV_API int pcv_kv_append_at(const pcv_kv_append_params* p, const pcv_dev_rows* rows, void* stream);
 PCV_API int pcv_kv_append_at_fp8(const pcv_kv_append_params* p, const pcv_kv_fp8_scales* f, const pcv_dev_rows* rows,
                                  void* stream);

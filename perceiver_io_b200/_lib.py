@@ -72,6 +72,12 @@ EXPORTS = (
     "pcv_attn_decode_window",
     "pcv_attn_decode_window_fp8_supported",
     "pcv_attn_decode_window_fp8",
+    "pcv_attn_cached_window_supported",
+    "pcv_attn_cached_window_workspace_bytes",
+    "pcv_attn_cached_window",
+    "pcv_attn_cached_window_fp8_supported",
+    "pcv_attn_cached_window_fp8_workspace_bytes",
+    "pcv_attn_cached_window_fp8",
     "pcv_kv_append_at",
     "pcv_kv_append_at_fp8",
     "pcv_rotary_apply_at",
@@ -405,13 +411,23 @@ def lib() -> C.CDLL:
         l.pcv_attn_decode_window.argtypes = [C.POINTER(AttnParams), rows, C.c_void_p]
         l.pcv_attn_decode_window_fp8_supported.argtypes = [C.POINTER(AttnParams), C.POINTER(DecodeFp8), rows]
         l.pcv_attn_decode_window_fp8.argtypes = [C.POINTER(AttnParams), C.POINTER(DecodeFp8), rows, C.c_void_p]
+        l.pcv_attn_cached_window_supported.argtypes = [C.POINTER(AttnParams), rows, C.c_int32]
+        l.pcv_attn_cached_window_workspace_bytes.argtypes = [C.POINTER(AttnParams), C.POINTER(C.c_size_t)]
+        l.pcv_attn_cached_window.argtypes = [C.POINTER(AttnParams), rows, C.c_int32, C.c_void_p]
+        l.pcv_attn_cached_window_fp8_supported.argtypes = [C.POINTER(AttnParams), C.POINTER(DecodeFp8), rows, C.c_int32]
+        l.pcv_attn_cached_window_fp8_workspace_bytes.argtypes = [C.POINTER(AttnParams), C.POINTER(C.c_size_t)]
+        l.pcv_attn_cached_window_fp8.argtypes = [C.POINTER(AttnParams), C.POINTER(DecodeFp8), rows, C.c_int32,
+                                                 C.c_void_p]
         l.pcv_kv_append_at.argtypes = [C.POINTER(KvAppendParams), rows, C.c_void_p]
         l.pcv_kv_append_at_fp8.argtypes = [C.POINTER(KvAppendParams), C.POINTER(KvFp8Scales), rows, C.c_void_p]
         l.pcv_rotary_apply_at.argtypes = [C.POINTER(RotaryParams), rows, C.c_void_p]
         l.pcv_rotary_apply_at_fp8.argtypes = [C.POINTER(RotaryParams), C.POINTER(RotaryFp8), rows, C.c_void_p]
         for name in ("pcv_attn_decode_window_supported", "pcv_attn_decode_window_workspace_bytes",
                      "pcv_attn_decode_window", "pcv_attn_decode_window_fp8_supported", "pcv_attn_decode_window_fp8",
-                     "pcv_kv_append_at", "pcv_kv_append_at_fp8", "pcv_rotary_apply_at", "pcv_rotary_apply_at_fp8"):
+                     "pcv_kv_append_at", "pcv_kv_append_at_fp8", "pcv_rotary_apply_at", "pcv_rotary_apply_at_fp8",
+                     "pcv_attn_cached_window_supported", "pcv_attn_cached_window_workspace_bytes",
+                     "pcv_attn_cached_window", "pcv_attn_cached_window_fp8_supported",
+                     "pcv_attn_cached_window_fp8_workspace_bytes", "pcv_attn_cached_window_fp8"):
             getattr(l, name).restype = C.c_int
         l.pcv_ln_linear_bwd_supported.argtypes = [C.POINTER(LnLinearBwdParams)]
         l.pcv_ln_linear_bwd_supported.restype = C.c_int

@@ -572,6 +572,58 @@ int pcv_attn_decode_window_fp8(const pcv_attn_params* p, const pcv_decode_fp8* f
   return decode_launch(p, f, rows, true, true, stream);
 }
 
+// The tensor-core attention of 1 to 64 query rows on a device-resident window of an arena (pcv_attn_window.cu); the
+// e4m3 entry (fp8) refuses a NULL f.
+static int window_check(const pcv_attn_params* p, const pcv_decode_fp8* f, const pcv_dev_rows* rows, int32_t band,
+                        bool fp8) {
+  const char* name = fp8 ? "attn_cached_window_fp8" : "attn_cached_window";
+  PCV_REQUIRE(!fp8 || f != nullptr, PCV_ERR_INVALID, "%s: fp8 params are NULL", name);
+  PCV_REQUIRE(rows != nullptr, PCV_ERR_INVALID, "%s: rows is NULL", name);
+  int rc = validate_attn(p);
+  if (rc != PCV_OK) return rc;
+  const char* why = "";
+  PCV_REQUIRE(attn_window_supported(*p, fp8 ? f : nullptr, *rows, band, &why), PCV_ERR_UNSUPPORTED,
+              "%s not applicable: %s", name, why);
+  return PCV_OK;
+}
+
+int pcv_attn_cached_window_supported(const pcv_attn_params* p, const pcv_dev_rows* rows, int32_t band) {
+  return window_check(p, nullptr, rows, band, false) == PCV_OK ? 1 : 0;
+}
+
+int pcv_attn_cached_window_fp8_supported(const pcv_attn_params* p, const pcv_decode_fp8* f, const pcv_dev_rows* rows,
+                                         int32_t band) {
+  return window_check(p, f, rows, band, true) == PCV_OK ? 1 : 0;
+}
+
+static int window_workspace(const pcv_attn_params* p, size_t* bytes, const char* name) {
+  int rc = validate_attn(p);
+  if (rc != PCV_OK) return rc;
+  PCV_REQUIRE(bytes != nullptr, PCV_ERR_INVALID, "%s: bytes is NULL", name);
+  return attn_window_workspace_bytes(*p, bytes);
+}
+
+int pcv_attn_cached_window_workspace_bytes(const pcv_attn_params* p, size_t* bytes) {
+  return window_workspace(p, bytes, "attn_cached_window");
+}
+
+int pcv_attn_cached_window_fp8_workspace_bytes(const pcv_attn_params* p, size_t* bytes) {
+  return window_workspace(p, bytes, "attn_cached_window_fp8");
+}
+
+int pcv_attn_cached_window(const pcv_attn_params* p, const pcv_dev_rows* rows, int32_t band, void* stream) {
+  const int rc = window_check(p, nullptr, rows, band, false);
+  if (rc != PCV_OK) return rc;
+  return launch_attn_window(*p, nullptr, *rows, band, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pcv_attn_cached_window_fp8(const pcv_attn_params* p, const pcv_decode_fp8* f, const pcv_dev_rows* rows,
+                               int32_t band, void* stream) {
+  const int rc = window_check(p, f, rows, band, true);
+  if (rc != PCV_OK) return rc;
+  return launch_attn_window(*p, f, *rows, band, reinterpret_cast<cudaStream_t>(stream));
+}
+
 int pcv_kv_append_at(const pcv_kv_append_params* p, const pcv_dev_rows* rows, void* stream) {
   PCV_REQUIRE(p != nullptr && rows != nullptr, PCV_ERR_INVALID, "kv_append_at: params or rows are NULL");
   return launch_kv_append(*p, nullptr, rows, reinterpret_cast<cudaStream_t>(stream));

@@ -11,17 +11,28 @@ run, and in-graph int32 ops advance them at the end of each step.
     dec = GraphedDecoder(model, batch=B, max_new_tokens=T, kv_cache="bf16")   # or "fp8": e4m3 arenas
     logits = dec.prefill(input_ids, prefix_len, pad_mask=None)                # (B, vocab): eager prompt pass
     logits = dec.step(token_ids)                                              # (B, 1) int64 -> (B, vocab), one replay
+    logits = dec.extend(token_ids)                                            # (B, k) int64 -> (B, k, vocab)
+    dec.rewind(n)                                                             # drop the last n fed tokens
     dec.reorder(beam_idx)                                                     # beam search (eager)
 
 Rows: cross-attention arena row r holds token r of the sequence (prompt and generated tokens); self-attention arena
 row r holds token ``prefix_len + r`` (prefix_len of the prompt).  The windows follow the 🤗 wrapper's truncation, as
 :func:`decode_windows` states it.  ``step`` returns a view of the graph's static logits, valid until the next step.
 
-Not covered: steps of more than one token, contrastive search, a ring buffer bounded at ``max_seq_len`` (the arenas
-grow by ``max_new_tokens`` rows) and wiring into 🤗 ``generate()``.
+``extend`` feeds 1 to 64 tokens in one replay of a graph recorded for that count on first use (``step``'s graph for
+one token) and returns the logits after each of them: every token attends exactly the keys the one-token loop gives it
+(``ops.attention_window`` with a causal band of the group's window width), so speculative decoding can verify k draft
+tokens in one replay, keep the accepted prefix and ``rewind`` the rest.  ``rewind(n)`` moves the row counters back by
+n tokens with eager int32 ops (no host read, no re-capture); the arena rows past the new end are overwritten later.  The
+batch rows share one window per layer group, so ``rewind`` takes one count for all of them: a batched speculative loop
+rewinds to the smallest accepted count and feeds the remaining accepted tokens again.
+
+Not covered: per-batch-row accept counts, steps of more than 64 tokens, contrastive search, a ring buffer bounded at
+``max_seq_len`` (the arenas grow by ``max_new_tokens`` rows) and wiring into 🤗 ``generate()``.
 """
 from __future__ import annotations
 
+import operator
 from typing import List, NamedTuple
 
 import torch
@@ -65,6 +76,35 @@ def window_positions(pad: torch.Tensor, window: torch.Tensor, cols: torch.Tensor
     inside = (cols >= window[0]) & (cols < window[1])
     shift = ((pad != 0) & inside).sum(dim=1, keepdim=True)
     return (window[1] - window[0] - 1 - shift).clamp_min(0).long()
+
+
+def window_positions_rows(pad: torch.Tensor, bounds: torch.Tensor, cols: torch.Tensor, k: int,
+                          width: int) -> torch.Tensor:
+    """(B, k) int64 absolute positions of the k tokens of a step whose last token is row ``bounds[1] - 1``: token i at
+    row ``r_i = bounds[1] - k + i`` takes :func:`window_positions` of its own one-token window
+    ``[max(0, r_i + 1 - width), r_i + 1)``.  Tensors alone, no host read; ``pad`` and ``cols`` as there."""
+    r = bounds[1] - k + torch.arange(k, device=cols.device, dtype=cols.dtype)
+    begin = (r + 1 - width).clamp_min(0)
+    inside = (cols >= begin[:, None]) & (cols <= r[:, None])
+    shift = ((pad != 0)[:, None, :] & inside).sum(dim=2)
+    return (r - begin - shift).clamp_min(0).long()
+
+
+def extend_bounds(bounds: torch.Tensor, k: int) -> torch.Tensor:
+    """The (groups, 6) int32 bounds of a k-token step from the one-token state ``bounds`` (``[begin, end, row, 1, row,
+    0]`` per layer group, end = row + 1): the window's end moves to the last token's row + 1, everything else stays —
+    the window starts at the first token's begin, appends and rotations start at its row."""
+    out = bounds.clone()
+    out[:, 1] += k - 1
+    return out
+
+
+def advance_bounds_(bounds: torch.Tensor, inc: torch.Tensor, wmax: torch.Tensor, n: int) -> torch.Tensor:
+    """Move the one-token state ``bounds`` by n tokens in place (n < 0 rewinds): row and end += n, begin = max(0,
+    end - the group's window width ``wmax``).  ``inc`` is ``[0, 1, 1, 0, 1, 0]``."""
+    bounds.add_(inc, alpha=n)
+    bounds[:, 0].copy_((bounds[:, 1] - wmax).clamp_min_(0))
+    return bounds
 
 
 class _Attn:
@@ -111,9 +151,10 @@ class GraphedDecoder:
         self.device = w.device
         self.dtype = w.dtype
         self.captures = 0
-        self._graph = None
+        self._graphs = {}      # tokens per step -> GraphedForward
         self._bounds = None
         self._remaining = 0
+        self._fed = 0          # tokens fed since prefill (what rewind may drop)
         sa = model.self_attention
         nrot = sa.num_rotary_layers
         ca = model.cross_attention[0].module
@@ -170,14 +211,15 @@ class GraphedDecoder:
                                      [w.sa_begin, w.sa_end, rows[1], 1, rows[1], 0]], dtype=torch.int32, device=dev)
         self._inc = torch.tensor([0, 1, 1, 0, 1, 0], dtype=torch.int32, device=dev)
         self._wmax = torch.tensor([m.max_seq_len, m.max_latents], dtype=torch.int32, device=dev)
-        self._token = torch.zeros(B, 1, dtype=torch.long, device=dev)
-        self._graph = None
+        self._width = (m.max_seq_len, m.max_latents)
+        self._graphs = {}
         self._remaining = T
+        self._fed = 0
         return out.logits[:, -1]
 
-    # ---- one token ---------------------------------------------------------------------------------------------------
-    def _attend(self, a: _Attn, q, k, v):
-        H, g = a.mha.num_heads, self._bounds[a.group]
+    # ---- one step of 1 to 64 tokens ----------------------------------------------------------------------------------
+    def _attend(self, a: _Attn, bounds, q, k, v):
+        H, g = a.mha.num_heads, bounds[a.group]
         fp8 = self.fp8
         ops.kv_append_at(a.K, a.V, k, v, g[2:3], *((a.kv8.k_inv, a.kv8.v_inv) if fp8 else ()))
         keys = a.K
@@ -185,10 +227,12 @@ class GraphedDecoder:
             ops.rotary_apply_at(k, H, a.table, g[2:4], a.S, a.k_inv_h)
             q = ops.rotary_apply_at(q, H, a.table, g[4:6], torch.empty(q.shape, dtype=q.dtype, device=q.device))
             keys = a.S
-        o = ops.attention_decode_window(q, keys, a.V, g[0:2], H, a.mha.dp_scale,
-                                        pad_mask=self._pad if a.group == 0 else None, causal=a.mha.causal_attention,
-                                        k_descale=a.kv8.k_descale if fp8 else None,
-                                        v_descale=a.kv8.v_descale if fp8 else None)
+        kw = dict(pad_mask=self._pad if a.group == 0 else None, causal=a.mha.causal_attention,
+                  k_descale=a.kv8.k_descale if fp8 else None, v_descale=a.kv8.v_descale if fp8 else None)
+        if q.shape[1] == 1:
+            o = ops.attention_decode_window(q, keys, a.V, g[0:2], H, a.mha.dp_scale, **kw)
+        else:   # every token sees its own one-token window: a causal band of the group's window width
+            o = ops.attention_window(q, keys, a.V, g[0:2], H, a.mha.dp_scale, band=self._width[a.group], **kw)
         return modules.fused_linear(a.mha, "_pcv_o_fold", None, a.mha.o_proj, o, a.key)
 
     @staticmethod
@@ -198,14 +242,18 @@ class GraphedDecoder:
     def _step_fn(self, token: torch.Tensor) -> torch.Tensor:
         m = self.model
         adapter = m.input_adapter
+        k = token.shape[1]
+        b = self._bounds if k == 1 else extend_bounds(self._bounds, k)
         x = adapter.txt_embedding(token)
         if getattr(adapter, "_abs_pos_emb", False):
-            x = x + adapter.pos_embedding(window_positions(self._pad, self._bounds[0, 0:2], self._cols))
+            pos = (window_positions(self._pad, b[0, 0:2], self._cols) if k == 1
+                   else window_positions_rows(self._pad, b[0], self._cols, k, self._width[0]))
+            x = x + adapter.pos_embedding(pos)
         # cross-attention (cached: the keys of this token are its own q_norm'd row, reference modules.py:222-224)
         ca_layer, ca = m.cross_attention, self._layers[0].owner
         xq = ca.q_norm(x)
         a = ca.attention
-        h = self._residual(ca_layer[0], self._attend(self._layers[0], a.q_proj(xq), a.k_proj(xq), a.v_proj(xq)), x)
+        h = self._residual(ca_layer[0], self._attend(self._layers[0], b, a.q_proj(xq), a.k_proj(xq), a.v_proj(xq)), x)
         h = ca_layer[1](h).last_hidden_state
         for layer, st in zip(m.self_attention, self._layers[1:]):
             sa = st.owner
@@ -213,47 +261,80 @@ class GraphedDecoder:
             if qkv is None:
                 xn = sa.norm(h)
                 qkv = sa.attention.q_proj(xn), sa.attention.k_proj(xn), sa.attention.v_proj(xn)
-            h = self._residual(layer[0], self._attend(st, *qkv), h)
+            h = self._residual(layer[0], self._attend(st, b, *qkv), h)
             h = layer[1](h).last_hidden_state
         if m.config.output_norm:
             h = m.out_norm(h)
-        logits = m.output_adapter(h, txt_embedding=adapter.txt_embedding)[:, -1]
-        # the next step's rows and windows: row += 1, end += 1, begin = max(0, end - window limit)
-        b = self._bounds
-        b.add_(self._inc)
-        b[:, 0].copy_((b[:, 1] - self._wmax).clamp_min_(0))
-        return logits
+        logits = m.output_adapter(h, txt_embedding=adapter.txt_embedding)
+        # the next step's rows and windows: row += k, end += k, begin = max(0, end - window limit)
+        advance_bounds_(self._bounds, self._inc, self._wmax, k)
+        return logits[:, -1] if k == 1 else logits
 
-    def _capture(self) -> None:
-        snapshot = self._bounds.clone()   # the warm-up calls advance the rows; their arena writes are rewritten later
-        old = torch.cuda.get_sync_debug_mode()
-        torch.cuda.set_sync_debug_mode(0)  # recording a graph synchronises the device once
-        try:
-            self._graph = GraphedForward(self._step_fn, self._token)
-        finally:
-            torch.cuda.set_sync_debug_mode(old)
-        self._bounds.copy_(snapshot)
-        self.captures += 1
+    def _replay(self, token_ids: torch.Tensor, fn: str) -> torch.Tensor:
+        """One replay of the graph of ``token_ids.shape[1]`` tokens per step, recorded on first use."""
+        k = token_ids.shape[1] if token_ids.dim() == 2 else 0
+        kmax = 1 if fn == "step" else ops.WINDOW_MAX_ROWS
+        if self._bounds is None:
+            raise RuntimeError("GraphedDecoder: call prefill() first")
+        if tuple(token_ids.shape) != (self.batch, k) or token_ids.dtype != torch.long or not 1 <= k <= kmax:
+            want = "1)" if fn == "step" else f"k) with 1 <= k <= {ops.WINDOW_MAX_ROWS}"
+            raise ValueError(f"GraphedDecoder.{fn} takes ({self.batch}, {want} int64 tokens, got "
+                             f"{tuple(token_ids.shape)} {token_ids.dtype}")
+        if self._remaining < k:
+            raise RuntimeError(f"GraphedDecoder: {self._remaining} of max_new_tokens={self.max_new_tokens} tokens remain "
+                               f"(the arenas hold no room for {k} more); rewind, or call prefill() again")
+        if torch.is_autocast_enabled():
+            raise RuntimeError("GraphedDecoder does not run under autocast")
+        graph = self._graphs.get(k)
+        if graph is None:
+            snapshot = self._bounds.clone()   # the warm-up calls advance the rows; their arena writes are rewritten later
+            old = torch.cuda.get_sync_debug_mode()
+            torch.cuda.set_sync_debug_mode(0)  # recording a graph synchronises the device once
+            try:
+                graph = GraphedForward(self._step_fn, token_ids)
+            finally:
+                torch.cuda.set_sync_debug_mode(old)
+            self._bounds.copy_(snapshot)
+            self._graphs[k] = graph
+            self.captures += 1
+        out = graph(token_ids)
+        self._remaining -= k
+        self._fed += k
+        return out
 
     def step(self, token_ids: torch.Tensor) -> torch.Tensor:
         """Append the tokens ``token_ids`` (B, 1) int64 and return the next logits (B, vocab) — one graph replay (the
         first call records the graph).  A view of the graph's static output, valid until the next step."""
+        return self._replay(token_ids, "step")
+
+    def extend(self, token_ids: torch.Tensor) -> torch.Tensor:
+        """Append the k tokens ``token_ids`` (B, k) int64, 1 <= k <= 64, and return the logits after each of them (B, k,
+        vocab) — one replay of the graph recorded for k on first use (k = 1 shares ``step``'s graph).  Token i sees
+        exactly the keys it would see had the k tokens been fed by k ``step`` calls.  Consumes k tokens of the
+        budget.  A view of the graph's static output, valid until the next step."""
+        if token_ids.dim() == 2 and token_ids.shape[1] == 1:
+            return self._replay(token_ids, "extend")[:, None]
+        return self._replay(token_ids, "extend")
+
+    def rewind(self, n: int) -> None:
+        """Drop the last ``n`` fed tokens from every layer group: the next token is fed at the row of the first dropped
+        one, as if the n tokens had never been fed.  Eager int32 ops on the row counters (no host read of the device,
+        no re-capture); gives n tokens back to the budget.  One count for all batch rows (they share the windows): a
+        batched speculative loop rewinds to the smallest accepted count and feeds the rest again."""
         if self._bounds is None:
             raise RuntimeError("GraphedDecoder: call prefill() first")
-        if self._remaining < 1:
-            raise RuntimeError(f"GraphedDecoder: {self._remaining} of max_new_tokens={self.max_new_tokens} steps remain "
-                               "(the arenas are full); call prefill() again")
-        if tuple(token_ids.shape) != (self.batch, 1) or token_ids.dtype != torch.long:
-            raise ValueError(f"GraphedDecoder.step takes ({self.batch}, 1) int64 tokens, got {tuple(token_ids.shape)} "
-                             f"{token_ids.dtype}")
-        if torch.is_autocast_enabled():
-            raise RuntimeError("GraphedDecoder does not run under autocast")
-        if self._graph is None:
-            self._token.copy_(token_ids)
-            self._capture()
-        out = self._graph(token_ids)
-        self._remaining -= 1
-        return out
+        try:
+            count = operator.index(n) if not isinstance(n, bool) else None
+        except TypeError:
+            count = None
+        if count is None or count < 0 or count > self._fed:
+            raise ValueError(f"GraphedDecoder.rewind: n must be an integer in [0, {self._fed}] (the tokens fed since "
+                             f"prefill), got {n!r}")
+        n = count
+        if n:
+            advance_bounds_(self._bounds, self._inc, self._wmax, -n)
+            self._remaining += n
+            self._fed -= n
 
     def reorder(self, beam_idx: torch.Tensor) -> None:
         """Permute the batch rows of every arena, rotated-key arena and the pad rows (beam search), eagerly."""

@@ -29,7 +29,7 @@ __all__ = [
     "attention_fp8", "attention_fp8_supported", "fp8_descales", "fp8_quantize", "fp8_transpose_v", "kv_project_fp8",
     "kv_project_fp8_supported", "ln_linear", "ln_linear_backward", "kv_append_fp8", "attention_decode_fp8",
     "attention_decode_fp8_supported", "fp8_pair_descale", "fp8_dequantize", "rotated_cache_shadow", "rotary_at", "rotary_fp8",
-    "attention_decode_window", "kv_append_at", "rotary_apply_at", "rotary_angle_table",
+    "attention_decode_window", "kv_append_at", "rotary_apply_at", "rotary_angle_table", "attention_window",
 ]
 
 
@@ -1201,6 +1201,53 @@ def attention_decode_window(q, k, v, bounds: torch.Tensor, num_heads: int, scale
         out = _new_output(p, _compute_dtype(q.dtype), k.device)
         _run_decode(p, f, _dev_rows(bounds, p.M), k.device)
     del keep
+    return out
+
+
+#: Query rows of one :func:`attention_window` call (one m64 tensor-core tile).
+WINDOW_MAX_ROWS = 64
+
+
+def attention_window(q, k, v, bounds: torch.Tensor, num_heads: int, scale: float, band: int = 0, pad_mask=None,
+                     causal: bool = False, k_descale=None, v_descale=None) -> torch.Tensor:
+    """Attention of 1 to 64 query rows on the key window ``[bounds[0], bounds[1])`` of KV arenas on the tensor cores,
+    the window read from device memory when the kernel runs (pcv_attn_cached_window / _fp8): nothing is read back to
+    the host, so the call can be recorded in a CUDA graph and replayed for every window.
+
+    q: (B or 1, N <= 64, H*dqk) bf16 / fp16; k, v: (B, capacity, H*d) arenas of q's dtype (head dims multiples of 8) or
+    ``float8_e4m3fn`` codes (head dims multiples of 16, with ``k_descale`` (H,) and ``v_descale`` (H, dv) as in
+    :func:`attention_decode_fp8`); ``pad_mask`` (B, capacity), indexed by the absolute arena row.  Query i sits at row
+    ``r_i = end - N + i``.  With ``band`` W > 0 (``causal`` only) query i sees exactly the keys ``[r_i + 1 - W, r_i]``:
+    a key outside its band contributes nothing, a padded key inside it takes the finite fill — N rows of one call
+    are then N one-token steps whose windows are ``[max(0, r_i + 1 - W), r_i + 1)``.  With W = 0 the causal mask is
+    right-aligned to the window's end and masks as :func:`attention`.  A window of length <= 0 gives zeros.  P is
+    rounded to q's dtype before P V, as :func:`attention` does.  Returns (B, N, H*dv) in q's dtype."""
+    _require_cuda(q, k, v, bounds, pad_mask, k_descale, v_descale)
+    if q.dtype not in (torch.bfloat16, torch.float16):
+        raise ValueError(f"attention_window: q must be bf16 / fp16, got {q.dtype}")
+    fp8 = k.dtype == F8
+    if fp8 != (v.dtype == F8) or (not fp8 and (k.dtype != q.dtype or v.dtype != q.dtype)):
+        raise ValueError(f"attention_window: the K / V arenas ({k.dtype} / {v.dtype}) must both be q's dtype "
+                         f"({q.dtype}) or float8_e4m3fn")
+    if fp8 != (k_descale is not None and v_descale is not None) or (not fp8 and (k_descale, v_descale) != (None, None)):
+        raise ValueError("attention_window: k_descale and v_descale go with e4m3 arenas, and only with them")
+    if band < 0 or (band > 0 and not causal):
+        raise ValueError(f"attention_window: band must be >= 0 and needs causal=True, got band={band} causal={causal}")
+    with torch.cuda.device(k.device):
+        if fp8:
+            p, f, keep = _fill_decode(q, k, v, num_heads, scale, pad_mask, causal, k_descale, v_descale)
+        else:
+            p, keep = _fill_attn_params(_rows_contiguous(q), _rows_contiguous(k), _rows_contiguous(v), num_heads, scale,
+                                        pad_mask, causal, None, 0, "auto")
+            f = None
+        p.impl = _lib.PCV_IMPL_AUTO
+        out = _new_output(p, q.dtype, k.device)
+        rows = _dev_rows(bounds, p.M)
+        entry = "pcv_attn_cached_window" + ("_fp8" if fp8 else "")
+        ws = _workspace(p, k.device, entry, C.byref(p))
+        check(getattr(_lib.lib(), entry)(*(C.byref(s) for s in (p, f, rows) if s is not None), int(band), _stream()),
+              entry)
+    del ws, keep
     return out
 
 

@@ -6,7 +6,15 @@ alternating step by step: the eager cached step with bf16 and with FP8 (e4m3) ca
 one), and GraphedDecoder with each cache.  Each step is timed with CUDA events around the call and a synchronise, so the
 wall time of a step includes its host work.  Prints one JSON line (also written to --out) with the card's name and
 power limit; ms per token as median (min-max).  --profile traces the steps with torch.profiler instead (a run of its
-own) and reports device time per step (the sum of kernel times) and kernels per step."""
+own) and reports device time per step (the sum of kernel times) and kernels per step.
+
+--step-tokens 1,4,8,16,64 measures multi-token replays instead (GraphedDecoder.extend): at each batch and for bf16 and
+FP8 arenas, one replay of k tokens on the full context, then rewind(k) so that every replay sees the same windows; the
+(cache, k) arms alternate replay by replay.  It reports ms per replay and ms per token, median (min-max); with --profile,
+device time and kernels per replay from a trace.  --kernel-leg times the attention kernels alone at the decode-core
+shape (B = 8, 16384 cached tokens, C = 1024, H = 8) for k = 2, 4, 5, 16, 64 query rows: ops.attention_window on bf16
+and e4m3 arenas, pcv_attn_decode_window (k <= 4), ops.attention_decode_fp8 (pcv_attn_cached_fp8 above 4 rows) and
+ops.attention on a bf16 cache, alternated, CUDA events around 20 launches."""
 import argparse
 import json
 import os
@@ -96,16 +104,122 @@ def run(batch, steps, profile=False):
     return res
 
 
+def run_tokens(batch, ks, reps, profile=False):
+    """ms per replay of GraphedDecoder.extend(k) on the full context, each replay followed by rewind(k)."""
+    torch.manual_seed(0)
+    cfg = P.CausalSequenceModelConfig(**GIANTMIDI)
+    model = P.CausalSequenceModel(cfg).cuda().bfloat16().eval()
+    n, prefix = cfg.max_seq_len, cfg.max_seq_len - cfg.max_latents
+    tokens = torch.randint(0, cfg.vocab_size, (batch, n + max(ks)), device="cuda")
+    arms = [(kind, k) for kind in ("bf16", "fp8") for k in ks]
+    decs, times = {}, {a: [] for a in arms}
+    with torch.no_grad():
+        for kind in ("bf16", "fp8"):
+            decs[kind] = P.GraphedDecoder(model, batch=batch, max_new_tokens=max(ks), kv_cache=kind)
+            decs[kind].prefill(tokens[:, :n], prefix)
+
+        def replay(kind, k):
+            dec = decs[kind]
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            e0.record()
+            dec.extend(tokens[:, n:n + k])
+            e1.record()
+            dec.rewind(k)
+            torch.cuda.synchronize()
+            return e0.elapsed_time(e1)
+
+        for _ in range(2):       # every graph recorded and warmed up
+            for a in arms:
+                replay(*a)
+        res = {"batch": batch, "context": n}
+        if profile:
+            from torch.profiler import ProfilerActivity, profile as trace
+
+            for a in arms:
+                with trace(activities=[ProfilerActivity.CPU, ProfilerActivity.CUDA]) as prof:
+                    for _ in range(reps):
+                        replay(*a)
+                kern = [e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
+                res[f"{a[0]}_k{a[1]}_kernel_ms_per_replay"] = round(
+                    sum(e.time_range.elapsed_us() for e in kern) / reps / 1e3, 4)
+                res[f"{a[0]}_k{a[1]}_kernels_per_replay"] = round(len(kern) / reps, 1)
+        else:
+            for _ in range(reps):
+                for a in arms:
+                    times[a].append(replay(*a))
+            for kind, k in arms:
+                res[f"{kind}_k{k}_ms_per_replay"] = stats(times[(kind, k)])
+                res[f"{kind}_k{k}_ms_per_token"] = stats([t / k for t in times[(kind, k)]])
+    del decs, model
+    torch.cuda.empty_cache()
+    return res
+
+
+def kernel_leg(ks=(2, 4, 5, 16, 64), reps=7, iters=20):
+    """The attention kernels alone at the decode-core shape: ms per call, median (min-max) of `reps` alternated
+    rounds of `iters` launches."""
+    from perceiver_io_b200 import ops
+
+    B, M, C, H = 8, 16384, 1024, 8
+    g = torch.Generator(device="cuda").manual_seed(0)
+    k = torch.randn(B, M, C, device="cuda", generator=g).bfloat16()
+    v = torch.randn(B, M, C, device="cuda", generator=g).bfloat16()
+    kd = (k.float().abs().reshape(-1, H, C // H).amax(dim=(0, 2)) / 448.0).contiguous()
+    vd = (v.float().abs().reshape(-1, H, C // H).amax(dim=0) / 448.0).contiguous()
+    k8, v8 = ops.fp8_quantize(k, kd, H), ops.fp8_quantize(v, vd, H)
+    bounds = torch.tensor([0, M], dtype=torch.int32, device="cuda")
+    scale = (C // H) ** -0.5
+    out = {"shape": {"B": B, "cached": M, "C": C, "H": H}}
+    for n in ks:
+        q = torch.randn(B, n, C, device="cuda", generator=g).bfloat16()
+        arms = {
+            "window_bf16": lambda: ops.attention_window(q, k, v, bounds, H, scale, causal=True),
+            "window_fp8": lambda: ops.attention_window(q, k8, v8, bounds, H, scale, causal=True, k_descale=kd,
+                                                       v_descale=vd),
+            "decode_fp8" if n <= 4 else "cached_fp8": lambda: ops.attention_decode_fp8(q, k8, v8, kd, vd, H, scale,
+                                                                                        causal=True),
+            "attention_bf16": lambda: ops.attention(q, k, v, H, scale, causal=True),
+        }
+        if n <= 4:
+            arms["decode_window_bf16"] = lambda: ops.attention_decode_window(q, k, v, bounds, H, scale, causal=True)
+            arms["decode_window_fp8"] = lambda: ops.attention_decode_window(q, k8, v8, bounds, H, scale, causal=True,
+                                                                            k_descale=kd, v_descale=vd)
+        times = {a: [] for a in arms}
+        for fn in arms.values():
+            fn()
+        torch.cuda.synchronize()
+        for _ in range(reps):
+            for a, fn in arms.items():
+                e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                e0.record()
+                for _ in range(iters):
+                    fn()
+                e1.record()
+                torch.cuda.synchronize()
+                times[a].append(e0.elapsed_time(e1) / iters)
+        out[f"k{n}"] = {a: stats(t) for a, t in times.items()}
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=30)
     ap.add_argument("--batches", default="1,16")
     ap.add_argument("--out", default=None)
     ap.add_argument("--profile", action="store_true", help="trace the steps instead of timing them")
+    ap.add_argument("--step-tokens", default=None, help="e.g. 1,4,8,16,64: time k-token replays (extend + rewind)")
+    ap.add_argument("--kernel-leg", action="store_true", help="time the attention kernels at the decode-core shape")
     a = ap.parse_args()
     assert torch.cuda.is_available(), "graph_decode_bench measures on a GPU"
-    res = {"card": card(), ("step_profile" if a.profile else "step"):
-           [run(int(b), a.steps, a.profile) for b in a.batches.split(",")]}
+    res = {"card": card()}
+    if a.kernel_leg:
+        res["kernel_leg"] = kernel_leg()
+    elif a.step_tokens:
+        ks = [int(k) for k in a.step_tokens.split(",")]
+        res["tokens_profile" if a.profile else "tokens"] = [run_tokens(int(b), ks, a.steps, a.profile)
+                                                            for b in a.batches.split(",")]
+    else:
+        res["step_profile" if a.profile else "step"] = [run(int(b), a.steps, a.profile) for b in a.batches.split(",")]
     line = json.dumps(res)
     print(line)
     if a.out:
