@@ -568,6 +568,11 @@ PCV_API int pcv_rotary_apply_fp8(const pcv_rotary_params* p, const pcv_rotary_fp
  * in their params is fixed for the life of a graph; only the int32s behind `bounds` change (in-graph tensor ops write
  * them).  None of these entry points synchronises or reads device memory on the host.
  *
+ * Every batch row has its own bounds when `bounds_stride_b` > 0: batch row b (the arena's batch row; also with a batch-1
+ * q, q_stride_b == 0) reads bounds + b * bounds_stride_b, so each row of a batched decode loop can sit at its own rows
+ * (per-row rewind of speculative decoding).  bounds_stride_b == 0: every row reads the same bounds.  A negative stride
+ * is refused before any CUDA call.  The grid and the workspace do not depend on the bounds either way.
+ *
  * pcv_attn_decode_window (_fp8): the streaming decode kernel on the key window [bounds[0], bounds[1]) of an arena.
  * k, v and pad_mask point at arena row 0 and M == capacity (the arena's rows); pad bytes are indexed by the absolute
  * arena row.  The split count is planned on the host from `capacity`, so the grid and the workspace
@@ -589,7 +594,7 @@ PCV_API int pcv_rotary_apply_fp8(const pcv_rotary_params* p, const pcv_rotary_fp
 typedef struct pcv_dev_rows {
   const int32_t* bounds;   /* device int32s; meaning per entry point above                  */
   int32_t capacity;        /* rows of the arena (host-known, fixed for the life of a graph) */
-  int32_t reserved;
+  int32_t bounds_stride_b; /* int32s between the bounds of batch rows b and b + 1; 0: shared */
 } pcv_dev_rows;
 
 PCV_API int pcv_attn_decode_window_supported(const pcv_attn_params* p, const pcv_dev_rows* rows);

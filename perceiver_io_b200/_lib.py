@@ -269,7 +269,7 @@ class RotaryFp8(C.Structure):
 
 
 class DevRows(C.Structure):
-    _fields_ = [("bounds", C.c_void_p), ("capacity", C.c_int32), ("reserved", C.c_int32)]
+    _fields_ = [("bounds", C.c_void_p), ("capacity", C.c_int32), ("bounds_stride_b", C.c_int32)]
 
 
 class LnLinearBwdParams(C.Structure):

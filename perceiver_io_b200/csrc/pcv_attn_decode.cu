@@ -32,7 +32,11 @@ constexpr int kMaxQ = 4;
 
 struct DecParams {
   pcv_attn_params a;
-  int nsplit, keys_per_split;
+  int nsplit;
+  union {
+    int keys_per_split;  // without WIN
+    int win_stride_b;    // WIN: int32s between the windows of batch rows b and b + 1 (0: one shared window)
+  };
   float* ws_o;        // [B*H][nsplit][NQ][dv]
   float* ws_m;        // [B*H][nsplit][NQ]
   float* ws_l;        // [B*H][nsplit][NQ]
@@ -66,9 +70,10 @@ __device__ __forceinline__ void unpack_chunk(const uint4& u, float (&f)[FP8 ? 16
 
 // LPK lanes share one key; NQ query rows.  FP8 (pcv_attn_decode_fp8): K / V are e4m3 rows (a 16-byte chunk carries 16
 // channels), k_descale[h] is folded into the scaled q and v_descale[h, c] multiplies the accumulator once, before the
-// merge; everything else is shared.  WIN (pcv_attn_decode_window): the keys are the window [win[0], win[1]) of an arena
-// of a.M rows, read from device memory: every split takes an equal share of the window, the causal mask is
-// right-aligned to its end, and an empty window writes zeros.  f8 and win are unused without FP8 / WIN.
+// merge; everything else is shared.  WIN (pcv_attn_decode_window): the keys are batch row b's window [w[0], w[1]),
+// w = win + b * p.win_stride_b, of an arena of a.M rows, read from device memory: every split takes an equal share of
+// the window, the causal mask is right-aligned to its end, and an empty window writes zeros.  f8 and win are unused
+// without FP8 / WIN.
 template <typename T, int LPK, int NQ, bool FP8, bool WIN>
 __global__ void __launch_bounds__(kDecThreads)
     attn_decode_kernel(const DecParams p, const pcv_decode_fp8 f8, const int32_t* win) {
@@ -89,8 +94,9 @@ __global__ void __launch_bounds__(kDecThreads)
   const int bh = b * a.H + h;
   int kb, ke, wend = 0;
   if constexpr (WIN) {
-    const int w0 = max(win[0], 0);
-    wend = min(win[1], a.M);
+    const int32_t* w = win + (int64_t)b * p.win_stride_b;
+    const int w0 = max(w[0], 0);
+    wend = min(w[1], a.M);
     const int kps = (max(wend - w0, 0) + p.nsplit - 1) / p.nsplit;
     kb = w0 + split * kps;
     ke = min(wend, kb + kps);
@@ -386,6 +392,7 @@ bool attn_decode_supported(const pcv_attn_params& a, const pcv_decode_fp8* f, co
   if (rows != nullptr) {
     if (rows->bounds == nullptr) return fail("rows->bounds is NULL");
     if (rows->capacity != a.M) return fail("M must equal rows->capacity (k / v / pad_mask point at arena row 0)");
+    if (rows->bounds_stride_b < 0) return fail("rows->bounds_stride_b must be >= 0");
   }
   if (a.dtype != PCV_BF16 && a.dtype != PCV_F16) return fail("dtype (of q and out) must be bf16 or fp16");
   if (a.impl != PCV_IMPL_AUTO && a.impl != PCV_IMPL_DECODE) return fail("impl must be AUTO or DECODE");
@@ -454,6 +461,7 @@ int launch_attn_decode(const pcv_attn_params& a, const pcv_decode_fp8* f, const 
   const int lpk = lanes_per_key(a, f != nullptr);
   const pcv_decode_fp8 f8 = f != nullptr ? *f : pcv_decode_fp8{};
   const int32_t* win = rows != nullptr ? rows->bounds : nullptr;
+  if (rows != nullptr) p.win_stride_b = rows->bounds_stride_b;  // the window kernel splits the window, not M
   auto launch = [&](auto t) {
     using T = decltype(t);
     if (f != nullptr)

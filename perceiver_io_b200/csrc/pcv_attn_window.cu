@@ -4,9 +4,10 @@
 // one-token loop gives that token.  The arena holds bf16 / fp16 rows of q's type or e4m3 codes.
 //
 //   grid = B * nsplit * H CTAs, head index fastest; nsplit is planned on the host from the arena's capacity (as
-//   pcv_attn_cached_fp8 plans it from M), so the grid and the workspace are fixed for the life of a graph.  The window
-//   [bounds[0], bounds[1]) is read from device memory when the kernel runs and clamped to [0, capacity); its 64-key
-//   tiles start at its begin (not tile-aligned) and every split takes an equal share of them.  256 threads:
+//   pcv_attn_cached_fp8 plans it from M), so the grid and the workspace are fixed for the life of a graph.  Batch row
+//   b's window [w[0], w[1]), w = bounds + b * bounds_stride_b, is read from device memory when the kernel runs and
+//   clamped to [0, capacity); its 64-key tiles start at its begin (not tile-aligned) and every split takes an equal
+//   share of them.  256 threads:
 //     warpgroup 1, the loader: 16-bit rows go straight into a ring of SWIZZLE_128B stages with 16-byte cp.async (keys
 //       past the window's end and the channel tail of a k16 step are zero-filled); e4m3 rows are loaded into registers
 //       and converted exactly to q's type, as attn_cached_fp8_kernel does.  full / empty mbarriers guard the ring.
@@ -65,6 +66,7 @@ struct WindowParams {
   float* ws_m;                  // [B*H][nsplit][N]
   float* ws_l;                  // [B*H][nsplit][N]
   unsigned int* tickets;        // [B*H], zero on entry; the last CTA of a (b, h) resets its ticket
+  int win_stride_b;             // int32s between the windows of batch rows b and b + 1 (0: one shared window)
 };
 
 // 16 bytes global -> shared, zero-filled when !live (nothing is read then)
@@ -98,7 +100,8 @@ __global__ void __launch_bounds__(kThreads, NVB == 1 ? 2 : 1) attn_window_kernel
   const int b = blockIdx.x / (a.H * p.nsplit);
   const int bh = b * a.H + h;
   // the window clamped to the arena; this split takes its tiles [t0, t1), tile t = keys w0 + 64 t .. (< wend)
-  const int w0 = max(p.win[0], 0), wend = min(p.win[1], a.M);
+  const int32_t* win = p.win + (int64_t)b * p.win_stride_b;
+  const int w0 = max(win[0], 0), wend = min(win[1], a.M);
   const int ntiles = (max(wend - w0, 0) + kKeys - 1) / kKeys;
   const int tps = (ntiles + p.nsplit - 1) / p.nsplit;
   const int t0 = min(ntiles, split * tps), t1 = min(ntiles, t0 + tps);
@@ -445,6 +448,7 @@ bool attn_window_supported(const pcv_attn_params& a, const pcv_decode_fp8* f, co
   if (rows.bounds == nullptr) return fail("rows->bounds is NULL");
   if (rows.capacity < 1) return fail("rows->capacity must be >= 1");
   if (rows.capacity != a.M) return fail("M must equal rows->capacity (k / v / pad_mask point at arena row 0)");
+  if (rows.bounds_stride_b < 0) return fail("rows->bounds_stride_b must be >= 0");
   if (a.dtype != PCV_BF16 && a.dtype != PCV_F16)
     return fail(f != nullptr ? "dtype (of q and out) must be bf16 or fp16"
                              : "dtype (of q, the K / V arenas and out) must be bf16 or fp16");
@@ -491,6 +495,7 @@ int launch_attn_window(const pcv_attn_params& a, const pcv_decode_fp8* f, const 
   p.a = a;
   if (f != nullptr) p.f = *f;
   p.win = rows.bounds;
+  p.win_stride_b = rows.bounds_stride_b;
   p.band = band;
   p.nsplit = pl.nsplit;
   p.nkb = pl.nkb;

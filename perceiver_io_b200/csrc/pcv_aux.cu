@@ -184,14 +184,16 @@ __global__ void __launch_bounds__(256) rescale_kernel(const pcv_rescale_params p
 
 // ---------------------------------------------------------------------------------------------
 // rotary: one thread per channel pair.
-// AT (pcv_rotary_apply_at): the angle row of input row i is at.bounds[0] + i, and so is its output row when
-// at.bounds[1] != 0; rows whose angle row lies outside [0, at.capacity) are skipped.
+// AT (pcv_rotary_apply_at): with row b's bounds w = at.bounds + b * at.bounds_stride_b, the angle row of input row i
+// is w[0] + i, and so is its output row when w[1] != 0; rows whose angle row lies outside [0, at.capacity) are skipped.
 // ---------------------------------------------------------------------------------------------
 template <bool AT>
-__device__ __forceinline__ bool at_rows(const pcv_rotary_params& p, const pcv_dev_rows& at, int i, int* arow, int* yrow) {
+__device__ __forceinline__ bool at_rows(const pcv_rotary_params& p, const pcv_dev_rows& at, int b, int i, int* arow,
+                                        int* yrow) {
   if constexpr (AT) {
-    *arow = at.bounds[0] + i;
-    *yrow = at.bounds[1] ? *arow : i;
+    const int32_t* w = at.bounds + (int64_t)b * at.bounds_stride_b;
+    *arow = w[0] + i;
+    *yrow = w[1] ? *arow : i;
     return *arow >= 0 && *arow < at.capacity;
   } else {
     *arow = p.angle_row0 + i;
@@ -214,7 +216,7 @@ __global__ void __launch_bounds__(256) rotary_kernel(const pcv_rotary_params p, 
     const int b = (int)(rest / p.n);
     const int c = 2 * pr;
     int arow, yrow;
-    if (!at_rows<AT>(p, at, i, &arow, &yrow)) continue;
+    if (!at_rows<AT>(p, at, b, i, &arow, &yrow)) continue;
     const T* x = reinterpret_cast<const T*>(p.x) + (int64_t)b * p.x_stride_b + (int64_t)i * p.x_stride_n +
                  (int64_t)h * p.x_stride_h;
     T* y = reinterpret_cast<T*>(p.y) + (int64_t)b * p.y_stride_b + (int64_t)yrow * p.y_stride_n +
@@ -252,11 +254,12 @@ struct CopyArgs {
   int B;
 };
 
-// AT (pcv_kv_append_at): the first destination row is at.bounds[0]; rows outside [0, at.capacity) are skipped
+// AT (pcv_kv_append_at): the first destination row of batch row b is at.bounds[b * at.bounds_stride_b]; rows outside
+// [0, at.capacity) are skipped
 template <bool AT>
-__device__ __forceinline__ bool dst_row(const CopySeg& s, const pcv_dev_rows& at, int row, int* r) {
+__device__ __forceinline__ bool dst_row(const CopySeg& s, const pcv_dev_rows& at, int b, int row, int* r) {
   if constexpr (AT) {
-    *r = at.bounds[0] + row;
+    *r = at.bounds[(int64_t)b * at.bounds_stride_b] + row;
     return *r >= 0 && *r < at.capacity;
   } else {
     *r = s.dst_row0 + row;
@@ -280,7 +283,7 @@ __global__ void __launch_bounds__(256) kv_append_kernel(const CopyArgs a, const 
       const int row = (int)(rr % s.rows);
       const int b = (int)(rr / s.rows);
       int drow;
-      if (!dst_row<AT>(s, at, row, &drow)) continue;
+      if (!dst_row<AT>(s, at, b, row, &drow)) continue;
       const int4 val = *reinterpret_cast<const int4*>(s.src + b * s.s_sb + row * s.s_sl + ((int64_t)w << 4));
       *reinterpret_cast<int4*>(s.dst + b * s.d_sb + (int64_t)drow * s.d_sl + ((int64_t)w << 4)) = val;
     }
@@ -294,7 +297,7 @@ __global__ void __launch_bounds__(256) kv_append_kernel(const CopyArgs a, const 
       const int row = (int)(rr % s.rows);
       const int b = (int)(rr / s.rows);
       int drow;
-      if (!dst_row<AT>(s, at, row, &drow)) continue;
+      if (!dst_row<AT>(s, at, b, row, &drow)) continue;
       const unsigned short val =
           *reinterpret_cast<const unsigned short*>(s.src + b * s.s_sb + row * s.s_sl + ((int64_t)w << 1));
       *reinterpret_cast<unsigned short*>(s.dst + b * s.d_sb + (int64_t)drow * s.d_sl + ((int64_t)w << 1)) = val;
@@ -327,7 +330,7 @@ __global__ void __launch_bounds__(256) kv_append_fp8_kernel(const QuantArgs a, c
     const int row = (int)(rr % s.rows);
     const int b = (int)(rr / s.rows);
     int drow;
-    if (!dst_row<AT>(s, at, row, &drow)) continue;
+    if (!dst_row<AT>(s, at, b, row, &drow)) continue;
     const char* src = s.src + b * s.s_sb + row * s.s_sl;
     int4* dst = reinterpret_cast<int4*>(s.dst + b * s.d_sb + (int64_t)drow * s.d_sl + ((int64_t)w << 4));
     if (!quant) {
@@ -368,7 +371,7 @@ __global__ void __launch_bounds__(256)
     const int b = (int)(rest / p.n);
     const int c = 2 * pr;
     int arow, yrow;
-    if (!at_rows<AT>(p, at, i, &arow, &yrow)) continue;
+    if (!at_rows<AT>(p, at, b, i, &arow, &yrow)) continue;
     const T* x = reinterpret_cast<const T*>(p.x) + (int64_t)b * p.x_stride_b + (int64_t)i * p.x_stride_n +
                  (int64_t)h * p.x_stride_h;
     uint8_t* y = reinterpret_cast<uint8_t*>(p.y) + (int64_t)b * p.y_stride_b + (int64_t)yrow * p.y_stride_n +
@@ -492,6 +495,7 @@ int launch_rescale(const pcv_rescale_params& p, cudaStream_t stream) {
 
 // the device rows of the *_at entry points
 static bool dev_rows_ok(const pcv_dev_rows* at) { return at == nullptr || (at->bounds != nullptr && at->capacity >= 1); }
+static bool dev_stride_ok(const pcv_dev_rows* at) { return at == nullptr || at->bounds_stride_b >= 0; }
 
 bool rotary_fp8_supported(const pcv_rotary_params& p, const pcv_rotary_fp8& f, const char** why) {
   auto fail = [&](const char* w) {
@@ -539,6 +543,8 @@ int launch_rotary(const pcv_rotary_params& p, const pcv_rotary_fp8* f, const pcv
     PCV_REQUIRE(p.dtype == PCV_BF16 || p.dtype == PCV_F16, PCV_ERR_INVALID, "rotary: unknown dtype %d", p.dtype);
   }
   PCV_REQUIRE(dev_rows_ok(at), PCV_ERR_INVALID, "%s: rows->bounds NULL or capacity < 1",
+              f != nullptr ? "rotary_at_fp8" : "rotary_at");
+  PCV_REQUIRE(dev_stride_ok(at), PCV_ERR_INVALID, "%s: rows->bounds_stride_b must be >= 0",
               f != nullptr ? "rotary_at_fp8" : "rotary_at");
   if (p.n == 0) return PCV_OK;
   const int64_t total = (int64_t)p.B * p.n * p.H * ((p.d + 1) / 2);  // one thread per channel pair
@@ -591,6 +597,7 @@ int launch_kv_append(const pcv_kv_append_params& p, const pcv_kv_fp8_scales* f, 
   if (at != nullptr) {
     const char* what = f != nullptr ? "kv_append_at_fp8" : "kv_append_at";
     PCV_REQUIRE(dev_rows_ok(at), PCV_ERR_INVALID, "%s: rows->bounds NULL or capacity < 1", what);
+    PCV_REQUIRE(dev_stride_ok(at), PCV_ERR_INVALID, "%s: rows->bounds_stride_b must be >= 0", what);
     PCV_REQUIRE(p.L_old == 0 && p.k_cache == nullptr && p.v_cache == nullptr, PCV_ERR_INVALID,
                 "%s: an append at device rows takes no cache (k_cache = v_cache = NULL, L_old = 0)", what);
   }

@@ -3,8 +3,8 @@ replay.
 
 An eager cached step spends most of its time on the host (module code, arena and rotated-shadow bookkeeping, a few
 hundred ctypes / ATen launches).  Every length in it changes each token, so it cannot be recorded as it is.
-``GraphedDecoder`` keeps the caches in static arenas and the lengths in a few device int32s: per layer group the key
-window ``[begin, end)`` and the new token's row.  The append (``ops.kv_append_at``), the rotary embedding
+``GraphedDecoder`` keeps the caches in static arenas and the lengths in a few device int32s: per batch row and layer
+group the key window ``[begin, end)`` and the new token's row.  The append (``ops.kv_append_at``), the rotary embedding
 (``ops.rotary_apply_at``) and the decode attention (``ops.attention_decode_window``) read their rows from there when they
 run, and in-graph int32 ops advance them at the end of each step.
 
@@ -13,6 +13,7 @@ run, and in-graph int32 ops advance them at the end of each step.
     logits = dec.step(token_ids)                                              # (B, 1) int64 -> (B, vocab), one replay
     logits = dec.extend(token_ids)                                            # (B, k) int64 -> (B, k, vocab)
     dec.rewind(n)                                                             # drop the last n fed tokens
+    dec.rewind(counts)                                                        # drop the last counts[b] of row b
     dec.reorder(beam_idx)                                                     # beam search (eager)
 
 Rows: cross-attention arena row r holds token r of the sequence (prompt and generated tokens); self-attention arena
@@ -23,16 +24,22 @@ row r holds token ``prefix_len + r`` (prefix_len of the prompt).  The windows fo
 one token) and returns the logits after each of them: every token attends exactly the keys the one-token loop gives it
 (``ops.attention_window`` with a causal band of the group's window width), so speculative decoding can verify k draft
 tokens in one replay, keep the accepted prefix and ``rewind`` the rest.  ``rewind(n)`` moves the row counters back by
-n tokens with eager int32 ops (no host read, no re-capture); the arena rows past the new end are overwritten later.  The
-batch rows share one window per layer group, so ``rewind`` takes one count for all of them: a batched speculative loop
-rewinds to the smallest accepted count and feeds the remaining accepted tokens again.
+n tokens with eager int32 ops (no host read, no re-capture); the arena rows past the new end are overwritten later.
+Every batch row has its own counters, so ``rewind`` also takes one count per batch row: a batched speculative loop
+drops exactly each row's rejected drafts, and the next ``extend`` feeds every row at its own next row (the kernels
+read each batch row's bounds; one graph per k serves every pattern of rows).
 
-Not covered: per-batch-row accept counts, steps of more than 64 tokens, contrastive search, a ring buffer bounded at
+Budget: ``max_new_tokens`` counts per batch row.  The arenas hold room for the row that has fed the most tokens, so
+``extend(k)`` is refused exactly when that row has fewer than k tokens left, and a per-row ``rewind`` gives back what
+that row regains.  The counts are host integers; nothing is read back from the device.
+
+Not covered: steps of more than 64 tokens, a different k per batch row, contrastive search, a ring buffer bounded at
 ``max_seq_len`` (the arenas grow by ``max_new_tokens`` rows) and wiring into 🤗 ``generate()``.
 """
 from __future__ import annotations
 
 import operator
+from collections.abc import Sequence
 from typing import List, NamedTuple
 
 import torch
@@ -41,7 +48,7 @@ from . import modules, ops
 from .graphs import GraphedForward
 from .utils import Residual
 
-# bounds columns of one layer group: [window begin, window end, new row, 1, new row, 0]
+# bounds columns of one batch row and layer group: [window begin, window end, new row, 1, new row, 0]
 #   [0:2] the decode window, [2:3] the append row, [2:4] rotary into the rotated-key arena, [4:6] rotary of q
 _NCOL = 6
 
@@ -72,20 +79,23 @@ def decode_windows(prompt_len: int, prefix_len: int, steps: int, max_seq_len: in
 def window_positions(pad: torch.Tensor, window: torch.Tensor, cols: torch.Tensor) -> torch.Tensor:
     """(B, 1) int64 absolute position of the last token of the window ``[window[0], window[1])`` of left-padded rows:
     ``positions(b, n, shift)[:, -1:]`` of the eager call, with ``n`` the window length and ``shift`` its padding count,
-    computed from tensors alone (no host read).  ``pad`` (B, rows) bytes, non-zero = padding; ``cols`` = arange(rows)."""
-    inside = (cols >= window[0]) & (cols < window[1])
+    computed from tensors alone (no host read).  ``pad`` (B, rows) bytes, non-zero = padding; ``cols`` = arange(rows).
+    ``window`` (B, 2): batch row b's own window ``window[b]``."""
+    lo, hi = window[..., 0:1], window[..., 1:2]
+    inside = (cols >= lo) & (cols < hi)
     shift = ((pad != 0) & inside).sum(dim=1, keepdim=True)
-    return (window[1] - window[0] - 1 - shift).clamp_min(0).long()
+    return (hi - lo - 1 - shift).clamp_min(0).long()
 
 
 def window_positions_rows(pad: torch.Tensor, bounds: torch.Tensor, cols: torch.Tensor, k: int,
                           width: int) -> torch.Tensor:
     """(B, k) int64 absolute positions of the k tokens of a step whose last token is row ``bounds[1] - 1``: token i at
     row ``r_i = bounds[1] - k + i`` takes :func:`window_positions` of its own one-token window
-    ``[max(0, r_i + 1 - width), r_i + 1)``.  Tensors alone, no host read; ``pad`` and ``cols`` as there."""
-    r = bounds[1] - k + torch.arange(k, device=cols.device, dtype=cols.dtype)
+    ``[max(0, r_i + 1 - width), r_i + 1)``.  Tensors alone, no host read; ``pad`` and ``cols`` as there.  ``bounds``
+    (B, >= 2): batch row b's own ``bounds[b]``."""
+    r = bounds[..., 1:2] - k + torch.arange(k, device=cols.device, dtype=cols.dtype)
     begin = (r + 1 - width).clamp_min(0)
-    inside = (cols >= begin[:, None]) & (cols <= r[:, None])
+    inside = (cols >= begin[..., None]) & (cols <= r[..., None])
     shift = ((pad != 0)[:, None, :] & inside).sum(dim=2)
     return (r - begin - shift).clamp_min(0).long()
 
@@ -93,18 +103,33 @@ def window_positions_rows(pad: torch.Tensor, bounds: torch.Tensor, cols: torch.T
 def extend_bounds(bounds: torch.Tensor, k: int) -> torch.Tensor:
     """The (groups, 6) int32 bounds of a k-token step from the one-token state ``bounds`` (``[begin, end, row, 1, row,
     0]`` per layer group, end = row + 1): the window's end moves to the last token's row + 1, everything else stays —
-    the window starts at the first token's begin, appends and rotations start at its row."""
+    the window starts at the first token's begin, appends and rotations start at its row.  (B, groups, 6) per-row
+    states move every batch row the same way."""
     out = bounds.clone()
-    out[:, 1] += k - 1
+    out[..., 1] += k - 1
     return out
 
 
-def advance_bounds_(bounds: torch.Tensor, inc: torch.Tensor, wmax: torch.Tensor, n: int) -> torch.Tensor:
+def advance_bounds_(bounds: torch.Tensor, inc: torch.Tensor, wmax: torch.Tensor, n) -> torch.Tensor:
     """Move the one-token state ``bounds`` by n tokens in place (n < 0 rewinds): row and end += n, begin = max(0,
-    end - the group's window width ``wmax``).  ``inc`` is ``[0, 1, 1, 0, 1, 0]``."""
-    bounds.add_(inc, alpha=n)
-    bounds[:, 0].copy_((bounds[:, 1] - wmax).clamp_min_(0))
+    end - the group's window width ``wmax``).  ``inc`` is ``[0, 1, 1, 0, 1, 0]``.  ``n`` an integer moves every row;
+    a (B,) int32 tensor on ``bounds``' device moves batch row b of a (B, groups, 6) state by ``n[b]``."""
+    if isinstance(n, torch.Tensor):
+        bounds.add_(inc * n[:, None, None])
+    else:
+        bounds.add_(inc, alpha=n)
+    bounds[..., 0].copy_((bounds[..., 1] - wmax).clamp_min_(0))
     return bounds
+
+
+def _as_count(x):
+    """x as an int when it is integer-like (operator.index) and not a bool, else None."""
+    if isinstance(x, bool):
+        return None
+    try:
+        return operator.index(x)
+    except TypeError:
+        return None
 
 
 class _Attn:
@@ -117,6 +142,10 @@ class _Attn:
 
 
 class GraphedDecoder:
+    # per-row counts: None while every batch row has fed the same tokens, else _lag[b] = the tokens row b has fed fewer
+    # than the furthest row (whose count is _fed)
+    _lag = None
+
     def __init__(self, model, batch: int, max_new_tokens: int, kv_cache: str = "bf16"):
         if max_new_tokens < 1:
             raise ValueError(f"GraphedDecoder: max_new_tokens must be >= 1, got {max_new_tokens}")
@@ -208,31 +237,33 @@ class GraphedDecoder:
         w = decode_windows(n0, prefix_len, 1, m.max_seq_len, m.max_latents)[0]
         rows = (n0, n0 - prefix_len)
         self._bounds = torch.tensor([[w.ca_begin, w.ca_end, rows[0], 1, rows[0], 0],
-                                     [w.sa_begin, w.sa_end, rows[1], 1, rows[1], 0]], dtype=torch.int32, device=dev)
+                                     [w.sa_begin, w.sa_end, rows[1], 1, rows[1], 0]],
+                                    dtype=torch.int32, device=dev).repeat(B, 1, 1)   # (B, groups, 6): per batch row
         self._inc = torch.tensor([0, 1, 1, 0, 1, 0], dtype=torch.int32, device=dev)
         self._wmax = torch.tensor([m.max_seq_len, m.max_latents], dtype=torch.int32, device=dev)
         self._width = (m.max_seq_len, m.max_latents)
         self._graphs = {}
         self._remaining = T
         self._fed = 0
+        self._lag = None
         return out.logits[:, -1]
 
     # ---- one step of 1 to 64 tokens ----------------------------------------------------------------------------------
     def _attend(self, a: _Attn, bounds, q, k, v):
-        H, g = a.mha.num_heads, bounds[a.group]
+        H, g = a.mha.num_heads, bounds[:, a.group]   # (B, 6): every batch row's own rows
         fp8 = self.fp8
-        ops.kv_append_at(a.K, a.V, k, v, g[2:3], *((a.kv8.k_inv, a.kv8.v_inv) if fp8 else ()))
+        ops.kv_append_at(a.K, a.V, k, v, g[:, 2:3], *((a.kv8.k_inv, a.kv8.v_inv) if fp8 else ()))
         keys = a.K
         if a.rotary:   # the new key into the rotated-key arena, q at the new token's row
-            ops.rotary_apply_at(k, H, a.table, g[2:4], a.S, a.k_inv_h)
-            q = ops.rotary_apply_at(q, H, a.table, g[4:6], torch.empty(q.shape, dtype=q.dtype, device=q.device))
+            ops.rotary_apply_at(k, H, a.table, g[:, 2:4], a.S, a.k_inv_h)
+            q = ops.rotary_apply_at(q, H, a.table, g[:, 4:6], torch.empty(q.shape, dtype=q.dtype, device=q.device))
             keys = a.S
         kw = dict(pad_mask=self._pad if a.group == 0 else None, causal=a.mha.causal_attention,
                   k_descale=a.kv8.k_descale if fp8 else None, v_descale=a.kv8.v_descale if fp8 else None)
         if q.shape[1] == 1:
-            o = ops.attention_decode_window(q, keys, a.V, g[0:2], H, a.mha.dp_scale, **kw)
+            o = ops.attention_decode_window(q, keys, a.V, g[:, 0:2], H, a.mha.dp_scale, **kw)
         else:   # every token sees its own one-token window: a causal band of the group's window width
-            o = ops.attention_window(q, keys, a.V, g[0:2], H, a.mha.dp_scale, band=self._width[a.group], **kw)
+            o = ops.attention_window(q, keys, a.V, g[:, 0:2], H, a.mha.dp_scale, band=self._width[a.group], **kw)
         return modules.fused_linear(a.mha, "_pcv_o_fold", None, a.mha.o_proj, o, a.key)
 
     @staticmethod
@@ -246,8 +277,8 @@ class GraphedDecoder:
         b = self._bounds if k == 1 else extend_bounds(self._bounds, k)
         x = adapter.txt_embedding(token)
         if getattr(adapter, "_abs_pos_emb", False):
-            pos = (window_positions(self._pad, b[0, 0:2], self._cols) if k == 1
-                   else window_positions_rows(self._pad, b[0], self._cols, k, self._width[0]))
+            pos = (window_positions(self._pad, b[:, 0, 0:2], self._cols) if k == 1
+                   else window_positions_rows(self._pad, b[:, 0], self._cols, k, self._width[0]))
             x = x + adapter.pos_embedding(pos)
         # cross-attention (cached: the keys of this token are its own q_norm'd row, reference modules.py:222-224)
         ca_layer, ca = m.cross_attention, self._layers[0].owner
@@ -282,7 +313,8 @@ class GraphedDecoder:
                              f"{tuple(token_ids.shape)} {token_ids.dtype}")
         if self._remaining < k:
             raise RuntimeError(f"GraphedDecoder: {self._remaining} of max_new_tokens={self.max_new_tokens} tokens remain "
-                               f"(the arenas hold no room for {k} more); rewind, or call prefill() again")
+                               f"to the furthest batch row (the arenas hold no room for {k} more); rewind, or call "
+                               f"prefill() again")
         if torch.is_autocast_enabled():
             raise RuntimeError("GraphedDecoder does not run under autocast")
         graph = self._graphs.get(k)
@@ -316,31 +348,77 @@ class GraphedDecoder:
             return self._replay(token_ids, "extend")[:, None]
         return self._replay(token_ids, "extend")
 
-    def rewind(self, n: int) -> None:
-        """Drop the last ``n`` fed tokens from every layer group: the next token is fed at the row of the first dropped
-        one, as if the n tokens had never been fed.  Eager int32 ops on the row counters (no host read of the device,
-        no re-capture); gives n tokens back to the budget.  One count for all batch rows (they share the windows): a
-        batched speculative loop rewinds to the smallest accepted count and feeds the rest again."""
+    def rewind(self, n) -> None:
+        """Drop fed tokens: the next token of a batch row is fed at the row of its first dropped one, as if the dropped
+        tokens had never been fed.  ``n`` an integer drops the last n tokens of every batch row; a sequence of B
+        integers, or a CPU integer tensor of shape (B,), drops the last ``n[b]`` of row b (per-row accept counts of
+        batched speculative decoding).  Each count is at most the tokens its row has fed since prefill.  Eager int32 ops
+        on the row counters (no host read of the device, no re-capture).  Gives back to the budget what the furthest
+        row regains.  A refused ``n`` leaves the state untouched."""
         if self._bounds is None:
             raise RuntimeError("GraphedDecoder: call prefill() first")
-        try:
-            count = operator.index(n) if not isinstance(n, bool) else None
-        except TypeError:
-            count = None
-        if count is None or count < 0 or count > self._fed:
-            raise ValueError(f"GraphedDecoder.rewind: n must be an integer in [0, {self._fed}] (the tokens fed since "
-                             f"prefill), got {n!r}")
-        n = count
-        if n:
-            advance_bounds_(self._bounds, self._inc, self._wmax, -n)
-            self._remaining += n
-            self._fed -= n
+        lag = self._lag or [0] * self.batch
+        if isinstance(n, (Sequence, torch.Tensor)) and not isinstance(n, (str, bytes)) and (
+                not isinstance(n, torch.Tensor) or n.dim() > 0):
+            counts = self._row_counts(n, lag)
+        else:
+            count = _as_count(n)
+            top = self._fed - max(lag)
+            if count is None or count < 0 or count > top:
+                raise ValueError(f"GraphedDecoder.rewind: n must be an integer in [0, {top}] (the tokens every batch "
+                                 f"row has fed since prefill), got {n!r}")
+            counts = [count] * self.batch
+        if len(set(counts)) == 1:   # one count: every row moves alike, the lags stay
+            if counts[0]:
+                advance_bounds_(self._bounds, self._inc, self._wmax, -counts[0])
+                self._remaining += counts[0]
+                self._fed -= counts[0]
+            return
+        per_row = torch.tensor(counts, dtype=torch.int32)
+        if self._bounds.is_cuda:   # pinned and asynchronous: no synchronisation
+            per_row = per_row.pin_memory().to(self._bounds.device, non_blocking=True)
+        advance_bounds_(self._bounds, self._inc, self._wmax, -per_row)
+        self._set_fed([self._fed - lg - c for lg, c in zip(lag, counts)])
+
+    def _row_counts(self, n, lag) -> List[int]:
+        """The per-row counts of ``rewind``, checked against every row's fed tokens."""
+        if isinstance(n, torch.Tensor):
+            if n.is_cuda:
+                raise ValueError("GraphedDecoder.rewind: per-row counts must be a CPU tensor (a CUDA tensor would need a "
+                                 "host read of the device)")
+            if n.dim() != 1 or n.dtype == torch.bool or n.dtype.is_floating_point or n.dtype.is_complex:
+                raise ValueError(f"GraphedDecoder.rewind: per-row counts must be a ({self.batch},) integer tensor, got "
+                                 f"{tuple(n.shape)} {n.dtype}")
+            n = n.tolist()
+        if len(n) != self.batch:
+            raise ValueError(f"GraphedDecoder.rewind: {self.batch} per-row counts (one per batch row), got {len(n)}")
+        counts = []
+        for b, c in enumerate(n):
+            count = _as_count(c)
+            fed = self._fed - lag[b]
+            if count is None or count < 0 or count > fed:
+                raise ValueError(f"GraphedDecoder.rewind: the count of batch row {b} must be an integer in [0, {fed}] "
+                                 f"(the tokens it has fed since prefill), got {c!r}")
+            counts.append(count)
+        return counts
+
+    def _set_fed(self, fed: List[int]) -> None:
+        """Host bookkeeping from the tokens every batch row has fed: the budget follows the furthest row."""
+        top = max(fed)
+        self._remaining += self._fed - top
+        self._fed = top
+        self._lag = [top - f for f in fed] if min(fed) != top else None
 
     def reorder(self, beam_idx: torch.Tensor) -> None:
-        """Permute the batch rows of every arena, rotated-key arena and the pad rows (beam search), eagerly."""
+        """Permute the batch rows of every arena, rotated-key arena, the pad rows and the row counters (beam search),
+        eagerly.  Sync-free while every row has fed the same tokens; once per-row rewinds left them at different
+        counts, ``beam_idx`` is read to the host once to permute the host bookkeeping."""
         idx = beam_idx.to(device=self.device, dtype=torch.long)
         for a in self._layers:
             for t in (a.K, a.V, a.S):
                 if t is not None:
                     t.copy_(t.index_select(0, idx))
         self._pad.copy_(self._pad.index_select(0, idx))
+        self._bounds.copy_(self._bounds.index_select(0, idx))
+        if self._lag is not None:
+            self._set_fed([self._fed - self._lag[i] for i in beam_idx.tolist()])

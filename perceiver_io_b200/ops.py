@@ -1170,12 +1170,17 @@ def rotated_cache_shadow(k: torch.Tensor):
 # --------------------------------------------------------------------------------------------------
 # device-resident rows: decode, append and rotary whose rows are read from device int32s when the kernel runs, so a
 # recorded CUDA graph replays every step of a decode loop (generation.GraphedDecoder).  They do no arena bookkeeping.
+# The bounds are 1-D (one set shared by every batch row) or (B, >= width) (row b reads bounds[b], at any row stride).
 # --------------------------------------------------------------------------------------------------
-def _dev_rows(bounds: torch.Tensor, capacity: int):
-    if bounds.dtype != torch.int32 or not bounds.is_cuda or bounds.numel() < 1 or bounds.stride(-1) != 1:
-        raise ValueError("bounds must be a CUDA int32 tensor with unit stride")
+def _dev_rows(bounds: torch.Tensor, capacity: int, batch: int, width: int, what: str):
+    if bounds.dtype != torch.int32 or not bounds.is_cuda or bounds.dim() not in (1, 2) or bounds.stride(-1) != 1:
+        raise ValueError(f"{what}: bounds must be a 1-D or 2-D CUDA int32 tensor with unit stride in its last dim")
+    if bounds.shape[-1] < width or (bounds.dim() == 2 and bounds.shape[0] != batch):
+        raise ValueError(f"{what}: bounds must be ({width},) shared by every batch row or ({batch}, {width}) per row, "
+                         f"got {tuple(bounds.shape)}")
     r = _lib.DevRows()
     r.bounds, r.capacity = bounds.data_ptr(), int(capacity)
+    r.bounds_stride_b = bounds.stride(0) if bounds.dim() == 2 else 0
     return r
 
 
@@ -1193,13 +1198,14 @@ def attention_decode_window(q, k, v, bounds: torch.Tensor, num_heads: int, scale
 
     q: (B or 1, N <= 4, H*dqk) bf16 / fp16; k, v: (B, capacity, H*d) arenas, bf16 / fp16 like q or ``float8_e4m3fn``
     codes (then ``k_descale`` (H,) and ``v_descale`` (H, dv) as in :func:`attention_decode_fp8`); ``pad_mask`` (B,
-    capacity), indexed by the absolute arena row; ``bounds`` a CUDA int32 tensor whose first two entries are the window.
-    The causal mask is right-aligned to the window's end; a window of length <= 0 gives zeros.  Returns (B, N, H*dv)."""
+    capacity), indexed by the absolute arena row; ``bounds`` a CUDA int32 tensor whose first two entries are the window,
+    or a (B, >= 2) one whose row b holds batch row b's window (unit stride in its last dim, any row stride).  The causal
+    mask is right-aligned to the window's end; a window of length <= 0 gives zeros.  Returns (B, N, H*dv)."""
     _require_cuda(q, k, v, bounds, pad_mask)
     with torch.cuda.device(k.device):
         p, f, keep = _fill_decode(q, k, v, num_heads, scale, pad_mask, causal, k_descale, v_descale)
         out = _new_output(p, _compute_dtype(q.dtype), k.device)
-        _run_decode(p, f, _dev_rows(bounds, p.M), k.device)
+        _run_decode(p, f, _dev_rows(bounds, p.M, p.B, 2, "attention_decode_window"), k.device)
     del keep
     return out
 
@@ -1216,8 +1222,9 @@ def attention_window(q, k, v, bounds: torch.Tensor, num_heads: int, scale: float
 
     q: (B or 1, N <= 64, H*dqk) bf16 / fp16; k, v: (B, capacity, H*d) arenas of q's dtype (head dims multiples of 8) or
     ``float8_e4m3fn`` codes (head dims multiples of 16, with ``k_descale`` (H,) and ``v_descale`` (H, dv) as in
-    :func:`attention_decode_fp8`); ``pad_mask`` (B, capacity), indexed by the absolute arena row.  Query i sits at row
-    ``r_i = end - N + i``.  With ``band`` W > 0 (``causal`` only) query i sees exactly the keys ``[r_i + 1 - W, r_i]``:
+    :func:`attention_decode_fp8`); ``pad_mask`` (B, capacity), indexed by the absolute arena row.  ``bounds`` 1-D is one
+    window for every batch row; (B, >= 2) gives batch row b its own window ``bounds[b, 0:2]`` (unit stride in its last
+    dim, any row stride; also with a batch-1 q).  Query i sits at row ``r_i = end - N + i`` of its batch row's window.  With ``band`` W > 0 (``causal`` only) query i sees exactly the keys ``[r_i + 1 - W, r_i]``:
     a key outside its band contributes nothing, a padded key inside it takes the finite fill — N rows of one call
     are then N one-token steps whose windows are ``[max(0, r_i + 1 - W), r_i + 1)``.  With W = 0 the causal mask is
     right-aligned to the window's end and masks as :func:`attention`.  A window of length <= 0 gives zeros.  P is
@@ -1242,7 +1249,7 @@ def attention_window(q, k, v, bounds: torch.Tensor, num_heads: int, scale: float
             f = None
         p.impl = _lib.PCV_IMPL_AUTO
         out = _new_output(p, q.dtype, k.device)
-        rows = _dev_rows(bounds, p.M)
+        rows = _dev_rows(bounds, p.M, p.B, 2, "attention_window")
         entry = "pcv_attn_cached_window" + ("_fp8" if fp8 else "")
         ws = _workspace(p, k.device, entry, C.byref(p))
         check(getattr(_lib.lib(), entry)(*(C.byref(s) for s in (p, f, rows) if s is not None), int(band), _stream()),
@@ -1254,7 +1261,8 @@ def attention_window(q, k, v, bounds: torch.Tensor, num_heads: int, scale: float
 def kv_append_at(k_arena: torch.Tensor, v_arena: torch.Tensor, k_new: torch.Tensor, v_new: torch.Tensor,
                  row: torch.Tensor, k_inv_scale=None, v_inv_scale=None) -> None:
     """Write the new rows k_new / v_new (B, n, C) to rows ``row[0] .. row[0] + n - 1`` of the arenas (B, capacity, C), the
-    row read from device memory when the kernel runs (pcv_kv_append_at); rows at or past capacity are skipped.
+    row read from device memory when the kernel runs (pcv_kv_append_at); rows at or past capacity are skipped.  ``row``
+    (B, >= 1) gives batch row b its own first row ``row[b, 0]``.
     ``float8_e4m3fn`` arenas store ``clamp(x * inv_scale, +-448)`` rounded to e4m3 (pcv_kv_append_at_fp8, per-channel
     ``k_inv_scale`` / ``v_inv_scale`` as in :func:`kv_append_fp8`)."""
     _require_cuda(k_arena, v_arena, k_new, v_new, row)
@@ -1266,7 +1274,8 @@ def kv_append_at(k_arena: torch.Tensor, v_arena: torch.Tensor, k_new: torch.Tens
     if k_arena.stride(-1) != 1 or v_arena.stride(-1) != 1:
         raise ValueError("kv_append_at: arenas need unit channel stride")
     _launch_kv_append(None, None, _rows_contiguous(k_new), _rows_contiguous(v_new), k_arena, v_arena, False, False,
-                      (k_inv_scale, v_inv_scale) if fp8 else None, _dev_rows(row, k_arena.shape[1]))
+                      (k_inv_scale, v_inv_scale) if fp8 else None,
+                      _dev_rows(row, k_arena.shape[1], k_arena.shape[0], 1, "kv_append_at"))
 
 
 def rotary_apply_at(x: torch.Tensor, num_heads: int, table: torch.Tensor, rows: torch.Tensor, out: torch.Tensor,
@@ -1274,7 +1283,8 @@ def rotary_apply_at(x: torch.Tensor, num_heads: int, table: torch.Tensor, rows: 
     """``out`` <- x (B, n, H*d) bf16 / fp16 rotated at the angle rows ``rows[0] + i`` of ``table`` (capacity, rotate_dim)
     (:func:`rotary_angle_table`), the rows read from device memory when the kernel runs (pcv_rotary_apply_at / _fp8).
     Row i goes to ``out[:, rows[0] + i]`` when ``rows[1] != 0`` (a key into a rotated-key arena of at least capacity
-    rows), else to ``out[:, i]``.  An e4m3 ``out`` stores the codes of the rotated rows times ``y_inv_scale[h]`` (H,).
+    rows), else to ``out[:, i]``.  ``rows`` (B, >= 2) gives batch row b its own ``rows[b, 0:2]``.  An e4m3 ``out``
+    stores the codes of the rotated rows times ``y_inv_scale[h]`` (H,).
     Bit-equal to :func:`rotary_at` / the rotated-key shadow of :func:`rotated_cache_keys` at the same positions."""
     _require_cuda(x, table, rows, out)
     x = _rows_contiguous(x)
@@ -1288,7 +1298,7 @@ def rotary_apply_at(x: torch.Tensor, num_heads: int, table: torch.Tensor, rows: 
     p = _rotary_params(x, out, num_heads, table[None], False, _pcv_dtype(x.dtype))
     f = _lib.RotaryFp8(x_descale=None, y_inv_scale=y_inv_scale.data_ptr()) if fp8 else None
     with torch.cuda.device(x.device):
-        _launch_rotary(p, f, _dev_rows(rows, table.shape[0]))
+        _launch_rotary(p, f, _dev_rows(rows, table.shape[0], x.shape[0], 2, "rotary_apply_at"))
     return out
 
 

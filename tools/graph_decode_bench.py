@@ -14,10 +14,20 @@ FP8 arenas, one replay of k tokens on the full context, then rewind(k) so that e
 device time and kernels per replay from a trace.  --kernel-leg times the attention kernels alone at the decode-core
 shape (B = 8, 16384 cached tokens, C = 1024, H = 8) for k = 2, 4, 5, 16, 64 query rows: ops.attention_window on bf16
 and e4m3 arenas, pcv_attn_decode_window (k <= 4), ops.attention_decode_fp8 (pcv_attn_cached_fp8 above 4 rows) and
-ops.attention on a bf16 cache, alternated, CUDA events around 20 launches."""
+ops.attention on a bf16 cache, alternated, CUDA events around 20 launches.
+
+--spec-rows 4,8 measures a batched speculative loop at each batch (bf16 arenas): every round feeds k draft tokens per
+row in one extend(k) replay; each draft is accepted with probability --accept until the row's first rejection (seeded
+per row).  Two arms, alternated round by round: "per_row" rewinds every row by its own rejected count; "refeed" is the
+loop without per-row rewinds: it rewinds every row to the smallest accepted count, and a row's other accepted tokens
+lead its next replay again (in place of drafts).  A token counts as accepted once it is kept by its row for good.  It
+reports ms per accepted token (replay and rewind, CUDA events and a synchronise around each round; over all rows) and
+replays per accepted token of one row, median (min-max) over --reps blocks of --steps rounds; every block starts from
+the prompt (a per-row rewind of everything fed)."""
 import argparse
 import json
 import os
+import random
 import statistics
 import sys
 
@@ -155,6 +165,72 @@ def run_tokens(batch, ks, reps, profile=False):
     return res
 
 
+def run_spec(batch, k, rounds, reps, accept):
+    """The batched speculative loop with per-row rewinds against the smallest-count rewind and refeed."""
+    torch.manual_seed(0)
+    cfg = P.CausalSequenceModelConfig(**GIANTMIDI)
+    model = P.CausalSequenceModel(cfg).cuda().bfloat16().eval()
+    n, prefix = cfg.max_seq_len, cfg.max_seq_len - cfg.max_latents
+    tokens = torch.randint(0, cfg.vocab_size, (batch, n + k), device="cuda")
+    feed = tokens[:, n:n + k]          # the token values do not change the work of a replay
+    arms = ("per_row", "refeed")
+    with torch.no_grad():
+        decs = {a: P.GraphedDecoder(model, batch=batch, max_new_tokens=(rounds + 1) * k) for a in arms}
+        for dec in decs.values():
+            dec.prefill(tokens[:, :n], prefix)
+            dec.extend(feed)           # the graph recorded and warmed up
+            dec.rewind(k)
+        torch.cuda.synchronize()
+
+        def accepted(rng, m):          # drafts kept before the first rejection, at most m
+            a = 0
+            while a < m and rng.random() < accept:
+                a += 1
+            return a
+
+        res = {"batch": batch, "k": k, "context": n, "accept": accept, "rounds_per_block": rounds}
+        blocks = {a: {"ms": [], "replays": []} for a in arms}
+        for rep in range(reps):
+            # the same seeded draws per row in both arms
+            rngs = {a: [random.Random(1000 * rep + b) for b in range(batch)] for a in arms}
+            fed = {a: [0] * batch for a in arms}
+            carry = [0] * batch        # refeed: accepted tokens a row has to feed again
+            ms = {a: 0.0 for a in arms}
+            for _ in range(rounds):
+                for a in arms:
+                    dec = decs[a]
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                    dec.extend(feed)
+                    if a == "per_row":
+                        acc = [accepted(r, k) for r in rngs[a]]
+                        dec.rewind([k - x for x in acc])
+                        fed[a] = [f + x for f, x in zip(fed[a], acc)]
+                    else:
+                        known = [min(c, k) for c in carry]
+                        got = [kn + accepted(r, k - kn) for kn, r in zip(known, rngs[a])]
+                        m = min(got)
+                        dec.rewind(k - m)
+                        carry = [c - kn + g - m for c, kn, g in zip(carry, known, got)]
+                        fed[a] = [f + m for f in fed[a]]
+                    e1.record()
+                    torch.cuda.synchronize()
+                    ms[a] += e0.elapsed_time(e1)
+            for a in arms:
+                kept = sum(fed[a])
+                blocks[a]["ms"].append(ms[a] / max(kept, 1))
+                blocks[a]["replays"].append(rounds * batch / max(kept, 1))
+                res.setdefault(f"{a}_accepted_per_row_per_round", []).append(round(kept / batch / rounds, 3))
+                decs[a].rewind(fed[a])   # back to the prompt for the next block
+        for a in arms:
+            res[f"{a}_ms_per_accepted_token"] = stats(blocks[a]["ms"])
+            res[f"{a}_replays_per_accepted_token"] = stats(blocks[a]["replays"])
+        res["speedup"] = round(statistics.median(blocks["refeed"]["ms"]) / statistics.median(blocks["per_row"]["ms"]), 2)
+    del decs, model
+    torch.cuda.empty_cache()
+    return res
+
+
 def kernel_leg(ks=(2, 4, 5, 16, 64), reps=7, iters=20):
     """The attention kernels alone at the decode-core shape: ms per call, median (min-max) of `reps` alternated
     rounds of `iters` launches."""
@@ -209,11 +285,18 @@ def main():
     ap.add_argument("--profile", action="store_true", help="trace the steps instead of timing them")
     ap.add_argument("--step-tokens", default=None, help="e.g. 1,4,8,16,64: time k-token replays (extend + rewind)")
     ap.add_argument("--kernel-leg", action="store_true", help="time the attention kernels at the decode-core shape")
+    ap.add_argument("--spec-rows", default=None, help="e.g. 4,8: a batched speculative loop of k-token drafts, "
+                                                     "per-row rewind against the smallest-count rewind and refeed")
+    ap.add_argument("--accept", type=float, default=0.7, help="--spec-rows: acceptance probability of a draft token")
+    ap.add_argument("--reps", type=int, default=5, help="--spec-rows: blocks of --steps rounds")
     a = ap.parse_args()
     assert torch.cuda.is_available(), "graph_decode_bench measures on a GPU"
     res = {"card": card()}
     if a.kernel_leg:
         res["kernel_leg"] = kernel_leg()
+    elif a.spec_rows:
+        res["spec_rows"] = [run_spec(int(b), int(k), a.steps, a.reps, a.accept) for b in a.batches.split(",")
+                            for k in a.spec_rows.split(",")]
     elif a.step_tokens:
         ks = [int(k) for k in a.step_tokens.split(",")]
         res["tokens_profile" if a.profile else "tokens"] = [run_tokens(int(b), ks, a.steps, a.profile)
