@@ -640,6 +640,51 @@ PCV_API int pcv_rotary_apply_at_fp8(const pcv_rotary_params* p, const pcv_rotary
                                     void* stream);
 
 /*
+ * Token sampling: pcv_sample draws one token per row of R logits rows of V entries, with temperature, top-k and top-p
+ * filtering in the semantics of the Hugging Face TemperatureLogitsWarper -> TopKLogitsWarper -> TopPLogitsWarper, then
+ * softmax + multinomial.  Row r belongs to batch row b = r / rows_per_batch.
+ *   x_i = float(logit_i) / temperature (a true fp32 division); temperature == 0 is greedy: the argmax, the lowest index
+ *   on ties, log-probability 0, nothing random drawn.
+ *   top_k > 0: keep every token with x_i >= the k-th largest x (all ties with it); 0 or >= V: off.
+ *   top_p < 1: with masses w_i = round(2^40 exp(x_i - max x)) (uint64) of the kept tokens, Z their sum and
+ *   W<=(v) the mass of the kept tokens with x <= v, token i is removed iff W<=(x_i) <= floor((1 - top_p) Z) (fp64
+ *   product); a tie group straddling the cut is kept whole, and the top group always stays.  1: off.
+ *   The token is the first index, in vocabulary order, whose kept prefix mass exceeds hi64(u * Z_kept), with u the 64
+ *   bits pcv_sample_uniforms exports for (seeds[b], b, positions[r]).
+ * A row's token is a pure function of its logit bits, the three filter values, seeds[b], b and positions[r]:
+ * independent of R, of the other rows, of the launch and of graph capture.  Seeds and positions are read from device
+ * memory when the kernel runs, so one recorded CUDA graph serves every seed and position.  Logits must be free of NaN
+ * and +inf.  Refusals (NULL pointers, V outside [1, PCV_SAMPLE_MAX_VOCAB], stride_row < V, R not a multiple of
+ * rows_per_batch, temperature < 0 or NaN, top_k < 0, top_p outside (0, 1] or NaN, an unknown dtype) come before any
+ * CUDA call, with the reason in pcv_last_error.
+ */
+#define PCV_SAMPLE_MAX_VOCAB 32768
+
+typedef struct pcv_sample_params {
+  const void* logits;        /* (R, V) rows of `dtype` (PCV_BF16 / PCV_F16 / PCV_F32), unit element stride */
+  int64_t stride_row;        /* elements between rows, >= V                                                */
+  int32_t R, V;
+  int32_t dtype;
+  int32_t rows_per_batch;    /* R / rows_per_batch batch rows                                              */
+  const uint64_t* seeds;     /* device, one per batch row                                                  */
+  const int32_t* positions;  /* device, one per row: the counter of the row's draw                          */
+  float temperature;         /* >= 0; 0: greedy                                                            */
+  int32_t top_k;             /* >= 0; 0: off                                                               */
+  float top_p;               /* (0, 1]; 1: off                                                             */
+  int32_t reserved;
+  int64_t* tokens;           /* device (R) out: token ids                                                  */
+  float* logprobs;           /* device (R) out or NULL: the token's log-probability under the filtered distribution */
+} pcv_sample_params;
+
+/* 1 if pcv_sample takes these params, else 0 (reason via pcv_last_error) */
+PCV_API int pcv_sample_supported(const pcv_sample_params* p);
+PCV_API int pcv_sample(const pcv_sample_params* p, void* stream);
+/* out[r] (device, R) = the 64 random bits of row r's draw: (seeds[r / rows_per_batch], r / rows_per_batch,
+ * positions[r]).  Arguments are checked before any CUDA call. */
+PCV_API int pcv_sample_uniforms(uint64_t* out, const uint64_t* seeds, const int32_t* positions, int32_t R,
+                                int32_t rows_per_batch, void* stream);
+
+/*
  * Backward of the LayerNorm -> Linear chain pcv_kv_project computes (training through kv_norm -> k_proj / v_proj,
  * q_norm -> q_proj, norm -> q/k/v_proj).  With x_hat = (x - mean) * rstd (row_stats of pcv_ln_stats),
  * y = x_hat * gamma + beta, out = y W^T + b, W = [W_k ; W_v] (n_k + n_v, C) and G = [grad_k | grad_v] (rows, n):

@@ -82,6 +82,9 @@ EXPORTS = (
     "pcv_kv_append_at_fp8",
     "pcv_rotary_apply_at",
     "pcv_rotary_apply_at_fp8",
+    "pcv_sample_supported",
+    "pcv_sample",
+    "pcv_sample_uniforms",
     "pcv_ln_linear_bwd_supported",
     "pcv_ln_linear_bwd_workspace_bytes",
     "pcv_ln_linear_bwd",
@@ -272,6 +275,19 @@ class DevRows(C.Structure):
     _fields_ = [("bounds", C.c_void_p), ("capacity", C.c_int32), ("bounds_stride_b", C.c_int32)]
 
 
+SAMPLE_MAX_VOCAB = 32768   # PCV_SAMPLE_MAX_VOCAB
+
+
+class SampleParams(C.Structure):
+    _fields_ = [
+        ("logits", C.c_void_p), ("stride_row", C.c_int64),
+        ("R", C.c_int32), ("V", C.c_int32), ("dtype", C.c_int32), ("rows_per_batch", C.c_int32),
+        ("seeds", C.c_void_p), ("positions", C.c_void_p),
+        ("temperature", C.c_float), ("top_k", C.c_int32), ("top_p", C.c_float), ("reserved", C.c_int32),
+        ("tokens", C.c_void_p), ("logprobs", C.c_void_p),
+    ]
+
+
 class LnLinearBwdParams(C.Structure):
     _fields_ = [
         ("x", C.c_void_p), ("x_stride_row", C.c_int64), ("row_stats", C.c_void_p),
@@ -428,6 +444,11 @@ def lib() -> C.CDLL:
                      "pcv_attn_cached_window_supported", "pcv_attn_cached_window_workspace_bytes",
                      "pcv_attn_cached_window", "pcv_attn_cached_window_fp8_supported",
                      "pcv_attn_cached_window_fp8_workspace_bytes", "pcv_attn_cached_window_fp8"):
+            getattr(l, name).restype = C.c_int
+        l.pcv_sample_supported.argtypes = [C.POINTER(SampleParams)]
+        l.pcv_sample.argtypes = [C.POINTER(SampleParams), C.c_void_p]
+        l.pcv_sample_uniforms.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
+        for name in ("pcv_sample_supported", "pcv_sample", "pcv_sample_uniforms"):
             getattr(l, name).restype = C.c_int
         l.pcv_ln_linear_bwd_supported.argtypes = [C.POINTER(LnLinearBwdParams)]
         l.pcv_ln_linear_bwd_supported.restype = C.c_int

@@ -375,6 +375,19 @@ int pcv_attn_dropout_mask_range(uint8_t* keep, int32_t B, int32_t H, int32_t N, 
                              reinterpret_cast<cudaStream_t>(stream));
 }
 
+int pcv_sample_supported(const pcv_sample_params* p) { return sample_check(p) == PCV_OK ? 1 : 0; }
+
+int pcv_sample(const pcv_sample_params* p, void* stream) {
+  const int rc = sample_check(p);
+  if (rc != PCV_OK) return rc;
+  return launch_sample(*p, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pcv_sample_uniforms(uint64_t* out, const uint64_t* seeds, const int32_t* positions, int32_t R,
+                        int32_t rows_per_batch, void* stream) {
+  return launch_sample_uniforms(out, seeds, positions, R, rows_per_batch, reinterpret_cast<cudaStream_t>(stream));
+}
+
 static int partial_dropout_check(const pcv_attn_params* p, float dropout_p, bool shard) {
   if (validate_attn(p) != PCV_OK) return 0;
   const char* why = "";

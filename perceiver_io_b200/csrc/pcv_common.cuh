@@ -174,5 +174,10 @@ int launch_attn_fwd_dropout(const pcv_attn_params& p, const float* stat_m, const
                             uint64_t seed, cudaStream_t stream);
 int launch_dropout_mask(uint8_t* keep, int B, int H, int N, int key_begin, int key_end, float dropout_p, uint64_t seed,
                         cudaStream_t stream);
+// token sampling (pcv_sample.cu)
+int sample_check(const pcv_sample_params* p);
+int launch_sample(const pcv_sample_params& p, cudaStream_t stream);
+int launch_sample_uniforms(uint64_t* out, const uint64_t* seeds, const int32_t* positions, int R, int rows_per_batch,
+                           cudaStream_t stream);
 
 }  // namespace pcv

@@ -18,19 +18,17 @@
 #include <cmath>
 #include <cstdint>
 
+#include "pcv_hash.cuh"
+
 namespace pcv {
 
 __device__ __forceinline__ uint32_t drop_qword(uint32_t bh, uint32_t q) { return bh * 0x9E3779B1u + (q >> 1); }
 __device__ __forceinline__ uint32_t drop_qside(uint32_t seed_lo, uint32_t qword) { return qword * 0x9E3779B1u ^ seed_lo; }
 __device__ __forceinline__ uint32_t drop_kside(uint32_t seed_hi, uint32_t k) { return (k >> 1) * 0x85EBCA6Bu ^ seed_hi; }
-__device__ __forceinline__ uint32_t drop_round(uint32_t x, uint32_t c, uint32_t k) {
-  const uint64_t pr = (uint64_t)x * c;
-  return (uint32_t)(pr >> 32) ^ (uint32_t)pr ^ k;
-}
 __device__ __forceinline__ uint32_t drop_finish(uint32_t qside, uint32_t kside) {
   uint32_t x = qside ^ kside;
-  x = drop_round(x, 0xD2511F53u, 0x9E3779B9u);
-  return drop_round(x, 0xCD9E8D57u, 0xBB67AE85u);
+  x = hash_round(x, 0xD2511F53u, 0x9E3779B9u);
+  return hash_round(x, 0xCD9E8D57u, 0xBB67AE85u);
 }
 __device__ __forceinline__ uint32_t drop_bits(uint32_t seed_lo, uint32_t seed_hi, uint32_t bh, uint32_t q, uint32_t k) {
   return drop_finish(drop_qside(seed_lo, drop_qword(bh, q)), drop_kside(seed_hi, k));

@@ -1,0 +1,373 @@
+// pcv_sample.cu — token sampling on the device (pcv_sample, pcv_sample_uniforms): one token per logits row under
+// temperature, top-k and top-p, with 🤗's TemperatureLogitsWarper -> TopKLogitsWarper -> TopPLogitsWarper semantics and
+// inverse-CDF sampling.  oracle/sample_oracle.py restates every step in numpy.
+//
+// One CTA of 512 threads per row ρ (batch row b = ρ / rows_per_batch); the row's fp32 x is staged in shared memory.
+//   1. x_i = float(logit_i) / temperature, a true fp32 division.  temperature == 0: the argmax of the logits, the lowest
+//      index on ties (torch.argmax); nothing random is drawn and the log-probability written is 0.
+//   2. top-k: keep every token with x_i >= the k-th largest x (tokens tied with it stay).  A radix select over
+//      order-preserving uint32 keys (-0 folded onto +0), four passes of 256-bin count histograms.
+//   3. masses: w_i = round(2^40 · exp(x_i - max x)) in uint64 fixed point (exp in fp64, round half to even), Z = Σ w_i
+//      over the kept tokens; V <= 32768 keeps Z below 2^56.  Every sum from here on is an integer sum.
+//   4. top-p: with W≤(v) = Σ_{kept, x_j <= v} w_j and cut = floor((1 - (double)top_p) · (double)Z) (fp64 ops), token i
+//      is removed iff W≤(x_i) <= cut — 🤗's `cumulative_probs <= 1 - top_p` applied to whole tie groups (a group that
+//      straddles the cut stays whole).  The top tie group always stays.  A radix select over the same keys with
+//      mass-weighted uint64 histograms.
+//   5. draw: 64 bits u = sample_bits(seeds[b], b, positions[ρ]), t = hi64(u · Z_kept); the token is the first index, in
+//      vocabulary order, whose kept prefix mass exceeds t (softmax + multinomial on the filtered scores, drawn in index
+//      order).  The log-probability written is log(w_token) - log(Z_kept) in fp64, rounded to fp32.
+// No floating-point atomics anywhere: the histograms are integer atomics, the scans are fixed-order warp shuffles.
+//
+// Determinism: a row's token is a pure function of the row's logit bits, temperature, top_k, top_p, its seed, b and its
+// position.  It does not depend on R, on the other rows, on the launch or on graph capture; two launches are
+// bit-identical.  The logits must be free of NaN and +inf.
+#include "pcv_common.cuh"
+#include "pcv_hash.cuh"
+
+namespace pcv {
+
+namespace sm90 {
+int set_smem_limit(const void* kernel, int smem);  // pcv_sm90_host.cu
+}
+
+namespace {
+
+constexpr int kThreads = 512;
+constexpr int kWarps = kThreads / 32;
+constexpr double kMassScale = 1099511627776.0;  // 2^40
+using u64 = unsigned long long;
+
+// The 64 random bits of (seed, b, position): two evaluations of three hash_round rounds with distinct keys, the two
+// multipliers in swapped order so the halves' rounds collide independently.  The seed's low word enters before the first
+// round and its high word before the second, so seeds that differ in either word (adjacent seeds included) pass through
+// at least two rounds.
+__device__ __forceinline__ uint32_t sample_half(uint32_t word, uint32_t seed_lo, uint32_t seed_hi, uint32_t ca,
+                                                uint32_t cb, uint32_t k0, uint32_t k1, uint32_t k2) {
+  uint32_t x = hash_round(word ^ seed_lo, ca, k0);
+  x = hash_round(x ^ seed_hi, cb, k1);
+  return hash_round(x, ca, k2);
+}
+
+__device__ __forceinline__ u64 sample_bits(u64 seed, uint32_t b, uint32_t pos) {
+  const uint32_t word = (b * 0x9E3779B1u + pos) * 0x85EBCA6Bu;
+  const uint32_t lo = (uint32_t)seed, hi = (uint32_t)(seed >> 32);
+  const uint32_t h0 = sample_half(word, lo, hi, 0xD2511F53u, 0xCD9E8D57u, 0x3C6EF372u, 0xA54FF53Au, 0x510E527Fu);
+  const uint32_t h1 = sample_half(word, lo, hi, 0xCD9E8D57u, 0xD2511F53u, 0x9B05688Cu, 0x1F83D9ABu, 0x5BE0CD19u);
+  return ((u64)h1 << 32) | h0;
+}
+
+// order-preserving key of a float: a < b <=> key(a) < key(b); -0 and +0 share a key
+__device__ __forceinline__ uint32_t order_key(float x) {
+  uint32_t u = __float_as_uint(x);
+  if (u == 0x80000000u) u = 0u;
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float key_value(uint32_t k) {
+  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+
+// w = round(2^40 exp(x - m)); 0 below x - m = -29, where 2^40 exp(x - m) < 0.28
+__device__ __forceinline__ u64 token_mass(float x, float m) {
+  const double d = (double)x - (double)m;  // exact: both are floats within 2^6 of each other where it matters
+  return d < -29.0 ? 0ull : __double2ull_rn(exp(d) * kMassScale);
+}
+
+__device__ __forceinline__ u64 warp_sum_u64(u64 v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+__device__ __forceinline__ u64 warp_max_u64(u64 v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = max(v, (u64)__shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+
+// every thread gets the block's maximum
+__device__ __forceinline__ u64 block_max_u64(u64 v, u64* red) {
+  v = warp_max_u64(v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  v = red[threadIdx.x & (kWarps - 1)];
+  v = warp_max_u64(v);
+  __syncthreads();
+  return v;
+}
+
+// hist[bin] += 1 for every lane with bin < 256: one shared atomic per distinct bin of the warp.  Called by all 32 lanes.
+__device__ __forceinline__ void hist_count(uint32_t* hist, uint32_t bin) {
+  if (!__ballot_sync(0xffffffffu, bin < 256u)) return;
+  const unsigned group = __match_any_sync(0xffffffffu, bin);
+  if (bin < 256u && (threadIdx.x & 31) == (unsigned)(__ffs(group) - 1)) atomicAdd(hist + bin, (uint32_t)__popc(group));
+}
+
+// hist[bin] += v for every lane with bin < 256; lanes with one bin are summed in registers first, so a warp issues one
+// shared atomic per distinct bin.  Called by all 32 lanes.
+__device__ __forceinline__ void hist_mass(u64* hist, uint32_t bin, u64 v) {
+  if (!__ballot_sync(0xffffffffu, bin < 256u)) return;
+  const unsigned group = __match_any_sync(0xffffffffu, bin);
+  u64 sum = 0;
+  if (group == 0xffffffffu) {
+    sum = warp_sum_u64(v);
+  } else {
+#pragma unroll 1
+    for (int j = 0; j < 32; ++j) {
+      const u64 o = __shfl_sync(0xffffffffu, v, j);
+      if ((group >> j) & 1u) sum += o;
+    }
+  }
+  if (bin < 256u && (threadIdx.x & 31) == (unsigned)(__ffs(group) - 1)) atomicAdd(hist + bin, sum);
+}
+
+template <typename T>
+__device__ __forceinline__ float load_f(const T* p) {
+  return Elem<T>::to_f(*p);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads) sample_kernel(const pcv_sample_params p) {
+  extern __shared__ __align__(16) float xs[];   // the row's x (V floats)
+  __shared__ u64 mhist[256];       // top-p masses
+  __shared__ uint32_t chist[256];  // top-k counts
+  __shared__ u64 red[kWarps];
+  __shared__ u64 sel[2];           // radix state: [0] key prefix, [1] count still needed / mass below
+  const int V = p.V, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int64_t row = blockIdx.x;
+  const T* src = static_cast<const T*>(p.logits) + row * p.stride_row;
+  const bool greedy = p.temperature == 0.f;
+
+  u64 best = 0;
+  for (int i = tid; i < V; i += kThreads) {
+    float x = load_f(src + i);
+    if (!greedy) x = x / p.temperature;
+    xs[i] = x;
+    best = max(best, ((u64)order_key(x) << 32) | (uint32_t)~(uint32_t)i);
+  }
+  best = block_max_u64(best, red);   // the largest key, and of its ties the lowest index
+  if (greedy) {
+    if (tid == 0) {
+      p.tokens[row] = (int64_t)(uint32_t)~(uint32_t)best;
+      if (p.logprobs) p.logprobs[row] = 0.f;
+    }
+    return;
+  }
+  const uint32_t top = (uint32_t)(best >> 32);
+  const float m = key_value(top);
+
+  // ---- top-k: the k-th largest key, kept iff key >= lo ----
+  uint32_t lo = 0;
+  if (p.top_k > 0 && p.top_k < V) {
+    if (tid == 0) sel[0] = 0, sel[1] = (u64)p.top_k;
+    for (int shift = 24; shift >= 0; shift -= 8) {
+      for (int i = tid; i < 256; i += kThreads) chist[i] = 0;
+      __syncthreads();
+      const uint32_t prefix = (uint32_t)sel[0], hi_mask = shift == 24 ? 0u : ~0u << (shift + 8);
+      for (int base = 0; base < V; base += kThreads) {
+        const int i = base + tid;
+        uint32_t bin = 256u;
+        if (i < V) {
+          const uint32_t k = order_key(xs[i]);
+          if ((k & hi_mask) == prefix) bin = (k >> shift) & 255u;
+        }
+        hist_count(chist, bin);
+      }
+      __syncthreads();
+      if (warp == 0) {   // lane l owns bins 8l .. 8l+7; find d with above(d) < need <= above(d) + h[d], from the top
+        uint32_t h[8], own = 0;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) h[j] = chist[8 * lane + j], own += h[j];
+        uint32_t incl = own;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+          const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
+          if (lane >= o) incl += t;
+        }
+        uint32_t above = __shfl_sync(0xffffffffu, incl, 31) - incl;   // the counts of the lanes above this one
+        const uint32_t need = (uint32_t)sel[1];
+#pragma unroll
+        for (int j = 7; j >= 0; --j) {
+          if (above < need && above + h[j] >= need) {
+            sel[0] = prefix | ((uint32_t)(8 * lane + j) << shift);
+            sel[1] = need - above;
+          }
+          above += h[j];
+        }
+      }
+      __syncthreads();
+    }
+    lo = (uint32_t)sel[0];
+    __syncthreads();   // every thread has read sel before top-p reuses it
+  }
+
+  // ---- top-p: the least kept key whose W≤ exceeds the cut ----
+  if (p.top_p < 1.f) {
+    if (tid == 0) sel[0] = 0, sel[1] = 0;
+    bool done = false;
+    for (int shift = 24; shift >= 0 && !done; shift -= 8) {
+      for (int i = tid; i < 256; i += kThreads) mhist[i] = 0;
+      __syncthreads();
+      const uint32_t prefix = (uint32_t)sel[0], hi_mask = shift == 24 ? 0u : ~0u << (shift + 8);
+      const u64 below0 = sel[1];
+      for (int base = 0; base < V; base += kThreads) {
+        const int i = base + tid;
+        uint32_t bin = 256u;
+        u64 w = 0;
+        if (i < V) {
+          const float x = xs[i];
+          const uint32_t k = order_key(x);
+          if (k >= lo && (k & hi_mask) == prefix) {
+            w = token_mass(x, m);
+            if (w) bin = (k >> shift) & 255u;
+          }
+        }
+        hist_mass(mhist, bin, w);
+      }
+      __syncthreads();
+      if (warp == 0) {   // lane l owns bins 8l .. 8l+7; the first bin, ascending, whose cumulative mass exceeds the cut
+        u64 h[8], own = 0;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) h[j] = mhist[8 * lane + j], own += h[j];
+        u64 incl = own;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+          const u64 t = __shfl_up_sync(0xffffffffu, incl, o);
+          if (lane >= o) incl += t;
+        }
+        __shared__ u64 cut_s;
+        if (shift == 24) {   // the first pass sees every kept token: Z and the cut
+          const u64 Z = __shfl_sync(0xffffffffu, incl, 31);
+          const double c = floor((1.0 - (double)p.top_p) * (double)Z);
+          if (lane == 0) cut_s = (u64)c;
+          __syncwarp();
+          if (cut_s >= Z) {   // nothing would stay: the top tie group does
+            if (lane == 0) sel[0] = top, sel[1] = ~0ull;
+          }
+        }
+        __syncwarp();
+        if (sel[1] != ~0ull) {
+          const u64 cut = cut_s;
+          u64 below = below0 + incl - own;
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            if (below <= cut && below + h[j] > cut) {
+              sel[0] = prefix | ((uint32_t)(8 * lane + j) << shift);
+              sel[1] = below;
+            }
+            below += h[j];
+          }
+        }
+      }
+      __syncthreads();
+      done = sel[1] == ~0ull;
+    }
+    lo = max(lo, (uint32_t)sel[0]);
+  }
+
+  // ---- draw: warp w owns a contiguous segment of the vocabulary ----
+  const int seg = ((V + kWarps * 32 - 1) / (kWarps * 32)) * 32;
+  const int s0 = warp * seg, s1 = min(V, s0 + seg);
+  u64 part = 0;
+  for (int i = s0 + lane; i < s1; i += 32) {
+    const float x = xs[i];
+    if (order_key(x) >= lo) part += token_mass(x, m);
+  }
+  part = warp_sum_u64(part);
+  __syncthreads();   // red[] was last read by block_max_u64
+  if (lane == 0) red[warp] = part;
+  __syncthreads();
+  u64 before = 0, Zk = 0;
+#pragma unroll
+  for (int w = 0; w < kWarps; ++w) {
+    const u64 v = red[w];
+    before += w < warp ? v : 0ull;
+    Zk += v;
+  }
+  const int64_t b = row / p.rows_per_batch;
+  const u64 bits = sample_bits(p.seeds[b], (uint32_t)b, (uint32_t)p.positions[row]);
+  const u64 t = __umul64hi(bits, Zk);
+  if (t < before || t >= before + part) return;   // exactly one warp holds the draw (its part is > 0)
+  u64 acc = before;
+  for (int base = s0; base < s1; base += 32) {
+    const int i = base + lane;
+    u64 w = 0;
+    if (i < s1) {
+      const float x = xs[i];
+      if (order_key(x) >= lo) w = token_mass(x, m);
+    }
+    u64 incl = w;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const u64 v = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += v;
+    }
+    const unsigned hit = __ballot_sync(0xffffffffu, acc + incl > t);
+    if (hit) {
+      if (lane == __ffs(hit) - 1) {
+        p.tokens[row] = i;
+        if (p.logprobs) p.logprobs[row] = (float)(log((double)w) - log((double)Zk));
+      }
+      return;
+    }
+    acc += __shfl_sync(0xffffffffu, incl, 31);
+  }
+}
+
+__global__ void sample_uniforms_kernel(uint64_t* out, const uint64_t* seeds, const int32_t* positions, int R, int rpb) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= R) return;
+  const int b = r / rpb;
+  out[r] = sample_bits(seeds[b], (uint32_t)b, (uint32_t)positions[r]);
+}
+
+}  // namespace
+
+int sample_check(const pcv_sample_params* p) {
+  PCV_REQUIRE(p != nullptr, PCV_ERR_INVALID, "sample: params is NULL");
+  PCV_REQUIRE(p->logits && p->seeds && p->positions && p->tokens, PCV_ERR_INVALID,
+              "sample: logits / seeds / positions / tokens pointer is NULL");
+  PCV_REQUIRE(p->dtype == PCV_BF16 || p->dtype == PCV_F16 || p->dtype == PCV_F32, PCV_ERR_INVALID,
+              "sample: unknown dtype %d (bf16, fp16 or fp32 logits)", p->dtype);
+  PCV_REQUIRE(p->V >= 1 && p->V <= PCV_SAMPLE_MAX_VOCAB, PCV_ERR_UNSUPPORTED, "sample: V=%d must be in [1, %d]", p->V,
+              PCV_SAMPLE_MAX_VOCAB);
+  PCV_REQUIRE(p->R >= 1, PCV_ERR_INVALID, "sample: R=%d must be >= 1", p->R);
+  PCV_REQUIRE(p->stride_row >= p->V, PCV_ERR_INVALID, "sample: stride_row=%lld is below V=%d",
+              (long long)p->stride_row, p->V);
+  PCV_REQUIRE(p->rows_per_batch >= 1 && p->R % p->rows_per_batch == 0, PCV_ERR_INVALID,
+              "sample: R=%d is not a multiple of rows_per_batch=%d", p->R, p->rows_per_batch);
+  PCV_REQUIRE(p->temperature >= 0.f, PCV_ERR_INVALID, "sample: temperature must be >= 0 (0: greedy), got %g",
+              (double)p->temperature);
+  PCV_REQUIRE(p->top_k >= 0, PCV_ERR_INVALID, "sample: top_k must be >= 0 (0: off), got %d", p->top_k);
+  PCV_REQUIRE(p->top_p > 0.f && p->top_p <= 1.f, PCV_ERR_INVALID, "sample: top_p must be in (0, 1] (1: off), got %g",
+              (double)p->top_p);
+  return PCV_OK;
+}
+
+int launch_sample(const pcv_sample_params& p, cudaStream_t stream) {
+  const int smem = p.V * (int)sizeof(float);
+  const void* kern = p.dtype == PCV_BF16  ? reinterpret_cast<const void*>(&sample_kernel<__nv_bfloat16>)
+                     : p.dtype == PCV_F16 ? reinterpret_cast<const void*>(&sample_kernel<__half>)
+                                          : reinterpret_cast<const void*>(&sample_kernel<float>);
+  if (smem > 48 * 1024) {   // once per kernel and device, for the largest row
+    const int rc = sm90::set_smem_limit(kern, PCV_SAMPLE_MAX_VOCAB * (int)sizeof(float));
+    if (rc != PCV_OK) return rc;
+  }
+  if (p.dtype == PCV_BF16) sample_kernel<__nv_bfloat16><<<p.R, kThreads, smem, stream>>>(p);
+  else if (p.dtype == PCV_F16) sample_kernel<__half><<<p.R, kThreads, smem, stream>>>(p);
+  else sample_kernel<float><<<p.R, kThreads, smem, stream>>>(p);
+  PCV_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return PCV_OK;
+}
+
+int launch_sample_uniforms(uint64_t* out, const uint64_t* seeds, const int32_t* positions, int R, int rows_per_batch,
+                           cudaStream_t stream) {
+  PCV_REQUIRE(out && seeds && positions, PCV_ERR_INVALID, "sample_uniforms: out / seeds / positions pointer is NULL");
+  PCV_REQUIRE(R >= 1 && rows_per_batch >= 1 && R % rows_per_batch == 0, PCV_ERR_INVALID,
+              "sample_uniforms: R=%d must be >= 1 and a multiple of rows_per_batch=%d", R, rows_per_batch);
+  sample_uniforms_kernel<<<(R + 255) / 256, 256, 0, stream>>>(out, seeds, positions, R, rows_per_batch);
+  PCV_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return PCV_OK;
+}
+
+}  // namespace pcv

@@ -15,6 +15,10 @@ run, and in-graph int32 ops advance them at the end of each step.
     dec.rewind(n)                                                             # drop the last n fed tokens
     dec.rewind(counts)                                                        # drop the last counts[b] of row b
     dec.reorder(beam_idx)                                                     # beam search (eager)
+    dec.set_seed(seed); dec.set_sampling(temperature=1.0, top_k=10, top_p=1.0)  # sampling on the device
+    first = dec.draw(logits)                                                  # (B, 1): prefill's logits, eager
+    tokens = dec.generate(first, n)                                           # (B, n): n replays, no host sync
+    tokens, logits = dec.sample(token_ids)                                    # (B, k) drafts -> (B, k) draws
 
 Rows: cross-attention arena row r holds token r of the sequence (prompt and generated tokens); self-attention arena
 row r holds token ``prefix_len + r`` (prefix_len of the prompt).  The windows follow the 🤗 wrapper's truncation, as
@@ -33,11 +37,24 @@ Budget: ``max_new_tokens`` counts per batch row.  The arenas hold room for the r
 ``extend(k)`` is refused exactly when that row has fewer than k tokens left, and a per-row ``rewind`` gives back what
 that row regains.  The counts are host integers; nothing is read back from the device.
 
+Sampling: ``sample`` and ``generate`` replay graphs that also run the device sampler (``ops.sample_tokens``:
+temperature, top-k and top-p with the 🤗 warpers' semantics) on the graph's own logits, so a generated token costs one
+replay and nothing else.  The sampling values are host values recorded into the graphs (one set of graphs per
+``set_sampling`` triple, recorded on first use); the seeds (``set_seed``, one per batch row) and the positions live on
+the device.  Counter rule: the token that will be fed at cross-attention arena row p of batch row b is drawn with the
+counter (seed_b, b, p).  A replay that feeds k tokens at rows r .. r+k-1 draws at positions r+1 .. r+k, computed in the
+graph from the row counters, so after a ``rewind`` the same positions draw the same bits again: a rewound sequence that
+is fed the same tokens resamples identically.  ``sample(drafts)`` returns the token drawn after each draft, so
+speculative acceptance is ``drafts[:, i+1] == tokens[:, i]`` on the device: the accepted tokens are draws from the
+model's own filtered distribution.
+
 Not covered: steps of more than 64 tokens, a different k per batch row, contrastive search, a ring buffer bounded at
-``max_seq_len`` (the arenas grow by ``max_new_tokens`` rows) and wiring into 🤗 ``generate()``.
+``max_seq_len`` (the arenas grow by ``max_new_tokens`` rows), EOS handling (callers truncate after EOS), per-row
+sampling values, repetition penalties and wiring into 🤗 ``generate()``.
 """
 from __future__ import annotations
 
+import math
 import operator
 from collections.abc import Sequence
 from typing import List, NamedTuple
@@ -122,6 +139,13 @@ def advance_bounds_(bounds: torch.Tensor, inc: torch.Tensor, wmax: torch.Tensor,
     return bounds
 
 
+def sample_positions(bounds: torch.Tensor, steps: torch.Tensor, k: int) -> torch.Tensor:
+    """(B, k) int32 counters of the draws of a k-token replay from the one-token state ``bounds`` (B, groups, 6) before
+    the replay: the tokens fed at cross-attention rows r .. r+k-1 (r = ``bounds[b, 0, 2]``) are followed by draws at
+    positions r+1 .. r+k.  ``steps`` is ``arange(1, 65)`` int32 on ``bounds``' device.  Tensors alone, no host read."""
+    return bounds[:, 0, 2:3] + steps[:k]
+
+
 def _as_count(x):
     """x as an int when it is integer-like (operator.index) and not a bool, else None."""
     if isinstance(x, bool):
@@ -145,6 +169,7 @@ class GraphedDecoder:
     # per-row counts: None while every batch row has fed the same tokens, else _lag[b] = the tokens row b has fed fewer
     # than the furthest row (whose count is _fed)
     _lag = None
+    _seeds = None   # (B,) int64 sampler seeds, set in __init__
 
     def __init__(self, model, batch: int, max_new_tokens: int, kv_cache: str = "bf16"):
         if max_new_tokens < 1:
@@ -180,7 +205,11 @@ class GraphedDecoder:
         self.device = w.device
         self.dtype = w.dtype
         self.captures = 0
-        self._graphs = {}      # tokens per step -> GraphedForward
+        self._graphs = {}      # tokens per step, or ("sample", tokens per step, sampling values) -> GraphedForward
+        self._seeds = torch.zeros(batch, dtype=torch.int64, device=w.device)
+        self._seeded = False
+        self._sampling = (1.0, 0, 1.0)
+        self._steps = torch.arange(1, ops.WINDOW_MAX_ROWS + 1, dtype=torch.int32, device=w.device)
         self._bounds = None
         self._remaining = 0
         self._fed = 0          # tokens fed since prefill (what rewind may drop)
@@ -301,14 +330,25 @@ class GraphedDecoder:
         advance_bounds_(self._bounds, self._inc, self._wmax, k)
         return logits[:, -1] if k == 1 else logits
 
+    def _sample_fn(self, token: torch.Tensor):
+        """_step_fn followed by the sampler on its logits: (tokens (B, k), logits (B, k, vocab))."""
+        k = token.shape[1]
+        pos = sample_positions(self._bounds, self._steps, k)   # before _step_fn advances the rows
+        logits = self._step_fn(token)
+        if k == 1:
+            logits = logits[:, None]
+        t, top_k, top_p = self._sampling
+        return ops.sample_tokens(logits, self._seeds, pos, t, top_k, top_p), logits
+
     def _replay(self, token_ids: torch.Tensor, fn: str) -> torch.Tensor:
-        """One replay of the graph of ``token_ids.shape[1]`` tokens per step, recorded on first use."""
+        """One replay of the graph of ``token_ids.shape[1]`` tokens per step, recorded on first use (``fn`` "sample":
+        the graph that also samples, one per sampling triple)."""
         k = token_ids.shape[1] if token_ids.dim() == 2 else 0
-        kmax = 1 if fn == "step" else ops.WINDOW_MAX_ROWS
+        kmax = 1 if fn in ("step", "generate") else ops.WINDOW_MAX_ROWS
         if self._bounds is None:
             raise RuntimeError("GraphedDecoder: call prefill() first")
         if tuple(token_ids.shape) != (self.batch, k) or token_ids.dtype != torch.long or not 1 <= k <= kmax:
-            want = "1)" if fn == "step" else f"k) with 1 <= k <= {ops.WINDOW_MAX_ROWS}"
+            want = "1)" if kmax == 1 else f"k) with 1 <= k <= {ops.WINDOW_MAX_ROWS}"
             raise ValueError(f"GraphedDecoder.{fn} takes ({self.batch}, {want} int64 tokens, got "
                              f"{tuple(token_ids.shape)} {token_ids.dtype}")
         if self._remaining < k:
@@ -317,17 +357,19 @@ class GraphedDecoder:
                                f"prefill() again")
         if torch.is_autocast_enabled():
             raise RuntimeError("GraphedDecoder does not run under autocast")
-        graph = self._graphs.get(k)
+        sample = fn in ("sample", "generate")
+        key = ("sample", k, self._sampling) if sample else k
+        graph = self._graphs.get(key)
         if graph is None:
             snapshot = self._bounds.clone()   # the warm-up calls advance the rows; their arena writes are rewritten later
             old = torch.cuda.get_sync_debug_mode()
             torch.cuda.set_sync_debug_mode(0)  # recording a graph synchronises the device once
             try:
-                graph = GraphedForward(self._step_fn, token_ids)
+                graph = GraphedForward(self._sample_fn if sample else self._step_fn, token_ids)
             finally:
                 torch.cuda.set_sync_debug_mode(old)
             self._bounds.copy_(snapshot)
-            self._graphs[k] = graph
+            self._graphs[key] = graph
             self.captures += 1
         out = graph(token_ids)
         self._remaining -= k
@@ -347,6 +389,94 @@ class GraphedDecoder:
         if token_ids.dim() == 2 and token_ids.shape[1] == 1:
             return self._replay(token_ids, "extend")[:, None]
         return self._replay(token_ids, "extend")
+
+    # ---- sampling ------------------------------------------------------------------------------------------------
+    def set_seed(self, seed) -> None:
+        """Load the per-batch-row seeds of the sampler: one integer for every row, or B integers (each in [0, 2^64)).
+        An eager copy into the graphs' seed buffer: no re-capture.  Without a call, the first sampling call draws one
+        seed from torch's CPU generator (``ops.new_dropout_seed``)."""
+        seeds = [seed] * self.batch if _as_count(seed) is not None else seed
+        if isinstance(seeds, torch.Tensor):
+            seeds = seeds.tolist() if not seeds.is_cuda and seeds.dim() == 1 else None
+        if not isinstance(seeds, Sequence) or isinstance(seeds, (str, bytes)) or len(seeds) != self.batch:
+            raise ValueError(f"GraphedDecoder.set_seed: one integer or {self.batch} integers (one per batch row), got "
+                             f"{seed!r}")
+        vals = []
+        for b, s in enumerate(seeds):
+            v = _as_count(s)
+            if v is None or not 0 <= v < 2 ** 64:
+                raise ValueError(f"GraphedDecoder.set_seed: the seed of batch row {b} must be an integer in [0, 2^64), "
+                                 f"got {s!r}")
+            vals.append(v - 2 ** 64 if v >= 2 ** 63 else v)   # the uint64 bit pattern in an int64
+        host = torch.tensor(vals, dtype=torch.int64)
+        if self._seeds.is_cuda:   # pinned and asynchronous: no synchronisation
+            host = host.pin_memory()
+        self._seeds.copy_(host, non_blocking=True)
+        self._seeded = True
+
+    def set_sampling(self, temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0) -> None:
+        """The sampler's values for ``draw``, ``sample`` and ``generate``: ``temperature`` >= 0 (0: greedy), ``top_k`` >= 0
+        (0: off), ``top_p`` in (0, 1] (1: off), as ``ops.sample_tokens`` takes them.  The first replay under a new triple
+        records its graphs."""
+        t, p, k = float(temperature), float(top_p), _as_count(top_k)
+        if not t >= 0.0 or math.isinf(t):
+            raise ValueError(f"GraphedDecoder.set_sampling: temperature must be finite and >= 0 (0: greedy), got "
+                             f"{temperature!r}")
+        if k is None or k < 0:
+            raise ValueError(f"GraphedDecoder.set_sampling: top_k must be an integer >= 0 (0: off), got {top_k!r}")
+        if not 0.0 < p <= 1.0:
+            raise ValueError(f"GraphedDecoder.set_sampling: top_p must be in (0, 1] (1: off), got {top_p!r}")
+        self._sampling = (t, min(k, 2 ** 31 - 1), p)
+
+    def _ready_to_sample(self, what: str) -> None:
+        if self._bounds is None:
+            raise RuntimeError("GraphedDecoder: call prefill() first")
+        vocab = self.model.config.vocab_size
+        if vocab > ops.SAMPLE_MAX_VOCAB:
+            raise RuntimeError(f"GraphedDecoder.{what}: the device sampler takes vocabularies up to "
+                               f"{ops.SAMPLE_MAX_VOCAB}, this model has {vocab}")
+        if not self._seeded:
+            self.set_seed(ops.new_dropout_seed())
+
+    def draw(self, logits: torch.Tensor) -> torch.Tensor:
+        """(B, 1) int64 tokens drawn, eagerly, from ``logits`` (B, vocab) — typically ``prefill``'s — at each batch row's
+        next position (the row its next fed token takes)."""
+        self._ready_to_sample("draw")
+        if logits.dim() != 2 or logits.shape[0] != self.batch:
+            raise ValueError(f"GraphedDecoder.draw takes ({self.batch}, vocab) logits, got {tuple(logits.shape)}")
+        t, top_k, top_p = self._sampling
+        pos = sample_positions(self._bounds, self._steps, 1) - 1
+        return ops.sample_tokens(logits[:, None], self._seeds, pos, t, top_k, top_p)
+
+    def sample(self, token_ids: torch.Tensor):
+        """Feed the k tokens ``token_ids`` (B, k) int64, 1 <= k <= 64, in one replay and return ``(tokens, logits)``:
+        ``tokens[:, i]`` (B, k) int64 is drawn on the device from ``logits[:, i]`` (B, k, vocab), the logits after token
+        i, at the position of the row it would be fed at.  Consumes k tokens of the budget.  Views of the graph's static
+        outputs, valid until the next replay."""
+        self._ready_to_sample("sample")
+        return self._replay(token_ids, "sample")
+
+    def generate(self, first_tokens: torch.Tensor, n: int) -> torch.Tensor:
+        """Feed ``first_tokens`` (B, 1) int64 and then every drawn token, for n replays of the one-token sampling graph;
+        return the n drawn tokens (B, n) int64.  Each replay's input is copied on the device from the previous one's
+        output: no host read and no synchronisation.  Consumes n tokens of the budget; asking for more than remain is
+        refused before any replay, leaving the state untouched."""
+        self._ready_to_sample("generate")
+        count = _as_count(n)
+        if count is None or count < 1:
+            raise ValueError(f"GraphedDecoder.generate: n must be an integer >= 1, got {n!r}")
+        if self._remaining < count:
+            raise RuntimeError(f"GraphedDecoder.generate: {self._remaining} of max_new_tokens={self.max_new_tokens} "
+                               f"tokens remain to the furthest batch row, {count} asked for")
+        if tuple(first_tokens.shape) != (self.batch, 1) or first_tokens.dtype != torch.long:
+            raise ValueError(f"GraphedDecoder.generate takes ({self.batch}, 1) int64 first tokens, got "
+                             f"{tuple(first_tokens.shape)} {first_tokens.dtype}")
+        out = torch.empty(self.batch, count, dtype=torch.long, device=self.device)
+        tokens = first_tokens
+        for i in range(count):
+            tokens, _ = self._replay(tokens, "generate")
+            out[:, i:i + 1].copy_(tokens)
+        return out
 
     def rewind(self, n) -> None:
         """Drop fed tokens: the next token of a batch row is fed at the row of its first dropped one, as if the dropped
@@ -420,5 +550,7 @@ class GraphedDecoder:
                     t.copy_(t.index_select(0, idx))
         self._pad.copy_(self._pad.index_select(0, idx))
         self._bounds.copy_(self._bounds.index_select(0, idx))
+        if self._seeds is not None:
+            self._seeds.copy_(self._seeds.index_select(0, idx))
         if self._lag is not None:
             self._set_fed([self._fed - self._lag[i] for i in beam_idx.tolist()])

@@ -30,6 +30,7 @@ __all__ = [
     "kv_project_fp8_supported", "ln_linear", "ln_linear_backward", "kv_append_fp8", "attention_decode_fp8",
     "attention_decode_fp8_supported", "fp8_pair_descale", "fp8_dequantize", "rotated_cache_shadow", "rotary_at", "rotary_fp8",
     "attention_decode_window", "kv_append_at", "rotary_apply_at", "rotary_angle_table", "attention_window",
+    "sample_tokens", "sample_uniforms",
 ]
 
 
@@ -1299,6 +1300,78 @@ def rotary_apply_at(x: torch.Tensor, num_heads: int, table: torch.Tensor, rows: 
     f = _lib.RotaryFp8(x_descale=None, y_inv_scale=y_inv_scale.data_ptr()) if fp8 else None
     with torch.cuda.device(x.device):
         _launch_rotary(p, f, _dev_rows(rows, table.shape[0], x.shape[0], 2, "rotary_apply_at"))
+    return out
+
+
+# --------------------------------------------------------------------------------------------------
+# token sampling (pcv_sample): temperature, top-k and top-p with the 🤗 warpers' semantics, drawn on the device from a
+# counter-based stream keyed by (seed of the batch row, batch row, position), so it can be recorded in a CUDA graph.
+# --------------------------------------------------------------------------------------------------
+#: The largest vocabulary :func:`sample_tokens` takes.
+SAMPLE_MAX_VOCAB = _lib.SAMPLE_MAX_VOCAB
+
+
+def _sample_counters(seeds: torch.Tensor, positions: torch.Tensor, lead: tuple, what: str):
+    _require_cuda(seeds, positions)
+    if seeds.dtype != torch.int64 or tuple(seeds.shape) != lead[:1]:
+        raise ValueError(f"{what}: seeds must be a ({lead[0]},) int64 CUDA tensor (one per batch row), got "
+                         f"{tuple(seeds.shape)} {seeds.dtype}")
+    if positions.dtype != torch.int32 or tuple(positions.shape) != lead:
+        raise ValueError(f"{what}: positions must be a {lead} int32 CUDA tensor (one per logits row), got "
+                         f"{tuple(positions.shape)} {positions.dtype}")
+    return seeds.contiguous(), positions.contiguous()
+
+
+def sample_tokens(logits: torch.Tensor, seeds: torch.Tensor, positions: torch.Tensor, temperature: float = 1.0,
+                  top_k: int = 0, top_p: float = 1.0, logprobs: bool = False):
+    """One token per logits row, drawn on the device (pcv_sample): ``logits / temperature``, then top-k, then top-p, then
+    softmax + multinomial — the semantics of 🤗's ``TemperatureLogitsWarper`` -> ``TopKLogitsWarper`` ->
+    ``TopPLogitsWarper``, except that a tie group straddling the top-p cut is kept whole.  ``temperature=0`` is greedy
+    (the first maximal index); ``top_k=0`` and ``top_p=1`` turn those filters off.  The three values are taken in fp32.
+
+    logits: (B, V) or (B, k, V) bf16 / fp16 / fp32, V <= :data:`SAMPLE_MAX_VOCAB`; seeds: (B,) int64 CUDA, one per batch
+    row; positions: (B,) or (B, k) int32 CUDA, the counter of every row's draw.  A row's token is a pure function of
+    its logits, the three values, its seed, its batch row and its position (nothing is read back to the host, so the
+    call can be recorded in a CUDA graph).  Returns int64 tokens of the logits' leading shape and, with ``logprobs``,
+    their fp32 log-probabilities under the filtered distribution (0 when greedy).  Arguments the kernel does not take
+    raise ``ValueError`` with its reason before any launch."""
+    _require_cuda(logits)
+    if logits.dim() not in (2, 3) or logits.dtype not in (torch.bfloat16, torch.float16, torch.float32):
+        raise ValueError(f"sample_tokens: logits must be (B, V) or (B, k, V) bf16 / fp16 / fp32, got "
+                         f"{tuple(logits.shape)} {logits.dtype}")
+    lead = tuple(logits.shape[:-1])
+    seeds, positions = _sample_counters(seeds, positions, lead, "sample_tokens")
+    V = logits.shape[-1]
+    rows = (logits if logits.stride(-1) == 1 else logits.contiguous()).reshape(-1, V)
+    tokens = torch.empty(lead, dtype=torch.int64, device=logits.device)
+    lp = torch.empty(lead, dtype=torch.float32, device=logits.device) if logprobs else None
+    p = _lib.SampleParams()
+    p.logits, p.stride_row, p.R, p.V = rows.data_ptr(), rows.stride(0), rows.shape[0], V
+    p.dtype = _lib.PCV_F32 if logits.dtype == torch.float32 else _pcv_dtype(logits.dtype)
+    p.rows_per_batch = 1 if logits.dim() == 2 else logits.shape[1]
+    p.seeds, p.positions = seeds.data_ptr(), positions.data_ptr()
+    p.temperature, p.top_p = float(temperature), float(top_p)
+    p.top_k = min(int(top_k), 2 ** 31 - 1)
+    p.tokens, p.logprobs = tokens.data_ptr(), (lp.data_ptr() if lp is not None else None)
+    lib = _lib.lib()
+    if not lib.pcv_sample_supported(C.byref(p)):
+        raise ValueError(f"sample_tokens: {lib.pcv_last_error().decode()}")
+    with torch.cuda.device(logits.device):
+        check(lib.pcv_sample(C.byref(p), _stream()), "pcv_sample")
+    return (tokens, lp) if logprobs else tokens
+
+
+def sample_uniforms(seeds: torch.Tensor, positions: torch.Tensor) -> torch.Tensor:
+    """The 64 random bits (as int64) of the draw of every row of :func:`sample_tokens` with these seeds (B,) and
+    positions (B,) or (B, k) — pcv_sample_uniforms."""
+    lead = tuple(positions.shape)
+    if len(lead) not in (1, 2):
+        raise ValueError(f"sample_uniforms: positions must be (B,) or (B, k), got {lead}")
+    seeds, positions = _sample_counters(seeds, positions, lead, "sample_uniforms")
+    out = torch.empty(lead, dtype=torch.int64, device=positions.device)
+    with torch.cuda.device(positions.device):
+        check(_lib.lib().pcv_sample_uniforms(out.data_ptr(), seeds.data_ptr(), positions.data_ptr(), positions.numel(),
+                                             1 if len(lead) == 1 else lead[1], _stream()), "pcv_sample_uniforms")
     return out
 
 

@@ -23,7 +23,15 @@ loop without per-row rewinds: it rewinds every row to the smallest accepted coun
 lead its next replay again (in place of drafts).  A token counts as accepted once it is kept by its row for good.  It
 reports ms per accepted token (replay and rewind, CUDA events and a synchronise around each round; over all rows) and
 replays per accepted token of one row, median (min-max) over --reps blocks of --steps rounds; every block starts from
-the prompt (a per-row rewind of everything fed)."""
+the prompt (a per-row rewind of everything fed).
+
+--sample measures sampling.  Model leg: at each batch, bf16 and FP8 arenas, and the sampling values top_k=10 /
+top_p=0.5 / greedy, two arms alternate token by token: "eager" is GraphedDecoder.step followed by the eager 🤗-equivalent
+warper chain (divide, topk + masked_fill, sort + softmax + cumsum + scatter, softmax + multinomial; argmax when greedy),
+what a caller writes without the device sampler; "generate" is one GraphedDecoder.generate replay.  Each token is timed
+with CUDA events around the call and a synchronise (host work included); ms per token, median (min-max).  Kernel leg:
+ops.sample_tokens against the eager chain alone at V = 389 and 32000 and R = 1, 16 and 1024 rows, alternated, CUDA
+events around 50 launches."""
 import argparse
 import json
 import os
@@ -277,6 +285,105 @@ def kernel_leg(ks=(2, 4, 5, 16, 64), reps=7, iters=20):
     return out
 
 
+SAMPLE_CONFIGS = {"top_k=10": (1.0, 10, 1.0), "top_p=0.5": (1.0, 0, 0.5), "greedy": (0.0, 0, 1.0)}
+
+
+def eager_sample(logits, temperature, top_k, top_p):
+    """The 🤗 warper chain and multinomial in eager torch: (B, V) logits -> (B, 1) tokens."""
+    if temperature == 0:
+        return logits.argmax(-1, keepdim=True)
+    s = logits.float() / temperature
+    if top_k:
+        s = s.masked_fill(s < torch.topk(s, top_k)[0][..., -1:], float("-inf"))
+    if top_p < 1:
+        srt, idx = torch.sort(s, descending=False)
+        remove = srt.softmax(-1).cumsum(-1) <= 1 - top_p
+        remove[..., -1:] = False
+        s = s.masked_fill(remove.scatter(-1, idx, remove), float("-inf"))
+    return torch.multinomial(s.softmax(-1), 1)
+
+
+def run_sample(batch, steps):
+    """ms per token: step + the eager chain against one generate replay, per cache kind and sampling config."""
+    torch.manual_seed(0)
+    cfg = P.CausalSequenceModelConfig(**GIANTMIDI)
+    model = P.CausalSequenceModel(cfg).cuda().bfloat16().eval()
+    n, prefix = cfg.max_seq_len, cfg.max_seq_len - cfg.max_latents
+    warm = 3
+    tokens = torch.randint(0, cfg.vocab_size, (batch, n), device="cuda")
+    out = []
+    with torch.no_grad():
+        for kind in ("bf16", "fp8"):
+            decs = {}
+            for arm in ("eager", "generate"):
+                decs[arm] = P.GraphedDecoder(model, batch=batch, max_new_tokens=warm + steps, kv_cache=kind)
+                decs[arm].set_seed(1)
+            for name, vals in SAMPLE_CONFIGS.items():
+                state = {}
+                for arm, dec in decs.items():
+                    dec.set_sampling(*vals)
+                    state[arm] = {"tok": dec.draw(dec.prefill(tokens, prefix)), "times": []}
+
+                def one(arm):
+                    st, dec = state[arm], decs[arm]
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                    if arm == "eager":
+                        st["tok"] = eager_sample(dec.step(st["tok"]), *vals)
+                    else:
+                        st["tok"] = dec.generate(st["tok"], 1)
+                    e1.record()
+                    torch.cuda.synchronize()
+                    return e0.elapsed_time(e1)
+
+                for _ in range(warm):
+                    for arm in decs:
+                        one(arm)
+                for _ in range(steps):
+                    for arm in decs:
+                        state[arm]["times"].append(one(arm))
+                res = {"batch": batch, "cache": kind, "sampling": name,
+                       "eager_ms_per_token": stats(state["eager"]["times"]),
+                       "generate_ms_per_token": stats(state["generate"]["times"])}
+                res["speedup"] = round(statistics.median(state["eager"]["times"])
+                                       / statistics.median(state["generate"]["times"]), 3)
+                out.append(res)
+    del decs, model
+    torch.cuda.empty_cache()
+    return out
+
+
+def sample_kernel_leg(reps=7, iters=50):
+    """ms per call of ops.sample_tokens and of the eager chain, median (min-max) over reps blocks of iters calls."""
+    from perceiver_io_b200 import ops
+
+    out = []
+    for V in (389, 32000):
+        for R in (1, 16, 1024):
+            logits = torch.randn(R, V, device="cuda").bfloat16() * 3
+            seeds = torch.arange(R, device="cuda")
+            pos = torch.zeros(R, dtype=torch.int32, device="cuda")
+            for name, vals in SAMPLE_CONFIGS.items():
+                arms = {"kernel": lambda: ops.sample_tokens(logits, seeds, pos, *vals),
+                        "eager": lambda: eager_sample(logits, *vals)}
+                times = {a: [] for a in arms}
+                for a, f in arms.items():
+                    f()
+                torch.cuda.synchronize()
+                for _ in range(reps):
+                    for a, f in arms.items():
+                        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                        e0.record()
+                        for _ in range(iters):
+                            f()
+                        e1.record()
+                        torch.cuda.synchronize()
+                        times[a].append(e0.elapsed_time(e1) / iters)
+                out.append({"V": V, "R": R, "sampling": name, "kernel_ms": stats(times["kernel"]),
+                            "eager_ms": stats(times["eager"])})
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=30)
@@ -289,10 +396,15 @@ def main():
                                                      "per-row rewind against the smallest-count rewind and refeed")
     ap.add_argument("--accept", type=float, default=0.7, help="--spec-rows: acceptance probability of a draft token")
     ap.add_argument("--reps", type=int, default=5, help="--spec-rows: blocks of --steps rounds")
+    ap.add_argument("--sample", action="store_true", help="step + the eager warper chain against generate, and the "
+                                                          "sampler kernel against the eager chain")
     a = ap.parse_args()
     assert torch.cuda.is_available(), "graph_decode_bench measures on a GPU"
     res = {"card": card()}
-    if a.kernel_leg:
+    if a.sample:
+        res["sample_kernel"] = sample_kernel_leg()
+        res["sample"] = [r for b in a.batches.split(",") for r in run_sample(int(b), a.steps)]
+    elif a.kernel_leg:
         res["kernel_leg"] = kernel_leg()
     elif a.spec_rows:
         res["spec_rows"] = [run_spec(int(b), int(k), a.steps, a.reps, a.accept) for b in a.batches.split(",")
