@@ -501,32 +501,40 @@ int pcv_attn_decode_fp8(const pcv_attn_params* p, const pcv_decode_fp8* f, void*
   return decode_launch(p, f, nullptr, true, false, stream);
 }
 
-// The tensor-core attention of 1 to 64 query rows on an e4m3 cache (pcv_attn_cached.cu).
-static int cached_check(const pcv_attn_params* p, const pcv_decode_fp8* f) {
-  PCV_REQUIRE(f != nullptr, PCV_ERR_INVALID, "attn_cached_fp8: fp8 params are NULL");
+// The tensor-core attention of 1 to 64 query rows (pcv_attn_cached.cu) on a whole e4m3 cache or, for the window
+// entries (window), on a device-resident window of an arena; the e4m3 entries (fp8) refuse a NULL f.
+static int cached_check(const pcv_attn_params* p, const pcv_decode_fp8* f, const pcv_dev_rows* rows, int32_t band,
+                        bool fp8, bool window) {
+  const char* name = !window ? "attn_cached_fp8" : (fp8 ? "attn_cached_window_fp8" : "attn_cached_window");
+  PCV_REQUIRE(!fp8 || f != nullptr, PCV_ERR_INVALID, "%s: fp8 params are NULL", name);
+  PCV_REQUIRE(!window || rows != nullptr, PCV_ERR_INVALID, "%s: rows is NULL", name);
   int rc = validate_attn(p);
   if (rc != PCV_OK) return rc;
   const char* why = "";
-  PCV_REQUIRE(attn_cached_fp8_supported(*p, *f, &why), PCV_ERR_UNSUPPORTED,
-              "cached e4m3 attention not applicable: %s", why);
+  PCV_REQUIRE(attn_cached_supported(*p, f, rows, band, &why), PCV_ERR_UNSUPPORTED, "%s not applicable: %s",
+              window ? name : "cached e4m3 attention", why);
   return PCV_OK;
 }
 
+static int cached_workspace(const pcv_attn_params* p, size_t* bytes, const char* name) {
+  int rc = validate_attn(p);
+  if (rc != PCV_OK) return rc;
+  PCV_REQUIRE(bytes != nullptr, PCV_ERR_INVALID, "%s: bytes is NULL", name);
+  return attn_cached_workspace_bytes(*p, bytes);
+}
+
 int pcv_attn_cached_fp8_supported(const pcv_attn_params* p, const pcv_decode_fp8* f) {
-  return cached_check(p, f) == PCV_OK ? 1 : 0;
+  return cached_check(p, f, nullptr, 0, true, false) == PCV_OK ? 1 : 0;
 }
 
 int pcv_attn_cached_fp8_workspace_bytes(const pcv_attn_params* p, size_t* bytes) {
-  int rc = validate_attn(p);
-  if (rc != PCV_OK) return rc;
-  PCV_REQUIRE(bytes != nullptr, PCV_ERR_INVALID, "attn_cached_fp8: bytes is NULL");
-  return attn_cached_fp8_workspace_bytes(*p, bytes);
+  return cached_workspace(p, bytes, "attn_cached_fp8");
 }
 
 int pcv_attn_cached_fp8(const pcv_attn_params* p, const pcv_decode_fp8* f, void* stream) {
-  const int rc = cached_check(p, f);
+  const int rc = cached_check(p, f, nullptr, 0, true, false);
   if (rc != PCV_OK) return rc;
-  return launch_attn_cached_fp8(*p, *f, reinterpret_cast<cudaStream_t>(stream));
+  return launch_attn_cached(*p, f, nullptr, 0, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int pcv_kv_append_fp8_supported(const pcv_kv_append_params* p, const pcv_kv_fp8_scales* f) {
@@ -585,56 +593,34 @@ int pcv_attn_decode_window_fp8(const pcv_attn_params* p, const pcv_decode_fp8* f
   return decode_launch(p, f, rows, true, true, stream);
 }
 
-// The tensor-core attention of 1 to 64 query rows on a device-resident window of an arena (pcv_attn_window.cu); the
-// e4m3 entry (fp8) refuses a NULL f.
-static int window_check(const pcv_attn_params* p, const pcv_decode_fp8* f, const pcv_dev_rows* rows, int32_t band,
-                        bool fp8) {
-  const char* name = fp8 ? "attn_cached_window_fp8" : "attn_cached_window";
-  PCV_REQUIRE(!fp8 || f != nullptr, PCV_ERR_INVALID, "%s: fp8 params are NULL", name);
-  PCV_REQUIRE(rows != nullptr, PCV_ERR_INVALID, "%s: rows is NULL", name);
-  int rc = validate_attn(p);
-  if (rc != PCV_OK) return rc;
-  const char* why = "";
-  PCV_REQUIRE(attn_window_supported(*p, fp8 ? f : nullptr, *rows, band, &why), PCV_ERR_UNSUPPORTED,
-              "%s not applicable: %s", name, why);
-  return PCV_OK;
-}
-
 int pcv_attn_cached_window_supported(const pcv_attn_params* p, const pcv_dev_rows* rows, int32_t band) {
-  return window_check(p, nullptr, rows, band, false) == PCV_OK ? 1 : 0;
+  return cached_check(p, nullptr, rows, band, false, true) == PCV_OK ? 1 : 0;
 }
 
 int pcv_attn_cached_window_fp8_supported(const pcv_attn_params* p, const pcv_decode_fp8* f, const pcv_dev_rows* rows,
                                          int32_t band) {
-  return window_check(p, f, rows, band, true) == PCV_OK ? 1 : 0;
-}
-
-static int window_workspace(const pcv_attn_params* p, size_t* bytes, const char* name) {
-  int rc = validate_attn(p);
-  if (rc != PCV_OK) return rc;
-  PCV_REQUIRE(bytes != nullptr, PCV_ERR_INVALID, "%s: bytes is NULL", name);
-  return attn_window_workspace_bytes(*p, bytes);
+  return cached_check(p, f, rows, band, true, true) == PCV_OK ? 1 : 0;
 }
 
 int pcv_attn_cached_window_workspace_bytes(const pcv_attn_params* p, size_t* bytes) {
-  return window_workspace(p, bytes, "attn_cached_window");
+  return cached_workspace(p, bytes, "attn_cached_window");
 }
 
 int pcv_attn_cached_window_fp8_workspace_bytes(const pcv_attn_params* p, size_t* bytes) {
-  return window_workspace(p, bytes, "attn_cached_window_fp8");
+  return cached_workspace(p, bytes, "attn_cached_window_fp8");
 }
 
 int pcv_attn_cached_window(const pcv_attn_params* p, const pcv_dev_rows* rows, int32_t band, void* stream) {
-  const int rc = window_check(p, nullptr, rows, band, false);
+  const int rc = cached_check(p, nullptr, rows, band, false, true);
   if (rc != PCV_OK) return rc;
-  return launch_attn_window(*p, nullptr, *rows, band, reinterpret_cast<cudaStream_t>(stream));
+  return launch_attn_cached(*p, nullptr, rows, band, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int pcv_attn_cached_window_fp8(const pcv_attn_params* p, const pcv_decode_fp8* f, const pcv_dev_rows* rows,
                                int32_t band, void* stream) {
-  const int rc = window_check(p, f, rows, band, true);
+  const int rc = cached_check(p, f, rows, band, true, true);
   if (rc != PCV_OK) return rc;
-  return launch_attn_window(*p, f, *rows, band, reinterpret_cast<cudaStream_t>(stream));
+  return launch_attn_cached(*p, f, rows, band, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int pcv_kv_append_at(const pcv_kv_append_params* p, const pcv_dev_rows* rows, void* stream) {

@@ -129,16 +129,13 @@ int debug_pair_workers(int32_t* workers, int32_t* clusters_fit);  // the current
 bool attn_decode_supported(const pcv_attn_params& p, const pcv_decode_fp8* f, const pcv_dev_rows* rows, const char** why);
 int launch_attn_decode(const pcv_attn_params& p, const pcv_decode_fp8* f, const pcv_dev_rows* rows, cudaStream_t stream);
 int attn_decode_workspace_bytes(const pcv_attn_params& p, size_t* bytes);
-// the tensor-core attention of 1 to 64 query rows over e4m3 K / V rows (pcv_attn_cached_fp8, pcv_attn_cached.cu)
-bool attn_cached_fp8_supported(const pcv_attn_params& p, const pcv_decode_fp8& f, const char** why);
-int attn_cached_fp8_workspace_bytes(const pcv_attn_params& p, size_t* bytes);
-int launch_attn_cached_fp8(const pcv_attn_params& p, const pcv_decode_fp8& f, cudaStream_t stream);
-// the tensor-core attention of 1 to 64 query rows over a device-resident window of a bf16 / fp16 or e4m3 (f) arena,
-// with a causal band (pcv_attn_cached_window (_fp8), pcv_attn_window.cu)
-bool attn_window_supported(const pcv_attn_params& p, const pcv_decode_fp8* f, const pcv_dev_rows& rows, int band,
+// the tensor-core attention of 1 to 64 query rows (pcv_attn_cached.cu): rows == nullptr for the whole e4m3 cache
+// (pcv_attn_cached_fp8; f required, band 0), else the window read from device memory of a bf16 / fp16 or e4m3 (f)
+// arena with a causal band (pcv_attn_cached_window (_fp8), M = the arena's capacity)
+bool attn_cached_supported(const pcv_attn_params& p, const pcv_decode_fp8* f, const pcv_dev_rows* rows, int band,
                            const char** why);
-int attn_window_workspace_bytes(const pcv_attn_params& p, size_t* bytes);
-int launch_attn_window(const pcv_attn_params& p, const pcv_decode_fp8* f, const pcv_dev_rows& rows, int band,
+int attn_cached_workspace_bytes(const pcv_attn_params& p, size_t* bytes);
+int launch_attn_cached(const pcv_attn_params& p, const pcv_decode_fp8* f, const pcv_dev_rows* rows, int band,
                        cudaStream_t stream);
 
 int launch_combine(const pcv_combine_params& p, cudaStream_t stream);

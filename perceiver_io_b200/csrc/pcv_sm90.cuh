@@ -74,8 +74,8 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
 //   41-43  peer_tail_kernel   41 partial states of all ranks, 42 grid arrival, 43 outputs of all ranks (flag waits)
 //   51-52  lnlin_dx_kernel    51 ring slot free, 52 stage loaded
 //   53-54  lnlin_dw_kernel    53 ring slot free, 54 stage loaded
-//   61-62  attn_cached_fp8_kernel  61 converted stage free, 62 converted K / V tile ready
-//   63-64  attn_window_kernel      63 stage free, 64 K / V tile ready
+//   61-64  attn_cached_kernel  whole cache: 61 converted stage free, 62 converted K / V tile ready; window: 63 stage
+//                              free, 64 K / V tile ready
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity, uint32_t site = 0) {
   uint32_t spins = 0;
   uint64_t t0 = 0;

@@ -2,7 +2,7 @@
 (perceiver_io_b200/csrc/pcv_attn_cached.cu, pcv_attn_cached_fp8), shared by its GPU tests (test_gpu_cached_fp8.py) and
 their CPU companion (test_cached_fp8_cpu.py).  Nothing here needs a GPU.
 
-launch_attn_cached_fp8 instantiates attn_cached_fp8_kernel<BF16, NVB>:
+launch_attn_cached without device rows instantiates attn_cached_kernel<BF16, FP8 = true, WIN = false, NVB>:
   - BF16: bf16 or fp16 (the dtype of q and out, and of the converted K / V tiles);
   - NVB: the 64-channel boxes of a V row, ceil(dv / 64), 1 to 4.
 The Q / K box count ceil(dqk / 64) is a runtime value (the number of Q K^T k-steps and the stage size).
@@ -96,7 +96,7 @@ def variant_of(dt, dv):
 
 
 def reachable_variants():
-    """Every instantiation launch_attn_cached_fp8 can reach: head dims 16..256 in multiples of 16, both dtypes."""
+    """Every whole-cache instantiation launch_attn_cached can reach: head dims 16..256 in multiples of 16, both dtypes."""
     return {variant_of(dt, dv) for dt, dv in itertools.product(DTYPES, range(16, 257, 16))}
 
 
@@ -151,7 +151,7 @@ def _rn(x, dtype):
 
 
 def emulate(q, k8, v8, kd, vd, H, scale, pad, causal, dt, sms=SMS):
-    """The output of attn_cached_fp8_kernel restated in torch: fp32 scores from exact codes and the 16-bit q, the row
+    """The output of the whole-cache attn_cached_kernel restated in torch: fp32 scores from exact codes and the 16-bit q, the row
     maximum of round(s c), p = 2^(s c - m) with one rounding (fp64 then fp32), the fp32 running sums per 64-key tile,
     P rounded to the 16-bit type before P V, v_descale on the fp32 accumulator, the merge of the splits in split order
     and the rounding of o / l.  q (Bq, N, H*dqk) 16-bit, k8 / v8 (B, M, H*d) e4m3, kd (H,), vd (H, dv)."""

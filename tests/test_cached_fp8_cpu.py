@@ -1,10 +1,12 @@
-"""CPU checks of the tensor-core attention on an FP8 KV cache (pcv_attn_cached_fp8, csrc/pcv_attn_cached.cu): its entry
-points refuse what they do not cover before any CUDA call, the workspace and the split plan are the restated ones of
-cached_fp8_variants.py, the variant matrix of the GPU tests reaches every instantiation, the build of the kernel has no
-spills and no serialised wgmma, the host route picks the kernel by query rows, and the CPU emulation of the kernel's
-arithmetic stays within half of the element-wise gate of test_gpu_cached_fp8.py."""
+"""CPU checks of the tensor-core attention on an FP8 KV cache (pcv_attn_cached_fp8, the whole-cache instantiations of
+attn_cached_kernel in csrc/pcv_attn_cached.cu): its entry points refuse what they do not cover before any CUDA call, the
+workspace and the split plan are the restated ones of cached_fp8_variants.py, the variant matrix of the GPU tests reaches
+every instantiation, the build of the kernel has no spills and no serialised wgmma, the host route picks the kernel by
+query rows, and the CPU emulation of the kernel's arithmetic stays within half of the element-wise gate of
+test_gpu_cached_fp8.py."""
 import ctypes
 import os
+import re
 
 import pytest
 import torch
@@ -170,15 +172,27 @@ def test_variant_matrix_reaches_every_instantiation():
     assert {(96, 96), (128, 80)} <= {(d, v) for _, d, v in CV.VARIANT_CASES}
 
 
-def test_build_has_no_spills_and_no_serialised_wgmma():
+def cached_kernel_entries(win):
+    """The ptxas log entries of attn_cached_kernel<BF16, FP8, WIN, NVB> with the given WIN, and the log's text; None
+    when the library was not built in this tree."""
     log = os.path.join(ROOT, "build", "pcv_attn_cached.ptxas.log")
     if not os.path.exists(log):
-        pytest.skip("the library was not built in this tree")
+        return None, None
     text = open(log).read()
     entries = text.split("Compiling entry function")[1:]
-    kernels = [e for e in entries if "attn_cached_fp8_kernel" in e.split("\n")[0]]
+    args = [(re.search(r"attn_cached_kernelILb([01])ELb([01])ELb([01])ELi([1-4])E", e.split("\n")[0]), e)
+            for e in entries]
+    assert sum(m is not None for m, _ in args) == 24   # 8 whole-cache + 16 window instantiations, nothing else
+    return [e for m, e in args if m is not None and m.group(3) == str(int(win))], text
+
+
+def test_whole_cache_instantiations_have_no_spills_and_no_serialised_wgmma():
+    kernels, text = cached_kernel_entries(win=False)
+    if kernels is None:
+        pytest.skip("the library was not built in this tree")
     assert len(kernels) == 8, len(kernels)
     for e in kernels:
+        assert "ELb1ELb0ELi" in e.split("\n")[0]   # e4m3 rows only
         assert "0 bytes spill stores, 0 bytes spill loads" in e, e[:300]
     assert "C7515" not in text and "C7512" not in text
 

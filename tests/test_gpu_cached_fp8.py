@@ -1,5 +1,6 @@
-"""-m gpu: the tensor-core attention on an FP8 KV cache (attn_cached_fp8_kernel<BF16, NVB>, csrc/pcv_attn_cached.cu)
-at its row, tile, split and mask edges, and the cached steps of 5 to 64 new tokens that reach it through the model.
+"""-m gpu: the tensor-core attention on an FP8 KV cache (attn_cached_kernel<BF16, true, false, NVB>,
+csrc/pcv_attn_cached.cu) at its row, tile, split and mask edges, and the cached steps of 5 to 64 new tokens that reach
+it through the model.
 The matrix, the restated plan and the CPU emulation live in cached_fp8_variants.py (test_cached_fp8_cpu.py checks that
 the matrix covers every instantiation and that the emulated arithmetic stays within half of the gate used here).
 

@@ -1,11 +1,10 @@
-"""CPU checks of the banded-window tensor-core attention (pcv_attn_cached_window / _fp8, csrc/pcv_attn_window.cu) and of
-the k-token steps of GraphedDecoder: the entry points refuse what they do not cover before any CUDA call, the
-workspace and the split plan are the restated ones of window_variants.py, the variant matrix reaches every
-instantiation, the build has no spills and no serialised wgmma, the CPU emulation of the kernel's arithmetic stays within
-half of the element-wise gate of test_gpu_window.py, and the decoder's k-step bounds and positions give every fed token
-the window of the one-token loop through any sequence of extend and rewind."""
+"""CPU checks of the banded-window tensor-core attention (pcv_attn_cached_window / _fp8, the window instantiations of
+attn_cached_kernel in csrc/pcv_attn_cached.cu) and of the k-token steps of GraphedDecoder: the entry points refuse what
+they do not cover before any CUDA call, the workspace and the split plan are the restated ones of window_variants.py,
+the variant matrix reaches every instantiation, the build has no spills and no serialised wgmma, the CPU emulation of
+the kernel's arithmetic stays within half of the element-wise gate of test_gpu_window.py, and the decoder's k-step bounds
+and positions give every fed token the window of the one-token loop through any sequence of extend and rewind."""
 import ctypes
-import os
 import random
 
 import numpy as np
@@ -14,8 +13,8 @@ import torch
 
 import window_variants as WV
 from cached_fp8_variants import device_sms, left_pad
-from conftest import ROOT
 from perceiver_io_b200 import _lib
+from test_cached_fp8_cpu import cached_kernel_entries
 from test_graph_decode_cpu import _truncation_loop
 
 ENTRIES = ("pcv_attn_cached_window", "pcv_attn_cached_window_fp8")
@@ -187,18 +186,14 @@ def test_variant_matrix_reaches_every_instantiation():
     assert cover == reach, reach - cover
 
 
-def test_build_has_no_spills_and_no_serialised_wgmma():
-    log = os.path.join(ROOT, "build", "pcv_attn_window.ptxas.log")
-    if not os.path.exists(log):
+def test_window_instantiations_have_no_spills_and_no_serialised_wgmma():
+    kernels, text = cached_kernel_entries(win=True)
+    if kernels is None:
         pytest.skip("the library was not built in this tree")
-    text = open(log).read()
-    entries = text.split("Compiling entry function")[1:]
-    kernels = [e for e in entries if "attn_window_kernel" in e.split("\n")[0]]
     assert len(kernels) == 16, len(kernels)
     for e in kernels:
         assert "0 bytes spill stores, 0 bytes spill loads" in e, e[:300]
     assert "C7515" not in text and "C7512" not in text
-    assert not any("attn_cached_fp8_kernel" in e.split("\n")[0] for e in entries)
 
 
 def test_row_keys_restate_the_one_token_windows():

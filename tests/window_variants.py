@@ -1,12 +1,12 @@
 """Variant matrix, schedule rules, mask semantics and CPU emulation of the banded-window tensor-core attention over a KV
-arena (perceiver_io_b200/csrc/pcv_attn_window.cu, pcv_attn_cached_window / _fp8), shared by its GPU tests
+arena (perceiver_io_b200/csrc/pcv_attn_cached.cu, pcv_attn_cached_window / _fp8), shared by its GPU tests
 (test_gpu_window.py) and their CPU companion (test_window_cpu.py).  Nothing here needs a GPU.
 
-launch_attn_window instantiates attn_window_kernel<BF16, FP8, NVB>:
+launch_attn_cached with device rows instantiates attn_cached_kernel<BF16, FP8, WIN = true, NVB>:
   - BF16: bf16 or fp16 (the dtype of q and out, and of the K / V tiles in shared memory);
   - FP8: e4m3 arena rows (converted in shared memory) or rows of q's 16-bit type;
   - NVB: the 64-channel boxes of a V row, ceil(dv / 64), 1 to 4.
-Each rule below names the function of pcv_attn_window.cu it restates."""
+Each rule below names the function of pcv_attn_cached.cu it restates."""
 import itertools
 import math
 
@@ -20,7 +20,7 @@ KINDS = ("16bit", "e4m3")
 
 # ---- the restated rules ----
 def plan(B, H, capacity, dqk, dv, sms=SMS):
-    """plan_window: plan_cached of pcv_attn_cached.cu on M = capacity (the split count is fixed for the arena)."""
+    """plan_cached on M = capacity (the split count is fixed for the arena)."""
     return cached_plan(B, H, capacity, dqk, dv, sms)
 
 
@@ -30,8 +30,8 @@ def clamp_window(b0, b1, capacity):
 
 
 def split_tiles(b0, b1, capacity, nsplit):
-    """attn_window_kernel: the key range [kb, ke) of every split.  The window's 64-key tiles start at its begin; split s
-    takes tiles [min(T, s tps), min(T, s tps + tps)) with tps = ceil(T / nsplit), T = ceil(length / 64)."""
+    """attn_cached_kernel (WIN): the key range [kb, ke) of every split.  The window's 64-key tiles start at its begin;
+    split s takes tiles [min(T, s tps), min(T, s tps + tps)) with tps = ceil(T / nsplit), T = ceil(length / 64)."""
     w0, wend = clamp_window(b0, b1, capacity)
     T = -(-max(wend - w0, 0) // KEYS)
     tps = -(-T // nsplit)
@@ -77,7 +77,7 @@ def variant_of(dt, kind, dv):
 
 
 def reachable_variants():
-    """Every instantiation launch_attn_window can reach: head dims up to 256 in multiples of 8 (16-bit rows) or 16
+    """Every window instantiation launch_attn_cached can reach: head dims up to 256 in multiples of 8 (16-bit rows) or 16
     (e4m3 rows), both dtypes."""
     return {variant_of(dt, kind, dv) for dt, kind in itertools.product(DTYPES, KINDS)
             for dv in range(8 if kind == "16bit" else 16, 257, 8 if kind == "16bit" else 16)}
@@ -114,7 +114,7 @@ def masks(N, b0, b1, capacity, band, causal, pad):
 
 
 def emulate(q, k, v, kd, vd, H, scale, b0, b1, band, pad, causal, dt, sms=SMS):
-    """The output of attn_window_kernel restated in torch: fp32 scores of the 16-bit q and the exact K rows (e4m3 codes
+    """The output of the window attn_cached_kernel restated in torch: fp32 scores of the 16-bit q and the exact K rows (e4m3 codes
     when kd is given), the row maximum of round(s c) over the attended keys, p = 2^(s c - m) with one rounding, fp32
     running sums per 64-key tile from the window's begin, no rescale while a row has no key, P rounded to the 16-bit
     type before P V, v_descale on the fp32 accumulator, the merge in split order with empty splits at weight 0, and
