@@ -685,6 +685,63 @@ PCV_API int pcv_sample_uniforms(uint64_t* out, const uint64_t* seeds, const int3
                                 int32_t rows_per_batch, void* stream);
 
 /*
+ * Speculative sampling with a draft model's probabilities (Leviathan et al. 2023; Chen et al. 2023): pcv_spec_verify
+ * decides one round of G drafts for each of B batch rows.  Row b fed tokens t_0 .. t_G (tokens[b]) to both models; t_1
+ * .. t_G are the draft's draws.  Target row i (i = 0 .. G) holds the target's logits after t_i, draft row i (i < G) the
+ * logits the draft drew t_{i+1} from.  P_i / Zp_i are the kept masses of target row i and their sum under (temperature,
+ * top_k, top_p), exactly as pcv_sample computes them (greedy: 2^40 at the first maximal index, 0 elsewhere); Q_i / Zq_i
+ * those of draft row i under the draft_* values.  All arithmetic is exact integer arithmetic:
+ *   accept t_{i+1} = x iff hi64(u_a * Q_i(x) * Zp_i) < P_i(x) * Zq_i   (min(1, p/q) to 2^-64), with u_a the accept
+ *   stream's bits at (seeds[b], b, positions[b, i]).  A draft with Q_i(x) = 0 (one not drawn from Q) is accepted iff
+ *   P_i(x) > 0; a token outside [0, V) is rejected.
+ *   n_b = the first rejected i, or G.
+ *   n_b < G: the correction is the first index, in vocabulary order, whose prefix sum of
+ *   R(y) = max(0, P(y) Zq - Q(y) Zp) (row n_b) exceeds hi64(u_r * ΣR), u_r the residual stream's bits at
+ *   positions[b, n_b].  ΣR = 0 (reached only by a draft that neither P nor Q gives mass): a draw from P with u_r.
+ *   n_b = G: the bonus token, the first index whose prefix P_G mass exceeds hi64(u_r * Zp_G), u_r at positions[b, G].
+ *   out_tokens[b, :n_b] = t_1 .. t_{n_b}, out_tokens[b, n_b] = the correction or bonus token, the rest -1;
+ *   accepted[b] = n_b.
+ * The accept and residual streams are counter-based hashes independent of each other and of pcv_sample's draw stream
+ * at equal (seed, b, position), so the draft may share the target's seeds; pcv_spec_uniforms exports them.  A row's
+ * result is a pure function of its logit bits, both sets of filter values, its tokens, seeds[b], b and its positions:
+ * independent of B, of the launch and of graph capture.  Two kernels, no host read: one CTA per (b, i), then one thread
+ * per batch row resolves n_b in place in out_tokens, which is the only scratch.  Refusals (NULL pointers, V outside
+ * [1, PCV_SAMPLE_MAX_VOCAB], G outside [1, PCV_SPEC_MAX_DRAFTS], B < 1, a stride below V, draft_dtype != dtype, an
+ * unknown dtype, out_tokens overlapping tokens, either set of filter values out of range) come before any CUDA call,
+ * with the reason in pcv_last_error.
+ */
+#define PCV_SPEC_MAX_DRAFTS 63
+
+typedef struct pcv_spec_verify_params {
+  const void* target;          /* (B, G+1, V) target logits of `dtype`, unit element stride                       */
+  int64_t t_stride_b, t_stride_row;
+  const void* draft;           /* (B, G, V) draft logits of `draft_dtype` (== dtype), unit element stride           */
+  int64_t d_stride_b, d_stride_row;
+  const int64_t* tokens;       /* device (B, G+1) contiguous: the fed tokens t_0 .. t_G                             */
+  const uint64_t* seeds;       /* device (B)                                                                        */
+  const int32_t* positions;    /* device (B, G+1) contiguous: the counter of a token decided by target row i        */
+  int32_t B, G, V;
+  int32_t dtype, draft_dtype;  /* PCV_BF16 / PCV_F16 / PCV_F32                                                      */
+  int32_t reserved;
+  float temperature;           /* the target's filter values, as pcv_sample takes them                              */
+  int32_t top_k;
+  float top_p;
+  float draft_temperature;     /* the draft's                                                                       */
+  int32_t draft_top_k;
+  float draft_top_p;
+  int64_t* out_tokens;         /* device (B, G+1) out                                                               */
+  int32_t* accepted;           /* device (B) out: n_b                                                               */
+} pcv_spec_verify_params;
+
+/* 1 if pcv_spec_verify takes these params, else 0 (reason via pcv_last_error) */
+PCV_API int pcv_spec_verify_supported(const pcv_spec_verify_params* p);
+PCV_API int pcv_spec_verify(const pcv_spec_verify_params* p, void* stream);
+/* out[r] (device, R) = the 64 bits of stream stream_id (0: accept, 1: residual) at (seeds[r / rows_per_batch],
+ * r / rows_per_batch, positions[r]).  Arguments are checked before any CUDA call. */
+PCV_API int pcv_spec_uniforms(uint64_t* out, const uint64_t* seeds, const int32_t* positions, int32_t R,
+                              int32_t rows_per_batch, int32_t stream_id, void* stream);
+
+/*
  * Backward of the LayerNorm -> Linear chain pcv_kv_project computes (training through kv_norm -> k_proj / v_proj,
  * q_norm -> q_proj, norm -> q/k/v_proj).  With x_hat = (x - mean) * rstd (row_stats of pcv_ln_stats),
  * y = x_hat * gamma + beta, out = y W^T + b, W = [W_k ; W_v] (n_k + n_v, C) and G = [grad_k | grad_v] (rows, n):

@@ -32,6 +32,6 @@ from .modules import (  # noqa: F401
 )
 from .config import PerceiverARConfig, CausalSequenceModelConfig  # noqa: F401
 from .patch import patch  # noqa: F401
-from .generation import GraphedDecoder, decode_windows  # noqa: F401
+from .generation import GraphedDecoder, decode_windows, speculative_budget, speculative_generate  # noqa: F401
 
 __version__ = "0.1.0"

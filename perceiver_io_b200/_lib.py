@@ -85,6 +85,9 @@ EXPORTS = (
     "pcv_sample_supported",
     "pcv_sample",
     "pcv_sample_uniforms",
+    "pcv_spec_verify_supported",
+    "pcv_spec_verify",
+    "pcv_spec_uniforms",
     "pcv_ln_linear_bwd_supported",
     "pcv_ln_linear_bwd_workspace_bytes",
     "pcv_ln_linear_bwd",
@@ -288,6 +291,22 @@ class SampleParams(C.Structure):
     ]
 
 
+SPEC_MAX_DRAFTS = 63   # PCV_SPEC_MAX_DRAFTS
+
+
+class SpecVerifyParams(C.Structure):
+    _fields_ = [
+        ("target", C.c_void_p), ("t_stride_b", C.c_int64), ("t_stride_row", C.c_int64),
+        ("draft", C.c_void_p), ("d_stride_b", C.c_int64), ("d_stride_row", C.c_int64),
+        ("tokens", C.c_void_p), ("seeds", C.c_void_p), ("positions", C.c_void_p),
+        ("B", C.c_int32), ("G", C.c_int32), ("V", C.c_int32),
+        ("dtype", C.c_int32), ("draft_dtype", C.c_int32), ("reserved", C.c_int32),
+        ("temperature", C.c_float), ("top_k", C.c_int32), ("top_p", C.c_float),
+        ("draft_temperature", C.c_float), ("draft_top_k", C.c_int32), ("draft_top_p", C.c_float),
+        ("out_tokens", C.c_void_p), ("accepted", C.c_void_p),
+    ]
+
+
 class LnLinearBwdParams(C.Structure):
     _fields_ = [
         ("x", C.c_void_p), ("x_stride_row", C.c_int64), ("row_stats", C.c_void_p),
@@ -448,7 +467,11 @@ def lib() -> C.CDLL:
         l.pcv_sample_supported.argtypes = [C.POINTER(SampleParams)]
         l.pcv_sample.argtypes = [C.POINTER(SampleParams), C.c_void_p]
         l.pcv_sample_uniforms.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p]
-        for name in ("pcv_sample_supported", "pcv_sample", "pcv_sample_uniforms"):
+        l.pcv_spec_verify_supported.argtypes = [C.POINTER(SpecVerifyParams)]
+        l.pcv_spec_verify.argtypes = [C.POINTER(SpecVerifyParams), C.c_void_p]
+        l.pcv_spec_uniforms.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
+        for name in ("pcv_sample_supported", "pcv_sample", "pcv_sample_uniforms", "pcv_spec_verify_supported",
+                     "pcv_spec_verify", "pcv_spec_uniforms"):
             getattr(l, name).restype = C.c_int
         l.pcv_ln_linear_bwd_supported.argtypes = [C.POINTER(LnLinearBwdParams)]
         l.pcv_ln_linear_bwd_supported.restype = C.c_int

@@ -388,6 +388,20 @@ int pcv_sample_uniforms(uint64_t* out, const uint64_t* seeds, const int32_t* pos
   return launch_sample_uniforms(out, seeds, positions, R, rows_per_batch, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int pcv_spec_verify_supported(const pcv_spec_verify_params* p) { return spec_verify_check(p) == PCV_OK ? 1 : 0; }
+
+int pcv_spec_verify(const pcv_spec_verify_params* p, void* stream) {
+  const int rc = spec_verify_check(p);
+  if (rc != PCV_OK) return rc;
+  return launch_spec_verify(*p, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pcv_spec_uniforms(uint64_t* out, const uint64_t* seeds, const int32_t* positions, int32_t R, int32_t rows_per_batch,
+                      int32_t stream_id, void* stream) {
+  return launch_spec_uniforms(out, seeds, positions, R, rows_per_batch, stream_id,
+                              reinterpret_cast<cudaStream_t>(stream));
+}
+
 static int partial_dropout_check(const pcv_attn_params* p, float dropout_p, bool shard) {
   if (validate_attn(p) != PCV_OK) return 0;
   const char* why = "";

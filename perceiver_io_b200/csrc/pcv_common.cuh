@@ -176,5 +176,9 @@ int sample_check(const pcv_sample_params* p);
 int launch_sample(const pcv_sample_params& p, cudaStream_t stream);
 int launch_sample_uniforms(uint64_t* out, const uint64_t* seeds, const int32_t* positions, int R, int rows_per_batch,
                            cudaStream_t stream);
+int spec_verify_check(const pcv_spec_verify_params* p);
+int launch_spec_verify(const pcv_spec_verify_params& p, cudaStream_t stream);
+int launch_spec_uniforms(uint64_t* out, const uint64_t* seeds, const int32_t* positions, int R, int rows_per_batch,
+                         int stream_id, cudaStream_t stream);
 
 }  // namespace pcv

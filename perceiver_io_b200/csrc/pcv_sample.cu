@@ -21,6 +21,10 @@
 // Determinism: a row's token is a pure function of the row's logit bits, temperature, top_k, top_p, its seed, b and its
 // position.  It does not depend on R, on the other rows, on the launch or on graph capture; two launches are
 // bit-identical.  The logits must be free of NaN and +inf.
+//
+// Speculative sampling (pcv_spec_verify, pcv_spec_uniforms): the rejection rule of Leviathan et al. / Chen et al. on the
+// same integer masses, steps 1-4 shared with sample_kernel (stage_row, kept_threshold); the rule is stated at
+// spec_verify_kernel and in include/pcv_attn.h, and oracle/spec_oracle.py restates it with Python integers.
 #include "pcv_common.cuh"
 #include "pcv_hash.cuh"
 
@@ -124,40 +128,37 @@ __device__ __forceinline__ float load_f(const T* p) {
   return Elem<T>::to_f(*p);
 }
 
+// Step 1 of the sampler on the row src[0 .. V): stages x in xs (x / temperature unless greedy) and returns the
+// largest order key in the high word and the complement of the lowest index holding it in the low word.  Called by all
+// threads.
 template <typename T>
-__global__ void __launch_bounds__(kThreads) sample_kernel(const pcv_sample_params p) {
-  extern __shared__ __align__(16) float xs[];   // the row's x (V floats)
-  __shared__ u64 mhist[256];       // top-p masses
-  __shared__ uint32_t chist[256];  // top-k counts
-  __shared__ u64 red[kWarps];
-  __shared__ u64 sel[2];           // radix state: [0] key prefix, [1] count still needed / mass below
-  const int V = p.V, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int64_t row = blockIdx.x;
-  const T* src = static_cast<const T*>(p.logits) + row * p.stride_row;
-  const bool greedy = p.temperature == 0.f;
-
+__device__ __forceinline__ u64 stage_row(const T* src, int V, float temperature, float* xs, u64* red) {
+  const bool greedy = temperature == 0.f;
   u64 best = 0;
-  for (int i = tid; i < V; i += kThreads) {
+  for (int i = threadIdx.x; i < V; i += kThreads) {
     float x = load_f(src + i);
-    if (!greedy) x = x / p.temperature;
+    if (!greedy) x = x / temperature;
     xs[i] = x;
     best = max(best, ((u64)order_key(x) << 32) | (uint32_t)~(uint32_t)i);
   }
-  best = block_max_u64(best, red);   // the largest key, and of its ties the lowest index
-  if (greedy) {
-    if (tid == 0) {
-      p.tokens[row] = (int64_t)(uint32_t)~(uint32_t)best;
-      if (p.logprobs) p.logprobs[row] = 0.f;
-    }
-    return;
-  }
-  const uint32_t top = (uint32_t)(best >> 32);
+  return block_max_u64(best, red);   // the largest key, and of its ties the lowest index
+}
+
+// Steps 2-4 of the sampler (temperature > 0) on the staged row xs whose largest key is top: the least kept key lo under
+// v.top_k and v.top_p.  Called by all threads.
+template <typename Values>
+__device__ __forceinline__ uint32_t kept_threshold(int V, const Values& v, uint32_t top, const float* xs) {
+  __shared__ u64 mhist[256];       // top-p masses
+  __shared__ uint32_t chist[256];  // top-k counts
+  __shared__ u64 sel[2];           // radix state: [0] key prefix, [1] count still needed / mass below
+  __shared__ u64 cut_s;            // the top-p cut
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const float m = key_value(top);
 
   // ---- top-k: the k-th largest key, kept iff key >= lo ----
   uint32_t lo = 0;
-  if (p.top_k > 0 && p.top_k < V) {
-    if (tid == 0) sel[0] = 0, sel[1] = (u64)p.top_k;
+  if (v.top_k > 0 && v.top_k < V) {
+    if (tid == 0) sel[0] = 0, sel[1] = (u64)v.top_k;
     for (int shift = 24; shift >= 0; shift -= 8) {
       for (int i = tid; i < 256; i += kThreads) chist[i] = 0;
       __syncthreads();
@@ -200,7 +201,7 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const pcv_sample_param
   }
 
   // ---- top-p: the least kept key whose W≤ exceeds the cut ----
-  if (p.top_p < 1.f) {
+  if (v.top_p < 1.f) {
     if (tid == 0) sel[0] = 0, sel[1] = 0;
     bool done = false;
     for (int shift = 24; shift >= 0 && !done; shift -= 8) {
@@ -233,10 +234,9 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const pcv_sample_param
           const u64 t = __shfl_up_sync(0xffffffffu, incl, o);
           if (lane >= o) incl += t;
         }
-        __shared__ u64 cut_s;
         if (shift == 24) {   // the first pass sees every kept token: Z and the cut
           const u64 Z = __shfl_sync(0xffffffffu, incl, 31);
-          const double c = floor((1.0 - (double)p.top_p) * (double)Z);
+          const double c = floor((1.0 - (double)v.top_p) * (double)Z);
           if (lane == 0) cut_s = (u64)c;
           __syncwarp();
           if (cut_s >= Z) {   // nothing would stay: the top tie group does
@@ -262,6 +262,27 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const pcv_sample_param
     }
     lo = max(lo, (uint32_t)sel[0]);
   }
+  return lo;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads) sample_kernel(const pcv_sample_params p) {
+  extern __shared__ __align__(16) float xs[];   // the row's x (V floats)
+  __shared__ u64 red[kWarps];
+  const int V = p.V, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int64_t row = blockIdx.x;
+  const T* src = static_cast<const T*>(p.logits) + row * p.stride_row;
+  const u64 best = stage_row(src, V, p.temperature, xs, red);
+  if (p.temperature == 0.f) {
+    if (tid == 0) {
+      p.tokens[row] = (int64_t)(uint32_t)~(uint32_t)best;
+      if (p.logprobs) p.logprobs[row] = 0.f;
+    }
+    return;
+  }
+  const uint32_t top = (uint32_t)(best >> 32);
+  const float m = key_value(top);
+  const uint32_t lo = kept_threshold(V, p, top, xs);
 
   // ---- draw: warp w owns a contiguous segment of the vocabulary ----
   const int seg = ((V + kWarps * 32 - 1) / (kWarps * 32)) * 32;
@@ -319,6 +340,230 @@ __global__ void sample_uniforms_kernel(uint64_t* out, const uint64_t* seeds, con
   out[r] = sample_bits(seeds[b], (uint32_t)b, (uint32_t)positions[r]);
 }
 
+
+// ---- speculative sampling (pcv_spec_verify) ----------------------------------------------------------------------------
+using u128 = unsigned __int128;
+constexpr u64 kMassOne = 1ull << 40;   // the mass of a greedy row's one token
+constexpr int kAcceptStream = 0, kResidualStream = 1;
+
+// The accept (stream 0) and residual (stream 1) bits of (seed, b, position): sample_bits' construction with round keys
+// of their own, so the three streams are independent at equal counters and every existing draw keeps its bits.
+__device__ __forceinline__ u64 spec_bits(u64 seed, uint32_t b, uint32_t pos, int stream) {
+  const uint32_t word = (b * 0x9E3779B1u + pos) * 0x85EBCA6Bu;
+  const uint32_t lo = (uint32_t)seed, hi = (uint32_t)(seed >> 32);
+  const bool acc = stream == kAcceptStream;
+  const uint32_t h0 = sample_half(word, lo, hi, 0xD2511F53u, 0xCD9E8D57u, acc ? 0x428A2F98u : 0x923F82A4u,
+                                  acc ? 0x71374491u : 0xAB1C5ED5u, acc ? 0xB5C0FBCFu : 0xD807AA98u);
+  const uint32_t h1 = sample_half(word, lo, hi, 0xCD9E8D57u, 0xD2511F53u, acc ? 0xE9B5DBA5u : 0x12835B01u,
+                                  acc ? 0x3956C25Bu : 0x243185BEu, acc ? 0x59F111F1u : 0x550C7DC3u);
+  return ((u64)h1 << 32) | h0;
+}
+
+// filter values in the field names kept_threshold reads
+struct FilterValues {
+  float temperature;
+  int32_t top_k;
+  float top_p;
+};
+
+// A filtered row.  greedy: the one kept token is `arg`.  Otherwise the kept tokens are those with order_key(x) >= lo,
+// each of mass token_mass(x, m), with x the row's scaled value in xs.
+struct RowFilter {
+  bool greedy;
+  int arg;
+  float m;
+  uint32_t lo;
+};
+
+template <typename T>
+__device__ __forceinline__ RowFilter filter_row(const T* src, int V, const FilterValues& v, float* xs, u64* red) {
+  const u64 best = stage_row(src, V, v.temperature, xs, red);
+  if (v.temperature == 0.f) return RowFilter{true, (int)(uint32_t)~(uint32_t)best, 0.f, 0u};
+  const uint32_t top = (uint32_t)(best >> 32);
+  return RowFilter{false, 0, key_value(top), kept_threshold(V, v, top, xs)};
+}
+
+// the kept mass of token i of a filtered row whose scaled value is x
+__device__ __forceinline__ u64 kept_mass(const RowFilter& f, float x, int i) {
+  return f.greedy ? (i == f.arg ? kMassOne : 0ull) : (order_key(x) >= f.lo ? token_mass(x, f.m) : 0ull);
+}
+
+// floor(u * z / 2^64), exact for z < 2^128 with u * floor(z / 2^64) < 2^128 (here z < 2^111)
+__device__ __forceinline__ u128 mul_hi64(u64 u, u128 z) {
+  return (u128)u * (u64)(z >> 64) + __umul64hi(u, (u64)z);
+}
+
+__device__ __forceinline__ u128 shfl_u128(u128 v, int src) {
+  const u64 lo = __shfl_sync(0xffffffffu, (u64)v, src), hi = __shfl_sync(0xffffffffu, (u64)(v >> 64), src);
+  return ((u128)hi << 64) | lo;
+}
+__device__ __forceinline__ u128 shfl_up_u128(u128 v, int o) {
+  const u64 lo = __shfl_up_sync(0xffffffffu, (u64)v, o), hi = __shfl_up_sync(0xffffffffu, (u64)(v >> 64), o);
+  return ((u128)hi << 64) | lo;
+}
+__device__ __forceinline__ u128 shfl_xor_u128(u128 v, int o) {
+  const u64 lo = __shfl_xor_sync(0xffffffffu, (u64)v, o), hi = __shfl_xor_sync(0xffffffffu, (u64)(v >> 64), o);
+  return ((u128)hi << 64) | lo;
+}
+
+// every thread gets the block's sum
+__device__ __forceinline__ u64 block_sum_u64(u64 v, u64* red) {
+  v = warp_sum_u64(v);
+  __syncthreads();   // red[] may still be read
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  u64 s = 0;
+#pragma unroll
+  for (int w = 0; w < kWarps; ++w) s += red[w];
+  return s;
+}
+
+// Warp w's contiguous segment [s0, s1) of the vocabulary, its weight sum and the sums before it and over the block.
+struct Segment {
+  int s0, s1;
+  u128 before, part, total;
+};
+
+template <typename W>
+__device__ __forceinline__ Segment segment_sums(int V, W weight, u128* red) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int seg = ((V + kWarps * 32 - 1) / (kWarps * 32)) * 32;
+  Segment s;
+  s.s0 = warp * seg;
+  s.s1 = min(V, s.s0 + seg);
+  u128 part = 0;
+  for (int y = s.s0 + lane; y < s.s1; y += 32) part += weight(y);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) part += shfl_xor_u128(part, o);
+  __syncthreads();   // red[] of an earlier call has been read
+  if (lane == 0) red[warp] = part;
+  __syncthreads();
+  s.part = part;
+  s.before = 0;
+  s.total = 0;
+#pragma unroll
+  for (int w = 0; w < kWarps; ++w) {
+    const u128 v = red[w];
+    s.before += w < warp ? v : (u128)0;
+    s.total += v;
+  }
+  return s;
+}
+
+// *out = the first index, in vocabulary order, whose prefix weight exceeds t (t < s.total): written by the one warp
+// whose segment holds it.
+template <typename W>
+__device__ __forceinline__ void segment_find(W weight, const Segment& s, u128 t, int64_t* out) {
+  const int lane = threadIdx.x & 31;
+  if (t < s.before || t >= s.before + s.part) return;
+  u128 acc = s.before;
+  for (int base = s.s0; base < s.s1; base += 32) {
+    const int y = base + lane;
+    u128 incl = y < s.s1 ? weight(y) : (u128)0;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const u128 v = shfl_up_u128(incl, o);
+      if (lane >= o) incl += v;
+    }
+    const unsigned hit = __ballot_sync(0xffffffffu, acc + incl > t);
+    if (hit) {
+      if (lane == __ffs(hit) - 1) *out = y;
+      return;
+    }
+    acc += shfl_u128(incl, 31);
+  }
+}
+
+// One CTA per (batch row b, target row i), i = 0 .. G.  With P / Zp the kept masses and their sum of target row i and
+// Q / Zq those of draft row i under the draft's filter values (i < G), x = tokens[b, i + 1]:
+//   accept x iff hi64(u_a * Q(x) * Zp) < P(x) * Zq  (u_a: the accept stream at (seeds[b], b, positions[b, i]));
+//   accepted: out[b, i] = -1.  Rejected: out[b, i] = the residual draw: the first index whose prefix sum of
+//   R(y) = max(0, P(y) Zq - Q(y) Zp) exceeds hi64(u_r * ΣR) (u_r: the residual stream at the same counter), or, when
+//   ΣR = 0, the draw from P.  i = G: out[b, G] = the draw from P with u_r (the bonus token).
+// The draft row is filtered first and only its filter (m, lo, Zq, Q(x)) is kept: the target row then takes the same
+// shared buffer, and the residual pass recomputes Q(y) from the draft logits in global memory.
+template <typename T>
+__global__ void __launch_bounds__(kThreads) spec_verify_kernel(const pcv_spec_verify_params p) {
+  extern __shared__ __align__(16) float xs[];   // the row's x (V floats): the draft row's, then the target row's
+  __shared__ u64 red[kWarps];
+  __shared__ u128 red128[kWarps];
+  const int V = p.V, G = p.G, tid = threadIdx.x;
+  const int b = blockIdx.x / (G + 1), i = blockIdx.x % (G + 1);
+  const int64_t cell = (int64_t)b * (G + 1) + i;
+  const bool has_draft = i < G;
+  const T* tsrc = static_cast<const T*>(p.target) + b * p.t_stride_b + i * p.t_stride_row;
+  const T* dsrc = static_cast<const T*>(p.draft) + b * p.d_stride_b + (has_draft ? i : 0) * p.d_stride_row;
+  const int64_t x = has_draft ? p.tokens[cell + 1] : -1;
+  const bool x_in = x >= 0 && x < V;   // a token outside the vocabulary has P = Q = 0: it is rejected
+
+  RowFilter fq{true, -1, 0.f, 0u};
+  u64 Zq = 0, Qx = 0;
+  if (has_draft) {
+    fq = filter_row(dsrc, V, FilterValues{p.draft_temperature, p.draft_top_k, p.draft_top_p}, xs, red);
+    u64 part = 0;
+    for (int y = tid; y < V; y += kThreads) part += kept_mass(fq, xs[y], y);
+    Zq = block_sum_u64(part, red);
+    if (x_in) Qx = kept_mass(fq, xs[x], (int)x);
+    __syncthreads();   // every thread has read xs before the target row replaces it
+  }
+  const RowFilter fp = filter_row(tsrc, V, FilterValues{p.temperature, p.top_k, p.top_p}, xs, red);
+  u64 part = 0;
+  for (int y = tid; y < V; y += kThreads) part += kept_mass(fp, xs[y], y);
+  const u64 Zp = block_sum_u64(part, red);
+
+  const u64 seed = p.seeds[b];
+  const uint32_t pos = (uint32_t)p.positions[cell];
+  if (has_draft) {
+    const u64 Px = x_in ? kept_mass(fp, xs[x], (int)x) : 0ull;
+    const u64 ua = spec_bits(seed, (uint32_t)b, pos, kAcceptStream);
+    if (mul_hi64(ua, (u128)Qx * Zp) < (u128)Px * Zq) {
+      if (tid == 0) p.out_tokens[cell] = -1;
+      return;
+    }
+  }
+  const u64 ur = spec_bits(seed, (uint32_t)b, pos, kResidualStream);
+  const float tq = p.draft_temperature;
+  auto target_mass = [&](int y) -> u128 { return kept_mass(fp, xs[y], y); };
+  auto residual = [&](int y) -> u128 {
+    const u128 a = (u128)kept_mass(fp, xs[y], y) * Zq;
+    const u128 c = (u128)kept_mass(fq, fq.greedy ? 0.f : load_f(dsrc + y) / tq, y) * Zp;
+    return a > c ? a - c : (u128)0;
+  };
+  bool from_residual = has_draft;
+  Segment s;
+  if (from_residual) {
+    s = segment_sums(V, residual, red128);
+    from_residual = s.total != 0;   // ΣR = 0 only for a draft Q and P both give no mass: draw from P
+  }
+  if (!from_residual) s = segment_sums(V, target_mass, red128);
+  const u128 t = mul_hi64(ur, s.total);
+  if (from_residual) segment_find(residual, s, t, p.out_tokens + cell);
+  else segment_find(target_mass, s, t, p.out_tokens + cell);
+}
+
+// One thread per batch row: n = the first rejected draft (its cell holds the correction) or G (the bonus), then the
+// row's output in place: the n accepted drafts, the correction or bonus token, -1 after it.
+__global__ void spec_resolve_kernel(const pcv_spec_verify_params p) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= p.B) return;
+  const int G = p.G;
+  int64_t* out = p.out_tokens + (int64_t)b * (G + 1);
+  const int64_t* fed = p.tokens + (int64_t)b * (G + 1);
+  int n = 0;
+  while (n < G && out[n] < 0) ++n;
+  for (int j = 0; j < n; ++j) out[j] = fed[j + 1];
+  for (int j = n + 1; j <= G; ++j) out[j] = -1;
+  p.accepted[b] = n;
+}
+
+__global__ void spec_uniforms_kernel(uint64_t* out, const uint64_t* seeds, const int32_t* positions, int R, int rpb,
+                                     int stream) {
+  const int r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= R) return;
+  const int b = r / rpb;
+  out[r] = spec_bits(seeds[b], (uint32_t)b, (uint32_t)positions[r], stream);
+}
+
 }  // namespace
 
 int sample_check(const pcv_sample_params* p) {
@@ -365,6 +610,76 @@ int launch_sample_uniforms(uint64_t* out, const uint64_t* seeds, const int32_t* 
   PCV_REQUIRE(R >= 1 && rows_per_batch >= 1 && R % rows_per_batch == 0, PCV_ERR_INVALID,
               "sample_uniforms: R=%d must be >= 1 and a multiple of rows_per_batch=%d", R, rows_per_batch);
   sample_uniforms_kernel<<<(R + 255) / 256, 256, 0, stream>>>(out, seeds, positions, R, rows_per_batch);
+  PCV_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return PCV_OK;
+}
+
+static bool sampling_values_ok(const char* who, float temperature, int32_t top_k, float top_p) {
+  PCV_REQUIRE(temperature >= 0.f, false, "spec_verify: %s temperature must be >= 0 (0: greedy), got %g", who,
+              (double)temperature);
+  PCV_REQUIRE(top_k >= 0, false, "spec_verify: %s top_k must be >= 0 (0: off), got %d", who, top_k);
+  PCV_REQUIRE(top_p > 0.f && top_p <= 1.f, false, "spec_verify: %s top_p must be in (0, 1] (1: off), got %g", who,
+              (double)top_p);
+  return true;
+}
+
+int spec_verify_check(const pcv_spec_verify_params* p) {
+  PCV_REQUIRE(p != nullptr, PCV_ERR_INVALID, "spec_verify: params is NULL");
+  PCV_REQUIRE(p->target && p->draft && p->tokens && p->seeds && p->positions && p->out_tokens && p->accepted,
+              PCV_ERR_INVALID, "spec_verify: target / draft / tokens / seeds / positions / out_tokens / accepted pointer "
+              "is NULL");
+  PCV_REQUIRE(p->dtype == PCV_BF16 || p->dtype == PCV_F16 || p->dtype == PCV_F32, PCV_ERR_INVALID,
+              "spec_verify: unknown dtype %d (bf16, fp16 or fp32 logits)", p->dtype);
+  PCV_REQUIRE(p->draft_dtype == p->dtype, PCV_ERR_INVALID,
+              "spec_verify: the draft logits' dtype %d differs from the target logits' dtype %d", p->draft_dtype,
+              p->dtype);
+  PCV_REQUIRE(p->V >= 1 && p->V <= PCV_SAMPLE_MAX_VOCAB, PCV_ERR_UNSUPPORTED, "spec_verify: V=%d must be in [1, %d]",
+              p->V, PCV_SAMPLE_MAX_VOCAB);
+  PCV_REQUIRE(p->G >= 1 && p->G <= PCV_SPEC_MAX_DRAFTS, PCV_ERR_UNSUPPORTED, "spec_verify: G=%d must be in [1, %d]",
+              p->G, PCV_SPEC_MAX_DRAFTS);
+  PCV_REQUIRE(p->B >= 1, PCV_ERR_INVALID, "spec_verify: B=%d must be >= 1", p->B);
+  PCV_REQUIRE(p->t_stride_b >= p->V && p->t_stride_row >= p->V && p->d_stride_b >= p->V && p->d_stride_row >= p->V,
+              PCV_ERR_INVALID, "spec_verify: a stride (target %lld / %lld, draft %lld / %lld) is below V=%d",
+              (long long)p->t_stride_b, (long long)p->t_stride_row, (long long)p->d_stride_b,
+              (long long)p->d_stride_row, p->V);
+  const int64_t cells = (int64_t)p->B * (p->G + 1);
+  PCV_REQUIRE(p->out_tokens + cells <= p->tokens || p->tokens + cells <= p->out_tokens, PCV_ERR_INVALID,
+              "spec_verify: out_tokens overlaps tokens");
+  if (!sampling_values_ok("target", p->temperature, p->top_k, p->top_p)) return PCV_ERR_INVALID;
+  if (!sampling_values_ok("draft", p->draft_temperature, p->draft_top_k, p->draft_top_p)) return PCV_ERR_INVALID;
+  return PCV_OK;
+}
+
+int launch_spec_verify(const pcv_spec_verify_params& p, cudaStream_t stream) {
+  const int smem = p.V * (int)sizeof(float);
+  const void* kern = p.dtype == PCV_BF16  ? reinterpret_cast<const void*>(&spec_verify_kernel<__nv_bfloat16>)
+                     : p.dtype == PCV_F16 ? reinterpret_cast<const void*>(&spec_verify_kernel<__half>)
+                                          : reinterpret_cast<const void*>(&spec_verify_kernel<float>);
+  if (smem > 48 * 1024) {   // once per kernel and device, for the largest row
+    const int rc = sm90::set_smem_limit(kern, PCV_SAMPLE_MAX_VOCAB * (int)sizeof(float));
+    if (rc != PCV_OK) return rc;
+  }
+  const int grid = p.B * (p.G + 1);
+  if (p.dtype == PCV_BF16) spec_verify_kernel<__nv_bfloat16><<<grid, kThreads, smem, stream>>>(p);
+  else if (p.dtype == PCV_F16) spec_verify_kernel<__half><<<grid, kThreads, smem, stream>>>(p);
+  else spec_verify_kernel<float><<<grid, kThreads, smem, stream>>>(p);
+  PCV_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  spec_resolve_kernel<<<(p.B + 127) / 128, 128, 0, stream>>>(p);
+  PCV_CHECK_CUDA(cudaGetLastError());
+  count_launch();
+  return PCV_OK;
+}
+
+int launch_spec_uniforms(uint64_t* out, const uint64_t* seeds, const int32_t* positions, int R, int rows_per_batch,
+                         int stream_id, cudaStream_t stream) {
+  PCV_REQUIRE(out && seeds && positions, PCV_ERR_INVALID, "spec_uniforms: out / seeds / positions pointer is NULL");
+  PCV_REQUIRE(R >= 1 && rows_per_batch >= 1 && R % rows_per_batch == 0, PCV_ERR_INVALID,
+              "spec_uniforms: R=%d must be >= 1 and a multiple of rows_per_batch=%d", R, rows_per_batch);
+  PCV_REQUIRE(stream_id == 0 || stream_id == 1, PCV_ERR_INVALID,
+              "spec_uniforms: stream_id=%d must be 0 (accept) or 1 (residual)", stream_id);
+  spec_uniforms_kernel<<<(R + 255) / 256, 256, 0, stream>>>(out, seeds, positions, R, rows_per_batch, stream_id);
   PCV_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PCV_OK;

@@ -19,6 +19,9 @@ run, and in-graph int32 ops advance them at the end of each step.
     first = dec.draw(logits)                                                  # (B, 1): prefill's logits, eager
     tokens = dec.generate(first, n)                                           # (B, n): n replays, no host sync
     tokens, logits = dec.sample(token_ids)                                    # (B, k) drafts -> (B, k) draws
+    tokens, q = dec.generate(first, n, logits=True)                           # and the (B, n, vocab) logits drawn from
+    out, accepted = dec.verify(token_ids, draft_logits, draft_sampling)       # (B, G+1) -> one speculative round
+    tokens, stats = speculative_generate(target, draft, first, n, draft_tokens=G)
 
 Rows: cross-attention arena row r holds token r of the sequence (prompt and generated tokens); self-attention arena
 row r holds token ``prefix_len + r`` (prefix_len of the prompt).  The windows follow the 🤗 wrapper's truncation, as
@@ -46,7 +49,9 @@ counter (seed_b, b, p).  A replay that feeds k tokens at rows r .. r+k-1 draws a
 graph from the row counters, so after a ``rewind`` the same positions draw the same bits again: a rewound sequence that
 is fed the same tokens resamples identically.  ``sample(drafts)`` returns the token drawn after each draft, so
 speculative acceptance is ``drafts[:, i+1] == tokens[:, i]`` on the device: the accepted tokens are draws from the
-model's own filtered distribution.
+model's own filtered distribution.  ``verify`` and :func:`speculative_generate` use a draft model's probabilities
+instead: min(1, p/q) acceptance and a draw from max(0, p - q) on rejection (``ops.spec_verify``), so every emitted token
+is distributed as the target's own draw and a draft is accepted with probability Σ min(p, q).
 
 Not covered: steps of more than 64 tokens, a different k per batch row, contrastive search, a ring buffer bounded at
 ``max_seq_len`` (the arenas grow by ``max_new_tokens`` rows), EOS handling (callers truncate after EOS), per-row
@@ -146,6 +151,13 @@ def sample_positions(bounds: torch.Tensor, steps: torch.Tensor, k: int) -> torch
     return bounds[:, 0, 2:3] + steps[:k]
 
 
+def _triple(vals):
+    if not isinstance(vals, (tuple, list)) or len(vals) != 3:
+        raise ValueError(f"GraphedDecoder.verify: draft_sampling must be a (temperature, top_k, top_p) triple, got "
+                         f"{vals!r}")
+    return vals
+
+
 def _as_count(x):
     """x as an int when it is integer-like (operator.index) and not a bool, else None."""
     if isinstance(x, bool):
@@ -154,6 +166,18 @@ def _as_count(x):
         return operator.index(x)
     except TypeError:
         return None
+
+
+def _sampling_triple(what: str, temperature, top_k, top_p):
+    """(temperature, top_k, top_p) checked as ``ops.sample_tokens`` takes them (top_k clamped to int32)."""
+    t, p, k = float(temperature), float(top_p), _as_count(top_k)
+    if not t >= 0.0 or math.isinf(t):
+        raise ValueError(f"{what}: temperature must be finite and >= 0 (0: greedy), got {temperature!r}")
+    if k is None or k < 0:
+        raise ValueError(f"{what}: top_k must be an integer >= 0 (0: off), got {top_k!r}")
+    if not 0.0 < p <= 1.0:
+        raise ValueError(f"{what}: top_p must be in (0, 1] (1: off), got {top_p!r}")
+    return t, min(k, 2 ** 31 - 1), p
 
 
 class _Attn:
@@ -170,6 +194,7 @@ class GraphedDecoder:
     # than the furthest row (whose count is _fed)
     _lag = None
     _seeds = None   # (B,) int64 sampler seeds, set in __init__
+    _draft_sampling = (1.0, 0, 1.0)   # the draft's values of the verify graph being recorded or replayed
 
     def __init__(self, model, batch: int, max_new_tokens: int, kv_cache: str = "bf16"):
         if max_new_tokens < 1:
@@ -340,9 +365,17 @@ class GraphedDecoder:
         t, top_k, top_p = self._sampling
         return ops.sample_tokens(logits, self._seeds, pos, t, top_k, top_p), logits
 
-    def _replay(self, token_ids: torch.Tensor, fn: str) -> torch.Tensor:
+    def _verify_fn(self, token: torch.Tensor, draft_logits: torch.Tensor):
+        """_step_fn followed by ``ops.spec_verify`` on its logits: (tokens (B, k), accepted (B,))."""
+        pos = sample_positions(self._bounds, self._steps, token.shape[1])   # before _step_fn advances the rows
+        logits = self._step_fn(token)
+        self._verify_logits = logits   # the static target logits of the verify graph recorded last (for tests)
+        return ops.spec_verify(logits, draft_logits, token, self._seeds, pos, self._sampling, self._draft_sampling)
+
+    def _replay(self, token_ids: torch.Tensor, fn: str, *extra: torch.Tensor) -> torch.Tensor:
         """One replay of the graph of ``token_ids.shape[1]`` tokens per step, recorded on first use (``fn`` "sample":
-        the graph that also samples, one per sampling triple)."""
+        the graph that also samples, one per sampling triple; "verify": the graph that also verifies drafts, one per
+        pair of sampling triples, with ``extra`` its draft logits)."""
         k = token_ids.shape[1] if token_ids.dim() == 2 else 0
         kmax = 1 if fn in ("step", "generate") else ops.WINDOW_MAX_ROWS
         if self._bounds is None:
@@ -359,19 +392,22 @@ class GraphedDecoder:
             raise RuntimeError("GraphedDecoder does not run under autocast")
         sample = fn in ("sample", "generate")
         key = ("sample", k, self._sampling) if sample else k
+        fwd = self._sample_fn if sample else self._step_fn
+        if fn == "verify":
+            key, fwd = ("verify", k, self._sampling, self._draft_sampling), self._verify_fn
         graph = self._graphs.get(key)
         if graph is None:
             snapshot = self._bounds.clone()   # the warm-up calls advance the rows; their arena writes are rewritten later
             old = torch.cuda.get_sync_debug_mode()
             torch.cuda.set_sync_debug_mode(0)  # recording a graph synchronises the device once
             try:
-                graph = GraphedForward(self._sample_fn if sample else self._step_fn, token_ids)
+                graph = GraphedForward(fwd, token_ids, *extra)
             finally:
                 torch.cuda.set_sync_debug_mode(old)
             self._bounds.copy_(snapshot)
             self._graphs[key] = graph
             self.captures += 1
-        out = graph(token_ids)
+        out = graph(token_ids, *extra)
         self._remaining -= k
         self._fed += k
         return out
@@ -418,15 +454,7 @@ class GraphedDecoder:
         """The sampler's values for ``draw``, ``sample`` and ``generate``: ``temperature`` >= 0 (0: greedy), ``top_k`` >= 0
         (0: off), ``top_p`` in (0, 1] (1: off), as ``ops.sample_tokens`` takes them.  The first replay under a new triple
         records its graphs."""
-        t, p, k = float(temperature), float(top_p), _as_count(top_k)
-        if not t >= 0.0 or math.isinf(t):
-            raise ValueError(f"GraphedDecoder.set_sampling: temperature must be finite and >= 0 (0: greedy), got "
-                             f"{temperature!r}")
-        if k is None or k < 0:
-            raise ValueError(f"GraphedDecoder.set_sampling: top_k must be an integer >= 0 (0: off), got {top_k!r}")
-        if not 0.0 < p <= 1.0:
-            raise ValueError(f"GraphedDecoder.set_sampling: top_p must be in (0, 1] (1: off), got {top_p!r}")
-        self._sampling = (t, min(k, 2 ** 31 - 1), p)
+        self._sampling = _sampling_triple("GraphedDecoder.set_sampling", temperature, top_k, top_p)
 
     def _ready_to_sample(self, what: str) -> None:
         if self._bounds is None:
@@ -456,11 +484,13 @@ class GraphedDecoder:
         self._ready_to_sample("sample")
         return self._replay(token_ids, "sample")
 
-    def generate(self, first_tokens: torch.Tensor, n: int) -> torch.Tensor:
+    def generate(self, first_tokens: torch.Tensor, n: int, logits: bool = False):
         """Feed ``first_tokens`` (B, 1) int64 and then every drawn token, for n replays of the one-token sampling graph;
         return the n drawn tokens (B, n) int64.  Each replay's input is copied on the device from the previous one's
         output: no host read and no synchronisation.  Consumes n tokens of the budget; asking for more than remain is
-        refused before any replay, leaving the state untouched."""
+        refused before any replay, leaving the state untouched.  With ``logits=True`` also return the logits each token
+        was drawn from, (B, n, vocab), copied on the device after each replay (a draft model's probabilities for
+        :meth:`verify`)."""
         self._ready_to_sample("generate")
         count = _as_count(n)
         if count is None or count < 1:
@@ -472,11 +502,40 @@ class GraphedDecoder:
             raise ValueError(f"GraphedDecoder.generate takes ({self.batch}, 1) int64 first tokens, got "
                              f"{tuple(first_tokens.shape)} {first_tokens.dtype}")
         out = torch.empty(self.batch, count, dtype=torch.long, device=self.device)
+        kept = None
         tokens = first_tokens
         for i in range(count):
-            tokens, _ = self._replay(tokens, "generate")
+            tokens, lg = self._replay(tokens, "generate")
             out[:, i:i + 1].copy_(tokens)
-        return out
+            if logits:
+                if kept is None:
+                    kept = torch.empty(self.batch, count, lg.shape[-1], dtype=lg.dtype, device=self.device)
+                kept[:, i:i + 1].copy_(lg)
+        return (out, kept) if logits else out
+
+    def verify(self, token_ids: torch.Tensor, draft_logits: torch.Tensor, draft_sampling=(1.0, 0, 1.0)):
+        """One round of speculative sampling with a draft model's probabilities, in one replay.
+
+        ``token_ids`` (B, G+1) int64, 1 <= G <= 63: t_0 (the newest emitted token not fed yet) and the draft's G draws;
+        ``draft_logits`` (B, G, vocab), of this model's logits dtype: the logits the draft drew t_1 .. t_G from, under
+        ``draft_sampling`` = (temperature, top_k, top_p).  The replay feeds the G+1 tokens (as :meth:`extend`) and runs
+        ``ops.spec_verify`` on the logits after each of them, under this decoder's ``set_sampling`` values, at the
+        positions :meth:`sample` would draw at.  Returns ``(tokens, accepted)``: (B, G+1) int64, the n_b accepted
+        drafts, the correction or bonus token, then -1; and (B,) int32 n_b.  Views of the graph's static outputs, valid
+        until the next replay; nothing is read back to the host.  Consumes G+1 tokens of the budget: the caller then
+        rewinds row b by G - n_b.  The graph is recorded on first use, one per (G, target values, draft values)."""
+        self._ready_to_sample("verify")
+        draft = _sampling_triple("GraphedDecoder.verify: draft_sampling", *_triple(draft_sampling))
+        k = token_ids.shape[1] if token_ids.dim() == 2 else 0
+        if not 2 <= k <= ops.SPEC_MAX_DRAFTS + 1:
+            raise ValueError(f"GraphedDecoder.verify takes ({self.batch}, G+1) int64 tokens with 1 <= G <= "
+                             f"{ops.SPEC_MAX_DRAFTS}, got {tuple(token_ids.shape)}")
+        vocab = self.model.config.vocab_size
+        if tuple(draft_logits.shape) != (self.batch, k - 1, vocab) or draft_logits.dtype != self.dtype:
+            raise ValueError(f"GraphedDecoder.verify takes ({self.batch}, {k - 1}, {vocab}) {self.dtype} draft logits, "
+                             f"got {tuple(draft_logits.shape)} {draft_logits.dtype}")
+        self._draft_sampling = draft
+        return self._replay(token_ids, "verify", draft_logits)
 
     def rewind(self, n) -> None:
         """Drop fed tokens: the next token of a batch row is fed at the row of its first dropped one, as if the dropped
@@ -554,3 +613,88 @@ class GraphedDecoder:
             self._seeds.copy_(self._seeds.index_select(0, idx))
         if self._lag is not None:
             self._set_fed([self._fed - self._lag[i] for i in beam_idx.tolist()])
+
+
+def speculative_budget(n: int, draft_tokens: int, batch: int) -> int:
+    """The ``max_new_tokens`` (budget left after ``prefill``) both decoders of :func:`speculative_generate` need for n
+    tokens with G = ``draft_tokens`` drafts per round: n + G for one batch row, n + 2G + 1 for more.
+
+    A row that has emitted e < n tokens has fed e of them, and a round feeds G+1 more before the rewind: at most
+    n - 1 + G + 1 = n + G.  With more than one row a finished row can stand at n + G (it accepted every draft of its
+    last round) and still be fed, and rewound, G+1 tokens per round while another row finishes: n + 2G + 1."""
+    return n + draft_tokens if batch == 1 else n + 2 * draft_tokens + 1
+
+
+def speculative_generate(target: "GraphedDecoder", draft: "GraphedDecoder", first: torch.Tensor, n: int,
+                         draft_tokens: int = 4):
+    """Speculative sampling with a draft model (Leviathan et al. 2023; Chen et al. 2023): n tokens per batch row, each
+    distributed exactly as ``target.generate`` would draw it under the target's ``set_sampling`` values.
+
+    Both decoders must have been prefilled with the same prompt (same batch and vocabulary); ``first`` (B, 1) int64 is
+    drawn from the target (``target.draw``).  Each round of G = ``draft_tokens`` drafts:
+      1. ``draft.generate(t_0, G+1, logits=True)``: the first G draws are the drafts, the last is discarded (it makes the
+         draft feed t_0 .. t_G, as the target does);
+      2. ``target.verify``: min(1, p/q) acceptance, the residual or bonus token, on the device;
+      3. one device-to-host read of ``accepted`` — the round's only synchronisation;
+      4. both decoders rewind row b by G - n_b (a row that already has n tokens by G+1: it stops advancing);
+      5. the next t_0 of row b is its correction or bonus token, gathered on the device.
+    Needs :func:`speculative_budget` (n, G, B) tokens of budget left in both decoders, refused before any replay.
+
+    Returns ``(tokens, stats)``: (B, n) int64, and a dict with ``rounds``, and per batch row ``proposed`` (drafts
+    offered while the row was unfinished) and ``accepted`` (of those, accepted)."""
+    G, count = _as_count(draft_tokens), _as_count(n)
+    if G is None or not 1 <= G <= ops.SPEC_MAX_DRAFTS:
+        raise ValueError(f"speculative_generate: draft_tokens must be an integer in [1, {ops.SPEC_MAX_DRAFTS}], got "
+                         f"{draft_tokens!r}")
+    if count is None or count < 1:
+        raise ValueError(f"speculative_generate: n must be an integer >= 1, got {n!r}")
+    B = target.batch
+    if draft.batch != B:
+        raise ValueError(f"speculative_generate: the draft's batch {draft.batch} != the target's {B}")
+    if draft.model.config.vocab_size != target.model.config.vocab_size:
+        raise ValueError(f"speculative_generate: the draft's vocabulary {draft.model.config.vocab_size} != the "
+                         f"target's {target.model.config.vocab_size}")
+    if target._bounds is None or draft._bounds is None:
+        raise RuntimeError("speculative_generate: prefill() both decoders first")
+    if tuple(first.shape) != (B, 1) or first.dtype != torch.long:
+        raise ValueError(f"speculative_generate takes ({B}, 1) int64 first tokens, got {tuple(first.shape)} "
+                         f"{first.dtype}")
+    need = speculative_budget(count, G, B)
+    for name, dec in (("target", target), ("draft", draft)):
+        if dec._remaining < need:
+            raise RuntimeError(f"speculative_generate: the {name} has {dec._remaining} tokens of budget left, n={count} "
+                               f"with {G} drafts per round needs {need} (speculative_budget)")
+    dev = target.device
+    width = count + G + 2                       # column width - 1 takes the tokens a round does not keep
+    buf = torch.empty(B, width, dtype=torch.long, device=dev)
+    done, proposed, accepted_total = [0] * B, [0] * B, [0] * B
+    t0, rounds = first, 0
+    cols = torch.arange(G + 1)
+    while min(done) < count:
+        drafts, q_logits = draft.generate(t0, G + 1, logits=True)
+        fed = torch.cat([t0, drafts[:, :G]], dim=1)
+        tokens, accepted = target.verify(fed, q_logits[:, :G], draft_sampling=draft._sampling)
+        acc = accepted.to("cpu").tolist()       # the round's one synchronisation
+        rounds += 1
+        # host-built indices: where each row's kept tokens go in buf, and which column of [t0 | tokens] is the next t0
+        idx = torch.full((B, G + 2), width - 1, dtype=torch.long)
+        back = []
+        for b in range(B):
+            if done[b] >= count:
+                idx[b, G + 1] = 0
+                back.append(G + 1)
+                continue
+            nb = acc[b]
+            idx[b, :nb + 1] = done[b] + cols[:nb + 1]
+            idx[b, G + 1] = nb + 1
+            back.append(G - nb)
+            done[b] += nb + 1
+            proposed[b] += G
+            accepted_total[b] += nb
+        if dev.type == "cuda":                  # pinned and asynchronous: no synchronisation
+            idx = idx.pin_memory().to(dev, non_blocking=True)
+        buf.scatter_(1, idx[:, :G + 1], tokens)
+        t0 = torch.cat([t0, tokens], dim=1).gather(1, idx[:, G + 1:])
+        target.rewind(back)
+        draft.rewind(back)
+    return buf[:, :count], {"rounds": rounds, "proposed": proposed, "accepted": accepted_total}

@@ -35,7 +35,9 @@ class GraphedForward:
     def __init__(self, fn: Callable, *example_inputs: torch.Tensor, warmup: int = 3):
         if not example_inputs or not all(isinstance(t, torch.Tensor) and t.is_cuda for t in example_inputs):
             raise RuntimeError("GraphedForward needs CUDA example inputs (there is no CPU path)")
-        self._fn = fn
+        # fn is not kept: a bound method of an owner that holds this object (GraphedDecoder) would make a reference cycle,
+        # and the cycle collector could then destroy the graph while another stream is capturing, which invalidates
+        # that capture.
         self._inputs = [t.clone() for t in example_inputs]
         side = torch.cuda.Stream(device=self._inputs[0].device)
         side.wait_stream(torch.cuda.current_stream())

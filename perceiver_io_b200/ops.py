@@ -30,7 +30,7 @@ __all__ = [
     "kv_project_fp8_supported", "ln_linear", "ln_linear_backward", "kv_append_fp8", "attention_decode_fp8",
     "attention_decode_fp8_supported", "fp8_pair_descale", "fp8_dequantize", "rotated_cache_shadow", "rotary_at", "rotary_fp8",
     "attention_decode_window", "kv_append_at", "rotary_apply_at", "rotary_angle_table", "attention_window",
-    "sample_tokens", "sample_uniforms",
+    "sample_tokens", "sample_uniforms", "spec_verify", "spec_uniforms",
 ]
 
 
@@ -1372,6 +1372,97 @@ def sample_uniforms(seeds: torch.Tensor, positions: torch.Tensor) -> torch.Tenso
     with torch.cuda.device(positions.device):
         check(_lib.lib().pcv_sample_uniforms(out.data_ptr(), seeds.data_ptr(), positions.data_ptr(), positions.numel(),
                                              1 if len(lead) == 1 else lead[1], _stream()), "pcv_sample_uniforms")
+    return out
+
+
+# --------------------------------------------------------------------------------------------------
+# speculative sampling (pcv_spec_verify): the rejection rule with a draft model's probabilities, on the sampler's integer
+# masses, with accept and residual bits from two counter-based streams of their own.
+# --------------------------------------------------------------------------------------------------
+#: The most drafts :func:`spec_verify` decides per batch row in one call.
+SPEC_MAX_DRAFTS = _lib.SPEC_MAX_DRAFTS
+_SPEC_STREAMS = {"accept": 0, "residual": 1}
+
+
+def _sampling_values(vals, what: str):
+    if not isinstance(vals, (tuple, list)) or len(vals) != 3:
+        raise ValueError(f"spec_verify: {what} must be a (temperature, top_k, top_p) triple, got {vals!r}")
+    t, k, p = vals
+    return float(t), min(int(k), 2 ** 31 - 1), float(p)
+
+
+def spec_verify(target_logits: torch.Tensor, draft_logits: torch.Tensor, tokens: torch.Tensor, seeds: torch.Tensor,
+                positions: torch.Tensor, sampling=(1.0, 0, 1.0), draft_sampling=(1.0, 0, 1.0)):
+    """One round of speculative sampling for every batch row, on the device (pcv_spec_verify).
+
+    Row b fed ``tokens[b]`` = t_0 .. t_G (B, G+1) int64 to both models, t_1 .. t_G drawn by the draft.
+    ``target_logits`` (B, G+1, V): the target's logits after each t_i; ``draft_logits`` (B, G, V), of the same dtype
+    (bf16 / fp16 / fp32): the logits the draft drew t_{i+1} from.  ``sampling`` and ``draft_sampling`` are the
+    (temperature, top_k, top_p) triples of the two models, as :func:`sample_tokens` takes them; p and q are the two
+    filtered distributions.  Draft t_{i+1} is accepted with probability min(1, p/q) (to 2^-64, in exact integer
+    arithmetic on the sampler's masses); the first rejected one is replaced by a draw from max(0, p - q), and when every
+    draft is accepted a bonus token is drawn from the last target row.  ``seeds`` (B,) int64 and ``positions`` (B, G+1)
+    int32 are the counters: the accept and residual bits of target row i use (seeds[b], b, positions[b, i]) on two
+    streams independent of :func:`sample_tokens`' own, so the draft may share the target's seeds.
+
+    Returns ``(tokens, accepted)``: (B, G+1) int64 with the n_b accepted drafts, then the correction or bonus token, then
+    -1; and (B,) int32 n_b.  Nothing is read back to the host, so the call can be recorded in a CUDA graph.  Arguments
+    the kernel does not take raise ``ValueError`` with its reason before any launch."""
+    _require_cuda(target_logits, draft_logits, tokens)
+    if target_logits.dim() != 3 or target_logits.dtype not in (torch.bfloat16, torch.float16, torch.float32):
+        raise ValueError(f"spec_verify: target_logits must be (B, G+1, V) bf16 / fp16 / fp32, got "
+                         f"{tuple(target_logits.shape)} {target_logits.dtype}")
+    B, G1, V = target_logits.shape
+    if tuple(draft_logits.shape) != (B, G1 - 1, V) or draft_logits.dtype != target_logits.dtype:
+        raise ValueError(f"spec_verify: draft_logits must be ({B}, {G1 - 1}, {V}) {target_logits.dtype} like the target "
+                         f"rows, got {tuple(draft_logits.shape)} {draft_logits.dtype}")
+    if tuple(tokens.shape) != (B, G1) or tokens.dtype != torch.int64:
+        raise ValueError(f"spec_verify: tokens must be ({B}, {G1}) int64 (t_0 .. t_G), got {tuple(tokens.shape)} "
+                         f"{tokens.dtype}")
+    seeds, positions = _sample_counters(seeds, positions, (B, G1), "spec_verify")
+    t, k, p_ = _sampling_values(sampling, "sampling")
+    dt, dk, dp = _sampling_values(draft_sampling, "draft_sampling")
+    target = target_logits if target_logits.stride(-1) == 1 else target_logits.contiguous()
+    draft = draft_logits if draft_logits.stride(-1) == 1 else draft_logits.contiguous()
+    tokens = tokens.contiguous()
+    out = torch.empty(B, G1, dtype=torch.int64, device=target.device)
+    accepted = torch.empty(B, dtype=torch.int32, device=target.device)
+    p = _lib.SpecVerifyParams()
+    p.target, p.t_stride_b, p.t_stride_row = target.data_ptr(), target.stride(0), target.stride(1)
+    p.draft, p.d_stride_b, p.d_stride_row = draft.data_ptr(), draft.stride(0), draft.stride(1)
+    if G1 == 2:   # a dimension of size 1 may carry any stride: the kernel never steps along it
+        p.d_stride_row = max(p.d_stride_row, V)
+    if B == 1:
+        p.t_stride_b, p.d_stride_b = max(p.t_stride_b, V), max(p.d_stride_b, V)
+    p.tokens, p.seeds, p.positions = tokens.data_ptr(), seeds.data_ptr(), positions.data_ptr()
+    p.B, p.G, p.V = B, G1 - 1, V
+    p.dtype = _lib.PCV_F32 if target.dtype == torch.float32 else _pcv_dtype(target.dtype)
+    p.draft_dtype = p.dtype
+    p.temperature, p.top_k, p.top_p = t, k, p_
+    p.draft_temperature, p.draft_top_k, p.draft_top_p = dt, dk, dp
+    p.out_tokens, p.accepted = out.data_ptr(), accepted.data_ptr()
+    lib = _lib.lib()
+    if not lib.pcv_spec_verify_supported(C.byref(p)):
+        raise ValueError(f"spec_verify: {lib.pcv_last_error().decode()}")
+    with torch.cuda.device(target.device):
+        check(lib.pcv_spec_verify(C.byref(p), _stream()), "pcv_spec_verify")
+    return out, accepted
+
+
+def spec_uniforms(seeds: torch.Tensor, positions: torch.Tensor, stream: str = "accept") -> torch.Tensor:
+    """The 64 bits (as int64) of :func:`spec_verify`'s ``stream`` ("accept" or "residual") at these seeds (B,) and
+    positions (B,) or (B, k) — pcv_spec_uniforms."""
+    if stream not in _SPEC_STREAMS:
+        raise ValueError(f"spec_uniforms: stream must be 'accept' or 'residual', got {stream!r}")
+    lead = tuple(positions.shape)
+    if len(lead) not in (1, 2):
+        raise ValueError(f"spec_uniforms: positions must be (B,) or (B, k), got {lead}")
+    seeds, positions = _sample_counters(seeds, positions, lead, "spec_uniforms")
+    out = torch.empty(lead, dtype=torch.int64, device=positions.device)
+    with torch.cuda.device(positions.device):
+        check(_lib.lib().pcv_spec_uniforms(out.data_ptr(), seeds.data_ptr(), positions.data_ptr(), positions.numel(),
+                                           1 if len(lead) == 1 else lead[1], _SPEC_STREAMS[stream], _stream()),
+              "pcv_spec_uniforms")
     return out
 
 
