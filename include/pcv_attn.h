@@ -37,7 +37,7 @@
 extern "C" {
 #endif
 
-#define PCV_ABI_VERSION 1
+#define PCV_ABI_VERSION 2
 
 #if defined(__GNUC__)
 #define PCV_API __attribute__((visibility("default")))
@@ -383,18 +383,11 @@ PCV_API int pcv_attn_bwd_supported(const pcv_attn_bwd_params* p);
 PCV_API int pcv_attn_bwd_workspace_bytes(const pcv_attn_bwd_params* p, size_t* bytes);
 PCV_API int pcv_attn_bwd(const pcv_attn_bwd_params* p, void* stream);
 /*
- * Training forward WITH attention-probability dropout (modules.py:161, nn.Dropout on the softmax output).  Second pass
- * after a write_partial pcv_attn_fwd over all keys (whose part_m / part_l are `stat_m` / `stat_l`): recomputes the
- * probabilities tile by tile, drops each element (b, h, query, key) with probability round(256 p)/256 — a pure function of
- * (dropout_seed, b, h, query, key), regenerated by pcv_attn_bwd from the same seed — scales the survivors by 1/(1 - p) and
- * writes out = dropout(P) V into p->out.  p->workspace must hold pcv_attn_fwd_dropout_workspace_bytes().  Head dims:
- * multiples of 8, at most 128; no key sharding.  pcv_attn_dropout_mask exports the keep mask (B, H, N, M) as bytes
- * (tests / debugging).
+ * The keep mask of attention-probability dropout (modules.py:161, nn.Dropout on the softmax output) as (B, H, N, M)
+ * bytes, 1 = the element survives (tests / debugging).  Each element (b, h, query, key) is dropped with probability
+ * round(256 p)/256 by a pure function of (dropout_seed, b, h, query, key): the mask pcv_attn_fwd_partial_dropout applies
+ * and pcv_attn_bwd regenerates from the same seed.
  */
-PCV_API int pcv_attn_fwd_dropout_supported(const pcv_attn_params* p, float dropout_p);
-PCV_API int pcv_attn_fwd_dropout_workspace_bytes(const pcv_attn_params* p, size_t* bytes);
-PCV_API int pcv_attn_fwd_dropout(const pcv_attn_params* p, const float* stat_m, const float* stat_l, float dropout_p,
-                                 uint64_t dropout_seed, void* stream);
 PCV_API int pcv_attn_dropout_mask(uint8_t* keep, int32_t B, int32_t H, int32_t N, int32_t M, float dropout_p,
                                   uint64_t dropout_seed, void* stream);
 /*

@@ -41,9 +41,6 @@ EXPORTS = (
     "pcv_attn_bwd_supported",
     "pcv_attn_bwd_workspace_bytes",
     "pcv_attn_bwd",
-    "pcv_attn_fwd_dropout_supported",
-    "pcv_attn_fwd_dropout_workspace_bytes",
-    "pcv_attn_fwd_dropout",
     "pcv_attn_dropout_mask",
     "pcv_attn_dropout_mask_range",
     "pcv_attn_fwd_partial_dropout_supported",
@@ -384,13 +381,6 @@ def lib() -> C.CDLL:
         l.pcv_attn_bwd_workspace_bytes.restype = C.c_int
         l.pcv_attn_bwd.argtypes = [C.POINTER(AttnBwdParams), C.c_void_p]
         l.pcv_attn_bwd.restype = C.c_int
-        l.pcv_attn_fwd_dropout_supported.argtypes = [C.POINTER(AttnParams), C.c_float]
-        l.pcv_attn_fwd_dropout_supported.restype = C.c_int
-        l.pcv_attn_fwd_dropout_workspace_bytes.argtypes = [C.POINTER(AttnParams), C.POINTER(C.c_size_t)]
-        l.pcv_attn_fwd_dropout_workspace_bytes.restype = C.c_int
-        l.pcv_attn_fwd_dropout.argtypes = [C.POINTER(AttnParams), C.c_void_p, C.c_void_p, C.c_float, C.c_uint64,
-                                           C.c_void_p]
-        l.pcv_attn_fwd_dropout.restype = C.c_int
         l.pcv_attn_dropout_mask.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_float,
                                             C.c_uint64, C.c_void_p]
         l.pcv_attn_dropout_mask.restype = C.c_int
@@ -487,8 +477,8 @@ def lib() -> C.CDLL:
                      "pcv_attn_fwd", "pcv_attn_combine", "pcv_rotary_apply", "pcv_kv_append",
                      "pcv_partial_rescale"):
             getattr(l, name).restype = C.c_int
-        if l.pcv_abi_version() != 1:
-            raise PcvError(f"libpcv_attn ABI version {l.pcv_abi_version()} != 1 expected by the Python host")
+        if l.pcv_abi_version() != 2:
+            raise PcvError(f"libpcv_attn ABI version {l.pcv_abi_version()} != 2 expected by the Python host")
         _lib = l
         return _lib
 

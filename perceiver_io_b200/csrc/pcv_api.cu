@@ -345,25 +345,6 @@ int pcv_attn_bwd_shard(const pcv_attn_bwd_params* p, const pcv_key_shard* s, voi
   return launch_attn_bwd(*p, s, reinterpret_cast<cudaStream_t>(stream));
 }
 
-int pcv_attn_fwd_dropout_supported(const pcv_attn_params* p, float dropout_p) {
-  if (p == nullptr) return 0;
-  const char* why = "";
-  const bool ok = attn_fwd_dropout_supported(*p, dropout_p, &why);
-  if (!ok) set_error("attn_fwd_dropout not applicable: %s", why);
-  return ok ? 1 : 0;
-}
-
-int pcv_attn_fwd_dropout_workspace_bytes(const pcv_attn_params* p, size_t* bytes) {
-  PCV_REQUIRE(p != nullptr, PCV_ERR_INVALID, "attn_fwd_dropout_workspace_bytes: params is NULL");
-  return attn_fwd_dropout_workspace_bytes(*p, bytes);
-}
-
-int pcv_attn_fwd_dropout(const pcv_attn_params* p, const float* stat_m, const float* stat_l, float dropout_p,
-                         uint64_t dropout_seed, void* stream) {
-  PCV_REQUIRE(p != nullptr, PCV_ERR_INVALID, "attn_fwd_dropout: params is NULL");
-  return launch_attn_fwd_dropout(*p, stat_m, stat_l, dropout_p, dropout_seed, reinterpret_cast<cudaStream_t>(stream));
-}
-
 int pcv_attn_dropout_mask(uint8_t* keep, int32_t B, int32_t H, int32_t N, int32_t M, float dropout_p,
                           uint64_t dropout_seed, void* stream) {
   return launch_dropout_mask(keep, B, H, N, 0, M, dropout_p, dropout_seed, reinterpret_cast<cudaStream_t>(stream));

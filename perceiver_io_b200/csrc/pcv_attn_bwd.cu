@@ -1,5 +1,5 @@
 // pcv_attn_bwd.cu — training kernels of the fused attention core on the Hopper tensor cores (SURVEY.md §8(f)2):
-// backward (C ABI pcv_attn_bwd) and attention-probability dropout (pcv_attn_fwd_dropout, pcv_attn_dropout_mask).
+// backward (C ABI pcv_attn_bwd, with attention-probability dropout) and the dropout mask export (pcv_attn_dropout_mask).
 //
 // Reference: autograd through perceiver/model/core/modules.py:141-167 (einsum scores, masked_fill_ with the finite
 // fill, softmax, dropout, einsum with V).  With P = softmax(scale * Q K^T + fill), O = P V and the saved row statistics
@@ -16,8 +16,7 @@
 //   bwd_dq_kernel    query-tile outer.  One CTA owns (b, h, 128 queries) and a range of key tiles (K and V streamed
 //                    through a TMA ring); S = Q K^T, dP = dO V^T, dS in registers, dQ += dS K (K tile read MN-major,
 //                    as V is in the forward).  dQ accumulates in registers over the CTA's key range and is added into an
-//                    fp32 buffer once per CTA.  With FWD it is the second forward pass of a training step with dropout:
-//                    O += dropout(P) V from the saved statistics (no running maximum).
+//                    fp32 buffer once per CTA.
 //
 // Head dims above 128 (up to 192: a third 64-channel box) run the dK/dV kernel as a dV pass and a dK pass and the dQ
 // kernel as bwd_dq64_kernel (64-key stages, ordered fp32 partials instead of atomics); see there.
@@ -63,7 +62,6 @@ struct BwdParams {
   uint32_t seed_lo, seed_hi;
   int key_base;              // global index of local key 0 (even; 0 unless key-sharded): the mask hashes key_base + j
   float drop_rp;             // 1 / (1 - drop_thresh / 256)
-  float* o32;                // forward-with-dropout kernel: (B, N, H*dv) fp32 accumulation buffer
   int total_tiles;           // dkdv kernel: B*H*nk
   int splits, tiles_per_split;  // dq kernel
 };
@@ -110,8 +108,7 @@ __global__ void __launch_bounds__(256) bwd_prep_kernel(const T* __restrict__ out
     const T* o = out + b * o_sb + (int64_t)n * o_sn + h * o_sh;
     const T* g = dout + b * g_sb + (int64_t)n * g_sn + h * g_sh;
     float acc = 0.f;
-    if (dout != nullptr)
-      for (int c = lane; c < dv; c += 32) acc += Elem<T>::to_f(o[c]) * Elem<T>::to_f(g[c]);
+    for (int c = lane; c < dv; c += 32) acc += Elem<T>::to_f(o[c]) * Elem<T>::to_f(g[c]);
     delta = warp_sum(acc);
     const int64_t r = bh * N + n;
     const float m = stat_m[r], l = stat_l[r];
@@ -158,8 +155,8 @@ struct Cfg1 {
   static constexpr int kSmem = kKVBytes + kSlots * kStage + 2048;
 };
 
-// kernel 2 (dQ) and 3 (forward with dropout): CTA = (b, h, 128 queries, key range); warpgroups 1-2 own 64 queries each;
-// Q (and dO) stay resident, K / V tiles stream through a TMA ring.
+// kernel 2 (dQ): CTA = (b, h, 128 queries, key range); warpgroups 1-2 own 64 queries each; Q and dO stay resident,
+// K / V tiles stream through a TMA ring.
 template <int NQB, int NVB>
 struct Cfg2 {
   static constexpr int kQBytes = (NQB + NVB) * kBoxBytes;
@@ -375,8 +372,8 @@ bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq64, const __grid_constant_
   }
 }
 
-// FWD = false: dQ += scale * dS K, reduced into p.dq32.   FWD = true: O += dropout(P) V, reduced into p.o32.
-template <int NQB, int NVB, bool BF16, bool FWD>
+// dQ += scale * dS K, reduced into p.dq32
+template <int NQB, int NVB, bool BF16>
 __global__ void __launch_bounds__(kThreads, 1)
 bwd_dq_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
               const __grid_constant__ CUtensorMap tv, const __grid_constant__ CUtensorMap tdo, const BwdParams p) {
@@ -405,10 +402,9 @@ bwd_dq_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CU
   if (wg == 0) {
     reg_dealloc<40>();
     if (threadIdx.x == 0) {
-      mbar_arrive_expect_tx(&bar.fix_full, (FWD ? NQB : NQB + NVB) * kBoxBytes);
+      mbar_arrive_expect_tx(&bar.fix_full, C::kQBytes);
       for (int c = 0; c < NQB; ++c) tma_load_4d(sQ + c * kBoxBytes, &tq, &bar.fix_full, c * 64, qt * kT, h, p.q_bcast ? 0 : b);
-      if (!FWD)
-        for (int c = 0; c < NVB; ++c) tma_load_4d(sdO + c * kBoxBytes, &tdo, &bar.fix_full, c * 64, qt * kT, h, b);
+      for (int c = 0; c < NVB; ++c) tma_load_4d(sdO + c * kBoxBytes, &tdo, &bar.fix_full, c * 64, qt * kT, h, b);
       uint32_t it = 0;
       for (int kt = kt0; kt < kt1; ++kt, ++it) {
         const uint32_t s = it % NS;
@@ -441,10 +437,9 @@ bwd_dq_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CU
     delta[i] = blk[stat_delta_idx(r)];
     fillp[i] = blk[stat_fillp_idx(r)];
   }
-  constexpr int NA = FWD ? NVB : NQB;  // accumulator boxes: O (v channels) or dQ (qk channels)
-  float acc[NA][32];
+  float acc[NQB][32];
 #pragma unroll
-  for (int c = 0; c < NA; ++c)
+  for (int c = 0; c < NQB; ++c)
 #pragma unroll
     for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
   mbar_wait(&bar.fix_full, 0, 32);
@@ -453,24 +448,22 @@ bwd_dq_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CU
     const uint32_t s = it % NS;
     const uint32_t stk = ring + s * C::kStage, stv = stk + NQB * kBoxBytes;
     mbar_wait(&bar.full[s], (it / NS) & 1, 33);
-    float sc[64], dp[FWD ? 1 : 64];
+    float sc[64], dp[64];
     wgmma_fence();
 #pragma unroll
     for (int c = 0; c < NQB; ++c)
 #pragma unroll
       for (int kk = 0; kk < 4; ++kk)
         wgmma_ss<128, BF16>(sc, make_desc(q_base + c * kBoxBytes + kk * 32), make_desc(stk + c * kBoxBytes + kk * 32), (c | kk) != 0);
-    if constexpr (!FWD) {
 #pragma unroll
-      for (int c = 0; c < NVB; ++c)
+    for (int c = 0; c < NVB; ++c)
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk)
-          wgmma_ss<128, BF16>(dp, make_desc(do_base + c * kBoxBytes + kk * 32), make_desc(stv + c * kBoxBytes + kk * 32), (c | kk) != 0);
-    }
+      for (int kk = 0; kk < 4; ++kk)
+        wgmma_ss<128, BF16>(dp, make_desc(do_base + c * kBoxBytes + kk * 32), make_desc(stv + c * kBoxBytes + kk * 32), (c | kk) != 0);
     wgmma_commit();
     wgmma_wait<0>();
     fence_regs(sc);
-    if constexpr (!FWD) fence_regs(dp);
+    fence_regs(dp);
     uint32_t a[8][4];
 #pragma unroll
     for (int g = 0; g < 16; ++g) {
@@ -487,45 +480,38 @@ bwd_dq_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CU
           const uint32_t jg = (uint32_t)(p.key_base + j);
           keep = drop_keep(drop_bits(p.seed_lo, p.seed_hi, (uint32_t)bh, (uint32_t)n, jg), n, jg, p.drop_thresh);
         }
-        if constexpr (FWD) {
-          val[e4] = keep ? P * p.drop_rp : 0.f;
-        } else {
-          const float dP = keep ? dp[4 * g + e4] * p.drop_rp : 0.f;
-          val[e4] = (oob || filled) ? 0.f : P * (dP - delta[i]);
-        }
+        const float dP = keep ? dp[4 * g + e4] * p.drop_rp : 0.f;
+        val[e4] = (oob || filled) ? 0.f : P * (dP - delta[i]);
       }
       a[g >> 1][(g & 1) * 2 + 0] = pack2(val[0], val[1], BF16);
       a[g >> 1][(g & 1) * 2 + 1] = pack2(val[2], val[3], BF16);
     }
     wgmma_fence();
 #pragma unroll
-    for (int c = 0; c < NA; ++c)
+    for (int c = 0; c < NQB; ++c)
 #pragma unroll
-      for (int kk = 0; kk < 8; ++kk)
-        wgmma_rs<64, BF16>(acc[c], a[kk], make_desc((FWD ? stv : stk) + c * kBoxBytes + kk * 2048));
+      for (int kk = 0; kk < 8; ++kk) wgmma_rs<64, BF16>(acc[c], a[kk], make_desc(stk + c * kBoxBytes + kk * 2048));
     wgmma_commit();
     wgmma_wait<0>();
 #pragma unroll
-    for (int c = 0; c < NA; ++c) fence_regs(acc[c]);
+    for (int c = 0; c < NQB; ++c) fence_regs(acc[c]);
     warp_arrive(&bar.empty[s]);
   }
   // reduce this CTA's share into the fp32 buffer
-  const int width = FWD ? p.dv : p.dqk;
-  const float mul = FWD ? 1.f : p.scale;
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     const int n = nrow[i];
     if (n >= p.N) continue;
-    const int bq = FWD ? b : (p.q_bcast ? 0 : b);
-    float* dst = (FWD ? p.o32 : p.dq32) + (((int64_t)bq * p.N + n) * p.H + h) * width;
+    const int bq = p.q_bcast ? 0 : b;
+    float* dst = p.dq32 + (((int64_t)bq * p.N + n) * p.H + h) * p.dqk;
 #pragma unroll
-    for (int c = 0; c < NA; ++c)
+    for (int c = 0; c < NQB; ++c)
 #pragma unroll
       for (int g = 0; g < 8; ++g) {
         const int col = c * 64 + 8 * g + cq;
-        if (col < width) {
-          atomicAdd(dst + col, acc[c][4 * g + 2 * i] * mul);
-          atomicAdd(dst + col + 1, acc[c][4 * g + 2 * i + 1] * mul);
+        if (col < p.dqk) {
+          atomicAdd(dst + col, acc[c][4 * g + 2 * i] * p.scale);
+          atomicAdd(dst + col + 1, acc[c][4 * g + 2 * i + 1] * p.scale);
         }
       }
   }
@@ -747,37 +733,33 @@ bool wide_bwd(int dqk, int dv) { return dqk > 128 || dv > 128; }
 // and so the workspace size, follow from the problem alone, and so does the order in which dQ is summed.
 constexpr int kWideSplitSms = 132;
 
-// Workspace of the backward and of the dropout forward: the row-statistics blocks, an fp32 accumulator of acc_bytes
-// (dQ of the backward, O of the dropout forward; zeroed before the kernels), the pad bits, then part_bytes of dQ
-// partials (the wide backward; written whole by its dQ kernel, so not zeroed).
+// Workspace of the backward: the row-statistics blocks, an fp32 dQ accumulator of acc_bytes (zeroed before the
+// kernels; none for a key shard's or the wide backward), the pad bits, then part_bytes of dQ partials (the wide
+// backward; written whole by its dQ kernel, so not zeroed).
 struct BwdLayout {
   int Npad, nq, nk;
   int dq_splits, dq_tiles_per_split, dq_parts;  // the wide backward's dQ split and partial count (else 0)
   size_t acc_bytes, off_acc, off_pad, part_bytes, off_part, total;  // the statistics start at offset 0
 };
 
-BwdLayout bwd_layout(int B, int H, int N, int M, bool pad, size_t acc_bytes) {
-  BwdLayout L;
-  L.nq = (N + kT - 1) / kT;
-  L.nk = (M + kT - 1) / kT;
-  L.Npad = L.nq * kT;
-  L.dq_splits = L.dq_tiles_per_split = L.dq_parts = 0;
-  L.acc_bytes = acc_bytes;
-  L.off_acc = align256((size_t)kStatsBytes * B * H * 2 * L.nq);
-  L.off_pad = L.off_acc + align256(acc_bytes);
-  L.part_bytes = 0;
-  L.off_part = L.total = L.off_pad + (pad ? align256(sizeof(uint32_t) * (size_t)B * pad_words_per_row(M)) : 0);
-  return L;
-}
-
 // shard != nullptr: a key shard's backward, whose dQ kernel up to head dim 128 accumulates straight into the caller's
 // fp32 grad_q32 (no accumulator in the workspace)
 BwdLayout bwd_layout(const pcv_attn_bwd_params& a, const pcv_key_shard* shard) {
   const int Bq = a.q_stride_b == 0 ? 1 : a.B;
   const size_t dq_bytes = sizeof(float) * (size_t)Bq * a.N * a.H * a.dqk;
-  if (!wide_bwd(a.dqk, a.dv))
-    return bwd_layout(a.B, a.H, a.N, a.M, a.pad_mask != nullptr, shard != nullptr ? 0 : dq_bytes);
-  BwdLayout L = bwd_layout(a.B, a.H, a.N, a.M, a.pad_mask != nullptr, 0);
+  const bool wide = wide_bwd(a.dqk, a.dv);
+  BwdLayout L;
+  L.nq = (a.N + kT - 1) / kT;
+  L.nk = (a.M + kT - 1) / kT;
+  L.Npad = L.nq * kT;
+  L.dq_splits = L.dq_tiles_per_split = L.dq_parts = 0;
+  L.acc_bytes = wide || shard != nullptr ? 0 : dq_bytes;
+  L.off_acc = align256((size_t)kStatsBytes * a.B * a.H * 2 * L.nq);
+  L.off_pad = L.off_acc + align256(L.acc_bytes);
+  L.part_bytes = 0;
+  L.off_part = L.total =
+      L.off_pad + (a.pad_mask != nullptr ? align256(sizeof(uint32_t) * (size_t)a.B * pad_words_per_row(a.M)) : 0);
+  if (!wide) return L;
   dq_split(a.B * a.H * L.nq, L.nk, kWideSplitSms, L.dq_tiles_per_split, L.dq_splits);
   L.dq_parts = (Bq == 1 ? a.B : 1) * L.dq_splits;  // a batch-1 q receives one contribution per batch row and split
   L.part_bytes = dq_bytes * L.dq_parts;
@@ -785,31 +767,17 @@ BwdLayout bwd_layout(const pcv_attn_bwd_params& a, const pcv_key_shard* shard) {
   return L;
 }
 
-BwdLayout fwd_drop_layout(const pcv_attn_params& a) {
-  return bwd_layout(a.B, a.H, a.N, a.M, a.pad_mask != nullptr, sizeof(float) * (size_t)a.B * a.N * a.H * a.dv);
-}
-
-// operands of delta = rowsum(dO * O) in bwd_prep_kernel; left null when only the statistics are wanted
-struct DeltaOperands {
-  const void* out = nullptr;
-  const void* dout = nullptr;
-  int64_t o_sb = 0, o_sn = 0, o_sh = 0, g_sb = 0, g_sn = 0, g_sh = 0;
-};
-
 struct BwdMaps {
-  CUtensorMap q, k, v;            // 128-row boxes
-  CUtensorMap dout, q64, dout64;  // backward only; the dK/dV kernel stages Q and dO in 64-row boxes
-  CUtensorMap k64, v64;           // wide backward only; bwd_dq64_kernel stages K and V in 64-row boxes
+  CUtensorMap q, k, v, dout;  // 128-row boxes
+  CUtensorMap q64, dout64;    // the dK/dV kernel stages Q and dO in 64-row boxes
+  CUtensorMap k64, v64;       // wide backward only; bwd_dq64_kernel stages K and V in 64-row boxes
 };
 
-// The host steps the backward and the dropout forward share; A is pcv_attn_bwd_params or pcv_attn_params, which name
-// the q / k / v operands alike.  Fills the BwdParams core and the dq-kernel split, zeroes the fp32 accumulator, writes
-// the row statistics, packs the pad mask and encodes the q / k / v tensor maps.  The call's keys are [m_offset,
-// m_offset + M) of m_total (the causal diagonal and the dropout hash use global key indices).
-template <class A>
-int bwd_setup(const A& a, const BwdLayout& L, const float* stat_m, const float* stat_l, const DeltaOperands& d,
-              float dropout_p, uint64_t seed, int m_total, int m_offset, cudaStream_t stream, BwdParams& p, BwdMaps& m,
-              int& sms) {
+// Fills the BwdParams core and the dq-kernel split, zeroes the fp32 accumulator, writes the row statistics, packs the
+// pad mask and encodes the q / k / v tensor maps.  The call's keys are [m_offset, m_offset + M) of m_total (the causal
+// diagonal and the dropout hash use global key indices).
+int bwd_setup(const pcv_attn_bwd_params& a, const BwdLayout& L, int m_total, int m_offset, cudaStream_t stream,
+              BwdParams& p, BwdMaps& m, int& sms) {
   int dev = 0;
   PCV_CHECK_CUDA(cudaGetDevice(&dev));
   PCV_CHECK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
@@ -826,7 +794,7 @@ int bwd_setup(const A& a, const BwdLayout& L, const float* stat_m, const float* 
   p.cshift = (m_total - a.N) - m_offset;
   p.key_base = m_offset;
   p.stats = reinterpret_cast<const float*>(ws);
-  set_dropout(p, dropout_p, seed);
+  set_dropout(p, a.dropout_p, a.dropout_seed);
   if (L.dq_splits > 0) {
     p.tiles_per_split = L.dq_tiles_per_split;
     p.splits = L.dq_splits;
@@ -841,12 +809,14 @@ int bwd_setup(const A& a, const BwdLayout& L, const float* stat_m, const float* 
     float* stats = reinterpret_cast<float*>(ws);
     if (a.dtype == PCV_BF16)
       bwd_prep_kernel<__nv_bfloat16><<<blocks, 256, 0, stream>>>(
-          reinterpret_cast<const __nv_bfloat16*>(d.out), reinterpret_cast<const __nv_bfloat16*>(d.dout), stat_m, stat_l,
-          stats, a.B, a.H, a.N, L.Npad, a.dv, d.o_sb, d.o_sn, d.o_sh, d.g_sb, d.g_sn, d.g_sh);
+          reinterpret_cast<const __nv_bfloat16*>(a.out), reinterpret_cast<const __nv_bfloat16*>(a.grad_out), a.stat_m,
+          a.stat_l, stats, a.B, a.H, a.N, L.Npad, a.dv, a.o_stride_b, a.o_stride_n, a.o_stride_h, a.go_stride_b,
+          a.go_stride_n, a.go_stride_h);
     else
       bwd_prep_kernel<__half><<<blocks, 256, 0, stream>>>(
-          reinterpret_cast<const __half*>(d.out), reinterpret_cast<const __half*>(d.dout), stat_m, stat_l, stats, a.B,
-          a.H, a.N, L.Npad, a.dv, d.o_sb, d.o_sn, d.o_sh, d.g_sb, d.g_sn, d.g_sh);
+          reinterpret_cast<const __half*>(a.out), reinterpret_cast<const __half*>(a.grad_out), a.stat_m, a.stat_l,
+          stats, a.B, a.H, a.N, L.Npad, a.dv, a.o_stride_b, a.o_stride_n, a.o_stride_h, a.go_stride_b, a.go_stride_n,
+          a.go_stride_h);
     PCV_CHECK_CUDA(cudaGetLastError());
     count_launch();
   }
@@ -866,25 +836,22 @@ int bwd_setup(const A& a, const BwdLayout& L, const float* stat_m, const float* 
   return make_tmap_4d(&m.v, a.v, a.dtype, a.dv, a.M, a.H, a.B, a.v_stride_m, a.v_stride_h, a.v_stride_b, kT);
 }
 
-// FWD: the dropout forward (bwd_dq_kernel in its FWD form).  Else the backward: the dK/dV kernel, then the dQ kernel.
+// the dK/dV kernel, then the dQ kernel
 template <int NQB, int NVB, bool BF16>
-int launch_tc_kernels(bool fwd, const BwdMaps& m, const BwdParams& p, int sms, cudaStream_t stream) {
-  using C2 = Cfg2<NQB, NVB>;
-  const dim3 grid2(p.B * p.H * p.nq * p.splits);
-  if (fwd)  // no dO in the forward pass
-    return launch_kernel(bwd_dq_kernel<NQB, NVB, BF16, true>, grid2, kThreads, C2::kSmem, 0, stream, m.q, m.k, m.v, m.v, p);
+int launch_tc_kernels(const BwdMaps& m, const BwdParams& p, int sms, cudaStream_t stream) {
   const int rc = launch_kernel(bwd_dkdv_kernel<NQB, NVB, BF16>, dim3(std::min(p.total_tiles, sms)), kThreads,
                                Cfg1<NQB, NVB>::kSmem, 0, stream, m.q64, m.k, m.v, m.dout64, p);
   if (rc != PCV_OK) return rc;
-  return launch_kernel(bwd_dq_kernel<NQB, NVB, BF16, false>, grid2, kThreads, C2::kSmem, 0, stream, m.q, m.k, m.v, m.dout, p);
+  return launch_kernel(bwd_dq_kernel<NQB, NVB, BF16>, dim3(p.B * p.H * p.nq * p.splits), kThreads, Cfg2<NQB, NVB>::kSmem,
+                       0, stream, m.q, m.k, m.v, m.dout, p);
 }
 
 // head dims up to 64 take one 64-channel box, up to 128 two
 template <bool BF16>
-int launch_tc(bool fwd, const BwdMaps& m, const BwdParams& p, int sms, cudaStream_t stream) {
+int launch_tc(const BwdMaps& m, const BwdParams& p, int sms, cudaStream_t stream) {
   if (p.dqk <= 64)
-    return p.dv <= 64 ? launch_tc_kernels<1, 1, BF16>(fwd, m, p, sms, stream) : launch_tc_kernels<1, 2, BF16>(fwd, m, p, sms, stream);
-  return p.dv <= 64 ? launch_tc_kernels<2, 1, BF16>(fwd, m, p, sms, stream) : launch_tc_kernels<2, 2, BF16>(fwd, m, p, sms, stream);
+    return p.dv <= 64 ? launch_tc_kernels<1, 1, BF16>(m, p, sms, stream) : launch_tc_kernels<1, 2, BF16>(m, p, sms, stream);
+  return p.dv <= 64 ? launch_tc_kernels<2, 1, BF16>(m, p, sms, stream) : launch_tc_kernels<2, 2, BF16>(m, p, sms, stream);
 }
 
 // The wide backward (a head dim above 128): the dK/dV kernel as a dV pass and a dK pass, then bwd_dq64_kernel into the
@@ -999,13 +966,11 @@ int launch_attn_bwd(const pcv_attn_bwd_params& a, const pcv_key_shard* shard, cu
               "attn_bwd: workspace too small (%zu < %zu)", a.workspace_bytes, L.total);
   PCV_REQUIRE((reinterpret_cast<uintptr_t>(a.workspace) & 255u) == 0, PCV_ERR_INVALID,
               "attn_bwd: workspace must be 256-byte aligned");
-  const DeltaOperands d{a.out, a.grad_out, a.o_stride_b, a.o_stride_n, a.o_stride_h,
-                        a.go_stride_b, a.go_stride_n, a.go_stride_h};
   BwdParams p{};
   BwdMaps m;
   int sms = 0;
   const int m_total = shard != nullptr ? shard->m_total : a.M, m_offset = shard != nullptr ? shard->m_offset : 0;
-  int rc = bwd_setup(a, L, a.stat_m, a.stat_l, d, a.dropout_p, a.dropout_seed, m_total, m_offset, stream, p, m, sms);
+  int rc = bwd_setup(a, L, m_total, m_offset, stream, p, m, sms);
   if (rc != PCV_OK) return rc;
   const bool wide = wide_bwd(a.dqk, a.dv);
   const int Bq = a.q_stride_b == 0 ? 1 : a.B;
@@ -1046,62 +1011,12 @@ int launch_attn_bwd(const pcv_attn_bwd_params& a, const pcv_key_shard* shard, cu
     return launch_sum_dq(a.dtype, p.dq32, L.dq_parts, a.grad_q, Bq, a.N, a.H, a.dqk, a.gq_stride_b, a.gq_stride_n,
                          a.gq_stride_h, stream);
   }
-  rc = bf16 ? launch_tc<true>(false, m, p, sms, stream) : launch_tc<false>(false, m, p, sms, stream);
+  rc = bf16 ? launch_tc<true>(m, p, sms, stream) : launch_tc<false>(m, p, sms, stream);
   if (rc != PCV_OK || shard != nullptr) return rc;
   return launch_cast(bf16, p.dq32, a.grad_q, Bq, a.N, a.H, a.dqk, a.gq_stride_b, a.gq_stride_n, a.gq_stride_h, stream);
 }
 
-// ---- forward with attention dropout + mask export --------------------------------------------------------------
-bool attn_fwd_dropout_supported(const pcv_attn_params& a, float dropout_p, const char** why) {
-  auto no = [&](const char* w) {
-    if (why) *why = w;
-    return false;
-  };
-  if (a.dtype != PCV_BF16 && a.dtype != PCV_F16) return no("dtype must be bf16 or fp16");
-  if (a.B < 1 || a.H < 1 || a.N < 1 || a.M < 1) return no("empty problem");
-  if (a.dqk < 8 || a.dv < 8 || a.dqk > 128 || a.dv > 128 || a.dqk % 8 || a.dv % 8)
-    return no("head dims must be multiples of 8 in [8, 128]");
-  if (!(dropout_p > 0.f && dropout_p < 1.f)) return no("dropout_p must be in (0, 1)");
-  if (a.m_total != a.M || a.m_offset != 0 || a.write_partial) return no("sharded / partial calls take no dropout");
-  if (!al16(a.q) || !al16(a.k) || !al16(a.v)) return no("tensors must be 16-byte aligned");
-  const int64_t strides[] = {a.q_stride_b, a.q_stride_n, a.q_stride_h, a.k_stride_b, a.k_stride_m,
-                             a.k_stride_h, a.v_stride_b, a.v_stride_m, a.v_stride_h};
-  for (int64_t st : strides)
-    if (st % 8) return no("strides must be multiples of 8 elements");
-  if (const char* w = device_problem()) return no(w);
-  return true;
-}
-
-int attn_fwd_dropout_workspace_bytes(const pcv_attn_params& a, size_t* bytes) {
-  PCV_REQUIRE(bytes != nullptr, PCV_ERR_INVALID, "attn_fwd_dropout_workspace_bytes: bytes is NULL");
-  *bytes = fwd_drop_layout(a).total;
-  return PCV_OK;
-}
-
-int launch_attn_fwd_dropout(const pcv_attn_params& a, const float* stat_m, const float* stat_l, float dropout_p,
-                            uint64_t seed, cudaStream_t stream) {
-  const char* why = "";
-  PCV_REQUIRE(attn_fwd_dropout_supported(a, dropout_p, &why), PCV_ERR_UNSUPPORTED, "attn_fwd_dropout: %s", why);
-  PCV_REQUIRE(stat_m != nullptr && stat_l != nullptr && a.out != nullptr, PCV_ERR_INVALID,
-              "attn_fwd_dropout: statistics / output pointer is NULL");
-  const BwdLayout L = fwd_drop_layout(a);
-  PCV_REQUIRE(a.workspace != nullptr && a.workspace_bytes >= L.total, PCV_ERR_WORKSPACE,
-              "attn_fwd_dropout: workspace too small (%zu < %zu)", a.workspace_bytes, L.total);
-  PCV_REQUIRE((reinterpret_cast<uintptr_t>(a.workspace) & 255u) == 0, PCV_ERR_INVALID,
-              "attn_fwd_dropout: workspace must be 256-byte aligned");
-  BwdParams p{};
-  BwdMaps m;
-  int sms = 0;
-  // statistics only (no delta): out / grad_out are not read
-  int rc = bwd_setup(a, L, stat_m, stat_l, DeltaOperands{}, dropout_p, seed, a.M, 0, stream, p, m, sms);
-  if (rc != PCV_OK) return rc;
-  p.o32 = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(a.workspace) + L.off_acc);
-  const bool bf16 = a.dtype == PCV_BF16;
-  rc = bf16 ? launch_tc<true>(true, m, p, sms, stream) : launch_tc<false>(true, m, p, sms, stream);
-  if (rc != PCV_OK) return rc;
-  return launch_cast(bf16, p.o32, a.out, a.B, a.N, a.H, a.dv, a.o_stride_b, a.o_stride_n, a.o_stride_h, stream);
-}
-
+// ---- dropout mask export ---------------------------------------------------------------------------------------
 int launch_dropout_mask(uint8_t* keep, int B, int H, int N, int key_begin, int key_end, float dropout_p, uint64_t seed,
                         cudaStream_t stream) {
   PCV_REQUIRE(keep != nullptr && B > 0 && H > 0 && N > 0 && key_begin >= 0 && key_end > key_begin, PCV_ERR_INVALID,

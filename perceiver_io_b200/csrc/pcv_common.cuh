@@ -165,10 +165,6 @@ int launch_ln_linear_bwd(const pcv_ln_linear_bwd_params& p, cudaStream_t stream)
 bool attn_bwd_supported(const pcv_attn_bwd_params& p, const pcv_key_shard* shard, const char** why);
 int attn_bwd_workspace_bytes(const pcv_attn_bwd_params& p, const pcv_key_shard* shard, size_t* bytes);
 int launch_attn_bwd(const pcv_attn_bwd_params& p, const pcv_key_shard* shard, cudaStream_t stream);
-bool attn_fwd_dropout_supported(const pcv_attn_params& p, float dropout_p, const char** why);
-int attn_fwd_dropout_workspace_bytes(const pcv_attn_params& p, size_t* bytes);
-int launch_attn_fwd_dropout(const pcv_attn_params& p, const float* stat_m, const float* stat_l, float dropout_p,
-                            uint64_t seed, cudaStream_t stream);
 int launch_dropout_mask(uint8_t* keep, int B, int H, int N, int key_begin, int key_end, float dropout_p, uint64_t seed,
                         cudaStream_t stream);
 // token sampling (pcv_sample.cu)

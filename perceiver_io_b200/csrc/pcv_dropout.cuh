@@ -1,6 +1,6 @@
 // pcv_dropout.cuh — the attention-probability dropout mask (modules.py:161: nn.Dropout on the softmax output), shared
-// by the one-pass dropout forward (attn_fwd_drop_kernel, pcv_attn_tc.cu), the backward kernels and the second-pass
-// dropout forward (pcv_attn_bwd.cu) and the mask export (pcv_attn_dropout_mask / pcv_attn_dropout_mask_range).
+// by the dropout forward (attn_fwd_drop_kernel, pcv_attn_tc.cu), the backward kernels (pcv_attn_bwd.cu) and the mask
+// export (pcv_attn_dropout_mask / pcv_attn_dropout_mask_range).
 // oracle/dropout_oracle.py restates it in numpy.
 //
 // Counter-based: the keep decision of element (b, h, query q, key k) is a pure function of (seed, b*H+h, q, k), so every

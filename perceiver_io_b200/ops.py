@@ -337,7 +337,8 @@ def attention_backward(q, k, v, out, grad_out, stat_m, stat_l, num_heads: int, s
     ``out`` is the forward output, ``stat_m`` / ``stat_l`` the (B, H, N) row statistics of ``attention_partial`` over all
     keys.  grad_q has q's batch size (a batch-1 ``q`` shared by the batch receives the sum).  ``check_only`` launches
     nothing and returns whether the kernels cover these operands.  ``dropout_p`` / ``dropout_seed``: the values the
-    forward (``attention_dropout_forward``) ran with — the kernels regenerate its mask."""
+    dropout forward (``attention_partial`` or ``attention_dropout_forward``) ran with — the kernels regenerate its
+    mask."""
     return _backward(q, k, v, out, grad_out, stat_m, stat_l, num_heads, scale, pad_mask, causal, dropout_p, dropout_seed,
                      mode="check" if check_only else "run", pad=False)
 
@@ -386,23 +387,22 @@ def new_dropout_seed() -> int:
 
 def attention_dropout_forward(q, k, v, stat_m, stat_l, num_heads: int, scale: float, dropout_p: float, dropout_seed: int,
                               pad_mask=None, causal: bool = False, check_only: bool = False):
-    """out = dropout(softmax(...)) V for training (reference modules.py:161), second pass after ``attention_partial``
-    over all keys (``stat_m`` / ``stat_l`` = its part_m / part_l): pcv_attn_fwd_dropout.  The keep decision of every
+    """out = dropout(softmax(...)) V for training (reference modules.py:161): the dropout forward of
+    ``attention_partial`` (pcv_attn_fwd_partial_dropout) over all keys, then ``combine_partials``.  The kernel recomputes
+    the row statistics, so ``stat_m`` / ``stat_l`` (the (B, H, N) part_m / part_l of ``attention_partial`` over all
+    keys) are only checked, when given, to be the statistics the backward would take.  The keep decision of every
     (b, h, query, key) is a pure function of ``dropout_seed`` (``dropout_keep_mask`` exports it); the drop probability is
     ``dropout_p`` rounded to 1/256.  ``check_only``: launch nothing, return whether the kernel covers the operands."""
     out_dtype = q.dtype
     q, k, v, _ = _prep(q, k, v)
     _require_cuda(stat_m, stat_l, pad_mask)
-    with torch.cuda.device(k.device):
-        p, keep = _fill_attn_params(q, k, v, num_heads, scale, pad_mask, causal, None, 0, "auto")
-        if check_only:
-            return bool(_lib.lib().pcv_attn_fwd_dropout_supported(C.byref(p), float(dropout_p)))
-        _check_stats(p, stat_m, stat_l)
-        out = _new_output(p, q.dtype, k.device)
-        ws = _workspace(p, k.device, "pcv_attn_fwd_dropout", C.byref(p))
-        check(_lib.lib().pcv_attn_fwd_dropout(C.byref(p), stat_m.data_ptr(), stat_l.data_ptr(), float(dropout_p),
-                                              int(dropout_seed), _stream()), "pcv_attn_fwd_dropout")
-    del keep, ws
+    if check_only:
+        return _partial_dropout_supported(q, k, v, num_heads, pad_mask, causal, dropout_p, "auto")
+    if stat_m is not None or stat_l is not None:
+        _check_stats(_fill_attn_params(q, k, v, num_heads, scale, pad_mask, causal, None, 0, "auto")[0], stat_m, stat_l)
+    po, pm, pl = attention_partial(q, k, v, num_heads, scale, pad_mask=pad_mask, causal=causal, dropout_p=dropout_p,
+                                   dropout_seed=dropout_seed)
+    out = combine_partials(po[None], pm[None], pl[None], q.dtype)
     return out if out.dtype == out_dtype else out.to(out_dtype)
 
 
@@ -435,7 +435,7 @@ def _dropout_scale(dropout_p: float) -> float:
 
 
 def _partial_dropout_supported(q, k, v, num_heads: int, pad_mask, causal: bool, dropout_p: float, impl: str) -> bool:
-    """Whether the one-pass dropout forward (attention_partial with dropout_p > 0) takes these prepared operands."""
+    """Whether the dropout forward (attention_partial with dropout_p > 0) takes these prepared operands."""
     with torch.cuda.device(k.device):
         p, keep = _fill_attn_params(q, k, v, num_heads, 1.0, pad_mask, causal, None, 0, impl)
         dummy = torch.empty(16, device=k.device)
@@ -446,9 +446,8 @@ def _partial_dropout_supported(q, k, v, num_heads: int, pad_mask, causal: bool, 
 
 class _FusedAttention(torch.autograd.Function):
     """Forward = the fused CUDA kernel (partial-state mode, so the row max and denominator are kept).  With dropout:
-    the partial forward and the second-pass dropout kernel (``attention_dropout_forward``) where that covers the call
-    (head dims that are multiples of 8 up to 128), else the one-pass dropout forward (``attention_partial`` with
-    ``dropout_p``) for every head dim the forward takes.
+    the dropout forward (``attention_partial`` with ``dropout_p``) on the single-CTA tensor-core kernel, whichever other
+    kernel ``impl`` names, for every head dim that kernel takes.
     Backward = the tensor-core backward kernels (pcv_attn_bwd: dK/dV and dQ kernels, SURVEY.md §8(f) rank 2) for head
     dims up to 192; head dims that are not multiples of 8 are zero-padded as in the forward (``_backward``).  Other
     shapes (head dims above 192, the decode forward) take the labelled SHIM below: the
@@ -468,24 +467,18 @@ class _FusedAttention(torch.autograd.Function):
             return out
         # head dims that are not multiples of 8 are zero-padded, so that the statistics exist for the backward kernels
         qc, kc, vc, dims = _prep(q, k, v, num_heads=num_heads, pad=True)
-        if dropout_p > 0.0 and dims is None and attention_dropout_forward(
-                qc, kc, vc, None, None, num_heads, scale, dropout_p, dropout_seed, pad_mask, causal, check_only=True):
-            # statistics from the fused kernel, then the dropout pass (second kernel) writes the output
-            pm, pl = attention_partial(qc, kc, vc, num_heads, scale, pad_mask=pad_mask, causal=causal, impl=impl)[1:]
-            out = attention_dropout_forward(qc, kc, vc, pm, pl, num_heads, scale, dropout_p, dropout_seed, pad_mask,
-                                            causal)
-        else:
-            # one pass: the (dropped) numerator and the dropout-free statistics, merged by the combine kernel
-            if dropout_p > 0.0 and not _partial_dropout_supported(qc, kc, vc, num_heads, pad_mask, causal, dropout_p,
-                                                                  impl):
+        if dropout_p > 0.0:
+            impl = impl if impl == "tcgen05" else "auto"  # only the single-CTA tensor-core kernel takes dropout
+            if not _partial_dropout_supported(qc, kc, vc, num_heads, pad_mask, causal, dropout_p, impl):
                 raise NotImplementedError("attention dropout is not available for this call: "
                                           + _lib.lib().pcv_last_error().decode())
-            po, pm, pl = attention_partial(qc, kc, vc, num_heads, scale, pad_mask=pad_mask, causal=causal, impl=impl,
-                                           dropout_p=dropout_p, dropout_seed=dropout_seed)
-            out = combine_partials(po[None], pm[None], pl[None], qc.dtype)
-            del po
-            if dims is not None:
-                out = _unpad_heads(out, num_heads, dims[1])
+        # the (dropped) numerator and the dropout-free statistics, merged by the combine kernel
+        po, pm, pl = attention_partial(qc, kc, vc, num_heads, scale, pad_mask=pad_mask, causal=causal, impl=impl,
+                                       dropout_p=dropout_p, dropout_seed=dropout_seed)
+        out = combine_partials(po[None], pm[None], pl[None], qc.dtype)
+        del po
+        if dims is not None:
+            out = _unpad_heads(out, num_heads, dims[1])
         out = out if out.dtype == q.dtype else out.to(q.dtype)
         ctx.save_for_backward(q, k, v, pad_mask, out, pm, pl)
         return out
@@ -603,7 +596,7 @@ def attention_partial(q, k, v, num_heads: int, scale: float, pad_mask=None, caus
     """One M-shard's un-normalised softmax state: (part_o (B,H,N,dv) f32, part_m (B,H,N), part_l (B,H,N)).
 
     ``k``/``v``/``pad_mask`` hold this shard's keys [m_offset, m_offset+M) of ``m_total``.  ``out`` may
-    supply the three (contiguous, float32) destination tensors.  ``dropout_p`` > 0: the one-pass dropout forward
+    supply the three (contiguous, float32) destination tensors.  ``dropout_p`` > 0: the dropout forward
     (pcv_attn_fwd_partial_dropout, or pcv_attn_fwd_partial_dropout_shard on a key shard, m_offset even) — part_o is
     the numerator with the mask of ``dropout_keep_mask`` over the shard's global key range applied and scaled by
     1/(1-p), part_m / part_l stay the dropout-free statistics."""

@@ -3,8 +3,7 @@ shared by its GPU tests (test_gpu_bwd_variants.py) and their CPU companion (test
 needs a GPU.
 
 launch_attn_bwd instantiates, with NQB = pad64(dqk) / 64 and NVB = pad64(dv) / 64 boxes of 64 channels, bf16 or fp16:
-  - head dims up to 128 (launch_tc): bwd_dkdv_kernel<NQB, NVB, BF16, kOutBoth> and bwd_dq_kernel<NQB, NVB, BF16, false>;
-    the dropout forward (launch_attn_fwd_dropout) runs bwd_dq_kernel<NQB, NVB, BF16, true>;
+  - head dims up to 128 (launch_tc): bwd_dkdv_kernel<NQB, NVB, BF16, kOutBoth> and bwd_dq_kernel<NQB, NVB, BF16>;
   - a head dim above 128 (launch_wide, NQB or NVB = 3): bwd_dkdv_kernel<.., kOutDV> (the dV pass),
     bwd_dkdv_kernel<.., kOutDK> (the dK pass) and bwd_dq64_kernel<NQB, NVB, BF16>.
 Every kernel below keeps a TMA ring of NS stages whose phase runs on across the persistent kernels' tiles / work items;
@@ -31,21 +30,17 @@ def is_wide(dqk, dv):
 
 
 # ---- the instantiations one call reaches ----
-def variants_of(dqk, dv, dt, fwd_dropout=True):
-    """Kernel symbols (name, NQB, NVB, dtype, flag) a backward (and, up to 128, a dropout forward) with these head dims
-    launches.  flag: OUT of bwd_dkdv_kernel (0 both, 1 dV, 2 dK), FWD of bwd_dq_kernel, None for bwd_dq64_kernel."""
+def variants_of(dqk, dv, dt):
+    """Kernel symbols (name, NQB, NVB, dtype, flag) a backward with these head dims launches.  flag: OUT of
+    bwd_dkdv_kernel (0 both, 1 dV, 2 dK), None for bwd_dq_kernel and bwd_dq64_kernel."""
     nq, nv = boxes(dqk), boxes(dv)
     if is_wide(dqk, dv):
         return {("dkdv", nq, nv, dt, 1), ("dkdv", nq, nv, dt, 2), ("dq64", nq, nv, dt, None)}
-    out = {("dkdv", nq, nv, dt, 0), ("dq", nq, nv, dt, False)}
-    if fwd_dropout:
-        out.add(("dq", nq, nv, dt, True))
-    return out
+    return {("dkdv", nq, nv, dt, 0), ("dq", nq, nv, dt, None)}
 
 
 def reachable_variants():
-    """Every instantiation launch_attn_bwd / launch_attn_fwd_dropout can reach: head dims 8..192 in multiples of 8
-    (attn_bwd_supported; the dropout forward takes 8..128)."""
+    """Every instantiation launch_attn_bwd can reach: head dims 8..192 in multiples of 8 (attn_bwd_supported)."""
     out = set()
     for dqk, dv in itertools.product(range(8, 193, 8), repeat=2):
         for dt in DTYPES:

@@ -32,9 +32,12 @@ def test_every_declared_symbol_is_exported():
         assert hasattr(lib, name), name
 
 
-def test_abi_version_and_error_string_without_gpu():
+def test_abi_version_2_and_error_string_without_gpu():
     lib = _lib.lib()
-    assert lib.pcv_abi_version() == 1
+    assert lib.pcv_abi_version() == 2
+    # no second-pass dropout forward: pcv_attn_fwd_partial_dropout + pcv_attn_combine are the dropout forward
+    for name in ("pcv_attn_fwd_dropout", "pcv_attn_fwd_dropout_supported", "pcv_attn_fwd_dropout_workspace_bytes"):
+        assert not hasattr(lib, name), name
     # argument validation happens before any CUDA call, so it is testable on a CPU-only box
     rc = lib.pcv_attn_fwd(None, None)
     assert rc == 1
@@ -103,8 +106,8 @@ def test_product_package_never_imports_the_oracle():
                 assert not re.search(r"^\s*(from|import)\s+oracle\b", text, re.M), f
 
 
-def test_training_entry_points_validate_before_any_cuda_call():
-    """pcv_attn_bwd / pcv_attn_fwd_dropout / pcv_attn_dropout_mask reject bad arguments on a CPU-only box (no launch)."""
+def test_backward_and_mask_entry_points_validate_before_any_cuda_call():
+    """pcv_attn_bwd / pcv_attn_dropout_mask reject bad arguments on a CPU-only box (no launch)."""
     lib = _lib.lib()
     assert lib.pcv_attn_bwd(None, None) == 1 and b"NULL" in lib.pcv_last_error()
     assert lib.pcv_attn_bwd_supported(None) == 0
@@ -118,7 +121,5 @@ def test_training_entry_points_validate_before_any_cuda_call():
     stats = 768 * 2 * 4 * 4
     dq32 = 4 * 2 * 200 * 4 * 64
     assert need.value == (stats + 255) // 256 * 256 + (dq32 + 255) // 256 * 256
-    assert lib.pcv_attn_fwd_dropout(None, None, None, ctypes.c_float(0.1), ctypes.c_uint64(1), None) == 1
-    assert lib.pcv_attn_fwd_dropout_supported(None, ctypes.c_float(0.1)) == 0
     assert lib.pcv_attn_dropout_mask(None, 1, 1, 8, 8, ctypes.c_float(0.1), ctypes.c_uint64(1), None) == 1
     assert b"dropout_mask" in lib.pcv_last_error()

@@ -15,10 +15,10 @@ def _lib_blob():
         return f.read()
 
 
-def test_library_holds_exactly_the_intended_backward_instantiations():
+def test_library_holds_exactly_the_backward_instantiations():
     """bwd_dkdv_kernel<NQB, NVB, BF16, OUT>: the single-pass kernels (OUT 0) for NQB, NVB <= 2; for the five box pairs
-    with a third box, a dV pass (OUT 1) and a dK pass (OUT 2).  bwd_dq_kernel<NQB, NVB, BF16, FWD> stays at <= 2 boxes
-    (with the dropout-forward form); bwd_dq64_kernel<NQB, NVB, BF16> covers the five wide pairs."""
+    with a third box, a dV pass (OUT 1) and a dK pass (OUT 2).  bwd_dq_kernel<NQB, NVB, BF16> stays at <= 2 boxes;
+    bwd_dq64_kernel<NQB, NVB, BF16> covers the five wide pairs."""
     blob = _lib_blob()
     small = {(q, v) for q in (1, 2) for v in (1, 2)}
     wide = {(q, v) for q in (1, 2, 3) for v in (1, 2, 3)} - small
@@ -27,9 +27,8 @@ def test_library_holds_exactly_the_intended_backward_instantiations():
             for a, b, c, o in re.findall(rb"15bwd_dkdv_kernelILi(\d)ELi(\d)ELb([01])ELi(\d)EEEv", blob)}
     assert dkdv == ({(q, v, bf, 0) for q, v in small for bf in (False, True)}
                     | {(q, v, bf, o) for q, v in wide for bf in (False, True) for o in (1, 2)})
-    dq = {(int(a), int(b), c == b"1", f == b"1")
-          for a, b, c, f in re.findall(rb"13bwd_dq_kernelILi(\d)ELi(\d)ELb([01])ELb([01])EEEv", blob)}
-    assert dq == {(q, v, bf, fwd) for q, v in small for bf in (False, True) for fwd in (False, True)}
+    dq = {(int(a), int(b), c == b"1") for a, b, c in re.findall(rb"13bwd_dq_kernelILi(\d)ELi(\d)ELb([01])EEEv", blob)}
+    assert dq == {(q, v, bf) for q, v in small for bf in (False, True)}
     dq64 = {(int(a), int(b), c == b"1") for a, b, c in re.findall(rb"15bwd_dq64_kernelILi(\d)ELi(\d)ELb([01])EEEv", blob)}
     assert dq64 == {(q, v, bf) for q, v in wide for bf in (False, True)}
 

@@ -22,7 +22,7 @@ LOG2E = 1.4426950408889634
 def test_matrix_reaches_every_instantiation():
     covered = set().union(*(variants_of(dqk, dv, dt) for dqk, dv, dt in VARIANT_CASES))
     reach = reachable_variants()
-    assert len(reach) == 2 * (4 * 3 + 5 * 3)  # 4 small pairs x (dK/dV, dQ, dropout forward), 5 wide x 3 kernels
+    assert len(reach) == 2 * (4 * 2 + 5 * 3)  # 4 small pairs x (dK/dV, dQ), 5 wide x 3 kernels
     assert covered == reach, sorted(reach - covered, key=str)
     # head dims that are not multiples of 64 everywhere: every box has a zero-filled tail
     assert all(dqk % 64 and dv % 64 for dqk, dv, _ in VARIANT_CASES)
@@ -213,52 +213,6 @@ def test_whole_tensor_gate_has_no_yardstick_below_three_keys():
     assert min(over[(1, "bf16")], over[(1, "fp16")]) >= 50  # unless the two fp32 sums happen to round alike
     assert over[(2, "bf16")] + over[(2, "fp16")] > 0
     assert over[(3, "bf16")] == over[(3, "fp16")] == 0
-
-
-def emulate_dropout_forward(q, k, v, H, scale, pad, causal, dtype, keep, rp):
-    """bwd_dq_kernel<.., true> (the second-pass dropout forward): P = 2^(t + nlse) in fp32 from the fp32 statistics
-    (fillp on a row without a live key), P * keep / (1 - p) rounded to 16 bits, fp32 accumulation, the output rounded."""
-    f32 = torch.float32
-    B, M, N = k.shape[0], k.shape[1], q.shape[1]
-    qh = q.to(f32).expand(B, -1, -1).reshape(B, N, H, -1).transpose(1, 2)
-    kh = k.to(f32).reshape(B, M, H, -1).transpose(1, 2)
-    vh = v.to(f32).reshape(B, M, H, -1).transpose(1, 2)
-    filled = _filled(B, N, M, pad, causal).expand(B, H, N, M)
-    t = (qh @ kh.transpose(-1, -2)) * f32_(scale * LOG2E)
-    dead = filled.all(-1, keepdim=True)
-    m = torch.where(dead, torch.zeros(()), t.masked_fill(filled, -math.inf).amax(-1, keepdim=True))
-    l = torch.where(dead, torch.full_like(m, float(M)), torch.exp2(t - m).masked_fill(filled, 0.0).sum(-1, keepdim=True))
-    P = torch.exp2(t - (m + torch.log2(l)))
-    P = torch.where(filled, torch.where(dead, 1.0 / l, torch.zeros_like(l)).expand_as(P), P)
-    o = _round(_round(P * keep.to(f32) * rp, dtype) @ vh, dtype)
-    return o.transpose(1, 2).reshape(B, N, -1)
-
-
-@pytest.mark.parametrize("dt", ["bf16", "fp16"])
-def test_dropout_forward_row_gate_on_the_emulated_arithmetic(dt):
-    """The GPU module's dropout-forward case (batch-1 q, about 30 % of the keys padded and poisoned, batch row 1 wholly
-    padded) on the emulated kernel arithmetic, under gpu_util.assert_rows, the per-row derived gate of the forward
-    tests: the bound of a row is twice eager's error on that row, and the kernel rounds P / (1 - p) once where eager
-    rounds P and then P / (1 - p), so the two errors are of one size and the worst of ~2400 rows sits well up
-    towards the bound."""
-    from gpu_util import assert_rows
-    from test_gpu_dropout import _core_drop
-
-    dtype = DTYPE[dt]
-    B, N, M, H = 3, 200, 300, 2
-    worst = 0.0
-    for dqk, dv in ((40, 56), (120, 120)):
-        pad = _pad(B, M, seed=8)
-        q, k, v, _ = _poisoned(B, N, M, H, dqk, dv, dtype, seed=9, poison=pad, bcast=True)
-        for p in (0.1, 0.5):
-            keep = torch.rand(B, H, N, M, generator=torch.Generator().manual_seed(10)) >= p
-            rp = 1.0 / (1.0 - p)
-            for causal in (False, True):
-                got = emulate_dropout_forward(q, k, v, H, dqk ** -0.5, pad, causal, dtype, keep, rp)
-                ref = _core_drop(q, k, v, H, dqk ** -0.5, pad, causal, torch.float64, keep, rp)
-                eager = _core_drop(q, k, v, H, dqk ** -0.5, pad, causal, dtype, keep, rp)
-                worst = max(worst, assert_rows(got, ref, eager, H, f"emulated {dt} qk{dqk} v{dv} p {p} causal {causal}"))
-    print(f"[dropout forward rows] {dt}: emulated worst err/bound {worst:.3f}")
 
 
 # ---- the gate: power against the bugs it is meant to see ----

@@ -1,5 +1,6 @@
-"""-m gpu: every instantiation of the attention backward (bwd_dkdv_kernel, bwd_dq_kernel, bwd_dq64_kernel; the dropout
-forward bwd_dq_kernel<.., true>) at its schedule, tile and mask edges, against fp64 autograd of the reference algorithm.
+"""-m gpu: every instantiation of the attention backward (bwd_dkdv_kernel, bwd_dq_kernel, bwd_dq64_kernel) at its
+schedule, tile and mask edges, against fp64 autograd of the reference algorithm, and the dropout forward at the same
+head dims up to 128.
 The matrix and the schedule shapes live in bwd_variants.py; test_bwd_variants_cpu.py checks that the matrix covers every
 instantiation, that the shapes have their plan structure, and that the gate is calibrated and sees the bugs it is for.
 
@@ -261,7 +262,7 @@ def test_causal_diagonal_sweep(case):
 
 
 # --------------------------------------------------------------------------------------------------
-# dropout on the exported mask: the backward, and the FWD form of bwd_dq_kernel (attention_dropout_forward)
+# dropout on the exported mask: the backward, and the dropout forward (attention_dropout_forward)
 # --------------------------------------------------------------------------------------------------
 DROP_BWD = [(40, 120, "bf16"), (184, 56, "bf16"), (120, 56, "fp16"), (40, 184, "fp16")]
 

@@ -97,6 +97,16 @@ CASES = [
 
 @pytest.mark.parametrize("case", CASES, ids=[f"B{c[0]}N{c[1]}M{c[2]}H{c[3]}d{c[4]}x{c[5]}{c[6] or ''}{'c' if c[7] else ''}{'b' if c[8] else ''}p{c[9]}" for c in CASES])
 def test_dropout_forward_and_backward_match_reference_on_the_exported_mask(case):
+    _check_against_reference(case, "auto")
+
+
+@pytest.mark.parametrize("impl", ["auto", "tcgen05", "tcgen05_pair", "simt"])
+def test_every_impl_takes_dropout(impl):
+    """The dropout forward runs on the single-CTA tensor-core kernel whichever forward kernel ``impl`` names."""
+    _check_against_reference(CASES[1], impl)
+
+
+def _check_against_reference(case, impl):
     B, N, M, H, dqk, dv, pad_kind, causal, bcast, p = case
     q, k, v, go, pad = _inputs(B, N, M, H, dqk, dv, pad_kind, bcast, seed=5)
     scale = dqk ** -0.5
@@ -107,7 +117,8 @@ def test_dropout_forward_and_backward_match_reference_on_the_exported_mask(case)
     qq, kk, vv = (t.detach().clone().requires_grad_() for t in (q, k, v))
     ops.backward_config["impl"] = "kernel"
     try:
-        out = ops.attention(qq, kk, vv, H, scale, pad_mask=pad, causal=causal, dropout_p=p, dropout_seed=seed)
+        out = ops.attention(qq, kk, vv, H, scale, pad_mask=pad, causal=causal, impl=impl, dropout_p=p,
+                            dropout_seed=seed)
         out.backward(go)
     finally:
         ops.backward_config["impl"] = "auto"
@@ -117,10 +128,11 @@ def test_dropout_forward_and_backward_match_reference_on_the_exported_mask(case)
     bound, eager_err, ref_max = derived_bound(r64[0], e16[0])
     bound = max(bound, FLOOR * ref_max)
     err = (out.double() - r64[0]).abs().max().item()
-    print(f"[dropout parity] {case} out: err {err:.3e} bound {bound:.3e} (eager {eager_err:.3e}, max|ref| {ref_max:.3e})")
+    print(f"[dropout parity] {case} {impl} out: err {err:.3e} bound {bound:.3e} (eager {eager_err:.3e}, "
+          f"max|ref| {ref_max:.3e})")
     assert err <= bound, f"out: err {err:.3e} > bound {bound:.3e}"
     mags = grad_magnitudes(q, k, v, go, H, scale, pad, causal, keep, rp)
-    assert_grad_set((qq.grad, kk.grad, vv.grad), r64[1:], e16[1:], mags, q.dtype, f"dropout {case}")
+    assert_grad_set((qq.grad, kk.grad, vv.grad), r64[1:], e16[1:], mags, q.dtype, f"dropout {case} {impl}")
 
 
 def test_module_dropout_train_and_eval():

@@ -1,5 +1,5 @@
 """-m gpu: the one-pass dropout forward (attn_fwd_drop_kernel, ops.attention_partial with dropout_p) and the backward
-shim with dropout, for the head dims the second-pass dropout kernel does not take (above 128, or not multiples of 8).
+shim with dropout, at head dims above 128 or not multiples of 8.
 
 - The kernel leaves the softmax statistics alone: part_m / part_l equal the dropout-free kernel's bit for bit.
 - The mask it applies is the exported one: with q = 0 every score is 0, so with v = e_(j mod dv) part_o counts the kept
@@ -112,15 +112,22 @@ def _pid(c):
 
 
 @pytest.mark.parametrize("case", PARITY, ids=_pid)
-def test_forward_and_gradients_match_the_reference_on_the_exported_mask(case):
+def test_one_pass_forward_and_gradients_match_the_reference_on_the_exported_mask(case, monkeypatch):
     B, N, M, H, dqk, dv, pad_kind, causal, bcast, p, dtype = case
     q, k, v, go, pad = _inputs(B, N, M, H, dqk, dv, pad_kind, bcast, seed=7, dtype=dtype)
     scale = dqk ** -0.5
-    assert not ops.attention_dropout_forward(q, k, v, None, None, H, scale, p, SEED, pad, causal, check_only=True)
     keep = ops.dropout_keep_mask(B, H, N, M, p, SEED)
     _, rp = _rp(p)
+    partial, drops = ops.attention_partial, []
+
+    def recording_partial(*args, **kwargs):
+        drops.append(kwargs.get("dropout_p", 0.0))
+        return partial(*args, **kwargs)
+
+    monkeypatch.setattr(ops, "attention_partial", recording_partial)
     qq, kk, vv = (t.detach().clone().requires_grad_() for t in (q, k, v))
     out = ops.attention(qq, kk, vv, H, scale, pad_mask=pad, causal=causal, dropout_p=p, dropout_seed=SEED)
+    assert drops == [p]  # the one-pass route: one partial forward, with the mask applied
     out.backward(go)
 
     r64, eager = (_drop_ref(q, k, v, go, H, scale, pad, causal, dt, keep, rp) for dt in (torch.float64, dtype))

@@ -71,7 +71,7 @@ def main():
     res["bwd_launches_per_call"] = (_lib.launch_count() - n0) / (a.steps + 3)
     res["bwd_kernel_tflops_algorithmic"] = 2.5 * flops_fwd / res["bwd_kernel_ms"] * 1e-9
     res["bwd_kernel_tflops_executed"] = 3.5 * flops_fwd / res["bwd_kernel_ms"] * 1e-9
-    # training step with attention dropout 0.1: statistics pass + dropout pass forward, backward regenerating the mask
+    # training step with attention dropout 0.1: the dropout forward, the backward regenerating the mask
     res["fwd_dropout_pass_ms"] = timed(
         lambda: ops.attention_dropout_forward(q, k, v, pm, pl, H, scale, 0.1, 1234), a.steps)
     res["bwd_dropout_kernel_ms"] = timed(

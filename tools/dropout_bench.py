@@ -1,10 +1,9 @@
 """Times the attention-dropout training paths and prints one JSON line (with the card's name and power limit):
 
-- north-star shape (B=8, N=512, M=65536, H=8, head dim 128): the partial forward, the second-pass dropout kernel
-  (attention_dropout_forward) and the one-pass dropout forward (attention_partial with dropout_p), side by side, so
-  the two dropout forwards can be compared, and the dropout backward on the tensor-core kernels;
-- the masked-LM recipe's encoder cross-attention (B=64, N=256, M=2048, H=8, head dims 32 / 160): the partial forward,
-  the one-pass dropout forward and the backward through the torch shim.
+- north-star shape (B=8, N=512, M=65536, H=8, head dim 128): the dropout-free partial forward, the dropout forward
+  (attention_partial with dropout_p) and the dropout backward on the tensor-core kernels;
+- the masked-LM recipe's encoder cross-attention (B=64, N=256, M=2048, H=8, head dims 32 / 160): the dropout-free
+  partial forward, the dropout forward and the backward under autograd.
 
 Run on the GPU box: python tools/dropout_bench.py [--steps 20] [--p 0.1]"""
 import argparse
@@ -72,10 +71,8 @@ def main():
     res["north_star"] = {
         "shape": {"B": B, "N": N, "M": M, "H": H, "dqk": d, "dv": d},
         "partial_forward_ms": timed(lambda: ops.attention_partial(q, k, v, H, scale), a.steps),
-        "second_pass_dropout_ms": timed(lambda: ops.attention_dropout_forward(q, k, v, pm, pl, H, scale, p, seed),
-                                        a.steps),
-        "one_pass_dropout_forward_ms": timed(lambda: ops.attention_partial(q, k, v, H, scale, dropout_p=p,
-                                                                           dropout_seed=seed), a.steps),
+        "dropout_forward_ms": timed(lambda: ops.attention_partial(q, k, v, H, scale, dropout_p=p, dropout_seed=seed),
+                                    a.steps),
         "backward_kernels_ms": timed(lambda: ops.attention_backward(q, k, v, out, go, pm, pl, H, scale, dropout_p=p,
                                                                     dropout_seed=seed), a.steps),
     }
@@ -86,12 +83,12 @@ def main():
     scale = dqk ** -0.5
     with torch.no_grad():
         ms_part = timed(lambda: ops.attention_partial(q, k, v, H, scale), a.steps)
-        ms_one = timed(lambda: ops.attention_partial(q, k, v, H, scale, dropout_p=p, dropout_seed=seed), a.steps)
+        ms_drop = timed(lambda: ops.attention_partial(q, k, v, H, scale, dropout_p=p, dropout_seed=seed), a.steps)
     out = ops.attention(q, k, v, H, scale, dropout_p=p, dropout_seed=seed)
     res["mlm_encoder_cross_attention"] = {
         "shape": {"B": B, "N": N, "M": M, "H": H, "dqk": dqk, "dv": dv},
-        "partial_forward_ms": ms_part, "one_pass_dropout_forward_ms": ms_one,
-        "backward_shim_ms": timed(lambda: out.backward(go, retain_graph=True), a.steps),
+        "partial_forward_ms": ms_part, "dropout_forward_ms": ms_drop,
+        "backward_ms": timed(lambda: out.backward(go, retain_graph=True), a.steps),
     }
     print(json.dumps(res), flush=True)
 
