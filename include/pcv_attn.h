@@ -735,6 +735,96 @@ PCV_API int pcv_spec_uniforms(uint64_t* out, const uint64_t* seeds, const int32_
                               int32_t rows_per_batch, int32_t stream_id, void* stream);
 
 /*
+ * Beam search: pcv_beam_step runs one step of the Hugging Face GenerationMixin._beam_search (do_sample=False, no logits
+ * processors) for B items of K beams each, on state buffers that live on the device.  Beam k of item b is logits row
+ * b*K + k.  E = n_eos, beams_to_keep = max(2, E + 1) * K (as the Hugging Face code keeps them).  For each item:
+ *   1. logp = log_softmax(fp32 logits) per beam row: d_i = (double)x_i - (double)max, S = Σ exp(d_i) in fp64,
+ *      logp_i = fp32(d_i - log S);
+ *   2. acc = fp32(running_scores[b, k] + logp); the top beams_to_keep of the K*V values by score descending, then flat
+ *      index k*V + token ascending (the tie rule);
+ *   3. a candidate hits the stopping criteria if its token is an EOS id or it is the max_length-th generated token
+ *      (generated count + 1 >= max_length);
+ *   4. running beams: hitting candidates get -1e9 added (fp32) and the top K (ties by candidate position) give
+ *      next_tokens, parents (global beam rows b*K + parent beam) and the running scores;
+ *   5. finished set: of the first K candidates those that just hit are eligible; scores are divided in fp32 by
+ *      fp32(pow(g, length_penalty)) (fp64 pow of the fp64 penalty, g = generated count + 1), get -1e9 if early_stopping is TRUE and the
+ *      item's K finished flags are all set, -1e9 if the item's early-stop heuristic is satisfied, -1e9 if not eligible,
+ *      and are merged with the K finished entries; the top K are kept, ties by position in [finished | candidates];
+ *   6. the early-stop heuristic (sticky) on the new state, as the Hugging Face code computes it, and the item's done
+ *      flag: heuristic satisfied, or early_stopping TRUE and every finished flag set.
+ * Token histories (running and finished, hist_len columns per beam) are gathered by parent; column `generated count`
+ * takes the new token.  The last item CTA to finish sets counters[2] = every item done and counters[0] += 1.  The
+ * generated count and max_length are read from counters when the kernels run, so one recorded CUDA graph serves every
+ * step.  Initial state: running scores 0 for beam 0 and -1e9 for the others, finished scores -1e9, flags 0, histories
+ * filled with the output fill value, item_flags {1, 0}, counters {0, max_length, 0, 0}.  Two launches (one CTA per
+ * beam row, one per item), no host read, integer atomics only; an item's result is a pure function of its logit bits
+ * and state.  Refusals (NULL pointers, V outside [1, PCV_SAMPLE_MAX_VOCAB], K outside [1, PCV_BEAM_MAX_BEAMS], n_eos
+ * outside [0, PCV_BEAM_MAX_EOS], K*V < beams_to_keep, an EOS id outside [0, V), a non-finite length_penalty, an
+ * unknown early_stopping code or dtype, stride_row < V, overlapping outputs) come before any CUDA call, with the reason
+ * in pcv_last_error.
+ */
+#define PCV_BEAM_MAX_BEAMS 8
+#define PCV_BEAM_MAX_EOS 4
+enum pcv_early_stopping { PCV_EARLY_STOP_FALSE = 0, PCV_EARLY_STOP_TRUE = 1, PCV_EARLY_STOP_NEVER = 2 };
+
+typedef struct pcv_beam_step_params {
+  const void* logits;          /* (B*K, V) rows of `dtype` (PCV_BF16 / PCV_F16 / PCV_F32), unit element stride */
+  int64_t stride_row;          /* elements between rows, >= V                                                  */
+  double length_penalty;       /* fp64, as the Hugging Face code raises the length to it                       */
+  int32_t B, K, V, dtype;
+  int32_t n_eos;
+  int32_t eos[PCV_BEAM_MAX_EOS];
+  int32_t early_stopping;      /* pcv_early_stopping                                                           */
+  int32_t hist_len;            /* columns of every history row (>= max_length)                                 */
+  float* running_scores;       /* (B, K) state                                                                  */
+  float* finished_scores;      /* (B, K) state                                                                  */
+  int32_t* finished_flags;     /* (B, K) state                                                                  */
+  int64_t* running_hist;       /* (B, K, hist_len) state                                                        */
+  int64_t* finished_hist;      /* (B, K, hist_len) state                                                        */
+  int64_t* hist_scratch;       /* (B, 2K, hist_len) scratch                                                     */
+  int32_t* item_flags;         /* (B, 2) state: [early-stop heuristic not satisfied, item done]                 */
+  int32_t* counters;           /* 4 int32s: [generated count, max_length, every item done, arrivals (0)]        */
+  float* cand_scores;          /* (B*K, beams_to_keep) scratch                                                  */
+  int32_t* cand_index;         /* (B*K, beams_to_keep) scratch                                                  */
+  int64_t* next_tokens;        /* (B*K) out                                                                     */
+  int32_t* parents;            /* (B*K) out: the global beam row each beam continues                            */
+} pcv_beam_step_params;
+
+/* 1 if pcv_beam_step takes these params, else 0 (reason via pcv_last_error) */
+PCV_API int pcv_beam_step_supported(const pcv_beam_step_params* p);
+PCV_API int pcv_beam_step(const pcv_beam_step_params* p, void* stream);
+
+/*
+ * pcv_kv_gather_rows: after a beam step, every beam row i with parents[i] != i takes its parent's generated rows.  For
+ * every arena of the device table and every such row i, rows [first_row, cur) with cur = rows->bounds[i *
+ * bounds_stride_b + bounds_col] (clamped to first_row + max_rows) are copied from row parents[i] into row i, through
+ * the entry's scratch (parent -> scratch, then scratch -> child, two launches), so cycles and many-to-one moves read
+ * only the rows as they were before the call.  Rows whose parent is themselves, rows before first_row or at / past cur,
+ * and every other arena byte are untouched.  The grid is (n_entries, R) whatever the bounds: the call can be recorded
+ * in a CUDA graph.  Each entry's arena and scratch are 16-byte aligned, row_bytes and the strides multiples of 16, and
+ * the scratch holds max_rows rows per beam row (the caller builds the table; only the params are checked).
+ */
+typedef struct pcv_kv_gather_entry {
+  void* arena;                 /* batch row 0, arena row 0                                                      */
+  void* scratch;               /* beam row 0's max_rows rows                                                    */
+  int64_t arena_stride_b;      /* bytes between batch rows of the arena                                         */
+  int64_t scratch_stride_b;    /* bytes between beam rows of the scratch                                        */
+  int32_t row_bytes;
+  int32_t first_row;           /* the first generated row of the arena's layer group                            */
+  int32_t bounds_col;          /* the int32 of a beam row's bounds that holds its current row                   */
+  int32_t max_rows;            /* generated rows the arena holds after first_row                                */
+} pcv_kv_gather_entry;
+
+typedef struct pcv_kv_gather_params {
+  const pcv_kv_gather_entry* table;   /* device (n_entries)                                                     */
+  int32_t n_entries, R;
+  const int32_t* parents;             /* device (R): the global beam row each row continues                     */
+} pcv_kv_gather_params;
+
+PCV_API int pcv_kv_gather_rows_supported(const pcv_kv_gather_params* p, const pcv_dev_rows* rows);
+PCV_API int pcv_kv_gather_rows(const pcv_kv_gather_params* p, const pcv_dev_rows* rows, void* stream);
+
+/*
  * Backward of the LayerNorm -> Linear chain pcv_kv_project computes (training through kv_norm -> k_proj / v_proj,
  * q_norm -> q_proj, norm -> q/k/v_proj).  With x_hat = (x - mean) * rstd (row_stats of pcv_ln_stats),
  * y = x_hat * gamma + beta, out = y W^T + b, W = [W_k ; W_v] (n_k + n_v, C) and G = [grad_k | grad_v] (rows, n):

@@ -85,6 +85,10 @@ EXPORTS = (
     "pcv_spec_verify_supported",
     "pcv_spec_verify",
     "pcv_spec_uniforms",
+    "pcv_beam_step_supported",
+    "pcv_beam_step",
+    "pcv_kv_gather_rows_supported",
+    "pcv_kv_gather_rows",
     "pcv_ln_linear_bwd_supported",
     "pcv_ln_linear_bwd_workspace_bytes",
     "pcv_ln_linear_bwd",
@@ -304,6 +308,36 @@ class SpecVerifyParams(C.Structure):
     ]
 
 
+BEAM_MAX_BEAMS = 8   # PCV_BEAM_MAX_BEAMS
+BEAM_MAX_EOS = 4     # PCV_BEAM_MAX_EOS
+
+
+class BeamStepParams(C.Structure):
+    _fields_ = [
+        ("logits", C.c_void_p), ("stride_row", C.c_int64), ("length_penalty", C.c_double),
+        ("B", C.c_int32), ("K", C.c_int32), ("V", C.c_int32), ("dtype", C.c_int32),
+        ("n_eos", C.c_int32), ("eos", C.c_int32 * BEAM_MAX_EOS),
+        ("early_stopping", C.c_int32), ("hist_len", C.c_int32),
+        ("running_scores", C.c_void_p), ("finished_scores", C.c_void_p), ("finished_flags", C.c_void_p),
+        ("running_hist", C.c_void_p), ("finished_hist", C.c_void_p), ("hist_scratch", C.c_void_p),
+        ("item_flags", C.c_void_p), ("counters", C.c_void_p),
+        ("cand_scores", C.c_void_p), ("cand_index", C.c_void_p),
+        ("next_tokens", C.c_void_p), ("parents", C.c_void_p),
+    ]
+
+
+class KvGatherEntry(C.Structure):
+    _fields_ = [
+        ("arena", C.c_void_p), ("scratch", C.c_void_p),
+        ("arena_stride_b", C.c_int64), ("scratch_stride_b", C.c_int64),
+        ("row_bytes", C.c_int32), ("first_row", C.c_int32), ("bounds_col", C.c_int32), ("max_rows", C.c_int32),
+    ]
+
+
+class KvGatherParams(C.Structure):
+    _fields_ = [("table", C.c_void_p), ("n_entries", C.c_int32), ("R", C.c_int32), ("parents", C.c_void_p)]
+
+
 class LnLinearBwdParams(C.Structure):
     _fields_ = [
         ("x", C.c_void_p), ("x_stride_row", C.c_int64), ("row_stats", C.c_void_p),
@@ -462,6 +496,12 @@ def lib() -> C.CDLL:
         l.pcv_spec_uniforms.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]
         for name in ("pcv_sample_supported", "pcv_sample", "pcv_sample_uniforms", "pcv_spec_verify_supported",
                      "pcv_spec_verify", "pcv_spec_uniforms"):
+            getattr(l, name).restype = C.c_int
+        l.pcv_beam_step_supported.argtypes = [C.POINTER(BeamStepParams)]
+        l.pcv_beam_step.argtypes = [C.POINTER(BeamStepParams), C.c_void_p]
+        l.pcv_kv_gather_rows_supported.argtypes = [C.POINTER(KvGatherParams), rows]
+        l.pcv_kv_gather_rows.argtypes = [C.POINTER(KvGatherParams), rows, C.c_void_p]
+        for name in ("pcv_beam_step_supported", "pcv_beam_step", "pcv_kv_gather_rows_supported", "pcv_kv_gather_rows"):
             getattr(l, name).restype = C.c_int
         l.pcv_ln_linear_bwd_supported.argtypes = [C.POINTER(LnLinearBwdParams)]
         l.pcv_ln_linear_bwd_supported.restype = C.c_int

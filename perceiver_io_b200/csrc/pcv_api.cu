@@ -383,6 +383,24 @@ int pcv_spec_uniforms(uint64_t* out, const uint64_t* seeds, const int32_t* posit
                               reinterpret_cast<cudaStream_t>(stream));
 }
 
+int pcv_beam_step_supported(const pcv_beam_step_params* p) { return beam_step_check(p) == PCV_OK ? 1 : 0; }
+
+int pcv_beam_step(const pcv_beam_step_params* p, void* stream) {
+  const int rc = beam_step_check(p);
+  if (rc != PCV_OK) return rc;
+  return launch_beam_step(*p, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pcv_kv_gather_rows_supported(const pcv_kv_gather_params* p, const pcv_dev_rows* rows) {
+  return kv_gather_check(p, rows) == PCV_OK ? 1 : 0;
+}
+
+int pcv_kv_gather_rows(const pcv_kv_gather_params* p, const pcv_dev_rows* rows, void* stream) {
+  const int rc = kv_gather_check(p, rows);
+  if (rc != PCV_OK) return rc;
+  return launch_kv_gather(*p, *rows, reinterpret_cast<cudaStream_t>(stream));
+}
+
 static int partial_dropout_check(const pcv_attn_params* p, float dropout_p, bool shard) {
   if (validate_attn(p) != PCV_OK) return 0;
   const char* why = "";

@@ -176,5 +176,10 @@ int spec_verify_check(const pcv_spec_verify_params* p);
 int launch_spec_verify(const pcv_spec_verify_params& p, cudaStream_t stream);
 int launch_spec_uniforms(uint64_t* out, const uint64_t* seeds, const int32_t* positions, int R, int rows_per_batch,
                          int stream_id, cudaStream_t stream);
+// beam search (pcv_beam.cu)
+int beam_step_check(const pcv_beam_step_params* p);
+int launch_beam_step(const pcv_beam_step_params& p, cudaStream_t stream);
+int kv_gather_check(const pcv_kv_gather_params* p, const pcv_dev_rows* rows);
+int launch_kv_gather(const pcv_kv_gather_params& p, const pcv_dev_rows& rows, cudaStream_t stream);
 
 }  // namespace pcv

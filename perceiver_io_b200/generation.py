@@ -22,6 +22,7 @@ run, and in-graph int32 ops advance them at the end of each step.
     tokens, q = dec.generate(first, n, logits=True)                           # and the (B, n, vocab) logits drawn from
     out, accepted = dec.verify(token_ids, draft_logits, draft_sampling)       # (B, G+1) -> one speculative round
     tokens, stats = speculative_generate(target, draft, first, n, draft_tokens=G)
+    out = dec.beam_search(input_ids, prefix_len, n, num_beams=K)              # batch = B*K: (B, R, n), (B, R)
 
 Rows: cross-attention arena row r holds token r of the sequence (prompt and generated tokens); self-attention arena
 row r holds token ``prefix_len + r`` (prefix_len of the prompt).  The windows follow the 🤗 wrapper's truncation, as
@@ -53,9 +54,15 @@ model's own filtered distribution.  ``verify`` and :func:`speculative_generate` 
 instead: min(1, p/q) acceptance and a draw from max(0, p - q) on rejection (``ops.spec_verify``), so every emitted token
 is distributed as the target's own draw and a draft is accepted with probability Σ min(p, q).
 
+Beam search: ``beam_search`` runs 🤗's ``_beam_search`` (``do_sample=False``, no logits processors: EOS ids, length
+penalty, ``early_stopping`` and ``num_return_sequences`` as 🤗 takes them) with one replay per token: the replay feeds
+the K beams' tokens, runs the device beam step (``ops.beam_step``) on the logits and gathers, by parent, only the arena
+rows generated since the prefill (``ops.kv_gather_rows``): every beam of an item was prefilled with the same prompt, so
+the prompt rows never move.
+
 Not covered: steps of more than 64 tokens, a different k per batch row, contrastive search, a ring buffer bounded at
-``max_seq_len`` (the arenas grow by ``max_new_tokens`` rows), EOS handling (callers truncate after EOS), per-row
-sampling values, repetition penalties and wiring into 🤗 ``generate()``.
+``max_seq_len`` (the arenas grow by ``max_new_tokens`` rows), EOS handling outside beam search (callers truncate after
+EOS), beam sampling, per-row sampling values, repetition penalties and wiring into 🤗 ``generate()``.
 """
 from __future__ import annotations
 
@@ -180,6 +187,23 @@ def _sampling_triple(what: str, temperature, top_k, top_p):
     return t, min(k, 2 ** 31 - 1), p
 
 
+class BeamSearchOutput(NamedTuple):
+    sequences: torch.Tensor   # (B, R, n) int64 generated tokens, the output fill value after a hypothesis's end
+    scores: torch.Tensor      # (B, R) fp32, 🤗's sequences_scores
+
+
+def _eos_ids(eos_token_id) -> List[int]:
+    if eos_token_id is None:
+        return []
+    ids = [eos_token_id] if _as_count(eos_token_id) is not None else eos_token_id
+    if isinstance(ids, torch.Tensor):
+        ids = ids.flatten().tolist()
+    if not isinstance(ids, Sequence) or isinstance(ids, (str, bytes)) or any(_as_count(e) is None for e in ids):
+        raise ValueError(f"GraphedDecoder.beam_search: eos_token_id must be None, an integer or a list of integers, got "
+                         f"{eos_token_id!r}")
+    return [_as_count(e) for e in ids]
+
+
 class _Attn:
     """Static state of one attention layer: arenas, rotated-key arena, scales."""
 
@@ -195,6 +219,8 @@ class GraphedDecoder:
     _lag = None
     _seeds = None   # (B,) int64 sampler seeds, set in __init__
     _draft_sampling = (1.0, 0, 1.0)   # the draft's values of the verify graph being recorded or replayed
+    _beam_state = None                # ops.BeamState of the last beam_search
+    _beam_table = None                # ops.KvGatherTable of the last beam_search (its scratch is reused)
 
     def __init__(self, model, batch: int, max_new_tokens: int, kv_cache: str = "bf16"):
         if max_new_tokens < 1:
@@ -536,6 +562,116 @@ class GraphedDecoder:
                              f"got {tuple(draft_logits.shape)} {draft_logits.dtype}")
         self._draft_sampling = draft
         return self._replay(token_ids, "verify", draft_logits)
+
+    # ---- beam search ----------------------------------------------------------------------------------------------
+    def _beam_args(self, B: int, n, num_beams, eos_token_id, length_penalty, early_stopping, num_return_sequences,
+                   check_every):
+        """The checked arguments of ``beam_search``: (K, n, eos ids, length_penalty, early_stopping, R, check_every)."""
+        what = "GraphedDecoder.beam_search"
+        K, count, R, every = _as_count(num_beams), _as_count(n), _as_count(num_return_sequences), _as_count(check_every)
+        if K is None or not 1 <= K <= ops.BEAM_MAX_BEAMS:
+            raise ValueError(f"{what}: num_beams must be an integer in [1, {ops.BEAM_MAX_BEAMS}], got {num_beams!r}")
+        if self.batch != B * K:
+            raise ValueError(f"{what}: the decoder's batch {self.batch} must be batch * num_beams = {B} * {K}")
+        if count is None or count < 1 or count - 1 > self.max_new_tokens:
+            raise ValueError(f"{what}: n must be an integer in [1, max_new_tokens + 1 = {self.max_new_tokens + 1}] "
+                             f"(token 1 comes from the prefill), got {n!r}")
+        if R is None or not 1 <= R <= K:
+            raise ValueError(f"{what}: num_return_sequences must be an integer in [1, num_beams={K}], got "
+                             f"{num_return_sequences!r}")
+        if every is None or every < 1:
+            raise ValueError(f"{what}: check_every must be an integer >= 1, got {check_every!r}")
+        vocab = self.model.config.vocab_size
+        if vocab > ops.SAMPLE_MAX_VOCAB:
+            raise RuntimeError(f"{what}: the device beam step takes vocabularies up to {ops.SAMPLE_MAX_VOCAB}, this "
+                               f"model has {vocab}")
+        eos = _eos_ids(eos_token_id)
+        if len(eos) > ops.BEAM_MAX_EOS or any(not 0 <= e < vocab for e in eos):
+            raise ValueError(f"{what}: at most {ops.BEAM_MAX_EOS} EOS ids, each in [0, {vocab}), got {eos}")
+        if K * vocab < ops.beams_to_keep(K, len(eos)):
+            raise ValueError(f"{what}: num_beams * vocab = {K * vocab} is below the {ops.beams_to_keep(K, len(eos))} "
+                             f"candidates a step keeps")
+        lp = float(length_penalty)
+        if not math.isfinite(lp):
+            raise ValueError(f"{what}: length_penalty must be finite, got {length_penalty!r}")
+        ops.early_stopping_code(early_stopping)
+        return K, count, eos, lp, early_stopping, R, every
+
+    def beam_search(self, input_ids: torch.Tensor, prefix_len: int, n: int, num_beams: int, pad_mask=None,
+                    eos_token_id=None, pad_token_id=None, length_penalty: float = 1.0, early_stopping=False,
+                    num_return_sequences: int = 1, check_every: int = 16) -> BeamSearchOutput:
+        """🤗's beam search (``GenerationMixin._beam_search`` with ``do_sample=False`` and no logits processors) of n
+        generated tokens for the B prompts ``input_ids`` (B, n0), with K = ``num_beams`` beams each; the decoder's batch
+        must be B * K.  Returns ``BeamSearchOutput(sequences, scores)``: 🤗's ``sequences[:, :num_return_sequences]``
+        (generated part, (B, R, n) int64, the output fill value — ``pad_token_id or eos_token_id[0]`` with EOS ids, else
+        -1 — after each hypothesis's end) and its ``sequences_scores`` (B, R) fp32.
+
+        Prefills ``input_ids.repeat_interleave(K, 0)`` (beam k of item b is batch row b*K + k), runs the device beam
+        step (``ops.beam_step``) eagerly on the prefill's logits, then n - 1 replays of one graph: feed the K beams'
+        tokens, the beam step on their logits, and the gather of the rows generated since the prefill by parent
+        (``ops.kv_gather_rows``).  Each replay's input is copied on the device from the previous replay's output.  With
+        EOS ids, the device's "every item done" flag is read every ``check_every`` replays and the loop stops once it
+        is set (🤗's stop condition; a stopped item's finished set no longer changes, so the output is the same);
+        without, nothing is read until the end.  The graph is recorded on first use after each prefill, keyed by (K, EOS
+        ids, length_penalty, early_stopping).  Refusals come before any replay."""
+        B = input_ids.shape[0] if input_ids.dim() == 2 else 0
+        K, count, eos, lp, es, R, every = self._beam_args(B, n, num_beams, eos_token_id, length_penalty,
+                                                          early_stopping, num_return_sequences, check_every)
+        if torch.is_autocast_enabled():
+            raise RuntimeError("GraphedDecoder does not run under autocast")
+        fill = (pad_token_id or eos[0]) if eos else -1
+
+        def beams(t):   # (B, ...) -> (B*K, ...), beam k of item b at row b*K + k (repeat_interleave without a sync)
+            return t[:, None].expand(t.shape[0], K, *t.shape[1:]).reshape(-1, *t.shape[1:])
+
+        logits = self.prefill(beams(input_ids), prefix_len, beams(pad_mask) if pad_mask is not None else None)
+        state = self._beam_state
+        if state is None or (state.B, state.K, state.n_eos) != (B, K, len(eos)):
+            state = self._beam_state = ops.BeamState(B, K, len(eos), self.max_new_tokens + 1, fill, self.device)
+        state.fill = fill   # reset() fills the histories with it
+        n0 = input_ids.shape[1]
+        first = (n0, n0 - prefix_len)
+        # prefill allocated new arenas: a new table, but the scratch of the last one when the shapes match
+        table = self._beam_table = ops.KvGatherTable(
+            [(t, first[a.group], a.group * _NCOL + 2) for a in self._layers for t in (a.K, a.V, a.S) if t is not None],
+            reuse=self._beam_table)
+        rows = self._bounds.view(self.batch, -1)
+
+        def beam_fn(token):
+            tokens, parents = ops.beam_step(self._step_fn(token), state, eos, lp, es)
+            ops.kv_gather_rows(table, parents, rows)
+            return tokens
+
+        gkey = ("beam", K, tuple(eos), lp, str(es))
+        state.reset(count)
+        if count > 1 and gkey not in self._graphs:
+            # recorded before the first step: the warm-up calls append, and gather, only rows that are rewritten later
+            snapshot = self._bounds.clone()
+            old = torch.cuda.get_sync_debug_mode()
+            torch.cuda.set_sync_debug_mode(0)
+            try:
+                self._graphs[gkey] = GraphedForward(beam_fn, state.tokens)
+            finally:
+                torch.cuda.set_sync_debug_mode(old)
+            self._bounds.copy_(snapshot)
+            self.captures += 1
+            state.reset(count)
+        ops.beam_step(logits, state, eos, lp, es)
+        graph = self._graphs.get(gkey)
+        for i in range(count - 1):
+            graph(state.tokens)
+            self._remaining -= 1
+            self._fed += 1
+            if eos and (i + 1) % every == 0 and i + 1 < count - 1:
+                old = torch.cuda.get_sync_debug_mode()
+                torch.cuda.set_sync_debug_mode(0)
+                try:
+                    stop = bool(state.counters[2].item())   # the one host read: every item done
+                finally:
+                    torch.cuda.set_sync_debug_mode(old)
+                if stop:
+                    break
+        return BeamSearchOutput(state.finished_hist[:, :R, :count].clone(), state.finished[:, :R].clone())
 
     def rewind(self, n) -> None:
         """Drop fed tokens: the next token of a batch row is fed at the row of its first dropped one, as if the dropped

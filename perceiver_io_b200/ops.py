@@ -30,7 +30,8 @@ __all__ = [
     "kv_project_fp8_supported", "ln_linear", "ln_linear_backward", "kv_append_fp8", "attention_decode_fp8",
     "attention_decode_fp8_supported", "fp8_pair_descale", "fp8_dequantize", "rotated_cache_shadow", "rotary_at", "rotary_fp8",
     "attention_decode_window", "kv_append_at", "rotary_apply_at", "rotary_angle_table", "attention_window",
-    "sample_tokens", "sample_uniforms", "spec_verify", "spec_uniforms",
+    "sample_tokens", "sample_uniforms", "spec_verify", "spec_uniforms", "BeamState", "beam_step", "KvGatherTable",
+    "kv_gather_rows",
 ]
 
 
@@ -1457,6 +1458,178 @@ def spec_uniforms(seeds: torch.Tensor, positions: torch.Tensor, stream: str = "a
                                            1 if len(lead) == 1 else lead[1], _SPEC_STREAMS[stream], _stream()),
               "pcv_spec_uniforms")
     return out
+
+
+# --------------------------------------------------------------------------------------------------
+# beam search (pcv_beam_step, pcv_kv_gather_rows): 🤗's beam step on device-resident state, and the KV gather of the
+# generated rows by parent, both recordable in a CUDA graph.
+# --------------------------------------------------------------------------------------------------
+#: The most beams and EOS ids :func:`beam_step` takes.
+BEAM_MAX_BEAMS = _lib.BEAM_MAX_BEAMS
+BEAM_MAX_EOS = _lib.BEAM_MAX_EOS
+
+
+def early_stopping_code(early_stopping) -> int:
+    """pcv_early_stopping of 🤗's ``early_stopping``: the bools False / True or the string "never", nothing else (🤗
+    tests ``early_stopping is True`` and ``== "never"``, so a string "True" would not mean True there)."""
+    if early_stopping is False or early_stopping is True:
+        return int(early_stopping)
+    if isinstance(early_stopping, str) and early_stopping == "never":
+        return 2
+    raise ValueError(f"early_stopping must be False, True or 'never', got {early_stopping!r}")
+
+
+def beams_to_keep(num_beams: int, n_eos: int) -> int:
+    return max(2, n_eos + 1) * num_beams
+
+
+class BeamState:
+    """The device state of :func:`beam_step` for B items of K beams and ``n_eos`` EOS ids: running and finished scores,
+    finished flags, token histories (B, K, hist_len) filled with ``fill``, the per-item heuristic and done flags, the
+    counters [generated count, max_length, every item done, 0], and the step's scratch and outputs (``tokens`` (B*K, 1)
+    int64, ``parents`` (B*K,) int32).  ``reset(max_length)`` re-initialises every buffer in place."""
+
+    def __init__(self, B: int, K: int, n_eos: int, hist_len: int, fill: int, device):
+        keep = beams_to_keep(K, n_eos)
+        self.B, self.K, self.n_eos, self.hist_len, self.fill = B, K, n_eos, hist_len, int(fill)
+        f32, i32, i64 = torch.float32, torch.int32, torch.int64
+        self.running = torch.empty(B, K, dtype=f32, device=device)
+        self.finished = torch.empty(B, K, dtype=f32, device=device)
+        self.finished_flags = torch.empty(B, K, dtype=i32, device=device)
+        self.running_hist = torch.empty(B, K, hist_len, dtype=i64, device=device)
+        self.finished_hist = torch.empty(B, K, hist_len, dtype=i64, device=device)
+        self.hist_scratch = torch.empty(B, 2 * K, hist_len, dtype=i64, device=device)
+        self.item_flags = torch.empty(B, 2, dtype=i32, device=device)
+        self.counters = torch.empty(4, dtype=i32, device=device)
+        self.cand_scores = torch.empty(B * K, keep, dtype=f32, device=device)
+        self.cand_index = torch.empty(B * K, keep, dtype=i32, device=device)
+        self.tokens = torch.zeros(B * K, 1, dtype=i64, device=device)
+        self.parents = torch.zeros(B * K, dtype=i32, device=device)
+
+    def reset(self, max_length: int) -> None:
+        """Start a search of ``max_length`` generated tokens: eager in-place fills, no synchronisation."""
+        self.running.fill_(-1e9)
+        self.running[:, 0].fill_(0.0)
+        self.finished.fill_(-1e9)
+        self.finished_flags.zero_()
+        self.running_hist.fill_(self.fill)
+        self.finished_hist.fill_(self.fill)
+        self.item_flags[:, 0].fill_(1)
+        self.item_flags[:, 1].fill_(0)
+        self.counters.zero_()
+        self.counters[1:2].fill_(int(max_length))   # fill_ with a host scalar: a kernel argument, no copy or sync
+
+
+def beam_step(logits: torch.Tensor, state: BeamState, eos=(), length_penalty: float = 1.0, early_stopping=False):
+    """One step of 🤗's beam search (``do_sample=False``, no logits processors) on the device (pcv_beam_step), in place
+    on ``state``: logits (B*K, V) bf16 / fp16 / fp32, V <= :data:`SAMPLE_MAX_VOCAB`, beam k of item b in row b*K + k.
+    Returns ``(state.tokens, state.parents)``: the (B*K, 1) int64 next tokens and the (B*K,) int32 global beam row each
+    beam continues.  Nothing is read back to the host, so the call can be recorded in a CUDA graph: the generated count
+    and max_length live in ``state.counters``.  Arguments the kernel does not take raise ``ValueError`` with its reason
+    before any launch."""
+    _require_cuda(logits)
+    if logits.dim() != 2 or logits.dtype not in (torch.bfloat16, torch.float16, torch.float32):
+        raise ValueError(f"beam_step: logits must be (B*K, V) bf16 / fp16 / fp32, got {tuple(logits.shape)} "
+                         f"{logits.dtype}")
+    eos = list(eos)
+    if logits.shape[0] != state.B * state.K or len(eos) != state.n_eos:
+        raise ValueError(f"beam_step: the state is for {state.B}x{state.K} beams and {state.n_eos} EOS ids, got "
+                         f"{logits.shape[0]} logits rows and {len(eos)} EOS ids")
+    rows = logits if logits.stride(-1) == 1 else logits.contiguous()
+    p = _lib.BeamStepParams()
+    p.logits, p.stride_row = rows.data_ptr(), rows.stride(0) if rows.shape[0] > 1 else rows.shape[1]
+    p.B, p.K, p.V = state.B, state.K, rows.shape[1]
+    p.dtype = _lib.PCV_F32 if rows.dtype == torch.float32 else _pcv_dtype(rows.dtype)
+    if len(eos) > BEAM_MAX_EOS:
+        raise ValueError(f"beam_step: at most {BEAM_MAX_EOS} EOS ids, got {len(eos)}")
+    p.n_eos = len(eos)
+    for i, e in enumerate(eos):
+        p.eos[i] = max(-2 ** 31, min(int(e), 2 ** 31 - 1))
+    p.length_penalty = float(length_penalty)
+    p.early_stopping = early_stopping_code(early_stopping)
+    p.hist_len = state.hist_len
+    for f in ("running", "finished", "finished_flags", "running_hist", "finished_hist", "hist_scratch", "item_flags",
+              "counters", "cand_scores", "cand_index"):
+        setattr(p, {"running": "running_scores", "finished": "finished_scores"}.get(f, f), getattr(state, f).data_ptr())
+    p.next_tokens, p.parents = state.tokens.data_ptr(), state.parents.data_ptr()
+    lib = _lib.lib()
+    if not lib.pcv_beam_step_supported(C.byref(p)):
+        raise ValueError(f"beam_step: {lib.pcv_last_error().decode()}")
+    with torch.cuda.device(logits.device):
+        check(lib.pcv_beam_step(C.byref(p), _stream()), "pcv_beam_step")
+    return state.tokens, state.parents
+
+
+class KvGatherTable:
+    """The device table of :func:`kv_gather_rows`: ``entries`` is a list of ``(arena, first_row, bounds_col)`` with arena
+    a (R, capacity, C) tensor (any dtype, 16-byte rows) whose generated rows start at ``first_row``, and ``bounds_col``
+    the int32 of a beam row's bounds that holds its current row.  Each arena needs a scratch of (R, capacity -
+    first_row, C): taken from ``reuse`` (an earlier table, e.g. of the previous prefill's arenas) where one of that
+    shape, dtype and device is at the same position, else allocated.  The scratch only carries rows within one
+    :func:`kv_gather_rows` call, so tables on one stream may share it; the device table is uploaded again only when
+    its bytes differ from ``reuse``'s."""
+
+    def __init__(self, entries, reuse: Optional["KvGatherTable"] = None):
+        if not entries:
+            raise ValueError("KvGatherTable: no arenas")
+        self.scratch, self.arenas = [], []
+        table = (_lib.KvGatherEntry * len(entries))()
+        R = entries[0][0].shape[0]
+        for e, (arena, first, col) in zip(table, entries):
+            _require_cuda(arena)
+            row_bytes = arena.shape[2] * arena.element_size()
+            if (arena.dim() != 3 or arena.shape[0] != R or not arena.is_contiguous() or row_bytes % 16
+                    or arena.data_ptr() % 16):
+                raise ValueError(f"KvGatherTable: arenas must be contiguous (R={R}, capacity, C) tensors with 16-byte "
+                                 f"aligned rows, got {tuple(arena.shape)} {arena.dtype}")
+            if not 0 <= first < arena.shape[1] or col < 0:
+                raise ValueError(f"KvGatherTable: first_row={first} must be in [0, {arena.shape[1]}) and bounds_col "
+                                 f"={col} >= 0")
+            rows = arena.shape[1] - first
+            i = len(self.scratch)
+            old = reuse.scratch[i] if reuse is not None and i < len(reuse.scratch) else None
+            shape = (R, rows, arena.shape[2])
+            if old is not None and tuple(old.shape) == shape and old.dtype == arena.dtype and old.device == arena.device:
+                s = old
+            else:
+                s = torch.empty(shape, dtype=arena.dtype, device=arena.device)
+            e.arena, e.scratch = arena.data_ptr(), s.data_ptr()
+            e.arena_stride_b, e.scratch_stride_b = arena.stride(0) * arena.element_size(), rows * row_bytes
+            e.row_bytes, e.first_row, e.bounds_col, e.max_rows = row_bytes, int(first), int(col), rows
+            self.scratch.append(s)
+            self.arenas.append(arena)
+        self.R = R
+        self.n = len(entries)
+        self.packed = bytes(table)
+        dev = entries[0][0].device
+        if reuse is not None and reuse.packed == self.packed and reuse.table.device == dev:
+            self.table, self._host = reuse.table, reuse._host
+            return
+        raw = torch.frombuffer(bytearray(self.packed), dtype=torch.uint8).pin_memory()   # asynchronous: no sync
+        self.table = raw.to(dev, non_blocking=True)
+        self._host = raw   # alive until the copy has run
+
+
+def kv_gather_rows(table: KvGatherTable, parents: torch.Tensor, bounds: torch.Tensor) -> None:
+    """Every beam row i with ``parents[i] != i`` takes its parent's rows [first_row, cur) of every arena of ``table``,
+    cur = ``bounds[i, bounds_col]`` read on the device when the kernel runs (pcv_kv_gather_rows).  Cycles and
+    many-to-one moves read the rows as they were before the call; every other byte is untouched.  ``parents`` (R,) int32
+    CUDA; ``bounds`` (R, >= 1) int32 CUDA with unit stride in its last dim.  Recordable in a CUDA graph."""
+    _require_cuda(parents, bounds)
+    if parents.dtype != torch.int32 or tuple(parents.shape) != (table.R,) or not parents.is_contiguous():
+        raise ValueError(f"kv_gather_rows: parents must be a contiguous ({table.R},) int32 tensor, got "
+                         f"{tuple(parents.shape)} {parents.dtype}")
+    if bounds.dtype != torch.int32 or bounds.dim() != 2 or bounds.shape[0] != table.R or bounds.stride(-1) != 1:
+        raise ValueError(f"kv_gather_rows: bounds must be a ({table.R}, cols) int32 tensor with unit column stride")
+    p = _lib.KvGatherParams()
+    p.table, p.n_entries, p.R, p.parents = table.table.data_ptr(), table.n, table.R, parents.data_ptr()
+    r = _lib.DevRows()
+    r.bounds, r.capacity, r.bounds_stride_b = bounds.data_ptr(), bounds.shape[1], bounds.stride(0)
+    lib = _lib.lib()
+    if not lib.pcv_kv_gather_rows_supported(C.byref(p), C.byref(r)):
+        raise ValueError(f"kv_gather_rows: {lib.pcv_last_error().decode()}")
+    with torch.cuda.device(parents.device):
+        check(lib.pcv_kv_gather_rows(C.byref(p), C.byref(r), _stream()), "pcv_kv_gather_rows")
 
 
 def tcgen05_supported(q, k, v, num_heads: int, pad_mask=None, causal: bool = False) -> bool:
