@@ -20,47 +20,18 @@
 // pcv_kv_gather_rows: for every beam row whose parent is another row, copy the parent's generated rows [first row,
 // current row) of every arena in the table into the child's, through a scratch region in two launches (parent ->
 // scratch, scratch -> child), so cycles and many-to-one moves read only pre-step rows.
-#include "pcv_common.cuh"
+#include "pcv_vocab.cuh"
 
 namespace pcv {
 
-namespace sm90 {
-int set_smem_limit(const void* kernel, int smem);  // pcv_sm90_host.cu
-}
-
 namespace {
 
-constexpr int kThreads = 512;
-constexpr int kWarps = kThreads / 32;
 constexpr int kMaxKeep = (PCV_BEAM_MAX_EOS + 1) * PCV_BEAM_MAX_BEAMS;   // beams_to_keep at most
 constexpr int kMaxCand = PCV_BEAM_MAX_BEAMS * kMaxKeep;                 // row candidates of one item
 constexpr float kNeg = -1.0e9f;
 
-// order-preserving key of a float: a < b <=> key(a) < key(b); -0 and +0 share a key
-__device__ __forceinline__ uint32_t beam_key(float x) {
-  uint32_t u = __float_as_uint(x);
-  if (u == 0x80000000u) u = 0u;
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-
-// hist[bin] += 1 for every lane with bin < 256: one shared atomic per distinct bin of the warp.  All 32 lanes call it.
-__device__ __forceinline__ void beam_hist(uint32_t* hist, uint32_t bin) {
-  if (!__ballot_sync(0xffffffffu, bin < 256u)) return;
-  const unsigned group = __match_any_sync(0xffffffffu, bin);
-  if (bin < 256u && (threadIdx.x & 31) == (unsigned)(__ffs(group) - 1)) atomicAdd(hist + bin, (uint32_t)__popc(group));
-}
-
 __device__ __forceinline__ int keep_count(const pcv_beam_step_params& p) {
   return (p.n_eos + 1 > 2 ? p.n_eos + 1 : 2) * p.K;
-}
-
-template <typename T>
-__device__ __forceinline__ float load_f(const T* s) {
-  return Elem<T>::to_f(*s);
-}
-template <>
-__device__ __forceinline__ float load_f<float>(const float* s) {
-  return *s;
 }
 
 template <typename T>
@@ -68,8 +39,6 @@ __global__ void __launch_bounds__(kThreads) beam_rows_kernel(const pcv_beam_step
   extern __shared__ __align__(16) float xs[];   // the row's x, then its acc (V floats)
   __shared__ float redf[kWarps];
   __shared__ double redd[kWarps];
-  __shared__ uint32_t hist[256];
-  __shared__ uint32_t sel[2];                   // radix state: key prefix, count still needed
   __shared__ uint32_t wgt[kWarps], weq[kWarps];
   __shared__ uint32_t ckey[kMaxKeep];
   __shared__ int32_t cidx[kMaxKeep];
@@ -107,56 +76,16 @@ __global__ void __launch_bounds__(kThreads) beam_rows_kernel(const pcv_beam_step
     xs[i] = __fadd_rn(run, __double2float_rn(d - logS));
   }
 
-  // ---- the nsel-th largest key (radix select, four passes of 256 bins) ----
+  // ---- the nsel-th largest key ----
   const int nsel = keep < V ? keep : V;
-  if (tid == 0) sel[0] = 0, sel[1] = (uint32_t)nsel;
-  for (int shift = 24; shift >= 0; shift -= 8) {
-    for (int i = tid; i < 256; i += kThreads) hist[i] = 0;
-    __syncthreads();
-    const uint32_t prefix = sel[0], hi_mask = shift == 24 ? 0u : ~0u << (shift + 8);
-    for (int base = 0; base < V; base += kThreads) {
-      const int i = base + tid;
-      uint32_t bin = 256u;
-      if (i < V) {
-        const uint32_t key = beam_key(xs[i]);
-        if ((key & hi_mask) == prefix) bin = (key >> shift) & 255u;
-      }
-      beam_hist(hist, bin);
-    }
-    __syncthreads();
-    if (warp == 0) {   // lane l owns bins 8l .. 8l+7; find d with above(d) < need <= above(d) + h[d], from the top
-      uint32_t h[8], own = 0;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) h[j] = hist[8 * lane + j], own += h[j];
-      uint32_t incl = own;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
-        if (lane >= o) incl += t;
-      }
-      uint32_t above = __shfl_sync(0xffffffffu, incl, 31) - incl;
-      const uint32_t need = sel[1];
-      __syncwarp();
-#pragma unroll
-      for (int j = 7; j >= 0; --j) {
-        if (above < need && above + h[j] >= need) {
-          sel[0] = prefix | ((uint32_t)(8 * lane + j) << shift);
-          sel[1] = need - above;
-        }
-        above += h[j];
-      }
-    }
-    __syncthreads();
-  }
-  const uint32_t thr = sel[0];
+  const uint32_t thr = select_key(xs, V, (uint32_t)nsel);
 
   // ---- collect: every key above thr, then the keys equal to it in index order; warp w owns one segment ----
-  const int seg = ((V + kWarps * 32 - 1) / (kWarps * 32)) * 32;
-  const int s0 = warp * seg, s1 = min(V, s0 + seg);
+  const auto [s0, s1] = warp_segment(V);
   uint32_t ngt = 0, neq = 0;
   for (int base = s0; base < s1; base += 32) {
     const int i = base + lane;
-    const uint32_t key = i < s1 ? beam_key(xs[i]) : 0u;
+    const uint32_t key = i < s1 ? order_key(xs[i]) : 0u;
     ngt += __popc(__ballot_sync(0xffffffffu, i < s1 && key > thr));
     neq += __popc(__ballot_sync(0xffffffffu, i < s1 && key == thr));
   }
@@ -172,7 +101,7 @@ __global__ void __launch_bounds__(kThreads) beam_rows_kernel(const pcv_beam_step
   const uint32_t need_eq = (uint32_t)nsel - gt_total;
   for (int base = s0; base < s1; base += 32) {
     const int i = base + lane;
-    const uint32_t key = i < s1 ? beam_key(xs[i]) : 0u;
+    const uint32_t key = i < s1 ? order_key(xs[i]) : 0u;
     const unsigned below = (1u << lane) - 1u;
     const unsigned bg = __ballot_sync(0xffffffffu, i < s1 && key > thr);
     const unsigned be = __ballot_sync(0xffffffffu, i < s1 && key == thr);
@@ -217,7 +146,7 @@ __device__ __forceinline__ int take_top(const float* v, int n, bool* taken) {
   uint32_t bk = 0;
   for (int c = 0; c < n; ++c) {
     if (taken[c]) continue;
-    const uint32_t key = beam_key(v[c]);
+    const uint32_t key = order_key(v[c]);
     if (best < 0 || key > bk) best = c, bk = key;
   }
   taken[best] = true;
@@ -250,7 +179,7 @@ __global__ void __launch_bounds__(kThreads) beam_item_kernel(const pcv_beam_step
     const float sc = p.cand_scores[(int64_t)b * nc + c];
     const int32_t ix = p.cand_index[(int64_t)b * nc + c];
     score_s[c] = sc;
-    key_s[c] = ix < 0 ? 0u : beam_key(sc);                  // fillers rank below every candidate
+    key_s[c] = ix < 0 ? 0u : order_key(sc);                 // fillers rank below every candidate
     idx_s[c] = ix < 0 ? 0x7fffffff - c : ix;
   }
   __syncthreads();
@@ -452,20 +381,10 @@ int beam_step_check(const pcv_beam_step_params* p) {
 }
 
 int launch_beam_step(const pcv_beam_step_params& p, cudaStream_t stream) {
-  const int smem = p.V * (int)sizeof(float);
-  const void* kern = p.dtype == PCV_BF16  ? reinterpret_cast<const void*>(&beam_rows_kernel<__nv_bfloat16>)
-                     : p.dtype == PCV_F16 ? reinterpret_cast<const void*>(&beam_rows_kernel<__half>)
-                                          : reinterpret_cast<const void*>(&beam_rows_kernel<float>);
-  if (smem > 48 * 1024) {   // once per kernel and device, for the largest row
-    const int rc = sm90::set_smem_limit(kern, PCV_SAMPLE_MAX_VOCAB * (int)sizeof(float));
-    if (rc != PCV_OK) return rc;
-  }
-  const int rows = p.B * p.K;
-  if (p.dtype == PCV_BF16) beam_rows_kernel<__nv_bfloat16><<<rows, kThreads, smem, stream>>>(p);
-  else if (p.dtype == PCV_F16) beam_rows_kernel<__half><<<rows, kThreads, smem, stream>>>(p);
-  else beam_rows_kernel<float><<<rows, kThreads, smem, stream>>>(p);
-  PCV_CHECK_CUDA(cudaGetLastError());
-  count_launch();
+  void (*const kern[3])(pcv_beam_step_params) = {beam_rows_kernel<__nv_bfloat16>, beam_rows_kernel<__half>,
+                                                 beam_rows_kernel<float>};
+  const int rc = launch_row_kernel(kern, p.dtype, p.V, p.B * p.K, p, stream);
+  if (rc != PCV_OK) return rc;
   beam_item_kernel<<<p.B, kThreads, 0, stream>>>(p);
   PCV_CHECK_CUDA(cudaGetLastError());
   count_launch();

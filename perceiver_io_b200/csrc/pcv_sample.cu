@@ -25,19 +25,13 @@
 // Speculative sampling (pcv_spec_verify, pcv_spec_uniforms): the rejection rule of Leviathan et al. / Chen et al. on the
 // same integer masses, steps 1-4 shared with sample_kernel (stage_row, kept_threshold); the rule is stated at
 // spec_verify_kernel and in include/pcv_attn.h, and oracle/spec_oracle.py restates it with Python integers.
-#include "pcv_common.cuh"
 #include "pcv_hash.cuh"
+#include "pcv_vocab.cuh"
 
 namespace pcv {
 
-namespace sm90 {
-int set_smem_limit(const void* kernel, int smem);  // pcv_sm90_host.cu
-}
-
 namespace {
 
-constexpr int kThreads = 512;
-constexpr int kWarps = kThreads / 32;
 constexpr double kMassScale = 1099511627776.0;  // 2^40
 using u64 = unsigned long long;
 
@@ -58,16 +52,6 @@ __device__ __forceinline__ u64 sample_bits(u64 seed, uint32_t b, uint32_t pos) {
   const uint32_t h0 = sample_half(word, lo, hi, 0xD2511F53u, 0xCD9E8D57u, 0x3C6EF372u, 0xA54FF53Au, 0x510E527Fu);
   const uint32_t h1 = sample_half(word, lo, hi, 0xCD9E8D57u, 0xD2511F53u, 0x9B05688Cu, 0x1F83D9ABu, 0x5BE0CD19u);
   return ((u64)h1 << 32) | h0;
-}
-
-// order-preserving key of a float: a < b <=> key(a) < key(b); -0 and +0 share a key
-__device__ __forceinline__ uint32_t order_key(float x) {
-  uint32_t u = __float_as_uint(x);
-  if (u == 0x80000000u) u = 0u;
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float key_value(uint32_t k) {
-  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
 }
 
 // w = round(2^40 exp(x - m)); 0 below x - m = -29, where 2^40 exp(x - m) < 0.28
@@ -98,13 +82,6 @@ __device__ __forceinline__ u64 block_max_u64(u64 v, u64* red) {
   return v;
 }
 
-// hist[bin] += 1 for every lane with bin < 256: one shared atomic per distinct bin of the warp.  Called by all 32 lanes.
-__device__ __forceinline__ void hist_count(uint32_t* hist, uint32_t bin) {
-  if (!__ballot_sync(0xffffffffu, bin < 256u)) return;
-  const unsigned group = __match_any_sync(0xffffffffu, bin);
-  if (bin < 256u && (threadIdx.x & 31) == (unsigned)(__ffs(group) - 1)) atomicAdd(hist + bin, (uint32_t)__popc(group));
-}
-
 // hist[bin] += v for every lane with bin < 256; lanes with one bin are summed in registers first, so a warp issues one
 // shared atomic per distinct bin.  Called by all 32 lanes.
 __device__ __forceinline__ void hist_mass(u64* hist, uint32_t bin, u64 v) {
@@ -121,11 +98,6 @@ __device__ __forceinline__ void hist_mass(u64* hist, uint32_t bin, u64 v) {
     }
   }
   if (bin < 256u && (threadIdx.x & 31) == (unsigned)(__ffs(group) - 1)) atomicAdd(hist + bin, sum);
-}
-
-template <typename T>
-__device__ __forceinline__ float load_f(const T* p) {
-  return Elem<T>::to_f(*p);
 }
 
 // Step 1 of the sampler on the row src[0 .. V): stages x in xs (x / temperature unless greedy) and returns the
@@ -149,56 +121,14 @@ __device__ __forceinline__ u64 stage_row(const T* src, int V, float temperature,
 template <typename Values>
 __device__ __forceinline__ uint32_t kept_threshold(int V, const Values& v, uint32_t top, const float* xs) {
   __shared__ u64 mhist[256];       // top-p masses
-  __shared__ uint32_t chist[256];  // top-k counts
-  __shared__ u64 sel[2];           // radix state: [0] key prefix, [1] count still needed / mass below
+  __shared__ u64 sel[2];           // radix state: [0] key prefix, [1] mass below
   __shared__ u64 cut_s;            // the top-p cut
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const float m = key_value(top);
 
   // ---- top-k: the k-th largest key, kept iff key >= lo ----
   uint32_t lo = 0;
-  if (v.top_k > 0 && v.top_k < V) {
-    if (tid == 0) sel[0] = 0, sel[1] = (u64)v.top_k;
-    for (int shift = 24; shift >= 0; shift -= 8) {
-      for (int i = tid; i < 256; i += kThreads) chist[i] = 0;
-      __syncthreads();
-      const uint32_t prefix = (uint32_t)sel[0], hi_mask = shift == 24 ? 0u : ~0u << (shift + 8);
-      for (int base = 0; base < V; base += kThreads) {
-        const int i = base + tid;
-        uint32_t bin = 256u;
-        if (i < V) {
-          const uint32_t k = order_key(xs[i]);
-          if ((k & hi_mask) == prefix) bin = (k >> shift) & 255u;
-        }
-        hist_count(chist, bin);
-      }
-      __syncthreads();
-      if (warp == 0) {   // lane l owns bins 8l .. 8l+7; find d with above(d) < need <= above(d) + h[d], from the top
-        uint32_t h[8], own = 0;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) h[j] = chist[8 * lane + j], own += h[j];
-        uint32_t incl = own;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          const uint32_t t = __shfl_up_sync(0xffffffffu, incl, o);
-          if (lane >= o) incl += t;
-        }
-        uint32_t above = __shfl_sync(0xffffffffu, incl, 31) - incl;   // the counts of the lanes above this one
-        const uint32_t need = (uint32_t)sel[1];
-#pragma unroll
-        for (int j = 7; j >= 0; --j) {
-          if (above < need && above + h[j] >= need) {
-            sel[0] = prefix | ((uint32_t)(8 * lane + j) << shift);
-            sel[1] = need - above;
-          }
-          above += h[j];
-        }
-      }
-      __syncthreads();
-    }
-    lo = (uint32_t)sel[0];
-    __syncthreads();   // every thread has read sel before top-p reuses it
-  }
+  if (v.top_k > 0 && v.top_k < V) lo = select_key(xs, V, (uint32_t)v.top_k);
 
   // ---- top-p: the least kept key whose W≤ exceeds the cut ----
   if (v.top_p < 1.f) {
@@ -265,8 +195,10 @@ __device__ __forceinline__ uint32_t kept_threshold(int V, const Values& v, uint3
   return lo;
 }
 
+// Without the minimum of one CTA per SM in its launch bounds, ptxas fits this kernel in 40 registers (three 512-thread
+// CTAs per SM) by spilling to local memory.
 template <typename T>
-__global__ void __launch_bounds__(kThreads) sample_kernel(const pcv_sample_params p) {
+__global__ void __launch_bounds__(kThreads, 1) sample_kernel(const pcv_sample_params p) {
   extern __shared__ __align__(16) float xs[];   // the row's x (V floats)
   __shared__ u64 red[kWarps];
   const int V = p.V, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -285,8 +217,7 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const pcv_sample_param
   const uint32_t lo = kept_threshold(V, p, top, xs);
 
   // ---- draw: warp w owns a contiguous segment of the vocabulary ----
-  const int seg = ((V + kWarps * 32 - 1) / (kWarps * 32)) * 32;
-  const int s0 = warp * seg, s1 = min(V, s0 + seg);
+  const auto [s0, s1] = warp_segment(V);
   u64 part = 0;
   for (int i = s0 + lane; i < s1; i += 32) {
     const float x = xs[i];
@@ -427,10 +358,10 @@ struct Segment {
 template <typename W>
 __device__ __forceinline__ Segment segment_sums(int V, W weight, u128* red) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  const int seg = ((V + kWarps * 32 - 1) / (kWarps * 32)) * 32;
+  const WarpSegment ws = warp_segment(V);
   Segment s;
-  s.s0 = warp * seg;
-  s.s1 = min(V, s.s0 + seg);
+  s.s0 = ws.s0;
+  s.s1 = ws.s1;
   u128 part = 0;
   for (int y = s.s0 + lane; y < s.s1; y += 32) part += weight(y);
 #pragma unroll
@@ -588,20 +519,8 @@ int sample_check(const pcv_sample_params* p) {
 }
 
 int launch_sample(const pcv_sample_params& p, cudaStream_t stream) {
-  const int smem = p.V * (int)sizeof(float);
-  const void* kern = p.dtype == PCV_BF16  ? reinterpret_cast<const void*>(&sample_kernel<__nv_bfloat16>)
-                     : p.dtype == PCV_F16 ? reinterpret_cast<const void*>(&sample_kernel<__half>)
-                                          : reinterpret_cast<const void*>(&sample_kernel<float>);
-  if (smem > 48 * 1024) {   // once per kernel and device, for the largest row
-    const int rc = sm90::set_smem_limit(kern, PCV_SAMPLE_MAX_VOCAB * (int)sizeof(float));
-    if (rc != PCV_OK) return rc;
-  }
-  if (p.dtype == PCV_BF16) sample_kernel<__nv_bfloat16><<<p.R, kThreads, smem, stream>>>(p);
-  else if (p.dtype == PCV_F16) sample_kernel<__half><<<p.R, kThreads, smem, stream>>>(p);
-  else sample_kernel<float><<<p.R, kThreads, smem, stream>>>(p);
-  PCV_CHECK_CUDA(cudaGetLastError());
-  count_launch();
-  return PCV_OK;
+  void (*const kern[3])(pcv_sample_params) = {sample_kernel<__nv_bfloat16>, sample_kernel<__half>, sample_kernel<float>};
+  return launch_row_kernel(kern, p.dtype, p.V, p.R, p, stream);
 }
 
 int launch_sample_uniforms(uint64_t* out, const uint64_t* seeds, const int32_t* positions, int R, int rows_per_batch,
@@ -652,20 +571,10 @@ int spec_verify_check(const pcv_spec_verify_params* p) {
 }
 
 int launch_spec_verify(const pcv_spec_verify_params& p, cudaStream_t stream) {
-  const int smem = p.V * (int)sizeof(float);
-  const void* kern = p.dtype == PCV_BF16  ? reinterpret_cast<const void*>(&spec_verify_kernel<__nv_bfloat16>)
-                     : p.dtype == PCV_F16 ? reinterpret_cast<const void*>(&spec_verify_kernel<__half>)
-                                          : reinterpret_cast<const void*>(&spec_verify_kernel<float>);
-  if (smem > 48 * 1024) {   // once per kernel and device, for the largest row
-    const int rc = sm90::set_smem_limit(kern, PCV_SAMPLE_MAX_VOCAB * (int)sizeof(float));
-    if (rc != PCV_OK) return rc;
-  }
-  const int grid = p.B * (p.G + 1);
-  if (p.dtype == PCV_BF16) spec_verify_kernel<__nv_bfloat16><<<grid, kThreads, smem, stream>>>(p);
-  else if (p.dtype == PCV_F16) spec_verify_kernel<__half><<<grid, kThreads, smem, stream>>>(p);
-  else spec_verify_kernel<float><<<grid, kThreads, smem, stream>>>(p);
-  PCV_CHECK_CUDA(cudaGetLastError());
-  count_launch();
+  void (*const kern[3])(pcv_spec_verify_params) = {
+      spec_verify_kernel<__nv_bfloat16>, spec_verify_kernel<__half>, spec_verify_kernel<float>};
+  const int rc = launch_row_kernel(kern, p.dtype, p.V, p.B * (p.G + 1), p, stream);
+  if (rc != PCV_OK) return rc;
   spec_resolve_kernel<<<(p.B + 127) / 128, 128, 0, stream>>>(p);
   PCV_CHECK_CUDA(cudaGetLastError());
   count_launch();
