@@ -735,8 +735,8 @@ PCV_API int pcv_spec_uniforms(uint64_t* out, const uint64_t* seeds, const int32_
                               int32_t rows_per_batch, int32_t stream_id, void* stream);
 
 /*
- * Beam search: pcv_beam_step runs one step of the Hugging Face GenerationMixin._beam_search (do_sample=False, no logits
- * processors) for B items of K beams each, on state buffers that live on the device.  Beam k of item b is logits row
+ * Beam search: pcv_beam_step runs one step of the Hugging Face GenerationMixin._beam_search (do_sample=False; logits
+ * processors through pcv_logits_process and pcv_beam_step_logprobs) for B items of K beams each, on state buffers that live on the device.  Beam k of item b is logits row
  * b*K + k.  E = n_eos, beams_to_keep = max(2, E + 1) * K (as the Hugging Face code keeps them).  For each item:
  *   1. logp = log_softmax(fp32 logits) per beam row: d_i = (double)x_i - (double)max, S = Σ exp(d_i) in fp64,
  *      logp_i = fp32(d_i - log S);
@@ -793,6 +793,64 @@ typedef struct pcv_beam_step_params {
 /* 1 if pcv_beam_step takes these params, else 0 (reason via pcv_last_error) */
 PCV_API int pcv_beam_step_supported(const pcv_beam_step_params* p);
 PCV_API int pcv_beam_step(const pcv_beam_step_params* p, void* stream);
+/* pcv_beam_step on rows that already are fp32 log-probabilities (pcv_logits_process with log_softmax = 1): step 1 is
+ * skipped, logp_i = x_i, and everything after it is the same.  The same params and refusals, and dtype must be
+ * PCV_F32. */
+PCV_API int pcv_beam_step_logprobs_supported(const pcv_beam_step_params* p);
+PCV_API int pcv_beam_step_logprobs(const pcv_beam_step_params* p, void* stream);
+
+/*
+ * Logits processors: pcv_logits_process applies the Hugging Face RepetitionPenaltyLogitsProcessor (without
+ * prompt_ignore_length), NoRepeatNGramLogitsProcessor and MinNewTokensLengthLogitsProcessor, in that order, to R rows,
+ * one 512-thread CTA per row.  Processed row r reads logits row s = r (row_map NULL) or s = r * row_group + row_map[r]
+ * and writes out row s, fp32:
+ *   0. x = the fp32 logits; with log_softmax = 1, x_i = fp32(d_i - log S), d_i = (double)x_i - (double)max and
+ *      S = Σ exp(d_i) in fp64, exactly as step 1 of pcv_beam_step;
+ *   1. repetition_penalty θ (1: off): every distinct id of the history in [0, V) once, x = x < 0 ? fp32(x * fp32(θ))
+ *      : fp32(x / fp32(θ));
+ *   2. no_repeat_ngram N (0: off), L the history length: if L + 1 >= N, for every start s in [0, L - N + 1) with
+ *      hist[s .. s+N-1) == hist[L-N+1 .. L), x[hist[s+N-1]] = -inf (N = 1 bans every id of the history);
+ *   3. min_new_tokens M (0: off): if L - prompt_len < M, x[eos] = -inf for every EOS id.
+ * Ids outside [0, V) take part in the n-gram matching; their own score is never written.  The history of row r is
+ * history row h = r / rows_per_hist: prefix[h * prefix_stride + 0 .. Lp) then tail[h * tail_stride + 0 .. Lt), where
+ * Lp = prefix_len ? prefix_len[r * prefix_len_stride] : prefix_count and Lt = tail_len ? tail_len[r *
+ * tail_len_stride] : 0 are read when the kernel runs (so one recorded CUDA graph serves every step), each clamped to
+ * [0, its cap].  No floating-point atomics: a row's output is a pure function of its inputs.  Refusals (NULL pointers,
+ * V outside [1, PCV_SAMPLE_MAX_VOCAB], R < 1, an unknown dtype, a stride below V, θ not finite and > 0, N outside [0,
+ * PCV_PROCESS_MAX_NGRAM], M < 0, M > 0 without EOS ids, n_eos outside [0, PCV_PROCESS_MAX_EOS], an EOS id outside
+ * [0, V), rows_per_hist < 1, negative caps, counts or strides) come before any CUDA call, with the reason in
+ * pcv_last_error.
+ */
+#define PCV_PROCESS_MAX_NGRAM 8
+#define PCV_PROCESS_MAX_EOS 4
+
+typedef struct pcv_logits_process_params {
+  const void* logits;          /* rows of `dtype` (PCV_BF16 / PCV_F16 / PCV_F32), unit element stride         */
+  int64_t stride_row;          /* elements between logits rows, >= V                                          */
+  float* out;                  /* fp32 rows, unit element stride                                              */
+  int64_t out_stride_row;      /* elements between out rows, >= V                                             */
+  const int32_t* row_map;      /* device (R) or NULL                                                          */
+  const int64_t* prefix;       /* history prefixes                                                            */
+  int64_t prefix_stride;       /* elements between history rows' prefixes                                     */
+  const int64_t* tail;         /* history tails, or NULL (then tail_len must be NULL)                         */
+  int64_t tail_stride;
+  const int32_t* prefix_len;   /* device or NULL (then prefix_count)                                          */
+  const int32_t* tail_len;     /* device or NULL (then 0)                                                     */
+  int32_t prefix_len_stride, tail_len_stride;
+  int32_t prefix_count, prefix_cap, tail_cap;
+  int32_t R, V, dtype, row_group, rows_per_hist;
+  int32_t log_softmax;         /* 0 or 1                                                                      */
+  float repetition_penalty;
+  int32_t no_repeat_ngram;
+  int32_t min_new_tokens;
+  int32_t prompt_len;          /* the prompt's padded width: new tokens = L - prompt_len                      */
+  int32_t n_eos;
+  int32_t eos[PCV_PROCESS_MAX_EOS];
+} pcv_logits_process_params;
+
+/* 1 if pcv_logits_process takes these params, else 0 (reason via pcv_last_error) */
+PCV_API int pcv_logits_process_supported(const pcv_logits_process_params* p);
+PCV_API int pcv_logits_process(const pcv_logits_process_params* p, void* stream);
 
 /*
  * pcv_kv_gather_rows: after a beam step, every beam row i with parents[i] != i takes its parent's generated rows.  For

@@ -87,6 +87,10 @@ EXPORTS = (
     "pcv_spec_uniforms",
     "pcv_beam_step_supported",
     "pcv_beam_step",
+    "pcv_beam_step_logprobs_supported",
+    "pcv_beam_step_logprobs",
+    "pcv_logits_process_supported",
+    "pcv_logits_process",
     "pcv_kv_gather_rows_supported",
     "pcv_kv_gather_rows",
     "pcv_contrastive_candidates_supported",
@@ -330,6 +334,24 @@ class BeamStepParams(C.Structure):
     ]
 
 
+PROCESS_MAX_NGRAM = 8   # PCV_PROCESS_MAX_NGRAM
+PROCESS_MAX_EOS = 4     # PCV_PROCESS_MAX_EOS
+
+
+class LogitsProcessParams(C.Structure):
+    _fields_ = [
+        ("logits", C.c_void_p), ("stride_row", C.c_int64), ("out", C.c_void_p), ("out_stride_row", C.c_int64),
+        ("row_map", C.c_void_p), ("prefix", C.c_void_p), ("prefix_stride", C.c_int64),
+        ("tail", C.c_void_p), ("tail_stride", C.c_int64), ("prefix_len", C.c_void_p), ("tail_len", C.c_void_p),
+        ("prefix_len_stride", C.c_int32), ("tail_len_stride", C.c_int32),
+        ("prefix_count", C.c_int32), ("prefix_cap", C.c_int32), ("tail_cap", C.c_int32),
+        ("R", C.c_int32), ("V", C.c_int32), ("dtype", C.c_int32), ("row_group", C.c_int32), ("rows_per_hist", C.c_int32),
+        ("log_softmax", C.c_int32), ("repetition_penalty", C.c_float), ("no_repeat_ngram", C.c_int32),
+        ("min_new_tokens", C.c_int32), ("prompt_len", C.c_int32), ("n_eos", C.c_int32),
+        ("eos", C.c_int32 * PROCESS_MAX_EOS),
+    ]
+
+
 class KvGatherEntry(C.Structure):
     _fields_ = [
         ("arena", C.c_void_p), ("scratch", C.c_void_p),
@@ -533,7 +555,13 @@ def lib() -> C.CDLL:
         l.pcv_beam_step.argtypes = [C.POINTER(BeamStepParams), C.c_void_p]
         l.pcv_kv_gather_rows_supported.argtypes = [C.POINTER(KvGatherParams), rows]
         l.pcv_kv_gather_rows.argtypes = [C.POINTER(KvGatherParams), rows, C.c_void_p]
-        for name in ("pcv_beam_step_supported", "pcv_beam_step", "pcv_kv_gather_rows_supported", "pcv_kv_gather_rows"):
+        l.pcv_beam_step_logprobs_supported.argtypes = [C.POINTER(BeamStepParams)]
+        l.pcv_beam_step_logprobs.argtypes = [C.POINTER(BeamStepParams), C.c_void_p]
+        l.pcv_logits_process_supported.argtypes = [C.POINTER(LogitsProcessParams)]
+        l.pcv_logits_process.argtypes = [C.POINTER(LogitsProcessParams), C.c_void_p]
+        for name in ("pcv_beam_step_supported", "pcv_beam_step", "pcv_kv_gather_rows_supported", "pcv_kv_gather_rows",
+                     "pcv_beam_step_logprobs_supported", "pcv_beam_step_logprobs", "pcv_logits_process_supported",
+                     "pcv_logits_process"):
             getattr(l, name).restype = C.c_int
         l.pcv_contrastive_candidates_supported.argtypes = [C.POINTER(ContrastiveCandidatesParams)]
         l.pcv_contrastive_candidates.argtypes = [C.POINTER(ContrastiveCandidatesParams), C.c_void_p]

@@ -388,7 +388,27 @@ int pcv_beam_step_supported(const pcv_beam_step_params* p) { return beam_step_ch
 int pcv_beam_step(const pcv_beam_step_params* p, void* stream) {
   const int rc = beam_step_check(p);
   if (rc != PCV_OK) return rc;
-  return launch_beam_step(*p, reinterpret_cast<cudaStream_t>(stream));
+  return launch_beam_step(*p, false, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pcv_beam_step_logprobs_supported(const pcv_beam_step_params* p) {
+  return beam_step_check(p, true) == PCV_OK ? 1 : 0;
+}
+
+int pcv_beam_step_logprobs(const pcv_beam_step_params* p, void* stream) {
+  const int rc = beam_step_check(p, true);
+  if (rc != PCV_OK) return rc;
+  return launch_beam_step(*p, true, reinterpret_cast<cudaStream_t>(stream));
+}
+
+int pcv_logits_process_supported(const pcv_logits_process_params* p) {
+  return logits_process_check(p) == PCV_OK ? 1 : 0;
+}
+
+int pcv_logits_process(const pcv_logits_process_params* p, void* stream) {
+  const int rc = logits_process_check(p);
+  if (rc != PCV_OK) return rc;
+  return launch_logits_process(*p, reinterpret_cast<cudaStream_t>(stream));
 }
 
 int pcv_kv_gather_rows_supported(const pcv_kv_gather_params* p, const pcv_dev_rows* rows) {

@@ -1,5 +1,6 @@
 // pcv_beam.cu — beam search on the device: one beam step (pcv_beam_step) with the semantics of 🤗's
-// GenerationMixin._beam_search (do_sample=False, no logits processors), and the KV-arena gather of the generated rows
+// GenerationMixin._beam_search (do_sample=False; logits processors through pcv_logits_process and
+// pcv_beam_step_logprobs, which starts from processed log-probabilities), and the KV-arena gather of the generated rows
 // that follows it (pcv_kv_gather_rows).  oracle/beam_oracle.py restates the step in numpy.
 //
 // pcv_beam_step, two launches, no host read:
@@ -35,8 +36,15 @@ __device__ __forceinline__ int keep_count(const pcv_beam_step_params& p) {
   return (p.n_eos + 1 > 2 ? p.n_eos + 1 : 2) * p.K;
 }
 
+// the step's params, and whether its rows already are fp32 log-probabilities (pcv_beam_step_logprobs: logp_i = x_i)
+struct BeamRows {
+  pcv_beam_step_params p;
+  int logprobs;
+};
+
 template <typename T>
-__global__ void __launch_bounds__(kThreads) beam_rows_kernel(const pcv_beam_step_params p) {
+__global__ void __launch_bounds__(kThreads) beam_rows_kernel(const BeamRows a) {
+  const pcv_beam_step_params& p = a.p;
   extern __shared__ __align__(16) float xs[];   // the row's x, then its acc (V floats)
   __shared__ uint32_t ckey[kMaxKeep];
   __shared__ int32_t cidx[kMaxKeep];
@@ -45,12 +53,16 @@ __global__ void __launch_bounds__(kThreads) beam_rows_kernel(const pcv_beam_step
   const T* src = static_cast<const T*>(p.logits) + (int64_t)row * p.stride_row;
 
   // ---- logp and acc ----
-  const RowStats st = stage_max_sum(src, V, xs);
-  const double logS = log(st.S);
   const float run = p.running_scores[row];
-  for (int i = tid; i < V; i += kThreads) {
-    const double d = (double)xs[i] - (double)st.m;
-    xs[i] = __fadd_rn(run, __double2float_rn(d - logS));
+  if (a.logprobs) {
+    for (int i = tid; i < V; i += kThreads) xs[i] = __fadd_rn(run, load_f(src + i));
+  } else {
+    const RowStats st = stage_max_sum(src, V, xs);
+    const double logS = log(st.S);
+    for (int i = tid; i < V; i += kThreads) {
+      const double d = (double)xs[i] - (double)st.m;
+      xs[i] = __fadd_rn(run, __double2float_rn(d - logS));
+    }
   }
 
   // ---- the nsel-th largest key, and the nsel candidates ----
@@ -276,8 +288,11 @@ bool disjoint(const void* a, size_t na, const void* b, size_t nb) {
 
 }  // namespace
 
-int beam_step_check(const pcv_beam_step_params* p) {
+int beam_step_check(const pcv_beam_step_params* p, bool logprobs) {
   PCV_REQUIRE(p != nullptr, PCV_ERR_INVALID, "beam_step: params is NULL");
+  PCV_REQUIRE(!logprobs || p->dtype == PCV_F32, PCV_ERR_INVALID,
+              "beam_step_logprobs: dtype %d must be fp32 (%d): the rows are processed log-probabilities", p->dtype,
+              PCV_F32);
   PCV_REQUIRE(p->logits && p->running_scores && p->finished_scores && p->finished_flags && p->running_hist &&
                   p->finished_hist && p->hist_scratch && p->item_flags && p->counters && p->cand_scores &&
                   p->cand_index && p->next_tokens && p->parents,
@@ -321,10 +336,10 @@ int beam_step_check(const pcv_beam_step_params* p) {
   return PCV_OK;
 }
 
-int launch_beam_step(const pcv_beam_step_params& p, cudaStream_t stream) {
-  void (*const kern[3])(pcv_beam_step_params) = {beam_rows_kernel<__nv_bfloat16>, beam_rows_kernel<__half>,
-                                                 beam_rows_kernel<float>};
-  const int rc = launch_row_kernel(kern, p.dtype, p.V, p.B * p.K, p, stream);
+int launch_beam_step(const pcv_beam_step_params& p, bool logprobs, cudaStream_t stream) {
+  void (*const kern[3])(BeamRows) = {beam_rows_kernel<__nv_bfloat16>, beam_rows_kernel<__half>,
+                                     beam_rows_kernel<float>};
+  const int rc = launch_row_kernel(kern, p.dtype, p.V, p.B * p.K, BeamRows{p, logprobs ? 1 : 0}, stream);
   if (rc != PCV_OK) return rc;
   beam_item_kernel<<<p.B, kThreads, 0, stream>>>(p);
   PCV_CHECK_CUDA(cudaGetLastError());

@@ -177,8 +177,8 @@ int launch_spec_verify(const pcv_spec_verify_params& p, cudaStream_t stream);
 int launch_spec_uniforms(uint64_t* out, const uint64_t* seeds, const int32_t* positions, int R, int rows_per_batch,
                          int stream_id, cudaStream_t stream);
 // beam search (pcv_beam.cu)
-int beam_step_check(const pcv_beam_step_params* p);
-int launch_beam_step(const pcv_beam_step_params& p, cudaStream_t stream);
+int beam_step_check(const pcv_beam_step_params* p, bool logprobs = false);
+int launch_beam_step(const pcv_beam_step_params& p, bool logprobs, cudaStream_t stream);
 int kv_gather_check(const pcv_kv_gather_params* p, const pcv_dev_rows* rows);
 int launch_kv_gather(const pcv_kv_gather_params& p, const pcv_dev_rows& rows, cudaStream_t stream);
 // contrastive search (pcv_contrastive.cu)
@@ -186,5 +186,8 @@ int contrastive_candidates_check(const pcv_contrastive_candidates_params* p);
 int launch_contrastive_candidates(const pcv_contrastive_candidates_params& p, cudaStream_t stream);
 int contrastive_rank_check(const pcv_contrastive_rank_params* p);
 int launch_contrastive_rank(const pcv_contrastive_rank_params& p, cudaStream_t stream);
+// logits processors (pcv_process.cu)
+int logits_process_check(const pcv_logits_process_params* p);
+int launch_logits_process(const pcv_logits_process_params& p, cudaStream_t stream);
 
 }  // namespace pcv

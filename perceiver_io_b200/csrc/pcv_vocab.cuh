@@ -191,11 +191,11 @@ template <typename P>
 int launch_row_kernel(void (*const (&kern)[3])(P), int dtype, int V, int grid, const P& p, cudaStream_t stream) {
   static_assert(PCV_BF16 == 0 && PCV_F16 == 1 && PCV_F32 == 2, "kern[] is indexed by dtype");
   const int smem = V * (int)sizeof(float);
-  if (smem > 48 * 1024) {   // once per kernel and device, for the largest row
-    const int rc = sm90::set_smem_limit(reinterpret_cast<const void*>(kern[dtype]),
-                                        PCV_SAMPLE_MAX_VOCAB * (int)sizeof(float));
-    if (rc != PCV_OK) return rc;
-  }
+  // once per kernel and device, for the largest row: whatever V, since the kernels' static shared memory adds to the
+  // dynamic V floats and can take a V below 48 KB of floats over the default limit
+  const int rc = sm90::set_smem_limit(reinterpret_cast<const void*>(kern[dtype]),
+                                      PCV_SAMPLE_MAX_VOCAB * (int)sizeof(float));
+  if (rc != PCV_OK) return rc;
   kern[dtype]<<<grid, kThreads, smem, stream>>>(p);
   PCV_CHECK_CUDA(cudaGetLastError());
   count_launch();

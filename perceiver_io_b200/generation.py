@@ -55,25 +55,32 @@ model's own filtered distribution.  ``verify`` and :func:`speculative_generate` 
 instead: min(1, p/q) acceptance and a draw from max(0, p - q) on rejection (``ops.spec_verify``), so every emitted token
 is distributed as the target's own draw and a draft is accepted with probability Σ min(p, q).
 
-Beam search: ``beam_search`` runs 🤗's ``_beam_search`` (``do_sample=False``, no logits processors: EOS ids, length
+Beam search: ``beam_search`` runs 🤗's ``_beam_search`` (``do_sample=False``, the processors above: EOS ids, length
 penalty, ``early_stopping`` and ``num_return_sequences`` as 🤗 takes them) with one replay per token: the replay feeds
 the K beams' tokens, runs the device beam step (``ops.beam_step``) on the logits and gathers, by parent, only the arena
 rows generated since the prefill (``ops.kv_gather_rows``): every beam of an item was prefilled with the same prompt, so
 the prompt rows never move.
 
-Contrastive search: ``contrastive_search`` runs 🤗 4.28's ``contrastive_search`` (``penalty_alpha``, ``top_k``, no
-logits processors or warpers) with one replay per token: the replay feeds each item's K candidates on K batch rows,
+Contrastive search: ``contrastive_search`` runs 🤗 4.28's ``contrastive_search`` (``penalty_alpha``, ``top_k``, the
+processors above run in fp32 where 4.28 runs them in the model dtype, no warpers) with one replay per token: the replay feeds each item's K candidates on K batch rows,
 ranks them on the device by model confidence minus the degeneration penalty, the largest cosine between a candidate's
 final hidden row and the item's context of hidden rows (``ops.contrastive_step``), and copies the selected row's newly
 appended arena row into the item's other rows (``ops.kv_gather_rows(..., last_rows=1)``): the K rows of an item share
 every earlier row, so a step moves one row, whatever its length.  The ranking is fp64 where 🤗 computes in the model
 dtype, so on near-ties the two may choose differently.
 
+Logits processors: ``set_sampling``, ``beam_search`` and ``contrastive_search`` take 🤗's ``repetition_penalty``,
+``no_repeat_ngram_size`` and ``min_new_tokens``, run in the graph by ``ops.process_logits`` on an fp32 copy of the
+logits (the log-softmax for beam search), in the order of 🤗's ``_get_logits_processor`` and before temperature /
+top-k / top-p.  A row's history is 🤗's ``input_ids``: the prompt as passed to ``prefill`` and every token fed since,
+which each step graph writes into a token arena at its cross-attention row (so ``rewind`` needs nothing and ``reorder``
+permutes it).  With ``set_sampling`` EOS ids ``generate`` pads a finished row and stops early, as 🤗's ``_sample``.
+
 Not covered: steps of more than 64 tokens, a different k per batch row, a ring buffer bounded at ``max_seq_len`` (the
-arenas grow by ``max_new_tokens`` rows), EOS handling outside beam and contrastive search (callers truncate after EOS),
-beam sampling, contrastive search with sampling or a different top_k per item, per-row sampling values, logits
-processors and warpers (repetition penalties, minimum lengths) in beam and contrastive search, and wiring into 🤗
-``generate()``.
+arenas grow by ``max_new_tokens`` rows), beam sampling, contrastive search with sampling or a different top_k per item,
+per-row sampling or processor values, ``min_length``, bad-words lists, forced tokens, min-p, logits processors under
+speculative verification (``verify``, ``speculative_generate``, ``generate(logits=True)`` refuse them), and wiring
+into 🤗 ``generate()``.
 """
 from __future__ import annotations
 
@@ -198,6 +205,30 @@ def _sampling_triple(what: str, temperature, top_k, top_p):
     return t, min(k, 2 ** 31 - 1), p
 
 
+_NO_PROCESS = (1.0, 0, 0)   # (repetition_penalty, no_repeat_ngram_size, min_new_tokens) with every processor off
+
+
+def _process_values(what: str, repetition_penalty, no_repeat_ngram_size, min_new_tokens, eos):
+    """(θ, N, M) checked as ``ops.process_logits`` takes them; M > 0 needs EOS ids (🤗 drops the processor silently
+    there; this refuses)."""
+    t, n, m = repetition_penalty, _as_count(no_repeat_ngram_size), _as_count(min_new_tokens)
+    # the kernel takes θ in fp32: it must stay finite and > 0 there
+    t32 = float(torch.tensor(float(t), dtype=torch.float32)) if isinstance(t, (int, float)) else math.nan
+    if isinstance(t, bool) or not isinstance(t, (int, float)) or not math.isfinite(t32) or not t32 > 0:
+        raise ValueError(f"{what}: repetition_penalty must be a number > 0 that is finite and > 0 in fp32 (1: off), got "
+                         f"{repetition_penalty!r}")
+    if n is None or not 0 <= n <= ops.PROCESS_MAX_NGRAM:
+        raise ValueError(f"{what}: no_repeat_ngram_size must be an integer in [0, {ops.PROCESS_MAX_NGRAM}] (0: off), got "
+                         f"{no_repeat_ngram_size!r}")
+    if m is None or not 0 <= m < 2 ** 31:
+        raise ValueError(f"{what}: min_new_tokens must be an integer >= 0 (0: off), got {min_new_tokens!r}")
+    if m > 0 and not eos:
+        raise ValueError(f"{what}: min_new_tokens={m} needs eos_token_id (it bans the EOS ids until {m} tokens are new)")
+    if len(eos) > ops.PROCESS_MAX_EOS:
+        raise ValueError(f"{what}: at most {ops.PROCESS_MAX_EOS} EOS ids, got {len(eos)}")
+    return float(t), n, m
+
+
 class BeamSearchOutput(NamedTuple):
     sequences: torch.Tensor   # (B, R, n) int64 generated tokens, the output fill value after a hypothesis's end
     scores: torch.Tensor      # (B, R) fp32, 🤗's sequences_scores
@@ -235,6 +266,10 @@ class GraphedDecoder:
     _cs_state = None                  # ops.ContrastiveState of the last contrastive_search
     _cs_table = None                  # ops.KvGatherTable of the last contrastive_search (its scratch is reused)
     _hidden = None                    # the final hidden rows (B, k, D) of the last _step_fn call
+    _tokens = None                    # (B, n0 + max_new_tokens) int64: the prompt and every fed token, by arena row
+    _process = _NO_PROCESS            # the sampling graphs' (repetition_penalty, no_repeat_ngram_size, min_new_tokens)
+    _eos = ()                         # the sampling EOS ids, and the token fed after one
+    _pad_token = None
 
     def __init__(self, model, batch: int, max_new_tokens: int, kv_cache: str = "bf16"):
         if max_new_tokens < 1:
@@ -328,6 +363,10 @@ class GraphedDecoder:
             if self.fp8:
                 a.kv8 = modules._kv8_scales(a.owner, a.norms, rotate_dim if a.rotary else 0)
                 a.k_inv_h = 1.0 / a.kv8.k_descale.float().contiguous()
+        self._tokens = torch.zeros(B, caps[0], dtype=torch.int64, device=dev)
+        self._tokens[:, :n0].copy_(input_ids)
+        self._n0 = n0
+        self._unfinished = torch.ones(B, 1, dtype=torch.bool, device=dev)
         self._pad = torch.zeros(B, caps[0], dtype=torch.uint8, device=dev)
         if pad_mask is not None:
             self._pad[:, :n0].copy_(pad_mask != 0)
@@ -373,6 +412,10 @@ class GraphedDecoder:
         adapter = m.input_adapter
         k = token.shape[1]
         b = self._bounds if k == 1 else extend_bounds(self._bounds, k)
+        # the token history: each fed token at its cross-attention row (clamped: warm-up calls may run past the arena,
+        # and every row at or past the current one is written again before it is read)
+        rows = b[:, 0, 2:3] if k == 1 else b[:, 0, 2:3] + (self._steps[:k] - 1)
+        self._tokens.scatter_(1, rows.clamp_max(self._tokens.shape[1] - 1).long(), token)
         x = adapter.txt_embedding(token)
         if getattr(adapter, "_abs_pos_emb", False):
             pos = (window_positions(self._pad, b[:, 0, 0:2], self._cols) if k == 1
@@ -407,8 +450,33 @@ class GraphedDecoder:
         logits = self._step_fn(token)
         if k == 1:
             logits = logits[:, None]
+        logits = self._processed(logits, pos)
         t, top_k, top_p = self._sampling
         return ops.sample_tokens(logits, self._seeds, pos, t, top_k, top_p), logits
+
+    def _processed(self, logits: torch.Tensor, pos: torch.Tensor) -> torch.Tensor:
+        """``logits`` (B, k, V) through the ``set_sampling`` processors (fp32), or as they are when every one is off.
+        The draw at position p sees the history's first p tokens (🤗's input_ids at that draw)."""
+        if self._process == _NO_PROCESS:
+            return logits
+        B, k, V = logits.shape
+        theta, N, M = self._process
+        return ops.process_logits(logits.reshape(B * k, V), self._tokens, pos.reshape(-1), rows_per_hist=k,
+                                  repetition_penalty=theta, no_repeat_ngram_size=N, min_new_tokens=M,
+                                  prompt_len=self._n0, eos=self._eos).view(B, k, V)
+
+    def _generate_fn(self, token: torch.Tensor):
+        """_sample_fn with 🤗 ``_sample``'s EOS rule: a finished row's draw is replaced by the pad token."""
+        tokens, logits = self._sample_fn(token)
+        tokens = torch.where(self._unfinished, tokens, self._pad_token)
+        self._unfinished &= ~self._is_eos(tokens)
+        return tokens, logits
+
+    def _is_eos(self, tokens: torch.Tensor) -> torch.Tensor:
+        hit = tokens == self._eos[0]
+        for e in self._eos[1:]:
+            hit |= tokens == e
+        return hit
 
     def _verify_fn(self, token: torch.Tensor, draft_logits: torch.Tensor):
         """_step_fn followed by ``ops.spec_verify`` on its logits: (tokens (B, k), accepted (B,))."""
@@ -437,12 +505,17 @@ class GraphedDecoder:
             raise RuntimeError("GraphedDecoder does not run under autocast")
         sample = fn in ("sample", "generate")
         key = ("sample", k, self._sampling) if sample else k
+        if sample and self._process != _NO_PROCESS:
+            key += (self._process, self._eos)
         fwd = self._sample_fn if sample else self._step_fn
+        if fn == "generate" and self._eos:
+            key, fwd = ("generate", self._sampling, self._process, self._eos, self._pad_token), self._generate_fn
         if fn == "verify":
             key, fwd = ("verify", k, self._sampling, self._draft_sampling), self._verify_fn
         graph = self._graphs.get(key)
         if graph is None:
             snapshot = self._bounds.clone()   # the warm-up calls advance the rows; their arena writes are rewritten later
+            unfinished = self._unfinished.clone()   # and may finish rows of the generate graph
             old = torch.cuda.get_sync_debug_mode()
             torch.cuda.set_sync_debug_mode(0)  # recording a graph synchronises the device once
             try:
@@ -450,6 +523,7 @@ class GraphedDecoder:
             finally:
                 torch.cuda.set_sync_debug_mode(old)
             self._bounds.copy_(snapshot)
+            self._unfinished.copy_(unfinished)
             self._graphs[key] = graph
             self.captures += 1
         out = graph(token_ids, *extra)
@@ -495,11 +569,34 @@ class GraphedDecoder:
         self._seeds.copy_(host, non_blocking=True)
         self._seeded = True
 
-    def set_sampling(self, temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0) -> None:
+    def set_sampling(self, temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0, *,
+                     repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0, min_new_tokens: int = 0,
+                     eos_token_id=None, pad_token_id=None) -> None:
         """The sampler's values for ``draw``, ``sample`` and ``generate``: ``temperature`` >= 0 (0: greedy), ``top_k`` >= 0
-        (0: off), ``top_p`` in (0, 1] (1: off), as ``ops.sample_tokens`` takes them.  The first replay under a new triple
-        records its graphs."""
-        self._sampling = _sampling_triple("GraphedDecoder.set_sampling", temperature, top_k, top_p)
+        (0: off), ``top_p`` in (0, 1] (1: off), as ``ops.sample_tokens`` takes them.
+
+        Before them, 🤗's logits processors run on an fp32 copy of the logits (``ops.process_logits``), in the order of
+        🤗's ``_get_logits_processor``: ``repetition_penalty`` θ > 0 (1: off), ``no_repeat_ngram_size`` N in [0, 8] (0:
+        off) and ``min_new_tokens`` M >= 0 (0: off; needs ``eos_token_id``), counted from the prompt's padded width.  A
+        row's history is the prompt as passed to ``prefill`` and every token fed to that row since (the draw at the row
+        a token will take sees every earlier row).  ``eos_token_id`` (an id or a list) also makes ``generate`` stop:
+        see there; ``pad_token_id`` is what a finished row is fed (None: the first EOS id).  The first replay under
+        new values records their graphs; with every processor off and no EOS ids the graphs are the plain sampling
+        ones.  Invalid values are refused with the reason, leaving the old values in place."""
+        what = "GraphedDecoder.set_sampling"
+        sampling = _sampling_triple(what, temperature, top_k, top_p)
+        eos = tuple(_eos_ids(eos_token_id, what))
+        process = _process_values(what, repetition_penalty, no_repeat_ngram_size, min_new_tokens, eos)
+        vocab = self.model.config.vocab_size
+        if any(not 0 <= e < vocab for e in eos):
+            raise ValueError(f"{what}: every EOS id must be in [0, {vocab}), got {list(eos)}")
+        pad = None
+        if eos:
+            pad = eos[0] if pad_token_id is None else _as_count(pad_token_id)
+            if pad is None or not 0 <= pad < vocab:
+                raise ValueError(f"{what}: pad_token_id must be None or an id in [0, {vocab}) (it is fed after an EOS), "
+                                 f"got {pad_token_id!r}")
+        self._sampling, self._process, self._eos, self._pad_token = sampling, process, eos, pad
 
     def _ready_to_sample(self, what: str) -> None:
         if self._bounds is None:
@@ -519,7 +616,7 @@ class GraphedDecoder:
             raise ValueError(f"GraphedDecoder.draw takes ({self.batch}, vocab) logits, got {tuple(logits.shape)}")
         t, top_k, top_p = self._sampling
         pos = sample_positions(self._bounds, self._steps, 1) - 1
-        return ops.sample_tokens(logits[:, None], self._seeds, pos, t, top_k, top_p)
+        return ops.sample_tokens(self._processed(logits[:, None], pos), self._seeds, pos, t, top_k, top_p)
 
     def sample(self, token_ids: torch.Tensor):
         """Feed the k tokens ``token_ids`` (B, k) int64, 1 <= k <= 64, in one replay and return ``(tokens, logits)``:
@@ -529,24 +626,38 @@ class GraphedDecoder:
         self._ready_to_sample("sample")
         return self._replay(token_ids, "sample")
 
-    def generate(self, first_tokens: torch.Tensor, n: int, logits: bool = False):
+    def generate(self, first_tokens: torch.Tensor, n: int, logits: bool = False, check_every: int = 16):
         """Feed ``first_tokens`` (B, 1) int64 and then every drawn token, for n replays of the one-token sampling graph;
         return the n drawn tokens (B, n) int64.  Each replay's input is copied on the device from the previous one's
         output: no host read and no synchronisation.  Consumes n tokens of the budget; asking for more than remain is
         refused before any replay, leaving the state untouched.  With ``logits=True`` also return the logits each token
         was drawn from, (B, n, vocab), copied on the device after each replay (a draft model's probabilities for
-        :meth:`verify`)."""
+        :meth:`verify`; refused while a ``set_sampling`` processor is on).
+
+        With ``set_sampling`` EOS ids, 🤗 ``_sample``'s rule: a row that has emitted an EOS id (``first_tokens``
+        included) is fed, and returns, the pad token from then on; the device's "every row finished" flag is read
+        every ``check_every`` replays and the loop stops once it is set.  The output stays (B, n), padded; replays not
+        run stay in the budget."""
         self._ready_to_sample("generate")
-        count = _as_count(n)
+        count, every = _as_count(n), _as_count(check_every)
         if count is None or count < 1:
             raise ValueError(f"GraphedDecoder.generate: n must be an integer >= 1, got {n!r}")
+        if every is None or every < 1:
+            raise ValueError(f"GraphedDecoder.generate: check_every must be an integer >= 1, got {check_every!r}")
+        if logits and self._process != _NO_PROCESS:
+            raise ValueError("GraphedDecoder.generate: logits=True (a draft's distribution for verify) is not covered "
+                             "with logits processors on")
         if self._remaining < count:
             raise RuntimeError(f"GraphedDecoder.generate: {self._remaining} of max_new_tokens={self.max_new_tokens} "
                                f"tokens remain to the furthest batch row, {count} asked for")
         if tuple(first_tokens.shape) != (self.batch, 1) or first_tokens.dtype != torch.long:
             raise ValueError(f"GraphedDecoder.generate takes ({self.batch}, 1) int64 first tokens, got "
                              f"{tuple(first_tokens.shape)} {first_tokens.dtype}")
-        out = torch.empty(self.batch, count, dtype=torch.long, device=self.device)
+        if self._eos:
+            out = torch.full((self.batch, count), self._pad_token, dtype=torch.long, device=self.device)
+            torch.logical_not(self._is_eos(first_tokens), out=self._unfinished)
+        else:
+            out = torch.empty(self.batch, count, dtype=torch.long, device=self.device)
         kept = None
         tokens = first_tokens
         for i in range(count):
@@ -556,6 +667,15 @@ class GraphedDecoder:
                 if kept is None:
                     kept = torch.empty(self.batch, count, lg.shape[-1], dtype=lg.dtype, device=self.device)
                 kept[:, i:i + 1].copy_(lg)
+            if self._eos and (i + 1) % every == 0 and i + 1 < count:
+                old = torch.cuda.get_sync_debug_mode()
+                torch.cuda.set_sync_debug_mode(0)
+                try:
+                    stop = not bool(self._unfinished.any().item())   # the one host read: every row finished
+                finally:
+                    torch.cuda.set_sync_debug_mode(old)
+                if stop:
+                    break
         return (out, kept) if logits else out
 
     def verify(self, token_ids: torch.Tensor, draft_logits: torch.Tensor, draft_sampling=(1.0, 0, 1.0)):
@@ -570,6 +690,9 @@ class GraphedDecoder:
         until the next replay; nothing is read back to the host.  Consumes G+1 tokens of the budget: the caller then
         rewinds row b by G - n_b.  The graph is recorded on first use, one per (G, target values, draft values)."""
         self._ready_to_sample("verify")
+        if self._process != _NO_PROCESS:
+            raise ValueError("GraphedDecoder.verify: speculative verification is not covered with logits processors on "
+                             "(the draft's processed distribution)")
         draft = _sampling_triple("GraphedDecoder.verify: draft_sampling", *_triple(draft_sampling))
         k = token_ids.shape[1] if token_ids.dim() == 2 else 0
         if not 2 <= k <= ops.SPEC_MAX_DRAFTS + 1:
@@ -618,8 +741,9 @@ class GraphedDecoder:
 
     def beam_search(self, input_ids: torch.Tensor, prefix_len: int, n: int, num_beams: int, pad_mask=None,
                     eos_token_id=None, pad_token_id=None, length_penalty: float = 1.0, early_stopping=False,
-                    num_return_sequences: int = 1, check_every: int = 16) -> BeamSearchOutput:
-        """🤗's beam search (``GenerationMixin._beam_search`` with ``do_sample=False`` and no logits processors) of n
+                    num_return_sequences: int = 1, check_every: int = 16, repetition_penalty: float = 1.0,
+                    no_repeat_ngram_size: int = 0, min_new_tokens: int = 0) -> BeamSearchOutput:
+        """🤗's beam search (``GenerationMixin._beam_search`` with ``do_sample=False``) of n
         generated tokens for the B prompts ``input_ids`` (B, n0), with K = ``num_beams`` beams each; the decoder's batch
         must be B * K.  Returns ``BeamSearchOutput(sequences, scores)``: 🤗's ``sequences[:, :num_return_sequences]``
         (generated part, (B, R, n) int64, the output fill value — ``pad_token_id or eos_token_id[0]`` with EOS ids, else
@@ -632,10 +756,18 @@ class GraphedDecoder:
         EOS ids, the device's "every item done" flag is read every ``check_every`` replays and the loop stops once it
         is set (🤗's stop condition; a stopped item's finished set no longer changes, so the output is the same);
         without, nothing is read until the end.  The graph is recorded on first use after each prefill, keyed by (K, EOS
-        ids, length_penalty, early_stopping).  Refusals come before any replay."""
+        ids, length_penalty, early_stopping).  Refusals come before any replay.
+
+        ``repetition_penalty``, ``no_repeat_ngram_size`` and ``min_new_tokens`` are 🤗's logits processors, as
+        ``set_sampling`` takes them (``min_new_tokens`` needs EOS ids): 🤗 runs them on the fp32 log-softmax of every
+        beam's logits, with the prompt and the beam's own generated tokens as its history, so the step and every replay
+        then run ``ops.process_logits(..., log_softmax=True)`` and ``ops.beam_step(..., logprobs=True)``.  With every
+        processor off the graph is the plain one."""
         B = input_ids.shape[0] if input_ids.dim() == 2 else 0
         K, count, eos, lp, es, R, every = self._beam_args(B, n, num_beams, eos_token_id, length_penalty,
                                                           early_stopping, num_return_sequences, check_every)
+        process = _process_values("GraphedDecoder.beam_search", repetition_penalty, no_repeat_ngram_size,
+                                  min_new_tokens, eos)
         if torch.is_autocast_enabled():
             raise RuntimeError("GraphedDecoder does not run under autocast")
         fill = (pad_token_id or eos[0]) if eos else -1
@@ -655,13 +787,25 @@ class GraphedDecoder:
             [(t, first[a.group], a.group * _NCOL + 2) for a in self._layers for t in (a.K, a.V, a.S) if t is not None],
             reuse=self._beam_table)
         rows = self._bounds.view(self.batch, -1)
+        on = process != _NO_PROCESS
+        if on:
+            logp = torch.empty(self.batch, self.model.config.vocab_size, dtype=torch.float32, device=self.device)
+            hist = state.running_hist.view(self.batch, -1)
+
+        def step(logits):   # the beam step, after the processors on the log-softmax when one is on
+            if not on:
+                return ops.beam_step(logits, state, eos, lp, es)
+            ops.process_logits(logits, self._tokens, n0, tail=hist, tail_len=state.counters[0:1], out=logp,
+                               log_softmax=True, repetition_penalty=process[0], no_repeat_ngram_size=process[1],
+                               min_new_tokens=process[2], prompt_len=n0, eos=eos)
+            return ops.beam_step(logp, state, eos, lp, es, logprobs=True)
 
         def beam_fn(token):
-            tokens, parents = ops.beam_step(self._step_fn(token), state, eos, lp, es)
+            tokens, parents = step(self._step_fn(token))
             ops.kv_gather_rows(table, parents, rows)
             return tokens
 
-        gkey = ("beam", K, tuple(eos), lp, str(es))
+        gkey = ("beam", K, tuple(eos), lp, str(es)) + ((process,) if on else ())
         state.reset(count)
         if count > 1 and gkey not in self._graphs:
             # recorded before the first step: the warm-up calls append, and gather, only rows that are rewritten later
@@ -675,7 +819,7 @@ class GraphedDecoder:
             self._bounds.copy_(snapshot)
             self.captures += 1
             state.reset(count)
-        ops.beam_step(logits, state, eos, lp, es)
+        step(logits)
         graph = self._graphs.get(gkey)
         for i in range(count - 1):
             graph(state.tokens)
@@ -729,8 +873,10 @@ class GraphedDecoder:
         return K, count, float(penalty_alpha), eos, pad, every
 
     def contrastive_search(self, input_ids: torch.Tensor, prefix_len: int, n: int, penalty_alpha: float, top_k: int,
-                           pad_mask=None, eos_token_id=None, pad_token_id=None, check_every: int = 16) -> torch.Tensor:
-        """🤗 4.28's contrastive search (``GenerationMixin.contrastive_search`` with no logits processors or warpers) of
+                           pad_mask=None, eos_token_id=None, pad_token_id=None, check_every: int = 16,
+                           repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0,
+                           min_new_tokens: int = 0) -> torch.Tensor:
+        """🤗 4.28's contrastive search (``GenerationMixin.contrastive_search`` without warpers) of
         n generated tokens for the B prompts ``input_ids`` (B, n0), with K = ``top_k`` candidates and α =
         ``penalty_alpha``; the decoder's batch must be B * K and n <= ``max_new_tokens``.  Returns the generated tokens
         (B, n) int64: ``pad_token_id`` after an item has emitted an EOS id (``pad_token_id=None`` with EOS ids means the
@@ -749,10 +895,18 @@ class GraphedDecoder:
         other rows (``ops.kv_gather_rows(..., last_rows=1)``).  Each replay's input is its predecessor's output.  With
         EOS ids the device's "every item finished" flag is read every ``check_every`` replays and the loop stops once
         it is set; nothing else is read.  The graph is recorded once after each prefill, keyed by (K, α, EOS ids, pad).
-        Refusals come before any replay."""
+        Refusals come before any replay.
+
+        ``repetition_penalty``, ``no_repeat_ngram_size`` and ``min_new_tokens`` are 🤗's logits processors, as
+        ``set_sampling`` takes them (``min_new_tokens`` needs EOS ids): they run on the selected row's logits, with the
+        prompt and the tokens emitted so far as its history, before the softmax and top-k that pick the candidates
+        (the first candidates included), through ``ops.process_logits``.  4.28 runs them in the model dtype; here they
+        run in fp32, like the ranking's fp64, so on near-ties the two may choose differently."""
         B = input_ids.shape[0] if input_ids.dim() == 2 else 0
         K, count, alpha, eos, pad, every = self._contrastive_args(B, n, penalty_alpha, top_k, eos_token_id, pad_token_id,
                                                                   check_every)
+        process = _process_values("GraphedDecoder.contrastive_search", repetition_penalty, no_repeat_ngram_size,
+                                  min_new_tokens, eos)
         if torch.is_autocast_enabled():
             raise RuntimeError("GraphedDecoder does not run under autocast")
 
@@ -776,18 +930,26 @@ class GraphedDecoder:
             [(t, first[a.group], a.group * _NCOL + 2) for a in self._layers for t in (a.K, a.V, a.S) if t is not None],
             reuse=self._cs_table)
         rows = self._bounds.view(self.batch, -1)
+        proc = None
+        if process != _NO_PROCESS:
+            # the selected row of every item, with the item's prompt (its row b*K) and emitted tokens as its history
+            proc = dict(prefix=self._tokens[::K], prefix_len=n0, tail=state.history, tail_len=state.counters[1:2],
+                        out=torch.empty(self.batch, logits.shape[-1], dtype=torch.float32, device=self.device),
+                        repetition_penalty=process[0], no_repeat_ngram_size=process[1], min_new_tokens=process[2],
+                        prompt_len=n0, eos=eos)
 
         def cs_fn(token):
             logits = self._step_fn(token)
-            tokens, parents = ops.contrastive_step(logits, self._hidden, state, alpha, eos)
+            tokens, parents = ops.contrastive_step(logits, self._hidden, state, alpha, eos, process=proc)
             ops.kv_gather_rows(table, parents, rows, last_rows=1)
             return tokens
 
         def start():
             state.reset(hidden, ctx_pad)
-            ops.contrastive_candidates(logits, state)
+            first = logits if proc is None else ops.process_logits(logits, row_map=state.sel, **proc)
+            ops.contrastive_candidates(first, state)
 
-        gkey = ("contrastive", K, alpha, tuple(eos), pad)
+        gkey = ("contrastive", K, alpha, tuple(eos), pad) + ((process,) if proc is not None else ())
         start()
         if gkey not in self._graphs:
             # the warm-up calls append, and select, only rows that the replays rewrite; the state is reloaded after
@@ -888,6 +1050,8 @@ class GraphedDecoder:
                 if t is not None:
                     t.copy_(t.index_select(0, idx))
         self._pad.copy_(self._pad.index_select(0, idx))
+        if self._tokens is not None:
+            self._tokens.copy_(self._tokens.index_select(0, idx))
         self._bounds.copy_(self._bounds.index_select(0, idx))
         if self._seeds is not None:
             self._seeds.copy_(self._seeds.index_select(0, idx))
@@ -936,6 +1100,9 @@ def speculative_generate(target: "GraphedDecoder", draft: "GraphedDecoder", firs
                          f"target's {target.model.config.vocab_size}")
     if target._bounds is None or draft._bounds is None:
         raise RuntimeError("speculative_generate: prefill() both decoders first")
+    if target._process != _NO_PROCESS or draft._process != _NO_PROCESS:
+        raise ValueError("speculative_generate: not covered with logits processors on (the draft's processed "
+                         "distribution)")
     if tuple(first.shape) != (B, 1) or first.dtype != torch.long:
         raise ValueError(f"speculative_generate takes ({B}, 1) int64 first tokens, got {tuple(first.shape)} "
                          f"{first.dtype}")

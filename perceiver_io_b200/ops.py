@@ -1521,13 +1521,16 @@ class BeamState:
         self.counters[1:2].fill_(int(max_length))   # fill_ with a host scalar: a kernel argument, no copy or sync
 
 
-def beam_step(logits: torch.Tensor, state: BeamState, eos=(), length_penalty: float = 1.0, early_stopping=False):
-    """One step of 🤗's beam search (``do_sample=False``, no logits processors) on the device (pcv_beam_step), in place
+def beam_step(logits: torch.Tensor, state: BeamState, eos=(), length_penalty: float = 1.0, early_stopping=False,
+              logprobs: bool = False):
+    """One step of 🤗's beam search (``do_sample=False``) on the device (pcv_beam_step), in place
     on ``state``: logits (B*K, V) bf16 / fp16 / fp32, V <= :data:`SAMPLE_MAX_VOCAB`, beam k of item b in row b*K + k.
     Returns ``(state.tokens, state.parents)``: the (B*K, 1) int64 next tokens and the (B*K,) int32 global beam row each
     beam continues.  Nothing is read back to the host, so the call can be recorded in a CUDA graph: the generated count
-    and max_length live in ``state.counters``.  Arguments the kernel does not take raise ``ValueError`` with its reason
-    before any launch."""
+    and max_length live in ``state.counters``.  With ``logprobs=True`` the rows are fp32 log-probabilities already
+    (:func:`process_logits` with ``log_softmax=True``: 🤗's processors run on the log-softmax) and the step starts from
+    them (pcv_beam_step_logprobs).  Arguments the kernel does not take raise ``ValueError`` with its reason before any
+    launch."""
     _require_cuda(logits)
     if logits.dim() != 2 or logits.dtype not in (torch.bfloat16, torch.float16, torch.float32):
         raise ValueError(f"beam_step: logits must be (B*K, V) bf16 / fp16 / fp32, got {tuple(logits.shape)} "
@@ -1554,10 +1557,11 @@ def beam_step(logits: torch.Tensor, state: BeamState, eos=(), length_penalty: fl
         setattr(p, {"running": "running_scores", "finished": "finished_scores"}.get(f, f), getattr(state, f).data_ptr())
     p.next_tokens, p.parents = state.tokens.data_ptr(), state.parents.data_ptr()
     lib = _lib.lib()
-    if not lib.pcv_beam_step_supported(C.byref(p)):
+    entry = "pcv_beam_step_logprobs" if logprobs else "pcv_beam_step"
+    if not getattr(lib, entry + "_supported")(C.byref(p)):
         raise ValueError(f"beam_step: {lib.pcv_last_error().decode()}")
     with torch.cuda.device(logits.device):
-        check(lib.pcv_beam_step(C.byref(p), _stream()), "pcv_beam_step")
+        check(getattr(lib, entry)(C.byref(p), _stream()), entry)
     return state.tokens, state.parents
 
 
@@ -1735,15 +1739,19 @@ def contrastive_candidates(logits: torch.Tensor, state: ContrastiveState) -> tor
     return state.tokens
 
 
-def contrastive_step(logits: torch.Tensor, hidden: torch.Tensor, state: ContrastiveState, alpha: float, eos=()):
+def contrastive_step(logits: torch.Tensor, hidden: torch.Tensor, state: ContrastiveState, alpha: float, eos=(),
+                     process: Optional[dict] = None):
     """One step of contrastive search after the model ran candidate j of item b at row b*K + j: ranks the candidates of
     the last :func:`contrastive_candidates` by ``(1 - alpha) p_j - alpha * max cos(context, h_j)`` in fp64, emits the
     best one (``state.fill`` once the item has emitted an EOS id) into ``state.history``, appends its hidden row to the
     context (pcv_contrastive_rank), then takes the next candidates from its logits row.  ``logits`` (B*K, V) and
     ``hidden`` (B*K, D) or (B*K, 1, D) of ``state.dtype``: the candidate pass's outputs.  Returns ``(state.tokens,
     state.parents)``: the next inputs and the batch row each row continues (for ``kv_gather_rows(..., last_rows=1)``).
-    Nothing is read back to the host, so the call can be recorded in a CUDA graph; arguments the kernels do not take
-    raise ``ValueError`` before any launch."""
+    ``process``, if given, holds the keyword arguments of :func:`process_logits` (``row_map`` excepted: it is
+    ``state.sel``): 🤗's logits processors run on the selected rows between the ranking and the candidates, when
+    ``state.sel`` and ``state.history`` hold this step's selection, and the candidates are taken from the fp32 rows
+    they write (``process["out"]``, (B*K, V) fp32, allocated when absent).  Nothing is read back to the host, so the
+    call can be recorded in a CUDA graph; arguments the kernels do not take raise ``ValueError`` before any launch."""
     rows = _logits_rows(logits, state, "contrastive_step")
     _require_cuda(hidden)
     BK, D = state.B * state.K, state.D
@@ -1770,9 +1778,14 @@ def contrastive_step(logits: torch.Tensor, hidden: torch.Tensor, state: Contrast
     lib = _lib.lib()
     if not lib.pcv_contrastive_rank_supported(C.byref(p)):
         raise ValueError(f"contrastive_step: {lib.pcv_last_error().decode()}")
+    pp = None
+    if process is not None:
+        pp, rows = _process_params(rows, row_map=state.sel, **process)
     q = _candidates_params(rows, state)
     with torch.cuda.device(logits.device):
         check(lib.pcv_contrastive_rank(C.byref(p), _stream()), "pcv_contrastive_rank")
+        if pp is not None:
+            check(lib.pcv_logits_process(C.byref(pp), _stream()), "pcv_logits_process")
         check(lib.pcv_contrastive_candidates(C.byref(q), _stream()), "pcv_contrastive_candidates")
     return state.tokens, state.parents
 
@@ -2233,3 +2246,130 @@ def ln_linear(x: torch.Tensor, norm_weight: Optional[torch.Tensor], norm_bias: O
     beta = None if norm_bias is None else norm_bias.to(dt)
     outs = _LnLinear.apply(x, gamma, beta, w.contiguous(), b, w_cat, col_st, n_k, n_v, float(eps))
     return (outs[0], outs[1]) if (n_k and n_v) else ((outs[0], None) if n_k else (None, outs[0]))
+
+
+# --------------------------------------------------------------------------------------------------
+# logits processors (pcv_logits_process): 🤗's repetition penalty, n-gram blocking and minimum new tokens on fp32 rows,
+# with the token histories and their lengths on the device, recordable in a CUDA graph.
+# --------------------------------------------------------------------------------------------------
+#: The largest no_repeat_ngram_size and EOS count :func:`process_logits` takes.
+PROCESS_MAX_NGRAM = _lib.PROCESS_MAX_NGRAM
+PROCESS_MAX_EOS = _lib.PROCESS_MAX_EOS
+
+
+def _history(what: str, ids, length, R: int, per: int, device):
+    """(pointer, row stride, cap, length pointer, length stride, count) of one history segment."""
+    _require_cuda(ids)
+    if ids.dtype != torch.int64 or ids.dim() != 2 or ids.stride(1) != 1:
+        raise ValueError(f"process_logits: {what} must be a (rows, cap) int64 tensor with unit column stride, got "
+                         f"{tuple(ids.shape)} {ids.dtype}")
+    need = -(-R // per)
+    if ids.shape[0] < need:
+        raise ValueError(f"process_logits: {what} has {ids.shape[0]} rows; {R} processed rows at {per} per history "
+                         f"row read {need}")
+    if ids.device != device:
+        raise ValueError(f"process_logits: {what} is on {ids.device}, the logits on {device}")
+    if isinstance(length, torch.Tensor):
+        _require_cuda(length)
+        if length.device != device:
+            raise ValueError(f"process_logits: {what}_len is on {length.device}, the logits on {device}")
+        if length.dtype != torch.int32 or length.numel() not in (1, R) or (length.numel() == R and R > 1 and (
+                length.dim() != 1 or length.stride(0) != 1)):
+            raise ValueError(f"process_logits: {what}_len must be an int32 tensor of 1 or ({R},) elements, got "
+                             f"{tuple(length.shape)} {length.dtype}")
+        return ids.data_ptr(), ids.stride(0), ids.shape[1], length.data_ptr(), 1 if length.numel() > 1 else 0, 0
+    n = _as_int(length)
+    if n is None or not 0 <= n <= ids.shape[1]:
+        raise ValueError(f"process_logits: {what}_len must be an integer in [0, {ids.shape[1]}] or an int32 CUDA "
+                         f"tensor, got {length!r}")
+    return ids.data_ptr(), ids.stride(0), ids.shape[1], None, 0, n
+
+
+def process_logits(logits: torch.Tensor, prefix: torch.Tensor, prefix_len, *, tail: Optional[torch.Tensor] = None,
+                   tail_len: Optional[torch.Tensor] = None, rows_per_hist: int = 1, row_map: Optional[torch.Tensor] = None,
+                   out: Optional[torch.Tensor] = None, log_softmax: bool = False, repetition_penalty: float = 1.0,
+                   no_repeat_ngram_size: int = 0, min_new_tokens: int = 0, prompt_len: int = 0, eos=()) -> torch.Tensor:
+    """🤗's ``RepetitionPenaltyLogitsProcessor`` -> ``NoRepeatNGramLogitsProcessor`` -> ``MinNewTokensLengthLogitsProcessor``
+    on the device (pcv_logits_process), on fp32 rows; the rule is stated in ``include/pcv_attn.h``.
+
+    ``logits`` (rows, V) bf16 / fp16 / fp32, V <= :data:`SAMPLE_MAX_VOCAB`.  Without ``row_map`` every row r is
+    processed; with ``row_map`` (G,) int32 CUDA, row ``r * (rows // G) + row_map[r]`` of every group r of rows is.
+    ``log_softmax=True`` processes the rows' fp32 log-softmax (the beam step's arithmetic) instead of the logits.
+    Processed row r's history (🤗's ``input_ids``) is history row ``h = r // rows_per_hist``: ``prefix[h, :Lp]`` then
+    ``tail[h, :Lt]``, int64 tensors with unit column stride; ``prefix_len`` is a host integer or an int32 CUDA tensor
+    of one or one-per-processed-row elements, ``tail_len`` an int32 CUDA tensor of the same kind, both read when the
+    kernel runs (clamped to the segment's width).  ``min_new_tokens`` counts from ``prompt_len``; it needs ``eos`` ids.
+    Returns ``out`` (allocated as fp32 rows like ``logits`` when None) with the processed rows written and the others
+    untouched.  Recordable in a CUDA graph; arguments the kernel does not take raise ``ValueError`` with its reason
+    before any launch."""
+    p, out = _process_params(logits, prefix, prefix_len, tail=tail, tail_len=tail_len, rows_per_hist=rows_per_hist,
+                             row_map=row_map, out=out, log_softmax=log_softmax, repetition_penalty=repetition_penalty,
+                             no_repeat_ngram_size=no_repeat_ngram_size, min_new_tokens=min_new_tokens,
+                             prompt_len=prompt_len, eos=eos)
+    with torch.cuda.device(out.device):
+        check(_lib.lib().pcv_logits_process(C.byref(p), _stream()), "pcv_logits_process")
+    return out
+
+
+def _process_params(logits, prefix, prefix_len, *, tail=None, tail_len=None, rows_per_hist=1, row_map=None, out=None,
+                    log_softmax=False, repetition_penalty=1.0, no_repeat_ngram_size=0, min_new_tokens=0, prompt_len=0,
+                    eos=()):
+    """The checked ``pcv_logits_process_params`` of :func:`process_logits` and its output rows; no launch."""
+    _require_cuda(logits, prefix)
+    if logits.dim() != 2 or logits.dtype not in (torch.bfloat16, torch.float16, torch.float32):
+        raise ValueError(f"process_logits: logits must be (rows, V) bf16 / fp16 / fp32, got {tuple(logits.shape)} "
+                         f"{logits.dtype}")
+    rows = logits if logits.stride(-1) == 1 else logits.contiguous()
+    n, V = rows.shape
+    R, group = n, 1
+    dev = rows.device
+    if row_map is not None:
+        _require_cuda(row_map)
+        if row_map.device != dev:
+            raise ValueError(f"process_logits: row_map is on {row_map.device}, the logits on {dev}")
+        if row_map.dtype != torch.int32 or row_map.dim() != 1 or not row_map.is_contiguous() or row_map.numel() < 1 \
+                or n % row_map.numel():
+            raise ValueError(f"process_logits: row_map must be a contiguous (G,) int32 tensor with G dividing the {n} "
+                             f"rows, got {tuple(row_map.shape)} {row_map.dtype}")
+        R, group = row_map.numel(), n // row_map.numel()
+    per = _as_int(rows_per_hist)
+    if per is None or per < 1:
+        raise ValueError(f"process_logits: rows_per_hist must be an integer >= 1, got {rows_per_hist!r}")
+    if out is None:
+        out = torch.empty(n, V, dtype=torch.float32, device=rows.device)
+    elif not out.is_cuda or out.device != dev or out.dtype != torch.float32 or tuple(out.shape) != (n, V) or \
+            out.stride(-1) != 1:
+        raise ValueError(f"process_logits: out must be ({n}, {V}) fp32 with unit column stride, got "
+                         f"{tuple(out.shape)} {out.dtype}")
+    p = _lib.LogitsProcessParams()
+    p.logits, p.stride_row = rows.data_ptr(), rows.stride(0) if n > 1 else V
+    p.out, p.out_stride_row = out.data_ptr(), out.stride(0) if n > 1 else V
+    p.row_map, p.row_group, p.R, p.V, p.rows_per_hist = (row_map.data_ptr() if row_map is not None else None), group, \
+        R, V, per
+    p.dtype = _lib.PCV_F32 if rows.dtype == torch.float32 else _pcv_dtype(rows.dtype)
+    p.prefix, p.prefix_stride, p.prefix_cap, p.prefix_len, p.prefix_len_stride, p.prefix_count = _history(
+        "prefix", prefix, prefix_len, R, per, dev)
+    if tail is not None:
+        _require_cuda(tail)
+        if not isinstance(tail_len, torch.Tensor):
+            raise ValueError("process_logits: a tail needs tail_len, an int32 CUDA tensor")
+        p.tail, p.tail_stride, p.tail_cap, p.tail_len, p.tail_len_stride, _ = _history("tail", tail, tail_len, R, per,
+                                                                                       dev)
+    elif tail_len is not None:
+        raise ValueError("process_logits: tail_len without a tail")
+    theta, N, M, n0 = float(repetition_penalty), _as_int(no_repeat_ngram_size), _as_int(min_new_tokens), _as_int(prompt_len)
+    if N is None or M is None or n0 is None or not -2 ** 31 <= min(N, M, n0) <= max(N, M, n0) < 2 ** 31:
+        raise ValueError(f"process_logits: no_repeat_ngram_size, min_new_tokens and prompt_len must be int32 integers, "
+                         f"got {no_repeat_ngram_size!r}, {min_new_tokens!r}, {prompt_len!r}")
+    p.log_softmax, p.repetition_penalty, p.no_repeat_ngram, p.min_new_tokens, p.prompt_len = int(bool(log_softmax)), \
+        theta, N, M, n0
+    eos = list(eos)
+    if len(eos) > PROCESS_MAX_EOS:
+        raise ValueError(f"process_logits: at most {PROCESS_MAX_EOS} EOS ids, got {len(eos)}")
+    p.n_eos = len(eos)
+    for i, e in enumerate(eos):
+        p.eos[i] = max(-2 ** 31, min(int(e), 2 ** 31 - 1))
+    lib = _lib.lib()
+    if not lib.pcv_logits_process_supported(C.byref(p)):
+        raise ValueError(f"process_logits: {lib.pcv_last_error().decode()}")
+    return p, out
