@@ -637,7 +637,10 @@ PCV_API int pcv_rotary_apply_at_fp8(const pcv_rotary_params* p, const pcv_rotary
  * filtering in the semantics of the Hugging Face TemperatureLogitsWarper -> TopKLogitsWarper -> TopPLogitsWarper, then
  * softmax + multinomial.  Row r belongs to batch row b = r / rows_per_batch.
  *   x_i = float(logit_i) / temperature (a true fp32 division); temperature == 0 is greedy: the argmax, the lowest index
- *   on ties, log-probability 0, nothing random drawn.
+ *   on ties, log-probability 0, nothing random drawn.  A row whose largest x is -inf or +inf (every logit -inf, e.g.
+ *   after n-gram blocking has banned the whole vocabulary, or logit / temperature overflowing fp32) has no finite
+ *   softmax and is taken as greedy too: the lowest index of the largest x (index 0 when every x is -inf, as
+ *   torch.argmax), log-probability 0.  The Hugging Face warpers raise an error on such a row.
  *   top_k > 0: keep every token with x_i >= the k-th largest x (all ties with it); 0 or >= V: off.
  *   top_p < 1: with masses w_i = round(2^40 exp(x_i - max x)) (uint64) of the kept tokens, Z their sum and
  *   W<=(v) the mass of the kept tokens with x <= v, token i is removed iff W<=(x_i) <= floor((1 - top_p) Z) (fp64
@@ -682,8 +685,9 @@ PCV_API int pcv_sample_uniforms(uint64_t* out, const uint64_t* seeds, const int3
  * decides one round of G drafts for each of B batch rows.  Row b fed tokens t_0 .. t_G (tokens[b]) to both models; t_1
  * .. t_G are the draft's draws.  Target row i (i = 0 .. G) holds the target's logits after t_i, draft row i (i < G) the
  * logits the draft drew t_{i+1} from.  P_i / Zp_i are the kept masses of target row i and their sum under (temperature,
- * top_k, top_p), exactly as pcv_sample computes them (greedy: 2^40 at the first maximal index, 0 elsewhere); Q_i / Zq_i
- * those of draft row i under the draft_* values.  All arithmetic is exact integer arithmetic:
+ * top_k, top_p), exactly as pcv_sample computes them (greedy, and a row pcv_sample takes as greedy because its largest
+ * scaled value is not finite: 2^40 at the first maximal index, 0 elsewhere); Q_i / Zq_i those of draft row i under the
+ * draft_* values, by the same rule, so that Q is the distribution pcv_sample drew the draft from.  All arithmetic is exact integer arithmetic:
  *   accept t_{i+1} = x iff hi64(u_a * Q_i(x) * Zp_i) < P_i(x) * Zq_i   (min(1, p/q) to 2^-64), with u_a the accept
  *   stream's bits at (seeds[b], b, positions[b, i]).  A draft with Q_i(x) = 0 (one not drawn from Q) is accepted iff
  *   P_i(x) > 0; a token outside [0, V) is rejected.
@@ -894,7 +898,8 @@ PCV_API int pcv_kv_gather_rows(const pcv_kv_gather_params* p, const pcv_dev_rows
  *   pcv_contrastive_candidates, one 512-thread CTA per item: x = the fp32 logits of row b*K + sel[b] (sel = 0 after the
  *     prompt, whose K rows are equal); the K largest x, value descending then index ascending on ties (-0 == +0), are
  *     the candidates cand[b, j]; p_j = exp(x_j - m) / Σ_i exp(x_i - m) in fp64 (m = max x); next_tokens[b*K + j] =
- *     cand[b, j].
+ *     cand[b, j].  A row with -inf entries ranks them last, in index order; a row whose every entry is -inf has no
+ *     finite softmax (NaN probabilities, as in 4.28) and is unsupported.
  *   pcv_contrastive_rank, after the model ran row b*K + j on candidate j and produced its final hidden row h_j:
  *     1. cos(c_s, h_j) = (Σ_d c_sd h_jd) / (sqrt(‖c_s‖²) sqrt(‖h_j‖²)) in fp64 (16-bit products are exact; one fixed
  *        summation order), 0 when either norm is 0; c_s are the item's context rows;

@@ -8,7 +8,8 @@ TEST INFRASTRUCTURE ONLY — nothing under perceiver_io_b200/ imports this file.
                           word = ((b * 0x9E3779B1 + pos) * 0x85EBCA6B) mod 2^32
                           x = round(word ^ seed_lo, ca, k0); x = round(x ^ seed_hi, cb, k1); x = round(x, ca, k2)
                           bits = half_1 << 32 | half_0
-    x_i                 float32(logit_i) / float32(temperature), IEEE fp32 division (temperature 0: greedy argmax)
+    x_i                 float32(logit_i) / float32(temperature), IEEE fp32 division (temperature 0: greedy argmax;
+                        a row whose max x is +-inf has no finite mass and is greedy too: the first index of the max)
     top-k               keep x_i >= the k-th largest x (ties with it stay); 0 or >= V: off
     w_i                 round_half_even(2^40 exp(float64(x_i) - float64(max x))), 0 where x_i - max x < -29
     top-p               cut = floor((1 - float64(float32(top_p))) * float64(Z)); drop i iff W<=(x_i) <= cut, the top
@@ -66,7 +67,19 @@ def uniform_bits(seed, b, pos) -> np.ndarray:
 def scaled(logits, temperature: float) -> np.ndarray:
     """x = float32(logit) / float32(temperature) in IEEE fp32."""
     x = np.asarray(logits, dtype=np.float32)
-    return x / np.float32(temperature)
+    with np.errstate(over="ignore"):
+        return x / np.float32(temperature)
+
+
+def greedy_token(logits, temperature: float):
+    """The token of a row drawn greedily, or None: temperature 0, or a max scaled value of +-inf (no finite mass).
+    The first index of the max x (of the max logit when greedy), as torch.argmax."""
+    x = np.asarray(logits, dtype=np.float32)
+    if temperature != 0:
+        x = scaled(x, temperature)
+        if np.isfinite(x.max()):
+            return None
+    return int(np.argmax(x))
 
 
 class Filtered(NamedTuple):
@@ -81,7 +94,14 @@ class Filtered(NamedTuple):
 
 
 def filter_row(logits, temperature: float, top_k: int, top_p: float) -> Filtered:
-    """The kept set and masses of one row (temperature > 0)."""
+    """The kept set and masses of one row; a greedy row (``greedy_token``) keeps its one token at mass 2^40."""
+    tok = greedy_token(logits, temperature)
+    if tok is not None:
+        x = np.asarray(logits, dtype=np.float32) if temperature == 0 else scaled(logits, temperature)
+        kept = np.zeros(x.shape[0], dtype=bool)
+        kept[tok] = True
+        w = np.where(kept, np.uint64(2 ** 40), np.uint64(0))
+        return Filtered(x, kept, w, 2 ** 40, -1, x[tok:tok + 1], np.array([2 ** 40], np.uint64), 0)
     x = scaled(logits, temperature)
     V = x.shape[0]
     m = x.max()
@@ -111,10 +131,6 @@ def filter_row(logits, temperature: float, top_k: int, top_p: float) -> Filtered
 
 def probs(logits, temperature: float, top_k: int, top_p: float) -> np.ndarray:
     """fp64 probabilities of the filtered distribution (w / Z_kept; one-hot of the argmax when greedy)."""
-    if temperature == 0:
-        out = np.zeros(len(logits))
-        out[int(np.argmax(np.asarray(logits, dtype=np.float32)))] = 1.0
-        return out
     f = filter_row(logits, temperature, top_k, top_p)
     return np.where(f.kept, f.w.astype(np.float64), 0.0) / float(f.z_kept)
 
@@ -130,10 +146,10 @@ def sample_row(logits, temperature: float, top_k: int, top_p: float, seed: int, 
                logit_err: float = 0.0) -> Draw:
     """The device's draw for one row, and whether it is ambiguous (see the module docstring)."""
     logits = np.asarray(logits, dtype=np.float32)
-    if temperature == 0:
-        tok = int(np.argmax(logits))
+    tok = greedy_token(logits, temperature)
+    if tok is not None:
         amb = False
-        if logit_err > 0 and len(logits) > 1:
+        if temperature == 0 and logit_err > 0 and len(logits) > 1:
             rest = np.delete(logits, tok).astype(np.float64)
             amb = bool(rest.max() >= float(logits[tok]) - 2 * logit_err)
         return Draw(tok, 0.0, amb, "greedy runner-up" if amb else "")

@@ -3,8 +3,9 @@
 
 TEST INFRASTRUCTURE ONLY — nothing under perceiver_io_b200/ imports this file.
 
-    masses          P_i / Zp_i: sample_oracle.filter_row's kept masses of target row i under the target's values (greedy:
-                    2^40 at the first maximal index); Q_i / Zq_i: the same for draft row i under the draft's values
+    masses          P_i / Zp_i: sample_oracle.filter_row's kept masses of target row i under the target's values (greedy,
+                    temperature 0 or a max scaled value of +-inf: 2^40 at the first maximal index); Q_i / Zq_i: the same
+                    for draft row i under the draft's values
     accept          t_{i+1} = x is accepted iff (u_a * Q_i(x) * Zp_i) >> 64 < P_i(x) * Zq_i
     n               the first rejected i, or G
     correction      R(y) = max(0, P(y) Zq - Q(y) Zp) on row n; the first index whose prefix sum of R exceeds
@@ -71,9 +72,10 @@ class Masses(NamedTuple):
 
 def masses(logits, temperature: float, top_k: int, top_p: float) -> Masses:
     logits = np.asarray(logits, dtype=np.float32)
-    if temperature == 0:
+    tok = S.greedy_token(logits, temperature)
+    if tok is not None:
         w = [0] * len(logits)
-        w[int(np.argmax(logits))] = ONE
+        w[tok] = ONE
         return Masses(w, ONE, 0, False)
     f = S.filter_row(logits, temperature, top_k, top_p)
     w = [int(v) for v in np.where(f.kept, f.w, np.uint64(0))]

@@ -4,7 +4,8 @@
 //
 // One CTA of 512 threads per row ρ (batch row b = ρ / rows_per_batch); the row's fp32 x is staged in shared memory.
 //   1. x_i = float(logit_i) / temperature, a true fp32 division.  temperature == 0: the argmax of the logits, the lowest
-//      index on ties (torch.argmax); nothing random is drawn and the log-probability written is 0.
+//      index on ties (torch.argmax); nothing random is drawn and the log-probability written is 0.  A row whose largest
+//      x is +-inf has no finite mass and is greedy too: the lowest index of the largest x.
 //   2. top-k: keep every token with x_i >= the k-th largest x (tokens tied with it stay).  A radix select over
 //      order-preserving uint32 keys (-0 folded onto +0), four passes of 256-bin count histograms.
 //   3. masses: w_i = round(2^40 · exp(x_i - max x)) in uint64 fixed point (exp in fp64, round half to even), Z = Σ w_i
@@ -205,15 +206,15 @@ __global__ void __launch_bounds__(kThreads, 1) sample_kernel(const pcv_sample_pa
   const int64_t row = blockIdx.x;
   const T* src = static_cast<const T*>(p.logits) + row * p.stride_row;
   const u64 best = stage_row(src, V, p.temperature, xs, red);
-  if (p.temperature == 0.f) {
+  const uint32_t top = (uint32_t)(best >> 32);
+  const float m = key_value(top);
+  if (p.temperature == 0.f || !isfinite(m)) {   // a non-finite max leaves no finite mass: the row is greedy
     if (tid == 0) {
       p.tokens[row] = (int64_t)(uint32_t)~(uint32_t)best;
       if (p.logprobs) p.logprobs[row] = 0.f;
     }
     return;
   }
-  const uint32_t top = (uint32_t)(best >> 32);
-  const float m = key_value(top);
   const uint32_t lo = kept_threshold(V, p, top, xs);
 
   // ---- draw: warp w owns a contiguous segment of the vocabulary ----
@@ -309,8 +310,8 @@ struct RowFilter {
 template <typename T>
 __device__ __forceinline__ RowFilter filter_row(const T* src, int V, const FilterValues& v, float* xs, u64* red) {
   const u64 best = stage_row(src, V, v.temperature, xs, red);
-  if (v.temperature == 0.f) return RowFilter{true, (int)(uint32_t)~(uint32_t)best, 0.f, 0u};
   const uint32_t top = (uint32_t)(best >> 32);
+  if (v.temperature == 0.f || !isfinite(key_value(top))) return RowFilter{true, (int)(uint32_t)~(uint32_t)best, 0.f, 0u};
   return RowFilter{false, 0, key_value(top), kept_threshold(V, v, top, xs)};
 }
 
