@@ -280,6 +280,22 @@ struct FwdCfg {
   static_assert(kSlots >= 2, "shared memory budget");
 };
 
+// Position of a key tile in the pipelined schedule's ring: the slot of its first K box and the parity of that slot's
+// current fill.  Tiles start at multiples of STEP (the K and V boxes of a tile), which divides NS, so the tile's V
+// group (slot + NQB) has the same parity and one compare wraps the position: no division by the ring size, which is
+// not a power of two.
+template <int STEP, int NS>
+struct RingPos {
+  uint32_t slot = 0, phase = 0;
+  __device__ __forceinline__ void advance() {
+    slot += STEP;
+    if (slot == NS) {
+      slot = 0;
+      phase ^= 1;
+    }
+  }
+};
+
 struct FwdBarriers {
   uint64_t full[16], empty[16];
   uint64_t q_full, q_empty;
@@ -483,7 +499,8 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
   if (wg == 0) {
     reg_dealloc<kProducerRegs>();
     if (threadIdx.x == 0) {
-      uint32_t it = 0;
+      uint32_t it = 0;  // serial schedule: ring index of the next box
+      RingPos<NQB + KVB, NS> pos;  // pipelined schedule: the next tile's box groups
       for (int si = seg_lo; si < seg_hi; ++si) {
         const Segment sg = p.segs[si];
         mbar_wait(&bar.q_empty, ((si - seg_lo) & 1) ^ 1, 1);
@@ -504,28 +521,28 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
             else
               tma_load_4d(dst, tm, fb, ch, t * kTileN, sg.h, sg.b);
           };
-          // the next nb boxes, from ring index it on: wait until their slots are free, expect their bytes
-          auto begin_group = [&](int nb) {
-            const uint32_t g = it % NS;
-            mbar_wait(&bar.empty[g], ((it / NS) & 1) ^ 1, 2);
+          // nb boxes from ring slot g on, whose fill has parity ph: wait until the slots are free, expect their bytes
+          auto begin_group = [&](uint32_t g, uint32_t ph, int nb) {
+            mbar_wait(&bar.empty[g], ph ^ 1, 2);
             mbar_arrive_expect_tx(&bar.full[g], nb * kBoxBytes);
-            it += nb;
-            return g;
           };
           // The pipelined schedule guards the K boxes of a tile with one full / empty pair and its V boxes with
           // another, those of the group's first slot (a tile's boxes never wrap around the ring); the serial schedule
           // every box with its own.
           if constexpr (kPipelined) {
-            const uint32_t gk = begin_group(NQB);
+            const uint32_t gk = pos.slot, gv = pos.slot + NQB;
+            begin_group(gk, pos.phase, NQB);
 #pragma unroll
             for (int c = 0; c < NQB; ++c) load_box(c, gk + c, &bar.full[gk]);
-            const uint32_t gv = begin_group(KVB);
+            begin_group(gv, pos.phase, KVB);
 #pragma unroll
             for (int c = 0; c < KVB; ++c) load_box(NQB + c, gv + c, &bar.full[gv]);
+            pos.advance();
           } else {
 #pragma unroll 1
-            for (int c = 0; c < NQB + KVB; ++c) {
-              const uint32_t s = begin_group(1);
+            for (int c = 0; c < NQB + KVB; ++c, ++it) {
+              const uint32_t s = it % NS;
+              begin_group(s, (it / NS) & 1, 1);
               load_box(c, s, &bar.full[s]);
             }
           }
@@ -540,60 +557,76 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
   }
 
   reg_alloc<kConsumerRegs>();
-  const int cw = wg - 1;                 // consumer warpgroup: query rows [64*cw, 64*cw + 64) of the tile
+  const int cw = (int)warp_uniform(wg) - 1;  // consumer warpgroup: query rows [64*cw, 64*cw + 64) of the tile
   const int tid = threadIdx.x - 128 * wg;
   const int warp = tid >> 5, lane = tid & 31;
   const int rloc = 64 * cw + 16 * warp + (lane >> 2);  // rows rloc and rloc + 8
   const int cq = 2 * (lane & 3);                      // first of the two columns of every 8-column group
-  const uint32_t q_base = smem_u32(sQ) + cw * 64 * 128;
-  const uint32_t ring_base = smem_u32(sRing);
-  uint32_t it = 0;  // ring index of the next box (the producer's order: the NQB K boxes, then the NVB V boxes of a tile)
-
-  auto wait_full = [&](uint32_t i, uint32_t site) { mbar_wait(&bar.full[i % NS], (i / NS) & 1, site); };
-  // releases the box group (see the producer) whose first box is ring index i
-  auto release = [&](uint32_t i) {
-    if (PAIR) wg_arrive_pair(&bar.empty[i % NS]);
-    else wg_arrive(&bar.empty[i % NS]);
+  // wgmma descriptors: a warp-uniform low word set up outside the GEMM turn plus a compile-time byte offset (desc_at),
+  // so that each wgmma costs one uniform add.  Q stays at one place for the whole kernel; ring slot g has the low word
+  // ring_lo + g * kSlotLo.  On the pipelined schedule the 16-bit P V at NVB == 2 reads both V boxes of a tile
+  // (adjacent slots) in one m64n128 wgmma: LBO = one box.
+  constexpr uint32_t kSlotLo = kBoxBytes >> 4;
+  constexpr uint32_t kPvLbo = (kPipelined && !FP8 && NVB == 2) ? kBoxBytes : 16;
+  const uint32_t q_lo = warp_uniform(desc_lo(smem_u32(sQ) + cw * 64 * 128));
+  const uint32_t ring_lo = warp_uniform(desc_lo(smem_u32(sRing)));
+  const uint32_t ring_lo_v = warp_uniform(desc_lo(smem_u32(sRing), kPvLbo));
+  // low word of the K group at ring slot g.  Marked uniform it is built in the uniform datapath; at NVB == 1 the mark
+  // makes ptxas spill the segment bounds (8 bytes), so those kernels leave it unmarked.
+  auto k_lo = [&](uint32_t g) {
+    const uint32_t lo = ring_lo + g * kSlotLo;
+    return NVB == 2 ? warp_uniform(lo) : lo;
   };
-  // S = Q K^T of the tile whose first K box is ring index i: one commit group
-  auto issue_qk = [&](float (&s)[64], uint32_t i) {
-    wait_full(i, 6);
+  RingPos<NQB + KVB, NS> pos;  // pipelined schedule: the next tile's box groups (the producer's order)
+  uint32_t it = 0;  // serial schedule: ring index of the next box (the NQB K boxes, then the NVB V boxes of a tile)
+
+  // releases the box group (see the producer) whose first box is ring slot g
+  auto release = [&](uint32_t g) {
+    if (PAIR) wg_arrive_pair(&bar.empty[g]);
+    else wg_arrive(&bar.empty[g]);
+  };
+  // S (+)= Q box c K^T with the K box at low word kb: four k16 steps of 16-bit channels or k32 steps of e4m3 ones,
+  // 32 bytes each.  FP8 issues all four k32 steps of a box even past dqk (TMA zero fill): a runtime guard around the
+  // wgmma makes ptxas serialise every wgmma of the kernel (C7515)
+  auto qk_box = [&](float (&s)[64], int c, uint32_t kb) {
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      if constexpr (FP8)
+        wgmma_ss_e4m3_n128(s, desc_at(q_lo, c * kBoxBytes + kk * 32), desc_at(kb, kk * 32), (c | kk) != 0);
+      else
+        wgmma_ss<128, BF16>(s, desc_at(q_lo, c * kBoxBytes + kk * 32), desc_at(kb, kk * 32), (c | kk) != 0);
+    }
+  };
+  // O += P V box at low word vb (16-bit, 64 channels): eight k16 steps of 16 key rows, 2048 bytes each
+  auto pv_box = [&](float (&ov)[32], const uint32_t (&pa)[8][4], uint32_t vb) {
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk) wgmma_rs<64, BF16>(ov, pa[kk], desc_at(vb, kk * 2048));
+  };
+  // S = Q K^T of the tile whose K group starts at ring slot g (low word kb), filled with parity ph: one commit group
+  auto issue_qk = [&](float (&s)[64], uint32_t g, uint32_t ph, uint32_t kb) {
+    mbar_wait(&bar.full[g], ph, 6);
     wgmma_fence();
 #pragma unroll
-    for (int c = 0; c < NQB; ++c)
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {  // k16 steps of 16-bit channels, k32 steps of e4m3 ones: 32 bytes each
-        // FP8 issues all four k32 steps of a box even past dqk (TMA zero fill): a runtime guard around the wgmma makes
-        // ptxas serialise every wgmma of the kernel (C7515)
-        if constexpr (FP8)
-          wgmma_ss_e4m3_n128(s, make_desc(q_base + c * kBoxBytes + kk * 32),
-                             make_desc(ring_base + (i + c) % NS * kBoxBytes + kk * 32), (c | kk) != 0);
-        else
-          wgmma_ss<128, BF16>(s, make_desc(q_base + c * kBoxBytes + kk * 32),
-                              make_desc(ring_base + (i + c) % NS * kBoxBytes + kk * 32), (c | kk) != 0);
-      }
+    for (int c = 0; c < NQB; ++c) qk_box(s, c, kb + c * kSlotLo);
     wgmma_commit();
   };
   // P as the A operand of P V: 16-bit fragments of 8 k16 steps, or e4m3 fragments of 4 k32 steps
   using PFrag = uint32_t[FP8 ? 4 : 8][4];
-  // O += P V of the tile whose first V box is ring index i: one commit group
-  auto issue_pv = [&](float (&o)[NVB][32], const PFrag& pa, uint32_t i) {
-    wait_full(i, 7);
+  // O += P V of the tile whose V group starts at ring slot g (low word vb), filled with parity ph: one commit group
+  auto issue_pv = [&](float (&o)[NVB][32], const PFrag& pa, uint32_t g, uint32_t ph, uint32_t vb) {
+    mbar_wait(&bar.full[g], ph, 7);
     wgmma_fence();
-    if constexpr (FP8) {
+    if constexpr (FP8) {  // the V^T box of a tile: 64-channel halves 8192 bytes apart, k32 steps of 32 bytes
 #pragma unroll
       for (int v = 0; v < NVB; ++v)
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk)
-          wgmma_rs_e4m3_n64(o[v], pa[kk], make_desc(ring_base + i % NS * kBoxBytes + v * 8192 + kk * 32));
+        for (int kk = 0; kk < 4; ++kk) wgmma_rs_e4m3_n64(o[v], pa[kk], desc_at(vb, v * 8192 + kk * 32));
     } else if constexpr (NVB == 2) {  // both V boxes in one m64n128 per k16 step (adjacent slots, see FwdCfg)
 #pragma unroll
       for (int kk = 0; kk < 8; ++kk)
-        wgmma_rs<128, BF16>(reinterpret_cast<float(&)[64]>(o), pa[kk],
-                            make_desc(ring_base + i % NS * kBoxBytes + kk * 2048, kBoxBytes));
+        wgmma_rs<128, BF16>(reinterpret_cast<float(&)[64]>(o), pa[kk], desc_at(vb, kk * 2048));
     } else {
-#pragma unroll
-      for (int kk = 0; kk < 8; ++kk) wgmma_rs<64, BF16>(o[0], pa[kk], make_desc(ring_base + i % NS * kBoxBytes + kk * 2048));
+      pv_box(o[0], pa, vb);
     }
     wgmma_commit();
   };
@@ -601,11 +634,11 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
     if constexpr (FP8) pack_p_e4m3(s, pa, lane);
     else pack_p<BF16>(s, pa);
   };
-  // after the P V whose first V box is ring index i completed: O is final in registers, release the V boxes
-  auto pv_done = [&](float (&o)[NVB][32], uint32_t i) {
+  // after the P V whose V group starts at ring slot g completed: O is final in registers, release the V boxes
+  auto pv_done = [&](float (&o)[NVB][32], uint32_t g) {
 #pragma unroll
     for (int v = 0; v < NVB; ++v) fence_regs(o[v]);
-    release(i);
+    release(g);
   };
   // Ping-pong turns.  Warpgroup cw waits on its own named barrier (id 1 + cw) before it issues its GEMMs and hands
   // the turn over by arriving on the other's (id 2 - cw) after it committed them; a phase counts 256 threads (128
@@ -656,42 +689,46 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
     if constexpr (kPipelined) {
       float s[64], alpha[2];
       PFrag pa;
-      uint32_t ik = it;  // ring index of the first K box of the current tile
       if (sg.t1 > sg.t0) {
         // prologue: S of the first tile, its softmax (O is still zero: nothing to rescale)
+        uint32_t kb = k_lo(pos.slot);
         turn_begin();
-        issue_qk(s, ik);
+        issue_qk(s, pos.slot, pos.phase, kb);
         turn_end(false);
         wgmma_wait<0>();
         fence_regs(s);
-        release(ik);
+        release(pos.slot);
         tile_softmax<DROP, FP8>(s, m_run, l_run, alpha, p, sg.b, sg.t0 * kTileN, n0, cq, interior(sg.t0 * kTileN), qside,
                                 sl2);
         pack(s, pa);
         for (int t = sg.t0 + 1; t < sg.t1; ++t) {
-          const uint32_t iv = ik + NQB;  // V boxes of tile t - 1
-          ik += NQB + KVB;
+          const uint32_t gv = pos.slot + NQB, vph = pos.phase;  // V boxes of tile t - 1
+          const uint32_t vb = ring_lo_v + gv * kSlotLo;
+          pos.advance();
+          kb = k_lo(pos.slot);
           turn_begin();
-          issue_qk(s, ik);
-          issue_pv(o, pa, iv);
+          issue_qk(s, pos.slot, pos.phase, kb);
+          issue_pv(o, pa, gv, vph, vb);
           turn_end(false);
           wgmma_wait<1>();  // S of tile t is ready; P V of tile t - 1 still runs under the softmax below
           fence_regs(s);
-          release(ik);
+          release(pos.slot);
           tile_softmax<DROP, FP8>(s, m_run, l_run, alpha, p, sg.b, t * kTileN, n0, cq, interior(t * kTileN), qside, sl2);
           wgmma_wait<0>();
-          pv_done(o, iv);
+          pv_done(o, gv);
           rescale_o(o, alpha);
           pack(s, pa);
         }
         // epilogue: P V of the last tile
+        const uint32_t gv = pos.slot + NQB;
+        const uint32_t vb = ring_lo_v + gv * kSlotLo;
         turn_begin();
-        issue_pv(o, pa, ik + NQB);
+        issue_pv(o, pa, gv, pos.phase, vb);
         turn_end(si + 1 == seg_hi);  // the last turn of this CTA
         wgmma_wait<0>();
-        pv_done(o, ik + NQB);
+        pv_done(o, gv);
+        pos.advance();
       }
-      it += (uint32_t)(sg.t1 - sg.t0) * (NQB + KVB);
     } else {
       for (int t = sg.t0; t < sg.t1; ++t) {
         float s[64];
@@ -700,14 +737,11 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
           const uint32_t sl = it % NS;
           mbar_wait(&bar.full[sl], (it / NS) & 1, 4);
           wgmma_fence();
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk)
-            wgmma_ss<128, BF16>(s, make_desc(q_base + c * kBoxBytes + kk * 32),
-                                make_desc(ring_base + sl * kBoxBytes + kk * 32), (c | kk) != 0);
+          qk_box(s, c, ring_lo + sl * kSlotLo);
           wgmma_commit();
           wgmma_wait<0>();
           fence_regs(s);
-          release(it);
+          release(sl);
         }
         float alpha[2];
         tile_softmax<DROP>(s, m_run, l_run, alpha, p, sg.b, t * kTileN, n0, cq, interior(t * kTileN), qside);
@@ -719,13 +753,11 @@ __device__ __forceinline__ void attn_fwd_body(const CUtensorMap& tq, const CUten
           const uint32_t sl = it % NS;
           mbar_wait(&bar.full[sl], (it / NS) & 1, 5);
           wgmma_fence();
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk)
-            wgmma_rs<64, BF16>(o[v], pa[kk], make_desc(ring_base + sl * kBoxBytes + kk * 2048));
+          pv_box(o[v], pa, ring_lo + sl * kSlotLo);
           wgmma_commit();
           wgmma_wait<0>();
           fence_regs(o[v]);
-          release(it);
+          release(sl);
         }
       }
     }

@@ -235,6 +235,27 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr, uint32_t lbo_b
   return d;
 }
 
+// The same descriptor split for address arithmetic in loops: a 32-bit low word (start address >> 4 and LBO) and the
+// constant high word (SBO = 1024, SWIZZLE_128B).  desc_at(desc_lo(a, lbo), off) == make_desc(a + off, lbo) whenever
+// a + off < 2^18 bytes: the start field holds bits [4, 18) of the address, and every shared-memory address (228 KB at
+// most on sm_90) is below 2^18, so adding off >> 4 never carries out of the 14-bit field into the LBO.  Offsets are
+// multiples of 16 bytes (k-step steps of 32 bytes inside a 128-byte row, whole 1024-byte atoms, whole boxes), so
+// nothing is lost by the shift.  With a loop-invariant low word and compile-time offsets every descriptor of a wgmma
+// loop is one add of an immediate, which ptxas keeps in uniform registers when the low word is warp-uniform.
+constexpr uint32_t kDescHi128 = (1024u >> 4) | (1u << 30);
+__device__ __forceinline__ uint32_t desc_lo(uint32_t smem_addr, uint32_t lbo_bytes = 16) {
+  return ((smem_addr & 0x3FFFF) >> 4) | (((lbo_bytes >> 4) & 0x3FFF) << 16);
+}
+__device__ __forceinline__ uint64_t desc_at(uint32_t lo, uint32_t byte_off) {
+  return ((uint64_t)kDescHi128 << 32) | (lo + (byte_off >> 4));
+}
+// x, which every lane of the (converged) warp already holds, marked warp-uniform for ptxas by a shuffle from lane 0.
+// ptxas cannot tell that a value derived from threadIdx / 128 or carried through a loop whose trip count was loaded
+// from memory is the same in every lane; without the mark it builds descriptors in vector registers and moves each one
+// into the uniform registers the wgmma reads (R2UR), inside the GEMM issue.  With it the descriptor arithmetic runs in
+// the uniform datapath, and ptxas drops the shuffle itself where it can see it is redundant.
+__device__ __forceinline__ uint32_t warp_uniform(uint32_t x) { return __shfl_sync(0xffffffffu, x, 0); }
+
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
