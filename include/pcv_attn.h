@@ -196,6 +196,7 @@ typedef struct pcv_merge_params {
  * In-place change of reference maximum of a partial state (used between the two all-reduces of the
  * M-sharded path, perceiver_io_b200/dist.py):  w = 2^(part_m[r] - new_m[r]);  part_o[r,:] *= w;
  * part_l[r] *= w;  part_m[r] = new_m[r].   rows = B*H*N.  new_m[r] >= part_m[r] is expected.
+ * part_o rows are read and written as float4 when dv % 4 == 0 and part_o is 16-byte aligned, element-wise otherwise.
  */
 typedef struct pcv_rescale_params {
   float* part_o;        /* (rows, dv) */
@@ -215,6 +216,9 @@ typedef struct pcv_rescale_params {
  * (so all ranks end up with the full (B, N, H, dv) result after a barrier).  The caller provides the barriers
  * (before: all partial states written; after: all outputs written) — perceiver_io_b200/dist.py uses the
  * symmetric-memory signal pads for that.
+ * Fast path (every lane issues all its loads of a row before it consumes one): taken when dv % 4 == 0, dv <= 128,
+ * the three output strides are multiples of 4 elements, every part_o[g] is 16-byte aligned and every out[g] 8-byte
+ * aligned.  Any other call runs the general path (element-wise loads and stores), with the same result.
  */
 #define PCV_MAX_PEERS 8
 typedef struct pcv_peer_combine_params {

@@ -48,8 +48,11 @@ attn_simt_kernel(const pcv_attn_params p, int nsplit, int keys_per_split, float*
   uint32_t* Vs = Ks + kKeysPerTile * qs;
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int b = blockIdx.y / p.H, h = blockIdx.y % p.H;
-  const int n0 = blockIdx.x * kRowsPerCta;
+  // blockIdx.x = bh * tiles + query tile: B*H is not bounded by gridDim.y's 65535
+  const int tiles = (p.N + kRowsPerCta - 1) / kRowsPerCta;
+  const int bh = (int)(blockIdx.x / (unsigned)tiles);
+  const int b = bh / p.H, h = bh % p.H;
+  const int n0 = (int)(blockIdx.x - (unsigned)bh * tiles) * kRowsPerCta;
   const int split = blockIdx.z;
   const int kb = split * keys_per_split;
   const int ke = min(p.M, kb + keys_per_split);
@@ -222,7 +225,7 @@ int launch_t(const pcv_attn_params& p, const SimtPlan& pl, cudaStream_t stream) 
       wl = wm + (size_t)pl.nsplit * R;
     }
   }
-  dim3 grid((p.N + kRowsPerCta - 1) / kRowsPerCta, p.B * p.H, pl.nsplit);
+  dim3 grid((unsigned)((int64_t)(p.N + kRowsPerCta - 1) / kRowsPerCta * p.B * p.H), 1, pl.nsplit);
   prof_mark_begin(stream);
   kern<<<grid, kWarps * 32, pl.smem_bytes, stream>>>(p, pl.nsplit, pl.keys_per_split, wo, wm, wl);
   prof_mark_end(stream);
@@ -255,6 +258,8 @@ int launch_attn_simt(const pcv_attn_params& p, cudaStream_t stream) {
   const SimtPlan pl = make_plan(p);
   PCV_REQUIRE(p.dqk <= 1024, PCV_ERR_UNSUPPORTED, "simt attention: dqk=%d exceeds 1024", p.dqk);
   PCV_REQUIRE(pl.smem_bytes <= 200 * 1024, PCV_ERR_UNSUPPORTED, "simt attention: tile does not fit shared memory");
+  PCV_REQUIRE((int64_t)(p.N + kRowsPerCta - 1) / kRowsPerCta * p.B * p.H <= INT32_MAX, PCV_ERR_UNSUPPORTED,
+              "simt attention: B*H*ceil(N/32) exceeds the grid");
   size_t need = 0;
   attn_simt_workspace_bytes(p, &need);
   PCV_REQUIRE(need == 0 || (p.workspace != nullptr && p.workspace_bytes >= need), PCV_ERR_WORKSPACE,

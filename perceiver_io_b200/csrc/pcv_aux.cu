@@ -74,10 +74,11 @@ int combine_t(const float* po, const float* pm, const float* pl, int nparts, int
 
 // ---------------------------------------------------------------------------------------------
 // combine over peers: one warp per owned row; every lane keeps num_peers 16-byte loads in flight (the
-// remote ones cross NVLink), then pushes the normalised row to every rank's output buffer.
+// remote ones cross NVLink), then pushes the normalised row to every rank's output buffer.  `fast` is
+// peers_fast_path(p), the same for the whole grid.
 // ---------------------------------------------------------------------------------------------
 template <typename T>
-__global__ void __launch_bounds__(256) combine_peers_kernel(const pcv_peer_combine_params p) {
+__global__ void __launch_bounds__(256) combine_peers_kernel(const pcv_peer_combine_params p, const bool fast) {
   const int64_t r = p.row_begin + (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (r >= p.row_end) return;
@@ -87,7 +88,7 @@ __global__ void __launch_bounds__(256) combine_peers_kernel(const pcv_peer_combi
   const int b = (int)(r / ((int64_t)p.N * p.H));
   const int64_t o_off = (int64_t)b * p.o_stride_b + (int64_t)n * p.o_stride_n + (int64_t)h * p.o_stride_h;
 
-  if ((p.dv & 3) == 0 && p.dv <= 128) {
+  if (fast) {
     // fast path (dv <= 128): every remote load of the row — row max, denominator and this lane's 16 bytes of the
     // numerator from every peer — is issued BEFORE anything is consumed, so the warp pays one NVLink round trip
     float mg[PCV_MAX_PEERS], lg[PCV_MAX_PEERS];
@@ -156,16 +157,17 @@ __global__ void __launch_bounds__(256) combine_peers_kernel(const pcv_peer_combi
 }
 
 // ---------------------------------------------------------------------------------------------
-// rescale: one warp per row, float4 where the row length allows.
+// rescale: one warp per row, float4 where the row length and part_o's alignment allow (`vec`, the same for the
+// whole grid: with dv % 4 == 0 every row of a 16-byte aligned part_o is 16-byte aligned).
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) rescale_kernel(const pcv_rescale_params p) {
+__global__ void __launch_bounds__(256) rescale_kernel(const pcv_rescale_params p, const bool vec) {
   const int64_t r = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (r >= p.rows) return;
   const float mo = p.part_m[r], mn = p.new_m[r];
   const float w = (mo == -INFINITY) ? 0.f : exp2f(mo - mn);
   float* row = p.part_o + r * p.dv;
-  if ((p.dv & 3) == 0) {
+  if (vec) {
     float4* row4 = reinterpret_cast<float4*>(row);
     for (int c = lane; c < (p.dv >> 2); c += 32) {
       float4 x = row4[c];
@@ -459,6 +461,15 @@ int launch_merge_partials(const pcv_merge_params& p, cudaStream_t stream) {
                                   p.out_o, p.out_m, p.out_l, stream);
 }
 
+// the rule stated beside pcv_peer_combine_params: 16-byte loads of every part_o row and 8-byte stores of every
+// output row (c = 4 * lane, so every element offset a lane touches is a multiple of 4)
+static bool peers_fast_path(const pcv_peer_combine_params& p) {
+  if ((p.dv & 3) != 0 || p.dv > 128 || ((p.o_stride_b | p.o_stride_n | p.o_stride_h) & 3) != 0) return false;
+  for (int g = 0; g < p.num_peers; ++g)
+    if (!al16(p.part_o[g]) || (reinterpret_cast<uintptr_t>(p.out[g]) & 7u) != 0) return false;
+  return true;
+}
+
 int launch_combine_peers(const pcv_peer_combine_params& p, cudaStream_t stream) {
   PCV_REQUIRE(p.num_peers >= 1 && p.num_peers <= PCV_MAX_PEERS, PCV_ERR_INVALID, "combine_peers: num_peers=%d", p.num_peers);
   PCV_REQUIRE(p.rank >= 0 && p.rank < p.num_peers, PCV_ERR_INVALID, "combine_peers: bad rank %d", p.rank);
@@ -468,16 +479,15 @@ int launch_combine_peers(const pcv_peer_combine_params& p, cudaStream_t stream) 
   PCV_REQUIRE(p.row_begin >= 0 && p.row_begin <= p.row_end && p.row_end <= R, PCV_ERR_INVALID, "combine_peers: bad row range");
   for (int g = 0; g < p.num_peers; ++g)
     PCV_REQUIRE(p.part_o[g] && p.part_m[g] && p.part_l[g] && p.out[g], PCV_ERR_INVALID, "combine_peers: null pointer for peer %d", g);
-  if ((p.dv & 3) == 0)
-    PCV_REQUIRE(((p.o_stride_b | p.o_stride_n | p.o_stride_h) & 3) == 0, PCV_ERR_INVALID, "combine_peers: output strides must be multiples of 4");
   const int64_t rows = p.row_end - p.row_begin;
   if (rows == 0) return PCV_OK;
   const int warps = 8;
   const unsigned blocks = (unsigned)((rows + warps - 1) / warps);
+  const bool fast = peers_fast_path(p);
   if (p.dtype == PCV_BF16)
-    combine_peers_kernel<__nv_bfloat16><<<blocks, warps * 32, 0, stream>>>(p);
+    combine_peers_kernel<__nv_bfloat16><<<blocks, warps * 32, 0, stream>>>(p, fast);
   else
-    combine_peers_kernel<__half><<<blocks, warps * 32, 0, stream>>>(p);
+    combine_peers_kernel<__half><<<blocks, warps * 32, 0, stream>>>(p, fast);
   PCV_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PCV_OK;
@@ -487,7 +497,8 @@ int launch_rescale(const pcv_rescale_params& p, cudaStream_t stream) {
   PCV_REQUIRE(p.part_o && p.part_m && p.part_l && p.new_m, PCV_ERR_INVALID, "rescale: null pointer argument");
   PCV_REQUIRE(p.rows >= 1 && p.dv >= 1, PCV_ERR_INVALID, "rescale: bad dimension");
   const int warps = 8;
-  rescale_kernel<<<(unsigned)((p.rows + warps - 1) / warps), warps * 32, 0, stream>>>(p);
+  const bool vec = (p.dv & 3) == 0 && al16(p.part_o);
+  rescale_kernel<<<(unsigned)((p.rows + warps - 1) / warps), warps * 32, 0, stream>>>(p, vec);
   PCV_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return PCV_OK;
