@@ -13,13 +13,14 @@
 //                    the queries in sub-steps of 64.  Scores are computed TRANSPOSED, S^T = K Q^T and dP^T = V dO^T
 //                    (wgmma SS, accumulator rows = keys), so P^T and dS^T, rounded to bf16/fp16, stay in registers and
 //                    feed dV += P^T dO and dK += dS^T Q as the A operand (wgmma RS, B = dO / Q stage read MN-major).
-//   bwd_dq_kernel    query-tile outer.  One CTA owns (b, h, 128 queries) and a range of key tiles (K and V streamed
-//                    through a TMA ring); S = Q K^T, dP = dO V^T, dS in registers, dQ += dS K (K tile read MN-major,
-//                    as V is in the forward).  dQ accumulates in registers over the CTA's key range and is added into an
-//                    fp32 buffer once per CTA.
+//   bwd_dq_kernel    query-tile outer.  A work item is (b, h, 128 queries) and a range of key tiles (K and V streamed
+//                    through a TMA ring in stages of KS keys); S = Q K^T, dP = dO V^T, dS in registers, dQ += dS K (K
+//                    stage read MN-major, as V is in the forward).  dQ accumulates in registers over the item's key
+//                    range and leaves once per item: added into an fp32 buffer (KS = 128), or stored as an ordered
+//                    fp32 partial (KS = 64).
 //
 // Head dims above 128 (up to 192: a third 64-channel box) run the dK/dV kernel as a dV pass and a dK pass and the dQ
-// kernel as bwd_dq64_kernel (64-key stages, ordered fp32 partials instead of atomics); see there.
+// kernel on 64-key stages; see dq_ordered_partials.
 //
 // Warpgroup 0 is the TMA producer (one lane), warpgroups 1 and 2 each own 64 rows of the tile.
 #include "pcv_common.cuh"
@@ -53,11 +54,10 @@ struct BwdParams {
   const uint32_t* pad_bits;  // (B, pad_wpr) bit set = padding key; nullptr if none
   int pad_wpr;
   const float* stats;        // (B, H, 2*nq) blocks of kStatsBytes (layout: see bwd_prep_kernel)
-  float* dq32;               // (Bq, N, H*dqk) fp32, zero-initialised; CTAs reduce into it
+  float* dq32;               // (Bq, N, H*dqk) fp32, zero-initialised, that CTAs reduce into; or the dQ partials
   void* dk;
   void* dv_out;
   int64_t dk_sb, dk_sm, dk_sh, dv_sb, dv_sm, dv_sh;
-  int wide_store;            // dk / dv rows are 32-byte aligned: 256-bit stores
   uint32_t drop_thresh;      // attention dropout: element kept iff its random byte >= drop_thresh (0 = no dropout)
   uint32_t seed_lo, seed_hi;
   int key_base;              // global index of local key 0 (even; 0 unless key-sharded): the mask hashes key_base + j
@@ -126,23 +126,6 @@ __global__ void __launch_bounds__(256) bwd_prep_kernel(const T* __restrict__ out
   }
 }
 
-// dq32 (Bq, N, H*dqk) fp32 -> dq in the operand dtype with its own strides
-template <typename T>
-__global__ void __launch_bounds__(256) bwd_cast_dq_kernel(const float* __restrict__ dq32, T* __restrict__ dq, int Bq,
-                                                          int N, int H, int dqk, int64_t sb, int64_t sn, int64_t sh) {
-  const int64_t total = (int64_t)Bq * N * H * dqk;
-  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
-       idx += (int64_t)gridDim.x * blockDim.x) {
-    const int c = (int)(idx % dqk);
-    int64_t r = idx / dqk;
-    const int h = (int)(r % H);
-    r /= H;
-    const int n = (int)(r % N);
-    const int b = (int)(r / N);
-    dq[b * sb + (int64_t)n * sn + h * sh + c] = Elem<T>::from_f(dq32[idx]);
-  }
-}
-
 // ---------------------------------------------------------------------------------------------------------------
 // kernel 1: dK, dV.  CTA = one 128-key tile (K, V resident in shared memory; persistent over tiles), warpgroups 1-2
 // own 64 keys each and walk the queries in sub-steps of 64 (Q / dO pieces through a TMA ring).
@@ -155,12 +138,13 @@ struct Cfg1 {
   static constexpr int kSmem = kKVBytes + kSlots * kStage + 2048;
 };
 
-// kernel 2 (dQ): CTA = (b, h, 128 queries, key range); warpgroups 1-2 own 64 queries each; Q and dO stay resident,
-// K / V tiles stream through a TMA ring.
-template <int NQB, int NVB>
+// kernel 2 (dQ): work item = (b, h, 128 queries, key range); warpgroups 1-2 own 64 queries each; Q and dO stay
+// resident per item, K / V stream through a TMA ring in stages of KS keys (a KS-row box per 64 channels).
+template <int NQB, int NVB, int KS>
 struct Cfg2 {
   static constexpr int kQBytes = (NQB + NVB) * kBoxBytes;
-  static constexpr int kStage = (NQB + NVB) * kBoxBytes;
+  static constexpr int kKSBox = KS * 128;
+  static constexpr int kStage = (NQB + NVB) * kKSBox;
   static constexpr int kSlots = (kSmemLimit - kQBytes - 2048) / kStage > 4 ? 4 : (kSmemLimit - kQBytes - 2048) / kStage;
   static constexpr int kSmem = kQBytes + kSlots * kStage + 2048;
   static_assert(kSlots >= 2, "shared memory budget");
@@ -174,6 +158,31 @@ struct BwdBarriers {
 __device__ __forceinline__ bool filled_key(const BwdParams& p, int b, int j, int n) {
   if (p.pad_bits != nullptr && ((p.pad_bits[(int64_t)b * p.pad_wpr + (j >> 5)] >> (j & 31)) & 1u)) return true;
   return p.causal && j > n + p.cshift;
+}
+
+// The score-gradient rule of one element (query n, local key j, score s = q.k, dP = dO.v) with the row statistics of
+// query n: P = 2^(s * scale_log2 + nlse), fillp on a filled key, 0 outside the problem; pd = P after dropout (the dV
+// operand) and ds = P (dP' - delta) with dP' = dP after dropout, 0 on filled keys and outside the problem.  A caller
+// that uses one of the two lets the compiler drop the other.  Without dropout neither is scaled (drop_rp would be
+// exactly 1: dropout_rule).  bwd_dkdv_kernel writes the same rule out in its element loop: through this helper its
+// wide dV and dK passes ran about 10 % slower on an H100 SXM (700 W).
+struct ScoreGrad {
+  float pd, ds;
+};
+
+__device__ __forceinline__ ScoreGrad score_grad(const BwdParams& p, int b, int bh, int n, int j, float s, float dP,
+                                                float nlse, float delta, float fillp) {
+  const bool oob = j >= p.M || n >= p.N;
+  const bool filled = !oob && filled_key(p, b, j, n);
+  const float P = oob ? 0.f : (filled ? fillp : ex2(fmaf(s, p.scale_log2, nlse)));
+  float pd = P;
+  if (p.drop_thresh) {
+    const uint32_t jg = (uint32_t)(p.key_base + j);
+    const bool keep = drop_keep(drop_bits(p.seed_lo, p.seed_hi, (uint32_t)bh, (uint32_t)n, jg), n, jg, p.drop_thresh);
+    dP = keep ? dP * p.drop_rp : 0.f;
+    pd = keep ? P * p.drop_rp : 0.f;
+  }
+  return {pd, (oob || filled) ? 0.f : P * (dP - delta)};
 }
 
 // Outputs of one bwd_dkdv_kernel launch.  With a head dim above 128 (a third 64-channel box) the dK and dV accumulators
@@ -372,174 +381,22 @@ bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tq64, const __grid_constant_
   }
 }
 
-// dQ += scale * dS K, reduced into p.dq32
-template <int NQB, int NVB, bool BF16>
+// The dQ epilogue of KS-key stages.  Head dims above 128 run the dQ kernel on 64-key stages: S and dP then take 32
+// registers each beside the three dQ accumulator boxes, and that is what keeps those instantiations spill-free (a
+// 128-key stage needs 64 + 64).  Their work items store their dQ share (already scaled) as one fp32 partial
+// (Bq, N, H*dqk) per (batch contribution, split), partial index (q_bcast ? b : 0) * splits + split, and
+// bwd_sum_dq_kernel adds the partials in index order, so the wide dQ is bitwise reproducible.  128-key stages add their
+// share into the zeroed fp32 p.dq32 with atomics.
+constexpr bool dq_ordered_partials(int ks) { return ks == 64; }
+
+// dQ += scale * dS K.  CTAs walk the work items (b, h, query tile, split) persistently, as the dK/dV kernel walks its
+// key tiles; with 128-key stages the grid is one CTA per item.  A split covers tiles_per_split tiles of 128 keys, i.e.
+// tiles_per_split * 128 / KS stages.
+template <int NQB, int NVB, bool BF16, int KS>
 __global__ void __launch_bounds__(kThreads, 1)
 bwd_dq_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk,
               const __grid_constant__ CUtensorMap tv, const __grid_constant__ CUtensorMap tdo, const BwdParams p) {
-  using C = Cfg2<NQB, NVB>;
-  constexpr int NS = C::kSlots;
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* sQ = smem;
-  uint8_t* sdO = smem + NQB * kBoxBytes;
-  uint8_t* sRing = smem + C::kQBytes;
-  BwdBarriers& bar = *reinterpret_cast<BwdBarriers*>(sRing + NS * C::kStage);
-  const int wg = threadIdx.x / 128;
-  const int unit = blockIdx.x / p.splits, split = blockIdx.x % p.splits;
-  const int bh = unit / p.nq, qt = unit % p.nq, b = bh / p.H, h = bh % p.H;
-  const int kt0 = split * p.tiles_per_split, kt1 = min(p.nk, kt0 + p.tiles_per_split);
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < NS; ++s) {
-      mbar_init(&bar.full[s], 1);
-      mbar_init(&bar.empty[s], 8);
-    }
-    mbar_init(&bar.fix_full, 1);
-    fence_mbar_init();
-  }
-  __syncthreads();
-
-  if (wg == 0) {
-    reg_dealloc<40>();
-    if (threadIdx.x == 0) {
-      mbar_arrive_expect_tx(&bar.fix_full, C::kQBytes);
-      for (int c = 0; c < NQB; ++c) tma_load_4d(sQ + c * kBoxBytes, &tq, &bar.fix_full, c * 64, qt * kT, h, p.q_bcast ? 0 : b);
-      for (int c = 0; c < NVB; ++c) tma_load_4d(sdO + c * kBoxBytes, &tdo, &bar.fix_full, c * 64, qt * kT, h, b);
-      uint32_t it = 0;
-      for (int kt = kt0; kt < kt1; ++kt, ++it) {
-        const uint32_t s = it % NS;
-        mbar_wait(&bar.empty[s], ((it / NS) & 1) ^ 1, 31);
-        mbar_arrive_expect_tx(&bar.full[s], C::kStage);
-        uint8_t* st = sRing + s * C::kStage;
-        for (int c = 0; c < NQB; ++c) tma_load_4d(st + c * kBoxBytes, &tk, &bar.full[s], c * 64, kt * kT, h, b);
-        for (int c = 0; c < NVB; ++c) tma_load_4d(st + (NQB + c) * kBoxBytes, &tv, &bar.full[s], c * 64, kt * kT, h, b);
-      }
-    }
-    return;
-  }
-
-  reg_alloc<232>();
-  const int cw = wg - 1;
-  const int tid = threadIdx.x - 128 * wg;
-  const int warp = tid >> 5, lane = tid & 31;
-  const int qloc = 64 * cw + 16 * warp + (lane >> 2);
-  const int cq = 2 * (lane & 3);
-  const uint32_t q_base = smem_u32(sQ) + cw * 64 * 128, do_base = smem_u32(sdO) + cw * 64 * 128;
-  const uint32_t ring = smem_u32(sRing);
-  int nrow[2];
-  float nlse[2], delta[2], fillp[2];
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    nrow[i] = qt * kT + qloc + 8 * i;
-    const float* blk = p.stats + ((int64_t)bh * (p.Npad / 64) + nrow[i] / 64) * (kStatsBytes / 4);
-    const int r = nrow[i] % 64;
-    nlse[i] = blk[stat_nlse_idx(r)];
-    delta[i] = blk[stat_delta_idx(r)];
-    fillp[i] = blk[stat_fillp_idx(r)];
-  }
-  float acc[NQB][32];
-#pragma unroll
-  for (int c = 0; c < NQB; ++c)
-#pragma unroll
-    for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
-  mbar_wait(&bar.fix_full, 0, 32);
-  uint32_t it = 0;
-  for (int kt = kt0; kt < kt1; ++kt, ++it) {
-    const uint32_t s = it % NS;
-    const uint32_t stk = ring + s * C::kStage, stv = stk + NQB * kBoxBytes;
-    mbar_wait(&bar.full[s], (it / NS) & 1, 33);
-    float sc[64], dp[64];
-    wgmma_fence();
-#pragma unroll
-    for (int c = 0; c < NQB; ++c)
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk)
-        wgmma_ss<128, BF16>(sc, make_desc(q_base + c * kBoxBytes + kk * 32), make_desc(stk + c * kBoxBytes + kk * 32), (c | kk) != 0);
-#pragma unroll
-    for (int c = 0; c < NVB; ++c)
-#pragma unroll
-      for (int kk = 0; kk < 4; ++kk)
-        wgmma_ss<128, BF16>(dp, make_desc(do_base + c * kBoxBytes + kk * 32), make_desc(stv + c * kBoxBytes + kk * 32), (c | kk) != 0);
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs(sc);
-    fence_regs(dp);
-    uint32_t a[8][4];
-#pragma unroll
-    for (int g = 0; g < 16; ++g) {
-      float val[4];
-#pragma unroll
-      for (int e4 = 0; e4 < 4; ++e4) {
-        const int i = e4 >> 1, e = e4 & 1;
-        const int j = kt * kT + 8 * g + cq + e, n = nrow[i];
-        const bool oob = j >= p.M || n >= p.N;
-        const bool filled = !oob && filled_key(p, b, j, n);
-        const float P = oob ? 0.f : (filled ? fillp[i] : ex2(fmaf(sc[4 * g + e4], p.scale_log2, nlse[i])));
-        bool keep = true;
-        if (p.drop_thresh) {
-          const uint32_t jg = (uint32_t)(p.key_base + j);
-          keep = drop_keep(drop_bits(p.seed_lo, p.seed_hi, (uint32_t)bh, (uint32_t)n, jg), n, jg, p.drop_thresh);
-        }
-        const float dP = keep ? dp[4 * g + e4] * p.drop_rp : 0.f;
-        val[e4] = (oob || filled) ? 0.f : P * (dP - delta[i]);
-      }
-      a[g >> 1][(g & 1) * 2 + 0] = pack2(val[0], val[1], BF16);
-      a[g >> 1][(g & 1) * 2 + 1] = pack2(val[2], val[3], BF16);
-    }
-    wgmma_fence();
-#pragma unroll
-    for (int c = 0; c < NQB; ++c)
-#pragma unroll
-      for (int kk = 0; kk < 8; ++kk) wgmma_rs<64, BF16>(acc[c], a[kk], make_desc(stk + c * kBoxBytes + kk * 2048));
-    wgmma_commit();
-    wgmma_wait<0>();
-#pragma unroll
-    for (int c = 0; c < NQB; ++c) fence_regs(acc[c]);
-    warp_arrive(&bar.empty[s]);
-  }
-  // reduce this CTA's share into the fp32 buffer
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const int n = nrow[i];
-    if (n >= p.N) continue;
-    const int bq = p.q_bcast ? 0 : b;
-    float* dst = p.dq32 + (((int64_t)bq * p.N + n) * p.H + h) * p.dqk;
-#pragma unroll
-    for (int c = 0; c < NQB; ++c)
-#pragma unroll
-      for (int g = 0; g < 8; ++g) {
-        const int col = c * 64 + 8 * g + cq;
-        if (col < p.dqk) {
-          atomicAdd(dst + col, acc[c][4 * g + 2 * i] * p.scale);
-          atomicAdd(dst + col + 1, acc[c][4 * g + 2 * i + 1] * p.scale);
-        }
-      }
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// kernel 2 for head dims above 128 (NQB or NVB = 3): dQ with 64-key K / V stages, so S and dP take 32 registers each
-// (a 128-key tile would need 64 + 64 beside the three dQ boxes).  The work items are bwd_dq_kernel's CTAs, (b, h,
-// 128 queries, split of 128-key tiles), walked persistently as the dK/dV kernel walks its key tiles (in the
-// one-item-per-CTA form ptxas spills the dQ accumulators at NQB = 3).  No atomics: every work item stores its dQ share
-// (already scaled) as one fp32 partial (Bq, N, H*dqk) per (batch contribution, split), partial index
-// (q_bcast ? b : 0) * splits + split, and bwd_sum_dq_kernel adds the partials in index order, so dQ is bitwise
-// reproducible.
-// ---------------------------------------------------------------------------------------------------------------
-template <int NQB, int NVB>
-struct Cfg3 {
-  static constexpr int kQBytes = (NQB + NVB) * kBoxBytes;
-  static constexpr int kStage = (NQB + NVB) * kBox64;
-  static constexpr int kSlots = (kSmemLimit - kQBytes - 2048) / kStage > 4 ? 4 : (kSmemLimit - kQBytes - 2048) / kStage;
-  static constexpr int kSmem = kQBytes + kSlots * kStage + 2048;
-  static_assert(kSlots >= 2, "shared memory budget");
-};
-
-template <int NQB, int NVB, bool BF16>
-__global__ void __launch_bounds__(kThreads, 1)
-bwd_dq64_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ CUtensorMap tk64,
-                const __grid_constant__ CUtensorMap tv64, const __grid_constant__ CUtensorMap tdo, const BwdParams p) {
-  using C = Cfg3<NQB, NVB>;
+  using C = Cfg2<NQB, NVB, KS>;
   constexpr int NS = C::kSlots;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -549,7 +406,7 @@ bwd_dq64_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
   BwdBarriers& bar = *reinterpret_cast<BwdBarriers*>(sRing + NS * C::kStage);
   const int wg = threadIdx.x / 128;
   const int total = p.B * p.H * p.nq * p.splits;  // work items (b, h, query tile, split)
-  const int nk64 = (p.M + 63) / 64;
+  const int nks = (p.M + KS - 1) / KS, per_split = p.tiles_per_split * (kT / KS);  // stages in all, per split
   if (threadIdx.x == 0) {
     for (int s = 0; s < NS; ++s) {
       mbar_init(&bar.full[s], 1);
@@ -568,7 +425,7 @@ bwd_dq64_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
       for (int w = blockIdx.x; w < total; w += gridDim.x, ++wl) {
         const int unit = w / p.splits, split = w % p.splits;
         const int bh = unit / p.nq, qt = unit % p.nq, b = bh / p.H, h = bh % p.H;
-        const int kt0 = 2 * split * p.tiles_per_split, kt1 = min(nk64, kt0 + 2 * p.tiles_per_split);
+        const int kt0 = split * per_split, kt1 = min(nks, kt0 + per_split);
         mbar_wait(&bar.fix_empty, (wl & 1) ^ 1, 34);
         mbar_arrive_expect_tx(&bar.fix_full, C::kQBytes);
         for (int c = 0; c < NQB; ++c)
@@ -576,12 +433,12 @@ bwd_dq64_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
         for (int c = 0; c < NVB; ++c) tma_load_4d(sdO + c * kBoxBytes, &tdo, &bar.fix_full, c * 64, qt * kT, h, b);
         for (int kt = kt0; kt < kt1; ++kt, ++it) {
           const uint32_t s = it % NS;
-          mbar_wait(&bar.empty[s], ((it / NS) & 1) ^ 1, 35);
+          mbar_wait(&bar.empty[s], ((it / NS) & 1) ^ 1, 31);
           mbar_arrive_expect_tx(&bar.full[s], C::kStage);
           uint8_t* st = sRing + s * C::kStage;
-          for (int c = 0; c < NQB; ++c) tma_load_4d(st + c * kBox64, &tk64, &bar.full[s], c * 64, kt * 64, h, b);
+          for (int c = 0; c < NQB; ++c) tma_load_4d(st + c * C::kKSBox, &tk, &bar.full[s], c * 64, kt * KS, h, b);
           for (int c = 0; c < NVB; ++c)
-            tma_load_4d(st + (NQB + c) * kBox64, &tv64, &bar.full[s], c * 64, kt * 64, h, b);
+            tma_load_4d(st + (NQB + c) * C::kKSBox, &tv, &bar.full[s], c * 64, kt * KS, h, b);
         }
       }
     }
@@ -601,9 +458,9 @@ bwd_dq64_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
   for (int w = blockIdx.x; w < total; w += gridDim.x, ++wl) {
     const int unit = w / p.splits, split = w % p.splits;
     const int bh = unit / p.nq, qt = unit % p.nq, b = bh / p.H, h = bh % p.H;
-    const int kt0 = 2 * split * p.tiles_per_split, kt1 = min(nk64, kt0 + 2 * p.tiles_per_split);
+    const int kt0 = split * per_split, kt1 = min(nks, kt0 + per_split);
     const float* blk = p.stats + ((int64_t)bh * (p.Npad / 64) + 2 * qt + cw) * (kStatsBytes / 4);
-    mbar_wait(&bar.fix_full, wl & 1, 36);
+    mbar_wait(&bar.fix_full, wl & 1, 32);
     float acc[NQB][32];
 #pragma unroll
     for (int c = 0; c < NQB; ++c)
@@ -611,43 +468,34 @@ bwd_dq64_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
       for (int i = 0; i < 32; ++i) acc[c][i] = 0.f;
     for (int kt = kt0; kt < kt1; ++kt, ++it) {
       const uint32_t s = it % NS;
-      const uint32_t stk = ring + s * C::kStage, stv = stk + NQB * kBox64;
-      mbar_wait(&bar.full[s], (it / NS) & 1, 37);
-      float sc[32], dp[32];
+      const uint32_t stk = ring + s * C::kStage, stv = stk + NQB * C::kKSBox;
+      mbar_wait(&bar.full[s], (it / NS) & 1, 33);
+      float sc[KS / 2], dp[KS / 2];
       wgmma_fence();
 #pragma unroll
       for (int c = 0; c < NQB; ++c)
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk)
-          wgmma_ss<64, BF16>(sc, make_desc(q_base + c * kBoxBytes + kk * 32), make_desc(stk + c * kBox64 + kk * 32), (c | kk) != 0);
+          wgmma_ss<KS, BF16>(sc, make_desc(q_base + c * kBoxBytes + kk * 32), make_desc(stk + c * C::kKSBox + kk * 32), (c | kk) != 0);
 #pragma unroll
       for (int c = 0; c < NVB; ++c)
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk)
-          wgmma_ss<64, BF16>(dp, make_desc(do_base + c * kBoxBytes + kk * 32), make_desc(stv + c * kBox64 + kk * 32), (c | kk) != 0);
+          wgmma_ss<KS, BF16>(dp, make_desc(do_base + c * kBoxBytes + kk * 32), make_desc(stv + c * C::kKSBox + kk * 32), (c | kk) != 0);
       wgmma_commit();
       wgmma_wait<0>();
       fence_regs(sc);
       fence_regs(dp);
-      uint32_t a[4][4];
+      uint32_t a[KS / 16][4];
 #pragma unroll
-      for (int g = 0; g < 8; ++g) {
+      for (int g = 0; g < KS / 8; ++g) {
         float val[4];
 #pragma unroll
         for (int e4 = 0; e4 < 4; ++e4) {
           const int i = e4 >> 1, e = e4 & 1;
-          const int j = kt * 64 + 8 * g + cq + e, n = qt * kT + qloc + 8 * i, r = r0 + 8 * i;
-          const float nlse = blk[stat_nlse_idx(r)], delta = blk[stat_delta_idx(r)], fillp = blk[stat_fillp_idx(r)];
-          const bool oob = j >= p.M || n >= p.N;
-          const bool filled = !oob && filled_key(p, b, j, n);
-          const float P = oob ? 0.f : (filled ? fillp : ex2(fmaf(sc[4 * g + e4], p.scale_log2, nlse)));
-          bool keep = true;
-          if (p.drop_thresh) {
-            const uint32_t jg = (uint32_t)(p.key_base + j);
-            keep = drop_keep(drop_bits(p.seed_lo, p.seed_hi, (uint32_t)bh, (uint32_t)n, jg), n, jg, p.drop_thresh);
-          }
-          const float dP = keep ? dp[4 * g + e4] * p.drop_rp : 0.f;
-          val[e4] = (oob || filled) ? 0.f : P * (dP - delta);
+          const int r = r0 + 8 * i;
+          val[e4] = score_grad(p, b, bh, qt * kT + qloc + 8 * i, kt * KS + 8 * g + cq + e, sc[4 * g + e4], dp[4 * g + e4],
+                               blk[stat_nlse_idx(r)], blk[stat_delta_idx(r)], blk[stat_fillp_idx(r)]).ds;
         }
         a[g >> 1][(g & 1) * 2 + 0] = pack2(val[0], val[1], BF16);
         a[g >> 1][(g & 1) * 2 + 1] = pack2(val[2], val[3], BF16);
@@ -656,7 +504,7 @@ bwd_dq64_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
 #pragma unroll
       for (int c = 0; c < NQB; ++c)
 #pragma unroll
-        for (int kk = 0; kk < 4; ++kk) wgmma_rs<64, BF16>(acc[c], a[kk], make_desc(stk + c * kBox64 + kk * 2048));
+        for (int kk = 0; kk < KS / 16; ++kk) wgmma_rs<64, BF16>(acc[c], a[kk], make_desc(stk + c * C::kKSBox + kk * 2048));
       wgmma_commit();
       wgmma_wait<0>();
 #pragma unroll
@@ -664,9 +512,8 @@ bwd_dq64_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
       warp_arrive(&bar.empty[s]);
     }
     warp_arrive(&bar.fix_empty);
-    // this work item's partial: every element of it is written by exactly one work item
     const int Bq = p.q_bcast ? 1 : p.B, bq = p.q_bcast ? 0 : b;
-    const int64_t part = (int64_t)(p.q_bcast ? b : 0) * p.splits + split;
+    const int64_t part = dq_ordered_partials(KS) ? (int64_t)(p.q_bcast ? b : 0) * p.splits + split : 0;
 #pragma unroll
     for (int i = 0; i < 2; ++i) {
       const int n = qt * kT + qloc + 8 * i;
@@ -677,14 +524,21 @@ bwd_dq64_kernel(const __grid_constant__ CUtensorMap tq, const __grid_constant__ 
 #pragma unroll
         for (int g = 0; g < 8; ++g) {
           const int col = c * 64 + 8 * g + cq;
-          if (col < p.dqk)
-            *reinterpret_cast<float2*>(dst + col) = make_float2(acc[c][4 * g + 2 * i] * p.scale, acc[c][4 * g + 2 * i + 1] * p.scale);
+          if (col >= p.dqk) continue;
+          const float x = acc[c][4 * g + 2 * i] * p.scale, y = acc[c][4 * g + 2 * i + 1] * p.scale;
+          if constexpr (dq_ordered_partials(KS)) {  // every element of the partial is written by exactly one item
+            *reinterpret_cast<float2*>(dst + col) = make_float2(x, y);
+          } else {
+            atomicAdd(dst + col, x);
+            atomicAdd(dst + col + 1, y);
+          }
         }
     }
   }
 }
 
-// the dQ partials of bwd_dq64_kernel (nparts x (Bq, N, H*dqk) fp32), added in partial order -> dq in the operand dtype
+// the dQ partials (nparts x (Bq, N, H*dqk) fp32; one, the atomics' buffer, up to head dim 128), added in partial order
+// from 0.f -> dq (bf16, fp16 or fp32) with its own strides
 template <typename T>
 __global__ void __launch_bounds__(256) bwd_sum_dq_kernel(const float* __restrict__ part, int nparts, T* __restrict__ dq,
                                                          int Bq, int N, int H, int dqk, int64_t sb, int64_t sn, int64_t sh) {
@@ -725,9 +579,9 @@ void dq_split(int units, int nk, int sms, int& tiles_per_split, int& splits) {
   splits = (nk + tiles_per_split - 1) / tiles_per_split;
 }
 
-// Head dims above 128 take the wide variants: the dK/dV kernel with up to three boxes (in two passes above four boxes
-// in all) and bwd_dq64_kernel with its ordered dQ partials.
-bool wide_bwd(int dqk, int dv) { return dqk > 128 || dv > 128; }
+// Head dims above 128 take the wide variants: the dK/dV kernel with a third box as a dV and a dK pass, and the dQ
+// kernel on 64-key stages with its ordered dQ partials (dq_ordered_partials).
+constexpr bool wide_bwd(int dqk, int dv) { return dqk > 128 || dv > 128; }
 
 // The wide dQ split is planned for a fixed SM count (the H100 SXM's 132), not the device's: the number of dQ partials,
 // and so the workspace size, follow from the problem alone, and so does the order in which dQ is summed.
@@ -767,14 +621,18 @@ BwdLayout bwd_layout(const pcv_attn_bwd_params& a, const pcv_key_shard* shard) {
   return L;
 }
 
+// Key rows of the dQ kernel's ring stages: 64 for the wide head dims (see dq_ordered_partials), else a whole tile.
+constexpr int dq_stage_keys(int dqk, int dv) { return wide_bwd(dqk, dv) ? 64 : kT; }
+
+// The tensor maps of one backward: Q and dO resident in the dQ kernel (128-row boxes) and staged by the dK/dV kernel
+// (64-row boxes); K and V resident in the dK/dV kernel (128-row boxes) and staged by the dQ kernel (KS-row boxes).
 struct BwdMaps {
-  CUtensorMap q, k, v, dout;  // 128-row boxes
-  CUtensorMap q64, dout64;    // the dK/dV kernel stages Q and dO in 64-row boxes
-  CUtensorMap k64, v64;       // wide backward only; bwd_dq64_kernel stages K and V in 64-row boxes
+  CUtensorMap q, dout, q64, dout64;
+  CUtensorMap k, v, k_dq, v_dq;
 };
 
 // Fills the BwdParams core and the dq-kernel split, zeroes the fp32 accumulator, writes the row statistics, packs the
-// pad mask and encodes the q / k / v tensor maps.  The call's keys are [m_offset, m_offset + M) of m_total (the causal
+// pad mask and encodes the tensor maps.  The call's keys are [m_offset, m_offset + M) of m_total (the causal
 // diagonal and the dropout hash use global key indices).
 int bwd_setup(const pcv_attn_bwd_params& a, const BwdLayout& L, int m_total, int m_offset, cudaStream_t stream,
               BwdParams& p, BwdMaps& m, int& sms) {
@@ -828,76 +686,70 @@ int bwd_setup(const pcv_attn_bwd_params& a, const BwdLayout& L, int m_total, int
     p.pad_wpr = pad_words_per_row(a.M);
   }
 
-  const int Bq = a.q_stride_b == 0 ? 1 : a.B;
-  rc = make_tmap_4d(&m.q, a.q, a.dtype, a.dqk, a.N, a.H, Bq, a.q_stride_n, a.q_stride_h, a.q_stride_b, kT);
-  if (rc != PCV_OK) return rc;
-  rc = make_tmap_4d(&m.k, a.k, a.dtype, a.dqk, a.M, a.H, a.B, a.k_stride_m, a.k_stride_h, a.k_stride_b, kT);
-  if (rc != PCV_OK) return rc;
-  return make_tmap_4d(&m.v, a.v, a.dtype, a.dv, a.M, a.H, a.B, a.v_stride_m, a.v_stride_h, a.v_stride_b, kT);
-}
-
-// the dK/dV kernel, then the dQ kernel
-template <int NQB, int NVB, bool BF16>
-int launch_tc_kernels(const BwdMaps& m, const BwdParams& p, int sms, cudaStream_t stream) {
-  const int rc = launch_kernel(bwd_dkdv_kernel<NQB, NVB, BF16>, dim3(std::min(p.total_tiles, sms)), kThreads,
-                               Cfg1<NQB, NVB>::kSmem, 0, stream, m.q64, m.k, m.v, m.dout64, p);
-  if (rc != PCV_OK) return rc;
-  return launch_kernel(bwd_dq_kernel<NQB, NVB, BF16>, dim3(p.B * p.H * p.nq * p.splits), kThreads, Cfg2<NQB, NVB>::kSmem,
-                       0, stream, m.q, m.k, m.v, m.dout, p);
-}
-
-// head dims up to 64 take one 64-channel box, up to 128 two
-template <bool BF16>
-int launch_tc(const BwdMaps& m, const BwdParams& p, int sms, cudaStream_t stream) {
-  if (p.dqk <= 64)
-    return p.dv <= 64 ? launch_tc_kernels<1, 1, BF16>(m, p, sms, stream) : launch_tc_kernels<1, 2, BF16>(m, p, sms, stream);
-  return p.dv <= 64 ? launch_tc_kernels<2, 1, BF16>(m, p, sms, stream) : launch_tc_kernels<2, 2, BF16>(m, p, sms, stream);
-}
-
-// The wide backward (a head dim above 128): the dK/dV kernel as a dV pass and a dK pass, then bwd_dq64_kernel into the
-// dQ partials.
-template <int NQB, int NVB, bool BF16>
-int launch_wide_kernels(const BwdMaps& m, const BwdParams& p, int sms, cudaStream_t stream) {
-  using C1 = Cfg1<NQB, NVB>;
-  const dim3 grid1(std::min(p.total_tiles, sms));
-  int rc = launch_kernel(bwd_dkdv_kernel<NQB, NVB, BF16, kOutDV>, grid1, kThreads, C1::kSmem, 0, stream, m.q64, m.k, m.v,
-                         m.dout64, p);
-  if (rc != PCV_OK) return rc;
-  rc = launch_kernel(bwd_dkdv_kernel<NQB, NVB, BF16, kOutDK>, grid1, kThreads, C1::kSmem, 0, stream, m.q64, m.k, m.v,
-                     m.dout64, p);
-  if (rc != PCV_OK) return rc;
-  return launch_kernel(bwd_dq64_kernel<NQB, NVB, BF16>, dim3(std::min(p.B * p.H * p.nq * p.splits, sms)), kThreads,
-                       Cfg3<NQB, NVB>::kSmem, 0, stream, m.q, m.k64, m.v64, m.dout, p);
-}
-
-// every (NQB, NVB) in {1, 2, 3}^2 with a 3
-template <bool BF16>
-int launch_wide(const BwdMaps& m, const BwdParams& p, int sms, cudaStream_t stream) {
-  const int nqb = (p.dqk + 63) / 64, nvb = (p.dv + 63) / 64;
-  if (nqb == 3) {
-    if (nvb == 1) return launch_wide_kernels<3, 1, BF16>(m, p, sms, stream);
-    if (nvb == 2) return launch_wide_kernels<3, 2, BF16>(m, p, sms, stream);
-    return launch_wide_kernels<3, 3, BF16>(m, p, sms, stream);
+  const int Bq = a.q_stride_b == 0 ? 1 : a.B, ks = dq_stage_keys(a.dqk, a.dv);
+  const struct {
+    CUtensorMap* map;
+    const void* base;
+    int channels, rows, batch;
+    int64_t s_row, s_h, s_b;
+    int box;
+  } maps[] = {
+      {&m.q, a.q, a.dqk, a.N, Bq, a.q_stride_n, a.q_stride_h, a.q_stride_b, kT},
+      {&m.q64, a.q, a.dqk, a.N, Bq, a.q_stride_n, a.q_stride_h, a.q_stride_b, 64},
+      {&m.dout, a.grad_out, a.dv, a.N, a.B, a.go_stride_n, a.go_stride_h, a.go_stride_b, kT},
+      {&m.dout64, a.grad_out, a.dv, a.N, a.B, a.go_stride_n, a.go_stride_h, a.go_stride_b, 64},
+      {&m.k, a.k, a.dqk, a.M, a.B, a.k_stride_m, a.k_stride_h, a.k_stride_b, kT},
+      {&m.k_dq, a.k, a.dqk, a.M, a.B, a.k_stride_m, a.k_stride_h, a.k_stride_b, ks},
+      {&m.v, a.v, a.dv, a.M, a.B, a.v_stride_m, a.v_stride_h, a.v_stride_b, kT},
+      {&m.v_dq, a.v, a.dv, a.M, a.B, a.v_stride_m, a.v_stride_h, a.v_stride_b, ks},
+  };
+  for (const auto& t : maps) {
+    rc = make_tmap_4d(t.map, t.base, a.dtype, t.channels, t.rows, a.H, t.batch, t.s_row, t.s_h, t.s_b, t.box);
+    if (rc != PCV_OK) return rc;
   }
-  return nqb == 1 ? launch_wide_kernels<1, 3, BF16>(m, p, sms, stream) : launch_wide_kernels<2, 3, BF16>(m, p, sms, stream);
-}
-
-// fp32 accumulator (Bq, N, H*width) -> the 16-bit output with its own strides
-int launch_cast(bool bf16, const float* acc, void* dst, int Bq, int N, int H, int width, int64_t sb, int64_t sn,
-                int64_t sh, cudaStream_t stream) {
-  const int64_t total = (int64_t)Bq * N * H * width;
-  const int blocks = (int)std::min<int64_t>((total + 255) / 256, 4096);
-  if (bf16)
-    bwd_cast_dq_kernel<__nv_bfloat16><<<blocks, 256, 0, stream>>>(acc, reinterpret_cast<__nv_bfloat16*>(dst), Bq, N, H,
-                                                                  width, sb, sn, sh);
-  else
-    bwd_cast_dq_kernel<__half><<<blocks, 256, 0, stream>>>(acc, reinterpret_cast<__half*>(dst), Bq, N, H, width, sb, sn, sh);
-  PCV_CHECK_CUDA(cudaGetLastError());
-  count_launch();
   return PCV_OK;
 }
 
-// the wide backward's dQ partials, summed in order -> dq (dtype: bf16, fp16 or fp32) with its own strides
+// One backward of NQB x NVB boxes: the dK/dV kernel (a dV and a dK pass for the wide head dims), then the dQ kernel on
+// its KS-key stages, one CTA per work item on 128-key stages and persistent on at most one CTA per SM on 64-key ones.
+template <int NQB, int NVB, bool BF16>
+int launch_shape(const BwdMaps& m, const BwdParams& p, int sms, cudaStream_t stream) {
+  constexpr int KS = dq_stage_keys(NQB * 64, NVB * 64);
+  const dim3 grid1(std::min(p.total_tiles, sms));
+  constexpr int smem1 = Cfg1<NQB, NVB>::kSmem;
+  int rc;
+  if constexpr (wide_bwd(NQB * 64, NVB * 64)) {
+    rc = launch_kernel(bwd_dkdv_kernel<NQB, NVB, BF16, kOutDV>, grid1, kThreads, smem1, 0, stream, m.q64, m.k, m.v,
+                       m.dout64, p);
+    if (rc == PCV_OK)
+      rc = launch_kernel(bwd_dkdv_kernel<NQB, NVB, BF16, kOutDK>, grid1, kThreads, smem1, 0, stream, m.q64, m.k, m.v,
+                         m.dout64, p);
+  } else {
+    rc = launch_kernel(bwd_dkdv_kernel<NQB, NVB, BF16>, grid1, kThreads, smem1, 0, stream, m.q64, m.k, m.v, m.dout64, p);
+  }
+  if (rc != PCV_OK) return rc;
+  const int items = p.B * p.H * p.nq * p.splits;
+  return launch_kernel(bwd_dq_kernel<NQB, NVB, BF16, KS>, dim3(KS == kT ? items : std::min(items, sms)), kThreads,
+                       Cfg2<NQB, NVB, KS>::kSmem, 0, stream, m.q, m.k_dq, m.v_dq, m.dout, p);
+}
+
+template <int NQB, bool BF16>
+int launch_nvb(int nvb, const BwdMaps& m, const BwdParams& p, int sms, cudaStream_t stream) {
+  return nvb == 1 ? launch_shape<NQB, 1, BF16>(m, p, sms, stream)
+         : nvb == 2 ? launch_shape<NQB, 2, BF16>(m, p, sms, stream)
+                    : launch_shape<NQB, 3, BF16>(m, p, sms, stream);
+}
+
+// (NQB, NVB) in {1, 2, 3}^2: the 64-channel boxes of head dims up to 192
+template <bool BF16>
+int launch_dispatch(const BwdMaps& m, const BwdParams& p, int sms, cudaStream_t stream) {
+  const int nqb = (p.dqk + 63) / 64, nvb = (p.dv + 63) / 64;
+  return nqb == 1 ? launch_nvb<1, BF16>(nvb, m, p, sms, stream)
+         : nqb == 2 ? launch_nvb<2, BF16>(nvb, m, p, sms, stream)
+                    : launch_nvb<3, BF16>(nvb, m, p, sms, stream);
+}
+
+// the dQ partials, summed in order -> dq (dtype: bf16, fp16 or fp32) with its own strides
 int launch_sum_dq(int dtype, const float* part, int nparts, void* dst, int Bq, int N, int H, int dqk, int64_t sb,
                   int64_t sn, int64_t sh, cudaStream_t stream) {
   const int64_t total = (int64_t)Bq * N * H * dqk;
@@ -983,37 +835,17 @@ int launch_attn_bwd(const pcv_attn_bwd_params& a, const pcv_key_shard* shard, cu
   p.dk_sb = a.gk_stride_b; p.dk_sm = a.gk_stride_m; p.dk_sh = a.gk_stride_h;
   p.dv_sb = a.gv_stride_b; p.dv_sm = a.gv_stride_m; p.dv_sh = a.gv_stride_h;
   p.total_tiles = a.B * a.H * L.nk;
-  {
-    const int64_t st[] = {a.gk_stride_b, a.gk_stride_m, a.gk_stride_h, a.gv_stride_b, a.gv_stride_m, a.gv_stride_h};
-    bool wide = ((reinterpret_cast<uintptr_t>(a.grad_k) | reinterpret_cast<uintptr_t>(a.grad_v)) & 31u) == 0;
-    for (int64_t x : st) wide = wide && (x % 16 == 0);
-    p.wide_store = wide ? 1 : 0;
-  }
 
-  rc = make_tmap_4d(&m.dout, a.grad_out, a.dtype, a.dv, a.N, a.H, a.B, a.go_stride_n, a.go_stride_h, a.go_stride_b, kT);
+  rc = a.dtype == PCV_BF16 ? launch_dispatch<true>(m, p, sms, stream) : launch_dispatch<false>(m, p, sms, stream);
   if (rc != PCV_OK) return rc;
-  rc = make_tmap_4d(&m.q64, a.q, a.dtype, a.dqk, a.N, a.H, Bq, a.q_stride_n, a.q_stride_h, a.q_stride_b, 64);
-  if (rc != PCV_OK) return rc;
-  rc = make_tmap_4d(&m.dout64, a.grad_out, a.dtype, a.dv, a.N, a.H, a.B, a.go_stride_n, a.go_stride_h, a.go_stride_b, 64);
-  if (rc != PCV_OK) return rc;
-
-  const bool bf16 = a.dtype == PCV_BF16;
-  if (wide) {
-    rc = make_tmap_4d(&m.k64, a.k, a.dtype, a.dqk, a.M, a.H, a.B, a.k_stride_m, a.k_stride_h, a.k_stride_b, 64);
-    if (rc != PCV_OK) return rc;
-    rc = make_tmap_4d(&m.v64, a.v, a.dtype, a.dv, a.M, a.H, a.B, a.v_stride_m, a.v_stride_h, a.v_stride_b, 64);
-    if (rc != PCV_OK) return rc;
-    rc = bf16 ? launch_wide<true>(m, p, sms, stream) : launch_wide<false>(m, p, sms, stream);
-    if (rc != PCV_OK) return rc;
-    if (shard != nullptr)  // the same fixed-order sum, kept in fp32: (Bq, N, H*dqk) dense
-      return launch_sum_dq(PCV_F32, p.dq32, L.dq_parts, shard->grad_q32, Bq, a.N, a.H, a.dqk,
-                           (int64_t)a.N * a.H * a.dqk, (int64_t)a.H * a.dqk, a.dqk, stream);
-    return launch_sum_dq(a.dtype, p.dq32, L.dq_parts, a.grad_q, Bq, a.N, a.H, a.dqk, a.gq_stride_b, a.gq_stride_n,
-                         a.gq_stride_h, stream);
-  }
-  rc = bf16 ? launch_tc<true>(m, p, sms, stream) : launch_tc<false>(m, p, sms, stream);
-  if (rc != PCV_OK || shard != nullptr) return rc;
-  return launch_cast(bf16, p.dq32, a.grad_q, Bq, a.N, a.H, a.dqk, a.gq_stride_b, a.gq_stride_n, a.gq_stride_h, stream);
+  // dQ in the caller's dtype and strides: the partials in order, or the one fp32 buffer of the atomics up to head dim
+  // 128; a key shard's grad_q32 already holds the latter and takes the former as it is, fp32 (Bq, N, H*dqk) dense
+  if (shard != nullptr)
+    return wide ? launch_sum_dq(PCV_F32, p.dq32, L.dq_parts, shard->grad_q32, Bq, a.N, a.H, a.dqk,
+                                (int64_t)a.N * a.H * a.dqk, (int64_t)a.H * a.dqk, a.dqk, stream)
+                : PCV_OK;
+  return launch_sum_dq(a.dtype, p.dq32, wide ? L.dq_parts : 1, a.grad_q, Bq, a.N, a.H, a.dqk, a.gq_stride_b,
+                       a.gq_stride_n, a.gq_stride_h, stream);
 }
 
 // ---- dropout mask export ---------------------------------------------------------------------------------------

@@ -69,8 +69,7 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
 //   11-12  kvproj_kernel      11 ring slot free, 12 stage loaded
 //   21-24  bwd_dkdv_kernel    21 K/V tile free, 22 Q/dO slot free, 23 K/V tile loaded, 24 Q/dO stage loaded
 //          (its dV and dK passes for head dims above 128 are the same body)
-//   31-33  bwd_dq_kernel      31 K/V slot free, 32 Q (and dO) loaded, 33 K/V stage loaded
-//   34-37  bwd_dq64_kernel    34 Q/dO free, 35 K/V slot free, 36 Q/dO loaded, 37 K/V stage loaded
+//   31-34  bwd_dq_kernel      31 K/V slot free, 32 Q/dO loaded, 33 K/V stage loaded, 34 Q/dO free
 //   41-43  peer_tail_kernel   41 partial states of all ranks, 42 grid arrival, 43 outputs of all ranks (flag waits)
 //   51-52  lnlin_dx_kernel    51 ring slot free, 52 stage loaded
 //   53-54  lnlin_dw_kernel    53 ring slot free, 54 stage loaded

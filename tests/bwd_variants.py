@@ -2,10 +2,11 @@
 shared by its GPU tests (test_gpu_bwd_variants.py) and their CPU companion (test_bwd_variants_cpu.py).  Nothing here
 needs a GPU.
 
-launch_attn_bwd instantiates, with NQB = pad64(dqk) / 64 and NVB = pad64(dv) / 64 boxes of 64 channels, bf16 or fp16:
-  - head dims up to 128 (launch_tc): bwd_dkdv_kernel<NQB, NVB, BF16, kOutBoth> and bwd_dq_kernel<NQB, NVB, BF16>;
-  - a head dim above 128 (launch_wide, NQB or NVB = 3): bwd_dkdv_kernel<.., kOutDV> (the dV pass),
-    bwd_dkdv_kernel<.., kOutDK> (the dK pass) and bwd_dq64_kernel<NQB, NVB, BF16>.
+launch_attn_bwd instantiates (launch_shape), with NQB = pad64(dqk) / 64 and NVB = pad64(dv) / 64 boxes of 64
+channels, bf16 or fp16:
+  - head dims up to 128: bwd_dkdv_kernel<NQB, NVB, BF16, kOutBoth> and bwd_dq_kernel<NQB, NVB, BF16, 128>;
+  - a head dim above 128 (NQB or NVB = 3): bwd_dkdv_kernel<.., kOutDV> (the dV pass), bwd_dkdv_kernel<.., kOutDK>
+    (the dK pass) and bwd_dq_kernel<NQB, NVB, BF16, 64>.
 Every kernel below keeps a TMA ring of NS stages whose phase runs on across the persistent kernels' tiles / work items;
 the schedule shapes make that carry-over, the ring's wrap and the dQ split edges actually happen."""
 import itertools
@@ -32,11 +33,11 @@ def is_wide(dqk, dv):
 # ---- the instantiations one call reaches ----
 def variants_of(dqk, dv, dt):
     """Kernel symbols (name, NQB, NVB, dtype, flag) a backward with these head dims launches.  flag: OUT of
-    bwd_dkdv_kernel (0 both, 1 dV, 2 dK), None for bwd_dq_kernel and bwd_dq64_kernel."""
+    bwd_dkdv_kernel (0 both, 1 dV, 2 dK), KS (the keys per ring stage) of bwd_dq_kernel."""
     nq, nv = boxes(dqk), boxes(dv)
     if is_wide(dqk, dv):
-        return {("dkdv", nq, nv, dt, 1), ("dkdv", nq, nv, dt, 2), ("dq64", nq, nv, dt, None)}
-    return {("dkdv", nq, nv, dt, 0), ("dq", nq, nv, dt, None)}
+        return {("dkdv", nq, nv, dt, 1), ("dkdv", nq, nv, dt, 2), ("dq", nq, nv, dt, 64)}
+    return {("dkdv", nq, nv, dt, 0), ("dq", nq, nv, dt, 128)}
 
 
 def reachable_variants():
@@ -54,14 +55,10 @@ def cfg1_slots(nqb, nvb):
     return min(8, (SMEM_LIMIT - (nqb + nvb) * BOX - BARRIERS) // ((nqb + nvb) * BOX64))
 
 
-def cfg2_slots(nqb, nvb):
-    """Cfg2<NQB, NVB>::kSlots (bwd_dq_kernel): Q and dO resident, (NQB + NVB) 128-row K / V boxes per stage, at most 4."""
-    return min(4, (SMEM_LIMIT - (nqb + nvb) * BOX - BARRIERS) // ((nqb + nvb) * BOX))
-
-
-def cfg3_slots(nqb, nvb):
-    """Cfg3<NQB, NVB>::kSlots (bwd_dq64_kernel): Q and dO resident, (NQB + NVB) 64-row K / V boxes per stage, at most 4."""
-    return min(4, (SMEM_LIMIT - (nqb + nvb) * BOX - BARRIERS) // ((nqb + nvb) * BOX64))
+def dq_slots(nqb, nvb, ks):
+    """Cfg2<NQB, NVB, KS>::kSlots (bwd_dq_kernel): Q and dO resident, (NQB + NVB) KS-row K / V boxes per stage, at
+    most 4."""
+    return min(4, (SMEM_LIMIT - (nqb + nvb) * BOX - BARRIERS) // ((nqb + nvb) * ks * 128))
 
 
 # ---- the plan ----
@@ -76,7 +73,7 @@ def dq_split(units, nk, sms):
 
 
 def plan(B, H, N, M, dqk, dv, sms):
-    """The launch geometry launch_attn_bwd derives (bwd_layout, bwd_setup, launch_tc_kernels / launch_wide_kernels)."""
+    """The launch geometry launch_attn_bwd derives (bwd_layout, bwd_setup, launch_shape)."""
     nq, nk = (N + TILE - 1) // TILE, (M + TILE - 1) // TILE              # bwd_layout
     nqb, nvb = boxes(dqk), boxes(dv)
     wide = is_wide(dqk, dv)
@@ -87,14 +84,12 @@ def plan(B, H, N, M, dqk, dv, sms):
     p = dict(nq=nq, nk=nk, nq64=(N + 63) // 64, wide=wide, tiles=tiles, dkdv_grid=min(tiles, sms),
              last_split_key0=(splits - 1) * tps * TILE,
              dkdv_ns=cfg1_slots(nqb, nvb), tps=tps, splits=splits)
-    if wide:  # bwd_dq64_kernel: persistent over (b, h, query tile, split) items, 64-key stages
-        items = B * H * nq * splits
-        nk64 = (M + 63) // 64
-        p.update(dq_ns=cfg3_slots(nqb, nvb), dq_items=items, dq_grid=min(items, sms),
-                 dq_stages=[min(nk64, 2 * s * tps + 2 * tps) - 2 * s * tps for s in range(splits)])
-    else:    # bwd_dq_kernel: one CTA per (b, h, query tile, split), 128-key stages
-        p.update(dq_ns=cfg2_slots(nqb, nvb), dq_items=B * H * nq * splits, dq_grid=B * H * nq * splits,
-                 dq_stages=[min(nk, s * tps + tps) - s * tps for s in range(splits)])
+    # bwd_dq_kernel: work items (b, h, query tile, split); 64-key stages walked persistently by at most one CTA per SM
+    # (wide), else 128-key stages on one CTA per item.  A split is tps tiles of 128 keys: tps * 128 / KS stages.
+    ks = 64 if wide else TILE
+    items, nks, per_split = B * H * nq * splits, (M + ks - 1) // ks, tps * (TILE // ks)
+    p.update(dq_ks=ks, dq_ns=dq_slots(nqb, nvb, ks), dq_items=items, dq_grid=min(items, sms) if wide else items,
+             dq_stages=[min(nks, s * per_split + per_split) - s * per_split for s in range(splits)])
     return p
 
 

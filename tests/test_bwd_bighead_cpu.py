@@ -2,11 +2,14 @@
 argument checks of pcv_attn_bwd_supported (before any CUDA call), and the zero-padding of head dims that are not
 multiples of 8 around the backward kernels, with an fp64 CPU stand-in for the kernels."""
 import ctypes
+import os
 import re
+import subprocess
 
 import pytest
 import torch
 
+from conftest import ROOT
 from perceiver_io_b200 import _lib, ops
 
 
@@ -15,10 +18,10 @@ def _lib_blob():
         return f.read()
 
 
-def test_library_holds_exactly_the_backward_instantiations():
+def test_library_holds_exactly_the_backward_instantiations_with_one_dq_template():
     """bwd_dkdv_kernel<NQB, NVB, BF16, OUT>: the single-pass kernels (OUT 0) for NQB, NVB <= 2; for the five box pairs
-    with a third box, a dV pass (OUT 1) and a dK pass (OUT 2).  bwd_dq_kernel<NQB, NVB, BF16> stays at <= 2 boxes;
-    bwd_dq64_kernel<NQB, NVB, BF16> covers the five wide pairs."""
+    with a third box, a dV pass (OUT 1) and a dK pass (OUT 2).  bwd_dq_kernel<NQB, NVB, BF16, KS>: 128-key stages at
+    <= 2 boxes, 64-key stages for the five wide pairs; no other dQ or dQ-cast kernel."""
     blob = _lib_blob()
     small = {(q, v) for q in (1, 2) for v in (1, 2)}
     wide = {(q, v) for q in (1, 2, 3) for v in (1, 2, 3)} - small
@@ -27,10 +30,41 @@ def test_library_holds_exactly_the_backward_instantiations():
             for a, b, c, o in re.findall(rb"15bwd_dkdv_kernelILi(\d)ELi(\d)ELb([01])ELi(\d)EEEv", blob)}
     assert dkdv == ({(q, v, bf, 0) for q, v in small for bf in (False, True)}
                     | {(q, v, bf, o) for q, v in wide for bf in (False, True) for o in (1, 2)})
-    dq = {(int(a), int(b), c == b"1") for a, b, c in re.findall(rb"13bwd_dq_kernelILi(\d)ELi(\d)ELb([01])EEEv", blob)}
-    assert dq == {(q, v, bf) for q, v in small for bf in (False, True)}
-    dq64 = {(int(a), int(b), c == b"1") for a, b, c in re.findall(rb"15bwd_dq64_kernelILi(\d)ELi(\d)ELb([01])EEEv", blob)}
-    assert dq64 == {(q, v, bf) for q, v in wide for bf in (False, True)}
+    dq = {(int(a), int(b), c == b"1", int(k))
+          for a, b, c, k in re.findall(rb"13bwd_dq_kernelILi(\d)ELi(\d)ELb([01])ELi(\d+)EEEv", blob)}
+    assert dq == ({(q, v, bf, 128) for q, v in small for bf in (False, True)}
+                  | {(q, v, bf, 64) for q, v in wide for bf in (False, True)})
+    assert b"bwd_dq64_kernel" not in blob and b"bwd_cast_dq_kernel" not in blob
+
+
+# ptxas at the commit that folded the two dQ kernels into one (CUDA 12.9, the Makefile's flags): (stack, spill stores,
+# spill loads) bytes of the kernels that spill; every other backward kernel is spill-free.  All use 168 registers
+# (384-thread CTAs, one per SM).
+BWD_SPILLS = {f"bwd_{k}<2, 2, {bf}, {x}>": v for bf in ("false", "true")
+              for k, x, v in (("dkdv_kernel", 0, (40, 52, 56)), ("dq_kernel", 128, (24, 28, 52)))}
+
+
+def test_backward_kernels_hold_their_registers_and_spills():
+    log = os.path.join(ROOT, "build", "pcv_attn_bwd.ptxas.log")
+    if not os.path.exists(log):
+        pytest.skip("the library was not built in this tree")
+    text = open(log).read()
+    seen = set()
+    for e in text.split("Compiling entry function")[1:]:
+        mangled = e.split("'")[1]
+        if not re.search(r"bwd_(dkdv|dq)_kernel", mangled):
+            continue
+        name = subprocess.run(["c++filt", mangled], capture_output=True, text=True).stdout
+        name = re.sub(r"^void (pcv::\(anonymous namespace\)::)?", "", name.split("(CUtensorMap")[0].strip())
+        seen.add(name)
+        own = next(line for line in e.split("\n") if "spill" in line)   # the kernel's own line, not a callee's
+        stack, stores, loads = map(int, re.search(r"(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill "
+                                                   r"loads", own).groups())
+        limit = BWD_SPILLS.get(name, (0, 0, 0))
+        assert stack <= limit[0] and stores <= limit[1] and loads <= limit[2], (name, own)
+        assert int(e.split("Used ")[1].split(" registers")[0]) == 168, (name, e[:300])
+    assert len(seen) == 2 * (4 + 5 * 2) + 2 * 9, sorted(seen)   # dK/dV kernels, then the dQ kernels
+    assert set(BWD_SPILLS) <= seen
 
 
 def _bwd_params(dqk, dv, **kw):

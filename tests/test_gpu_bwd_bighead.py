@@ -1,5 +1,5 @@
 """-m gpu: the attention backward for head dims above 128 (up to 192): the dK/dV kernel's dV and dK passes and
-bwd_dq64_kernel (64-key stages, ordered dQ partials), against float64 autograd of the reference algorithm with the
+bwd_dq_kernel on 64-key stages (ordered dQ partials), against float64 autograd of the reference algorithm with the
 gates of test_gpu_bwd.py (gpu_util.assert_grads)."""
 import pytest
 import torch

@@ -1,5 +1,5 @@
-"""-m gpu: every instantiation of the attention backward (bwd_dkdv_kernel, bwd_dq_kernel, bwd_dq64_kernel) at its
-schedule, tile and mask edges, against fp64 autograd of the reference algorithm, and the dropout forward at the same
+"""-m gpu: every instantiation of the attention backward (bwd_dkdv_kernel, bwd_dq_kernel on 128- and 64-key stages) at
+its schedule, tile and mask edges, against fp64 autograd of the reference algorithm, and the dropout forward at the same
 head dims up to 128.
 The matrix and the schedule shapes live in bwd_variants.py; test_bwd_variants_cpu.py checks that the matrix covers every
 instantiation, that the shapes have their plan structure, and that the gate is calibrated and sees the bugs it is for.

@@ -17,9 +17,11 @@ import sys
 
 import torch
 
-SHAPES = [(64, 64), (128, 128), (131, 131), (32, 160)]
+# head dims reaching every backward box pair (NQB, NVB) in {1, 2, 3}^2
+SHAPES = [(64, 64), (128, 128), (131, 131), (32, 160), (64, 128), (128, 64), (160, 64), (184, 120), (120, 184)]
 # (operand dtype, batch-1 q, pad mask, causal)
-VARIANTS = [(torch.bfloat16, True, True, False), (torch.float32, False, False, True), (torch.bfloat16, False, True, True)]
+VARIANTS = [(torch.bfloat16, True, True, False), (torch.float32, False, False, True), (torch.bfloat16, False, True, True),
+            (torch.float16, True, False, True)]
 B, N, M, H, SEED = 2, 200, 700, 2, 0x5EED
 
 
@@ -60,7 +62,7 @@ def run(root: str, out_path: str) -> None:
         for dtype, bq1, with_pad, causal in VARIANTS:
             q, k, v, go, pad = _inputs(dqk, dv, dtype, bq1, with_pad, g)
             scale = dqk ** -0.5
-            atomic_dq = dqk <= 128  # grad_q is accumulated with fp32 atomics up to head dim 128 (padded)
+            atomic_dq = max(dqk, dv) <= 128  # grad_q is accumulated with fp32 atomics up to head dim 128 (padded)
             tag = f"{dqk}/{dv} {str(dtype)[6:]} bq1={bq1} pad={with_pad} causal={causal}"
             kw = dict(pad_mask=pad, causal=causal)
             record(f"{tag} attention", lambda: ops.attention(q, k, v, H, scale, **kw))
