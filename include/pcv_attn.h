@@ -861,6 +861,62 @@ PCV_API int pcv_logits_process_supported(const pcv_logits_process_params* p);
 PCV_API int pcv_logits_process(const pcv_logits_process_params* p, void* stream);
 
 /*
+ * Prompt-lookup drafts: pcv_prompt_lookup finds each batch row's drafts in its own history, with the rule of the
+ * Hugging Face PromptLookupCandidateGenerator.get_candidates (no logits processor) applied to each row alone.  One CTA
+ * per row.  Row b's history is h = ids[b, s .. L), s = start[b] (its left-padding count; NULL: 0) clamped to [0, L],
+ * L = length[b * length_stride] + length_offset (+ n_b in round mode) clamped to [0, cap]; len = L - s:
+ *   1. for n = min(N, len - 1) down to 1: the first window h[e-n+1 .. e] (smallest e) equal to h[len-n .. len) with
+ *      e <= len - 2 (it has a continuation);
+ *   2. the draft is h[e+1 .. min(e+1+G, len)) of the largest n that has such a window, cut before its first EOS id
+ *      (empty after the cut: no draft, and no other window is tried), then capped at the row's limit;
+ *   3. counts[b] = its length, drafts[b, :counts[b]] = the draft, drafts[b, counts[b] .. G) = h[len-1] (filler; 0 for
+ *      an empty history).
+ * The limit is limit[b] (NULL: G) in search mode (k = 0).  Round mode (1 <= k <= G+1) first settles the round that fed
+ * fed[b, 0 .. k) (t_0 and counts[b] drafts, then filler) and drew draws[b, i] after fed[b, i]: a row is live while
+ * unfinished[b] != 0 and left[b] > 0.  A live row accepts n_b = the leading i < counts[b] with fed[b, i+1] ==
+ * draws[b, i], emits those drafts and t = draws[b, n_b], sets left[b] -= n_b + 1, unfinished[b] = 0 if t is an EOS id,
+ * writes t into ids at row L - 1 (the row it will be fed at) and searches with the limit left[b] - 1 if it is still
+ * live.  A row that is not live keeps t = fed[b, 0], n_b = 0 and gets no draft (its history ends at t: L is one
+ * less).  accepted[b] = n_b, t0[b] = t.
+ * Integer comparisons only, a block-min over window ends and no atomics on results: a row's output is a pure
+ * function of its ids, lengths, G, N, the EOS ids and its limit / state, independent of B, the launch and graph
+ * capture.  Refusals (NULL pointers, B < 1, cap < 1, ids_stride < cap, G outside [1, PCV_LOOKUP_MAX_DRAFTS], N outside
+ * [1, PCV_LOOKUP_MAX_NGRAM], n_eos outside [0, PCV_LOOKUP_MAX_EOS], drafts_stride < G, k outside [0, G+1], a round
+ * without its state, t0_stride < 1) come before any CUDA call, with the reason in pcv_last_error.
+ */
+#define PCV_LOOKUP_MAX_DRAFTS 63
+#define PCV_LOOKUP_MAX_NGRAM 16
+#define PCV_LOOKUP_MAX_EOS 4
+
+typedef struct pcv_prompt_lookup_params {
+  int64_t* ids;                /* device (B, cap) history rows (round mode writes t into them)                    */
+  int64_t ids_stride;          /* elements between rows, >= cap                                                  */
+  const int32_t* start;        /* device (B) left-padding counts, or NULL (0)                                    */
+  const int32_t* length;       /* device: L = length[b * length_stride] + length_offset                         */
+  int32_t length_stride, length_offset;
+  const int32_t* limit;        /* device (B) per-row draft caps, or NULL (G); search mode only                   */
+  int32_t B, cap, G, N;
+  int32_t n_eos;
+  int32_t k;                   /* 0: search only; 1 .. G+1: settle the round that fed k tokens, then search      */
+  int64_t eos[PCV_LOOKUP_MAX_EOS];
+  int64_t* drafts;             /* device (B, drafts_stride) out                                                   */
+  int64_t drafts_stride;
+  int32_t* counts;             /* device (B) out (round mode: in first, the drafts the round fed)                 */
+  int32_t reserved;
+  const int64_t* fed;          /* round mode: device (B, k) contiguous, t_0 then the drafts and filler            */
+  const int64_t* draws;        /* round mode: device (B, k) contiguous, the draw after each fed token             */
+  int64_t* t0;                 /* round mode: device (B, t0_stride) out, the next t_0                              */
+  int64_t t0_stride;
+  int32_t* accepted;           /* round mode: device (B) out, n_b                                                  */
+  int32_t* unfinished;         /* round mode: device (B) state                                                     */
+  int32_t* left;               /* round mode: device (B) state, the tokens each row still emits                    */
+} pcv_prompt_lookup_params;
+
+/* 1 if pcv_prompt_lookup takes these params, else 0 (reason via pcv_last_error) */
+PCV_API int pcv_prompt_lookup_supported(const pcv_prompt_lookup_params* p);
+PCV_API int pcv_prompt_lookup(const pcv_prompt_lookup_params* p, void* stream);
+
+/*
  * pcv_kv_gather_rows: after a beam step, every beam row i with parents[i] != i takes its parent's generated rows.  For
  * every arena of the device table and every such row i, rows [first_row, cur) with cur = rows->bounds[i *
  * bounds_stride_b + bounds_col] (clamped to first_row + max_rows) are copied from row parents[i] into row i, through

@@ -91,6 +91,8 @@ EXPORTS = (
     "pcv_beam_step_logprobs",
     "pcv_logits_process_supported",
     "pcv_logits_process",
+    "pcv_prompt_lookup_supported",
+    "pcv_prompt_lookup",
     "pcv_kv_gather_rows_supported",
     "pcv_kv_gather_rows",
     "pcv_contrastive_candidates_supported",
@@ -352,6 +354,23 @@ class LogitsProcessParams(C.Structure):
     ]
 
 
+LOOKUP_MAX_DRAFTS = 63   # PCV_LOOKUP_MAX_DRAFTS
+LOOKUP_MAX_NGRAM = 16    # PCV_LOOKUP_MAX_NGRAM
+LOOKUP_MAX_EOS = 4       # PCV_LOOKUP_MAX_EOS
+
+
+class PromptLookupParams(C.Structure):
+    _fields_ = [
+        ("ids", C.c_void_p), ("ids_stride", C.c_int64), ("start", C.c_void_p), ("length", C.c_void_p),
+        ("length_stride", C.c_int32), ("length_offset", C.c_int32), ("limit", C.c_void_p),
+        ("B", C.c_int32), ("cap", C.c_int32), ("G", C.c_int32), ("N", C.c_int32), ("n_eos", C.c_int32),
+        ("k", C.c_int32), ("eos", C.c_int64 * LOOKUP_MAX_EOS),
+        ("drafts", C.c_void_p), ("drafts_stride", C.c_int64), ("counts", C.c_void_p), ("reserved", C.c_int32),
+        ("fed", C.c_void_p), ("draws", C.c_void_p), ("t0", C.c_void_p), ("t0_stride", C.c_int64),
+        ("accepted", C.c_void_p), ("unfinished", C.c_void_p), ("left", C.c_void_p),
+    ]
+
+
 class KvGatherEntry(C.Structure):
     _fields_ = [
         ("arena", C.c_void_p), ("scratch", C.c_void_p),
@@ -563,6 +582,10 @@ def lib() -> C.CDLL:
                      "pcv_beam_step_logprobs_supported", "pcv_beam_step_logprobs", "pcv_logits_process_supported",
                      "pcv_logits_process"):
             getattr(l, name).restype = C.c_int
+        l.pcv_prompt_lookup_supported.argtypes = [C.POINTER(PromptLookupParams)]
+        l.pcv_prompt_lookup_supported.restype = C.c_int
+        l.pcv_prompt_lookup.argtypes = [C.POINTER(PromptLookupParams), C.c_void_p]
+        l.pcv_prompt_lookup.restype = C.c_int
         l.pcv_contrastive_candidates_supported.argtypes = [C.POINTER(ContrastiveCandidatesParams)]
         l.pcv_contrastive_candidates.argtypes = [C.POINTER(ContrastiveCandidatesParams), C.c_void_p]
         l.pcv_contrastive_rank_supported.argtypes = [C.POINTER(ContrastiveRankParams)]

@@ -411,6 +411,16 @@ int pcv_logits_process(const pcv_logits_process_params* p, void* stream) {
   return launch_logits_process(*p, reinterpret_cast<cudaStream_t>(stream));
 }
 
+int pcv_prompt_lookup_supported(const pcv_prompt_lookup_params* p) {
+  return prompt_lookup_check(p) == PCV_OK ? 1 : 0;
+}
+
+int pcv_prompt_lookup(const pcv_prompt_lookup_params* p, void* stream) {
+  const int rc = prompt_lookup_check(p);
+  if (rc != PCV_OK) return rc;
+  return launch_prompt_lookup(*p, reinterpret_cast<cudaStream_t>(stream));
+}
+
 int pcv_kv_gather_rows_supported(const pcv_kv_gather_params* p, const pcv_dev_rows* rows) {
   return kv_gather_check(p, rows) == PCV_OK ? 1 : 0;
 }

@@ -189,5 +189,8 @@ int launch_contrastive_rank(const pcv_contrastive_rank_params& p, cudaStream_t s
 // logits processors (pcv_process.cu)
 int logits_process_check(const pcv_logits_process_params* p);
 int launch_logits_process(const pcv_logits_process_params& p, cudaStream_t stream);
+// prompt-lookup drafts (pcv_lookup.cu)
+int prompt_lookup_check(const pcv_prompt_lookup_params* p);
+int launch_prompt_lookup(const pcv_prompt_lookup_params& p, cudaStream_t stream);
 
 }  // namespace pcv

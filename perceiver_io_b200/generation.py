@@ -22,6 +22,7 @@ run, and in-graph int32 ops advance them at the end of each step.
     tokens, q = dec.generate(first, n, logits=True)                           # and the (B, n, vocab) logits drawn from
     out, accepted = dec.verify(token_ids, draft_logits, draft_sampling)       # (B, G+1) -> one speculative round
     tokens, stats = speculative_generate(target, draft, first, n, draft_tokens=G)
+    tokens, stats = dec.prompt_lookup_generate(first, n, num_output_tokens=G)   # n-gram drafts from the row's history
     out = dec.beam_search(input_ids, prefix_len, n, num_beams=K)              # batch = B*K: (B, R, n), (B, R)
     tokens = dec.contrastive_search(input_ids, prefix_len, n, penalty_alpha=0.6, top_k=K)   # batch = B*K: (B, n)
 
@@ -270,6 +271,8 @@ class GraphedDecoder:
     _process = _NO_PROCESS            # the sampling graphs' (repetition_penalty, no_repeat_ngram_size, min_new_tokens)
     _eos = ()                         # the sampling EOS ids, and the token fed after one
     _pad_token = None
+    _lookup_state = ()                # prompt lookup: (next t_0 and drafts (B, 64), state (4, B), start (B,)) buffers
+    _lookup_args = (0, 0)             # the (G, N) of the lookup graph being recorded or replayed
 
     def __init__(self, model, batch: int, max_new_tokens: int, kv_cache: str = "bf16"):
         if max_new_tokens < 1:
@@ -485,6 +488,19 @@ class GraphedDecoder:
         self._verify_logits = logits   # the static target logits of the verify graph recorded last (for tests)
         return ops.spec_verify(logits, draft_logits, token, self._seeds, pos, self._sampling, self._draft_sampling)
 
+    def _lookup_fn(self, token: torch.Tensor) -> torch.Tensor:
+        """_sample_fn followed by the round mode of ``ops.prompt_lookup``: settle the round, write the next t_0 and
+        search the next drafts (into ``_lookup_state``).  Returns the draws (B, k)."""
+        k = token.shape[1]
+        tokens, _ = self._sample_fn(token)
+        tokens = tokens.contiguous()
+        nxt, state, start = self._lookup_state
+        G, N = self._lookup_args
+        # after _step_fn, bounds[:, 0, 2] is t_0's row + k; t_0's successor goes to row + n_b + 1 = L_b - 1
+        ops.prompt_lookup_round(self._tokens, self._bounds[:, 0, 2], 2 - k, token, tokens, nxt, state, G, N,
+                                start=start, eos=self._eos)
+        return tokens
+
     def _replay(self, token_ids: torch.Tensor, fn: str, *extra: torch.Tensor) -> torch.Tensor:
         """One replay of the graph of ``token_ids.shape[1]`` tokens per step, recorded on first use (``fn`` "sample":
         the graph that also samples, one per sampling triple; "verify": the graph that also verifies drafts, one per
@@ -512,10 +528,13 @@ class GraphedDecoder:
             key, fwd = ("generate", self._sampling, self._process, self._eos, self._pad_token), self._generate_fn
         if fn == "verify":
             key, fwd = ("verify", k, self._sampling, self._draft_sampling), self._verify_fn
+        if fn == "lookup":
+            key, fwd = ("lookup", k, self._sampling, self._process, self._eos, self._lookup_args), self._lookup_fn
         graph = self._graphs.get(key)
         if graph is None:
             snapshot = self._bounds.clone()   # the warm-up calls advance the rows; their arena writes are rewritten later
             unfinished = self._unfinished.clone()   # and may finish rows of the generate graph
+            lookup = [t.clone() for t in self._lookup_state] if fn == "lookup" else []   # and settle lookup rounds
             old = torch.cuda.get_sync_debug_mode()
             torch.cuda.set_sync_debug_mode(0)  # recording a graph synchronises the device once
             try:
@@ -524,6 +543,8 @@ class GraphedDecoder:
                 torch.cuda.set_sync_debug_mode(old)
             self._bounds.copy_(snapshot)
             self._unfinished.copy_(unfinished)
+            for t, saved in zip(self._lookup_state, lookup):
+                t.copy_(saved)
             self._graphs[key] = graph
             self.captures += 1
         out = graph(token_ids, *extra)
@@ -704,6 +725,94 @@ class GraphedDecoder:
                              f"got {tuple(draft_logits.shape)} {draft_logits.dtype}")
         self._draft_sampling = draft
         return self._replay(token_ids, "verify", draft_logits)
+
+    # ---- prompt lookup ----------------------------------------------------------------------------------------------
+    def prompt_lookup_generate(self, first: torch.Tensor, n: int, num_output_tokens: int = 10,
+                               max_matching_ngram_size: int = 2):
+        """Prompt-lookup decoding (🤗 ``generate(prompt_lookup_num_tokens=G, max_matching_ngram_size=N)``): n tokens
+        per batch row, each the model's own draw at its position under the ``set_sampling`` values, with drafts
+        copied from the row's own history.  Returns ``(tokens, stats)``: (B, n) int64, and a dict with ``rounds``,
+        ``k`` (the tokens each round fed) and per batch row ``proposed`` (drafts offered while the row was live) and
+        ``accepted`` (of those, accepted).
+
+        ``first`` (B, 1) int64 is the token after the prompt (``draw``).  A row's history is what ``prefill`` was given
+        after its left padding, then every token it was fed, then t_0 (its newest token, fed by the next round).  Its
+        drafts are ``ops.prompt_lookup``'s: the up to G = ``num_output_tokens`` ids after the first earlier occurrence
+        of its last n ids (n = N = ``max_matching_ngram_size`` down to 1), cut before an EOS id and capped so that the
+        row never drafts past its n tokens; the processors play no part in them (🤗 crops candidates on fake logits).
+        A round is one replay of k = max(draft count) + 1 tokens per row, t_0 then the drafts (filler after a row's
+        own, never accepted): the sampler draws after each, the device accepts the leading drafts equal to the draws
+        (``drafts[:, i+1] == tokens[:, i]``, so every emitted token is the draw at its position), takes the draw after
+        the last accepted draft as the next t_0, finishes a row that emitted an EOS id, and searches the next drafts
+        (``ops.prompt_lookup_round``), all in the graph.  Then one device-to-host read of the accept counts, the next
+        draft counts and the finished flags; row b is rewound by k - 1 - n_b, or by k once it is finished or has n
+        tokens (it stops advancing).  Before the first round the drafts of ``first`` are searched eagerly and their
+        counts read once.  The graph is recorded on first use, one per (k, sampling values, processors, EOS ids, G, N).
+
+        With ``set_sampling`` EOS ids, 🤗 ``_sample``'s rule: a row that has emitted an EOS id (``first`` included)
+        emits the pad token from then on; the loop stops once every row is finished or has n tokens.  Needs
+        :func:`prompt_lookup_budget` (n, G, B) tokens of budget left, refused before any replay."""
+        what = "GraphedDecoder.prompt_lookup_generate"
+        G, N, count = _as_count(num_output_tokens), _as_count(max_matching_ngram_size), _as_count(n)
+        if G is None or not 1 <= G <= ops.LOOKUP_MAX_DRAFTS:
+            raise ValueError(f"{what}: num_output_tokens must be an integer in [1, {ops.LOOKUP_MAX_DRAFTS}], got "
+                             f"{num_output_tokens!r}")
+        if N is None or not 1 <= N <= ops.LOOKUP_MAX_NGRAM:
+            raise ValueError(f"{what}: max_matching_ngram_size must be an integer in [1, {ops.LOOKUP_MAX_NGRAM}], got "
+                             f"{max_matching_ngram_size!r}")
+        if count is None or count < 1:
+            raise ValueError(f"{what}: n must be an integer >= 1, got {n!r}")
+        self._ready_to_sample("prompt_lookup_generate")
+        B, dev = self.batch, self.device
+        if tuple(first.shape) != (B, 1) or first.dtype != torch.long:
+            raise ValueError(f"{what} takes ({B}, 1) int64 first tokens, got {tuple(first.shape)} {first.dtype}")
+        need = prompt_lookup_budget(count, G, B)
+        if self._remaining < need:
+            raise RuntimeError(f"{what}: {self._remaining} tokens of budget left, n={count} with up to {G} drafts per "
+                               f"round needs {need} (prompt_lookup_budget)")
+        if torch.is_autocast_enabled():
+            raise RuntimeError("GraphedDecoder does not run under autocast")
+        if not self._lookup_state:   # one set per decoder: the recorded graphs keep their addresses
+            self._lookup_state = (torch.zeros(B, ops.LOOKUP_MAX_DRAFTS + 1, dtype=torch.long, device=dev),
+                                  torch.zeros(4, B, dtype=torch.int32, device=dev),
+                                  torch.zeros(B, dtype=torch.int32, device=dev))
+        nxt, state, start = self._lookup_state
+        self._lookup_args = (G, N)
+        # the first round's drafts: first at the row it will be fed at, searched eagerly
+        rows = self._bounds[:, 0, 2]
+        self._tokens.scatter_(1, rows[:, None].long(), first)
+        start.copy_(self._pad[:, :self._n0].sum(dim=1))
+        if self._eos:
+            state[2].copy_(~self._is_eos(first[:, 0]))
+        else:
+            state[2].fill_(1)
+        state[3].fill_(count)
+        state[0].copy_(state[2] * min(count - 1, G))   # the first search's per-row limit
+        drafts, counts = ops.prompt_lookup(self._tokens, rows, G, N, start=start, limit=state[0], eos=self._eos,
+                                           length_offset=1)
+        nxt[:, :1].copy_(first)
+        nxt[:, 1:G + 1].copy_(drafts)
+        state[1].copy_(counts)
+        cnt, unf = state[1:3].to("cpu").tolist()   # the drafts of the first round
+        width = count + G + 2                      # column width - 1 takes the tokens a round does not keep
+        fill = self._pad_token if self._eos else 0
+        buf = torch.full((B, width), fill, dtype=torch.long, device=dev)
+        done, proposed, accepted = [0] * B, [0] * B, [0] * B
+        ks = []
+        while True:
+            live = [bool(u) and d < count for u, d in zip(unf, done)]
+            if not any(live):
+                break
+            k = max(c for c, l in zip(cnt, live) if l) + 1
+            tokens = self._replay(nxt[:, :k], "lookup")
+            acc, nxt_cnt, unf = state[:3].to("cpu").tolist()   # the round's one synchronisation
+            ks.append(k)
+            idx, back = _settle_round(acc, live, [c if l else 0 for c, l in zip(cnt, live)], done, proposed, accepted,
+                                      k, width, dev)
+            buf.scatter_(1, idx[:, :k], tokens)
+            self.rewind(back)
+            cnt = nxt_cnt
+        return buf[:, :count], {"rounds": len(ks), "k": ks, "proposed": proposed, "accepted": accepted}
 
     # ---- beam search ----------------------------------------------------------------------------------------------
     def _beam_args(self, B: int, n, num_beams, eos_token_id, length_penalty, early_stopping, num_return_sequences,
@@ -1059,6 +1168,47 @@ class GraphedDecoder:
             self._set_fed([self._fed - self._lag[i] for i in beam_idx.tolist()])
 
 
+def _settle_round(acc: List[int], live: List[bool], offered: List[int], done: List[int], proposed: List[int],
+                  accepted: List[int], k: int, width: int, device):
+    """Host bookkeeping of one verified round that fed k tokens (t_0 and up to k - 1 drafts) to every batch row, from
+    the n_b read back: live row b emitted its n_b accepted drafts and one more token, which go to columns done[b] ..
+    done[b] + n_b of the output (``done``, ``proposed`` and ``accepted`` are updated in place; ``offered[b]`` drafts
+    were proposed); a row that is not live emits nothing.  Returns ``(idx, back)``: (B, k+1) int64 on ``device``,
+    whose first k columns place the round's k emitted-token columns in a (B, ``width``) output (column width - 1
+    takes what is not kept) and whose last column is the column of ``[t_0 | tokens]`` that holds the row's next t_0;
+    and the per-row rewind counts, k - 1 - n_b for a live row and k for the others (they stop advancing)."""
+    B = len(acc)
+    idx = torch.full((B, k + 1), width - 1, dtype=torch.long)
+    back = []
+    for b in range(B):
+        if not live[b]:
+            idx[b, k] = 0
+            back.append(k)
+            continue
+        nb = acc[b]
+        idx[b, :nb + 1] = done[b] + torch.arange(nb + 1)
+        idx[b, k] = nb + 1
+        back.append(k - 1 - nb)
+        done[b] += nb + 1
+        proposed[b] += offered[b]
+        accepted[b] += nb
+    if device.type == "cuda":                  # pinned and asynchronous: no synchronisation
+        idx = idx.pin_memory().to(device, non_blocking=True)
+    return idx, back
+
+
+def prompt_lookup_budget(n: int, num_output_tokens: int, batch: int) -> int:
+    """The ``max_new_tokens`` (budget left after ``prefill``) :meth:`GraphedDecoder.prompt_lookup_generate` needs for n
+    tokens with G = ``num_output_tokens``: n for one batch row, n + min(G, n - 1) + 1 for more.
+
+    A live row that has emitted e < n tokens has fed e of them (its newest, t_0, is fed by the next round) and drafts
+    at most min(G, n - e - 1), so a round feeds k <= min(G, n - 1) + 1 tokens.  Alone, the row is fed k <= n - e:
+    e + k <= n.  With more rows, k follows the row with the most drafts: a live row reaches at most e + k <= n - 1 +
+    min(G, n - 1) + 1, and a row that is done has fed at most n and is still fed, then rewound, k tokens per round
+    while another row is live: n + min(G, n - 1) + 1."""
+    return n if batch == 1 else n + min(num_output_tokens, n - 1) + 1
+
+
 def speculative_budget(n: int, draft_tokens: int, batch: int) -> int:
     """The ``max_new_tokens`` (budget left after ``prefill``) both decoders of :func:`speculative_generate` need for n
     tokens with G = ``draft_tokens`` drafts per round: n + G for one batch row, n + 2G + 1 for more.
@@ -1116,30 +1266,14 @@ def speculative_generate(target: "GraphedDecoder", draft: "GraphedDecoder", firs
     buf = torch.empty(B, width, dtype=torch.long, device=dev)
     done, proposed, accepted_total = [0] * B, [0] * B, [0] * B
     t0, rounds = first, 0
-    cols = torch.arange(G + 1)
     while min(done) < count:
         drafts, q_logits = draft.generate(t0, G + 1, logits=True)
         fed = torch.cat([t0, drafts[:, :G]], dim=1)
         tokens, accepted = target.verify(fed, q_logits[:, :G], draft_sampling=draft._sampling)
         acc = accepted.to("cpu").tolist()       # the round's one synchronisation
         rounds += 1
-        # host-built indices: where each row's kept tokens go in buf, and which column of [t0 | tokens] is the next t0
-        idx = torch.full((B, G + 2), width - 1, dtype=torch.long)
-        back = []
-        for b in range(B):
-            if done[b] >= count:
-                idx[b, G + 1] = 0
-                back.append(G + 1)
-                continue
-            nb = acc[b]
-            idx[b, :nb + 1] = done[b] + cols[:nb + 1]
-            idx[b, G + 1] = nb + 1
-            back.append(G - nb)
-            done[b] += nb + 1
-            proposed[b] += G
-            accepted_total[b] += nb
-        if dev.type == "cuda":                  # pinned and asynchronous: no synchronisation
-            idx = idx.pin_memory().to(dev, non_blocking=True)
+        idx, back = _settle_round(acc, [d < count for d in done], [G] * B, done, proposed, accepted_total, G + 1,
+                                  width, dev)
         buf.scatter_(1, idx[:, :G + 1], tokens)
         t0 = torch.cat([t0, tokens], dim=1).gather(1, idx[:, G + 1:])
         target.rewind(back)

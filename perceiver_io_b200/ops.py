@@ -2373,3 +2373,115 @@ def _process_params(logits, prefix, prefix_len, *, tail=None, tail_len=None, row
     if not lib.pcv_logits_process_supported(C.byref(p)):
         raise ValueError(f"process_logits: {lib.pcv_last_error().decode()}")
     return p, out
+
+
+# --------------------------------------------------------------------------------------------------
+# prompt-lookup drafts (pcv_prompt_lookup): each batch row's n-gram drafts from its own history, found on the device;
+# the round mode settles a verified round first.  Recordable in a CUDA graph.
+# --------------------------------------------------------------------------------------------------
+#: The largest num_output_tokens (G), max_matching_ngram_size (N) and EOS count :func:`prompt_lookup` takes.
+LOOKUP_MAX_DRAFTS = _lib.LOOKUP_MAX_DRAFTS
+LOOKUP_MAX_NGRAM = _lib.LOOKUP_MAX_NGRAM
+LOOKUP_MAX_EOS = _lib.LOOKUP_MAX_EOS
+
+
+def _row_ints(what: str, t, B: int, device, dtype=torch.int32):
+    """The pointer and element stride of a (B,) tensor of ``dtype`` on ``device`` (any element stride)."""
+    _require_cuda(t)
+    if t.device != device or t.dtype != dtype or t.dim() != 1 or t.shape[0] != B:
+        raise ValueError(f"prompt_lookup: {what} must be a ({B},) {dtype} tensor on {device}, got {tuple(t.shape)} "
+                         f"{t.dtype} on {t.device}")
+    return t.data_ptr(), t.stride(0)
+
+
+def _lookup_params(ids, lengths, G, N, start, limit, eos, length_offset):
+    """The checked ``pcv_prompt_lookup_params`` of a search; no launch."""
+    _require_cuda(ids)
+    if ids.dtype != torch.int64 or ids.dim() != 2 or ids.stride(1) != 1:
+        raise ValueError(f"prompt_lookup: ids must be a (B, cap) int64 tensor with unit column stride, got "
+                         f"{tuple(ids.shape)} {ids.dtype}")
+    B, cap = ids.shape
+    dev = ids.device
+    p = _lib.PromptLookupParams()
+    p.ids, p.ids_stride, p.B, p.cap = ids.data_ptr(), ids.stride(0) if B > 1 else cap, B, cap
+    p.length, stride = _row_ints("lengths", lengths, B, dev)
+    p.length_stride = stride
+    if start is not None:
+        p.start, _ = _row_ints("start", start, B, dev)
+        if start.stride(0) != 1:
+            raise ValueError("prompt_lookup: start must be contiguous")
+    if limit is not None:
+        p.limit, _ = _row_ints("limit", limit, B, dev)
+        if limit.stride(0) != 1:
+            raise ValueError("prompt_lookup: limit must be contiguous")
+    g, n, off = _as_int(G), _as_int(N), _as_int(length_offset)
+    if g is None or n is None or off is None or not -2 ** 31 <= min(g, n, off) <= max(g, n, off) < 2 ** 31:
+        raise ValueError(f"prompt_lookup: num_output_tokens, max_matching_ngram_size and length_offset must be int32 "
+                         f"integers, got {G!r}, {N!r}, {length_offset!r}")
+    p.G, p.N, p.length_offset = g, n, off
+    eos = list(eos)
+    if len(eos) > LOOKUP_MAX_EOS or any(_as_int(e) is None or not -2 ** 63 <= e < 2 ** 63 for e in eos):
+        raise ValueError(f"prompt_lookup: at most {LOOKUP_MAX_EOS} int64 EOS ids, got {eos!r}")
+    p.n_eos = len(eos)
+    for i, e in enumerate(eos):
+        p.eos[i] = int(e)
+    return p
+
+
+def _launch_lookup(p) -> None:
+    lib = _lib.lib()
+    if not lib.pcv_prompt_lookup_supported(C.byref(p)):
+        raise ValueError(f"prompt_lookup: {lib.pcv_last_error().decode()}")
+    check(lib.pcv_prompt_lookup(C.byref(p), _stream()), "pcv_prompt_lookup")
+
+
+def prompt_lookup(ids: torch.Tensor, lengths: torch.Tensor, num_output_tokens: int = 10,
+                  max_matching_ngram_size: int = 2, *, start: Optional[torch.Tensor] = None,
+                  limit: Optional[torch.Tensor] = None, eos=(), length_offset: int = 0):
+    """Prompt-lookup drafts of every batch row (pcv_prompt_lookup): 🤗's ``PromptLookupCandidateGenerator.get_candidates``
+    (no logits processor) on each row alone, with G = ``num_output_tokens`` and N = ``max_matching_ngram_size``; the
+    rule is stated in ``include/pcv_attn.h``.
+
+    ``ids`` (B, cap) int64 CUDA with unit column stride.  Row b's history is ``ids[b, start[b] : L_b]`` with
+    ``L_b = lengths[b] + length_offset`` (``lengths`` a (B,) int32 CUDA tensor of any element stride, read when the
+    kernel runs) and ``start`` (B,) int32 its left-padding count (None: 0).  ``limit`` (B,) int32 caps each row's
+    draft (None: G); ``eos`` cuts a draft before its first EOS id.  Returns ``(drafts, counts)``: (B, G) int64, the
+    draft then the history's last id as filler, and (B,) int32 draft lengths.  Nothing is read back to the host;
+    recordable in a CUDA graph.  Arguments the kernel does not take raise ``ValueError`` before any launch."""
+    p = _lookup_params(ids, lengths, num_output_tokens, max_matching_ngram_size, start, limit, eos, length_offset)
+    drafts = torch.empty(p.B, max(p.G, 1), dtype=torch.int64, device=ids.device)
+    counts = torch.empty(p.B, dtype=torch.int32, device=ids.device)
+    p.drafts, p.drafts_stride, p.counts = drafts.data_ptr(), p.G, counts.data_ptr()
+    _launch_lookup(p)
+    return drafts, counts
+
+
+def prompt_lookup_round(ids: torch.Tensor, lengths: torch.Tensor, length_offset: int, fed: torch.Tensor,
+                        draws: torch.Tensor, next_tokens: torch.Tensor, state: torch.Tensor, num_output_tokens: int,
+                        max_matching_ngram_size: int, *, start: Optional[torch.Tensor] = None, eos=()) -> None:
+    """Round mode of :func:`prompt_lookup`: settle the speculative round that fed ``fed`` (B, k) int64 (t_0, the
+    drafts, filler) and drew ``draws`` (B, k) int64, then search the next drafts; the rule is stated in
+    ``include/pcv_attn.h``.  ``state`` (4, B) int32 CUDA, contiguous: [accepted (out), counts (in: the drafts fed;
+    out: the next), unfinished, left].  ``next_tokens`` (B, >= G+1) int64 with unit column stride takes the next t_0
+    in column 0 and the next drafts in columns 1 .. G; row L_b - 1 of ``ids`` (``L_b = lengths[b] + length_offset +
+    n_b``) takes t_0.  In place, no host read; recordable in a CUDA graph."""
+    p = _lookup_params(ids, lengths, num_output_tokens, max_matching_ngram_size, start, None, eos, length_offset)
+    B, dev = p.B, ids.device
+    k = fed.shape[1] if fed.dim() == 2 else 0
+    for what, t in (("fed", fed), ("draws", draws)):
+        _require_cuda(t)
+        if t.device != dev or t.dtype != torch.int64 or tuple(t.shape) != (B, k) or not t.is_contiguous():
+            raise ValueError(f"prompt_lookup_round: {what} must be a contiguous ({B}, k) int64 tensor on {dev}, got "
+                             f"{tuple(t.shape)} {t.dtype}")
+    _require_cuda(next_tokens, state)
+    if next_tokens.device != dev or next_tokens.dtype != torch.int64 or next_tokens.dim() != 2 or \
+            next_tokens.shape[0] != B or next_tokens.shape[1] < p.G + 1 or next_tokens.stride(1) != 1:
+        raise ValueError(f"prompt_lookup_round: next_tokens must be a ({B}, >= {p.G + 1}) int64 tensor with unit "
+                         f"column stride on {dev}")
+    if state.device != dev or state.dtype != torch.int32 or tuple(state.shape) != (4, B) or not state.is_contiguous():
+        raise ValueError(f"prompt_lookup_round: state must be a contiguous (4, {B}) int32 tensor on {dev}")
+    p.k, p.fed, p.draws = k, fed.data_ptr(), draws.data_ptr()
+    p.t0, p.t0_stride = next_tokens.data_ptr(), next_tokens.stride(0) if B > 1 else next_tokens.shape[1]
+    p.drafts, p.drafts_stride = next_tokens.data_ptr() + 8, p.t0_stride
+    p.accepted, p.counts, p.unfinished, p.left = (state[i].data_ptr() for i in range(4))
+    _launch_lookup(p)
