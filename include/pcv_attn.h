@@ -580,13 +580,14 @@ PCV_API int pcv_rotary_apply_fp8(const pcv_rotary_params* p, const pcv_rotary_fp
  * 16 (e4m3 rows, with pcv_decode_fp8 as in pcv_attn_decode_fp8) and at most 256; no write_partial, no key shard.
  *
  * pcv_kv_append_at (_fp8): pcv_kv_append (_fp8) of the n new rows to arena rows bounds[0] .. bounds[0] + n - 1, with
- * k_cache = v_cache = NULL and L_old = 0; k_dst / v_dst point at arena row 0.  Rows that would land at or past
- * `capacity` are skipped.
+ * k_cache = v_cache = NULL and L_old = 0; k_dst / v_dst point at arena row 0.  Rows that would land before row 0 or
+ * at or past `capacity` are skipped.
  *
  * pcv_rotary_apply_at (_fp8): pcv_rotary_apply (_fp8) with the angle rows of a precomputed (capacity, rotate_dim) fp32
  * table (`angles`, a_stride_b = 0): input row i uses table row bounds[0] + i and is written to output row bounds[0] + i
  * when bounds[1] != 0 (a new key rotated straight into a rotated-key arena), else to row i (q into a fixed buffer).
- * angle_row0 is ignored; rows whose table row is at or past `capacity` are skipped.
+ * angle_row0 is ignored; rows whose table row is negative or at or past `capacity` are skipped, whichever output row
+ * they would go to.
  */
 typedef struct pcv_dev_rows {
   const int32_t* bounds;   /* device int32s; meaning per entry point above                  */

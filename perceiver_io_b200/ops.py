@@ -1257,8 +1257,8 @@ def attention_window(q, k, v, bounds: torch.Tensor, num_heads: int, scale: float
 def kv_append_at(k_arena: torch.Tensor, v_arena: torch.Tensor, k_new: torch.Tensor, v_new: torch.Tensor,
                  row: torch.Tensor, k_inv_scale=None, v_inv_scale=None) -> None:
     """Write the new rows k_new / v_new (B, n, C) to rows ``row[0] .. row[0] + n - 1`` of the arenas (B, capacity, C), the
-    row read from device memory when the kernel runs (pcv_kv_append_at); rows at or past capacity are skipped.  ``row``
-    (B, >= 1) gives batch row b its own first row ``row[b, 0]``.
+    row read from device memory when the kernel runs (pcv_kv_append_at); rows that would land before row 0 or at or
+    past capacity are skipped.  ``row`` (B, >= 1) gives batch row b its own first row ``row[b, 0]``.
     ``float8_e4m3fn`` arenas store ``clamp(x * inv_scale, +-448)`` rounded to e4m3 (pcv_kv_append_at_fp8, per-channel
     ``k_inv_scale`` / ``v_inv_scale`` as in :func:`kv_append_fp8`)."""
     _require_cuda(k_arena, v_arena, k_new, v_new, row)
@@ -1279,8 +1279,9 @@ def rotary_apply_at(x: torch.Tensor, num_heads: int, table: torch.Tensor, rows: 
     """``out`` <- x (B, n, H*d) bf16 / fp16 rotated at the angle rows ``rows[0] + i`` of ``table`` (capacity, rotate_dim)
     (:func:`rotary_angle_table`), the rows read from device memory when the kernel runs (pcv_rotary_apply_at / _fp8).
     Row i goes to ``out[:, rows[0] + i]`` when ``rows[1] != 0`` (a key into a rotated-key arena of at least capacity
-    rows), else to ``out[:, i]``.  ``rows`` (B, >= 2) gives batch row b its own ``rows[b, 0:2]``.  An e4m3 ``out``
-    stores the codes of the rotated rows times ``y_inv_scale[h]`` (H,).
+    rows), else to ``out[:, i]``.  Rows whose table row ``rows[0] + i`` is negative or at or past ``table.shape[0]``
+    are skipped: their output row is not written.  ``rows`` (B, >= 2) gives batch row b its own ``rows[b, 0:2]``.  An
+    e4m3 ``out`` stores the codes of the rotated rows times ``y_inv_scale[h]`` (H,).
     Bit-equal to :func:`rotary_at` / the rotated-key shadow of :func:`rotated_cache_keys` at the same positions."""
     _require_cuda(x, table, rows, out)
     x = _rows_contiguous(x)
