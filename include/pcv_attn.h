@@ -298,6 +298,9 @@ typedef struct pcv_ln_stats_params {
  *   out[g]   : rank g's output (B,N,H,dv) in p->dtype with the strides below; every rank ends with the full result
  *   flags[g] : rank g's flag block, >= 32 zero-initialised uint32 words (never reset: values are epochs)
  * Rank r merges rows [R*r/G, R*(r+1)/G) of the flattened (b,h,n) space, R = B*H*N.
+ * The merge loads 16 bytes of part rows and stores 4 channels (8 bytes) of output rows at once, so every part[g] must
+ * be 16-byte aligned, every out[g] 8-byte aligned, o_stride_b / o_stride_n / o_stride_h multiples of 4 elements and
+ * every flags[g] 4-byte aligned; other calls are refused with PCV_ERR_INVALID before any CUDA call.
  */
 typedef struct pcv_shard_fuse {
   void* part[PCV_MAX_PEERS];

@@ -226,6 +226,18 @@ int pcv_attn_fwd_sharded(const pcv_attn_params* p, const pcv_shard_fuse* f, void
   PCV_REQUIRE(f->epoch >= 1, PCV_ERR_INVALID, "attn_fwd_sharded: epoch must start at 1");
   for (int g = 0; g < f->num_peers; ++g)
     PCV_REQUIRE(f->part[g] && f->out[g] && f->flags[g], PCV_ERR_INVALID, "attn_fwd_sharded: NULL buffer of rank %d", g);
+  // the tail loads 16 bytes of every part[g] row, stores 8 bytes (4 channels) of every out[g] row at o_off + 4 * lane
+  // and spins on 32-bit flag words: refuse what those accesses cannot address instead of faulting on the device
+  for (int g = 0; g < f->num_peers; ++g) {
+    PCV_REQUIRE(al16(f->part[g]), PCV_ERR_INVALID, "attn_fwd_sharded: part[%d] must be 16-byte aligned", g);
+    PCV_REQUIRE((reinterpret_cast<uintptr_t>(f->out[g]) & 7u) == 0, PCV_ERR_INVALID,
+                "attn_fwd_sharded: out[%d] must be 8-byte aligned", g);
+    PCV_REQUIRE((reinterpret_cast<uintptr_t>(f->flags[g]) & 3u) == 0, PCV_ERR_INVALID,
+                "attn_fwd_sharded: flags[%d] must be 4-byte aligned", g);
+  }
+  PCV_REQUIRE(((f->o_stride_b | f->o_stride_n | f->o_stride_h) & 3) == 0, PCV_ERR_INVALID,
+              "attn_fwd_sharded: output strides (%lld, %lld, %lld) must be multiples of 4 elements",
+              (long long)f->o_stride_b, (long long)f->o_stride_n, (long long)f->o_stride_h);
   pcv_attn_params q = *p;
   q.write_partial = 1;
   // validate_attn wants part_* for a partial launch; they are replaced by part[rank] inside the launcher
